@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — collision cost+gradient evaluations/s of the discrete hot path on B200 (BASELINE.json metric).
+"""bench.py — collision cost+gradient evaluations/s of the discrete hot path on an H100 (BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            # our arm (CUDA, through libisdf_b200.so)
   python bench.py --impl reference --gpus N --steps K ...   # the reference's CPU algorithm (OpenMP structure) on host cores
@@ -13,6 +13,8 @@ schedule each step uses was learned from another trajectory — as in a real opt
 evaluation) figures are reported beside it in `extra`.
 At N > 1 every rank evaluates the pose samples s % N == rank and the 19N+1 doubles are summed over NVLink peer memory.
 Other BASELINE configs as strong-scaling workloads of their own: --workload swept (configs[3]), --workload batch1024 (configs[4]).
+--dump-outputs DIR writes what the last timed step computed (the arrays a caller of the timed entry point receives) as DIR/<name>.npy;
+the inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -165,22 +167,18 @@ def measured_peak_hbm():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json, burst)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet, HBM3)"
 
 
-def ncu_capture(key="k_discrete_dram_bytes_per_launch"):
-    """a figure of the dominant kernel from the committed ncu --set full capture (profiles/roofline_traffic.json), or None."""
-    p = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p)).get(key)
-        except Exception:
-            return None
-    return None
-
-
-def ncu_traffic():
-    return ncu_capture("k_discrete_dram_bytes_per_launch")
+def dump_outputs(out_dir, arrays):
+    """write the last timed step's outputs as out_dir/<name>.npy (float64, at most 64 MB in all)"""
+    if not out_dir:
+        return
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: np.ascontiguousarray(v, dtype=np.float64) for k, v in arrays.items()}
+    assert sum(a.nbytes for a in arrays.values()) <= 64 << 20
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 # ---- CPU arm: the reference's algorithm (oracle port, OpenMP `parallel for schedule(dynamic)` + `critical`) -----------------
@@ -586,7 +584,7 @@ def run_ours(args):
     d_T = torch.from_numpy(T).to(dev)
     d_Cs = torch.from_numpy(iters).to(dev)                  # every iterate resident in HBM before the timed region
     d_out = torch.zeros(19 * N + 1, dtype=torch.float64, device=dev)
-    flush = torch.empty(512 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(512 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 50 MB L2 (H100)
     stream = torch.cuda.current_stream().cuda_stream
     ref_nccl = None
     if world > 1:                                         # untimed cross-check for the fused exchange: same shards, NCCL sum
@@ -653,6 +651,7 @@ def run_ours(args):
     times = timed(range(n_warm, n_warm + args.steps))       # THE timed region: K distinct iterates, each on the schedule of its predecessor
     barrier()
     wall = time.perf_counter() - t_wall0
+    last_out = d_out.cpu().numpy().copy()                   # the last timed step's [cost | gradC | gradT]
     launches = ev.stats().kernel_launches - l0
     k_last = n_warm + args.steps - 1
     # context figures (not the headline): warm L2; the SAME iterate repeated (round 1's measurement: the schedule is a perfect predictor);
@@ -745,9 +744,8 @@ def run_ours(args):
                 "e2e": {"value": 1e3 / ms_e2e, "unit": UNIT, "h2d_bytes_per_step": 8 * 19 * N, "d2h_bytes_per_step": 8 * (19 * N + 1) + 8,
                         "ms_per_step": ms_e2e, "api": "isdf_eval_discrete (host buffers)"},
                 "gpu_launches": int(launches),
-                "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": ncu_traffic(),
+                "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None,
                              "peak_source": peak_src, "kernel": "k_discrete_mesh", "algorithmic_bytes_per_launch": ab // world,
-                             "fp64_pipe_active_pct_ncu": ncu_capture("fp64_pipe_active_pct"), "issue_slots_busy_pct_ncu": ncu_capture("issue_slots_busy_pct"),
                              "note": "window bytes counted at 1 B/voxel per sample (SURVEY §8d); the kernel is FP64/latency bound, see DESIGN.md"},
                 "extra": {"pairs_per_eval": int(pairs), "pairs_per_s": pairs / (ms * 1e-3), "ms_per_step_warm_l2": statistics.mean(warm),
                           "evals_per_s_warm_l2": 1e3 / statistics.mean(warm), "ms_min": min(times), "ms_max": max(times),
@@ -803,6 +801,7 @@ def run_ours(args):
                                 "error seen through the hinge, reported as SURVEY 8c demands — not a parity claim"}
             except Exception as e:
                 line["extra"]["sign_policy_deviation_vs_reference_fwn"] = {"error": repr(e)}
+        dump_outputs(args.dump_outputs, {"cost": last_out[:1], "grad_coeffs": last_out[1:1 + 18 * N], "grad_durations": last_out[1 + 18 * N:]})
         print(json.dumps(line))
     if world > 1:
         import torch.distributed as dist
@@ -908,6 +907,7 @@ def run_swept(args):
         torch.cuda.synchronize()
         times.append(max_over_ranks(e0.elapsed_time(e1)))
     launches = ev.stats().kernel_launches - l0
+    last_out = d_out.cpu().numpy().copy()
     e2e = []
     for it in range(n_warm + args.steps):
         Ck = iters[it]                                      # the iterates of the device-timed loop, in the same order
@@ -956,6 +956,7 @@ def run_swept(args):
             c, gC, gT = ev.eval_swept(T, iters[0])
             g, og = np.concatenate([gC, gT]), np.concatenate([ref["gradC"], ref["gradT"]])
             line["parity"] = {"cost_rel": abs(c - ref["cost"]) / abs(ref["cost"]), "grad_rel_l2": float(np.linalg.norm(g - og) / np.linalg.norm(og)), "tolerance": 1e-6}
+        dump_outputs(args.dump_outputs, {"cost": last_out[:1], "grad_coeffs": last_out[1:1 + 18 * N], "grad_durations": last_out[1 + 18 * N:]})
         print(json.dumps(line))
     if world > 1:
         import torch.distributed as dist
@@ -1015,6 +1016,7 @@ def run_batch(args):
         torch.cuda.synchronize()
         times.append(max_over_ranks(e0.elapsed_time(e1)))
     launches = ev.stats().kernel_launches - l0
+    last_cost, last_grad = d_cost.cpu().numpy().copy(), d_grad.cpu().numpy().copy()
     e2e = []
     hh, tt = heads.reshape(B, 3, 3).transpose(0, 2, 1), tails.reshape(B, 3, 3).transpose(0, 2, 1)   # back to row-major 3x3 for the python wrapper
     for it in range(2 + max(3, args.steps // 4)):
@@ -1082,6 +1084,7 @@ def run_batch(args):
             line["cpu_baseline"] = {"value": nb / dt, "unit": "problems/s", "cores": oc.threads_num, "kind": "port",
                                     "sample": f"{nb} of the {Btot} problems, one at a time: oracle MINCO + OpenMP discrete term (reference loop structure) + oracle adjoint"}
             line["parity"] = {"cost_rel_max_over_sample": worst, "tolerance": 1e-6}
+        dump_outputs(args.dump_outputs, {"cost": last_cost, "grad": last_grad})   # rank 0's problems
         print(json.dumps(line))
     ev.close()
     if world > 1:
@@ -1156,6 +1159,7 @@ def main():
                     help="discrete = BASELINE configs[2] (headline); swept = configs[3]; batch1024 = configs[4] — each a strong-scaling workload of its own")
     ap.add_argument("--batch-total", type=int, default=1024, help="--workload batch1024: total problems (sharded over the ranks)")
     ap.add_argument("--lbfgs-iterations", type=int, default=8, help="--workload batch1024: iteration cap of the device-resident L-BFGS measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args) if args.workload == "discrete" else run_reference_other(args)

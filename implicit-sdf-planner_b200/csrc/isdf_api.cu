@@ -1,4 +1,4 @@
-// libisdf_b200.so — C-ABI layer (include/isdf.h) over the sm_100a kernels. No CPU fallback anywhere: every entry
+// libisdf_b200.so — C-ABI layer (include/isdf.h) over the sm_90a kernels. No CPU fallback anywhere: every entry
 // point either runs CUDA kernels or fails with ISDF_ERR_CUDA / ISDF_ERR_STATE.
 #include "../../include/isdf.h"
 #include "isdf_types.cuh"
@@ -58,8 +58,9 @@ struct isdf_ctx {
     DevBuf<int> d_tickets;       // pieces_done counter of the epilogue kernel
     DevBuf<double> d_tot; DevBuf<unsigned> d_split_done;   // per-sample collision sums handed from the scan kernels to the epilogue
     DevBuf<int> d_items, d_item_count; DevBuf<unsigned> d_work, d_split_work; DevBuf<double> d_subsum;   // work items (longest first, heavy samples split)
-    int warp_slots = 148 * 16;   // resident warps of the mesh kernel on this device (SMs x CTAs/SM x warps/CTA)
-    int sm_count = 148, mesh_blocks = 4, analytic_blocks = 4;   // persistent grids: one CTA per resident slot
+    int warp_slots = 132 * 16;   // resident warps of the mesh kernel on this device (SMs x CTAs/SM x warps/CTA)
+    int sm_count = 132, mesh_blocks = 4, analytic_blocks = 4;   // persistent grids: one CTA per resident slot
+    size_t smem_per_sm = 228 * 1024;   // shared memory of one SM (H100: 228 KB, at most 227 KB to one CTA)
     long long order_for = -1;    // (N, rank, world) signature the order array is valid for
     DevBuf<unsigned long long> d_counter, d_dbg, d_trace;
     DevBuf<double> d_mx, d_mbc, d_mT, d_mC, d_mlu, d_men, d_mgC, d_mgT, d_mcost, d_mgrad, d_mout, d_mCpp, d_msv;   // batched callback (isdf_minco.cuh)
@@ -128,7 +129,7 @@ extern "C" int isdf_create(const isdf_config *cfg, int device, isdf_ctx **out) {
     CU_TRY(cudaGetDeviceCount(&ndev));
     if (device < 0 || device >= ndev) return fail(ISDF_ERR_CUDA, "no such CUDA device (this library has no CPU fallback)");
     CU_TRY(cudaSetDevice(device));
-    // fail loudly if the sm_100a image cannot run here
+    // fail loudly if the sm_90a image cannot run here
     int nb_mesh = 0, nb_analytic = 0;
     CU_TRY(discrete_resident_blocks(&nb_mesh, &nb_analytic));
     // pose-window offsets are packed 10 bits per axis (isdf_discrete.cuh); the inclusive index range of a window is at most
@@ -140,6 +141,7 @@ extern "C" int isdf_create(const isdf_config *cfg, int device, isdf_ctx **out) {
         cudaDeviceProp prop;
         if (cudaGetDeviceProperties(&prop, device) == cudaSuccess && nb_mesh > 0 && nb_analytic > 0) {
             c->sm_count = prop.multiProcessorCount;
+            c->smem_per_sm = prop.sharedMemPerMultiprocessor;
             c->mesh_blocks = nb_mesh; c->analytic_blocks = nb_analytic;
             c->warp_slots = prop.multiProcessorCount * nb_mesh * DISC_WARPS;
         }
@@ -320,7 +322,7 @@ extern "C" int isdf_set_shape_mesh_ex(isdf_ctx *c, const double *V, int nV, cons
     // exact candidate lists for every cell a query can land in and not be settled by the cell's distance bracket alone: the discrete
     // path queries within safety_hor of the surface, the swept-volume path within its range bound 2*safety_hor + 0.1 (swm:383) — a
     // flat pass over ~100 listed triangles answers such a query in a tenth of the time of a far-field tree search, and the sign
-    // descent of the swept-volume path is a CHAIN of them (profiles/r02_tuning.md, swept path)
+    // descent of the swept-volume path is a CHAIN of them
     {
         const double hd = 0.5 * std::sqrt(3.0) * m.gcell;
         const double list_reach = std::max(c->cfg.safety_hor, 2.0 * c->cfg.safety_hor + 0.1) + 2.0 * m.ghd;
@@ -700,7 +702,7 @@ static int launch_discrete(isdf_ctx *c, int N, const double *d_T, const double *
     // longest-first order from the previous evaluation of the same problem shape (first evaluation: natural order)
     const long long sig = ((long long)N << 20) ^ ((long long)c->rank << 10) ^ c->world ^ ((long long)K << 40);
     const bool mesh = (c->shape.kind == ISDF_SHAPE_MESH);
-    // only mesh samples have a heavy tail worth splitting. Every sample of a launch may be split (item trace at world = 8, profiles/r02_tuning.md:
+    // only mesh samples have a heavy tail worth splitting. Every sample of a launch may be split (item trace at world = 8:
     // with M/4 slots the 515 heaviest samples were split and the NEXT heaviest — unsplit, 15-25 queries, 80-110 us — set the kernel time)
     const int max_split = mesh ? (int)std::min<long long>(M, MAX_SPLIT_SLOTS) : 0;
     const size_t max_items = (size_t)M + (size_t)(ROW_CLASSES - 1) * max_split;
@@ -1271,7 +1273,8 @@ extern "C" int isdf_frontend_feasibility_device(isdf_ctx *c, uint32_t *d_masks, 
     const size_t smem = sizeof(uint32_t) * 4 * (size_t)A.ks * A.ks * A.ks;
     CU_TRY(cudaFuncSetAttribute(k_frontend_feasibility, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const long long nrun = (long long)c->grid.X * c->grid.Y * ((c->grid.Z + FE_ZRUN - 1) / FE_ZRUN);
-    const unsigned grid = (unsigned)std::min<long long>((nrun + 255) / 256, 148ll * 64);
+    const long long sms = c->sm_count;
+    const unsigned grid = (unsigned)std::min<long long>((nrun + 255) / 256, sms * 64);
     if (c->fe_ncore > 0 && nrun < (1ll << 32) && !getenv("ISDF_FE_ONE_PASS")) {
         // two passes: the kernel core settles most voxels of a cluttered map, the mask accumulation runs on the survivors only
         CU_TRY(c->d_fe_surv.ensure((size_t)nrun));
@@ -1285,14 +1288,15 @@ extern "C" int isdf_frontend_feasibility_device(isdf_ctx *c, uint32_t *d_masks, 
             CU_TRY(cudaMemsetAsync(d_masks, 0, sizeof(uint32_t) * 4 * (size_t)nvox, (cudaStream_t)cuda_stream));
             const long long nword = (long long)c->grid.X * c->grid.Y * c->grid.Zw;
             CU_TRY(cudaFuncSetAttribute(k_frontend_survivors_tab, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tsmem));
-            k_frontend_core_words<<<(unsigned)std::min<long long>((nword + 255) / 256, 148ll * 32), 256, 0, (cudaStream_t)cuda_stream>>>(A);
+            k_frontend_core_words<<<(unsigned)std::min<long long>((nword + 255) / 256, sms * 32), 256, 0, (cudaStream_t)cuda_stream>>>(A);
             // 32 warps per SM hide the row reads: two CTAs of 512 threads when two tables fit into shared memory, else one of 1024
-            if (2 * (tsmem + 1024) <= 220 * 1024) k_frontend_survivors_tab<<<148 * 2, 512, tsmem, (cudaStream_t)cuda_stream>>>(A);
-            else k_frontend_survivors_tab<<<148, 1024, tsmem, (cudaStream_t)cuda_stream>>>(A);
+            // (1 KB of every CTA's shared memory is reserved by the runtime)
+            if (2 * (tsmem + 1024) <= c->smem_per_sm) k_frontend_survivors_tab<<<(unsigned)sms * 2, 512, tsmem, (cudaStream_t)cuda_stream>>>(A);
+            else k_frontend_survivors_tab<<<(unsigned)sms, 1024, tsmem, (cudaStream_t)cuda_stream>>>(A);
         } else {
             CU_TRY(cudaFuncSetAttribute(k_frontend_survivors, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             k_frontend_core<<<grid, 256, 0, (cudaStream_t)cuda_stream>>>(A);
-            k_frontend_survivors<<<148 * 16, 256, smem, (cudaStream_t)cuda_stream>>>(A);
+            k_frontend_survivors<<<(unsigned)sms * 16, 256, smem, (cudaStream_t)cuda_stream>>>(A);
         }
         c->stats.kernel_launches += 2;
     } else {

@@ -5,7 +5,7 @@
 // wired into the sample loop exactly as hpp:619-626 wires its swept-volume sibling; PCSmapManager::getPointsInAABB
 // (PCSmap_manager.h:148-170); getSDFWithGradWhenRobotAtState (sw_manager.hpp:537-541).
 //
-// Mapping (B200-first, not the reference's OpenMP-over-samples + critical section):
+// Mapping (GPU-first, not the reference's OpenMP-over-samples + critical section):
 //   * the pose window is read from the BIT-packed occupancy: lane = (x,y) row, one or two 32-bit loads + funnel shift give the
 //     row's z-run; only the occupied voxels are enumerated, in the reference's (x, y, z) order per row, and compacted through a
 //     per-warp shared-memory queue so that every cull pass runs on 32 live voxels (the reference tests every voxel and
@@ -48,7 +48,7 @@ constexpr int ROW_CLASSES = 32;         // a pose window's voxels are summed in 
 constexpr unsigned SPLIT_WORK_MIN = 256u;  // never split a sample lighter than this (work units: 64 per mesh query + 1 per culled pair)
 constexpr int MAX_SPLIT_SLOTS = 16384;  // split samples per launch (2 KB of class sums each)
 constexpr int WINDOW_AXIS_MAX = 1023;   // voxels per window axis: window offsets are packed 10 bits per axis
-// CTAs per SM the register allocator must leave room for — A/B-measured on B200 (profiles/r01_tuning.md, r02_tuning.md)
+// CTAs per SM the register allocator must leave room for: 4 CTAs x 128 threads x 128 registers fill the 64 K-register file of an SM
 constexpr int ANALYTIC_MIN_BLOCKS = 4;
 #ifndef ISDF_MESH_MIN_BLOCKS
 #define ISDF_MESH_MIN_BLOCKS 4
@@ -675,7 +675,7 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
             // Voxel (row r, z offset dz) of the window belongs to class (r + 5 dz) % 32: the voxels an obstacle patch puts near the robot
             // — a few rows x a few z, the ones that cost mesh queries — land in ~as many different classes as there are voxels, so the
             // parts of a split sample get near-equal numbers of queries (row-interleaved classes gave a wall patch to 5 of 32 classes:
-            // item timeline in profiles/r02_tuning.md). A split part scans the same rows and keeps its classes' voxels (a bit filter).
+            // measured item timeline). A split part scans the same rows and keeps its classes' voxels (a bit filter).
             // Lanes are rows in ascending order and a lane emits its voxels z-ascending, so emitting a batch lane by lane — at once when it
             // fits into the ring, else row by row (dense walls) — keeps every CLASS's voxels in (row, z) order for whole samples and parts.
             const int w = it.c1 - it.c0;

@@ -1,7 +1,7 @@
 // Translation unit of the discrete-path kernels (isdf_discrete.cuh): k_discrete_mesh, k_discrete_analytic, k_discrete_epilogue,
 // k_build_items. Compiled WITH FMA contraction (nvcc default): nothing on this path replays a sequential decision of the
-// reference, its parity bar is the north star's 1e-6 (observed ~1e-15), and un-fused FP64 cost the mesh kernel ~12 % (ncu,
-// profiles/r01_p). The swept-volume search, whose accept/reject sequence must replay the reference's bit for bit, stays in
+// reference, its parity bar is the north star's 1e-6 (observed ~1e-15), and un-fused FP64 costs the mesh kernel
+// time. The swept-volume search, whose accept/reject sequence must replay the reference's bit for bit, stays in
 // isdf_api.cu under -fmad=false. ISDF_FAST_TRI selects the division-free closest-point test (isdf_mesh.cuh) for this TU only.
 #define ISDF_DISCRETE_TU 1
 #ifndef ISDF_NO_FAST_TRI   // A/B builds only
@@ -15,7 +15,7 @@ namespace isdf {
 
 cudaError_t discrete_launch_scan(const DiscArgs &A, bool mesh, unsigned grid, cudaStream_t st) {
 #ifdef ISDF_CARVEOUT
-    static bool carved = false;   // A/B: ask for the smallest shared-memory carve-out that still holds 4 CTAs/SM (132 KB -> 124 KB of L1)
+    static bool carved = false;   // A/B: ask for the smallest shared-memory carve-out that still holds 4 CTAs/SM
     if (!carved) {
         carved = true;
         cudaFuncSetAttribute(k_discrete_mesh<false>, cudaFuncAttributePreferredSharedMemoryCarveout, ISDF_CARVEOUT);
@@ -42,7 +42,7 @@ cudaError_t discrete_launch_build_items(const unsigned *work, int rank, int worl
 
 cudaError_t discrete_resident_blocks(int *mesh_blocks, int *analytic_blocks) {
     cudaFuncAttributes fa;
-    cudaError_t e = cudaFuncGetAttributes(&fa, (const void *)k_discrete_analytic);   // fails loudly if the sm_100a image cannot run here
+    cudaError_t e = cudaFuncGetAttributes(&fa, (const void *)k_discrete_analytic);   // fails loudly if the sm_90a image cannot run here
     if (e != cudaSuccess) return e;
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(mesh_blocks, k_discrete_mesh<false>, DISC_THREADS, 0);
     if (e != cudaSuccess) return e;

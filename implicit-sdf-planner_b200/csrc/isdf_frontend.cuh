@@ -5,7 +5,7 @@
 // inflated, byte-packed map (PCSmap_manager.h:46-78) at the voxel; visit_kernels_by_distance (sw_manager.hpp:852-913) tries the
 // level attitude and then a BFS over the attitude grid until a kernel fits; checkKernelValue (:914-941) maps that back to angles.
 //
-// B200 mapping: the question "which attitudes fit at voxel v" is answered for EVERY voxel in one pass, as a 128-bit mask per
+// GPU mapping: the question "which attitudes fit at voxel v" is answered for EVERY voxel in one pass, as a 128-bit mask per
 // voxel, so the graph search itself does O(1) lookups. The convolution is turned inside out: instead of testing up to 121 kernels
 // x 169 rows per voxel, each kernel offset (a,b,c) carries the SET OF ATTITUDES whose kernel occupies it (a 128-bit mask,
 // kernel_size^3 x 16 B = 35 KB in shared memory); a voxel ORs the masks of the OCCUPIED voxels of its window — found with the same

@@ -1,5 +1,5 @@
 // Device-side FP64 vector math, MINCO basis, quadrotor flatness map + adjoint, hinge.
-// Written for sm_100a; every function is __device__ __forceinline__ so the fused kernels keep state in registers.
+// Written for sm_90a; every function is __device__ __forceinline__ so the fused kernels keep state in registers.
 // Reference semantics: flatness.hpp:53-148, 230-406; back_end_optimizer.hpp:127-173, 332-356, 472-488.
 #pragma once
 #include <cuda_runtime.h>

@@ -1,7 +1,7 @@
 // Device-side triangle-mesh signed distance: the Generalshape mesh path (Shape.cpp:105-151), which the reference
 // evaluates with libigl's AABB tree (exact closest point) and fast winding number (sign).
 //
-// B200 layout: a binary BVH whose nodes carry BOTH children's boxes (one 112-byte fetch decides the descent),
+// Device layout: a binary BVH whose nodes carry BOTH children's boxes (one 112-byte fetch decides the descent),
 // leaves of <= 4 triangles stored in leaf order as (a, b-a, c-a), 7 pseudonormals per triangle (face, 3 edges,
 // 3 vertices) for the sign, and a coarse body-frame inside/outside bitmap that resolves the sign of points that
 // have no triangle within the query bound. The whole structure for a 4000-triangle robot is < 2 MB: L2-resident.
@@ -514,7 +514,7 @@ __device__ __forceinline__ void warp_argmin_update(double dd, d3 q, int t, int f
 }
 
 // Warp-cooperative nearest triangle from a cell's candidate list: lanes test 32 candidates per pass, REDUX arg-min.
-// (Two candidates per lane and pass — a second independent chain — was measured slower: profiles/r02_tuning.md.)
+// (Two candidates per lane and pass — a second independent chain — was measured slower.)
 __device__ __forceinline__ double list_closest_range(const DevMesh &M, d3 p, uint32_t off, int cnt, d3 &cbest, int &tri, int &feat, int lane);
 __device__ __forceinline__ double list_closest_pre(const DevMesh &M, d3 p, uint32_t off, int cnt, int first_id, d3 &cbest, int &tri, int &feat, int lane);
 __device__ __forceinline__ double list_closest(const DevMesh &M, d3 p, int cell, d3 &cbest, int &tri, int &feat, int lane) {
@@ -638,7 +638,7 @@ __device__ __forceinline__ double mesh_finish(const DevMesh &M, d3 p, d3 e, doub
     return s * sqrt(d2);
 }
 // compile-time choice of the sign source: the closed-mesh instantiation of a kernel carries no winding-number code at all (the discrete
-// scan kernel is sensitive to its code size: profiles/r02_tuning.md, v5)
+// scan kernel is sensitive to its code size)
 template <bool WINDING>
 __device__ __forceinline__ double mesh_finish_t(const DevMesh &M, d3 p, d3 e, double d2, int tri, int feat, d3 &g) {
     double s;

@@ -3,7 +3,7 @@
 // gradientDescent (:1000-1062), getSDFAtTimeStamp (:550-556), getSDF_DOTAtTimeStampOptimized (:593-662),
 // getGradPrelAtTimeStamp (:566-572), Trajectory::locatePieceIdx / getPos_Vel_Acc_Jerk (trajectory.hpp:105-149, 545-570).
 //
-// B200 mapping — the reference runs one OpenMP thread per obstacle point through a long scalar search; here
+// GPU mapping — the reference runs one OpenMP thread per obstacle point through a long scalar search; here
 //   k_sv_table : the coarse time grid t = 0, 0.2, ... (same running sum as the reference's for-loop) and the robot
 //                pose at each coarse time are computed ONCE per evaluation and shared by every point (the reference
 //                recomputes the pose per point per sample);
@@ -527,7 +527,7 @@ constexpr bool SV_ANALYTIC_CTA = ISDF_SV_ANALYTIC_CTA != 0;   // analytic shapes
 #ifndef ISDF_SVM_WARPS
 #define ISDF_SVM_WARPS 8
 #endif
-constexpr int SVM_WARPS = ISDF_SVM_WARPS;   // A/B on B200 (profiles/r01_tuning.md)
+constexpr int SVM_WARPS = ISDF_SVM_WARPS;   // warps per obstacle point (-DISDF_SVM_WARPS for A/B builds)
 constexpr int SVM_THREADS = SVM_WARPS * 32;
 
 struct SvmShared {

@@ -6,7 +6,7 @@
 namespace isdf {
 
 // Occupancy as one BIT per voxel, z fastest: word (ix*Y + iy)*Zw + (iz >> 5), bit iz & 31. A 512^3 map is 16 MiB
-// (L2-resident on B200) instead of the reference's 1 GiB of doubles (GridMap3D.h:215); a 14-voxel z-run of a
+// (L2-resident on H100: 50 MB of L2) instead of the reference's 1 GiB of doubles (GridMap3D.h:215); a 14-voxel z-run of a
 // pose window is one or two 32-bit loads + a funnel shift.
 struct DevGrid {
     const uint32_t *bits;

@@ -1,4 +1,4 @@
-/* isdf.h — C ABI of libisdf_b200.so: B200-native (sm_100a) collision cost/gradient evaluator for the
+/* isdf.h — C ABI of libisdf_b200.so: H100-native (sm_90a) collision cost/gradient evaluator for the
  * Implicit-SDF-Planner back end. Plain pointers and sizes only; no torch / Eigen / ROS types.
  *
  * Every entry point names the reference interface it replaces (paths relative to /root/reference/src):

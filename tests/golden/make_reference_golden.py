@@ -8,7 +8,10 @@ Run in the build container (where /root/reference exists):  python tests/golden/
   minco_reference.npz — outputs of the reference's utils/minco.hpp (MINCO_S3NU forward, energy gradients, propogateGrad) on seeded problems, and
                         of its utils/trajectory.hpp (getPos_Vel_Acc_Jerk, locatePieceIdx, getTotalDuration) on the resulting trajectories;
   lbfgs_reference.npz — what the reference's utils/lbfgs.hpp does on seeded problems: every evaluated point, solution, value, return code;
-  grid_reference.npz  — the reference's map_manager/src/Gridmap3D.cpp: grid indices, cube centres, in-map flags and AABB gathers on seeded grids."""
+  grid_reference.npz  — the reference's map_manager/src/Gridmap3D.cpp: grid indices, cube centres, in-map flags and AABB gathers on seeded grids;
+  ref_shapes_obj.npz  — the bytes of the OBJ files behind ref_meshes.npz, so that the product's OBJ reader is checked on the files themselves;
+  sign_policy_reference.npz — the oracle's discrete cost and gradient with the reference-faithful sign s = 1 - 2 w (w from the reference-compiled
+                        FWN header) on the inputs of test_gpu_reference_pins.py::test_sign_policy_deviation_from_reference_faithful_fwn."""
 import os
 import sys
 import numpy as np
@@ -20,6 +23,7 @@ sys.path.insert(0, os.path.join(ROOT, "implicit-sdf-planner_b200", "py"))
 import isdf_b200 as I          # noqa: E402
 import oracle_lib as O         # noqa: E402
 from test_reference_pins import flat_inputs, _minco_cases, _lbfgs_problems, _traj_times, _grid_cases   # noqa: E402
+from test_gpu_reference_pins import sign_policy_case, SIGN_POLICY_MESHES   # noqa: E402
 
 
 REF_SHAPES = "/root/reference/src/plan_manager/shapes"
@@ -45,11 +49,25 @@ def ref_meshes():
         print(name, V.shape, F.shape, "w range", w.min(), w.max())
     np.savez_compressed(os.path.join(HERE, "ref_meshes.npz"), names=np.array(list(MESHES)), **out)
     print("ref_meshes.npz written")
+    raw = {name: np.frombuffer(open(os.path.join(REF_SHAPES, name + ".obj"), "rb").read(), dtype=np.uint8) for name in MESHES}
+    np.savez_compressed(os.path.join(HERE, "ref_shapes_obj.npz"), **raw)
+    print("ref_shapes_obj.npz written")
+
+
+def sign_policy_reference():
+    out = {}
+    for name in SIGN_POLICY_MESHES:
+        cfg, occ, T, Cc, V, F, pp = sign_policy_case(name)
+        c, gC, gT, _ = O.eval_discrete(O.config_from(cfg), occ, [0, 0, 0], 1.0, O.Shape.mesh(V, F, pp, wn_mode=O.WN_REF), T, Cc)
+        out.update({f"{name}_cost": np.array(c), f"{name}_gradC": gC, f"{name}_gradT": gT})
+    np.savez_compressed(os.path.join(HERE, "sign_policy_reference.npz"), **out)
+    print("sign_policy_reference.npz written")
 
 
 def main():
     O.build()
     ref_meshes()
+    sign_policy_reference()
     cfg = O.config_from(I.default_config_values())
     ref = O.RefFlat(cfg)
     v, a, j, pg, vg, qg, og = flat_inputs(256, seed=123)

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box with -m gpu): every call goes through the C-ABI of libisdf_b200.so and is
+"""GPU parity tests (run on an H100 with -m gpu): every call goes through the C-ABI of libisdf_b200.so and is
 compared with the oracle on identical seeded inputs.
 
 Tolerances (stated, FP64 path):

@@ -17,7 +17,7 @@ def checker(tmp_path_factory):
     if shutil.which("nvcc") is None:
         pytest.skip("nvcc not available")
     exe = str(tmp_path_factory.mktemp("hm") / "host_mesh_check")
-    r = subprocess.run(["nvcc", "-std=c++17", "-O2", "-fmad=false", "-gencode", "arch=compute_100a,code=sm_100a", "-o", exe,
+    r = subprocess.run(["nvcc", "-std=c++17", "-O2", "-fmad=false", "-gencode", "arch=compute_90a,code=sm_90a", "-o", exe,
                         os.path.join(ROOT, "tests", "host_mesh_check.cu")], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr[-2000:]
     return exe
