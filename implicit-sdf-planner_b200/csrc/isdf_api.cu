@@ -52,6 +52,7 @@ struct isdf_ctx {
     bool have_shape = false;
     DevShape shape;
     DevBuf<BvhNode> d_nodes; DevBuf<WideNode> d_wnodes; DevBuf<double> d_tris, d_pn, d_obb; DevBuf<float> d_cell_dist; DevBuf<uint32_t> d_cell_seed, d_cell_off, d_cand; DevBuf<uint16_t> d_cell_cnt; DevBuf<uint4> d_cell_rec; DevBuf<WnNode> d_wn;
+    double mesh_list_reach = 0;  // radius (cell-centre distance) up to which cells got candidate lists (isdf_dbg_mesh_grid)
     // evaluation scratch
     DevBuf<double> d_T, d_C, d_out, d_piece_cost;
     double *count_out_dev = nullptr;   // host entry points: where the epilogue drops the pair count (behind the result vector)
@@ -326,6 +327,7 @@ extern "C" int isdf_set_shape_mesh_ex(isdf_ctx *c, const double *V, int nV, cons
     {
         const double hd = 0.5 * std::sqrt(3.0) * m.gcell;
         const double list_reach = std::max(c->cfg.safety_hor, 2.0 * c->cfg.safety_hor + 0.1) + 2.0 * m.ghd;
+        c->mesh_list_reach = list_reach;
         CU_TRY(c->d_cell_cnt.ensure(ncell)); CU_TRY(c->d_cell_off.ensure(ncell));
         const unsigned warps_grid = (unsigned)((ncell + 3) / 4);
         k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->d_cell_cnt.p, nullptr, nullptr);
@@ -1507,6 +1509,25 @@ extern "C" int isdf_dbg_flatness(isdf_ctx *c, int n, const double *vaj, const do
     if (e == cudaSuccess) e = cudaMemcpyAsync(out, dout.p, sizeof(double) * 16 * n, cudaMemcpyDeviceToHost, c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     return e == cudaSuccess ? 0 : -3;
+}
+// read-only view of the current mesh's body-frame cell grid, so tests can tell which search branch answers a query:
+// geom = {glo[3], gcell, ghd, gpad, sign_radius, list_reach}, gdim[3]; cell_dist / cell_cnt (gdim[0]*gdim[1]*gdim[2] entries, z fastest)
+// are optional — call with NULL first to size them. cell_cnt is 0 for every cell without a candidate list (all of them when no
+// list was built).
+extern "C" int isdf_dbg_mesh_grid(isdf_ctx *c, double *geom, int32_t *gdim, float *cell_dist, uint16_t *cell_cnt) {
+    if (!c || !geom || !gdim) return -1;
+    if (!c->have_shape || c->shape.kind != ISDF_SHAPE_MESH) return -2;
+    const DevMesh &m = c->shape.mesh;
+    for (int a = 0; a < 3; a++) { geom[a] = m.glo[a]; gdim[a] = m.gdim[a]; }
+    geom[3] = m.gcell; geom[4] = m.ghd; geom[5] = m.gpad; geom[6] = m.sign_radius; geom[7] = c->mesh_list_reach;
+    const size_t ncell = (size_t)m.gdim[0] * m.gdim[1] * m.gdim[2];
+    if (cudaSetDevice(c->device) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) return -3;
+    if (cell_dist && cudaMemcpy(cell_dist, c->d_cell_dist.p, sizeof(float) * ncell, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (cell_cnt) {
+        if (!m.cell_cnt) std::memset(cell_cnt, 0, sizeof(uint16_t) * ncell);
+        else if (cudaMemcpy(cell_cnt, m.cell_cnt, sizeof(uint16_t) * ncell, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    }
+    return 0;
 }
 extern "C" int isdf_dbg_swept_stats(isdf_ctx *c, unsigned long long *out, long long n) {
     if (!c || !out || (size_t)n > c->sv.d_dbg.n) return -1;

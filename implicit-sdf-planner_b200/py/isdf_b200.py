@@ -418,6 +418,23 @@ class Evaluator:
             raise IsdfError(-1, "isdf_dbg_item_stats failed")
         return n.value, parts.value
 
+    def dbg_mesh_grid(self, arrays=True):
+        """the current mesh's body-frame cell grid, copied to the host: dict(glo, gcell, ghd, gpad, sign_radius, list_reach, gdim) and,
+        with arrays, cell_dist (float32) and cell_cnt (uint16; 0 = no candidate list) shaped gdim (z fastest)"""
+        vp, dp = C.c_void_p, C.POINTER(C.c_double)
+        ip, fp, up = C.POINTER(C.c_int32), C.POINTER(C.c_float), C.POINTER(C.c_uint16)
+        self.lib.isdf_dbg_mesh_grid.argtypes = [vp, dp, ip, fp, up]
+        geom, gdim = np.zeros(8), np.zeros(3, dtype=np.int32)
+        if self.lib.isdf_dbg_mesh_grid(self.h, _dp(geom), gdim.ctypes.data_as(ip), None, None) != 0:
+            raise IsdfError(-1, "isdf_dbg_mesh_grid failed (is a mesh shape set?)")
+        out = dict(glo=geom[0:3].copy(), gcell=geom[3], ghd=geom[4], gpad=geom[5], sign_radius=geom[6], list_reach=geom[7], gdim=tuple(int(g) for g in gdim))
+        if arrays:
+            dist, cnt = np.zeros(tuple(gdim), dtype=np.float32), np.zeros(tuple(gdim), dtype=np.uint16)
+            if self.lib.isdf_dbg_mesh_grid(self.h, _dp(geom), gdim.ctypes.data_as(ip), dist.ctypes.data_as(fp), cnt.ctypes.data_as(up)) != 0:
+                raise IsdfError(-1, "isdf_dbg_mesh_grid failed")
+            out["cell_dist"], out["cell_cnt"] = dist, cnt
+        return out
+
     def dbg_flatness(self, v, a, j, quat_grad, omg_grad, vel_grad):
         """device flatness map + adjoint as compiled into the epilogue kernel -> (quat, omg, gV, gA, gJ)"""
         vaj = np.ascontiguousarray(np.concatenate([_f64(v).reshape(-1, 3), _f64(a).reshape(-1, 3), _f64(j).reshape(-1, 3)], axis=1))
