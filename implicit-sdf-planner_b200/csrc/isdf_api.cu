@@ -7,6 +7,7 @@
 #include "isdf_minco.cuh"
 #include "isdf_frontend.cuh"
 #include "isdf_lbfgs.cuh"
+#include "isdf_clearance.cuh"
 #include <queue>
 #include "isdf_host_mesh.cuh"
 #include <cstdio>
@@ -91,6 +92,10 @@ struct isdf_ctx {
     bool peer_fused = false;             // sharded *_device evaluations finish with the exchange
     int peer_world_alloc = 0, peer_cap = 0;
     DevBuf<int> d_peer_status;
+    // trajectory clearance check (isdf_clearance.cuh)
+    int clr_blocks = 1;                  // resident CTAs per SM of the clearance scan kernel
+    DevBuf<double> d_clr_in, d_clr_clear; DevBuf<long long> d_clr_vox; DevBuf<ClrSummary> d_clr_sum; DevBuf<int> d_clr_cursor;
+    DevBuf<unsigned long long> d_clr_counters;   // {candidate pairs, exact mesh searches} of the last check (isdf_dbg_clearance_counts)
     isdf_stats stats;
 };
 
@@ -131,8 +136,9 @@ extern "C" int isdf_create(const isdf_config *cfg, int device, isdf_ctx **out) {
     if (device < 0 || device >= ndev) return fail(ISDF_ERR_CUDA, "no such CUDA device (this library has no CPU fallback)");
     CU_TRY(cudaSetDevice(device));
     // fail loudly if the sm_90a image cannot run here
-    int nb_mesh = 0, nb_analytic = 0;
+    int nb_mesh = 0, nb_analytic = 0, nb_clr = 0;
     CU_TRY(discrete_resident_blocks(&nb_mesh, &nb_analytic));
+    CU_TRY(clearance_resident_blocks(&nb_clr));
     // pose-window offsets are packed 10 bits per axis (isdf_discrete.cuh); the inclusive index range of a window is at most
     // kernel_size + 2 voxels when the map resolution equals occupancy_resolution (isdf_set_map checks the resolution)
     if (cfg->kernel_size + 2 > WINDOW_AXIS_MAX) return fail(ISDF_ERR_UNSUPPORTED, "kernel_size too large (pose windows are limited to 1023 voxels per axis)");
@@ -146,6 +152,7 @@ extern "C" int isdf_create(const isdf_config *cfg, int device, isdf_ctx **out) {
             c->mesh_blocks = nb_mesh; c->analytic_blocks = nb_analytic;
             c->warp_slots = prop.multiProcessorCount * nb_mesh * DISC_WARPS;
         }
+        c->clr_blocks = std::max(nb_clr, 1);
     }
     std::memset(&c->stats, 0, sizeof(c->stats));
     std::memset(&c->grid, 0, sizeof(c->grid));
@@ -182,6 +189,7 @@ extern "C" int isdf_destroy(isdf_ctx *c) {
     for (int p = 0; p < PEER_MAX; p++) if (c->peer_open[p]) cudaIpcCloseMemHandle(c->peer_open[p]);
     if (c->peer_buf) cudaFree(c->peer_buf);
     c->d_peer_status.release();
+    c->d_clr_in.release(); c->d_clr_clear.release(); c->d_clr_vox.release(); c->d_clr_sum.release(); c->d_clr_cursor.release(); c->d_clr_counters.release();
     c->d_fe_rot.release(); c->d_fe_kernels.release(); c->d_fe_order.release(); c->d_fe_ok.release(); c->d_fe_masks.release(); c->d_fe_out.release(); c->d_fe_ind.release(); c->d_fe_father.release(); c->d_fe_child.release(); c->d_fe_core.release(); c->d_fe_urows.release(); c->d_fe_surv.release(); c->d_fe_chunks.release(); c->d_fe_tab.release(); c->d_fe_count.release();
     c->d_mx.release(); c->d_mbc.release(); c->d_mT.release(); c->d_mC.release(); c->d_mlu.release(); c->d_men.release(); c->d_mgC.release(); c->d_mgT.release(); c->d_mcost.release(); c->d_mgrad.release(); c->d_mout.release(); c->d_mCpp.release(); c->d_msv.release();
     c->sv.release();
@@ -1020,6 +1028,122 @@ extern "C" int isdf_get_batch_trajectories(isdf_ctx *c, double *T, double *coeff
     return 0;
 }
 
+// ---- trajectory clearance check (isdf_clearance.cuh) -------------------------------------------------------------------------------
+extern "C" int isdf_clearance_default_params(isdf_clearance_params *p) {
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    isdf_config d;
+    isdf_default_config(&d);
+    p->samples_per_piece = d.integral_intervs; p->pieces_per_traj = 0;
+    p->reach = d.safety_hor; p->margin = d.safety_hor;
+    return 0;
+}
+
+// number of trajectories of a call (0 when N / N0 do not define one)
+static int clearance_batch(int N, const isdf_clearance_params *p) {
+    if (N < 1 || !p || p->pieces_per_traj < 0) return 0;
+    if (p->pieces_per_traj == 0) return 1;
+    return (N % p->pieces_per_traj == 0) ? N / p->pieces_per_traj : 0;
+}
+
+// every check that needs no device work, in the order of include/isdf.h's error list
+static int clearance_check(isdf_ctx *c, int N, const isdf_clearance_params *p) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    if (N < 1) return fail(ISDF_ERR_INVALID, "N < 1");
+    if (p->samples_per_piece < 1) return fail(ISDF_ERR_INVALID, "samples_per_piece < 1");
+    if (!(p->reach > 0.0) || !std::isfinite(p->reach)) return fail(ISDF_ERR_INVALID, "reach must be positive and finite");
+    if (std::isnan(p->margin) || p->margin > p->reach) return fail(ISDF_ERR_INVALID, "margin must not exceed reach");
+    if (clearance_batch(N, p) == 0) return fail(ISDF_ERR_INVALID, "pieces_per_traj must be 0 or divide N");
+    if ((long long)N * (p->samples_per_piece + 1) > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "N * (samples_per_piece + 1) must fit in 31 bits");
+    if (c->world > 1) return fail(ISDF_ERR_UNSUPPORTED, "the clearance check is not sharded: call it on a context with isdf_set_shard(ctx, 0, 1)");
+    if (!c->have_map) return fail(ISDF_ERR_STATE, "map not set");
+    if (!c->have_shape) return fail(ISDF_ERR_STATE, "shape not set");
+    // the window of a sample spans at most 2 H sqrt(3) / res + 3 voxels per axis (rotated H box, one voxel of slack on each side); the
+    // 1023-voxel limit of the pose-window offsets applies as in the discrete path
+    const double H = c->dcfg.half_bd + p->reach;
+    if (2.0 * H * std::sqrt(3.0) / c->grid.res + 4.0 > (double)WINDOW_AXIS_MAX)
+        return fail(ISDF_ERR_INVALID, "reach too large for this map resolution: a sample window would exceed 1023 voxels per axis");
+    return 0;
+}
+
+static int clearance_launch_ctx(isdf_ctx *c, int N, const double *d_T, const double *d_C, const isdf_clearance_params *p, double *d_clear,
+                                long long *d_vox, ClrSummary *d_sum, cudaStream_t st) {
+    ClrArgs A;
+    A.grid = c->grid; A.shape = c->shape; A.fp = c->dcfg.fp; A.half_bd = c->dcfg.half_bd;
+    A.reach = p->reach; A.margin = p->margin;
+    A.N = N; A.K = p->samples_per_piece; A.N0 = p->pieces_per_traj == 0 ? N : p->pieces_per_traj;
+    A.T = d_T; A.C = d_C; A.clear = d_clear; A.voxel = d_vox; A.summary = d_sum;
+    CU_TRY(c->d_clr_cursor.ensure(1));
+    CU_TRY(c->d_clr_counters.ensure(2));
+    CU_TRY(cudaMemsetAsync(c->d_clr_cursor.p, 0, sizeof(int), st));
+    CU_TRY(cudaMemsetAsync(c->d_clr_counters.p, 0, 2 * sizeof(unsigned long long), st));
+    A.cursor = c->d_clr_cursor.p; A.counters = c->d_clr_counters.p;
+    const int mode = c->shape.kind != ISDF_SHAPE_MESH ? 0 : (c->shape.mesh.sign_mode == MESH_SIGN_WINDING ? 2 : 1);
+    const long long S = (long long)N * (A.K + 1);
+    const long long want = (S + CLR_WARPS - 1) / CLR_WARPS;
+    const unsigned grid = (unsigned)std::max<long long>(1, std::min(want, (long long)c->sm_count * c->clr_blocks));
+    CU_TRY(clearance_launch(A, mode, grid, st));
+    c->stats.kernel_launches += 2;   // scan kernel, summary kernel
+    return 0;
+}
+
+// on failure every summary reads "not shown to be free": min_clearance, t_min, first_hit NaN, voxel_min / piece_min / sample_min /
+// colliding_samples -1, collision_free 0
+static isdf_clearance_summary clearance_failed_summary() {
+    isdf_clearance_summary s;
+    s.min_clearance = s.t_min = s.first_hit = std::numeric_limits<double>::quiet_NaN();
+    s.voxel_min = -1; s.piece_min = s.sample_min = s.colliding_samples = -1; s.collision_free = 0;
+    return s;
+}
+static void clearance_poison_host(int N, const isdf_clearance_params *p, isdf_clearance_summary *summary) {
+    const int B = clearance_batch(N, p);
+    if (summary) for (int b = 0; b < std::max(B, 1); b++) summary[b] = clearance_failed_summary();
+}
+
+extern "C" int isdf_trajectory_clearance_device(isdf_ctx *c, int N, const double *d_T, const double *d_coeffs, const isdf_clearance_params *p,
+                                                double *d_sample_clearance, int64_t *d_sample_voxel, isdf_clearance_summary *d_summary,
+                                                void *cuda_stream) {
+    int r = clearance_check(c, N, p);
+    if (r == 0 && (!d_T || !d_coeffs || !d_sample_clearance || !d_sample_voxel || !d_summary)) r = fail(ISDF_ERR_INVALID, "NULL device pointer");
+    if (r == 0 && set_device(c)) r = ISDF_ERR_CUDA;
+    if (r == 0) r = clearance_launch_ctx(c, N, d_T, d_coeffs, p, d_sample_clearance, (long long *)d_sample_voxel, (ClrSummary *)d_summary,
+                                         (cudaStream_t)cuda_stream);
+    if (r != 0 && c && d_summary && clearance_batch(N, p) > 0) {   // best effort: the pointer itself may be what was wrong
+        std::vector<isdf_clearance_summary> bad((size_t)clearance_batch(N, p), clearance_failed_summary());
+        cudaSetDevice(c->device);
+        cudaStreamSynchronize((cudaStream_t)cuda_stream);
+        cudaMemcpy(d_summary, bad.data(), sizeof(isdf_clearance_summary) * bad.size(), cudaMemcpyHostToDevice);
+        cudaGetLastError();
+    }
+    return r;
+}
+
+extern "C" int isdf_trajectory_clearance(isdf_ctx *c, int N, const double *T, const double *coeffs, const isdf_clearance_params *p,
+                                         double *sample_clearance, int64_t *sample_voxel, isdf_clearance_summary *summary) {
+    int r = clearance_check(c, N, p);
+    if (r == 0 && (!T || !coeffs || !summary)) r = fail(ISDF_ERR_INVALID, "NULL argument");
+    if (r) { clearance_poison_host(N, p, summary); return r; }
+    auto body = [&]() -> int {
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        const int B = clearance_batch(N, p);
+        const size_t S = (size_t)N * (p->samples_per_piece + 1);
+        CU_TRY(c->d_clr_in.ensure((size_t)19 * N));
+        CU_TRY(c->d_clr_clear.ensure(S)); CU_TRY(c->d_clr_vox.ensure(S)); CU_TRY(c->d_clr_sum.ensure((size_t)B));
+        CU_TRY(cudaMemcpyAsync(c->d_clr_in.p, coeffs, sizeof(double) * 18 * N, cudaMemcpyHostToDevice, c->stream));
+        CU_TRY(cudaMemcpyAsync(c->d_clr_in.p + 18 * (size_t)N, T, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
+        int rr = clearance_launch_ctx(c, N, c->d_clr_in.p + 18 * (size_t)N, c->d_clr_in.p, p, c->d_clr_clear.p, c->d_clr_vox.p, c->d_clr_sum.p, c->stream);
+        if (rr) return rr;
+        CU_TRY(cudaMemcpyAsync(summary, c->d_clr_sum.p, sizeof(isdf_clearance_summary) * B, cudaMemcpyDeviceToHost, c->stream));
+        if (sample_clearance) CU_TRY(cudaMemcpyAsync(sample_clearance, c->d_clr_clear.p, sizeof(double) * S, cudaMemcpyDeviceToHost, c->stream));
+        if (sample_voxel) CU_TRY(cudaMemcpyAsync(sample_voxel, c->d_clr_vox.p, sizeof(int64_t) * S, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaStreamSynchronize(c->stream));
+        return 0;
+    };
+    r = body();
+    if (r) clearance_poison_host(N, p, summary);
+    return r;
+}
+
 // ---- multi-GPU: rank-ordered sum of the sharded evaluation through NVLink peer memory (isdf_peer.cuh) ------------------------------
 static size_t peer_bytes(int world, int cap) { return sizeof(unsigned long long) * 2 * PEER_MAX + sizeof(double) * 2 * (size_t)world * cap; }
 
@@ -1533,6 +1657,13 @@ extern "C" int isdf_dbg_swept_stats(isdf_ctx *c, unsigned long long *out, long l
     if (!c || !out || (size_t)n > c->sv.d_dbg.n) return -1;
     cudaStreamSynchronize(c->stream);
     return cudaMemcpy(out, c->sv.d_dbg.p, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -3;
+}
+// {candidate pairs (voxel centre inside the H box), exact mesh searches} of the last clearance check
+extern "C" int isdf_dbg_clearance_counts(isdf_ctx *c, unsigned long long *out) {
+    if (!c || !out || !c->d_clr_counters.p) return -1;
+    cudaSetDevice(c->device);
+    cudaStreamSynchronize(c->stream);
+    return cudaMemcpy(out, c->d_clr_counters.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -1;
 }
 extern "C" int isdf_dbg_trace_stride(void) { return TRACE_STRIDE; }
 extern "C" int isdf_dbg_item_trace(isdf_ctx *c, unsigned long long *out, long long n) {

@@ -1,0 +1,31 @@
+// Translation unit of the trajectory clearance kernels (isdf_clearance.cuh): k_clearance_scan<0|1|2>, k_clearance_summary.
+// Compiled WITH FMA contraction and the division-free closest-point test, like the discrete path; a third unit of its own so that the
+// objects of the other two stay exactly what they are.
+#define ISDF_CLEARANCE_TU 1
+#define ISDF_FAST_TRI 1
+#include "../../include/isdf.h"
+#include "isdf_types.cuh"
+#include "isdf_clearance.cuh"
+
+namespace isdf {
+
+cudaError_t clearance_launch(const ClrArgs &A, int mode, unsigned grid, cudaStream_t st) {
+    if (mode == 2) k_clearance_scan<2><<<grid, CLR_THREADS, 0, st>>>(A);
+    else if (mode == 1) k_clearance_scan<1><<<grid, CLR_THREADS, 0, st>>>(A);
+    else k_clearance_scan<0><<<grid, CLR_THREADS, 0, st>>>(A);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    k_clearance_summary<<<(unsigned)(A.N / A.N0), CLR_SUM_THREADS, 0, st>>>(A);
+    return cudaGetLastError();
+}
+
+cudaError_t clearance_resident_blocks(int *blocks) {
+    int b0 = 0, b1 = 0, b2 = 0;
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b0, k_clearance_scan<0>, CLR_THREADS, 0);
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b1, k_clearance_scan<1>, CLR_THREADS, 0);
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b2, k_clearance_scan<2>, CLR_THREADS, 0);
+    *blocks = min(b0, min(b1, b2));
+    return e;
+}
+
+}  // namespace isdf

@@ -66,7 +66,7 @@ __device__ __forceinline__ void peer_allreduce_block(const PeerArgs &P, double *
     }
 }
 
-#ifndef ISDF_DISCRETE_TU   // instantiated once, in isdf_api.cu
+#if !defined(ISDF_DISCRETE_TU) && !defined(ISDF_CLEARANCE_TU)   // instantiated once, in isdf_api.cu
 __global__ void __launch_bounds__(512) k_peer_allreduce(const __grid_constant__ PeerArgs P, double *vec, int n) {
     peer_allreduce_block(P, vec, n);
 }

@@ -31,7 +31,8 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_gather_obstacle_points", "isdf_callback_batch", "isdf_callback_batch_device", "isdf_get_batch_trajectories",
                "isdf_lbfgs_default_params", "isdf_lbfgs_batch", "isdf_lbfgs_batch_device", "isdf_set_points_batch",
                "isdf_frontend_build_kernels", "isdf_frontend_get_kernels", "isdf_frontend_feasibility", "isdf_frontend_feasibility_device",
-               "isdf_frontend_check_batch", "isdf_peer_export", "isdf_peer_connect", "isdf_peer_allreduce_device", "isdf_peer_status", "isdf_peer_disconnect"]
+               "isdf_frontend_check_batch", "isdf_peer_export", "isdf_peer_connect", "isdf_peer_allreduce_device", "isdf_peer_status", "isdf_peer_disconnect",
+               "isdf_clearance_default_params", "isdf_trajectory_clearance", "isdf_trajectory_clearance_device"]
 
 
 class KernelConfig(C.Structure):
@@ -56,6 +57,20 @@ class LbfgsParams(C.Structure):
     """isdf_lbfgs_params"""
     _fields_ = [(n, C.c_int32) for n in ["mem_size", "past", "max_iterations", "max_linesearch", "max_rounds", "reserved_"]] + \
                [(n, C.c_double) for n in ["g_epsilon", "delta", "min_step", "max_step", "f_dec_coeff", "cautious_factor", "machine_prec"]]
+
+
+class ClearanceParams(C.Structure):
+    """isdf_clearance_params"""
+    _fields_ = [("samples_per_piece", C.c_int32), ("pieces_per_traj", C.c_int32), ("reach", C.c_double), ("margin", C.c_double)]
+
+
+class ClearanceSummary(C.Structure):
+    """isdf_clearance_summary (one per trajectory)"""
+    _fields_ = [("min_clearance", C.c_double), ("t_min", C.c_double), ("first_hit", C.c_double), ("voxel_min", C.c_int64),
+                ("piece_min", C.c_int32), ("sample_min", C.c_int32), ("colliding_samples", C.c_int32), ("collision_free", C.c_int32)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
 
 
 class Stats(C.Structure):
@@ -126,6 +141,9 @@ def load_library(path=None):
     lib.isdf_peer_status.argtypes = [vp]
     lib.isdf_peer_disconnect.argtypes = [vp]
     lib.isdf_eval_swept_given.argtypes = [vp, C.c_int, dp, dp, dp, dp, dp, dp, dp, dp]
+    lib.isdf_clearance_default_params.argtypes = [C.POINTER(ClearanceParams)]
+    lib.isdf_trajectory_clearance.argtypes = [vp, C.c_int, dp, dp, C.POINTER(ClearanceParams), dp, C.POINTER(C.c_int64), C.POINTER(ClearanceSummary)]
+    lib.isdf_trajectory_clearance_device.argtypes = [vp, C.c_int, vp, vp, C.POINTER(ClearanceParams), vp, vp, vp, vp]
     for s in ABI_SYMBOLS:
         if s != "isdf_last_error":
             getattr(lib, s).restype = C.c_int
@@ -300,6 +318,47 @@ class Evaluator:
         T, Cc, en = np.zeros(B * N0), np.zeros(18 * B * N0), np.zeros(B)
         self._check(self.lib.isdf_get_batch_trajectories(self.h, _dp(T), _dp(Cc), _dp(en)))
         return T, Cc, en
+
+    # ---- trajectory clearance check (see include/isdf.h) ----
+    def clearance_params(self, K_c=None, reach=None, margin=None, N0=0):
+        p = ClearanceParams()
+        self._check(self.lib.isdf_clearance_default_params(C.byref(p)))
+        if K_c is not None:
+            p.samples_per_piece = int(K_c)
+        if reach is not None:
+            p.reach = float(reach)
+            p.margin = float(reach) if margin is None else p.margin
+        if margin is not None:
+            p.margin = float(margin)
+        p.pieces_per_traj = int(N0)
+        return p
+
+    def trajectory_clearance(self, T, coeffs, K_c, reach, margin, N0=0):
+        """per-sample clearance (N*(K_c+1)), witness voxel addresses (int64, -1 = nothing within reach) and one summary dict per
+        trajectory (pieces b*N0 .. b*N0+N0-1; N0 = 0: a single trajectory)"""
+        T = _f64(T).reshape(-1)
+        N = T.size
+        Cc = _f64(coeffs).reshape(-1)
+        assert Cc.size == 18 * N
+        p = self.clearance_params(K_c, reach, margin, N0)
+        B = 1 if N0 == 0 else max(N // N0, 1)
+        clear, vox = np.zeros(N * (int(K_c) + 1)), np.zeros(N * (int(K_c) + 1), dtype=np.int64)
+        summ = (ClearanceSummary * B)()
+        self._check(self.lib.isdf_trajectory_clearance(self.h, N, _dp(T), _dp(Cc), C.byref(p), _dp(clear), vox.ctypes.data_as(C.POINTER(C.c_int64)), summ))
+        return clear, vox, [s.as_dict() for s in summ]
+
+    def trajectory_clearance_device(self, N, d_T, d_coeffs, params, d_clear, d_voxel, d_summary, stream=0):
+        """raw device pointers (e.g. torch .data_ptr()); d_summary holds N/N0 isdf_clearance_summary records (48 bytes each)"""
+        self._check(self.lib.isdf_trajectory_clearance_device(self.h, N, C.c_void_p(d_T), C.c_void_p(d_coeffs), C.byref(params), C.c_void_p(d_clear),
+                                                              C.c_void_p(d_voxel), C.c_void_p(d_summary), C.c_void_p(stream)))
+
+    def dbg_clearance_counts(self):
+        """{candidate pairs, exact mesh searches} of the last clearance check (isdf_dbg_clearance_counts, not part of include/isdf.h)"""
+        out = (C.c_ulonglong * 2)()
+        self.lib.isdf_dbg_clearance_counts.argtypes = [C.c_void_p, C.POINTER(C.c_ulonglong)]
+        if self.lib.isdf_dbg_clearance_counts(self.h, out) != 0:
+            raise IsdfError(-1, "isdf_dbg_clearance_counts failed")
+        return int(out[0]), int(out[1])
 
     # ---- front end: attitude kernels (see include/isdf.h) ----
     def frontend_build_kernels(self, max_roll=45.0, max_pitch=45.0, ang_res=9.0, front_end_safeh=0.0):

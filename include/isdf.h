@@ -200,6 +200,58 @@ int isdf_lbfgs_batch_device(isdf_ctx *ctx, int B, int N0, const double *d_head, 
                             const isdf_lbfgs_params *params, double *d_x, double *d_f, int32_t *d_ret, int32_t *d_iterations, int32_t *d_evaluations,
                             int32_t *rounds, void *cuda_stream);
 
+/* ---- trajectory clearance check: is a trajectory collision-free over the WHOLE map, and by how much? ------------------------------
+ * The reference has no working counterpart (SweptVolumeManager::isTrajCollide, swm:759-767, always returns false), and the cost terms
+ * cannot stand in for it: the hinge is smoothed and positive only inside safety_hor, the swept-volume term only sees the gathered obstacle
+ * list, the discrete term only the bd/2 box at its own sample spacing.
+ * Definition:
+ *   Samples. N pieces (T, coeffs in the layout of isdf_eval_discrete); piece i has K_c + 1 pose samples at local times j * step,
+ *     step = T_i * (1 / K_c), j = 0..K_c — the discrete path's pose: position of the piece polynomial, flatness quaternion, R = quat_rot(q).
+ *     Junction times are sampled twice (last sample of one piece, first of the next), as in the integral loop. The check is SAMPLED: nothing
+ *     is certified between two samples T_i / K_c apart.
+ *   Candidates of a sample: the occupied map voxels whose centre c (getGridCubeCenter) satisfies |R^T (c - x)|_inf <= H,
+ *     H = half_bd + reach, half_bd = kernel_size * occupancy_resolution / 2 (a strict > on any axis excludes, as hpp:800). Only voxels of
+ *     the map count: a window reaching past the map border is cut off there (no projInMap clamping).
+ *   clear(s) = min(reach, min over candidates of sdf(R^T (c - x))), sdf = getonlySDF of the shape (analytic: the closed form of
+ *     isdf_shape_query(..., ISDF_QUERY_SDF); mesh: s * dist in the context's sign mode).
+ *   Witness: the address ix*Y*Z + iy*Z + iz of the candidate realising the minimum when it is < reach (the smallest address among exact
+ *     ties), otherwise -1.
+ *   For SDFs that are true distances (exact-sign meshes, Ball) the H box loses nothing: every voxel closer than reach to a robot that fits
+ *     in the bd/2 box lies inside it. For the other analytic shapes and winding-sign meshes the box is part of the definition.
+ *   Trajectories: pieces b*N0 .. b*N0+N0-1 form trajectory b (N0 = 0: one trajectory of all N pieces). A sample's trajectory time is the
+ *     sum of the T of the earlier pieces of its trajectory, added in ascending order, plus j * step.
+ *   Summary per trajectory: min_clearance; the first sample in (piece, j) order attaining it — piece_min (index WITHIN the trajectory),
+ *     sample_min (= j), t_min (trajectory time), voxel_min (its witness); first_hit = trajectory time of the first sample with
+ *     clear < margin (-1 if none); colliding_samples = samples with clear < margin; collision_free = (colliding_samples == 0).
+ *   A sample whose pose is not finite has clearance NaN, counts as colliding, and makes its trajectory's min_clearance NaN.
+ * Results are deterministic: bit-identical run to run, through either entry point, and for a trajectory checked alone or inside a batch.
+ * Errors: ISDF_ERR_INVALID for bad parameters (K_c < 1, reach <= 0 or not finite, margin > reach, N % N0 != 0) and for a window wider than
+ * 1023 voxels per axis (2 H sqrt(3) / res + 4 > 1023); ISDF_ERR_STATE without a map or a shape; ISDF_ERR_UNSUPPORTED on a sharded context
+ * (isdf_set_shard world > 1). On failure every summary has min_clearance NaN and collision_free 0.
+ * Statistics: the call counts its launches in isdf_stats.kernel_launches and touches no other field. */
+typedef struct isdf_clearance_params {
+    int32_t samples_per_piece;   /* K_c >= 1 */
+    int32_t pieces_per_traj;     /* N0; 0 = one trajectory of N pieces; else N % N0 == 0 */
+    double reach;                /* > 0, finite: search bound and cap of every reported clearance */
+    double margin;               /* a sample collides when clear < margin; margin <= reach */
+} isdf_clearance_params;
+
+typedef struct isdf_clearance_summary {
+    double min_clearance, t_min, first_hit;        /* first_hit = -1 when collision-free */
+    int64_t voxel_min;                             /* -1 when nothing lies within reach */
+    int32_t piece_min, sample_min, colliding_samples, collision_free;
+} isdf_clearance_summary;
+
+/* K_c = integral_intervs of the default config, N0 = 0, reach = margin = safety_hor of the default config */
+int isdf_clearance_default_params(isdf_clearance_params *p);
+/* host buffers: sample_clearance / sample_voxel (N*(K_c+1), sample i*(K_c+1)+j) may be NULL; summary: N/N0 entries (1 for N0 = 0) */
+int isdf_trajectory_clearance(isdf_ctx *ctx, int N, const double *T, const double *coeffs, const isdf_clearance_params *p,
+                              double *sample_clearance, int64_t *sample_voxel, isdf_clearance_summary *summary);
+/* device-resident variant: every pointer on ctx's device (none may be NULL), asynchronous on cuda_stream (NULL = default stream) */
+int isdf_trajectory_clearance_device(isdf_ctx *ctx, int N, const double *d_T, const double *d_coeffs, const isdf_clearance_params *p,
+                                     double *d_sample_clearance, int64_t *d_sample_voxel, isdf_clearance_summary *d_summary,
+                                     void *cuda_stream);
+
 /* ---- multi-GPU reduction through NVLink / NVSwitch peer memory (optional; ncclAllReduce over the same 19N+1 doubles is the
  * library alternative). One process per GPU. Sequence on every rank:
  *   isdf_set_shard(ctx, rank, world); isdf_peer_export(ctx, world, max_doubles, h) -> all-gather the 64-byte handles ->
