@@ -24,7 +24,7 @@ __global__ void k_mesh_cells(const __grid_constant__ DevMesh M, int nx, int ny, 
                              float *dist, uint32_t *seed);
 
 __global__ void k_mesh_cell_lists(const __grid_constant__ DevMesh M, long long ncell, double hd, double list_reach, uint16_t *cnt,
-                                  const uint32_t *off, uint32_t *cand);
+                                  const uint32_t *off, uint32_t *cand, float *cand_lb);
 __global__ void k_mesh_cell_pack(long long ncell, const float *dist, const uint32_t *seed, const uint32_t *off, const uint16_t *cnt, uint4 *rec);
 
 static thread_local std::string g_err;
@@ -52,7 +52,7 @@ struct isdf_ctx {
     // shape
     bool have_shape = false;
     DevShape shape;
-    DevBuf<BvhNode> d_nodes; DevBuf<WideNode> d_wnodes; DevBuf<double> d_tris, d_pn, d_obb; DevBuf<float> d_cell_dist; DevBuf<uint32_t> d_cell_seed, d_cell_off, d_cand; DevBuf<uint16_t> d_cell_cnt; DevBuf<uint4> d_cell_rec; DevBuf<WnNode> d_wn;
+    DevBuf<BvhNode> d_nodes; DevBuf<WideNode> d_wnodes; DevBuf<double> d_tris, d_pn, d_obb; DevBuf<float> d_cell_dist; DevBuf<uint32_t> d_cell_seed, d_cell_off, d_cand; DevBuf<float> d_cand_lb; DevBuf<uint16_t> d_cell_cnt; DevBuf<uint4> d_cell_rec; DevBuf<WnNode> d_wn;
     double mesh_list_reach = 0;  // radius (cell-centre distance) up to which cells got candidate lists (isdf_dbg_mesh_grid)
     // evaluation scratch
     DevBuf<double> d_T, d_C, d_out, d_piece_cost;
@@ -183,7 +183,7 @@ extern "C" int isdf_destroy(isdf_ctx *c) {
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
     if (c->aux_stream) cudaStreamSynchronize(c->aux_stream);
-    c->d_bits.release(); c->d_nodes.release(); c->d_wnodes.release(); c->d_tris.release(); c->d_pn.release(); c->d_obb.release(); c->d_cell_dist.release(); c->d_cell_seed.release(); c->d_cell_off.release(); c->d_cand.release(); c->d_cell_cnt.release(); c->d_cell_rec.release(); c->d_wn.release();
+    c->d_bits.release(); c->d_nodes.release(); c->d_wnodes.release(); c->d_tris.release(); c->d_pn.release(); c->d_obb.release(); c->d_cell_dist.release(); c->d_cell_seed.release(); c->d_cell_off.release(); c->d_cand.release(); c->d_cand_lb.release(); c->d_cell_cnt.release(); c->d_cell_rec.release(); c->d_wn.release();
     c->d_T.release(); c->d_C.release(); c->d_out.release(); c->d_piece_cost.release();
     c->d_tickets.release(); c->d_counter.release(); c->d_items.release(); c->d_item_count.release(); c->d_tot.release(); c->d_split_done.release(); c->d_work.release(); c->d_split_work.release(); c->d_subsum.release(); c->d_dbg.release(); c->d_trace.release();
     for (int p = 0; p < PEER_MAX; p++) if (c->peer_open[p]) cudaIpcCloseMemHandle(c->peer_open[p]);
@@ -319,7 +319,7 @@ extern "C" int isdf_set_shape_mesh_ex(isdf_ctx *c, const double *V, int nV, cons
     {
         DevMesh build = m;
         build.gdim[0] = 0;            // no grid while it is being built: plain unbounded BVH queries
-        build.cell_dist = nullptr; build.cell_seed = nullptr; build.cell_off = nullptr; build.cell_cnt = nullptr; build.cand = nullptr;
+        build.cell_dist = nullptr; build.cell_seed = nullptr; build.cell_off = nullptr; build.cell_cnt = nullptr; build.cand = nullptr; build.cand_lb = nullptr;
         k_mesh_cells<<<(unsigned)((ncell + 127) / 128), 128, 0, c->stream>>>(build, m.gdim[0], m.gdim[1], m.gdim[2], m.glo[0], m.glo[1], m.glo[2],
                                                                            m.gcell, c->d_cell_dist.p, c->d_cell_seed.p);
         c->stats.kernel_launches++;
@@ -327,7 +327,7 @@ extern "C" int isdf_set_shape_mesh_ex(isdf_ctx *c, const double *V, int nV, cons
         CU_TRY(cudaStreamSynchronize(c->stream));
     }
     m.cell_dist = c->d_cell_dist.p; m.cell_seed = c->d_cell_seed.p;
-    m.cell_off = nullptr; m.cell_cnt = nullptr; m.cand = nullptr;
+    m.cell_off = nullptr; m.cell_cnt = nullptr; m.cand = nullptr; m.cand_lb = nullptr;
     // exact candidate lists for every cell a query can land in and not be settled by the cell's distance bracket alone: the discrete
     // path queries within safety_hor of the surface, the swept-volume path within its range bound 2*safety_hor + 0.1 (swm:383) — a
     // flat pass over ~100 listed triangles answers such a query in a tenth of the time of a far-field tree search, and the sign
@@ -338,7 +338,7 @@ extern "C" int isdf_set_shape_mesh_ex(isdf_ctx *c, const double *V, int nV, cons
         c->mesh_list_reach = list_reach;
         CU_TRY(c->d_cell_cnt.ensure(ncell)); CU_TRY(c->d_cell_off.ensure(ncell));
         const unsigned warps_grid = (unsigned)((ncell + 3) / 4);
-        k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->d_cell_cnt.p, nullptr, nullptr);
+        k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->d_cell_cnt.p, nullptr, nullptr, nullptr);
         c->stats.kernel_launches++;
         CU_TRY(cudaGetLastError());
         std::vector<uint16_t> cnt(ncell);
@@ -348,18 +348,18 @@ extern "C" int isdf_set_shape_mesh_ex(isdf_ctx *c, const double *V, int nV, cons
         size_t total = 0;
         for (size_t i = 0; i < ncell; i++) { off[i] = (uint32_t)total; total += cnt[i]; }
         if (total > 0 && total < (1ull << 31)) {
-            CU_TRY(c->d_cand.ensure(total));
+            CU_TRY(c->d_cand.ensure(total)); CU_TRY(c->d_cand_lb.ensure(total));
             CU_TRY(cudaMemcpyAsync(c->d_cell_off.p, off.data(), sizeof(uint32_t) * ncell, cudaMemcpyHostToDevice, c->stream));
-            k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->d_cell_cnt.p, c->d_cell_off.p, c->d_cand.p);
+            k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->d_cell_cnt.p, c->d_cell_off.p, c->d_cand.p, c->d_cand_lb.p);
             c->stats.kernel_launches++;
             CU_TRY(cudaGetLastError());
             CU_TRY(cudaStreamSynchronize(c->stream));
-            m.cell_off = c->d_cell_off.p; m.cell_cnt = c->d_cell_cnt.p; m.cand = c->d_cand.p;
+            m.cell_off = c->d_cell_off.p; m.cell_cnt = c->d_cell_cnt.p; m.cand = c->d_cand.p; m.cand_lb = c->d_cand_lb.p;
         }
         if (getenv("ISDF_VERBOSE")) {
             size_t listed = 0; for (size_t i = 0; i < ncell; i++) listed += cnt[i] != 0;
-            fprintf(stderr, "[isdf] mesh cell grid %d x %d x %d (cell %.3f m), %zu cells with a candidate list, %zu candidates (%.1f MB)\n", m.gdim[0], m.gdim[1], m.gdim[2],
-                    m.gcell, listed, total, total * 4e-6);
+            fprintf(stderr, "[isdf] mesh cell grid %d x %d x %d (cell %.3f m), %zu cells with a candidate list, %zu candidates (%.1f MB: ids and lower bounds)\n", m.gdim[0], m.gdim[1],
+                    m.gdim[2], m.gcell, listed, total, total * 8e-6);
         }
     }
     // fused 16-byte cell records for the discrete scan kernel's cull stage
@@ -399,11 +399,14 @@ __global__ void k_mesh_cells(const __grid_constant__ DevMesh M, int nx, int ny, 
 }
 
 // Candidate lists (one warp per cell). Pass 1 (cand == nullptr): count the triangles within d_c + 2 hd of the cell centre and
-// store the count (0 for cells that are too far, too deep or whose list would exceed LIST_CAP). Pass 2: fill the lists.
+// store the count (0 for cells that are too far, too deep or whose list would exceed LIST_CAP). Pass 2: fill the lists, sorted by
+// ascending distance from the cell centre (ties: triangle index), with each distance's lower bound in cand_lb.
 constexpr int LIST_CAP = MESH_LIST_CAP;
 __global__ void __launch_bounds__(128) k_mesh_cell_lists(const __grid_constant__ DevMesh M, long long ncell, double hd, double list_reach,
-                                                         uint16_t *cnt, const uint32_t *off, uint32_t *cand) {
+                                                         uint16_t *cnt, const uint32_t *off, uint32_t *cand, float *cand_lb) {
     __shared__ WideStack stk[4];
+    __shared__ double s_d2[4][LIST_CAP];   // pass 2: the cell's hits in emission order, then ranked
+    __shared__ int s_tri[4][LIST_CAP];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const long long cell = (long long)blockIdx.x * 4 + warp;
     if (cell >= ncell) return;
@@ -419,12 +422,32 @@ __global__ void __launch_bounds__(128) k_mesh_cell_lists(const __grid_constant__
     const unsigned lt_mask = (1u << lane) - 1u;
     int n = 0;
     const uint32_t base = cand ? off[cell] : 0u;
-    wide_range(M, ctr, R * R, lane, &stk[warp], [&](bool hit, int t) {
+    wide_range(M, ctr, R * R, lane, &stk[warp], [&](bool hit, int t, double d2) {
         const unsigned bal = __ballot_sync(0xffffffffu, hit);
-        if (cand && hit) cand[base + n + __popc(bal & lt_mask)] = (uint32_t)t;
+        const int slot = n + __popc(bal & lt_mask);
+        if (cand && hit && slot < LIST_CAP) { s_d2[warp][slot] = d2; s_tri[warp][slot] = t; }
         n += __popc(bal);
     });
-    if (cand == nullptr && lane == 0) cnt[cell] = (n <= LIST_CAP) ? (uint16_t)n : (uint16_t)0;
+    if (cand == nullptr) {
+        if (lane == 0) cnt[cell] = (n <= LIST_CAP) ? (uint16_t)n : (uint16_t)0;
+        return;
+    }
+    // rank sort: entry i goes to the number of entries before it in (squared distance, triangle) order
+    __syncwarp();
+    n = min(n, LIST_CAP);
+    for (int i = lane; i < n; i += 32) {
+        const double di = s_d2[warp][i];
+        const int ti = s_tri[warp][i];
+        int rank = 0;
+        for (int j = 0; j < n; j++) {
+            const double dj = s_d2[warp][j];
+            rank += (dj < di || (dj == di && s_tri[warp][j] < ti)) ? 1 : 0;
+        }
+        cand[base + rank] = (uint32_t)ti;
+        // lower bound of the exact distance: relative and absolute slack for the rounding of the FP64 closest-point test, then rounded
+        // down to float (monotone in di, so the bounds are non-decreasing along the list)
+        cand_lb[base + rank] = __double2float_rd(fmax(sqrt(di) * (1.0 - 1e-9) - 1e-12, 0.0));
+    }
 }
 
 __global__ void k_shape_query(const __grid_constant__ DevShape S, const double *p, int n, double *sdf, double *grad, int what) {
@@ -1651,6 +1674,29 @@ extern "C" int isdf_dbg_mesh_grid(isdf_ctx *c, double *geom, int32_t *gdim, floa
         if (!m.cell_cnt) std::memset(cell_cnt, 0, sizeof(uint16_t) * ncell);
         else if (cudaMemcpy(cell_cnt, m.cell_cnt, sizeof(uint16_t) * ncell, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
     }
+    return 0;
+}
+// the current mesh's candidate lists, so tests can check their order and bounds: sizes = {candidates, triangles}; cell_off (one per
+// cell, as isdf_dbg_mesh_grid), cand / cand_lb (sizes[0] each) and tris (the leaf-order triangle records, 16 doubles each) are
+// optional — call with NULL first to size them.
+extern "C" int isdf_dbg_mesh_lists(isdf_ctx *c, long long *sizes, uint32_t *cell_off, uint32_t *cand, float *cand_lb, double *tris) {
+    if (!c || !sizes) return -1;
+    if (!c->have_shape || c->shape.kind != ISDF_SHAPE_MESH) return -2;
+    const DevMesh &m = c->shape.mesh;
+    const size_t ncell = (size_t)m.gdim[0] * m.gdim[1] * m.gdim[2];
+    if (cudaSetDevice(c->device) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) return -3;
+    size_t total = 0;
+    if (m.cand) {   // the last cell's offset + count
+        uint32_t off_last = 0; uint16_t cnt_last = 0;
+        if (cudaMemcpy(&off_last, m.cell_off + ncell - 1, sizeof(uint32_t), cudaMemcpyDeviceToHost) != cudaSuccess ||
+            cudaMemcpy(&cnt_last, m.cell_cnt + ncell - 1, sizeof(uint16_t), cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+        total = (size_t)off_last + cnt_last;
+    }
+    sizes[0] = (long long)total; sizes[1] = m.ntris;
+    if (cell_off && m.cand && cudaMemcpy(cell_off, m.cell_off, sizeof(uint32_t) * ncell, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (cand && total && cudaMemcpy(cand, m.cand, sizeof(uint32_t) * total, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (cand_lb && total && cudaMemcpy(cand_lb, m.cand_lb, sizeof(float) * total, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (tris && cudaMemcpy(tris, m.tris, sizeof(double) * TRI_STRIDE * (size_t)m.ntris, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
     return 0;
 }
 extern "C" int isdf_dbg_swept_stats(isdf_ctx *c, unsigned long long *out, long long n) {

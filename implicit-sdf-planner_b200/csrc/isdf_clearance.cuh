@@ -151,10 +151,12 @@ __global__ void __launch_bounds__(CLR_THREADS) k_clearance_scan(const __grid_con
                     // bounded search: nothing within the bound means sdf >= bound (outside) — the relative widening keeps exact ties answerable
                     if (Mh.sign_radius > 0.0) reach_q = fmax(bv, Mh.sign_radius) * (1.0 + 1e-12);
                 }
-                const int first_id = (cnt != 0 && lane < cnt) ? (int)__ldg(Mh.cand + v.off + lane) : -1;
+                const bool has = cnt != 0 && lane < cnt;
+                const int first_id = has ? (int)__ldg(Mh.cand + v.off + lane) : -1;
+                const float first_lb = has ? __ldg(Mh.cand_lb + v.off + lane) : 0.0f;
                 double d2; d3 c = mk3(0, 0, 0); int tri, feat;
                 nsearch++;
-                if (!mesh_search_rec(Mh, p, reach_q, lane, &sm.stk, cnt, v.off, first_id, (int)v.seed, (v.cnt >> 31) != 0u, d2, c, tri, feat)) continue;
+                if (!mesh_search_rec(Mh, p, reach_q, lane, &sm.stk, cnt, v.off, first_id, first_lb, (int)v.seed, (v.cnt >> 31) != 0u, d2, c, tri, feat)) continue;
                 d3 g;
                 const double sdf = mesh_finish_t<MODE == 2>(Mh, p, p - c, d2, tri, feat, g);
                 if (clr_better(sdf, v.addr, bv, ba)) { bv = sdf; ba = v.addr; }

@@ -23,8 +23,9 @@
 //     difference SDF evaluations of getSDFwithGrad1 (Shape.hpp:58-87). Evaluating those only for active voxels is exact
 //     because an inactive voxel contributes nothing (hpp:809-821);
 //   * k_discrete_mesh — voxels that survive the exact culls (body-frame box, inflated mesh AABB, per-cell distance lower
-//     bound) are answered by WARP-COOPERATIVE nearest-triangle searches (the cell's exact candidate list near the surface, 64
-//     candidates per pass with a division-free closest-point test; elsewhere the 32-ary tree seeded with the cell's nearest
+//     bound) are answered by WARP-COOPERATIVE nearest-triangle searches (the cell's exact candidate list near the surface, 32
+//     candidates per pass with a division-free closest-point test, pruned by the list's sorted distance bounds and, with an exact
+//     sign, by safety_hor; elsewhere the 32-ary tree seeded with the cell's nearest
 //     triangle); sign, gradient, hinge and pose chain rule of the answered voxels are DEFERRED and evaluated one voxel per lane;
 //     the warp-uniform pose (position, rotation, quaternion) lives in shared memory, not in 16 x 2 registers of every lane;
 //   * k_discrete_epilogue — the per-sample chain rule (penalties, flatness adjoint, beta-basis outer products) as one THREAD
@@ -71,7 +72,8 @@ struct DiscArgs {
     unsigned long long *pair_counter;  // may be null
     double *count_out;                 // host entry point only: the pair count (bit pattern) lands behind the result vector, one D2H copy fetches both
     unsigned long long *dbg;           // may be null: per sample {cycles, pairs, work}
-    unsigned long long *trace;         // may be null: per work-item slot {begin, end} in ns of the global timer (+ 6 phase cycle counts with -DISDF_PHASE_TIMING)
+    unsigned long long *trace;         // may be null: per work-item slot {begin, end} in ns of the global timer (+ 4 phase cycle counts, total
+                                       // cycles, queries | pairs and triangle records tested with -DISDF_PHASE_TIMING)
     const int *items;                  // may be null: 3 ints per work item {local sample m, -1 = all classes or c0 | c1 << 8, split slot or -1}
     const int *item_count;             // number of valid items (device)
     int *item_cursor;                  // persistent warps draw items from this counter (zero on entry; the epilogue zeroes it again)
@@ -266,7 +268,7 @@ __device__ __forceinline__ void sample_epilogue(const DiscArgs &A, int i, int j,
 struct Item { int s, c0, c1, hslot, slot; };
 __device__ __forceinline__ unsigned long long global_ns() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
 #ifdef ISDF_PHASE_TIMING
-constexpr int TRACE_STRIDE = 8;
+constexpr int TRACE_STRIDE = 9;
 #define ISDF_PT(x) x
 #else
 constexpr int TRACE_STRIDE = 2;
@@ -530,7 +532,8 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
         const int i = s / (K + 1), j = s - i * (K + 1);
         const long long t_begin = A.dbg ? clock64() : 0;
         if (A.trace && lane == 0) A.trace[TRACE_STRIDE * (size_t)it.slot] = global_ns();
-        ISDF_PT(long long pt_pose = 0; long long pt_cull = 0; long long pt_search = 0; long long pt_tail = 0; long long pt_t0 = clock64(); long long pt_all0 = pt_t0;)
+        ISDF_PT(long long pt_pose = 0; long long pt_cull = 0; long long pt_search = 0; long long pt_tail = 0; long long pt_t0 = clock64(); long long pt_all0 = pt_t0;
+                if (lane == 0) sm.stk.tested = 0u; __syncwarp();)
         unsigned npairs = 0, nquery = 0;
         const bool whole = (it.c1 - it.c0) == ROW_CLASSES;
 
@@ -637,21 +640,25 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
             auto search_all = [&](bool final) __attribute__((always_inline)) {
                 ISDF_PT(const long long pt_a = clock64(); const long long pt_tail0 = pt_tail;)
                 nquery += nsv;
-                auto first_ids = [&](int k) -> int {
-                    if (k >= nsv) return -1;
-                    const uint32_t cnt = sm.sv[k].cnt & 0x7fffffffu;
-                    return (lane < (int)cnt) ? (int)__ldg(Mh.cand + sm.sv[k].off + lane) : -1;
+                auto first_ids = [&](int k, int &id, float &lb) {   // first-pass candidate and its lower bound
+                    id = -1; lb = 0.0f;
+                    if (k >= nsv) return;
+                    const uint32_t cnt = sm.sv[k].cnt & 0x7fffffffu, off = sm.sv[k].off;
+                    if (lane < (int)cnt) { id = (int)__ldg(Mh.cand + off + lane); lb = __ldg(Mh.cand_lb + off + lane); }
                 };
-                int ids0 = first_ids(0), ids1 = first_ids(1);
+                int ids0, ids1;
+                float lbs0, lbs1;
+                first_ids(0, ids0, lbs0); first_ids(1, ids1, lbs1);
                 int k = 0;
                 do {
                     if (k < nsv) {
-                        const int ids2 = first_ids(k + 2);
+                        int ids2; float lbs2;
+                        first_ids(k + 2, ids2, lbs2);
                         const Survivor &v = sm.sv[k];
                         const d3 p = mk3(v.px, v.py, v.pz);
                         const uint32_t cnt_in = v.cnt, qcode = v.code;
                         double d2; d3 c = mk3(0, 0, 0); int tri, feat;
-                        if (mesh_search_rec(Mh, p, sf, lane, &sm.stk, (int)(cnt_in & 0x7fffffffu), v.off, ids0, (int)v.seed, (cnt_in >> 31) != 0u, d2, c, tri, feat)) {
+                        if (mesh_search_rec(Mh, p, sf, lane, &sm.stk, (int)(cnt_in & 0x7fffffffu), v.off, ids0, lbs0, (int)v.seed, (cnt_in >> 31) != 0u, d2, c, tri, feat)) {
                             if (lane == 0) {
                                 QRes r;
                                 r.ex = p.x - c.x; r.ey = p.y - c.y; r.ez = p.z - c.z; r.tri = tri; r.code = qcode;
@@ -660,7 +667,7 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
                             }
                             nres++;
                         }
-                        ids0 = ids1; ids1 = ids2;
+                        ids0 = ids1; ids1 = ids2; lbs0 = lbs1; lbs1 = lbs2;
                     }
                     k++;
                     if (nres == 32 || (final && k >= nsv && nres > 0)) flush_tails();   // the only call site
@@ -780,7 +787,7 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
         if (A.trace && lane == 0) {
             unsigned long long *tr = A.trace + TRACE_STRIDE * (size_t)it.slot;
             tr[1] = global_ns();
-            ISDF_PT(tr[2] = pt_pose; tr[3] = pt_cull; tr[4] = pt_search; tr[5] = pt_tail; tr[6] = clock64() - pt_all0; tr[7] = ((unsigned long long)nquery << 32) | npairs;)
+            ISDF_PT(tr[2] = pt_pose; tr[3] = pt_cull; tr[4] = pt_search; tr[5] = pt_tail; tr[6] = clock64() - pt_all0; tr[7] = ((unsigned long long)nquery << 32) | npairs; tr[8] = sm.stk.tested;)
         }
         __syncwarp();
     }

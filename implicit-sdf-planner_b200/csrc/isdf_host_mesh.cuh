@@ -28,7 +28,7 @@ struct HostMesh {
     double blo[3] = {0, 0, 0}, bhi[3] = {0, 0, 0};
     DevMesh view() const {  // host pointers; same code path as the device for the bitmap construction
         DevMesh m;
-        m.nodes = nodes.data(); m.wnodes = wnodes.data(); m.tris = tris.data(); m.pnormals = pnormals.data(); m.leaf_obb = leaf_obb.empty() ? nullptr : leaf_obb.data(); m.cell_dist = nullptr; m.cell_seed = nullptr; m.cell_off = nullptr; m.cell_cnt = nullptr; m.cand = nullptr; m.cell_rec = nullptr;
+        m.nodes = nodes.data(); m.wnodes = wnodes.data(); m.tris = tris.data(); m.pnormals = pnormals.data(); m.leaf_obb = leaf_obb.empty() ? nullptr : leaf_obb.data(); m.cell_dist = nullptr; m.cell_seed = nullptr; m.cell_off = nullptr; m.cell_cnt = nullptr; m.cand = nullptr; m.cand_lb = nullptr; m.cell_rec = nullptr;
         m.sign_mode = sign_mode; m.wn = wn.empty() ? nullptr : wn.data(); m.wn_beta2 = wn_beta2;
         m.ntris = ntris;
         for (int a = 0; a < 3; a++) { m.gdim[a] = gdim[a]; m.glo[a] = glo[a]; m.blo[a] = blo[a]; m.bhi[a] = bhi[a]; }

@@ -58,7 +58,11 @@ struct DevMesh {
     // query in such a cell is a flat, traversal-free loop over it; cell_cnt == 0 means "search the tree" (far or deep cells).
     const uint32_t *cell_off;   // offset into cand
     const uint16_t *cell_cnt;   // number of candidates (0 = no list)
-    const uint32_t *cand;       // triangle indices (leaf order)
+    const uint32_t *cand;       // triangle indices (leaf order), each list sorted by ascending distance from the cell centre (ties: index)
+    // parallel to cand: a float lower bound of dist(cell centre, triangle), non-decreasing along each list. A query point p at
+    // distance r from the centre is at least cand_lb[k] - r from triangle cand[k] (1-Lipschitz), so once that exceeds the best
+    // distance found so far the triangle — and, the list being sorted, every later one — cannot be the closest
+    const float *cand_lb;
     // the same four per-cell values fused into one 16-byte record {float bits of cell_dist, cell_seed, cell_off, cell_cnt}: the
     // discrete scan kernel's cull stage fetches it with ONE 128-bit load and hands offset / count / seed to the search, instead
     // of three dependent loads per query (packed by k_mesh_cell_pack at isdf_set_shape_mesh time; may be null)
@@ -341,7 +345,18 @@ __host__ __device__ inline double mesh_sdf_grad(const DevMesh &M, d3 p, double r
 // `stk` is a per-warp shared-memory scratch of WIDE_STACK (node, d2) pairs.
 constexpr int WIDE_STACK = 96;
 // the stacked bounds are floats ROUNDED DOWN: still lower bounds, so pruning stays exact (a node is at worst opened needlessly)
-struct WideStack { int node[WIDE_STACK]; float d2[WIDE_STACK]; int leaf[32]; float leaf_d2[32]; };
+struct WideStack {
+    int node[WIDE_STACK]; float d2[WIDE_STACK]; int leaf[32]; float leaf_d2[32];
+#ifdef ISDF_PHASE_TIMING
+    unsigned tested;   // triangle records tested by mesh_search_rec (diagnostic build only)
+#endif
+};
+#ifdef ISDF_PHASE_TIMING
+// every lane of the warp passes the number of records it tested since the last count
+#define ISDF_COUNT_TESTED(stk, n) do { const unsigned n_ = __reduce_add_sync(0xffffffffu, (unsigned)(n)); if ((stk) && (threadIdx.x & 31) == 0) (stk)->tested += n_; } while (0)
+#else
+#define ISDF_COUNT_TESTED(stk, n) do { (void)(n); } while (0)
+#endif
 
 __device__ __forceinline__ double wide_closest(const DevMesh &M, d3 p, double bound2, int seed, d3 &cbest, int &tri, int &feat,
                                                int lane, WideStack *stk) {
@@ -356,6 +371,7 @@ __device__ __forceinline__ double wide_closest(const DevMesh &M, d3 p, double bo
         const double dd = dot3(e, e);
         if (dd < best) { best = dd; cbest = q; tri = seed; feat = f; }
     }
+    ISDF_COUNT_TESTED(stk, seed >= 0 && lane == 0);
     int sp = 0;
     int cur = 0; double cur_d2 = 0.0;
     for (;;) {
@@ -385,9 +401,11 @@ __device__ __forceinline__ double wide_closest(const DevMesh &M, d3 p, double bo
             for (int base = 0; base < nleaf; base += 8) {
                 const int idx = base + (lane >> 2), slot = lane & 3;
                 double dd = 1e300; d3 q = mk3(0, 0, 0); int f = 0, t = -1;
+                [[maybe_unused]] int ntest = 0;   // records tested (ISDF_PHASE_TIMING builds)
                 if (idx < nleaf && (double)stk->leaf_d2[idx] < best) {
                     const int code = ~stk->leaf[idx];
                     const int first = code >> 3, cnt = (code & 7) + 1;
+                    ntest = (cnt - slot + 3) >> 2;
                     for (int k = slot; k < cnt; k += 4) {   // leaves of up to 8 triangles: slots take triangle k and k+4
                         const double *T = M.tris + TRI_STRIDE * (size_t)(first + k);
                         int ff;
@@ -397,6 +415,7 @@ __device__ __forceinline__ double wide_closest(const DevMesh &M, d3 p, double bo
                         if (d < dd) { dd = d; q = qq; f = ff; t = first + k; }
                     }
                 }
+                ISDF_COUNT_TESTED(stk, ntest);
                 // arg-min: 32-bit order-preserving key (float rounded down) + one REDUX; exact tie-break among equal keys
                 const bool cand = dd < best;
                 const unsigned key = cand ? __float_as_uint(__double2float_rd(dd)) : 0xffffffffu;
@@ -439,8 +458,9 @@ __device__ __forceinline__ double wide_closest(const DevMesh &M, d3 p, double bo
     }
 }
 
-// Warp-cooperative range query on the 32-ary tree: calls emit(valid, tri) for every triangle whose exact distance to c is
-// <= sqrt(R2), 32 triangles per call (lanes without one pass valid = false). Used to build the per-cell candidate lists.
+// Warp-cooperative range query on the 32-ary tree: calls emit(valid, tri, d2) for every triangle whose exact distance to c is
+// <= sqrt(R2) (d2: its squared distance), 32 triangles per call (lanes without one pass valid = false). Used to build the per-cell
+// candidate lists.
 template <class Emit>
 __device__ __forceinline__ void wide_range(const DevMesh &M, d3 c, double R2, int lane, WideStack *stk, Emit &&emit) {
     const unsigned lt_mask = (1u << lane) - 1u;
@@ -460,6 +480,7 @@ __device__ __forceinline__ void wide_range(const DevMesh &M, d3 c, double R2, in
         for (int base = 0; base < nleaf; base += 4) {      // 4 leaves x 8 triangle slots
             const int idx = base + (lane >> 3), slot = lane & 7;
             bool hit = false; int t = -1;
+            double d2 = 0.0;
             if (idx < nleaf) {
                 const int code = ~stk->leaf[idx];
                 const int first = code >> 3, cnt = (code & 7) + 1;
@@ -469,10 +490,11 @@ __device__ __forceinline__ void wide_range(const DevMesh &M, d3 c, double R2, in
                     int ff;
                     const d3 q = tri_closest_rec(c, T, ff);
                     const d3 e = c - q;
-                    hit = dot3(e, e) <= R2;
+                    d2 = dot3(e, e);
+                    hit = d2 <= R2;
                 }
             }
-            emit(hit, t);
+            emit(hit, t, d2);
         }
         unsigned imask = __ballot_sync(0xffffffffu, alive && ch >= 0);
         while (imask) {
@@ -515,34 +537,64 @@ __device__ __forceinline__ void warp_argmin_update(double dd, d3 q, int t, int f
 
 // Warp-cooperative nearest triangle from a cell's candidate list: lanes test 32 candidates per pass, REDUX arg-min.
 // (Two candidates per lane and pass — a second independent chain — was measured slower.)
-__device__ __forceinline__ double list_closest_range(const DevMesh &M, d3 p, uint32_t off, int cnt, d3 &cbest, int &tri, int &feat, int lane);
-__device__ __forceinline__ double list_closest_pre(const DevMesh &M, d3 p, uint32_t off, int cnt, int first_id, d3 &cbest, int &tri, int &feat, int lane);
-__device__ __forceinline__ double list_closest(const DevMesh &M, d3 p, int cell, d3 &cbest, int &tri, int &feat, int lane) {
-    return list_closest_range(M, p, M.cell_off[cell], (int)M.cell_cnt[cell], cbest, tri, feat, lane);
+//
+// The pass is pruned with the lists' lower bounds (DevMesh::cand_lb). p lies within r_up of the centre of the cell whose list this
+// is, so candidate k is at least cand_lb[k] - r_up away from p. A lane whose bound already exceeds the best distance found so far
+// skips its candidate (no 128-byte record load, no test), and since each list is sorted by that bound the warp stops as soon as the
+// first candidate of the next pass is ruled out. The bounds carry slack for rounding and the test is strict, so a candidate exactly
+// tied with the best is still tested and the arg-min's tie rule decides as it would without pruning.
+__device__ __forceinline__ bool list_lb_prunes(float lb, double r_up, double best) {
+    const double g = (double)lb - r_up;
+    return g > 0.0 && g * g > best;
 }
-__device__ __forceinline__ double list_closest_range(const DevMesh &M, d3 p, uint32_t off, int cnt, d3 &cbest, int &tri, int &feat, int lane) {
-    return list_closest_pre(M, p, off, cnt, (lane < cnt) ? (int)__ldg(M.cand + off + lane) : -1, cbest, tri, feat, lane);
+// upper bound of |p - c| for the centre c of cell (ix, iy, iz): the lists were built in a translation unit without FMA contraction
+// and the scan kernels contract, so the two may round c differently by an ulp
+__device__ __forceinline__ double list_centre_dist_up(const DevMesh &M, d3 p, double ix, double iy, double iz) {
+    const d3 e = mk3(p.x - (M.glo[0] + (ix + 0.5) * M.gcell), p.y - (M.glo[1] + (iy + 0.5) * M.gcell), p.z - (M.glo[2] + (iz + 0.5) * M.gcell));
+    return sqrt(dot3(e, e)) * (1.0 + 1e-9) + 1e-12;
 }
-// first_id: this lane's candidate of the FIRST pass (cand[off + lane], -1 beyond the list) — the caller may have loaded it long
-// before (software pipelining across queries); the ids of every following pass are requested one pass ahead.
-__device__ __forceinline__ double list_closest_pre(const DevMesh &M, d3 p, uint32_t off, int cnt, int first_id, d3 &cbest, int &tri, int &feat, int lane) {
-    double best = 1e300;
+// first_id / first_lb: this lane's candidate of the FIRST pass and its bound (cand[off + lane], cand_lb[off + lane]; -1 beyond the
+// list) — the caller may have loaded them long before (software pipelining across queries); those of every following pass are
+// requested one pass ahead. r_up: list_centre_dist_up of p and the list's cell. bound2 seeds the best squared distance: when no
+// candidate is closer, tri = -1 (and the returned value is not a distance).
+__device__ __forceinline__ double list_closest_pre(const DevMesh &M, d3 p, uint32_t off, int cnt, int first_id, float first_lb, double r_up,
+                                                   double bound2, d3 &cbest, int &tri, int &feat, int lane, WideStack *tally = nullptr) {
+    // the list's first candidate is the triangle nearest to the cell centre, so p's closest triangle lies within that distance plus
+    // r_up: an upper bound (the slack undoes the bound's round-down) that prunes the first pass too. No candidate is returned unless
+    // it is below bound2, and the closest one always is below this bound, so starting from the smaller of the two changes no answer.
+    const double ub = (double)__shfl_sync(0xffffffffu, first_lb, 0) * (1.0 + 1e-6) + 1e-9 + r_up;
+    double best = fmin(bound2, ub * ub);
     tri = -1; feat = 0;
     int t = first_id;
+    float lb = first_lb;
     for (int base = 0; base < cnt; base += 32) {
         const int nb = base + 32 + lane;
-        const int t_next = (nb < cnt) ? (int)__ldg(M.cand + off + nb) : -1;   // ids of the next pass, in flight during this one
+        int t_next = -1;
+        float lb_next = 0.0f;
+        if (nb < cnt) { t_next = (int)__ldg(M.cand + off + nb); lb_next = __ldg(M.cand_lb + off + nb); }   // next pass, in flight during this one
+        const bool test = t >= 0 && !list_lb_prunes(lb, r_up, best);
         double dd = 1e300; d3 q = mk3(0, 0, 0); int f = 0;
-        if (t >= 0) {
+        if (test) {
             const double *T = M.tris + TRI_STRIDE * (size_t)t;
             q = tri_closest_rec(p, T, f);
             const d3 e = p - q;
             dd = dot3(e, e);
         }
+        ISDF_COUNT_TESTED(tally, test);
         warp_argmin_update(dd, q, t, f, best, cbest, tri, feat);
-        t = t_next;
+        if (base + 32 < cnt && list_lb_prunes(__shfl_sync(0xffffffffu, lb_next, 0), r_up, best)) break;
+        t = t_next; lb = lb_next;
     }
     return best;
+}
+__device__ __forceinline__ double list_closest(const DevMesh &M, d3 p, int cell, d3 &cbest, int &tri, int &feat, int lane) {
+    const uint32_t off = M.cell_off[cell];
+    const int cnt = (int)M.cell_cnt[cell];
+    const int nz = M.gdim[2], ny = M.gdim[1];
+    const int iz = cell % nz, iy = (cell / nz) % ny, ix = cell / (nz * ny);
+    const bool has = lane < cnt;
+    return list_closest_pre(M, p, off, cnt, has ? (int)__ldg(M.cand + off + lane) : -1, has ? __ldg(M.cand_lb + off + lane) : 0.0f,
+                            list_centre_dist_up(M, p, ix, iy, iz), 1e300, cbest, tri, feat, lane);
 }
 
 // Latency-oriented list pass for callers that run ONE query at a time on an otherwise idle SM (the swept-volume path's descent and
@@ -609,16 +661,26 @@ __device__ __forceinline__ bool mesh_search_warp(const DevMesh &M, d3 p, double 
 }
 
 // The same search with the cell's record already fetched (DevMesh::cell_rec): cnt / off = candidate list (cnt 0: none), seed =
-// nearest triangle of the cell centre (-1 outside the grid), inside = the cell centre is inside the mesh.
+// nearest triangle of the cell centre (-1 outside the grid), inside = the cell centre is inside the mesh. first_id / first_lb: the
+// list's first pass as list_closest_pre takes it. With an exact sign (pseudonormal, reach >= sign_radius) both searches start from
+// the bound reach^2: nothing closer means sdf >= reach when the cell centre is outside (false), and a second, unbounded search when
+// it is inside.
 __device__ __forceinline__ bool mesh_search_rec(const DevMesh &M, d3 p, double reach, int lane, WideStack *stk, int cnt, uint32_t off,
-                                                int first_id, int seed, bool inside, double &d2, d3 &c, int &tri, int &feat) {
-    if (cnt != 0) {
-        d2 = list_closest_pre(M, p, off, cnt, first_id, c, tri, feat, lane);
-        return true;
-    }
+                                                int first_id, float first_lb, int seed, bool inside, double &d2, d3 &c, int &tri, int &feat) {
     const bool bounded = (reach < 1e150) && (M.sign_radius > 0.0) && (reach >= M.sign_radius) && (M.sign_mode == MESH_SIGN_PSEUDONORMAL);
     double bound2 = bounded ? reach * reach : 1e300;
-    for (;;) {   // one inlined copy of the tree search: first within `reach`, then (deep inside only) unbounded
+    if (cnt != 0) {
+        // the list's cell is p's cell, found exactly as the callers' cull stages find it
+        const double r_up = list_centre_dist_up(M, p, floor((p.x - M.glo[0]) * M.inv_gcell), floor((p.y - M.glo[1]) * M.inv_gcell),
+                                                floor((p.z - M.glo[2]) * M.inv_gcell));
+        for (;;) {   // one inlined copy of the list pass: first within `reach`, then (deep inside only) unbounded
+            d2 = list_closest_pre(M, p, off, cnt, first_id, first_lb, r_up, bound2, c, tri, feat, lane, stk);
+            if (tri >= 0 || bound2 >= 1e299) return true;
+            if (!inside) return false;
+            bound2 = 1e300;
+        }
+    }
+    for (;;) {   // one inlined copy of the tree search, the same way (a separate loop: merged with the list pass, it spills)
 #ifdef ISDF_OUTLINE_TREE_SEARCH
         d2 = wide_closest_outlined(M, p, bound2, seed, c, tri, feat, lane, stk);
 #else

@@ -494,6 +494,26 @@ class Evaluator:
             out["cell_dist"], out["cell_cnt"] = dist, cnt
         return out
 
+    def dbg_mesh_lists(self):
+        """the current mesh's candidate lists, copied to the host: dict(cell_off (shaped as dbg_mesh_grid's arrays), cand (uint32),
+        cand_lb (float32), tris (ntris x 3 x 3: the leaf-order triangles cand indexes, as vertices a, a + ab, a + ac))"""
+        vp, llp = C.c_void_p, C.POINTER(C.c_longlong)
+        u32p, fp = C.POINTER(C.c_uint32), C.POINTER(C.c_float)
+        self.lib.isdf_dbg_mesh_lists.argtypes = [vp, llp, u32p, u32p, fp, C.POINTER(C.c_double)]
+        sizes = np.zeros(2, dtype=np.int64)
+        if self.lib.isdf_dbg_mesh_lists(self.h, sizes.ctypes.data_as(llp), None, None, None, None) != 0:
+            raise IsdfError(-1, "isdf_dbg_mesh_lists failed (is a mesh shape set?)")
+        gdim = self.dbg_mesh_grid(arrays=False)["gdim"]
+        off = np.zeros(gdim, dtype=np.uint32)
+        cand, lb = np.zeros(int(sizes[0]), dtype=np.uint32), np.zeros(int(sizes[0]), dtype=np.float32)
+        rec = np.zeros((int(sizes[1]), 16))
+        if self.lib.isdf_dbg_mesh_lists(self.h, sizes.ctypes.data_as(llp), off.ctypes.data_as(u32p), cand.ctypes.data_as(u32p),
+                                        lb.ctypes.data_as(fp), _dp(rec)) != 0:
+            raise IsdfError(-1, "isdf_dbg_mesh_lists failed")
+        a = rec[:, 0:3]
+        tris = np.stack([a, a + rec[:, 3:6], a + rec[:, 6:9]], axis=1)
+        return dict(cell_off=off, cand=cand, cand_lb=lb, tris=tris)
+
     def dbg_flatness(self, v, a, j, quat_grad, omg_grad, vel_grad):
         """device flatness map + adjoint as compiled into the epilogue kernel -> (quat, omg, gV, gA, gJ)"""
         vaj = np.ascontiguousarray(np.concatenate([_f64(v).reshape(-1, 3), _f64(a).reshape(-1, 3), _f64(j).reshape(-1, 3)], axis=1))
