@@ -8,6 +8,7 @@
 #include "isdf_frontend.cuh"
 #include "isdf_lbfgs.cuh"
 #include "isdf_clearance.cuh"
+#include "isdf_map.cuh"
 #include <queue>
 #include "isdf_host_mesh.cuh"
 #include <cstdio>
@@ -49,6 +50,7 @@ struct isdf_ctx {
     bool have_map = false;
     DevGrid grid;
     DevBuf<uint32_t> d_bits;
+    long long map_points_used = 0, map_points_skipped = 0;   // isdf_set_map_cloud*; 0 for dense maps
     // shape
     bool have_shape = false;
     DevShape shape;
@@ -485,30 +487,31 @@ extern "C" int isdf_shape_query(isdf_ctx *c, const double *p_rel, int n, double 
 }
 
 // ---- map ------------------------------------------------------------------------------------------------------
-template <typename T>
-__global__ void k_pack_bits(const T *occ, uint32_t *bits, int rows, int Z, int Zw) {
-    // one warp per 32-voxel word: ballot of "voxel != 0"
-    const long long gw = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int lane = threadIdx.x & 31;
-    const long long nwords = (long long)rows * Zw;
-    if (gw >= nwords) return;
-    const int row = (int)(gw / Zw), w = (int)(gw - (long long)row * Zw);
-    const int z = w * 32 + lane;
-    const bool o = (z < Z) && (occ[(size_t)row * Z + z] != (T)0);
-    const unsigned b = __ballot_sync(0xffffffffu, o);
-    if (lane == 0) bits[gw] = b;
+// the limits every map must meet, whichever entry point sets it
+static int map_size_check(isdf_ctx *c, long long X, long long Y, long long Z, double res) {
+    if (X * Y >= (1ll << 31) / ((Z + 31) / 32)) return fail(ISDF_ERR_INVALID, "map too large");
+    if (Z > 65535) return fail(ISDF_ERR_UNSUPPORTED, "Z > 65535");
+    // a pose window spans 2 * half_bd / res + 2 voxels per axis of THIS map (its resolution need not equal occupancy_resolution); the scan
+    // kernels pack window offsets into 10 bits per axis
+    if (c && 2.0 * c->dcfg.half_bd / res + 2.0 > (double)WINDOW_AXIS_MAX)
+        return fail(ISDF_ERR_UNSUPPORTED, "map resolution too fine for kernel_size * occupancy_resolution: a pose window would exceed 1023 voxels per axis");
+    return 0;
+}
+
+// the map the bits in c->d_bits describe
+static void commit_map(isdf_ctx *c, int X, int Y, int Z, const double *bmin, const double *bmax, double res, long long used, long long skipped) {
+    DevGrid &g = c->grid;
+    g.bits = c->d_bits.p; g.X = X; g.Y = Y; g.Z = Z; g.Zw = (Z + 31) / 32; g.res = res;
+    for (int a = 0; a < 3; a++) { g.bmin[a] = bmin[a]; g.bmax[a] = bmax[a]; }
+    c->map_points_used = used; c->map_points_skipped = skipped;
+    c->have_map = true;
 }
 
 template <typename T>
 static int set_map_impl(isdf_ctx *c, const T *occ, int X, int Y, int Z, const double *bmin, double res) {
     if (!c || !occ || !bmin) return fail(ISDF_ERR_INVALID, "NULL argument");
     if (X < 1 || Y < 1 || Z < 1 || !(res > 0)) return fail(ISDF_ERR_INVALID, "bad map size");
-    if ((long long)X * Y >= (1ll << 31) / ((Z + 31) / 32)) return fail(ISDF_ERR_INVALID, "map too large");
-    if (Z > 65535) return fail(ISDF_ERR_UNSUPPORTED, "Z > 65535");
-    // a pose window spans 2 * half_bd / res + 2 voxels per axis of THIS map (its resolution need not equal occupancy_resolution); the scan
-    // kernels pack window offsets into 10 bits per axis
-    if (c && 2.0 * c->dcfg.half_bd / res + 2.0 > (double)WINDOW_AXIS_MAX)
-        return fail(ISDF_ERR_UNSUPPORTED, "map resolution too fine for kernel_size * occupancy_resolution: a pose window would exceed 1023 voxels per axis");
+    if (int rc = map_size_check(c, X, Y, Z, res)) return rc;
     if (set_device(c)) return ISDF_ERR_CUDA;
     const size_t nvox = (size_t)X * Y * Z;
     T *d_occ = nullptr;
@@ -519,18 +522,17 @@ static int set_map_impl(isdf_ctx *c, const T *occ, int X, int Y, int Z, const do
     if (e == cudaSuccess) e = c->d_bits.ensure(nwords);
     if (e == cudaSuccess) {
         const long long threads = (long long)nwords * 32;
-        k_pack_bits<T><<<(unsigned)((threads + 255) / 256), 256, 0, c->stream>>>(d_occ, c->d_bits.p, X * Y, Z, Zw);
+        k_pack_bits<<<(unsigned)((threads + 255) / 256), 256, 0, c->stream>>>(NonZero<T>{d_occ}, c->d_bits.p, X * Y, Z, Zw);
         c->stats.kernel_launches++;
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     cudaFree(d_occ);
     if (e != cudaSuccess) return fail(ISDF_ERR_CUDA, std::string("isdf_set_map: ") + cudaGetErrorString(e));
-    DevGrid &g = c->grid;
-    g.bits = c->d_bits.p; g.X = X; g.Y = Y; g.Z = Z; g.Zw = Zw; g.res = res;
     const int dims[3] = {X, Y, Z};
-    for (int a = 0; a < 3; a++) { g.bmin[a] = bmin[a]; g.bmax[a] = bmin[a] + dims[a] * res; }
-    c->have_map = true;
+    double bmax[3];
+    for (int a = 0; a < 3; a++) bmax[a] = bmin[a] + dims[a] * res;
+    commit_map(c, X, Y, Z, bmin, bmax, res, 0, 0);
     return 0;
 }
 
@@ -540,6 +542,174 @@ extern "C" int isdf_set_map_u8(isdf_ctx *c, const uint8_t *occ, int X, int Y, in
 extern "C" int isdf_set_map_f64(isdf_ctx *c, const double *grid_map, int X, int Y, int Z, const double *bmin, double res) {
     return set_map_impl<double>(c, grid_map, X, Y, Z, bmin, res);
 }
+
+// ---- map from a point cloud (PCSmapManager::rcvGlobalMapHandler, PCSmap_manager.cpp:111-181) ---------------------------
+// the context is checked last, so that every other refusal can be seen without a device
+static int cloud_args_check(isdf_ctx *c, const void *pts, int64_t n, int32_t stride, double res) {
+    if (!pts) return fail(ISDF_ERR_INVALID, "points is NULL");
+    if (n < 1 || n >= (1ll << 32)) return fail(ISDF_ERR_INVALID, "point count must be in [1, 2^32)");
+    if (stride < 12 || stride % 4 != 0) return fail(ISDF_ERR_INVALID, "stride_bytes must be a multiple of 4 and at least 12 (x, y, z float32 at 0, 4, 8)");
+    if ((uintptr_t)pts % 4 != 0) return fail(ISDF_ERR_INVALID, "points must be 4-byte aligned");
+    if (!(res > 0) || !std::isfinite(res)) return fail(ISDF_ERR_INVALID, "res must be finite and positive");
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    return 0;
+}
+
+static int cloud_grid_blocks(isdf_ctx *c, long long n) { return (int)std::min<long long>((n + 255) / 256, (long long)c->sm_count * 8); }
+
+// d_pts on the device and ready on stream st (which this synchronises once, for the bounds); the grid is built on c->stream
+static int set_map_cloud_impl(isdf_ctx *c, const char *d_pts, long long n, int stride, double res, int thr, cudaStream_t st) {
+    const int blocks = cloud_grid_blocks(c, n);
+    auto cuda_fail = [&](cudaError_t e) {
+        c->have_map = false;
+        return fail(ISDF_ERR_CUDA, std::string("isdf_set_map_cloud: ") + cudaGetErrorString(e));
+    };
+    // 1. bounds: exact float extrema of the finite records (order-preserving uint32 min / max) and the number of skipped records
+    uint32_t ext[7];
+    {
+        ScopedDevBuf<uint32_t> d_ext;
+        cudaError_t e = d_ext.ensure(7);
+        if (e == cudaSuccess) e = cudaMemsetAsync(d_ext.p, 0xff, 3 * sizeof(uint32_t), st);
+        if (e == cudaSuccess) e = cudaMemsetAsync(d_ext.p + 3, 0, 4 * sizeof(uint32_t), st);
+        if (e == cudaSuccess) {
+            k_cloud_bounds<<<blocks, 256, 0, st>>>(d_pts, n, stride, d_ext.p);
+            c->stats.kernel_launches++;
+            e = cudaGetLastError();
+        }
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ext, d_ext.p, sizeof(ext), cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) return cuda_fail(e);
+    }
+    const long long skipped = ext[6], used = n - skipped;
+    if (used == 0) return fail(ISDF_ERR_INVALID, "the cloud has no point with finite coordinates");
+    // 2. the reference's frame: HUGE_NUMBER start (PCSmap_manager.cpp:6,11-12), strict updates (:111-143), createGridMap's sizes (Gridmap3D.cpp:25-39)
+    double bmin[3], bmax[3], dim[3];
+    for (int a = 0; a < 3; a++) {
+        float lo, hi;
+        const uint32_t ulo = ordered_to_float(ext[a]), uhi = ordered_to_float(ext[3 + a]);
+        std::memcpy(&lo, &ulo, 4); std::memcpy(&hi, &uhi, 4);
+        bmin[a] = 999999999.0; bmax[a] = -999999999.0;
+        if ((double)lo < bmin[a]) bmin[a] = lo;
+        if ((double)hi > bmax[a]) bmax[a] = hi;
+        dim[a] = std::ceil((bmax[a] - bmin[a]) / res);
+    }
+    char dims_msg[160];
+    std::snprintf(dims_msg, sizeof dims_msg, " (the cloud asks for %.0f x %.0f x %.0f voxels at res %g)", dim[0], dim[1], dim[2], res);
+    for (int a = 0; a < 3; a++) {
+        if (!(dim[a] >= 1)) return fail(ISDF_ERR_INVALID, std::string("degenerate cloud extent: an axis has fewer than one voxel") + dims_msg);
+        if (dim[a] > 2147483647.0) return fail(ISDF_ERR_INVALID, std::string("map too large") + dims_msg);
+    }
+    const int X = (int)dim[0], Y = (int)dim[1], Z = (int)dim[2];
+    if (int rc = map_size_check(c, X, Y, Z, res)) return fail(rc, g_err + dims_msg);
+    // 3. occupancy (the previous map is given up from here on)
+    c->have_map = false;
+    CloudFrame F;
+    for (int a = 0; a < 3; a++) F.bmin[a] = bmin[a];
+    F.res = res; F.X = X; F.Y = Y; F.Z = Z; F.Zw = (Z + 31) / 32;
+    const size_t nwords = (size_t)X * Y * F.Zw;
+    cudaError_t e = c->d_bits.ensure(nwords);
+    if (e != cudaSuccess) return cuda_fail(e);
+    const long long pack_threads = (long long)nwords * 32;
+    const unsigned pack_blocks = (unsigned)((pack_threads + 255) / 256);
+    ScopedDevBuf<uint32_t> d_cnt;   // sta_threshold > 1: per-voxel counts, freed after the final synchronise
+    if (thr <= 0) {
+        k_pack_bits<<<pack_blocks, 256, 0, c->stream>>>(AllSet{}, c->d_bits.p, X * Y, Z, F.Zw);
+        c->stats.kernel_launches++;
+        e = cudaGetLastError();
+    } else if (thr == 1) {
+        e = cudaMemsetAsync(c->d_bits.p, 0, nwords * sizeof(uint32_t), c->stream);
+        if (e == cudaSuccess) {
+            k_cloud_mark<<<blocks, 256, 0, c->stream>>>(d_pts, n, stride, F, c->d_bits.p);
+            c->stats.kernel_launches++;
+            e = cudaGetLastError();
+        }
+    } else {
+        const size_t nvox = (size_t)X * Y * Z;
+        e = d_cnt.ensure(nvox);
+        if (e == cudaSuccess) e = cudaMemsetAsync(d_cnt.p, 0, nvox * sizeof(uint32_t), c->stream);
+        if (e == cudaSuccess) {
+            k_cloud_count<<<blocks, 256, 0, c->stream>>>(d_pts, n, stride, F, d_cnt.p);
+            k_pack_bits<<<pack_blocks, 256, 0, c->stream>>>(CountAtLeast{d_cnt.p, (uint32_t)thr}, c->d_bits.p, X * Y, Z, F.Zw);
+            c->stats.kernel_launches += 2;
+            e = cudaGetLastError();
+        }
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess) return cuda_fail(e);
+    commit_map(c, X, Y, Z, bmin, bmax, res, used, skipped);
+    return 0;
+}
+
+extern "C" int isdf_set_map_cloud(isdf_ctx *c, const void *points, int64_t n, int32_t stride_bytes, double res, int32_t sta_threshold) {
+    if (int rc = cloud_args_check(c, points, n, stride_bytes, res)) return rc;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    ScopedDevBuf<char> d_pts;
+    const size_t bytes = (size_t)n * stride_bytes;
+    cudaError_t e = d_pts.ensure(bytes);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_pts.p, points, bytes, cudaMemcpyHostToDevice, c->stream);
+    if (e != cudaSuccess) {
+        c->have_map = false;
+        return fail(ISDF_ERR_CUDA, std::string("isdf_set_map_cloud: ") + cudaGetErrorString(e));
+    }
+    return set_map_cloud_impl(c, d_pts.p, n, stride_bytes, res, sta_threshold, c->stream);
+}
+
+extern "C" int isdf_set_map_cloud_device(isdf_ctx *c, const void *d_points, int64_t n, int32_t stride_bytes, double res, int32_t sta_threshold,
+                                         void *cuda_stream) {
+    if (int rc = cloud_args_check(c, d_points, n, stride_bytes, res)) return rc;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    return set_map_cloud_impl(c, (const char *)d_points, n, stride_bytes, res, sta_threshold, (cudaStream_t)cuda_stream);
+}
+
+extern "C" int isdf_get_map_info(isdf_ctx *c, isdf_map_info *out) {
+    if (!c || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (!c->have_map) return fail(ISDF_ERR_STATE, "map not set");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    const DevGrid &g = c->grid;
+    ScopedDevBuf<unsigned long long> d_pop;
+    unsigned long long pop = 0;
+    const long long nwords = (long long)g.X * g.Y * g.Zw;
+    CU_TRY(d_pop.ensure(1));
+    CU_TRY(cudaMemsetAsync(d_pop.p, 0, sizeof(unsigned long long), c->stream));
+    k_popcount<<<cloud_grid_blocks(c, nwords), 256, 0, c->stream>>>(g.bits, nwords, d_pop.p);
+    c->stats.kernel_launches++;
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaMemcpyAsync(&pop, d_pop.p, sizeof(pop), cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(cudaStreamSynchronize(c->stream));
+    std::memset(out, 0, sizeof(*out));
+    out->X = g.X; out->Y = g.Y; out->Z = g.Z; out->res = g.res;
+    for (int a = 0; a < 3; a++) { out->bmin[a] = g.bmin[a]; out->bmax[a] = g.bmax[a]; }
+    out->occupied_voxels = (int64_t)pop;
+    out->points_used = c->map_points_used; out->points_skipped = c->map_points_skipped;
+    return 0;
+}
+
+// the bit grid expanded to one T per voxel, a bounded number of (x, y) rows at a time through device scratch
+template <typename T>
+static int get_map_impl(isdf_ctx *c, T *out, int64_t n) {
+    if (!c || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (!c->have_map) return fail(ISDF_ERR_STATE, "map not set");
+    const DevGrid &g = c->grid;
+    const long long rows = (long long)g.X * g.Y;
+    if (n != rows * g.Z) return fail(ISDF_ERR_INVALID, "n must be X*Y*Z of the map");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    const long long chunk_rows = std::max<long long>(1, (32ll << 20) / ((long long)g.Z * sizeof(T)));   // <= 32 MiB of scratch per chunk
+    ScopedDevBuf<T> d_out;
+    CU_TRY(d_out.ensure((size_t)std::min(rows, chunk_rows) * g.Z));
+    for (long long r0 = 0; r0 < rows; r0 += chunk_rows) {
+        const int nr = (int)std::min(chunk_rows, rows - r0);
+        const long long cnt = (long long)nr * g.Z;
+        k_unpack_bits<T><<<cloud_grid_blocks(c, cnt), 256, 0, c->stream>>>(g.bits, d_out.p, r0, nr, g.Z, g.Zw);
+        c->stats.kernel_launches++;
+        CU_TRY(cudaGetLastError());
+        CU_TRY(cudaMemcpyAsync(out + r0 * g.Z, d_out.p, cnt * sizeof(T), cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaStreamSynchronize(c->stream));
+    }
+    return 0;
+}
+
+extern "C" int isdf_get_map_u8(isdf_ctx *c, uint8_t *occ, int64_t n) { return get_map_impl<uint8_t>(c, occ, n); }
+extern "C" int isdf_get_map_f64(isdf_ctx *c, double *grid_map, int64_t n) { return get_map_impl<double>(c, grid_map, n); }
 
 // getPointsInAABB (pcs:148-170): one CTA; thread = (x, y) row of the clamped index box — popcount of the row's z-run, block-wide exclusive scan
 // for the row's output offset, then every thread writes its row's voxel centres in z order: the reference's x -> y -> z output order

@@ -32,7 +32,8 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_lbfgs_default_params", "isdf_lbfgs_batch", "isdf_lbfgs_batch_device", "isdf_set_points_batch",
                "isdf_frontend_build_kernels", "isdf_frontend_get_kernels", "isdf_frontend_feasibility", "isdf_frontend_feasibility_device",
                "isdf_frontend_check_batch", "isdf_peer_export", "isdf_peer_connect", "isdf_peer_allreduce_device", "isdf_peer_status", "isdf_peer_disconnect",
-               "isdf_clearance_default_params", "isdf_trajectory_clearance", "isdf_trajectory_clearance_device"]
+               "isdf_clearance_default_params", "isdf_trajectory_clearance", "isdf_trajectory_clearance_device",
+               "isdf_set_map_cloud", "isdf_set_map_cloud_device", "isdf_get_map_info", "isdf_get_map_u8", "isdf_get_map_f64"]
 
 
 class KernelConfig(C.Structure):
@@ -71,6 +72,17 @@ class ClearanceSummary(C.Structure):
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+class MapInfo(C.Structure):
+    """isdf_map_info"""
+    _fields_ = [("X", C.c_int32), ("Y", C.c_int32), ("Z", C.c_int32), ("reserved_", C.c_int32), ("res", C.c_double),
+                ("bmin", C.c_double * 3), ("bmax", C.c_double * 3), ("occupied_voxels", C.c_int64), ("points_used", C.c_int64),
+                ("points_skipped", C.c_int64)]
+
+    def as_dict(self):
+        return dict(dims=(self.X, self.Y, self.Z), res=self.res, bmin=np.array(self.bmin[:]), bmax=np.array(self.bmax[:]),
+                    occupied_voxels=self.occupied_voxels, points_used=self.points_used, points_skipped=self.points_skipped)
 
 
 class Stats(C.Structure):
@@ -144,6 +156,11 @@ def load_library(path=None):
     lib.isdf_clearance_default_params.argtypes = [C.POINTER(ClearanceParams)]
     lib.isdf_trajectory_clearance.argtypes = [vp, C.c_int, dp, dp, C.POINTER(ClearanceParams), dp, C.POINTER(C.c_int64), C.POINTER(ClearanceSummary)]
     lib.isdf_trajectory_clearance_device.argtypes = [vp, C.c_int, vp, vp, C.POINTER(ClearanceParams), vp, vp, vp, vp]
+    lib.isdf_set_map_cloud.argtypes = [vp, vp, C.c_int64, C.c_int32, C.c_double, C.c_int32]
+    lib.isdf_set_map_cloud_device.argtypes = [vp, vp, C.c_int64, C.c_int32, C.c_double, C.c_int32, vp]
+    lib.isdf_get_map_info.argtypes = [vp, C.POINTER(MapInfo)]
+    lib.isdf_get_map_u8.argtypes = [vp, C.POINTER(C.c_uint8), C.c_int64]
+    lib.isdf_get_map_f64.argtypes = [vp, dp, C.c_int64]
     for s in ABI_SYMBOLS:
         if s != "isdf_last_error":
             getattr(lib, s).restype = C.c_int
@@ -230,6 +247,63 @@ class Evaluator:
         X, Y, Z = grid.shape
         b = _f64(bmin).reshape(3)
         self._check(self.lib.isdf_set_map_f64(self.h, _dp(grid), X, Y, Z, _dp(b), float(res)))
+
+    def set_map_cloud(self, points, res, sta_threshold=1, stride_bytes=None):
+        """the occupancy grid from a float32 point cloud (PCSmapManager::rcvGlobalMapHandler; see isdf_set_map_cloud in include/isdf.h).
+        points: (n, 3) or (n, k >= 3) float32 with x, y, z in the first three columns, or a 1-D float32 / uint8 buffer of n records of
+        stride_bytes each (a PointCloud2's data with point_step). Any other dtype raises rather than being rounded silently."""
+        pts = np.asarray(points)
+        if pts.dtype == np.float32 and pts.ndim == 2:
+            if pts.shape[1] < 3:
+                raise ValueError("points need at least 3 columns (x, y, z)")
+            pts = np.ascontiguousarray(pts)
+            stride = pts.shape[1] * 4 if stride_bytes is None else int(stride_bytes)
+            if stride != pts.shape[1] * 4:
+                raise ValueError("stride_bytes must equal the row size of a 2-D points array")
+            n = pts.shape[0]
+        elif pts.dtype in (np.float32, np.uint8) and pts.ndim == 1:
+            if stride_bytes is None:
+                raise ValueError("a flat record buffer needs stride_bytes")
+            pts = np.ascontiguousarray(pts)
+            stride = int(stride_bytes)
+            n = pts.nbytes // stride if stride > 0 else 0
+        else:
+            raise TypeError(f"points must be float32 (n, k>=3) or a flat float32/uint8 record buffer, got {pts.dtype} {pts.shape}")
+        self._check(self.lib.isdf_set_map_cloud(self.h, pts.ctypes.data_as(C.c_void_p) if n else None, n, stride, float(res), int(sta_threshold)))
+
+    def set_map_cloud_device(self, points, n=None, stride_bytes=None, res=1.0, sta_threshold=1, stream=0):
+        """points on the context's device: a float32 torch tensor (n, k >= 3), contiguous, or a raw device pointer with n and stride_bytes"""
+        if hasattr(points, "data_ptr"):
+            if str(points.dtype) != "torch.float32" or points.dim() != 2 or points.shape[1] < 3:
+                raise TypeError(f"points must be a float32 (n, k>=3) tensor, got {points.dtype} {tuple(points.shape)}")
+            if not points.is_contiguous():
+                raise ValueError("points must be contiguous")
+            ptr, n, stride = points.data_ptr(), points.shape[0], points.shape[1] * 4
+            if stride_bytes is not None and int(stride_bytes) != stride:
+                raise ValueError("stride_bytes must equal the row size of a points tensor")
+        else:
+            if n is None or stride_bytes is None:
+                raise ValueError("a raw device pointer needs n and stride_bytes")
+            ptr, stride = int(points), int(stride_bytes)
+        self._check(self.lib.isdf_set_map_cloud_device(self.h, C.c_void_p(ptr), int(n), stride, float(res), int(sta_threshold), C.c_void_p(stream)))
+
+    def map_info(self):
+        """isdf_map_info of the current map as a dict(dims, res, bmin, bmax, occupied_voxels, points_used, points_skipped)"""
+        m = MapInfo()
+        self._check(self.lib.isdf_get_map_info(self.h, C.byref(m)))
+        return m.as_dict()
+
+    def get_map_u8(self):
+        X, Y, Z = self.map_info()["dims"]
+        out = np.empty((X, Y, Z), dtype=np.uint8)
+        self._check(self.lib.isdf_get_map_u8(self.h, out.ctypes.data_as(C.POINTER(C.c_uint8)), out.size))
+        return out
+
+    def get_map_f64(self):
+        X, Y, Z = self.map_info()["dims"]
+        out = np.empty((X, Y, Z), dtype=np.float64)
+        self._check(self.lib.isdf_get_map_f64(self.h, _dp(out), out.size))
+        return out
 
     def points_in_aabb(self, centre, half, cap=100000):
         out = np.zeros((cap, 3))

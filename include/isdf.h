@@ -128,6 +128,55 @@ int isdf_shape_query(isdf_ctx *ctx, const double *p_rel, int n, double *sdf, dou
 int isdf_set_map_u8(isdf_ctx *ctx, const uint8_t *occ, int X, int Y, int Z, const double *bmin, double res);
 /* the reference's own storage: one double per voxel (GridMap3D.h:215) */
 int isdf_set_map_f64(isdf_ctx *ctx, const double *grid_map, int X, int Y, int Z, const double *bmin, double res);
+
+/* PCSmapManager::rcvGlobalMapHandler (PCSmap_manager.cpp:111-181) on the device: the occupancy grid from a point cloud.
+ * points: n records of stride_bytes each, with x, y, z as float32 at byte offsets 0, 4, 8 (pcl::PointXYZ: stride 16; a PointCloud2's
+ * data with point_step as the stride).
+ *   Bounds      per axis min starts at 999999999 and max at -999999999 (HUGE_NUMBER, PCSmap_manager.cpp:6,11-12) and is updated with
+ *               strict < / > from (double) of every finite coordinate (:111-143).
+ *   Dimensions  X = (int)ceil((max - min) / res) per axis in FP64 (createGridMap, Gridmap3D.cpp:25-39).
+ *   Index       getGridIndex (Gridmap3D.cpp:135-175) restated exactly: ix = (int)floor(((double)x - min) / res), clamped to X - 1,
+ *               including its "iy < 0 => ix = 0" branches (they cannot fire for points inside the bounds). A point on max at an exact
+ *               multiple of res lands in the top layer X - 1.
+ *   Occupancy   a voxel is occupied when its point count is >= sta_threshold (:151-181); sta_threshold <= 0 marks every voxel occupied,
+ *               as in the reference. Every shipped config uses 1.
+ *   Frame       bmin = min and bmax = max (the reference's boundary_xyzmax is the cloud's maximum, not bmin + X*res). Every index the
+ *               library derives from a map is clamp(floor((clamp(c, bmin, bmax) - bmin) / res), 0, size - 1), which is the same for
+ *               either bmax, so the evaluation, gather, clearance and front-end entry points behave on a cloud-built map exactly as on
+ *               the same occupancy given to isdf_set_map_u8 with the same bmin and res.
+ * Deviations from the reference:
+ *   - records with a NaN or Inf coordinate are skipped, from the bounds and the counts, and counted in points_skipped (undefined
+ *     behaviour in the reference: NaN passes isInMap and (int)floor(NaN) becomes an address);
+ *   - ISDF_ERR_INVALID for n < 1 or n >= 2^32, stride_bytes < 12 or not a multiple of 4, points not 4-byte aligned, res not finite
+ *     and positive, a NULL pointer, no finite point, or a degenerate extent (an axis with X < 1: every point shares that coordinate;
+ *     the reference allocates a zero-size grid and writes past it);
+ *   - the size limits of isdf_set_map_u8 apply with its codes (X*Y*ceil(Z/32) < 2^31, Z <= 65535, the 1023-voxel pose window), and
+ *     the message names the dimensions the cloud asked for.
+ * Argument checks run before any device call. A refused call leaves the previous map in place; a CUDA failure leaves no map (later
+ * calls get ISDF_ERR_STATE). The result is the same bits whatever the order of the points and through either entry point. The call
+ * counts its launches in isdf_stats.kernel_launches and touches no other field. sta_threshold > 1 needs 4 bytes of device scratch per
+ * voxel during the call. */
+int isdf_set_map_cloud(isdf_ctx *ctx, const void *points, int64_t n, int32_t stride_bytes, double res, int32_t sta_threshold);
+/* the same with the points on ctx's device. Work before the call on cuda_stream is waited for: the call synchronises cuda_stream once
+ * (the grid size depends on the bounds), builds the grid on ctx's own stream and returns when the map is set, so d_points may be
+ * reused at once. */
+int isdf_set_map_cloud_device(isdf_ctx *ctx, const void *d_points, int64_t n, int32_t stride_bytes, double res, int32_t sta_threshold,
+                              void *cuda_stream);
+
+typedef struct isdf_map_info {
+    int32_t X, Y, Z, reserved_;
+    double res, bmin[3], bmax[3];         /* bmax: the cloud's maximum for cloud maps (reference boundary_xyzmax); bmin + size*res otherwise */
+    int64_t occupied_voxels;              /* popcount of the grid */
+    int64_t points_used, points_skipped;  /* cloud maps only (0 otherwise); skipped = records with a non-finite coordinate */
+} isdf_map_info;
+/* any map, however it was set; ISDF_ERR_STATE without one */
+int isdf_get_map_info(isdf_ctx *ctx, isdf_map_info *out);
+/* the grid as 0 / 1 in the setters' layout (address ix*Y*Z + iy*Z + iz), n = X*Y*Z elements (ISDF_ERR_INVALID otherwise). The f64
+ * form fills the reference's occupancy_map->grid_map directly (after createGridMap(bmin, bmax) with isdf_get_map_info's frame). The
+ * grid is expanded on the device in bounded chunks. */
+int isdf_get_map_u8(isdf_ctx *ctx, uint8_t *occ, int64_t n);
+int isdf_get_map_f64(isdf_ctx *ctx, double *grid_map, int64_t n);
+
 /* PCSmapManager::getPointsInAABB (pcs:148-170) on the device map; writes up to cap centres (cap x 3), returns count in *n */
 int isdf_points_in_aabb(isdf_ctx *ctx, const double *centre, double half_extent, double *out_points, int cap, int *n);
 
