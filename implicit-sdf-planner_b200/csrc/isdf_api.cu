@@ -39,78 +39,90 @@ static int fail(int code, const std::string &msg) { g_err = msg; return code; }
         }                                                                                             \
     } while (0)
 
+// One plain struct per subsystem; each keeps the flag that says its state is valid next to the buffers that state lives in. Every
+// buffer owns its memory; ~isdf_ctx releases the rest.
 struct isdf_ctx {
     int device = 0;
     isdf_config cfg;
     DevCfg dcfg;
+    int rank = 0, world = 1;   // shard
     cudaStream_t stream = nullptr, aux_stream = nullptr;   // aux: work-item build, off the evaluation's critical path
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev_main_done = nullptr, ev_items_done = nullptr;
-    bool items_pending = false;
-    // map
-    bool have_map = false;
-    DevGrid grid;
-    DevBuf<uint32_t> d_bits;
-    long long map_points_used = 0, map_points_skipped = 0;   // isdf_set_map_cloud*; 0 for dense maps
-    // shape
-    bool have_shape = false;
-    DevShape shape;
-    DevBuf<BvhNode> d_nodes; DevBuf<WideNode> d_wnodes; DevBuf<double> d_tris, d_pn, d_obb; DevBuf<float> d_cell_dist; DevBuf<uint32_t> d_cell_seed, d_cell_off, d_cand; DevBuf<float> d_cand_lb; DevBuf<uint16_t> d_cell_cnt; DevBuf<uint4> d_cell_rec; DevBuf<WnNode> d_wn;
-    double mesh_list_reach = 0;  // radius (cell-centre distance) up to which cells got candidate lists (isdf_dbg_mesh_grid)
-    // evaluation scratch
-    DevBuf<double> d_T, d_C, d_out, d_piece_cost;
-    double *count_out_dev = nullptr;   // host entry points: where the epilogue drops the pair count (behind the result vector)
-    DevBuf<int> d_tickets;       // pieces_done counter of the epilogue kernel
-    DevBuf<double> d_tot; DevBuf<unsigned> d_split_done;   // per-sample collision sums handed from the scan kernels to the epilogue
-    DevBuf<int> d_items, d_item_count; DevBuf<unsigned> d_work, d_split_work; DevBuf<double> d_subsum;   // work items (longest first, heavy samples split)
     int warp_slots = 132 * 16;   // resident warps of the mesh kernel on this device (SMs x CTAs/SM x warps/CTA)
     int sm_count = 132, mesh_blocks = 4, analytic_blocks = 4;   // persistent grids: one CTA per resident slot
     size_t smem_per_sm = 228 * 1024;   // shared memory of one SM (H100: 228 KB, at most 227 KB to one CTA)
-    long long order_for = -1;    // (N, rank, world) signature the order array is valid for
-    DevBuf<unsigned long long> d_counter, d_dbg, d_trace;
-    DevBuf<double> d_mx, d_mbc, d_mT, d_mC, d_mlu, d_men, d_mgC, d_mgT, d_mcost, d_mgrad, d_mout, d_mCpp, d_msv;   // batched callback (isdf_minco.cuh)
-    int minco_B = 0, minco_N = 0;
-    DevBuf<double> d_lb_x, d_lb_f, d_lb_grad, d_lb_state; DevBuf<int> d_lb_int, d_lb_head;   // device-resident lock-step L-BFGS (isdf_lbfgs.cuh)
-    int *h_lb_active = nullptr;  // pinned
+    int clr_blocks = 1;                // resident CTAs per SM of the clearance scan kernel
     bool dbg_on = false;
-    bool no_items = false;       // diagnostics: always launch in natural order, never split (isdf_dbg_schedule)
-    int warp_slots_override = 0; // diagnostics: pretend the device has this many resident warps (forces splitting)
-    double *h_stage = nullptr;   // pinned
-    size_t h_stage_n = 0;
-    // swept volume
-    SweptState sv;
-    // shard
-    int rank = 0, world = 1;
-    // front end attitude kernels (isdf_frontend.cuh)
-    DevBuf<double> d_fe_rot; DevBuf<uint8_t> d_fe_kernels, d_fe_order, d_fe_ok; DevBuf<uint32_t> d_fe_masks, d_fe_out;
-    DevBuf<int> d_fe_ind; DevBuf<double> d_fe_father, d_fe_child;
-    DevBuf<uint2> d_fe_core, d_fe_urows, d_fe_surv, d_fe_chunks; DevBuf<uint4> d_fe_tab; int fe_nurow = 0, fe_nchunk = 0, fe_ntab = 0; DevBuf<unsigned> d_fe_count; int fe_ncore = 0;
-    bool fe_ready = false;
-    int fe_xk = 0, fe_yk = 0, fe_ks = 0;
-    double fe_max_roll = 0, fe_max_pitch = 0, fe_ang_res = 0, fe_margin = 0;
-    // peer-memory reduction (isdf_peer.cuh)
-    void *peer_buf = nullptr;            // own exchange buffer (cudaMalloc, exported through CUDA IPC)
-    void *peer_open[PEER_MAX] = {};      // peers' buffers opened here (null for self / unused)
-    PeerArgs peer = {};                  // world == 0: not connected
-    bool peer_fused = false;             // sharded *_device evaluations finish with the exchange
-    int peer_world_alloc = 0, peer_cap = 0;
-    DevBuf<int> d_peer_status;
-    // trajectory clearance check (isdf_clearance.cuh)
-    int clr_blocks = 1;                  // resident CTAs per SM of the clearance scan kernel
-    DevBuf<double> d_clr_in, d_clr_clear; DevBuf<long long> d_clr_vox; DevBuf<ClrSummary> d_clr_sum; DevBuf<int> d_clr_cursor;
-    DevBuf<unsigned long long> d_clr_counters;   // {candidate pairs, exact mesh searches} of the last check (isdf_dbg_clearance_counts)
-    isdf_stats stats;
+    isdf_stats stats = {};
+    struct {
+        bool have_map = false;
+        DevGrid grid = {};
+        DevBuf<uint32_t> d_bits;
+        long long points_used = 0, points_skipped = 0;   // isdf_set_map_cloud*; 0 for dense maps
+    } map;
+    struct {   // the robot shape; the buffers hold a mesh's device view
+        bool have_shape = false;
+        DevShape shape = {};
+        DevBuf<BvhNode> d_nodes; DevBuf<WideNode> d_wnodes; DevBuf<double> d_tris, d_pn, d_obb; DevBuf<float> d_cell_dist; DevBuf<uint32_t> d_cell_seed, d_cell_off, d_cand; DevBuf<float> d_cand_lb; DevBuf<uint16_t> d_cell_cnt; DevBuf<uint4> d_cell_rec; DevBuf<WnNode> d_wn;
+        double list_reach = 0;  // radius (cell-centre distance) up to which cells got candidate lists (isdf_dbg_mesh_grid)
+    } mesh;
+    struct {   // discrete evaluation: scan / epilogue scratch and the work-item schedule
+        long long order_for = -1;    // (N, rank, world) signature the work items are valid for
+        bool items_pending = false;  // the aux stream is building them
+        DevBuf<double> d_piece_cost;
+        double *count_out_dev = nullptr;   // host entry points: where the epilogue drops the pair count (behind the result vector)
+        DevBuf<int> d_tickets;       // pieces_done counter of the epilogue kernel
+        DevBuf<double> d_tot; DevBuf<unsigned> d_split_done;   // per-sample collision sums handed from the scan kernels to the epilogue
+        DevBuf<int> d_items, d_item_count; DevBuf<unsigned> d_work, d_split_work; DevBuf<double> d_subsum;   // work items (longest first, heavy samples split)
+        DevBuf<unsigned long long> d_counter, d_dbg, d_trace;
+        bool no_items = false;       // diagnostics: always launch in natural order, never split (isdf_dbg_schedule)
+        int warp_slots_override = 0; // diagnostics: pretend the device has this many resident warps (forces splitting)
+    } disc;
+    struct {   // host entry points of the discrete and swept-volume terms: one pinned block, one copy each way
+        PinnedBuf<double> h;
+        DevBuf<double> d_C, d_out;
+    } stage;
+    struct {   // batched callback (isdf_minco.cuh); B = 0: none evaluated yet
+        DevBuf<double> d_x, d_bc, d_T, d_C, d_lu, d_energy, d_gC, d_gT, d_cost, d_grad, d_out, d_Cpp, d_sv;
+        int B = 0, N0 = 0;
+    } batch;
+    struct {   // device-resident lock-step L-BFGS (isdf_lbfgs.cuh)
+        DevBuf<double> d_x, d_f, d_grad, d_state; DevBuf<int> d_int, d_head;
+        PinnedBuf<int> h_active;
+    } lbfgs;
+    SweptState sv;   // swept volume
+    struct {   // front end attitude kernels (isdf_frontend.cuh)
+        bool ready = false;
+        DevBuf<double> d_rot; DevBuf<uint8_t> d_kernels, d_order, d_ok; DevBuf<uint32_t> d_masks, d_out;
+        DevBuf<int> d_ind; DevBuf<double> d_father, d_child;
+        DevBuf<uint2> d_core, d_urows, d_surv, d_chunks; DevBuf<uint4> d_tab; int nurow = 0, nchunk = 0, ntab = 0; DevBuf<unsigned> d_count; int ncore = 0;
+        int xk = 0, yk = 0, ks = 0;
+        double max_roll = 0, max_pitch = 0, ang_res = 0, margin = 0;
+    } fe;
+    struct {   // trajectory clearance check (isdf_clearance.cuh)
+        DevBuf<double> d_in, d_clear; DevBuf<long long> d_vox; DevBuf<ClrSummary> d_sum; DevBuf<int> d_cursor;
+        DevBuf<unsigned long long> d_counters;   // {candidate pairs, exact mesh searches} of the last check (isdf_dbg_clearance_counts)
+    } clr;
+    struct {   // peer-memory reduction (isdf_peer.cuh)
+        DevBuf<char> buf;                    // own exchange buffer (exported through CUDA IPC)
+        void *open[PEER_MAX] = {};           // peers' buffers opened here (null for self / unused)
+        PeerArgs args = {};                  // world == 0: not connected
+        bool fused = false;                  // sharded *_device evaluations finish with the exchange
+        int world_alloc = 0, cap = 0;
+        DevBuf<int> d_status;
+        void close_handles() { for (void *&p : open) if (p) { cudaIpcCloseMemHandle(p); p = nullptr; } }
+    } peer;
+
+    ~isdf_ctx() {
+        peer.close_handles();
+        peer.buf = {};
+        for (cudaEvent_t e : {ev0, ev1, ev_main_done, ev_items_done}) if (e) cudaEventDestroy(e);
+        if (aux_stream) cudaStreamDestroy(aux_stream);
+        if (stream) cudaStreamDestroy(stream);
+    }
 };
 
 static int set_device(isdf_ctx *c) { CU_TRY(cudaSetDevice(c->device)); return 0; }
-
-static int ensure_stage(isdf_ctx *c, size_t n) {
-    if (n <= c->h_stage_n) return 0;
-    if (c->h_stage) cudaFreeHost(c->h_stage);
-    c->h_stage = nullptr; c->h_stage_n = 0;
-    CU_TRY(cudaMallocHost((void **)&c->h_stage, n * sizeof(double)));
-    c->h_stage_n = n;
-    return 0;
-}
 
 extern "C" const char *isdf_last_error(void) { return g_err.c_str(); }
 
@@ -156,9 +168,6 @@ extern "C" int isdf_create(const isdf_config *cfg, int device, isdf_ctx **out) {
         }
         c->clr_blocks = std::max(nb_clr, 1);
     }
-    std::memset(&c->stats, 0, sizeof(c->stats));
-    std::memset(&c->grid, 0, sizeof(c->grid));
-    std::memset(&c->shape, 0, sizeof(c->shape));
     DevCfg &d = c->dcfg;
     d.fp.mass = cfg->vehicle_mass; d.fp.grav = cfg->grav_acc; d.fp.dh_over_m = cfg->horiz_drag / cfg->vehicle_mass;
     d.fp.cp = cfg->paras_drag; d.fp.veps = cfg->speed_eps;
@@ -173,8 +182,8 @@ extern "C" int isdf_create(const isdf_config *cfg, int device, isdf_ctx **out) {
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_items_done, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreate(&c->ev0);
     if (e == cudaSuccess) e = cudaEventCreate(&c->ev1);
-    if (e == cudaSuccess) e = c->d_counter.ensure(4);
-    if (e == cudaSuccess) e = cudaMemset(c->d_counter.p, 0, 4 * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = c->disc.d_counter.ensure(4);
+    if (e == cudaSuccess) e = cudaMemset(c->disc.d_counter.p, 0, 4 * sizeof(unsigned long long));
     if (e != cudaSuccess) { delete c; return fail(ISDF_ERR_CUDA, std::string("isdf_create: ") + cudaGetErrorString(e)); }
     *out = c;
     return 0;
@@ -184,26 +193,7 @@ extern "C" int isdf_destroy(isdf_ctx *c) {
     if (!c) return 0;
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
-    if (c->aux_stream) cudaStreamSynchronize(c->aux_stream);
-    c->d_bits.release(); c->d_nodes.release(); c->d_wnodes.release(); c->d_tris.release(); c->d_pn.release(); c->d_obb.release(); c->d_cell_dist.release(); c->d_cell_seed.release(); c->d_cell_off.release(); c->d_cand.release(); c->d_cand_lb.release(); c->d_cell_cnt.release(); c->d_cell_rec.release(); c->d_wn.release();
-    c->d_T.release(); c->d_C.release(); c->d_out.release(); c->d_piece_cost.release();
-    c->d_tickets.release(); c->d_counter.release(); c->d_items.release(); c->d_item_count.release(); c->d_tot.release(); c->d_split_done.release(); c->d_work.release(); c->d_split_work.release(); c->d_subsum.release(); c->d_dbg.release(); c->d_trace.release();
-    for (int p = 0; p < PEER_MAX; p++) if (c->peer_open[p]) cudaIpcCloseMemHandle(c->peer_open[p]);
-    if (c->peer_buf) cudaFree(c->peer_buf);
-    c->d_peer_status.release();
-    c->d_clr_in.release(); c->d_clr_clear.release(); c->d_clr_vox.release(); c->d_clr_sum.release(); c->d_clr_cursor.release(); c->d_clr_counters.release();
-    c->d_fe_rot.release(); c->d_fe_kernels.release(); c->d_fe_order.release(); c->d_fe_ok.release(); c->d_fe_masks.release(); c->d_fe_out.release(); c->d_fe_ind.release(); c->d_fe_father.release(); c->d_fe_child.release(); c->d_fe_core.release(); c->d_fe_urows.release(); c->d_fe_surv.release(); c->d_fe_chunks.release(); c->d_fe_tab.release(); c->d_fe_count.release();
-    c->d_mx.release(); c->d_mbc.release(); c->d_mT.release(); c->d_mC.release(); c->d_mlu.release(); c->d_men.release(); c->d_mgC.release(); c->d_mgT.release(); c->d_mcost.release(); c->d_mgrad.release(); c->d_mout.release(); c->d_mCpp.release(); c->d_msv.release();
-    c->sv.release();
-    if (c->h_stage) cudaFreeHost(c->h_stage);
-    if (c->h_lb_active) cudaFreeHost(c->h_lb_active);
-    c->d_lb_x.release(); c->d_lb_f.release(); c->d_lb_grad.release(); c->d_lb_state.release(); c->d_lb_int.release(); c->d_lb_head.release();
-    if (c->ev0) cudaEventDestroy(c->ev0);
-    if (c->ev1) cudaEventDestroy(c->ev1);
-    if (c->ev_main_done) cudaEventDestroy(c->ev_main_done);
-    if (c->ev_items_done) cudaEventDestroy(c->ev_items_done);
-    if (c->aux_stream) cudaStreamDestroy(c->aux_stream);
-    if (c->stream) cudaStreamDestroy(c->stream);
+    cudaStreamSynchronize(c->aux_stream);
     delete c;
     return 0;
 }
@@ -217,13 +207,13 @@ extern "C" int isdf_get_stats(isdf_ctx *c, isdf_stats *out) {
 extern "C" int isdf_set_shard(isdf_ctx *c, int rank, int world) {
     if (!c || world < 1 || rank < 0 || rank >= world) return fail(ISDF_ERR_INVALID, "bad shard");
     if (world > c->cfg.integral_intervs + 1) return fail(ISDF_ERR_INVALID, "world larger than samples per piece");
-    c->rank = rank; c->world = world; c->order_for = -1;
+    c->rank = rank; c->world = world; c->disc.order_for = -1;
     return 0;
 }
 
 // ---- shapes ---------------------------------------------------------------------------------------------------
 static void shape_common(isdf_ctx *c, const double *rot, const double *trans) {
-    DevShape &s = c->shape;
+    DevShape &s = c->mesh.shape;
     const double I[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
     for (int i = 0; i < 9; i++) s.rot[i] = rot ? rot[i] : I[i];
     for (int i = 0; i < 3; i++) s.trans[i] = trans ? trans[i] : 0.0;
@@ -242,12 +232,12 @@ extern "C" int isdf_set_shape_analytic(isdf_ctx *c, int kind, const double *para
     if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
     if (kind < 0 || kind >= ISDF_SHAPE_MESH) return fail(ISDF_ERR_INVALID, "kind is not an analytic shape");
     if (nparams < 0 || nparams > 12 || (nparams > 0 && !params)) return fail(ISDF_ERR_INVALID, "bad params");
-    std::memset(&c->shape, 0, sizeof(c->shape));
-    c->shape.kind = kind;
-    for (int i = 0; i < nparams; i++) c->shape.par[i] = params[i];
+    std::memset(&c->mesh.shape, 0, sizeof(c->mesh.shape));
+    c->mesh.shape.kind = kind;
+    for (int i = 0; i < nparams; i++) c->mesh.shape.par[i] = params[i];
     shape_common(c, rot, trans);
-    c->have_shape = true; c->fe_ready = false;
-    c->order_for = -1;   // work items of another shape class may carry split slots
+    c->mesh.have_shape = true; c->fe.ready = false;
+    c->disc.order_for = -1;   // work items of another shape class may carry split slots
     return 0;
 }
 
@@ -301,34 +291,37 @@ extern "C" int isdf_set_shape_mesh_ex(isdf_ctx *c, const double *V, int nV, cons
     // 2*safety_hor + 0.1 >= safety_hor
     if (!build_host_mesh(V, nV, F, nF, poly_params, c->cfg.safety_hor, hm, err, sign_mode))
         return fail(err.find("not a closed") != std::string::npos ? ISDF_ERR_UNSUPPORTED : ISDF_ERR_INVALID, err);
-    if (!hm.wn.empty()) CU_TRY(c->d_wn.upload(hm.wn.data(), hm.wn.size(), c->stream));
-    CU_TRY(c->d_nodes.upload(hm.nodes.data(), hm.nodes.size(), c->stream));
-    CU_TRY(c->d_wnodes.upload(hm.wnodes.data(), hm.wnodes.size(), c->stream));
-    CU_TRY(c->d_tris.upload(hm.tris.data(), hm.tris.size(), c->stream));
-    CU_TRY(c->d_pn.upload(hm.pnormals.data(), hm.pnormals.size(), c->stream));
-    CU_TRY(c->d_obb.upload(hm.leaf_obb.data(), hm.leaf_obb.size(), c->stream));
+    // the uploads may reallocate the buffers the current shape lives in: give it up (and what was built on it) first
+    c->mesh.have_shape = false; c->fe.ready = false;
+    c->disc.order_for = -1;
+    if (!hm.wn.empty()) CU_TRY(c->mesh.d_wn.upload(hm.wn.data(), hm.wn.size(), c->stream));
+    CU_TRY(c->mesh.d_nodes.upload(hm.nodes.data(), hm.nodes.size(), c->stream));
+    CU_TRY(c->mesh.d_wnodes.upload(hm.wnodes.data(), hm.wnodes.size(), c->stream));
+    CU_TRY(c->mesh.d_tris.upload(hm.tris.data(), hm.tris.size(), c->stream));
+    CU_TRY(c->mesh.d_pn.upload(hm.pnormals.data(), hm.pnormals.size(), c->stream));
+    CU_TRY(c->mesh.d_obb.upload(hm.leaf_obb.data(), hm.leaf_obb.size(), c->stream));
     CU_TRY(cudaStreamSynchronize(c->stream));
-    std::memset(&c->shape, 0, sizeof(c->shape));
-    c->shape.kind = ISDF_SHAPE_MESH;
+    std::memset(&c->mesh.shape, 0, sizeof(c->mesh.shape));
+    c->mesh.shape.kind = ISDF_SHAPE_MESH;
     shape_common(c, nullptr, nullptr);
     DevMesh m = hm.view();
-    m.nodes = c->d_nodes.p; m.wnodes = c->d_wnodes.p; m.tris = c->d_tris.p; m.pnormals = c->d_pn.p; m.leaf_obb = c->d_obb.p;
-    m.wn = hm.wn.empty() ? nullptr : c->d_wn.p;
+    m.nodes = c->mesh.d_nodes.p; m.wnodes = c->mesh.d_wnodes.p; m.tris = c->mesh.d_tris.p; m.pnormals = c->mesh.d_pn.p; m.leaf_obb = c->mesh.d_obb.p;
+    m.wn = hm.wn.empty() ? nullptr : c->mesh.d_wn.p;
     // per-cell signed distance + seed triangle, computed on the device with the freshly uploaded BVH
     const size_t ncell = (size_t)m.gdim[0] * m.gdim[1] * m.gdim[2];
-    CU_TRY(c->d_cell_dist.ensure(ncell));
-    CU_TRY(c->d_cell_seed.ensure(ncell));
+    CU_TRY(c->mesh.d_cell_dist.ensure(ncell));
+    CU_TRY(c->mesh.d_cell_seed.ensure(ncell));
     {
         DevMesh build = m;
         build.gdim[0] = 0;            // no grid while it is being built: plain unbounded BVH queries
         build.cell_dist = nullptr; build.cell_seed = nullptr; build.cell_off = nullptr; build.cell_cnt = nullptr; build.cand = nullptr; build.cand_lb = nullptr;
         k_mesh_cells<<<(unsigned)((ncell + 127) / 128), 128, 0, c->stream>>>(build, m.gdim[0], m.gdim[1], m.gdim[2], m.glo[0], m.glo[1], m.glo[2],
-                                                                           m.gcell, c->d_cell_dist.p, c->d_cell_seed.p);
+                                                                           m.gcell, c->mesh.d_cell_dist.p, c->mesh.d_cell_seed.p);
         c->stats.kernel_launches++;
         CU_TRY(cudaGetLastError());
         CU_TRY(cudaStreamSynchronize(c->stream));
     }
-    m.cell_dist = c->d_cell_dist.p; m.cell_seed = c->d_cell_seed.p;
+    m.cell_dist = c->mesh.d_cell_dist.p; m.cell_seed = c->mesh.d_cell_seed.p;
     m.cell_off = nullptr; m.cell_cnt = nullptr; m.cand = nullptr; m.cand_lb = nullptr;
     // exact candidate lists for every cell a query can land in and not be settled by the cell's distance bracket alone: the discrete
     // path queries within safety_hor of the surface, the swept-volume path within its range bound 2*safety_hor + 0.1 (swm:383) — a
@@ -337,26 +330,26 @@ extern "C" int isdf_set_shape_mesh_ex(isdf_ctx *c, const double *V, int nV, cons
     {
         const double hd = 0.5 * std::sqrt(3.0) * m.gcell;
         const double list_reach = std::max(c->cfg.safety_hor, 2.0 * c->cfg.safety_hor + 0.1) + 2.0 * m.ghd;
-        c->mesh_list_reach = list_reach;
-        CU_TRY(c->d_cell_cnt.ensure(ncell)); CU_TRY(c->d_cell_off.ensure(ncell));
+        c->mesh.list_reach = list_reach;
+        CU_TRY(c->mesh.d_cell_cnt.ensure(ncell)); CU_TRY(c->mesh.d_cell_off.ensure(ncell));
         const unsigned warps_grid = (unsigned)((ncell + 3) / 4);
-        k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->d_cell_cnt.p, nullptr, nullptr, nullptr);
+        k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->mesh.d_cell_cnt.p, nullptr, nullptr, nullptr);
         c->stats.kernel_launches++;
         CU_TRY(cudaGetLastError());
         std::vector<uint16_t> cnt(ncell);
-        CU_TRY(cudaMemcpyAsync(cnt.data(), c->d_cell_cnt.p, sizeof(uint16_t) * ncell, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaMemcpyAsync(cnt.data(), c->mesh.d_cell_cnt.p, sizeof(uint16_t) * ncell, cudaMemcpyDeviceToHost, c->stream));
         CU_TRY(cudaStreamSynchronize(c->stream));
         std::vector<uint32_t> off(ncell);
         size_t total = 0;
         for (size_t i = 0; i < ncell; i++) { off[i] = (uint32_t)total; total += cnt[i]; }
         if (total > 0 && total < (1ull << 31)) {
-            CU_TRY(c->d_cand.ensure(total)); CU_TRY(c->d_cand_lb.ensure(total));
-            CU_TRY(cudaMemcpyAsync(c->d_cell_off.p, off.data(), sizeof(uint32_t) * ncell, cudaMemcpyHostToDevice, c->stream));
-            k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->d_cell_cnt.p, c->d_cell_off.p, c->d_cand.p, c->d_cand_lb.p);
+            CU_TRY(c->mesh.d_cand.ensure(total)); CU_TRY(c->mesh.d_cand_lb.ensure(total));
+            CU_TRY(cudaMemcpyAsync(c->mesh.d_cell_off.p, off.data(), sizeof(uint32_t) * ncell, cudaMemcpyHostToDevice, c->stream));
+            k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->mesh.d_cell_cnt.p, c->mesh.d_cell_off.p, c->mesh.d_cand.p, c->mesh.d_cand_lb.p);
             c->stats.kernel_launches++;
             CU_TRY(cudaGetLastError());
             CU_TRY(cudaStreamSynchronize(c->stream));
-            m.cell_off = c->d_cell_off.p; m.cell_cnt = c->d_cell_cnt.p; m.cand = c->d_cand.p; m.cand_lb = c->d_cand_lb.p;
+            m.cell_off = c->mesh.d_cell_off.p; m.cell_cnt = c->mesh.d_cell_cnt.p; m.cand = c->mesh.d_cand.p; m.cand_lb = c->mesh.d_cand_lb.p;
         }
         if (getenv("ISDF_VERBOSE")) {
             size_t listed = 0; for (size_t i = 0; i < ncell; i++) listed += cnt[i] != 0;
@@ -365,15 +358,14 @@ extern "C" int isdf_set_shape_mesh_ex(isdf_ctx *c, const double *V, int nV, cons
         }
     }
     // fused 16-byte cell records for the discrete scan kernel's cull stage
-    CU_TRY(c->d_cell_rec.ensure(ncell));
-    k_mesh_cell_pack<<<(unsigned)((ncell + 255) / 256), 256, 0, c->stream>>>((long long)ncell, m.cell_dist, m.cell_seed, m.cell_off, m.cell_cnt, c->d_cell_rec.p);
+    CU_TRY(c->mesh.d_cell_rec.ensure(ncell));
+    k_mesh_cell_pack<<<(unsigned)((ncell + 255) / 256), 256, 0, c->stream>>>((long long)ncell, m.cell_dist, m.cell_seed, m.cell_off, m.cell_cnt, c->mesh.d_cell_rec.p);
     c->stats.kernel_launches++;
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaStreamSynchronize(c->stream));
-    m.cell_rec = c->d_cell_rec.p;
-    c->shape.mesh = m;
-    c->have_shape = true; c->fe_ready = false;
-    c->order_for = -1;
+    m.cell_rec = c->mesh.d_cell_rec.p;
+    c->mesh.shape.mesh = m;
+    c->mesh.have_shape = true;
     return 0;
 }
 
@@ -467,14 +459,14 @@ __global__ void k_shape_query(const __grid_constant__ DevShape S, const double *
 
 extern "C" int isdf_shape_query(isdf_ctx *c, const double *p_rel, int n, double *sdf, double *grad, int what) {
     if (!c || !p_rel || n < 0) return fail(ISDF_ERR_INVALID, "bad argument");
-    if (!c->have_shape) return fail(ISDF_ERR_STATE, "shape not set");
+    if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
     if (what < 0 || what > 2) return fail(ISDF_ERR_INVALID, "bad query kind");
     if (n == 0) return 0;
     if (set_device(c)) return ISDF_ERR_CUDA;
-    ScopedDevBuf<double> dp, ds, dg;
+    DevBuf<double> dp, ds, dg;
     CU_TRY(dp.upload(p_rel, (size_t)3 * n, c->stream));
     CU_TRY(ds.ensure(n)); CU_TRY(dg.ensure((size_t)3 * n));
-    k_shape_query<<<(n + 127) / 128, 128, 0, c->stream>>>(c->shape, dp.p, n, ds.p, dg.p, what);
+    k_shape_query<<<(n + 127) / 128, 128, 0, c->stream>>>(c->mesh.shape, dp.p, n, ds.p, dg.p, what);
     c->stats.kernel_launches++;
     CU_TRY(cudaGetLastError());
     std::vector<double> hs(n), hg((size_t)3 * n);
@@ -498,13 +490,13 @@ static int map_size_check(isdf_ctx *c, long long X, long long Y, long long Z, do
     return 0;
 }
 
-// the map the bits in c->d_bits describe
+// the map the bits in c->map.d_bits describe
 static void commit_map(isdf_ctx *c, int X, int Y, int Z, const double *bmin, const double *bmax, double res, long long used, long long skipped) {
-    DevGrid &g = c->grid;
-    g.bits = c->d_bits.p; g.X = X; g.Y = Y; g.Z = Z; g.Zw = (Z + 31) / 32; g.res = res;
+    DevGrid &g = c->map.grid;
+    g.bits = c->map.d_bits.p; g.X = X; g.Y = Y; g.Z = Z; g.Zw = (Z + 31) / 32; g.res = res;
     for (int a = 0; a < 3; a++) { g.bmin[a] = bmin[a]; g.bmax[a] = bmax[a]; }
-    c->map_points_used = used; c->map_points_skipped = skipped;
-    c->have_map = true;
+    c->map.points_used = used; c->map.points_skipped = skipped;
+    c->map.have_map = true;
 }
 
 template <typename T>
@@ -513,21 +505,20 @@ static int set_map_impl(isdf_ctx *c, const T *occ, int X, int Y, int Z, const do
     if (X < 1 || Y < 1 || Z < 1 || !(res > 0)) return fail(ISDF_ERR_INVALID, "bad map size");
     if (int rc = map_size_check(c, X, Y, Z, res)) return rc;
     if (set_device(c)) return ISDF_ERR_CUDA;
+    c->map.have_map = false;   // d_bits.ensure may free the current grid
     const size_t nvox = (size_t)X * Y * Z;
-    T *d_occ = nullptr;
-    CU_TRY(cudaMalloc((void **)&d_occ, nvox * sizeof(T)));
-    cudaError_t e = cudaMemcpyAsync(d_occ, occ, nvox * sizeof(T), cudaMemcpyHostToDevice, c->stream);
+    DevBuf<T> d_occ;
+    cudaError_t e = d_occ.upload(occ, nvox, c->stream);
     const int Zw = (Z + 31) / 32;
     const size_t nwords = (size_t)X * Y * Zw;
-    if (e == cudaSuccess) e = c->d_bits.ensure(nwords);
+    if (e == cudaSuccess) e = c->map.d_bits.ensure(nwords);
     if (e == cudaSuccess) {
         const long long threads = (long long)nwords * 32;
-        k_pack_bits<<<(unsigned)((threads + 255) / 256), 256, 0, c->stream>>>(NonZero<T>{d_occ}, c->d_bits.p, X * Y, Z, Zw);
+        k_pack_bits<<<(unsigned)((threads + 255) / 256), 256, 0, c->stream>>>(NonZero<T>{d_occ.p}, c->map.d_bits.p, X * Y, Z, Zw);
         c->stats.kernel_launches++;
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    cudaFree(d_occ);
     if (e != cudaSuccess) return fail(ISDF_ERR_CUDA, std::string("isdf_set_map: ") + cudaGetErrorString(e));
     const int dims[3] = {X, Y, Z};
     double bmax[3];
@@ -561,13 +552,13 @@ static int cloud_grid_blocks(isdf_ctx *c, long long n) { return (int)std::min<lo
 static int set_map_cloud_impl(isdf_ctx *c, const char *d_pts, long long n, int stride, double res, int thr, cudaStream_t st) {
     const int blocks = cloud_grid_blocks(c, n);
     auto cuda_fail = [&](cudaError_t e) {
-        c->have_map = false;
+        c->map.have_map = false;
         return fail(ISDF_ERR_CUDA, std::string("isdf_set_map_cloud: ") + cudaGetErrorString(e));
     };
     // 1. bounds: exact float extrema of the finite records (order-preserving uint32 min / max) and the number of skipped records
     uint32_t ext[7];
     {
-        ScopedDevBuf<uint32_t> d_ext;
+        DevBuf<uint32_t> d_ext;
         cudaError_t e = d_ext.ensure(7);
         if (e == cudaSuccess) e = cudaMemsetAsync(d_ext.p, 0xff, 3 * sizeof(uint32_t), st);
         if (e == cudaSuccess) e = cudaMemsetAsync(d_ext.p + 3, 0, 4 * sizeof(uint32_t), st);
@@ -602,24 +593,24 @@ static int set_map_cloud_impl(isdf_ctx *c, const char *d_pts, long long n, int s
     const int X = (int)dim[0], Y = (int)dim[1], Z = (int)dim[2];
     if (int rc = map_size_check(c, X, Y, Z, res)) return fail(rc, g_err + dims_msg);
     // 3. occupancy (the previous map is given up from here on)
-    c->have_map = false;
+    c->map.have_map = false;
     CloudFrame F;
     for (int a = 0; a < 3; a++) F.bmin[a] = bmin[a];
     F.res = res; F.X = X; F.Y = Y; F.Z = Z; F.Zw = (Z + 31) / 32;
     const size_t nwords = (size_t)X * Y * F.Zw;
-    cudaError_t e = c->d_bits.ensure(nwords);
+    cudaError_t e = c->map.d_bits.ensure(nwords);
     if (e != cudaSuccess) return cuda_fail(e);
     const long long pack_threads = (long long)nwords * 32;
     const unsigned pack_blocks = (unsigned)((pack_threads + 255) / 256);
-    ScopedDevBuf<uint32_t> d_cnt;   // sta_threshold > 1: per-voxel counts, freed after the final synchronise
+    DevBuf<uint32_t> d_cnt;   // sta_threshold > 1: per-voxel counts, freed after the final synchronise
     if (thr <= 0) {
-        k_pack_bits<<<pack_blocks, 256, 0, c->stream>>>(AllSet{}, c->d_bits.p, X * Y, Z, F.Zw);
+        k_pack_bits<<<pack_blocks, 256, 0, c->stream>>>(AllSet{}, c->map.d_bits.p, X * Y, Z, F.Zw);
         c->stats.kernel_launches++;
         e = cudaGetLastError();
     } else if (thr == 1) {
-        e = cudaMemsetAsync(c->d_bits.p, 0, nwords * sizeof(uint32_t), c->stream);
+        e = cudaMemsetAsync(c->map.d_bits.p, 0, nwords * sizeof(uint32_t), c->stream);
         if (e == cudaSuccess) {
-            k_cloud_mark<<<blocks, 256, 0, c->stream>>>(d_pts, n, stride, F, c->d_bits.p);
+            k_cloud_mark<<<blocks, 256, 0, c->stream>>>(d_pts, n, stride, F, c->map.d_bits.p);
             c->stats.kernel_launches++;
             e = cudaGetLastError();
         }
@@ -629,7 +620,7 @@ static int set_map_cloud_impl(isdf_ctx *c, const char *d_pts, long long n, int s
         if (e == cudaSuccess) e = cudaMemsetAsync(d_cnt.p, 0, nvox * sizeof(uint32_t), c->stream);
         if (e == cudaSuccess) {
             k_cloud_count<<<blocks, 256, 0, c->stream>>>(d_pts, n, stride, F, d_cnt.p);
-            k_pack_bits<<<pack_blocks, 256, 0, c->stream>>>(CountAtLeast{d_cnt.p, (uint32_t)thr}, c->d_bits.p, X * Y, Z, F.Zw);
+            k_pack_bits<<<pack_blocks, 256, 0, c->stream>>>(CountAtLeast{d_cnt.p, (uint32_t)thr}, c->map.d_bits.p, X * Y, Z, F.Zw);
             c->stats.kernel_launches += 2;
             e = cudaGetLastError();
         }
@@ -643,12 +634,12 @@ static int set_map_cloud_impl(isdf_ctx *c, const char *d_pts, long long n, int s
 extern "C" int isdf_set_map_cloud(isdf_ctx *c, const void *points, int64_t n, int32_t stride_bytes, double res, int32_t sta_threshold) {
     if (int rc = cloud_args_check(c, points, n, stride_bytes, res)) return rc;
     if (set_device(c)) return ISDF_ERR_CUDA;
-    ScopedDevBuf<char> d_pts;
+    DevBuf<char> d_pts;
     const size_t bytes = (size_t)n * stride_bytes;
     cudaError_t e = d_pts.ensure(bytes);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_pts.p, points, bytes, cudaMemcpyHostToDevice, c->stream);
     if (e != cudaSuccess) {
-        c->have_map = false;
+        c->map.have_map = false;
         return fail(ISDF_ERR_CUDA, std::string("isdf_set_map_cloud: ") + cudaGetErrorString(e));
     }
     return set_map_cloud_impl(c, d_pts.p, n, stride_bytes, res, sta_threshold, c->stream);
@@ -663,10 +654,10 @@ extern "C" int isdf_set_map_cloud_device(isdf_ctx *c, const void *d_points, int6
 
 extern "C" int isdf_get_map_info(isdf_ctx *c, isdf_map_info *out) {
     if (!c || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
-    if (!c->have_map) return fail(ISDF_ERR_STATE, "map not set");
+    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    const DevGrid &g = c->grid;
-    ScopedDevBuf<unsigned long long> d_pop;
+    const DevGrid &g = c->map.grid;
+    DevBuf<unsigned long long> d_pop;
     unsigned long long pop = 0;
     const long long nwords = (long long)g.X * g.Y * g.Zw;
     CU_TRY(d_pop.ensure(1));
@@ -680,7 +671,7 @@ extern "C" int isdf_get_map_info(isdf_ctx *c, isdf_map_info *out) {
     out->X = g.X; out->Y = g.Y; out->Z = g.Z; out->res = g.res;
     for (int a = 0; a < 3; a++) { out->bmin[a] = g.bmin[a]; out->bmax[a] = g.bmax[a]; }
     out->occupied_voxels = (int64_t)pop;
-    out->points_used = c->map_points_used; out->points_skipped = c->map_points_skipped;
+    out->points_used = c->map.points_used; out->points_skipped = c->map.points_skipped;
     return 0;
 }
 
@@ -688,13 +679,13 @@ extern "C" int isdf_get_map_info(isdf_ctx *c, isdf_map_info *out) {
 template <typename T>
 static int get_map_impl(isdf_ctx *c, T *out, int64_t n) {
     if (!c || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
-    if (!c->have_map) return fail(ISDF_ERR_STATE, "map not set");
-    const DevGrid &g = c->grid;
+    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
+    const DevGrid &g = c->map.grid;
     const long long rows = (long long)g.X * g.Y;
     if (n != rows * g.Z) return fail(ISDF_ERR_INVALID, "n must be X*Y*Z of the map");
     if (set_device(c)) return ISDF_ERR_CUDA;
     const long long chunk_rows = std::max<long long>(1, (32ll << 20) / ((long long)g.Z * sizeof(T)));   // <= 32 MiB of scratch per chunk
-    ScopedDevBuf<T> d_out;
+    DevBuf<T> d_out;
     CU_TRY(d_out.ensure((size_t)std::min(rows, chunk_rows) * g.Z));
     for (long long r0 = 0; r0 < rows; r0 += chunk_rows) {
         const int nr = (int)std::min(chunk_rows, rows - r0);
@@ -759,11 +750,11 @@ __global__ void __launch_bounds__(256) k_points_in_aabb(const DevGrid G, double 
 
 extern "C" int isdf_points_in_aabb(isdf_ctx *c, const double *centre, double half_extent, double *out_points, int cap, int *n) {
     if (!c || !centre || !n || cap < 0 || (cap > 0 && !out_points)) return fail(ISDF_ERR_INVALID, "bad argument");
-    if (!c->have_map) return fail(ISDF_ERR_STATE, "map not set");
+    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    ScopedDevBuf<double> d; ScopedDevBuf<int> dn;
+    DevBuf<double> d; DevBuf<int> dn;
     CU_TRY(d.ensure((size_t)3 * (cap > 0 ? cap : 1))); CU_TRY(dn.ensure(1));
-    k_points_in_aabb<<<1, 256, 0, c->stream>>>(c->grid, centre[0], centre[1], centre[2], half_extent, d.p, cap, dn.p);
+    k_points_in_aabb<<<1, 256, 0, c->stream>>>(c->map.grid, centre[0], centre[1], centre[2], half_extent, d.p, cap, dn.p);
     c->stats.kernel_launches++;
     CU_TRY(cudaGetLastError());
     int cnt = 0;
@@ -843,16 +834,16 @@ __global__ void __launch_bounds__(256) k_gather_points(const DevGrid G, int nQ, 
 extern "C" int isdf_gather_obstacle_points(isdf_ctx *c, const double *waypoints, int nQ, double half_extent, const double *offset,
                                            double *out_points, int cap, int *n, int set_as_points) {
     if (!c || !waypoints || nQ < 1 || !n || cap < 0 || (cap > 0 && !out_points && !set_as_points)) return fail(ISDF_ERR_INVALID, "bad argument");
-    if (!c->have_map) return fail(ISDF_ERR_STATE, "map not set");
+    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    ScopedDevBuf<double> dw, dout; ScopedDevBuf<GatherBox> db; ScopedDevBuf<int> dn;
+    DevBuf<double> dw, dout; DevBuf<GatherBox> db; DevBuf<int> dn;
     const int capd = cap > 0 ? cap : 1;
     CU_TRY(dw.upload(waypoints, (size_t)3 * nQ, c->stream));
     CU_TRY(dout.ensure((size_t)3 * capd)); CU_TRY(db.ensure(nQ)); CU_TRY(dn.ensure((size_t)nQ + 1));
     const double ox = offset ? offset[0] : 0.0, oy = offset ? offset[1] : 0.0, oz = offset ? offset[2] : 0.0;
-    k_gather_boxes<<<(nQ + 127) / 128, 128, 0, c->stream>>>(c->grid, dw.p, nQ, half_extent, ox, oy, oz, db.p);
-    k_gather_points<false><<<nQ, 256, 0, c->stream>>>(c->grid, nQ, db.p, dn.p + 1, nullptr, 0, dn.p);
-    k_gather_points<true><<<nQ, 256, 0, c->stream>>>(c->grid, nQ, db.p, dn.p + 1, dout.p, capd, dn.p);
+    k_gather_boxes<<<(nQ + 127) / 128, 128, 0, c->stream>>>(c->map.grid, dw.p, nQ, half_extent, ox, oy, oz, db.p);
+    k_gather_points<false><<<nQ, 256, 0, c->stream>>>(c->map.grid, nQ, db.p, dn.p + 1, nullptr, 0, dn.p);
+    k_gather_points<true><<<nQ, 256, 0, c->stream>>>(c->map.grid, nQ, db.p, dn.p + 1, dout.p, capd, dn.p);
     c->stats.kernel_launches += 3;
     CU_TRY(cudaGetLastError());
     int cnt = 0;
@@ -875,76 +866,86 @@ extern "C" int isdf_gather_obstacle_points(isdf_ctx *c, const double *waypoints,
 }
 
 // ---- discrete evaluation ------------------------------------------------------------------------------------
+// whether a sharded *_device evaluation finishes with the peer exchange (an unsharded call, isdf_set_shard(ctx, 0, 1), stays local)
+static bool fused_exchange(const isdf_ctx *c) { return c->peer.fused && c->peer.args.world > 1 && c->world > 1; }
+
+// what the exchange needs for an evaluation of N pieces. The caller commits the next epoch only once its exchange is enqueued: a
+// local failure must not leave this rank one epoch ahead.
+static int peer_fuse_check(const isdf_ctx *c, int N) {
+    if (c->peer.args.world != c->world || c->peer.args.rank != c->rank) return fail(ISDF_ERR_STATE, "peer group does not match isdf_set_shard");
+    if (19 * N + 1 > c->peer.args.cap) return fail(ISDF_ERR_INVALID, "peer exchange buffer too small for this N (isdf_peer_export max_doubles)");
+    return 0;
+}
+
 static int launch_discrete(isdf_ctx *c, int N, const double *d_T, const double *d_C, double *d_out, cudaStream_t st) {
     const int K = c->cfg.integral_intervs;
     const long long S = (long long)N * (K + 1);
     if (S > 0x7fffffffll) return fail(ISDF_ERR_UNSUPPORTED, "N * (integral_intervs + 1) must fit in 31 bits");
-    CU_TRY(c->d_piece_cost.ensure(N));
-    if (c->d_tickets.n < 2) {   // [0] pieces_done of the epilogue, [1] work-item cursor of the persistent scan warps
-        CU_TRY(c->d_tickets.ensure(2));
-        CU_TRY(cudaMemsetAsync(c->d_tickets.p, 0, 2 * sizeof(int), st));
+    CU_TRY(c->disc.d_piece_cost.ensure(N));
+    if (c->disc.d_tickets.n < 2) {   // [0] pieces_done of the epilogue, [1] work-item cursor of the persistent scan warps
+        CU_TRY(c->disc.d_tickets.ensure(2));
+        CU_TRY(cudaMemsetAsync(c->disc.d_tickets.p, 0, 2 * sizeof(int), st));
     }
-    CU_TRY(c->d_tot.ensure((size_t)S * 8));
+    CU_TRY(c->disc.d_tot.ensure((size_t)S * 8));
     DiscArgs A;
-    A.cfg = c->dcfg; A.grid = c->grid; A.shape = c->shape; A.N = N; A.T = d_T; A.C = d_C;
-    A.tot = c->d_tot.p; A.pieces_done = c->d_tickets.p; A.item_cursor = c->d_tickets.p + 1;
-    A.piece_cost = c->d_piece_cost.p; A.out = d_out; A.pair_counter = c->d_counter.p; A.count_out = c->count_out_dev;
+    A.cfg = c->dcfg; A.grid = c->map.grid; A.shape = c->mesh.shape; A.N = N; A.T = d_T; A.C = d_C;
+    A.tot = c->disc.d_tot.p; A.pieces_done = c->disc.d_tickets.p; A.item_cursor = c->disc.d_tickets.p + 1;
+    A.piece_cost = c->disc.d_piece_cost.p; A.out = d_out; A.pair_counter = c->disc.d_counter.p; A.count_out = c->disc.count_out_dev;
     A.rank = c->rank; A.world = c->world;
     A.peer = PeerArgs{};
-    const bool fused = c->peer_fused && c->peer.world > 1 && c->world > 1;   // an unsharded call (isdf_set_shard(ctx, 0, 1)) stays local
+    const bool fused = fused_exchange(c);
     if (fused) {
-        if (c->peer.world != c->world || c->peer.rank != c->rank) return fail(ISDF_ERR_STATE, "peer group does not match isdf_set_shard");
-        if (19 * N + 1 > c->peer.cap) return fail(ISDF_ERR_INVALID, "peer exchange buffer too small for this N (isdf_peer_export max_doubles)");
-        A.peer = c->peer; A.peer.epoch = c->peer.epoch + 1;   // committed below, once the exchange kernel is really enqueued
+        if (int r = peer_fuse_check(c, N)) return r;
+        A.peer = c->peer.args; A.peer.epoch = c->peer.args.epoch + 1;   // committed below, once the exchange kernel is really enqueued
     }
     A.dbg = nullptr;
     A.trace = nullptr;
-    if (c->dbg_on) { CU_TRY(c->d_dbg.ensure((size_t)3 * S)); CU_TRY(cudaMemsetAsync(c->d_dbg.p, 0, sizeof(unsigned long long) * 3 * S, st)); A.dbg = c->d_dbg.p; }
+    if (c->dbg_on) { CU_TRY(c->disc.d_dbg.ensure((size_t)3 * S)); CU_TRY(cudaMemsetAsync(c->disc.d_dbg.p, 0, sizeof(unsigned long long) * 3 * S, st)); A.dbg = c->disc.d_dbg.p; }
     const long long M = (S - c->rank + c->world - 1) / c->world;
-    CU_TRY(cudaMemsetAsync(c->d_counter.p, 0, sizeof(unsigned long long), st));
+    CU_TRY(cudaMemsetAsync(c->disc.d_counter.p, 0, sizeof(unsigned long long), st));
     // longest-first order from the previous evaluation of the same problem shape (first evaluation: natural order)
     const long long sig = ((long long)N << 20) ^ ((long long)c->rank << 10) ^ c->world ^ ((long long)K << 40);
-    const bool mesh = (c->shape.kind == ISDF_SHAPE_MESH);
+    const bool mesh = (c->mesh.shape.kind == ISDF_SHAPE_MESH);
     // only mesh samples have a heavy tail worth splitting. Every sample of a launch may be split (item trace at world = 8:
     // with M/4 slots the 515 heaviest samples were split and the NEXT heaviest — unsplit, 15-25 queries, 80-110 us — set the kernel time)
     const int max_split = mesh ? (int)std::min<long long>(M, MAX_SPLIT_SLOTS) : 0;
     const size_t max_items = (size_t)M + (size_t)(ROW_CLASSES - 1) * max_split;
-    CU_TRY(c->d_work.ensure((size_t)S));
-    if (c->d_items.n < 3 * max_items + (size_t)M) { CU_TRY(c->d_items.ensure(3 * max_items + (size_t)M)); c->order_for = -1; }   // a regrown table holds no items yet
-    CU_TRY(c->d_item_count.ensure(1));
-    CU_TRY(c->d_subsum.ensure((size_t)std::max(max_split, 1) * ROW_CLASSES * 8));
-    if (c->d_split_work.n < (size_t)std::max(max_split, 1)) {
-        CU_TRY(c->d_split_work.ensure((size_t)std::max(max_split, 1)));
-        CU_TRY(cudaMemsetAsync(c->d_split_work.p, 0, sizeof(unsigned) * std::max(max_split, 1), st));
+    CU_TRY(c->disc.d_work.ensure((size_t)S));
+    if (c->disc.d_items.n < 3 * max_items + (size_t)M) { CU_TRY(c->disc.d_items.ensure(3 * max_items + (size_t)M)); c->disc.order_for = -1; }   // a regrown table holds no items yet
+    CU_TRY(c->disc.d_item_count.ensure(1));
+    CU_TRY(c->disc.d_subsum.ensure((size_t)std::max(max_split, 1) * ROW_CLASSES * 8));
+    if (c->disc.d_split_work.n < (size_t)std::max(max_split, 1)) {
+        CU_TRY(c->disc.d_split_work.ensure((size_t)std::max(max_split, 1)));
+        CU_TRY(cudaMemsetAsync(c->disc.d_split_work.p, 0, sizeof(unsigned) * std::max(max_split, 1), st));
     }
-    if (c->d_split_done.n < (size_t)std::max(max_split, 1)) {
-        CU_TRY(c->d_split_done.ensure((size_t)std::max(max_split, 1)));
-        CU_TRY(cudaMemsetAsync(c->d_split_done.p, 0, sizeof(unsigned) * std::max(max_split, 1), st));
+    if (c->disc.d_split_done.n < (size_t)std::max(max_split, 1)) {
+        CU_TRY(c->disc.d_split_done.ensure((size_t)std::max(max_split, 1)));
+        CU_TRY(cudaMemsetAsync(c->disc.d_split_done.p, 0, sizeof(unsigned) * std::max(max_split, 1), st));
     }
-    A.work = c->d_work.p;
-    if (c->dbg_on) { CU_TRY(c->d_trace.ensure(TRACE_STRIDE * max_items)); CU_TRY(cudaMemsetAsync(c->d_trace.p, 0, sizeof(unsigned long long) * TRACE_STRIDE * max_items, st)); A.trace = c->d_trace.p; }
+    A.work = c->disc.d_work.p;
+    if (c->dbg_on) { CU_TRY(c->disc.d_trace.ensure(TRACE_STRIDE * max_items)); CU_TRY(cudaMemsetAsync(c->disc.d_trace.p, 0, sizeof(unsigned long long) * TRACE_STRIDE * max_items, st)); A.trace = c->disc.d_trace.p; }
     // a launch with far more samples than resident warps (batched callbacks: millions) balances itself through the persistent warps'
     // dynamic item counter: sorting / splitting would only cost a long single-CTA pass over the work array
-    const bool want_items = !c->no_items && M <= 1024ll * ITEMS_CACHE * 4;
-    const bool have_items = (c->order_for == sig) && want_items;
-    A.items = have_items ? c->d_items.p : nullptr;
-    A.item_count = c->d_item_count.p; A.subsum = c->d_subsum.p; A.split_work = c->d_split_work.p; A.split_done = c->d_split_done.p;
+    const bool want_items = !c->disc.no_items && M <= 1024ll * ITEMS_CACHE * 4;
+    const bool have_items = (c->disc.order_for == sig) && want_items;
+    A.items = have_items ? c->disc.d_items.p : nullptr;
+    A.item_count = c->disc.d_item_count.p; A.subsum = c->disc.d_subsum.p; A.split_work = c->disc.d_split_work.p; A.split_done = c->disc.d_split_done.p;
     // persistent grid: one CTA per resident slot (or fewer when there are fewer items than warps)
     const long long want = ((have_items ? (long long)max_items : M) + DISC_WARPS - 1) / DISC_WARPS;
     const long long resident = (long long)c->sm_count * (mesh ? c->mesh_blocks : c->analytic_blocks);
     const unsigned grid = (unsigned)std::max<long long>(1, std::min(want, resident));
-    if (c->items_pending) CU_TRY(cudaStreamWaitEvent(st, c->ev_items_done, 0));   // the table this launch reads (or overwrites next)
+    if (c->disc.items_pending) CU_TRY(cudaStreamWaitEvent(st, c->ev_items_done, 0));   // the table this launch reads (or overwrites next)
     CU_TRY(discrete_launch_scan(A, mesh, grid, st));
     CU_TRY(discrete_launch_epilogue(A, st));
-    if (fused) c->peer.epoch = A.peer.epoch;
+    if (fused) c->peer.args.epoch = A.peer.epoch;
     // build the next evaluation's work items on the aux stream: overlaps the caller's D2H / all-reduce / host work
     if (want_items) {
         CU_TRY(cudaEventRecord(c->ev_main_done, st));
         CU_TRY(cudaStreamWaitEvent(c->aux_stream, c->ev_main_done, 0));
-        CU_TRY(discrete_launch_build_items(c->d_work.p, c->rank, c->world, (int)M, max_split, c->warp_slots_override > 0 ? c->warp_slots_override : c->warp_slots, c->d_items.p, c->d_item_count.p, c->aux_stream));
+        CU_TRY(discrete_launch_build_items(c->disc.d_work.p, c->rank, c->world, (int)M, max_split, c->disc.warp_slots_override > 0 ? c->disc.warp_slots_override : c->warp_slots, c->disc.d_items.p, c->disc.d_item_count.p, c->aux_stream));
         CU_TRY(cudaEventRecord(c->ev_items_done, c->aux_stream));
-        c->items_pending = true;
-        c->order_for = sig;
+        c->disc.items_pending = true;
+        c->disc.order_for = sig;
         c->stats.kernel_launches++;   // work-item builder
     }
     c->stats.kernel_launches += 2;   // scan kernel, epilogue
@@ -956,8 +957,8 @@ static int check_eval_state(isdf_ctx *c, int N, bool need_map) {
     if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
     if (N < 1) return fail(ISDF_ERR_INVALID, "N < 1");
     const bool coll = (c->cfg.flags & ISDF_WITH_COLLISION) != 0;
-    if (coll && !c->have_shape) return fail(ISDF_ERR_STATE, "shape not set");
-    if (need_map && coll && !c->have_map) return fail(ISDF_ERR_STATE, "map not set");
+    if (coll && !c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
+    if (need_map && coll && !c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
     return 0;
 }
 
@@ -971,49 +972,62 @@ extern "C" int isdf_eval_discrete_device(isdf_ctx *c, int N, const double *d_T, 
 
 static void poison(double *cost) { if (cost) *cost = std::numeric_limits<double>::quiet_NaN(); }
 
-extern "C" int isdf_eval_discrete(isdf_ctx *c, int N, const double *T, const double *coeffs, double *cost, double *gradC, double *gradT) {
-    int r = check_eval_state(c, N, true);
-    if (r) { poison(cost); return r; }
-    if (!T || !coeffs || !cost || !gradC || !gradT) { poison(cost); return fail(ISDF_ERR_INVALID, "NULL argument"); }
+// The host form of the discrete and swept-volume evaluations: [coefficients 18N | durations N] go in through one pinned block and
+// ONE copy, `before` runs after that copy, `launch(d_T, d_C, d_out, count_out)` between ev0 and ev1, and [cost | gradC | gradT |
+// counter word] come back in ONE copy. The result is added to *cost, gradC and gradT, as the reference accumulates (hpp:539-550,
+// hpp:640-645); the counter word goes to the stat `counted`. On failure *cost is NaN.
+template <typename Before, typename Launch>
+static int eval_host(isdf_ctx *c, int N, const double *T, const double *coeffs, double *cost, double *gradC, double *gradT,
+                     int64_t isdf_stats::*counted, Before before, Launch launch) {
     auto body = [&]() -> int {
         if (set_device(c)) return ISDF_ERR_CUDA;
         const size_t nin = (size_t)19 * N, nout = (size_t)19 * N + 1;
-        // one pinned staging block, ONE copy each way: [coefficients 18N | durations N] in, [cost | gradC | gradT | pair count] out
-        if (ensure_stage(c, nin + nout + 1)) return ISDF_ERR_CUDA;
-        CU_TRY(c->d_C.ensure(nin)); CU_TRY(c->d_out.ensure(nout + 1));
-        std::memcpy(c->h_stage, coeffs, sizeof(double) * 18 * N);
-        std::memcpy(c->h_stage + 18 * (size_t)N, T, sizeof(double) * N);
-        CU_TRY(cudaMemcpyAsync(c->d_C.p, c->h_stage, sizeof(double) * nin, cudaMemcpyHostToDevice, c->stream));
+        CU_TRY(c->stage.h.ensure(nin + nout + 1));
+        CU_TRY(c->stage.d_C.ensure(nin)); CU_TRY(c->stage.d_out.ensure(nout + 1));
+        std::memcpy(c->stage.h.p, coeffs, sizeof(double) * 18 * N);
+        std::memcpy(c->stage.h.p + 18 * (size_t)N, T, sizeof(double) * N);
+        CU_TRY(cudaMemcpyAsync(c->stage.d_C.p, c->stage.h.p, sizeof(double) * nin, cudaMemcpyHostToDevice, c->stream));
+        if (int rr = before()) return rr;
         CU_TRY(cudaEventRecord(c->ev0, c->stream));
-        c->count_out_dev = c->d_out.p + nout;
-        int rr = launch_discrete(c, N, c->d_C.p + 18 * (size_t)N, c->d_C.p, c->d_out.p, c->stream);
-        c->count_out_dev = nullptr;
-        if (rr) return rr;
+        if (int rr = launch(c->stage.d_C.p + 18 * (size_t)N, c->stage.d_C.p, c->stage.d_out.p, c->stage.d_out.p + nout)) return rr;
         CU_TRY(cudaEventRecord(c->ev1, c->stream));
-        double *h_out = c->h_stage + nin;
-        CU_TRY(cudaMemcpyAsync(h_out, c->d_out.p, sizeof(double) * (nout + 1), cudaMemcpyDeviceToHost, c->stream));
+        double *h_out = c->stage.h.p + nin;
+        CU_TRY(cudaMemcpyAsync(h_out, c->stage.d_out.p, sizeof(double) * (nout + 1), cudaMemcpyDeviceToHost, c->stream));
         CU_TRY(cudaStreamSynchronize(c->stream));
-        unsigned long long pairs = 0;
-        std::memcpy(&pairs, h_out + nout, sizeof(pairs));
-        if (c->peer_fused && c->peer.world > 1 && c->world > 1 && isdf_peer_status(c) != ISDF_OK) return ISDF_ERR_CUDA;   // exchange timed out: the vector is NaN
+        unsigned long long count = 0;
+        std::memcpy(&count, h_out + nout, sizeof(count));
+        if (fused_exchange(c) && isdf_peer_status(c) != ISDF_OK) return ISDF_ERR_CUDA;   // exchange timed out: the vector is NaN
         float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
-        c->stats.last_kernel_ms = ms; c->stats.last_pairs = (int64_t)pairs;
-        *cost += h_out[0];                                   // accumulate like hpp:539-550
+        c->stats.last_kernel_ms = ms; c->stats.*counted = (int64_t)count;
+        *cost += h_out[0];
         for (size_t k = 0; k < (size_t)18 * N; k++) gradC[k] += h_out[1 + k];
         for (int k = 0; k < N; k++) gradT[k] += h_out[1 + 18 * N + k];
         return 0;
     };
-    r = body();
+    const int r = body();
     if (r) poison(cost);
     return r;
 }
 
+extern "C" int isdf_eval_discrete(isdf_ctx *c, int N, const double *T, const double *coeffs, double *cost, double *gradC, double *gradT) {
+    int r = check_eval_state(c, N, true);
+    if (r) { poison(cost); return r; }
+    if (!T || !coeffs || !cost || !gradC || !gradT) { poison(cost); return fail(ISDF_ERR_INVALID, "NULL argument"); }
+    return eval_host(c, N, T, coeffs, cost, gradC, gradT, &isdf_stats::last_pairs, [] { return 0; },
+                     [&](const double *d_T, const double *d_C, double *d_out, double *count_out) {
+                         c->disc.count_out_dev = count_out;
+                         const int rr = launch_discrete(c, N, d_T, d_C, d_out, c->stream);
+                         c->disc.count_out_dev = nullptr;
+                         return rr;
+                     });
+}
+
 extern "C" int isdf_get_piece_costs(isdf_ctx *c, double *piece_cost, int n) {
     if (!c || !piece_cost || n < 0) return fail(ISDF_ERR_INVALID, "bad argument");
-    if ((size_t)n > c->d_piece_cost.n) return fail(ISDF_ERR_STATE, "no discrete evaluation with that many pieces yet");
+    if ((size_t)n > c->disc.d_piece_cost.n) return fail(ISDF_ERR_STATE, "no discrete evaluation with that many pieces yet");
     if (set_device(c)) return ISDF_ERR_CUDA;
     CU_TRY(cudaStreamSynchronize(c->stream));
-    CU_TRY(cudaMemcpy(piece_cost, c->d_piece_cost.p, sizeof(double) * n, cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(piece_cost, c->disc.d_piece_cost.p, sizeof(double) * n, cudaMemcpyDeviceToHost));
     return 0;
 }
 
@@ -1024,39 +1038,39 @@ static int callback_batch_launch(isdf_ctx *c, int B, int N0, const double *d_hea
     const size_t smem = minco_smem_bytes(N0);
     if (smem > 220 * 1024) return fail(ISDF_ERR_UNSUPPORTED, "pieces per problem too large for the shared-memory banded solver (N0 <= 290)");
     if (BN * (size_t)(c->cfg.integral_intervs + 1) > 0x7fffffffull) return fail(ISDF_ERR_UNSUPPORTED, "batch too large: B*N0*(K+1) must fit in 31 bits");
-    CU_TRY(c->d_mT.ensure(BN)); CU_TRY(c->d_mC.ensure(18 * BN)); CU_TRY(c->d_mlu.ensure(78 * BN)); CU_TRY(c->d_men.ensure(B));
-    CU_TRY(c->d_mgC.ensure(18 * BN)); CU_TRY(c->d_mgT.ensure(BN)); CU_TRY(c->d_mout.ensure(19 * BN + 1));
+    CU_TRY(c->batch.d_T.ensure(BN)); CU_TRY(c->batch.d_C.ensure(18 * BN)); CU_TRY(c->batch.d_lu.ensure(78 * BN)); CU_TRY(c->batch.d_energy.ensure(B));
+    CU_TRY(c->batch.d_gC.ensure(18 * BN)); CU_TRY(c->batch.d_gT.ensure(BN)); CU_TRY(c->batch.d_out.ensure(19 * BN + 1));
     MincoArgs M;
     M.B = B; M.N = N0; M.x = d_x; M.head = d_head; M.tail = d_tail; M.bc_stride = bc_stride; M.rho = rho;
-    M.T = c->d_mT.p; M.C = c->d_mC.p; M.lu = c->d_mlu.p; M.energy = c->d_men.p; M.gC_e = c->d_mgC.p; M.gT_e = c->d_mgT.p;
+    M.T = c->batch.d_T.p; M.C = c->batch.d_C.p; M.lu = c->batch.d_lu.p; M.energy = c->batch.d_energy.p; M.gC_e = c->batch.d_gC.p; M.gT_e = c->batch.d_gT.p;
     M.disc_out = nullptr; M.piece_cost = nullptr; M.cost = d_cost; M.grad = d_grad;
     // per-problem obstacle point sets registered for exactly this batch (isdf_set_points_batch): the LIVE composition of costFunctionLmbm
     // (hpp:386-405) — swept-volume term, then time-integral term
     const bool with_swept = (c->sv.B == B);
     M.Cpp = nullptr; M.sv_out = nullptr;
     if (with_swept) {
-        if (c->shape.kind == ISDF_SHAPE_MESH && c->shape.mesh.sign_mode == MESH_SIGN_WINDING)
+        if (c->mesh.shape.kind == ISDF_SHAPE_MESH && c->mesh.shape.mesh.sign_mode == MESH_SIGN_WINDING)
             return fail(ISDF_ERR_UNSUPPORTED, "swept-volume term with a winding-sign mesh (see isdf_set_shape_mesh_ex)");
-        CU_TRY(c->d_mCpp.ensure(18 * BN)); CU_TRY(c->d_msv.ensure((size_t)B * (19 * (size_t)N0 + 1)));
-        M.Cpp = c->d_mCpp.p;
+        CU_TRY(c->batch.d_Cpp.ensure(18 * BN)); CU_TRY(c->batch.d_sv.ensure((size_t)B * (19 * (size_t)N0 + 1)));
+        M.Cpp = c->batch.d_Cpp.p;
     }
     CU_TRY(cudaFuncSetAttribute(k_minco_forward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CU_TRY(cudaFuncSetAttribute(k_minco_backward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k_minco_forward<<<B, 32, smem, st>>>(M);
     if (with_swept) {
         int launches = 0;
-        cudaError_t e = c->sv.launch_batch(c->dcfg, c->shape, N0, M.T, M.Cpp, c->d_msv.p, st, &launches);
+        cudaError_t e = c->sv.launch_batch(c->dcfg, c->mesh.shape, N0, M.T, M.Cpp, c->batch.d_sv.p, st, &launches);
         c->stats.kernel_launches += launches;
         c->stats.evals_swept++;
         if (e != cudaSuccess) return fail(e == cudaErrorInvalidValue ? ISDF_ERR_INVALID : ISDF_ERR_CUDA, std::string("batched swept: ") + cudaGetErrorString(e));
-        M.sv_out = c->d_msv.p;
+        M.sv_out = c->batch.d_sv.p;
     }
-    int r = launch_discrete(c, (int)BN, M.T, M.C, c->d_mout.p, st);
+    int r = launch_discrete(c, (int)BN, M.T, M.C, c->batch.d_out.p, st);
     if (r) return r;
-    M.disc_out = c->d_mout.p; M.piece_cost = c->d_piece_cost.p;
+    M.disc_out = c->batch.d_out.p; M.piece_cost = c->disc.d_piece_cost.p;
     k_minco_backward<<<B, 32, smem, st>>>(M);
     c->stats.kernel_launches += 2;
-    c->minco_B = B; c->minco_N = N0;
+    c->batch.B = B; c->batch.N0 = N0;
     CU_TRY(cudaGetLastError());
     return 0;
 }
@@ -1078,6 +1092,16 @@ extern "C" int isdf_callback_batch_device(isdf_ctx *c, int B, int N0, const doub
     return callback_batch_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, rho, d_x, d_cost, d_grad, (cudaStream_t)cuda_stream);
 }
 
+// the host entry points' boundary conditions (9 doubles, or 9 per problem) on the device: *d_head, then *d_tail
+static int upload_bc(isdf_ctx *c, int B, int per_problem_bc, const double *head, const double *tail, const double **d_head, const double **d_tail) {
+    const size_t nbc = per_problem_bc ? (size_t)9 * B : 9;
+    CU_TRY(c->batch.d_bc.ensure(2 * nbc));
+    CU_TRY(cudaMemcpyAsync(c->batch.d_bc.p, head, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
+    CU_TRY(cudaMemcpyAsync(c->batch.d_bc.p + nbc, tail, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
+    *d_head = c->batch.d_bc.p; *d_tail = c->batch.d_bc.p + nbc;
+    return 0;
+}
+
 extern "C" int isdf_callback_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc, double rho,
                                    const double *x, double *cost, double *grad) {
     auto poison_all = [&]() { if (cost && B > 0) for (int b = 0; b < B; b++) cost[b] = std::numeric_limits<double>::quiet_NaN(); };
@@ -1086,18 +1110,17 @@ extern "C" int isdf_callback_batch(isdf_ctx *c, int B, int N0, const double *hea
     if (!head || !tail || !x || !cost || !grad) { poison_all(); return fail(ISDF_ERR_INVALID, "NULL argument"); }
     auto body = [&]() -> int {
         if (set_device(c)) return ISDF_ERR_CUDA;
-        const size_t dim = (size_t)N0 + 3 * (size_t)(N0 - 1), nbc = per_problem_bc ? (size_t)9 * B : 9;
-        CU_TRY(c->d_mx.upload(x, dim * B, c->stream));
-        CU_TRY(c->d_mbc.ensure(2 * nbc));
-        CU_TRY(cudaMemcpyAsync(c->d_mbc.p, head, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
-        CU_TRY(cudaMemcpyAsync(c->d_mbc.p + nbc, tail, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
-        CU_TRY(c->d_mcost.ensure(B)); CU_TRY(c->d_mgrad.ensure(dim * B));
+        const size_t dim = (size_t)N0 + 3 * (size_t)(N0 - 1);
+        CU_TRY(c->batch.d_x.upload(x, dim * B, c->stream));
+        const double *d_head, *d_tail;
+        if (int rr = upload_bc(c, B, per_problem_bc, head, tail, &d_head, &d_tail)) return rr;
+        CU_TRY(c->batch.d_cost.ensure(B)); CU_TRY(c->batch.d_grad.ensure(dim * B));
         CU_TRY(cudaEventRecord(c->ev0, c->stream));
-        int rr = callback_batch_launch(c, B, N0, c->d_mbc.p, c->d_mbc.p + nbc, per_problem_bc ? 9 : 0, rho, c->d_mx.p, c->d_mcost.p, c->d_mgrad.p, c->stream);
+        int rr = callback_batch_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, rho, c->batch.d_x.p, c->batch.d_cost.p, c->batch.d_grad.p, c->stream);
         if (rr) return rr;
         CU_TRY(cudaEventRecord(c->ev1, c->stream));
-        CU_TRY(cudaMemcpyAsync(cost, c->d_mcost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaMemcpyAsync(grad, c->d_mgrad.p, sizeof(double) * dim * B, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaMemcpyAsync(cost, c->batch.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaMemcpyAsync(grad, c->batch.d_grad.p, sizeof(double) * dim * B, cudaMemcpyDeviceToHost, c->stream));
         CU_TRY(cudaStreamSynchronize(c->stream));
         float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
         c->stats.last_kernel_ms = ms;
@@ -1139,21 +1162,21 @@ extern "C" int isdf_lbfgs_batch_device(isdf_ctx *c, int B, int N0, const double 
     cudaStream_t st = (cudaStream_t)cuda_stream;
     const int n = 4 * N0 - 3, m = prm->mem_size, npf = prm->past > 1 ? prm->past : 1;
     const size_t per = (size_t)4 * n + npf + 2 * (size_t)m + 2 * (size_t)m * n + LB_NSCALAR;   // doubles of state per instance
-    CU_TRY(c->d_lb_state.ensure(per * B)); CU_TRY(c->d_lb_grad.ensure((size_t)B * n)); CU_TRY(c->d_lb_int.ensure((size_t)B * LB_NINT + 4));
-    if (!c->h_lb_active) CU_TRY(cudaMallocHost((void **)&c->h_lb_active, sizeof(int)));
-    CU_TRY(cudaMemsetAsync(c->d_lb_state.p, 0, sizeof(double) * per * B, st));
-    CU_TRY(cudaMemsetAsync(c->d_lb_int.p, 0, sizeof(int) * ((size_t)B * LB_NINT + 4), st));   // phase = WANT_INIT
+    CU_TRY(c->lbfgs.d_state.ensure(per * B)); CU_TRY(c->lbfgs.d_grad.ensure((size_t)B * n)); CU_TRY(c->lbfgs.d_int.ensure((size_t)B * LB_NINT + 4));
+    CU_TRY(c->lbfgs.h_active.ensure(1));
+    CU_TRY(cudaMemsetAsync(c->lbfgs.d_state.p, 0, sizeof(double) * per * B, st));
+    CU_TRY(cudaMemsetAsync(c->lbfgs.d_int.p, 0, sizeof(int) * ((size_t)B * LB_NINT + 4), st));   // phase = WANT_INIT
     LbfgsArgs L;
     L.B = B; L.n = n;
     L.pr.mem_size = m; L.pr.past = prm->past; L.pr.max_iterations = prm->max_iterations; L.pr.max_linesearch = prm->max_linesearch;
     L.pr.g_epsilon = prm->g_epsilon; L.pr.delta = prm->delta; L.pr.min_step = prm->min_step; L.pr.max_step = prm->max_step;
     L.pr.f_dec_coeff = prm->f_dec_coeff; L.pr.cautious_factor = prm->cautious_factor; L.pr.machine_prec = prm->machine_prec;
-    double *p = c->d_lb_state.p;
-    L.x = d_x; L.f = d_f; L.grad = c->d_lb_grad.p;
+    double *p = c->lbfgs.d_state.p;
+    L.x = d_x; L.f = d_f; L.grad = c->lbfgs.d_grad.p;
     L.xp = p; p += (size_t)B * n; L.g = p; p += (size_t)B * n; L.gp = p; p += (size_t)B * n; L.d = p; p += (size_t)B * n;
     L.pf = p; p += (size_t)B * npf; L.alpha = p; p += (size_t)B * m; L.ys = p; p += (size_t)B * m;
     L.S = p; p += (size_t)B * m * n; L.Y = p; p += (size_t)B * m * n; L.sc = p;
-    L.st = c->d_lb_int.p; L.active = c->d_lb_int.p + (size_t)B * LB_NINT;
+    L.st = c->lbfgs.d_int.p; L.active = c->lbfgs.d_int.p + (size_t)B * LB_NINT;
     // olddnorm starts at 1 (lbfgs.hpp:541): scalar slot 2 of every instance
     {
         std::vector<double> init((size_t)B * LB_NSCALAR, 0.0);
@@ -1164,16 +1187,16 @@ extern "C" int isdf_lbfgs_batch_device(isdf_ctx *c, int B, int N0, const double 
     int rounds = 0;
     for (;;) {
         // every instance's requested point is evaluated (finished instances ride along unchanged: their state is frozen)
-        r = callback_batch_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, rho, d_x, d_f, c->d_lb_grad.p, st);
+        r = callback_batch_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, rho, d_x, d_f, c->lbfgs.d_grad.p, st);
         if (r) return r;
         CU_TRY(cudaMemsetAsync(L.active, 0, sizeof(int), st));
         k_lbfgs_feed<<<(unsigned)((B + 63) / 64), 64, 0, st>>>(L);
         c->stats.kernel_launches++;
         CU_TRY(cudaGetLastError());
-        CU_TRY(cudaMemcpyAsync(c->h_lb_active, L.active, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(c->lbfgs.h_active.p, L.active, sizeof(int), cudaMemcpyDeviceToHost, st));
         CU_TRY(cudaStreamSynchronize(st));
         ++rounds;
-        if (*c->h_lb_active == 0) break;
+        if (*c->lbfgs.h_active.p == 0) break;
         if (prm->max_rounds > 0 && rounds >= prm->max_rounds) break;
     }
     // results: f = fx of every instance (scalar slot 0), return codes and counters
@@ -1192,32 +1215,31 @@ extern "C" int isdf_lbfgs_batch(isdf_ctx *c, int B, int N0, const double *head, 
     if (r) return r;
     if (!head || !tail || !x || !f) return fail(ISDF_ERR_INVALID, "NULL argument");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    const size_t n = (size_t)4 * N0 - 3, nbc = per_problem_bc ? (size_t)9 * B : 9;
-    CU_TRY(c->d_lb_x.upload(x, n * B, c->stream));
-    CU_TRY(c->d_mbc.ensure(2 * nbc));
-    CU_TRY(cudaMemcpyAsync(c->d_mbc.p, head, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
-    CU_TRY(cudaMemcpyAsync(c->d_mbc.p + nbc, tail, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
-    CU_TRY(c->d_lb_f.ensure(B)); CU_TRY(c->d_lb_head.ensure((size_t)3 * B));
-    r = isdf_lbfgs_batch_device(c, B, N0, c->d_mbc.p, c->d_mbc.p + nbc, per_problem_bc, rho, prm, c->d_lb_x.p, c->d_lb_f.p, c->d_lb_head.p, c->d_lb_head.p + B,
-                                c->d_lb_head.p + 2 * (size_t)B, rounds_out, c->stream);
+    const size_t n = (size_t)4 * N0 - 3;
+    CU_TRY(c->lbfgs.d_x.upload(x, n * B, c->stream));
+    const double *d_head, *d_tail;
+    if ((r = upload_bc(c, B, per_problem_bc, head, tail, &d_head, &d_tail))) return r;
+    CU_TRY(c->lbfgs.d_f.ensure(B)); CU_TRY(c->lbfgs.d_head.ensure((size_t)3 * B));
+    r = isdf_lbfgs_batch_device(c, B, N0, d_head, d_tail, per_problem_bc, rho, prm, c->lbfgs.d_x.p, c->lbfgs.d_f.p, c->lbfgs.d_head.p, c->lbfgs.d_head.p + B,
+                                c->lbfgs.d_head.p + 2 * (size_t)B, rounds_out, c->stream);
     if (r) return r;
-    CU_TRY(cudaMemcpy(x, c->d_lb_x.p, sizeof(double) * n * B, cudaMemcpyDeviceToHost));
-    CU_TRY(cudaMemcpy(f, c->d_lb_f.p, sizeof(double) * B, cudaMemcpyDeviceToHost));
-    if (ret) CU_TRY(cudaMemcpy(ret, c->d_lb_head.p, sizeof(int) * B, cudaMemcpyDeviceToHost));
-    if (iterations) CU_TRY(cudaMemcpy(iterations, c->d_lb_head.p + B, sizeof(int) * B, cudaMemcpyDeviceToHost));
-    if (evaluations) CU_TRY(cudaMemcpy(evaluations, c->d_lb_head.p + 2 * (size_t)B, sizeof(int) * B, cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(x, c->lbfgs.d_x.p, sizeof(double) * n * B, cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(f, c->lbfgs.d_f.p, sizeof(double) * B, cudaMemcpyDeviceToHost));
+    if (ret) CU_TRY(cudaMemcpy(ret, c->lbfgs.d_head.p, sizeof(int) * B, cudaMemcpyDeviceToHost));
+    if (iterations) CU_TRY(cudaMemcpy(iterations, c->lbfgs.d_head.p + B, sizeof(int) * B, cudaMemcpyDeviceToHost));
+    if (evaluations) CU_TRY(cudaMemcpy(evaluations, c->lbfgs.d_head.p + 2 * (size_t)B, sizeof(int) * B, cudaMemcpyDeviceToHost));
     return 0;
 }
 
 extern "C" int isdf_get_batch_trajectories(isdf_ctx *c, double *T, double *coeffs, double *energy) {
     if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
-    if (c->minco_B <= 0) return fail(ISDF_ERR_STATE, "no batched callback evaluated yet");
+    if (c->batch.B <= 0) return fail(ISDF_ERR_STATE, "no batched callback evaluated yet");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    const size_t BN = (size_t)c->minco_B * c->minco_N;
+    const size_t BN = (size_t)c->batch.B * c->batch.N0;
     CU_TRY(cudaStreamSynchronize(c->stream));
-    if (T) CU_TRY(cudaMemcpy(T, c->d_mT.p, sizeof(double) * BN, cudaMemcpyDeviceToHost));
-    if (coeffs) CU_TRY(cudaMemcpy(coeffs, c->d_mC.p, sizeof(double) * 18 * BN, cudaMemcpyDeviceToHost));
-    if (energy) CU_TRY(cudaMemcpy(energy, c->d_men.p, sizeof(double) * c->minco_B, cudaMemcpyDeviceToHost));
+    if (T) CU_TRY(cudaMemcpy(T, c->batch.d_T.p, sizeof(double) * BN, cudaMemcpyDeviceToHost));
+    if (coeffs) CU_TRY(cudaMemcpy(coeffs, c->batch.d_C.p, sizeof(double) * 18 * BN, cudaMemcpyDeviceToHost));
+    if (energy) CU_TRY(cudaMemcpy(energy, c->batch.d_energy.p, sizeof(double) * c->batch.B, cudaMemcpyDeviceToHost));
     return 0;
 }
 
@@ -1249,12 +1271,12 @@ static int clearance_check(isdf_ctx *c, int N, const isdf_clearance_params *p) {
     if (clearance_batch(N, p) == 0) return fail(ISDF_ERR_INVALID, "pieces_per_traj must be 0 or divide N");
     if ((long long)N * (p->samples_per_piece + 1) > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "N * (samples_per_piece + 1) must fit in 31 bits");
     if (c->world > 1) return fail(ISDF_ERR_UNSUPPORTED, "the clearance check is not sharded: call it on a context with isdf_set_shard(ctx, 0, 1)");
-    if (!c->have_map) return fail(ISDF_ERR_STATE, "map not set");
-    if (!c->have_shape) return fail(ISDF_ERR_STATE, "shape not set");
+    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
+    if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
     // the window of a sample spans at most 2 H sqrt(3) / res + 3 voxels per axis (rotated H box, one voxel of slack on each side); the
     // 1023-voxel limit of the pose-window offsets applies as in the discrete path
     const double H = c->dcfg.half_bd + p->reach;
-    if (2.0 * H * std::sqrt(3.0) / c->grid.res + 4.0 > (double)WINDOW_AXIS_MAX)
+    if (2.0 * H * std::sqrt(3.0) / c->map.grid.res + 4.0 > (double)WINDOW_AXIS_MAX)
         return fail(ISDF_ERR_INVALID, "reach too large for this map resolution: a sample window would exceed 1023 voxels per axis");
     return 0;
 }
@@ -1262,16 +1284,16 @@ static int clearance_check(isdf_ctx *c, int N, const isdf_clearance_params *p) {
 static int clearance_launch_ctx(isdf_ctx *c, int N, const double *d_T, const double *d_C, const isdf_clearance_params *p, double *d_clear,
                                 long long *d_vox, ClrSummary *d_sum, cudaStream_t st) {
     ClrArgs A;
-    A.grid = c->grid; A.shape = c->shape; A.fp = c->dcfg.fp; A.half_bd = c->dcfg.half_bd;
+    A.grid = c->map.grid; A.shape = c->mesh.shape; A.fp = c->dcfg.fp; A.half_bd = c->dcfg.half_bd;
     A.reach = p->reach; A.margin = p->margin;
     A.N = N; A.K = p->samples_per_piece; A.N0 = p->pieces_per_traj == 0 ? N : p->pieces_per_traj;
     A.T = d_T; A.C = d_C; A.clear = d_clear; A.voxel = d_vox; A.summary = d_sum;
-    CU_TRY(c->d_clr_cursor.ensure(1));
-    CU_TRY(c->d_clr_counters.ensure(2));
-    CU_TRY(cudaMemsetAsync(c->d_clr_cursor.p, 0, sizeof(int), st));
-    CU_TRY(cudaMemsetAsync(c->d_clr_counters.p, 0, 2 * sizeof(unsigned long long), st));
-    A.cursor = c->d_clr_cursor.p; A.counters = c->d_clr_counters.p;
-    const int mode = c->shape.kind != ISDF_SHAPE_MESH ? 0 : (c->shape.mesh.sign_mode == MESH_SIGN_WINDING ? 2 : 1);
+    CU_TRY(c->clr.d_cursor.ensure(1));
+    CU_TRY(c->clr.d_counters.ensure(2));
+    CU_TRY(cudaMemsetAsync(c->clr.d_cursor.p, 0, sizeof(int), st));
+    CU_TRY(cudaMemsetAsync(c->clr.d_counters.p, 0, 2 * sizeof(unsigned long long), st));
+    A.cursor = c->clr.d_cursor.p; A.counters = c->clr.d_counters.p;
+    const int mode = c->mesh.shape.kind != ISDF_SHAPE_MESH ? 0 : (c->mesh.shape.mesh.sign_mode == MESH_SIGN_WINDING ? 2 : 1);
     const long long S = (long long)N * (A.K + 1);
     const long long want = (S + CLR_WARPS - 1) / CLR_WARPS;
     const unsigned grid = (unsigned)std::max<long long>(1, std::min(want, (long long)c->sm_count * c->clr_blocks));
@@ -1320,15 +1342,15 @@ extern "C" int isdf_trajectory_clearance(isdf_ctx *c, int N, const double *T, co
         if (set_device(c)) return ISDF_ERR_CUDA;
         const int B = clearance_batch(N, p);
         const size_t S = (size_t)N * (p->samples_per_piece + 1);
-        CU_TRY(c->d_clr_in.ensure((size_t)19 * N));
-        CU_TRY(c->d_clr_clear.ensure(S)); CU_TRY(c->d_clr_vox.ensure(S)); CU_TRY(c->d_clr_sum.ensure((size_t)B));
-        CU_TRY(cudaMemcpyAsync(c->d_clr_in.p, coeffs, sizeof(double) * 18 * N, cudaMemcpyHostToDevice, c->stream));
-        CU_TRY(cudaMemcpyAsync(c->d_clr_in.p + 18 * (size_t)N, T, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
-        int rr = clearance_launch_ctx(c, N, c->d_clr_in.p + 18 * (size_t)N, c->d_clr_in.p, p, c->d_clr_clear.p, c->d_clr_vox.p, c->d_clr_sum.p, c->stream);
+        CU_TRY(c->clr.d_in.ensure((size_t)19 * N));
+        CU_TRY(c->clr.d_clear.ensure(S)); CU_TRY(c->clr.d_vox.ensure(S)); CU_TRY(c->clr.d_sum.ensure((size_t)B));
+        CU_TRY(cudaMemcpyAsync(c->clr.d_in.p, coeffs, sizeof(double) * 18 * N, cudaMemcpyHostToDevice, c->stream));
+        CU_TRY(cudaMemcpyAsync(c->clr.d_in.p + 18 * (size_t)N, T, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
+        int rr = clearance_launch_ctx(c, N, c->clr.d_in.p + 18 * (size_t)N, c->clr.d_in.p, p, c->clr.d_clear.p, c->clr.d_vox.p, c->clr.d_sum.p, c->stream);
         if (rr) return rr;
-        CU_TRY(cudaMemcpyAsync(summary, c->d_clr_sum.p, sizeof(isdf_clearance_summary) * B, cudaMemcpyDeviceToHost, c->stream));
-        if (sample_clearance) CU_TRY(cudaMemcpyAsync(sample_clearance, c->d_clr_clear.p, sizeof(double) * S, cudaMemcpyDeviceToHost, c->stream));
-        if (sample_voxel) CU_TRY(cudaMemcpyAsync(sample_voxel, c->d_clr_vox.p, sizeof(int64_t) * S, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaMemcpyAsync(summary, c->clr.d_sum.p, sizeof(isdf_clearance_summary) * B, cudaMemcpyDeviceToHost, c->stream));
+        if (sample_clearance) CU_TRY(cudaMemcpyAsync(sample_clearance, c->clr.d_clear.p, sizeof(double) * S, cudaMemcpyDeviceToHost, c->stream));
+        if (sample_voxel) CU_TRY(cudaMemcpyAsync(sample_voxel, c->clr.d_vox.p, sizeof(int64_t) * S, cudaMemcpyDeviceToHost, c->stream));
         CU_TRY(cudaStreamSynchronize(c->stream));
         return 0;
     };
@@ -1343,67 +1365,67 @@ static size_t peer_bytes(int world, int cap) { return sizeof(unsigned long long)
 extern "C" int isdf_peer_export(isdf_ctx *c, int world, int max_doubles, unsigned char *handle64) {
     if (!c || !handle64 || world < 2 || world > PEER_MAX || max_doubles < 1) return fail(ISDF_ERR_INVALID, "bad argument (2 <= world <= 16)");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    if (c->peer.world) return fail(ISDF_ERR_STATE, "already connected: isdf_peer_disconnect first");
-    if (c->peer_buf) { cudaFree(c->peer_buf); c->peer_buf = nullptr; }
-    CU_TRY(cudaMalloc(&c->peer_buf, peer_bytes(world, max_doubles)));
-    CU_TRY(cudaMemset(c->peer_buf, 0, peer_bytes(world, max_doubles)));
-    CU_TRY(c->d_peer_status.ensure(1));
-    CU_TRY(cudaMemset(c->d_peer_status.p, 0, sizeof(int)));
+    if (c->peer.args.world) return fail(ISDF_ERR_STATE, "already connected: isdf_peer_disconnect first");
+    c->peer.buf = {};
+    CU_TRY(c->peer.buf.ensure(peer_bytes(world, max_doubles)));
+    CU_TRY(cudaMemset(c->peer.buf.p, 0, peer_bytes(world, max_doubles)));
+    CU_TRY(c->peer.d_status.ensure(1));
+    CU_TRY(cudaMemset(c->peer.d_status.p, 0, sizeof(int)));
     cudaIpcMemHandle_t h;
-    CU_TRY(cudaIpcGetMemHandle(&h, c->peer_buf));
+    CU_TRY(cudaIpcGetMemHandle(&h, c->peer.buf.p));
     static_assert(sizeof(h) == 64, "cudaIpcMemHandle_t is 64 bytes");
     std::memcpy(handle64, &h, 64);
-    c->peer_world_alloc = world; c->peer_cap = max_doubles;
+    c->peer.world_alloc = world; c->peer.cap = max_doubles;
     return 0;
 }
 
 extern "C" int isdf_peer_connect(isdf_ctx *c, int world, int rank, const unsigned char *handles, int fuse_into_eval) {
     if (!c || !handles || rank < 0 || rank >= world) return fail(ISDF_ERR_INVALID, "bad argument");
-    if (!c->peer_buf || world != c->peer_world_alloc) return fail(ISDF_ERR_STATE, "isdf_peer_export with the same world first");
-    if (c->peer.world != 0) return fail(ISDF_ERR_STATE, "already connected: isdf_peer_disconnect first");
+    if (!c->peer.buf.p || world != c->peer.world_alloc) return fail(ISDF_ERR_STATE, "isdf_peer_export with the same world first");
+    if (c->peer.args.world != 0) return fail(ISDF_ERR_STATE, "already connected: isdf_peer_disconnect first");
     if (set_device(c)) return ISDF_ERR_CUDA;
     PeerArgs P = {};
-    P.world = world; P.rank = rank; P.cap = c->peer_cap; P.epoch = 0; P.status = c->d_peer_status.p;
+    P.world = world; P.rank = rank; P.cap = c->peer.cap; P.epoch = 0; P.status = c->peer.d_status.p;
     for (int p = 0; p < world; p++) {
-        void *base = c->peer_buf;
+        void *base = c->peer.buf.p;
         if (p != rank) {
             cudaIpcMemHandle_t h;
             std::memcpy(&h, handles + (size_t)64 * p, 64);
             cudaError_t e = cudaIpcOpenMemHandle(&base, h, cudaIpcMemLazyEnablePeerAccess);
             if (e != cudaSuccess) {
-                for (int q = 0; q < p; q++) if (c->peer_open[q]) { cudaIpcCloseMemHandle(c->peer_open[q]); c->peer_open[q] = nullptr; }
+                c->peer.close_handles();
                 return fail(ISDF_ERR_CUDA, std::string("cudaIpcOpenMemHandle: ") + cudaGetErrorString(e));
             }
-            c->peer_open[p] = base;
+            c->peer.open[p] = base;
         }
         P.flags[p] = (unsigned long long *)base;
         P.slots[p] = (double *)((char *)base + sizeof(unsigned long long) * 2 * PEER_MAX);
     }
-    c->peer = P;
-    c->peer_fused = fuse_into_eval != 0;
+    c->peer.args = P;
+    c->peer.fused = fuse_into_eval != 0;
     return 0;
 }
 
 extern "C" int isdf_peer_allreduce_device(isdf_ctx *c, double *d_vec, int n, void *cuda_stream) {
     if (!c || !d_vec || n < 1) return fail(ISDF_ERR_INVALID, "bad argument");
-    if (c->peer.world < 2) return fail(ISDF_ERR_STATE, "not connected (isdf_peer_connect)");
-    if (n > c->peer.cap) return fail(ISDF_ERR_INVALID, "vector longer than the exchange buffer");
+    if (c->peer.args.world < 2) return fail(ISDF_ERR_STATE, "not connected (isdf_peer_connect)");
+    if (n > c->peer.args.cap) return fail(ISDF_ERR_INVALID, "vector longer than the exchange buffer");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    PeerArgs P = c->peer;
-    P.epoch = c->peer.epoch + 1;
+    PeerArgs P = c->peer.args;
+    P.epoch = c->peer.args.epoch + 1;
     k_peer_allreduce<<<1, 512, 0, (cudaStream_t)cuda_stream>>>(P, d_vec, n);
     c->stats.kernel_launches++;
     CU_TRY(cudaGetLastError());
-    c->peer.epoch = P.epoch;
+    c->peer.args.epoch = P.epoch;
     return 0;
 }
 
 extern "C" int isdf_peer_status(isdf_ctx *c) {
     if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
-    if (!c->d_peer_status.p) return 0;
+    if (!c->peer.d_status.p) return 0;
     if (set_device(c)) return ISDF_ERR_CUDA;
     int st = 0;
-    CU_TRY(cudaMemcpy(&st, c->d_peer_status.p, sizeof(int), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(&st, c->peer.d_status.p, sizeof(int), cudaMemcpyDeviceToHost));
     if (st) return fail(ISDF_ERR_CUDA, "peer exchange timed out: a rank did not reach the same evaluation");
     return 0;
 }
@@ -1412,9 +1434,9 @@ extern "C" int isdf_peer_disconnect(isdf_ctx *c) {
     if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
     if (set_device(c)) return ISDF_ERR_CUDA;
     cudaDeviceSynchronize();
-    for (int p = 0; p < PEER_MAX; p++) if (c->peer_open[p]) { cudaIpcCloseMemHandle(c->peer_open[p]); c->peer_open[p] = nullptr; }
-    if (c->peer_buf) { cudaFree(c->peer_buf); c->peer_buf = nullptr; }
-    c->peer = PeerArgs{}; c->peer_fused = false; c->peer_world_alloc = 0; c->peer_cap = 0;
+    c->peer.close_handles();
+    c->peer.buf = {};
+    c->peer.args = PeerArgs{}; c->peer.fused = false; c->peer.world_alloc = 0; c->peer.cap = 0;
     return 0;
 }
 
@@ -1437,25 +1459,25 @@ static void attitude_rotation(double rotx, double roty, double R[9]) {
 
 static FrontArgs front_args(isdf_ctx *c) {
     FrontArgs A = {};
-    A.grid = c->grid; A.shape = c->shape;
-    for (int i = 0; i < 9; i++) A.rot[i] = c->shape.rot[i];
-    for (int i = 0; i < 3; i++) A.trans[i] = c->shape.trans[i];
-    if (c->shape.kind != ISDF_SHAPE_MESH) {   // the kernel applies ((pos - trans) * Rotate) * R_obj itself and evaluates the bare body
+    A.grid = c->map.grid; A.shape = c->mesh.shape;
+    for (int i = 0; i < 9; i++) A.rot[i] = c->mesh.shape.rot[i];
+    for (int i = 0; i < 3; i++) A.trans[i] = c->mesh.shape.trans[i];
+    if (c->mesh.shape.kind != ISDF_SHAPE_MESH) {   // the kernel applies ((pos - trans) * Rotate) * R_obj itself and evaluates the bare body
         const double I[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
         for (int i = 0; i < 9; i++) A.shape.rot[i] = I[i];
         for (int i = 0; i < 3; i++) A.shape.trans[i] = 0.0;
     }
-    A.ks = c->fe_ks; A.xk = c->fe_xk; A.yk = c->fe_yk; A.natt = c->fe_xk * c->fe_yk;
-    A.res = c->cfg.occupancy_resolution; A.margin = c->fe_margin;
-    A.att_rot = c->d_fe_rot.p; A.kernels = c->d_fe_kernels.p; A.offset_masks = c->d_fe_masks.p; A.order = c->d_fe_order.p;
-    A.max_roll = c->fe_max_roll; A.max_pitch = c->fe_max_pitch; A.ang_res = c->fe_ang_res;
-    A.core_rows = c->d_fe_core.p; A.ncore = c->fe_ncore; A.urows = c->d_fe_urows.p; A.nurow = c->fe_nurow; A.chunks = c->d_fe_chunks.p; A.nchunk = c->fe_nchunk; A.tab = c->d_fe_tab.p; A.ntab = c->fe_ntab; A.surv = c->d_fe_surv.p; A.surv_count = c->d_fe_count.p;
+    A.ks = c->fe.ks; A.xk = c->fe.xk; A.yk = c->fe.yk; A.natt = c->fe.xk * c->fe.yk;
+    A.res = c->cfg.occupancy_resolution; A.margin = c->fe.margin;
+    A.att_rot = c->fe.d_rot.p; A.kernels = c->fe.d_kernels.p; A.offset_masks = c->fe.d_masks.p; A.order = c->fe.d_order.p;
+    A.max_roll = c->fe.max_roll; A.max_pitch = c->fe.max_pitch; A.ang_res = c->fe.ang_res;
+    A.core_rows = c->fe.d_core.p; A.ncore = c->fe.ncore; A.urows = c->fe.d_urows.p; A.nurow = c->fe.nurow; A.chunks = c->fe.d_chunks.p; A.nchunk = c->fe.nchunk; A.tab = c->fe.d_tab.p; A.ntab = c->fe.ntab; A.surv = c->fe.d_surv.p; A.surv_count = c->fe.d_count.p;
     return A;
 }
 
 extern "C" int isdf_frontend_build_kernels(isdf_ctx *c, const isdf_kernel_config *kc, int *xkernel_size, int *ykernel_size) {
     if (!c || !kc) return fail(ISDF_ERR_INVALID, "NULL argument");
-    if (!c->have_shape) return fail(ISDF_ERR_STATE, "shape not set");
+    if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
     if (!(kc->kernel_ang_res > 0) || kc->kernel_max_roll < 0 || kc->kernel_max_pitch < 0) return fail(ISDF_ERR_INVALID, "bad attitude grid");
     const int ks = c->cfg.kernel_size;
     if (ks < 1 || (ks & 1) == 0) return fail(ISDF_ERR_INVALID, "kernel_size must be odd (Shape.hpp:258)");
@@ -1500,13 +1522,14 @@ extern "C" int isdf_frontend_build_kernels(isdf_ctx *c, const isdf_kernel_config
                 if (deep > 800) break;   // maxdeepth (swm:852)
             }
         }
-    CU_TRY(c->d_fe_rot.upload(rot.data(), rot.size(), c->stream));
-    CU_TRY(c->d_fe_order.upload(order.data(), order.size(), c->stream));
-    CU_TRY(c->d_fe_kernels.ensure((size_t)natt * n3));
-    CU_TRY(c->d_fe_masks.ensure((size_t)4 * n3));
-    c->fe_xk = xk; c->fe_yk = yk; c->fe_ks = ks;
-    c->fe_max_roll = kc->kernel_max_roll; c->fe_max_pitch = kc->kernel_max_pitch; c->fe_ang_res = kc->kernel_ang_res;
-    c->fe_margin = std::max(kc->front_end_safeh, c->cfg.occupancy_resolution / 2);   // Shape.hpp:423
+    c->fe.ready = false;   // the current kernels and tables are overwritten from here on
+    CU_TRY(c->fe.d_rot.upload(rot.data(), rot.size(), c->stream));
+    CU_TRY(c->fe.d_order.upload(order.data(), order.size(), c->stream));
+    CU_TRY(c->fe.d_kernels.ensure((size_t)natt * n3));
+    CU_TRY(c->fe.d_masks.ensure((size_t)4 * n3));
+    c->fe.xk = xk; c->fe.yk = yk; c->fe.ks = ks;
+    c->fe.max_roll = kc->kernel_max_roll; c->fe.max_pitch = kc->kernel_max_pitch; c->fe.ang_res = kc->kernel_ang_res;
+    c->fe.margin = std::max(kc->front_end_safeh, c->cfg.occupancy_resolution / 2);   // Shape.hpp:423
     FrontArgs A = front_args(c);
     const long long nt = (long long)natt * n3;
     k_frontend_kernels<<<(unsigned)((nt + 255) / 256), 256, 0, c->stream>>>(A);
@@ -1517,7 +1540,7 @@ extern "C" int isdf_frontend_build_kernels(isdf_ctx *c, const isdf_kernel_config
     // the kernel core (offsets every attitude occupies), row by row, densest rows first: pass 1 of the two-pass feasibility kernel
     {
         std::vector<uint32_t> om((size_t)4 * n3);
-        CU_TRY(cudaMemcpy(om.data(), c->d_fe_masks.p, sizeof(uint32_t) * om.size(), cudaMemcpyDeviceToHost));
+        CU_TRY(cudaMemcpy(om.data(), c->fe.d_masks.p, sizeof(uint32_t) * om.size(), cudaMemcpyDeviceToHost));
         uint32_t valid[4];
         for (int k = 0; k < 4; k++) { const int lo = 32 * k; valid[k] = natt >= lo + 32 ? 0xffffffffu : (natt > lo ? ((1u << (natt - lo)) - 1u) : 0u); }
         std::vector<uint2> rows, urows;
@@ -1532,8 +1555,8 @@ extern "C" int isdf_frontend_build_kernels(isdf_ctx *c, const isdf_kernel_config
                 if (bits) rows.push_back(make_uint2((uint32_t)a | ((uint32_t)b << 8), bits));
                 if (ubits) urows.push_back(make_uint2((uint32_t)a | ((uint32_t)b << 8), ubits));
             }
-        c->fe_nurow = (int)urows.size();
-        if (!urows.empty()) CU_TRY(c->d_fe_urows.upload(urows.data(), urows.size(), c->stream));
+        c->fe.nurow = (int)urows.size();
+        if (!urows.empty()) CU_TRY(c->fe.d_urows.upload(urows.data(), urows.size(), c->stream));
         // pattern tables of the union rows, in chunks of <= FE_CHUNK_BITS offsets (pass 2 of the table-driven kernels)
         std::vector<uint2> chunks; std::vector<uint4> tab;
         for (const uint2 &ur : urows) {
@@ -1551,15 +1574,15 @@ extern "C" int isdf_frontend_build_kernels(isdf_ctx *c, const isdf_kernel_config
                 }
             }
         }
-        c->fe_nchunk = (int)chunks.size(); c->fe_ntab = (int)tab.size();
+        c->fe.nchunk = (int)chunks.size(); c->fe.ntab = (int)tab.size();
         if (getenv("ISDF_VERBOSE")) fprintf(stderr, "[isdf] front end: %d attitudes, kernel core %zu rows, union %zu rows, %zu chunks, %zu table entries (%.1f KB)\n", natt, rows.size(), urows.size(), chunks.size(), tab.size(), tab.size() * 16e-3);
-        if (!chunks.empty()) { CU_TRY(c->d_fe_chunks.upload(chunks.data(), chunks.size(), c->stream)); CU_TRY(c->d_fe_tab.upload(tab.data(), tab.size(), c->stream)); }
+        if (!chunks.empty()) { CU_TRY(c->fe.d_chunks.upload(chunks.data(), chunks.size(), c->stream)); CU_TRY(c->fe.d_tab.upload(tab.data(), tab.size(), c->stream)); }
         std::stable_sort(rows.begin(), rows.end(), [](const uint2 &p, const uint2 &q) { return __builtin_popcount(p.y) > __builtin_popcount(q.y); });
-        c->fe_ncore = (int)rows.size();
-        if (!rows.empty()) CU_TRY(c->d_fe_core.upload(rows.data(), rows.size(), c->stream));
+        c->fe.ncore = (int)rows.size();
+        if (!rows.empty()) CU_TRY(c->fe.d_core.upload(rows.data(), rows.size(), c->stream));
         CU_TRY(cudaStreamSynchronize(c->stream));
     }
-    c->fe_ready = true;
+    c->fe.ready = true;
     if (xkernel_size) *xkernel_size = xk;
     if (ykernel_size) *ykernel_size = yk;
     return 0;
@@ -1567,18 +1590,18 @@ extern "C" int isdf_frontend_build_kernels(isdf_ctx *c, const isdf_kernel_config
 
 extern "C" int isdf_frontend_get_kernels(isdf_ctx *c, uint8_t *out, int n) {
     if (!c || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
-    if (!c->fe_ready) return fail(ISDF_ERR_STATE, "isdf_frontend_build_kernels first (and again after changing the shape)");
-    const size_t want = (size_t)c->fe_xk * c->fe_yk * c->fe_ks * c->fe_ks * c->fe_ks;
+    if (!c->fe.ready) return fail(ISDF_ERR_STATE, "isdf_frontend_build_kernels first (and again after changing the shape)");
+    const size_t want = (size_t)c->fe.xk * c->fe.yk * c->fe.ks * c->fe.ks * c->fe.ks;
     if ((size_t)n != want) return fail(ISDF_ERR_INVALID, "n must be xkernel_size * ykernel_size * kernel_size^3");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    CU_TRY(cudaMemcpy(out, c->d_fe_kernels.p, want, cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(out, c->fe.d_kernels.p, want, cudaMemcpyDeviceToHost));
     return 0;
 }
 
 static int frontend_state(isdf_ctx *c) {
     if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
-    if (!c->fe_ready) return fail(ISDF_ERR_STATE, "isdf_frontend_build_kernels first (and again after changing the shape)");
-    if (!c->have_map) return fail(ISDF_ERR_STATE, "map not set");
+    if (!c->fe.ready) return fail(ISDF_ERR_STATE, "isdf_frontend_build_kernels first (and again after changing the shape)");
+    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
     return 0;
 }
 
@@ -1591,21 +1614,21 @@ extern "C" int isdf_frontend_feasibility_device(isdf_ctx *c, uint32_t *d_masks, 
     A.out = d_masks;
     const size_t smem = sizeof(uint32_t) * 4 * (size_t)A.ks * A.ks * A.ks;
     CU_TRY(cudaFuncSetAttribute(k_frontend_feasibility, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const long long nrun = (long long)c->grid.X * c->grid.Y * ((c->grid.Z + FE_ZRUN - 1) / FE_ZRUN);
+    const long long nrun = (long long)c->map.grid.X * c->map.grid.Y * ((c->map.grid.Z + FE_ZRUN - 1) / FE_ZRUN);
     const long long sms = c->sm_count;
     const unsigned grid = (unsigned)std::min<long long>((nrun + 255) / 256, sms * 64);
-    if (c->fe_ncore > 0 && nrun < (1ll << 32) && !getenv("ISDF_FE_ONE_PASS")) {
+    if (c->fe.ncore > 0 && nrun < (1ll << 32) && !getenv("ISDF_FE_ONE_PASS")) {
         // two passes: the kernel core settles most voxels of a cluttered map, the mask accumulation runs on the survivors only
-        CU_TRY(c->d_fe_surv.ensure((size_t)nrun));
-        CU_TRY(c->d_fe_count.ensure(1));
-        A.surv = c->d_fe_surv.p; A.surv_count = c->d_fe_count.p;
-        CU_TRY(cudaMemsetAsync(c->d_fe_count.p, 0, sizeof(unsigned), (cudaStream_t)cuda_stream));
-        const size_t tsmem = sizeof(uint4) * ((size_t)c->fe_ntab + (size_t)c->fe_nchunk);
-        if (c->fe_nchunk > 0 && tsmem <= 200 * 1024 && !getenv("ISDF_FE_NO_TABLES")) {
+        CU_TRY(c->fe.d_surv.ensure((size_t)nrun));
+        CU_TRY(c->fe.d_count.ensure(1));
+        A.surv = c->fe.d_surv.p; A.surv_count = c->fe.d_count.p;
+        CU_TRY(cudaMemsetAsync(c->fe.d_count.p, 0, sizeof(unsigned), (cudaStream_t)cuda_stream));
+        const size_t tsmem = sizeof(uint4) * ((size_t)c->fe.ntab + (size_t)c->fe.nchunk);
+        if (c->fe.nchunk > 0 && tsmem <= 200 * 1024 && !getenv("ISDF_FE_NO_TABLES")) {
             // throughput form: zero-filled output, bit-parallel core pass (32 voxels per thread), table-driven accumulation on the survivors
-            const long long nvox = (long long)c->grid.X * c->grid.Y * c->grid.Z;
+            const long long nvox = (long long)c->map.grid.X * c->map.grid.Y * c->map.grid.Z;
             CU_TRY(cudaMemsetAsync(d_masks, 0, sizeof(uint32_t) * 4 * (size_t)nvox, (cudaStream_t)cuda_stream));
-            const long long nword = (long long)c->grid.X * c->grid.Y * c->grid.Zw;
+            const long long nword = (long long)c->map.grid.X * c->map.grid.Y * c->map.grid.Zw;
             CU_TRY(cudaFuncSetAttribute(k_frontend_survivors_tab, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tsmem));
             k_frontend_core_words<<<(unsigned)std::min<long long>((nword + 255) / 256, sms * 32), 256, 0, (cudaStream_t)cuda_stream>>>(A);
             // 32 warps per SM hide the row reads: two CTAs of 512 threads when two tables fit into shared memory, else one of 1024
@@ -1631,13 +1654,13 @@ extern "C" int isdf_frontend_feasibility(isdf_ctx *c, uint32_t *masks) {
     if (r) return r;
     if (!masks) return fail(ISDF_ERR_INVALID, "NULL argument");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    const size_t nvox = (size_t)c->grid.X * c->grid.Y * c->grid.Z;
-    CU_TRY(c->d_fe_out.ensure(4 * nvox));
+    const size_t nvox = (size_t)c->map.grid.X * c->map.grid.Y * c->map.grid.Z;
+    CU_TRY(c->fe.d_out.ensure(4 * nvox));
     CU_TRY(cudaEventRecord(c->ev0, c->stream));
-    r = isdf_frontend_feasibility_device(c, c->d_fe_out.p, c->stream);
+    r = isdf_frontend_feasibility_device(c, c->fe.d_out.p, c->stream);
     if (r) return r;
     CU_TRY(cudaEventRecord(c->ev1, c->stream));
-    CU_TRY(cudaMemcpyAsync(masks, c->d_fe_out.p, sizeof(uint32_t) * 4 * nvox, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(cudaMemcpyAsync(masks, c->fe.d_out.p, sizeof(uint32_t) * 4 * nvox, cudaMemcpyDeviceToHost, c->stream));
     CU_TRY(cudaStreamSynchronize(c->stream));
     float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
     c->stats.last_kernel_ms = ms;
@@ -1650,21 +1673,21 @@ extern "C" int isdf_frontend_check_batch(isdf_ctx *c, int n, const int32_t *ind,
     if (n < 0 || (n > 0 && (!ind || !father_roll_pitch || !child_roll_pitch || !ok))) return fail(ISDF_ERR_INVALID, "bad argument");
     if (n == 0) return 0;
     for (int q = 0; q < n; q++)
-        if (ind[3 * q] < 0 || ind[3 * q] >= c->grid.X || ind[3 * q + 1] < 0 || ind[3 * q + 1] >= c->grid.Y || ind[3 * q + 2] < 0 || ind[3 * q + 2] >= c->grid.Z)
+        if (ind[3 * q] < 0 || ind[3 * q] >= c->map.grid.X || ind[3 * q + 1] < 0 || ind[3 * q + 1] >= c->map.grid.Y || ind[3 * q + 2] < 0 || ind[3 * q + 2] >= c->map.grid.Z)
             return fail(ISDF_ERR_INVALID, "voxel index outside the map");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    CU_TRY(c->d_fe_ind.upload(ind, (size_t)3 * n, c->stream));
-    CU_TRY(c->d_fe_father.upload(father_roll_pitch, (size_t)2 * n, c->stream));
-    CU_TRY(c->d_fe_child.ensure((size_t)2 * n)); CU_TRY(c->d_fe_ok.ensure(n)); CU_TRY(c->d_fe_out.ensure((size_t)4 * n));
+    CU_TRY(c->fe.d_ind.upload(ind, (size_t)3 * n, c->stream));
+    CU_TRY(c->fe.d_father.upload(father_roll_pitch, (size_t)2 * n, c->stream));
+    CU_TRY(c->fe.d_child.ensure((size_t)2 * n)); CU_TRY(c->fe.d_ok.ensure(n)); CU_TRY(c->fe.d_out.ensure((size_t)4 * n));
     FrontArgs A = front_args(c);
-    A.out = c->d_fe_out.p; A.nq = n; A.q_ind = c->d_fe_ind.p; A.q_father = c->d_fe_father.p; A.q_child = c->d_fe_child.p; A.q_ok = c->d_fe_ok.p;
+    A.out = c->fe.d_out.p; A.nq = n; A.q_ind = c->fe.d_ind.p; A.q_father = c->fe.d_father.p; A.q_child = c->fe.d_child.p; A.q_ok = c->fe.d_ok.p;
     const size_t smem = sizeof(uint32_t) * 4 * (size_t)A.ks * A.ks * A.ks;
     CU_TRY(cudaFuncSetAttribute(k_frontend_check, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k_frontend_check<<<(unsigned)((n + 255) / 256), 256, smem, c->stream>>>(A);
     c->stats.kernel_launches++;
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(child_roll_pitch, c->d_fe_child.p, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaMemcpyAsync(ok, c->d_fe_ok.p, n, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(cudaMemcpyAsync(child_roll_pitch, c->fe.d_child.p, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(cudaMemcpyAsync(ok, c->fe.d_ok.p, n, cudaMemcpyDeviceToHost, c->stream));
     CU_TRY(cudaStreamSynchronize(c->stream));
     return 0;
 }
@@ -1673,7 +1696,6 @@ extern "C" int isdf_frontend_check_batch(isdf_ctx *c, int n, const int32_t *ind,
 extern "C" int isdf_set_points(isdf_ctx *c, const double *pts, int P) {
     if (!c || P < 0 || (P > 0 && !pts)) return fail(ISDF_ERR_INVALID, "bad argument");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    c->sv.B = 0;   // a single point set replaces any per-problem sets
     CU_TRY(c->sv.set_points(pts, P, c->stream));
     return 0;
 }
@@ -1693,23 +1715,22 @@ extern "C" int isdf_set_points_batch(isdf_ctx *c, int B, const int32_t *offsets,
 static int swept_common(isdf_ctx *c, int N, const double *d_T, const double *d_C, double *d_out, cudaStream_t st,
                         const double *g_t, const double *g_s, const double *g_g) {
     if (c->sv.P <= 0) return fail(ISDF_ERR_STATE, "obstacle points not set (isdf_set_points)");
-    if (c->shape.kind == ISDF_SHAPE_MESH && c->shape.mesh.sign_mode == MESH_SIGN_WINDING)
+    if (c->mesh.shape.kind == ISDF_SHAPE_MESH && c->mesh.shape.mesh.sign_mode == MESH_SIGN_WINDING)
         return fail(ISDF_ERR_UNSUPPORTED, "the swept-volume search prunes with distance brackets that need a true distance function: winding-sign meshes "
                                           "(open meshes / soups, ISDF_MESH_SIGN_WINDING) are supported by the discrete path and isdf_shape_query only");
     int launches = 0;
-    cudaError_t e = c->sv.launch(c->dcfg, c->shape, N, d_T, d_C, d_out, c->rank, c->world, st, g_t, g_s, g_g, &launches);
+    cudaError_t e = c->sv.launch(c->dcfg, c->mesh.shape, N, d_T, d_C, d_out, c->rank, c->world, st, g_t, g_s, g_g, &launches);
     c->stats.kernel_launches += launches;
     c->stats.evals_swept++;
     if (e != cudaSuccess) return fail(e == cudaErrorInvalidValue ? ISDF_ERR_INVALID : ISDF_ERR_CUDA, std::string("swept: ") + cudaGetErrorString(e));
-    if (c->peer_fused && c->peer.world > 1 && c->world > 1) {   // an unsharded call (isdf_set_shard(ctx, 0, 1)) stays local
-        if (c->peer.world != c->world || c->peer.rank != c->rank) return fail(ISDF_ERR_STATE, "peer group does not match isdf_set_shard");
-        if (19 * N + 1 > c->peer.cap) return fail(ISDF_ERR_INVALID, "peer exchange buffer too small for this N (isdf_peer_export max_doubles)");
-        PeerArgs P = c->peer;
-        P.epoch = c->peer.epoch + 1;
+    if (fused_exchange(c)) {
+        if (int r = peer_fuse_check(c, N)) return r;
+        PeerArgs P = c->peer.args;
+        P.epoch = c->peer.args.epoch + 1;
         k_peer_allreduce<<<1, 512, 0, st>>>(P, d_out, 19 * N + 1);
         c->stats.kernel_launches++;
         CU_TRY(cudaGetLastError());
-        c->peer.epoch = P.epoch;   // committed only once the exchange is enqueued: a local failure must not leave this rank one epoch ahead
+        c->peer.args.epoch = P.epoch;
     }
     return 0;
 }
@@ -1717,7 +1738,7 @@ static int swept_common(isdf_ctx *c, int N, const double *d_T, const double *d_C
 extern "C" int isdf_eval_swept_device(isdf_ctx *c, int N, const double *d_T, const double *d_coeffs, double *d_out, void *cuda_stream) {
     int r = check_eval_state(c, N, false);
     if (r) return r;
-    if (!c->have_shape) return fail(ISDF_ERR_STATE, "shape not set");
+    if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
     if (!d_T || !d_coeffs || !d_out) return fail(ISDF_ERR_INVALID, "NULL device pointer");
     if (set_device(c)) return ISDF_ERR_CUDA;
     return swept_common(c, N, d_T, d_coeffs, d_out, (cudaStream_t)cuda_stream, nullptr, nullptr, nullptr);
@@ -1727,43 +1748,23 @@ static int eval_swept_host(isdf_ctx *c, int N, const double *T, const double *co
                            const double *g_g, double *cost, double *gradC, double *gradT) {
     int r = check_eval_state(c, N, false);
     if (r) { poison(cost); return r; }
-    if (!c->have_shape) { poison(cost); return fail(ISDF_ERR_STATE, "shape not set"); }
+    if (!c->mesh.have_shape) { poison(cost); return fail(ISDF_ERR_STATE, "shape not set"); }
     if (!T || !coeffs || !cost || !gradC || !gradT) { poison(cost); return fail(ISDF_ERR_INVALID, "NULL argument"); }
-    auto body = [&]() -> int {
-        if (set_device(c)) return ISDF_ERR_CUDA;
-        const size_t nin = (size_t)19 * N, nout = (size_t)19 * N + 1;
-        if (ensure_stage(c, nin + nout + 1)) return ISDF_ERR_CUDA;
-        CU_TRY(c->d_C.ensure(nin)); CU_TRY(c->d_out.ensure(nout + 1));
-        std::memcpy(c->h_stage, coeffs, sizeof(double) * 18 * N);
-        std::memcpy(c->h_stage + 18 * (size_t)N, T, sizeof(double) * N);
-        CU_TRY(cudaMemcpyAsync(c->d_C.p, c->h_stage, sizeof(double) * nin, cudaMemcpyHostToDevice, c->stream));
-        ScopedDevBuf<double> dgt, dgs, dgg;
-        if (g_t) {
-            CU_TRY(dgt.upload(g_t, c->sv.P, c->stream)); CU_TRY(dgs.upload(g_s, c->sv.P, c->stream));
-            CU_TRY(dgg.upload(g_g, (size_t)3 * c->sv.P, c->stream));
-        }
-        CU_TRY(cudaEventRecord(c->ev0, c->stream));
-        c->sv.count_out = c->d_out.p + nout;
-        int rr = swept_common(c, N, c->d_C.p + 18 * (size_t)N, c->d_C.p, c->d_out.p, c->stream, dgt.p, dgs.p, dgg.p);
-        c->sv.count_out = nullptr;
-        if (rr) return rr;
-        CU_TRY(cudaEventRecord(c->ev1, c->stream));
-        double *h_out = c->h_stage + nin;
-        CU_TRY(cudaMemcpyAsync(h_out, c->d_out.p, sizeof(double) * (nout + 1), cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaStreamSynchronize(c->stream));
-        unsigned long long nsdf = 0;
-        std::memcpy(&nsdf, h_out + nout, sizeof(nsdf));
-        if (c->peer_fused && c->peer.world > 1 && c->world > 1 && isdf_peer_status(c) != ISDF_OK) return ISDF_ERR_CUDA;   // exchange timed out: the vector is NaN
-        float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
-        c->stats.last_kernel_ms = ms; c->stats.last_sdf_evals = (int64_t)nsdf;
-        *cost += h_out[0];                                   // accumulate like hpp:640-645
-        for (size_t k = 0; k < (size_t)18 * N; k++) gradC[k] += h_out[1 + k];
-        for (int k = 0; k < N; k++) gradT[k] += h_out[1 + 18 * N + k];
-        return 0;
-    };
-    r = body();
-    if (r) poison(cost);
-    return r;
+    DevBuf<double> dgt, dgs, dgg;   // isdf_eval_swept_given: the given t*, sdf and gradients
+    return eval_host(c, N, T, coeffs, cost, gradC, gradT, &isdf_stats::last_sdf_evals,
+                     [&]() -> int {
+                         if (g_t) {
+                             CU_TRY(dgt.upload(g_t, c->sv.P, c->stream)); CU_TRY(dgs.upload(g_s, c->sv.P, c->stream));
+                             CU_TRY(dgg.upload(g_g, (size_t)3 * c->sv.P, c->stream));
+                         }
+                         return 0;
+                     },
+                     [&](const double *d_T, const double *d_C, double *d_out, double *count_out) {
+                         c->sv.count_out = count_out;
+                         const int rr = swept_common(c, N, d_T, d_C, d_out, c->stream, dgt.p, dgs.p, dgg.p);
+                         c->sv.count_out = nullptr;
+                         return rr;
+                     });
 }
 
 extern "C" int isdf_eval_swept(isdf_ctx *c, int N, const double *T, const double *coeffs, double *cost, double *gradC, double *gradT) {
@@ -1796,18 +1797,18 @@ extern "C" int isdf_dbg_enable(isdf_ctx *c, int on) { if (!c) return -1; c->dbg_
 // GPU); 0 restores the device's own figure.
 extern "C" int isdf_dbg_schedule(isdf_ctx *c, int natural_order, int warp_slots) {
     if (!c) return -1;
-    c->no_items = natural_order != 0; c->warp_slots_override = warp_slots > 0 ? warp_slots : 0; c->order_for = -1;
+    c->disc.no_items = natural_order != 0; c->disc.warp_slots_override = warp_slots > 0 ? warp_slots : 0; c->disc.order_for = -1;
     return 0;
 }
 // number of work items / split samples of the table built by the last discrete evaluation
 extern "C" int isdf_dbg_item_stats(isdf_ctx *c, int *item_count, int *split_parts) {
-    if (!c || !item_count || !split_parts || !c->d_item_count.p) return -1;
+    if (!c || !item_count || !split_parts || !c->disc.d_item_count.p) return -1;
     if (cudaSetDevice(c->device) != cudaSuccess) return -3;
     cudaStreamSynchronize(c->stream); cudaStreamSynchronize(c->aux_stream);
     int n = 0;
-    if (cudaMemcpy(&n, c->d_item_count.p, sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (cudaMemcpy(&n, c->disc.d_item_count.p, sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
     std::vector<int> it((size_t)3 * std::max(n, 1));
-    if (n > 0 && cudaMemcpy(it.data(), c->d_items.p, sizeof(int) * 3 * n, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (n > 0 && cudaMemcpy(it.data(), c->disc.d_items.p, sizeof(int) * 3 * n, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
     int parts = 0;
     for (int k = 0; k < n; k++) if (it[3 * k + 2] >= 0) parts++;
     *item_count = n; *split_parts = parts;
@@ -1818,7 +1819,7 @@ extern "C" int isdf_dbg_item_stats(isdf_ctx *c, int *item_count, int *split_part
 extern "C" int isdf_dbg_flatness(isdf_ctx *c, int n, const double *vaj, const double *grads, double *out) {
     if (!c || n < 1 || !vaj || !grads || !out) return -1;
     if (cudaSetDevice(c->device) != cudaSuccess) return -3;
-    ScopedDevBuf<double> dv, dg, dout;
+    DevBuf<double> dv, dg, dout;
     cudaError_t e = dv.upload(vaj, (size_t)9 * n, c->stream);
     if (e == cudaSuccess) e = dg.upload(grads, (size_t)10 * n, c->stream);
     if (e == cudaSuccess) e = dout.ensure((size_t)16 * n);
@@ -1833,13 +1834,13 @@ extern "C" int isdf_dbg_flatness(isdf_ctx *c, int n, const double *vaj, const do
 // list was built).
 extern "C" int isdf_dbg_mesh_grid(isdf_ctx *c, double *geom, int32_t *gdim, float *cell_dist, uint16_t *cell_cnt) {
     if (!c || !geom || !gdim) return -1;
-    if (!c->have_shape || c->shape.kind != ISDF_SHAPE_MESH) return -2;
-    const DevMesh &m = c->shape.mesh;
+    if (!c->mesh.have_shape || c->mesh.shape.kind != ISDF_SHAPE_MESH) return -2;
+    const DevMesh &m = c->mesh.shape.mesh;
     for (int a = 0; a < 3; a++) { geom[a] = m.glo[a]; gdim[a] = m.gdim[a]; }
-    geom[3] = m.gcell; geom[4] = m.ghd; geom[5] = m.gpad; geom[6] = m.sign_radius; geom[7] = c->mesh_list_reach;
+    geom[3] = m.gcell; geom[4] = m.ghd; geom[5] = m.gpad; geom[6] = m.sign_radius; geom[7] = c->mesh.list_reach;
     const size_t ncell = (size_t)m.gdim[0] * m.gdim[1] * m.gdim[2];
     if (cudaSetDevice(c->device) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) return -3;
-    if (cell_dist && cudaMemcpy(cell_dist, c->d_cell_dist.p, sizeof(float) * ncell, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (cell_dist && cudaMemcpy(cell_dist, c->mesh.d_cell_dist.p, sizeof(float) * ncell, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
     if (cell_cnt) {
         if (!m.cell_cnt) std::memset(cell_cnt, 0, sizeof(uint16_t) * ncell);
         else if (cudaMemcpy(cell_cnt, m.cell_cnt, sizeof(uint16_t) * ncell, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
@@ -1851,8 +1852,8 @@ extern "C" int isdf_dbg_mesh_grid(isdf_ctx *c, double *geom, int32_t *gdim, floa
 // optional — call with NULL first to size them.
 extern "C" int isdf_dbg_mesh_lists(isdf_ctx *c, long long *sizes, uint32_t *cell_off, uint32_t *cand, float *cand_lb, double *tris) {
     if (!c || !sizes) return -1;
-    if (!c->have_shape || c->shape.kind != ISDF_SHAPE_MESH) return -2;
-    const DevMesh &m = c->shape.mesh;
+    if (!c->mesh.have_shape || c->mesh.shape.kind != ISDF_SHAPE_MESH) return -2;
+    const DevMesh &m = c->mesh.shape.mesh;
     const size_t ncell = (size_t)m.gdim[0] * m.gdim[1] * m.gdim[2];
     if (cudaSetDevice(c->device) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) return -3;
     size_t total = 0;
@@ -1876,19 +1877,19 @@ extern "C" int isdf_dbg_swept_stats(isdf_ctx *c, unsigned long long *out, long l
 }
 // {candidate pairs (voxel centre inside the H box), exact mesh searches} of the last clearance check
 extern "C" int isdf_dbg_clearance_counts(isdf_ctx *c, unsigned long long *out) {
-    if (!c || !out || !c->d_clr_counters.p) return -1;
+    if (!c || !out || !c->clr.d_counters.p) return -1;
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
-    return cudaMemcpy(out, c->d_clr_counters.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -1;
+    return cudaMemcpy(out, c->clr.d_counters.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -1;
 }
 extern "C" int isdf_dbg_trace_stride(void) { return TRACE_STRIDE; }
 extern "C" int isdf_dbg_item_trace(isdf_ctx *c, unsigned long long *out, long long n) {
-    if (!c || !out || (size_t)n > c->d_trace.n) return -1;
+    if (!c || !out || (size_t)n > c->disc.d_trace.n) return -1;
     if (cudaSetDevice(c->device) != cudaSuccess) return -3;
-    return cudaMemcpy(out, c->d_trace.p, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -3;
+    return cudaMemcpy(out, c->disc.d_trace.p, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -3;
 }
 extern "C" int isdf_dbg_sample_stats(isdf_ctx *c, unsigned long long *out, long long n) {
-    if (!c || !out || (size_t)n > c->d_dbg.n) return -1;
+    if (!c || !out || (size_t)n > c->disc.d_dbg.n) return -1;
     if (cudaSetDevice(c->device) != cudaSuccess) return -3;
-    return cudaMemcpy(out, c->d_dbg.p, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -3;
+    return cudaMemcpy(out, c->disc.d_dbg.p, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -3;
 }

@@ -1004,9 +1004,11 @@ struct SweptState {
     double *count_out = nullptr;   // set by the host entry point around one launch
     bool dbg_on = false;
 
+    // the only place that replaces the point set: it gives up the current one (and any per-problem sets: set_points_batch sets B
+    // after it) before it touches the buffers
     cudaError_t set_points(const double *pts, int n, cudaStream_t st) {
         cudaError_t e = cudaSuccess;
-        P = 0;
+        P = 0; B = 0;
         if (n == 0) return e;
         if ((e = d_pts.upload(pts, (size_t)3 * n, st)) != cudaSuccess) return e;
         if ((e = d_tstar.ensure(n)) != cudaSuccess) return e;
@@ -1088,7 +1090,6 @@ struct SweptState {
     std::vector<int> h_off;
     DevBuf<int> d_off;
     cudaError_t set_points_batch(int nB, const int *off, const double *pts, cudaStream_t st) {
-        B = 0;
         cudaError_t e = set_points(pts, off[nB], st);
         if (e != cudaSuccess) return e;
         if ((e = d_off.upload(off, (size_t)nB + 1, st)) != cudaSuccess) return e;
@@ -1136,11 +1137,6 @@ struct SweptState {
         k_sv_finish_b<<<dim3(1, B), 32, 0, st>>>(Bt);
         *launches = 3 + (maxP > 0 ? 1 : 0);
         return cudaGetLastError();
-    }
-    void release() {
-        d_off.release();
-        d_pts.release(); d_tstar.release(); d_sdf.release(); d_grel.release(); d_times.release(); d_poses.release(); d_state.release();
-        d_partial.release(); d_piece_gdt.release(); d_piece_cost.release(); d_piece.release(); d_meta.release(); d_counter.release(); d_dbg.release(); d_work.release(); d_order.release();
     }
 };
 

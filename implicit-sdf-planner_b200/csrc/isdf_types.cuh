@@ -2,6 +2,7 @@
 #pragma once
 #include "isdf_math.cuh"
 #include "isdf_shapes.cuh"
+#include <utility>
 
 namespace isdf {
 
@@ -26,15 +27,19 @@ struct DevCfg {
     int flags;
 };
 
-// growable device buffer (host-side helper)
-template <typename T>
-struct DevBuf {
+// Growable buffer (host-side helper) that owns its allocation: device memory (DevBuf) or pinned host memory (PinnedBuf, staging for
+// one-copy transfers). ensure / upload only grow, and growing discards the contents. Move-only; `buf = {}` frees it.
+template <typename T, bool PINNED>
+struct OwnedBuf {
     T *p = nullptr; size_t n = 0;
+    OwnedBuf() = default;
+    OwnedBuf(OwnedBuf &&o) noexcept : p(o.p), n(o.n) { o.p = nullptr; o.n = 0; }
+    OwnedBuf &operator=(OwnedBuf &&o) noexcept { std::swap(p, o.p); std::swap(n, o.n); return *this; }
+    ~OwnedBuf() { if (p) PINNED ? cudaFreeHost(p) : cudaFree(p); }
     cudaError_t ensure(size_t cnt) {
         if (cnt <= n) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr; n = 0;
-        cudaError_t e = cudaMalloc((void **)&p, cnt * sizeof(T));
+        *this = OwnedBuf();
+        cudaError_t e = PINNED ? cudaMallocHost((void **)&p, cnt * sizeof(T)) : cudaMalloc((void **)&p, cnt * sizeof(T));
         if (e == cudaSuccess) n = cnt;
         return e;
     }
@@ -43,17 +48,9 @@ struct DevBuf {
         if (e != cudaSuccess) return e;
         return cudaMemcpyAsync(p, h, cnt * sizeof(T), cudaMemcpyHostToDevice, st);
     }
-    void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
 };
-
-// function-local scratch buffer: released on EVERY exit path (the CU_TRY early returns of the query entry points included)
-template <typename T>
-struct ScopedDevBuf : DevBuf<T> {
-    ScopedDevBuf() = default;
-    ScopedDevBuf(const ScopedDevBuf &) = delete;
-    ScopedDevBuf &operator=(const ScopedDevBuf &) = delete;
-    ~ScopedDevBuf() { this->release(); }
-};
+template <typename T> using DevBuf = OwnedBuf<T, false>;
+template <typename T> using PinnedBuf = OwnedBuf<T, true>;
 
 constexpr int PARTIAL_STRIDE = 20;  // per sample / per point: 18 gradC entries (axis*6+k), gradT term, cost term
 

@@ -15,6 +15,10 @@
  *   - Matrices follow Eigen's defaults: `coeffs`/`gradC` are MatrixX3d (6N x 3) COLUMN-major:
  *     element (6*i + k, axis) at [axis*6N + 6*i + k] = t^k coefficient of piece i (hpp:434,460).
  *   - There is no CPU fallback: if no CUDA device / kernel image is usable, isdf_create fails.
+ *   - Setters that replace state (maps, the robot shape, the front-end kernels, obstacle point sets) check their arguments first: a
+ *     refused call leaves the previous state in place. Before a setter touches the device memory the current state lives in, it gives
+ *     that state up (a new shape also gives up the front-end kernels), and it sets the new state only once it is complete: a CUDA
+ *     failure leaves no map / shape / kernels / point set, and later calls that need one get ISDF_ERR_STATE.
  */
 #ifndef ISDF_H
 #define ISDF_H
@@ -152,10 +156,9 @@ int isdf_set_map_f64(isdf_ctx *ctx, const double *grid_map, int X, int Y, int Z,
  *     the reference allocates a zero-size grid and writes past it);
  *   - the size limits of isdf_set_map_u8 apply with its codes (X*Y*ceil(Z/32) < 2^31, Z <= 65535, the 1023-voxel pose window), and
  *     the message names the dimensions the cloud asked for.
- * Argument checks run before any device call. A refused call leaves the previous map in place; a CUDA failure leaves no map (later
- * calls get ISDF_ERR_STATE). The result is the same bits whatever the order of the points and through either entry point. The call
- * counts its launches in isdf_stats.kernel_launches and touches no other field. sta_threshold > 1 needs 4 bytes of device scratch per
- * voxel during the call. */
+ * Argument checks run before any device call; refused calls and CUDA failures behave as Conventions says. The result is the same bits
+ * whatever the order of the points and through either entry point. The call counts its launches in isdf_stats.kernel_launches and
+ * touches no other field. sta_threshold > 1 needs 4 bytes of device scratch per voxel during the call. */
 int isdf_set_map_cloud(isdf_ctx *ctx, const void *points, int64_t n, int32_t stride_bytes, double res, int32_t sta_threshold);
 /* the same with the points on ctx's device. Work before the call on cuda_stream is waited for: the call synchronises cuda_stream once
  * (the grid size depends on the bounds), builds the grid on ctx's own stream and returns when the map is set, so d_points may be
