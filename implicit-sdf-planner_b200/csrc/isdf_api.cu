@@ -1875,6 +1875,13 @@ extern "C" int isdf_dbg_swept_stats(isdf_ctx *c, unsigned long long *out, long l
     cudaStreamSynchronize(c->stream);
     return cudaMemcpy(out, c->sv.d_dbg.p, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -3;
 }
+// the swept-volume term of the last batched callback, B x (19 N0 + 1): per problem [cost | gradC 18 N0 | gradT N0], as the callback adds it
+extern "C" int isdf_dbg_batch_swept_out(isdf_ctx *c, double *out, long long n) {
+    if (!c || !out || n < 0 || (size_t)n > c->batch.d_sv.n) return -1;
+    if (cudaSetDevice(c->device) != cudaSuccess) return -3;
+    cudaStreamSynchronize(c->stream);
+    return cudaMemcpy(out, c->batch.d_sv.p, sizeof(double) * n, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -3;
+}
 // {candidate pairs (voxel centre inside the H box), exact mesh searches} of the last clearance check
 extern "C" int isdf_dbg_clearance_counts(isdf_ctx *c, unsigned long long *out) {
     if (!c || !out || !c->clr.d_counters.p) return -1;

@@ -996,7 +996,9 @@ __global__ void k_sv_finish_b(const __grid_constant__ SvBatch Bt) { __shared__ S
 // ---- host-side state ----------------------------------------------------------------------------------------------
 struct SweptState {
     int P = 0;
-    DevBuf<double> d_pts, d_tstar, d_sdf, d_grel, d_times, d_poses, d_state, d_partial, d_piece_gdt, d_piece_cost;
+    // traj_duration (updateTraj, swm:287-296) persists across evaluations: d_state[0] for the single-problem entry points, d_state_b[4 b]
+    // for problem b of the batched callback — separate, so that neither path sees the other's trajectories
+    DevBuf<double> d_pts, d_tstar, d_sdf, d_grel, d_times, d_poses, d_state, d_state_b, d_partial, d_piece_gdt, d_piece_cost;
     DevBuf<int> d_piece, d_meta;
     DevBuf<unsigned long long> d_counter, d_dbg;
     DevBuf<unsigned> d_work; DevBuf<int> d_order;
@@ -1105,9 +1107,13 @@ struct SweptState {
         if ((e = d_times.ensure((size_t)B * SV_MAX_COARSE)) != cudaSuccess) return e;
         if ((e = d_poses.ensure((size_t)12 * B * SV_MAX_COARSE)) != cudaSuccess) return e;
         if ((e = d_meta.ensure((size_t)4 * B)) != cudaSuccess) return e;
-        if (d_state.n < (size_t)4 * B) {   // traj_duration of every problem persists across evaluations (updateTraj quirk, swm:287-296): starts at 0
-            if ((e = d_state.ensure((size_t)4 * B)) != cudaSuccess) return e;
-            if ((e = cudaMemsetAsync(d_state.p, 0, sizeof(double) * 4 * B, st)) != cudaSuccess) return e;
+        if (d_state_b.n < (size_t)4 * B) {   // a problem's traj_duration starts at 0; growing B keeps the durations of the problems already there
+            DevBuf<double> grown;
+            if ((e = grown.ensure((size_t)4 * B)) != cudaSuccess) return e;
+            if ((e = cudaMemsetAsync(grown.p, 0, sizeof(double) * 4 * B, st)) != cudaSuccess) return e;
+            if (d_state_b.n && (e = cudaMemcpyAsync(grown.p, d_state_b.p, sizeof(double) * d_state_b.n, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return e;
+            if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return e;   // the old buffer is freed below
+            d_state_b = std::move(grown);
         }
         if (d_counter.n == 0) { if ((e = d_counter.ensure(2)) != cudaSuccess) return e; }
         if ((e = d_piece_gdt.ensure((size_t)B * N)) != cudaSuccess) return e;
@@ -1116,7 +1122,7 @@ struct SweptState {
         SvArgs &A = Bt.base;
         A.cfg = cfg; A.shape = shape; A.N = N; A.T = d_T; A.C = d_Cpp; A.P = 0; A.pts = d_pts.p;
         A.tstar = d_tstar.p; A.sdf = d_sdf.p; A.grel = d_grel.p; A.times = d_times.p; A.poses = d_poses.p; A.meta = d_meta.p;
-        A.state = d_state.p; A.partial = d_partial.p; A.piece = d_piece.p; A.piece_gdt = d_piece_gdt.p; A.piece_cost = d_piece_cost.p;
+        A.state = d_state_b.p; A.partial = d_partial.p; A.piece = d_piece.p; A.piece_gdt = d_piece_gdt.p; A.piece_cost = d_piece_cost.p;
         A.out = d_out; A.counter = d_counter.p; A.count_out = nullptr; A.rank = 0; A.world = 1; A.g_t = nullptr; A.g_s = nullptr; A.g_g = nullptr; A.dbg = nullptr; A.dbg2 = nullptr;
         A.work = nullptr; A.order = nullptr; A.use_order = 0;
         Bt.B = B; Bt.pt_off = d_off.p; Bt.out_stride = 19ll * N + 1;

@@ -361,6 +361,17 @@ class Evaluator:
             off[b + 1] = off[b] + len(p)
         pts = _f64(np.concatenate([np.asarray(p, float).reshape(-1, 3) for p in point_sets])) if B and off[B] else np.zeros((0, 3))
         self._check(self.lib.isdf_set_points_batch(self.h, B, off.ctypes.data_as(C.POINTER(C.c_int32)), _dp(pts) if pts.size else None))
+        if B:
+            self.n_points = int(off[B])       # swept_results() then returns every problem's points, problem-major
+
+    def dbg_batch_swept_out(self, B, N0):
+        """the swept-volume term of the last batched callback (isdf_dbg_batch_swept_out, not part of include/isdf.h): (B, 19*N0+1) rows
+        [cost | gradC 18*N0 | gradT N0]"""
+        out = np.zeros((B, 19 * N0 + 1))
+        self.lib.isdf_dbg_batch_swept_out.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.c_longlong]
+        if self.lib.isdf_dbg_batch_swept_out(self.h, _dp(out.reshape(-1)), out.size) != 0:
+            raise IsdfError(-1, "isdf_dbg_batch_swept_out failed")
+        return out
 
     def lbfgs_params(self, **kw):
         p = LbfgsParams()

@@ -218,7 +218,12 @@ int isdf_get_piece_costs(isdf_ctx *ctx, double *piece_cost, int n);
  * reference — swept-volume term (addSaftyPenaOnSweptVolumeParallel, hpp:386-391) then time-integral term (hpp:399-405) — for every problem,
  * each stage one launch over the whole batch (grid.y = problem). */
 /* problem b owns the points [offsets[b], offsets[b+1]) of pts (offsets: B+1 ints, offsets[0] = 0; what plan_manager.cpp:232-254 builds per plan);
- * t* of every point starts at 0 and persists across evaluations like lastTstar. B = 0 switches the batched swept-volume term off again. */
+ * t* of every point starts at 0 and persists across evaluations like lastTstar. B = 0 switches the batched swept-volume term off again.
+ * Persisted trajectory duration (updateTraj, swm:287-296): a trajectory of 300 s or longer is not taken; the search then scans the
+ * duration of the last trajectory shorter than 300 s (0 if there was none). The batched callback keeps one such duration per problem
+ * index b; isdf_eval_swept / _device / _given keep one of their own. They never share a value. All start at 0 when the context is
+ * created and live as long as it: isdf_set_points and isdf_set_points_batch leave them alone, and registering a larger B keeps the
+ * durations of problems 0 .. B_old-1 and starts the new problems at 0. */
 int isdf_set_points_batch(isdf_ctx *ctx, int B, const int32_t *offsets, const double *pts);
 int isdf_callback_batch(isdf_ctx *ctx, int B, int N0, const double *head, const double *tail, int per_problem_bc, double rho,
                         const double *x, double *cost, double *grad);
@@ -338,7 +343,8 @@ int isdf_frontend_check_batch(isdf_ctx *ctx, int n, const int32_t *ind, const do
                               double *child_roll_pitch, uint8_t *ok);
 
 /* ---- swept-volume term: addSaftyPenaOnSweptVolumeParallel (hpp:557-649) + getSDFofSweptVolume (swm:710-747) --- */
-/* parallel_points (plan_manager.cpp:246-254): P x 3 row-major world-frame voxel centres; resets lastTstar to 0 */
+/* parallel_points (plan_manager.cpp:246-254): P x 3 row-major world-frame voxel centres; resets lastTstar to 0 (not the persisted
+ * trajectory duration: see isdf_set_points_batch) */
 int isdf_set_points(isdf_ctx *ctx, const double *pts, int P);
 int isdf_eval_swept(isdf_ctx *ctx, int N, const double *T, const double *coeffs,
                     double *cost, double *gradC, double *gradT);

@@ -156,19 +156,46 @@ int orc_eval_discrete(const orc_config *c, const uint8_t *occ, int X, int Y, int
 }
 
 // Swept-volume path. tstar in/out (lastTstar). sdf_out / grel_out optional. given_* optional (tier-T1 tail parity).
-int orc_eval_swept(const orc_config *c, void *shape, int N, const double *T, const double *C, int npts, const double *pts,
-                   double *tstar, double *cost, double *gradC, double *gradT, double *sdf_out, double *grel_out,
-                   long long *nsdf, int use_omp, const double *given_tstar, const double *given_sdf, const double *given_grel) {
+// traj_duration (optional, in/out): the SweptVolumeManager's duration before the evaluation (NULL: 0, a fresh manager) and after it —
+// the replay of quirk Q14 across a sequence of evaluations.
+int orc_eval_swept_ex(const orc_config *c, void *shape, int N, const double *T, const double *C, int npts, const double *pts,
+                      double *tstar, double *cost, double *gradC, double *gradT, double *sdf_out, double *grel_out,
+                      long long *nsdf, int use_omp, const double *given_tstar, const double *given_sdf, const double *given_grel,
+                      double *traj_duration) {
     Params P = to_params(c);
     Traj tr; tr.N = N; tr.T = T; tr.C = C;
     EvalOut out;
     SweptGiven gv{given_tstar, given_sdf, given_grel};
-    eval_swept(P, ((OrcShape *)shape)->s, tr, npts, pts, tstar, out, use_omp != 0, sdf_out, grel_out, given_tstar ? &gv : nullptr);
+    const double prev = traj_duration ? *traj_duration : 0.0;
+    eval_swept(P, ((OrcShape *)shape)->s, tr, npts, pts, tstar, out, use_omp != 0, sdf_out, grel_out, given_tstar ? &gv : nullptr, prev);
     *cost = out.cost;
     std::memcpy(gradC, out.gradC.data(), sizeof(double) * 18 * N);
     std::memcpy(gradT, out.gradT.data(), sizeof(double) * N);
     if (nsdf) *nsdf = out.n_sdf;
+    if (traj_duration) { const double td = tr.total(); *traj_duration = td < 3 * 1e2 ? td : prev; }
     return 0;
+}
+int orc_eval_swept(const orc_config *c, void *shape, int N, const double *T, const double *C, int npts, const double *pts,
+                   double *tstar, double *cost, double *gradC, double *gradT, double *sdf_out, double *grel_out,
+                   long long *nsdf, int use_omp, const double *given_tstar, const double *given_sdf, const double *given_grel) {
+    return orc_eval_swept_ex(c, shape, N, T, C, npts, pts, tstar, cost, gradC, gradT, sdf_out, grel_out, nsdf, use_omp, given_tstar, given_sdf,
+                             given_grel, nullptr);
+}
+
+// Coarse in-range decisions of the swept-volume search (SweptVolume::coarse) for npts points: bits npts x words (point-major), margin and
+// carried per point. traj_duration is the duration before the evaluation, as for orc_eval_swept_ex. Returns the number of coarse samples.
+int orc_sv_coarse(const orc_config *c, void *shape, int N, const double *T, const double *C, int npts, const double *pts, double traj_duration,
+                  uint32_t *bits, int words, double *margin, int *carried) {
+    Params P = to_params(c);
+    Traj tr; tr.N = N; tr.T = T; tr.C = C;
+    int nc = 0;
+#pragma omp parallel for schedule(dynamic, 4) reduction(max : nc)
+    for (int k = 0; k < npts; k++) {
+        SweptVolume sv; sv.P = &P; sv.S = &((OrcShape *)shape)->s; sv.tr = &tr; sv.F.reset(P.mass, P.grav, P.dh, P.dv, P.cp, P.veps);
+        sv.traj_duration = traj_duration; sv.update();
+        nc = std::max(nc, sv.coarse(V3(pts[3 * k], pts[3 * k + 1], pts[3 * k + 2]), bits + (size_t)words * k, words, margin[k], carried[k]));
+    }
+    return nc;
 }
 
 // Single swept-volume SDF query (getSDFofSweptVolume<true>(p, t, g, false), swm:710-747)

@@ -361,6 +361,27 @@ struct SweptVolume {
             rts.push_back(range_time_seed);
         }
     }
+    // test hook: choiceTInit's coarse loop as above, recorded instead of acted on. Sets bit k of bits (words of 32) when coarse sample k is
+    // in range; returns the number of coarse samples (at most 32 * words: later samples are counted, not recorded). margin = the smallest
+    // |dis - inf| over the samples (how far the closest coarse decision is from flipping). carried = closed runs after the first whose fine
+    // scan leaves range_mindis unchanged, so that their descent starts from an earlier run's seed.
+    int coarse(const V3 &p, uint32_t *bits, int words, double &margin, int &carried) {
+        const double inf = 2 * P->safety_hor + 0.1;
+        for (int w = 0; w < words; w++) bits[w] = 0u;
+        margin = 1e300;
+        int nc = 0;
+        for (double t = 0; t < traj_duration; t += 0.2) {
+            const double dis = sdf_at(p, t);
+            margin = std::min(margin, std::abs(dis - inf));
+            if (dis < inf && nc < 32 * words) bits[nc >> 5] |= 1u << (nc & 31);
+            nc++;
+        }
+        std::vector<double> rl, rr, rts;
+        choice_t_init(p, 0.02, rl, rr, rts);
+        carried = 0;
+        for (size_t i = 1; i < rts.size(); i++) carried += rts[i] == rts[i - 1];
+        return nc;
+    }
     // gradientDescent (swm:1000-1062): sign-descent with step halving, quirk Q5
     void gradient_descent(double t_min, double t_max, double x0, double &fx, double &x, const V3 &p) {
         const int max_iter = 300; const double alpha = 0.02, tol = 1e-5;
@@ -417,14 +438,16 @@ inline bool grad_cost_p_sw(const Params &P, const V3 &pos_eva, const V3 &pos_obj
 // If tstar_given != nullptr the t* search is skipped and the tail is evaluated at the given t*/sdf*/g_rel
 // (parity tier T1, SURVEY §7).
 struct SweptGiven { const double *tstar, *sdf, *grel; };
+// prev_duration: the SweptVolumeManager's traj_duration before this evaluation (0 for a fresh manager), which a trajectory of 300 s or
+// longer leaves in place (quirk Q14)
 inline void eval_swept(const Params &P, const Shape &S, const Traj &tr, int npts, const double *pts, double *tstar,
                        EvalOut &out, bool use_omp, double *sdf_out = nullptr, double *grel_out = nullptr,
-                       const SweptGiven *given = nullptr) {
+                       const SweptGiven *given = nullptr, double prev_duration = 0.0) {
     Flat F; F.reset(P.mass, P.grav, P.dh, P.dv, P.cp, P.veps);
     const int N = tr.N;
     out.gradC.assign((size_t)18 * N, 0.0); out.gradT.assign(N, 0.0); out.cost = 0; out.n_sdf = 0;
     auto body = [&](int k, double gdC[18], double &gdT, double &pena, int &piece, long long &nsdf) {
-        SweptVolume sv; sv.P = &P; sv.S = &S; sv.tr = &tr; sv.F = F; sv.update();
+        SweptVolume sv; sv.P = &P; sv.S = &S; sv.tr = &tr; sv.F = F; sv.traj_duration = prev_duration; sv.update();
         const V3 pe(pts[3 * k], pts[3 * k + 1], pts[3 * k + 2]);
         V3 grel;  // uninitialised Vector3d in the reference (hpp:574); zero here — unused when no interval (quirk Q3)
         double sdf_value;

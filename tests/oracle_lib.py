@@ -61,6 +61,9 @@ def lib():
                                         C.c_void_p, C.c_int, dp, dp, dp, dp, dp, C.POINTER(C.c_longlong), C.c_int, C.c_int, C.c_int]
         L.orc_eval_swept.argtypes = [C.POINTER(OrcConfig), C.c_void_p, C.c_int, dp, dp, C.c_int, dp, dp, dp, dp, dp, dp, dp,
                                      C.POINTER(C.c_longlong), C.c_int, dp, dp, dp]
+        L.orc_eval_swept_ex.argtypes = L.orc_eval_swept.argtypes + [dp]
+        L.orc_sv_coarse.argtypes = [C.POINTER(OrcConfig), C.c_void_p, C.c_int, dp, dp, C.c_int, dp, C.c_double, C.POINTER(C.c_uint32), C.c_int, dp,
+                                    C.POINTER(C.c_int32)]
         L.orc_sdf_swept.restype = C.c_double
         L.orc_sdf_swept.argtypes = [C.POINTER(OrcConfig), C.c_void_p, C.c_int, dp, dp, dp, dp, dp]
         L.orc_points_in_aabb.argtypes = [C.POINTER(C.c_uint8), C.c_int, C.c_int, C.c_int, dp, C.c_double, dp, C.c_double, dp, C.c_int]
@@ -384,7 +387,9 @@ def eval_discrete(cfg, occ, bmin, res, shape, T, coeffs, use_omp=False, rank=0, 
     return cost.value, gC, gT, npairs.value
 
 
-def eval_swept(cfg, shape, T, coeffs, pts, tstar=None, use_omp=False, given=None):
+def eval_swept(cfg, shape, T, coeffs, pts, tstar=None, use_omp=False, given=None, prev_duration=0.0):
+    """prev_duration: the persisted trajectory duration before this evaluation (a fresh SweptVolumeManager has 0); the result's
+    "duration" is the one after it (quirk Q14: a trajectory of 300 s or longer keeps the previous one)"""
     T = f64(T).reshape(-1)
     N = T.size
     Cc = f64(coeffs).reshape(-1)
@@ -396,9 +401,22 @@ def eval_swept(cfg, shape, T, coeffs, pts, tstar=None, use_omp=False, given=None
     g_t = g_s = g_g = None
     if given is not None:
         g_t, g_s, g_g = f64(given[0]), f64(given[1]), f64(given[2]).reshape(-1)
-    lib().orc_eval_swept(C.byref(cfg), shape.h, N, _p(T), _p(Cc), P, _p(pts), _p(ts), C.byref(cost), _p(gC), _p(gT), _p(sdf), _p(grel),
-                         C.byref(nsdf), int(use_omp), _p(g_t), _p(g_s), _p(g_g))
-    return dict(cost=cost.value, gradC=gC, gradT=gT, tstar=ts, sdf=sdf, grel=grel, nsdf=nsdf.value)
+    dur = C.c_double(prev_duration)
+    lib().orc_eval_swept_ex(C.byref(cfg), shape.h, N, _p(T), _p(Cc), P, _p(pts), _p(ts), C.byref(cost), _p(gC), _p(gT), _p(sdf), _p(grel),
+                            C.byref(nsdf), int(use_omp), _p(g_t), _p(g_s), _p(g_g), C.byref(dur))
+    return dict(cost=cost.value, gradC=gC, gradT=gT, tstar=ts, sdf=sdf, grel=grel, nsdf=nsdf.value, duration=dur.value)
+
+
+def sv_coarse(cfg, shape, T, coeffs, pts, prev_duration=0.0, words=48):
+    """the swept-volume search's coarse decisions per point: (nc, bits (P, words) uint32, margin (P,), carried (P,)) — see orc_sv_coarse"""
+    T = f64(T).reshape(-1)
+    Cc = f64(coeffs).reshape(-1)
+    pts = f64(pts).reshape(-1, 3)
+    P = pts.shape[0]
+    bits, margin, carried = np.zeros((P, words), dtype=np.uint32), np.zeros(P), np.zeros(P, dtype=np.int32)
+    nc = lib().orc_sv_coarse(C.byref(cfg), shape.h, T.size, _p(T), _p(Cc), P, _p(pts), float(prev_duration),
+                             bits.ctypes.data_as(C.POINTER(C.c_uint32)), words, _p(margin), carried.ctypes.data_as(C.POINTER(C.c_int32)))
+    return nc, bits, margin, carried
 
 
 def points_in_aabb(occ, bmin, res, centre, half, cap=100000):

@@ -270,45 +270,65 @@ def sv_case(N=4, seed=3, npts=400):
     return cfg, T, Cc, pts
 
 
-@pytest.mark.parametrize("name", ["Ball", "Torus", "RoundedCone", "SmoothIntersection", "CSG", "TwistBox"])
-def test_swept_tail_parity_given_tstar(name):
+@pytest.mark.parametrize("name,tilt", [(n, False) for n in ["Ball", "Torus", "RoundedCone", "SmoothIntersection", "CSG", "TwistBox"]] +
+                         [("CSG", True), ("TwistBox", True)])
+def test_swept_tail_parity_given_tstar(name, tilt):
     """tier T1: chain-rule tail at the oracle's t*, sdf*, g_rel"""
     cfg, T, Cc, pts = sv_case()
-    osh = O.Shape.named(name)
+    R, t = tilted() if tilt else (None, None)
+    osh = O.Shape.named(name, R, t)
     ref = O.eval_swept(O.config_from(cfg), osh, T, Cc, pts)
+    assert (ref["sdf"] < 9.99).sum() >= 10
     ev = I.Evaluator(cfg)
-    ev.set_shape_named(name)
+    ev.set_shape_named(name, R, t)
     ev.set_points(pts)
     got = ev.eval_swept_given(T, Cc, ref["tstar"], ref["sdf"], ref["grel"])
     check_eval(got, (ref["cost"], ref["gradC"], ref["gradT"]), tol=1e-9, what=f"T1 {name}")
     ev.close()
 
 
-@pytest.mark.parametrize("name", ["Ball", "Torus", "RoundedCone", "SmoothIntersection", "Box"])
-def test_swept_end_to_end_parity(name):
-    """tier T2: device-side search. Same accept/reject decisions => same t* to rounding."""
+@pytest.mark.parametrize("tilt", [False, True], ids=["untilted", "tilted"])
+@pytest.mark.parametrize("name", I.NAMED_SHAPES + ["Box"])
+def test_swept_end_to_end_parity(name, tilt):
+    """tier T2: device-side search. Same accept/reject decisions => same hit set, t*, SV-SDF, evaluation count and cost / gradient to
+    rounding (strict: t* 1e-12, SV-SDF 1e-10, cost / gradient 1e-9) — for every shape, also TwistBox, BendBox and Trefoil, whose SDFs call
+    sin / cos / atan2 (device and glibc results may differ in the last ulp; here that moves SV-SDF values by <= 7e-16, no decision).
+    CappedCone has no hit: its SDF grows slowly with distance (0.3 at 3 m, 1.2 at 25 m), so every point stays within range at every coarse
+    sample — one open run, dropped — and the test checks exactly that."""
     cfg, T, Cc, pts = sv_case(seed=5)
+    R, t = tilted() if tilt else (None, None)
     if name == "Box":
-        osh = O.Shape.analytic(I.SHAPE_KINDS["BOX"], [1.5, 0.3, 0.3])
+        osh = O.Shape.analytic(I.SHAPE_KINDS["BOX"], [1.5, 0.3, 0.3], R, t)
     else:
-        osh = O.Shape.named(name)
+        osh = O.Shape.named(name, R, t)
     ref = O.eval_swept(O.config_from(cfg), osh, T, Cc, pts)
     ev = I.Evaluator(cfg)
     if name == "Box":
-        ev.set_shape_analytic(I.SHAPE_KINDS["BOX"], [1.5, 0.3, 0.3])
+        ev.set_shape_analytic(I.SHAPE_KINDS["BOX"], [1.5, 0.3, 0.3], R, t)
     else:
-        ev.set_shape_named(name)
+        ev.set_shape_named(name, R, t)
     ev.set_points(pts)
     got = ev.eval_swept(T, Cc)
     ts, sd, gr = ev.swept_results()
     hit = ref["sdf"] < 9.99
+    dt_all = np.abs(ts - ref["tstar"])
+    dt, ds = dt_all[hit], np.abs(sd - ref["sdf"])[hit]
+    evals = ev.stats().last_sdf_evals
+    rc = abs(got[0] - ref["cost"]) / max(abs(ref["cost"]), 1e-300)
+    rg = rel_l2(grads(got[1], got[2]), grads(ref["gradC"], ref["gradT"]))
+    first = np.flatnonzero((dt_all > 1e-12) | ((sd < 9.99) != hit))
+    print(f"{name} {'tilted' if tilt else 'untilted'}: points {len(pts)} hits {hit.sum()} max|dt*| {dt.max() if dt.size else 0:.1e} "
+          f"max|dsdf| {ds.max() if ds.size else 0:.1e} cost rel {rc:.1e} grad rel-L2 {rg:.1e} evals {evals} vs {ref['nsdf']}"
+          + (f"; first differing point {first[0]}: t* {ts[first[0]]!r} vs {ref['tstar'][first[0]]!r}, sdf {sd[first[0]]!r} vs {ref['sdf'][first[0]]!r}"
+             if first.size else ""))
     assert np.array_equal(sd < 9.99, hit)
-    dt = np.abs(ts - ref["tstar"])[hit]
-    print(f"{name}: points {len(pts)} hits {hit.sum()} max|dt*| {dt.max() if dt.size else 0:.3e} cost {got[0]:.6g} vs {ref['cost']:.6g}")
-    assert (dt <= 8e-5).mean() >= 0.99, f"t* mismatch on {(dt > 8e-5).sum()} points"
-    assert np.allclose(sd[hit], ref["sdf"][hit], rtol=0, atol=1e-6)
-    check_eval(got, (ref["cost"], ref["gradC"], ref["gradT"]), tol=1e-6, what=f"T2 {name}")
-    assert ev.stats().last_sdf_evals == ref["nsdf"]
+    if name == "CappedCone":
+        assert hit.sum() == 0 and np.all(sd == 10.0) and got[0] == 0.0
+    else:
+        assert hit.sum() >= 5
+    assert dt_all.max() <= 1e-12 and (ds.max() if ds.size else 0) <= 1e-10
+    check_eval(got, (ref["cost"], ref["gradC"], ref["gradT"]), tol=1e-9, what=f"T2 {name}")
+    assert evals == ref["nsdf"]
     ev.close()
 
 
