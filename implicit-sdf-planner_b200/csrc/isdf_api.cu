@@ -6,6 +6,7 @@
 #include "isdf_swept.cuh"
 #include "isdf_minco.cuh"
 #include "isdf_frontend.cuh"
+#include "isdf_frontpath.cuh"
 #include "isdf_lbfgs.cuh"
 #include "isdf_clearance.cuh"
 #include "isdf_map.cuh"
@@ -99,6 +100,13 @@ struct isdf_ctx {
         int xk = 0, yk = 0, ks = 0;
         double max_roll = 0, max_pitch = 0, ang_res = 0, margin = 0;
     } fe;
+    struct {   // front-end path search (isdf_frontpath.cuh): rebuilt from the current map and kernels by every call, so nothing here outlives them
+        DevBuf<uint32_t> d_trav, d_front, d_colliding; DevBuf<unsigned long long> d_g; DevBuf<unsigned> d_flags;
+        DevBuf<int> d_tgt, d_len, d_off, d_nodes; DevBuf<double> d_xyz, d_rp, d_cost; DevBuf<uint8_t> d_found;
+        PinnedBuf<unsigned> h_flag;
+        cudaEvent_t ev[4] = {};
+        isdf_frontpath_info info = {};
+    } fp;
     struct {   // trajectory clearance check (isdf_clearance.cuh)
         DevBuf<double> d_in, d_clear; DevBuf<long long> d_vox; DevBuf<ClrSummary> d_sum; DevBuf<int> d_cursor;
         DevBuf<unsigned long long> d_counters;   // {candidate pairs, exact mesh searches} of the last check (isdf_dbg_clearance_counts)
@@ -117,6 +125,7 @@ struct isdf_ctx {
         peer.close_handles();
         peer.buf = {};
         for (cudaEvent_t e : {ev0, ev1, ev_main_done, ev_items_done}) if (e) cudaEventDestroy(e);
+        for (cudaEvent_t e : fp.ev) if (e) cudaEventDestroy(e);
         if (aux_stream) cudaStreamDestroy(aux_stream);
         if (stream) cudaStreamDestroy(stream);
     }
@@ -1605,13 +1614,11 @@ static int frontend_state(isdf_ctx *c) {
     return 0;
 }
 
-extern "C" int isdf_frontend_feasibility_device(isdf_ctx *c, uint32_t *d_masks, void *cuda_stream) {
-    int r = frontend_state(c);
-    if (r) return r;
-    if (!d_masks) return fail(ISDF_ERR_INVALID, "NULL device pointer");
-    if (set_device(c)) return ISDF_ERR_CUDA;
+// the feasibility pipeline into d_masks (4 words per voxel), or, with d_trav set, into the traversability bits (isdf_frontpath.cuh)
+static int frontend_feasibility_run(isdf_ctx *c, uint32_t *d_masks, uint32_t *d_trav, void *cuda_stream) {
     FrontArgs A = front_args(c);
-    A.out = d_masks;
+    A.out = d_masks; A.trav = d_trav;
+    if (d_trav) CU_TRY(cudaMemsetAsync(d_trav, 0, sizeof(uint32_t) * (size_t)c->map.grid.X * c->map.grid.Y * c->map.grid.Zw, (cudaStream_t)cuda_stream));
     const size_t smem = sizeof(uint32_t) * 4 * (size_t)A.ks * A.ks * A.ks;
     CU_TRY(cudaFuncSetAttribute(k_frontend_feasibility, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const long long nrun = (long long)c->map.grid.X * c->map.grid.Y * ((c->map.grid.Z + FE_ZRUN - 1) / FE_ZRUN);
@@ -1627,7 +1634,7 @@ extern "C" int isdf_frontend_feasibility_device(isdf_ctx *c, uint32_t *d_masks, 
         if (c->fe.nchunk > 0 && tsmem <= 200 * 1024 && !getenv("ISDF_FE_NO_TABLES")) {
             // throughput form: zero-filled output, bit-parallel core pass (32 voxels per thread), table-driven accumulation on the survivors
             const long long nvox = (long long)c->map.grid.X * c->map.grid.Y * c->map.grid.Z;
-            CU_TRY(cudaMemsetAsync(d_masks, 0, sizeof(uint32_t) * 4 * (size_t)nvox, (cudaStream_t)cuda_stream));
+            if (!d_trav) CU_TRY(cudaMemsetAsync(d_masks, 0, sizeof(uint32_t) * 4 * (size_t)nvox, (cudaStream_t)cuda_stream));
             const long long nword = (long long)c->map.grid.X * c->map.grid.Y * c->map.grid.Zw;
             CU_TRY(cudaFuncSetAttribute(k_frontend_survivors_tab, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tsmem));
             k_frontend_core_words<<<(unsigned)std::min<long long>((nword + 255) / 256, sms * 32), 256, 0, (cudaStream_t)cuda_stream>>>(A);
@@ -1647,6 +1654,14 @@ extern "C" int isdf_frontend_feasibility_device(isdf_ctx *c, uint32_t *d_masks, 
     }
     CU_TRY(cudaGetLastError());
     return 0;
+}
+
+extern "C" int isdf_frontend_feasibility_device(isdf_ctx *c, uint32_t *d_masks, void *cuda_stream) {
+    int r = frontend_state(c);
+    if (r) return r;
+    if (!d_masks) return fail(ISDF_ERR_INVALID, "NULL device pointer");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    return frontend_feasibility_run(c, d_masks, nullptr, cuda_stream);
 }
 
 extern "C" int isdf_frontend_feasibility(isdf_ctx *c, uint32_t *masks) {
@@ -1689,6 +1704,213 @@ extern "C" int isdf_frontend_check_batch(isdf_ctx *c, int n, const int32_t *ind,
     CU_TRY(cudaMemcpyAsync(child_roll_pitch, c->fe.d_child.p, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, c->stream));
     CU_TRY(cudaMemcpyAsync(ok, c->fe.d_ok.p, n, cudaMemcpyDeviceToHost, c->stream));
     CU_TRY(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+// ---- front-end path search (isdf_frontpath.cuh) ------------------------------------------------------------------------------------
+constexpr int FP_ROUNDS_PER_CHECK = 8;   // relaxation rounds launched between two reads of the frontier flag
+
+static int path_args_check(isdf_ctx *c, const isdf_frontpath_params *prm) {
+    if (int r = frontend_state(c)) return r;
+    if (c->world > 1) return fail(ISDF_ERR_UNSUPPORTED, "the front-end path search is not sharded: call it on a context with isdf_set_shard(ctx, 0, 1)");
+    if (prm) for (int32_t v : prm->reserved_) if (v != 0) return fail(ISDF_ERR_INVALID, "isdf_frontpath_params: reserved fields must be zero");
+    return 0;
+}
+
+// isInMap (Gridmap3D.cpp) + getGridIndex (Gridmap3D.cpp:135-175) with its clamps and its "iy < 0 => ix = 0" branches (they cannot fire
+// for a point inside the map)
+static int path_voxel(const DevGrid &G, const double *p, int id[3], const char *what) {
+    for (int a = 0; a < 3; a++)
+        if (!std::isfinite(p[a])) return fail(ISDF_ERR_INVALID, std::string(what) + " is not finite");
+    for (int a = 0; a < 3; a++)
+        if (p[a] < G.bmin[a] || p[a] > G.bmax[a]) return fail(ISDF_ERR_INVALID, std::string(what) + " is outside the map");
+    int ix = (int)std::floor((p[0] - G.bmin[0]) / G.res), iy = (int)std::floor((p[1] - G.bmin[1]) / G.res), iz = (int)std::floor((p[2] - G.bmin[2]) / G.res);
+    if (ix < 0) ix = 0;
+    if (ix >= G.X) ix = G.X - 1;
+    if (iy < 0) ix = 0;
+    if (iy >= G.Y) iy = G.Y - 1;
+    if (iz < 0) ix = 0;
+    if (iz >= G.Z) iz = G.Z - 1;
+    id[0] = ix; id[1] = iy; id[2] = iz;
+    return 0;
+}
+
+static PathArgs path_args(isdf_ctx *c, const int s[3], unsigned long long *d_g) {
+    const size_t nword = (size_t)c->map.grid.X * c->map.grid.Y * c->map.grid.Zw;
+    PathArgs P = {};
+    P.grid = c->map.grid; P.trav = c->fp.d_trav.p; P.g = d_g;
+    P.front0 = c->fp.d_front.p; P.front1 = c->fp.d_front.p + nword;
+    P.flags = c->fp.d_flags.p; P.rounds = c->fp.d_flags.p + FP_FLAG_RING;
+    P.sx = s[0]; P.sy = s[1]; P.sz = s[2];
+    return P;
+}
+
+// traversability grid, then the field from source s into d_g (X*Y*Z bit patterns), on stream st; fills c->fp.info
+static int path_field(isdf_ctx *c, const int s[3], unsigned long long *d_g, cudaStream_t st) {
+    const DevGrid &G = c->map.grid;
+    const size_t nword = (size_t)G.X * G.Y * G.Zw, nvox = (size_t)G.X * G.Y * G.Z;
+    for (cudaEvent_t &e : c->fp.ev) if (!e) CU_TRY(cudaEventCreate(&e));
+    CU_TRY(c->fp.d_trav.ensure(nword));
+    CU_TRY(c->fp.d_front.ensure(2 * nword));
+    CU_TRY(c->fp.d_flags.ensure(FP_FLAG_RING + 1));
+    CU_TRY(c->fp.h_flag.ensure(2));
+    CU_TRY(cudaEventRecord(c->fp.ev[0], st));
+    if (int r = frontend_feasibility_run(c, nullptr, c->fp.d_trav.p, st)) return r;
+    CU_TRY(cudaEventRecord(c->fp.ev[1], st));
+    const PathArgs P = path_args(c, s, d_g);
+    CU_TRY(cudaMemsetAsync(c->fp.d_front.p, 0, sizeof(uint32_t) * 2 * nword, st));
+    CU_TRY(cudaMemsetAsync(c->fp.d_flags.p, 0, sizeof(unsigned) * (FP_FLAG_RING + 1), st));
+    const long long sms = c->sm_count;
+    k_fp_init<<<(unsigned)std::min<long long>(((long long)nvox + 255) / 256, sms * 32), 256, 0, st>>>(P);
+    c->stats.kernel_launches++;
+    const unsigned blocks = (unsigned)std::min<long long>(((long long)nword + 255) / 256, sms * 16);
+    for (int r = 0;;) {
+        for (int k = 0; k < FP_ROUNDS_PER_CHECK; k++, r++) k_fp_relax<<<blocks, 256, 0, st>>>(P, r);
+        c->stats.kernel_launches += FP_ROUNDS_PER_CHECK;
+        CU_TRY(cudaGetLastError());
+        CU_TRY(cudaMemcpyAsync(c->fp.h_flag.p, P.flags + r % FP_FLAG_RING, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
+        if (!c->fp.h_flag.p[0]) break;
+    }
+    CU_TRY(cudaEventRecord(c->fp.ev[2], st));
+    CU_TRY(cudaMemcpyAsync(c->fp.h_flag.p + 1, P.rounds, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    isdf_frontpath_info &I = c->fp.info;
+    I = {};
+    I.rounds = (int32_t)c->fp.h_flag.p[1];
+    I.field_bytes = (int64_t)(nvox * sizeof(double));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, c->fp.ev[0], c->fp.ev[1]); I.traversability_ms = ms;
+    cudaEventElapsedTime(&ms, c->fp.ev[1], c->fp.ev[2]); I.field_ms = ms;
+    return 0;
+}
+
+// field from start, then the B paths into c->fp.d_xyz / d_rp / d_cost / d_found; off (B + 1) is filled as soon as the lengths are known,
+// also when they exceed cap
+static int path_run(isdf_ctx *c, const double *start, int B, const double *goals, int cap, std::vector<int> &off, cudaStream_t st) {
+    const DevGrid &G = c->map.grid;
+    int s[3];
+    if (int r = path_voxel(G, start, s, "start")) return r;
+    std::vector<int> tgt((size_t)3 * B);
+    for (int b = 0; b < B; b++)
+        if (int r = path_voxel(G, goals + 3 * (size_t)b, &tgt[3 * (size_t)b], "a goal")) return r;
+    CU_TRY(c->fp.d_g.ensure((size_t)G.X * G.Y * G.Z));
+    if (int r = path_field(c, s, c->fp.d_g.p, st)) return r;
+    PathArgs P = path_args(c, s, c->fp.d_g.p);
+    CU_TRY(c->fp.d_tgt.upload(tgt.data(), tgt.size(), st));
+    CU_TRY(c->fp.d_len.ensure(B)); CU_TRY(c->fp.d_off.ensure((size_t)B + 1));
+    CU_TRY(c->fp.d_cost.ensure(B)); CU_TRY(c->fp.d_found.ensure(B));
+    P.nt = B; P.tgt = c->fp.d_tgt.p; P.len = c->fp.d_len.p; P.off = c->fp.d_off.p; P.cost = c->fp.d_cost.p; P.found = c->fp.d_found.p;
+    const unsigned wblocks = (unsigned)(((long long)B * 32 + 127) / 128);
+    k_fp_walk<<<wblocks, 128, 0, st>>>(P, 0);
+    c->stats.kernel_launches++;
+    CU_TRY(cudaGetLastError());
+    std::vector<int> len(B);
+    CU_TRY(cudaMemcpyAsync(len.data(), c->fp.d_len.p, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    off.assign((size_t)B + 1, 0);
+    long long total = 0;
+    for (int b = 0; b < B; b++) {
+        total += len[b];
+        if (total > INT32_MAX) return fail(ISDF_ERR_INVALID, "the paths hold more than 2^31 - 1 nodes");
+        off[b + 1] = (int)total;
+    }
+    if (total > cap) return fail(ISDF_ERR_INVALID, "cap is smaller than the total path length (reported in n / offsets[B])");
+    CU_TRY(c->fp.d_off.upload(off.data(), off.size(), st));
+    CU_TRY(c->fp.d_nodes.ensure((size_t)3 * total)); CU_TRY(c->fp.d_colliding.ensure((size_t)4 * total));
+    CU_TRY(c->fp.d_xyz.ensure((size_t)3 * total)); CU_TRY(c->fp.d_rp.ensure((size_t)2 * total));
+    P.nodes = c->fp.d_nodes.p; P.xyz = c->fp.d_xyz.p; P.rp = c->fp.d_rp.p; P.colliding = c->fp.d_colliding.p;
+    k_fp_walk<<<wblocks, 128, 0, st>>>(P, 1);
+    FrontArgs A = front_args(c);
+    A.nq = (int)total; A.q_ind = c->fp.d_nodes.p; A.out = c->fp.d_colliding.p;
+    const size_t smem = sizeof(uint32_t) * 4 * (size_t)A.ks * A.ks * A.ks;
+    CU_TRY(cudaFuncSetAttribute(k_fp_node_masks, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_fp_node_masks<<<(unsigned)((total + 255) / 256), 256, smem, st>>>(A);
+    k_fp_attitudes<<<(unsigned)((B + 127) / 128), 128, 0, st>>>(A, P);
+    c->stats.kernel_launches += 3;
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaEventRecord(c->fp.ev[3], st));
+    CU_TRY(cudaStreamSynchronize(st));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, c->fp.ev[2], c->fp.ev[3]); c->fp.info.paths_ms = ms;
+    return 0;
+}
+
+extern "C" int isdf_frontend_path_batch(isdf_ctx *c, const double *start, int B, const double *goals, const isdf_frontpath_params *prm, int cap,
+                                        double *path_xyz, double *path_rp, int32_t *offsets, double *costs, uint8_t *found) {
+    if (!start || !goals || B < 1 || cap < 0 || (cap > 0 && !path_xyz) || !offsets || !costs || !found) return fail(ISDF_ERR_INVALID, "bad argument");
+    if (int r = path_args_check(c, prm)) return r;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    std::vector<int> off;
+    const int r = path_run(c, start, B, goals, cap, off, c->stream);
+    if (!off.empty()) std::memcpy(offsets, off.data(), sizeof(int32_t) * off.size());
+    if (r) return r;
+    const size_t total = (size_t)off[B];
+    CU_TRY(cudaMemcpyAsync(path_xyz, c->fp.d_xyz.p, sizeof(double) * 3 * total, cudaMemcpyDeviceToHost, c->stream));
+    if (path_rp) CU_TRY(cudaMemcpyAsync(path_rp, c->fp.d_rp.p, sizeof(double) * 2 * total, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(cudaMemcpyAsync(costs, c->fp.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(cudaMemcpyAsync(found, c->fp.d_found.p, B, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+extern "C" int isdf_frontend_path(isdf_ctx *c, const double *start, const double *goal, const isdf_frontpath_params *prm, int cap,
+                                  double *path_xyz, double *path_rp, int32_t *n, double *cost, uint8_t *found) {
+    if (!n) return fail(ISDF_ERR_INVALID, "n is NULL");
+    int32_t off[2] = {0, 0};
+    const int r = isdf_frontend_path_batch(c, start, 1, goal, prm, cap, path_xyz, path_rp, off, cost, found);
+    *n = off[1];
+    return r;
+}
+
+extern "C" int isdf_frontend_path_batch_device(isdf_ctx *c, const double *start, int B, const double *d_goals, const isdf_frontpath_params *prm,
+                                               int cap, double *d_path_xyz, double *d_path_rp, int32_t *d_offsets, double *d_costs,
+                                               uint8_t *d_found, void *cuda_stream) {
+    if (!start || !d_goals || B < 1 || cap < 0 || (cap > 0 && !d_path_xyz) || !d_offsets || !d_costs || !d_found) return fail(ISDF_ERR_INVALID, "bad argument");
+    if (int r = path_args_check(c, prm)) return r;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    const cudaStream_t st = (cudaStream_t)cuda_stream;
+    std::vector<double> goals((size_t)3 * B);
+    CU_TRY(cudaMemcpyAsync(goals.data(), d_goals, sizeof(double) * goals.size(), cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    std::vector<int> off;
+    const int r = path_run(c, start, B, goals.data(), cap, off, st);
+    if (!off.empty()) {
+        CU_TRY(cudaMemcpyAsync(d_offsets, off.data(), sizeof(int32_t) * off.size(), cudaMemcpyHostToDevice, st));
+        CU_TRY(cudaStreamSynchronize(st));   // off is a host temporary
+    }
+    if (r) return r;
+    const size_t total = (size_t)off[B];
+    CU_TRY(cudaMemcpyAsync(d_path_xyz, c->fp.d_xyz.p, sizeof(double) * 3 * total, cudaMemcpyDeviceToDevice, st));
+    if (d_path_rp) CU_TRY(cudaMemcpyAsync(d_path_rp, c->fp.d_rp.p, sizeof(double) * 2 * total, cudaMemcpyDeviceToDevice, st));
+    CU_TRY(cudaMemcpyAsync(d_costs, c->fp.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToDevice, st));
+    CU_TRY(cudaMemcpyAsync(d_found, c->fp.d_found.p, B, cudaMemcpyDeviceToDevice, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    return 0;
+}
+
+extern "C" int isdf_frontend_path_field_device(isdf_ctx *c, const double *start, const isdf_frontpath_params *prm, double *d_g, void *cuda_stream) {
+    if (!start || !d_g) return fail(ISDF_ERR_INVALID, "bad argument");
+    if (int r = path_args_check(c, prm)) return r;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    int s[3];
+    if (int r = path_voxel(c->map.grid, start, s, "start")) return r;
+    return path_field(c, s, reinterpret_cast<unsigned long long *>(d_g), (cudaStream_t)cuda_stream);
+}
+
+extern "C" int isdf_frontend_path_info(isdf_ctx *c, isdf_frontpath_info *out) {
+    if (!c || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
+    *out = c->fp.info;
+    return 0;
+}
+
+// the traversability bits of the last path or field call (X*Y*ceil(Z/32) words of the map it ran on, grid.bits' layout)
+extern "C" int isdf_dbg_frontpath_traversable(isdf_ctx *c, uint32_t *out, long long n) {
+    if (!c || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (!c->map.have_map || n != (long long)c->map.grid.X * c->map.grid.Y * c->map.grid.Zw || (size_t)n > c->fp.d_trav.n)
+        return fail(ISDF_ERR_STATE, "no traversability grid of the current map's size");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    CU_TRY(cudaMemcpy(out, c->fp.d_trav.p, sizeof(uint32_t) * (size_t)n, cudaMemcpyDeviceToHost));
     return 0;
 }
 

@@ -34,6 +34,8 @@ struct FrontArgs {
     uint8_t *kernels;        // natt x ks^3 booleans, address a*ks*ks + b*ks + c
     uint32_t *offset_masks;  // ks^3 x 4
     uint32_t *out;           // X*Y*Z x 4 (feasibility) — or n x 4 for the batched check
+    uint32_t *trav;          // non-null: traversability output instead of masks (isdf_frontpath.cuh), one bit per voxel in the layout of
+                             // grid.bits, zero-filled beforehand: bit set = some attitude fits and the voxel itself is free
     // two-pass feasibility: rows of the kernel CORE (offsets occupied in EVERY attitude's kernel), the survivor list and its counter
     const uint2 *core_rows;  // ncore x {a | b << 8, bits over c}
     int ncore;
@@ -128,6 +130,16 @@ __device__ __forceinline__ void frontend_stage_masks(const FrontArgs &A, uint32_
     __syncthreads();
 }
 
+// traversability output: fit bit j = some attitude fits at voxel iz0 + j of a z-run (runs never straddle a 32-voxel word); the run's
+// free voxels among them are ORed into A.trav
+__device__ __forceinline__ void frontend_mark_run(const FrontArgs &A, int ix, int iy, int iz0, unsigned fit) {
+    if (!fit) return;
+    const size_t w = ((size_t)ix * A.grid.Y + iy) * A.grid.Zw + (iz0 >> 5);
+    const unsigned bits = (fit << (iz0 & 31)) & ~__ldg(A.grid.bits + w);
+    if (bits) atomicOr(A.trav + w, bits);
+}
+__device__ __forceinline__ bool any4(uint4 v) { return (v.x | v.y | v.z | v.w) != 0u; }
+
 // One thread per run of FE_ZRUN voxels along z: the run's window rows are read once (ks + FE_ZRUN - 1 bits), every occupied map
 // voxel found in a row is applied to each of the run's voxels it overlaps (offset c = bit - j), one 128-bit shared-memory load
 // and four ORs per (occupied voxel, run voxel) pair.
@@ -182,6 +194,14 @@ __global__ void __launch_bounds__(256) k_frontend_feasibility(const __grid_const
                 }
             }
         }
+        if (A.trav) {
+            unsigned fit = 0u;
+#pragma unroll
+            for (int j = 0; j < FE_ZRUN; j++)
+                if (iz0 + j < G.Z && any4(make_uint4(~m[j].x & valid.x, ~m[j].y & valid.y, ~m[j].z & valid.z, ~m[j].w & valid.w))) fit |= 1u << j;
+            frontend_mark_run(A, ix, iy, iz0, fit);
+            continue;
+        }
         uint4 *o = reinterpret_cast<uint4 *>(A.out) + ((size_t)ix * G.Y + iy) * G.Z + iz0;
 #pragma unroll
         for (int j = 0; j < FE_ZRUN; j++)
@@ -230,9 +250,11 @@ __global__ void __launch_bounds__(256) k_frontend_core(const __grid_constant__ F
             }
             const unsigned exist = (iz0 + FE_ZRUN <= G.Z) ? ((1u << FE_ZRUN) - 1u) : ((1u << (G.Z - iz0)) - 1u);
             uint4 *o = reinterpret_cast<uint4 *>(A.out) + ((size_t)ix * G.Y + iy) * G.Z + iz0;
+            if (!A.trav) {                                                // a settled voxel is not traversable: nothing to mark
 #pragma unroll
-            for (int j = 0; j < FE_ZRUN; j++)
-                if (((exist & ~alive) >> j) & 1u) o[j] = make_uint4(0u, 0u, 0u, 0u);
+                for (int j = 0; j < FE_ZRUN; j++)
+                    if (((exist & ~alive) >> j) & 1u) o[j] = make_uint4(0u, 0u, 0u, 0u);
+            }
         }
         // warp-wide append of the runs that still have an open voxel
         const unsigned open = __ballot_sync(0xffffffffu, alive != 0u);
@@ -292,6 +314,14 @@ __global__ void __launch_bounds__(256) k_frontend_survivors(const __grid_constan
                     if (c >= 0 && c < ks && ((alive >> j) & 1u)) { const uint4 t = mrow[c]; m[j].x |= t.x; m[j].y |= t.y; m[j].z |= t.z; m[j].w |= t.w; }
                 }
             }
+        }
+        if (A.trav) {
+            unsigned fit = 0u;
+#pragma unroll
+            for (int j = 0; j < FE_ZRUN; j++)
+                if (((alive >> j) & 1u) && any4(make_uint4(~m[j].x & valid.x, ~m[j].y & valid.y, ~m[j].z & valid.z, ~m[j].w & valid.w))) fit |= 1u << j;
+            frontend_mark_run(A, ix, iy, iz0, fit);
+            continue;
         }
         uint4 *o = reinterpret_cast<uint4 *>(A.out) + ((size_t)ix * G.Y + iy) * G.Z + iz0;
 #pragma unroll
@@ -431,6 +461,14 @@ __global__ void __launch_bounds__(1024) k_frontend_survivors_tab(const __grid_co
                 m[j].x |= v.x; m[j].y |= v.y; m[j].z |= v.z; m[j].w |= v.w;
             }
         }
+        if (A.trav) {
+            unsigned fit = 0u;
+#pragma unroll
+            for (int j = 0; j < FE_ZRUN; j++)
+                if (((alive >> j) & 1u) && any4(make_uint4(~m[j].x & valid.x, ~m[j].y & valid.y, ~m[j].z & valid.z, ~m[j].w & valid.w))) fit |= 1u << j;
+            frontend_mark_run(A, ix, iy, iz0, fit);
+            continue;
+        }
         uint4 *o = reinterpret_cast<uint4 *>(A.out) + ((size_t)ix * G.Y + iy) * G.Z + iz0;
 #pragma unroll
         for (int j = 0; j < FE_ZRUN; j++)
@@ -438,16 +476,9 @@ __global__ void __launch_bounds__(1024) k_frontend_survivors_tab(const __grid_co
     }
 }
 
-__global__ void __launch_bounds__(256) k_frontend_check(const __grid_constant__ FrontArgs A) {
-    extern __shared__ __align__(16) uint32_t fe_sm[];
-    frontend_stage_masks(A, fe_sm);
-    const int q = blockIdx.x * blockDim.x + threadIdx.x;
-    if (q >= A.nq) return;
-    const int ix = A.q_ind[3 * q], iy = A.q_ind[3 * q + 1], iz = A.q_ind[3 * q + 2];
-    const double fr = A.q_father[2 * q], fp = A.q_father[2 * q + 1];
-    uint32_t m[4];
-    frontend_colliding(A, fe_sm, ix, iy, iz, m);
-    for (int k = 0; k < 4; k++) A.out[4 * (size_t)q + k] = ~m[k];
+// checkKernelValue's choice given the colliding set m of the child voxel: the first attitude in visit_kernels_by_distance's order that
+// fits; returns 0 (child = father) when none does
+__device__ __forceinline__ uint8_t frontend_visit(const FrontArgs &A, const uint32_t m[4], double fr, double fp, double &cr_out, double &cp_out) {
     const int fi = (int)((fr + A.max_roll) / A.ang_res), fj = (int)((fp + A.max_pitch) / A.ang_res);   // checkKernelValue (swm:917-918)
     double cr = fr, cp = fp;
     uint8_t ok = 0;
@@ -464,6 +495,22 @@ __global__ void __launch_bounds__(256) k_frontend_check(const __grid_constant__ 
             }
         }
     }
+    cr_out = cr; cp_out = cp;
+    return ok;
+}
+
+__global__ void __launch_bounds__(256) k_frontend_check(const __grid_constant__ FrontArgs A) {
+    extern __shared__ __align__(16) uint32_t fe_sm[];
+    frontend_stage_masks(A, fe_sm);
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= A.nq) return;
+    const int ix = A.q_ind[3 * q], iy = A.q_ind[3 * q + 1], iz = A.q_ind[3 * q + 2];
+    const double fr = A.q_father[2 * q], fp = A.q_father[2 * q + 1];
+    uint32_t m[4];
+    frontend_colliding(A, fe_sm, ix, iy, iz, m);
+    for (int k = 0; k < 4; k++) A.out[4 * (size_t)q + k] = ~m[k];
+    double cr, cp;
+    const uint8_t ok = frontend_visit(A, m, fr, fp, cr, cp);
     A.q_child[2 * q] = cr; A.q_child[2 * q + 1] = cp; A.q_ok[q] = ok;
 }
 

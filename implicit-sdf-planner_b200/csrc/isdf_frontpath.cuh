@@ -1,0 +1,188 @@
+// Front-end path search: the exact shortest 26-connected path over the attitude-feasible voxels, as a cost-to-come FIELD.
+//
+// Reference: AstarPathSearcher::AstarPathSearch / getPath / getastarSE3Path (front_end_Astar.hpp:197-402), a serial A* that calls
+// checkKernelValue once per neighbour of every expanded node. A voxel can be entered iff it is in the map, not occupied and SOME attitude
+// fits there (visit_kernels_by_distance tries every attitude), i.e. iff its feasibility mask is not zero: a property of the voxel alone.
+// So the search is a shortest-path problem on a fixed graph, and its cost-to-come field is data-parallel.
+//
+// GPU mapping:
+//   traversability  the feasibility kernels of isdf_frontend.cuh in their traversability output mode: one bit per voxel, grid.bits' layout
+//   k_fp_init       g = +inf everywhere, g(source) = 0, the source in frontier 0
+//   k_fp_relax      one round of label-correcting relaxation: a thread per 32-voxel word of the current frontier; every frontier voxel u
+//                   offers g(u) + w to its 26 neighbours with atomicMin on the bit pattern of the non-negative double (order-preserving,
+//                   so the result does not depend on the order); improved voxels form the next frontier. Rounds are launched in chunks;
+//                   a round whose frontier is empty returns at once, and the host reads one flag per chunk.
+//   k_fp_walk       one warp per target: lane l tests offset l of the parent rule, the first lane of the ballot is the parent.
+//                   Pass 0 counts the path, pass 1 writes it (voxel indices and cube centres) at the target's offset.
+//   k_fp_node_masks the colliding-attitude set of every path node (frontend_colliding: the mask OR of isdf_frontend_check_batch)
+//   k_fp_attitudes  one thread per target: the attitude chain along its path, frontend_visit from the father's attitude
+#pragma once
+#include "isdf_frontend.cuh"
+
+namespace isdf {
+
+constexpr unsigned long long FP_INF = 0x7ff0000000000000ull;   // +inf as a bit pattern: above every finite non-negative double
+constexpr int FP_FLAG_RING = 4;                                  // flags[r % ring] != 0: round r has a frontier
+
+struct PathArgs {
+    DevGrid grid;
+    const uint32_t *trav;        // traversability bits, grid.bits' layout
+    unsigned long long *g;       // X*Y*Z FP64 bit patterns, address ix*Y*Z + iy*Z + iz
+    uint32_t *front0, *front1;   // frontier bit sets of even / odd rounds, grid.bits' layout
+    unsigned *flags;             // FP_FLAG_RING words
+    unsigned *rounds;            // rounds that had a frontier
+    int sx, sy, sz;              // the source voxel
+    // targets and paths
+    int nt;
+    const int *tgt;              // nt x 3
+    int *len;                    // nt: path length in nodes (pass 0)
+    const int *off;              // nt + 1: first node of each path (pass 1)
+    int *nodes;                  // 3 per node
+    double *xyz;                 // 3 per node: cube centres
+    double *rp;                  // 2 per node: roll, pitch
+    double *cost;                // nt
+    uint8_t *found;              // nt
+    const uint32_t *colliding;   // 4 per node (k_fp_node_masks)
+};
+
+__device__ __forceinline__ bool fp_trav(const PathArgs &P, int x, int y, int z) {
+    return (__ldg(P.trav + ((size_t)x * P.grid.Y + y) * P.grid.Zw + (z >> 5)) >> (z & 31)) & 1u;
+}
+// edge cost sqrt(i*i + j*j + k*k) of front_end_Astar.hpp:230 (IEEE sqrt: correctly rounded)
+__device__ __forceinline__ double fp_edge(int n) { return sqrt((double)n); }
+
+__global__ void k_fp_init(const __grid_constant__ PathArgs P) {
+    const long long nvox = (long long)P.grid.X * P.grid.Y * P.grid.Z;
+    const long long s = ((long long)P.sx * P.grid.Y + P.sy) * P.grid.Z + P.sz;
+    for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < nvox; v += (long long)gridDim.x * blockDim.x) {
+        P.g[v] = (v == s) ? 0ull : FP_INF;
+        if (v == s) {
+            P.front0[((size_t)P.sx * P.grid.Y + P.sy) * P.grid.Zw + (P.sz >> 5)] = 1u << (P.sz & 31);
+            P.flags[0] = 1u;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256) k_fp_relax(const __grid_constant__ PathArgs P, int r) {
+    // the flag of round r + 2 is cleared before anyone can set it (round r + 1 sets it); round r sets the flag of round r + 1
+    if (blockIdx.x == 0 && threadIdx.x == 0) P.flags[(r + 2) % FP_FLAG_RING] = 0u;
+    if (*(volatile unsigned *)(P.flags + r % FP_FLAG_RING) == 0u) return;
+    if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(P.rounds, 1u);
+    const DevGrid &G = P.grid;
+    uint32_t *cur = (r & 1) ? P.front1 : P.front0, *nxt = (r & 1) ? P.front0 : P.front1;
+    const long long nword = (long long)G.X * G.Y * G.Zw;
+    bool improved = false;
+    for (long long wi = (long long)blockIdx.x * blockDim.x + threadIdx.x; wi < nword; wi += (long long)gridDim.x * blockDim.x) {
+        uint32_t bits = cur[wi];
+        if (!bits) continue;
+        cur[wi] = 0u;   // this set becomes round r + 2's next frontier
+        const int zw = (int)(wi % G.Zw), iy = (int)((wi / G.Zw) % G.Y), ix = (int)(wi / ((long long)G.Zw * G.Y));
+        while (bits) {
+            const int iz = 32 * zw + __ffs((int)bits) - 1;
+            bits &= bits - 1;
+            // a value read while another thread lowers it is still the cost of a path; the lowering thread re-queues u
+            const double gu = __longlong_as_double((long long)__ldcg(P.g + ((size_t)ix * G.Y + iy) * G.Z + iz));
+            for (int di = -1; di <= 1; di++) {
+                const int x = ix + di;
+                if (x < 0 || x >= G.X) continue;
+                for (int dj = -1; dj <= 1; dj++) {
+                    const int y = iy + dj;
+                    if (y < 0 || y >= G.Y) continue;
+                    for (int dk = -1; dk <= 1; dk++) {
+                        const int z = iz + dk;
+                        if (z < 0 || z >= G.Z || (di == 0 && dj == 0 && dk == 0) || !fp_trav(P, x, y, z)) continue;
+                        const unsigned long long cand = (unsigned long long)__double_as_longlong(gu + fp_edge(di * di + dj * dj + dk * dk));
+                        unsigned long long *gv = P.g + ((size_t)x * G.Y + y) * G.Z + z;
+                        if (cand >= __ldcg(gv)) continue;
+                        if (cand < atomicMin(gv, cand)) {
+                            atomicOr(nxt + ((size_t)x * G.Y + y) * G.Zw + (z >> 5), 1u << (z & 31));
+                            improved = true;
+                        }
+                    }
+                }
+            }
+        }
+    }
+    if (__any_sync(0xffffffffu, improved) && (threadIdx.x & 31) == 0) P.flags[(r + 1) % FP_FLAG_RING] = 1u;
+}
+
+// parent rule: among the 26 neighbours u of v with g(u) + w(u, v) == g(v), the first in the reference's offset order (i, j, k = -1..1,
+// i outermost; lane = 9 (i + 1) + 3 (j + 1) + (k + 1)). The whole warp calls this.
+__device__ __forceinline__ bool fp_parent(const PathArgs &P, int &x, int &y, int &z, int lane) {
+    const DevGrid &G = P.grid;
+    const double gv = __longlong_as_double((long long)P.g[((size_t)x * G.Y + y) * G.Z + z]);
+    const int di = lane / 9 - 1, dj = (lane / 3) % 3 - 1, dk = lane % 3 - 1;
+    const int ux = x + di, uy = y + dj, uz = z + dk;
+    bool ok = false;
+    if (lane < 27 && lane != 13 && ux >= 0 && ux < G.X && uy >= 0 && uy < G.Y && uz >= 0 && uz < G.Z) {
+        const unsigned long long gu = P.g[((size_t)ux * G.Y + uy) * G.Z + uz];
+        ok = gu != FP_INF && __longlong_as_double((long long)gu) + fp_edge(di * di + dj * dj + dk * dk) == gv;
+    }
+    const unsigned b = __ballot_sync(0xffffffffu, ok);
+    if (!b) return false;
+    const int l = __ffs((int)b) - 1;
+    x += l / 9 - 1; y += (l / 3) % 3 - 1; z += l % 3 - 1;
+    return true;
+}
+
+__global__ void __launch_bounds__(128) k_fp_walk(const __grid_constant__ PathArgs P, int pass) {
+    const int t = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+    if (t >= P.nt) return;   // whole warps
+    const DevGrid &G = P.grid;
+    int x = P.tgt[3 * t], y = P.tgt[3 * t + 1], z = P.tgt[3 * t + 2];
+    const unsigned long long gt = P.g[((size_t)x * G.Y + y) * G.Z + z];
+    const bool found = gt != FP_INF;
+    auto put = [&](int k, int px, int py, int pz) {
+        if (lane != 0) return;
+        int *n = P.nodes + 3 * (size_t)k;
+        n[0] = px; n[1] = py; n[2] = pz;
+        double *c = P.xyz + 3 * (size_t)k;   // getGridCubeCenter (Gridmap3D.cpp:177-194)
+        c[0] = (px + 0.5) * G.res + G.bmin[0]; c[1] = (py + 0.5) * G.res + G.bmin[1]; c[2] = (pz + 0.5) * G.res + G.bmin[2];
+    };
+    if (!found) {   // no path: the start alone
+        if (pass == 0) { if (lane == 0) { P.len[t] = 1; P.found[t] = 0; P.cost[t] = __longlong_as_double((long long)FP_INF); } }
+        else put(P.off[t], P.sx, P.sy, P.sz);
+        return;
+    }
+    // g strictly decreases along parents (every edge costs >= 1), so the walk ends at the source within X*Y*Z steps
+    const long long cap = (long long)G.X * G.Y * G.Z;
+    long long n = 1;
+    const int last = (pass == 1) ? P.off[t + 1] - 1 : 0;
+    if (pass == 1) put(last, x, y, z);
+    while (!(x == P.sx && y == P.sy && z == P.sz) && n < cap) {
+        if (!fp_parent(P, x, y, z, lane)) break;
+        if (pass == 1) put(last - (int)n, x, y, z);
+        n++;
+    }
+    if (pass == 0 && lane == 0) { P.len[t] = (int)n; P.found[t] = 1; P.cost[t] = __longlong_as_double((long long)gt); }
+}
+
+// the colliding-attitude set of each of n path nodes (A.q_ind = the nodes, A.out = 4 words per node)
+__global__ void __launch_bounds__(256) k_fp_node_masks(const __grid_constant__ FrontArgs A) {
+    extern __shared__ __align__(16) uint32_t fe_sm[];
+    frontend_stage_masks(A, fe_sm);
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= A.nq) return;
+    uint32_t m[4];
+    frontend_colliding(A, fe_sm, A.q_ind[3 * q], A.q_ind[3 * q + 1], A.q_ind[3 * q + 2], m);
+    for (int k = 0; k < 4; k++) A.out[4 * (size_t)q + k] = m[k];
+}
+
+// node 0 level, node m + 1 = checkKernelValue(attitude of node m, node m + 1): isdf_frontend_check_batch applied as a chain
+__global__ void k_fp_attitudes(const __grid_constant__ FrontArgs A, const __grid_constant__ PathArgs P) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= P.nt) return;
+    const int a = P.off[t], b = P.off[t + 1];
+    double fr = 0.0, fp = 0.0;
+    P.rp[2 * (size_t)a] = 0.0; P.rp[2 * (size_t)a + 1] = 0.0;
+    for (int k = a + 1; k < b; k++) {
+        const uint32_t *c = P.colliding + 4 * (size_t)k;
+        const uint32_t m[4] = {c[0], c[1], c[2], c[3]};
+        double cr, cp;
+        frontend_visit(A, m, fr, fp, cr, cp);
+        P.rp[2 * (size_t)k] = cr; P.rp[2 * (size_t)k + 1] = cp;
+        fr = cr; fp = cp;
+    }
+}
+
+}  // namespace isdf

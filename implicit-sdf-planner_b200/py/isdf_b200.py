@@ -33,7 +33,9 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_frontend_build_kernels", "isdf_frontend_get_kernels", "isdf_frontend_feasibility", "isdf_frontend_feasibility_device",
                "isdf_frontend_check_batch", "isdf_peer_export", "isdf_peer_connect", "isdf_peer_allreduce_device", "isdf_peer_status", "isdf_peer_disconnect",
                "isdf_clearance_default_params", "isdf_trajectory_clearance", "isdf_trajectory_clearance_device",
-               "isdf_set_map_cloud", "isdf_set_map_cloud_device", "isdf_get_map_info", "isdf_get_map_u8", "isdf_get_map_f64"]
+               "isdf_set_map_cloud", "isdf_set_map_cloud_device", "isdf_get_map_info", "isdf_get_map_u8", "isdf_get_map_f64",
+               "isdf_frontend_path", "isdf_frontend_path_batch", "isdf_frontend_path_batch_device", "isdf_frontend_path_field_device",
+               "isdf_frontend_path_info"]
 
 
 class KernelConfig(C.Structure):
@@ -83,6 +85,20 @@ class MapInfo(C.Structure):
     def as_dict(self):
         return dict(dims=(self.X, self.Y, self.Z), res=self.res, bmin=np.array(self.bmin[:]), bmax=np.array(self.bmax[:]),
                     occupied_voxels=self.occupied_voxels, points_used=self.points_used, points_skipped=self.points_skipped)
+
+
+class FrontPathParams(C.Structure):
+    """isdf_frontpath_params"""
+    _fields_ = [("reserved_", C.c_int32 * 4)]
+
+
+class FrontPathInfo(C.Structure):
+    """isdf_frontpath_info"""
+    _fields_ = [("rounds", C.c_int32), ("reserved_", C.c_int32), ("field_bytes", C.c_int64), ("traversability_ms", C.c_double),
+                ("field_ms", C.c_double), ("paths_ms", C.c_double)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved_"}
 
 
 class Stats(C.Structure):
@@ -161,6 +177,12 @@ def load_library(path=None):
     lib.isdf_get_map_info.argtypes = [vp, C.POINTER(MapInfo)]
     lib.isdf_get_map_u8.argtypes = [vp, C.POINTER(C.c_uint8), C.c_int64]
     lib.isdf_get_map_f64.argtypes = [vp, dp, C.c_int64]
+    fpp, u8p = C.POINTER(FrontPathParams), C.POINTER(C.c_uint8)
+    lib.isdf_frontend_path.argtypes = [vp, dp, dp, fpp, C.c_int, dp, dp, ip, dp, u8p]
+    lib.isdf_frontend_path_batch.argtypes = [vp, dp, C.c_int, dp, fpp, C.c_int, dp, dp, ip, dp, u8p]
+    lib.isdf_frontend_path_batch_device.argtypes = [vp, dp, C.c_int, vp, fpp, C.c_int, vp, vp, vp, vp, vp, vp]
+    lib.isdf_frontend_path_field_device.argtypes = [vp, dp, fpp, vp, vp]
+    lib.isdf_frontend_path_info.argtypes = [vp, C.POINTER(FrontPathInfo)]
     for s in ABI_SYMBOLS:
         if s != "isdf_last_error":
             getattr(lib, s).restype = C.c_int
@@ -475,6 +497,80 @@ class Evaluator:
         self._check(self.lib.isdf_frontend_check_batch(self.h, n, ind.ctypes.data_as(C.POINTER(C.c_int32)), _dp(father.reshape(-1)), _dp(child.reshape(-1)),
                                                        ok.ctypes.data_as(C.POINTER(C.c_uint8))))
         return child, ok.astype(bool)
+
+    # ---- front-end path search (see include/isdf.h) ----
+    def _path_cap(self, cap):
+        if cap is not None:
+            return int(cap)
+        info = self.map_info()
+        return 4 * sum(info["dims"])
+
+    def frontend_path_batch(self, start, goals, cap=None):
+        """one start, B goals -> dict(paths: list of (n_b, 3) cube centres, roll_pitch: list of (n_b, 2) degrees, offsets (B + 1),
+        costs (B), found (B) bool). cap = None: a first guess, repeated once with the exact total when the paths are longer."""
+        st = _f64(start).reshape(3)
+        goals = _f64(goals).reshape(-1, 3)
+        B = goals.shape[0]
+        cap = self._path_cap(cap)
+        for attempt in range(2):
+            xyz, rp = np.zeros((max(cap, 1), 3)), np.zeros((max(cap, 1), 2))
+            off, cost, found = np.zeros(B + 1, dtype=np.int32), np.zeros(B), np.zeros(B, dtype=np.uint8)
+            r = self.lib.isdf_frontend_path_batch(self.h, _dp(st), B, _dp(goals), None, cap, _dp(xyz), _dp(rp),
+                                                  off.ctypes.data_as(C.POINTER(C.c_int32)), _dp(cost), found.ctypes.data_as(C.POINTER(C.c_uint8)))
+            if r == -1 and attempt == 0 and off[B] > cap:
+                cap = int(off[B])
+                continue
+            self._check(r)
+            break
+        n = int(off[B])
+        return dict(paths=[xyz[off[b]:off[b + 1]] for b in range(B)], roll_pitch=[rp[off[b]:off[b + 1]] for b in range(B)],
+                    xyz=xyz[:n], rp=rp[:n], offsets=off, costs=cost, found=found.astype(bool))
+
+    def frontend_path(self, start, goal, cap=None):
+        """-> (path (n, 3), roll_pitch (n, 2), cost, found), through isdf_frontend_path"""
+        st, gl = _f64(start).reshape(3), _f64(goal).reshape(3)
+        cap = self._path_cap(cap)
+        for attempt in range(2):
+            xyz, rp = np.zeros((max(cap, 1), 3)), np.zeros((max(cap, 1), 2))
+            n, cost, found = C.c_int32(0), C.c_double(0), C.c_uint8(0)
+            r = self.lib.isdf_frontend_path(self.h, _dp(st), _dp(gl), None, cap, _dp(xyz), _dp(rp), C.byref(n), C.byref(cost), C.byref(found))
+            if r == -1 and attempt == 0 and n.value > cap:
+                cap = n.value
+                continue
+            self._check(r)
+            break
+        return xyz[:n.value], rp[:n.value], cost.value, bool(found.value)
+
+    def frontend_path_raw(self, start, goal, cap):
+        """isdf_frontend_path with the caller's cap: (status, n)"""
+        st, gl = _f64(start).reshape(3), _f64(goal).reshape(3)
+        xyz, rp = np.zeros((max(cap, 1), 3)), np.zeros((max(cap, 1), 2))
+        n, cost, found = C.c_int32(-7), C.c_double(0), C.c_uint8(0)
+        r = self.lib.isdf_frontend_path(self.h, _dp(st), _dp(gl), None, int(cap), _dp(xyz), _dp(rp), C.byref(n), C.byref(cost), C.byref(found))
+        return r, n.value
+
+    def frontend_path_batch_device(self, start, B, d_goals, cap, d_xyz, d_rp, d_offsets, d_costs, d_found, stream=None):
+        st = _f64(start).reshape(3)
+        self._check(self.lib.isdf_frontend_path_batch_device(self.h, _dp(st), B, d_goals, None, cap, d_xyz, d_rp, d_offsets, d_costs, d_found, stream))
+
+    def frontend_path_field_device(self, start, d_g, stream=None):
+        st = _f64(start).reshape(3)
+        self._check(self.lib.isdf_frontend_path_field_device(self.h, _dp(st), None, d_g, stream))
+
+    def frontend_path_info(self):
+        out = FrontPathInfo()
+        self._check(self.lib.isdf_frontend_path_info(self.h, C.byref(out)))
+        return out.as_dict()
+
+    def dbg_frontpath_traversable(self):
+        """traversability of the last path / field call as an (X, Y, Z) bool array (isdf_dbg_frontpath_traversable, not part of include/isdf.h)"""
+        X, Y, Z = self.map_info()["dims"]
+        Zw = (Z + 31) // 32
+        words = np.zeros(X * Y * Zw, dtype=np.uint32)
+        self.lib.isdf_dbg_frontpath_traversable.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.c_longlong]
+        self._check(self.lib.isdf_dbg_frontpath_traversable(self.h, words.ctypes.data_as(C.POINTER(C.c_uint32)), words.size))
+        bits = np.unpackbits(words.view(np.uint8), bitorder="little").reshape(X, Y, Zw * 32)
+        return bits[:, :, :Z].astype(bool)
 
     # ---- multi-GPU reduction over peer memory (see include/isdf.h) ----
     def peer_export(self, world, max_doubles):

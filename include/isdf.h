@@ -342,6 +342,62 @@ int isdf_frontend_feasibility_device(isdf_ctx *ctx, uint32_t *d_masks, void *cud
 int isdf_frontend_check_batch(isdf_ctx *ctx, int n, const int32_t *ind, const double *father_roll_pitch,
                               double *child_roll_pitch, uint8_t *ok);
 
+/* ---- front-end path search: replaces AstarPathSearcher::AstarPathSearch + getPath / getastarSE3Path (front_end_Astar.hpp:197-402) ----
+ * Definition
+ *   Traversable(v) v is in the map, not occupied, and its isdf_frontend_feasibility mask is not zero (some attitude fits; checkKernelValue's
+ *                  visit_kernels_by_distance tries every attitude, swm:852-913).
+ *   Source s, target t  getGridIndex (grid:135-175) of the start and of the goal; both must pass isInMap (bmin <= p <= bmax on every axis).
+ *   Field g        g(s) = 0. For v != s, g(v) is the minimum, over 26-connected paths s = v0, v1, ..., vk = v whose nodes v1..vk are all
+ *                  traversable, of the left-to-right FP64 sum of the edge costs sqrt((double)(di^2 + dj^2 + dk^2)); +inf where no path
+ *                  exists. s itself need not be traversable. FP addition of a positive cost is monotone, so the minimum does not depend on
+ *                  any processing order and a textbook FP64 Dijkstra computes the same bits. The field is exact on EVERY voxel: the
+ *                  relaxation is label-correcting and runs until no value changes.
+ *   Parent(v)      for v != s with g(v) < inf: among the 26 neighbours u with g(u) + w(u, v) == g(v) in FP64 (such a u is traversable or
+ *                  is s), the first in the reference's offset order u = v + (i, j, k), i, j, k = -1..1, i outermost (front_end_Astar.hpp:207-211).
+ *   Path to t      the parents from t back to s, reversed: node 0 is s, the last node is t; coordinates are cube centres (getGridCubeCenter).
+ *                  Found iff g(t) < inf (t traversable, or t == s: a one-node path, even on an occupied voxel); the cost is g(t). No path
+ *                  is not an error: found = 0, cost +inf and a one-node path (the start).
+ *   Attitudes      node 0 has (roll, pitch) = (0, 0) (GridNode's defaults); node m + 1 has checkKernelValue(attitude of node m, node m + 1):
+ *                  isdf_frontend_check_batch applied as a chain along the returned path.
+ * Deviations from the reference, on purpose: its open set keeps the stale key of an improved open node (:324-333) and its heuristic is
+ *   inflated by 1.001 (:172-187), so its cost is >= the optimum and depends on pop order; here the path is the exact shortest one. Its
+ *   AstarGetSucc overwrites a neighbour's attitude on every expansion that looks at it (:227-229), so the attitude getastarSE3Path reports
+ *   can come from a node that is not the path father; here the attitudes are replayed father to child along the returned path.
+ * Batch: one start and B goals (candidate goals, or restarts sharing a start). The field is built once per call; every goal's result is
+ *   bit-identical to a call with that goal alone, and results are bit-identical run to run and through either entry point.
+ * Outputs: the B paths back to back, path b in rows [offsets[b], offsets[b+1]) of path_xyz (cap x 3) and path_roll_pitch (cap x 2,
+ *   degrees; may be NULL); costs and found: B each. The single-goal call reports its length in *n.
+ * Errors: ISDF_ERR_STATE without a map or without front-end kernels (isdf_frontend_build_kernels; again after a shape change);
+ *   ISDF_ERR_INVALID for a NULL pointer, B < 1, a non-finite start or goal, a start or goal outside the map, non-zero reserved parameters,
+ *   or cap smaller than the total path length (then *n / offsets still report the lengths needed); ISDF_ERR_UNSUPPORTED on a sharded
+ *   context (isdf_set_shard world > 1).
+ * State: every call rebuilds the traversability grid and the field from the current map and front-end kernels, so nothing computed for an
+ *   earlier map, shape or kernel set is ever used. Device memory, allocated on first use and reused: the FP64 field (8 B per voxel, 1 GiB at
+ *   512^3) and three bit grids (traversability and two frontiers, 1 bit per voxel each). The calls count their launches in
+ *   isdf_stats.kernel_launches and touch no other field of isdf_stats. */
+typedef struct isdf_frontpath_params {   /* NULL = defaults; the reserved fields must be zero */
+    int32_t reserved_[4];
+} isdf_frontpath_params;
+typedef struct isdf_frontpath_info {       /* the last path or field call */
+    int32_t rounds;                        /* relaxation rounds that had a non-empty frontier */
+    int32_t reserved_;
+    int64_t field_bytes;                   /* device bytes of the FP64 field */
+    double traversability_ms, field_ms, paths_ms;   /* device time of the three stages (CUDA events on the call's stream) */
+} isdf_frontpath_info;
+int isdf_frontend_path(isdf_ctx *ctx, const double *start, const double *goal, const isdf_frontpath_params *params, int cap,
+                       double *path_xyz, double *path_roll_pitch, int32_t *n, double *cost, uint8_t *found);
+int isdf_frontend_path_batch(isdf_ctx *ctx, const double *start, int B, const double *goals, const isdf_frontpath_params *params, int cap,
+                             double *path_xyz, double *path_roll_pitch, int32_t *offsets, double *costs, uint8_t *found);
+/* device variant: d_goals (B x 3) and every output on ctx's device, start (3 doubles) on the host. Work queued on cuda_stream before the
+ * call is waited for; the call runs on cuda_stream, synchronises it between stages and returns when the outputs are written. */
+int isdf_frontend_path_batch_device(isdf_ctx *ctx, const double *start, int B, const double *d_goals, const isdf_frontpath_params *params,
+                                    int cap, double *d_path_xyz, double *d_path_roll_pitch, int32_t *d_offsets, double *d_costs,
+                                    uint8_t *d_found, void *cuda_stream);
+/* the cost-to-come field from start (host, 3 doubles): d_g = X*Y*Z doubles on ctx's device, address ix*Y*Z + iy*Z + iz, +inf where no
+ * path exists. Same errors and stream behaviour as the device variant. */
+int isdf_frontend_path_field_device(isdf_ctx *ctx, const double *start, const isdf_frontpath_params *params, double *d_g, void *cuda_stream);
+int isdf_frontend_path_info(isdf_ctx *ctx, isdf_frontpath_info *out);
+
 /* ---- swept-volume term: addSaftyPenaOnSweptVolumeParallel (hpp:557-649) + getSDFofSweptVolume (swm:710-747) --- */
 /* parallel_points (plan_manager.cpp:246-254): P x 3 row-major world-frame voxel centres; resets lastTstar to 0 (not the persisted
  * trajectory duration: see isdf_set_points_batch) */
