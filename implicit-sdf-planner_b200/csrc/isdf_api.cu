@@ -53,7 +53,6 @@ struct isdf_ctx {
     int sm_count = 132, mesh_blocks = 4, analytic_blocks = 4;   // persistent grids: one CTA per resident slot
     size_t smem_per_sm = 228 * 1024;   // shared memory of one SM (H100: 228 KB, at most 227 KB to one CTA)
     int clr_blocks = 1;                // resident CTAs per SM of the clearance scan kernel
-    bool dbg_on = false;
     isdf_stats stats = {};
     struct {
         bool have_map = false;
@@ -75,7 +74,7 @@ struct isdf_ctx {
         DevBuf<int> d_tickets;       // pieces_done counter of the epilogue kernel
         DevBuf<double> d_tot; DevBuf<unsigned> d_split_done;   // per-sample collision sums handed from the scan kernels to the epilogue
         DevBuf<int> d_items, d_item_count; DevBuf<unsigned> d_work, d_split_work; DevBuf<double> d_subsum;   // work items (longest first, heavy samples split)
-        DevBuf<unsigned long long> d_counter, d_dbg, d_trace;
+        DevBuf<unsigned long long> d_counter;
         bool no_items = false;       // diagnostics: always launch in natural order, never split (isdf_dbg_schedule)
         int warp_slots_override = 0; // diagnostics: pretend the device has this many resident warps (forces splitting)
     } disc;
@@ -907,9 +906,6 @@ static int launch_discrete(isdf_ctx *c, int N, const double *d_T, const double *
         if (int r = peer_fuse_check(c, N)) return r;
         A.peer = c->peer.args; A.peer.epoch = c->peer.args.epoch + 1;   // committed below, once the exchange kernel is really enqueued
     }
-    A.dbg = nullptr;
-    A.trace = nullptr;
-    if (c->dbg_on) { CU_TRY(c->disc.d_dbg.ensure((size_t)3 * S)); CU_TRY(cudaMemsetAsync(c->disc.d_dbg.p, 0, sizeof(unsigned long long) * 3 * S, st)); A.dbg = c->disc.d_dbg.p; }
     const long long M = (S - c->rank + c->world - 1) / c->world;
     CU_TRY(cudaMemsetAsync(c->disc.d_counter.p, 0, sizeof(unsigned long long), st));
     // longest-first order from the previous evaluation of the same problem shape (first evaluation: natural order)
@@ -932,7 +928,6 @@ static int launch_discrete(isdf_ctx *c, int N, const double *d_T, const double *
         CU_TRY(cudaMemsetAsync(c->disc.d_split_done.p, 0, sizeof(unsigned) * std::max(max_split, 1), st));
     }
     A.work = c->disc.d_work.p;
-    if (c->dbg_on) { CU_TRY(c->disc.d_trace.ensure(TRACE_STRIDE * max_items)); CU_TRY(cudaMemsetAsync(c->disc.d_trace.p, 0, sizeof(unsigned long long) * TRACE_STRIDE * max_items, st)); A.trace = c->disc.d_trace.p; }
     // a launch with far more samples than resident warps (batched callbacks: millions) balances itself through the persistent warps'
     // dynamic item counter: sorting / splitting would only cost a long single-CTA pass over the work array
     const bool want_items = !c->disc.no_items && M <= 1024ll * ITEMS_CACHE * 4;
@@ -1624,14 +1619,16 @@ static int frontend_feasibility_run(isdf_ctx *c, uint32_t *d_masks, uint32_t *d_
     const long long nrun = (long long)c->map.grid.X * c->map.grid.Y * ((c->map.grid.Z + FE_ZRUN - 1) / FE_ZRUN);
     const long long sms = c->sm_count;
     const unsigned grid = (unsigned)std::min<long long>((nrun + 255) / 256, sms * 64);
-    if (c->fe.ncore > 0 && nrun < (1ll << 32) && !getenv("ISDF_FE_ONE_PASS")) {
+    // the input picks the pipeline: one pass when no voxel can be settled early (empty kernel core) or the runs outgrow 32-bit
+    // survivor indices; two passes otherwise, table-driven when the pattern tables fit into shared memory
+    if (c->fe.ncore > 0 && nrun < (1ll << 32)) {
         // two passes: the kernel core settles most voxels of a cluttered map, the mask accumulation runs on the survivors only
         CU_TRY(c->fe.d_surv.ensure((size_t)nrun));
         CU_TRY(c->fe.d_count.ensure(1));
         A.surv = c->fe.d_surv.p; A.surv_count = c->fe.d_count.p;
         CU_TRY(cudaMemsetAsync(c->fe.d_count.p, 0, sizeof(unsigned), (cudaStream_t)cuda_stream));
         const size_t tsmem = sizeof(uint4) * ((size_t)c->fe.ntab + (size_t)c->fe.nchunk);
-        if (c->fe.nchunk > 0 && tsmem <= 200 * 1024 && !getenv("ISDF_FE_NO_TABLES")) {
+        if (c->fe.nchunk > 0 && tsmem <= 200 * 1024) {
             // throughput form: zero-filled output, bit-parallel core pass (32 voxels per thread), table-driven accumulation on the survivors
             const long long nvox = (long long)c->map.grid.X * c->map.grid.Y * c->map.grid.Z;
             if (!d_trav) CU_TRY(cudaMemsetAsync(d_masks, 0, sizeof(uint32_t) * 4 * (size_t)nvox, (cudaStream_t)cuda_stream));
@@ -2012,7 +2009,6 @@ extern "C" int isdf_get_swept_results(isdf_ctx *c, double *tstar, double *sdf, d
 
 
 // ---- internal diagnostics (not part of include/isdf.h) ------------------------------------------------------------
-extern "C" int isdf_dbg_enable(isdf_ctx *c, int on) { if (!c) return -1; c->dbg_on = on != 0; c->sv.dbg_on = on != 0; return 0; }
 // scheduling diagnostics: natural_order != 0 -> every launch in natural sample order, nothing split (the state of a context's FIRST
 // evaluation); warp_slots > 0 -> build the work items as if the device had that many resident warps (huge values shrink the
 // balanced share per warp and force every non-trivial sample to be split, so tests can compare split parts against the oracle on one
@@ -2092,11 +2088,6 @@ extern "C" int isdf_dbg_mesh_lists(isdf_ctx *c, long long *sizes, uint32_t *cell
     if (tris && cudaMemcpy(tris, m.tris, sizeof(double) * TRI_STRIDE * (size_t)m.ntris, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
     return 0;
 }
-extern "C" int isdf_dbg_swept_stats(isdf_ctx *c, unsigned long long *out, long long n) {
-    if (!c || !out || (size_t)n > c->sv.d_dbg.n) return -1;
-    cudaStreamSynchronize(c->stream);
-    return cudaMemcpy(out, c->sv.d_dbg.p, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -3;
-}
 // the swept-volume term of the last batched callback, B x (19 N0 + 1): per problem [cost | gradC 18 N0 | gradT N0], as the callback adds it
 extern "C" int isdf_dbg_batch_swept_out(isdf_ctx *c, double *out, long long n) {
     if (!c || !out || n < 0 || (size_t)n > c->batch.d_sv.n) return -1;
@@ -2110,15 +2101,4 @@ extern "C" int isdf_dbg_clearance_counts(isdf_ctx *c, unsigned long long *out) {
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
     return cudaMemcpy(out, c->clr.d_counters.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -1;
-}
-extern "C" int isdf_dbg_trace_stride(void) { return TRACE_STRIDE; }
-extern "C" int isdf_dbg_item_trace(isdf_ctx *c, unsigned long long *out, long long n) {
-    if (!c || !out || (size_t)n > c->disc.d_trace.n) return -1;
-    if (cudaSetDevice(c->device) != cudaSuccess) return -3;
-    return cudaMemcpy(out, c->disc.d_trace.p, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -3;
-}
-extern "C" int isdf_dbg_sample_stats(isdf_ctx *c, unsigned long long *out, long long n) {
-    if (!c || !out || (size_t)n > c->disc.d_dbg.n) return -1;
-    if (cudaSetDevice(c->device) != cudaSuccess) return -3;
-    return cudaMemcpy(out, c->disc.d_dbg.p, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -3;
 }

@@ -51,10 +51,7 @@ constexpr int MAX_SPLIT_SLOTS = 16384;  // split samples per launch (2 KB of cla
 constexpr int WINDOW_AXIS_MAX = 1023;   // voxels per window axis: window offsets are packed 10 bits per axis
 // CTAs per SM the register allocator must leave room for: 4 CTAs x 128 threads x 128 registers fill the 64 K-register file of an SM
 constexpr int ANALYTIC_MIN_BLOCKS = 4;
-#ifndef ISDF_MESH_MIN_BLOCKS
-#define ISDF_MESH_MIN_BLOCKS 4
-#endif
-constexpr int MESH_MIN_BLOCKS = ISDF_MESH_MIN_BLOCKS;
+constexpr int MESH_MIN_BLOCKS = 4;
 constexpr int EPI_THREADS = 288;
 constexpr int ITEMS_CACHE = 24;   // k_build_items: samples per thread whose work value is kept in registers (M <= 24576: any single trajectory)
 
@@ -71,9 +68,6 @@ struct DiscArgs {
     double *out;           // 19N+1: cost | gradC | gradT
     unsigned long long *pair_counter;  // may be null
     double *count_out;                 // host entry point only: the pair count (bit pattern) lands behind the result vector, one D2H copy fetches both
-    unsigned long long *dbg;           // may be null: per sample {cycles, pairs, work}
-    unsigned long long *trace;         // may be null: per work-item slot {begin, end} in ns of the global timer (+ 4 phase cycle counts, total
-                                       // cycles, queries | pairs and triangle records tested with -DISDF_PHASE_TIMING)
     const int *items;                  // may be null: 3 ints per work item {local sample m, -1 = all classes or c0 | c1 << 8, split slot or -1}
     const int *item_count;             // number of valid items (device)
     int *item_cursor;                  // persistent warps draw items from this counter (zero on entry; the epilogue zeroes it again)
@@ -265,15 +259,7 @@ __device__ __forceinline__ void sample_epilogue(const DiscArgs &A, int i, int j,
 
 // ============================================================================================================================
 // Work item of a warp: {global sample, first class, one-past-last class, split slot}.
-struct Item { int s, c0, c1, hslot, slot; };
-__device__ __forceinline__ unsigned long long global_ns() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
-#ifdef ISDF_PHASE_TIMING
-constexpr int TRACE_STRIDE = 9;
-#define ISDF_PT(x) x
-#else
-constexpr int TRACE_STRIDE = 2;
-#define ISDF_PT(x)
-#endif
+struct Item { int s, c0, c1, hslot; };
 
 // Persistent-warp scheduler: the warp's next work item, or false when the table is exhausted. Which warp takes which item
 // never touches the arithmetic, so results stay bit-reproducible.
@@ -284,7 +270,6 @@ __device__ __forceinline__ bool next_item(const DiscArgs &A, Item &it, int lane)
     int slot = 0;
     if (lane == 0) slot = atomicAdd(A.item_cursor, 1);
     slot = __shfl_sync(0xffffffffu, slot, 0);
-    it.slot = slot;
     if (A.items) {
         if (slot >= __ldg(A.item_count)) return false;
         const int m = __ldg(A.items + 3 * slot), part = __ldg(A.items + 3 * slot + 1);
@@ -300,14 +285,13 @@ __device__ __forceinline__ bool next_item(const DiscArgs &A, Item &it, int lane)
 
 // Shared tail of both scan kernels for an item that covers the WHOLE sample: lanes 0..7 hold the eight collision sums.
 // The per-sample chain rule and the per-piece reduction run afterwards in k_discrete_epilogue with one THREAD per sample.
-__device__ __forceinline__ void sample_finish_whole(const DiscArgs &A, const Item &it, double mine, unsigned npairs, long long t_begin, unsigned work) {
+__device__ __forceinline__ void sample_finish_whole(const DiscArgs &A, const Item &it, double mine, unsigned npairs, unsigned work) {
     const int lane = threadIdx.x & 31;
     const int s = it.s;
     if (lane < 8) A.tot[(size_t)s * 8 + lane] = mine;
     if (lane == 0) {
         if (A.pair_counter && npairs) atomicAdd(A.pair_counter, (unsigned long long)npairs);
         if (A.work) A.work[s] = work;
-        if (A.dbg) { A.dbg[3 * (size_t)s] = (unsigned long long)(clock64() - t_begin); A.dbg[3 * (size_t)s + 1] = npairs; A.dbg[3 * (size_t)s + 2] = work; }
     }
 }
 
@@ -407,7 +391,6 @@ __global__ void __launch_bounds__(DISC_THREADS, ANALYTIC_MIN_BLOCKS) k_discrete_
         const int i = s / (K + 1), j = s - i * (K + 1);
         const double Ti = __ldg(A.T + i);
         const double step = Ti * (1.0 / K);
-        const long long t_begin = A.dbg ? clock64() : 0;
 
         d3 pos; quat4 q; rot3 R;
         sample_pose(A, i, j, step, pos, q, R);
@@ -484,7 +467,7 @@ __global__ void __launch_bounds__(DISC_THREADS, ANALYTIC_MIN_BLOCKS) k_discrete_
             const double t4 = warp_sum(acc.q0), t5 = warp_sum(acc.q1), t6 = warp_sum(acc.q2), t7 = warp_sum(acc.q3);
             mine = lane == 0 ? t0 : lane == 1 ? t1 : lane == 2 ? t2 : lane == 3 ? t3 : lane == 4 ? t4 : lane == 5 ? t5 : lane == 6 ? t6 : t7;
         }
-        sample_finish_whole(A, it, mine, npairs, t_begin, npairs);
+        sample_finish_whole(A, it, mine, npairs, npairs);
         __syncwarp();
     }
 }
@@ -530,10 +513,6 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
     while (next_item(A, it, lane)) {
         const int s = it.s;
         const int i = s / (K + 1), j = s - i * (K + 1);
-        const long long t_begin = A.dbg ? clock64() : 0;
-        if (A.trace && lane == 0) A.trace[TRACE_STRIDE * (size_t)it.slot] = global_ns();
-        ISDF_PT(long long pt_pose = 0; long long pt_cull = 0; long long pt_search = 0; long long pt_tail = 0; long long pt_t0 = clock64(); long long pt_all0 = pt_t0;
-                if (lane == 0) sm.stk.tested = 0u; __syncwarp();)
         unsigned npairs = 0, nquery = 0;
         const bool whole = (it.c1 - it.c0) == ROW_CLASSES;
 
@@ -554,7 +533,6 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
             }
             for (int k = lane; k < ROW_CLASSES * 8; k += 32) (&sm.cacc[0][0])[k] = 0.0;
             __syncwarp();
-            ISDF_PT(pt_pose = clock64() - pt_t0;)
             const int ny = W.iy1 - W.iy0 + 1;
             const int nrows = (W.ix1 - W.ix0 + 1) * ny;
             const float inv_ny = 1.0f / (float)ny;
@@ -564,7 +542,6 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
             // contributions are then added to the class accumulators in voxel order by lanes 0..7 (one per component)
             auto flush_tails = [&]() __attribute__((always_inline)) {
                 __syncwarp();
-                ISDF_PT(const long long pt_a = clock64();)
                 bool active = false;
                 if (lane < nres) {
                     const QRes r = sm.qr[lane];
@@ -590,13 +567,11 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
                 }
                 __syncwarp();
                 nres = 0;
-                ISDF_PT(pt_tail += clock64() - pt_a;)
             };
 
             int nsv = 0;   // queued survivors (warp-uniform)
             // cull stage for the n oldest voxels of the ring (n <= 32): survivors are appended to the survivor queue
             auto cull = [&](int n) __attribute__((always_inline)) {
-                ISDF_PT(const long long pt_a = clock64();)
                 bool pass = false, box = false;
                 uint32_t code = 0;
                 d3 prel = mk3(0, 0, 0);
@@ -632,13 +607,11 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
                 }
                 nsv += __popc(bal);
                 __syncwarp();
-                ISDF_PT(pt_cull += clock64() - pt_a;)
             };
             // search stage for every queued survivor, in voxel order, software-pipelined ACROSS queries: while query k runs, the
             // first 32 candidate ids of query k+2 are being loaded and the triangle records of query k+1's first pass are
             // prefetched into L1 — the id -> record -> arithmetic chain of a query starts with its operands already close
             auto search_all = [&](bool final) __attribute__((always_inline)) {
-                ISDF_PT(const long long pt_a = clock64(); const long long pt_tail0 = pt_tail;)
                 nquery += nsv;
                 auto first_ids = [&](int k, int &id, float &lb) {   // first-pass candidate and its lower bound
                     id = -1; lb = 0.0f;
@@ -674,7 +647,6 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
                 } while (k < nsv);
                 __syncwarp();
                 nsv = 0;
-                ISDF_PT(pt_search += (clock64() - pt_a) - (pt_tail - pt_tail0);)
             };
 
             // Producer loop (one cull and one search call site): batches of 32 window rows are loaded (lane = row), their occupied voxels
@@ -755,7 +727,7 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
             if (whole) {
                 double mine = 0.0;
                 if (lane < 8) for (int c = 0; c < ROW_CLASSES; c++) mine += sm.cacc[c][lane];
-                sample_finish_whole(A, it, mine, npairs, t_begin, 64u * nquery + npairs);
+                sample_finish_whole(A, it, mine, npairs, 64u * nquery + npairs);
             } else {
                 // split part: publish this part's class sums; the LAST part of the sample to arrive (one ticket per split slot) adds
                 // all 32 class sums in class order — the same additions a whole-sample item performs — so that the epilogue sees
@@ -778,16 +750,11 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
                     unsigned total_work = 0;
                     if (lane == 0) { total_work = atomicExch(A.split_work + it.hslot, 0u); A.split_done[it.hslot] = 0u; }
                     total_work = __shfl_sync(0xffffffffu, total_work, 0);
-                    sample_finish_whole(A, it, mine, 0u, t_begin, total_work);
+                    sample_finish_whole(A, it, mine, 0u, total_work);
                 }
             }
         } else {
-            sample_finish_whole(A, it, 0.0, 0u, t_begin, 0u);
-        }
-        if (A.trace && lane == 0) {
-            unsigned long long *tr = A.trace + TRACE_STRIDE * (size_t)it.slot;
-            tr[1] = global_ns();
-            ISDF_PT(tr[2] = pt_pose; tr[3] = pt_cull; tr[4] = pt_search; tr[5] = pt_tail; tr[6] = clock64() - pt_all0; tr[7] = ((unsigned long long)nquery << 32) | npairs; tr[8] = sm.stk.tested;)
+            sample_finish_whole(A, it, 0.0, 0u, 0u);
         }
         __syncwarp();
     }

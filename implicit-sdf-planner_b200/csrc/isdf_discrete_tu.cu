@@ -4,9 +4,7 @@
 // time. The swept-volume search, whose accept/reject sequence must replay the reference's bit for bit, stays in
 // isdf_api.cu under -fmad=false. ISDF_FAST_TRI selects the division-free closest-point test (isdf_mesh.cuh) for this TU only.
 #define ISDF_DISCRETE_TU 1
-#ifndef ISDF_NO_FAST_TRI   // A/B builds only
 #define ISDF_FAST_TRI 1
-#endif
 #include "../../include/isdf.h"
 #include "isdf_types.cuh"
 #include "isdf_discrete.cuh"
@@ -14,14 +12,6 @@
 namespace isdf {
 
 cudaError_t discrete_launch_scan(const DiscArgs &A, bool mesh, unsigned grid, cudaStream_t st) {
-#ifdef ISDF_CARVEOUT
-    static bool carved = false;   // A/B: ask for the smallest shared-memory carve-out that still holds 4 CTAs/SM
-    if (!carved) {
-        carved = true;
-        cudaFuncSetAttribute(k_discrete_mesh<false>, cudaFuncAttributePreferredSharedMemoryCarveout, ISDF_CARVEOUT);
-        cudaFuncSetAttribute(k_discrete_mesh<true>, cudaFuncAttributePreferredSharedMemoryCarveout, ISDF_CARVEOUT);
-    }
-#endif
     if (mesh && A.shape.mesh.sign_mode == MESH_SIGN_WINDING) k_discrete_mesh<true><<<grid, DISC_THREADS, 0, st>>>(A);
     else if (mesh) k_discrete_mesh<false><<<grid, DISC_THREADS, 0, st>>>(A);
     else k_discrete_analytic<<<grid, DISC_THREADS, 0, st>>>(A);

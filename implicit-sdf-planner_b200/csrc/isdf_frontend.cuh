@@ -143,10 +143,7 @@ __device__ __forceinline__ bool any4(uint4 v) { return (v.x | v.y | v.z | v.w) !
 // One thread per run of FE_ZRUN voxels along z: the run's window rows are read once (ks + FE_ZRUN - 1 bits), every occupied map
 // voxel found in a row is applied to each of the run's voxels it overlaps (offset c = bit - j), one 128-bit shared-memory load
 // and four ORs per (occupied voxel, run voxel) pair.
-#ifndef ISDF_FE_ZRUN
-#define ISDF_FE_ZRUN 4
-#endif
-constexpr int FE_ZRUN = ISDF_FE_ZRUN;
+constexpr int FE_ZRUN = 4;
 __global__ void __launch_bounds__(256) k_frontend_feasibility(const __grid_constant__ FrontArgs A) {
     extern __shared__ __align__(16) uint32_t fe_sm[];
     frontend_stage_masks(A, fe_sm);

@@ -347,16 +347,7 @@ constexpr int WIDE_STACK = 96;
 // the stacked bounds are floats ROUNDED DOWN: still lower bounds, so pruning stays exact (a node is at worst opened needlessly)
 struct WideStack {
     int node[WIDE_STACK]; float d2[WIDE_STACK]; int leaf[32]; float leaf_d2[32];
-#ifdef ISDF_PHASE_TIMING
-    unsigned tested;   // triangle records tested by mesh_search_rec (diagnostic build only)
-#endif
 };
-#ifdef ISDF_PHASE_TIMING
-// every lane of the warp passes the number of records it tested since the last count
-#define ISDF_COUNT_TESTED(stk, n) do { const unsigned n_ = __reduce_add_sync(0xffffffffu, (unsigned)(n)); if ((stk) && (threadIdx.x & 31) == 0) (stk)->tested += n_; } while (0)
-#else
-#define ISDF_COUNT_TESTED(stk, n) do { (void)(n); } while (0)
-#endif
 
 __device__ __forceinline__ double wide_closest(const DevMesh &M, d3 p, double bound2, int seed, d3 &cbest, int &tri, int &feat,
                                                int lane, WideStack *stk) {
@@ -371,7 +362,6 @@ __device__ __forceinline__ double wide_closest(const DevMesh &M, d3 p, double bo
         const double dd = dot3(e, e);
         if (dd < best) { best = dd; cbest = q; tri = seed; feat = f; }
     }
-    ISDF_COUNT_TESTED(stk, seed >= 0 && lane == 0);
     int sp = 0;
     int cur = 0; double cur_d2 = 0.0;
     for (;;) {
@@ -401,11 +391,9 @@ __device__ __forceinline__ double wide_closest(const DevMesh &M, d3 p, double bo
             for (int base = 0; base < nleaf; base += 8) {
                 const int idx = base + (lane >> 2), slot = lane & 3;
                 double dd = 1e300; d3 q = mk3(0, 0, 0); int f = 0, t = -1;
-                [[maybe_unused]] int ntest = 0;   // records tested (ISDF_PHASE_TIMING builds)
                 if (idx < nleaf && (double)stk->leaf_d2[idx] < best) {
                     const int code = ~stk->leaf[idx];
                     const int first = code >> 3, cnt = (code & 7) + 1;
-                    ntest = (cnt - slot + 3) >> 2;
                     for (int k = slot; k < cnt; k += 4) {   // leaves of up to 8 triangles: slots take triangle k and k+4
                         const double *T = M.tris + TRI_STRIDE * (size_t)(first + k);
                         int ff;
@@ -415,7 +403,6 @@ __device__ __forceinline__ double wide_closest(const DevMesh &M, d3 p, double bo
                         if (d < dd) { dd = d; q = qq; f = ff; t = first + k; }
                     }
                 }
-                ISDF_COUNT_TESTED(stk, ntest);
                 // arg-min: 32-bit order-preserving key (float rounded down) + one REDUX; exact tie-break among equal keys
                 const bool cand = dd < best;
                 const unsigned key = cand ? __float_as_uint(__double2float_rd(dd)) : 0xffffffffu;
@@ -558,7 +545,7 @@ __device__ __forceinline__ double list_centre_dist_up(const DevMesh &M, d3 p, do
 // requested one pass ahead. r_up: list_centre_dist_up of p and the list's cell. bound2 seeds the best squared distance: when no
 // candidate is closer, tri = -1 (and the returned value is not a distance).
 __device__ __forceinline__ double list_closest_pre(const DevMesh &M, d3 p, uint32_t off, int cnt, int first_id, float first_lb, double r_up,
-                                                   double bound2, d3 &cbest, int &tri, int &feat, int lane, WideStack *tally = nullptr) {
+                                                   double bound2, d3 &cbest, int &tri, int &feat, int lane) {
     // the list's first candidate is the triangle nearest to the cell centre, so p's closest triangle lies within that distance plus
     // r_up: an upper bound (the slack undoes the bound's round-down) that prunes the first pass too. No candidate is returned unless
     // it is below bound2, and the closest one always is below this bound, so starting from the smaller of the two changes no answer.
@@ -580,7 +567,6 @@ __device__ __forceinline__ double list_closest_pre(const DevMesh &M, d3 p, uint3
             const d3 e = p - q;
             dd = dot3(e, e);
         }
-        ISDF_COUNT_TESTED(tally, test);
         warp_argmin_update(dd, q, t, f, best, cbest, tri, feat);
         if (base + 32 < cnt && list_lb_prunes(__shfl_sync(0xffffffffu, lb_next, 0), r_up, best)) break;
         t = t_next; lb = lb_next;
@@ -630,15 +616,6 @@ __device__ __forceinline__ double list_closest_lat(const DevMesh &M, d3 p, uint3
     return best;
 }
 
-#ifdef ISDF_OUTLINE_TREE_SEARCH
-// Out-of-line copy of the tree search for the discrete scan kernel, where candidate lists answer almost every query: the kernel's
-// hot loop then stays small (instruction cache) — the call's spills are paid only on the rare tree path.
-static __device__ __noinline__ double wide_closest_outlined(const DevMesh &M, d3 p, double bound2, int seed, d3 &cbest, int &tri, int &feat,
-                                                            int lane, WideStack *stk) {
-    return wide_closest(M, p, bound2, seed, cbest, tri, feat, lane, stk);
-}
-#endif
-
 // Search half of getSDFwithGrad1 for the mesh shape, warp-cooperative: closest triangle of p (cell = p's cell index, or -1
 // outside the grid; the caller has already ruled out "far"). Returns false when nothing lies within `reach` and p is outside
 // (sdf >= reach: the caller's hinge / range test is inactive); otherwise (d2, c, tri, feat), identical on every lane.
@@ -674,18 +651,14 @@ __device__ __forceinline__ bool mesh_search_rec(const DevMesh &M, d3 p, double r
         const double r_up = list_centre_dist_up(M, p, floor((p.x - M.glo[0]) * M.inv_gcell), floor((p.y - M.glo[1]) * M.inv_gcell),
                                                 floor((p.z - M.glo[2]) * M.inv_gcell));
         for (;;) {   // one inlined copy of the list pass: first within `reach`, then (deep inside only) unbounded
-            d2 = list_closest_pre(M, p, off, cnt, first_id, first_lb, r_up, bound2, c, tri, feat, lane, stk);
+            d2 = list_closest_pre(M, p, off, cnt, first_id, first_lb, r_up, bound2, c, tri, feat, lane);
             if (tri >= 0 || bound2 >= 1e299) return true;
             if (!inside) return false;
             bound2 = 1e300;
         }
     }
     for (;;) {   // one inlined copy of the tree search, the same way (a separate loop: merged with the list pass, it spills)
-#ifdef ISDF_OUTLINE_TREE_SEARCH
-        d2 = wide_closest_outlined(M, p, bound2, seed, c, tri, feat, lane, stk);
-#else
         d2 = wide_closest(M, p, bound2, seed, c, tri, feat, lane, stk);
-#endif
         if (tri >= 0 || bound2 >= 1e299) return true;
         if (!inside) return false;
         bound2 = 1e300;

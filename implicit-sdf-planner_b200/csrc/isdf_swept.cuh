@@ -7,15 +7,16 @@
 //   k_sv_table : the coarse time grid t = 0, 0.2, ... (same running sum as the reference's for-loop) and the robot
 //                pose at each coarse time are computed ONCE per evaluation and shared by every point (the reference
 //                recomputes the pose per point per sample);
-//   k_sv_points: analytic shapes — one WARP per obstacle point. Lanes split the coarse scan (ballot -> in-range bitmap -> intervals via
-//                bit scans), split each fine scan, and run the sign-descent SPECULATIVELY: in one pass the 32 lanes
-//                evaluate f(x), the six finite-difference samples of the gradient and all 18 candidate steps
-//                x -/+ 0.02/2^d, so an outer iteration costs one SDF latency instead of up to 9 + 7 dependent ones.
+//   k_sv_points_cta<MESH>: one CTA (8 warps) per obstacle point. The threads split the coarse scan (in-range bitmap -> intervals
+//                via bit scans) and each fine scan.
+//                Mesh robots: every exact SDF value is a warp-cooperative closest-triangle search, the scans are pruned with the
+//                body-frame cell grid's Lipschitz brackets and the warps evaluate the descent's step candidates in parallel
+//                (details at the kernel).
+//                Analytic shapes: warp 0 runs the sign descent SPECULATIVELY: in one pass the 32 lanes evaluate f(x), the six
+//                finite-difference samples of the gradient and all 18 candidate steps x -/+ 0.02/2^d, so an outer iteration
+//                costs one SDF latency instead of up to 9 + 7 dependent ones.
 //                Accept/reject decisions replay the reference's sequential logic exactly (same comparisons, same
 //                iteration accounting);
-//   k_sv_points_cta<MESH>: one CTA (8 warps) per obstacle point; mesh robots: every exact SDF value is a warp-cooperative
-//                closest-triangle search, the scans are pruned with the body-frame cell grid's Lipschitz brackets and
-//                the warps evaluate the descent's step candidates in parallel (details at the kernel);
 //   k_sv_reduce / k_sv_finish: deterministic per-piece reduction (fixed thread->point map, fixed trees) and the
 //                gradT(j<i) prefix of hpp:642-645 as a suffix sum.
 #pragma once
@@ -53,8 +54,6 @@ __device__ __forceinline__ void stage_traj_block(double *sC, double *sT, const d
     }
 }
 
-constexpr int SV_WARPS = 4;
-constexpr int SV_THREADS = SV_WARPS * 32;
 constexpr int SV_MAX_COARSE = 1536;  // traj_duration < 300 s (updateTraj ignores longer ones, swm:291) at 0.2 s
 constexpr int SV_FLAG_WORDS = SV_MAX_COARSE / 32;
 
@@ -134,8 +133,6 @@ struct SvArgs {
     unsigned *work;
     int *order;
     int use_order;
-    unsigned long long *dbg2;       // -DISDF_PHASE_TIMING: 4 per point, descent sub-phases of warp 0
-    unsigned long long *dbg;        // -DISDF_PHASE_TIMING: 8 per point {total, coarse, bracket pass, exact pass, descent, intervals, exact searches, -}
 };
 
 // ---- k_sv_table ---------------------------------------------------------------------------------------------------
@@ -179,7 +176,7 @@ __device__ __forceinline__ void sv_table_body(const SvArgs &A, const int bx) {
     }
 }
 
-// ---- helpers for k_sv_points ------------------------------------------------------------------------------------
+// ---- helpers for k_sv_points_cta --------------------------------------------------------------------------------
 // Cell-grid bracket of the mesh SDF at a body-frame point: the SDF is 1-Lipschitz, so every point of a cell lies within
 // ghd of the cell centre's signed distance. Outside the grid only the lower bound gpad is known.
 __device__ __forceinline__ void mesh_bracket(const DevMesh &M, d3 prel, double &lo, double &hi) {
@@ -379,136 +376,6 @@ __device__ __forceinline__ void sv_point_tail(const SvArgs &A, const double *sC,
     A.piece[pk] = piece;
 }
 
-// ---- k_sv_points: one warp per obstacle point, analytic shapes ----------------------------------------------------------
-__device__ __forceinline__ void sv_points_body(const SvArgs &A, const int bx) {
-    extern __shared__ __align__(16) double smem[];
-    double *sC = smem, *sT = smem + 18 * A.N;
-    __shared__ uint32_t sflags[SV_WARPS][SV_FLAG_WORDS];
-#pragma nv_diag_suppress static_var_with_dynamic_init
-    __shared__ cuda::barrier<cuda::thread_scope_block> bar;
-    stage_traj_block(sC, sT, A.C, A.T, A.N, &bar);
-    const TrajView tr = {sT, sC, A.N};
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int Mloc = (A.P - A.rank + A.world - 1) / A.world;
-    const int m = bx * SV_WARPS + warp;
-    if (m >= Mloc) return;
-    const int pk = A.rank + A.world * m;
-    const d3 p = mk3(A.pts[3 * pk], A.pts[3 * pk + 1], A.pts[3 * pk + 2]);
-    const DevCfg &cfg = A.cfg;
-    const double dur = A.state[0];
-    const int nc = A.meta[0];
-    const double inf = 2 * cfg.safety + 0.1;   // safty_hor_inf (swm:383)
-
-    double sdf_value = 1e1, tstar = A.tstar[pk];
-    d3 grel = mk3(0, 0, 0);
-    unsigned nevals = 0;
-    bool found = false;
-
-    if (A.g_t) {
-        sdf_value = A.g_s[pk]; tstar = A.g_t[pk]; grel = mk3(A.g_g[3 * pk], A.g_g[3 * pk + 1], A.g_g[3 * pk + 2]);
-        found = true;
-    } else {
-        // ---- coarse scan: in-range bitmap -------------------------------------------------------------------------
-        uint32_t *fl = sflags[warp];
-        for (int base = 0; base < nc; base += 32) {
-            const int k = base + lane;
-            bool in = false;
-            if (k < nc) {
-                const double *o = A.poses + 12 * (size_t)k;
-                const d3 d = mk3(p.x - __ldg(o), p.y - __ldg(o + 1), p.z - __ldg(o + 2));
-                const d3 prel = mk3(__ldg(o + 3) * d.x + __ldg(o + 6) * d.y + __ldg(o + 9) * d.z,
-                                    __ldg(o + 4) * d.x + __ldg(o + 7) * d.y + __ldg(o + 10) * d.z,
-                                    __ldg(o + 5) * d.x + __ldg(o + 8) * d.y + __ldg(o + 11) * d.z);
-                in = shape_sdf_analytic(A.shape, prel) < inf;
-            }
-            const unsigned b = __ballot_sync(0xffffffffu, in);
-            if (lane == 0) fl[base >> 5] = b;
-        }
-        __syncwarp();
-        nevals += nc;
-        const int nwords = (nc + 31) >> 5;
-        // last run entry (in-range sample whose predecessor is out of range): its SDF initialises range_mindis (quirk Q2)
-        int last_entry = -1;
-        for (int w = nwords - 1; w >= 0 && last_entry < 0; w--) {
-            const uint32_t cur = fl[w];
-            const uint32_t prevbit = (w > 0) ? (fl[w - 1] >> 31) : 0u;
-            const uint32_t starts = cur & ~((cur << 1) | prevbit);
-            if (starts) last_entry = w * 32 + (31 - __clz(starts));
-        }
-        if (last_entry >= 0) {
-            double range_mindis = sv_sdf_at(A, tr, p, A.times[last_entry]);   // same value the coarse pass saw
-            double range_time_seed = 0.0;
-            double min_sdf_star = 1e1;
-            // walk the closed runs in order
-            int pos = 0;
-            while (pos < nc) {
-                // next set bit at or after pos
-                int kin = -1;
-                for (int w = pos >> 5; w < nwords; w++) {
-                    uint32_t cur = fl[w];
-                    if (w == (pos >> 5)) cur &= ~((1u << (pos & 31)) - 1u);
-                    if (cur) { kin = w * 32 + __ffs(cur) - 1; break; }
-                }
-                if (kin < 0) break;
-                // next clear bit after kin
-                int kout = -1;
-                for (int w = kin >> 5; w < nwords; w++) {
-                    uint32_t cur = ~fl[w];
-                    if (w == (kin >> 5)) cur &= ~((1u << (kin & 31)) - 1u);
-                    if (w == nwords - 1 && (nc & 31)) cur &= (1u << (nc & 31)) - 1u;
-                    if (cur) { kout = w * 32 + __ffs(cur) - 1; break; }
-                }
-                if (kout < 0) break;  // run still open at the end of the scan: dropped (quirk Q2)
-                const double lb = fmax(0.0, A.times[kin] - 0.2);
-                const double ub = fmin(dur, A.times[kout] + 0.2);
-                // ---- fine scan of [lb, ub) at dt = 0.02 (swm:423-438): t advances by repeated addition ----------------
-                {
-                    double t = lb;
-                    for (int q = 0; q < lane; q++) t += 0.02;
-                    int mi = lane;
-                    while (__any_sync(0xffffffffu, t < ub)) {
-                        const bool valid = t < ub;
-                        double dis = 1e300;
-                        if (valid) dis = sv_sdf_at(A, tr, p, t);
-                        nevals += __popc(__ballot_sync(0xffffffffu, valid));
-                        // warp argmin, ties -> smaller sample index (first occurrence wins under the strict '<')
-                        double bd = dis; int bi = mi; double bt = t;
-#pragma unroll
-                        for (int o = 16; o > 0; o >>= 1) {
-                            const double od = __shfl_xor_sync(0xffffffffu, bd, o);
-                            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                            const double otm = __shfl_xor_sync(0xffffffffu, bt, o);
-                            if (od < bd || (od == bd && oi < bi)) { bd = od; bi = oi; bt = otm; }
-                        }
-                        if (bd < range_mindis) { range_mindis = bd; range_time_seed = bt; }
-                        for (int q = 0; q < 32; q++) t += 0.02;
-                        mi += 32;
-                    }
-                }
-                // ---- descent inside the interval (swm:730-734) ---------------------------------------------------------
-                const double tmin_ = fmax(0.0, lb), tmax_ = fmin(ub, dur);
-                double sdf_star = 1e1, t_star = 0;
-                sv_gradient_descent(A, tr, p, tmin_, tmax_, range_time_seed, sdf_star, t_star, nevals, lane);
-                if (sdf_star < min_sdf_star) { min_sdf_star = sdf_star; tstar = t_star; found = true; }
-                pos = kout;
-            }
-            if (found) {
-                sdf_value = min_sdf_star;
-                // getGradPrelAtTimeStamp (swm:566-572) at the winning t*
-                d3 x, v, a, j;
-                traj_pvaj(tr, tstar, x, v, a, j);
-                const rot3 R = quat_rot(flat_quat_only(cfg.fp, v, a));
-                grel = warp_grad(A.shape, rot_applyT(R, p - x), lane);
-            }
-        }
-    }
-
-    if (lane == 0) {
-        if (A.counter && nevals) atomicAdd(A.counter, (unsigned long long)nevals);
-        sv_point_tail(A, sC, tr, pk, p, found, tstar, sdf_value, grel);
-    }
-}
-
 // ---- k_sv_points_cta: one CTA (SVM_WARPS warps) per obstacle point (designed for mesh robots) ----------------------------------------
 // The work per point is extremely uneven (half of the points never come within range; a few need >100 closest-triangle
 // searches in sequence), and with 10^2-10^4 points the kernel is a single wave: its duration is the SLOWEST point, not the
@@ -520,14 +387,7 @@ __device__ __forceinline__ void sv_points_body(const SvArgs &A, const int bx) {
 //   * the SDF value and gradient of an accepted candidate are carried into the next iteration (same point, same function),
 //     which removes the re-evaluation at the new x — guarded by a bit-compare of the body-frame point.
 // Decisions, values and the reference-equivalent evaluation count are those of the sequential algorithm.
-#ifndef ISDF_SV_ANALYTIC_CTA
-#define ISDF_SV_ANALYTIC_CTA 1
-#endif
-constexpr bool SV_ANALYTIC_CTA = ISDF_SV_ANALYTIC_CTA != 0;   // analytic shapes: CTA per point (k_sv_points_cta<false>) or warp per point (k_sv_points)
-#ifndef ISDF_SVM_WARPS
-#define ISDF_SVM_WARPS 8
-#endif
-constexpr int SVM_WARPS = ISDF_SVM_WARPS;   // warps per obstacle point (-DISDF_SVM_WARPS for A/B builds)
+constexpr int SVM_WARPS = 8;   // warps per obstacle point
 constexpr int SVM_THREADS = SVM_WARPS * 32;
 
 struct SvmShared {
@@ -538,10 +398,6 @@ struct SvmShared {
     double cand_f[9], cand_x[9], cand_g[9][3], cand_q[9][3];
     double bc[4];
     double bestg[SVM_WARPS][32][6];      // fine scan: gradient and body-frame point of every lane's best sample (the descent starts there)
-#ifdef ISDF_PHASE_TIMING
-    unsigned dbg_rounds, dbg_exact, dbg_requery;   // descent candidate batches; fine-scan samples that needed an exact search; descent re-queries at x
-    long long dbg_t[4];               // descent, warp 0: pose at x, re-query at x, candidate (pose + query), wait + replay
-#endif
 };
 
 __device__ __forceinline__ bool same_bits(d3 a, d3 b) { return a.x == b.x && a.y == b.y && a.z == b.z; }
@@ -561,25 +417,14 @@ __device__ __forceinline__ void svm_descent(const SvArgs &A, const TrajView &tr,
     x = x0;
     g = have0 ? g0 : mk3(0, 0, 0); gq = have0 ? q0 : mk3(0, 0, 0);
     double fval = have0 ? f0 : 0.0;
-#ifdef ISDF_PHASE_TIMING
-    long long dt_mark = clock64();
-#define DT_ADD(i) do { if (threadIdx.x == 0) { const long long n_ = clock64(); S.dbg_t[i] += n_ - dt_mark; dt_mark = n_; } } while (0)
-#else
-#define DT_ADD(i) ((void)0)
-#endif
     while (iter < 300 && !stop && fabs(x - prev_x) > tol) {
-        DT_ADD(3);
         d3 xt, v, a, j;
         traj_pvaj(tr, x, xt, v, a, j);
         FlatState fs;
         flat_state(A.cfg.fp, v, a, j, fs);
         const rot3 R = quat_rot(flat_quat(fs));
         const d3 tmp = rot_applyT(R, p - xt);
-        DT_ADD(0);
         if (!(have && same_bits(tmp, gq))) {          // CTA-uniform: every thread computed the same tmp
-#ifdef ISDF_PHASE_TIMING
-            if (threadIdx.x == 0) S.dbg_requery++;
-#endif
             if (warp == 0) {
                 d3 g0 = mk3(0, 0, 0);
                 const double f0 = mesh_sdf_grad_warp_lat(M, tmp, 1e300, g0, lane, stk);
@@ -589,7 +434,6 @@ __device__ __forceinline__ void svm_descent(const SvArgs &A, const TrajView &tr,
             fval = S.bc[0]; g = mk3(S.bc[1], S.bc[2], S.bc[3]); gq = tmp; have = true;
             __syncthreads();
         }
-        DT_ADD(1);
         if (iter == 0) { fx = fval; if (warp == 0) nevals++; }
         const d3 omg = flat_omega(fs);
         const d3 rv = rot_applyT(R, v), wx = cross3(omg, tmp);
@@ -598,9 +442,6 @@ __device__ __forceinline__ void svm_descent(const SvArgs &A, const TrajView &tr,
         prev_x = x;
         bool accepted = false;
         for (int b0 = 1; b0 < 10 && !accepted; b0 += SVM_WARPS) {
-#ifdef ISDF_PHASE_TIMING
-            if (threadIdx.x == 0) S.dbg_rounds++;
-#endif
             const int mydiv = b0 + warp;
             if (mydiv < 10) {
                 double tau = alpha;
@@ -615,7 +456,6 @@ __device__ __forceinline__ void svm_descent(const SvArgs &A, const TrajView &tr,
                     S.cand_q[mydiv - 1][0] = qc.x; S.cand_q[mydiv - 1][1] = qc.y; S.cand_q[mydiv - 1][2] = qc.z;
                 }
             }
-            DT_ADD(2);
             __syncthreads();
             const int dend = min(b0 + SVM_WARPS, 10);
             for (int div = b0; div < dend; div++) {      // the reference's sequential loop over the halvings
@@ -663,25 +503,12 @@ __device__ __forceinline__ void sv_points_cta_body(const SvArgs &A, const int bx
     d3 grel = mk3(0, 0, 0);
     unsigned nevals = 0;      // per warp; lane 0 of every warp adds its share to the counter
     bool found = false;
-#ifdef ISDF_PHASE_TIMING
-    if (threadIdx.x == 0) { S.dbg_rounds = 0; S.dbg_exact = 0; S.dbg_requery = 0; S.dbg_t[0] = S.dbg_t[1] = S.dbg_t[2] = S.dbg_t[3] = 0; }
-    __syncthreads();
-    const long long pt_begin = clock64();
-    long long pt_coarse = 0, pt_p1 = 0, pt_p2 = 0, pt_gd = 0, pt_mark = 0;
-    unsigned pt_intervals = 0;
-#define PT_MARK() (pt_mark = clock64())
-#define PT_ADD(acc) ((acc) += clock64() - pt_mark)
-#else
-#define PT_MARK() ((void)0)
-#define PT_ADD(acc) ((void)0)
-#endif
 
     if (A.g_t) {
         sdf_value = A.g_s[pk]; tstar = A.g_t[pk]; grel = mk3(A.g_g[3 * pk], A.g_g[3 * pk + 1], A.g_g[3 * pk + 2]);
         found = true;
     } else {
         // ---- coarse scan (swm:392-421): in-range bitmap; the cell bracket settles all but a thin band around `inf` ---------
-        PT_MARK();
         // consecutive samples go to different warps (an obstacle point's undecided samples — the thin band around `inf` — are
         // consecutive in time and each costs a cooperative search: spread, they run on all warps at once)
         for (int w = tid; w < SV_FLAG_WORDS; w += SVM_THREADS) S.flags[w] = 0u;
@@ -710,7 +537,6 @@ __device__ __forceinline__ void sv_points_cta_body(const SvArgs &A, const int bx
             if (in) atomicOr(&S.flags[k >> 5], 1u << (k & 31));
         }
         __syncthreads();
-        PT_ADD(pt_coarse);
         if (warp == 0) nevals += nc;
         const uint32_t *fl = S.flags;
         const int nwords = (nc + 31) >> 5;
@@ -761,7 +587,6 @@ __device__ __forceinline__ void sv_points_cta_body(const SvArgs &A, const int bx
                 // bound exceeds the smallest cell upper bound of the interval cannot be that sample: pass 1 brackets every
                 // sample from the cell grid (no search), pass 2 runs the exact search on the survivors only.
                 const int first = lane * SVM_WARPS + warp;      // sample index of this thread in a round of SVM_THREADS
-                PT_MARK();
                 double cut = 1e300;
                 if (MESH) {
                     double t = lb;
@@ -778,8 +603,6 @@ __device__ __forceinline__ void sv_points_cta_body(const SvArgs &A, const int bx
                     for (int w = 1; w < SVM_WARPS; w++) cut = fmin(cut, S.red_d[w]);
                     __syncthreads();
                 }
-                PT_ADD(pt_p1);
-                PT_MARK();
                 bool seed_have = false; double seed_f = 0.0; d3 seed_g = mk3(0, 0, 0), seed_q = mk3(0, 0, 0);
                 {
                     double t = lb;
@@ -798,9 +621,6 @@ __device__ __forceinline__ void sv_points_cta_body(const SvArgs &A, const int bx
                                 mesh_bracket(M, prel, blo, bhi);
                                 need = blo <= cut;
                             }
-#ifdef ISDF_PHASE_TIMING
-                            if (need) atomicAdd(&S.dbg_exact, 1u);
-#endif
                             d3 gl = mk3(0, 0, 0);
                             dis = mesh_sdf_each(M, need, prel, inf, 1e300, lane, stk, &gl);
                             if (dis < bd) { double *bg = S.bestg[warp][lane]; bg[0] = gl.x; bg[1] = gl.y; bg[2] = gl.z; bg[3] = prel.x; bg[4] = prel.y; bg[5] = prel.z; }
@@ -832,8 +652,6 @@ __device__ __forceinline__ void sv_points_cta_body(const SvArgs &A, const int bx
                     __syncthreads();
                     if (bd < range_mindis) { range_mindis = bd; range_time_seed = bt; }
                 }
-                PT_ADD(pt_p2);
-                PT_MARK();
                 // ---- descent inside the interval (swm:730-734) ---------------------------------------------------------
                 const double tmin_ = fmax(0.0, lb), tmax_ = fmin(ub, dur);
                 double sdf_star = 1e1, t_star = 0;
@@ -849,10 +667,6 @@ __device__ __forceinline__ void sv_points_cta_body(const SvArgs &A, const int bx
                     __syncthreads();
                 }
                 if (sdf_star < min_sdf_star) { min_sdf_star = sdf_star; tstar = t_star; found = true; g_best = g_s; q_best = q_s; }
-                PT_ADD(pt_gd);
-#ifdef ISDF_PHASE_TIMING
-                pt_intervals++;
-#endif
                 pos = kout;
             }
             if (found) {
@@ -873,14 +687,6 @@ __device__ __forceinline__ void sv_points_cta_body(const SvArgs &A, const int bx
             }
         }
     }
-#ifdef ISDF_PHASE_TIMING
-    if (A.dbg && tid == 0) {
-        unsigned long long *o = A.dbg + 8 * (size_t)pk;
-        o[0] = (unsigned long long)(clock64() - pt_begin); o[1] = pt_coarse; o[2] = pt_p1; o[3] = pt_p2; o[4] = pt_gd;
-        o[5] = pt_intervals | ((unsigned long long)S.dbg_requery << 16); o[6] = S.dbg_exact; o[7] = S.dbg_rounds;
-        if (A.dbg2) { unsigned long long *o2 = A.dbg2 + 4 * (size_t)pk; for (int q = 0; q < 4; q++) o2[q] = (unsigned long long)S.dbg_t[q]; }
-    }
-#endif
     if (lane == 0 && A.counter && nevals) atomicAdd(A.counter, (unsigned long long)nevals);
     if (tid == 0) sv_point_tail(A, sC, tr, pk, p, found, tstar, sdf_value, grel);
     if (tid == 0 && A.work) A.work[pk] = (unsigned)min((clock64() - work_begin) >> 4, 0xffffffffll);
@@ -972,14 +778,12 @@ __device__ __forceinline__ void sv_make_view(const SvBatch &Bt, int b, SvArgs &V
         V.partial = Bt.base.partial + (size_t)p0 * PARTIAL_STRIDE; V.piece = Bt.base.piece + p0;
         V.piece_gdt = Bt.base.piece_gdt + (size_t)b * N; V.piece_cost = Bt.base.piece_cost + (size_t)b * N;
         V.out = Bt.base.out + (size_t)b * Bt.out_stride;
-        if (V.dbg) V.dbg = Bt.base.dbg + (size_t)8 * p0;
     }
     __syncthreads();
 }
 static_assert(sizeof(SvArgs) % 8 == 0, "SvArgs is copied as 64-bit words");
 
 __global__ void __launch_bounds__(256) k_sv_table(const __grid_constant__ SvArgs A) { sv_table_body(A, blockIdx.x); }
-__global__ void __launch_bounds__(SV_THREADS) k_sv_points(const __grid_constant__ SvArgs A) { sv_points_body(A, blockIdx.x); }
 template <bool MESH>
 __global__ void __launch_bounds__(SVM_THREADS) k_sv_points_cta(const __grid_constant__ SvArgs A) { sv_points_cta_body<MESH>(A, blockIdx.x); }
 __global__ void __launch_bounds__(256) k_sv_reduce(const __grid_constant__ SvArgs A) { if ((int)blockIdx.x == A.N) sv_order_body(A); else sv_reduce_body(A, blockIdx.x); }
@@ -1000,11 +804,10 @@ struct SweptState {
     // for problem b of the batched callback — separate, so that neither path sees the other's trajectories
     DevBuf<double> d_pts, d_tstar, d_sdf, d_grel, d_times, d_poses, d_state, d_state_b, d_partial, d_piece_gdt, d_piece_cost;
     DevBuf<int> d_piece, d_meta;
-    DevBuf<unsigned long long> d_counter, d_dbg;
+    DevBuf<unsigned long long> d_counter;
     DevBuf<unsigned> d_work; DevBuf<int> d_order;
     bool order_ready = false; int order_rank = -1, order_world = -1;
     double *count_out = nullptr;   // set by the host entry point around one launch
-    bool dbg_on = false;
 
     // the only place that replaces the point set: it gives up the current one (and any per-problem sets: set_points_batch sets B
     // after it) before it touches the buffers
@@ -1057,12 +860,6 @@ struct SweptState {
         const bool record = (g_t == nullptr) && shape.kind == ISDF_SHAPE_MESH;
         if (order_rank != rank || order_world != world) { order_ready = false; order_rank = rank; order_world = world; }
         A.work = record ? d_work.p : nullptr; A.order = d_order.p; A.use_order = (record && order_ready) ? 1 : 0;
-        A.dbg = nullptr; A.dbg2 = nullptr;
-        if (dbg_on) {
-            if ((e = d_dbg.ensure((size_t)12 * P)) != cudaSuccess) return e;
-            if ((e = cudaMemsetAsync(d_dbg.p, 0, sizeof(unsigned long long) * 12 * P, st)) != cudaSuccess) return e;
-            A.dbg = d_dbg.p; A.dbg2 = d_dbg.p + 8 * (size_t)P;
-        }
         const size_t sm = sizeof(double) * 19 * (size_t)N;
         if (sm > 200 * 1024) return cudaErrorInvalidValue;
         if ((e = cudaMemsetAsync(d_counter.p, 0, sizeof(unsigned long long), st)) != cudaSuccess) return e;
@@ -1070,20 +867,17 @@ struct SweptState {
             cudaFuncSetAttribute(k_sv_table, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
             cudaFuncSetAttribute(k_sv_points_cta<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
             cudaFuncSetAttribute(k_sv_points_cta<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-            cudaFuncSetAttribute(k_sv_points, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
         }
         k_sv_table<<<SV_TABLE_CTAS, SV_TABLE_THREADS, sm, st>>>(A);
         const int Mloc = (P - rank + world - 1) / world;
-        const unsigned grid = (unsigned)((Mloc + SV_WARPS - 1) / SV_WARPS);
-        if (grid > 0) {
+        if (Mloc > 0) {
             if (shape.kind == ISDF_SHAPE_MESH) k_sv_points_cta<true><<<(unsigned)Mloc, SVM_THREADS, sm, st>>>(A);
-            else if (SV_ANALYTIC_CTA) k_sv_points_cta<false><<<(unsigned)Mloc, SVM_THREADS, sm, st>>>(A);
-            else k_sv_points<<<grid, SV_THREADS, sm, st>>>(A);
+            else k_sv_points_cta<false><<<(unsigned)Mloc, SVM_THREADS, sm, st>>>(A);
         }
-        k_sv_reduce<<<N + ((record && grid > 0) ? 1 : 0), 256, 0, st>>>(A);   // + one CTA that sorts the points for the next evaluation
-        if (record && grid > 0) order_ready = true;
+        k_sv_reduce<<<N + ((record && Mloc > 0) ? 1 : 0), 256, 0, st>>>(A);   // + one CTA that sorts the points for the next evaluation
+        if (record && Mloc > 0) order_ready = true;
         k_sv_finish<<<1, 32, 0, st>>>(A);
-        *launches = 3 + (grid > 0 ? 1 : 0);
+        *launches = 3 + (Mloc > 0 ? 1 : 0);
         return cudaGetLastError();
     }
     // ---- batched: B problems, each with its own obstacle point set (concatenated; offsets), its own trajectory (T: B x N, C: B x 18N,
@@ -1123,7 +917,7 @@ struct SweptState {
         A.cfg = cfg; A.shape = shape; A.N = N; A.T = d_T; A.C = d_Cpp; A.P = 0; A.pts = d_pts.p;
         A.tstar = d_tstar.p; A.sdf = d_sdf.p; A.grel = d_grel.p; A.times = d_times.p; A.poses = d_poses.p; A.meta = d_meta.p;
         A.state = d_state_b.p; A.partial = d_partial.p; A.piece = d_piece.p; A.piece_gdt = d_piece_gdt.p; A.piece_cost = d_piece_cost.p;
-        A.out = d_out; A.counter = d_counter.p; A.count_out = nullptr; A.rank = 0; A.world = 1; A.g_t = nullptr; A.g_s = nullptr; A.g_g = nullptr; A.dbg = nullptr; A.dbg2 = nullptr;
+        A.out = d_out; A.counter = d_counter.p; A.count_out = nullptr; A.rank = 0; A.world = 1; A.g_t = nullptr; A.g_s = nullptr; A.g_g = nullptr;
         A.work = nullptr; A.order = nullptr; A.use_order = 0;
         Bt.B = B; Bt.pt_off = d_off.p; Bt.out_stride = 19ll * N + 1;
         const size_t sm = sizeof(double) * 19 * (size_t)N;

@@ -9,7 +9,7 @@ import os
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("ISDF_B200_LIB") or os.path.join(os.path.dirname(_HERE), "libisdf_b200.so")  # env override: A/B builds
+LIB_PATH = os.path.join(os.path.dirname(_HERE), "libisdf_b200.so")
 
 # isdf_shape_kind (include/isdf.h)
 SHAPE_KINDS = dict(BALL=0, POINT=1, TORUS=2, CAPPED_TORUS=3, CAPPED_CONE=4, ROUNDED_CONE=5, WIREFRAME_BOX=6,

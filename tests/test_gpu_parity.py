@@ -658,36 +658,80 @@ def test_frontend_state_errors():
     ev.close()
 
 
-@pytest.mark.gpu
-def test_frontend_two_pass_equals_one_pass_ragged_z():
-    """the two-pass feasibility kernels (kernel core first, mask accumulation on the survivors) against the one-pass kernel and the
-    oracle, on a map whose z extent is not a multiple of the z-run length and that is dense enough for the core to settle most voxels"""
-    import os
-    cfg, _, _, _, _ = small_case(N=2, K=4, seed=3, kernel_size=7)
+def _fe_table_bytes(K):
+    """shared memory of the pattern tables isdf_frontend_build_kernels makes from the kernels K (attitude, a, b, c): per union row (a, b),
+    chunks of <= 8 offsets along c from its first to its last occupied one, all-zero chunks skipped; 16 B x 2^len per chunk + 16 B"""
+    union = K.any(axis=0)
+    total = 0
+    for a in range(union.shape[0]):
+        for b in range(union.shape[1]):
+            occ = np.flatnonzero(union[a, b])
+            if occ.size == 0:
+                continue
+            for c0 in range(occ[0], occ[-1] + 1, 8):
+                n = min(8, occ[-1] - c0 + 1)
+                if union[a, b, c0:c0 + n].any():
+                    total += 16 * 2 ** n + 16
+    return total
+
+
+FE_PIPELINES = {
+    # name: (robot, kernel size, front_end_safeh); the input alone selects the pipeline (precondition asserted below)
+    "tables": ("mesh", 7, 0.8),                # the rounded-cone mesh: kernel core, tables of ~22 KB -> core words + table-driven survivors
+    "no_tables": ("bigbox", 9, 0.0),           # a box of half extents 4, 4, 0.6 m: tables of ~241 KB > 200 KB -> core per z-run + offset-mask survivors
+    "one_pass": ("Cappedtorus", 13, 0.0),      # an open ring: no voxel is occupied in every attitude (empty core) -> one-pass kernel
+}
+
+
+def _check_fe_pipeline(pipeline):
+    import frontpath_oracle as FO
+    robot, ks, safeh = FE_PIPELINES[pipeline]
+    cfg, _, _, _, _ = small_case(N=2, K=4, seed=3, kernel_size=ks)
+    res = cfg.occupancy_resolution
     X, Y, Z = 37, 29, 43                                   # z: one full 32-voxel word + a ragged one, not a multiple of the run length
     occ = W.random_map(X, Y, Z, p=0.04, seed=9, slabs=1)
-    V, F = MESHES["rcone"]()
-    poly = [0.1, 0.0, -0.1, 120.0, 10.0, 0.0]
     ev = I.Evaluator(cfg)
-    ev.set_map_u8(occ, [0, 0, 0], cfg.occupancy_resolution)
-    ev.set_shape_mesh(V, F, poly)
-    ev.frontend_build_kernels(45.0, 45.0, 9.0, 0.8)
-    two = ev.frontend_feasibility(X, Y, Z)                 # zero fill + bit-parallel core pass + table-driven accumulation
-    os.environ["ISDF_FE_NO_TABLES"] = "1"
-    try:
-        two_b = ev.frontend_feasibility(X, Y, Z)           # core pass per z-run + offset-mask accumulation
-    finally:
-        del os.environ["ISDF_FE_NO_TABLES"]
-    os.environ["ISDF_FE_ONE_PASS"] = "1"
-    try:
-        one = ev.frontend_feasibility(X, Y, Z)
-    finally:
-        del os.environ["ISDF_FE_ONE_PASS"]
-    assert np.array_equal(one, two) and np.array_equal(one, two_b)
-    fe = O.FrontEnd(O.Shape.mesh(V, F, poly), occ, ks=7, res=cfg.occupancy_resolution, front_end_safeh=0.8)
+    ev.set_map_u8(occ, [0, 0, 0], res)
+    if robot == "mesh":
+        V, F = MESHES["rcone"]()
+        poly = [0.1, 0.0, -0.1, 120.0, 10.0, 0.0]
+        ev.set_shape_mesh(V, F, poly); osh = O.Shape.mesh(V, F, poly)
+    elif robot == "bigbox":
+        ext = [4.0, 4.0, 0.6]
+        ev.set_shape_analytic(I.SHAPE_KINDS["BOX"], ext); osh = O.Shape.analytic(I.SHAPE_KINDS["BOX"], ext)
+    else:
+        ev.set_shape_named(robot); osh = O.Shape.named(robot)
+    ev.frontend_build_kernels(45.0, 45.0, 9.0, safeh)
+    fe = O.FrontEnd(osh, occ, ks=ks, res=res, front_end_safeh=safeh)
+    K = fe.kernels()
+    assert np.array_equal(ev.frontend_kernels(ks), K), f"{pipeline}: kernels differ"
+    # precondition: the input selects the pipeline this case is about
+    assert K.astype(bool).all(axis=0).any() == (pipeline != "one_pass"), f"{pipeline}: kernel core"   # offsets every attitude occupies
+    if pipeline != "one_pass":
+        assert (_fe_table_bytes(K.astype(bool)) > 200 * 1024) == (pipeline == "no_tables"), f"{pipeline}: table size"
+    before = ev.stats().kernel_launches
+    masks = ev.frontend_feasibility(X, Y, Z)
+    assert ev.stats().kernel_launches - before == (1 if pipeline == "one_pass" else 2), f"{pipeline}: launch count"
     ix, iy, iz = np.meshgrid(np.arange(X), np.arange(Y), np.arange(Z), indexing="ij")
     ref = fe.feasibility(np.stack([ix, iy, iz], -1).reshape(-1, 3))
-    assert np.array_equal(two, ref)
-    settled = (two == 0).all(axis=1).mean()
-    assert 0.05 < settled < 1.0
+    assert np.array_equal(masks, ref), f"{pipeline}: {(masks != ref).any(axis=1).sum()} voxels differ"
+    if pipeline != "one_pass":
+        settled = (masks == 0).all(axis=1).mean()
+        assert 0.05 < settled < 1.0, f"{pipeline}: settled fraction {settled}"
+    # the bit output: the path search runs the same pipeline into the traversability grid
+    trav = FO.traversable(occ, ref)
+    assert trav.any() and not trav.all(), f"{pipeline}: degenerate traversability"
+    cand = np.argwhere(trav)
+    ev.frontend_path((cand[0] + 0.5) * res, (cand[-1] + 0.5) * res)
+    assert np.array_equal(ev.dbg_frontpath_traversable(), trav), f"{pipeline}: traversability grid differs"
     ev.close()
+
+
+@pytest.mark.gpu
+def test_frontend_two_pass_equals_one_pass_ragged_z():
+    """the two-pass feasibility pipelines (kernel core first, mask accumulation on the survivors, with or without pattern tables) and the
+    one-pass kernel, each reached through the input that selects it, against the oracle on a map whose z extent is not a multiple of the
+    z-run length (4) or of the 32-voxel word: the masks bit for bit, and the traversability grid the path search builds from the same
+    pipeline's bit output"""
+    for pipeline in FE_PIPELINES:
+        _check_fe_pipeline(pipeline)
