@@ -8,6 +8,7 @@
 #include "isdf_frontend.cuh"
 #include "isdf_frontpath.cuh"
 #include "isdf_lbfgs.cuh"
+#include "isdf_midend.cuh"
 #include "isdf_clearance.cuh"
 #include "isdf_map.cuh"
 #include <queue>
@@ -86,10 +87,14 @@ struct isdf_ctx {
         DevBuf<double> d_x, d_bc, d_T, d_C, d_lu, d_energy, d_gC, d_gT, d_cost, d_grad, d_out, d_Cpp, d_sv;
         int B = 0, N0 = 0;
     } batch;
-    struct {   // device-resident lock-step L-BFGS (isdf_lbfgs.cuh)
+    struct LbfgsBufs {   // device-resident lock-step L-BFGS (isdf_lbfgs.cuh)
         DevBuf<double> d_x, d_f, d_grad, d_state; DevBuf<int> d_int, d_head;
         PinnedBuf<int> h_active;
     } lbfgs;
+    struct {   // mid-end (isdf_midend.cuh): buffers of its own, so that no mid-end call touches the back end's batch, swept or L-BFGS state
+        DevBuf<double> d_x, d_bc, d_wp, d_T, d_C, d_lu, d_energy, d_gC, d_gT, d_out, d_pc, d_cost, d_grad;
+        LbfgsBufs lb;
+    } mid;
     SweptState sv;   // swept volume
     struct {   // front end attitude kernels (isdf_frontend.cuh)
         bool ready = false;
@@ -1047,7 +1052,7 @@ static int callback_batch_launch(isdf_ctx *c, int B, int N0, const double *d_hea
     MincoArgs M;
     M.B = B; M.N = N0; M.x = d_x; M.head = d_head; M.tail = d_tail; M.bc_stride = bc_stride; M.rho = rho;
     M.T = c->batch.d_T.p; M.C = c->batch.d_C.p; M.lu = c->batch.d_lu.p; M.energy = c->batch.d_energy.p; M.gC_e = c->batch.d_gC.p; M.gT_e = c->batch.d_gT.p;
-    M.disc_out = nullptr; M.piece_cost = nullptr; M.cost = d_cost; M.grad = d_grad;
+    M.disc_out = nullptr; M.piece_cost = nullptr; M.cost = d_cost; M.grad = d_grad; M.seq_terms = 0;
     // per-problem obstacle point sets registered for exactly this batch (isdf_set_points_batch): the LIVE composition of costFunctionLmbm
     // (hpp:386-405) — swept-volume term, then time-integral term
     const bool with_swept = (c->sv.B == B);
@@ -1153,34 +1158,31 @@ extern "C" int isdf_lbfgs_default_params(isdf_lbfgs_params *p) {
     return 0;
 }
 
+// The lock-step rounds of isdf_lbfgs_batch_device and isdf_midend_batch_device: every round `eval(d_x, d_f, d_grad)` evaluates the point
+// every instance requested (finished instances ride along unchanged: their state is frozen), then one k_lbfgs_feed consumes the results.
 // d_x: B x n (in: starting points, out: solutions); d_f: B; d_ret / d_iterations / d_evaluations: B ints (any of the three may be null).
 // Synchronous with respect to the host (one 4-byte read per round decides termination), all data stays on the device.
-extern "C" int isdf_lbfgs_batch_device(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc, double rho,
-                                       const isdf_lbfgs_params *prm, double *d_x, double *d_f, int *d_ret, int *d_iterations, int *d_evaluations,
-                                       int *rounds_out, void *cuda_stream) {
-    int r = callback_batch_check(c, B, N0);
-    if (r) return r;
-    if ((r = lbfgs_check(prm))) return r;
-    if (!d_head || !d_tail || !d_x || !d_f) return fail(ISDF_ERR_INVALID, "NULL device pointer");
-    if (set_device(c)) return ISDF_ERR_CUDA;
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    const int n = 4 * N0 - 3, m = prm->mem_size, npf = prm->past > 1 ? prm->past : 1;
+template <typename Eval>
+static int lbfgs_rounds(isdf_ctx *c, isdf_ctx::LbfgsBufs &lb, int B, int n, const isdf_lbfgs_params *prm, int cancel_after, double *d_x, double *d_f,
+                        int *d_ret, int *d_iterations, int *d_evaluations, int *rounds_out, cudaStream_t st, Eval eval) {
+    const int m = prm->mem_size, npf = prm->past > 1 ? prm->past : 1;
     const size_t per = (size_t)4 * n + npf + 2 * (size_t)m + 2 * (size_t)m * n + LB_NSCALAR;   // doubles of state per instance
-    CU_TRY(c->lbfgs.d_state.ensure(per * B)); CU_TRY(c->lbfgs.d_grad.ensure((size_t)B * n)); CU_TRY(c->lbfgs.d_int.ensure((size_t)B * LB_NINT + 4));
-    CU_TRY(c->lbfgs.h_active.ensure(1));
-    CU_TRY(cudaMemsetAsync(c->lbfgs.d_state.p, 0, sizeof(double) * per * B, st));
-    CU_TRY(cudaMemsetAsync(c->lbfgs.d_int.p, 0, sizeof(int) * ((size_t)B * LB_NINT + 4), st));   // phase = WANT_INIT
+    CU_TRY(lb.d_state.ensure(per * B)); CU_TRY(lb.d_grad.ensure((size_t)B * n)); CU_TRY(lb.d_int.ensure((size_t)B * LB_NINT + 4));
+    CU_TRY(lb.h_active.ensure(1));
+    CU_TRY(cudaMemsetAsync(lb.d_state.p, 0, sizeof(double) * per * B, st));
+    CU_TRY(cudaMemsetAsync(lb.d_int.p, 0, sizeof(int) * ((size_t)B * LB_NINT + 4), st));   // phase = WANT_INIT
     LbfgsArgs L;
     L.B = B; L.n = n;
     L.pr.mem_size = m; L.pr.past = prm->past; L.pr.max_iterations = prm->max_iterations; L.pr.max_linesearch = prm->max_linesearch;
     L.pr.g_epsilon = prm->g_epsilon; L.pr.delta = prm->delta; L.pr.min_step = prm->min_step; L.pr.max_step = prm->max_step;
     L.pr.f_dec_coeff = prm->f_dec_coeff; L.pr.cautious_factor = prm->cautious_factor; L.pr.machine_prec = prm->machine_prec;
-    double *p = c->lbfgs.d_state.p;
-    L.x = d_x; L.f = d_f; L.grad = c->lbfgs.d_grad.p;
+    L.pr.cancel_after = cancel_after;
+    double *p = lb.d_state.p;
+    L.x = d_x; L.f = d_f; L.grad = lb.d_grad.p;
     L.xp = p; p += (size_t)B * n; L.g = p; p += (size_t)B * n; L.gp = p; p += (size_t)B * n; L.d = p; p += (size_t)B * n;
     L.pf = p; p += (size_t)B * npf; L.alpha = p; p += (size_t)B * m; L.ys = p; p += (size_t)B * m;
     L.S = p; p += (size_t)B * m * n; L.Y = p; p += (size_t)B * m * n; L.sc = p;
-    L.st = c->lbfgs.d_int.p; L.active = c->lbfgs.d_int.p + (size_t)B * LB_NINT;
+    L.st = lb.d_int.p; L.active = lb.d_int.p + (size_t)B * LB_NINT;
     // olddnorm starts at 1 (lbfgs.hpp:541): scalar slot 2 of every instance
     {
         std::vector<double> init((size_t)B * LB_NSCALAR, 0.0);
@@ -1190,17 +1192,15 @@ extern "C" int isdf_lbfgs_batch_device(isdf_ctx *c, int B, int N0, const double 
     }
     int rounds = 0;
     for (;;) {
-        // every instance's requested point is evaluated (finished instances ride along unchanged: their state is frozen)
-        r = callback_batch_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, rho, d_x, d_f, c->lbfgs.d_grad.p, st);
-        if (r) return r;
+        if (int r = eval(d_x, d_f, lb.d_grad.p)) return r;
         CU_TRY(cudaMemsetAsync(L.active, 0, sizeof(int), st));
         k_lbfgs_feed<<<(unsigned)((B + 63) / 64), 64, 0, st>>>(L);
         c->stats.kernel_launches++;
         CU_TRY(cudaGetLastError());
-        CU_TRY(cudaMemcpyAsync(c->lbfgs.h_active.p, L.active, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(lb.h_active.p, L.active, sizeof(int), cudaMemcpyDeviceToHost, st));
         CU_TRY(cudaStreamSynchronize(st));
         ++rounds;
-        if (*c->lbfgs.h_active.p == 0) break;
+        if (*lb.h_active.p == 0) break;
         if (prm->max_rounds > 0 && rounds >= prm->max_rounds) break;
     }
     // results: f = fx of every instance (scalar slot 0), return codes and counters
@@ -1211,6 +1211,21 @@ extern "C" int isdf_lbfgs_batch_device(isdf_ctx *c, int B, int N0, const double 
     CU_TRY(cudaStreamSynchronize(st));
     if (rounds_out) *rounds_out = rounds;
     return 0;
+}
+
+extern "C" int isdf_lbfgs_batch_device(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc, double rho,
+                                       const isdf_lbfgs_params *prm, double *d_x, double *d_f, int *d_ret, int *d_iterations, int *d_evaluations,
+                                       int *rounds_out, void *cuda_stream) {
+    int r = callback_batch_check(c, B, N0);
+    if (r) return r;
+    if ((r = lbfgs_check(prm))) return r;
+    if (!d_head || !d_tail || !d_x || !d_f) return fail(ISDF_ERR_INVALID, "NULL device pointer");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    return lbfgs_rounds(c, c->lbfgs, B, 4 * N0 - 3, prm, 0, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st,
+                        [&](const double *x, double *f, double *g) {
+                            return callback_batch_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, rho, x, f, g, st);
+                        });
 }
 
 extern "C" int isdf_lbfgs_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc, double rho,
@@ -1245,6 +1260,203 @@ extern "C" int isdf_get_batch_trajectories(isdf_ctx *c, double *T, double *coeff
     if (coeffs) CU_TRY(cudaMemcpy(coeffs, c->batch.d_C.p, sizeof(double) * 18 * BN, cudaMemcpyDeviceToHost));
     if (energy) CU_TRY(cudaMemcpy(energy, c->batch.d_energy.p, sizeof(double) * c->batch.B, cudaMemcpyDeviceToHost));
     return 0;
+}
+
+// ---- mid-end: waypoint selection and getOriTraj for B paths (isdf_midend.cuh) ------------------------------------------------------------
+extern "C" int isdf_path_waypoints(int B, const int32_t *path_off, const double *path_xyz, double res, double parlength, int cap,
+                                   double *waypoints, int32_t *wp_off, int32_t *pieces) {
+    if (B < 1 || !path_off || !path_xyz || !wp_off || !pieces || cap < 0 || (cap > 0 && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument, B < 1 or cap < 0");
+    if (!(std::isfinite(res) && res > 0.0) || !(std::isfinite(parlength) && parlength > 0.0)) return fail(ISDF_ERR_INVALID, "res and parlength must be finite and positive");
+    if (path_off[0] != 0) return fail(ISDF_ERR_INVALID, "path_off[0] must be 0");
+    for (int b = 0; b < B; b++) if (path_off[b + 1] <= path_off[b]) return fail(ISDF_ERR_INVALID, "every path needs at least one node (path_off must increase)");
+    long long total = 0;
+    wp_off[0] = 0;
+    for (int b = 0; b < B; b++) {
+        const long long S = path_off[b + 1] - path_off[b];
+        const double *path = path_xyz + 3 * (size_t)path_off[b];
+        long long n = 0;
+        if (S > 2) {   // plan_manager.cpp:206-213 and :235-245; S <= 2 would not terminate in the reference (include/isdf.h)
+            double pl = parlength;
+            double gap = std::ceil(pl / res);
+            while (gap >= (double)(S - 1)) { pl /= 1.5; gap = std::ceil(pl / res); }
+            const long long g = (long long)gap;
+            for (long long ind = g; ind < S - 1; ind += g, n++)
+                if (total + n < cap) for (int k = 0; k < 3; k++) waypoints[3 * (total + n) + k] = path[3 * ind + k];
+        }
+        total += n;
+        if (total > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "too many waypoints");
+        wp_off[b + 1] = (int32_t)total;
+        pieces[b] = (int32_t)(n + 1);
+    }
+    if (total > cap) return fail(ISDF_ERR_INVALID, "cap smaller than the number of waypoints (wp_off reports it)");
+    return 0;
+}
+
+extern "C" int isdf_midend_default_params(isdf_midend_params *p) {
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    // config_CappedCone.yaml: weight_pr 1000, rho_mid_end 200, inittime 2.5; earlyExit's k > 8e3 (mid_end.hpp:630)
+    p->weight_pr = 1000.0; p->rho = 200.0; p->init_time = 2.5; p->cancel_after = 8000; p->reserved_ = 0;
+    isdf_lbfgs_default_params(&p->lbfgs);
+    p->lbfgs.max_iterations = 100000;   // mid_end.cpp:53; delta = relCostTolMidEnd 1e-6 (:54), the rest as the back end's
+    return 0;
+}
+
+static int midend_check(isdf_ctx *c, int B, int N0, const isdf_midend_params *p) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (B < 1 || N0 < 1) return fail(ISDF_ERR_INVALID, "B < 1 or N0 < 1");
+    if ((long long)B * (4 * (long long)N0 - 3) > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "B*(4*N0-3) overflows");
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    if (p->reserved_ != 0) return fail(ISDF_ERR_INVALID, "reserved_ must be 0");
+    if (!(std::isfinite(p->weight_pr) && p->weight_pr >= 0.0) || !std::isfinite(p->rho) || !(std::isfinite(p->init_time) && p->init_time > 0.0) ||
+        p->cancel_after < 0)
+        return fail(ISDF_ERR_INVALID, "mid-end parameter out of range");
+    if (int r = lbfgs_check(&p->lbfgs)) return r;
+    if (minco_smem_bytes(N0) > 220 * 1024) return fail(ISDF_ERR_UNSUPPORTED, "pieces per problem too large for the shared-memory banded solver (N0 <= 290)");
+    if (c->world != 1) return fail(ISDF_ERR_STATE, "the mid-end shards by PROBLEM: keep isdf_set_shard(ctx, 0, 1) and give each rank its own problems");
+    return 0;
+}
+
+static MincoArgs midend_minco_args(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int bc_stride, double rho, const double *d_x) {
+    MincoArgs M;
+    M.B = B; M.N = N0; M.x = d_x; M.head = d_head; M.tail = d_tail; M.bc_stride = bc_stride; M.rho = rho;
+    M.T = c->mid.d_T.p; M.C = c->mid.d_C.p; M.Cpp = nullptr; M.sv_out = nullptr; M.lu = c->mid.d_lu.p; M.energy = c->mid.d_energy.p;
+    M.gC_e = c->mid.d_gC.p; M.gT_e = c->mid.d_gT.p; M.disc_out = c->mid.d_out.p; M.piece_cost = c->mid.d_pc.p;
+    M.cost = nullptr; M.grad = nullptr; M.seq_terms = 1;
+    return M;
+}
+
+static int midend_buffers(isdf_ctx *c, int B, int N0) {
+    const size_t BN = (size_t)B * N0, smem = minco_smem_bytes(N0);
+    CU_TRY(c->mid.d_T.ensure(BN)); CU_TRY(c->mid.d_C.ensure(18 * BN)); CU_TRY(c->mid.d_lu.ensure(78 * BN)); CU_TRY(c->mid.d_energy.ensure(B));
+    CU_TRY(c->mid.d_gC.ensure(18 * BN)); CU_TRY(c->mid.d_gT.ensure(BN)); CU_TRY(c->mid.d_out.ensure(19 * BN + 1)); CU_TRY(c->mid.d_pc.ensure(BN));
+    CU_TRY(cudaFuncSetAttribute(k_minco_forward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CU_TRY(cudaFuncSetAttribute(k_minco_backward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    return 0;
+}
+
+// one evaluation of OriTraj::costFunction for all B problems: MINCO forward -> pose term -> adjoint with the terms added one at a time
+static int midend_eval_launch(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int bc_stride, const isdf_midend_params *p,
+                              const double *d_wp, const double *d_x, double *d_cost, double *d_grad, cudaStream_t st) {
+    const size_t BN = (size_t)B * N0, smem = minco_smem_bytes(N0);
+    MincoArgs M = midend_minco_args(c, B, N0, d_head, d_tail, bc_stride, p->rho, d_x);
+    M.cost = d_cost; M.grad = d_grad;
+    k_minco_forward<<<B, 32, smem, st>>>(M);
+    MidendArgs P;
+    P.B = B; P.N = N0; P.K = c->cfg.integral_intervs; P.weight = p->weight_pr; P.T = M.T; P.C = M.C; P.wp = d_wp; P.out = c->mid.d_out.p; P.piece_cost = c->mid.d_pc.p;
+    k_midend_pose<<<(unsigned)((BN + 127) / 128), 128, 0, st>>>(P);
+    k_minco_backward<<<B, 32, smem, st>>>(M);
+    c->stats.kernel_launches += 3;
+    CU_TRY(cudaGetLastError());
+    return 0;
+}
+
+// the mid-end's host entry points stage their inputs in c->mid: boundary conditions (*d_head, *d_tail) and waypoints
+static int midend_upload(isdf_ctx *c, int B, int N0, int per_problem_bc, const double *head, const double *tail, const double *waypoints,
+                         const double **d_head, const double **d_tail, const double **d_wp) {
+    const size_t nbc = per_problem_bc ? (size_t)9 * B : 9, nwp = (size_t)3 * B * (N0 - 1);
+    CU_TRY(c->mid.d_bc.ensure(2 * nbc)); CU_TRY(c->mid.d_wp.ensure(nwp > 0 ? nwp : 1));
+    CU_TRY(cudaMemcpyAsync(c->mid.d_bc.p, head, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
+    CU_TRY(cudaMemcpyAsync(c->mid.d_bc.p + nbc, tail, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
+    if (nwp) CU_TRY(cudaMemcpyAsync(c->mid.d_wp.p, waypoints, sizeof(double) * nwp, cudaMemcpyHostToDevice, c->stream));
+    *d_head = c->mid.d_bc.p; *d_tail = c->mid.d_bc.p + nbc; *d_wp = c->mid.d_wp.p;
+    return 0;
+}
+
+extern "C" int isdf_midend_callback_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc,
+                                          const isdf_midend_params *p, const double *waypoints, const double *x, double *cost, double *grad) {
+    auto poison_all = [&]() { if (cost && B > 0) for (int b = 0; b < B; b++) cost[b] = std::numeric_limits<double>::quiet_NaN(); };
+    int r = midend_check(c, B, N0, p);
+    if (r) { poison_all(); return r; }
+    if (!head || !tail || !x || !cost || !grad || (N0 > 1 && !waypoints)) { poison_all(); return fail(ISDF_ERR_INVALID, "NULL argument"); }
+    auto body = [&]() -> int {
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        const size_t dim = (size_t)4 * N0 - 3;
+        const double *d_head, *d_tail, *d_wp;
+        if (int rr = midend_upload(c, B, N0, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return rr;
+        CU_TRY(c->mid.d_x.upload(x, dim * B, c->stream));
+        CU_TRY(c->mid.d_cost.ensure(B)); CU_TRY(c->mid.d_grad.ensure(dim * B));
+        if (int rr = midend_buffers(c, B, N0)) return rr;
+        if (int rr = midend_eval_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, p, d_wp, c->mid.d_x.p, c->mid.d_cost.p, c->mid.d_grad.p, c->stream)) return rr;
+        CU_TRY(cudaMemcpyAsync(cost, c->mid.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaMemcpyAsync(grad, c->mid.d_grad.p, sizeof(double) * dim * B, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaStreamSynchronize(c->stream));
+        return 0;
+    };
+    r = body();
+    if (r) poison_all();
+    return r;
+}
+
+static int midend_batch_run(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc, const isdf_midend_params *p,
+                            const double *d_wp, double *d_x, double *d_T, double *d_coeffs, double *d_f, int *d_ret, int *d_iterations,
+                            int *d_evaluations, int *rounds_out, cudaStream_t st) {
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    const int n = 4 * N0 - 3;
+    const size_t BN = (size_t)B * N0;
+    if (int r = midend_buffers(c, B, N0)) return r;
+    // x = [backwardT(init_time) | waypoints] (mid_end.cpp:21-36; backwardT as back_end_optimizer.hpp:243-256)
+    const double T0 = p->init_time, tau0 = T0 > 1.0 ? (std::sqrt(2.0 * T0 - 1.0) - 1.0) : (1.0 - std::sqrt(2.0 / T0 - 1.0));
+    k_midend_init<<<(unsigned)(((size_t)B * n + 127) / 128), 128, 0, st>>>(B, N0, tau0, d_wp, d_x);
+    c->stats.kernel_launches++;
+    CU_TRY(cudaGetLastError());
+    const int bc_stride = per_problem_bc ? 9 : 0;
+    int r = lbfgs_rounds(c, c->mid.lb, B, n, &p->lbfgs, p->cancel_after, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st,
+                         [&](const double *x, double *f, double *g) { return midend_eval_launch(c, B, N0, d_head, d_tail, bc_stride, p, d_wp, x, f, g, st); });
+    if (r) return r;
+    // the final trajectories: forwardT + MINCO of the returned x (mid_end.cpp:65-71 / 79-85)
+    if (d_T || d_coeffs) {
+        MincoArgs M = midend_minco_args(c, B, N0, d_head, d_tail, bc_stride, p->rho, d_x);
+        k_minco_forward<<<B, 32, minco_smem_bytes(N0), st>>>(M);
+        c->stats.kernel_launches++;
+        CU_TRY(cudaGetLastError());
+        if (d_T) CU_TRY(cudaMemcpyAsync(d_T, M.T, sizeof(double) * BN, cudaMemcpyDeviceToDevice, st));
+        if (d_coeffs) CU_TRY(cudaMemcpyAsync(d_coeffs, M.C, sizeof(double) * 18 * BN, cudaMemcpyDeviceToDevice, st));
+        CU_TRY(cudaStreamSynchronize(st));
+    }
+    return 0;
+}
+
+extern "C" int isdf_midend_batch_device(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc,
+                                        const isdf_midend_params *p, const double *d_waypoints, double *d_x, double *d_T, double *d_coeffs,
+                                        double *d_f, int32_t *d_ret, int32_t *d_iterations, int32_t *d_evaluations, int32_t *rounds, void *cuda_stream) {
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    auto poison_all = [&]() { if (c && d_f && B > 0 && cudaSetDevice(c->device) == cudaSuccess) { cudaMemsetAsync(d_f, 0xff, sizeof(double) * B, st); cudaStreamSynchronize(st); } };
+    int r = midend_check(c, B, N0, p);
+    if (!r && (!d_head || !d_tail || !d_x || !d_f || (N0 > 1 && !d_waypoints))) r = fail(ISDF_ERR_INVALID, "NULL device pointer");
+    if (!r) r = midend_batch_run(c, B, N0, d_head, d_tail, per_problem_bc, p, d_waypoints, d_x, d_T, d_coeffs, d_f, d_ret, d_iterations, d_evaluations, rounds, st);
+    if (r) poison_all();
+    return r;
+}
+
+extern "C" int isdf_midend_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc,
+                                 const isdf_midend_params *p, const double *waypoints, double *x, double *T, double *coeffs,
+                                 double *f, int32_t *ret, int32_t *iterations, int32_t *evaluations, int32_t *rounds) {
+    auto poison_all = [&]() { if (f && B > 0) for (int b = 0; b < B; b++) f[b] = std::numeric_limits<double>::quiet_NaN(); };
+    int r = midend_check(c, B, N0, p);
+    if (r) { poison_all(); return r; }
+    if (!head || !tail || !x || !f || (N0 > 1 && !waypoints)) { poison_all(); return fail(ISDF_ERR_INVALID, "NULL argument"); }
+    auto body = [&]() -> int {
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        const size_t n = (size_t)4 * N0 - 3, BN = (size_t)B * N0;
+        const double *d_head, *d_tail, *d_wp;
+        if (int rr = midend_upload(c, B, N0, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return rr;
+        CU_TRY(c->mid.lb.d_x.ensure(n * B)); CU_TRY(c->mid.lb.d_f.ensure((size_t)19 * BN + B)); CU_TRY(c->mid.lb.d_head.ensure((size_t)3 * B));
+        double *d_f = c->mid.lb.d_f.p, *d_T = d_f + B, *d_C = d_T + BN;
+        int *d_i = c->mid.lb.d_head.p;
+        if (int rr = midend_batch_run(c, B, N0, d_head, d_tail, per_problem_bc, p, d_wp, c->mid.lb.d_x.p, d_T, d_C, d_f, d_i, d_i + B, d_i + 2 * (size_t)B,
+                                      rounds, c->stream)) return rr;
+        CU_TRY(cudaMemcpy(x, c->mid.lb.d_x.p, sizeof(double) * n * B, cudaMemcpyDeviceToHost));
+        CU_TRY(cudaMemcpy(f, d_f, sizeof(double) * B, cudaMemcpyDeviceToHost));
+        if (T) CU_TRY(cudaMemcpy(T, d_T, sizeof(double) * BN, cudaMemcpyDeviceToHost));
+        if (coeffs) CU_TRY(cudaMemcpy(coeffs, d_C, sizeof(double) * 18 * BN, cudaMemcpyDeviceToHost));
+        if (ret) CU_TRY(cudaMemcpy(ret, d_i, sizeof(int) * B, cudaMemcpyDeviceToHost));
+        if (iterations) CU_TRY(cudaMemcpy(iterations, d_i + B, sizeof(int) * B, cudaMemcpyDeviceToHost));
+        if (evaluations) CU_TRY(cudaMemcpy(evaluations, d_i + 2 * (size_t)B, sizeof(int) * B, cudaMemcpyDeviceToHost));
+        return 0;
+    };
+    r = body();
+    if (r) poison_all();
+    return r;
 }
 
 // ---- trajectory clearance check (isdf_clearance.cuh) -------------------------------------------------------------------------------

@@ -28,6 +28,7 @@ enum {   // lbfgs.hpp:148-197
 struct LbfgsDevParams {
     int mem_size, past, max_iterations, max_linesearch;
     double g_epsilon, delta, min_step, max_step, f_dec_coeff, cautious_factor, machine_prec;
+    int cancel_after;   // > 0: LB_CANCELED once k > cancel_after (the mid-end's progress callback earlyExit, mid_end.hpp:613-631); 0: never
 };
 
 constexpr int LB_NSCALAR = 8;   // fx, step, olddnorm, finit, dgtest, mu, nu, -
@@ -115,7 +116,8 @@ __global__ void __launch_bounds__(64) k_lbfgs_feed(const LbfgsArgs A) {
         next = 0;
         iterations = k;
         bool stop = false;
-        if (lb_norm_inf(g, n) / fmax(1.0, lb_norm_inf(x, n)) < pr.g_epsilon) { finish(LB_CONVERGENCE); stop = true; }
+        if (pr.cancel_after > 0 && k > pr.cancel_after) { finish(LB_CANCELED); stop = true; }   // where lbfgs.hpp:644-652 asks proc_progress
+        if (!stop && lb_norm_inf(g, n) / fmax(1.0, lb_norm_inf(x, n)) < pr.g_epsilon) { finish(LB_CONVERGENCE); stop = true; }
         if (!stop && 0 < past) {
             if (past <= k) {
                 const double rate = fabs(pf[k % past] - fx) / fmax(1.0, fabs(fx));

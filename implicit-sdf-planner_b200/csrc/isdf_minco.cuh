@@ -34,6 +34,7 @@ struct MincoArgs {
     const double *piece_cost; // B*N per-piece cost terms of that evaluation
     double *cost;             // B
     double *grad;             // B x (N + 3(N-1))
+    int seq_terms;            // 1: the piece costs are added to the energy one at a time (the mid-end, isdf_midend.cuh); 0: summed first
 };
 
 __device__ __forceinline__ double &band(double *a, int n, int i, int j) { return a[(size_t)(i - j + 6) * n + j]; }
@@ -248,7 +249,9 @@ __global__ void __launch_bounds__(32) k_minco_backward(const __grid_constant__ M
     if (lane == 0) {
         double cost = A.energy[b];
         if (A.sv_out) cost += A.sv_out[(size_t)b * (19 * N + 1)];
-        if (A.piece_cost) {
+        if (A.piece_cost && A.seq_terms) {
+            for (int i = 0; i < N; i++) cost += A.piece_cost[(size_t)b * N + i];
+        } else if (A.piece_cost) {
             double c = 0.0;
             for (int i = 0; i < N; i++) c += A.piece_cost[(size_t)b * N + i];
             cost += c;

@@ -4,6 +4,7 @@
 #include "isdf_cost_callback.hpp"
 #include "isdf_lbfgs.hpp"
 #include "isdf_obj.hpp"
+#include "isdf_midend.hpp"
 #include <algorithm>
 #include <cstring>
 #include <vector>
@@ -102,6 +103,44 @@ int isdf_host_lbfgs_batch_backend(isdf_ctx *ctx, int B, int N0, const double *he
     const int rounds = isdf_host_lbfgs_batch_generic(B, 4 * N0 - 3, x, f, ret, &batch_backend_eval, &be, mem_size, past, delta, g_epsilon, max_iterations,
                                                      iterations, evaluations);
     if (status) *status = be.status;
+    return rounds;
+}
+
+// ---- mid-end (host/isdf_midend.hpp): the cost, the sequential getOriTraj driver and the lock-step driver with its cancel rule ----
+void *isdf_host_midend_create(int N, int K, double weight, double rho, int cancel_after, const double *head, const double *tail, const double *waypoints) {
+    MidEnd *m = new MidEnd();
+    m->K = K; m->weight = weight; m->rho = rho; m->cancel_after = cancel_after;
+    m->setup(N, head, tail, waypoints);
+    return m;
+}
+void isdf_host_midend_destroy(void *me) { delete (MidEnd *)me; }
+// the signature of the reference-compiled L-BFGS's callback (c_eval_t): double (*)(void *, int n, const double *x, double *g)
+double isdf_host_midend_eval(void *me, int n, const double *x, double *g) { return MidEnd::costFunction(me, x, g, n, nullptr); }
+static LbfgsParams midend_lbfgs_params(int mem_size, int past, double delta, double g_epsilon, int max_iterations, double min_step) {
+    LbfgsParams pr; pr.mem_size = mem_size; pr.past = past; pr.delta = delta; pr.g_epsilon = g_epsilon; pr.max_iterations = max_iterations;
+    pr.min_step = min_step;
+    return pr;
+}
+int isdf_host_midend_optimize(void *me, double init_time, int mem_size, int past, double delta, double g_epsilon, int max_iterations, double min_step,
+                              double *x, double *f, double *T, double *coeffs, int *iterations, int *evaluations) {
+    LbfgsStats st; double fx = std::nan("");
+    const int r = ((MidEnd *)me)->getOriTraj(init_time, midend_lbfgs_params(mem_size, past, delta, g_epsilon, max_iterations, min_step), x, fx, T, coeffs, &st);
+    *f = fx; if (iterations) *iterations = st.iterations; if (evaluations) *evaluations = st.evaluations;
+    return r;
+}
+static void midend_batch_eval(void *inst, int nb, const int *ids, const double *x, double *f, double *g) {
+    MidEnd **m = static_cast<MidEnd **>(inst);
+    const int n = 4 * m[ids[0]]->N - 3;
+    for (int q = 0; q < nb; q++) f[q] = MidEnd::costFunction(m[ids[q]], x + (size_t)q * n, g + (size_t)q * n, n, nullptr);
+}
+// B instances (all of the same N) in lock step from x (B x (4N-3)) as given; returns the rounds
+int isdf_host_midend_lockstep(int B, void **me, int cancel_after, int mem_size, int past, double delta, double g_epsilon, int max_iterations,
+                              double min_step, double *x, double *f, int *ret, int *iterations, int *evaluations) {
+    LbfgsParams pr = midend_lbfgs_params(mem_size, past, delta, g_epsilon, max_iterations, min_step);
+    pr.cancel_after = cancel_after;
+    std::vector<LbfgsStats> st(B);
+    const int rounds = lbfgs_optimize_batch(B, 4 * ((MidEnd *)me[0])->N - 3, x, f, ret, &midend_batch_eval, me, pr, st.data());
+    for (int b = 0; b < B; b++) { iterations[b] = st[b].iterations; evaluations[b] = st[b].evaluations; }
     return rounds;
 }
 

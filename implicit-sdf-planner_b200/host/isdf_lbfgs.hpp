@@ -34,6 +34,7 @@ struct LbfgsParams {   // lbfgs_parameter_t (lbfgs.hpp:40-142)
     bool with_tole_ls = false;
     bool cast_x_range = false;
     double x_min = 0.0, x_max = 0.0;
+    int cancel_after = 0;   // lock-step driver only: LBFGS_CANCELED once k > cancel_after, where the sequential driver asks `progress`; 0 = never
 };
 
 enum {   // lbfgs.hpp:148-197
@@ -194,7 +195,8 @@ inline int lbfgs_optimize(int n, double *x, double &f, lbfgs_eval_raw_t eval, lb
 // evaluates them all (isdf_callback_batch: MINCO + collision term + adjoint for all problems in three launches), and each instance
 // consumes its result. An instance performs exactly the arithmetic of the sequential driver — it is the same code unrolled into a
 // state machine — so its iterates, iteration and evaluation counts and return code are identical to running it alone
-// (tests/test_host_adapters_cpu.py). No step bound / progress callback in this variant.
+// (tests/test_host_adapters_cpu.py). No step bound / progress callback in this variant; its one progress rule is pr.cancel_after (the
+// mid-end's earlyExit, mid_end.hpp:613-631), tested where the sequential driver calls `progress`.
 typedef void (*lbfgs_eval_batch_t)(void *instance, int nb, const int *ids, const double *x /* nb x n */, double *f /* nb */, double *g /* nb x n */);
 
 class LbfgsInstance {
@@ -274,6 +276,7 @@ private:
         using namespace detail;
         (void)ls;
         st.iterations = k;
+        if (pr.cancel_after > 0 && k > pr.cancel_after) { finish(LBFGS_CANCELED); return; }
         if (norm_inf(g.data(), n) / std::max(1.0, norm_inf(x.data(), n)) < pr.g_epsilon) { finish(LBFGS_CONVERGENCE); return; }
         if (0 < pr.past) {
             if (pr.past <= k) {

@@ -35,7 +35,8 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_clearance_default_params", "isdf_trajectory_clearance", "isdf_trajectory_clearance_device",
                "isdf_set_map_cloud", "isdf_set_map_cloud_device", "isdf_get_map_info", "isdf_get_map_u8", "isdf_get_map_f64",
                "isdf_frontend_path", "isdf_frontend_path_batch", "isdf_frontend_path_batch_device", "isdf_frontend_path_field_device",
-               "isdf_frontend_path_info"]
+               "isdf_frontend_path_info", "isdf_path_waypoints", "isdf_midend_default_params", "isdf_midend_callback_batch",
+               "isdf_midend_batch", "isdf_midend_batch_device"]
 
 
 class KernelConfig(C.Structure):
@@ -60,6 +61,12 @@ class LbfgsParams(C.Structure):
     """isdf_lbfgs_params"""
     _fields_ = [(n, C.c_int32) for n in ["mem_size", "past", "max_iterations", "max_linesearch", "max_rounds", "reserved_"]] + \
                [(n, C.c_double) for n in ["g_epsilon", "delta", "min_step", "max_step", "f_dec_coeff", "cautious_factor", "machine_prec"]]
+
+
+class MidendParams(C.Structure):
+    """isdf_midend_params"""
+    _fields_ = [("weight_pr", C.c_double), ("rho", C.c_double), ("init_time", C.c_double), ("cancel_after", C.c_int32), ("reserved_", C.c_int32),
+                ("lbfgs", LbfgsParams)]
 
 
 class ClearanceParams(C.Structure):
@@ -183,12 +190,41 @@ def load_library(path=None):
     lib.isdf_frontend_path_batch_device.argtypes = [vp, dp, C.c_int, vp, fpp, C.c_int, vp, vp, vp, vp, vp, vp]
     lib.isdf_frontend_path_field_device.argtypes = [vp, dp, fpp, vp, vp]
     lib.isdf_frontend_path_info.argtypes = [vp, C.POINTER(FrontPathInfo)]
+    mpp = C.POINTER(MidendParams)
+    lib.isdf_path_waypoints.argtypes = [C.c_int, ip, dp, C.c_double, C.c_double, C.c_int, dp, ip, ip]
+    lib.isdf_midend_default_params.argtypes = [mpp]
+    lib.isdf_midend_callback_batch.argtypes = [vp, C.c_int, C.c_int, dp, dp, C.c_int, mpp, dp, dp, dp, dp]
+    lib.isdf_midend_batch.argtypes = [vp, C.c_int, C.c_int, dp, dp, C.c_int, mpp, dp, dp, dp, dp, dp, ip, ip, ip, ip]
+    lib.isdf_midend_batch_device.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_int, mpp, vp, vp, vp, vp, vp, vp, vp, vp, ip, vp]
     for s in ABI_SYMBOLS:
         if s != "isdf_last_error":
             getattr(lib, s).restype = C.c_int
     if path is None:
         _lib = lib
     return lib
+
+
+def _colmajor(a):
+    """3x3 (or B x 3x3) row-major -> the library's column-major order"""
+    return np.ascontiguousarray(np.swapaxes(np.asarray(a, dtype=np.float64), -1, -2)).reshape(-1)
+
+
+def path_waypoints(paths, res, parlength=3.0):
+    """isdf_path_waypoints (plan_manager.cpp:204-245): paths = list of (n_b, 3) arrays -> (list of (N_b - 1, 3) waypoints, pieces N_b).
+    Host-only: needs no context or GPU."""
+    lib = load_library()
+    B = len(paths)
+    off = np.zeros(B + 1, dtype=np.int32)
+    for b, p in enumerate(paths):
+        off[b + 1] = off[b] + len(p)
+    xyz = _f64(np.concatenate([np.asarray(p, dtype=np.float64).reshape(-1, 3) for p in paths])) if B else np.zeros((0, 3))
+    cap = max(int(off[B]), 1)
+    wp, wo, pieces = np.zeros((cap, 3)), np.zeros(B + 1, dtype=np.int32), np.zeros(max(B, 1), dtype=np.int32)
+    ip = C.POINTER(C.c_int32)
+    r = lib.isdf_path_waypoints(B, off.ctypes.data_as(ip), _dp(xyz), float(res), float(parlength), cap, _dp(wp), wo.ctypes.data_as(ip), pieces.ctypes.data_as(ip))
+    if r != 0:
+        raise IsdfError(r, lib.isdf_last_error().decode())
+    return [wp[wo[b]:wo[b + 1]].copy() for b in range(B)], pieces[:B].copy()
 
 
 def _dp(a):
@@ -420,6 +456,84 @@ class Evaluator:
         self._check(self.lib.isdf_lbfgs_batch(self.h, B, N0, _dp(h), _dp(t), per, float(rho), C.byref(p), _dp(x), _dp(f), ret.ctypes.data_as(ip), it.ctypes.data_as(ip),
                                               evs.ctypes.data_as(ip), C.byref(rounds)))
         return dict(x=x.reshape(B, dim), f=f, ret=ret, iterations=it, evaluations=evs, rounds=rounds.value)
+
+    # ---- mid-end: warm start of the back end (see include/isdf.h) ----
+    def midend_params(self, **kw):
+        """isdf_midend_default_params with overrides; keys of isdf_lbfgs_params (mem_size, delta, ...) go to the nested lbfgs block,
+        reserved_ to the mid-end's own"""
+        p = MidendParams()
+        self._check(self.lib.isdf_midend_default_params(C.byref(p)))
+        lb = {n for n, _ in LbfgsParams._fields_} - {"reserved_"}
+        for k, v in kw.items():
+            setattr(p.lbfgs if k in lb else p, k, v)
+        return p
+
+    @staticmethod
+    def path_waypoints(paths, res, parlength=3.0):
+        return path_waypoints(paths, res, parlength)
+
+    @staticmethod
+    def _midend_args(head, tail, waypoints, B, N0):
+        head, tail = np.asarray(head, dtype=np.float64), np.asarray(tail, dtype=np.float64)
+        wp = _f64(waypoints).reshape(-1)
+        assert wp.size == 3 * B * (N0 - 1)
+        return int(head.ndim == 3), _colmajor(head), _colmajor(tail), (wp if wp.size else np.zeros(1))
+
+    def midend_callback_batch(self, head, tail, waypoints, X, params=None):
+        """OriTraj::costFunction for B problems: X (B, 4*N0-3), waypoints (B, N0-1, 3), head / tail (3,3) or (B,3,3) -> (cost[B], grad[B, 4*N0-3])"""
+        X = _f64(X)
+        B, dim = X.shape
+        N0 = (dim + 3) // 4
+        assert 4 * N0 - 3 == dim
+        per, h, t, wp = self._midend_args(head, tail, waypoints, B, N0)
+        p = params if params is not None else self.midend_params()
+        cost, grad = np.zeros(B), np.zeros((B, dim))
+        self._check(self.lib.isdf_midend_callback_batch(self.h, B, N0, _dp(h), _dp(t), per, C.byref(p), _dp(wp), _dp(X.reshape(-1)), _dp(cost),
+                                                        _dp(grad.reshape(-1))))
+        return cost, grad
+
+    def midend_batch(self, head, tail, waypoints, params=None):
+        """getOriTraj for B problems of N0 pieces: waypoints (B, N0-1, 3) -> dict(x (B, 4*N0-3), T (B, N0), coeffs (18*B*N0, the layout of
+        batch_trajectories), f, ret, iterations, evaluations, rounds)"""
+        wp3 = _f64(waypoints)
+        B, N0 = wp3.shape[0], wp3.shape[1] + 1
+        per, h, t, wp = self._midend_args(head, tail, wp3, B, N0)
+        p = params if params is not None else self.midend_params()
+        x, T, Cc, f = np.zeros((B, 4 * N0 - 3)), np.zeros((B, N0)), np.zeros(18 * B * N0), np.zeros(B)
+        ret, it, evs = (np.zeros(B, dtype=np.int32) for _ in range(3))
+        rounds = C.c_int32(0)
+        ip = C.POINTER(C.c_int32)
+        self._check(self.lib.isdf_midend_batch(self.h, B, N0, _dp(h), _dp(t), per, C.byref(p), _dp(wp), _dp(x.reshape(-1)), _dp(T.reshape(-1)), _dp(Cc), _dp(f),
+                                               ret.ctypes.data_as(ip), it.ctypes.data_as(ip), evs.ctypes.data_as(ip), C.byref(rounds)))
+        return dict(x=x, T=T, coeffs=Cc, f=f, ret=ret, iterations=it, evaluations=evs, rounds=rounds.value)
+
+    def midend_batch_device(self, B, N0, d_head, d_tail, per_problem_bc, d_waypoints, d_x, d_T, d_coeffs, d_f, d_ret, d_iterations, d_evaluations,
+                            params=None, stream=None):
+        """raw device pointers (e.g. torch .data_ptr()); returns the rounds"""
+        p = params if params is not None else self.midend_params()
+        rounds = C.c_int32(0)
+        self._check(self.lib.isdf_midend_batch_device(self.h, B, N0, d_head, d_tail, int(per_problem_bc), C.byref(p), d_waypoints, d_x, d_T, d_coeffs, d_f,
+                                                      d_ret, d_iterations, d_evaluations, C.byref(rounds), stream))
+        return rounds.value
+
+    def midend_from_paths(self, fp, res=None, parlength=3.0, params=None):
+        """generateTraj's mid-end for the result of frontend_path_batch: waypoints per plan, head = [front, 0, 0], tail = [back, 0, 0], the plans
+        grouped by N (one isdf_midend_batch per N). Returns one dict per N: N, idx (problem indices), waypoints (B_g, N-1, 3), head / tail
+        (B_g, 3, 3), x (the starting point for lbfgs_batch), T, coeffs, f, ret, iterations, evaluations, rounds. res = None: the map's resolution."""
+        if res is None:
+            res = self.map_info()["res"]
+        paths = fp["paths"]
+        wps, pieces = path_waypoints(paths, res, parlength)
+        groups = []
+        for N in sorted(set(int(n) for n in pieces)):
+            idx = np.flatnonzero(pieces == N)
+            head, tail = np.zeros((idx.size, 3, 3)), np.zeros((idx.size, 3, 3))
+            for q, b in enumerate(idx):
+                head[q, :, 0], tail[q, :, 0] = paths[b][0], paths[b][-1]
+            wp = np.array([wps[b] for b in idx]).reshape(idx.size, N - 1, 3)
+            r = self.midend_batch(head, tail, wp, params)
+            groups.append(dict(N=N, idx=idx, waypoints=wp, head=head, tail=tail, **r))
+        return groups
 
     def batch_trajectories(self, B, N0):
         T, Cc, en = np.zeros(B * N0), np.zeros(18 * B * N0), np.zeros(B)

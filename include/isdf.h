@@ -257,6 +257,73 @@ int isdf_lbfgs_batch_device(isdf_ctx *ctx, int B, int N0, const double *d_head, 
                             const isdf_lbfgs_params *params, double *d_x, double *d_f, int32_t *d_ret, int32_t *d_iterations, int32_t *d_evaluations,
                             int32_t *rounds, void *cuda_stream);
 
+/* ---- mid-end: warm start of the back end from front-end paths (PlannerManager::generateTraj, plan_manager.cpp:202-289) --------------
+ * The reference turns an A* path into the back end's starting point in two steps: it picks waypoints from the path, then OriTraj::getOriTraj
+ * (mid_end.cpp:3-94) runs an L-BFGS over a MINCO trajectory that pulls it towards them. Its solution opt_x is the x that optimize_traj_lmbm
+ * starts from (back_end_optimizer.cpp:117). Here both steps run for B paths at once; a solution goes straight into isdf_lbfgs_batch.
+ * Definition
+ *   Waypoints      plan_manager.cpp:204-245 for each path of size S: gap = ceil(parlength / res) (parlength: traj_parlength, 3.0 in the
+ *                  reference, :153; res: the map's resolution); while gap >= S - 1: parlength /= 1.5 (FP64), recompute gap; Q = path[gap],
+ *                  path[2 gap], ... for indices < S - 1; N = |Q| + 1. head = [path.front(), 0, 0], tail = [path.back(), 0, 0] (3x3 column-major
+ *                  as isdf_callback_batch takes them). Deviation: for S = 1 or 2 the reference never terminates (the loop divides until gap is
+ *                  0, then ind += 0); here N = 1 and no waypoints. The attitude and acceleration lists built in the same loop only feed the
+ *                  mid-end's addTimeIntPenalty, which is never called (mid_end.hpp:424-592), so they are not inputs.
+ *   Cost           OriTraj::costFunction (mid_end.hpp:262-304) on x = [tau (N0) | xi (3(N0-1), waypoint-major)], the back end's layout:
+ *                  T = forwardT(tau), MINCO -> jerk energy E and its partials; then, for waypoint i = 0..N0-2 (addPosePenalty, :201-260),
+ *                  piece i + 1 evaluated at s = T_{i+1} * (1 / K), K = isdf_config.integral_intervs (integralRes, :323) — NOT the junction
+ *                  where xi_i sits:
+ *                    d = p(s) - Q_i, n = sqrt((d0 d0 + d1 d1) + d2 d2), c_i = (n n) n, g = (3 (n n)) (d / n),
+ *                    gradC rows of piece i + 1 += w (beta0 (x) g), gradT(i + 1) += w (c_i (alpha (g . v(s)))), alpha = 1 / K;
+ *                  each term only when c_i > 0 (grad_cost_dir returns cost > 0, :198), so d = 0 adds nothing.
+ *                  cost = ((E + w c_1) + w c_2) + ... + rho sum(T) (every sum left to right), gradT += rho, then propogateGrad and
+ *                  backwardGradT / backwardGradP exactly as the back end's callback.
+ *   Quirk, kept    the T entry is multiplied by the cost c_i: the tau gradient is not the derivative of the cost.
+ *   Arithmetic     IEEE operations only (no pow): glibc's pow(|d|, 3) is not correctly rounded and CUDA's differs from it, so no formula is
+ *                  bit-equal to the reference on both sides. Host (host/isdf_midend.hpp) and device agree bit for bit; the difference from
+ *                  the reference's pow form is about one ulp per term (DESIGN §3.10).
+ *   Optimiser      getOriTraj: x starts at [backwardT(init_time) for every piece | the waypoints]; L-BFGS as isdf_lbfgs_batch with
+ *                  params.lbfgs (mid_end.cpp:48-54: mem 16, past 10, min_step 1e-32, g_epsilon 0, delta 1e-6, max_iterations 100000) and
+ *                  the progress callback earlyExit (mid_end.hpp:613-631): LBFGS_CANCELED (2) once k > cancel_after after a successful line
+ *                  search. ret >= 0 is getOriTraj's success (plan_manager.cpp:277 runs the back end only then). The final T and coeffs are
+ *                  forwardT + MINCO of the returned x, whatever ret is. f is the cost at the returned x; where the reference's
+ *                  lbfgs_optimize returns from its direction-norm test without writing f (lbfgs.hpp:814-817, code -1012), f is still
+ *                  the cost at x.
+ * Each problem's result is bit-identical to the sequential host driver on the same problem, alone or inside a batch.
+ * The mid-end needs neither a map nor a shape. It has its own device buffers: it leaves isdf_get_batch_trajectories, the swept-volume
+ * t* and persisted durations, the discrete work-item schedule and every isdf_stats field but kernel_launches as they were.
+ * Errors: ISDF_ERR_INVALID for a NULL argument, B < 1, N0 < 1, a parameter out of range or a non-zero reserved_; ISDF_ERR_UNSUPPORTED for
+ *   N0 > 290; ISDF_ERR_STATE on a sharded context (shard by problem, as isdf_callback_batch). On failure every cost[b] / f[b] is NaN. */
+/* waypoint selection, host-only (needs no context or GPU). paths: B paths back to back, path b in rows [path_off[b], path_off[b+1]) of
+ * path_xyz (what isdf_frontend_path_batch returns; every path at least one node). Writes the waypoints of plan b to rows
+ * [wp_off[b], wp_off[b+1]) of waypoints (cap x 3) and its N to pieces[b]. ISDF_ERR_INVALID when the total exceeds cap (wp_off and pieces
+ * are still written), for res or parlength not finite and positive, or for offsets that do not start at 0 and increase. */
+int isdf_path_waypoints(int B, const int32_t *path_off, const double *path_xyz, double res, double parlength, int cap,
+                        double *waypoints, int32_t *wp_off, int32_t *pieces);
+typedef struct isdf_midend_params {
+    double weight_pr;        /* weightPR (mid_end.hpp:315; yaml weight_pr 1000); >= 0 */
+    double rho;              /* rho_mid_end (yaml 200); finite */
+    double init_time;        /* inittime (yaml 2.5): every piece's starting duration (plan_manager.cpp:263); > 0 */
+    int32_t cancel_after;    /* earlyExit: LBFGS_CANCELED once k > cancel_after (8000); 0 = never */
+    int32_t reserved_;       /* must be 0 */
+    isdf_lbfgs_params lbfgs; /* mid_end.cpp:48-54; the other fields keep their lbfgs.hpp defaults */
+} isdf_midend_params;
+int isdf_midend_default_params(isdf_midend_params *p);
+/* one evaluation of the cost for B problems: waypoints B x (N0-1) x 3; x, grad B x (4*N0-3); cost B. head / tail / per_problem_bc as
+ * isdf_callback_batch. */
+int isdf_midend_callback_batch(isdf_ctx *ctx, int B, int N0, const double *head, const double *tail, int per_problem_bc,
+                               const isdf_midend_params *p, const double *waypoints, const double *x, double *cost, double *grad);
+/* getOriTraj for B problems: x (out, B x (4*N0-3)) starts at [backwardT(init_time) | waypoints] and returns the solution; f: B final costs.
+ * T (B*N0) and coeffs (6*B*N0 x 3 column-major, piece b*N0+i: the layout of isdf_get_batch_trajectories) are the final trajectories.
+ * Any of T / coeffs / ret / iterations / evaluations / rounds may be NULL. */
+int isdf_midend_batch(isdf_ctx *ctx, int B, int N0, const double *head, const double *tail, int per_problem_bc,
+                      const isdf_midend_params *p, const double *waypoints, double *x, double *T, double *coeffs,
+                      double *f, int32_t *ret, int32_t *iterations, int32_t *evaluations, int32_t *rounds);
+/* device-resident variant: every array on ctx's device (rounds on the host); runs on cuda_stream and returns when every instance has
+ * stopped. On failure d_f is filled with NaN when ctx and d_f are valid. */
+int isdf_midend_batch_device(isdf_ctx *ctx, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc,
+                             const isdf_midend_params *p, const double *d_waypoints, double *d_x, double *d_T, double *d_coeffs,
+                             double *d_f, int32_t *d_ret, int32_t *d_iterations, int32_t *d_evaluations, int32_t *rounds, void *cuda_stream);
+
 /* ---- trajectory clearance check: is a trajectory collision-free over the WHOLE map, and by how much? ------------------------------
  * The reference has no working counterpart (SweptVolumeManager::isTrajCollide, swm:759-767, always returns false), and the cost terms
  * cannot stand in for it: the hinge is smoothed and positive only inside safety_hor, the swept-volume term only sees the gathered obstacle
