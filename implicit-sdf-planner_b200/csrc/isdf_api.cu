@@ -75,7 +75,10 @@ struct isdf_ctx {
         DevBuf<int> d_tickets;       // pieces_done counter of the epilogue kernel
         DevBuf<double> d_tot; DevBuf<unsigned> d_split_done;   // per-sample collision sums handed from the scan kernels to the epilogue
         DevBuf<int> d_items, d_item_count; DevBuf<unsigned> d_work, d_split_work; DevBuf<double> d_subsum;   // work items (longest first, heavy samples split)
-        DevBuf<unsigned long long> d_counter;
+        DevBuf<unsigned long long> d_counter;   // {pairs, then k_discrete_prologue's {codes requested, runs, overflowed runs, codes written}}
+        DevBuf<double> d_pose; DevBuf<int2> d_wl_desc; DevBuf<uint32_t> d_wl_codes;   // mesh launches: per local sample pose and window list
+        int wl_budget = WL_CODES_PER_SAMPLE;   // window-list codes per local sample (isdf_dbg_window_lists; 0: no lists)
+        long long wl_samples = 0, wl_cap = 0;  // local samples and list capacity of the last launch with a prologue
         bool no_items = false;       // diagnostics: always launch in natural order, never split (isdf_dbg_schedule)
         int warp_slots_override = 0; // diagnostics: pretend the device has this many resident warps (forces splitting)
     } disc;
@@ -195,8 +198,8 @@ extern "C" int isdf_create(const isdf_config *cfg, int device, isdf_ctx **out) {
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_items_done, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreate(&c->ev0);
     if (e == cudaSuccess) e = cudaEventCreate(&c->ev1);
-    if (e == cudaSuccess) e = c->disc.d_counter.ensure(4);
-    if (e == cudaSuccess) e = cudaMemset(c->disc.d_counter.p, 0, 4 * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = c->disc.d_counter.ensure(5);
+    if (e == cudaSuccess) e = cudaMemset(c->disc.d_counter.p, 0, 5 * sizeof(unsigned long long));
     if (e != cudaSuccess) { delete c; return fail(ISDF_ERR_CUDA, std::string("isdf_create: ") + cudaGetErrorString(e)); }
     *out = c;
     return 0;
@@ -912,10 +915,25 @@ static int launch_discrete(isdf_ctx *c, int N, const double *d_T, const double *
         A.peer = c->peer.args; A.peer.epoch = c->peer.args.epoch + 1;   // committed below, once the exchange kernel is really enqueued
     }
     const long long M = (S - c->rank + c->world - 1) / c->world;
-    CU_TRY(cudaMemsetAsync(c->disc.d_counter.p, 0, sizeof(unsigned long long), st));
+    const bool mesh = (c->mesh.shape.kind == ISDF_SHAPE_MESH);
+    // mesh launches with collision: k_discrete_prologue computes every local sample's pose and lists each run's window voxels
+    const bool prologue = mesh && (c->dcfg.flags & ISDF_WITH_COLLISION);
+    A.pose = nullptr; A.wl_desc = nullptr; A.wl_codes = nullptr; A.wl_cap = 0; A.wl_count = c->disc.d_counter.p + 1;
+    if (prologue) {
+        // budget x world codes per local sample: a shard's runs are world times shorter (~54 / world samples on the bench
+        // trajectory), so the same windows need world times more codes per local sample. List offsets are ints.
+        const long long cap = std::min<long long>((long long)c->disc.wl_budget * M * c->world, 0x7fffffffll);
+        CU_TRY(c->disc.d_pose.ensure((size_t)8 * M));
+        CU_TRY(c->disc.d_wl_desc.ensure((size_t)M));
+        CU_TRY(c->disc.d_wl_codes.ensure((size_t)std::max(cap, 1ll)));
+        A.pose = c->disc.d_pose.p; A.wl_desc = c->disc.d_wl_desc.p; A.wl_codes = c->disc.d_wl_codes.p; A.wl_cap = (unsigned long long)cap;
+        c->disc.wl_cap = cap;
+    }
+    c->disc.wl_samples = prologue ? M : 0;
+    CU_TRY(cudaMemsetAsync(c->disc.d_counter.p, 0, 5 * sizeof(unsigned long long), st));   // pair counter, window-list counters
+    if (prologue) CU_TRY(discrete_launch_prologue(A, (int)M, st));
     // longest-first order from the previous evaluation of the same problem shape (first evaluation: natural order)
     const long long sig = ((long long)N << 20) ^ ((long long)c->rank << 10) ^ c->world ^ ((long long)K << 40);
-    const bool mesh = (c->mesh.shape.kind == ISDF_SHAPE_MESH);
     // only mesh samples have a heavy tail worth splitting. Every sample of a launch may be split (item trace at world = 8:
     // with M/4 slots the 515 heaviest samples were split and the NEXT heaviest — unsplit, 15-25 queries, 80-110 us — set the kernel time)
     const int max_split = mesh ? (int)std::min<long long>(M, MAX_SPLIT_SLOTS) : 0;
@@ -957,7 +975,7 @@ static int launch_discrete(isdf_ctx *c, int N, const double *d_T, const double *
         c->disc.order_for = sig;
         c->stats.kernel_launches++;   // work-item builder
     }
-    c->stats.kernel_launches += 2;   // scan kernel, epilogue
+    c->stats.kernel_launches += prologue ? 3 : 2;   // (prologue,) scan kernel, epilogue
     c->stats.evals_discrete++;
     return 0;
 }
@@ -2228,6 +2246,29 @@ extern "C" int isdf_get_swept_results(isdf_ctx *c, double *tstar, double *sdf, d
 extern "C" int isdf_dbg_schedule(isdf_ctx *c, int natural_order, int warp_slots) {
     if (!c) return -1;
     c->disc.no_items = natural_order != 0; c->disc.warp_slots_override = warp_slots > 0 ? warp_slots : 0; c->disc.order_for = -1;
+    return 0;
+}
+// window lists (k_discrete_prologue): budget >= 0 sets the list capacity of the following mesh evaluations in codes per sample of
+// the trajectory, i.e. budget x world per local sample (0: no lists, every sample's window is enumerated by the scan kernel);
+// budget < 0 keeps it. Of the last mesh evaluation with
+// collision: stats (6 entries, optional) = {runs, codes written, overflowed runs, local samples M, code capacity, codes requested};
+// pose (M x 8), desc (M x 2: list offset or -1, voxel count) and codes (min(requested, capacity) entries) are optional copies.
+extern "C" int isdf_dbg_window_lists(isdf_ctx *c, int budget, long long *stats, double *pose, int *desc, uint32_t *codes) {
+    if (!c) return -1;
+    if (budget >= 0) c->disc.wl_budget = budget;
+    if (!stats && !pose && !desc && !codes) return 0;
+    if (c->disc.wl_samples == 0) return -2;
+    if (cudaSetDevice(c->device) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) return -3;
+    unsigned long long cnt[4];
+    if (cudaMemcpy(cnt, c->disc.d_counter.p + 1, sizeof(cnt), cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    const size_t M = (size_t)c->disc.wl_samples, ncodes = (size_t)std::min<unsigned long long>(cnt[0], (unsigned long long)c->disc.wl_cap);
+    if (stats) {
+        stats[0] = (long long)cnt[1]; stats[1] = (long long)cnt[3]; stats[2] = (long long)cnt[2];
+        stats[3] = (long long)M; stats[4] = c->disc.wl_cap; stats[5] = (long long)cnt[0];
+    }
+    if (pose && cudaMemcpy(pose, c->disc.d_pose.p, sizeof(double) * 8 * M, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (desc && cudaMemcpy(desc, c->disc.d_wl_desc.p, sizeof(int2) * M, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (codes && ncodes && cudaMemcpy(codes, c->disc.d_wl_codes.p, sizeof(uint32_t) * ncodes, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
     return 0;
 }
 // number of work items / split samples of the table built by the last discrete evaluation

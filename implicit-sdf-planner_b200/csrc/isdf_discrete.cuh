@@ -54,6 +54,10 @@ constexpr int ANALYTIC_MIN_BLOCKS = 4;
 constexpr int MESH_MIN_BLOCKS = 4;
 constexpr int EPI_THREADS = 288;
 constexpr int ITEMS_CACHE = 24;   // k_build_items: samples per thread whose work value is kept in registers (M <= 24576: any single trajectory)
+// window-list capacity in codes per sample of the trajectory (64 B; world x that per local sample of a shard): the bench trajectory
+// needs ~4.3 (305 runs + one forced run start per 128 samples, ~164 occupied voxels per window), a 19 %-occupancy map ~14; a run
+// that does not fit is enumerated by the scan kernel
+constexpr int WL_CODES_PER_SAMPLE = 16;
 
 struct DiscArgs {
     DevCfg cfg;
@@ -75,6 +79,12 @@ struct DiscArgs {
     unsigned *split_work;              // split slot -> work accumulated by the parts (zero on entry, zeroed by the sample's last part)
     unsigned *split_done;              // split slot -> parts finished (zero on entry, zeroed by the sample's last part)
     unsigned *work;                    // may be null: per global sample, work measure written for the next evaluation
+    // mesh launches with collision (k_discrete_prologue -> k_discrete_mesh), indexed by local sample m:
+    double *pose;                      // 8 per sample: position x, y, z, quaternion w, x, y, z, unused
+    int2 *wl_desc;                     // {offset into wl_codes, or -1 = no list (the scan kernel enumerates the window itself), voxel count}
+    uint32_t *wl_codes;                // the occupied voxels of each run's window, in canonical order (WindowRows)
+    unsigned long long wl_cap;         // capacity of wl_codes
+    unsigned long long *wl_count;      // {codes requested, runs, overflowed runs, codes written} (zero on entry)
     int rank, world;       // this launch evaluates samples s with s % world == rank
     PeerArgs peer;         // peer.world > 1: the epilogue's last CTA also sums `out` over the ranks through peer memory (isdf_peer.cuh)
 };
@@ -497,6 +507,128 @@ __device__ __forceinline__ void row_split(int r, int ny, float inv_ny, int &rx, 
     if (ry < 0) { rx--; ry += ny; } else if (ry >= ny) { rx++; ry -= ny; }
 }
 
+__device__ __forceinline__ int warp_incl_scan(int v, int lane) {
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += t; }
+    return v;
+}
+
+// Cursor over the occupied voxels of a pose window in CANONICAL order: z-chunks of 32 voxels; inside a chunk the window rows
+// r = rx * ny + ry ascending, 32 rows per batch (lane = row); inside a row z ascending. A voxel's code is dx | dy << 10 | dz << 20
+// relative to the window origin, its class (r + 5 dz) % 32. The per-class sums of k_discrete_mesh add voxels in this order, so
+// the prologue's window lists and the scan kernel's own enumeration both go through this one cursor.
+struct WindowRows {
+    int ny, nrows, zs, kb;
+    float inv_ny;
+    __device__ __forceinline__ explicit WindowRows(const Window &W)
+        : ny(W.iy1 - W.iy0 + 1), nrows((W.ix1 - W.ix0 + 1) * ny), zs(W.iz0), kb(-32), inv_ny(1.0f / (float)ny) {}
+    // the next batch of rows, false once the window is exhausted: bits = the lane's row's occupied voxels in this z-chunk (bit k =
+    // chunk voxel k), restricted to the classes [c0, c0 + w) when w < 32; rowcode = the code of the row's first chunk voxel
+    __device__ __forceinline__ bool next(const DevGrid &G, const Window &W, int lane, int c0, int w, uint32_t &bits, uint32_t &rowcode) {
+        kb += 32;
+        if (kb >= nrows) { kb = 0; zs += 32; }
+        if (zs > W.iz1) return false;
+        const int nzc = min(32, W.iz1 - zs + 1);
+        const uint32_t zmask = (nzc == 32) ? 0xffffffffu : ((1u << nzc) - 1u);
+        const int r = kb + lane;
+        bits = 0;
+        if (r < nrows) {
+            int rx, ry;
+            row_split(r, ny, inv_ny, rx, ry);
+            bits = row_bits(G, W.ix0 + rx, W.iy0 + ry, zs, zmask);
+            rowcode = (uint32_t)rx | ((uint32_t)ry << 10) | ((uint32_t)(zs - W.iz0) << 20);
+            if (w < ROW_CLASSES && bits != 0u) {   // keep the voxels of the classes [c0, c0 + w)
+                uint32_t keep = 0u;
+                unsigned cls = (unsigned)(r + 5 * (zs - W.iz0)) & 31u;
+                for (int k = 0; k < nzc; k++) { keep |= (((cls - (unsigned)c0) & 31u) < (unsigned)w ? 1u : 0u) << k; cls = (cls + 5u) & 31u; }
+                bits &= keep;
+            }
+        }
+        return true;
+    }
+};
+
+// a lane's voxels of a WindowRows batch, z ascending, as put(first, code), put(first + 1, code), ...
+template <class Put>
+__device__ __forceinline__ void emit_row(uint32_t bits, uint32_t rowcode, int first, Put &&put) {
+    while (bits != 0u) {
+        const int z = __ffs(bits) - 1;
+        bits &= bits - 1;
+        put(first++, rowcode + ((uint32_t)z << 20));
+    }
+}
+
+// ============================================================================================================================
+// Prologue of a mesh launch: one thread per local sample computes its pose (sample_pose, stored as position + quaternion) and its
+// window; one warp per RUN (consecutive samples of the CTA's range with the same window: ~54 on the bench trajectory, whose samples
+// are ~1.2 cm apart in 1 m windows) lists the window's occupied voxels once, in canonical order, into wl_codes. Every sample of
+// the run points at that list. A run that does not fit into wl_codes gets no list; the scan kernel then enumerates its window
+// itself, in the same order, so the results do not depend on which samples got lists.
+constexpr int PRO_SAMPLES = 128;   // local samples per CTA; runs never cross a CTA's range, so no grid-wide step is needed
+
+__global__ void __launch_bounds__(PRO_SAMPLES) k_discrete_prologue(const __grid_constant__ DiscArgs A) {
+    __shared__ Window s_win[PRO_SAMPLES];
+    __shared__ int s_start[PRO_SAMPLES + 1];
+    __shared__ int s_wruns[PRO_SAMPLES / 32];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const DevGrid &G = A.grid;
+    const int K = A.cfg.K;
+    const int M = (A.N * (K + 1) - A.rank + A.world - 1) / A.world;
+    const int m0 = blockIdx.x * PRO_SAMPLES, n = min(PRO_SAMPLES, M - m0);
+    if (tid < n) {
+        const int m = m0 + tid, s = A.rank + A.world * m;
+        const int i = s / (K + 1), j = s - i * (K + 1);
+        d3 pos; quat4 q; rot3 R;
+        sample_pose(A, i, j, __ldg(A.T + i) * (1.0 / K), pos, q, R);
+        double4 *pp = reinterpret_cast<double4 *>(A.pose + 8 * (size_t)m);
+        pp[0] = make_double4(pos.x, pos.y, pos.z, q.w);
+        pp[1] = make_double4(q.x, q.y, q.z, 0.0);
+        s_win[tid] = window_of(G, pos, A.cfg.half_bd);
+    }
+    __syncthreads();
+    bool start = false;
+    if (tid < n) {
+        const Window &a = s_win[tid], &b = s_win[tid > 0 ? tid - 1 : 0];
+        start = tid == 0 || a.ix0 != b.ix0 || a.ix1 != b.ix1 || a.iy0 != b.iy0 || a.iy1 != b.iy1 || a.iz0 != b.iz0 || a.iz1 != b.iz1;
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, start);
+    if (lane == 0) s_wruns[warp] = __popc(bal);
+    __syncthreads();
+    int first = 0, nruns = 0;
+#pragma unroll
+    for (int k = 0; k < PRO_SAMPLES / 32; k++) { first += k < warp ? s_wruns[k] : 0; nruns += s_wruns[k]; }
+    if (start) s_start[first + __popc(bal & ((1u << lane) - 1u))] = tid;
+    if (tid == 0) s_start[nruns] = n;
+    __syncthreads();
+    for (int r = warp; r < nruns; r += PRO_SAMPLES / 32) {
+        const int a = s_start[r], b = s_start[r + 1];
+        const Window W = s_win[a];
+        uint32_t bits = 0, rowcode = 0;
+        int total = 0;
+        for (WindowRows rows(W); rows.next(G, W, lane, 0, ROW_CLASSES, bits, rowcode);) total += __popc(bits);
+        total = __reduce_add_sync(0xffffffffu, total);
+        unsigned long long off = 0;
+        if (lane == 0) off = atomicAdd(A.wl_count, (unsigned long long)total);
+        off = __shfl_sync(0xffffffffu, off, 0);
+        const bool fits = A.wl_cap != 0 && off + (unsigned long long)total <= A.wl_cap;   // capacity 0: no lists at all
+        if (fits) {
+            uint32_t *out = A.wl_codes + off;
+            int done = 0;
+            for (WindowRows rows(W); rows.next(G, W, lane, 0, ROW_CLASSES, bits, rowcode);) {
+                const int incl = warp_incl_scan(__popc(bits), lane);
+                emit_row(bits, rowcode, done + incl - __popc(bits), [&](int k, uint32_t code) { out[k] = code; });
+                done += __shfl_sync(0xffffffffu, incl, 31);
+            }
+        }
+        const int2 d = make_int2(fits ? (int)off : -1, total);
+        for (int t = a + lane; t < b; t += 32) A.wl_desc[m0 + t] = d;
+        if (lane == 0) {
+            atomicAdd(A.wl_count + 1, 1ull);
+            atomicAdd(A.wl_count + (fits ? 3 : 2), fits ? (unsigned long long)total : 1ull);
+        }
+    }
+}
+
 template <bool WINDING>
 __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh(const __grid_constant__ DiscArgs A) {
     __shared__ MeshWarpSmem wsm[DISC_WARPS];
@@ -506,22 +638,25 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
     const DevCfg &cfg = A.cfg;
     const DevMesh &Mh = A.shape.mesh;
     const DevGrid &G = A.grid;
-    const int K = cfg.K;
     MeshWarpSmem &sm = wsm[warp];
     const double h = cfg.half_bd, sf = cfg.safety;
     Item it;
     while (next_item(A, it, lane)) {
         const int s = it.s;
-        const int i = s / (K + 1), j = s - i * (K + 1);
         unsigned npairs = 0, nquery = 0;
         const bool whole = (it.c1 - it.c0) == ROW_CLASSES;
 
         if (cfg.flags & ISDF_WITH_COLLISION) {
             Window W;
-            {   // pose -> shared memory (every lane computes the same values; lane 0 publishes them)
-                const double Ti = __ldg(A.T + i);
-                d3 pos; quat4 q; rot3 R;
-                sample_pose(A, i, j, Ti * (1.0 / K), pos, q, R);
+            int2 wl;   // the sample's window list {offset, count} (offset -1: enumerate the window here)
+            {   // pose (k_discrete_prologue) -> shared memory (every lane loads the same values; lane 0 publishes them)
+                const int m = (s - A.rank) / A.world;
+                const double2 *pp = reinterpret_cast<const double2 *>(A.pose + 8 * (size_t)m);
+                const double2 p0 = __ldg(pp), p1 = __ldg(pp + 1), p2 = __ldg(pp + 2);
+                wl = __ldg(A.wl_desc + m);
+                const d3 pos = mk3(p0.x, p0.y, p1.x);
+                quat4 q; q.w = p1.y; q.x = p2.x; q.y = p2.y; q.z = __ldg(A.pose + 8 * (size_t)m + 6);
+                const rot3 R = quat_rot(q);
                 W = window_of(G, pos, h);
                 if (lane == 0) {
                     double *ps = sm.pose;
@@ -533,9 +668,8 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
             }
             for (int k = lane; k < ROW_CLASSES * 8; k += 32) (&sm.cacc[0][0])[k] = 0.0;
             __syncwarp();
-            const int ny = W.iy1 - W.iy0 + 1;
-            const int nrows = (W.ix1 - W.ix0 + 1) * ny;
-            const float inv_ny = 1.0f / (float)ny;
+            WindowRows rows(W);
+            const int ny = rows.ny;
             int nq = 0, head = 0, nres = 0;   // voxel ring fill / head, answered voxels awaiting their tail (warp-uniform)
 
             // deferred tails: sign, gradient, hinge, chain rule onto (position, quaternion) — one answered voxel per lane; the
@@ -649,56 +783,49 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
                 nsv = 0;
             };
 
-            // Producer loop (one cull and one search call site): batches of 32 window rows are loaded (lane = row), their occupied voxels
-            // are appended to the ring, and whenever 32 voxels are queued — or the window is exhausted — they are processed.
+            // Producer loop (one cull and one search call site): the sample's occupied voxels are appended to the ring in canonical
+            // order (WindowRows), and whenever 32 voxels are queued — or the window is exhausted — they are processed.
             // Voxel (row r, z offset dz) of the window belongs to class (r + 5 dz) % 32: the voxels an obstacle patch puts near the robot
             // — a few rows x a few z, the ones that cost mesh queries — land in ~as many different classes as there are voxels, so the
             // parts of a split sample get near-equal numbers of queries (row-interleaved classes gave a wall patch to 5 of 32 classes:
-            // measured item timeline). A split part scans the same rows and keeps its classes' voxels (a bit filter).
-            // Lanes are rows in ascending order and a lane emits its voxels z-ascending, so emitting a batch lane by lane — at once when it
-            // fits into the ring, else row by row (dense walls) — keeps every CLASS's voxels in (row, z) order for whole samples and parts.
+            // measured item timeline). A split part takes the same voxels and keeps its classes' ones.
+            // Source 1, the window list of the sample's run (k_discrete_prologue): 32 codes per coalesced load, the next load in flight
+            // during this batch's cull. Source 2, no list: batches of 32 window rows (lane = row) emitted lane by lane — at once when the
+            // batch fits into the ring, else row by row (dense walls). Both keep every CLASS's voxels in canonical order.
             const int w = it.c1 - it.c0;
-            int zs = W.iz0, kb = -32;
+            const bool listed = wl.x >= 0;
+            const uint32_t *list = A.wl_codes + (listed ? wl.x : 0);
+            int lk = 0;   // list: codes taken
+            uint32_t lnext = (listed && lane < wl.y) ? __ldg(list + lane) : 0u;
             uint32_t bits = 0, rowcode = 0;
             unsigned pending = 0;
             bool finished = false;
             for (;;) {
                 if (!finished) {
-                    if (pending == 0u) {   // next batch of rows
-                        kb += 32;
-                        if (kb >= nrows) { kb = 0; zs += 32; }
-                        if (zs > W.iz1) finished = true;
+                    if (listed) {
+                        if (lk >= wl.y) finished = true;
                         else {
-                            const int nzc = min(32, W.iz1 - zs + 1);
-                            const uint32_t zmask = (nzc == 32) ? 0xffffffffu : ((1u << nzc) - 1u);
-                            const int r = kb + lane;
-                            bits = 0;
-                            if (r < nrows) {
-                                int rx, ry;
-                                row_split(r, ny, inv_ny, rx, ry);
-                                bits = row_bits(G, W.ix0 + rx, W.iy0 + ry, zs, zmask);
-                                rowcode = (uint32_t)rx | ((uint32_t)ry << 10) | ((uint32_t)(zs - W.iz0) << 20);
-                                if (!whole && bits != 0u) {   // keep the voxels of the classes [c0, c1)
-                                    uint32_t keep = 0u;
-                                    unsigned cls = (unsigned)(r + 5 * (zs - W.iz0)) & 31u;
-                                    for (int k = 0; k < nzc; k++) { keep |= (((cls - (unsigned)it.c0) & 31u) < (unsigned)w ? 1u : 0u) << k; cls = (cls + 5u) & 31u; }
-                                    bits &= keep;
-                                }
+                            const uint32_t code = lnext;
+                            bool take = lk + lane < wl.y;
+                            lk += 32;
+                            if (lk + lane < wl.y) lnext = __ldg(list + lk + lane);
+                            if (!whole && take) {   // keep the voxels of the classes [c0, c1)
+                                const unsigned cls = ((code & 0x3ffu) * (unsigned)ny + ((code >> 10) & 0x3ffu) + 5u * (code >> 20)) & 31u;
+                                take = ((cls - (unsigned)it.c0) & 31u) < (unsigned)w;
                             }
+                            const unsigned tb = __ballot_sync(0xffffffffu, take);
+                            if (take) sm.vq[(head + nq + __popc(tb & lt_mask)) & 63] = code;
+                            nq += __popc(tb);
+                        }
+                    } else if (pending == 0u) {   // next batch of rows
+                        if (!rows.next(G, W, lane, it.c0, w, bits, rowcode)) finished = true;
+                        else {
                             pending = __ballot_sync(0xffffffffu, bits != 0u);
                             if (pending != 0u) {
-                                int incl = __popc(bits);
-#pragma unroll
-                                for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
+                                const int incl = warp_incl_scan(__popc(bits), lane);
                                 const int total = __shfl_sync(0xffffffffu, incl, 31);
                                 if (nq + total <= 64) {   // the whole batch fits: emit it at once
-                                    int pos = head + nq + incl - __popc(bits);
-                                    while (bits != 0u) {
-                                        const int z = __ffs(bits) - 1;
-                                        bits &= bits - 1;
-                                        sm.vq[pos & 63] = rowcode + ((uint32_t)z << 20);
-                                        pos++;
-                                    }
+                                    emit_row(bits, rowcode, head + nq + incl - __popc(bits), [&](int k, uint32_t code) { sm.vq[k & 63] = code; });
                                     nq += total;
                                     pending = 0u;
                                 }
@@ -892,6 +1019,8 @@ __global__ void __launch_bounds__(1024) k_build_items(const unsigned *work, int 
 
 // ---- launch interface of the discrete translation unit (isdf_discrete_tu.cu) ------------------------------------------------------
 cudaError_t discrete_launch_scan(const DiscArgs &A, bool mesh, unsigned grid, cudaStream_t st);
+// mesh launches with collision, before the scan: poses and window lists of the M local samples
+cudaError_t discrete_launch_prologue(const DiscArgs &A, int M, cudaStream_t st);
 cudaError_t discrete_launch_epilogue(const DiscArgs &A, cudaStream_t st);
 cudaError_t discrete_launch_build_items(const unsigned *work, int rank, int world, int M, int max_split, int warp_slots, int *items,
                                         int *item_count, cudaStream_t st);

@@ -18,6 +18,11 @@ cudaError_t discrete_launch_scan(const DiscArgs &A, bool mesh, unsigned grid, cu
     return cudaGetLastError();
 }
 
+cudaError_t discrete_launch_prologue(const DiscArgs &A, int M, cudaStream_t st) {
+    k_discrete_prologue<<<(unsigned)((M + PRO_SAMPLES - 1) / PRO_SAMPLES), PRO_SAMPLES, 0, st>>>(A);
+    return cudaGetLastError();
+}
+
 cudaError_t discrete_launch_epilogue(const DiscArgs &A, cudaStream_t st) {
     k_discrete_epilogue<<<(unsigned)A.N, EPI_THREADS, 0, st>>>(A);
     return cudaGetLastError();

@@ -765,6 +765,34 @@ class Evaluator:
         if self.lib.isdf_dbg_schedule(self.h, int(natural_order), int(warp_slots)) != 0:
             raise IsdfError(-1, "isdf_dbg_schedule failed")
 
+    def dbg_window_lists(self, budget=-1, arrays=False):
+        """window lists of the last mesh evaluation with collision (k_discrete_prologue). budget >= 0 sets the list capacity of the
+        following evaluations in codes per sample of the trajectory, i.e. budget x world per local sample of a shard (0: no lists, the
+        scan kernel enumerates every window itself). Returns
+        dict(runs, written, overflow, samples, capacity, requested) and, with arrays, pose (M x 8: position, quaternion w x y z, unused),
+        desc (M x 2: list offset or -1, voxel count) and codes (uint32: dx | dy << 10 | dz << 20). With budget >= 0 and nothing
+        evaluated yet, returns None."""
+        vp, lp, dp = C.c_void_p, C.POINTER(C.c_longlong), C.POINTER(C.c_double)
+        ip, up = C.POINTER(C.c_int32), C.POINTER(C.c_uint32)
+        self.lib.isdf_dbg_window_lists.argtypes = [vp, C.c_int, lp, dp, ip, up]
+        if self.lib.isdf_dbg_window_lists(self.h, int(budget), None, None, None, None) != 0:
+            raise IsdfError(-1, "isdf_dbg_window_lists failed")
+        st = np.zeros(6, dtype=np.int64)
+        r = self.lib.isdf_dbg_window_lists(self.h, -1, st.ctypes.data_as(lp), None, None, None)
+        if r == -2 and budget >= 0:
+            return None
+        if r != 0:
+            raise IsdfError(r, "isdf_dbg_window_lists failed (no mesh evaluation with collision yet?)")
+        out = dict(runs=int(st[0]), written=int(st[1]), overflow=int(st[2]), samples=int(st[3]), capacity=int(st[4]), requested=int(st[5]))
+        if arrays:
+            M = out["samples"]
+            pose, desc = np.zeros((M, 8)), np.zeros((M, 2), dtype=np.int32)
+            codes = np.zeros(max(min(out["requested"], out["capacity"]), 1), dtype=np.uint32)
+            if self.lib.isdf_dbg_window_lists(self.h, -1, None, _dp(pose), desc.ctypes.data_as(ip), codes.ctypes.data_as(up)) != 0:
+                raise IsdfError(-1, "isdf_dbg_window_lists failed")
+            out.update(pose=pose, desc=desc, codes=codes[:min(out["requested"], out["capacity"])])
+        return out
+
     def dbg_item_stats(self):
         n, parts = C.c_int(0), C.c_int(0)
         self.lib.isdf_dbg_item_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
