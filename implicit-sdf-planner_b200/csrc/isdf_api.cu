@@ -81,6 +81,11 @@ struct isdf_ctx {
         long long wl_samples = 0, wl_cap = 0;  // local samples and list capacity of the last launch with a prologue
         bool no_items = false;       // diagnostics: always launch in natural order, never split (isdf_dbg_schedule)
         int warp_slots_override = 0; // diagnostics: pretend the device has this many resident warps (forces splitting)
+        // the last launch, for isdf_dbg_item_table: its local samples and shard, whether its scan read a work-item table, and the
+        // builder it enqueued after itself (0 none, 1 k_build_items<true>, 2 k_build_items<false>) with that builder's arguments
+        long long last_M = 0;
+        int last_rank = 0, last_world = 1, last_max_split = 0, last_warp_slots = 0, last_builder = 0;
+        bool last_have_items = false;
     } disc;
     struct {   // host entry points of the discrete and swept-volume terms: one pinned block, one copy each way
         PinnedBuf<double> h;
@@ -965,11 +970,15 @@ static int launch_discrete(isdf_ctx *c, int N, const double *d_T, const double *
     CU_TRY(discrete_launch_scan(A, mesh, grid, st));
     CU_TRY(discrete_launch_epilogue(A, st));
     if (fused) c->peer.args.epoch = A.peer.epoch;
+    const int warp_slots = c->disc.warp_slots_override > 0 ? c->disc.warp_slots_override : c->warp_slots;
+    c->disc.last_M = M; c->disc.last_rank = c->rank; c->disc.last_world = c->world; c->disc.last_max_split = max_split;
+    c->disc.last_warp_slots = warp_slots; c->disc.last_have_items = have_items;
+    c->disc.last_builder = want_items ? (items_cached(M) ? 1 : 2) : 0;
     // build the next evaluation's work items on the aux stream: overlaps the caller's D2H / all-reduce / host work
     if (want_items) {
         CU_TRY(cudaEventRecord(c->ev_main_done, st));
         CU_TRY(cudaStreamWaitEvent(c->aux_stream, c->ev_main_done, 0));
-        CU_TRY(discrete_launch_build_items(c->disc.d_work.p, c->rank, c->world, (int)M, max_split, c->disc.warp_slots_override > 0 ? c->disc.warp_slots_override : c->warp_slots, c->disc.d_items.p, c->disc.d_item_count.p, c->aux_stream));
+        CU_TRY(discrete_launch_build_items(c->disc.d_work.p, c->rank, c->world, (int)M, max_split, warp_slots, c->disc.d_items.p, c->disc.d_item_count.p, c->aux_stream));
         CU_TRY(cudaEventRecord(c->ev_items_done, c->aux_stream));
         c->disc.items_pending = true;
         c->disc.order_for = sig;
@@ -2283,6 +2292,32 @@ extern "C" int isdf_dbg_item_stats(isdf_ctx *c, int *item_count, int *split_part
     int parts = 0;
     for (int k = 0; k < n; k++) if (it[3 * k + 2] >= 0) parts++;
     *item_count = n; *split_parts = parts;
+    return 0;
+}
+// the work-item table k_build_items built after the last discrete evaluation, with the work values it read. info (8 entries) =
+// {local samples M, rank, world, max_split, warp_slots, item_count (0 when no table was built), builder (0 none, 1 cached: work values
+// in registers, 2 uncached: re-read from memory), whether the last scan read a table}. items (item_count x 3: local sample, -1 or
+// c0 | c1 << 8, split slot or -1; up to cap_items rows) and work (M values d_work[rank + world m]) are optional. Read it before the
+// next evaluation: its scan overwrites the work values.
+extern "C" int isdf_dbg_item_table(isdf_ctx *c, long long *info, int *items, long long cap_items, unsigned *work) {
+    if (!c || !info) return -1;
+    if (c->disc.last_M == 0) return -2;
+    if (cudaSetDevice(c->device) != cudaSuccess) return -3;
+    if (cudaStreamSynchronize(c->stream) != cudaSuccess || cudaStreamSynchronize(c->aux_stream) != cudaSuccess) return -3;
+    int n = 0;
+    if (c->disc.last_builder && cudaMemcpy(&n, c->disc.d_item_count.p, sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    const long long M = c->disc.last_M;
+    const long long v[8] = {M, c->disc.last_rank, c->disc.last_world, c->disc.last_max_split, c->disc.last_warp_slots, n, c->disc.last_builder,
+                            c->disc.last_have_items ? 1 : 0};
+    std::memcpy(info, v, sizeof(v));
+    const long long rows = std::min<long long>(n, std::max(cap_items, 0ll));
+    if (items && rows > 0 && cudaMemcpy(items, c->disc.d_items.p, sizeof(int) * 3 * rows, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (work) {
+        const size_t S = (size_t)(c->disc.last_rank + c->disc.last_world * (M - 1) + 1);
+        std::vector<unsigned> all(S);
+        if (cudaMemcpy(all.data(), c->disc.d_work.p, sizeof(unsigned) * S, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+        for (long long m = 0; m < M; m++) work[m] = all[(size_t)(c->disc.last_rank + c->disc.last_world * m)];
+    }
     return 0;
 }
 // the device flatness map and its adjoint as compiled into the epilogue kernel: vaj n x 9 (vel, acc, jer), grads n x 10

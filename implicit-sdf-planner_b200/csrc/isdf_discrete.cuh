@@ -54,6 +54,8 @@ constexpr int ANALYTIC_MIN_BLOCKS = 4;
 constexpr int MESH_MIN_BLOCKS = 4;
 constexpr int EPI_THREADS = 288;
 constexpr int ITEMS_CACHE = 24;   // k_build_items: samples per thread whose work value is kept in registers (M <= 24576: any single trajectory)
+// whether k_build_items keeps the work values of M local samples in registers (k_build_items<true>) or re-reads them (<false>)
+inline bool items_cached(long long M) { return M <= 1024ll * ITEMS_CACHE; }
 // window-list capacity in codes per sample of the trajectory (64 B; world x that per local sample of a shard): the bench trajectory
 // needs ~4.3 (305 runs + one forced run start per 128 samples, ~164 occupied voxels per window), a 19 %-occupancy map ~14; a run
 // that does not fit is enumerated by the scan kernel

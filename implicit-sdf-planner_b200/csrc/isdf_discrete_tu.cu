@@ -30,7 +30,7 @@ cudaError_t discrete_launch_epilogue(const DiscArgs &A, cudaStream_t st) {
 
 cudaError_t discrete_launch_build_items(const unsigned *work, int rank, int world, int M, int max_split, int warp_slots, int *items,
                                         int *item_count, cudaStream_t st) {
-    if (M <= 1024 * ITEMS_CACHE) k_build_items<true><<<1, 1024, 0, st>>>(work, rank, world, M, max_split, warp_slots, items, item_count);
+    if (items_cached(M)) k_build_items<true><<<1, 1024, 0, st>>>(work, rank, world, M, max_split, warp_slots, items, item_count);
     else k_build_items<false><<<1, 1024, 0, st>>>(work, rank, world, M, max_split, warp_slots, items, item_count);
     return cudaGetLastError();
 }

@@ -800,6 +800,25 @@ class Evaluator:
             raise IsdfError(-1, "isdf_dbg_item_stats failed")
         return n.value, parts.value
 
+    def dbg_item_table(self):
+        """the work-item table k_build_items built after the last discrete evaluation (isdf_dbg_item_table). Read it before the next
+        evaluation, whose scan overwrites the work values. Returns dict(M, rank, world, max_split, warp_slots, item_count,
+        builder ("none", "cached" or "uncached"), have_items: whether the last scan read a table,
+        items: item_count x 3 int32 {local sample m, part (-1 = every class, else c0 | c1 << 8), split slot or -1},
+        work: M uint32, the work values the builder read)"""
+        vp, lp, ip, up = C.c_void_p, C.POINTER(C.c_longlong), C.POINTER(C.c_int32), C.POINTER(C.c_uint32)
+        self.lib.isdf_dbg_item_table.argtypes = [vp, lp, ip, C.c_longlong, up]
+        info = np.zeros(8, dtype=np.int64)
+        r = self.lib.isdf_dbg_item_table(self.h, info.ctypes.data_as(lp), None, 0, None)
+        if r != 0:
+            raise IsdfError(r, "isdf_dbg_item_table failed (no discrete evaluation yet?)")
+        M, n = int(info[0]), int(info[5])
+        items, work = np.zeros((max(n, 1), 3), dtype=np.int32), np.zeros(M, dtype=np.uint32)
+        if self.lib.isdf_dbg_item_table(self.h, info.ctypes.data_as(lp), items.ctypes.data_as(ip), n, work.ctypes.data_as(up)) != 0:
+            raise IsdfError(-1, "isdf_dbg_item_table failed")
+        return dict(M=M, rank=int(info[1]), world=int(info[2]), max_split=int(info[3]), warp_slots=int(info[4]), item_count=n,
+                    builder=("none", "cached", "uncached")[int(info[6])], have_items=bool(info[7]), items=items[:n], work=work)
+
     def dbg_mesh_grid(self, arrays=True):
         """the current mesh's body-frame cell grid, copied to the host: dict(glo, gcell, ghd, gpad, sign_radius, list_reach, gdim) and,
         with arrays, cell_dist (float32) and cell_cnt (uint16; 0 = no candidate list) shaped gdim (z fastest)"""
