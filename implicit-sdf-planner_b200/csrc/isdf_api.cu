@@ -1228,7 +1228,12 @@ static int lbfgs_rounds(isdf_ctx *c, isdf_ctx::LbfgsBufs &lb, int B, int n, cons
         CU_TRY(cudaStreamSynchronize(st));
         ++rounds;
         if (*lb.h_active.p == 0) break;
-        if (prm->max_rounds > 0 && rounds >= prm->max_rounds) break;
+        if (prm->max_rounds > 0 && rounds >= prm->max_rounds) {   // instances still running end on their last accepted iterate, ret -1008
+            k_lbfgs_cap<<<(unsigned)((B + 63) / 64), 64, 0, st>>>(L);
+            c->stats.kernel_launches++;
+            CU_TRY(cudaGetLastError());
+            break;
+        }
     }
     // results: f = fx of every instance (scalar slot 0), return codes and counters
     CU_TRY(cudaMemcpy2DAsync(d_f, sizeof(double), L.sc, sizeof(double) * LB_NSCALAR, sizeof(double), B, cudaMemcpyDeviceToDevice, st));
@@ -1243,37 +1248,80 @@ static int lbfgs_rounds(isdf_ctx *c, isdf_ctx::LbfgsBufs &lb, int B, int n, cons
 extern "C" int isdf_lbfgs_batch_device(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc, double rho,
                                        const isdf_lbfgs_params *prm, double *d_x, double *d_f, int *d_ret, int *d_iterations, int *d_evaluations,
                                        int *rounds_out, void *cuda_stream) {
-    int r = callback_batch_check(c, B, N0);
-    if (r) return r;
-    if ((r = lbfgs_check(prm))) return r;
-    if (!d_head || !d_tail || !d_x || !d_f) return fail(ISDF_ERR_INVALID, "NULL device pointer");
-    if (set_device(c)) return ISDF_ERR_CUDA;
     cudaStream_t st = (cudaStream_t)cuda_stream;
-    return lbfgs_rounds(c, c->lbfgs, B, 4 * N0 - 3, prm, 0, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st,
-                        [&](const double *x, double *f, double *g) {
-                            return callback_batch_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, rho, x, f, g, st);
-                        });
+    auto poison_all = [&]() { if (c && d_f && B > 0 && cudaSetDevice(c->device) == cudaSuccess) { cudaMemsetAsync(d_f, 0xff, sizeof(double) * B, st); cudaStreamSynchronize(st); } };
+    int r = callback_batch_check(c, B, N0);
+    if (!r) r = lbfgs_check(prm);
+    if (!r && (!d_head || !d_tail || !d_x || !d_f)) r = fail(ISDF_ERR_INVALID, "NULL device pointer");
+    if (!r && set_device(c)) r = ISDF_ERR_CUDA;
+    if (!r) r = lbfgs_rounds(c, c->lbfgs, B, 4 * N0 - 3, prm, 0, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st,
+                             [&](const double *x, double *f, double *g) {
+                                 return callback_batch_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, rho, x, f, g, st);
+                             });
+    if (r) poison_all();
+    return r;
 }
 
 extern "C" int isdf_lbfgs_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc, double rho,
                                 const isdf_lbfgs_params *prm, double *x, double *f, int *ret, int *iterations, int *evaluations, int *rounds_out) {
+    auto poison_all = [&]() { if (f && B > 0) for (int b = 0; b < B; b++) f[b] = std::numeric_limits<double>::quiet_NaN(); };
     int r = callback_batch_check(c, B, N0);
-    if (r) return r;
-    if (!head || !tail || !x || !f) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (r) { poison_all(); return r; }
+    if (!head || !tail || !x || !f) { poison_all(); return fail(ISDF_ERR_INVALID, "NULL argument"); }
+    auto body = [&]() -> int {
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        const size_t n = (size_t)4 * N0 - 3;
+        CU_TRY(c->lbfgs.d_x.upload(x, n * B, c->stream));
+        const double *d_head, *d_tail;
+        if (int rr = upload_bc(c, B, per_problem_bc, head, tail, &d_head, &d_tail)) return rr;
+        CU_TRY(c->lbfgs.d_f.ensure(B)); CU_TRY(c->lbfgs.d_head.ensure((size_t)3 * B));
+        if (int rr = isdf_lbfgs_batch_device(c, B, N0, d_head, d_tail, per_problem_bc, rho, prm, c->lbfgs.d_x.p, c->lbfgs.d_f.p, c->lbfgs.d_head.p,
+                                             c->lbfgs.d_head.p + B, c->lbfgs.d_head.p + 2 * (size_t)B, rounds_out, c->stream)) return rr;
+        CU_TRY(cudaMemcpy(x, c->lbfgs.d_x.p, sizeof(double) * n * B, cudaMemcpyDeviceToHost));
+        CU_TRY(cudaMemcpy(f, c->lbfgs.d_f.p, sizeof(double) * B, cudaMemcpyDeviceToHost));
+        if (ret) CU_TRY(cudaMemcpy(ret, c->lbfgs.d_head.p, sizeof(int) * B, cudaMemcpyDeviceToHost));
+        if (iterations) CU_TRY(cudaMemcpy(iterations, c->lbfgs.d_head.p + B, sizeof(int) * B, cudaMemcpyDeviceToHost));
+        if (evaluations) CU_TRY(cudaMemcpy(evaluations, c->lbfgs.d_head.p + 2 * (size_t)B, sizeof(int) * B, cudaMemcpyDeviceToHost));
+        return 0;
+    };
+    r = body();
+    if (r) poison_all();
+    return r;
+}
+
+// Diagnostic (not part of include/isdf.h): the unchanged lbfgs_rounds + k_lbfgs_feed for B instances of dimension n on a HOST objective.
+// Every round copies all B requested points (finished instances' included: they ride along unchanged) to the host, calls
+// eval(user, B, n, x, f, g) and uploads f and g. x: B x n (in: starting points, out: solutions); f, ret, iterations, evaluations: B
+// (ret / iterations / evaluations may be NULL); rounds: the rounds run (may be NULL).
+typedef void (*isdf_dbg_lbfgs_eval_t)(void *user, int B, int n, const double *x, double *f, double *g);
+extern "C" int isdf_dbg_lbfgs_rounds(isdf_ctx *c, int B, int n, const isdf_lbfgs_params *prm, int cancel_after, isdf_dbg_lbfgs_eval_t eval, void *user,
+                                     double *x, double *f, int *ret, int *iterations, int *evaluations, int *rounds_out) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (B < 1 || n < 1 || (long long)B * n > 0x7fffffffll || cancel_after < 0) return fail(ISDF_ERR_INVALID, "B < 1, n < 1, B*n overflows or cancel_after < 0");
+    if (int r = lbfgs_check(prm)) return r;
+    if (!eval || !x || !f) return fail(ISDF_ERR_INVALID, "NULL argument");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    const size_t n = (size_t)4 * N0 - 3;
-    CU_TRY(c->lbfgs.d_x.upload(x, n * B, c->stream));
-    const double *d_head, *d_tail;
-    if ((r = upload_bc(c, B, per_problem_bc, head, tail, &d_head, &d_tail))) return r;
-    CU_TRY(c->lbfgs.d_f.ensure(B)); CU_TRY(c->lbfgs.d_head.ensure((size_t)3 * B));
-    r = isdf_lbfgs_batch_device(c, B, N0, d_head, d_tail, per_problem_bc, rho, prm, c->lbfgs.d_x.p, c->lbfgs.d_f.p, c->lbfgs.d_head.p, c->lbfgs.d_head.p + B,
-                                c->lbfgs.d_head.p + 2 * (size_t)B, rounds_out, c->stream);
+    const size_t bn = (size_t)B * n;
+    isdf_ctx::LbfgsBufs &lb = c->lbfgs;
+    CU_TRY(lb.d_x.upload(x, bn, c->stream));
+    CU_TRY(lb.d_f.ensure(B)); CU_TRY(lb.d_head.ensure((size_t)3 * B));
+    std::vector<double> hx(bn), hf(B), hg(bn);
+    int r = lbfgs_rounds(c, lb, B, n, prm, cancel_after, lb.d_x.p, lb.d_f.p, lb.d_head.p, lb.d_head.p + B, lb.d_head.p + 2 * (size_t)B, rounds_out, c->stream,
+                         [&](const double *d_x, double *d_f, double *d_g) -> int {
+                             CU_TRY(cudaMemcpyAsync(hx.data(), d_x, sizeof(double) * bn, cudaMemcpyDeviceToHost, c->stream));
+                             CU_TRY(cudaStreamSynchronize(c->stream));
+                             eval(user, B, n, hx.data(), hf.data(), hg.data());
+                             CU_TRY(cudaMemcpyAsync(d_f, hf.data(), sizeof(double) * B, cudaMemcpyHostToDevice, c->stream));
+                             CU_TRY(cudaMemcpyAsync(d_g, hg.data(), sizeof(double) * bn, cudaMemcpyHostToDevice, c->stream));
+                             CU_TRY(cudaStreamSynchronize(c->stream));
+                             return 0;
+                         });
     if (r) return r;
-    CU_TRY(cudaMemcpy(x, c->lbfgs.d_x.p, sizeof(double) * n * B, cudaMemcpyDeviceToHost));
-    CU_TRY(cudaMemcpy(f, c->lbfgs.d_f.p, sizeof(double) * B, cudaMemcpyDeviceToHost));
-    if (ret) CU_TRY(cudaMemcpy(ret, c->lbfgs.d_head.p, sizeof(int) * B, cudaMemcpyDeviceToHost));
-    if (iterations) CU_TRY(cudaMemcpy(iterations, c->lbfgs.d_head.p + B, sizeof(int) * B, cudaMemcpyDeviceToHost));
-    if (evaluations) CU_TRY(cudaMemcpy(evaluations, c->lbfgs.d_head.p + 2 * (size_t)B, sizeof(int) * B, cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(x, lb.d_x.p, sizeof(double) * bn, cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(f, lb.d_f.p, sizeof(double) * B, cudaMemcpyDeviceToHost));
+    if (ret) CU_TRY(cudaMemcpy(ret, lb.d_head.p, sizeof(int) * B, cudaMemcpyDeviceToHost));
+    if (iterations) CU_TRY(cudaMemcpy(iterations, lb.d_head.p + B, sizeof(int) * B, cudaMemcpyDeviceToHost));
+    if (evaluations) CU_TRY(cudaMemcpy(evaluations, lb.d_head.p + 2 * (size_t)B, sizeof(int) * B, cudaMemcpyDeviceToHost));
     return 0;
 }
 

@@ -187,4 +187,24 @@ __global__ void __launch_bounds__(64) k_lbfgs_feed(const LbfgsArgs A) {
     if (phase != LB_DONE) atomicAdd(A.active, 1);
 }
 
+// A round cap (isdf_lbfgs_params::max_rounds) that ends the rounds while instances are still running: each of them stops as it would
+// under max_iterations = its iterations so far, on its last accepted iterate. Inside a line search that is xp / finit (x holds the next,
+// never evaluated, trial); waiting for a direction-reset evaluation, x / fx already are. Before any accepted iteration both are x0 / f(x0).
+__global__ void __launch_bounds__(64) k_lbfgs_cap(const LbfgsArgs A) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= A.B) return;
+    int *st = A.st + (size_t)b * LB_NINT;
+    const int phase = st[0];
+    if (phase == LB_DONE) return;
+    const int n = A.n;
+    double *sc = A.sc + (size_t)b * LB_NSCALAR;
+    if (phase == LB_WANT_LS) {
+        double *x = A.x + (size_t)b * n;
+        const double *xp = A.xp + (size_t)b * n;
+        for (int i = 0; i < n; i++) x[i] = xp[i];
+        sc[0] = sc[3];   // fx = finit
+    }
+    st[0] = LB_DONE; st[1] = LBERR_MAXIMUMITERATION;
+}
+
 }  // namespace isdf

@@ -57,15 +57,33 @@ int isdf_host_read_obj(const char *path, double *V, int capV, int32_t *F, int ca
 int isdf_host_set_shape_obj(isdf_ctx *ctx, const char *path, const double *poly_params6) { return set_shape_obj(ctx, path, poly_params6); }
 double isdf_host_shape_sdf_grad(isdf_ctx *ctx, const double *p, double *grad) { DeviceShape s(ctx); return s.getSDFwithGrad1(p, grad); }
 
-// L-BFGS on any raw callback (known-answer tests, CPU baseline with the oracle as the callback) ...
-int isdf_host_lbfgs_generic(int n, double *x, double *f, lbfgs_eval_raw_t eval, void *instance, int mem_size, int past, double delta,
-                            double g_epsilon, int max_iterations, int *iterations, int *evaluations) {
+// the full lbfgs_parameter_t but s_curv_coeff (unused by the fork's Armijo-only line search) and the off-by-default with_tole_ls /
+// cast_x_range; min_step 1e-32 is config_CappedCone.yaml:101
+static LbfgsParams lbfgs_params(int mem_size, int past, double delta, double g_epsilon, int max_iterations, int max_linesearch, double min_step,
+                                double max_step, double f_dec_coeff, double cautious_factor, double machine_prec) {
     LbfgsParams pr; pr.mem_size = mem_size; pr.past = past; pr.delta = delta; pr.g_epsilon = g_epsilon; pr.max_iterations = max_iterations;
-    pr.min_step = 1.0e-32;                                   // config_CappedCone.yaml:101
+    pr.max_linesearch = max_linesearch; pr.min_step = min_step; pr.max_step = max_step; pr.f_dec_coeff = f_dec_coeff;
+    pr.cautious_factor = cautious_factor; pr.machine_prec = machine_prec;
+    return pr;
+}
+
+// L-BFGS on any raw callback (known-answer tests, CPU baseline with the oracle as the callback) ...
+int isdf_host_lbfgs_generic_ex(int n, double *x, double *f, lbfgs_eval_raw_t eval, void *instance, int mem_size, int past, double delta,
+                               double g_epsilon, int max_iterations, int max_linesearch, double min_step, double max_step, double f_dec_coeff,
+                               double cautious_factor, double machine_prec, int *iterations, int *evaluations) {
+    const LbfgsParams pr = lbfgs_params(mem_size, past, delta, g_epsilon, max_iterations, max_linesearch, min_step, max_step, f_dec_coeff,
+                                        cautious_factor, machine_prec);
     LbfgsStats st; double fx = 0;
     const int r = lbfgs_optimize(n, x, fx, eval, nullptr, nullptr, instance, pr, &st);
     *f = fx; if (iterations) *iterations = st.iterations; if (evaluations) *evaluations = st.evaluations;
     return r;
+}
+// the same with the line-search parameters at lbfgs_parameter_t's defaults (min_step: config_CappedCone.yaml's); callers built against this
+// signature keep working
+int isdf_host_lbfgs_generic(int n, double *x, double *f, lbfgs_eval_raw_t eval, void *instance, int mem_size, int past, double delta,
+                            double g_epsilon, int max_iterations, int *iterations, int *evaluations) {
+    return isdf_host_lbfgs_generic_ex(n, x, f, eval, instance, mem_size, past, delta, g_epsilon, max_iterations, 64, 1.0e-32, 1.0e+20, 1.0e-4, 1.0e-6,
+                                      1.0e-16, iterations, evaluations);
 }
 // ... and on the GPU-backed callback (BackEnd::costFunctionLbfgs)
 int isdf_host_lbfgs_backend(void *be, double *x, int n, double *f, int mem_size, int past, double delta, double g_epsilon, int max_iterations,
@@ -74,15 +92,23 @@ int isdf_host_lbfgs_backend(void *be, double *x, int n, double *f, int mem_size,
 }
 
 // lock-step batched driver on any batched callback (CPU tests: identical to the sequential driver instance by instance) ...
-int isdf_host_lbfgs_batch_generic(int B, int n, double *x, double *f, int *ret, lbfgs_eval_batch_t eval, void *instance, int mem_size, int past,
-                                  double delta, double g_epsilon, int max_iterations, int *iterations, int *evaluations) {
-    LbfgsParams pr; pr.mem_size = mem_size; pr.past = past; pr.delta = delta; pr.g_epsilon = g_epsilon; pr.max_iterations = max_iterations;
-    pr.min_step = 1.0e-32;
+int isdf_host_lbfgs_batch_generic_ex(int B, int n, double *x, double *f, int *ret, lbfgs_eval_batch_t eval, void *instance, int mem_size, int past,
+                                     double delta, double g_epsilon, int max_iterations, int max_linesearch, double min_step, double max_step,
+                                     double f_dec_coeff, double cautious_factor, double machine_prec, int cancel_after, int *iterations, int *evaluations) {
+    LbfgsParams pr = lbfgs_params(mem_size, past, delta, g_epsilon, max_iterations, max_linesearch, min_step, max_step, f_dec_coeff, cautious_factor,
+                                  machine_prec);
+    pr.cancel_after = cancel_after;
     if (B < 1 || n < 1 || mem_size < 1) return -1;
     std::vector<LbfgsStats> st(B);
     const int rounds = lbfgs_optimize_batch(B, n, x, f, ret, eval, instance, pr, st.data());
     for (int b = 0; b < B; b++) { if (iterations) iterations[b] = st[b].iterations; if (evaluations) evaluations[b] = st[b].evaluations; }
     return rounds;
+}
+// the same with the line-search parameters at their defaults and no cancel rule (the signature older callers were built against)
+int isdf_host_lbfgs_batch_generic(int B, int n, double *x, double *f, int *ret, lbfgs_eval_batch_t eval, void *instance, int mem_size, int past,
+                                  double delta, double g_epsilon, int max_iterations, int *iterations, int *evaluations) {
+    return isdf_host_lbfgs_batch_generic_ex(B, n, x, f, ret, eval, instance, mem_size, past, delta, g_epsilon, max_iterations, 64, 1.0e-32, 1.0e+20,
+                                            1.0e-4, 1.0e-6, 1.0e-16, 0, iterations, evaluations);
 }
 // ... and on the device callback for B random-restart problems (isdf_callback_batch: MINCO + time-integral/collision term + adjoint)
 struct BatchBackEnd { isdf_ctx *ctx; int N0; const double *heads, *tails; double rho; std::vector<double> h, t; int status; };

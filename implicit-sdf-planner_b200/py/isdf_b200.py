@@ -457,6 +457,43 @@ class Evaluator:
                                               evs.ctypes.data_as(ip), C.byref(rounds)))
         return dict(x=x.reshape(B, dim), f=f, ret=ret, iterations=it, evaluations=evs, rounds=rounds.value)
 
+    def lbfgs_batch_device(self, B, N0, d_head, d_tail, per_problem_bc, rho, d_x, d_f, d_ret=None, d_iterations=None, d_evaluations=None, params=None,
+                           stream=None):
+        """isdf_lbfgs_batch_device on raw device pointers (e.g. torch .data_ptr()); returns the rounds"""
+        p = params if params is not None else self.lbfgs_params()
+        rounds = C.c_int32(0)
+        self._check(self.lib.isdf_lbfgs_batch_device(self.h, B, N0, d_head, d_tail, int(per_problem_bc), float(rho), C.byref(p), d_x, d_f, d_ret,
+                                                     d_iterations, d_evaluations, C.byref(rounds), stream))
+        return rounds.value
+
+    _DBG_LBFGS_EVAL = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double))
+
+    def dbg_lbfgs_rounds(self, fun, X0, params=None, cancel_after=0):
+        """the device lock-step L-BFGS rounds (lbfgs_rounds + k_lbfgs_feed) on a host objective (isdf_dbg_lbfgs_rounds, not part of
+        include/isdf.h). fun(X (B, n)) -> (f (B,), G (B, n)) is called once per round with every instance's requested point, finished
+        instances included. Returns dict(x, f, ret, iterations, evaluations, rounds, trace): trace[r] is round r + 1's requested points."""
+        X = np.ascontiguousarray(_f64(X0)).copy()
+        B, n = X.shape
+        trace = []
+
+        def cb(_user, b, nn, xp, fp, gp):
+            xs = np.ctypeslib.as_array(xp, shape=(b, nn)).copy()
+            trace.append(xs)
+            fv, gv = fun(xs.copy())
+            np.ctypeslib.as_array(fp, shape=(b,))[:] = fv
+            np.ctypeslib.as_array(gp, shape=(b, nn))[:] = gv
+        cfn = self._DBG_LBFGS_EVAL(cb)
+        ip = C.POINTER(C.c_int32)
+        self.lib.isdf_dbg_lbfgs_rounds.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(LbfgsParams), C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_double),
+                                                   C.POINTER(C.c_double), ip, ip, ip, ip]
+        p = params if params is not None else self.lbfgs_params()
+        f = np.zeros(B)
+        ret, it, evs = (np.zeros(B, dtype=np.int32) for _ in range(3))
+        rounds = C.c_int32(0)
+        self._check(self.lib.isdf_dbg_lbfgs_rounds(self.h, B, n, C.byref(p), int(cancel_after), C.cast(cfn, C.c_void_p), None, _dp(X.reshape(-1)), _dp(f),
+                                                   ret.ctypes.data_as(ip), it.ctypes.data_as(ip), evs.ctypes.data_as(ip), C.byref(rounds)))
+        return dict(x=X, f=f, ret=ret, iterations=it, evaluations=evs, rounds=rounds.value, trace=np.array(trace).reshape(len(trace), B, n))
+
     # ---- mid-end: warm start of the back end (see include/isdf.h) ----
     def midend_params(self, **kw):
         """isdf_midend_default_params with overrides; keys of isdf_lbfgs_params (mem_size, delta, ...) go to the nested lbfgs block,

@@ -242,14 +242,18 @@ int isdf_get_batch_trajectories(isdf_ctx *ctx, double *T, double *coeffs, double
  * to the sequential driver host/isdf_lbfgs.hpp run on the same callback. The reference's own driver is single-instance (and its live LMBM
  * shim non-re-entrant, lmbm/lmbm.cpp:4-6). */
 typedef struct isdf_lbfgs_params {     /* lbfgs_parameter_t (lbfgs.hpp:40-142); with_tole_ls / cast_x_range off as in the shipped configs */
-    int32_t mem_size, past, max_iterations, max_linesearch;
-    int32_t max_rounds;                /* 0 = until every instance has stopped; otherwise a cap on batched evaluations */
+    int32_t mem_size;                  /* 1..64 */
+    int32_t past, max_iterations, max_linesearch;
+    int32_t max_rounds;                /* 0 = until every instance has stopped; otherwise a cap on batched evaluations. An instance still
+                                          running when the cap ends the call stops as under max_iterations = its iterations so far: x and f
+                                          are its last accepted iterate and its value (x0 and f(x0) before the first accepted iteration),
+                                          ret is LBFGSERR_MAXIMUMITERATION (-1008), iterations and evaluations are its counts so far */
     int32_t reserved_;
     double g_epsilon, delta, min_step, max_step, f_dec_coeff, cautious_factor, machine_prec;
 } isdf_lbfgs_params;
 int isdf_lbfgs_default_params(isdf_lbfgs_params *p);   /* config_CappedCone.yaml:99-102: mem 16, past 10, min_step 1e-32, g_epsilon 0, delta 1e-6 */
 /* x: B x (4*N0-3) in/out; f: B; ret / iterations / evaluations: B (any may be NULL); rounds: batched evaluations used (may be NULL).
- * head / tail / rho / per_problem_bc as isdf_callback_batch. */
+ * head / tail / rho / per_problem_bc as isdf_callback_batch. On failure every f[b] is NaN (d_f too, when ctx and d_f are valid). */
 int isdf_lbfgs_batch(isdf_ctx *ctx, int B, int N0, const double *head, const double *tail, int per_problem_bc, double rho,
                      const isdf_lbfgs_params *params, double *x, double *f, int32_t *ret, int32_t *iterations, int32_t *evaluations, int32_t *rounds);
 /* device-resident variant (all pointers on ctx's device; returns when every instance has stopped — one 4-byte read per round) */
@@ -287,7 +291,8 @@ int isdf_lbfgs_batch_device(isdf_ctx *ctx, int B, int N0, const double *d_head, 
  *                  search. ret >= 0 is getOriTraj's success (plan_manager.cpp:277 runs the back end only then). The final T and coeffs are
  *                  forwardT + MINCO of the returned x, whatever ret is. f is the cost at the returned x; where the reference's
  *                  lbfgs_optimize returns from its direction-norm test without writing f (lbfgs.hpp:814-817, code -1012), f is still
- *                  the cost at x.
+ *                  the cost at x. A plan still running when params.lbfgs.max_rounds ends the call reports ret = -1008
+ *                  (LBFGSERR_MAXIMUMITERATION, so not a success) with x, f, T and coeffs from its last accepted iterate.
  * Each problem's result is bit-identical to the sequential host driver on the same problem, alone or inside a batch.
  * The mid-end needs neither a map nor a shape. It has its own device buffers: it leaves isdf_get_batch_trajectories, the swept-volume
  * t* and persisted durations, the discrete work-item schedule and every isdf_stats field but kernel_launches as they were.

@@ -19,10 +19,13 @@ static double bridge_eval(void *inst, const Eigen::VectorXd &x, Eigen::VectorXd 
     return b->f(b->user, (int)x.size(), x.data(), g.data());
 }
 
-extern "C" int ref_lbfgs_optimize(int n, double *x, double *f, c_eval_t eval, void *user, int mem_size, int past, double delta, double g_epsilon,
-                                  int max_iterations, double min_step, long *evaluations) {
+extern "C" int ref_lbfgs_optimize_ex(int n, double *x, double *f, c_eval_t eval, void *user, int mem_size, int past, double delta, double g_epsilon,
+                                     int max_iterations, double min_step, int max_linesearch, double max_step, double f_dec_coeff, double cautious_factor,
+                                     double machine_prec, long *evaluations) {
     lbfgs::lbfgs_parameter_t pr;
     pr.mem_size = mem_size; pr.past = past; pr.delta = delta; pr.g_epsilon = g_epsilon; pr.max_iterations = max_iterations; pr.min_step = min_step;
+    pr.max_linesearch = max_linesearch; pr.max_step = max_step; pr.f_dec_coeff = f_dec_coeff; pr.cautious_factor = cautious_factor;
+    pr.machine_prec = machine_prec;
     Eigen::VectorXd xv(n);
     for (int i = 0; i < n; i++) xv(i) = x[i];
     Bridge b{eval, user, 0};
@@ -38,4 +41,13 @@ extern "C" int ref_lbfgs_optimize(int n, double *x, double *f, c_eval_t eval, vo
     *f = fx;
     if (evaluations) *evaluations = b.evals;
     return ret;
+}
+
+// the same with max_linesearch, max_step, f_dec_coeff, cautious_factor and machine_prec at lbfgs_parameter_t's defaults (the signature
+// older callers were built against)
+extern "C" int ref_lbfgs_optimize(int n, double *x, double *f, c_eval_t eval, void *user, int mem_size, int past, double delta, double g_epsilon,
+                                  int max_iterations, double min_step, long *evaluations) {
+    lbfgs::lbfgs_parameter_t d;
+    return ref_lbfgs_optimize_ex(n, x, f, eval, user, mem_size, past, delta, g_epsilon, max_iterations, min_step, d.max_linesearch, d.max_step,
+                                 d.f_dec_coeff, d.cautious_factor, d.machine_prec, evaluations);
 }

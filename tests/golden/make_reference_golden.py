@@ -11,7 +11,11 @@ Run in the build container (where /root/reference exists):  python tests/golden/
   grid_reference.npz  — the reference's map_manager/src/Gridmap3D.cpp: grid indices, cube centres, in-map flags and AABB gathers on seeded grids;
   ref_shapes_obj.npz  — the bytes of the OBJ files behind ref_meshes.npz, so that the product's OBJ reader is checked on the files themselves;
   sign_policy_reference.npz — the oracle's discrete cost and gradient with the reference-faithful sign s = 1 - 2 w (w from the reference-compiled
-                        FWN header) on the inputs of test_gpu_reference_pins.py::test_sign_policy_deviation_from_reference_faithful_fwn."""
+                        FWN header) on the inputs of test_gpu_reference_pins.py::test_sign_policy_deviation_from_reference_faithful_fwn;
+  lbfgs_branches_reference.npz — what the reference's utils/lbfgs.hpp does on every case of tests/lbfgs_cases.py: every evaluated point,
+                        solution, value, return code and evaluation count (for the one case pinned to the product's host driver, that
+                        driver's run, with the reference build's beside it under ref_*).
+`python tests/golden/make_reference_golden.py lbfgs_branches` writes only the last file (any of the functions below can be named)."""
 import os
 import sys
 import numpy as np
@@ -21,6 +25,7 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "implicit-sdf-planner_b200", "py"))
 import isdf_b200 as I          # noqa: E402
+import lbfgs_cases as LC       # noqa: E402
 import oracle_lib as O         # noqa: E402
 from test_reference_pins import flat_inputs, _minco_cases, _lbfgs_problems, _traj_times, _grid_cases   # noqa: E402
 from test_gpu_reference_pins import sign_policy_case, SIGN_POLICY_MESHES   # noqa: E402
@@ -62,6 +67,25 @@ def sign_policy_reference():
         out.update({f"{name}_cost": np.array(c), f"{name}_gradC": gC, f"{name}_gradT": gT})
     np.savez_compressed(os.path.join(HERE, "sign_policy_reference.npz"), **out)
     print("sign_policy_reference.npz written")
+
+
+def lbfgs_branches():
+    import host_lib as H
+    rl = O.RefLbfgs()
+    cs = LC.cases()
+    out = {"names": np.array([c["name"] for c in cs])}
+    for k, c in enumerate(cs):
+        f1, kw = LC.one(c["fun"]), LC.sequential_kwargs(c)
+        a = rl.minimize(f1, c["x0"], **kw)
+        runs = [("", a)]
+        if c["host_pinned"]:
+            runs = [("", H.lbfgs_minimize(f1, c["x0"], **kw)), ("ref_", a)]
+        for pre, r in runs:
+            out.update({f"c{k}_{pre}trace": np.array(r["trace"]).reshape(len(r["trace"]), -1), f"c{k}_{pre}x": r["x"], f"c{k}_{pre}f": np.array(r["f"]),
+                        f"c{k}_{pre}ret": np.array(r["ret"]), f"c{k}_{pre}evals": np.array(r["evaluations"])})
+        print(c["name"], a["ret"], a["evaluations"])
+    np.savez_compressed(os.path.join(HERE, "lbfgs_branches_reference.npz"), **out)
+    print("lbfgs_branches_reference.npz written")
 
 
 def main():
@@ -107,4 +131,10 @@ def main():
 
 
 if __name__ == "__main__":
-    main()
+    if len(sys.argv) > 1:
+        O.build()
+        for fn in sys.argv[1:]:
+            globals()[fn]()
+    else:
+        main()
+        lbfgs_branches()

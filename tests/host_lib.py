@@ -26,14 +26,15 @@ def lib():
         L.isdf_host_tau_maps.argtypes = [dp, C.c_int, dp, dp]
         L.isdf_host_shape_sdf_grad.restype = C.c_double
         L.isdf_host_shape_sdf_grad.argtypes = [C.c_void_p, dp, dp]
-        L.isdf_host_lbfgs_generic.argtypes = [C.c_int, dp, dp, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int,
-                                              C.POINTER(C.c_int), C.POINTER(C.c_int)]
+        L.isdf_host_lbfgs_generic_ex.argtypes = [C.c_int, dp, dp, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int,
+                                                 C.c_int] + [C.c_double] * 5 + [C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.isdf_host_lbfgs_backend.argtypes = [C.c_void_p, dp, C.c_int, dp, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int,
                                               C.POINTER(C.c_int), C.POINTER(C.c_int)]
         ip = C.POINTER(C.c_int)
         L.isdf_host_read_obj.argtypes = [C.c_char_p, dp, C.c_int, C.POINTER(C.c_int32), C.c_int, ip, ip]
         L.isdf_host_set_shape_obj.argtypes = [C.c_void_p, C.c_char_p, dp]
-        L.isdf_host_lbfgs_batch_generic.argtypes = [C.c_int, C.c_int, dp, dp, ip, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, ip, ip]
+        L.isdf_host_lbfgs_batch_generic_ex.argtypes = [C.c_int, C.c_int, dp, dp, ip, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double,
+                                                       C.c_int, C.c_int] + [C.c_double] * 5 + [C.c_int, ip, ip]
         L.isdf_host_lbfgs_batch_backend.argtypes = [C.c_void_p, C.c_int, C.c_int, dp, dp, C.c_double, dp, dp, ip, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int,
                                                     ip, ip, ip]
         _lib = L
@@ -43,8 +44,16 @@ def lib():
 EVAL_T = C.CFUNCTYPE(C.c_double, C.c_void_p, dp, dp, C.c_int, dp)   # lbfgs_eval_raw_t
 
 
-def lbfgs_minimize(fun, x0, mem_size=8, past=3, delta=1e-6, g_epsilon=1e-5, max_iterations=0):
-    """fun(x) -> (f, grad). Runs the product's L-BFGS driver on a python callback (KATs, CPU baseline)."""
+# lbfgs_parameter_t's defaults (lbfgs.hpp:40-142) but min_step, which is config_CappedCone.yaml:101's
+LS_DEFAULTS = dict(max_linesearch=64, min_step=1e-32, max_step=1e20, f_dec_coeff=1e-4, cautious_factor=1e-6, machine_prec=1e-16)
+
+
+def _ls_args(max_linesearch, min_step, max_step, f_dec_coeff, cautious_factor, machine_prec):
+    return [int(max_linesearch), float(min_step), float(max_step), float(f_dec_coeff), float(cautious_factor), float(machine_prec)]
+
+
+def lbfgs_minimize(fun, x0, mem_size=8, past=3, delta=1e-6, g_epsilon=1e-5, max_iterations=0, **ls):
+    """fun(x) -> (f, grad). Runs the product's L-BFGS driver on a python callback (KATs, CPU baseline). ls: any of LS_DEFAULTS' keys."""
     x = f(x0).copy()
     n = x.size
     count = [0]
@@ -60,16 +69,16 @@ def lbfgs_minimize(fun, x0, mem_size=8, past=3, delta=1e-6, g_epsilon=1e-5, max_
         return float(fv)
     cfn = EVAL_T(cb)
     fx, it, ev = C.c_double(0), C.c_int(0), C.c_int(0)
-    r = lib().isdf_host_lbfgs_generic(n, _p(x), C.byref(fx), C.cast(cfn, C.c_void_p), None, mem_size, past, delta, g_epsilon, max_iterations,
-                                      C.byref(it), C.byref(ev))
+    r = lib().isdf_host_lbfgs_generic_ex(n, _p(x), C.byref(fx), C.cast(cfn, C.c_void_p), None, mem_size, past, delta, g_epsilon, max_iterations,
+                                      *_ls_args(**{**LS_DEFAULTS, **ls}), C.byref(it), C.byref(ev))
     return dict(ret=r, x=x, f=fx.value, iterations=it.value, evaluations=ev.value, trace=trace)
 
 
 EVAL_BATCH_T = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.POINTER(C.c_int), dp, dp, dp)   # lbfgs_eval_batch_t
 
 
-def lbfgs_minimize_batch(fun, X0, mem_size=8, past=3, delta=1e-6, g_epsilon=1e-5, max_iterations=0):
-    """fun(id, x) -> (f, grad) per instance; B instances advanced in lock step by the product's batched driver."""
+def lbfgs_minimize_batch(fun, X0, mem_size=8, past=3, delta=1e-6, g_epsilon=1e-5, max_iterations=0, cancel_after=0, **ls):
+    """fun(id, x) -> (f, grad) per instance; B instances advanced in lock step by the product's batched driver. ls: as lbfgs_minimize."""
     X = f(X0).copy()
     B, n = X.shape
 
@@ -84,8 +93,9 @@ def lbfgs_minimize_batch(fun, X0, mem_size=8, past=3, delta=1e-6, g_epsilon=1e-5
     fx, ret, it, ev = np.zeros(B), np.zeros(B, dtype=np.int32), np.zeros(B, dtype=np.int32), np.zeros(B, dtype=np.int32)
     ip = C.POINTER(C.c_int)
     Xf = X.reshape(-1)
-    rounds = lib().isdf_host_lbfgs_batch_generic(B, n, _p(Xf), _p(fx), ret.ctypes.data_as(ip), C.cast(cfn, C.c_void_p), None, mem_size, past,
-                                                 delta, g_epsilon, max_iterations, it.ctypes.data_as(ip), ev.ctypes.data_as(ip))
+    rounds = lib().isdf_host_lbfgs_batch_generic_ex(B, n, _p(Xf), _p(fx), ret.ctypes.data_as(ip), C.cast(cfn, C.c_void_p), None, mem_size, past,
+                                                 delta, g_epsilon, max_iterations, *_ls_args(**{**LS_DEFAULTS, **ls}), int(cancel_after),
+                                                 it.ctypes.data_as(ip), ev.ctypes.data_as(ip))
     X = Xf.reshape(B, n)
     return dict(rounds=rounds, ret=ret, x=X, f=fx, iterations=it, evaluations=ev)
 

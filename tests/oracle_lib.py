@@ -314,8 +314,15 @@ class RefLbfgs:
         self.L.ref_lbfgs_optimize.argtypes = [C.c_int, dp, dp, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_double,
                                               C.POINTER(C.c_long)]
         self.L.ref_lbfgs_optimize.restype = C.c_int
+        # the full parameter set; a library built from an older wrapper has only ref_lbfgs_optimize
+        self.full = hasattr(self.L, "ref_lbfgs_optimize_ex")
+        if self.full:
+            self.L.ref_lbfgs_optimize_ex.argtypes = self.L.ref_lbfgs_optimize.argtypes[:-1] + [C.c_int, C.c_double, C.c_double, C.c_double, C.c_double,
+                                                                                               C.POINTER(C.c_long)]
+            self.L.ref_lbfgs_optimize_ex.restype = C.c_int
 
-    def minimize(self, fun, x0, mem_size=8, past=3, delta=1e-6, g_epsilon=1e-5, max_iterations=0, min_step=1e-32):
+    def minimize(self, fun, x0, mem_size=8, past=3, delta=1e-6, g_epsilon=1e-5, max_iterations=0, min_step=1e-32, max_linesearch=64, max_step=1e20,
+                 f_dec_coeff=1e-4, cautious_factor=1e-6, machine_prec=1e-16):
         """fun(x) -> (f, grad); returns ret, x, f, evaluations and the list of every point the optimiser evaluated"""
         x = f64(x0).copy()
         n = x.size
@@ -329,8 +336,14 @@ class RefLbfgs:
             return float(fv)
         cfn = self.EVAL_T(cb)
         fx, ev = C.c_double(0), C.c_long(0)
-        r = self.L.ref_lbfgs_optimize(n, _p(x), C.byref(fx), C.cast(cfn, C.c_void_p), None, mem_size, past, delta, g_epsilon, max_iterations, min_step,
-                                      C.byref(ev))
+        ls = (max_linesearch, max_step, f_dec_coeff, cautious_factor, machine_prec)
+        args = (n, _p(x), C.byref(fx), C.cast(cfn, C.c_void_p), None, mem_size, past, delta, g_epsilon, max_iterations, min_step)
+        if self.full:
+            r = self.L.ref_lbfgs_optimize_ex(*args, *ls, C.byref(ev))
+        elif ls == (64, 1e20, 1e-4, 1e-6, 1e-16):    # lbfgs_parameter_t's defaults, what ref_lbfgs_optimize sets
+            r = self.L.ref_lbfgs_optimize(*args, C.byref(ev))
+        else:
+            raise RuntimeError(f"{REF_LBFGS} predates ref_lbfgs_optimize_ex: rebuild it (make -C oracle ref) to set the line-search parameters")
         return dict(ret=r, x=x, f=fx.value, evaluations=ev.value, trace=trace)
 
 

@@ -80,4 +80,13 @@ def test_lbfgs_batch_argument_validation():
     with pytest.raises(I.IsdfError) as e:
         ev.lbfgs_batch(heads, tails, 20.0, X, bad)
     assert e.value.code == -1
+    # mem_size 1..64 (the history ring's bound); a refused call leaves f NaN
+    assert np.all(np.isfinite(ev.lbfgs_batch(heads, tails, 20.0, X, ev.lbfgs_params(mem_size=64, max_iterations=3))["f"]))
+    hh = np.ascontiguousarray(np.swapaxes(heads, 1, 2)).reshape(-1)
+    tt = np.ascontiguousarray(np.swapaxes(tails, 1, 2)).reshape(-1)
+    for p in (ev.lbfgs_params(mem_size=65), bad):
+        x, f = np.ascontiguousarray(X).copy(), np.zeros(2)
+        r = ev.lib.isdf_lbfgs_batch(ev.h, 2, 4, hh.ctypes.data_as(C.POINTER(C.c_double)), tt.ctypes.data_as(C.POINTER(C.c_double)), 1, 20.0, C.byref(p),
+                                    x.ctypes.data_as(C.POINTER(C.c_double)), f.ctypes.data_as(C.POINTER(C.c_double)), None, None, None, None)
+        assert r == -1 and np.all(np.isnan(f))
     ev.close()
