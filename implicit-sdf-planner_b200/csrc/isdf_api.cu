@@ -10,6 +10,7 @@
 #include "isdf_lbfgs.cuh"
 #include "isdf_midend.cuh"
 #include "isdf_clearance.cuh"
+#include "isdf_certify.cuh"
 #include "isdf_map.cuh"
 #include <queue>
 #include "isdf_host_mesh.cuh"
@@ -123,6 +124,12 @@ struct isdf_ctx {
         DevBuf<double> d_in, d_clear; DevBuf<long long> d_vox; DevBuf<ClrSummary> d_sum; DevBuf<int> d_cursor;
         DevBuf<unsigned long long> d_counters;   // {candidate pairs, exact mesh searches} of the last check (isdf_dbg_clearance_counts)
     } clr;
+    struct {   // continuous certificate (isdf_certify.cuh): samples, the two interval lists of the round loop, leaves, per-trajectory state
+        DevBuf<double> d_in, d_toff, d_st, d_sc; DevBuf<int> d_sp, d_hit, d_tot, d_cursor; DevBuf<long long> d_sv;
+        DevBuf<CertInterval> d_iv[2]; DevBuf<CertScratch> d_scr; DevBuf<CertLeaf> d_leaves; DevBuf<CertTraj> d_traj; DevBuf<CertSummary> d_sum;
+        PinnedBuf<int> h_tot;
+        long long last_leaves = 0;   // leaves of the last call (isdf_dbg_certify_leaves)
+    } cert;
     struct {   // peer-memory reduction (isdf_peer.cuh)
         DevBuf<char> buf;                    // own exchange buffer (exported through CUDA IPC)
         void *open[PEER_MAX] = {};           // peers' buffers opened here (null for self / unused)
@@ -1574,7 +1581,7 @@ static int clearance_check(isdf_ctx *c, int N, const isdf_clearance_params *p) {
 
 static int clearance_launch_ctx(isdf_ctx *c, int N, const double *d_T, const double *d_C, const isdf_clearance_params *p, double *d_clear,
                                 long long *d_vox, ClrSummary *d_sum, cudaStream_t st) {
-    ClrArgs A;
+    ClrArgs A = {};   // no sample list, no hit flags: the uniform samples of the definition
     A.grid = c->map.grid; A.shape = c->mesh.shape; A.fp = c->dcfg.fp; A.half_bd = c->dcfg.half_bd;
     A.reach = p->reach; A.margin = p->margin;
     A.N = N; A.K = p->samples_per_piece; A.N0 = p->pieces_per_traj == 0 ? N : p->pieces_per_traj;
@@ -1648,6 +1655,181 @@ extern "C" int isdf_trajectory_clearance(isdf_ctx *c, int N, const double *T, co
     r = body();
     if (r) clearance_poison_host(N, p, summary);
     return r;
+}
+
+// ---- continuous clearance certificate (isdf_certify.cuh) --------------------------------------------------------------------------
+extern "C" int isdf_certify_default_params(isdf_certify_params *p) {
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    std::memset(p, 0, sizeof(*p));
+    isdf_clearance_default_params(&p->clearance);
+    p->clearance.reach = 2.0 * p->clearance.margin;
+    p->max_depth = 16; p->max_samples_per_traj = 2048;
+    return 0;
+}
+
+// the shape conditions of the certificate (include/isdf.h): a true Euclidean distance outside the body and a body inside the half_bd box.
+// *r: the body radius about the body origin (0 for rotation-invariant bodies), padded against the rounding of its own computation
+static int certify_shape(isdf_ctx *c, double *r) {
+    if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
+    const DevShape &s = c->mesh.shape;
+    const double hb = c->dcfg.half_bd;
+    auto inside = [&](const double p[3]) { return std::fabs(p[0]) <= hb && std::fabs(p[1]) <= hb && std::fabs(p[2]) <= hb; };
+    double rr = 0.0;
+    if (s.kind == ISDF_SHAPE_BALL) {
+        if (!(s.par[0] >= 0.0 && s.par[0] <= hb)) return fail(ISDF_ERR_UNSUPPORTED, "certificate: the Ball's radius must lie in [0, half_bd]");
+    } else if (s.kind == ISDF_SHAPE_BOX) {
+        for (int i = 0; i < 3; i++)
+            for (int j = 0; j < 3; j++) {
+                const double d = s.rot[3 * i] * s.rot[3 * j] + s.rot[3 * i + 1] * s.rot[3 * j + 1] + s.rot[3 * i + 2] * s.rot[3 * j + 2];
+                if (!(std::fabs(d - (i == j ? 1.0 : 0.0)) <= 1e-12)) return fail(ISDF_ERR_UNSUPPORTED, "certificate: the Box rotation is not orthonormal to 1e-12");
+            }
+        if (!(s.par[0] >= 0.0 && s.par[1] >= 0.0 && s.par[2] >= 0.0)) return fail(ISDF_ERR_UNSUPPORTED, "certificate: negative Box half extents");
+        for (int k = 0; k < 8; k++) {   // body point of shape-frame corner q: Rotate q + trans (shape_pre inverted)
+            const double q[3] = {(k & 1) ? s.par[0] : -s.par[0], (k & 2) ? s.par[1] : -s.par[1], (k & 4) ? s.par[2] : -s.par[2]};
+            double p[3];
+            for (int j = 0; j < 3; j++) p[j] = s.rot[3 * j] * q[0] + s.rot[3 * j + 1] * q[1] + s.rot[3 * j + 2] * q[2] + s.trans[j];
+            if (!inside(p)) return fail(ISDF_ERR_UNSUPPORTED, "certificate: the Box reaches beyond the half_bd box");
+            rr = std::max(rr, std::sqrt(p[0] * p[0] + p[1] * p[1] + p[2] * p[2]));
+        }
+    } else if (s.kind == ISDF_SHAPE_MESH) {
+        if (s.mesh.sign_mode != MESH_SIGN_PSEUDONORMAL) return fail(ISDF_ERR_UNSUPPORTED, "certificate: a winding-sign mesh SDF is not a distance");
+        for (int k = 0; k < 8; k++) {
+            const double p[3] = {(k & 1) ? s.mesh.bhi[0] : s.mesh.blo[0], (k & 2) ? s.mesh.bhi[1] : s.mesh.blo[1], (k & 4) ? s.mesh.bhi[2] : s.mesh.blo[2]};
+            if (!inside(p)) return fail(ISDF_ERR_UNSUPPORTED, "certificate: the mesh's bounding box reaches beyond the half_bd box");
+            rr = std::max(rr, std::sqrt(p[0] * p[0] + p[1] * p[1] + p[2] * p[2]));
+        }
+    } else if (s.kind != ISDF_SHAPE_POINT) {
+        return fail(ISDF_ERR_UNSUPPORTED, "certificate: supported shapes are Ball, Point, Box and exact-sign meshes (their SDF is a distance)");
+    }
+    *r = rr * (1.0 + 1e-12);
+    return 0;
+}
+
+static int certify_batch(int N, const isdf_certify_params *p) { return p ? clearance_batch(N, &p->clearance) : 0; }
+
+// every check that needs no device work; *r as certify_shape
+static int certify_check(isdf_ctx *c, int N, const isdf_certify_params *p, double *r) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    if (p->reserved_[0] || p->reserved_[1]) return fail(ISDF_ERR_INVALID, "reserved_ must be 0");
+    if (p->max_depth < 0 || p->max_depth > 64) return fail(ISDF_ERR_INVALID, "max_depth must lie in [0, 64]");
+    if (p->max_samples_per_traj < 0) return fail(ISDF_ERR_INVALID, "max_samples_per_traj < 0");
+    const isdf_clearance_params &q = p->clearance;
+    if (!(q.margin >= 0.0) || !(q.margin < q.reach)) return fail(ISDF_ERR_INVALID, "the certificate needs 0 <= margin < reach");
+    if (int rr = clearance_check(c, N, &q)) return rr;
+    const long long B = certify_batch(N, p), K = q.samples_per_piece;
+    if ((long long)N * (2 * K + 1) + 3 * B * p->max_samples_per_traj > 0x7fffffffll)
+        return fail(ISDF_ERR_INVALID, "N (2 K_c + 1) + 3 B max_samples_per_traj must fit in 31 bits");
+    return certify_shape(c, r);
+}
+
+static CertArgs certify_args(isdf_ctx *c, double r, double reach, int N, const double *d_T, const double *d_C) {
+    CertArgs A = {};
+    A.fp = c->dcfg.fp; A.r = r; A.H = c->dcfg.half_bd + reach;
+    A.N = N; A.T = d_T; A.C = d_C;
+    return A;
+}
+
+static int certify_run(isdf_ctx *c, int N, const double *d_T, const double *d_C, const isdf_certify_params *p, double r, CertSummary *d_sum,
+                       cudaStream_t st) {
+    auto &z = c->cert;
+    const isdf_clearance_params &q = p->clearance;
+    const int K = q.samples_per_piece, N0 = q.pieces_per_traj == 0 ? N : q.pieces_per_traj, B = N / N0, M = p->max_samples_per_traj;
+    const size_t S0 = (size_t)N * (K + 1), I0 = (size_t)N * K, Smax = S0 + (size_t)B * M, Lmax = I0 + (size_t)B * M;
+    z.last_leaves = 0;
+    CU_TRY(z.d_toff.ensure(N)); CU_TRY(z.d_sp.ensure(Smax)); CU_TRY(z.d_st.ensure(Smax)); CU_TRY(z.d_sc.ensure(Smax)); CU_TRY(z.d_sv.ensure(Smax));
+    CU_TRY(z.d_hit.ensure(B)); CU_TRY(z.d_traj.ensure(B)); CU_TRY(z.d_tot.ensure(2)); CU_TRY(z.d_cursor.ensure(1)); CU_TRY(z.h_tot.ensure(1));
+    CU_TRY(z.d_iv[0].ensure(I0)); CU_TRY(z.d_leaves.ensure(Lmax));
+    CertArgs A = certify_args(c, r, q.reach, N, d_T, d_C);
+    A.margin = q.margin; A.K = K; A.N0 = N0; A.B = B; A.max_depth = p->max_depth; A.max_samples = M;
+    A.toff = z.d_toff.p; A.sp = z.d_sp.p; A.st = z.d_st.p; A.sc = z.d_sc.p; A.sv = z.d_sv.p; A.hit = z.d_hit.p;
+    A.leaves = z.d_leaves.p; A.traj = z.d_traj.p; A.summary = d_sum; A.tot = z.d_tot.p;
+    A.cur = z.d_iv[0].p;
+    CU_TRY(certify_init_launch(A, st));
+    c->stats.kernel_launches++;
+    // the scan: round 0 is the clearance check's own uniform samples, later rounds the new midpoints
+    ClrArgs S = {};
+    S.grid = c->map.grid; S.shape = c->mesh.shape; S.fp = c->dcfg.fp; S.half_bd = c->dcfg.half_bd;
+    S.reach = q.reach; S.margin = q.margin; S.N = N; S.K = K; S.N0 = N0; S.T = d_T; S.C = d_C;
+    S.clear = z.d_sc.p; S.voxel = z.d_sv.p; S.cursor = z.d_cursor.p; S.hit = z.d_hit.p;
+    const int mode = c->mesh.shape.kind != ISDF_SHAPE_MESH ? 0 : 1;   // winding-sign meshes are refused
+    auto scan = [&](long long n) -> int {
+        CU_TRY(cudaMemsetAsync(z.d_cursor.p, 0, sizeof(int), st));
+        const long long want = (n + CLR_WARPS - 1) / CLR_WARPS;
+        CU_TRY(clearance_scan_launch(S, mode, (unsigned)std::max<long long>(1, std::min(want, (long long)c->sm_count * c->clr_blocks)), st));
+        c->stats.kernel_launches++;
+        return 0;
+    };
+    if (int rr = scan((long long)S0)) return rr;
+    long long nact = (long long)I0, S_cur = (long long)S0, L_cur = 0;
+    int cur = 0;
+    for (;;) {
+        CU_TRY(z.d_iv[cur ^ 1].ensure((size_t)std::max(2 * nact, 1ll))); CU_TRY(z.d_scr.ensure((size_t)nact));
+        A.cur = z.d_iv[cur].p; A.next = z.d_iv[cur ^ 1].p; A.scr = z.d_scr.p;
+        A.S_cur = (int)S_cur; A.L_cur = (int)L_cur; A.nact = (int)nact;
+        CU_TRY(certify_round_launch(A, st));
+        c->stats.kernel_launches += 2;
+        CU_TRY(cudaMemcpyAsync(z.h_tot.p, z.d_tot.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
+        const long long ns = *z.h_tot.p;
+        L_cur += nact - ns;
+        if (ns == 0) break;
+        S.st = z.d_st.p + S_cur; S.sp = z.d_sp.p + S_cur; S.nlist = (int)ns; S.clear = z.d_sc.p + S_cur; S.voxel = z.d_sv.p + S_cur;
+        if (int rr = scan(ns)) return rr;
+        S_cur += ns; nact = 2 * ns; cur ^= 1;
+    }
+    CU_TRY(certify_finish_launch(A, st));
+    c->stats.kernel_launches++;
+    z.last_leaves = L_cur;
+    return 0;
+}
+
+// on failure every summary reads verdict 0 (UNDECIDED), lower_bound / min_clearance / t_min / first_hit NaN, counts -1
+static isdf_certify_summary certify_failed_summary() {
+    isdf_certify_summary s;
+    s.lower_bound = s.min_clearance = s.t_min = s.first_hit = std::numeric_limits<double>::quiet_NaN();
+    s.voxel_min = -1; s.verdict = 0; s.samples = s.undecided_intervals = s.depth = -1;
+    return s;
+}
+
+extern "C" int isdf_trajectory_certify_device(isdf_ctx *c, int N, const double *d_T, const double *d_coeffs, const isdf_certify_params *p,
+                                              isdf_certify_summary *d_summary, void *cuda_stream) {
+    double r = 0.0;
+    int rc = certify_check(c, N, p, &r);
+    if (rc == 0 && (!d_T || !d_coeffs || !d_summary)) rc = fail(ISDF_ERR_INVALID, "NULL device pointer");
+    if (rc == 0 && set_device(c)) rc = ISDF_ERR_CUDA;
+    if (rc == 0) rc = certify_run(c, N, d_T, d_coeffs, p, r, (CertSummary *)d_summary, (cudaStream_t)cuda_stream);
+    if (rc != 0 && c && d_summary && certify_batch(N, p) > 0) {   // best effort: the pointer itself may be what was wrong
+        std::vector<isdf_certify_summary> bad((size_t)certify_batch(N, p), certify_failed_summary());
+        cudaSetDevice(c->device);
+        cudaStreamSynchronize((cudaStream_t)cuda_stream);
+        cudaMemcpy(d_summary, bad.data(), sizeof(isdf_certify_summary) * bad.size(), cudaMemcpyHostToDevice);
+        cudaGetLastError();
+    }
+    return rc;
+}
+
+extern "C" int isdf_trajectory_certify(isdf_ctx *c, int N, const double *T, const double *coeffs, const isdf_certify_params *p,
+                                       isdf_certify_summary *summary) {
+    auto poison = [&]() { if (summary) for (int b = 0; b < std::max(certify_batch(N, p), 1); b++) summary[b] = certify_failed_summary(); };
+    double r = 0.0;
+    int rc = certify_check(c, N, p, &r);
+    if (rc == 0 && (!T || !coeffs || !summary)) rc = fail(ISDF_ERR_INVALID, "NULL argument");
+    if (rc) { poison(); return rc; }
+    auto body = [&]() -> int {
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        const int B = certify_batch(N, p);
+        CU_TRY(c->cert.d_in.ensure((size_t)19 * N)); CU_TRY(c->cert.d_sum.ensure((size_t)B));
+        CU_TRY(cudaMemcpyAsync(c->cert.d_in.p, coeffs, sizeof(double) * 18 * N, cudaMemcpyHostToDevice, c->stream));
+        CU_TRY(cudaMemcpyAsync(c->cert.d_in.p + 18 * (size_t)N, T, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
+        if (int rr = certify_run(c, N, c->cert.d_in.p + 18 * (size_t)N, c->cert.d_in.p, p, r, c->cert.d_sum.p, c->stream)) return rr;
+        CU_TRY(cudaMemcpyAsync(summary, c->cert.d_sum.p, sizeof(isdf_certify_summary) * B, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaStreamSynchronize(c->stream));
+        return 0;
+    };
+    rc = body();
+    if (rc) poison();
+    return rc;
 }
 
 // ---- multi-GPU: rank-ordered sum of the sharded evaluation through NVLink peer memory (isdf_peer.cuh) ------------------------------
@@ -2437,4 +2619,44 @@ extern "C" int isdf_dbg_clearance_counts(isdf_ctx *c, unsigned long long *out) {
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
     return cudaMemcpy(out, c->clr.d_counters.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -1;
+}
+
+// (D_a, D_b) of the certificate's motion bound for caller-given intervals (piece, ta, tb) of a trajectory block (T, coeffs: N pieces);
+// out: 2n doubles; *radius (may be NULL): the body radius r the bound used. Needs a supported shape, not a map. Diagnostic; not part
+// of include/isdf.h.
+extern "C" int isdf_dbg_certify_bound(isdf_ctx *c, int N, const double *T, const double *coeffs, double reach, int n, const int32_t *piece,
+                                      const double *ta, const double *tb, double *out, double *radius) {
+    if (!c || N < 1 || n < 1 || !T || !coeffs || !piece || !ta || !tb || !out || !(reach > 0.0)) return fail(ISDF_ERR_INVALID, "bad argument");
+    for (int k = 0; k < n; k++) if (piece[k] < 0 || piece[k] >= N) return fail(ISDF_ERR_INVALID, "piece out of range");
+    double r = 0.0;
+    if (int rr = certify_shape(c, &r)) return rr;
+    if (radius) *radius = r;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    DevBuf<double> d;
+    CU_TRY(d.ensure((size_t)19 * N + 4 * (size_t)n));
+    DevBuf<int> dp;
+    CU_TRY(dp.upload(piece, n, c->stream));
+    double *dC = d.p, *dT = d.p + 18 * (size_t)N, *dta = dT + N, *dtb = dta + n, *dout = dtb + n;
+    CU_TRY(cudaMemcpyAsync(dC, coeffs, sizeof(double) * 18 * N, cudaMemcpyHostToDevice, c->stream));
+    CU_TRY(cudaMemcpyAsync(dT, T, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
+    CU_TRY(cudaMemcpyAsync(dta, ta, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
+    CU_TRY(cudaMemcpyAsync(dtb, tb, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
+    const CertArgs A = certify_args(c, r, reach, N, dT, dC);
+    CU_TRY(certify_bound_launch(A, n, dp.p, dta, dtb, dout, c->stream));
+    c->stats.kernel_launches++;
+    CU_TRY(cudaMemcpyAsync(out, dout, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+// the final leaf intervals of the last certificate call: records {ta, tb, c_a, c_b, D_a, D_b (double); piece (index in the call's block),
+// state (1 safe, 0 undecided, -1 dropped) (int32)}, 56 bytes each, in the order they were finished; *n = their number, at most cap copied
+extern "C" int isdf_dbg_certify_leaves(isdf_ctx *c, void *out, long long cap, long long *n) {
+    if (!c || !n || cap < 0 || (cap > 0 && !out)) return fail(ISDF_ERR_INVALID, "bad argument");
+    *n = c->cert.last_leaves;
+    const long long k = std::min(cap, c->cert.last_leaves);
+    if (k == 0) return 0;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    CU_TRY(cudaMemcpy(out, c->cert.d_leaves.p, sizeof(CertLeaf) * (size_t)k, cudaMemcpyDeviceToHost));
+    return 0;
 }

@@ -22,6 +22,8 @@
 //     pseudonormal. Culls are strict (> b), so a candidate that TIES b is still answered and the (value, address) key decides.
 //   * winding-sign meshes (s = 1 - 2 w, not a distance): every candidate in the H box is answered exactly (unbounded nearest triangle,
 //     hierarchical winding number), as the discrete path does in that mode.
+//   * sample lists: with ClrArgs::st set, the same kernel scans caller-given (piece, local time) samples — the refinement rounds of
+//     the certificate (isdf_certify.cuh). The uniform path and its outputs are unchanged.
 //   * k_clearance_summary — one CTA per trajectory: min / first attaining sample / first hit / count over its samples. Only minima and
 //     integer counts are reduced, so the result does not depend on scheduling, and a trajectory's summary is the same bits whether it is
 //     checked alone or inside a batch.
@@ -60,6 +62,12 @@ struct ClrArgs {
     ClrSummary *summary;           // N / N0
     int *cursor;                   // persistent warps draw samples from this counter (zero on entry)
     unsigned long long *counters;  // may be null: {candidate pairs (box passed), exact mesh searches}
+    // sample list (isdf_certify.cuh): when st is set, sample s < nlist is piece sp[s] at local time st[s] instead of the uniform
+    // sample s of the definition; hit (may be null) gets hit[piece / N0] |= 1 for every sample with clear < margin or NaN
+    const int *sp;
+    const double *st;
+    int nlist;
+    int *hit;
 };
 
 // key order of the running best: (value, address); address -1 = "no witness" (a candidate that only equals reach never wins)
@@ -92,23 +100,24 @@ __global__ void __launch_bounds__(CLR_THREADS) k_clearance_scan(const __grid_con
     ClrWarpSmem &sm = wsm[warp];
     const DevGrid &G = A.grid;
     const DevMesh &Mh = A.shape.mesh;
-    const int K = A.K, S = A.N * (K + 1);
+    const int K = A.K, S = A.st ? A.nlist : A.N * (K + 1);
     const double H = A.half_bd + A.reach;
     for (;;) {
         int s = 0;
         if (lane == 0) s = atomicAdd(A.cursor, 1);
         s = __shfl_sync(0xffffffffu, s, 0);
         if (s >= S) break;
-        const int i = s / (K + 1), j = s - i * (K + 1);
+        const int i = A.st ? __ldg(A.sp + s) : s / (K + 1);
         Window W;
         bool empty, finite;
         {   // pose (every lane computes the same values; lane 0 publishes them) and the world window of the rotated H box
             double cx[6], cy[6], cz[6];
 #pragma unroll
             for (int k = 0; k < 6; k++) { cx[k] = __ldg(A.C + 6 * i + k); cy[k] = __ldg(A.C + 6 * A.N + 6 * i + k); cz[k] = __ldg(A.C + 12 * A.N + 6 * i + k); }
-            const double step = __ldg(A.T + i) * (1.0 / K);
+            // uniform samples: t = j * step, step = T_i * (1 / K_c), exactly as the definition states
+            const double t = A.st ? __ldg(A.st + s) : (s - i * (K + 1)) * (__ldg(A.T + i) * (1.0 / K));
             PieceEval pe;
-            piece_eval(cx, cy, cz, j * step, pe);
+            piece_eval(cx, cy, cz, t, pe);
             const quat4 q = flat_quat_only(A.fp, pe.vel, pe.acc);
             const rot3 R = quat_rot(q);
             const d3 pos = pe.pos;
@@ -211,8 +220,10 @@ __global__ void __launch_bounds__(CLR_THREADS) k_clearance_scan(const __grid_con
         }
         if (MODE == 0) clr_warp_argmin(bv, ba);
         if (lane == 0) {
-            A.clear[s] = !finite ? nan("") : (ba >= 0) ? bv : A.reach;   // a non-finite pose is never reported clear
+            const double cl = !finite ? nan("") : (ba >= 0) ? bv : A.reach;   // a non-finite pose is never reported clear
+            A.clear[s] = cl;
             A.voxel[s] = ba;
+            if (A.hit && !(cl >= A.margin)) atomicOr(A.hit + (A.st ? __ldg(A.sp + s) : s / (K + 1)) / A.N0, 1);   // piece again: i is not kept live
             if (A.counters) {
                 if (npairs) atomicAdd(A.counters, npairs);
                 if (nsearch) atomicAdd(A.counters + 1, nsearch);
@@ -271,6 +282,8 @@ __global__ void __launch_bounds__(CLR_SUM_THREADS) k_clearance_summary(const __g
 // ---- launch interface of the clearance translation unit (isdf_clearance_tu.cu) --------------------------------------------------------
 // mode: 0 analytic, 1 exact-sign mesh, 2 winding-sign mesh; grid = persistent CTAs
 cudaError_t clearance_launch(const ClrArgs &A, int mode, unsigned grid, cudaStream_t st);
+// the scan kernel alone (no summary): the certificate's sample rounds
+cudaError_t clearance_scan_launch(const ClrArgs &A, int mode, unsigned grid, cudaStream_t st);
 // resident CTAs per SM of the scan kernel (the smallest over the three modes)
 cudaError_t clearance_resident_blocks(int *blocks);
 

@@ -36,7 +36,9 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_set_map_cloud", "isdf_set_map_cloud_device", "isdf_get_map_info", "isdf_get_map_u8", "isdf_get_map_f64",
                "isdf_frontend_path", "isdf_frontend_path_batch", "isdf_frontend_path_batch_device", "isdf_frontend_path_field_device",
                "isdf_frontend_path_info", "isdf_path_waypoints", "isdf_midend_default_params", "isdf_midend_callback_batch",
-               "isdf_midend_batch", "isdf_midend_batch_device"]
+               "isdf_midend_batch", "isdf_midend_batch_device", "isdf_certify_default_params", "isdf_trajectory_certify",
+               "isdf_trajectory_certify_device"]
+CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 
 
 class KernelConfig(C.Structure):
@@ -81,6 +83,24 @@ class ClearanceSummary(C.Structure):
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+class CertifyParams(C.Structure):
+    """isdf_certify_params"""
+    _fields_ = [("clearance", ClearanceParams), ("max_depth", C.c_int32), ("max_samples_per_traj", C.c_int32), ("reserved_", C.c_int32 * 2)]
+
+
+class CertifySummary(C.Structure):
+    """isdf_certify_summary (one per trajectory)"""
+    _fields_ = [("lower_bound", C.c_double), ("min_clearance", C.c_double), ("t_min", C.c_double), ("first_hit", C.c_double),
+                ("voxel_min", C.c_int64), ("verdict", C.c_int32), ("samples", C.c_int32), ("undecided_intervals", C.c_int32), ("depth", C.c_int32)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+# record of isdf_dbg_certify_leaves (not part of include/isdf.h)
+CERT_LEAF_DTYPE = np.dtype([("ta", "<f8"), ("tb", "<f8"), ("ca", "<f8"), ("cb", "<f8"), ("Da", "<f8"), ("Db", "<f8"), ("piece", "<i4"), ("state", "<i4")])
 
 
 class MapInfo(C.Structure):
@@ -179,6 +199,9 @@ def load_library(path=None):
     lib.isdf_clearance_default_params.argtypes = [C.POINTER(ClearanceParams)]
     lib.isdf_trajectory_clearance.argtypes = [vp, C.c_int, dp, dp, C.POINTER(ClearanceParams), dp, C.POINTER(C.c_int64), C.POINTER(ClearanceSummary)]
     lib.isdf_trajectory_clearance_device.argtypes = [vp, C.c_int, vp, vp, C.POINTER(ClearanceParams), vp, vp, vp, vp]
+    lib.isdf_certify_default_params.argtypes = [C.POINTER(CertifyParams)]
+    lib.isdf_trajectory_certify.argtypes = [vp, C.c_int, dp, dp, C.POINTER(CertifyParams), C.POINTER(CertifySummary)]
+    lib.isdf_trajectory_certify_device.argtypes = [vp, C.c_int, vp, vp, C.POINTER(CertifyParams), vp, vp]
     lib.isdf_set_map_cloud.argtypes = [vp, vp, C.c_int64, C.c_int32, C.c_double, C.c_int32]
     lib.isdf_set_map_cloud_device.argtypes = [vp, vp, C.c_int64, C.c_int32, C.c_double, C.c_int32, vp]
     lib.isdf_get_map_info.argtypes = [vp, C.POINTER(MapInfo)]
@@ -617,6 +640,71 @@ class Evaluator:
         if self.lib.isdf_dbg_clearance_counts(self.h, out) != 0:
             raise IsdfError(-1, "isdf_dbg_clearance_counts failed")
         return int(out[0]), int(out[1])
+
+    # ---- continuous clearance certificate (see include/isdf.h) ----
+    def certify_params(self, K_c=None, reach=None, margin=None, N0=0, max_depth=None, max_samples=None):
+        p = CertifyParams()
+        self._check(self.lib.isdf_certify_default_params(C.byref(p)))
+        if K_c is not None:
+            p.clearance.samples_per_piece = int(K_c)
+        if reach is not None:
+            p.clearance.reach = float(reach)
+        if margin is not None:
+            p.clearance.margin = float(margin)
+        p.clearance.pieces_per_traj = int(N0)
+        if max_depth is not None:
+            p.max_depth = int(max_depth)
+        if max_samples is not None:
+            p.max_samples_per_traj = int(max_samples)
+        return p
+
+    def trajectory_certify(self, T, coeffs, K_c, reach, margin, N0=0, max_depth=None, max_samples=None):
+        """one summary dict per trajectory (pieces b*N0 .. b*N0+N0-1; N0 = 0: a single trajectory): verdict (CERTIFIED 1, COLLIDING -1,
+        UNDECIDED 0), lower_bound, min_clearance, t_min, first_hit, voxel_min, samples, undecided_intervals, depth"""
+        T = _f64(T).reshape(-1)
+        N = T.size
+        Cc = _f64(coeffs).reshape(-1)
+        assert Cc.size == 18 * N
+        p = self.certify_params(K_c, reach, margin, N0, max_depth, max_samples)
+        B = 1 if N0 == 0 else max(N // N0, 1)
+        summ = (CertifySummary * B)()
+        self._check(self.lib.isdf_trajectory_certify(self.h, N, _dp(T), _dp(Cc), C.byref(p), summ))
+        return [s.as_dict() for s in summ]
+
+    def trajectory_certify_device(self, N, d_T, d_coeffs, params, d_summary, stream=0):
+        """raw device pointers (e.g. torch .data_ptr()); d_summary holds N/N0 isdf_certify_summary records (56 bytes each)"""
+        self._check(self.lib.isdf_trajectory_certify_device(self.h, N, C.c_void_p(d_T), C.c_void_p(d_coeffs), C.byref(params),
+                                                            C.c_void_p(d_summary), C.c_void_p(stream)))
+
+    def dbg_certify_bound(self, T, coeffs, reach, piece, ta, tb):
+        """(D_a, D_b) of the certificate's motion bound for intervals (piece, ta, tb) of the block (T, coeffs) as an (n, 2) array, and the
+        body radius r it used (isdf_dbg_certify_bound, not part of include/isdf.h)"""
+        T, Cc = _f64(T).reshape(-1), _f64(coeffs).reshape(-1)
+        piece = np.ascontiguousarray(piece, dtype=np.int32).reshape(-1)
+        ta, tb = _f64(ta).reshape(-1), _f64(tb).reshape(-1)
+        n = piece.size
+        out = np.zeros((n, 2))
+        f = self.lib.isdf_dbg_certify_bound
+        f.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                      C.POINTER(C.c_double)]
+        f.restype = C.c_int
+        r = C.c_double(0.0)
+        self._check(f(self.h, T.size, T.ctypes.data, Cc.ctypes.data, float(reach), n, piece.ctypes.data, ta.ctypes.data, tb.ctypes.data,
+                      out.ctypes.data, C.byref(r)))
+        return out, r.value
+
+    def dbg_certify_leaves(self):
+        """the final leaf intervals of the last certificate call as a structured array (CERT_LEAF_DTYPE; piece = index in the call's
+        block), in the order they were finished (isdf_dbg_certify_leaves, not part of include/isdf.h)"""
+        f = self.lib.isdf_dbg_certify_leaves
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.POINTER(C.c_longlong)]
+        f.restype = C.c_int
+        n = C.c_longlong(0)
+        self._check(f(self.h, None, 0, C.byref(n)))
+        out = np.zeros(n.value, dtype=CERT_LEAF_DTYPE)
+        if n.value:
+            self._check(f(self.h, out.ctypes.data, n.value, C.byref(n)))
+        return out
 
     # ---- front end: attitude kernels (see include/isdf.h) ----
     def frontend_build_kernels(self, max_roll=45.0, max_pitch=45.0, ang_res=9.0, front_end_safeh=0.0):

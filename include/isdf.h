@@ -337,7 +337,7 @@ int isdf_midend_batch_device(isdf_ctx *ctx, int B, int N0, const double *d_head,
  *   Samples. N pieces (T, coeffs in the layout of isdf_eval_discrete); piece i has K_c + 1 pose samples at local times j * step,
  *     step = T_i * (1 / K_c), j = 0..K_c — the discrete path's pose: position of the piece polynomial, flatness quaternion, R = quat_rot(q).
  *     Junction times are sampled twice (last sample of one piece, first of the next), as in the integral loop. The check is SAMPLED: nothing
- *     is certified between two samples T_i / K_c apart.
+ *     is certified between two samples T_i / K_c apart (isdf_trajectory_certify below closes those gaps).
  *   Candidates of a sample: the occupied map voxels whose centre c (getGridCubeCenter) satisfies |R^T (c - x)|_inf <= H,
  *     H = half_bd + reach, half_bd = kernel_size * occupancy_resolution / 2 (a strict > on any axis excludes, as hpp:800). Only voxels of
  *     the map count: a window reaching past the map border is cut off there (no projInMap clamping).
@@ -380,6 +380,85 @@ int isdf_trajectory_clearance(isdf_ctx *ctx, int N, const double *T, const doubl
 int isdf_trajectory_clearance_device(isdf_ctx *ctx, int N, const double *d_T, const double *d_coeffs, const isdf_clearance_params *p,
                                      double *d_sample_clearance, int64_t *d_sample_voxel, isdf_clearance_summary *d_summary,
                                      void *cuda_stream);
+
+/* ---- continuous clearance certificate: is a trajectory clear at EVERY time, not only at its samples? ---------------------------
+ * The clearance check above is sampled; this call closes the gaps between the samples with a proven motion bound.
+ * Definition. Inputs and parameters are the clearance check's (T, coeffs, K_c, N0, reach, margin) with 0 <= margin < reach. One verdict
+ * per trajectory:
+ *   CERTIFIED (1)   for every time t of the trajectory and every occupied voxel centre c of the map, the Euclidean distance from c to
+ *                   the robot posed at t is at least margin;
+ *   COLLIDING (-1)  some evaluated pose sample has clear < margin (or a non-finite pose);
+ *   UNDECIDED (0)   neither was established within the refinement budget.
+ *   Obstacles are voxel CENTRES, as in the clearance check and the cost terms. Callers who want whole voxel cubes cleared add
+ *   res * sqrt(3) / 2 to margin.
+ * Mechanism.
+ *   The initial samples are exactly the clearance check's K_c + 1 samples per piece (bit-identical clearances). Each piece is divided
+ *   into K_c intervals [ta, tb] of local time (the last one ends at T_i); intervals never cross a junction. For an interval with
+ *   endpoint clearances c_a, c_b (capped at reach), D_e bounds the largest displacement of any body point over the interval from its
+ *   position at endpoint e: sup_{t in [ta,tb]} sup_{p in body} |x(t) + R(t) p - x(t_e) - R(t_e) p|. Then
+ *   lb = max(c_a - D_a, c_b - D_b) is a lower bound of the clearance at every t of the interval, and the interval is SAFE when
+ *   lb >= margin. An interval that is not safe is split at its midpoint ta + 0.5 (tb - ta), and the midpoint gets a new clearance
+ *   sample. Splitting stops when the trajectory has a colliding sample (it is COLLIDING; its remaining intervals are dropped), at
+ *   max_depth, or when the trajectory's new samples would exceed max_samples_per_traj (intervals earlier in time get the samples
+ *   first). Intervals left in the last two cases are undecided.
+ *   Motion bound: D_e = P_e + r Q_e + eps_e.
+ *     P_e   per axis, the piece polynomial re-expanded about t_e (Taylor coefficients d_1..d_5) gives sum |d_k| h^k, h = tb - ta;
+ *           P_e is the Euclidean norm of the three axis bounds.
+ *     Q_e   >= sup ||R(t) - R(t_e)||_2, in interval arithmetic: v and a enclosed over the interval in Taylor form;
+ *           zu = a + dh_over_m (1 + cp sqrt(|v|^2 + veps)) v + g e_z, z = zu / |zu|; R(z) in the closed form of the zero-yaw attitude,
+ *           rows [1 - zx^2/(1+zz), -zx zy/(1+zz), zx], [-zx zy/(1+zz), 1 - zy^2/(1+zz), zy], [-zx, -zy, zz] (quat_rot(flat_quat_only)
+ *           up to rounding); Q_e = Frobenius norm of the enclosure of R(z(t)) - R(z(t_e)). Q_e = +inf (the interval must be refined)
+ *           when the lower bound of |zu| or of 1 + zz is not positive.
+ *     r     body radius about the body origin: 0 for Ball and Point (rotation-invariant bodies); for Box the largest corner norm of the
+ *           transformed box; for a mesh the largest corner norm of its body-frame AABB.
+ *     eps_e pose pad 1e-10 (1 + A_e + 2H + (r + 2H) kappa_e / delta_e), H = half_bd + reach, A_e = sum over axes and k of |c_k| |t_e|^k,
+ *           kappa_e = (|a| + dh_over_m kap |v| + g) / |zu| and delta_e = 1 + zz at t_e: it covers the difference between this closed
+ *           form and the pose and SDF the scan computes in round-to-nearest with FMA contraction (DESIGN §3.11).
+ *     Every operation of the bound is rounded outward.
+ *   Why this is sound: for a body point q(t), |c - q(t)| >= |c - q(t_e)| - D_e. Capping at reach and leaving out voxels outside the H box
+ *   only lower c_e. This needs an SDF that is a true Euclidean distance outside the body, and a body inside the half_bd box (so that the
+ *   H box loses no voxel within reach); the call checks both.
+ * Supported shapes: Ball with 0 <= radius <= half_bd, Point, Box whose rotation is orthonormal to 1e-12 and whose corners lie in
+ *   [-half_bd, half_bd]^3, exact-sign meshes (ISDF_MESH_SIGN_EXACT) whose body-frame AABB lies in [-half_bd, half_bd]^3. Everything else
+ *   (other analytic shapes, winding-sign meshes, a robot wider than half_bd) is ISDF_ERR_UNSUPPORTED.
+ * Summary per trajectory: verdict; lower_bound = the minimum of lb over the final leaf intervals, a proven lower bound of the continuous
+ *   clearance whatever the verdict (never above reach); min_clearance, t_min (trajectory time) and voxel_min over every evaluated sample
+ *   (ties: earliest time, then smallest witness address); first_hit = trajectory time of the earliest evaluated sample with
+ *   clear < margin, or -1; samples (evaluated: N0 (K_c + 1) plus the new ones), undecided_intervals, depth (deepest leaf level).
+ * Results are deterministic run to run, identical through both entry points, and a trajectory's result is bit-identical alone or
+ * inside a batch (per-trajectory budgets, order-preserving compaction).
+ * Device work per round: one scan launch over the round's new samples, one interval pass (two kernels), one 4-byte read; at most
+ *   max_depth + 1 rounds. Device buffers are owned by the context and grow on demand.
+ * Errors: ISDF_ERR_INVALID for the clearance check's bad parameters, margin < 0, margin >= reach, max_depth outside [0, 64],
+ *   max_samples_per_traj < 0, a non-zero reserved_, sizes beyond 31-bit indexing, NULL pointers; ISDF_ERR_STATE without a map or a
+ *   shape; ISDF_ERR_UNSUPPORTED for an unsupported shape and on a sharded context. On failure every summary has verdict 0 and
+ *   lower_bound / min_clearance NaN.
+ * The call counts its launches in isdf_stats.kernel_launches and touches no other field; it leaves the discrete schedule, the
+ * swept-volume state, the mid-end buffers and the batch trajectories as they were. */
+typedef struct isdf_certify_params {
+    isdf_clearance_params clearance;  /* K_c, N0, reach, margin as the clearance check, with 0 <= margin < reach */
+    int32_t max_depth;                /* splits per initial interval, 0..64 */
+    int32_t max_samples_per_traj;     /* new samples per trajectory, >= 0 */
+    int32_t reserved_[2];             /* must be 0 */
+} isdf_certify_params;
+
+typedef struct isdf_certify_summary {
+    double lower_bound, min_clearance, t_min, first_hit;   /* first_hit = -1 when no evaluated sample collides */
+    int64_t voxel_min;                                     /* witness of the minimum sample, -1 when nothing lies within reach */
+    int32_t verdict;                                       /* 1 CERTIFIED, -1 COLLIDING, 0 UNDECIDED */
+    int32_t samples, undecided_intervals, depth;
+} isdf_certify_summary;
+
+/* K_c = integral_intervs and N0 = 0 as isdf_clearance_default_params, margin = safety_hor, reach = 2 safety_hor, max_depth 16,
+ * max_samples_per_traj 2048 (DESIGN §3.11) */
+int isdf_certify_default_params(isdf_certify_params *p);
+/* host buffers; summary: N/N0 entries (1 for N0 = 0) */
+int isdf_trajectory_certify(isdf_ctx *ctx, int N, const double *T, const double *coeffs, const isdf_certify_params *p,
+                            isdf_certify_summary *summary);
+/* device-resident variant: d_T, d_coeffs, d_summary on ctx's device; runs on cuda_stream (NULL = default stream) and returns when the
+ * summaries are written (the round loop reads 4 bytes per round) */
+int isdf_trajectory_certify_device(isdf_ctx *ctx, int N, const double *d_T, const double *d_coeffs, const isdf_certify_params *p,
+                                   isdf_certify_summary *d_summary, void *cuda_stream);
 
 /* ---- multi-GPU reduction through NVLink / NVSwitch peer memory (optional; ncclAllReduce over the same 19N+1 doubles is the
  * library alternative). One process per GPU. Sequence on every rank:
