@@ -42,6 +42,41 @@ static int fail(int code, const std::string &msg) { g_err = msg; return code; }
         }                                                                                             \
     } while (0)
 
+// The one failure path of the entry points whose outputs include/isdf.h poisons: run body() and, when it fails, poison().
+template <typename Body, typename Poison>
+static int poison_on_failure(Body body, Poison poison) {
+    const int r = body();
+    if (r) poison();
+    return r;
+}
+static void nan_fill(double *h, long long n) { if (h) for (long long i = 0; i < n; i++) h[i] = std::numeric_limits<double>::quiet_NaN(); }
+
+static int minco_fits(int N0) {
+    if (minco_smem_bytes(N0) > 220 * 1024) return fail(ISDF_ERR_UNSUPPORTED, "pieces per problem too large for the shared-memory banded solver (N0 <= 290)");
+    return 0;
+}
+
+// The MINCO forward / adjoint workspace (isdf_minco.cuh) of one batched optimiser: B problems of N0 pieces.
+struct MincoWork {
+    DevBuf<double> d_T, d_C, d_lu, d_energy, d_gC, d_gT, d_out;
+    int ensure(int B, int N0) {
+        if (int r = minco_fits(N0)) return r;
+        const size_t BN = (size_t)B * N0, smem = minco_smem_bytes(N0);
+        CU_TRY(d_T.ensure(BN)); CU_TRY(d_C.ensure(18 * BN)); CU_TRY(d_lu.ensure(78 * BN)); CU_TRY(d_energy.ensure(B));
+        CU_TRY(d_gC.ensure(18 * BN)); CU_TRY(d_gT.ensure(BN)); CU_TRY(d_out.ensure(19 * BN + 1));
+        CU_TRY(cudaFuncSetAttribute(k_minco_forward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CU_TRY(cudaFuncSetAttribute(k_minco_backward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        return 0;
+    }
+    // the workspace's part of the arguments; the terms (swept volume, discrete output, cost and gradient) are the caller's
+    MincoArgs args(int B, int N0, const double *head, const double *tail, int bc_stride, double rho, const double *x) {
+        MincoArgs M = {};
+        M.B = B; M.N = N0; M.x = x; M.head = head; M.tail = tail; M.bc_stride = bc_stride; M.rho = rho;
+        M.T = d_T.p; M.C = d_C.p; M.lu = d_lu.p; M.energy = d_energy.p; M.gC_e = d_gC.p; M.gT_e = d_gT.p;
+        return M;
+    }
+};
+
 // One plain struct per subsystem; each keeps the flag that says its state is valid next to the buffers that state lives in. Every
 // buffer owns its memory; ~isdf_ctx releases the rest.
 struct isdf_ctx {
@@ -72,8 +107,7 @@ struct isdf_ctx {
         long long order_for = -1;    // (N, rank, world) signature the work items are valid for
         bool items_pending = false;  // the aux stream is building them
         DevBuf<double> d_piece_cost;
-        double *count_out_dev = nullptr;   // host entry points: where the epilogue drops the pair count (behind the result vector)
-        DevBuf<int> d_tickets;       // pieces_done counter of the epilogue kernel
+        DevBuf<int> d_tickets;      // pieces_done counter of the epilogue kernel
         DevBuf<double> d_tot; DevBuf<unsigned> d_split_done;   // per-sample collision sums handed from the scan kernels to the epilogue
         DevBuf<int> d_items, d_item_count; DevBuf<unsigned> d_work, d_split_work; DevBuf<double> d_subsum;   // work items (longest first, heavy samples split)
         DevBuf<unsigned long long> d_counter;   // {pairs, then k_discrete_prologue's {codes requested, runs, overflowed runs, codes written}}
@@ -93,7 +127,8 @@ struct isdf_ctx {
         DevBuf<double> d_C, d_out;
     } stage;
     struct {   // batched callback (isdf_minco.cuh); B = 0: none evaluated yet
-        DevBuf<double> d_x, d_bc, d_T, d_C, d_lu, d_energy, d_gC, d_gT, d_cost, d_grad, d_out, d_Cpp, d_sv;
+        MincoWork minco;
+        DevBuf<double> d_x, d_bc, d_cost, d_grad, d_Cpp, d_sv;
         int B = 0, N0 = 0;
     } batch;
     struct LbfgsBufs {   // device-resident lock-step L-BFGS (isdf_lbfgs.cuh)
@@ -101,7 +136,8 @@ struct isdf_ctx {
         PinnedBuf<int> h_active;
     } lbfgs;
     struct {   // mid-end (isdf_midend.cuh): buffers of its own, so that no mid-end call touches the back end's batch, swept or L-BFGS state
-        DevBuf<double> d_x, d_bc, d_wp, d_T, d_C, d_lu, d_energy, d_gC, d_gT, d_out, d_pc, d_cost, d_grad;
+        MincoWork minco;
+        DevBuf<double> d_x, d_bc, d_wp, d_pc, d_cost, d_grad;
         LbfgsBufs lb;
     } mid;
     SweptState sv;   // swept volume
@@ -151,6 +187,13 @@ struct isdf_ctx {
 };
 
 static int set_device(isdf_ctx *c) { CU_TRY(cudaSetDevice(c->device)); return 0; }
+// the context's device, with the work enqueued on its stream (and, with aux, on its work-item stream) finished
+static int sync_ctx(isdf_ctx *c, bool aux = false) {
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    CU_TRY(cudaStreamSynchronize(c->stream));
+    if (aux) CU_TRY(cudaStreamSynchronize(c->aux_stream));
+    return 0;
+}
 
 extern "C" const char *isdf_last_error(void) { return g_err.c_str(); }
 
@@ -905,7 +948,19 @@ static int peer_fuse_check(const isdf_ctx *c, int N) {
     return 0;
 }
 
-static int launch_discrete(isdf_ctx *c, int N, const double *d_T, const double *d_C, double *d_out, cudaStream_t st) {
+// the exchange of d_vec (n doubles) at the next epoch, committed only once its kernel is enqueued
+static int peer_allreduce_launch(isdf_ctx *c, double *d_vec, int n, cudaStream_t st) {
+    PeerArgs P = c->peer.args;
+    P.epoch = c->peer.args.epoch + 1;
+    k_peer_allreduce<<<1, 512, 0, st>>>(P, d_vec, n);
+    c->stats.kernel_launches++;
+    CU_TRY(cudaGetLastError());
+    c->peer.args.epoch = P.epoch;
+    return 0;
+}
+
+// count_out (host entry points only): where the epilogue drops the pair count, behind the result vector
+static int launch_discrete(isdf_ctx *c, int N, const double *d_T, const double *d_C, double *d_out, double *count_out, cudaStream_t st) {
     const int K = c->cfg.integral_intervs;
     const long long S = (long long)N * (K + 1);
     if (S > 0x7fffffffll) return fail(ISDF_ERR_UNSUPPORTED, "N * (integral_intervs + 1) must fit in 31 bits");
@@ -918,7 +973,7 @@ static int launch_discrete(isdf_ctx *c, int N, const double *d_T, const double *
     DiscArgs A;
     A.cfg = c->dcfg; A.grid = c->map.grid; A.shape = c->mesh.shape; A.N = N; A.T = d_T; A.C = d_C;
     A.tot = c->disc.d_tot.p; A.pieces_done = c->disc.d_tickets.p; A.item_cursor = c->disc.d_tickets.p + 1;
-    A.piece_cost = c->disc.d_piece_cost.p; A.out = d_out; A.pair_counter = c->disc.d_counter.p; A.count_out = c->disc.count_out_dev;
+    A.piece_cost = c->disc.d_piece_cost.p; A.out = d_out; A.pair_counter = c->disc.d_counter.p; A.count_out = count_out;
     A.rank = c->rank; A.world = c->world;
     A.peer = PeerArgs{};
     const bool fused = fused_exchange(c);
@@ -1010,66 +1065,56 @@ extern "C" int isdf_eval_discrete_device(isdf_ctx *c, int N, const double *d_T, 
     if (r) return r;
     if (!d_T || !d_coeffs || !d_out) return fail(ISDF_ERR_INVALID, "NULL device pointer");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    return launch_discrete(c, N, d_T, d_coeffs, d_out, (cudaStream_t)cuda_stream);
+    return launch_discrete(c, N, d_T, d_coeffs, d_out, nullptr, (cudaStream_t)cuda_stream);
 }
-
-static void poison(double *cost) { if (cost) *cost = std::numeric_limits<double>::quiet_NaN(); }
 
 // The host form of the discrete and swept-volume evaluations: [coefficients 18N | durations N] go in through one pinned block and
 // ONE copy, `before` runs after that copy, `launch(d_T, d_C, d_out, count_out)` between ev0 and ev1, and [cost | gradC | gradT |
 // counter word] come back in ONE copy. The result is added to *cost, gradC and gradT, as the reference accumulates (hpp:539-550,
-// hpp:640-645); the counter word goes to the stat `counted`. On failure *cost is NaN.
+// hpp:640-645); the counter word goes to the stat `counted`. The caller poisons *cost on failure.
 template <typename Before, typename Launch>
 static int eval_host(isdf_ctx *c, int N, const double *T, const double *coeffs, double *cost, double *gradC, double *gradT,
                      int64_t isdf_stats::*counted, Before before, Launch launch) {
-    auto body = [&]() -> int {
-        if (set_device(c)) return ISDF_ERR_CUDA;
-        const size_t nin = (size_t)19 * N, nout = (size_t)19 * N + 1;
-        CU_TRY(c->stage.h.ensure(nin + nout + 1));
-        CU_TRY(c->stage.d_C.ensure(nin)); CU_TRY(c->stage.d_out.ensure(nout + 1));
-        std::memcpy(c->stage.h.p, coeffs, sizeof(double) * 18 * N);
-        std::memcpy(c->stage.h.p + 18 * (size_t)N, T, sizeof(double) * N);
-        CU_TRY(cudaMemcpyAsync(c->stage.d_C.p, c->stage.h.p, sizeof(double) * nin, cudaMemcpyHostToDevice, c->stream));
-        if (int rr = before()) return rr;
-        CU_TRY(cudaEventRecord(c->ev0, c->stream));
-        if (int rr = launch(c->stage.d_C.p + 18 * (size_t)N, c->stage.d_C.p, c->stage.d_out.p, c->stage.d_out.p + nout)) return rr;
-        CU_TRY(cudaEventRecord(c->ev1, c->stream));
-        double *h_out = c->stage.h.p + nin;
-        CU_TRY(cudaMemcpyAsync(h_out, c->stage.d_out.p, sizeof(double) * (nout + 1), cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaStreamSynchronize(c->stream));
-        unsigned long long count = 0;
-        std::memcpy(&count, h_out + nout, sizeof(count));
-        if (fused_exchange(c) && isdf_peer_status(c) != ISDF_OK) return ISDF_ERR_CUDA;   // exchange timed out: the vector is NaN
-        float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
-        c->stats.last_kernel_ms = ms; c->stats.*counted = (int64_t)count;
-        *cost += h_out[0];
-        for (size_t k = 0; k < (size_t)18 * N; k++) gradC[k] += h_out[1 + k];
-        for (int k = 0; k < N; k++) gradT[k] += h_out[1 + 18 * N + k];
-        return 0;
-    };
-    const int r = body();
-    if (r) poison(cost);
-    return r;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    const size_t nin = (size_t)19 * N, nout = (size_t)19 * N + 1;
+    CU_TRY(c->stage.h.ensure(nin + nout + 1));
+    CU_TRY(c->stage.d_C.ensure(nin)); CU_TRY(c->stage.d_out.ensure(nout + 1));
+    std::memcpy(c->stage.h.p, coeffs, sizeof(double) * 18 * N);
+    std::memcpy(c->stage.h.p + 18 * (size_t)N, T, sizeof(double) * N);
+    CU_TRY(cudaMemcpyAsync(c->stage.d_C.p, c->stage.h.p, sizeof(double) * nin, cudaMemcpyHostToDevice, c->stream));
+    if (int rr = before()) return rr;
+    CU_TRY(cudaEventRecord(c->ev0, c->stream));
+    if (int rr = launch(c->stage.d_C.p + 18 * (size_t)N, c->stage.d_C.p, c->stage.d_out.p, c->stage.d_out.p + nout)) return rr;
+    CU_TRY(cudaEventRecord(c->ev1, c->stream));
+    double *h_out = c->stage.h.p + nin;
+    CU_TRY(cudaMemcpyAsync(h_out, c->stage.d_out.p, sizeof(double) * (nout + 1), cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(cudaStreamSynchronize(c->stream));
+    unsigned long long count = 0;
+    std::memcpy(&count, h_out + nout, sizeof(count));
+    if (fused_exchange(c) && isdf_peer_status(c) != ISDF_OK) return ISDF_ERR_CUDA;   // exchange timed out: the vector is NaN
+    float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
+    c->stats.last_kernel_ms = ms; c->stats.*counted = (int64_t)count;
+    *cost += h_out[0];
+    for (size_t k = 0; k < (size_t)18 * N; k++) gradC[k] += h_out[1 + k];
+    for (int k = 0; k < N; k++) gradT[k] += h_out[1 + 18 * N + k];
+    return 0;
 }
 
 extern "C" int isdf_eval_discrete(isdf_ctx *c, int N, const double *T, const double *coeffs, double *cost, double *gradC, double *gradT) {
-    int r = check_eval_state(c, N, true);
-    if (r) { poison(cost); return r; }
-    if (!T || !coeffs || !cost || !gradC || !gradT) { poison(cost); return fail(ISDF_ERR_INVALID, "NULL argument"); }
-    return eval_host(c, N, T, coeffs, cost, gradC, gradT, &isdf_stats::last_pairs, [] { return 0; },
-                     [&](const double *d_T, const double *d_C, double *d_out, double *count_out) {
-                         c->disc.count_out_dev = count_out;
-                         const int rr = launch_discrete(c, N, d_T, d_C, d_out, c->stream);
-                         c->disc.count_out_dev = nullptr;
-                         return rr;
-                     });
+    return poison_on_failure([&]() -> int {
+        if (int r = check_eval_state(c, N, true)) return r;
+        if (!T || !coeffs || !cost || !gradC || !gradT) return fail(ISDF_ERR_INVALID, "NULL argument");
+        return eval_host(c, N, T, coeffs, cost, gradC, gradT, &isdf_stats::last_pairs, [] { return 0; },
+                         [&](const double *d_T, const double *d_C, double *d_out, double *count_out) {
+                             return launch_discrete(c, N, d_T, d_C, d_out, count_out, c->stream);
+                         });
+    }, [&] { nan_fill(cost, 1); });
 }
 
 extern "C" int isdf_get_piece_costs(isdf_ctx *c, double *piece_cost, int n) {
     if (!c || !piece_cost || n < 0) return fail(ISDF_ERR_INVALID, "bad argument");
     if ((size_t)n > c->disc.d_piece_cost.n) return fail(ISDF_ERR_STATE, "no discrete evaluation with that many pieces yet");
-    if (set_device(c)) return ISDF_ERR_CUDA;
-    CU_TRY(cudaStreamSynchronize(c->stream));
+    if (int r = sync_ctx(c)) return r;
     CU_TRY(cudaMemcpy(piece_cost, c->disc.d_piece_cost.p, sizeof(double) * n, cudaMemcpyDeviceToHost));
     return 0;
 }
@@ -1078,27 +1123,21 @@ extern "C" int isdf_get_piece_costs(isdf_ctx *c, double *piece_cost, int n) {
 static int callback_batch_launch(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int bc_stride, double rho,
                                  const double *d_x, double *d_cost, double *d_grad, cudaStream_t st) {
     const size_t BN = (size_t)B * N0;
-    const size_t smem = minco_smem_bytes(N0);
-    if (smem > 220 * 1024) return fail(ISDF_ERR_UNSUPPORTED, "pieces per problem too large for the shared-memory banded solver (N0 <= 290)");
+    if (int r = minco_fits(N0)) return r;
     if (BN * (size_t)(c->cfg.integral_intervs + 1) > 0x7fffffffull) return fail(ISDF_ERR_UNSUPPORTED, "batch too large: B*N0*(K+1) must fit in 31 bits");
-    CU_TRY(c->batch.d_T.ensure(BN)); CU_TRY(c->batch.d_C.ensure(18 * BN)); CU_TRY(c->batch.d_lu.ensure(78 * BN)); CU_TRY(c->batch.d_energy.ensure(B));
-    CU_TRY(c->batch.d_gC.ensure(18 * BN)); CU_TRY(c->batch.d_gT.ensure(BN)); CU_TRY(c->batch.d_out.ensure(19 * BN + 1));
-    MincoArgs M;
-    M.B = B; M.N = N0; M.x = d_x; M.head = d_head; M.tail = d_tail; M.bc_stride = bc_stride; M.rho = rho;
-    M.T = c->batch.d_T.p; M.C = c->batch.d_C.p; M.lu = c->batch.d_lu.p; M.energy = c->batch.d_energy.p; M.gC_e = c->batch.d_gC.p; M.gT_e = c->batch.d_gT.p;
-    M.disc_out = nullptr; M.piece_cost = nullptr; M.cost = d_cost; M.grad = d_grad; M.seq_terms = 0;
+    if (int r = c->batch.minco.ensure(B, N0)) return r;
+    MincoArgs M = c->batch.minco.args(B, N0, d_head, d_tail, bc_stride, rho, d_x);
+    M.cost = d_cost; M.grad = d_grad;
     // per-problem obstacle point sets registered for exactly this batch (isdf_set_points_batch): the LIVE composition of costFunctionLmbm
     // (hpp:386-405) — swept-volume term, then time-integral term
     const bool with_swept = (c->sv.B == B);
-    M.Cpp = nullptr; M.sv_out = nullptr;
     if (with_swept) {
         if (c->mesh.shape.kind == ISDF_SHAPE_MESH && c->mesh.shape.mesh.sign_mode == MESH_SIGN_WINDING)
             return fail(ISDF_ERR_UNSUPPORTED, "swept-volume term with a winding-sign mesh (see isdf_set_shape_mesh_ex)");
         CU_TRY(c->batch.d_Cpp.ensure(18 * BN)); CU_TRY(c->batch.d_sv.ensure((size_t)B * (19 * (size_t)N0 + 1)));
         M.Cpp = c->batch.d_Cpp.p;
     }
-    CU_TRY(cudaFuncSetAttribute(k_minco_forward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CU_TRY(cudaFuncSetAttribute(k_minco_backward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const size_t smem = minco_smem_bytes(N0);
     k_minco_forward<<<B, 32, smem, st>>>(M);
     if (with_swept) {
         int launches = 0;
@@ -1108,9 +1147,9 @@ static int callback_batch_launch(isdf_ctx *c, int B, int N0, const double *d_hea
         if (e != cudaSuccess) return fail(e == cudaErrorInvalidValue ? ISDF_ERR_INVALID : ISDF_ERR_CUDA, std::string("batched swept: ") + cudaGetErrorString(e));
         M.sv_out = c->batch.d_sv.p;
     }
-    int r = launch_discrete(c, (int)BN, M.T, M.C, c->batch.d_out.p, st);
+    int r = launch_discrete(c, (int)BN, M.T, M.C, c->batch.minco.d_out.p, nullptr, st);
     if (r) return r;
-    M.disc_out = c->batch.d_out.p; M.piece_cost = c->disc.d_piece_cost.p;
+    M.disc_out = c->batch.minco.d_out.p; M.piece_cost = c->disc.d_piece_cost.p;
     k_minco_backward<<<B, 32, smem, st>>>(M);
     c->stats.kernel_launches += 2;
     c->batch.B = B; c->batch.N0 = N0;
@@ -1135,32 +1174,31 @@ extern "C" int isdf_callback_batch_device(isdf_ctx *c, int B, int N0, const doub
     return callback_batch_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, rho, d_x, d_cost, d_grad, (cudaStream_t)cuda_stream);
 }
 
-// the host entry points' boundary conditions (9 doubles, or 9 per problem) on the device: *d_head, then *d_tail
-static int upload_bc(isdf_ctx *c, int B, int per_problem_bc, const double *head, const double *tail, const double **d_head, const double **d_tail) {
+// the host entry points' boundary conditions (9 doubles, or 9 per problem) in buf on c->stream: *d_head, then *d_tail
+static int upload_bc(isdf_ctx *c, DevBuf<double> &buf, int B, int per_problem_bc, const double *head, const double *tail, const double **d_head,
+                     const double **d_tail) {
     const size_t nbc = per_problem_bc ? (size_t)9 * B : 9;
-    CU_TRY(c->batch.d_bc.ensure(2 * nbc));
-    CU_TRY(cudaMemcpyAsync(c->batch.d_bc.p, head, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
-    CU_TRY(cudaMemcpyAsync(c->batch.d_bc.p + nbc, tail, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
-    *d_head = c->batch.d_bc.p; *d_tail = c->batch.d_bc.p + nbc;
+    CU_TRY(buf.ensure(2 * nbc));
+    CU_TRY(cudaMemcpyAsync(buf.p, head, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
+    CU_TRY(cudaMemcpyAsync(buf.p + nbc, tail, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
+    *d_head = buf.p; *d_tail = buf.p + nbc;
     return 0;
 }
 
 extern "C" int isdf_callback_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc, double rho,
                                    const double *x, double *cost, double *grad) {
-    auto poison_all = [&]() { if (cost && B > 0) for (int b = 0; b < B; b++) cost[b] = std::numeric_limits<double>::quiet_NaN(); };
-    int r = callback_batch_check(c, B, N0);
-    if (r) { poison_all(); return r; }
-    if (!head || !tail || !x || !cost || !grad) { poison_all(); return fail(ISDF_ERR_INVALID, "NULL argument"); }
-    auto body = [&]() -> int {
+    return poison_on_failure([&]() -> int {
+        if (int r = callback_batch_check(c, B, N0)) return r;
+        if (!head || !tail || !x || !cost || !grad) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
         const size_t dim = (size_t)N0 + 3 * (size_t)(N0 - 1);
         CU_TRY(c->batch.d_x.upload(x, dim * B, c->stream));
         const double *d_head, *d_tail;
-        if (int rr = upload_bc(c, B, per_problem_bc, head, tail, &d_head, &d_tail)) return rr;
+        if (int r = upload_bc(c, c->batch.d_bc, B, per_problem_bc, head, tail, &d_head, &d_tail)) return r;
         CU_TRY(c->batch.d_cost.ensure(B)); CU_TRY(c->batch.d_grad.ensure(dim * B));
         CU_TRY(cudaEventRecord(c->ev0, c->stream));
-        int rr = callback_batch_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, rho, c->batch.d_x.p, c->batch.d_cost.p, c->batch.d_grad.p, c->stream);
-        if (rr) return rr;
+        if (int r = isdf_callback_batch_device(c, B, N0, d_head, d_tail, per_problem_bc, rho, c->batch.d_x.p, c->batch.d_cost.p, c->batch.d_grad.p,
+                                               c->stream)) return r;
         CU_TRY(cudaEventRecord(c->ev1, c->stream));
         CU_TRY(cudaMemcpyAsync(cost, c->batch.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
         CU_TRY(cudaMemcpyAsync(grad, c->batch.d_grad.p, sizeof(double) * dim * B, cudaMemcpyDeviceToHost, c->stream));
@@ -1168,10 +1206,7 @@ extern "C" int isdf_callback_batch(isdf_ctx *c, int B, int N0, const double *hea
         float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
         c->stats.last_kernel_ms = ms;
         return 0;
-    };
-    r = body();
-    if (r) poison_all();
-    return r;
+    }, [&] { nan_fill(cost, B); });
 }
 
 // ---- device-resident lock-step L-BFGS over the batched callback (SURVEY §8f row 2; isdf_lbfgs.cuh) ----------------------------------------
@@ -1252,48 +1287,52 @@ static int lbfgs_rounds(isdf_ctx *c, isdf_ctx::LbfgsBufs &lb, int B, int n, cons
     return 0;
 }
 
+static void nan_fill_device(isdf_ctx *c, double *d, int n, cudaStream_t st) {
+    if (c && d && n > 0 && cudaSetDevice(c->device) == cudaSuccess) { cudaMemsetAsync(d, 0xff, sizeof(double) * n, st); cudaStreamSynchronize(st); }
+}
+
+// an L-BFGS call's results in lb to the host: x (B x n), f, and ret / iterations / evaluations from the d_head triple (each may be NULL)
+static int lbfgs_copy_out(const isdf_ctx::LbfgsBufs &lb, int B, size_t n, double *x, double *f, int *ret, int *iterations, int *evaluations) {
+    CU_TRY(cudaMemcpy(x, lb.d_x.p, sizeof(double) * n * B, cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(f, lb.d_f.p, sizeof(double) * B, cudaMemcpyDeviceToHost));
+    if (ret) CU_TRY(cudaMemcpy(ret, lb.d_head.p, sizeof(int) * B, cudaMemcpyDeviceToHost));
+    if (iterations) CU_TRY(cudaMemcpy(iterations, lb.d_head.p + B, sizeof(int) * B, cudaMemcpyDeviceToHost));
+    if (evaluations) CU_TRY(cudaMemcpy(evaluations, lb.d_head.p + 2 * (size_t)B, sizeof(int) * B, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
 extern "C" int isdf_lbfgs_batch_device(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc, double rho,
                                        const isdf_lbfgs_params *prm, double *d_x, double *d_f, int *d_ret, int *d_iterations, int *d_evaluations,
                                        int *rounds_out, void *cuda_stream) {
     cudaStream_t st = (cudaStream_t)cuda_stream;
-    auto poison_all = [&]() { if (c && d_f && B > 0 && cudaSetDevice(c->device) == cudaSuccess) { cudaMemsetAsync(d_f, 0xff, sizeof(double) * B, st); cudaStreamSynchronize(st); } };
-    int r = callback_batch_check(c, B, N0);
-    if (!r) r = lbfgs_check(prm);
-    if (!r && (!d_head || !d_tail || !d_x || !d_f)) r = fail(ISDF_ERR_INVALID, "NULL device pointer");
-    if (!r && set_device(c)) r = ISDF_ERR_CUDA;
-    if (!r) r = lbfgs_rounds(c, c->lbfgs, B, 4 * N0 - 3, prm, 0, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st,
-                             [&](const double *x, double *f, double *g) {
-                                 return callback_batch_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, rho, x, f, g, st);
-                             });
-    if (r) poison_all();
-    return r;
+    return poison_on_failure([&]() -> int {
+        if (int r = callback_batch_check(c, B, N0)) return r;
+        if (int r = lbfgs_check(prm)) return r;
+        if (!d_head || !d_tail || !d_x || !d_f) return fail(ISDF_ERR_INVALID, "NULL device pointer");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        return lbfgs_rounds(c, c->lbfgs, B, 4 * N0 - 3, prm, 0, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st,
+                            [&](const double *x, double *f, double *g) {
+                                return callback_batch_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, rho, x, f, g, st);
+                            });
+    }, [&] { nan_fill_device(c, d_f, B, st); });
 }
 
 extern "C" int isdf_lbfgs_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc, double rho,
                                 const isdf_lbfgs_params *prm, double *x, double *f, int *ret, int *iterations, int *evaluations, int *rounds_out) {
-    auto poison_all = [&]() { if (f && B > 0) for (int b = 0; b < B; b++) f[b] = std::numeric_limits<double>::quiet_NaN(); };
-    int r = callback_batch_check(c, B, N0);
-    if (r) { poison_all(); return r; }
-    if (!head || !tail || !x || !f) { poison_all(); return fail(ISDF_ERR_INVALID, "NULL argument"); }
-    auto body = [&]() -> int {
+    return poison_on_failure([&]() -> int {
+        if (int r = callback_batch_check(c, B, N0)) return r;
+        if (!head || !tail || !x || !f) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
+        isdf_ctx::LbfgsBufs &lb = c->lbfgs;
         const size_t n = (size_t)4 * N0 - 3;
-        CU_TRY(c->lbfgs.d_x.upload(x, n * B, c->stream));
+        CU_TRY(lb.d_x.upload(x, n * B, c->stream));
         const double *d_head, *d_tail;
-        if (int rr = upload_bc(c, B, per_problem_bc, head, tail, &d_head, &d_tail)) return rr;
-        CU_TRY(c->lbfgs.d_f.ensure(B)); CU_TRY(c->lbfgs.d_head.ensure((size_t)3 * B));
-        if (int rr = isdf_lbfgs_batch_device(c, B, N0, d_head, d_tail, per_problem_bc, rho, prm, c->lbfgs.d_x.p, c->lbfgs.d_f.p, c->lbfgs.d_head.p,
-                                             c->lbfgs.d_head.p + B, c->lbfgs.d_head.p + 2 * (size_t)B, rounds_out, c->stream)) return rr;
-        CU_TRY(cudaMemcpy(x, c->lbfgs.d_x.p, sizeof(double) * n * B, cudaMemcpyDeviceToHost));
-        CU_TRY(cudaMemcpy(f, c->lbfgs.d_f.p, sizeof(double) * B, cudaMemcpyDeviceToHost));
-        if (ret) CU_TRY(cudaMemcpy(ret, c->lbfgs.d_head.p, sizeof(int) * B, cudaMemcpyDeviceToHost));
-        if (iterations) CU_TRY(cudaMemcpy(iterations, c->lbfgs.d_head.p + B, sizeof(int) * B, cudaMemcpyDeviceToHost));
-        if (evaluations) CU_TRY(cudaMemcpy(evaluations, c->lbfgs.d_head.p + 2 * (size_t)B, sizeof(int) * B, cudaMemcpyDeviceToHost));
-        return 0;
-    };
-    r = body();
-    if (r) poison_all();
-    return r;
+        if (int r = upload_bc(c, c->batch.d_bc, B, per_problem_bc, head, tail, &d_head, &d_tail)) return r;
+        CU_TRY(lb.d_f.ensure(B)); CU_TRY(lb.d_head.ensure((size_t)3 * B));
+        if (int r = isdf_lbfgs_batch_device(c, B, N0, d_head, d_tail, per_problem_bc, rho, prm, lb.d_x.p, lb.d_f.p, lb.d_head.p, lb.d_head.p + B,
+                                            lb.d_head.p + 2 * (size_t)B, rounds_out, c->stream)) return r;
+        return lbfgs_copy_out(lb, B, n, x, f, ret, iterations, evaluations);
+    }, [&] { nan_fill(f, B); });
 }
 
 // Diagnostic (not part of include/isdf.h): the unchanged lbfgs_rounds + k_lbfgs_feed for B instances of dimension n on a HOST objective.
@@ -1324,23 +1363,18 @@ extern "C" int isdf_dbg_lbfgs_rounds(isdf_ctx *c, int B, int n, const isdf_lbfgs
                              return 0;
                          });
     if (r) return r;
-    CU_TRY(cudaMemcpy(x, lb.d_x.p, sizeof(double) * bn, cudaMemcpyDeviceToHost));
-    CU_TRY(cudaMemcpy(f, lb.d_f.p, sizeof(double) * B, cudaMemcpyDeviceToHost));
-    if (ret) CU_TRY(cudaMemcpy(ret, lb.d_head.p, sizeof(int) * B, cudaMemcpyDeviceToHost));
-    if (iterations) CU_TRY(cudaMemcpy(iterations, lb.d_head.p + B, sizeof(int) * B, cudaMemcpyDeviceToHost));
-    if (evaluations) CU_TRY(cudaMemcpy(evaluations, lb.d_head.p + 2 * (size_t)B, sizeof(int) * B, cudaMemcpyDeviceToHost));
-    return 0;
+    return lbfgs_copy_out(lb, B, (size_t)n, x, f, ret, iterations, evaluations);
 }
 
 extern "C" int isdf_get_batch_trajectories(isdf_ctx *c, double *T, double *coeffs, double *energy) {
     if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
     if (c->batch.B <= 0) return fail(ISDF_ERR_STATE, "no batched callback evaluated yet");
-    if (set_device(c)) return ISDF_ERR_CUDA;
+    if (int r = sync_ctx(c)) return r;
     const size_t BN = (size_t)c->batch.B * c->batch.N0;
-    CU_TRY(cudaStreamSynchronize(c->stream));
-    if (T) CU_TRY(cudaMemcpy(T, c->batch.d_T.p, sizeof(double) * BN, cudaMemcpyDeviceToHost));
-    if (coeffs) CU_TRY(cudaMemcpy(coeffs, c->batch.d_C.p, sizeof(double) * 18 * BN, cudaMemcpyDeviceToHost));
-    if (energy) CU_TRY(cudaMemcpy(energy, c->batch.d_energy.p, sizeof(double) * c->batch.B, cudaMemcpyDeviceToHost));
+    const MincoWork &w = c->batch.minco;
+    if (T) CU_TRY(cudaMemcpy(T, w.d_T.p, sizeof(double) * BN, cudaMemcpyDeviceToHost));
+    if (coeffs) CU_TRY(cudaMemcpy(coeffs, w.d_C.p, sizeof(double) * 18 * BN, cudaMemcpyDeviceToHost));
+    if (energy) CU_TRY(cudaMemcpy(energy, w.d_energy.p, sizeof(double) * c->batch.B, cudaMemcpyDeviceToHost));
     return 0;
 }
 
@@ -1393,27 +1427,21 @@ static int midend_check(isdf_ctx *c, int B, int N0, const isdf_midend_params *p)
         p->cancel_after < 0)
         return fail(ISDF_ERR_INVALID, "mid-end parameter out of range");
     if (int r = lbfgs_check(&p->lbfgs)) return r;
-    if (minco_smem_bytes(N0) > 220 * 1024) return fail(ISDF_ERR_UNSUPPORTED, "pieces per problem too large for the shared-memory banded solver (N0 <= 290)");
+    if (int r = minco_fits(N0)) return r;
     if (c->world != 1) return fail(ISDF_ERR_STATE, "the mid-end shards by PROBLEM: keep isdf_set_shard(ctx, 0, 1) and give each rank its own problems");
     return 0;
 }
 
-static MincoArgs midend_minco_args(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int bc_stride, double rho, const double *d_x) {
-    MincoArgs M;
-    M.B = B; M.N = N0; M.x = d_x; M.head = d_head; M.tail = d_tail; M.bc_stride = bc_stride; M.rho = rho;
-    M.T = c->mid.d_T.p; M.C = c->mid.d_C.p; M.Cpp = nullptr; M.sv_out = nullptr; M.lu = c->mid.d_lu.p; M.energy = c->mid.d_energy.p;
-    M.gC_e = c->mid.d_gC.p; M.gT_e = c->mid.d_gT.p; M.disc_out = c->mid.d_out.p; M.piece_cost = c->mid.d_pc.p;
-    M.cost = nullptr; M.grad = nullptr; M.seq_terms = 1;
-    return M;
+static int midend_buffers(isdf_ctx *c, int B, int N0) {
+    if (int r = c->mid.minco.ensure(B, N0)) return r;
+    CU_TRY(c->mid.d_pc.ensure((size_t)B * N0));
+    return 0;
 }
 
-static int midend_buffers(isdf_ctx *c, int B, int N0) {
-    const size_t BN = (size_t)B * N0, smem = minco_smem_bytes(N0);
-    CU_TRY(c->mid.d_T.ensure(BN)); CU_TRY(c->mid.d_C.ensure(18 * BN)); CU_TRY(c->mid.d_lu.ensure(78 * BN)); CU_TRY(c->mid.d_energy.ensure(B));
-    CU_TRY(c->mid.d_gC.ensure(18 * BN)); CU_TRY(c->mid.d_gT.ensure(BN)); CU_TRY(c->mid.d_out.ensure(19 * BN + 1)); CU_TRY(c->mid.d_pc.ensure(BN));
-    CU_TRY(cudaFuncSetAttribute(k_minco_forward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CU_TRY(cudaFuncSetAttribute(k_minco_backward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    return 0;
+static MincoArgs midend_minco_args(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int bc_stride, double rho, const double *d_x) {
+    MincoArgs M = c->mid.minco.args(B, N0, d_head, d_tail, bc_stride, rho, d_x);
+    M.disc_out = c->mid.minco.d_out.p; M.piece_cost = c->mid.d_pc.p; M.seq_terms = 1;
+    return M;
 }
 
 // one evaluation of OriTraj::costFunction for all B problems: MINCO forward -> pose term -> adjoint with the terms added one at a time
@@ -1424,7 +1452,7 @@ static int midend_eval_launch(isdf_ctx *c, int B, int N0, const double *d_head, 
     M.cost = d_cost; M.grad = d_grad;
     k_minco_forward<<<B, 32, smem, st>>>(M);
     MidendArgs P;
-    P.B = B; P.N = N0; P.K = c->cfg.integral_intervs; P.weight = p->weight_pr; P.T = M.T; P.C = M.C; P.wp = d_wp; P.out = c->mid.d_out.p; P.piece_cost = c->mid.d_pc.p;
+    P.B = B; P.N = N0; P.K = c->cfg.integral_intervs; P.weight = p->weight_pr; P.T = M.T; P.C = M.C; P.wp = d_wp; P.out = c->mid.minco.d_out.p; P.piece_cost = c->mid.d_pc.p;
     k_midend_pose<<<(unsigned)((BN + 127) / 128), 128, 0, st>>>(P);
     k_minco_backward<<<B, 32, smem, st>>>(M);
     c->stats.kernel_launches += 3;
@@ -1435,38 +1463,32 @@ static int midend_eval_launch(isdf_ctx *c, int B, int N0, const double *d_head, 
 // the mid-end's host entry points stage their inputs in c->mid: boundary conditions (*d_head, *d_tail) and waypoints
 static int midend_upload(isdf_ctx *c, int B, int N0, int per_problem_bc, const double *head, const double *tail, const double *waypoints,
                          const double **d_head, const double **d_tail, const double **d_wp) {
-    const size_t nbc = per_problem_bc ? (size_t)9 * B : 9, nwp = (size_t)3 * B * (N0 - 1);
-    CU_TRY(c->mid.d_bc.ensure(2 * nbc)); CU_TRY(c->mid.d_wp.ensure(nwp > 0 ? nwp : 1));
-    CU_TRY(cudaMemcpyAsync(c->mid.d_bc.p, head, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
-    CU_TRY(cudaMemcpyAsync(c->mid.d_bc.p + nbc, tail, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
+    const size_t nwp = (size_t)3 * B * (N0 - 1);
+    if (int r = upload_bc(c, c->mid.d_bc, B, per_problem_bc, head, tail, d_head, d_tail)) return r;
+    CU_TRY(c->mid.d_wp.ensure(nwp > 0 ? nwp : 1));
     if (nwp) CU_TRY(cudaMemcpyAsync(c->mid.d_wp.p, waypoints, sizeof(double) * nwp, cudaMemcpyHostToDevice, c->stream));
-    *d_head = c->mid.d_bc.p; *d_tail = c->mid.d_bc.p + nbc; *d_wp = c->mid.d_wp.p;
+    *d_wp = c->mid.d_wp.p;
     return 0;
 }
 
 extern "C" int isdf_midend_callback_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc,
                                           const isdf_midend_params *p, const double *waypoints, const double *x, double *cost, double *grad) {
-    auto poison_all = [&]() { if (cost && B > 0) for (int b = 0; b < B; b++) cost[b] = std::numeric_limits<double>::quiet_NaN(); };
-    int r = midend_check(c, B, N0, p);
-    if (r) { poison_all(); return r; }
-    if (!head || !tail || !x || !cost || !grad || (N0 > 1 && !waypoints)) { poison_all(); return fail(ISDF_ERR_INVALID, "NULL argument"); }
-    auto body = [&]() -> int {
+    return poison_on_failure([&]() -> int {
+        if (int r = midend_check(c, B, N0, p)) return r;
+        if (!head || !tail || !x || !cost || !grad || (N0 > 1 && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
         const size_t dim = (size_t)4 * N0 - 3;
         const double *d_head, *d_tail, *d_wp;
-        if (int rr = midend_upload(c, B, N0, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return rr;
+        if (int r = midend_upload(c, B, N0, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return r;
         CU_TRY(c->mid.d_x.upload(x, dim * B, c->stream));
         CU_TRY(c->mid.d_cost.ensure(B)); CU_TRY(c->mid.d_grad.ensure(dim * B));
-        if (int rr = midend_buffers(c, B, N0)) return rr;
-        if (int rr = midend_eval_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, p, d_wp, c->mid.d_x.p, c->mid.d_cost.p, c->mid.d_grad.p, c->stream)) return rr;
+        if (int r = midend_buffers(c, B, N0)) return r;
+        if (int r = midend_eval_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, p, d_wp, c->mid.d_x.p, c->mid.d_cost.p, c->mid.d_grad.p, c->stream)) return r;
         CU_TRY(cudaMemcpyAsync(cost, c->mid.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
         CU_TRY(cudaMemcpyAsync(grad, c->mid.d_grad.p, sizeof(double) * dim * B, cudaMemcpyDeviceToHost, c->stream));
         CU_TRY(cudaStreamSynchronize(c->stream));
         return 0;
-    };
-    r = body();
-    if (r) poison_all();
-    return r;
+    }, [&] { nan_fill(cost, B); });
 }
 
 static int midend_batch_run(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc, const isdf_midend_params *p,
@@ -1502,43 +1524,33 @@ extern "C" int isdf_midend_batch_device(isdf_ctx *c, int B, int N0, const double
                                         const isdf_midend_params *p, const double *d_waypoints, double *d_x, double *d_T, double *d_coeffs,
                                         double *d_f, int32_t *d_ret, int32_t *d_iterations, int32_t *d_evaluations, int32_t *rounds, void *cuda_stream) {
     cudaStream_t st = (cudaStream_t)cuda_stream;
-    auto poison_all = [&]() { if (c && d_f && B > 0 && cudaSetDevice(c->device) == cudaSuccess) { cudaMemsetAsync(d_f, 0xff, sizeof(double) * B, st); cudaStreamSynchronize(st); } };
-    int r = midend_check(c, B, N0, p);
-    if (!r && (!d_head || !d_tail || !d_x || !d_f || (N0 > 1 && !d_waypoints))) r = fail(ISDF_ERR_INVALID, "NULL device pointer");
-    if (!r) r = midend_batch_run(c, B, N0, d_head, d_tail, per_problem_bc, p, d_waypoints, d_x, d_T, d_coeffs, d_f, d_ret, d_iterations, d_evaluations, rounds, st);
-    if (r) poison_all();
-    return r;
+    return poison_on_failure([&]() -> int {
+        if (int r = midend_check(c, B, N0, p)) return r;
+        if (!d_head || !d_tail || !d_x || !d_f || (N0 > 1 && !d_waypoints)) return fail(ISDF_ERR_INVALID, "NULL device pointer");
+        return midend_batch_run(c, B, N0, d_head, d_tail, per_problem_bc, p, d_waypoints, d_x, d_T, d_coeffs, d_f, d_ret, d_iterations, d_evaluations, rounds, st);
+    }, [&] { nan_fill_device(c, d_f, B, st); });
 }
 
 extern "C" int isdf_midend_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc,
                                  const isdf_midend_params *p, const double *waypoints, double *x, double *T, double *coeffs,
                                  double *f, int32_t *ret, int32_t *iterations, int32_t *evaluations, int32_t *rounds) {
-    auto poison_all = [&]() { if (f && B > 0) for (int b = 0; b < B; b++) f[b] = std::numeric_limits<double>::quiet_NaN(); };
-    int r = midend_check(c, B, N0, p);
-    if (r) { poison_all(); return r; }
-    if (!head || !tail || !x || !f || (N0 > 1 && !waypoints)) { poison_all(); return fail(ISDF_ERR_INVALID, "NULL argument"); }
-    auto body = [&]() -> int {
+    return poison_on_failure([&]() -> int {
+        if (int r = midend_check(c, B, N0, p)) return r;
+        if (!head || !tail || !x || !f || (N0 > 1 && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
+        isdf_ctx::LbfgsBufs &lb = c->mid.lb;
         const size_t n = (size_t)4 * N0 - 3, BN = (size_t)B * N0;
         const double *d_head, *d_tail, *d_wp;
-        if (int rr = midend_upload(c, B, N0, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return rr;
-        CU_TRY(c->mid.lb.d_x.ensure(n * B)); CU_TRY(c->mid.lb.d_f.ensure((size_t)19 * BN + B)); CU_TRY(c->mid.lb.d_head.ensure((size_t)3 * B));
-        double *d_f = c->mid.lb.d_f.p, *d_T = d_f + B, *d_C = d_T + BN;
-        int *d_i = c->mid.lb.d_head.p;
-        if (int rr = midend_batch_run(c, B, N0, d_head, d_tail, per_problem_bc, p, d_wp, c->mid.lb.d_x.p, d_T, d_C, d_f, d_i, d_i + B, d_i + 2 * (size_t)B,
-                                      rounds, c->stream)) return rr;
-        CU_TRY(cudaMemcpy(x, c->mid.lb.d_x.p, sizeof(double) * n * B, cudaMemcpyDeviceToHost));
-        CU_TRY(cudaMemcpy(f, d_f, sizeof(double) * B, cudaMemcpyDeviceToHost));
+        if (int r = midend_upload(c, B, N0, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return r;
+        CU_TRY(lb.d_x.ensure(n * B)); CU_TRY(lb.d_f.ensure((size_t)19 * BN + B)); CU_TRY(lb.d_head.ensure((size_t)3 * B));
+        double *d_f = lb.d_f.p, *d_T = d_f + B, *d_C = d_T + BN;   // [f | T | coeffs]
+        int *d_i = lb.d_head.p;
+        if (int r = midend_batch_run(c, B, N0, d_head, d_tail, per_problem_bc, p, d_wp, lb.d_x.p, d_T, d_C, d_f, d_i, d_i + B, d_i + 2 * (size_t)B,
+                                     rounds, c->stream)) return r;
         if (T) CU_TRY(cudaMemcpy(T, d_T, sizeof(double) * BN, cudaMemcpyDeviceToHost));
         if (coeffs) CU_TRY(cudaMemcpy(coeffs, d_C, sizeof(double) * 18 * BN, cudaMemcpyDeviceToHost));
-        if (ret) CU_TRY(cudaMemcpy(ret, d_i, sizeof(int) * B, cudaMemcpyDeviceToHost));
-        if (iterations) CU_TRY(cudaMemcpy(iterations, d_i + B, sizeof(int) * B, cudaMemcpyDeviceToHost));
-        if (evaluations) CU_TRY(cudaMemcpy(evaluations, d_i + 2 * (size_t)B, sizeof(int) * B, cudaMemcpyDeviceToHost));
-        return 0;
-    };
-    r = body();
-    if (r) poison_all();
-    return r;
+        return lbfgs_copy_out(lb, B, n, x, f, ret, iterations, evaluations);
+    }, [&] { nan_fill(f, B); });
 }
 
 // ---- trajectory clearance check (isdf_clearance.cuh) -------------------------------------------------------------------------------
@@ -1579,25 +1591,32 @@ static int clearance_check(isdf_ctx *c, int N, const isdf_clearance_params *p) {
     return 0;
 }
 
-static int clearance_launch_ctx(isdf_ctx *c, int N, const double *d_T, const double *d_C, const isdf_clearance_params *p, double *d_clear,
-                                long long *d_vox, ClrSummary *d_sum, cudaStream_t st) {
-    ClrArgs A = {};   // no sample list, no hit flags: the uniform samples of the definition
-    A.grid = c->map.grid; A.shape = c->mesh.shape; A.fp = c->dcfg.fp; A.half_bd = c->dcfg.half_bd;
-    A.reach = p->reach; A.margin = p->margin;
-    A.N = N; A.K = p->samples_per_piece; A.N0 = p->pieces_per_traj == 0 ? N : p->pieces_per_traj;
-    A.T = d_T; A.C = d_C; A.clear = d_clear; A.voxel = d_vox; A.summary = d_sum;
-    CU_TRY(c->clr.d_cursor.ensure(1));
-    CU_TRY(c->clr.d_counters.ensure(2));
-    CU_TRY(cudaMemsetAsync(c->clr.d_cursor.p, 0, sizeof(int), st));
-    CU_TRY(cudaMemsetAsync(c->clr.d_counters.p, 0, 2 * sizeof(unsigned long long), st));
-    A.cursor = c->clr.d_cursor.p; A.counters = c->clr.d_counters.p;
-    const int mode = c->mesh.shape.kind != ISDF_SHAPE_MESH ? 0 : (c->mesh.shape.mesh.sign_mode == MESH_SIGN_WINDING ? 2 : 1);
-    const long long S = (long long)N * (A.K + 1);
-    const long long want = (S + CLR_WARPS - 1) / CLR_WARPS;
-    const unsigned grid = (unsigned)std::max<long long>(1, std::min(want, (long long)c->sm_count * c->clr_blocks));
-    CU_TRY(clearance_launch(A, mode, grid, st));
-    c->stats.kernel_launches += 2;   // scan kernel, summary kernel
+// a host trajectory block [coeffs 18N | T N] staged in buf on c->stream: the coefficients at buf.p, the durations at *d_T
+static int stage_traj(isdf_ctx *c, DevBuf<double> &buf, int N, const double *T, const double *coeffs, const double **d_T) {
+    CU_TRY(buf.ensure((size_t)19 * N));
+    CU_TRY(cudaMemcpyAsync(buf.p, coeffs, sizeof(double) * 18 * N, cudaMemcpyHostToDevice, c->stream));
+    CU_TRY(cudaMemcpyAsync(buf.p + 18 * (size_t)N, T, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
+    *d_T = buf.p + 18 * (size_t)N;
     return 0;
+}
+
+// the clearance scan of the uniform samples of q over N pieces of (d_T, d_C); outputs, cursor, counters, hit flags and sample list are
+// the caller's
+static ClrArgs clearance_args(const isdf_ctx *c, int N, const double *d_T, const double *d_C, const isdf_clearance_params &q) {
+    ClrArgs A = {};
+    A.grid = c->map.grid; A.shape = c->mesh.shape; A.fp = c->dcfg.fp; A.half_bd = c->dcfg.half_bd;
+    A.reach = q.reach; A.margin = q.margin;
+    A.N = N; A.K = q.samples_per_piece; A.N0 = q.pieces_per_traj == 0 ? N : q.pieces_per_traj;
+    A.T = d_T; A.C = d_C;
+    return A;
+}
+static int clearance_mode(const isdf_ctx *c) {
+    return c->mesh.shape.kind != ISDF_SHAPE_MESH ? 0 : (c->mesh.shape.mesh.sign_mode == MESH_SIGN_WINDING ? 2 : 1);
+}
+// CTAs of a scan over n samples: one warp per sample, at most every resident CTA
+static unsigned clearance_grid(const isdf_ctx *c, long long n) {
+    const long long want = (n + CLR_WARPS - 1) / CLR_WARPS;
+    return (unsigned)std::max<long long>(1, std::min(want, (long long)c->sm_count * c->clr_blocks));
 }
 
 // on failure every summary reads "not shown to be free": min_clearance, t_min, first_hit NaN, voxel_min / piece_min / sample_min /
@@ -1608,53 +1627,59 @@ static isdf_clearance_summary clearance_failed_summary() {
     s.voxel_min = -1; s.piece_min = s.sample_min = s.colliding_samples = -1; s.collision_free = 0;
     return s;
 }
-static void clearance_poison_host(int N, const isdf_clearance_params *p, isdf_clearance_summary *summary) {
-    const int B = clearance_batch(N, p);
-    if (summary) for (int b = 0; b < std::max(B, 1); b++) summary[b] = clearance_failed_summary();
+
+// the summaries of a failed clearance check or certificate: max(B, 1) records at a host pointer, or, with dc, B records at a device pointer
+// of dc's device after stream st (best effort: the pointer itself may be what was wrong)
+template <typename S>
+static void write_failed_summaries(S *out, int B, const S &bad, isdf_ctx *dc = nullptr, cudaStream_t st = nullptr) {
+    if (!out || (dc && B < 1)) return;
+    const std::vector<S> v((size_t)std::max(B, 1), bad);
+    if (!dc) { std::copy(v.begin(), v.end(), out); return; }
+    cudaSetDevice(dc->device);
+    cudaStreamSynchronize(st);
+    cudaMemcpy(out, v.data(), sizeof(S) * v.size(), cudaMemcpyHostToDevice);
+    cudaGetLastError();
 }
 
 extern "C" int isdf_trajectory_clearance_device(isdf_ctx *c, int N, const double *d_T, const double *d_coeffs, const isdf_clearance_params *p,
                                                 double *d_sample_clearance, int64_t *d_sample_voxel, isdf_clearance_summary *d_summary,
                                                 void *cuda_stream) {
-    int r = clearance_check(c, N, p);
-    if (r == 0 && (!d_T || !d_coeffs || !d_sample_clearance || !d_sample_voxel || !d_summary)) r = fail(ISDF_ERR_INVALID, "NULL device pointer");
-    if (r == 0 && set_device(c)) r = ISDF_ERR_CUDA;
-    if (r == 0) r = clearance_launch_ctx(c, N, d_T, d_coeffs, p, d_sample_clearance, (long long *)d_sample_voxel, (ClrSummary *)d_summary,
-                                         (cudaStream_t)cuda_stream);
-    if (r != 0 && c && d_summary && clearance_batch(N, p) > 0) {   // best effort: the pointer itself may be what was wrong
-        std::vector<isdf_clearance_summary> bad((size_t)clearance_batch(N, p), clearance_failed_summary());
-        cudaSetDevice(c->device);
-        cudaStreamSynchronize((cudaStream_t)cuda_stream);
-        cudaMemcpy(d_summary, bad.data(), sizeof(isdf_clearance_summary) * bad.size(), cudaMemcpyHostToDevice);
-        cudaGetLastError();
-    }
-    return r;
+    const cudaStream_t st = (cudaStream_t)cuda_stream;
+    return poison_on_failure([&]() -> int {
+        if (int r = clearance_check(c, N, p)) return r;
+        if (!d_T || !d_coeffs || !d_sample_clearance || !d_sample_voxel || !d_summary) return fail(ISDF_ERR_INVALID, "NULL device pointer");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        ClrArgs A = clearance_args(c, N, d_T, d_coeffs, *p);   // no sample list, no hit flags: the uniform samples of the definition
+        A.clear = d_sample_clearance; A.voxel = (long long *)d_sample_voxel; A.summary = (ClrSummary *)d_summary;
+        CU_TRY(c->clr.d_cursor.ensure(1)); CU_TRY(c->clr.d_counters.ensure(2));
+        CU_TRY(cudaMemsetAsync(c->clr.d_cursor.p, 0, sizeof(int), st));
+        CU_TRY(cudaMemsetAsync(c->clr.d_counters.p, 0, 2 * sizeof(unsigned long long), st));
+        A.cursor = c->clr.d_cursor.p; A.counters = c->clr.d_counters.p;
+        CU_TRY(clearance_launch(A, clearance_mode(c), clearance_grid(c, (long long)N * (A.K + 1)), st));
+        c->stats.kernel_launches += 2;   // scan kernel, summary kernel
+        return 0;
+    }, [&] { if (c) write_failed_summaries(d_summary, clearance_batch(N, p), clearance_failed_summary(), c, st); });
 }
 
 extern "C" int isdf_trajectory_clearance(isdf_ctx *c, int N, const double *T, const double *coeffs, const isdf_clearance_params *p,
                                          double *sample_clearance, int64_t *sample_voxel, isdf_clearance_summary *summary) {
-    int r = clearance_check(c, N, p);
-    if (r == 0 && (!T || !coeffs || !summary)) r = fail(ISDF_ERR_INVALID, "NULL argument");
-    if (r) { clearance_poison_host(N, p, summary); return r; }
-    auto body = [&]() -> int {
+    return poison_on_failure([&]() -> int {
+        if (int r = clearance_check(c, N, p)) return r;
+        if (!T || !coeffs || !summary) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
         const int B = clearance_batch(N, p);
         const size_t S = (size_t)N * (p->samples_per_piece + 1);
-        CU_TRY(c->clr.d_in.ensure((size_t)19 * N));
+        const double *d_T;
+        if (int r = stage_traj(c, c->clr.d_in, N, T, coeffs, &d_T)) return r;
         CU_TRY(c->clr.d_clear.ensure(S)); CU_TRY(c->clr.d_vox.ensure(S)); CU_TRY(c->clr.d_sum.ensure((size_t)B));
-        CU_TRY(cudaMemcpyAsync(c->clr.d_in.p, coeffs, sizeof(double) * 18 * N, cudaMemcpyHostToDevice, c->stream));
-        CU_TRY(cudaMemcpyAsync(c->clr.d_in.p + 18 * (size_t)N, T, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
-        int rr = clearance_launch_ctx(c, N, c->clr.d_in.p + 18 * (size_t)N, c->clr.d_in.p, p, c->clr.d_clear.p, c->clr.d_vox.p, c->clr.d_sum.p, c->stream);
-        if (rr) return rr;
+        if (int r = isdf_trajectory_clearance_device(c, N, d_T, c->clr.d_in.p, p, c->clr.d_clear.p, (int64_t *)c->clr.d_vox.p,
+                                                     (isdf_clearance_summary *)c->clr.d_sum.p, c->stream)) return r;
         CU_TRY(cudaMemcpyAsync(summary, c->clr.d_sum.p, sizeof(isdf_clearance_summary) * B, cudaMemcpyDeviceToHost, c->stream));
         if (sample_clearance) CU_TRY(cudaMemcpyAsync(sample_clearance, c->clr.d_clear.p, sizeof(double) * S, cudaMemcpyDeviceToHost, c->stream));
         if (sample_voxel) CU_TRY(cudaMemcpyAsync(sample_voxel, c->clr.d_vox.p, sizeof(int64_t) * S, cudaMemcpyDeviceToHost, c->stream));
         CU_TRY(cudaStreamSynchronize(c->stream));
         return 0;
-    };
-    r = body();
-    if (r) clearance_poison_host(N, p, summary);
-    return r;
+    }, [&] { write_failed_summaries(summary, clearance_batch(N, p), clearance_failed_summary()); });
 }
 
 // ---- continuous clearance certificate (isdf_certify.cuh) --------------------------------------------------------------------------
@@ -1748,15 +1773,11 @@ static int certify_run(isdf_ctx *c, int N, const double *d_T, const double *d_C,
     CU_TRY(certify_init_launch(A, st));
     c->stats.kernel_launches++;
     // the scan: round 0 is the clearance check's own uniform samples, later rounds the new midpoints
-    ClrArgs S = {};
-    S.grid = c->map.grid; S.shape = c->mesh.shape; S.fp = c->dcfg.fp; S.half_bd = c->dcfg.half_bd;
-    S.reach = q.reach; S.margin = q.margin; S.N = N; S.K = K; S.N0 = N0; S.T = d_T; S.C = d_C;
+    ClrArgs S = clearance_args(c, N, d_T, d_C, q);   // no counters: a certificate leaves isdf_dbg_clearance_counts as it was
     S.clear = z.d_sc.p; S.voxel = z.d_sv.p; S.cursor = z.d_cursor.p; S.hit = z.d_hit.p;
-    const int mode = c->mesh.shape.kind != ISDF_SHAPE_MESH ? 0 : 1;   // winding-sign meshes are refused
     auto scan = [&](long long n) -> int {
         CU_TRY(cudaMemsetAsync(z.d_cursor.p, 0, sizeof(int), st));
-        const long long want = (n + CLR_WARPS - 1) / CLR_WARPS;
-        CU_TRY(clearance_scan_launch(S, mode, (unsigned)std::max<long long>(1, std::min(want, (long long)c->sm_count * c->clr_blocks)), st));
+        CU_TRY(clearance_scan_launch(S, clearance_mode(c), clearance_grid(c, n), st));
         c->stats.kernel_launches++;
         return 0;
     };
@@ -1794,42 +1815,32 @@ static isdf_certify_summary certify_failed_summary() {
 
 extern "C" int isdf_trajectory_certify_device(isdf_ctx *c, int N, const double *d_T, const double *d_coeffs, const isdf_certify_params *p,
                                               isdf_certify_summary *d_summary, void *cuda_stream) {
-    double r = 0.0;
-    int rc = certify_check(c, N, p, &r);
-    if (rc == 0 && (!d_T || !d_coeffs || !d_summary)) rc = fail(ISDF_ERR_INVALID, "NULL device pointer");
-    if (rc == 0 && set_device(c)) rc = ISDF_ERR_CUDA;
-    if (rc == 0) rc = certify_run(c, N, d_T, d_coeffs, p, r, (CertSummary *)d_summary, (cudaStream_t)cuda_stream);
-    if (rc != 0 && c && d_summary && certify_batch(N, p) > 0) {   // best effort: the pointer itself may be what was wrong
-        std::vector<isdf_certify_summary> bad((size_t)certify_batch(N, p), certify_failed_summary());
-        cudaSetDevice(c->device);
-        cudaStreamSynchronize((cudaStream_t)cuda_stream);
-        cudaMemcpy(d_summary, bad.data(), sizeof(isdf_certify_summary) * bad.size(), cudaMemcpyHostToDevice);
-        cudaGetLastError();
-    }
-    return rc;
+    const cudaStream_t st = (cudaStream_t)cuda_stream;
+    return poison_on_failure([&]() -> int {
+        double r = 0.0;
+        if (int rc = certify_check(c, N, p, &r)) return rc;
+        if (!d_T || !d_coeffs || !d_summary) return fail(ISDF_ERR_INVALID, "NULL device pointer");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        return certify_run(c, N, d_T, d_coeffs, p, r, (CertSummary *)d_summary, st);
+    }, [&] { if (c) write_failed_summaries(d_summary, certify_batch(N, p), certify_failed_summary(), c, st); });
 }
 
 extern "C" int isdf_trajectory_certify(isdf_ctx *c, int N, const double *T, const double *coeffs, const isdf_certify_params *p,
                                        isdf_certify_summary *summary) {
-    auto poison = [&]() { if (summary) for (int b = 0; b < std::max(certify_batch(N, p), 1); b++) summary[b] = certify_failed_summary(); };
-    double r = 0.0;
-    int rc = certify_check(c, N, p, &r);
-    if (rc == 0 && (!T || !coeffs || !summary)) rc = fail(ISDF_ERR_INVALID, "NULL argument");
-    if (rc) { poison(); return rc; }
-    auto body = [&]() -> int {
+    return poison_on_failure([&]() -> int {
+        double r = 0.0;
+        if (int rc = certify_check(c, N, p, &r)) return rc;
+        if (!T || !coeffs || !summary) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
         const int B = certify_batch(N, p);
-        CU_TRY(c->cert.d_in.ensure((size_t)19 * N)); CU_TRY(c->cert.d_sum.ensure((size_t)B));
-        CU_TRY(cudaMemcpyAsync(c->cert.d_in.p, coeffs, sizeof(double) * 18 * N, cudaMemcpyHostToDevice, c->stream));
-        CU_TRY(cudaMemcpyAsync(c->cert.d_in.p + 18 * (size_t)N, T, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
-        if (int rr = certify_run(c, N, c->cert.d_in.p + 18 * (size_t)N, c->cert.d_in.p, p, r, c->cert.d_sum.p, c->stream)) return rr;
+        const double *d_T;
+        if (int rc = stage_traj(c, c->cert.d_in, N, T, coeffs, &d_T)) return rc;
+        CU_TRY(c->cert.d_sum.ensure((size_t)B));
+        if (int rc = isdf_trajectory_certify_device(c, N, d_T, c->cert.d_in.p, p, (isdf_certify_summary *)c->cert.d_sum.p, c->stream)) return rc;
         CU_TRY(cudaMemcpyAsync(summary, c->cert.d_sum.p, sizeof(isdf_certify_summary) * B, cudaMemcpyDeviceToHost, c->stream));
         CU_TRY(cudaStreamSynchronize(c->stream));
         return 0;
-    };
-    rc = body();
-    if (rc) poison();
-    return rc;
+    }, [&] { write_failed_summaries(summary, certify_batch(N, p), certify_failed_summary()); });
 }
 
 // ---- multi-GPU: rank-ordered sum of the sharded evaluation through NVLink peer memory (isdf_peer.cuh) ------------------------------
@@ -1884,13 +1895,7 @@ extern "C" int isdf_peer_allreduce_device(isdf_ctx *c, double *d_vec, int n, voi
     if (c->peer.args.world < 2) return fail(ISDF_ERR_STATE, "not connected (isdf_peer_connect)");
     if (n > c->peer.args.cap) return fail(ISDF_ERR_INVALID, "vector longer than the exchange buffer");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    PeerArgs P = c->peer.args;
-    P.epoch = c->peer.args.epoch + 1;
-    k_peer_allreduce<<<1, 512, 0, (cudaStream_t)cuda_stream>>>(P, d_vec, n);
-    c->stats.kernel_launches++;
-    CU_TRY(cudaGetLastError());
-    c->peer.args.epoch = P.epoch;
-    return 0;
+    return peer_allreduce_launch(c, d_vec, n, (cudaStream_t)cuda_stream);
 }
 
 extern "C" int isdf_peer_status(isdf_ctx *c) {
@@ -2400,25 +2405,21 @@ extern "C" int isdf_set_points_batch(isdf_ctx *c, int B, const int32_t *offsets,
     return 0;
 }
 
-static int swept_common(isdf_ctx *c, int N, const double *d_T, const double *d_C, double *d_out, cudaStream_t st,
+// count_out as launch_discrete's
+static int swept_common(isdf_ctx *c, int N, const double *d_T, const double *d_C, double *d_out, double *count_out, cudaStream_t st,
                         const double *g_t, const double *g_s, const double *g_g) {
     if (c->sv.P <= 0) return fail(ISDF_ERR_STATE, "obstacle points not set (isdf_set_points)");
     if (c->mesh.shape.kind == ISDF_SHAPE_MESH && c->mesh.shape.mesh.sign_mode == MESH_SIGN_WINDING)
         return fail(ISDF_ERR_UNSUPPORTED, "the swept-volume search prunes with distance brackets that need a true distance function: winding-sign meshes "
                                           "(open meshes / soups, ISDF_MESH_SIGN_WINDING) are supported by the discrete path and isdf_shape_query only");
     int launches = 0;
-    cudaError_t e = c->sv.launch(c->dcfg, c->mesh.shape, N, d_T, d_C, d_out, c->rank, c->world, st, g_t, g_s, g_g, &launches);
+    cudaError_t e = c->sv.launch(c->dcfg, c->mesh.shape, N, d_T, d_C, d_out, count_out, c->rank, c->world, st, g_t, g_s, g_g, &launches);
     c->stats.kernel_launches += launches;
     c->stats.evals_swept++;
     if (e != cudaSuccess) return fail(e == cudaErrorInvalidValue ? ISDF_ERR_INVALID : ISDF_ERR_CUDA, std::string("swept: ") + cudaGetErrorString(e));
     if (fused_exchange(c)) {
         if (int r = peer_fuse_check(c, N)) return r;
-        PeerArgs P = c->peer.args;
-        P.epoch = c->peer.args.epoch + 1;
-        k_peer_allreduce<<<1, 512, 0, st>>>(P, d_out, 19 * N + 1);
-        c->stats.kernel_launches++;
-        CU_TRY(cudaGetLastError());
-        c->peer.args.epoch = P.epoch;
+        return peer_allreduce_launch(c, d_out, 19 * N + 1, st);
     }
     return 0;
 }
@@ -2429,16 +2430,16 @@ extern "C" int isdf_eval_swept_device(isdf_ctx *c, int N, const double *d_T, con
     if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
     if (!d_T || !d_coeffs || !d_out) return fail(ISDF_ERR_INVALID, "NULL device pointer");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    return swept_common(c, N, d_T, d_coeffs, d_out, (cudaStream_t)cuda_stream, nullptr, nullptr, nullptr);
+    return swept_common(c, N, d_T, d_coeffs, d_out, nullptr, (cudaStream_t)cuda_stream, nullptr, nullptr, nullptr);
 }
 
-static int eval_swept_host(isdf_ctx *c, int N, const double *T, const double *coeffs, const double *g_t, const double *g_s,
-                           const double *g_g, double *cost, double *gradC, double *gradT) {
-    int r = check_eval_state(c, N, false);
-    if (r) { poison(cost); return r; }
-    if (!c->mesh.have_shape) { poison(cost); return fail(ISDF_ERR_STATE, "shape not set"); }
-    if (!T || !coeffs || !cost || !gradC || !gradT) { poison(cost); return fail(ISDF_ERR_INVALID, "NULL argument"); }
-    DevBuf<double> dgt, dgs, dgg;   // isdf_eval_swept_given: the given t*, sdf and gradients
+// g_t, g_s, g_g: isdf_eval_swept_given's t*, sdf and gradients (nullptr: search them). The caller poisons *cost on failure.
+static int eval_swept_host(isdf_ctx *c, int N, const double *T, const double *coeffs, const double *g_t, const double *g_s, const double *g_g,
+                           double *cost, double *gradC, double *gradT) {
+    if (int r = check_eval_state(c, N, false)) return r;
+    if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
+    if (!T || !coeffs || !cost || !gradC || !gradT) return fail(ISDF_ERR_INVALID, "NULL argument");
+    DevBuf<double> dgt, dgs, dgg;
     return eval_host(c, N, T, coeffs, cost, gradC, gradT, &isdf_stats::last_sdf_evals,
                      [&]() -> int {
                          if (g_t) {
@@ -2448,21 +2449,21 @@ static int eval_swept_host(isdf_ctx *c, int N, const double *T, const double *co
                          return 0;
                      },
                      [&](const double *d_T, const double *d_C, double *d_out, double *count_out) {
-                         c->sv.count_out = count_out;
-                         const int rr = swept_common(c, N, d_T, d_C, d_out, c->stream, dgt.p, dgs.p, dgg.p);
-                         c->sv.count_out = nullptr;
-                         return rr;
+                         return swept_common(c, N, d_T, d_C, d_out, count_out, c->stream, dgt.p, dgs.p, dgg.p);
                      });
 }
 
 extern "C" int isdf_eval_swept(isdf_ctx *c, int N, const double *T, const double *coeffs, double *cost, double *gradC, double *gradT) {
-    return eval_swept_host(c, N, T, coeffs, nullptr, nullptr, nullptr, cost, gradC, gradT);
+    return poison_on_failure([&] { return eval_swept_host(c, N, T, coeffs, nullptr, nullptr, nullptr, cost, gradC, gradT); },
+                             [&] { nan_fill(cost, 1); });
 }
 
 extern "C" int isdf_eval_swept_given(isdf_ctx *c, int N, const double *T, const double *coeffs, const double *tstar, const double *sdf,
                           const double *grel, double *cost, double *gradC, double *gradT) {
-    if (!tstar || !sdf || !grel) { poison(cost); return fail(ISDF_ERR_INVALID, "NULL argument"); }
-    return eval_swept_host(c, N, T, coeffs, tstar, sdf, grel, cost, gradC, gradT);
+    return poison_on_failure([&]() -> int {
+        if (!tstar || !sdf || !grel) return fail(ISDF_ERR_INVALID, "NULL argument");
+        return eval_swept_host(c, N, T, coeffs, tstar, sdf, grel, cost, gradC, gradT);
+    }, [&] { nan_fill(cost, 1); });
 }
 
 extern "C" int isdf_get_swept_results(isdf_ctx *c, double *tstar, double *sdf, double *grel) {
@@ -2483,7 +2484,7 @@ extern "C" int isdf_get_swept_results(isdf_ctx *c, double *tstar, double *sdf, d
 // balanced share per warp and force every non-trivial sample to be split, so tests can compare split parts against the oracle on one
 // GPU); 0 restores the device's own figure.
 extern "C" int isdf_dbg_schedule(isdf_ctx *c, int natural_order, int warp_slots) {
-    if (!c) return -1;
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
     c->disc.no_items = natural_order != 0; c->disc.warp_slots_override = warp_slots > 0 ? warp_slots : 0; c->disc.order_for = -1;
     return 0;
 }
@@ -2493,32 +2494,31 @@ extern "C" int isdf_dbg_schedule(isdf_ctx *c, int natural_order, int warp_slots)
 // collision: stats (6 entries, optional) = {runs, codes written, overflowed runs, local samples M, code capacity, codes requested};
 // pose (M x 8), desc (M x 2: list offset or -1, voxel count) and codes (min(requested, capacity) entries) are optional copies.
 extern "C" int isdf_dbg_window_lists(isdf_ctx *c, int budget, long long *stats, double *pose, int *desc, uint32_t *codes) {
-    if (!c) return -1;
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
     if (budget >= 0) c->disc.wl_budget = budget;
     if (!stats && !pose && !desc && !codes) return 0;
-    if (c->disc.wl_samples == 0) return -2;
-    if (cudaSetDevice(c->device) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) return -3;
+    if (c->disc.wl_samples == 0) return fail(ISDF_ERR_STATE, "no mesh evaluation with collision yet");
+    if (int r = sync_ctx(c)) return r;
     unsigned long long cnt[4];
-    if (cudaMemcpy(cnt, c->disc.d_counter.p + 1, sizeof(cnt), cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    CU_TRY(cudaMemcpy(cnt, c->disc.d_counter.p + 1, sizeof(cnt), cudaMemcpyDeviceToHost));
     const size_t M = (size_t)c->disc.wl_samples, ncodes = (size_t)std::min<unsigned long long>(cnt[0], (unsigned long long)c->disc.wl_cap);
     if (stats) {
         stats[0] = (long long)cnt[1]; stats[1] = (long long)cnt[3]; stats[2] = (long long)cnt[2];
         stats[3] = (long long)M; stats[4] = c->disc.wl_cap; stats[5] = (long long)cnt[0];
     }
-    if (pose && cudaMemcpy(pose, c->disc.d_pose.p, sizeof(double) * 8 * M, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
-    if (desc && cudaMemcpy(desc, c->disc.d_wl_desc.p, sizeof(int2) * M, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
-    if (codes && ncodes && cudaMemcpy(codes, c->disc.d_wl_codes.p, sizeof(uint32_t) * ncodes, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (pose) CU_TRY(cudaMemcpy(pose, c->disc.d_pose.p, sizeof(double) * 8 * M, cudaMemcpyDeviceToHost));
+    if (desc) CU_TRY(cudaMemcpy(desc, c->disc.d_wl_desc.p, sizeof(int2) * M, cudaMemcpyDeviceToHost));
+    if (codes && ncodes) CU_TRY(cudaMemcpy(codes, c->disc.d_wl_codes.p, sizeof(uint32_t) * ncodes, cudaMemcpyDeviceToHost));
     return 0;
 }
 // number of work items / split samples of the table built by the last discrete evaluation
 extern "C" int isdf_dbg_item_stats(isdf_ctx *c, int *item_count, int *split_parts) {
-    if (!c || !item_count || !split_parts || !c->disc.d_item_count.p) return -1;
-    if (cudaSetDevice(c->device) != cudaSuccess) return -3;
-    cudaStreamSynchronize(c->stream); cudaStreamSynchronize(c->aux_stream);
+    if (!c || !item_count || !split_parts || !c->disc.d_item_count.p) return fail(ISDF_ERR_INVALID, "NULL argument or no discrete evaluation yet");
+    if (int r = sync_ctx(c, true)) return r;
     int n = 0;
-    if (cudaMemcpy(&n, c->disc.d_item_count.p, sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    CU_TRY(cudaMemcpy(&n, c->disc.d_item_count.p, sizeof(int), cudaMemcpyDeviceToHost));
     std::vector<int> it((size_t)3 * std::max(n, 1));
-    if (n > 0 && cudaMemcpy(it.data(), c->disc.d_items.p, sizeof(int) * 3 * n, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (n > 0) CU_TRY(cudaMemcpy(it.data(), c->disc.d_items.p, sizeof(int) * 3 * n, cudaMemcpyDeviceToHost));
     int parts = 0;
     for (int k = 0; k < n; k++) if (it[3 * k + 2] >= 0) parts++;
     *item_count = n; *split_parts = parts;
@@ -2530,22 +2530,21 @@ extern "C" int isdf_dbg_item_stats(isdf_ctx *c, int *item_count, int *split_part
 // c0 | c1 << 8, split slot or -1; up to cap_items rows) and work (M values d_work[rank + world m]) are optional. Read it before the
 // next evaluation: its scan overwrites the work values.
 extern "C" int isdf_dbg_item_table(isdf_ctx *c, long long *info, int *items, long long cap_items, unsigned *work) {
-    if (!c || !info) return -1;
-    if (c->disc.last_M == 0) return -2;
-    if (cudaSetDevice(c->device) != cudaSuccess) return -3;
-    if (cudaStreamSynchronize(c->stream) != cudaSuccess || cudaStreamSynchronize(c->aux_stream) != cudaSuccess) return -3;
+    if (!c || !info) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (c->disc.last_M == 0) return fail(ISDF_ERR_STATE, "no discrete evaluation yet");
+    if (int r = sync_ctx(c, true)) return r;
     int n = 0;
-    if (c->disc.last_builder && cudaMemcpy(&n, c->disc.d_item_count.p, sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (c->disc.last_builder) CU_TRY(cudaMemcpy(&n, c->disc.d_item_count.p, sizeof(int), cudaMemcpyDeviceToHost));
     const long long M = c->disc.last_M;
     const long long v[8] = {M, c->disc.last_rank, c->disc.last_world, c->disc.last_max_split, c->disc.last_warp_slots, n, c->disc.last_builder,
                             c->disc.last_have_items ? 1 : 0};
     std::memcpy(info, v, sizeof(v));
     const long long rows = std::min<long long>(n, std::max(cap_items, 0ll));
-    if (items && rows > 0 && cudaMemcpy(items, c->disc.d_items.p, sizeof(int) * 3 * rows, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (items && rows > 0) CU_TRY(cudaMemcpy(items, c->disc.d_items.p, sizeof(int) * 3 * rows, cudaMemcpyDeviceToHost));
     if (work) {
         const size_t S = (size_t)(c->disc.last_rank + c->disc.last_world * (M - 1) + 1);
         std::vector<unsigned> all(S);
-        if (cudaMemcpy(all.data(), c->disc.d_work.p, sizeof(unsigned) * S, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+        CU_TRY(cudaMemcpy(all.data(), c->disc.d_work.p, sizeof(unsigned) * S, cudaMemcpyDeviceToHost));
         for (long long m = 0; m < M; m++) work[m] = all[(size_t)(c->disc.last_rank + c->disc.last_world * m)];
     }
     return 0;
@@ -2553,33 +2552,33 @@ extern "C" int isdf_dbg_item_table(isdf_ctx *c, long long *info, int *items, lon
 // the device flatness map and its adjoint as compiled into the epilogue kernel: vaj n x 9 (vel, acc, jer), grads n x 10
 // (quat_grad 4, omg_grad 3, vel_grad 3) -> out n x 16 (quat 4, omg 3, total grads wrt vel, acc, jer)
 extern "C" int isdf_dbg_flatness(isdf_ctx *c, int n, const double *vaj, const double *grads, double *out) {
-    if (!c || n < 1 || !vaj || !grads || !out) return -1;
-    if (cudaSetDevice(c->device) != cudaSuccess) return -3;
+    if (!c || n < 1 || !vaj || !grads || !out) return fail(ISDF_ERR_INVALID, "bad argument");
+    if (set_device(c)) return ISDF_ERR_CUDA;
     DevBuf<double> dv, dg, dout;
-    cudaError_t e = dv.upload(vaj, (size_t)9 * n, c->stream);
-    if (e == cudaSuccess) e = dg.upload(grads, (size_t)10 * n, c->stream);
-    if (e == cudaSuccess) e = dout.ensure((size_t)16 * n);
-    if (e == cudaSuccess) e = discrete_launch_dbg_flatness(c->dcfg.fp, n, dv.p, dg.p, dout.p, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out, dout.p, sizeof(double) * 16 * n, cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    return e == cudaSuccess ? 0 : -3;
+    CU_TRY(dv.upload(vaj, (size_t)9 * n, c->stream));
+    CU_TRY(dg.upload(grads, (size_t)10 * n, c->stream));
+    CU_TRY(dout.ensure((size_t)16 * n));
+    CU_TRY(discrete_launch_dbg_flatness(c->dcfg.fp, n, dv.p, dg.p, dout.p, c->stream));
+    CU_TRY(cudaMemcpyAsync(out, dout.p, sizeof(double) * 16 * n, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(cudaStreamSynchronize(c->stream));
+    return 0;
 }
 // read-only view of the current mesh's body-frame cell grid, so tests can tell which search branch answers a query:
 // geom = {glo[3], gcell, ghd, gpad, sign_radius, list_reach}, gdim[3]; cell_dist / cell_cnt (gdim[0]*gdim[1]*gdim[2] entries, z fastest)
 // are optional — call with NULL first to size them. cell_cnt is 0 for every cell without a candidate list (all of them when no
 // list was built).
 extern "C" int isdf_dbg_mesh_grid(isdf_ctx *c, double *geom, int32_t *gdim, float *cell_dist, uint16_t *cell_cnt) {
-    if (!c || !geom || !gdim) return -1;
-    if (!c->mesh.have_shape || c->mesh.shape.kind != ISDF_SHAPE_MESH) return -2;
+    if (!c || !geom || !gdim) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (!c->mesh.have_shape || c->mesh.shape.kind != ISDF_SHAPE_MESH) return fail(ISDF_ERR_STATE, "no mesh shape set");
     const DevMesh &m = c->mesh.shape.mesh;
     for (int a = 0; a < 3; a++) { geom[a] = m.glo[a]; gdim[a] = m.gdim[a]; }
     geom[3] = m.gcell; geom[4] = m.ghd; geom[5] = m.gpad; geom[6] = m.sign_radius; geom[7] = c->mesh.list_reach;
     const size_t ncell = (size_t)m.gdim[0] * m.gdim[1] * m.gdim[2];
-    if (cudaSetDevice(c->device) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) return -3;
-    if (cell_dist && cudaMemcpy(cell_dist, c->mesh.d_cell_dist.p, sizeof(float) * ncell, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (int r = sync_ctx(c)) return r;
+    if (cell_dist) CU_TRY(cudaMemcpy(cell_dist, c->mesh.d_cell_dist.p, sizeof(float) * ncell, cudaMemcpyDeviceToHost));
     if (cell_cnt) {
         if (!m.cell_cnt) std::memset(cell_cnt, 0, sizeof(uint16_t) * ncell);
-        else if (cudaMemcpy(cell_cnt, m.cell_cnt, sizeof(uint16_t) * ncell, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+        else CU_TRY(cudaMemcpy(cell_cnt, m.cell_cnt, sizeof(uint16_t) * ncell, cudaMemcpyDeviceToHost));
     }
     return 0;
 }
@@ -2587,38 +2586,38 @@ extern "C" int isdf_dbg_mesh_grid(isdf_ctx *c, double *geom, int32_t *gdim, floa
 // cell, as isdf_dbg_mesh_grid), cand / cand_lb (sizes[0] each) and tris (the leaf-order triangle records, 16 doubles each) are
 // optional — call with NULL first to size them.
 extern "C" int isdf_dbg_mesh_lists(isdf_ctx *c, long long *sizes, uint32_t *cell_off, uint32_t *cand, float *cand_lb, double *tris) {
-    if (!c || !sizes) return -1;
-    if (!c->mesh.have_shape || c->mesh.shape.kind != ISDF_SHAPE_MESH) return -2;
+    if (!c || !sizes) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (!c->mesh.have_shape || c->mesh.shape.kind != ISDF_SHAPE_MESH) return fail(ISDF_ERR_STATE, "no mesh shape set");
     const DevMesh &m = c->mesh.shape.mesh;
     const size_t ncell = (size_t)m.gdim[0] * m.gdim[1] * m.gdim[2];
-    if (cudaSetDevice(c->device) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) return -3;
+    if (int r = sync_ctx(c)) return r;
     size_t total = 0;
     if (m.cand) {   // the last cell's offset + count
         uint32_t off_last = 0; uint16_t cnt_last = 0;
-        if (cudaMemcpy(&off_last, m.cell_off + ncell - 1, sizeof(uint32_t), cudaMemcpyDeviceToHost) != cudaSuccess ||
-            cudaMemcpy(&cnt_last, m.cell_cnt + ncell - 1, sizeof(uint16_t), cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+        CU_TRY(cudaMemcpy(&off_last, m.cell_off + ncell - 1, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+        CU_TRY(cudaMemcpy(&cnt_last, m.cell_cnt + ncell - 1, sizeof(uint16_t), cudaMemcpyDeviceToHost));
         total = (size_t)off_last + cnt_last;
     }
     sizes[0] = (long long)total; sizes[1] = m.ntris;
-    if (cell_off && m.cand && cudaMemcpy(cell_off, m.cell_off, sizeof(uint32_t) * ncell, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
-    if (cand && total && cudaMemcpy(cand, m.cand, sizeof(uint32_t) * total, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
-    if (cand_lb && total && cudaMemcpy(cand_lb, m.cand_lb, sizeof(float) * total, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
-    if (tris && cudaMemcpy(tris, m.tris, sizeof(double) * TRI_STRIDE * (size_t)m.ntris, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+    if (cell_off && m.cand) CU_TRY(cudaMemcpy(cell_off, m.cell_off, sizeof(uint32_t) * ncell, cudaMemcpyDeviceToHost));
+    if (cand && total) CU_TRY(cudaMemcpy(cand, m.cand, sizeof(uint32_t) * total, cudaMemcpyDeviceToHost));
+    if (cand_lb && total) CU_TRY(cudaMemcpy(cand_lb, m.cand_lb, sizeof(float) * total, cudaMemcpyDeviceToHost));
+    if (tris) CU_TRY(cudaMemcpy(tris, m.tris, sizeof(double) * TRI_STRIDE * (size_t)m.ntris, cudaMemcpyDeviceToHost));
     return 0;
 }
 // the swept-volume term of the last batched callback, B x (19 N0 + 1): per problem [cost | gradC 18 N0 | gradT N0], as the callback adds it
 extern "C" int isdf_dbg_batch_swept_out(isdf_ctx *c, double *out, long long n) {
-    if (!c || !out || n < 0 || (size_t)n > c->batch.d_sv.n) return -1;
-    if (cudaSetDevice(c->device) != cudaSuccess) return -3;
-    cudaStreamSynchronize(c->stream);
-    return cudaMemcpy(out, c->batch.d_sv.p, sizeof(double) * n, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -3;
+    if (!c || !out || n < 0 || (size_t)n > c->batch.d_sv.n) return fail(ISDF_ERR_INVALID, "bad argument or no batched swept-volume term of that size");
+    if (int r = sync_ctx(c)) return r;
+    CU_TRY(cudaMemcpy(out, c->batch.d_sv.p, sizeof(double) * n, cudaMemcpyDeviceToHost));
+    return 0;
 }
 // {candidate pairs (voxel centre inside the H box), exact mesh searches} of the last clearance check
 extern "C" int isdf_dbg_clearance_counts(isdf_ctx *c, unsigned long long *out) {
-    if (!c || !out || !c->clr.d_counters.p) return -1;
-    cudaSetDevice(c->device);
-    cudaStreamSynchronize(c->stream);
-    return cudaMemcpy(out, c->clr.d_counters.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -1;
+    if (!c || !out || !c->clr.d_counters.p) return fail(ISDF_ERR_INVALID, "NULL argument or no clearance check yet");
+    if (int r = sync_ctx(c)) return r;
+    CU_TRY(cudaMemcpy(out, c->clr.d_counters.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    return 0;
 }
 
 // (D_a, D_b) of the certificate's motion bound for caller-given intervals (piece, ta, tb) of a trajectory block (T, coeffs: N pieces);
@@ -2632,16 +2631,16 @@ extern "C" int isdf_dbg_certify_bound(isdf_ctx *c, int N, const double *T, const
     if (int rr = certify_shape(c, &r)) return rr;
     if (radius) *radius = r;
     if (set_device(c)) return ISDF_ERR_CUDA;
-    DevBuf<double> d;
+    DevBuf<double> d;   // [coeffs 18N | T N | ta n | tb n | out 2n]
     CU_TRY(d.ensure((size_t)19 * N + 4 * (size_t)n));
+    const double *dT;
+    if (int rr = stage_traj(c, d, N, T, coeffs, &dT)) return rr;
     DevBuf<int> dp;
     CU_TRY(dp.upload(piece, n, c->stream));
-    double *dC = d.p, *dT = d.p + 18 * (size_t)N, *dta = dT + N, *dtb = dta + n, *dout = dtb + n;
-    CU_TRY(cudaMemcpyAsync(dC, coeffs, sizeof(double) * 18 * N, cudaMemcpyHostToDevice, c->stream));
-    CU_TRY(cudaMemcpyAsync(dT, T, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
+    double *dta = d.p + 19 * (size_t)N, *dtb = dta + n, *dout = dtb + n;
     CU_TRY(cudaMemcpyAsync(dta, ta, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
     CU_TRY(cudaMemcpyAsync(dtb, tb, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
-    const CertArgs A = certify_args(c, r, reach, N, dT, dC);
+    const CertArgs A = certify_args(c, r, reach, N, dT, d.p);
     CU_TRY(certify_bound_launch(A, n, dp.p, dta, dtb, dout, c->stream));
     c->stats.kernel_launches++;
     CU_TRY(cudaMemcpyAsync(out, dout, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, c->stream));

@@ -807,7 +807,6 @@ struct SweptState {
     DevBuf<unsigned long long> d_counter;
     DevBuf<unsigned> d_work; DevBuf<int> d_order;
     bool order_ready = false; int order_rank = -1, order_world = -1;
-    double *count_out = nullptr;   // set by the host entry point around one launch
 
     // the only place that replaces the point set: it gives up the current one (and any per-problem sets: set_points_batch sets B
     // after it) before it touches the buffers
@@ -845,7 +844,8 @@ struct SweptState {
         }
         return cudaSuccess;
     }
-    cudaError_t launch(const DevCfg &cfg, const DevShape &shape, int N, const double *d_T, const double *d_C, double *d_out,
+    // count_out (host entry points only): where the count lands, behind the result vector
+    cudaError_t launch(const DevCfg &cfg, const DevShape &shape, int N, const double *d_T, const double *d_C, double *d_out, double *count_out,
                        int rank, int world, cudaStream_t st, const double *g_t, const double *g_s, const double *g_g, int *launches) {
         cudaError_t e;
         if ((e = ensure_common()) != cudaSuccess) return e;

@@ -450,8 +450,7 @@ class Evaluator:
         [cost | gradC 18*N0 | gradT N0]"""
         out = np.zeros((B, 19 * N0 + 1))
         self.lib.isdf_dbg_batch_swept_out.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.c_longlong]
-        if self.lib.isdf_dbg_batch_swept_out(self.h, _dp(out.reshape(-1)), out.size) != 0:
-            raise IsdfError(-1, "isdf_dbg_batch_swept_out failed")
+        self._check(self.lib.isdf_dbg_batch_swept_out(self.h, _dp(out.reshape(-1)), out.size))
         return out
 
     def lbfgs_params(self, **kw):
@@ -637,8 +636,7 @@ class Evaluator:
         """{candidate pairs, exact mesh searches} of the last clearance check (isdf_dbg_clearance_counts, not part of include/isdf.h)"""
         out = (C.c_ulonglong * 2)()
         self.lib.isdf_dbg_clearance_counts.argtypes = [C.c_void_p, C.POINTER(C.c_ulonglong)]
-        if self.lib.isdf_dbg_clearance_counts(self.h, out) != 0:
-            raise IsdfError(-1, "isdf_dbg_clearance_counts failed")
+        self._check(self.lib.isdf_dbg_clearance_counts(self.h, out))
         return int(out[0]), int(out[1])
 
     # ---- continuous clearance certificate (see include/isdf.h) ----
@@ -887,8 +885,7 @@ class Evaluator:
         if the device had that many resident warps (huge values force every non-trivial sample to be split)."""
         vp = C.c_void_p
         self.lib.isdf_dbg_schedule.argtypes = [vp, C.c_int, C.c_int]
-        if self.lib.isdf_dbg_schedule(self.h, int(natural_order), int(warp_slots)) != 0:
-            raise IsdfError(-1, "isdf_dbg_schedule failed")
+        self._check(self.lib.isdf_dbg_schedule(self.h, int(natural_order), int(warp_slots)))
 
     def dbg_window_lists(self, budget=-1, arrays=False):
         """window lists of the last mesh evaluation with collision (k_discrete_prologue). budget >= 0 sets the list capacity of the
@@ -900,29 +897,25 @@ class Evaluator:
         vp, lp, dp = C.c_void_p, C.POINTER(C.c_longlong), C.POINTER(C.c_double)
         ip, up = C.POINTER(C.c_int32), C.POINTER(C.c_uint32)
         self.lib.isdf_dbg_window_lists.argtypes = [vp, C.c_int, lp, dp, ip, up]
-        if self.lib.isdf_dbg_window_lists(self.h, int(budget), None, None, None, None) != 0:
-            raise IsdfError(-1, "isdf_dbg_window_lists failed")
+        self._check(self.lib.isdf_dbg_window_lists(self.h, int(budget), None, None, None, None))
         st = np.zeros(6, dtype=np.int64)
         r = self.lib.isdf_dbg_window_lists(self.h, -1, st.ctypes.data_as(lp), None, None, None)
-        if r == -2 and budget >= 0:
+        if r == -2 and budget >= 0:     # ISDF_ERR_STATE: no mesh evaluation with collision yet
             return None
-        if r != 0:
-            raise IsdfError(r, "isdf_dbg_window_lists failed (no mesh evaluation with collision yet?)")
+        self._check(r)
         out = dict(runs=int(st[0]), written=int(st[1]), overflow=int(st[2]), samples=int(st[3]), capacity=int(st[4]), requested=int(st[5]))
         if arrays:
             M = out["samples"]
             pose, desc = np.zeros((M, 8)), np.zeros((M, 2), dtype=np.int32)
             codes = np.zeros(max(min(out["requested"], out["capacity"]), 1), dtype=np.uint32)
-            if self.lib.isdf_dbg_window_lists(self.h, -1, None, _dp(pose), desc.ctypes.data_as(ip), codes.ctypes.data_as(up)) != 0:
-                raise IsdfError(-1, "isdf_dbg_window_lists failed")
+            self._check(self.lib.isdf_dbg_window_lists(self.h, -1, None, _dp(pose), desc.ctypes.data_as(ip), codes.ctypes.data_as(up)))
             out.update(pose=pose, desc=desc, codes=codes[:min(out["requested"], out["capacity"])])
         return out
 
     def dbg_item_stats(self):
         n, parts = C.c_int(0), C.c_int(0)
         self.lib.isdf_dbg_item_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-        if self.lib.isdf_dbg_item_stats(self.h, C.byref(n), C.byref(parts)) != 0:
-            raise IsdfError(-1, "isdf_dbg_item_stats failed")
+        self._check(self.lib.isdf_dbg_item_stats(self.h, C.byref(n), C.byref(parts)))
         return n.value, parts.value
 
     def dbg_item_table(self):
@@ -934,13 +927,10 @@ class Evaluator:
         vp, lp, ip, up = C.c_void_p, C.POINTER(C.c_longlong), C.POINTER(C.c_int32), C.POINTER(C.c_uint32)
         self.lib.isdf_dbg_item_table.argtypes = [vp, lp, ip, C.c_longlong, up]
         info = np.zeros(8, dtype=np.int64)
-        r = self.lib.isdf_dbg_item_table(self.h, info.ctypes.data_as(lp), None, 0, None)
-        if r != 0:
-            raise IsdfError(r, "isdf_dbg_item_table failed (no discrete evaluation yet?)")
+        self._check(self.lib.isdf_dbg_item_table(self.h, info.ctypes.data_as(lp), None, 0, None))
         M, n = int(info[0]), int(info[5])
         items, work = np.zeros((max(n, 1), 3), dtype=np.int32), np.zeros(M, dtype=np.uint32)
-        if self.lib.isdf_dbg_item_table(self.h, info.ctypes.data_as(lp), items.ctypes.data_as(ip), n, work.ctypes.data_as(up)) != 0:
-            raise IsdfError(-1, "isdf_dbg_item_table failed")
+        self._check(self.lib.isdf_dbg_item_table(self.h, info.ctypes.data_as(lp), items.ctypes.data_as(ip), n, work.ctypes.data_as(up)))
         return dict(M=M, rank=int(info[1]), world=int(info[2]), max_split=int(info[3]), warp_slots=int(info[4]), item_count=n,
                     builder=("none", "cached", "uncached")[int(info[6])], have_items=bool(info[7]), items=items[:n], work=work)
 
@@ -951,13 +941,11 @@ class Evaluator:
         ip, fp, up = C.POINTER(C.c_int32), C.POINTER(C.c_float), C.POINTER(C.c_uint16)
         self.lib.isdf_dbg_mesh_grid.argtypes = [vp, dp, ip, fp, up]
         geom, gdim = np.zeros(8), np.zeros(3, dtype=np.int32)
-        if self.lib.isdf_dbg_mesh_grid(self.h, _dp(geom), gdim.ctypes.data_as(ip), None, None) != 0:
-            raise IsdfError(-1, "isdf_dbg_mesh_grid failed (is a mesh shape set?)")
+        self._check(self.lib.isdf_dbg_mesh_grid(self.h, _dp(geom), gdim.ctypes.data_as(ip), None, None))
         out = dict(glo=geom[0:3].copy(), gcell=geom[3], ghd=geom[4], gpad=geom[5], sign_radius=geom[6], list_reach=geom[7], gdim=tuple(int(g) for g in gdim))
         if arrays:
             dist, cnt = np.zeros(tuple(gdim), dtype=np.float32), np.zeros(tuple(gdim), dtype=np.uint16)
-            if self.lib.isdf_dbg_mesh_grid(self.h, _dp(geom), gdim.ctypes.data_as(ip), dist.ctypes.data_as(fp), cnt.ctypes.data_as(up)) != 0:
-                raise IsdfError(-1, "isdf_dbg_mesh_grid failed")
+            self._check(self.lib.isdf_dbg_mesh_grid(self.h, _dp(geom), gdim.ctypes.data_as(ip), dist.ctypes.data_as(fp), cnt.ctypes.data_as(up)))
             out["cell_dist"], out["cell_cnt"] = dist, cnt
         return out
 
@@ -968,15 +956,13 @@ class Evaluator:
         u32p, fp = C.POINTER(C.c_uint32), C.POINTER(C.c_float)
         self.lib.isdf_dbg_mesh_lists.argtypes = [vp, llp, u32p, u32p, fp, C.POINTER(C.c_double)]
         sizes = np.zeros(2, dtype=np.int64)
-        if self.lib.isdf_dbg_mesh_lists(self.h, sizes.ctypes.data_as(llp), None, None, None, None) != 0:
-            raise IsdfError(-1, "isdf_dbg_mesh_lists failed (is a mesh shape set?)")
+        self._check(self.lib.isdf_dbg_mesh_lists(self.h, sizes.ctypes.data_as(llp), None, None, None, None))
         gdim = self.dbg_mesh_grid(arrays=False)["gdim"]
         off = np.zeros(gdim, dtype=np.uint32)
         cand, lb = np.zeros(int(sizes[0]), dtype=np.uint32), np.zeros(int(sizes[0]), dtype=np.float32)
         rec = np.zeros((int(sizes[1]), 16))
-        if self.lib.isdf_dbg_mesh_lists(self.h, sizes.ctypes.data_as(llp), off.ctypes.data_as(u32p), cand.ctypes.data_as(u32p),
-                                        lb.ctypes.data_as(fp), _dp(rec)) != 0:
-            raise IsdfError(-1, "isdf_dbg_mesh_lists failed")
+        self._check(self.lib.isdf_dbg_mesh_lists(self.h, sizes.ctypes.data_as(llp), off.ctypes.data_as(u32p), cand.ctypes.data_as(u32p),
+                                                 lb.ctypes.data_as(fp), _dp(rec)))
         a = rec[:, 0:3]
         tris = np.stack([a, a + rec[:, 3:6], a + rec[:, 6:9]], axis=1)
         return dict(cell_off=off, cand=cand, cand_lb=lb, tris=tris)
@@ -989,6 +975,5 @@ class Evaluator:
         out = np.zeros((n, 16))
         dp = C.POINTER(C.c_double)
         self.lib.isdf_dbg_flatness.argtypes = [C.c_void_p, C.c_int, dp, dp, dp]
-        if self.lib.isdf_dbg_flatness(self.h, n, _dp(vaj), _dp(gr), _dp(out)) != 0:
-            raise IsdfError(-1, "isdf_dbg_flatness failed")
+        self._check(self.lib.isdf_dbg_flatness(self.h, n, _dp(vaj), _dp(gr), _dp(out)))
         return out[:, 0:4], out[:, 4:7], out[:, 7:10], out[:, 10:13], out[:, 13:16]
