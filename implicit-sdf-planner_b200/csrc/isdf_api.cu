@@ -11,6 +11,7 @@
 #include "isdf_midend.cuh"
 #include "isdf_clearance.cuh"
 #include "isdf_certify.cuh"
+#include "isdf_sweptvol.cuh"
 #include "isdf_map.cuh"
 #include <queue>
 #include "isdf_host_mesh.cuh"
@@ -166,6 +167,15 @@ struct isdf_ctx {
         PinnedBuf<int> h_tot;
         long long last_leaves = 0;   // leaves of the last call (isdf_dbg_certify_leaves)
     } cert;
+    struct {   // certified swept volume (isdf_sweptvol.cuh): per-call poses and bounds, brick lists, per-warp interval lists, field and mesh
+        DevBuf<double> d_in, d_toff, d_pose, d_Dab, d_pts, d_val, d_low, d_ts, d_V, d_vt;
+        DevBuf<uint8_t> d_dec, d_mask; DevBuf<int32_t> d_F;
+        DevBuf<long long> d_boff, d_bsum, d_voff, d_foff; DevBuf<int> d_blist, d_cursor;
+        DevBuf<SvolIv> d_scratch; DevBuf<unsigned long long> d_counters;
+        PinnedBuf<long long> h_n;
+        int refine_blocks = 0;   // resident CTAs per SM of the refinement kernel (0: not queried yet)
+        cudaEvent_t ev[5] = {};
+    } svol;
     struct {   // peer-memory reduction (isdf_peer.cuh)
         DevBuf<char> buf;                    // own exchange buffer (exported through CUDA IPC)
         void *open[PEER_MAX] = {};           // peers' buffers opened here (null for self / unused)
@@ -181,6 +191,7 @@ struct isdf_ctx {
         peer.buf = {};
         for (cudaEvent_t e : {ev0, ev1, ev_main_done, ev_items_done}) if (e) cudaEventDestroy(e);
         for (cudaEvent_t e : fp.ev) if (e) cudaEventDestroy(e);
+        for (cudaEvent_t e : svol.ev) if (e) cudaEventDestroy(e);
         if (aux_stream) cudaStreamDestroy(aux_stream);
         if (stream) cudaStreamDestroy(stream);
     }
@@ -1692,41 +1703,60 @@ extern "C" int isdf_certify_default_params(isdf_certify_params *p) {
     return 0;
 }
 
+// the shapes whose SDF is a signed Euclidean distance (include/isdf.h): Ball, Point, Box with an orthonormal rotation, exact-sign meshes.
+// `who` prefixes the messages. *r_rot: the radius about the body origin that rotation moves (0 for rotation-invariant bodies);
+// *r_body: the body's bounding radius about its origin; both padded against the rounding of their own computation. pts / npts: the
+// points whose norms give them (Box corners, mesh AABB corners), for the caller's own conditions on the body's extent.
+static int distance_shape(isdf_ctx *c, const char *who, double *r_rot, double *r_body, double pts[8][3], int *npts) {
+    if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
+    const DevShape &s = c->mesh.shape;
+    const std::string w(who);
+    double rr = 0.0, rb = 0.0;
+    *npts = 0;
+    if (s.kind == ISDF_SHAPE_BALL) {
+        rb = std::max(s.par[0], 0.0);
+    } else if (s.kind == ISDF_SHAPE_BOX) {
+        for (int i = 0; i < 3; i++)
+            for (int j = 0; j < 3; j++) {
+                const double d = s.rot[3 * i] * s.rot[3 * j] + s.rot[3 * i + 1] * s.rot[3 * j + 1] + s.rot[3 * i + 2] * s.rot[3 * j + 2];
+                if (!(std::fabs(d - (i == j ? 1.0 : 0.0)) <= 1e-12)) return fail(ISDF_ERR_UNSUPPORTED, w + ": the Box rotation is not orthonormal to 1e-12");
+            }
+        if (!(s.par[0] >= 0.0 && s.par[1] >= 0.0 && s.par[2] >= 0.0)) return fail(ISDF_ERR_UNSUPPORTED, w + ": negative Box half extents");
+        for (int k = 0; k < 8; k++) {   // body point of shape-frame corner q: Rotate q + trans (shape_pre inverted)
+            const double q[3] = {(k & 1) ? s.par[0] : -s.par[0], (k & 2) ? s.par[1] : -s.par[1], (k & 4) ? s.par[2] : -s.par[2]};
+            for (int j = 0; j < 3; j++) pts[k][j] = s.rot[3 * j] * q[0] + s.rot[3 * j + 1] * q[1] + s.rot[3 * j + 2] * q[2] + s.trans[j];
+        }
+        *npts = 8;
+    } else if (s.kind == ISDF_SHAPE_MESH) {
+        if (s.mesh.sign_mode != MESH_SIGN_PSEUDONORMAL) return fail(ISDF_ERR_UNSUPPORTED, w + ": a winding-sign mesh SDF is not a distance");
+        for (int k = 0; k < 8; k++) {
+            pts[k][0] = (k & 1) ? s.mesh.bhi[0] : s.mesh.blo[0]; pts[k][1] = (k & 2) ? s.mesh.bhi[1] : s.mesh.blo[1]; pts[k][2] = (k & 4) ? s.mesh.bhi[2] : s.mesh.blo[2];
+        }
+        *npts = 8;
+    } else if (s.kind != ISDF_SHAPE_POINT) {
+        return fail(ISDF_ERR_UNSUPPORTED, w + ": supported shapes are Ball, Point, Box and exact-sign meshes (their SDF is a distance)");
+    }
+    for (int k = 0; k < *npts; k++) rr = std::max(rr, std::sqrt(pts[k][0] * pts[k][0] + pts[k][1] * pts[k][1] + pts[k][2] * pts[k][2]));
+    if (*npts) rb = rr;
+    *r_rot = rr * (1.0 + 1e-12);
+    *r_body = rb * (1.0 + 1e-12);
+    return 0;
+}
+
 // the shape conditions of the certificate (include/isdf.h): a true Euclidean distance outside the body and a body inside the half_bd box.
 // *r: the body radius about the body origin (0 for rotation-invariant bodies), padded against the rounding of its own computation
 static int certify_shape(isdf_ctx *c, double *r) {
     if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
     const DevShape &s = c->mesh.shape;
     const double hb = c->dcfg.half_bd;
-    auto inside = [&](const double p[3]) { return std::fabs(p[0]) <= hb && std::fabs(p[1]) <= hb && std::fabs(p[2]) <= hb; };
-    double rr = 0.0;
-    if (s.kind == ISDF_SHAPE_BALL) {
-        if (!(s.par[0] >= 0.0 && s.par[0] <= hb)) return fail(ISDF_ERR_UNSUPPORTED, "certificate: the Ball's radius must lie in [0, half_bd]");
-    } else if (s.kind == ISDF_SHAPE_BOX) {
-        for (int i = 0; i < 3; i++)
-            for (int j = 0; j < 3; j++) {
-                const double d = s.rot[3 * i] * s.rot[3 * j] + s.rot[3 * i + 1] * s.rot[3 * j + 1] + s.rot[3 * i + 2] * s.rot[3 * j + 2];
-                if (!(std::fabs(d - (i == j ? 1.0 : 0.0)) <= 1e-12)) return fail(ISDF_ERR_UNSUPPORTED, "certificate: the Box rotation is not orthonormal to 1e-12");
-            }
-        if (!(s.par[0] >= 0.0 && s.par[1] >= 0.0 && s.par[2] >= 0.0)) return fail(ISDF_ERR_UNSUPPORTED, "certificate: negative Box half extents");
-        for (int k = 0; k < 8; k++) {   // body point of shape-frame corner q: Rotate q + trans (shape_pre inverted)
-            const double q[3] = {(k & 1) ? s.par[0] : -s.par[0], (k & 2) ? s.par[1] : -s.par[1], (k & 4) ? s.par[2] : -s.par[2]};
-            double p[3];
-            for (int j = 0; j < 3; j++) p[j] = s.rot[3 * j] * q[0] + s.rot[3 * j + 1] * q[1] + s.rot[3 * j + 2] * q[2] + s.trans[j];
-            if (!inside(p)) return fail(ISDF_ERR_UNSUPPORTED, "certificate: the Box reaches beyond the half_bd box");
-            rr = std::max(rr, std::sqrt(p[0] * p[0] + p[1] * p[1] + p[2] * p[2]));
-        }
-    } else if (s.kind == ISDF_SHAPE_MESH) {
-        if (s.mesh.sign_mode != MESH_SIGN_PSEUDONORMAL) return fail(ISDF_ERR_UNSUPPORTED, "certificate: a winding-sign mesh SDF is not a distance");
-        for (int k = 0; k < 8; k++) {
-            const double p[3] = {(k & 1) ? s.mesh.bhi[0] : s.mesh.blo[0], (k & 2) ? s.mesh.bhi[1] : s.mesh.blo[1], (k & 4) ? s.mesh.bhi[2] : s.mesh.blo[2]};
-            if (!inside(p)) return fail(ISDF_ERR_UNSUPPORTED, "certificate: the mesh's bounding box reaches beyond the half_bd box");
-            rr = std::max(rr, std::sqrt(p[0] * p[0] + p[1] * p[1] + p[2] * p[2]));
-        }
-    } else if (s.kind != ISDF_SHAPE_POINT) {
-        return fail(ISDF_ERR_UNSUPPORTED, "certificate: supported shapes are Ball, Point, Box and exact-sign meshes (their SDF is a distance)");
-    }
-    *r = rr * (1.0 + 1e-12);
+    if (s.kind == ISDF_SHAPE_BALL && !(s.par[0] >= 0.0 && s.par[0] <= hb)) return fail(ISDF_ERR_UNSUPPORTED, "certificate: the Ball's radius must lie in [0, half_bd]");
+    double pts[8][3], rb = 0.0;
+    int npts = 0;
+    if (int rc = distance_shape(c, "certificate", r, &rb, pts, &npts)) return rc;
+    for (int k = 0; k < npts; k++)
+        if (!(std::fabs(pts[k][0]) <= hb && std::fabs(pts[k][1]) <= hb && std::fabs(pts[k][2]) <= hb))
+            return fail(ISDF_ERR_UNSUPPORTED, s.kind == ISDF_SHAPE_BOX ? "certificate: the Box reaches beyond the half_bd box"
+                                                                     : "certificate: the mesh's bounding box reaches beyond the half_bd box");
     return 0;
 }
 
@@ -1841,6 +1871,283 @@ extern "C" int isdf_trajectory_certify(isdf_ctx *c, int N, const double *T, cons
         CU_TRY(cudaStreamSynchronize(c->stream));
         return 0;
     }, [&] { write_failed_summaries(summary, certify_batch(N, p), certify_failed_summary()); });
+}
+
+// ---- certified swept volume (isdf_sweptvol.cuh) ------------------------------------------------------------------------------------
+extern "C" int isdf_swept_default_params(isdf_swept_params *p) {
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    std::memset(p, 0, sizeof(*p));
+    isdf_config d;
+    isdf_default_config(&d);
+    p->samples_per_piece = d.integral_intervs;
+    p->max_depth = 16; p->max_samples_per_point = 512;
+    p->tol = d.occupancy_resolution / 100.0;
+    p->band = 2.0 * d.safety_hor;
+    return 0;
+}
+
+// every check that needs no device work and no trajectory, in the order of include/isdf.h's error list; *r_rot / *r_body as distance_shape
+static int swept_check(isdf_ctx *c, int N, const isdf_swept_params *p, double *r_rot, double *r_body) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    if (N < 1) return fail(ISDF_ERR_INVALID, "N < 1");
+    if (p->reserved_) return fail(ISDF_ERR_INVALID, "reserved_ must be 0");
+    if (p->samples_per_piece < 1) return fail(ISDF_ERR_INVALID, "samples_per_piece < 1");
+    if (!(p->tol > 0.0) || !std::isfinite(p->tol)) return fail(ISDF_ERR_INVALID, "tol must be positive and finite");
+    if (!(p->band > p->tol) || !std::isfinite(p->band)) return fail(ISDF_ERR_INVALID, "band must be finite and larger than tol");
+    if (p->max_depth < 0 || p->max_depth > 64) return fail(ISDF_ERR_INVALID, "max_depth must lie in [0, 64]");
+    if (p->max_samples_per_point < 0) return fail(ISDF_ERR_INVALID, "max_samples_per_point < 0");
+    if ((long long)N * (p->samples_per_piece + 1) > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "N * (samples_per_piece + 1) must fit in 31 bits");
+    if (c->world > 1) return fail(ISDF_ERR_UNSUPPORTED, "the swept volume is not sharded: call it on a context with isdf_set_shard(ctx, 0, 1)");
+    double pts[8][3];
+    int npts = 0;
+    if (int rc = distance_shape(c, "swept volume", r_rot, r_body, pts, &npts)) return rc;
+    if (c->mesh.shape.kind == ISDF_SHAPE_BALL && !(c->mesh.shape.par[0] >= 0.0))
+        return fail(ISDF_ERR_UNSUPPORTED, "swept volume: the Ball's radius must not be negative");
+    return 0;
+}
+
+static long long swept_nodes(const isdf_swept_grid *g) { return g ? (long long)g->X * g->Y * g->Z : 0; }
+
+static int swept_grid_check(const isdf_swept_grid *g) {
+    if (!g) return fail(ISDF_ERR_INVALID, "grid is NULL");
+    if (g->reserved_) return fail(ISDF_ERR_INVALID, "grid reserved_ must be 0");
+    if (!(g->res > 0.0) || !std::isfinite(g->res)) return fail(ISDF_ERR_INVALID, "grid res must be positive and finite");
+    if (g->X < 2 || g->Y < 2 || g->Z < 2) return fail(ISDF_ERR_INVALID, "grid sizes must be >= 2");
+    if (swept_nodes(g) >= 0x80000000ll) return fail(ISDF_ERR_INVALID, "X * Y * Z must be < 2^31");
+    const int n[3] = {g->X, g->Y, g->Z};
+    for (int a = 0; a < 3; a++)
+        if (!std::isfinite(g->bmin[a]) || !std::isfinite(g->bmin[a] + (double)(n[a] - 1) * g->res)) return fail(ISDF_ERR_INVALID, "grid coordinates must be finite");
+    return 0;
+}
+
+// the trajectory (host copies): durations finite and positive, coefficients finite
+static int swept_traj_check(int N, const double *T, const double *coeffs) {
+    for (int i = 0; i < N; i++) if (!(T[i] > 0.0) || !std::isfinite(T[i])) return fail(ISDF_ERR_INVALID, "every T must be positive and finite");
+    for (long long i = 0; i < 18ll * N; i++) if (!std::isfinite(coeffs[i])) return fail(ISDF_ERR_INVALID, "coeffs must be finite");
+    return 0;
+}
+// the same checks on a device trajectory (one copy of 19 N doubles to the host)
+static int swept_traj_check_device(isdf_ctx *c, int N, const double *d_T, const double *d_coeffs, cudaStream_t st) {
+    std::vector<double> h((size_t)19 * N);
+    CU_TRY(cudaMemcpyAsync(h.data(), d_coeffs, sizeof(double) * 18 * N, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaMemcpyAsync(h.data() + 18 * (size_t)N, d_T, sizeof(double) * N, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    (void)c;
+    return swept_traj_check(N, h.data() + 18 * (size_t)N, h.data());
+}
+
+// the field at the nodes of g (or at npts points d_pts when g is null) into device arrays; info (may be null) gets the counters and times
+static int swept_run(isdf_ctx *c, int N, const double *d_T, const double *d_C, const isdf_swept_params *p, double r_rot, double r_body,
+                     const isdf_swept_grid *g, int npts, const double *d_pts, double *d_val, double *d_low, double *d_ts, uint8_t *d_dec,
+                     isdf_swept_info *info, cudaStream_t st) {
+    auto &z = c->svol;
+    const int K = p->samples_per_piece, M = p->max_samples_per_point;
+    const long long NK = (long long)N * K, S = (long long)N * (K + 1);
+    CU_TRY(z.d_toff.ensure(N)); CU_TRY(z.d_pose.ensure((size_t)(12 * S))); CU_TRY(z.d_Dab.ensure((size_t)(2 * NK)));
+    CU_TRY(z.d_cursor.ensure(1)); CU_TRY(z.d_counters.ensure(4)); CU_TRY(z.h_n.ensure(1));
+    if (info) for (cudaEvent_t &e : z.ev) if (!e) CU_TRY(cudaEventCreate(&e));
+    SvolArgs A = {};
+    A.shape = c->mesh.shape; A.fp = c->dcfg.fp; A.r_rot = r_rot; A.r_body = r_body; A.band = p->band; A.tol = p->tol;
+    A.N = N; A.K = K; A.max_depth = p->max_depth; A.max_samples = M; A.T = d_T; A.C = d_C;
+    A.toff = z.d_toff.p; A.pose = z.d_pose.p; A.Dab = z.d_Dab.p;
+    A.value = d_val; A.lower = d_low; A.tstar = d_ts; A.decided = d_dec;
+    A.cursor = z.d_cursor.p; A.counters = z.d_counters.p;
+    if (info) CU_TRY(cudaEventRecord(z.ev[0], st));
+    CU_TRY(cudaMemsetAsync(z.d_counters.p, 0, 4 * sizeof(unsigned long long), st));
+    CU_TRY(sv_prep_launch(A, st));
+    c->stats.kernel_launches++;
+    if (info) CU_TRY(cudaEventRecord(z.ev[1], st));
+    long long nitems = npts, nbricks = 0;
+    if (g) {
+        for (int a = 0; a < 3; a++) A.bmin[a] = g->bmin[a];
+        A.res = g->res; A.X = g->X; A.Y = g->Y; A.Z = g->Z;
+        A.BX = (g->X + SV_BRICK - 1) / SV_BRICK; A.BY = (g->Y + SV_BRICK - 1) / SV_BRICK; A.BZ = (g->Z + SV_BRICK - 1) / SV_BRICK;
+        nbricks = (long long)A.BX * A.BY * A.BZ;
+        CU_TRY(z.d_boff.ensure((size_t)nbricks + 1)); CU_TRY(z.d_bsum.ensure((size_t)(nbricks + SV_SCAN_THREADS) / SV_SCAN_THREADS + 1));
+        A.boff = z.d_boff.p;
+        CU_TRY(sv_bricks_launch(A, (int)nbricks, false, st));
+        CU_TRY(sv_scan_launch(z.d_boff.p, nbricks, z.d_bsum.p, st));
+        c->stats.kernel_launches += 4;   // count pass, three scan kernels
+        CU_TRY(cudaMemcpyAsync(z.h_n.p, z.d_boff.p + nbricks, sizeof(long long), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
+        CU_TRY(z.d_blist.ensure((size_t)std::max(*z.h_n.p, 1ll)));
+        A.blist = z.d_blist.p;
+        CU_TRY(sv_bricks_launch(A, (int)nbricks, true, st));
+        c->stats.kernel_launches++;
+        nitems = nbricks;
+    } else {
+        A.pts = d_pts; A.npts = npts;
+    }
+    if (info) CU_TRY(cudaEventRecord(z.ev[2], st));
+    if (nitems > 0) {
+        if (!z.refine_blocks) { CU_TRY(sv_refine_resident_blocks(&z.refine_blocks)); z.refine_blocks = std::max(z.refine_blocks, 1); }
+        // each resident warp owns two interval lists: round 0's kept intervals (at most N K) and children (at most 2 M) per round
+        A.split_at = std::max(NK, 2ll * M);
+        A.scap = A.split_at + 2ll * M;
+        const long long want = (nitems + SV_WARPS - 1) / SV_WARPS;
+        const unsigned grid = (unsigned)std::max<long long>(1, std::min(want, (long long)c->sm_count * std::min(z.refine_blocks, 2)));
+        A.nwarps = (int)grid * SV_WARPS;
+        CU_TRY(z.d_scratch.ensure((size_t)(A.nwarps * A.scap)));
+        A.scratch = z.d_scratch.p;
+        CU_TRY(cudaMemsetAsync(z.d_cursor.p, 0, sizeof(int), st));
+        CU_TRY(sv_refine_launch(A, c->mesh.shape.kind == ISDF_SHAPE_MESH ? 1 : 0, (int)nitems, grid, st));
+        c->stats.kernel_launches++;
+    }
+    if (info) {
+        CU_TRY(cudaEventRecord(z.ev[3], st));
+        unsigned long long cnt[4];
+        CU_TRY(cudaMemcpyAsync(cnt, z.d_counters.p, sizeof(cnt), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
+        std::memset(info, 0, sizeof(*info));
+        info->nodes = g ? swept_nodes(g) : npts;
+        info->bricks = nbricks; info->bricks_culled = g ? (long long)cnt[3] : 0;
+        info->sdf_evals = (long long)cnt[0]; info->undecided = (long long)cnt[1]; info->deepest = (int)cnt[2];
+        float ms = 0.f;
+        CU_TRY(cudaEventElapsedTime(&ms, z.ev[0], z.ev[1])); info->prep_ms = ms;
+        CU_TRY(cudaEventElapsedTime(&ms, z.ev[1], z.ev[2])); info->cull_ms = ms;
+        CU_TRY(cudaEventElapsedTime(&ms, z.ev[2], z.ev[3])); info->refine_ms = ms;
+    }
+    return 0;
+}
+
+static void swept_poison_host(long long n, double *value, double *lower, double *tstar, uint8_t *decided) {
+    nan_fill(value, n); nan_fill(lower, n); nan_fill(tstar, n);
+    if (decided && n > 0) std::memset(decided, 0, (size_t)n);
+}
+
+extern "C" int isdf_swept_volume_sdf(isdf_ctx *c, int N, const double *T, const double *coeffs, const isdf_swept_params *p, int n,
+                                     const double *pts, double *value, double *lower, double *tstar, uint8_t *decided) {
+    return poison_on_failure([&]() -> int {
+        double r_rot = 0.0, r_body = 0.0;
+        if (int rc = swept_check(c, N, p, &r_rot, &r_body)) return rc;
+        if (!T || !coeffs || !value || (n > 0 && !pts)) return fail(ISDF_ERR_INVALID, "NULL argument");
+        if (n < 0) return fail(ISDF_ERR_INVALID, "n < 0");
+        if (int rc = swept_traj_check(N, T, coeffs)) return rc;
+        for (long long i = 0; i < 3ll * n; i++) if (!std::isfinite(pts[i])) return fail(ISDF_ERR_INVALID, "points must be finite");
+        if (n == 0) return 0;
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        auto &z = c->svol;
+        const double *d_T;
+        if (int rc = stage_traj(c, z.d_in, N, T, coeffs, &d_T)) return rc;
+        CU_TRY(z.d_pts.upload(pts, (size_t)3 * n, c->stream));
+        CU_TRY(z.d_val.ensure(n)); CU_TRY(z.d_low.ensure(n)); CU_TRY(z.d_ts.ensure(n)); CU_TRY(z.d_dec.ensure(n));
+        if (int rc = swept_run(c, N, d_T, z.d_in.p, p, r_rot, r_body, nullptr, n, z.d_pts.p, z.d_val.p, z.d_low.p, z.d_ts.p, z.d_dec.p, nullptr, c->stream))
+            return rc;
+        CU_TRY(cudaMemcpyAsync(value, z.d_val.p, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
+        if (lower) CU_TRY(cudaMemcpyAsync(lower, z.d_low.p, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
+        if (tstar) CU_TRY(cudaMemcpyAsync(tstar, z.d_ts.p, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
+        if (decided) CU_TRY(cudaMemcpyAsync(decided, z.d_dec.p, (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaStreamSynchronize(c->stream));
+        return 0;
+    }, [&] { swept_poison_host(std::max(n, 0), value, lower, tstar, decided); });
+}
+
+extern "C" int isdf_swept_volume_grid_device(isdf_ctx *c, int N, const double *d_T, const double *d_coeffs, const isdf_swept_params *p,
+                                             const isdf_swept_grid *g, double *d_value, double *d_lower, double *d_tstar, uint8_t *d_decided,
+                                             isdf_swept_info *info, void *cuda_stream) {
+    const cudaStream_t st = (cudaStream_t)cuda_stream;
+    return poison_on_failure([&]() -> int {
+        double r_rot = 0.0, r_body = 0.0;
+        if (int rc = swept_check(c, N, p, &r_rot, &r_body)) return rc;
+        if (int rc = swept_grid_check(g)) return rc;
+        if (!d_T || !d_coeffs || !d_value) return fail(ISDF_ERR_INVALID, "NULL device pointer");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        if (int rc = swept_traj_check_device(c, N, d_T, d_coeffs, st)) return rc;
+        return swept_run(c, N, d_T, d_coeffs, p, r_rot, r_body, g, 0, nullptr, d_value, d_lower, d_tstar, d_decided, info, st);
+    }, [&] {
+        const long long n = swept_nodes(g) > 0 && swept_nodes(g) < 0x80000000ll ? swept_nodes(g) : 0;
+        nan_fill_device(c, d_value, (int)n, st); nan_fill_device(c, d_lower, (int)n, st); nan_fill_device(c, d_tstar, (int)n, st);
+        if (c && d_decided && n > 0 && cudaSetDevice(c->device) == cudaSuccess) { cudaMemsetAsync(d_decided, 0, (size_t)n, st); cudaStreamSynchronize(st); }
+    });
+}
+
+// the field of g in the context's buffers (the host grid and mesh entries)
+static int swept_grid_ctx(isdf_ctx *c, int N, const double *T, const double *coeffs, const isdf_swept_params *p, const isdf_swept_grid *g,
+                          isdf_swept_info *info) {
+    double r_rot = 0.0, r_body = 0.0;
+    if (int rc = swept_check(c, N, p, &r_rot, &r_body)) return rc;
+    if (int rc = swept_grid_check(g)) return rc;
+    if (!T || !coeffs) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (int rc = swept_traj_check(N, T, coeffs)) return rc;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    auto &z = c->svol;
+    const size_t n = (size_t)swept_nodes(g);
+    const double *d_T;
+    if (int rc = stage_traj(c, z.d_in, N, T, coeffs, &d_T)) return rc;
+    CU_TRY(z.d_val.ensure(n)); CU_TRY(z.d_low.ensure(n)); CU_TRY(z.d_ts.ensure(n)); CU_TRY(z.d_dec.ensure(n));
+    return swept_run(c, N, d_T, z.d_in.p, p, r_rot, r_body, g, 0, nullptr, z.d_val.p, z.d_low.p, z.d_ts.p, z.d_dec.p, info, c->stream);
+}
+
+extern "C" int isdf_swept_volume_grid(isdf_ctx *c, int N, const double *T, const double *coeffs, const isdf_swept_params *p,
+                                      const isdf_swept_grid *g, double *value, double *lower, double *tstar, uint8_t *decided,
+                                      isdf_swept_info *info) {
+    return poison_on_failure([&]() -> int {
+        if (c && !value) return fail(ISDF_ERR_INVALID, "value is NULL");
+        if (int rc = swept_grid_ctx(c, N, T, coeffs, p, g, info)) return rc;
+        if (!value) return fail(ISDF_ERR_INVALID, "value is NULL");
+        auto &z = c->svol;
+        const size_t n = (size_t)swept_nodes(g);
+        CU_TRY(cudaMemcpyAsync(value, z.d_val.p, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
+        if (lower) CU_TRY(cudaMemcpyAsync(lower, z.d_low.p, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
+        if (tstar) CU_TRY(cudaMemcpyAsync(tstar, z.d_ts.p, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
+        if (decided) CU_TRY(cudaMemcpyAsync(decided, z.d_dec.p, n, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaStreamSynchronize(c->stream));
+        return 0;
+    }, [&] {
+        const long long n = swept_nodes(g) > 0 && swept_nodes(g) < 0x80000000ll ? swept_nodes(g) : 0;
+        swept_poison_host(n, value, lower, tstar, decided);
+    });
+}
+
+extern "C" int isdf_swept_volume_mesh(isdf_ctx *c, int N, const double *T, const double *coeffs, const isdf_swept_params *p,
+                                      const isdf_swept_grid *g, int64_t cap_v, int64_t cap_f, double *V, double *vtime, int32_t *F,
+                                      int64_t *nV, int64_t *nF, isdf_swept_info *info) {
+    return poison_on_failure([&]() -> int {
+        if (c && (!nV || !nF)) return fail(ISDF_ERR_INVALID, "nV / nF is NULL");
+        if (c && (cap_v < 0 || cap_f < 0)) return fail(ISDF_ERR_INVALID, "cap_v / cap_f < 0");
+        if (c && ((cap_v > 0 && (!V || !vtime)) || (cap_f > 0 && !F))) return fail(ISDF_ERR_INVALID, "NULL output with a positive cap");
+        if (int rc = swept_grid_ctx(c, N, T, coeffs, p, g, info)) return rc;
+        if (!nV || !nF) return fail(ISDF_ERR_INVALID, "nV / nF is NULL");
+        auto &z = c->svol;
+        const cudaStream_t st = c->stream;
+        const long long n = swept_nodes(g);
+        if (info) CU_TRY(cudaEventRecord(z.ev[3], st));
+        CU_TRY(z.d_mask.ensure((size_t)n)); CU_TRY(z.d_voff.ensure((size_t)n + 1)); CU_TRY(z.d_foff.ensure((size_t)n + 1));
+        CU_TRY(z.d_bsum.ensure((size_t)(n + SV_SCAN_THREADS) / SV_SCAN_THREADS + 1)); CU_TRY(z.h_n.ensure(2));
+        SvolMeshArgs Mg = {};
+        for (int a = 0; a < 3; a++) Mg.bmin[a] = g->bmin[a];
+        Mg.res = g->res; Mg.X = g->X; Mg.Y = g->Y; Mg.Z = g->Z;
+        Mg.value = z.d_val.p; Mg.tstar = z.d_ts.p; Mg.emask = z.d_mask.p; Mg.voff = z.d_voff.p; Mg.foff = z.d_foff.p;
+        CU_TRY(sv_mesh_count_launch(Mg, st));
+        CU_TRY(sv_scan_launch(z.d_voff.p, n, z.d_bsum.p, st));
+        CU_TRY(sv_scan_launch(z.d_foff.p, n, z.d_bsum.p, st));
+        c->stats.kernel_launches += 7;   // count, two three-kernel scans
+        CU_TRY(cudaMemcpyAsync(z.h_n.p, z.d_voff.p + n, sizeof(long long), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(z.h_n.p + 1, z.d_foff.p + n, sizeof(long long), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
+        *nV = z.h_n.p[0]; *nF = z.h_n.p[1];
+        if (*nV > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "more than 2^31 - 1 vertices: use a coarser grid");
+        if (*nV > cap_v || *nF > cap_f) return fail(ISDF_ERR_INVALID, "cap_v / cap_f smaller than the mesh (*nV / *nF hold the sizes needed)");
+        CU_TRY(z.d_V.ensure((size_t)std::max<long long>(3 * *nV, 1))); CU_TRY(z.d_vt.ensure((size_t)std::max<long long>(*nV, 1)));
+        CU_TRY(z.d_F.ensure((size_t)std::max<long long>(3 * *nF, 1)));
+        Mg.V = z.d_V.p; Mg.vtime = z.d_vt.p; Mg.F = z.d_F.p;
+        CU_TRY(sv_mesh_emit_launch(Mg, st));
+        c->stats.kernel_launches++;
+        if (info) {
+            CU_TRY(cudaEventRecord(z.ev[4], st));
+            CU_TRY(cudaEventSynchronize(z.ev[4]));
+            float ms = 0.f;
+            CU_TRY(cudaEventElapsedTime(&ms, z.ev[3], z.ev[4])); info->mesh_ms = ms;
+        }
+        if (*nV) {
+            CU_TRY(cudaMemcpyAsync(V, z.d_V.p, sizeof(double) * 3 * *nV, cudaMemcpyDeviceToHost, st));
+            CU_TRY(cudaMemcpyAsync(vtime, z.d_vt.p, sizeof(double) * *nV, cudaMemcpyDeviceToHost, st));
+        }
+        if (*nF) CU_TRY(cudaMemcpyAsync(F, z.d_F.p, sizeof(int32_t) * 3 * *nF, cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
+        return 0;
+    }, [&] { if (cap_v > 0) { nan_fill(V, 3 * cap_v); nan_fill(vtime, cap_v); } });
 }
 
 // ---- multi-GPU: rank-ordered sum of the sharded evaluation through NVLink peer memory (isdf_peer.cuh) ------------------------------

@@ -37,7 +37,8 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_frontend_path", "isdf_frontend_path_batch", "isdf_frontend_path_batch_device", "isdf_frontend_path_field_device",
                "isdf_frontend_path_info", "isdf_path_waypoints", "isdf_midend_default_params", "isdf_midend_callback_batch",
                "isdf_midend_batch", "isdf_midend_batch_device", "isdf_certify_default_params", "isdf_trajectory_certify",
-               "isdf_trajectory_certify_device"]
+               "isdf_trajectory_certify_device", "isdf_swept_default_params", "isdf_swept_volume_sdf", "isdf_swept_volume_grid",
+               "isdf_swept_volume_grid_device", "isdf_swept_volume_mesh"]
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 
 
@@ -97,6 +98,56 @@ class CertifySummary(C.Structure):
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+class SweptParams(C.Structure):
+    """isdf_swept_params"""
+    _fields_ = [("samples_per_piece", C.c_int32), ("max_depth", C.c_int32), ("max_samples_per_point", C.c_int32), ("reserved_", C.c_int32),
+                ("tol", C.c_double), ("band", C.c_double)]
+
+
+class SweptGrid(C.Structure):
+    """isdf_swept_grid"""
+    _fields_ = [("bmin", C.c_double * 3), ("res", C.c_double), ("X", C.c_int32), ("Y", C.c_int32), ("Z", C.c_int32), ("reserved_", C.c_int32)]
+
+
+class SweptInfo(C.Structure):
+    """isdf_swept_info"""
+    _fields_ = [("nodes", C.c_int64), ("bricks", C.c_int64), ("bricks_culled", C.c_int64), ("sdf_evals", C.c_int64), ("undecided", C.c_int64),
+                ("deepest", C.c_int32), ("reserved_", C.c_int32), ("prep_ms", C.c_double), ("cull_ms", C.c_double), ("refine_ms", C.c_double),
+                ("mesh_ms", C.c_double)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved_"}
+
+
+def swept_grid_for(T, coeffs, r_body, band, res, samples_per_piece=64):
+    """an isdf_swept_grid covering the trajectory's bounding box inflated by r_body + band + res, node spacing res. The box is taken over
+    the piece polynomials at samples_per_piece + 1 times per piece, widened by the largest distance between consecutive samples, so the
+    whole path lies inside it."""
+    T = np.asarray(T, dtype=np.float64).reshape(-1)
+    N = T.size
+    c = np.asarray(coeffs, dtype=np.float64).reshape(3, 6 * N)
+    pts = []
+    for i in range(N):
+        t = np.linspace(0.0, T[i], samples_per_piece + 1)
+        pts.append((c[:, 6 * i:6 * i + 6] @ (t[None, :] ** np.arange(6)[:, None])).T)
+    P = np.concatenate(pts)
+    gap = float(np.max(np.linalg.norm(np.diff(P, axis=0), axis=1))) if len(P) > 1 else 0.0
+    pad = float(r_body) + float(band) + float(res) + gap
+    lo, hi = P.min(axis=0) - pad, P.max(axis=0) + pad
+    n = np.maximum(np.ceil((hi - lo) / res).astype(int) + 1, 2)
+    g = SweptGrid()
+    g.bmin[:] = [float(x) for x in lo]
+    g.res = float(res)
+    g.X, g.Y, g.Z = (int(x) for x in n)
+    return g
+
+
+def swept_grid_nodes(g):
+    """(X, Y, Z, 3) node coordinates of an isdf_swept_grid, computed as the library does: bmin[a] + (double) i * res"""
+    ax = [g.bmin[a] + np.arange(n, dtype=np.float64) * g.res for a, n in enumerate((g.X, g.Y, g.Z))]
+    return np.stack(np.meshgrid(*ax, indexing="ij"), axis=-1)
 
 
 # record of isdf_dbg_certify_leaves (not part of include/isdf.h)
@@ -202,6 +253,13 @@ def load_library(path=None):
     lib.isdf_certify_default_params.argtypes = [C.POINTER(CertifyParams)]
     lib.isdf_trajectory_certify.argtypes = [vp, C.c_int, dp, dp, C.POINTER(CertifyParams), C.POINTER(CertifySummary)]
     lib.isdf_trajectory_certify_device.argtypes = [vp, C.c_int, vp, vp, C.POINTER(CertifyParams), vp, vp]
+    spp, sgp, sip = C.POINTER(SweptParams), C.POINTER(SweptGrid), C.POINTER(SweptInfo)
+    lib.isdf_swept_default_params.argtypes = [spp]
+    lib.isdf_swept_volume_sdf.argtypes = [vp, C.c_int, dp, dp, spp, C.c_int, dp, dp, dp, dp, C.POINTER(C.c_uint8)]
+    lib.isdf_swept_volume_grid.argtypes = [vp, C.c_int, dp, dp, spp, sgp, dp, dp, dp, C.POINTER(C.c_uint8), sip]
+    lib.isdf_swept_volume_grid_device.argtypes = [vp, C.c_int, vp, vp, spp, sgp, vp, vp, vp, vp, sip, vp]
+    lib.isdf_swept_volume_mesh.argtypes = [vp, C.c_int, dp, dp, spp, sgp, C.c_int64, C.c_int64, dp, dp, ip, C.POINTER(C.c_int64),
+                                           C.POINTER(C.c_int64), sip]
     lib.isdf_set_map_cloud.argtypes = [vp, vp, C.c_int64, C.c_int32, C.c_double, C.c_int32]
     lib.isdf_set_map_cloud_device.argtypes = [vp, vp, C.c_int64, C.c_int32, C.c_double, C.c_int32, vp]
     lib.isdf_get_map_info.argtypes = [vp, C.POINTER(MapInfo)]
@@ -703,6 +761,74 @@ class Evaluator:
         if n.value:
             self._check(f(self.h, out.ctypes.data, n.value, C.byref(n)))
         return out
+
+    # ---- certified swept volume (see include/isdf.h) ----
+    def swept_params(self, K=None, band=None, tol=None, max_depth=None, max_samples=None):
+        """isdf_swept_default_params with K = this context's integral_intervs, band = 2 safety_hor, tol = occupancy_resolution / 100,
+        then the given overrides"""
+        p = SweptParams()
+        self._check(self.lib.isdf_swept_default_params(C.byref(p)))
+        p.samples_per_piece = int(self.cfg.integral_intervs if K is None else K)
+        p.band = float(2.0 * self.cfg.safety_hor if band is None else band)
+        p.tol = float(self.cfg.occupancy_resolution / 100.0 if tol is None else tol)
+        if max_depth is not None:
+            p.max_depth = int(max_depth)
+        if max_samples is not None:
+            p.max_samples_per_point = int(max_samples)
+        return p
+
+    @staticmethod
+    def _traj(T, coeffs):
+        T = _f64(T).reshape(-1)
+        Cc = _f64(coeffs).reshape(-1)
+        assert Cc.size == 18 * T.size
+        return T, Cc
+
+    def swept_volume_sdf(self, T, coeffs, pts, params=None):
+        """(value, lower, tstar, decided) at points (n, 3): the certified swept-volume SDF of the trajectory"""
+        T, Cc = self._traj(T, coeffs)
+        p = params if params is not None else self.swept_params()
+        P = _f64(pts).reshape(-1, 3)
+        n = P.shape[0]
+        v, lo, ts, dec = np.zeros(n), np.zeros(n), np.zeros(n), np.zeros(n, dtype=np.uint8)
+        self._check(self.lib.isdf_swept_volume_sdf(self.h, T.size, _dp(T), _dp(Cc), C.byref(p), n, _dp(P), _dp(v), _dp(lo), _dp(ts),
+                                                   dec.ctypes.data_as(C.POINTER(C.c_uint8))))
+        return v, lo, ts, dec
+
+    def swept_volume_grid(self, T, coeffs, grid, params=None):
+        """(value, lower, tstar, decided) as (X, Y, Z) arrays, and the info dict of the call"""
+        T, Cc = self._traj(T, coeffs)
+        p = params if params is not None else self.swept_params()
+        shp = (grid.X, grid.Y, grid.Z)
+        v, lo, ts, dec = np.zeros(shp), np.zeros(shp), np.zeros(shp), np.zeros(shp, dtype=np.uint8)
+        info = SweptInfo()
+        self._check(self.lib.isdf_swept_volume_grid(self.h, T.size, _dp(T), _dp(Cc), C.byref(p), C.byref(grid), _dp(v), _dp(lo), _dp(ts),
+                                                    dec.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(info)))
+        return v, lo, ts, dec, info.as_dict()
+
+    def swept_volume_grid_device(self, N, d_T, d_coeffs, grid, params, d_value, d_lower=0, d_tstar=0, d_decided=0, stream=0, info=True):
+        """raw device pointers (e.g. torch .data_ptr(); 0 = not wanted for lower / tstar / decided); returns the info dict (or None)"""
+        inf = SweptInfo() if info else None
+        self._check(self.lib.isdf_swept_volume_grid_device(self.h, N, C.c_void_p(d_T), C.c_void_p(d_coeffs), C.byref(params), C.byref(grid),
+                                                           C.c_void_p(d_value), C.c_void_p(d_lower or None), C.c_void_p(d_tstar or None),
+                                                           C.c_void_p(d_decided or None), C.byref(inf) if info else None, C.c_void_p(stream)))
+        return inf.as_dict() if info else None
+
+    def swept_volume_mesh(self, T, coeffs, grid, params=None):
+        """(V (nV, 3), vtime (nV), F (nF, 3) int32, info dict): the surface {SV = 0} of the grid's field by marching tetrahedra"""
+        T, Cc = self._traj(T, coeffs)
+        p = params if params is not None else self.swept_params()
+        nV, nF = C.c_int64(0), C.c_int64(0)
+        info = SweptInfo()
+        f = self.lib.isdf_swept_volume_mesh
+        r = f(self.h, T.size, _dp(T), _dp(Cc), C.byref(p), C.byref(grid), 0, 0, None, None, None, C.byref(nV), C.byref(nF), C.byref(info))
+        if r != 0 and not (r == -1 and (nV.value > 0 or nF.value > 0)):
+            self._check(r)
+        V, vt, F = np.zeros((max(nV.value, 1), 3)), np.zeros(max(nV.value, 1)), np.zeros((max(nF.value, 1), 3), dtype=np.int32)
+        if r != 0:
+            self._check(f(self.h, T.size, _dp(T), _dp(Cc), C.byref(p), C.byref(grid), nV.value, nF.value, _dp(V), _dp(vt),
+                          F.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(nV), C.byref(nF), C.byref(info)))
+        return V[:nV.value].copy(), vt[:nV.value].copy(), F[:nF.value].copy(), info.as_dict()
 
     # ---- front end: attitude kernels (see include/isdf.h) ----
     def frontend_build_kernels(self, max_roll=45.0, max_pitch=45.0, ang_res=9.0, front_end_safeh=0.0):

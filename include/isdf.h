@@ -460,6 +460,97 @@ int isdf_trajectory_certify(isdf_ctx *ctx, int N, const double *T, const double 
 int isdf_trajectory_certify_device(isdf_ctx *ctx, int N, const double *d_T, const double *d_coeffs, const isdf_certify_params *p,
                                    isdf_certify_summary *d_summary, void *cuda_stream);
 
+/* ---- certified swept volume: the region a trajectory sweeps, as a signed distance field with a proven enclosure, and its surface ----
+ * Replaces SweptVolumeManager::calculateSwept / sw_calculate::calculation (a local descent per cube corner from random seeds, so an upper
+ * bound that can miss a branch of the trajectory) and the standalone use of getSDFofSweptVolume (PlannerManager::geneWall).
+ * Definition. One trajectory of N pieces (T, coeffs in the layout of isdf_eval_discrete); no map is needed. Trajectory time runs over
+ *   [0, sum T]; piece start times are summed left to right. The pose at a time is the clearance check's (and the certificate's).
+ *   SV(p) = min over t of sd(R(t)^T (p - x(t))), sd = getonlySDF of the context's shape (negative inside).
+ * Supported shapes: those whose SDF is a signed Euclidean distance — Ball (radius >= 0), Point, Box whose rotation is orthonormal to
+ *   1e-12, exact-sign meshes (ISDF_MESH_SIGN_EXACT). There is no half_bd condition. Everything else is ISDF_ERR_UNSUPPORTED.
+ *   r_rot = the certificate's r (0 for Ball and Point); r_body = the body's bounding radius about its origin (the Ball's radius, the Box's
+ *   largest corner norm, the mesh's largest body-frame AABB corner norm, 0 for Point).
+ * Per point p, in level-synchronous rounds (the result depends on nothing but p):
+ *   1. Initial intervals: K per piece, exactly the certificate's (local time j T_i (1/K), the last one ending at T_i), with the
+ *      certificate's motion bounds D_a, D_b (r = r_rot, H = band): for these shapes sd_t(p) >= sd_e(p) - D_e on the interval.
+ *   2. Sphere cull: an interval with max_e(|p - x(t_e)| - r_body - D_e) >= band (rounded down) is dropped without an SDF evaluation.
+ *   3. sd at the endpoints of the kept intervals. hi = min(band, smallest value); t* = the earliest time attaining it, -1 if hi == band.
+ *      Each interval has lb = max(sd_a - D_a, sd_b - D_b).
+ *   4. Each round, with hi as it stood at the round's start: an interval with lb < hi - tol is split at ta + 0.5 (tb - ta) and the
+ *      midpoint is evaluated; the others become leaves. Splitting stops at max_depth or when the point's new samples would exceed
+ *      max_samples_per_point (earlier intervals get the samples first); intervals left then are undecided leaves.
+ *   5. lower = min(hi, min leaf lb). The point is decided iff lower >= hi - tol (which covers lower >= band).
+ *   Outputs: value = hi (an attained SDF value, capped at band), lower, t* (trajectory time), decided. lower <= SV(p) <= value up to the
+ *   certificate's rounding pad (DESIGN §3.12). Results are bit-identical run to run, through every entry point, and for a point queried
+ *   alone or as a grid node.
+ * Grid: nodes (not cell centres) at bmin + (i, j, k) res, each coordinate computed as bmin[a] + (double) i * res; address i*Y*Z + j*Z + k
+ *   as the map's. X, Y, Z >= 2 and X*Y*Z < 2^31.
+ * Mesh: marching tetrahedra on the node values, value < 0 = inside.
+ *   Cells are split into the 6 Kuhn tetrahedra {000, e_a, e_a + e_b, 111}, (a, b, c) the permutations of (x, y, z) in lexicographic
+ *   order; the split is the same in every cell, so faces match and no ambiguity table is needed.
+ *   Vertices lie on the 7 edge directions of a node (+x, +y, +z, +x+y, +x+z, +y+z, +x+y+z), one per crossed edge (exactly one endpoint
+ *   inside), numbered in (node address, direction) order and shared by every tetrahedron that uses the edge. Position per coordinate:
+ *   s = f0 / (f0 - f1), v = p0 + s (p1 - p0), each operation rounded to nearest (no contraction); vtime = t* of the endpoint with the
+ *   smaller |value|, the first endpoint on ties.
+ *   Triangles in (cell address, tetrahedron, local) order. Per tetrahedron (v0..v3 of the list above, E(x, y) = the vertex on edge x-y):
+ *     one vertex i on its own side: (i, j, k, l) = the even permutation of (0, 1, 2, 3) starting with i — (0,1,2,3), (1,0,3,2),
+ *       (2,3,0,1), (3,2,1,0) — and the triangle E(i,j), E(i,k), E(i,l) when i is inside, E(i,j), E(i,l), E(i,k) when it is outside;
+ *     two inside {i < j}, two outside {k < l}, k and l swapped when (i, j, k, l) is an odd permutation: E(i,l), E(j,l), E(j,k) and
+ *       E(i,l), E(j,k), E(i,k);
+ *     tetrahedra of odd permutations (a, b, c) — (x,z,y), (y,x,z), (z,y,x) — swap the last two vertices of each triangle.
+ *   Normals (counter-clockwise) point toward increasing value; the surface of a field whose inside stays clear of the grid border is
+ *   closed and consistently oriented.
+ * Errors: ISDF_ERR_INVALID for NULL pointers, N < 1, non-finite or non-positive T, non-finite coeffs or points, a parameter out of range
+ *   (K < 1, tol <= 0, band <= tol, max_depth outside [0, 64], max_samples_per_point < 0, non-zero reserved_), a bad grid, or a cap too
+ *   small (*nV / *nF still report the sizes needed); ISDF_ERR_STATE without a shape; ISDF_ERR_UNSUPPORTED for an unsupported shape and on
+ *   a sharded context. On failure every value / lower / tstar is NaN and decided 0 (the mesh call: V and vtime NaN up to the caps).
+ * State: the calls count their launches in isdf_stats.kernel_launches and touch no other field. They leave the swept-volume term's t* and
+ *   persisted durations, the discrete schedule, the clearance / certificate buffers, the mid-end buffers and the batch trajectories as
+ *   they were. Device buffers are owned by the context and grow on demand; a grid call holds one interval list of 64 * (max(N K, 2 M) +
+ *   2 M) bytes per resident warp (M = max_samples_per_point). */
+typedef struct isdf_swept_params {
+    int32_t samples_per_piece;       /* K >= 1: initial intervals per piece */
+    int32_t max_depth;               /* splits per initial interval, 0..64 */
+    int32_t max_samples_per_point;   /* new samples per point, >= 0 */
+    int32_t reserved_;               /* must be 0 */
+    double tol;                      /* > 0: a point is decided when lower >= value - tol */
+    double band;                     /* > tol: cap of every reported value */
+} isdf_swept_params;
+
+typedef struct isdf_swept_grid {
+    double bmin[3];                  /* the node (0, 0, 0) */
+    double res;                      /* > 0: node spacing */
+    int32_t X, Y, Z;                 /* >= 2 each, X*Y*Z < 2^31 */
+    int32_t reserved_;               /* must be 0 */
+} isdf_swept_grid;
+
+typedef struct isdf_swept_info {     /* the last grid or mesh call */
+    int64_t nodes, bricks, bricks_culled;   /* bricks of 4^3 nodes; culled: no interval reaches below band (no SDF evaluation) */
+    int64_t sdf_evals, undecided;           /* SDF evaluations over every node; nodes not decided */
+    int32_t deepest, reserved_;             /* deepest leaf level */
+    double prep_ms, cull_ms, refine_ms, mesh_ms;   /* device time per stage (CUDA events on the call's stream); mesh_ms 0 for a grid call */
+} isdf_swept_info;
+
+/* K = integral_intervs, band = 2 safety_hor, tol = occupancy_resolution / 100 of the default config, max_depth 16,
+ * max_samples_per_point 512 (DESIGN §3.12) */
+int isdf_swept_default_params(isdf_swept_params *p);
+/* n points (n x 3, host); value (n) required, lower / tstar / decided (n each) may be NULL */
+int isdf_swept_volume_sdf(isdf_ctx *ctx, int N, const double *T, const double *coeffs, const isdf_swept_params *p, int n,
+                          const double *pts, double *value, double *lower, double *tstar, uint8_t *decided);
+/* the field at every grid node (X*Y*Z each, host); value required, the rest and info may be NULL */
+int isdf_swept_volume_grid(isdf_ctx *ctx, int N, const double *T, const double *coeffs, const isdf_swept_params *p,
+                           const isdf_swept_grid *grid, double *value, double *lower, double *tstar, uint8_t *decided,
+                           isdf_swept_info *info);
+/* device-resident variant: d_T, d_coeffs and the outputs on ctx's device; runs on cuda_stream (NULL = default stream) and returns when
+ * the field is written (the trajectory is checked on the host and the brick lists are sized with one 8-byte read) */
+int isdf_swept_volume_grid_device(isdf_ctx *ctx, int N, const double *d_T, const double *d_coeffs, const isdf_swept_params *p,
+                                  const isdf_swept_grid *grid, double *d_value, double *d_lower, double *d_tstar, uint8_t *d_decided,
+                                  isdf_swept_info *info, void *cuda_stream);
+/* the surface {SV = 0} of the grid's field: V (cap_v x 3), vtime (cap_v), F (cap_f x 3, vertex indices), sizes in *nV / *nF */
+int isdf_swept_volume_mesh(isdf_ctx *ctx, int N, const double *T, const double *coeffs, const isdf_swept_params *p,
+                           const isdf_swept_grid *grid, int64_t cap_v, int64_t cap_f, double *V, double *vtime, int32_t *F,
+                           int64_t *nV, int64_t *nF, isdf_swept_info *info);
+
 /* ---- multi-GPU reduction through NVLink / NVSwitch peer memory (optional; ncclAllReduce over the same 19N+1 doubles is the
  * library alternative). One process per GPU. Sequence on every rank:
  *   isdf_set_shard(ctx, rank, world); isdf_peer_export(ctx, world, max_doubles, h) -> all-gather the 64-byte handles ->
