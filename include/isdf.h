@@ -491,7 +491,8 @@ int isdf_trajectory_certify_device(isdf_ctx *ctx, int N, const double *d_T, cons
  *   Vertices lie on the 7 edge directions of a node (+x, +y, +z, +x+y, +x+z, +y+z, +x+y+z), one per crossed edge (exactly one endpoint
  *   inside), numbered in (node address, direction) order and shared by every tetrahedron that uses the edge. Position per coordinate:
  *   s = f0 / (f0 - f1), v = p0 + s (p1 - p0), each operation rounded to nearest (no contraction); vtime = t* of the endpoint with the
- *   smaller |value|, the first endpoint on ties.
+ *   smaller |value|, the first endpoint on ties. That endpoint may be capped at band (t* = -1), so vtime is -1 where band is smaller
+ *   than the inside endpoint's |value| (possible when band < res).
  *   Triangles in (cell address, tetrahedron, local) order. Per tetrahedron (v0..v3 of the list above, E(x, y) = the vertex on edge x-y):
  *     one vertex i on its own side: (i, j, k, l) = the even permutation of (0, 1, 2, 3) starting with i — (0,1,2,3), (1,0,3,2),
  *       (2,3,0,1), (3,2,1,0) — and the triangle E(i,j), E(i,k), E(i,l) when i is inside, E(i,j), E(i,l), E(i,k) when it is outside;
