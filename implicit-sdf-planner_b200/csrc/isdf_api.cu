@@ -12,6 +12,7 @@
 #include "isdf_clearance.cuh"
 #include "isdf_certify.cuh"
 #include "isdf_sweptvol.cuh"
+#include "isdf_dynlimits.cuh"
 #include "isdf_map.cuh"
 #include <queue>
 #include "isdf_host_mesh.cuh"
@@ -169,6 +170,11 @@ struct isdf_ctx {
         PinnedBuf<int> h_tot;
         long long last_leaves = 0;   // leaves of the last call (isdf_dbg_certify_leaves)
     } cert;
+    struct {   // dynamic-limit certificate (isdf_dynlimits.cuh): samples, the two interval lists of the round loop, per-trajectory state
+        DevBuf<double> d_in, d_toff; DevBuf<DynSample> d_smp; DevBuf<CertInterval> d_iv[2]; DevBuf<int> d_dec, d_tot;
+        DevBuf<DynTraj> d_traj; DevBuf<DynSummary> d_sum;
+        PinnedBuf<int> h_tot;
+    } dyn;
     struct {   // certified swept volume (isdf_sweptvol.cuh): per-call poses and bounds, brick lists, per-warp interval lists, field and mesh
         DevBuf<double> d_in, d_toff, d_pose, d_Dab, d_pts, d_val, d_low, d_ts, d_V, d_vt;
         DevBuf<uint8_t> d_dec, d_mask; DevBuf<int32_t> d_F;
@@ -1874,6 +1880,127 @@ extern "C" int isdf_trajectory_certify(isdf_ctx *c, int N, const double *T, cons
         CU_TRY(cudaStreamSynchronize(c->stream));
         return 0;
     }, [&] { write_failed_summaries(summary, certify_batch(N, p), certify_failed_summary()); });
+}
+
+// ---- dynamic-limit certificate (isdf_dynlimits.cuh) -------------------------------------------------------------------------------
+extern "C" int isdf_dynamics_default_params(isdf_ctx *c, isdf_dynamics_params *p) {
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    isdf_config d;
+    isdf_default_config(&d);
+    const isdf_config &g = c ? c->cfg : d;
+    std::memset(p, 0, sizeof(*p));
+    const double inf = std::numeric_limits<double>::infinity();
+    p->samples_per_piece = g.integral_intervs; p->pieces_per_traj = 0;
+    p->max_depth = 16; p->max_samples_per_traj = 2048;
+    p->vmax = g.vmax; p->amax = inf; p->omgmax = g.omgmax; p->thetamax = g.thetamax; p->thrust_min = -inf; p->thrust_max = inf;
+    p->tol_v = 1e-3; p->tol_a = 1e-3; p->tol_omg = 1e-3; p->tol_theta = 1e-4; p->tol_thrust = 1e-3;
+    return 0;
+}
+
+static_assert(sizeof(isdf_dynamics_summary) == sizeof(DynSummary) && offsetof(isdf_dynamics_summary, thrust_lower) == offsetof(DynSummary, thrust_lower) &&
+              offsetof(isdf_dynamics_summary, verdict) == offsetof(DynSummary, verdict) && offsetof(isdf_dynamics_summary, depth) == offsetof(DynSummary, depth),
+              "isdf_dynamics_summary layout");
+
+static int dynamics_batch(int N, const isdf_dynamics_params *p) {
+    if (N < 1 || !p || p->pieces_per_traj < 0) return 0;
+    if (p->pieces_per_traj == 0) return 1;
+    return (N % p->pieces_per_traj == 0) ? N / p->pieces_per_traj : 0;
+}
+
+// every check that needs no device work, in the order of include/isdf.h's error list
+static int dynamics_check(isdf_ctx *c, int N, const isdf_dynamics_params *p) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    if (N < 1) return fail(ISDF_ERR_INVALID, "N < 1");
+    if (p->samples_per_piece < 1) return fail(ISDF_ERR_INVALID, "samples_per_piece < 1");
+    if (dynamics_batch(N, p) == 0) return fail(ISDF_ERR_INVALID, "pieces_per_traj must be 0 or divide N");
+    if (p->max_depth < 0 || p->max_depth > 64) return fail(ISDF_ERR_INVALID, "max_depth must lie in [0, 64]");
+    if (p->max_samples_per_traj < 0) return fail(ISDF_ERR_INVALID, "max_samples_per_traj < 0");
+    for (double t : {p->tol_v, p->tol_a, p->tol_omg, p->tol_theta, p->tol_thrust})
+        if (!(t >= 0.0)) return fail(ISDF_ERR_INVALID, "tolerances must be >= 0 (+inf: verdict only)");
+    for (double l : {p->vmax, p->amax, p->omgmax, p->thetamax, p->thrust_min, p->thrust_max})
+        if (std::isnan(l)) return fail(ISDF_ERR_INVALID, "a limit is NaN");
+    if (p->thrust_min > p->thrust_max) return fail(ISDF_ERR_INVALID, "thrust_min > thrust_max");
+    if (p->reserved_[0] || p->reserved_[1]) return fail(ISDF_ERR_INVALID, "reserved_ must be 0");
+    const long long B = dynamics_batch(N, p), K = p->samples_per_piece;
+    if ((long long)N * (2 * K + 1) + 3 * B * p->max_samples_per_traj > 0x7fffffffll)
+        return fail(ISDF_ERR_INVALID, "N (2 K + 1) + 3 B max_samples_per_traj must fit in 31 bits");
+    if (c->world > 1) return fail(ISDF_ERR_UNSUPPORTED, "the dynamic-limit certificate is not sharded: call it on a context with isdf_set_shard(ctx, 0, 1)");
+    return 0;
+}
+
+static int dynamics_run(isdf_ctx *c, int N, const double *d_T, const double *d_C, const isdf_dynamics_params *p, DynSummary *d_sum,
+                        cudaStream_t st) {
+    auto &z = c->dyn;
+    const int K = p->samples_per_piece, N0 = p->pieces_per_traj == 0 ? N : p->pieces_per_traj, B = N / N0, M = p->max_samples_per_traj;
+    const size_t S0 = (size_t)N * (K + 1), I0 = (size_t)N * K, Smax = S0 + (size_t)B * M;
+    CU_TRY(z.d_toff.ensure(N)); CU_TRY(z.d_smp.ensure(Smax)); CU_TRY(z.d_traj.ensure(B)); CU_TRY(z.d_tot.ensure(2)); CU_TRY(z.h_tot.ensure(1));
+    CU_TRY(z.d_iv[0].ensure(I0));
+    DynArgs A = {};
+    A.fp = c->dcfg.fp; A.mass = c->cfg.vehicle_mass; A.dv = c->cfg.vert_drag;
+    const double lim[DYN_CH] = {p->vmax, p->amax, p->omgmax, p->thetamax, p->thrust_max, -p->thrust_min};
+    const double tol[DYN_CH] = {p->tol_v, p->tol_a, p->tol_omg, p->tol_theta, p->tol_thrust, p->tol_thrust};
+    for (int q = 0; q < DYN_CH; q++) { A.lim[q] = lim[q]; A.tol[q] = tol[q]; }
+    A.N = N; A.K = K; A.N0 = N0; A.B = B; A.max_depth = p->max_depth; A.max_samples = M;
+    A.T = d_T; A.C = d_C; A.toff = z.d_toff.p; A.smp = z.d_smp.p; A.traj = z.d_traj.p; A.summary = d_sum; A.tot = z.d_tot.p;
+    A.cur = z.d_iv[0].p;
+    CU_TRY(dyn_init_launch(A, st));
+    c->stats.kernel_launches++;
+    long long nact = (long long)I0, S_cur = (long long)S0;
+    int cur = 0;
+    for (;;) {
+        CU_TRY(z.d_iv[cur ^ 1].ensure((size_t)std::max(2 * nact, 1ll))); CU_TRY(z.d_dec.ensure((size_t)nact));
+        A.cur = z.d_iv[cur].p; A.next = z.d_iv[cur ^ 1].p; A.dec = z.d_dec.p;
+        A.S_cur = (int)S_cur; A.nact = (int)nact;
+        CU_TRY(dyn_round_launch(A, st));
+        c->stats.kernel_launches += 2;
+        CU_TRY(cudaMemcpyAsync(z.h_tot.p, z.d_tot.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
+        const long long ns = *z.h_tot.p;
+        if (ns == 0) break;
+        S_cur += ns; nact = 2 * ns; cur ^= 1;
+    }
+    CU_TRY(dyn_finish_launch(A, st));
+    c->stats.kernel_launches++;
+    return 0;
+}
+
+// on failure every summary reads verdict 0 (UNDECIDED), every bound and time NaN, masks 0, counts -1
+static isdf_dynamics_summary dynamics_failed_summary() {
+    isdf_dynamics_summary s;
+    const double nan = std::numeric_limits<double>::quiet_NaN();
+    for (int q = 0; q < 5; q++) s.upper[q] = s.attained[q] = s.t_attained[q] = nan;
+    s.thrust_lower = s.thrust_attained_min = s.t_thrust_attained_min = nan;
+    s.verdict = 0; s.violated = s.undecided = 0; s.samples = s.undecided_intervals = s.depth = -1;
+    return s;
+}
+
+extern "C" int isdf_trajectory_dynamics_device(isdf_ctx *c, int N, const double *d_T, const double *d_coeffs, const isdf_dynamics_params *p,
+                                               isdf_dynamics_summary *d_summary, void *cuda_stream) {
+    const cudaStream_t st = (cudaStream_t)cuda_stream;
+    return poison_on_failure([&]() -> int {
+        if (int rc = dynamics_check(c, N, p)) return rc;
+        if (!d_T || !d_coeffs || !d_summary) return fail(ISDF_ERR_INVALID, "NULL device pointer");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        return dynamics_run(c, N, d_T, d_coeffs, p, (DynSummary *)d_summary, st);
+    }, [&] { if (c) write_failed_summaries(d_summary, dynamics_batch(N, p), dynamics_failed_summary(), c, st); });
+}
+
+extern "C" int isdf_trajectory_dynamics(isdf_ctx *c, int N, const double *T, const double *coeffs, const isdf_dynamics_params *p,
+                                        isdf_dynamics_summary *summary) {
+    return poison_on_failure([&]() -> int {
+        if (int rc = dynamics_check(c, N, p)) return rc;
+        if (!T || !coeffs || !summary) return fail(ISDF_ERR_INVALID, "NULL argument");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        const int B = dynamics_batch(N, p);
+        const double *d_T;
+        if (int rc = stage_traj(c, c->dyn.d_in, N, T, coeffs, &d_T)) return rc;
+        CU_TRY(c->dyn.d_sum.ensure((size_t)B));
+        if (int rc = isdf_trajectory_dynamics_device(c, N, d_T, c->dyn.d_in.p, p, (isdf_dynamics_summary *)c->dyn.d_sum.p, c->stream)) return rc;
+        CU_TRY(cudaMemcpyAsync(summary, c->dyn.d_sum.p, sizeof(isdf_dynamics_summary) * B, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaStreamSynchronize(c->stream));
+        return 0;
+    }, [&] { write_failed_summaries(summary, dynamics_batch(N, p), dynamics_failed_summary()); });
 }
 
 // ---- certified swept volume (isdf_sweptvol.cuh) ------------------------------------------------------------------------------------

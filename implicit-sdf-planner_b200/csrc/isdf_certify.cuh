@@ -25,6 +25,7 @@
 #pragma once
 #include "isdf_types.cuh"
 #include "isdf_clearance.cuh"
+#include "isdf_interval.cuh"
 
 namespace isdf {
 
@@ -69,33 +70,6 @@ struct CertArgs {
     int *tot;                      // {splits of the round, ticket}
 };
 
-// ---- outward-rounded interval arithmetic -----------------------------------------------------------------------------------------
-struct ivl { double lo, hi; };
-__device__ __forceinline__ ivl iv(double x) { ivl r; r.lo = x; r.hi = x; return r; }
-__device__ __forceinline__ ivl iadd(ivl a, ivl b) { ivl r; r.lo = __dadd_rd(a.lo, b.lo); r.hi = __dadd_ru(a.hi, b.hi); return r; }
-__device__ __forceinline__ ivl isub(ivl a, ivl b) { ivl r; r.lo = __dadd_rd(a.lo, -b.hi); r.hi = __dadd_ru(a.hi, -b.lo); return r; }
-__device__ __forceinline__ ivl ineg(ivl a) { ivl r; r.lo = -a.hi; r.hi = -a.lo; return r; }
-__device__ __forceinline__ ivl imul(ivl a, ivl b) {
-    ivl r;
-    r.lo = fmin(fmin(__dmul_rd(a.lo, b.lo), __dmul_rd(a.lo, b.hi)), fmin(__dmul_rd(a.hi, b.lo), __dmul_rd(a.hi, b.hi)));
-    r.hi = fmax(fmax(__dmul_ru(a.lo, b.lo), __dmul_ru(a.lo, b.hi)), fmax(__dmul_ru(a.hi, b.lo), __dmul_ru(a.hi, b.hi)));
-    return r;
-}
-__device__ __forceinline__ ivl isqr(ivl a) {
-    const double m = fmax(fabs(a.lo), fabs(a.hi)), n = (a.lo > 0.0) ? a.lo : (a.hi < 0.0 ? -a.hi : 0.0);
-    ivl r; r.lo = __dmul_rd(n, n); r.hi = __dmul_ru(m, m); return r;
-}
-// a / b for b.lo > 0
-__device__ __forceinline__ ivl idivp(ivl a, ivl b) {
-    ivl r;
-    r.lo = a.lo >= 0.0 ? __ddiv_rd(a.lo, b.hi) : __ddiv_rd(a.lo, b.lo);
-    r.hi = a.hi >= 0.0 ? __ddiv_ru(a.hi, b.lo) : __ddiv_ru(a.hi, b.hi);
-    return r;
-}
-__device__ __forceinline__ ivl isqrt(ivl a) { ivl r; r.lo = __dsqrt_rd(fmax(a.lo, 0.0)); r.hi = __dsqrt_ru(a.hi); return r; }
-__device__ __forceinline__ double imag(ivl a) { return fmax(fabs(a.lo), fabs(a.hi)); }
-__device__ __forceinline__ ivl iwiden(ivl a, double rad) { ivl r; r.lo = __dadd_rd(a.lo, -rad); r.hi = __dadd_ru(a.hi, rad); return r; }
-
 // enclosure of the zero-yaw attitude R(z(v, a)) over boxes v, a (rows of R, 9 entries); false when |zu| or 1 + z_z may vanish.
 // kappa (upper bound of (|a| + dh kap |v| + g) / |zu|) and delta (lower bound of 1 + z_z) feed the pose pad.
 __device__ __forceinline__ bool cert_rot(const FlatParams &fp, const ivl v[3], const ivl a[3], ivl R[9], double &kappa, double &delta) {
@@ -133,7 +107,6 @@ __device__ __forceinline__ double cert_bound(const FlatParams &fp, double r, dou
     tp[0] = iv(1.0);
 #pragma unroll
     for (int k = 1; k < 6; k++) tp[k] = imul(tp[k - 1], iv(te));
-    const double binom[6][6] = {{1, 0, 0, 0, 0, 0}, {1, 1, 0, 0, 0, 0}, {1, 2, 1, 0, 0, 0}, {1, 3, 3, 1, 0, 0}, {1, 4, 6, 4, 1, 0}, {1, 5, 10, 10, 5, 1}};
     double P2 = 0.0, A = 0.0;
     ivl ve[3], vi[3], ae[3], ai[3];
 #pragma unroll
@@ -145,9 +118,7 @@ __device__ __forceinline__ double cert_bound(const FlatParams &fp, double r, dou
         ivl d1 = iv(0.0), d2 = iv(0.0);
 #pragma unroll
         for (int k = 1; k < 6; k++) {
-            ivl d = iv(0.0);
-#pragma unroll
-            for (int q = k; q < 6; q++) d = iadd(d, imul(imul(iv(binom[q][k]), iv(c[q])), tp[q - k]));
+            const ivl d = taylor_coeff(c, tp, k);
             m[k] = imag(d);
             if (k == 1) d1 = d;
             if (k == 2) d2 = d;

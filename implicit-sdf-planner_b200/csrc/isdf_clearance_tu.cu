@@ -1,6 +1,6 @@
 // Translation unit of the trajectory clearance kernels (isdf_clearance.cuh): k_clearance_scan<0|1|2>, k_clearance_summary, of the
-// continuous certificate built on them (isdf_certify.cuh) and of the certified swept volume that shares the certificate's pose and
-// motion bound (isdf_sweptvol.cuh).
+// continuous certificate built on them (isdf_certify.cuh), of the certified swept volume that shares the certificate's pose and
+// motion bound (isdf_sweptvol.cuh) and of the dynamic-limit certificate that shares its rounds (isdf_dynlimits.cuh).
 // Compiled WITH FMA contraction and the division-free closest-point test, like the discrete path; a third unit of its own so that the
 // objects of the other two stay exactly what they are.
 #define ISDF_CLEARANCE_TU 1
@@ -10,6 +10,7 @@
 #include "isdf_clearance.cuh"
 #include "isdf_certify.cuh"
 #include "isdf_sweptvol.cuh"
+#include "isdf_dynlimits.cuh"
 
 namespace isdf {
 
@@ -48,6 +49,25 @@ cudaError_t certify_finish_launch(const CertArgs &A, cudaStream_t st) {
 
 cudaError_t certify_bound_launch(const CertArgs &A, int n, const int *piece, const double *ta, const double *tb, double *out, cudaStream_t st) {
     k_certify_bound<<<(n + 127) / 128, 128, 0, st>>>(A, n, piece, ta, tb, out);
+    return cudaGetLastError();
+}
+
+cudaError_t dyn_init_launch(const DynArgs &A, cudaStream_t st) {
+    const int n = max(A.N * (A.K + 1), A.B);
+    k_dyn_init<<<(n + DYN_THREADS - 1) / DYN_THREADS, DYN_THREADS, 0, st>>>(A);
+    return cudaGetLastError();
+}
+
+cudaError_t dyn_round_launch(const DynArgs &A, cudaStream_t st) {
+    k_dyn_decide<<<A.B, DYN_THREADS, 0, st>>>(A);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess || A.nact == 0) return e;
+    k_dyn_emit<<<(A.nact + DYN_THREADS - 1) / DYN_THREADS, DYN_THREADS, 0, st>>>(A);
+    return cudaGetLastError();
+}
+
+cudaError_t dyn_finish_launch(const DynArgs &A, cudaStream_t st) {
+    k_dyn_finish<<<(A.B + DYN_THREADS - 1) / DYN_THREADS, DYN_THREADS, 0, st>>>(A);
     return cudaGetLastError();
 }
 

@@ -38,8 +38,11 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_frontend_path_info", "isdf_path_waypoints", "isdf_midend_default_params", "isdf_midend_callback_batch",
                "isdf_midend_batch", "isdf_midend_batch_device", "isdf_certify_default_params", "isdf_trajectory_certify",
                "isdf_trajectory_certify_device", "isdf_swept_default_params", "isdf_swept_volume_sdf", "isdf_swept_volume_grid",
-               "isdf_swept_volume_grid_device", "isdf_swept_volume_mesh"]
+               "isdf_swept_volume_grid_device", "isdf_swept_volume_mesh", "isdf_dynamics_default_params", "isdf_trajectory_dynamics",
+               "isdf_trajectory_dynamics_device"]
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
+FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
+DYN_QUANTITIES = ["speed", "acceleration", "body_rate", "tilt", "thrust"]   # q of isdf_dynamics_summary; mask bit 5: the thrust minimum
 
 
 class KernelConfig(C.Structure):
@@ -98,6 +101,23 @@ class CertifySummary(C.Structure):
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+class DynamicsParams(C.Structure):
+    """isdf_dynamics_params"""
+    _fields_ = [(n, C.c_int32) for n in ["samples_per_piece", "pieces_per_traj", "max_depth", "max_samples_per_traj"]] + \
+               [(n, C.c_double) for n in ["vmax", "amax", "omgmax", "thetamax", "thrust_min", "thrust_max",
+                                          "tol_v", "tol_a", "tol_omg", "tol_theta", "tol_thrust"]] + [("reserved_", C.c_int32 * 2)]
+
+
+class DynamicsSummary(C.Structure):
+    """isdf_dynamics_summary (one per trajectory)"""
+    _fields_ = [("upper", C.c_double * 5), ("attained", C.c_double * 5), ("t_attained", C.c_double * 5), ("thrust_lower", C.c_double),
+                ("thrust_attained_min", C.c_double), ("t_thrust_attained_min", C.c_double)] + \
+               [(n, C.c_int32) for n in ["verdict", "violated", "undecided", "samples", "undecided_intervals", "depth"]]
+
+    def as_dict(self):
+        return {n: (np.array(getattr(self, n)[:]) if n in ("upper", "attained", "t_attained") else getattr(self, n)) for n, _ in self._fields_}
 
 
 class SweptParams(C.Structure):
@@ -254,6 +274,9 @@ def load_library(path=None):
     lib.isdf_trajectory_certify.argtypes = [vp, C.c_int, dp, dp, C.POINTER(CertifyParams), C.POINTER(CertifySummary)]
     lib.isdf_trajectory_certify_device.argtypes = [vp, C.c_int, vp, vp, C.POINTER(CertifyParams), vp, vp]
     spp, sgp, sip = C.POINTER(SweptParams), C.POINTER(SweptGrid), C.POINTER(SweptInfo)
+    lib.isdf_dynamics_default_params.argtypes = [vp, C.POINTER(DynamicsParams)]
+    lib.isdf_trajectory_dynamics.argtypes = [vp, C.c_int, dp, dp, C.POINTER(DynamicsParams), C.POINTER(DynamicsSummary)]
+    lib.isdf_trajectory_dynamics_device.argtypes = [vp, C.c_int, vp, vp, C.POINTER(DynamicsParams), vp, vp]
     lib.isdf_swept_default_params.argtypes = [spp]
     lib.isdf_swept_volume_sdf.argtypes = [vp, C.c_int, dp, dp, spp, C.c_int, dp, dp, dp, dp, C.POINTER(C.c_uint8)]
     lib.isdf_swept_volume_grid.argtypes = [vp, C.c_int, dp, dp, spp, sgp, dp, dp, dp, C.POINTER(C.c_uint8), sip]
@@ -761,6 +784,45 @@ class Evaluator:
         if n.value:
             self._check(f(self.h, out.ctypes.data, n.value, C.byref(n)))
         return out
+
+    # ---- dynamic-limit certificate (see include/isdf.h) ----
+    def dynamics_params(self, K=None, N0=0, max_depth=None, max_samples=None, **kw):
+        """isdf_dynamics_default_params for this context, then the overrides: K, N0, max_depth, max_samples and any field of
+        isdf_dynamics_params by name (vmax, amax, omgmax, thetamax, thrust_min, thrust_max, tol_v, tol_a, tol_omg, tol_theta, tol_thrust)"""
+        p = DynamicsParams()
+        self._check(self.lib.isdf_dynamics_default_params(self.h, C.byref(p)))
+        if K is not None:
+            p.samples_per_piece = int(K)
+        p.pieces_per_traj = int(N0)
+        if max_depth is not None:
+            p.max_depth = int(max_depth)
+        if max_samples is not None:
+            p.max_samples_per_traj = int(max_samples)
+        for k, v in kw.items():
+            if k not in {n for n, _ in DynamicsParams._fields_} or k == "reserved_":
+                raise TypeError(f"unknown isdf_dynamics_params field {k}")
+            setattr(p, k, v)
+        return p
+
+    def trajectory_dynamics(self, T, coeffs, params=None, **kw):
+        """one summary dict per trajectory (pieces b*N0 .. b*N0+N0-1; N0 = 0: a single trajectory): verdict (FEASIBLE 1, VIOLATING -1,
+        UNDECIDED 0), upper / attained / t_attained (arrays over DYN_QUANTITIES), thrust_lower, thrust_attained_min, t_thrust_attained_min,
+        violated, undecided, samples, undecided_intervals, depth. params: an isdf_dynamics_params, or None for dynamics_params(**kw)"""
+        T = _f64(T).reshape(-1)
+        N = T.size
+        Cc = _f64(coeffs).reshape(-1)
+        assert Cc.size == 18 * N
+        p = params if params is not None else self.dynamics_params(**kw)
+        N0 = p.pieces_per_traj
+        B = 1 if N0 <= 0 else max(N // N0, 1)
+        summ = (DynamicsSummary * B)()
+        self._check(self.lib.isdf_trajectory_dynamics(self.h, N, _dp(T), _dp(Cc), C.byref(p), summ))
+        return [s.as_dict() for s in summ]
+
+    def trajectory_dynamics_device(self, N, d_T, d_coeffs, params, d_summary, stream=0):
+        """raw device pointers (e.g. torch .data_ptr()); d_summary holds N/N0 isdf_dynamics_summary records (168 bytes each)"""
+        self._check(self.lib.isdf_trajectory_dynamics_device(self.h, N, C.c_void_p(d_T), C.c_void_p(d_coeffs), C.byref(params),
+                                                             C.c_void_p(d_summary), C.c_void_p(stream)))
 
     # ---- certified swept volume (see include/isdf.h) ----
     def swept_params(self, K=None, band=None, tol=None, max_depth=None, max_samples=None):

@@ -460,6 +460,84 @@ int isdf_trajectory_certify(isdf_ctx *ctx, int N, const double *T, const double 
 int isdf_trajectory_certify_device(isdf_ctx *ctx, int N, const double *d_T, const double *d_coeffs, const isdf_certify_params *p,
                                    isdf_certify_summary *d_summary, void *cuda_stream);
 
+/* ---- dynamic-limit certificate: can the vehicle fly a trajectory at EVERY time, not only at the penalty's samples? -----------------
+ * The back end's dynamics term (addTimeIntPenaltyParallel, hpp:505-534) is a weighted penalty at the K + 1 samples of each piece; an
+ * optimised trajectory can exceed vmax at a sample and anywhere between two. This call proves bounds over every time instead.
+ * Definition. N pieces (T, coeffs in the layout of isdf_eval_discrete), pieces b*N0 .. b*N0+N0-1 form trajectory b (N0 = 0: one trajectory
+ *   of all N pieces). The coefficients and durations are taken as exact; local time t runs over [0, T_i]; the flatness parameters are the
+ *   context's (vehicle_mass, grav_acc, horiz_drag, vert_drag, paras_drag, speed_eps); yaw is zero, as in the back end. Quantities at t:
+ *     q = 0  speed         |v(t)|
+ *     q = 1  acceleration  |a(t)|
+ *     q = 2  body rate     |omega(t)|, omega of FlatnessMap::optimizated_forward(v, a, j, quat, omg) (flatness.hpp:88-148)
+ *     q = 3  tilt          theta(t) = acos(z_z), z = zu / |zu|, zu = a + dh/m (1 + cp sqrt(|v|^2 + veps)) v + g e_z (equal in exact
+ *                          arithmetic to the back end's acos(1 - 2 (q1^2 + q2^2)), hpp:505)
+ *     q = 4  thrust        f(t) = z . (mass a + dv w + mass g e_z), w = (1 + cp sqrt(|v|^2 + veps)) v, dv = vert_drag: FlatnessMap::forward
+ *                          at psi = dpsi = 0 (flatness.hpp:150-207)
+ *   Limits: vmax, amax, omgmax, thetamax bound q = 0..3 from above, thrust_min / thrust_max bound the thrust from both sides. +inf
+ *   (-inf for thrust_min) means the quantity is reported and not checked.
+ * Verdict per trajectory:
+ *   FEASIBLE (1)   every checked limit holds with a proof: upper <= limit, thrust_lower >= thrust_min;
+ *   VIOLATING (-1) an evaluated sample proves a limit broken (attained > limit, thrust_attained_min < thrust_min), or a sample is not finite;
+ *   UNDECIDED (0)  neither was established within the refinement budget.
+ * Mechanism.
+ *   The initial samples are the clearance check's K + 1 per piece at local times j (T_i (1/K)) (with K = integral_intervs, exactly where
+ *   the back-end penalty looks), and piece i has K intervals, the last ending at T_i; intervals never cross a junction.
+ *   Interval enclosure: the piece polynomial re-expanded about the midpoint te with Taylor coefficients d_k as intervals;
+ *   v in d_1 + [-1, 1] sum_{k>=2} k |d_k| h^(k-1), a and j likewise, h = sup |t - te|; every quantity is then evaluated in outward-rounded
+ *   interval arithmetic (norms, the flatness map, omega, z_z, the thrust); acos is padded outward by 8 ulp (CUDA documents 2). A division
+ *   by an enclosure that reaches 0 (|zu|, 1 + z_z, or sqrt(|v|^2 + veps) when speed_eps = 0 and paras_drag != 0) gives body rate
+ *   [0, +inf], tilt [0, pi] and thrust [-|F|, |F|] with F = mass a + dv w + mass g e_z: such an interval must be refined.
+ *   Sample: the same evaluation at h = 0 encloses the exact value at that time; its lower end is proven attained (for the thrust minimum,
+ *   its upper end).
+ *   Split rule: an interval is split at ta + 0.5 (tb - ta), with a new sample there, when for some quantity its upper end hi exceeds the
+ *   limit while the trajectory's attained value does not (the limit is locally undecided), or hi > attained + tol (the reported maximum
+ *   is not yet tight); the thrust minimum mirrors this at the lower end. tol = +inf gives pure verdict mode. A trajectory with a
+ *   non-finite sample splits no further. Splitting stops at max_depth or when the trajectory's new samples would exceed
+ *   max_samples_per_traj (intervals earlier in time get the samples first); a leaf whose hi exceeds a checked limit is undecided.
+ * Summary per trajectory: upper[q] = the maximum of hi over the final leaves, a proven upper bound of sup_t q(t); attained[q] and
+ *   t_attained[q] the largest value proven attained at an evaluated sample and its trajectory time (ties: earliest time); thrust_lower,
+ *   thrust_attained_min, t_thrust_attained_min the mirror for the thrust minimum; violated / undecided: bit q (q = 0..4, bit 4 the thrust
+ *   maximum) and bit 5 (the thrust minimum) of the limits proven broken / neither proven broken nor proven held; samples (N0 (K + 1) plus
+ *   the new ones), undecided_intervals, depth (deepest leaf level). With a non-finite sample the bounds are NaN.
+ * Results are deterministic run to run, identical through both entry points, and a trajectory's result is bit-identical alone or inside
+ * a batch (every fold is a maximum with ties to the earliest time; per-trajectory budgets; order-preserving compaction).
+ * Device work per round: one interval pass (two kernels) and one 4-byte read; at most max_depth + 1 rounds; no map or shape is needed.
+ * Errors: ISDF_ERR_INVALID for K < 1, N < 1, N0 < 0 or not dividing N, max_depth outside [0, 64], max_samples_per_traj < 0, a tolerance
+ *   that is NaN or negative, a NaN limit, thrust_min > thrust_max, a non-zero reserved_, sizes beyond 31-bit indexing, NULL pointers;
+ *   ISDF_ERR_UNSUPPORTED on a sharded context. On failure every summary has verdict 0, its bounds NaN and its counts -1.
+ * The call counts its launches in isdf_stats.kernel_launches and touches no other field; it leaves the discrete schedule, the clearance
+ * and certificate buffers, the swept-volume state, the mid-end buffers and the batch trajectories as they were. */
+typedef struct isdf_dynamics_params {
+    int32_t samples_per_piece;     /* K >= 1 */
+    int32_t pieces_per_traj;       /* N0; 0 = one trajectory of N pieces; else N % N0 == 0 */
+    int32_t max_depth;             /* splits per initial interval, 0..64 */
+    int32_t max_samples_per_traj;  /* new samples per trajectory, >= 0 */
+    double vmax, amax, omgmax, thetamax, thrust_min, thrust_max;   /* +inf (thrust_min -inf): report only */
+    double tol_v, tol_a, tol_omg, tol_theta, tol_thrust;           /* >= 0; +inf: verdict only */
+    int32_t reserved_[2];          /* must be 0 */
+} isdf_dynamics_params;
+
+typedef struct isdf_dynamics_summary {
+    double upper[5], attained[5], t_attained[5];                   /* q = speed, acceleration, body rate, tilt, thrust */
+    double thrust_lower, thrust_attained_min, t_thrust_attained_min;
+    int32_t verdict;                                               /* 1 FEASIBLE, -1 VIOLATING, 0 UNDECIDED */
+    int32_t violated, undecided;                                   /* bit masks: q = 0..4, bit 5 the thrust minimum */
+    int32_t samples, undecided_intervals, depth;
+} isdf_dynamics_summary;
+
+/* K = integral_intervs, N0 = 0, vmax / omgmax / thetamax of the context's config (of isdf_default_config for ctx NULL; thetamax 100 rad,
+ * the reference's config, never binds),
+ * every other limit report-only; tolerances 1e-3 m/s, 1e-3 m/s^2, 1e-3 rad/s, 1e-4 rad, 1e-3 N; max_depth 16, max_samples_per_traj 2048.
+ * The tolerances and budgets are starting points, not tuned (DESIGN §3.13). */
+int isdf_dynamics_default_params(isdf_ctx *ctx, isdf_dynamics_params *p);
+/* host buffers; summary: N/N0 entries (1 for N0 = 0) */
+int isdf_trajectory_dynamics(isdf_ctx *ctx, int N, const double *T, const double *coeffs, const isdf_dynamics_params *p,
+                             isdf_dynamics_summary *summary);
+/* device-resident variant: d_T, d_coeffs, d_summary on ctx's device; runs on cuda_stream (NULL = default stream) and returns when the
+ * summaries are written (the round loop reads 4 bytes per round) */
+int isdf_trajectory_dynamics_device(isdf_ctx *ctx, int N, const double *d_T, const double *d_coeffs, const isdf_dynamics_params *p,
+                                    isdf_dynamics_summary *d_summary, void *cuda_stream);
+
 /* ---- certified swept volume: the region a trajectory sweeps, as a signed distance field with a proven enclosure, and its surface ----
  * Replaces SweptVolumeManager::calculateSwept / sw_calculate::calculation (a local descent per cube corner from random seeds, so an upper
  * bound that can miss a branch of the trajectory) and the standalone use of getSDFofSweptVolume (PlannerManager::geneWall).
