@@ -91,6 +91,8 @@ struct RefineBufs {
     }
 };
 
+struct GatherBox;   // the index boxes of one waypoint of the obstacle gather (defined with the gather kernels)
+
 // One plain struct per subsystem; each keeps the flag that says its state is valid next to the buffers that state lives in. Every
 // buffer owns its memory; ~isdf_ctx releases the rest.
 struct isdf_ctx {
@@ -195,6 +197,15 @@ struct isdf_ctx {
         int refine_blocks = 0;   // resident CTAs per SM of the refinement kernel (0: not queried yet)
         cudaEvent_t ev[5] = {};
     } svol;
+    struct {   // batched obstacle gather: staged waypoints and offsets, per-row boxes, counts and offsets, the lists
+        DevBuf<GatherBox> d_box; DevBuf<int> d_wpoff, d_cnt, d_ptoff; DevBuf<long long> d_offs, d_total; DevBuf<double> d_wp, d_out;
+    } gat;
+    struct {   // planning step (isdf_plan_batch): one group's staging, mid-end and back-end results, and its returned trajectories
+        DevBuf<double> d_bc, d_wp, d_mx, d_mres, d_bbc, d_bx, d_bf, d_gT, d_gC; DevBuf<int> d_mi, d_bi;
+        DevBuf<CertSummary> d_csum; DevBuf<DynSummary> d_dsum;
+        cudaEvent_t ev[2] = {};
+        isdf_plan_info info = {};
+    } plan;
     struct {   // peer-memory reduction (isdf_peer.cuh)
         DevBuf<char> buf;                    // own exchange buffer (exported through CUDA IPC)
         void *open[PEER_MAX] = {};           // peers' buffers opened here (null for self / unused)
@@ -211,6 +222,7 @@ struct isdf_ctx {
         for (cudaEvent_t e : {ev0, ev1, ev_main_done, ev_items_done}) if (e) cudaEventDestroy(e);
         for (cudaEvent_t e : fp.ev) if (e) cudaEventDestroy(e);
         for (cudaEvent_t e : svol.ev) if (e) cudaEventDestroy(e);
+        for (cudaEvent_t e : plan.ev) if (e) cudaEventDestroy(e);
         if (aux_stream) cudaStreamDestroy(aux_stream);
         if (stream) cudaStreamDestroy(stream);
     }
@@ -965,6 +977,207 @@ extern "C" int isdf_gather_obstacle_points(isdf_ctx *c, const double *waypoints,
         }
     }
     return rc;
+}
+
+// ---- every plan's obstacle list in one call (isdf_gather_obstacle_points_batch) -----------------------------------------------------
+// B plans, plan b owning the waypoint rows [wp_off[b], wp_off[b+1]). Four launches over all plans: k_gather_boxes_batch (the index boxes of
+// every row, the 999 sentinel at each plan's first row), k_gather_points_batch<false> (grid (waypoint, plan): how many voxels each row
+// emits), k_gather_scan (the exclusive scan of the row counts) and k_gather_points_batch<true> (the ordered compaction at each row's
+// offset). The rows of all plans are scanned in one pass: plans lie back to back, so a row's offset is its plan's offset plus the counts of
+// the plan's earlier rows, and a plan's offset is the offset of its first row. The centres are computed as k_gather_points computes them,
+// in this -fmad=false unit.
+constexpr int GATHER_LIST_CAP = 1024;   // earlier boxes of a plan kept per CTA; with more, every earlier box of the plan is tested
+
+// the plan b with wp_off[b] <= q < wp_off[b+1] (empty plans skipped): the smallest b with wp_off[b+1] > q
+__device__ __forceinline__ int gather_plan_of(const int *wp_off, int B, int q) {
+    int lo = 0, hi = B - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (wp_off[mid + 1] > q) hi = mid; else lo = mid + 1;
+    }
+    return lo;
+}
+
+__global__ void k_gather_boxes_batch(const DevGrid G, const int *wp_off, int B, const double *wps, int R, double h, double ox, double oy, double oz,
+                                     GatherBox *boxes) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= R) return;
+    const bool first = wp_off[gather_plan_of(wp_off, B, q)] == q;
+    GatherBox b;
+    const double c[3] = {wps[3 * q] + ox, wps[3 * q + 1] + oy, wps[3 * q + 2] + oz};
+    const double l[3] = {first ? 999.0 : wps[3 * (q - 1)], first ? 999.0 : wps[3 * (q - 1) + 1], first ? 999.0 : wps[3 * (q - 1) + 2]};
+    const int dims[3] = {G.X, G.Y, G.Z};
+    for (int a = 0; a < 3; a++) {
+        b.a0[a] = grid_axis_index(c[a] - h, G.bmin[a], G.bmax[a], G.res, dims[a]); b.a1[a] = grid_axis_index(c[a] + h, G.bmin[a], G.bmax[a], G.res, dims[a]);
+        b.l0[a] = grid_axis_index(l[a] - h, G.bmin[a], G.bmax[a], G.res, dims[a]); b.l1[a] = grid_axis_index(l[a] + h, G.bmin[a], G.bmax[a], G.res, dims[a]);
+    }
+    boxes[q] = b;
+}
+
+// CTA (j, b): row wp_off[b] + j. An earlier box of the plan can claim a voxel of this box only if their include boxes (a0..a1) intersect;
+// those are listed once per CTA and the voxel loop tests only them. Count pass: counts[row]; write pass: the voxels at offs[row] (< cap).
+template <bool WRITE>
+__global__ void __launch_bounds__(256) k_gather_points_batch(const DevGrid G, const int *wp_off, const GatherBox *boxes, int *counts,
+                                                            const long long *offs, double *out, long long cap) {
+    __shared__ int warp_cnt[8];
+    __shared__ int nlist;
+    __shared__ long long running;
+    __shared__ int list[GATHER_LIST_CAP];
+    const int q0 = wp_off[blockIdx.y], j = blockIdx.x;
+    if (j >= wp_off[blockIdx.y + 1] - q0) return;   // the plan has fewer rows (uniform over the CTA)
+    const int q = q0 + j;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const GatherBox b = boxes[q];
+    if (threadIdx.x == 0) { running = WRITE ? offs[q] : 0; nlist = 0; }
+    __syncthreads();
+    for (int base = 0; base < j; base += blockDim.x) {
+        const int p = base + threadIdx.x;
+        bool hit = false;
+        if (p < j) {
+            const GatherBox &o = boxes[q0 + p];
+            hit = o.a0[0] <= b.a1[0] && o.a1[0] >= b.a0[0] && o.a0[1] <= b.a1[1] && o.a1[1] >= b.a0[1] && o.a0[2] <= b.a1[2] && o.a1[2] >= b.a0[2];
+        }
+        const unsigned bal = __ballot_sync(0xffffffffu, hit);
+        if (lane == 0) warp_cnt[warp] = __popc(bal);
+        __syncthreads();
+        int off = nlist;
+        for (int w = 0; w < warp; w++) off += warp_cnt[w];
+        if (hit) {
+            const int pos = off + __popc(bal & ((1u << lane) - 1u));
+            if (pos < GATHER_LIST_CAP) list[pos] = q0 + p;
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) { int t = 0; for (int w = 0; w < 8; w++) t += warp_cnt[w]; nlist += t; }
+        __syncthreads();
+    }
+    const int nl = nlist;
+    const int ny = b.a1[1] - b.a0[1] + 1, nz = b.a1[2] - b.a0[2] + 1;
+    const int nvox = (b.a1[0] - b.a0[0] + 1) * ny * nz;
+    for (int base = 0; base < nvox; base += blockDim.x) {
+        const int v = base + threadIdx.x;
+        bool emit = false; int i = 0, jj = 0, k = 0;
+        if (v < nvox) {
+            i = b.a0[0] + v / (ny * nz); jj = b.a0[1] + (v / nz) % ny; k = b.a0[2] + v % nz;
+            emit = gather_includes(G, b, i, jj, k);
+            if (nl <= GATHER_LIST_CAP) { for (int t = 0; emit && t < nl; t++) if (gather_includes(G, boxes[list[t]], i, jj, k)) emit = false; }
+            else { for (int p = q0; emit && p < q; p++) if (gather_includes(G, boxes[p], i, jj, k)) emit = false; }
+        }
+        const unsigned bal = __ballot_sync(0xffffffffu, emit);
+        if (lane == 0) warp_cnt[warp] = __popc(bal);
+        __syncthreads();
+        if (WRITE && emit) {
+            long long pos = running + __popc(bal & ((1u << lane) - 1u));
+            for (int w = 0; w < warp; w++) pos += warp_cnt[w];
+            if (pos < cap) { out[3 * pos] = (i + 0.5) * G.res + G.bmin[0]; out[3 * pos + 1] = (jj + 0.5) * G.res + G.bmin[1]; out[3 * pos + 2] = (k + 0.5) * G.res + G.bmin[2]; }
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) { int t = 0; for (int w = 0; w < 8; w++) t += warp_cnt[w]; running += t; }
+        __syncthreads();
+    }
+    if (!WRITE && threadIdx.x == 0) counts[q] = (int)running;
+}
+
+// one CTA: offs[r] = sum of counts[0 .. r-1] over the R rows (in chunks of 1024, each a warp-shuffle scan plus a scan of the warp totals),
+// pt_off[b] = the offset of plan b's first row (the total for plans at the end), *total = the sum of every count
+__global__ void __launch_bounds__(1024) k_gather_scan(const int *counts, int R, const int *wp_off, int B, long long *offs, int *pt_off, long long *total) {
+    __shared__ long long warp_sum[32];
+    __shared__ long long running;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) running = 0;
+    __syncthreads();
+    for (int base = 0; base < R; base += 1024) {
+        const int r = base + threadIdx.x;
+        const long long v = r < R ? counts[r] : 0;
+        long long incl = v;
+        for (int o = 1; o < 32; o <<= 1) { const long long t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
+        if (lane == 31) warp_sum[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            long long s = warp_sum[lane];
+            for (int o = 1; o < 32; o <<= 1) { const long long t = __shfl_up_sync(0xffffffffu, s, o); if (lane >= o) s += t; }
+            warp_sum[lane] = s;
+        }
+        __syncthreads();
+        const long long excl = running + (warp ? warp_sum[warp - 1] : 0) + incl - v;
+        if (r < R) offs[r] = excl;
+        __syncthreads();
+        if (threadIdx.x == 1023) running = excl + v;
+        __syncthreads();
+    }
+    for (int b = threadIdx.x; b <= B; b += blockDim.x) {
+        const long long o = wp_off[b] < R ? offs[wp_off[b]] : running;
+        pt_off[b] = (int)(o < 0x7fffffffll ? o : 0x7fffffffll);
+    }
+    if (threadIdx.x == 0) *total = running;
+}
+
+// the batched gather on stream st from staged inputs: d_wp (R x 3 rows), d_wp_off (its B + 1 offsets; h_wp_off the same on the host).
+// Counts and scans, reads the plans' offsets into pt_off (B + 1, also when the lists exceed cap) and the total into *total; then, when
+// the total fits cap, writes every list to c->gat.d_out.
+static int gather_batch_run(isdf_ctx *c, int B, const int *h_wp_off, const int *d_wp_off, const double *d_wp, double half, const double *offset,
+                            long long cap, std::vector<int> &pt_off, long long *total, cudaStream_t st) {
+    auto &g = c->gat;
+    const int R = h_wp_off[B];
+    int maxQ = 0;
+    for (int b = 0; b < B; b++) maxQ = std::max(maxQ, h_wp_off[b + 1] - h_wp_off[b]);
+    const size_t Rd = (size_t)std::max(R, 1);
+    CU_TRY(g.d_box.ensure(Rd)); CU_TRY(g.d_cnt.ensure(Rd)); CU_TRY(g.d_offs.ensure(Rd)); CU_TRY(g.d_ptoff.ensure((size_t)B + 1)); CU_TRY(g.d_total.ensure(1));
+    const double ox = offset ? offset[0] : 0.0, oy = offset ? offset[1] : 0.0, oz = offset ? offset[2] : 0.0;
+    if (R > 0) {
+        k_gather_boxes_batch<<<(R + 127) / 128, 128, 0, st>>>(c->map.grid, d_wp_off, B, d_wp, R, half, ox, oy, oz, g.d_box.p);
+        k_gather_points_batch<false><<<dim3(maxQ, B), 256, 0, st>>>(c->map.grid, d_wp_off, g.d_box.p, g.d_cnt.p, nullptr, nullptr, 0);
+        c->stats.kernel_launches += 2;
+    }
+    k_gather_scan<<<1, 1024, 0, st>>>(g.d_cnt.p, R, d_wp_off, B, g.d_offs.p, g.d_ptoff.p, g.d_total.p);
+    c->stats.kernel_launches++;
+    CU_TRY(cudaGetLastError());
+    pt_off.assign((size_t)B + 1, 0);
+    CU_TRY(cudaMemcpyAsync(pt_off.data(), g.d_ptoff.p, sizeof(int) * ((size_t)B + 1), cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaMemcpyAsync(total, g.d_total.p, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    if (*total > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "the obstacle lists hold more than 2^31 - 1 points");
+    if (*total > cap) return fail(ISDF_ERR_INVALID, "cap smaller than the obstacle lists (pt_off reports their sizes)");
+    if (*total == 0) return 0;
+    CU_TRY(g.d_out.ensure((size_t)3 * *total));
+    k_gather_points_batch<true><<<dim3(maxQ, B), 256, 0, st>>>(c->map.grid, d_wp_off, g.d_box.p, nullptr, g.d_offs.p, g.d_out.p, *total);
+    c->stats.kernel_launches++;
+    CU_TRY(cudaGetLastError());
+    return 0;
+}
+
+// the lists in c->gat.d_out become the batched swept-volume point sets (isdf_set_points_batch from device memory); no point at all gives
+// up both sets and switches the batched term off
+static int gather_set_points(isdf_ctx *c, int B, const std::vector<int> &pt_off, long long total, cudaStream_t st) {
+    if (total == 0) CU_TRY(c->sv.set_points(nullptr, 0, st));
+    else CU_TRY(c->sv.set_points_batch(B, pt_off.data(), c->gat.d_out.p, st, cudaMemcpyDeviceToDevice));
+    return 0;
+}
+
+extern "C" int isdf_gather_obstacle_points_batch(isdf_ctx *c, int B, const int32_t *wp_off, const double *waypoints, double half_extent,
+                                                 const double *offset, int64_t cap, double *out_points, int32_t *pt_off, int set_as_points) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (B < 1 || B > 65535) return fail(ISDF_ERR_INVALID, "B must lie in [1, 65535]");
+    if (!wp_off || !pt_off || cap < 0) return fail(ISDF_ERR_INVALID, "NULL argument or cap < 0");
+    if (wp_off[0] != 0) return fail(ISDF_ERR_INVALID, "wp_off[0] must be 0");
+    for (int b = 0; b < B; b++) if (wp_off[b + 1] < wp_off[b]) return fail(ISDF_ERR_INVALID, "wp_off must be non-decreasing");
+    if (wp_off[B] > 0 && !waypoints) return fail(ISDF_ERR_INVALID, "waypoints is NULL");
+    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    auto &g = c->gat;
+    const int R = wp_off[B];
+    CU_TRY(g.d_wpoff.upload(wp_off, (size_t)B + 1, c->stream));
+    if (R > 0) CU_TRY(g.d_wp.upload(waypoints, (size_t)3 * R, c->stream));
+    std::vector<int> off;
+    long long total = 0;
+    const int r = gather_batch_run(c, B, wp_off, g.d_wpoff.p, g.d_wp.p, half_extent, offset, out_points ? cap : 0x7fffffffll, off, &total, c->stream);
+    if (!off.empty()) std::memcpy(pt_off, off.data(), sizeof(int32_t) * off.size());
+    if (r) return r;
+    if (out_points && total > 0) {   // the write pass runs on the context's non-blocking stream
+        CU_TRY(cudaMemcpyAsync(out_points, g.d_out.p, sizeof(double) * 3 * total, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaStreamSynchronize(c->stream));
+    }
+    if (set_as_points) return gather_set_points(c, B, off, total, c->stream);
+    return 0;
 }
 
 // ---- discrete evaluation ------------------------------------------------------------------------------------
@@ -2835,6 +3048,290 @@ extern "C" int isdf_frontend_path_info(isdf_ctx *c, isdf_frontpath_info *out) {
     if (!c || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
     *out = c->fp.info;
     return 0;
+}
+
+// ---- planning step: PlannerManager::generateTraj for one start and B goals (include/isdf.h) --------------------------------------------
+// The stages are the existing entry points' internals on device buffers: path_run, isdf_path_waypoints, midend_batch_run per N group, the
+// batched gather with set_as_points, lbfgs_rounds over callback_batch_launch, k_minco_forward for the final trajectories, certify_run and
+// dynamics_run with N0 = N.
+extern "C" int isdf_plan_default_params(isdf_ctx *c, isdf_plan_params *p) {
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    std::memset(p, 0, sizeof(*p));
+    isdf_config d;
+    isdf_default_config(&d);
+    const isdf_config &g = c ? c->cfg : d;
+    p->parlength = 3.0;                                             // traj_parlength (plan_manager.cpp:153)
+    p->half_extent = g.kernel_size * g.occupancy_resolution / 3.0;  // (:135, :243)
+    p->rho = 20.0;
+    isdf_midend_default_params(&p->midend);
+    isdf_lbfgs_default_params(&p->backend);
+    p->backend.max_iterations = 10000;                              // LMBM's cap (lmbm.h:20-57), taken as an analogue
+    p->flags = ISDF_PLAN_CERTIFY | ISDF_PLAN_DYNAMICS;
+    isdf_certify_default_params(&p->certify);
+    isdf_dynamics_default_params(c, &p->dynamics);
+    return 0;
+}
+
+extern "C" int isdf_get_plan_info(isdf_ctx *c, isdf_plan_info *out) {
+    if (!c || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
+    *out = c->plan.info;
+    return 0;
+}
+
+// every check that needs no device work; *r_cert: the certificate's body radius (ISDF_PLAN_CERTIFY)
+static int plan_check(isdf_ctx *c, const isdf_plan_params *p, double *r_cert) {
+    if (int r = frontend_state(c)) return r;
+    if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
+    if (c->world > 1) return fail(ISDF_ERR_UNSUPPORTED, "the planning step is not sharded: call it on a context with isdf_set_shard(ctx, 0, 1)");
+    if (p->reserved_ != 0) return fail(ISDF_ERR_INVALID, "reserved_ must be 0");
+    if (p->flags & ~(ISDF_PLAN_CERTIFY | ISDF_PLAN_DYNAMICS)) return fail(ISDF_ERR_INVALID, "unknown flags");
+    if (!(std::isfinite(p->parlength) && p->parlength > 0.0)) return fail(ISDF_ERR_INVALID, "parlength must be finite and positive");
+    if (!(std::isfinite(p->half_extent) && p->half_extent >= 0.0)) return fail(ISDF_ERR_INVALID, "half_extent must be finite and >= 0");
+    for (double v : {p->offset[0], p->offset[1], p->offset[2], p->rho}) if (!std::isfinite(v)) return fail(ISDF_ERR_INVALID, "offset and rho must be finite");
+    if (int r = midend_check(c, 1, 1, &p->midend)) return r;
+    if (int r = lbfgs_check(&p->backend)) return r;
+    if (p->flags & ISDF_PLAN_CERTIFY) {
+        if (p->certify.clearance.pieces_per_traj != 0) return fail(ISDF_ERR_INVALID, "certify.clearance.pieces_per_traj must be 0 (the call sets N0 = N)");
+        if (int r = certify_check(c, 1, &p->certify, r_cert)) return r;
+    }
+    if (p->flags & ISDF_PLAN_DYNAMICS) {
+        if (p->dynamics.pieces_per_traj != 0) return fail(ISDF_ERR_INVALID, "dynamics.pieces_per_traj must be 0 (the call sets N0 = N)");
+        if (int r = dynamics_check(c, 1, &p->dynamics)) return r;
+    }
+    return 0;
+}
+
+static int plan_run(isdf_ctx *c, const double *start, int B, const double *goals, const isdf_plan_params *p, double r_cert, int cap_nodes,
+                    int32_t *path_off, double *path_xyz, int cap_pieces, int32_t *piece_off, double *T, double *coeffs, isdf_plan_result *res,
+                    isdf_certify_summary *certify, isdf_dynamics_summary *dynamics) {
+    const cudaStream_t st = c->stream;
+    auto &z = c->plan;
+    isdf_plan_info &info = z.info;
+    info = {};
+    for (cudaEvent_t &e : z.ev) if (!e) CU_TRY(cudaEventCreate(&e));
+    // the device time of one stage's work on st, added to acc
+    auto timed = [&](double &acc, auto body) -> int {
+        CU_TRY(cudaEventRecord(z.ev[0], st));
+        if (int r = body()) return r;
+        CU_TRY(cudaEventRecord(z.ev[1], st));
+        CU_TRY(cudaEventSynchronize(z.ev[1]));
+        float ms = 0;
+        CU_TRY(cudaEventElapsedTime(&ms, z.ev[0], z.ev[1]));
+        acc += ms;
+        return 0;
+    };
+    const double nan = std::numeric_limits<double>::quiet_NaN();
+    // 1. front end
+    std::vector<int> off;
+    if (int r = timed(info.frontend_ms, [&] { return path_run(c, start, B, goals, 0x7fffffff, off, st); })) return r;
+    const int nodes = off[B];
+    std::vector<double> xyz((size_t)3 * nodes), pcost(B);
+    std::vector<uint8_t> found(B);
+    CU_TRY(cudaMemcpyAsync(xyz.data(), c->fp.d_xyz.p, sizeof(double) * xyz.size(), cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaMemcpyAsync(pcost.data(), c->fp.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaMemcpyAsync(found.data(), c->fp.d_found.p, B, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    // 2. waypoints, stages known before the mid-end, sizes
+    std::vector<double> wps((size_t)3 * std::max(nodes, 1));
+    std::vector<int> wp_off((size_t)B + 1), N(B);
+    if (int r = isdf_path_waypoints(B, off.data(), xyz.data(), c->map.grid.res, p->parlength, nodes, wps.data(), wp_off.data(), N.data())) return r;
+    std::vector<int> poff((size_t)B + 1, 0);
+    for (int b = 0; b < B; b++) {
+        const bool traj = found[b] && minco_smem_bytes(N[b]) <= 220 * 1024;   // N <= 290 (minco_fits)
+        const long long t = (long long)poff[b] + (traj ? N[b] : 0);
+        if (t > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "the trajectories hold more than 2^31 - 1 pieces");
+        poff[b + 1] = (int)t;
+        isdf_plan_result &q = res[b];
+        q = {};
+        q.stage = !found[b] ? ISDF_PLAN_NO_PATH : (traj ? ISDF_PLAN_OPTIMISED : ISDF_PLAN_TOO_LONG);   // OPTIMISED: pending until the mid-end
+        q.path_nodes = off[b + 1] - off[b]; q.pieces = found[b] ? N[b] : 0;
+        q.path_cost = pcost[b]; q.midend_f = q.backend_f = nan; q.duration = 0.0;
+        if (certify) certify[b] = certify_failed_summary();
+        if (dynamics) dynamics[b] = dynamics_failed_summary();
+    }
+    if (path_off) std::memcpy(path_off, off.data(), sizeof(int32_t) * off.size());
+    std::memcpy(piece_off, poff.data(), sizeof(int32_t) * poff.size());
+    if ((path_xyz && nodes > cap_nodes) || poff[B] > cap_pieces)
+        return fail(ISDF_ERR_INVALID, "cap_nodes or cap_pieces too small (path_off / piece_off report the sizes needed)");
+    if (path_xyz && nodes) std::memcpy(path_xyz, xyz.data(), sizeof(double) * xyz.size());
+    // 3-7. per N group, ascending
+    std::vector<int> Ns;
+    for (int b = 0; b < B; b++) if (res[b].stage == ISDF_PLAN_OPTIMISED) Ns.push_back(N[b]);
+    std::sort(Ns.begin(), Ns.end());
+    Ns.erase(std::unique(Ns.begin(), Ns.end()), Ns.end());
+    for (const int Ng : Ns) {
+        std::vector<int> idx;
+        for (int b = 0; b < B; b++) if (res[b].stage == ISDF_PLAN_OPTIMISED && N[b] == Ng) idx.push_back(b);
+        const int Bg = (int)idx.size(), n = 4 * Ng - 3, W = Ng - 1;
+        const size_t BN = (size_t)Bg * Ng;
+        info.groups++;
+        // head = [path.front(), 0, 0], tail = [path.back(), 0, 0] (3x3 column-major, column 0 the position): [heads | tails]; the waypoints
+        std::vector<double> bc((size_t)18 * Bg, 0.0), gw((size_t)3 * std::max<size_t>(BN - Bg, 1));
+        for (int q = 0; q < Bg; q++) {
+            const int b = idx[q];
+            for (int k = 0; k < 3; k++) { bc[9 * (size_t)q + k] = xyz[3 * (size_t)off[b] + k]; bc[9 * ((size_t)Bg + q) + k] = xyz[3 * ((size_t)off[b + 1] - 1) + k]; }
+            std::copy(wps.begin() + 3 * (size_t)wp_off[b], wps.begin() + 3 * (size_t)wp_off[b + 1], gw.begin() + 3 * (size_t)q * W);
+        }
+        CU_TRY(z.d_bc.upload(bc.data(), bc.size(), st)); CU_TRY(z.d_wp.upload(gw.data(), gw.size(), st));
+        CU_TRY(z.d_mx.ensure((size_t)Bg * n)); CU_TRY(z.d_mres.ensure(19 * BN + Bg)); CU_TRY(z.d_mi.ensure((size_t)3 * Bg));
+        double *d_mf = z.d_mres.p, *d_mT = d_mf + Bg, *d_mC = d_mT + BN;   // [f | T | coeffs]
+        if (int r = midend_check(c, Bg, Ng, &p->midend)) return r;
+        int mrounds = 0;
+        if (int r = timed(info.midend_ms, [&] {
+                return midend_batch_run(c, Bg, Ng, z.d_bc.p, z.d_bc.p + 9 * (size_t)Bg, 1, &p->midend, z.d_wp.p, z.d_mx.p, d_mT, d_mC, d_mf, z.d_mi.p,
+                                        z.d_mi.p + Bg, z.d_mi.p + 2 * (size_t)Bg, &mrounds, st);
+            })) return r;
+        std::vector<double> mres(Bg + BN);   // [f | T]
+        std::vector<int> mi((size_t)3 * Bg);
+        CU_TRY(cudaMemcpyAsync(mres.data(), d_mf, sizeof(double) * mres.size(), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(mi.data(), z.d_mi.p, sizeof(int) * mi.size(), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
+        std::vector<int> ok, pos(Bg, -1);   // the plans that passed the mid-end (plan_manager.cpp:277) and their back-end instance
+        for (int q = 0; q < Bg; q++) {
+            isdf_plan_result &r = res[idx[q]];
+            r.midend_f = mres[q]; r.midend_ret = mi[q];
+            if (mi[q] >= 0) { pos[q] = (int)ok.size(); ok.push_back(q); }
+            else r.stage = ISDF_PLAN_MIDEND_FAILED;
+        }
+        const int Bp = (int)ok.size();
+        if (Bp > 0) {
+            // 4. the passed plans' obstacle lists become the batched point sets
+            std::vector<int> gwo((size_t)Bp + 1);
+            std::vector<double> pw((size_t)3 * std::max(Bp * W, 1));
+            for (int k = 0; k <= Bp; k++) gwo[k] = k * W;
+            for (int k = 0; k < Bp; k++) std::copy(gw.begin() + 3 * (size_t)ok[k] * W, gw.begin() + 3 * ((size_t)ok[k] + 1) * W, pw.begin() + 3 * (size_t)k * W);
+            CU_TRY(c->gat.d_wpoff.upload(gwo.data(), gwo.size(), st)); CU_TRY(c->gat.d_wp.upload(pw.data(), pw.size(), st));
+            std::vector<int> pto;
+            long long tot = 0;
+            if (int r = timed(info.gather_ms, [&] {
+                    if (int rr = gather_batch_run(c, Bp, gwo.data(), c->gat.d_wpoff.p, c->gat.d_wp.p, p->half_extent, p->offset, 0x7fffffffll, pto, &tot, st)) return rr;
+                    return gather_set_points(c, Bp, pto, tot, st);
+                })) return r;
+            for (int k = 0; k < Bp; k++) res[idx[ok[k]]].obstacle_points = pto[k + 1] - pto[k];
+            // 5. persisted durations: what updateTraj(mid-end trajectory) leaves on a fresh context (swm:287-296)
+            std::vector<double> dur(Bp);
+            for (int k = 0; k < Bp; k++) {
+                double td = 0.0;
+                for (int i = 0; i < Ng; i++) td += mres[Bg + (size_t)ok[k] * Ng + i];
+                dur[k] = td < 3 * 1e2 ? td : 0.0;
+            }
+            CU_TRY(c->sv.set_durations(Bp, dur.data(), st));
+            // 6. back end from the mid-end x
+            std::vector<double> bbc((size_t)18 * Bp);
+            for (int k = 0; k < Bp; k++) {
+                std::copy(bc.begin() + 9 * (size_t)ok[k], bc.begin() + 9 * ((size_t)ok[k] + 1), bbc.begin() + 9 * (size_t)k);
+                std::copy(bc.begin() + 9 * ((size_t)Bg + ok[k]), bc.begin() + 9 * ((size_t)Bg + ok[k] + 1), bbc.begin() + 9 * ((size_t)Bp + k));
+            }
+            CU_TRY(z.d_bbc.upload(bbc.data(), bbc.size(), st));
+            const double *d_bh = z.d_bbc.p, *d_bt = z.d_bbc.p + 9 * (size_t)Bp;
+            CU_TRY(z.d_bx.ensure((size_t)Bp * n)); CU_TRY(z.d_bf.ensure(Bp)); CU_TRY(z.d_bi.ensure((size_t)3 * Bp));
+            for (int k = 0; k < Bp; k++)
+                CU_TRY(cudaMemcpyAsync(z.d_bx.p + (size_t)k * n, z.d_mx.p + (size_t)ok[k] * n, sizeof(double) * n, cudaMemcpyDeviceToDevice, st));
+            if (int r = callback_batch_check(c, Bp, Ng)) return r;
+            int brounds = 0;
+            if (int r = timed(info.backend_ms, [&]() -> int {
+                    if (int rr = lbfgs_rounds(c, c->lbfgs, Bp, n, &p->backend, 0, z.d_bx.p, z.d_bf.p, z.d_bi.p, z.d_bi.p + Bp, z.d_bi.p + 2 * (size_t)Bp,
+                                              &brounds, st, [&](const double *x, double *f, double *g) {
+                                                  return callback_batch_launch(c, Bp, Ng, d_bh, d_bt, 9, p->rho, x, f, g, st);
+                                              })) return rr;
+                    // the final trajectories: forwardT + MINCO of the returned x (back_end_optimizer.cpp:140-163), into the batch trajectories
+                    MincoArgs M = c->batch.minco.args(Bp, Ng, d_bh, d_bt, 9, p->rho, z.d_bx.p);
+                    k_minco_forward<<<Bp, 32, minco_smem_bytes(Ng), st>>>(M);
+                    c->stats.kernel_launches++;
+                    CU_TRY(cudaGetLastError());
+                    c->batch.B = Bp; c->batch.N0 = Ng;
+                    return 0;
+                })) return r;
+            info.backend_rounds += brounds;
+            std::vector<double> bf(Bp);
+            std::vector<int> bi((size_t)3 * Bp);
+            CU_TRY(cudaMemcpyAsync(bf.data(), z.d_bf.p, sizeof(double) * Bp, cudaMemcpyDeviceToHost, st));
+            CU_TRY(cudaMemcpyAsync(bi.data(), z.d_bi.p, sizeof(int) * bi.size(), cudaMemcpyDeviceToHost, st));
+            CU_TRY(cudaStreamSynchronize(st));
+            for (int k = 0; k < Bp; k++) {
+                isdf_plan_result &r = res[idx[ok[k]]];
+                r.backend_f = bf[k]; r.backend_ret = bi[k]; r.backend_iterations = bi[Bp + k]; r.backend_evaluations = bi[2 * (size_t)Bp + k];
+            }
+        }
+        // the group's returned trajectories in goal order, one block (piece q*N + i): the back end's, or the mid-end's for MIDEND_FAILED
+        CU_TRY(z.d_gT.ensure(BN)); CU_TRY(z.d_gC.ensure(18 * BN));
+        for (int q = 0; q < Bg; q++) {
+            const bool be = pos[q] >= 0;
+            const double *sT = be ? c->batch.minco.d_T.p + (size_t)pos[q] * Ng : d_mT + (size_t)q * Ng;
+            const double *sC = be ? c->batch.minco.d_C.p + 6 * (size_t)pos[q] * Ng : d_mC + 6 * (size_t)q * Ng;
+            const size_t spitch = sizeof(double) * 6 * (be ? (size_t)Bp * Ng : BN);
+            CU_TRY(cudaMemcpyAsync(z.d_gT.p + (size_t)q * Ng, sT, sizeof(double) * Ng, cudaMemcpyDeviceToDevice, st));
+            CU_TRY(cudaMemcpy2DAsync(z.d_gC.p + 6 * (size_t)q * Ng, sizeof(double) * 6 * BN, sC, spitch, sizeof(double) * 6 * Ng, 3, cudaMemcpyDeviceToDevice, st));
+        }
+        std::vector<double> gT(BN), gC(18 * BN);
+        CU_TRY(cudaMemcpyAsync(gT.data(), z.d_gT.p, sizeof(double) * BN, cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(gC.data(), z.d_gC.p, sizeof(double) * 18 * BN, cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
+        for (int q = 0; q < Bg; q++) {
+            const size_t po = (size_t)poff[idx[q]];
+            double td = 0.0;
+            for (int i = 0; i < Ng; i++) { T[po + i] = gT[(size_t)q * Ng + i]; td += T[po + i]; }
+            res[idx[q]].duration = td;
+            for (int a = 0; a < 3; a++)
+                std::memcpy(coeffs + 18 * po + 6 * (size_t)a * Ng, gC.data() + 6 * ((size_t)a * BN + (size_t)q * Ng), sizeof(double) * 6 * Ng);
+        }
+        // 7. certificates on every returned trajectory of the group
+        if (p->flags & ISDF_PLAN_CERTIFY) {
+            isdf_certify_params pc = p->certify;
+            pc.clearance.pieces_per_traj = Ng;
+            double rr = r_cert;
+            if (int r = certify_check(c, (int)BN, &pc, &rr)) return r;
+            CU_TRY(z.d_csum.ensure(Bg));
+            if (int r = timed(info.certify_ms, [&] { return certify_run(c, (int)BN, z.d_gT.p, z.d_gC.p, &pc, rr, z.d_csum.p, st); })) return r;
+            std::vector<isdf_certify_summary> s(Bg);
+            CU_TRY(cudaMemcpyAsync(s.data(), z.d_csum.p, sizeof(isdf_certify_summary) * Bg, cudaMemcpyDeviceToHost, st));
+            CU_TRY(cudaStreamSynchronize(st));
+            for (int q = 0; q < Bg; q++) certify[idx[q]] = s[q];
+        }
+        if (p->flags & ISDF_PLAN_DYNAMICS) {
+            isdf_dynamics_params pd = p->dynamics;
+            pd.pieces_per_traj = Ng;
+            if (int r = dynamics_check(c, (int)BN, &pd)) return r;
+            CU_TRY(z.d_dsum.ensure(Bg));
+            if (int r = timed(info.dynamics_ms, [&] { return dynamics_run(c, (int)BN, z.d_gT.p, z.d_gC.p, &pd, z.d_dsum.p, st); })) return r;
+            std::vector<isdf_dynamics_summary> s(Bg);
+            CU_TRY(cudaMemcpyAsync(s.data(), z.d_dsum.p, sizeof(isdf_dynamics_summary) * Bg, cudaMemcpyDeviceToHost, st));
+            CU_TRY(cudaStreamSynchronize(st));
+            for (int q = 0; q < Bg; q++) dynamics[idx[q]] = s[q];
+        }
+    }
+    return 0;
+}
+
+extern "C" int isdf_plan_batch(isdf_ctx *c, const double *start, int B, const double *goals, const isdf_plan_params *p, int cap_nodes,
+                               int32_t *path_off, double *path_xyz, int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
+                               isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics) {
+    bool started = false;
+    const int rc = poison_on_failure([&]() -> int {
+        if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+        if (!start || !goals || B < 1 || !p || !piece_off || !results || cap_pieces < 0 || (cap_pieces > 0 && (!T || !coeffs)) ||
+            (path_xyz && (!path_off || cap_nodes < 0)))
+            return fail(ISDF_ERR_INVALID, "NULL argument, B < 1 or a cap < 0");
+        if (((p->flags & ISDF_PLAN_CERTIFY) && !certify) || ((p->flags & ISDF_PLAN_DYNAMICS) && !dynamics))
+            return fail(ISDF_ERR_INVALID, "a summary array of a requested certificate is NULL");
+        double r_cert = 0.0;
+        if (int r = plan_check(c, p, &r_cert)) return r;
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        started = true;
+        return plan_run(c, start, B, goals, p, r_cert, cap_nodes, path_off, path_xyz, cap_pieces, piece_off, T, coeffs, results, certify, dynamics);
+    }, [&] {
+        if (B < 1) return;
+        if (results)
+            for (int b = 0; b < B; b++) {
+                results[b] = {};
+                results[b].stage = ISDF_PLAN_FAILED;
+                results[b].path_cost = results[b].midend_f = results[b].backend_f = results[b].duration = std::numeric_limits<double>::quiet_NaN();
+            }
+        if (certify) write_failed_summaries(certify, B, certify_failed_summary());
+        if (dynamics) write_failed_summaries(dynamics, B, dynamics_failed_summary());
+    });
+    if (started) c->sv.set_points(nullptr, 0, c->stream);   // both point sets given up, the batched swept-volume term off
+    return rc;
 }
 
 // the traversability bits of the last path or field call (X*Y*ceil(Z/32) words of the map it ran on, grid.bits' layout)

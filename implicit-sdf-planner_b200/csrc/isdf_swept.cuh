@@ -809,12 +809,13 @@ struct SweptState {
     bool order_ready = false; int order_rank = -1, order_world = -1;
 
     // the only place that replaces the point set: it gives up the current one (and any per-problem sets: set_points_batch sets B
-    // after it) before it touches the buffers
-    cudaError_t set_points(const double *pts, int n, cudaStream_t st) {
+    // after it) before it touches the buffers. kind: where pts lives (host, or device memory of this context's device)
+    cudaError_t set_points(const double *pts, int n, cudaStream_t st, cudaMemcpyKind kind = cudaMemcpyHostToDevice) {
         cudaError_t e = cudaSuccess;
         P = 0; B = 0;
         if (n == 0) return e;
-        if ((e = d_pts.upload(pts, (size_t)3 * n, st)) != cudaSuccess) return e;
+        if ((e = d_pts.ensure((size_t)3 * n)) != cudaSuccess) return e;
+        if ((e = cudaMemcpyAsync(d_pts.p, pts, sizeof(double) * 3 * n, kind, st)) != cudaSuccess) return e;
         if ((e = d_tstar.ensure(n)) != cudaSuccess) return e;
         if ((e = d_sdf.ensure(n)) != cudaSuccess) return e;
         if ((e = d_grel.ensure((size_t)3 * n)) != cudaSuccess) return e;
@@ -885,8 +886,8 @@ struct SweptState {
     int B = 0, maxP = 0;
     std::vector<int> h_off;
     DevBuf<int> d_off;
-    cudaError_t set_points_batch(int nB, const int *off, const double *pts, cudaStream_t st) {
-        cudaError_t e = set_points(pts, off[nB], st);
+    cudaError_t set_points_batch(int nB, const int *off, const double *pts, cudaStream_t st, cudaMemcpyKind kind = cudaMemcpyHostToDevice) {
+        cudaError_t e = set_points(pts, off[nB], st, kind);
         if (e != cudaSuccess) return e;
         if ((e = d_off.upload(off, (size_t)nB + 1, st)) != cudaSuccess) return e;
         if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return e;
@@ -896,19 +897,32 @@ struct SweptState {
         B = nB;
         return cudaSuccess;
     }
+    // room for the persisted durations of nB problems
+    cudaError_t grow_state_b(int nB, cudaStream_t st) {
+        cudaError_t e = cudaSuccess;
+        if (d_state_b.n < (size_t)4 * nB) {   // a problem's traj_duration starts at 0; growing B keeps the durations of the problems already there
+            DevBuf<double> grown;
+            if ((e = grown.ensure((size_t)4 * nB)) != cudaSuccess) return e;
+            if ((e = cudaMemsetAsync(grown.p, 0, sizeof(double) * 4 * nB, st)) != cudaSuccess) return e;
+            if (d_state_b.n && (e = cudaMemcpyAsync(grown.p, d_state_b.p, sizeof(double) * d_state_b.n, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return e;
+            if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return e;   // the old buffer is freed below
+            d_state_b = std::move(grown);
+        }
+        return e;
+    }
+    // the persisted durations of problems 0 .. nB-1 of the batched term (dur: nB host values)
+    cudaError_t set_durations(int nB, const double *dur, cudaStream_t st) {
+        cudaError_t e;
+        if ((e = grow_state_b(nB, st)) != cudaSuccess) return e;
+        if ((e = cudaMemcpy2DAsync(d_state_b.p, 4 * sizeof(double), dur, sizeof(double), sizeof(double), nB, cudaMemcpyHostToDevice, st)) != cudaSuccess) return e;
+        return cudaStreamSynchronize(st);
+    }
     cudaError_t launch_batch(const DevCfg &cfg, const DevShape &shape, int N, const double *d_T, const double *d_Cpp, double *d_out, cudaStream_t st, int *launches) {
         cudaError_t e;
         if ((e = d_times.ensure((size_t)B * SV_MAX_COARSE)) != cudaSuccess) return e;
         if ((e = d_poses.ensure((size_t)12 * B * SV_MAX_COARSE)) != cudaSuccess) return e;
         if ((e = d_meta.ensure((size_t)4 * B)) != cudaSuccess) return e;
-        if (d_state_b.n < (size_t)4 * B) {   // a problem's traj_duration starts at 0; growing B keeps the durations of the problems already there
-            DevBuf<double> grown;
-            if ((e = grown.ensure((size_t)4 * B)) != cudaSuccess) return e;
-            if ((e = cudaMemsetAsync(grown.p, 0, sizeof(double) * 4 * B, st)) != cudaSuccess) return e;
-            if (d_state_b.n && (e = cudaMemcpyAsync(grown.p, d_state_b.p, sizeof(double) * d_state_b.n, cudaMemcpyDeviceToDevice, st)) != cudaSuccess) return e;
-            if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return e;   // the old buffer is freed below
-            d_state_b = std::move(grown);
-        }
+        if ((e = grow_state_b(B, st)) != cudaSuccess) return e;
         if (d_counter.n == 0) { if ((e = d_counter.ensure(2)) != cudaSuccess) return e; }
         if ((e = d_piece_gdt.ensure((size_t)B * N)) != cudaSuccess) return e;
         if ((e = d_piece_cost.ensure((size_t)B * N)) != cudaSuccess) return e;

@@ -39,10 +39,13 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_midend_batch", "isdf_midend_batch_device", "isdf_certify_default_params", "isdf_trajectory_certify",
                "isdf_trajectory_certify_device", "isdf_swept_default_params", "isdf_swept_volume_sdf", "isdf_swept_volume_grid",
                "isdf_swept_volume_grid_device", "isdf_swept_volume_mesh", "isdf_dynamics_default_params", "isdf_trajectory_dynamics",
-               "isdf_trajectory_dynamics_device"]
+               "isdf_trajectory_dynamics_device", "isdf_gather_obstacle_points_batch", "isdf_plan_default_params", "isdf_plan_batch",
+               "isdf_get_plan_info"]
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
 DYN_QUANTITIES = ["speed", "acceleration", "body_rate", "tilt", "thrust"]   # q of isdf_dynamics_summary; mask bit 5: the thrust minimum
+PLAN_CERTIFY, PLAN_DYNAMICS = 1, 2                                             # isdf_plan_params.flags
+PLAN_FAILED, NO_PATH, TOO_LONG, MIDEND_FAILED, OPTIMISED = -1, 0, 1, 2, 3      # isdf_plan_result.stage
 
 
 class KernelConfig(C.Structure):
@@ -118,6 +121,30 @@ class DynamicsSummary(C.Structure):
 
     def as_dict(self):
         return {n: (np.array(getattr(self, n)[:]) if n in ("upper", "attained", "t_attained") else getattr(self, n)) for n, _ in self._fields_}
+
+
+class PlanParams(C.Structure):
+    """isdf_plan_params"""
+    _fields_ = [("parlength", C.c_double), ("half_extent", C.c_double), ("offset", C.c_double * 3), ("rho", C.c_double), ("midend", MidendParams),
+                ("backend", LbfgsParams), ("flags", C.c_int32), ("reserved_", C.c_int32), ("certify", CertifyParams), ("dynamics", DynamicsParams)]
+
+
+class PlanResult(C.Structure):
+    """isdf_plan_result (one per goal)"""
+    _fields_ = [(n, C.c_int32) for n in ["stage", "path_nodes", "pieces", "obstacle_points", "midend_ret", "backend_ret", "backend_iterations",
+                                         "backend_evaluations"]] + [(n, C.c_double) for n in ["path_cost", "midend_f", "backend_f", "duration"]]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+class PlanInfo(C.Structure):
+    """isdf_plan_info"""
+    _fields_ = [("groups", C.c_int32), ("backend_rounds", C.c_int32)] + \
+               [(n, C.c_double) for n in ["frontend_ms", "midend_ms", "gather_ms", "backend_ms", "certify_ms", "dynamics_ms"]]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
 
 
 class SweptParams(C.Structure):
@@ -300,6 +327,11 @@ def load_library(path=None):
     lib.isdf_midend_callback_batch.argtypes = [vp, C.c_int, C.c_int, dp, dp, C.c_int, mpp, dp, dp, dp, dp]
     lib.isdf_midend_batch.argtypes = [vp, C.c_int, C.c_int, dp, dp, C.c_int, mpp, dp, dp, dp, dp, dp, ip, ip, ip, ip]
     lib.isdf_midend_batch_device.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_int, mpp, vp, vp, vp, vp, vp, vp, vp, vp, ip, vp]
+    lib.isdf_gather_obstacle_points_batch.argtypes = [vp, C.c_int, ip, dp, C.c_double, dp, C.c_int64, dp, ip, C.c_int]
+    lib.isdf_plan_default_params.argtypes = [vp, C.POINTER(PlanParams)]
+    lib.isdf_plan_batch.argtypes = [vp, dp, C.c_int, dp, C.POINTER(PlanParams), C.c_int, ip, dp, C.c_int, ip, dp, dp, C.POINTER(PlanResult),
+                                    C.POINTER(CertifySummary), C.POINTER(DynamicsSummary)]
+    lib.isdf_get_plan_info.argtypes = [vp, C.POINTER(PlanInfo)]
     for s in ABI_SYMBOLS:
         if s != "isdf_last_error":
             getattr(lib, s).restype = C.c_int
@@ -496,6 +528,30 @@ class Evaluator:
             self.n_points = n.value
         return out[:min(n.value, cap)].copy(), n.value
 
+    def gather_obstacle_points_batch(self, waypoints, half, offset=(0.0, 0.0, 0.0), set_as_points=False, cap=None):
+        """isdf_gather_obstacle_points_batch: one obstacle list per plan (waypoints: list of (n_b, 3) arrays, n_b may be 0) -> list of (P_b, 3)
+        arrays. cap = None: a first guess, repeated once with the reported total when the lists are longer."""
+        B = len(waypoints)
+        wo = np.zeros(B + 1, dtype=np.int32)
+        for b, w in enumerate(waypoints):
+            wo[b + 1] = wo[b] + len(w)
+        wp = _f64(np.concatenate([np.asarray(w, dtype=np.float64).reshape(-1, 3) for w in waypoints])) if B and wo[B] else np.zeros((1, 3))
+        off = _f64(offset).reshape(3)
+        ip = C.POINTER(C.c_int32)
+        cap = int(cap) if cap is not None else max(1024, 64 * int(wo[B]))
+        for attempt in range(2):
+            out, pt = np.zeros((max(cap, 1), 3)), np.zeros(B + 1, dtype=np.int32)
+            r = self.lib.isdf_gather_obstacle_points_batch(self.h, B, wo.ctypes.data_as(ip), _dp(wp), float(half), _dp(off), cap, _dp(out),
+                                                           pt.ctypes.data_as(ip), int(set_as_points))
+            if r == -1 and attempt == 0 and pt[B] > cap:
+                cap = int(pt[B])
+                continue
+            self._check(r)
+            break
+        if set_as_points and pt[B]:
+            self.n_points = int(pt[B])
+        return [out[pt[b]:pt[b + 1]].copy() for b in range(B)]
+
     def callback_batch(self, head, tail, rho, X):
         """B decision vectors [tau (N0) | xi (3(N0-1))] -> (cost[B], grad[B, 4*N0-3]); head/tail 3x3 (columns p, v, a), shared (3,3)
         or per problem (B,3,3); passed to the library column-major."""
@@ -674,6 +730,66 @@ class Evaluator:
             r = self.midend_batch(head, tail, wp, params)
             groups.append(dict(N=N, idx=idx, waypoints=wp, head=head, tail=tail, **r))
         return groups
+
+    # ---- planning step: generateTraj for one start and B goals (see include/isdf.h) ----
+    def plan_params(self, **kw):
+        """isdf_plan_default_params for this context, then overrides: parlength, half_extent, offset, rho, flags, reserved_, certify,
+        dynamics, midend (an isdf_midend_params) and backend (an isdf_lbfgs_params) by name; midend_<field> / backend_<field> set one field
+        of the nested blocks (midend_init_time=200.0, backend_max_iterations=50, midend_max_rounds=1, ...)"""
+        p = PlanParams()
+        self._check(self.lib.isdf_plan_default_params(self.h, C.byref(p)))
+        lb = {n for n, _ in LbfgsParams._fields_}
+        for k, v in kw.items():
+            if k == "offset":
+                p.offset[:] = [float(x) for x in v]
+            elif k.startswith("midend_"):
+                f = k[len("midend_"):]
+                setattr(p.midend.lbfgs if f in lb and f != "reserved_" else p.midend, f, v)
+            elif k.startswith("backend_"):
+                setattr(p.backend, k[len("backend_"):], v)
+            elif k in {n for n, _ in PlanParams._fields_}:
+                setattr(p, k, v)
+            else:
+                raise TypeError(f"unknown isdf_plan_params field {k}")
+        return p
+
+    def plan_batch(self, start, goals, params=None, **kw):
+        """isdf_plan_batch: one start, B goals -> (list of B dicts, info dict). Each dict: the isdf_plan_result fields, path (n, 3), T (N,),
+        coeffs (18 N, the plan's own 6N x 3 column-major block; empty without a trajectory), certify / dynamics summary dicts (None when the
+        flag is off). params: an isdf_plan_params, or None for plan_params(**kw). The caps are sized from the goals and the call repeated once
+        with the reported sizes when they are too small."""
+        p = params if params is not None else self.plan_params(**kw)
+        st = _f64(start).reshape(3)
+        goals = _f64(goals).reshape(-1, 3)
+        B = goals.shape[0]
+        ip = C.POINTER(C.c_int32)
+        cap_nodes, cap_pieces = self._path_cap(None) * B, 290 * B
+        for attempt in range(2):
+            xyz, po, T, Cc = np.zeros((max(cap_nodes, 1), 3)), np.zeros(B + 1, dtype=np.int32), np.zeros(max(cap_pieces, 1)), np.zeros(18 * max(cap_pieces, 1))
+            pf = np.zeros(B + 1, dtype=np.int32)
+            res, cs, ds = (PlanResult * B)(), (CertifySummary * B)(), (DynamicsSummary * B)()
+            r = self.lib.isdf_plan_batch(self.h, _dp(st), B, _dp(goals), C.byref(p), cap_nodes, pf.ctypes.data_as(ip), _dp(xyz), cap_pieces,
+                                         po.ctypes.data_as(ip), _dp(T), _dp(Cc), res, cs, ds)
+            if r == -1 and attempt == 0 and (pf[B] > cap_nodes or po[B] > cap_pieces):
+                cap_nodes, cap_pieces = max(cap_nodes, int(pf[B])), max(cap_pieces, int(po[B]))
+                continue
+            self._check(r)
+            break
+        out = []
+        for b in range(B):
+            d = res[b].as_dict()
+            d["path"] = xyz[pf[b]:pf[b + 1]].copy()
+            d["T"] = T[po[b]:po[b + 1]].copy()
+            d["coeffs"] = Cc[18 * po[b]:18 * po[b + 1]].copy()
+            d["certify"] = cs[b].as_dict() if p.flags & PLAN_CERTIFY else None
+            d["dynamics"] = ds[b].as_dict() if p.flags & PLAN_DYNAMICS else None
+            out.append(d)
+        return out, self.plan_info()
+
+    def plan_info(self):
+        info = PlanInfo()
+        self._check(self.lib.isdf_get_plan_info(self.h, C.byref(info)))
+        return info.as_dict()
 
     def batch_trajectories(self, B, N0):
         T, Cc, en = np.zeros(B * N0), np.zeros(18 * B * N0), np.zeros(B)

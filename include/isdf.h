@@ -189,6 +189,24 @@ int isdf_points_in_aabb(isdf_ctx *ctx, const double *centre, double half_extent,
  * order and the total in *n. If set_as_points != 0 the list also becomes the swept-volume point set (== isdf_set_points). */
 int isdf_gather_obstacle_points(isdf_ctx *ctx, const double *waypoints, int nQ, double half_extent, const double *offset,
                                 double *out_points, int cap, int *n, int set_as_points);
+/* Every plan's obstacle list in one call. B plans (1 <= B <= 65535); plan b's waypoints are rows [wp_off[b], wp_off[b+1]) of waypoints
+ * (x 3 row-major). A plan with no waypoints is allowed and gathers nothing.
+ *   Definition  plan b's list is exactly isdf_gather_obstacle_points(ctx, its waypoints, half_extent, offset): the same points in the same
+ *               (first-including waypoint, voxel address) order, with the 999 previous-waypoint sentinel for the plan's first box
+ *               (plan_manager.cpp:228). A plan's boxes are de-duplicated against its own earlier boxes only.
+ *   Output      the lists back to back in plan order in out_points (cap x 3); pt_off (B + 1) is their CSR, the offsets
+ *               isdf_set_points_batch takes. When cap is smaller than the total the call returns ISDF_ERR_INVALID, writes no point and
+ *               pt_off still reports the sizes needed. out_points may be NULL: cap is then ignored and only pt_off (and, with
+ *               set_as_points, the point sets) are produced.
+ *   set_as_points != 0: the lists also become the batched swept-volume point sets straight from device memory, bit-identical to
+ *               isdf_set_points_batch(ctx, B, pt_off, out_points): every t* starts at 0 (plan_manager.cpp:254) and the single-problem
+ *               set is given up. If no plan gathers a point, the batched term is switched off (as B = 0) and the single-problem set is
+ *               given up too.
+ * Device work: four launches over all plans (index boxes; per-waypoint counts, grid.y = plan; one scan of the counts; the ordered write)
+ * and one read of the offsets. Errors: ISDF_ERR_INVALID for a NULL argument, B out of range, offsets that do not start at 0 or decrease,
+ * cap < 0, or a total beyond 2^31 - 1; ISDF_ERR_STATE without a map. The call counts its launches in isdf_stats.kernel_launches. */
+int isdf_gather_obstacle_points_batch(isdf_ctx *ctx, int B, const int32_t *wp_off, const double *waypoints, double half_extent,
+                                      const double *offset, int64_t cap, double *out_points, int32_t *pt_off, int set_as_points);
 
 /* ---- discrete collision term: addTimeIntPenaltyParallel (hpp:432-554) with grad_cost_p (hpp:766-824) wired in */
 /* ACCUMULATES into *cost, gradC (6N x 3 col-major), gradT (N) exactly like the reference's reference arguments. */
@@ -726,6 +744,87 @@ int isdf_frontend_path_batch_device(isdf_ctx *ctx, const double *start, int B, c
  * path exists. Same errors and stream behaviour as the device variant. */
 int isdf_frontend_path_field_device(isdf_ctx *ctx, const double *start, const isdf_frontpath_params *params, double *d_g, void *cuda_stream);
 int isdf_frontend_path_info(isdf_ctx *ctx, isdf_frontpath_info *out);
+
+/* ---- planning step: PlannerManager::generateTraj (plan_manager.cpp:202-313) for one start and B goals, end to end on the device ----
+ * Definition, per goal b (each step is an existing entry point's definition):
+ *   1. Front end   isdf_frontend_path_batch(start, goals). A path not found is NO_PATH: no trajectory.
+ *   2. Waypoints   isdf_path_waypoints(parlength, the map's res) gives N. N > 290 (the limit of the mid-end and the callback) is TOO_LONG:
+ *                  no trajectory. head = [path.front(), 0, 0], tail = [path.back(), 0, 0] (:220-223).
+ *   3. Mid-end     isdf_midend_batch(per_problem_bc = 1, p->midend) over the plans with the same N: groups in ascending N, plans in goal
+ *                  order. midend_ret < 0 is MIDEND_FAILED: its trajectory is the mid-end's final one (what recent_traj holds, :270) and
+ *                  the back end does not run for it (:277).
+ *   4. Gather      isdf_gather_obstacle_points_batch(half_extent, offset, set_as_points = 1) over the waypoints of the group's plans that
+ *                  passed the mid-end. A plan with no point gets no swept-volume term, as the reference's loop over zero points.
+ *   5. Durations   before the back end, problem q's persisted trajectory duration (see isdf_set_points_batch) is what
+ *                  updateTraj(mid-end trajectory) (:272) leaves on a fresh context: its total duration (the left-to-right sum of T) when
+ *                  shorter than 300 s, else 0. Plans are therefore independent of each other and of the order of the groups.
+ *   6. Back end    isdf_lbfgs_batch(per_problem_bc = 1, p->rho, p->backend) from the mid-end x, with the context's flags. The final T and
+ *                  coeffs are forwardT + MINCO of the returned x whatever its ret (back_end_optimizer.cpp:140-163), computed without a
+ *                  further evaluation. Stage OPTIMISED; backend_ret < 0 is reported and the trajectory still returned (`if (1)`, :297).
+ *   7. Certificates with ISDF_PLAN_CERTIFY / ISDF_PLAN_DYNAMICS: isdf_trajectory_certify / isdf_trajectory_dynamics with p->certify /
+ *                  p->dynamics and N0 = N on every returned trajectory (OPTIMISED and MIDEND_FAILED).
+ * Deviation: the reference's back end is LMBM (lmbm.h, Fortran); the driver here is the project's device L-BFGS. max_iterations 10000 in
+ *   the defaults is LMBM's iteration cap (lmbm.h:20-57) taken as an analogue, not an equivalent.
+ * Guarantees: results are bit-identical run to run; each plan is bit-identical to the same call with that goal alone; every output is
+ *   bit-identical to the composition of the public calls above on a fresh context whenever every mid-end trajectory is shorter than 300 s
+ *   (the only case where step 5 differs from what the public calls can express: there, a group inherits the durations the group before
+ *   it left).
+ * Outputs:
+ *   paths       path_off (B + 1) and path_xyz (cap_nodes x 3) in the layout of isdf_frontend_path_batch (a NO_PATH plan has its one-node
+ *               path); either may be NULL (path_xyz NULL: cap_nodes is ignored).
+ *   trajectories plan b's pieces are [piece_off[b], piece_off[b+1]) (0 pieces for NO_PATH and TOO_LONG): T[piece_off[b] + i], and its own
+ *               6N x 3 column-major block at coeffs + 18 * piece_off[b] (cap_pieces pieces in all).
+ *   results     B records: stage, path_nodes, pieces (N; 0 for NO_PATH), obstacle_points (0 for plans that did not reach the back end),
+ *               midend_ret / backend_ret / backend_iterations / backend_evaluations (0 where the stage did not run), path_cost (the front
+ *               end's cost, +inf for NO_PATH), midend_f / backend_f (NaN where the stage did not run), duration (total of the returned
+ *               trajectory, 0 without one).
+ *   certify / dynamics  B summaries each (may be NULL when the flag is off); a plan without a trajectory gets the failed-call summary of
+ *               its certificate.
+ *   Caps too small: after the front end and the waypoints the call returns ISDF_ERR_INVALID; path_off and piece_off give the sizes needed.
+ * State the call leaves behind: both obstacle point sets given up and the batched swept-volume term off (also after a failure past the
+ *   argument checks); isdf_get_batch_trajectories returns the last group's final trajectories, and the swept-volume t* and per-problem
+ *   durations are whatever the last group left; isdf_stats.kernel_launches counts every launch of the call, the other isdf_stats fields
+ *   are whatever the last back-end callback left.
+ * Device memory: owned by the context, grown on demand. Between stages only the path lengths, the plans' waypoints, the rounds' 4-byte
+ *   reads and the results cross to the host.
+ * Errors: ISDF_ERR_STATE without a map, a shape or front-end kernels; ISDF_ERR_UNSUPPORTED on a sharded context and for ISDF_PLAN_CERTIFY
+ *   with a shape the certificate refuses (checked before any work); ISDF_ERR_INVALID for a NULL argument, B < 1, the stages' own parameter
+ *   checks, unknown flags, a non-zero reserved_, pieces_per_traj != 0 in p->certify or p->dynamics, a start or goal outside the map, or
+ *   caps too small. On failure every stage is -1, midend_f / backend_f are NaN, and the summaries read as their certificates' failures. */
+typedef enum isdf_plan_flags { ISDF_PLAN_CERTIFY = 1, ISDF_PLAN_DYNAMICS = 2 } isdf_plan_flags;
+typedef enum isdf_plan_stage {
+    ISDF_PLAN_FAILED = -1, ISDF_PLAN_NO_PATH = 0, ISDF_PLAN_TOO_LONG = 1, ISDF_PLAN_MIDEND_FAILED = 2, ISDF_PLAN_OPTIMISED = 3
+} isdf_plan_stage;
+typedef struct isdf_plan_params {
+    double parlength;               /* traj_parlength, 3.0 (plan_manager.cpp:153); finite, > 0 */
+    double half_extent;             /* gather half extent; default kernel_size * occupancy_resolution / 3 (:135, :243); finite, >= 0 */
+    double offset[3];               /* offsetAABBbox (config.hpp:146, default 0); finite */
+    double rho;                     /* back-end time weight, yaml rho 20; finite */
+    isdf_midend_params midend;      /* isdf_midend_default_params */
+    isdf_lbfgs_params backend;      /* isdf_lbfgs_default_params with max_iterations 10000 */
+    int32_t flags;                  /* isdf_plan_flags */
+    int32_t reserved_;              /* must be 0 */
+    isdf_certify_params certify;    /* pieces_per_traj must be 0: the call sets N0 = N per group */
+    isdf_dynamics_params dynamics;  /* likewise */
+} isdf_plan_params;
+typedef struct isdf_plan_result {
+    int32_t stage;                  /* isdf_plan_stage */
+    int32_t path_nodes, pieces, obstacle_points;
+    int32_t midend_ret, backend_ret, backend_iterations, backend_evaluations;
+    double path_cost, midend_f, backend_f, duration;
+} isdf_plan_result;
+typedef struct isdf_plan_info {     /* the last isdf_plan_batch call */
+    int32_t groups, backend_rounds;  /* distinct N that reached the mid-end; batched back-end evaluations summed over groups */
+    double frontend_ms, midend_ms, gather_ms, backend_ms, certify_ms, dynamics_ms;   /* CUDA events on the call's stream */
+} isdf_plan_info;
+/* the values above, flags ISDF_PLAN_CERTIFY | ISDF_PLAN_DYNAMICS, isdf_certify_default_params and isdf_dynamics_default_params(ctx);
+ * ctx may be NULL (isdf_default_config's values) */
+int isdf_plan_default_params(isdf_ctx *ctx, isdf_plan_params *p);
+int isdf_plan_batch(isdf_ctx *ctx, const double *start, int B, const double *goals, const isdf_plan_params *p,
+                    int cap_nodes, int32_t *path_off, double *path_xyz,
+                    int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
+                    isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics);
+int isdf_get_plan_info(isdf_ctx *ctx, isdf_plan_info *out);
 
 /* ---- swept-volume term: addSaftyPenaOnSweptVolumeParallel (hpp:557-649) + getSDFofSweptVolume (swm:710-747) --- */
 /* parallel_points (plan_manager.cpp:246-254): P x 3 row-major world-frame voxel centres; resets lastTstar to 0 (not the persisted
