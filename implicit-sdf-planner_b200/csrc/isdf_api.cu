@@ -58,22 +58,61 @@ static int minco_fits(int N0) {
     return 0;
 }
 
-// The MINCO forward / adjoint workspace (isdf_minco.cuh) of one batched optimiser: B problems of N0 pieces.
+// The problems of a batched call and where their pieces lie. Uniform (the entry points that take B, N0): problem b owns pieces
+// [b N0, b N0 + N0) and no offsets exist. Ragged (the *_ragged entry points, include/isdf.h): problem b owns pieces [piece_off[b], piece_off[b+1])
+// and decision-vector rows [4 piece_off[b] - 3 b, 4 piece_off[b+1] - 3 (b+1)); both offset arrays live on the device.
+struct Layout {
+    int B = 0, N = 0;                                  // problems; the most pieces of one problem (sizes shared memory and grids)
+    size_t P = 0, X = 0;                               // pieces; decision-vector rows
+    const int *d_off = nullptr, *d_xoff = nullptr;     // B + 1 piece and B + 1 decision-vector offsets on the device (null: uniform)
+};
+static Layout uniform_layout(int B, int N0) {
+    Layout L;
+    L.B = B; L.N = N0; L.P = (size_t)B * N0; L.X = (size_t)B * (4 * (size_t)N0 - 3);
+    return L;
+}
+// a ragged batch's offsets (host): the sizes into *L; the device offsets come from ragged_upload
+static int ragged_check(int B, const int32_t *piece_off, Layout *L) {
+    if (B < 1) return fail(ISDF_ERR_INVALID, "B < 1");
+    if (!piece_off) return fail(ISDF_ERR_INVALID, "piece_off is NULL");
+    if (piece_off[0] != 0) return fail(ISDF_ERR_INVALID, "piece_off[0] must be 0");
+    int N = 0;
+    for (int b = 0; b < B; b++) {
+        if (piece_off[b + 1] <= piece_off[b]) return fail(ISDF_ERR_INVALID, "every problem needs at least one piece (piece_off must increase)");
+        N = std::max(N, piece_off[b + 1] - piece_off[b]);
+    }
+    const size_t P = (size_t)piece_off[B], X = 4 * P - 3 * (size_t)B;
+    if (X > 0x7fffffffull) return fail(ISDF_ERR_INVALID, "4*P - 3*B overflows");
+    L->B = B; L->N = N; L->P = P; L->X = X;
+    return 0;
+}
+// the device offsets of a checked ragged batch, staged in buf on st: [piece offsets | decision-vector offsets]
+static int ragged_upload(DevBuf<int> &buf, const int32_t *piece_off, cudaStream_t st, Layout *L) {
+    const int B = L->B;
+    std::vector<int> h(2 * (size_t)B + 2);
+    for (int b = 0; b <= B; b++) { h[b] = piece_off[b]; h[(size_t)B + 1 + b] = 4 * piece_off[b] - 3 * b; }
+    CU_TRY(buf.upload(h.data(), h.size(), st));
+    CU_TRY(cudaStreamSynchronize(st));
+    L->d_off = buf.p; L->d_xoff = buf.p + B + 1;
+    return 0;
+}
+
+// The MINCO forward / adjoint workspace (isdf_minco.cuh) of one batched optimiser: the problems of a Layout.
 struct MincoWork {
     DevBuf<double> d_T, d_C, d_lu, d_energy, d_gC, d_gT, d_out;
-    int ensure(int B, int N0) {
-        if (int r = minco_fits(N0)) return r;
-        const size_t BN = (size_t)B * N0, smem = minco_smem_bytes(N0);
-        CU_TRY(d_T.ensure(BN)); CU_TRY(d_C.ensure(18 * BN)); CU_TRY(d_lu.ensure(78 * BN)); CU_TRY(d_energy.ensure(B));
+    int ensure(const Layout &L) {
+        if (int r = minco_fits(L.N)) return r;
+        const size_t BN = L.P, smem = minco_smem_bytes(L.N);
+        CU_TRY(d_T.ensure(BN)); CU_TRY(d_C.ensure(18 * BN)); CU_TRY(d_lu.ensure(78 * BN)); CU_TRY(d_energy.ensure(L.B));
         CU_TRY(d_gC.ensure(18 * BN)); CU_TRY(d_gT.ensure(BN)); CU_TRY(d_out.ensure(19 * BN + 1));
         CU_TRY(cudaFuncSetAttribute(k_minco_forward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         CU_TRY(cudaFuncSetAttribute(k_minco_backward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         return 0;
     }
     // the workspace's part of the arguments; the terms (swept volume, discrete output, cost and gradient) are the caller's
-    MincoArgs args(int B, int N0, const double *head, const double *tail, int bc_stride, double rho, const double *x) {
+    MincoArgs args(const Layout &L, const double *head, const double *tail, int bc_stride, double rho, const double *x) {
         MincoArgs M = {};
-        M.B = B; M.N = N0; M.x = x; M.head = head; M.tail = tail; M.bc_stride = bc_stride; M.rho = rho;
+        M.B = L.B; M.N = L.N; M.P = (int)L.P; M.poff = L.d_off; M.x = x; M.head = head; M.tail = tail; M.bc_stride = bc_stride; M.rho = rho;
         M.T = d_T.p; M.C = d_C.p; M.lu = d_lu.p; M.energy = d_energy.p; M.gC_e = d_gC.p; M.gT_e = d_gT.p;
         return M;
     }
@@ -146,7 +185,9 @@ struct isdf_ctx {
     struct {   // batched callback (isdf_minco.cuh); B = 0: none evaluated yet
         MincoWork minco;
         DevBuf<double> d_x, d_bc, d_cost, d_grad, d_Cpp, d_sv;
-        int B = 0, N0 = 0;
+        DevBuf<int> d_off;   // a ragged batch's offsets (ragged_upload)
+        int B = 0;
+        size_t P = 0;        // problems and pieces of the last evaluation
     } batch;
     struct LbfgsBufs {   // device-resident lock-step L-BFGS (isdf_lbfgs.cuh)
         DevBuf<double> d_x, d_f, d_grad, d_state; DevBuf<int> d_int, d_head;
@@ -155,6 +196,7 @@ struct isdf_ctx {
     struct {   // mid-end (isdf_midend.cuh): buffers of its own, so that no mid-end call touches the back end's batch, swept or L-BFGS state
         MincoWork minco;
         DevBuf<double> d_x, d_bc, d_wp, d_pc, d_cost, d_grad;
+        DevBuf<int> d_off;   // a ragged batch's offsets (ragged_upload)
         LbfgsBufs lb;
     } mid;
     SweptState sv;   // swept volume
@@ -1364,13 +1406,14 @@ extern "C" int isdf_get_piece_costs(isdf_ctx *c, double *piece_cost, int n) {
 }
 
 // ---- batched optimiser callback on the device (MINCO -> time-integral term -> adjoint), SURVEY §8f row 1 ----------------------
-static int callback_batch_launch(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int bc_stride, double rho,
+static int callback_batch_launch(isdf_ctx *c, const Layout &L, const double *d_head, const double *d_tail, int bc_stride, double rho,
                                  const double *d_x, double *d_cost, double *d_grad, cudaStream_t st) {
-    const size_t BN = (size_t)B * N0;
-    if (int r = minco_fits(N0)) return r;
+    const int B = L.B;
+    const size_t BN = L.P;
+    if (int r = minco_fits(L.N)) return r;
     if (BN * (size_t)(c->cfg.integral_intervs + 1) > 0x7fffffffull) return fail(ISDF_ERR_UNSUPPORTED, "batch too large: B*N0*(K+1) must fit in 31 bits");
-    if (int r = c->batch.minco.ensure(B, N0)) return r;
-    MincoArgs M = c->batch.minco.args(B, N0, d_head, d_tail, bc_stride, rho, d_x);
+    if (int r = c->batch.minco.ensure(L)) return r;
+    MincoArgs M = c->batch.minco.args(L, d_head, d_tail, bc_stride, rho, d_x);
     M.cost = d_cost; M.grad = d_grad;
     // per-problem obstacle point sets registered for exactly this batch (isdf_set_points_batch): the LIVE composition of costFunctionLmbm
     // (hpp:386-405) — swept-volume term, then time-integral term
@@ -1378,14 +1421,14 @@ static int callback_batch_launch(isdf_ctx *c, int B, int N0, const double *d_hea
     if (with_swept) {
         if (c->mesh.shape.kind == ISDF_SHAPE_MESH && c->mesh.shape.mesh.sign_mode == MESH_SIGN_WINDING)
             return fail(ISDF_ERR_UNSUPPORTED, "swept-volume term with a winding-sign mesh (see isdf_set_shape_mesh_ex)");
-        CU_TRY(c->batch.d_Cpp.ensure(18 * BN)); CU_TRY(c->batch.d_sv.ensure((size_t)B * (19 * (size_t)N0 + 1)));
+        CU_TRY(c->batch.d_Cpp.ensure(18 * BN)); CU_TRY(c->batch.d_sv.ensure(19 * BN + B));
         M.Cpp = c->batch.d_Cpp.p;
     }
-    const size_t smem = minco_smem_bytes(N0);
+    const size_t smem = minco_smem_bytes(L.N);
     k_minco_forward<<<B, 32, smem, st>>>(M);
     if (with_swept) {
         int launches = 0;
-        cudaError_t e = c->sv.launch_batch(c->dcfg, c->mesh.shape, N0, M.T, M.Cpp, c->batch.d_sv.p, st, &launches);
+        cudaError_t e = c->sv.launch_batch(c->dcfg, c->mesh.shape, L.N, L.d_off, BN, M.T, M.Cpp, c->batch.d_sv.p, st, &launches);
         c->stats.kernel_launches += launches;
         c->stats.evals_swept++;
         if (e != cudaSuccess) return fail(e == cudaErrorInvalidValue ? ISDF_ERR_INVALID : ISDF_ERR_CUDA, std::string("batched swept: ") + cudaGetErrorString(e));
@@ -1396,7 +1439,7 @@ static int callback_batch_launch(isdf_ctx *c, int B, int N0, const double *d_hea
     M.disc_out = c->batch.minco.d_out.p; M.piece_cost = c->disc.d_piece_cost.p;
     k_minco_backward<<<B, 32, smem, st>>>(M);
     c->stats.kernel_launches += 2;
-    c->batch.B = B; c->batch.N0 = N0;
+    c->batch.B = B; c->batch.P = BN;
     CU_TRY(cudaGetLastError());
     return 0;
 }
@@ -1415,7 +1458,26 @@ extern "C" int isdf_callback_batch_device(isdf_ctx *c, int B, int N0, const doub
     if (r) return r;
     if (!d_head || !d_tail || !d_x || !d_cost || !d_grad) return fail(ISDF_ERR_INVALID, "NULL device pointer");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    return callback_batch_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, rho, d_x, d_cost, d_grad, (cudaStream_t)cuda_stream);
+    return callback_batch_launch(c, uniform_layout(B, N0), d_head, d_tail, per_problem_bc ? 9 : 0, rho, d_x, d_cost, d_grad, (cudaStream_t)cuda_stream);
+}
+
+// a ragged batch's checks (callback_batch_check's, with the offsets in place of B, N0) and sizes
+static int callback_ragged_check(isdf_ctx *c, int B, const int32_t *piece_off, Layout *L) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (int r = ragged_check(B, piece_off, L)) return r;
+    if (c->world != 1) return fail(ISDF_ERR_STATE, "the batched callback shards by PROBLEM: keep isdf_set_shard(ctx, 0, 1) and give each rank its own problems");
+    return check_eval_state(c, (int)L->P, true);
+}
+
+extern "C" int isdf_callback_batch_ragged_device(isdf_ctx *c, int B, const int32_t *piece_off, const double *d_head, const double *d_tail,
+                                                 int per_problem_bc, double rho, const double *d_x, double *d_cost, double *d_grad, void *cuda_stream) {
+    Layout L;
+    if (int r = callback_ragged_check(c, B, piece_off, &L)) return r;
+    if (!d_head || !d_tail || !d_x || !d_cost || !d_grad) return fail(ISDF_ERR_INVALID, "NULL device pointer");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    const cudaStream_t st = (cudaStream_t)cuda_stream;
+    if (int r = ragged_upload(c->batch.d_off, piece_off, st, &L)) return r;
+    return callback_batch_launch(c, L, d_head, d_tail, per_problem_bc ? 9 : 0, rho, d_x, d_cost, d_grad, st);
 }
 
 // the host entry points' boundary conditions (9 doubles, or 9 per problem) in buf on c->stream: *d_head, then *d_tail
@@ -1453,6 +1515,30 @@ extern "C" int isdf_callback_batch(isdf_ctx *c, int B, int N0, const double *hea
     }, [&] { nan_fill(cost, B); });
 }
 
+extern "C" int isdf_callback_batch_ragged(isdf_ctx *c, int B, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
+                                          double rho, const double *x, double *cost, double *grad) {
+    return poison_on_failure([&]() -> int {
+        Layout L;
+        if (int r = callback_ragged_check(c, B, piece_off, &L)) return r;
+        if (!head || !tail || !x || !cost || !grad) return fail(ISDF_ERR_INVALID, "NULL argument");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        CU_TRY(c->batch.d_x.upload(x, L.X, c->stream));
+        const double *d_head, *d_tail;
+        if (int r = upload_bc(c, c->batch.d_bc, B, per_problem_bc, head, tail, &d_head, &d_tail)) return r;
+        CU_TRY(c->batch.d_cost.ensure(B)); CU_TRY(c->batch.d_grad.ensure(L.X));
+        CU_TRY(cudaEventRecord(c->ev0, c->stream));
+        if (int r = isdf_callback_batch_ragged_device(c, B, piece_off, d_head, d_tail, per_problem_bc, rho, c->batch.d_x.p, c->batch.d_cost.p,
+                                                      c->batch.d_grad.p, c->stream)) return r;
+        CU_TRY(cudaEventRecord(c->ev1, c->stream));
+        CU_TRY(cudaMemcpyAsync(cost, c->batch.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaMemcpyAsync(grad, c->batch.d_grad.p, sizeof(double) * L.X, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaStreamSynchronize(c->stream));
+        float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
+        c->stats.last_kernel_ms = ms;
+        return 0;
+    }, [&] { nan_fill(cost, B); });
+}
+
 // ---- device-resident lock-step L-BFGS over the batched callback (SURVEY §8f row 2; isdf_lbfgs.cuh) ----------------------------------------
 static int lbfgs_check(const isdf_lbfgs_params *p) {
     if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
@@ -1474,27 +1560,29 @@ extern "C" int isdf_lbfgs_default_params(isdf_lbfgs_params *p) {
 // The lock-step rounds of isdf_lbfgs_batch_device and isdf_midend_batch_device: every round `eval(d_x, d_f, d_grad)` evaluates the point
 // every instance requested (finished instances ride along unchanged: their state is frozen), then one k_lbfgs_feed consumes the results.
 // d_x: B x n (in: starting points, out: solutions); d_f: B; d_ret / d_iterations / d_evaluations: B ints (any of the three may be null).
-// Synchronous with respect to the host (one 4-byte read per round decides termination), all data stays on the device.
+// d_xoff (device, B + 1; may be null): instance b has rows [d_xoff[b], d_xoff[b+1]) of X in all, as a ragged batch's decision vectors; null:
+// every instance has n rows, X = B n. Synchronous with respect to the host (one 4-byte read per round decides termination), all data stays
+// on the device.
 template <typename Eval>
-static int lbfgs_rounds(isdf_ctx *c, isdf_ctx::LbfgsBufs &lb, int B, int n, const isdf_lbfgs_params *prm, int cancel_after, double *d_x, double *d_f,
-                        int *d_ret, int *d_iterations, int *d_evaluations, int *rounds_out, cudaStream_t st, Eval eval) {
+static int lbfgs_rounds(isdf_ctx *c, isdf_ctx::LbfgsBufs &lb, int B, int n, const int *d_xoff, size_t X, const isdf_lbfgs_params *prm, int cancel_after,
+                        double *d_x, double *d_f, int *d_ret, int *d_iterations, int *d_evaluations, int *rounds_out, cudaStream_t st, Eval eval) {
     const int m = prm->mem_size, npf = prm->past > 1 ? prm->past : 1;
-    const size_t per = (size_t)4 * n + npf + 2 * (size_t)m + 2 * (size_t)m * n + LB_NSCALAR;   // doubles of state per instance
-    CU_TRY(lb.d_state.ensure(per * B)); CU_TRY(lb.d_grad.ensure((size_t)B * n)); CU_TRY(lb.d_int.ensure((size_t)B * LB_NINT + 4));
+    const size_t total = 4 * X + (size_t)B * (npf + 2 * (size_t)m + LB_NSCALAR) + 2 * (size_t)m * X;   // doubles of state
+    CU_TRY(lb.d_state.ensure(total)); CU_TRY(lb.d_grad.ensure(X)); CU_TRY(lb.d_int.ensure((size_t)B * LB_NINT + 4));
     CU_TRY(lb.h_active.ensure(1));
-    CU_TRY(cudaMemsetAsync(lb.d_state.p, 0, sizeof(double) * per * B, st));
+    CU_TRY(cudaMemsetAsync(lb.d_state.p, 0, sizeof(double) * total, st));
     CU_TRY(cudaMemsetAsync(lb.d_int.p, 0, sizeof(int) * ((size_t)B * LB_NINT + 4), st));   // phase = WANT_INIT
     LbfgsArgs L;
-    L.B = B; L.n = n;
+    L.B = B; L.n = n; L.xoff = d_xoff;
     L.pr.mem_size = m; L.pr.past = prm->past; L.pr.max_iterations = prm->max_iterations; L.pr.max_linesearch = prm->max_linesearch;
     L.pr.g_epsilon = prm->g_epsilon; L.pr.delta = prm->delta; L.pr.min_step = prm->min_step; L.pr.max_step = prm->max_step;
     L.pr.f_dec_coeff = prm->f_dec_coeff; L.pr.cautious_factor = prm->cautious_factor; L.pr.machine_prec = prm->machine_prec;
     L.pr.cancel_after = cancel_after;
     double *p = lb.d_state.p;
     L.x = d_x; L.f = d_f; L.grad = lb.d_grad.p;
-    L.xp = p; p += (size_t)B * n; L.g = p; p += (size_t)B * n; L.gp = p; p += (size_t)B * n; L.d = p; p += (size_t)B * n;
+    L.xp = p; p += X; L.g = p; p += X; L.gp = p; p += X; L.d = p; p += X;
     L.pf = p; p += (size_t)B * npf; L.alpha = p; p += (size_t)B * m; L.ys = p; p += (size_t)B * m;
-    L.S = p; p += (size_t)B * m * n; L.Y = p; p += (size_t)B * m * n; L.sc = p;
+    L.S = p; p += (size_t)m * X; L.Y = p; p += (size_t)m * X; L.sc = p;
     L.st = lb.d_int.p; L.active = lb.d_int.p + (size_t)B * LB_NINT;
     // olddnorm starts at 1 (lbfgs.hpp:541): scalar slot 2 of every instance
     {
@@ -1535,9 +1623,9 @@ static void nan_fill_device(isdf_ctx *c, double *d, int n, cudaStream_t st) {
     if (c && d && n > 0 && cudaSetDevice(c->device) == cudaSuccess) { cudaMemsetAsync(d, 0xff, sizeof(double) * n, st); cudaStreamSynchronize(st); }
 }
 
-// an L-BFGS call's results in lb to the host: x (B x n), f, and ret / iterations / evaluations from the d_head triple (each may be NULL)
-static int lbfgs_copy_out(const isdf_ctx::LbfgsBufs &lb, int B, size_t n, double *x, double *f, int *ret, int *iterations, int *evaluations) {
-    CU_TRY(cudaMemcpy(x, lb.d_x.p, sizeof(double) * n * B, cudaMemcpyDeviceToHost));
+// an L-BFGS call's results in lb to the host: x (X rows), f, and ret / iterations / evaluations from the d_head triple (each may be NULL)
+static int lbfgs_copy_out(const isdf_ctx::LbfgsBufs &lb, int B, size_t X, double *x, double *f, int *ret, int *iterations, int *evaluations) {
+    CU_TRY(cudaMemcpy(x, lb.d_x.p, sizeof(double) * X, cudaMemcpyDeviceToHost));
     CU_TRY(cudaMemcpy(f, lb.d_f.p, sizeof(double) * B, cudaMemcpyDeviceToHost));
     if (ret) CU_TRY(cudaMemcpy(ret, lb.d_head.p, sizeof(int) * B, cudaMemcpyDeviceToHost));
     if (iterations) CU_TRY(cudaMemcpy(iterations, lb.d_head.p + B, sizeof(int) * B, cudaMemcpyDeviceToHost));
@@ -1554,9 +1642,28 @@ extern "C" int isdf_lbfgs_batch_device(isdf_ctx *c, int B, int N0, const double 
         if (int r = lbfgs_check(prm)) return r;
         if (!d_head || !d_tail || !d_x || !d_f) return fail(ISDF_ERR_INVALID, "NULL device pointer");
         if (set_device(c)) return ISDF_ERR_CUDA;
-        return lbfgs_rounds(c, c->lbfgs, B, 4 * N0 - 3, prm, 0, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st,
+        const Layout L = uniform_layout(B, N0);
+        return lbfgs_rounds(c, c->lbfgs, B, 4 * N0 - 3, nullptr, L.X, prm, 0, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st,
                             [&](const double *x, double *f, double *g) {
-                                return callback_batch_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, rho, x, f, g, st);
+                                return callback_batch_launch(c, L, d_head, d_tail, per_problem_bc ? 9 : 0, rho, x, f, g, st);
+                            });
+    }, [&] { nan_fill_device(c, d_f, B, st); });
+}
+
+extern "C" int isdf_lbfgs_batch_ragged_device(isdf_ctx *c, int B, const int32_t *piece_off, const double *d_head, const double *d_tail,
+                                              int per_problem_bc, double rho, const isdf_lbfgs_params *prm, double *d_x, double *d_f, int *d_ret,
+                                              int *d_iterations, int *d_evaluations, int *rounds_out, void *cuda_stream) {
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    return poison_on_failure([&]() -> int {
+        Layout L;
+        if (int r = callback_ragged_check(c, B, piece_off, &L)) return r;
+        if (int r = lbfgs_check(prm)) return r;
+        if (!d_head || !d_tail || !d_x || !d_f) return fail(ISDF_ERR_INVALID, "NULL device pointer");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        if (int r = ragged_upload(c->batch.d_off, piece_off, st, &L)) return r;
+        return lbfgs_rounds(c, c->lbfgs, B, 4 * L.N - 3, L.d_xoff, L.X, prm, 0, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st,
+                            [&](const double *x, double *f, double *g) {
+                                return callback_batch_launch(c, L, d_head, d_tail, per_problem_bc ? 9 : 0, rho, x, f, g, st);
                             });
     }, [&] { nan_fill_device(c, d_f, B, st); });
 }
@@ -1575,7 +1682,26 @@ extern "C" int isdf_lbfgs_batch(isdf_ctx *c, int B, int N0, const double *head, 
         CU_TRY(lb.d_f.ensure(B)); CU_TRY(lb.d_head.ensure((size_t)3 * B));
         if (int r = isdf_lbfgs_batch_device(c, B, N0, d_head, d_tail, per_problem_bc, rho, prm, lb.d_x.p, lb.d_f.p, lb.d_head.p, lb.d_head.p + B,
                                             lb.d_head.p + 2 * (size_t)B, rounds_out, c->stream)) return r;
-        return lbfgs_copy_out(lb, B, n, x, f, ret, iterations, evaluations);
+        return lbfgs_copy_out(lb, B, n * B, x, f, ret, iterations, evaluations);
+    }, [&] { nan_fill(f, B); });
+}
+
+extern "C" int isdf_lbfgs_batch_ragged(isdf_ctx *c, int B, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
+                                       double rho, const isdf_lbfgs_params *prm, double *x, double *f, int *ret, int *iterations, int *evaluations,
+                                       int *rounds_out) {
+    return poison_on_failure([&]() -> int {
+        Layout L;
+        if (int r = callback_ragged_check(c, B, piece_off, &L)) return r;
+        if (!head || !tail || !x || !f) return fail(ISDF_ERR_INVALID, "NULL argument");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        isdf_ctx::LbfgsBufs &lb = c->lbfgs;
+        CU_TRY(lb.d_x.upload(x, L.X, c->stream));
+        const double *d_head, *d_tail;
+        if (int r = upload_bc(c, c->batch.d_bc, B, per_problem_bc, head, tail, &d_head, &d_tail)) return r;
+        CU_TRY(lb.d_f.ensure(B)); CU_TRY(lb.d_head.ensure((size_t)3 * B));
+        if (int r = isdf_lbfgs_batch_ragged_device(c, B, piece_off, d_head, d_tail, per_problem_bc, rho, prm, lb.d_x.p, lb.d_f.p, lb.d_head.p,
+                                                   lb.d_head.p + B, lb.d_head.p + 2 * (size_t)B, rounds_out, c->stream)) return r;
+        return lbfgs_copy_out(lb, B, L.X, x, f, ret, iterations, evaluations);
     }, [&] { nan_fill(f, B); });
 }
 
@@ -1596,7 +1722,7 @@ extern "C" int isdf_dbg_lbfgs_rounds(isdf_ctx *c, int B, int n, const isdf_lbfgs
     CU_TRY(lb.d_x.upload(x, bn, c->stream));
     CU_TRY(lb.d_f.ensure(B)); CU_TRY(lb.d_head.ensure((size_t)3 * B));
     std::vector<double> hx(bn), hf(B), hg(bn);
-    int r = lbfgs_rounds(c, lb, B, n, prm, cancel_after, lb.d_x.p, lb.d_f.p, lb.d_head.p, lb.d_head.p + B, lb.d_head.p + 2 * (size_t)B, rounds_out, c->stream,
+    int r = lbfgs_rounds(c, lb, B, n, nullptr, bn, prm, cancel_after, lb.d_x.p, lb.d_f.p, lb.d_head.p, lb.d_head.p + B, lb.d_head.p + 2 * (size_t)B, rounds_out, c->stream,
                          [&](const double *d_x, double *d_f, double *d_g) -> int {
                              CU_TRY(cudaMemcpyAsync(hx.data(), d_x, sizeof(double) * bn, cudaMemcpyDeviceToHost, c->stream));
                              CU_TRY(cudaStreamSynchronize(c->stream));
@@ -1607,14 +1733,14 @@ extern "C" int isdf_dbg_lbfgs_rounds(isdf_ctx *c, int B, int n, const isdf_lbfgs
                              return 0;
                          });
     if (r) return r;
-    return lbfgs_copy_out(lb, B, (size_t)n, x, f, ret, iterations, evaluations);
+    return lbfgs_copy_out(lb, B, bn, x, f, ret, iterations, evaluations);
 }
 
 extern "C" int isdf_get_batch_trajectories(isdf_ctx *c, double *T, double *coeffs, double *energy) {
     if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
     if (c->batch.B <= 0) return fail(ISDF_ERR_STATE, "no batched callback evaluated yet");
     if (int r = sync_ctx(c)) return r;
-    const size_t BN = (size_t)c->batch.B * c->batch.N0;
+    const size_t BN = c->batch.P;
     const MincoWork &w = c->batch.minco;
     if (T) CU_TRY(cudaMemcpy(T, w.d_T.p, sizeof(double) * BN, cudaMemcpyDeviceToHost));
     if (coeffs) CU_TRY(cudaMemcpy(coeffs, w.d_C.p, sizeof(double) * 18 * BN, cudaMemcpyDeviceToHost));
@@ -1661,42 +1787,58 @@ extern "C" int isdf_midend_default_params(isdf_midend_params *p) {
     return 0;
 }
 
-static int midend_check(isdf_ctx *c, int B, int N0, const isdf_midend_params *p) {
-    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
-    if (B < 1 || N0 < 1) return fail(ISDF_ERR_INVALID, "B < 1 or N0 < 1");
-    if ((long long)B * (4 * (long long)N0 - 3) > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "B*(4*N0-3) overflows");
+// the mid-end parameters' checks, in the order of midend_check
+static int midend_params_check(const isdf_midend_params *p) {
     if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
     if (p->reserved_ != 0) return fail(ISDF_ERR_INVALID, "reserved_ must be 0");
     if (!(std::isfinite(p->weight_pr) && p->weight_pr >= 0.0) || !std::isfinite(p->rho) || !(std::isfinite(p->init_time) && p->init_time > 0.0) ||
         p->cancel_after < 0)
         return fail(ISDF_ERR_INVALID, "mid-end parameter out of range");
-    if (int r = lbfgs_check(&p->lbfgs)) return r;
+    return lbfgs_check(&p->lbfgs);
+}
+
+static int midend_check(isdf_ctx *c, int B, int N0, const isdf_midend_params *p) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (B < 1 || N0 < 1) return fail(ISDF_ERR_INVALID, "B < 1 or N0 < 1");
+    if ((long long)B * (4 * (long long)N0 - 3) > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "B*(4*N0-3) overflows");
+    if (int r = midend_params_check(p)) return r;
     if (int r = minco_fits(N0)) return r;
     if (c->world != 1) return fail(ISDF_ERR_STATE, "the mid-end shards by PROBLEM: keep isdf_set_shard(ctx, 0, 1) and give each rank its own problems");
     return 0;
 }
 
-static int midend_buffers(isdf_ctx *c, int B, int N0) {
-    if (int r = c->mid.minco.ensure(B, N0)) return r;
-    CU_TRY(c->mid.d_pc.ensure((size_t)B * N0));
+// midend_check for a ragged batch (the offsets in place of B, N0), and its sizes
+static int midend_ragged_check(isdf_ctx *c, int B, const int32_t *piece_off, const isdf_midend_params *p, Layout *L) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (int r = ragged_check(B, piece_off, L)) return r;
+    if (int r = midend_params_check(p)) return r;
+    if (int r = minco_fits(L->N)) return r;
+    if (c->world != 1) return fail(ISDF_ERR_STATE, "the mid-end shards by PROBLEM: keep isdf_set_shard(ctx, 0, 1) and give each rank its own problems");
     return 0;
 }
 
-static MincoArgs midend_minco_args(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int bc_stride, double rho, const double *d_x) {
-    MincoArgs M = c->mid.minco.args(B, N0, d_head, d_tail, bc_stride, rho, d_x);
+static int midend_buffers(isdf_ctx *c, const Layout &L) {
+    if (int r = c->mid.minco.ensure(L)) return r;
+    CU_TRY(c->mid.d_pc.ensure(L.P));
+    return 0;
+}
+
+static MincoArgs midend_minco_args(isdf_ctx *c, const Layout &L, const double *d_head, const double *d_tail, int bc_stride, double rho, const double *d_x) {
+    MincoArgs M = c->mid.minco.args(L, d_head, d_tail, bc_stride, rho, d_x);
     M.disc_out = c->mid.minco.d_out.p; M.piece_cost = c->mid.d_pc.p; M.seq_terms = 1;
     return M;
 }
 
 // one evaluation of OriTraj::costFunction for all B problems: MINCO forward -> pose term -> adjoint with the terms added one at a time
-static int midend_eval_launch(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int bc_stride, const isdf_midend_params *p,
+static int midend_eval_launch(isdf_ctx *c, const Layout &L, const double *d_head, const double *d_tail, int bc_stride, const isdf_midend_params *p,
                               const double *d_wp, const double *d_x, double *d_cost, double *d_grad, cudaStream_t st) {
-    const size_t BN = (size_t)B * N0, smem = minco_smem_bytes(N0);
-    MincoArgs M = midend_minco_args(c, B, N0, d_head, d_tail, bc_stride, p->rho, d_x);
+    const int B = L.B;
+    const size_t BN = L.P, smem = minco_smem_bytes(L.N);
+    MincoArgs M = midend_minco_args(c, L, d_head, d_tail, bc_stride, p->rho, d_x);
     M.cost = d_cost; M.grad = d_grad;
     k_minco_forward<<<B, 32, smem, st>>>(M);
     MidendArgs P;
-    P.B = B; P.N = N0; P.K = c->cfg.integral_intervs; P.weight = p->weight_pr; P.T = M.T; P.C = M.C; P.wp = d_wp; P.out = c->mid.minco.d_out.p; P.piece_cost = c->mid.d_pc.p;
+    P.B = B; P.N = L.N; P.P = (int)BN; P.poff = L.d_off; P.K = c->cfg.integral_intervs; P.weight = p->weight_pr; P.T = M.T; P.C = M.C; P.wp = d_wp; P.out = c->mid.minco.d_out.p; P.piece_cost = c->mid.d_pc.p;
     k_midend_pose<<<(unsigned)((BN + 127) / 128), 128, 0, st>>>(P);
     k_minco_backward<<<B, 32, smem, st>>>(M);
     c->stats.kernel_launches += 3;
@@ -1705,13 +1847,30 @@ static int midend_eval_launch(isdf_ctx *c, int B, int N0, const double *d_head, 
 }
 
 // the mid-end's host entry points stage their inputs in c->mid: boundary conditions (*d_head, *d_tail) and waypoints
-static int midend_upload(isdf_ctx *c, int B, int N0, int per_problem_bc, const double *head, const double *tail, const double *waypoints,
+static int midend_upload(isdf_ctx *c, const Layout &L, int per_problem_bc, const double *head, const double *tail, const double *waypoints,
                          const double **d_head, const double **d_tail, const double **d_wp) {
-    const size_t nwp = (size_t)3 * B * (N0 - 1);
+    const int B = L.B;
+    const size_t nwp = 3 * (L.P - B);
     if (int r = upload_bc(c, c->mid.d_bc, B, per_problem_bc, head, tail, d_head, d_tail)) return r;
     CU_TRY(c->mid.d_wp.ensure(nwp > 0 ? nwp : 1));
     if (nwp) CU_TRY(cudaMemcpyAsync(c->mid.d_wp.p, waypoints, sizeof(double) * nwp, cudaMemcpyHostToDevice, c->stream));
     *d_wp = c->mid.d_wp.p;
+    return 0;
+}
+
+// the host form of one mid-end evaluation of a checked batch
+static int midend_callback_run(isdf_ctx *c, const Layout &L, int per_problem_bc, const isdf_midend_params *p, const double *head, const double *tail,
+                               const double *waypoints, const double *x, double *cost, double *grad) {
+    const int B = L.B;
+    const double *d_head, *d_tail, *d_wp;
+    if (int r = midend_upload(c, L, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return r;
+    CU_TRY(c->mid.d_x.upload(x, L.X, c->stream));
+    CU_TRY(c->mid.d_cost.ensure(B)); CU_TRY(c->mid.d_grad.ensure(L.X));
+    if (int r = midend_buffers(c, L)) return r;
+    if (int r = midend_eval_launch(c, L, d_head, d_tail, per_problem_bc ? 9 : 0, p, d_wp, c->mid.d_x.p, c->mid.d_cost.p, c->mid.d_grad.p, c->stream)) return r;
+    CU_TRY(cudaMemcpyAsync(cost, c->mid.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(cudaMemcpyAsync(grad, c->mid.d_grad.p, sizeof(double) * L.X, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(cudaStreamSynchronize(c->stream));
     return 0;
 }
 
@@ -1721,40 +1880,43 @@ extern "C" int isdf_midend_callback_batch(isdf_ctx *c, int B, int N0, const doub
         if (int r = midend_check(c, B, N0, p)) return r;
         if (!head || !tail || !x || !cost || !grad || (N0 > 1 && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
-        const size_t dim = (size_t)4 * N0 - 3;
-        const double *d_head, *d_tail, *d_wp;
-        if (int r = midend_upload(c, B, N0, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return r;
-        CU_TRY(c->mid.d_x.upload(x, dim * B, c->stream));
-        CU_TRY(c->mid.d_cost.ensure(B)); CU_TRY(c->mid.d_grad.ensure(dim * B));
-        if (int r = midend_buffers(c, B, N0)) return r;
-        if (int r = midend_eval_launch(c, B, N0, d_head, d_tail, per_problem_bc ? 9 : 0, p, d_wp, c->mid.d_x.p, c->mid.d_cost.p, c->mid.d_grad.p, c->stream)) return r;
-        CU_TRY(cudaMemcpyAsync(cost, c->mid.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaMemcpyAsync(grad, c->mid.d_grad.p, sizeof(double) * dim * B, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaStreamSynchronize(c->stream));
-        return 0;
+        return midend_callback_run(c, uniform_layout(B, N0), per_problem_bc, p, head, tail, waypoints, x, cost, grad);
     }, [&] { nan_fill(cost, B); });
 }
 
-static int midend_batch_run(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc, const isdf_midend_params *p,
+extern "C" int isdf_midend_callback_batch_ragged(isdf_ctx *c, int B, const int32_t *piece_off, const double *head, const double *tail,
+                                                 int per_problem_bc, const isdf_midend_params *p, const double *waypoints, const double *x,
+                                                 double *cost, double *grad) {
+    return poison_on_failure([&]() -> int {
+        Layout L;
+        if (int r = midend_ragged_check(c, B, piece_off, p, &L)) return r;
+        if (!head || !tail || !x || !cost || !grad || (L.P > (size_t)B && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        if (int r = ragged_upload(c->mid.d_off, piece_off, c->stream, &L)) return r;
+        return midend_callback_run(c, L, per_problem_bc, p, head, tail, waypoints, x, cost, grad);
+    }, [&] { nan_fill(cost, B); });
+}
+
+static int midend_batch_run(isdf_ctx *c, const Layout &L, const double *d_head, const double *d_tail, int per_problem_bc, const isdf_midend_params *p,
                             const double *d_wp, double *d_x, double *d_T, double *d_coeffs, double *d_f, int *d_ret, int *d_iterations,
                             int *d_evaluations, int *rounds_out, cudaStream_t st) {
     if (set_device(c)) return ISDF_ERR_CUDA;
-    const int n = 4 * N0 - 3;
-    const size_t BN = (size_t)B * N0;
-    if (int r = midend_buffers(c, B, N0)) return r;
+    const int B = L.B, n = 4 * L.N - 3;
+    const size_t BN = L.P;
+    if (int r = midend_buffers(c, L)) return r;
     // x = [backwardT(init_time) | waypoints] (mid_end.cpp:21-36; backwardT as back_end_optimizer.hpp:243-256)
     const double T0 = p->init_time, tau0 = T0 > 1.0 ? (std::sqrt(2.0 * T0 - 1.0) - 1.0) : (1.0 - std::sqrt(2.0 / T0 - 1.0));
-    k_midend_init<<<(unsigned)(((size_t)B * n + 127) / 128), 128, 0, st>>>(B, N0, tau0, d_wp, d_x);
+    k_midend_init<<<(unsigned)((L.X + 127) / 128), 128, 0, st>>>(B, L.N, L.d_off, L.d_xoff, (long long)L.X, tau0, d_wp, d_x);
     c->stats.kernel_launches++;
     CU_TRY(cudaGetLastError());
     const int bc_stride = per_problem_bc ? 9 : 0;
-    int r = lbfgs_rounds(c, c->mid.lb, B, n, &p->lbfgs, p->cancel_after, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st,
-                         [&](const double *x, double *f, double *g) { return midend_eval_launch(c, B, N0, d_head, d_tail, bc_stride, p, d_wp, x, f, g, st); });
+    int r = lbfgs_rounds(c, c->mid.lb, B, n, L.d_xoff, L.X, &p->lbfgs, p->cancel_after, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st,
+                         [&](const double *x, double *f, double *g) { return midend_eval_launch(c, L, d_head, d_tail, bc_stride, p, d_wp, x, f, g, st); });
     if (r) return r;
     // the final trajectories: forwardT + MINCO of the returned x (mid_end.cpp:65-71 / 79-85)
     if (d_T || d_coeffs) {
-        MincoArgs M = midend_minco_args(c, B, N0, d_head, d_tail, bc_stride, p->rho, d_x);
-        k_minco_forward<<<B, 32, minco_smem_bytes(N0), st>>>(M);
+        MincoArgs M = midend_minco_args(c, L, d_head, d_tail, bc_stride, p->rho, d_x);
+        k_minco_forward<<<B, 32, minco_smem_bytes(L.N), st>>>(M);
         c->stats.kernel_launches++;
         CU_TRY(cudaGetLastError());
         if (d_T) CU_TRY(cudaMemcpyAsync(d_T, M.T, sizeof(double) * BN, cudaMemcpyDeviceToDevice, st));
@@ -1771,8 +1933,43 @@ extern "C" int isdf_midend_batch_device(isdf_ctx *c, int B, int N0, const double
     return poison_on_failure([&]() -> int {
         if (int r = midend_check(c, B, N0, p)) return r;
         if (!d_head || !d_tail || !d_x || !d_f || (N0 > 1 && !d_waypoints)) return fail(ISDF_ERR_INVALID, "NULL device pointer");
-        return midend_batch_run(c, B, N0, d_head, d_tail, per_problem_bc, p, d_waypoints, d_x, d_T, d_coeffs, d_f, d_ret, d_iterations, d_evaluations, rounds, st);
+        return midend_batch_run(c, uniform_layout(B, N0), d_head, d_tail, per_problem_bc, p, d_waypoints, d_x, d_T, d_coeffs, d_f, d_ret, d_iterations,
+                                d_evaluations, rounds, st);
     }, [&] { nan_fill_device(c, d_f, B, st); });
+}
+
+extern "C" int isdf_midend_batch_ragged_device(isdf_ctx *c, int B, const int32_t *piece_off, const double *d_head, const double *d_tail,
+                                               int per_problem_bc, const isdf_midend_params *p, const double *d_waypoints, double *d_x, double *d_T,
+                                               double *d_coeffs, double *d_f, int32_t *d_ret, int32_t *d_iterations, int32_t *d_evaluations,
+                                               int32_t *rounds, void *cuda_stream) {
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    return poison_on_failure([&]() -> int {
+        Layout L;
+        if (int r = midend_ragged_check(c, B, piece_off, p, &L)) return r;
+        if (!d_head || !d_tail || !d_x || !d_f || (L.P > (size_t)B && !d_waypoints)) return fail(ISDF_ERR_INVALID, "NULL device pointer");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        if (int r = ragged_upload(c->mid.d_off, piece_off, st, &L)) return r;
+        return midend_batch_run(c, L, d_head, d_tail, per_problem_bc, p, d_waypoints, d_x, d_T, d_coeffs, d_f, d_ret, d_iterations, d_evaluations, rounds, st);
+    }, [&] { nan_fill_device(c, d_f, B, st); });
+}
+
+// the host form of getOriTraj for a checked batch: inputs staged in c->mid, results copied back
+static int midend_host_run(isdf_ctx *c, const Layout &L, int per_problem_bc, const isdf_midend_params *p, const double *head, const double *tail,
+                           const double *waypoints, double *x, double *T, double *coeffs, double *f, int32_t *ret, int32_t *iterations,
+                           int32_t *evaluations, int32_t *rounds) {
+    const int B = L.B;
+    isdf_ctx::LbfgsBufs &lb = c->mid.lb;
+    const size_t BN = L.P;
+    const double *d_head, *d_tail, *d_wp;
+    if (int r = midend_upload(c, L, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return r;
+    CU_TRY(lb.d_x.ensure(L.X)); CU_TRY(lb.d_f.ensure((size_t)19 * BN + B)); CU_TRY(lb.d_head.ensure((size_t)3 * B));
+    double *d_f = lb.d_f.p, *d_T = d_f + B, *d_C = d_T + BN;   // [f | T | coeffs]
+    int *d_i = lb.d_head.p;
+    if (int r = midend_batch_run(c, L, d_head, d_tail, per_problem_bc, p, d_wp, lb.d_x.p, d_T, d_C, d_f, d_i, d_i + B, d_i + 2 * (size_t)B,
+                                 rounds, c->stream)) return r;
+    if (T) CU_TRY(cudaMemcpy(T, d_T, sizeof(double) * BN, cudaMemcpyDeviceToHost));
+    if (coeffs) CU_TRY(cudaMemcpy(coeffs, d_C, sizeof(double) * 18 * BN, cudaMemcpyDeviceToHost));
+    return lbfgs_copy_out(lb, B, L.X, x, f, ret, iterations, evaluations);
 }
 
 extern "C" int isdf_midend_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc,
@@ -1782,18 +1979,20 @@ extern "C" int isdf_midend_batch(isdf_ctx *c, int B, int N0, const double *head,
         if (int r = midend_check(c, B, N0, p)) return r;
         if (!head || !tail || !x || !f || (N0 > 1 && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
-        isdf_ctx::LbfgsBufs &lb = c->mid.lb;
-        const size_t n = (size_t)4 * N0 - 3, BN = (size_t)B * N0;
-        const double *d_head, *d_tail, *d_wp;
-        if (int r = midend_upload(c, B, N0, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return r;
-        CU_TRY(lb.d_x.ensure(n * B)); CU_TRY(lb.d_f.ensure((size_t)19 * BN + B)); CU_TRY(lb.d_head.ensure((size_t)3 * B));
-        double *d_f = lb.d_f.p, *d_T = d_f + B, *d_C = d_T + BN;   // [f | T | coeffs]
-        int *d_i = lb.d_head.p;
-        if (int r = midend_batch_run(c, B, N0, d_head, d_tail, per_problem_bc, p, d_wp, lb.d_x.p, d_T, d_C, d_f, d_i, d_i + B, d_i + 2 * (size_t)B,
-                                     rounds, c->stream)) return r;
-        if (T) CU_TRY(cudaMemcpy(T, d_T, sizeof(double) * BN, cudaMemcpyDeviceToHost));
-        if (coeffs) CU_TRY(cudaMemcpy(coeffs, d_C, sizeof(double) * 18 * BN, cudaMemcpyDeviceToHost));
-        return lbfgs_copy_out(lb, B, n, x, f, ret, iterations, evaluations);
+        return midend_host_run(c, uniform_layout(B, N0), per_problem_bc, p, head, tail, waypoints, x, T, coeffs, f, ret, iterations, evaluations, rounds);
+    }, [&] { nan_fill(f, B); });
+}
+
+extern "C" int isdf_midend_batch_ragged(isdf_ctx *c, int B, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
+                                        const isdf_midend_params *p, const double *waypoints, double *x, double *T, double *coeffs,
+                                        double *f, int32_t *ret, int32_t *iterations, int32_t *evaluations, int32_t *rounds) {
+    return poison_on_failure([&]() -> int {
+        Layout L;
+        if (int r = midend_ragged_check(c, B, piece_off, p, &L)) return r;
+        if (!head || !tail || !x || !f || (L.P > (size_t)B && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        if (int r = ragged_upload(c->mid.d_off, piece_off, c->stream, &L)) return r;
+        return midend_host_run(c, L, per_problem_bc, p, head, tail, waypoints, x, T, coeffs, f, ret, iterations, evaluations, rounds);
     }, [&] { nan_fill(f, B); });
 }
 
@@ -3051,9 +3250,9 @@ extern "C" int isdf_frontend_path_info(isdf_ctx *c, isdf_frontpath_info *out) {
 }
 
 // ---- planning step: PlannerManager::generateTraj for one start and B goals (include/isdf.h) --------------------------------------------
-// The stages are the existing entry points' internals on device buffers: path_run, isdf_path_waypoints, midend_batch_run per N group, the
-// batched gather with set_as_points, lbfgs_rounds over callback_batch_launch, k_minco_forward for the final trajectories, certify_run and
-// dynamics_run with N0 = N.
+// The stages are the existing entry points' internals on device buffers: path_run, isdf_path_waypoints, one ragged midend_batch_run, the
+// batched gather with set_as_points, one ragged lbfgs_rounds over callback_batch_launch, one ragged k_minco_forward for the final
+// trajectories, then certify_run and dynamics_run with N0 = N per group of plans with the same N.
 extern "C" int isdf_plan_default_params(isdf_ctx *c, isdf_plan_params *p) {
     if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
     std::memset(p, 0, sizeof(*p));
@@ -3154,150 +3353,175 @@ static int plan_run(isdf_ctx *c, const double *start, int B, const double *goals
     if ((path_xyz && nodes > cap_nodes) || poff[B] > cap_pieces)
         return fail(ISDF_ERR_INVALID, "cap_nodes or cap_pieces too small (path_off / piece_off report the sizes needed)");
     if (path_xyz && nodes) std::memcpy(path_xyz, xyz.data(), sizeof(double) * xyz.size());
-    // 3-7. per N group, ascending
+    // 3-6. one ragged mid-end over every plan that reaches it, one gather and one ragged back end over the plans that pass it, in goal order
+    std::vector<int> idx;   // the plans that reach the mid-end
+    for (int b = 0; b < B; b++) if (res[b].stage == ISDF_PLAN_OPTIMISED) idx.push_back(b);
     std::vector<int> Ns;
-    for (int b = 0; b < B; b++) if (res[b].stage == ISDF_PLAN_OPTIMISED) Ns.push_back(N[b]);
+    for (const int b : idx) Ns.push_back(N[b]);
     std::sort(Ns.begin(), Ns.end());
     Ns.erase(std::unique(Ns.begin(), Ns.end()), Ns.end());
-    for (const int Ng : Ns) {
-        std::vector<int> idx;
-        for (int b = 0; b < B; b++) if (res[b].stage == ISDF_PLAN_OPTIMISED && N[b] == Ng) idx.push_back(b);
-        const int Bg = (int)idx.size(), n = 4 * Ng - 3, W = Ng - 1;
-        const size_t BN = (size_t)Bg * Ng;
-        info.groups++;
-        // head = [path.front(), 0, 0], tail = [path.back(), 0, 0] (3x3 column-major, column 0 the position): [heads | tails]; the waypoints
-        std::vector<double> bc((size_t)18 * Bg, 0.0), gw((size_t)3 * std::max<size_t>(BN - Bg, 1));
-        for (int q = 0; q < Bg; q++) {
-            const int b = idx[q];
-            for (int k = 0; k < 3; k++) { bc[9 * (size_t)q + k] = xyz[3 * (size_t)off[b] + k]; bc[9 * ((size_t)Bg + q) + k] = xyz[3 * ((size_t)off[b + 1] - 1) + k]; }
-            std::copy(wps.begin() + 3 * (size_t)wp_off[b], wps.begin() + 3 * (size_t)wp_off[b + 1], gw.begin() + 3 * (size_t)q * W);
+    info.groups = (int)Ns.size();
+    const int Bg = (int)idx.size();
+    if (Bg == 0) return 0;
+    // plan idx[q] owns mid-end pieces [moff[q], moff[q+1]) and waypoint rows [moff[q] - q, moff[q+1] - q - 1); head = [path.front(), 0, 0],
+    // tail = [path.back(), 0, 0] (3x3 column-major, column 0 the position): [heads | tails]
+    std::vector<int> moff((size_t)Bg + 1, 0);
+    for (int q = 0; q < Bg; q++) moff[q + 1] = moff[q] + N[idx[q]];
+    const size_t MP = (size_t)moff[Bg];
+    std::vector<double> bc((size_t)18 * Bg, 0.0), gw(3 * std::max<size_t>(MP - Bg, 1));
+    for (int q = 0; q < Bg; q++) {
+        const int b = idx[q];
+        for (int k = 0; k < 3; k++) { bc[9 * (size_t)q + k] = xyz[3 * (size_t)off[b] + k]; bc[9 * ((size_t)Bg + q) + k] = xyz[3 * ((size_t)off[b + 1] - 1) + k]; }
+        std::copy(wps.begin() + 3 * (size_t)wp_off[b], wps.begin() + 3 * (size_t)wp_off[b + 1], gw.begin() + 3 * ((size_t)moff[q] - q));
+    }
+    Layout ML;
+    if (int r = midend_ragged_check(c, Bg, moff.data(), &p->midend, &ML)) return r;
+    if (int r = ragged_upload(c->mid.d_off, moff.data(), st, &ML)) return r;
+    CU_TRY(z.d_bc.upload(bc.data(), bc.size(), st)); CU_TRY(z.d_wp.upload(gw.data(), gw.size(), st));
+    CU_TRY(z.d_mx.ensure(ML.X)); CU_TRY(z.d_mres.ensure(19 * MP + Bg)); CU_TRY(z.d_mi.ensure((size_t)3 * Bg));
+    double *d_mf = z.d_mres.p, *d_mT = d_mf + Bg, *d_mC = d_mT + MP;   // [f | T | coeffs]
+    int mrounds = 0;
+    if (int r = timed(info.midend_ms, [&] {
+            return midend_batch_run(c, ML, z.d_bc.p, z.d_bc.p + 9 * (size_t)Bg, 1, &p->midend, z.d_wp.p, z.d_mx.p, d_mT, d_mC, d_mf, z.d_mi.p,
+                                    z.d_mi.p + Bg, z.d_mi.p + 2 * (size_t)Bg, &mrounds, st);
+        })) return r;
+    std::vector<double> mres(19 * MP + Bg);   // [f | T | coeffs]
+    std::vector<int> mi((size_t)3 * Bg);
+    CU_TRY(cudaMemcpyAsync(mres.data(), d_mf, sizeof(double) * mres.size(), cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaMemcpyAsync(mi.data(), z.d_mi.p, sizeof(int) * mi.size(), cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    std::vector<int> ok, pos(Bg, -1);   // the plans that passed the mid-end (plan_manager.cpp:277) and their back-end instance
+    for (int q = 0; q < Bg; q++) {
+        isdf_plan_result &r = res[idx[q]];
+        r.midend_f = mres[q]; r.midend_ret = mi[q];
+        if (mi[q] >= 0) { pos[q] = (int)ok.size(); ok.push_back(q); }
+        else r.stage = ISDF_PLAN_MIDEND_FAILED;
+    }
+    const int Bp = (int)ok.size();
+    std::vector<int> boff((size_t)Bp + 1, 0);   // back-end instance k owns pieces [boff[k], boff[k+1])
+    for (int k = 0; k < Bp; k++) boff[k + 1] = boff[k] + N[idx[ok[k]]];
+    const size_t BP = (size_t)boff[Bp];
+    std::vector<double> bres(19 * BP);          // the back end's final [T | coeffs]
+    if (Bp > 0) {
+        // 4. the passed plans' obstacle lists become the batched point sets
+        std::vector<int> gwo((size_t)Bp + 1, 0);
+        std::vector<double> pw(3 * std::max<size_t>(BP - Bp, 1));
+        for (int k = 0; k < Bp; k++) {
+            const int q = ok[k], W = N[idx[q]] - 1;
+            gwo[k + 1] = gwo[k] + W;
+            std::copy(gw.begin() + 3 * ((size_t)moff[q] - q), gw.begin() + 3 * ((size_t)moff[q] - q + W), pw.begin() + 3 * (size_t)gwo[k]);
         }
-        CU_TRY(z.d_bc.upload(bc.data(), bc.size(), st)); CU_TRY(z.d_wp.upload(gw.data(), gw.size(), st));
-        CU_TRY(z.d_mx.ensure((size_t)Bg * n)); CU_TRY(z.d_mres.ensure(19 * BN + Bg)); CU_TRY(z.d_mi.ensure((size_t)3 * Bg));
-        double *d_mf = z.d_mres.p, *d_mT = d_mf + Bg, *d_mC = d_mT + BN;   // [f | T | coeffs]
-        if (int r = midend_check(c, Bg, Ng, &p->midend)) return r;
-        int mrounds = 0;
-        if (int r = timed(info.midend_ms, [&] {
-                return midend_batch_run(c, Bg, Ng, z.d_bc.p, z.d_bc.p + 9 * (size_t)Bg, 1, &p->midend, z.d_wp.p, z.d_mx.p, d_mT, d_mC, d_mf, z.d_mi.p,
-                                        z.d_mi.p + Bg, z.d_mi.p + 2 * (size_t)Bg, &mrounds, st);
+        CU_TRY(c->gat.d_wpoff.upload(gwo.data(), gwo.size(), st)); CU_TRY(c->gat.d_wp.upload(pw.data(), pw.size(), st));
+        std::vector<int> pto;
+        long long tot = 0;
+        if (int r = timed(info.gather_ms, [&] {
+                if (int rr = gather_batch_run(c, Bp, gwo.data(), c->gat.d_wpoff.p, c->gat.d_wp.p, p->half_extent, p->offset, 0x7fffffffll, pto, &tot, st)) return rr;
+                return gather_set_points(c, Bp, pto, tot, st);
             })) return r;
-        std::vector<double> mres(Bg + BN);   // [f | T]
-        std::vector<int> mi((size_t)3 * Bg);
-        CU_TRY(cudaMemcpyAsync(mres.data(), d_mf, sizeof(double) * mres.size(), cudaMemcpyDeviceToHost, st));
-        CU_TRY(cudaMemcpyAsync(mi.data(), z.d_mi.p, sizeof(int) * mi.size(), cudaMemcpyDeviceToHost, st));
-        CU_TRY(cudaStreamSynchronize(st));
-        std::vector<int> ok, pos(Bg, -1);   // the plans that passed the mid-end (plan_manager.cpp:277) and their back-end instance
-        for (int q = 0; q < Bg; q++) {
-            isdf_plan_result &r = res[idx[q]];
-            r.midend_f = mres[q]; r.midend_ret = mi[q];
-            if (mi[q] >= 0) { pos[q] = (int)ok.size(); ok.push_back(q); }
-            else r.stage = ISDF_PLAN_MIDEND_FAILED;
-        }
-        const int Bp = (int)ok.size();
-        if (Bp > 0) {
-            // 4. the passed plans' obstacle lists become the batched point sets
-            std::vector<int> gwo((size_t)Bp + 1);
-            std::vector<double> pw((size_t)3 * std::max(Bp * W, 1));
-            for (int k = 0; k <= Bp; k++) gwo[k] = k * W;
-            for (int k = 0; k < Bp; k++) std::copy(gw.begin() + 3 * (size_t)ok[k] * W, gw.begin() + 3 * ((size_t)ok[k] + 1) * W, pw.begin() + 3 * (size_t)k * W);
-            CU_TRY(c->gat.d_wpoff.upload(gwo.data(), gwo.size(), st)); CU_TRY(c->gat.d_wp.upload(pw.data(), pw.size(), st));
-            std::vector<int> pto;
-            long long tot = 0;
-            if (int r = timed(info.gather_ms, [&] {
-                    if (int rr = gather_batch_run(c, Bp, gwo.data(), c->gat.d_wpoff.p, c->gat.d_wp.p, p->half_extent, p->offset, 0x7fffffffll, pto, &tot, st)) return rr;
-                    return gather_set_points(c, Bp, pto, tot, st);
-                })) return r;
-            for (int k = 0; k < Bp; k++) res[idx[ok[k]]].obstacle_points = pto[k + 1] - pto[k];
-            // 5. persisted durations: what updateTraj(mid-end trajectory) leaves on a fresh context (swm:287-296)
-            std::vector<double> dur(Bp);
-            for (int k = 0; k < Bp; k++) {
-                double td = 0.0;
-                for (int i = 0; i < Ng; i++) td += mres[Bg + (size_t)ok[k] * Ng + i];
-                dur[k] = td < 3 * 1e2 ? td : 0.0;
-            }
-            CU_TRY(c->sv.set_durations(Bp, dur.data(), st));
-            // 6. back end from the mid-end x
-            std::vector<double> bbc((size_t)18 * Bp);
-            for (int k = 0; k < Bp; k++) {
-                std::copy(bc.begin() + 9 * (size_t)ok[k], bc.begin() + 9 * ((size_t)ok[k] + 1), bbc.begin() + 9 * (size_t)k);
-                std::copy(bc.begin() + 9 * ((size_t)Bg + ok[k]), bc.begin() + 9 * ((size_t)Bg + ok[k] + 1), bbc.begin() + 9 * ((size_t)Bp + k));
-            }
-            CU_TRY(z.d_bbc.upload(bbc.data(), bbc.size(), st));
-            const double *d_bh = z.d_bbc.p, *d_bt = z.d_bbc.p + 9 * (size_t)Bp;
-            CU_TRY(z.d_bx.ensure((size_t)Bp * n)); CU_TRY(z.d_bf.ensure(Bp)); CU_TRY(z.d_bi.ensure((size_t)3 * Bp));
-            for (int k = 0; k < Bp; k++)
-                CU_TRY(cudaMemcpyAsync(z.d_bx.p + (size_t)k * n, z.d_mx.p + (size_t)ok[k] * n, sizeof(double) * n, cudaMemcpyDeviceToDevice, st));
-            if (int r = callback_batch_check(c, Bp, Ng)) return r;
-            int brounds = 0;
-            if (int r = timed(info.backend_ms, [&]() -> int {
-                    if (int rr = lbfgs_rounds(c, c->lbfgs, Bp, n, &p->backend, 0, z.d_bx.p, z.d_bf.p, z.d_bi.p, z.d_bi.p + Bp, z.d_bi.p + 2 * (size_t)Bp,
-                                              &brounds, st, [&](const double *x, double *f, double *g) {
-                                                  return callback_batch_launch(c, Bp, Ng, d_bh, d_bt, 9, p->rho, x, f, g, st);
-                                              })) return rr;
-                    // the final trajectories: forwardT + MINCO of the returned x (back_end_optimizer.cpp:140-163), into the batch trajectories
-                    MincoArgs M = c->batch.minco.args(Bp, Ng, d_bh, d_bt, 9, p->rho, z.d_bx.p);
-                    k_minco_forward<<<Bp, 32, minco_smem_bytes(Ng), st>>>(M);
-                    c->stats.kernel_launches++;
-                    CU_TRY(cudaGetLastError());
-                    c->batch.B = Bp; c->batch.N0 = Ng;
-                    return 0;
-                })) return r;
-            info.backend_rounds += brounds;
-            std::vector<double> bf(Bp);
-            std::vector<int> bi((size_t)3 * Bp);
-            CU_TRY(cudaMemcpyAsync(bf.data(), z.d_bf.p, sizeof(double) * Bp, cudaMemcpyDeviceToHost, st));
-            CU_TRY(cudaMemcpyAsync(bi.data(), z.d_bi.p, sizeof(int) * bi.size(), cudaMemcpyDeviceToHost, st));
-            CU_TRY(cudaStreamSynchronize(st));
-            for (int k = 0; k < Bp; k++) {
-                isdf_plan_result &r = res[idx[ok[k]]];
-                r.backend_f = bf[k]; r.backend_ret = bi[k]; r.backend_iterations = bi[Bp + k]; r.backend_evaluations = bi[2 * (size_t)Bp + k];
-            }
-        }
-        // the group's returned trajectories in goal order, one block (piece q*N + i): the back end's, or the mid-end's for MIDEND_FAILED
-        CU_TRY(z.d_gT.ensure(BN)); CU_TRY(z.d_gC.ensure(18 * BN));
-        for (int q = 0; q < Bg; q++) {
-            const bool be = pos[q] >= 0;
-            const double *sT = be ? c->batch.minco.d_T.p + (size_t)pos[q] * Ng : d_mT + (size_t)q * Ng;
-            const double *sC = be ? c->batch.minco.d_C.p + 6 * (size_t)pos[q] * Ng : d_mC + 6 * (size_t)q * Ng;
-            const size_t spitch = sizeof(double) * 6 * (be ? (size_t)Bp * Ng : BN);
-            CU_TRY(cudaMemcpyAsync(z.d_gT.p + (size_t)q * Ng, sT, sizeof(double) * Ng, cudaMemcpyDeviceToDevice, st));
-            CU_TRY(cudaMemcpy2DAsync(z.d_gC.p + 6 * (size_t)q * Ng, sizeof(double) * 6 * BN, sC, spitch, sizeof(double) * 6 * Ng, 3, cudaMemcpyDeviceToDevice, st));
-        }
-        std::vector<double> gT(BN), gC(18 * BN);
-        CU_TRY(cudaMemcpyAsync(gT.data(), z.d_gT.p, sizeof(double) * BN, cudaMemcpyDeviceToHost, st));
-        CU_TRY(cudaMemcpyAsync(gC.data(), z.d_gC.p, sizeof(double) * 18 * BN, cudaMemcpyDeviceToHost, st));
-        CU_TRY(cudaStreamSynchronize(st));
-        for (int q = 0; q < Bg; q++) {
-            const size_t po = (size_t)poff[idx[q]];
+        for (int k = 0; k < Bp; k++) res[idx[ok[k]]].obstacle_points = pto[k + 1] - pto[k];
+        // 5. persisted durations: what updateTraj(mid-end trajectory) leaves on a fresh context (swm:287-296)
+        std::vector<double> dur(Bp);
+        for (int k = 0; k < Bp; k++) {
+            const int q = ok[k];
             double td = 0.0;
-            for (int i = 0; i < Ng; i++) { T[po + i] = gT[(size_t)q * Ng + i]; td += T[po + i]; }
-            res[idx[q]].duration = td;
-            for (int a = 0; a < 3; a++)
-                std::memcpy(coeffs + 18 * po + 6 * (size_t)a * Ng, gC.data() + 6 * ((size_t)a * BN + (size_t)q * Ng), sizeof(double) * 6 * Ng);
+            for (int i = moff[q]; i < moff[q + 1]; i++) td += mres[Bg + (size_t)i];
+            dur[k] = td < 3 * 1e2 ? td : 0.0;
         }
-        // 7. certificates on every returned trajectory of the group
+        CU_TRY(c->sv.set_durations(Bp, dur.data(), st));
+        // 6. back end from the mid-end x
+        std::vector<double> bbc((size_t)18 * Bp);
+        for (int k = 0; k < Bp; k++) {
+            std::copy(bc.begin() + 9 * (size_t)ok[k], bc.begin() + 9 * ((size_t)ok[k] + 1), bbc.begin() + 9 * (size_t)k);
+            std::copy(bc.begin() + 9 * ((size_t)Bg + ok[k]), bc.begin() + 9 * ((size_t)Bg + ok[k] + 1), bbc.begin() + 9 * ((size_t)Bp + k));
+        }
+        Layout BL;
+        if (int r = callback_ragged_check(c, Bp, boff.data(), &BL)) return r;
+        if (int r = ragged_upload(c->batch.d_off, boff.data(), st, &BL)) return r;
+        CU_TRY(z.d_bbc.upload(bbc.data(), bbc.size(), st));
+        const double *d_bh = z.d_bbc.p, *d_bt = z.d_bbc.p + 9 * (size_t)Bp;
+        CU_TRY(z.d_bx.ensure(BL.X)); CU_TRY(z.d_bf.ensure(Bp)); CU_TRY(z.d_bi.ensure((size_t)3 * Bp));
+        for (int k = 0; k < Bp; k++) {
+            const int q = ok[k];
+            const size_t n = 4 * (size_t)N[idx[q]] - 3;
+            CU_TRY(cudaMemcpyAsync(z.d_bx.p + 4 * (size_t)boff[k] - 3 * (size_t)k, z.d_mx.p + 4 * (size_t)moff[q] - 3 * (size_t)q, sizeof(double) * n,
+                                   cudaMemcpyDeviceToDevice, st));
+        }
+        int brounds = 0;
+        if (int r = timed(info.backend_ms, [&]() -> int {
+                if (int rr = lbfgs_rounds(c, c->lbfgs, Bp, 4 * BL.N - 3, BL.d_xoff, BL.X, &p->backend, 0, z.d_bx.p, z.d_bf.p, z.d_bi.p, z.d_bi.p + Bp,
+                                          z.d_bi.p + 2 * (size_t)Bp, &brounds, st, [&](const double *x, double *f, double *g) {
+                                              return callback_batch_launch(c, BL, d_bh, d_bt, 9, p->rho, x, f, g, st);
+                                          })) return rr;
+                // the final trajectories: forwardT + MINCO of the returned x (back_end_optimizer.cpp:140-163), into the batch trajectories
+                MincoArgs M = c->batch.minco.args(BL, d_bh, d_bt, 9, p->rho, z.d_bx.p);
+                k_minco_forward<<<Bp, 32, minco_smem_bytes(BL.N), st>>>(M);
+                c->stats.kernel_launches++;
+                CU_TRY(cudaGetLastError());
+                c->batch.B = Bp; c->batch.P = BP;
+                return 0;
+            })) return r;
+        info.backend_rounds = brounds;
+        std::vector<double> bf(Bp);
+        std::vector<int> bi((size_t)3 * Bp);
+        CU_TRY(cudaMemcpyAsync(bf.data(), z.d_bf.p, sizeof(double) * Bp, cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(bi.data(), z.d_bi.p, sizeof(int) * bi.size(), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(bres.data(), c->batch.minco.d_T.p, sizeof(double) * BP, cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(bres.data() + BP, c->batch.minco.d_C.p, sizeof(double) * 18 * BP, cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
+        for (int k = 0; k < Bp; k++) {
+            isdf_plan_result &r = res[idx[ok[k]]];
+            r.backend_f = bf[k]; r.backend_ret = bi[k]; r.backend_iterations = bi[Bp + k]; r.backend_evaluations = bi[2 * (size_t)Bp + k];
+        }
+    }
+    // the returned trajectories, plan b's at piece_off[b]: the back end's, or the mid-end's for MIDEND_FAILED
+    for (int q = 0; q < Bg; q++) {
+        const bool be = pos[q] >= 0;
+        const int Nq = N[idx[q]];
+        const size_t po = (size_t)poff[idx[q]], p0 = be ? (size_t)boff[pos[q]] : (size_t)moff[q], rows = 6 * (be ? BP : MP);
+        const double *sT = be ? bres.data() : mres.data() + Bg, *sC = sT + (be ? BP : MP);
+        double td = 0.0;
+        for (int i = 0; i < Nq; i++) { T[po + i] = sT[p0 + i]; td += T[po + i]; }
+        res[idx[q]].duration = td;
+        for (int a = 0; a < 3; a++) std::memcpy(coeffs + 18 * po + 6 * (size_t)a * Nq, sC + a * rows + 6 * p0, sizeof(double) * 6 * Nq);
+    }
+    // 7. certificates on every returned trajectory, per group of plans with the same N, ascending
+    if (!(p->flags & (ISDF_PLAN_CERTIFY | ISDF_PLAN_DYNAMICS))) return 0;
+    for (const int Ng : Ns) {
+        std::vector<int> gi;   // the group's plans, in goal order
+        for (const int b : idx) if (N[b] == Ng) gi.push_back(b);
+        const int Bn = (int)gi.size();
+        const size_t BN = (size_t)Bn * Ng;
+        // the group's trajectories as one block (piece q*N + i of a 6BN x 3 column-major block)
+        std::vector<double> gT(BN), gC(18 * BN);
+        for (int q = 0; q < Bn; q++) {
+            const size_t po = (size_t)poff[gi[q]];
+            std::copy(T + po, T + po + Ng, gT.begin() + (size_t)q * Ng);
+            for (int a = 0; a < 3; a++)
+                std::copy(coeffs + 18 * po + 6 * (size_t)a * Ng, coeffs + 18 * po + 6 * ((size_t)a + 1) * Ng, gC.begin() + 6 * ((size_t)a * BN + (size_t)q * Ng));
+        }
+        CU_TRY(z.d_gT.upload(gT.data(), BN, st)); CU_TRY(z.d_gC.upload(gC.data(), 18 * BN, st));
         if (p->flags & ISDF_PLAN_CERTIFY) {
             isdf_certify_params pc = p->certify;
             pc.clearance.pieces_per_traj = Ng;
             double rr = r_cert;
             if (int r = certify_check(c, (int)BN, &pc, &rr)) return r;
-            CU_TRY(z.d_csum.ensure(Bg));
+            CU_TRY(z.d_csum.ensure(Bn));
             if (int r = timed(info.certify_ms, [&] { return certify_run(c, (int)BN, z.d_gT.p, z.d_gC.p, &pc, rr, z.d_csum.p, st); })) return r;
-            std::vector<isdf_certify_summary> s(Bg);
-            CU_TRY(cudaMemcpyAsync(s.data(), z.d_csum.p, sizeof(isdf_certify_summary) * Bg, cudaMemcpyDeviceToHost, st));
+            std::vector<isdf_certify_summary> s(Bn);
+            CU_TRY(cudaMemcpyAsync(s.data(), z.d_csum.p, sizeof(isdf_certify_summary) * Bn, cudaMemcpyDeviceToHost, st));
             CU_TRY(cudaStreamSynchronize(st));
-            for (int q = 0; q < Bg; q++) certify[idx[q]] = s[q];
+            for (int q = 0; q < Bn; q++) certify[gi[q]] = s[q];
         }
         if (p->flags & ISDF_PLAN_DYNAMICS) {
             isdf_dynamics_params pd = p->dynamics;
             pd.pieces_per_traj = Ng;
             if (int r = dynamics_check(c, (int)BN, &pd)) return r;
-            CU_TRY(z.d_dsum.ensure(Bg));
+            CU_TRY(z.d_dsum.ensure(Bn));
             if (int r = timed(info.dynamics_ms, [&] { return dynamics_run(c, (int)BN, z.d_gT.p, z.d_gC.p, &pd, z.d_dsum.p, st); })) return r;
-            std::vector<isdf_dynamics_summary> s(Bg);
-            CU_TRY(cudaMemcpyAsync(s.data(), z.d_dsum.p, sizeof(isdf_dynamics_summary) * Bg, cudaMemcpyDeviceToHost, st));
+            std::vector<isdf_dynamics_summary> s(Bn);
+            CU_TRY(cudaMemcpyAsync(s.data(), z.d_dsum.p, sizeof(isdf_dynamics_summary) * Bn, cudaMemcpyDeviceToHost, st));
             CU_TRY(cudaStreamSynchronize(st));
-            for (int q = 0; q < Bg; q++) dynamics[idx[q]] = s[q];
+            for (int q = 0; q < Bn; q++) dynamics[gi[q]] = s[q];
         }
     }
     return 0;

@@ -36,6 +36,8 @@ constexpr int LB_NINT = 12;     // phase, ret, k, end, bound, count, brackt, tou
 
 struct LbfgsArgs {
     int B, n;
+    const int *xoff;    // may be null: B + 1 offsets, instance b has dimension xoff[b+1] - xoff[b] and its vectors start at row xoff[b]
+                        // (a ragged batch, include/isdf.h); null: every instance has dimension n and starts at row b n
     LbfgsDevParams pr;
     double *x;          // B x n: the point every instance wants evaluated next (in: starting points; out: solutions)
     const double *f;    // B: callback values at x
@@ -43,7 +45,7 @@ struct LbfgsArgs {
     double *xp, *g, *gp, *d;   // B x n each
     double *pf;         // B x max(1, past)
     double *alpha, *ys; // B x m each
-    double *S, *Y;      // B x m x n each
+    double *S, *Y;      // B x m x n each (ragged: instance b's start at m xoff[b])
     double *sc;         // B x LB_NSCALAR
     int *st;            // B x LB_NINT
     int *active;        // [0]: instances not DONE after this launch (zeroed by the host before each launch)
@@ -55,16 +57,19 @@ __device__ __forceinline__ double lb_norm_inf(const double *a, int n) { double m
 __global__ void __launch_bounds__(64) k_lbfgs_feed(const LbfgsArgs A) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= A.B) return;
-    const int n = A.n, m = A.pr.mem_size, past = A.pr.past;
+    // the instance's first row; 32 bits suffice (the B x m x n histories of 2^32 rows would not fit in device memory) and keep the
+    // kernel's register pressure below its uniform form's
+    const unsigned o = A.xoff ? (unsigned)A.xoff[b] : (unsigned)b * (unsigned)A.n;
+    const int n = A.xoff ? (int)(A.xoff[b + 1] - o) : A.n, m = A.pr.mem_size, past = A.pr.past;
     const LbfgsDevParams &pr = A.pr;
     int *st = A.st + (size_t)b * LB_NINT;
     int phase = st[0];
     if (phase == LB_DONE) return;
     double *sc = A.sc + (size_t)b * LB_NSCALAR;
-    double *x = A.x + (size_t)b * n, *xp = A.xp + (size_t)b * n, *g = A.g + (size_t)b * n, *gp = A.gp + (size_t)b * n, *d = A.d + (size_t)b * n;
+    double *x = A.x + o, *xp = A.xp + o, *g = A.g + o, *gp = A.gp + o, *d = A.d + o;
     double *pf = A.pf + (size_t)b * (past > 1 ? past : 1), *alpha = A.alpha + (size_t)b * m, *ys_hist = A.ys + (size_t)b * m;
-    double *S = A.S + (size_t)b * m * n, *Y = A.Y + (size_t)b * m * n;
-    const double *grad = A.grad + (size_t)b * n;
+    double *S = A.S + (size_t)m * o, *Y = A.Y + (size_t)m * o;
+    const double *grad = A.grad + o;
     const double f = A.f[b];
     double fx = sc[0], step = sc[1], olddnorm = sc[2], finit = sc[3], dgtest = sc[4], mu = sc[5], nu = sc[6];
     int ret = st[1], k = st[2], end = st[3], bound = st[4], count = st[5], brackt = st[6], touched = st[7], iterations = st[8], evaluations = st[9];
@@ -196,11 +201,12 @@ __global__ void __launch_bounds__(64) k_lbfgs_cap(const LbfgsArgs A) {
     int *st = A.st + (size_t)b * LB_NINT;
     const int phase = st[0];
     if (phase == LB_DONE) return;
-    const int n = A.n;
+    const size_t o = A.xoff ? (size_t)A.xoff[b] : (size_t)b * A.n;
+    const int n = A.xoff ? A.xoff[b + 1] - A.xoff[b] : A.n;
     double *sc = A.sc + (size_t)b * LB_NSCALAR;
     if (phase == LB_WANT_LS) {
-        double *x = A.x + (size_t)b * n;
-        const double *xp = A.xp + (size_t)b * n;
+        double *x = A.x + o;
+        const double *xp = A.xp + o;
         for (int i = 0; i < n; i++) x[i] = xp[i];
         sc[0] = sc[3];   // fx = finit
     }

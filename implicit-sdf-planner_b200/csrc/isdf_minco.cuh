@@ -12,28 +12,33 @@
 // (host/isdf_minco.hpp), which the CPU tests pin against the oracle's dense solve.
 // The coefficient blocks of the B problems are written CONCATENATED (piece b*N + i of a 6BN x 3 column-major block), which is
 // exactly what one launch of the discrete kernels consumes: the time-integral term couples nothing across pieces.
+// A ragged batch (poff != null, include/isdf.h) gives problem b the pieces [poff[b], poff[b+1]) instead of [b N, b N + N): every per-piece
+// array is indexed by the problem's first piece p0, x by 4 p0 - 3 b, and the per-problem arithmetic is the same, so a problem's bits do
+// not depend on the batch around it.
 #pragma once
 #include "isdf_types.cuh"
 
 namespace isdf {
 
 struct MincoArgs {
-    int B, N;                 // problems, pieces per problem
-    const double *x;          // B x (N + 3(N-1)) decision vectors
+    int B, N;                 // problems, pieces per problem (ragged: the most pieces of one problem)
+    int P;                    // pieces of the batch (B N when uniform)
+    const int *poff;          // may be null: B + 1 piece offsets of a ragged batch; null: problem b owns pieces [b N, b N + N)
+    const double *x;          // B x (N + 3(N-1)) decision vectors (ragged: problem b's 4 N_b - 3 start at row 4 poff[b] - 3 b)
     const double *head, *tail;  // 3x3 column-major (columns p, v, a); bc_stride = 0: shared by the batch, 9: one per problem
     int bc_stride;
     double rho;
-    double *T;                // B*N durations (concatenated)
-    double *C;                // 18*B*N coefficients: column-major over the 6*B*N rows
-    double *Cpp;              // may be null: B x 18N, the same coefficients as one column-major 6N x 3 block PER PROBLEM (swept-volume kernels)
-    const double *sv_out;     // may be null: B x (19N+1), per problem [cost | gradC 18N | gradT N] of the batched swept-volume term
-    double *lu;               // B x 78N: factored band of every problem (kept for the adjoint solve)
+    double *T;                // P durations (concatenated)
+    double *C;                // 18P coefficients: column-major over the 6P rows
+    double *Cpp;              // may be null: 18P, the same coefficients as one column-major 6N x 3 block PER PROBLEM (swept-volume kernels)
+    const double *sv_out;     // may be null: 19P + B, per problem [cost | gradC 18N | gradT N] of the batched swept-volume term
+    double *lu;               // 78P: factored band of every problem (kept for the adjoint solve)
     double *energy;           // B
     double *gC_e, *gT_e;      // energy partials, same layouts as C / T
-    const double *disc_out;   // [cost | gradC 18BN | gradT BN] of the concatenated time-integral evaluation (null: none)
-    const double *piece_cost; // B*N per-piece cost terms of that evaluation
+    const double *disc_out;   // [cost | gradC 18P | gradT P] of the concatenated time-integral evaluation (null: none)
+    const double *piece_cost; // P per-piece cost terms of that evaluation
     double *cost;             // B
-    double *grad;             // B x (N + 3(N-1))
+    double *grad;             // laid out as x
     int seq_terms;            // 1: the piece costs are added to the energy one at a time (the mid-end, isdf_midend.cuh); 0: summed first
 };
 
@@ -58,18 +63,18 @@ __device__ __forceinline__ void minco_put(double *a, int n, int row, int col0, c
 
 __global__ void __launch_bounds__(32) k_minco_forward(const __grid_constant__ MincoArgs A) {
     extern __shared__ __align__(16) double sm[];
-    const int N = A.N, n = 6 * N, b = blockIdx.x, lane = threadIdx.x;
+    const int b = blockIdx.x, lane = threadIdx.x;
+    const int p0 = A.poff ? A.poff[b] : b * A.N, N = A.poff ? A.poff[b + 1] - p0 : A.N, n = 6 * N;   // first piece, pieces
     double *a = sm;                    // 13n
     double *rhs = sm + (size_t)13 * n; // 3n, column-major
     double *sT = rhs + (size_t)3 * n;  // N
-    const int dim = N + 3 * (N - 1);
-    const double *x = A.x + (size_t)b * dim;
+    const double *x = A.x + (size_t)4 * p0 - 3 * b;
     const double *head = A.head + (size_t)b * A.bc_stride, *tail = A.tail + (size_t)b * A.bc_stride;
     for (int i = lane; i < N; i += 32) {
         const double t = x[i];
         const double Ti = t > 0.0 ? ((0.5 * t + 1.0) * t + 1.0) : 1.0 / ((0.5 * t - 1.0) * t + 1.0);
         sT[i] = Ti;
-        A.T[(size_t)b * N + i] = Ti;
+        A.T[(size_t)p0 + i] = Ti;
     }
     for (int k = lane; k < 16 * n; k += 32) sm[k] = 0.0;
     __syncwarp();
@@ -136,13 +141,13 @@ __global__ void __launch_bounds__(32) k_minco_forward(const __grid_constant__ Mi
         __syncwarp();
     }
     // ---- outputs ------------------------------------------------------------------------------------------------------
-    const size_t rows = (size_t)6 * A.B * N;         // rows of the concatenated block
+    const size_t rows = (size_t)6 * A.P;             // rows of the concatenated block
     for (int k = lane; k < 3 * n; k += 32) {
         const int ax = k / n, row = k - ax * n;
-        A.C[(size_t)ax * rows + (size_t)6 * b * N + row] = rhs[k];
-        if (A.Cpp) A.Cpp[(size_t)b * 18 * N + k] = rhs[k];
+        A.C[(size_t)ax * rows + (size_t)6 * p0 + row] = rhs[k];
+        if (A.Cpp) A.Cpp[(size_t)18 * p0 + k] = rhs[k];
     }
-    for (int k = lane; k < 13 * n; k += 32) A.lu[(size_t)b * 13 * n + k] = a[k];
+    for (int k = lane; k < 13 * n; k += 32) A.lu[(size_t)78 * p0 + k] = a[k];
     // energy partials (minco.hpp:550-582); the energy itself is summed in the reference's (piece, axis) order by lane 0
     double *term = a;                                  // band no longer needed in shared memory: reuse as 3N scratch
     __syncwarp();
@@ -152,14 +157,14 @@ __global__ void __launch_bounds__(32) k_minco_forward(const __grid_constant__ Mi
         for (int ax = 0; ax < 3; ax++) {
             const double c3 = rhs[(size_t)ax * n + 6 * i + 3], c4 = rhs[(size_t)ax * n + 6 * i + 4], c5 = rhs[(size_t)ax * n + 6 * i + 5];
             term[3 * i + ax] = 36.0 * c3 * c3 * t1 + 144.0 * c4 * c3 * t2 + 192.0 * c4 * c4 * t3 + 240.0 * c5 * c3 * t3 + 720.0 * c5 * c4 * t4 + 720.0 * c5 * c5 * t5;
-            double *o = A.gC_e + (size_t)ax * rows + (size_t)6 * b * N + 6 * i;
+            double *o = A.gC_e + (size_t)ax * rows + (size_t)6 * p0 + 6 * i;
             o[0] = 0.0; o[1] = 0.0; o[2] = 0.0;
             o[3] = 72.0 * c3 * t1 + 144.0 * c4 * t2 + 240.0 * c5 * t3;
             o[4] = 144.0 * c3 * t2 + 384.0 * c4 * t3 + 720.0 * c5 * t4;
             o[5] = 240.0 * c3 * t3 + 720.0 * c4 * t4 + 1440.0 * c5 * t5;
             s += 36.0 * c3 * c3 + 288.0 * c4 * c3 * t1 + 576.0 * c4 * c4 * t2 + 720.0 * c5 * c3 * t2 + 2880.0 * c5 * c4 * t3 + 3600.0 * c5 * c5 * t4;
         }
-        A.gT_e[(size_t)b * N + i] = s;
+        A.gT_e[(size_t)p0 + i] = s;
     }
     __syncwarp();
     if (lane == 0) {
@@ -171,18 +176,19 @@ __global__ void __launch_bounds__(32) k_minco_forward(const __grid_constant__ Mi
 
 __global__ void __launch_bounds__(32) k_minco_backward(const __grid_constant__ MincoArgs A) {
     extern __shared__ __align__(16) double sm[];
-    const int N = A.N, n = 6 * N, b = blockIdx.x, lane = threadIdx.x;
+    const int b = blockIdx.x, lane = threadIdx.x;
+    const int p0 = A.poff ? A.poff[b] : b * A.N, N = A.poff ? A.poff[b + 1] - p0 : A.N, n = 6 * N;   // first piece, pieces
     double *a = sm;                     // 13n
     double *lam = sm + (size_t)13 * n;  // 3n
     double *gtm = lam + (size_t)3 * n;  // N: gradTimes
-    const int dim = N + 3 * (N - 1);
-    const size_t rows = (size_t)6 * A.B * N, BN = (size_t)A.B * N;
-    for (int k = lane; k < 13 * n; k += 32) a[k] = A.lu[(size_t)b * 13 * n + k];
+    const size_t rows = (size_t)6 * A.P, BN = (size_t)A.P;
+    const double *sv = A.sv_out ? A.sv_out + (size_t)19 * p0 + b : nullptr;   // this problem's [cost | gradC 18N | gradT N]
+    for (int k = lane; k < 13 * n; k += 32) a[k] = A.lu[(size_t)78 * p0 + k];
     for (int k = lane; k < 3 * n; k += 32) {
         const int ax = k / n, row = k - ax * n;
-        const size_t g = (size_t)ax * rows + (size_t)6 * b * N + row;
+        const size_t g = (size_t)ax * rows + (size_t)6 * p0 + row;
         double v = A.gC_e[g];                                                   // accumulation order of costFunctionLmbm (hpp:386-405): energy partials,
-        if (A.sv_out) v += A.sv_out[(size_t)b * (19 * N + 1) + 1 + k];         // + swept-volume term,
+        if (sv) v += sv[1 + k];                                                 // + swept-volume term,
         lam[k] = v + (A.disc_out ? A.disc_out[1 + g] : 0.0);                    // + time-integral term
     }
     __syncwarp();
@@ -208,19 +214,19 @@ __global__ void __launch_bounds__(32) k_minco_backward(const __grid_constant__ M
         __syncwarp();
     }
     // ---- propogateGrad (minco.hpp:584-654) + rho + backwardGradT/P (hpp:283-330) -----------------------------------------
-    double *g = A.grad + (size_t)b * dim;
-    const double *x = A.x + (size_t)b * dim;
+    double *g = A.grad + (size_t)4 * p0 - 3 * b;
+    const double *x = A.x + (size_t)4 * p0 - 3 * b;
     for (int k = lane; k < 3 * (N - 1); k += 32) {
         const int i = k / 3, ax = k - 3 * i;
         g[N + k] = lam[(size_t)ax * n + 6 * i + 5];
     }
     for (int i = lane; i < N; i += 32) {
-        const double Ti = A.T[(size_t)b * N + i];
+        const double Ti = A.T[(size_t)p0 + i];
         double s = 0.0;
         double r[6];
         for (int ax = 0; ax < 3; ax++) {
             double dval[6];
-            const double *c = A.C + (size_t)ax * rows + (size_t)6 * b * N + 6 * i;
+            const double *c = A.C + (size_t)ax * rows + (size_t)6 * p0 + 6 * i;
             for (int d = 1; d <= 5; d++) {
                 minco_basis(Ti, d, r);
                 double v = 0.0;
@@ -236,9 +242,9 @@ __global__ void __launch_bounds__(32) k_minco_backward(const __grid_constant__ M
                 s -= dval[1] * L[n - 3] + dval[2] * L[n - 2] + dval[3] * L[n - 1];
             }
         }
-        double gT = A.gT_e[(size_t)b * N + i];
-        if (A.sv_out) gT += A.sv_out[(size_t)b * (19 * N + 1) + 1 + 18 * N + i];
-        gT += (A.disc_out ? A.disc_out[1 + 18 * BN + (size_t)b * N + i] : 0.0);
+        double gT = A.gT_e[(size_t)p0 + i];
+        if (sv) gT += sv[1 + 18 * N + i];
+        gT += (A.disc_out ? A.disc_out[1 + 18 * BN + (size_t)p0 + i] : 0.0);
         double gt = s + gT;
         gt += A.rho;
         gtm[i] = gt;
@@ -248,16 +254,16 @@ __global__ void __launch_bounds__(32) k_minco_backward(const __grid_constant__ M
     }
     if (lane == 0) {
         double cost = A.energy[b];
-        if (A.sv_out) cost += A.sv_out[(size_t)b * (19 * N + 1)];
+        if (sv) cost += sv[0];
         if (A.piece_cost && A.seq_terms) {
-            for (int i = 0; i < N; i++) cost += A.piece_cost[(size_t)b * N + i];
+            for (int i = 0; i < N; i++) cost += A.piece_cost[(size_t)p0 + i];
         } else if (A.piece_cost) {
             double c = 0.0;
-            for (int i = 0; i < N; i++) c += A.piece_cost[(size_t)b * N + i];
+            for (int i = 0; i < N; i++) c += A.piece_cost[(size_t)p0 + i];
             cost += c;
         }
         double tsum = 0.0;
-        for (int i = 0; i < N; i++) tsum += A.T[(size_t)b * N + i];
+        for (int i = 0; i < N; i++) tsum += A.T[(size_t)p0 + i];
         cost += A.rho * tsum;
         A.cost[b] = cost;
     }

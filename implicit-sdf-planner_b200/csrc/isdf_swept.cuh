@@ -758,26 +758,28 @@ __device__ __forceinline__ void sv_finish_body(const SvArgs &A, const int bx) {
 // shared memory from the batch description) — both run the SAME bodies, so a problem's swept-volume term is bit-identical whether it is
 // evaluated alone or as one of B --------------------------------------------------------------------------------------------------------
 struct SvBatch {
-    SvArgs base;              // pointers = problem 0 / point 0; base.P unused
+    SvArgs base;              // pointers = problem 0 / point 0; base.P unused; base.N: pieces per problem (ragged: the most of one problem)
     int B;
     const int *pt_off;        // B + 1: problem b owns points [pt_off[b], pt_off[b+1])
-    long long out_stride;     // doubles between two problems' out vectors (19N + 1)
+    const int *piece_off;     // may be null: B + 1 piece offsets of a ragged batch (include/isdf.h); null: problem b owns pieces [b N, b N + N)
 };
+// problem b's view: its N, trajectory (T at piece p0, C at 18 p0), per-piece scratch (at p0) and output vector (19 p0 + b)
 __device__ __forceinline__ void sv_make_view(const SvBatch &Bt, int b, SvArgs &V) {
     const unsigned long long *src = reinterpret_cast<const unsigned long long *>(&Bt.base);
     unsigned long long *dst = reinterpret_cast<unsigned long long *>(&V);
     for (int k = threadIdx.x; k < (int)(sizeof(SvArgs) / 8); k += blockDim.x) dst[k] = src[k];
     __syncthreads();
     if (threadIdx.x == 0) {
-        const int N = Bt.base.N, p0 = Bt.pt_off[b];
+        const int p0 = Bt.pt_off[b], q0 = Bt.piece_off ? Bt.piece_off[b] : b * Bt.base.N;
+        V.N = Bt.piece_off ? Bt.piece_off[b + 1] - q0 : Bt.base.N;
         V.P = Bt.pt_off[b + 1] - p0;
-        V.T = Bt.base.T + (size_t)b * N; V.C = Bt.base.C + (size_t)b * 18 * N;
+        V.T = Bt.base.T + q0; V.C = Bt.base.C + (size_t)18 * q0;
         V.pts = Bt.base.pts + (size_t)3 * p0; V.tstar = Bt.base.tstar + p0; V.sdf = Bt.base.sdf + p0; V.grel = Bt.base.grel + (size_t)3 * p0;
         V.times = Bt.base.times + (size_t)b * SV_MAX_COARSE; V.poses = Bt.base.poses + (size_t)b * 12 * SV_MAX_COARSE;
         V.meta = Bt.base.meta + (size_t)b * 4; V.state = Bt.base.state + (size_t)b * 4;
         V.partial = Bt.base.partial + (size_t)p0 * PARTIAL_STRIDE; V.piece = Bt.base.piece + p0;
-        V.piece_gdt = Bt.base.piece_gdt + (size_t)b * N; V.piece_cost = Bt.base.piece_cost + (size_t)b * N;
-        V.out = Bt.base.out + (size_t)b * Bt.out_stride;
+        V.piece_gdt = Bt.base.piece_gdt + q0; V.piece_cost = Bt.base.piece_cost + q0;
+        V.out = Bt.base.out + (size_t)19 * q0 + b;
     }
     __syncthreads();
 }
@@ -794,10 +796,16 @@ template <bool MESH>
 __global__ void __launch_bounds__(SVM_THREADS) k_sv_points_cta_b(const __grid_constant__ SvBatch Bt) {
     __shared__ SvArgs V; sv_make_view(Bt, blockIdx.y, V); sv_points_cta_body<MESH>(V, blockIdx.x);
 }
-__global__ void __launch_bounds__(256) k_sv_reduce_b(const __grid_constant__ SvBatch Bt) { __shared__ SvArgs V; sv_make_view(Bt, blockIdx.y, V); sv_reduce_body(V, blockIdx.x); }
+__global__ void __launch_bounds__(256) k_sv_reduce_b(const __grid_constant__ SvBatch Bt) {
+    __shared__ SvArgs V; sv_make_view(Bt, blockIdx.y, V);
+    if ((int)blockIdx.x < V.N) sv_reduce_body(V, blockIdx.x);   // grid.x is the batch's most pieces
+}
 __global__ void k_sv_finish_b(const __grid_constant__ SvBatch Bt) { __shared__ SvArgs V; sv_make_view(Bt, blockIdx.y, V); sv_finish_body(V, blockIdx.x); }
 
 // ---- host-side state ----------------------------------------------------------------------------------------------
+// dynamic shared memory above which the kernels opt in to more: static + dynamic past 48 KB needs the opt-in, and the point kernels hold
+// about 22 KB of static shared memory (so trajectories of more than about 170 pieces need it)
+constexpr size_t SV_SMEM_OPTIN = 16 * 1024;
 struct SweptState {
     int P = 0;
     // traj_duration (updateTraj, swm:287-296) persists across evaluations: d_state[0] for the single-problem entry points, d_state_b[4 b]
@@ -864,7 +872,7 @@ struct SweptState {
         const size_t sm = sizeof(double) * 19 * (size_t)N;
         if (sm > 200 * 1024) return cudaErrorInvalidValue;
         if ((e = cudaMemsetAsync(d_counter.p, 0, sizeof(unsigned long long), st)) != cudaSuccess) return e;
-        if (sm > 48 * 1024) {
+        if (sm > SV_SMEM_OPTIN) {
             cudaFuncSetAttribute(k_sv_table, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
             cudaFuncSetAttribute(k_sv_points_cta<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
             cudaFuncSetAttribute(k_sv_points_cta<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
@@ -882,7 +890,8 @@ struct SweptState {
         return cudaGetLastError();
     }
     // ---- batched: B problems, each with its own obstacle point set (concatenated; offsets), its own trajectory (T: B x N, C: B x 18N,
-    // per-problem column-major blocks) and its own output vector (B x (19N+1)); one launch per stage, grid.y = problem -------------------
+    // per-problem column-major blocks) and its own output vector (B x (19N+1)); one launch per stage, grid.y = problem. A ragged batch
+    // (d_poff: B + 1 piece offsets on the device, P pieces, N the most of one problem) lays the same arrays out by its offsets ------------
     int B = 0, maxP = 0;
     std::vector<int> h_off;
     DevBuf<int> d_off;
@@ -917,15 +926,16 @@ struct SweptState {
         if ((e = cudaMemcpy2DAsync(d_state_b.p, 4 * sizeof(double), dur, sizeof(double), sizeof(double), nB, cudaMemcpyHostToDevice, st)) != cudaSuccess) return e;
         return cudaStreamSynchronize(st);
     }
-    cudaError_t launch_batch(const DevCfg &cfg, const DevShape &shape, int N, const double *d_T, const double *d_Cpp, double *d_out, cudaStream_t st, int *launches) {
+    cudaError_t launch_batch(const DevCfg &cfg, const DevShape &shape, int N, const int *d_poff, size_t nP, const double *d_T, const double *d_Cpp,
+                             double *d_out, cudaStream_t st, int *launches) {
         cudaError_t e;
         if ((e = d_times.ensure((size_t)B * SV_MAX_COARSE)) != cudaSuccess) return e;
         if ((e = d_poses.ensure((size_t)12 * B * SV_MAX_COARSE)) != cudaSuccess) return e;
         if ((e = d_meta.ensure((size_t)4 * B)) != cudaSuccess) return e;
         if ((e = grow_state_b(B, st)) != cudaSuccess) return e;
         if (d_counter.n == 0) { if ((e = d_counter.ensure(2)) != cudaSuccess) return e; }
-        if ((e = d_piece_gdt.ensure((size_t)B * N)) != cudaSuccess) return e;
-        if ((e = d_piece_cost.ensure((size_t)B * N)) != cudaSuccess) return e;
+        if ((e = d_piece_gdt.ensure(nP)) != cudaSuccess) return e;
+        if ((e = d_piece_cost.ensure(nP)) != cudaSuccess) return e;
         SvBatch Bt;
         SvArgs &A = Bt.base;
         A.cfg = cfg; A.shape = shape; A.N = N; A.T = d_T; A.C = d_Cpp; A.P = 0; A.pts = d_pts.p;
@@ -933,11 +943,11 @@ struct SweptState {
         A.state = d_state_b.p; A.partial = d_partial.p; A.piece = d_piece.p; A.piece_gdt = d_piece_gdt.p; A.piece_cost = d_piece_cost.p;
         A.out = d_out; A.counter = d_counter.p; A.count_out = nullptr; A.rank = 0; A.world = 1; A.g_t = nullptr; A.g_s = nullptr; A.g_g = nullptr;
         A.work = nullptr; A.order = nullptr; A.use_order = 0;
-        Bt.B = B; Bt.pt_off = d_off.p; Bt.out_stride = 19ll * N + 1;
+        Bt.B = B; Bt.pt_off = d_off.p; Bt.piece_off = d_poff;
         const size_t sm = sizeof(double) * 19 * (size_t)N;
         if (sm > 200 * 1024) return cudaErrorInvalidValue;
         if ((e = cudaMemsetAsync(d_counter.p, 0, sizeof(unsigned long long), st)) != cudaSuccess) return e;
-        if (sm > 48 * 1024) {
+        if (sm > SV_SMEM_OPTIN) {
             cudaFuncSetAttribute(k_sv_table_b, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
             cudaFuncSetAttribute(k_sv_points_cta_b<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
             cudaFuncSetAttribute(k_sv_points_cta_b<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);

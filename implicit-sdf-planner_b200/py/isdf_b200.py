@@ -40,7 +40,9 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_trajectory_certify_device", "isdf_swept_default_params", "isdf_swept_volume_sdf", "isdf_swept_volume_grid",
                "isdf_swept_volume_grid_device", "isdf_swept_volume_mesh", "isdf_dynamics_default_params", "isdf_trajectory_dynamics",
                "isdf_trajectory_dynamics_device", "isdf_gather_obstacle_points_batch", "isdf_plan_default_params", "isdf_plan_batch",
-               "isdf_get_plan_info"]
+               "isdf_get_plan_info", "isdf_callback_batch_ragged", "isdf_callback_batch_ragged_device", "isdf_lbfgs_batch_ragged",
+               "isdf_lbfgs_batch_ragged_device", "isdf_midend_callback_batch_ragged", "isdf_midend_batch_ragged",
+               "isdf_midend_batch_ragged_device"]
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
 DYN_QUANTITIES = ["speed", "acceleration", "body_rate", "tilt", "thrust"]   # q of isdf_dynamics_summary; mask bit 5: the thrust minimum
@@ -332,6 +334,13 @@ def load_library(path=None):
     lib.isdf_plan_batch.argtypes = [vp, dp, C.c_int, dp, C.POINTER(PlanParams), C.c_int, ip, dp, C.c_int, ip, dp, dp, C.POINTER(PlanResult),
                                     C.POINTER(CertifySummary), C.POINTER(DynamicsSummary)]
     lib.isdf_get_plan_info.argtypes = [vp, C.POINTER(PlanInfo)]
+    lib.isdf_callback_batch_ragged.argtypes = [vp, C.c_int, ip, dp, dp, C.c_int, C.c_double, dp, dp, dp]
+    lib.isdf_callback_batch_ragged_device.argtypes = [vp, C.c_int, ip, vp, vp, C.c_int, C.c_double, vp, vp, vp, vp]
+    lib.isdf_lbfgs_batch_ragged.argtypes = [vp, C.c_int, ip, dp, dp, C.c_int, C.c_double, C.POINTER(LbfgsParams), dp, dp, ip, ip, ip, ip]
+    lib.isdf_lbfgs_batch_ragged_device.argtypes = [vp, C.c_int, ip, vp, vp, C.c_int, C.c_double, C.POINTER(LbfgsParams), vp, vp, vp, vp, vp, ip, vp]
+    lib.isdf_midend_callback_batch_ragged.argtypes = [vp, C.c_int, ip, dp, dp, C.c_int, mpp, dp, dp, dp, dp]
+    lib.isdf_midend_batch_ragged.argtypes = [vp, C.c_int, ip, dp, dp, C.c_int, mpp, dp, dp, dp, dp, dp, ip, ip, ip, ip]
+    lib.isdf_midend_batch_ragged_device.argtypes = [vp, C.c_int, ip, vp, vp, C.c_int, mpp, vp, vp, vp, vp, vp, vp, vp, vp, ip, vp]
     for s in ABI_SYMBOLS:
         if s != "isdf_last_error":
             getattr(lib, s).restype = C.c_int
@@ -343,6 +352,63 @@ def load_library(path=None):
 def _colmajor(a):
     """3x3 (or B x 3x3) row-major -> the library's column-major order"""
     return np.ascontiguousarray(np.swapaxes(np.asarray(a, dtype=np.float64), -1, -2)).reshape(-1)
+
+
+class Ragged:
+    """The layout of a ragged batch (include/isdf.h): problem b has N_b = pieces[b] pieces, piece_off = [0, N_0, N_0 + N_1, ...]. pack_*
+    concatenates per-problem arrays into the library's layout, unpack_* splits its outputs back into per-problem arrays."""
+
+    def __init__(self, pieces):
+        self.pieces = np.asarray(pieces, dtype=np.int64).reshape(-1)
+        assert self.pieces.size >= 1 and (self.pieces >= 1).all(), "every problem needs at least one piece"
+        self.B = int(self.pieces.size)
+        self.piece_off = np.zeros(self.B + 1, dtype=np.int32)
+        self.piece_off[1:] = np.cumsum(self.pieces)
+        self.P = int(self.piece_off[-1])
+        b = np.arange(self.B + 1)
+        self.x_off = 4 * self.piece_off.astype(np.int64) - 3 * b            # decision-vector rows [x_off[b], x_off[b+1])
+        self.wp_off = self.piece_off.astype(np.int64) - b                   # waypoint rows [wp_off[b], wp_off[b+1])
+
+    def ptr(self):
+        return self.piece_off.ctypes.data_as(C.POINTER(C.c_int32))
+
+    @staticmethod
+    def _cat(parts):
+        parts = [np.asarray(p, dtype=np.float64).reshape(-1) for p in parts]
+        return np.ascontiguousarray(np.concatenate(parts)) if parts else np.zeros(0)
+
+    def pack_x(self, xs):
+        """B decision vectors [tau (N_b) | xi (3(N_b-1))] -> 4P - 3B rows"""
+        assert len(xs) == self.B and all(np.size(x) == 4 * n - 3 for x, n in zip(xs, self.pieces))
+        return self._cat(xs)
+
+    def unpack_x(self, x):
+        return [np.asarray(x[self.x_off[b]:self.x_off[b + 1]]).copy() for b in range(self.B)]
+
+    def pack_waypoints(self, wps):
+        """B arrays of (N_b - 1, 3) waypoints -> (P - B) x 3 rows, the wp_off layout of isdf_path_waypoints"""
+        assert len(wps) == self.B and all(np.size(w) == 3 * (n - 1) for w, n in zip(wps, self.pieces))
+        return self._cat(wps)
+
+    def pack_T(self, Ts):
+        assert len(Ts) == self.B and all(np.size(t) == n for t, n in zip(Ts, self.pieces))
+        return self._cat(Ts)
+
+    def unpack_T(self, T):
+        return [np.asarray(T[self.piece_off[b]:self.piece_off[b + 1]]).copy() for b in range(self.B)]
+
+    def pack_coeffs(self, Cs):
+        """B per-problem 6N_b x 3 column-major blocks (18 N_b values each) -> one 6P x 3 column-major block"""
+        assert len(Cs) == self.B and all(np.size(c) == 18 * n for c, n in zip(Cs, self.pieces))
+        out = np.zeros((3, 6 * self.P))
+        for b, c in enumerate(Cs):
+            out[:, 6 * self.piece_off[b]:6 * self.piece_off[b + 1]] = np.asarray(c, dtype=np.float64).reshape(3, -1)
+        return out.reshape(-1)
+
+    def unpack_coeffs(self, Cc):
+        """one 6P x 3 column-major block -> B per-problem 6N_b x 3 column-major blocks (18 N_b values each)"""
+        c3 = np.asarray(Cc).reshape(3, 6 * self.P)
+        return [c3[:, 6 * self.piece_off[b]:6 * self.piece_off[b + 1]].reshape(-1).copy() for b in range(self.B)]
 
 
 def path_waypoints(paths, res, parlength=3.0):
@@ -571,6 +637,33 @@ class Evaluator:
     def callback_batch_device(self, B, N0, d_head, d_tail, per_problem_bc, rho, d_x, d_cost, d_grad, stream=None):
         self._check(self.lib.isdf_callback_batch_device(self.h, B, N0, d_head, d_tail, int(per_problem_bc), float(rho), d_x, d_cost, d_grad, stream))
 
+    @staticmethod
+    def _bc(head, tail):
+        head, tail = np.asarray(head, dtype=np.float64), np.asarray(tail, dtype=np.float64)
+        return int(head.ndim == 3), _colmajor(head), _colmajor(tail)
+
+    def callback_batch_ragged(self, head, tail, rho, xs):
+        """isdf_callback_batch_ragged: xs = list of B decision vectors [tau (N_b) | xi (3(N_b-1))] -> (cost[B], list of B gradients); head / tail
+        as callback_batch"""
+        L = Ragged([(np.size(x) + 3) // 4 for x in xs])
+        per, h, t = self._bc(head, tail)
+        x = L.pack_x(xs)
+        cost, grad = np.zeros(L.B), np.zeros(x.size)
+        self._check(self.lib.isdf_callback_batch_ragged(self.h, L.B, L.ptr(), _dp(h), _dp(t), per, float(rho), _dp(x), _dp(cost), _dp(grad)))
+        return cost, L.unpack_x(grad)
+
+    def callback_batch_ragged_device(self, piece_off, d_head, d_tail, per_problem_bc, rho, d_x, d_cost, d_grad, stream=None):
+        off = np.ascontiguousarray(piece_off, dtype=np.int32)
+        self._check(self.lib.isdf_callback_batch_ragged_device(self.h, off.size - 1, off.ctypes.data_as(C.POINTER(C.c_int32)), d_head, d_tail,
+                                                               int(per_problem_bc), float(rho), d_x, d_cost, d_grad, stream))
+
+    def batch_trajectories_ragged(self, pieces):
+        """isdf_get_batch_trajectories after a ragged call: (list of B durations, list of B per-problem coefficient blocks, energies)"""
+        L = Ragged(pieces)
+        T, Cc, en = np.zeros(L.P), np.zeros(18 * L.P), np.zeros(L.B)
+        self._check(self.lib.isdf_get_batch_trajectories(self.h, _dp(T), _dp(Cc), _dp(en)))
+        return L.unpack_T(T), L.unpack_coeffs(Cc), en
+
     def set_points_batch(self, point_sets):
         """per-problem obstacle point sets for the batched callback (list of (P_b, 3) arrays); an empty list switches the batched swept term off"""
         B = len(point_sets)
@@ -623,6 +716,32 @@ class Evaluator:
         rounds = C.c_int32(0)
         self._check(self.lib.isdf_lbfgs_batch_device(self.h, B, N0, d_head, d_tail, int(per_problem_bc), float(rho), C.byref(p), d_x, d_f, d_ret,
                                                      d_iterations, d_evaluations, C.byref(rounds), stream))
+        return rounds.value
+
+    def lbfgs_batch_ragged(self, head, tail, rho, xs, params=None):
+        """isdf_lbfgs_batch_ragged: xs = list of B starting points of 4 N_b - 3 values -> dict(x (list of B), f, ret, iterations, evaluations,
+        rounds)"""
+        L = Ragged([(np.size(x) + 3) // 4 for x in xs])
+        per, h, t = self._bc(head, tail)
+        x = L.pack_x(xs).copy()
+        f = np.zeros(L.B)
+        ret, it, evs = (np.zeros(L.B, dtype=np.int32) for _ in range(3))
+        rounds = C.c_int32(0)
+        ip = C.POINTER(C.c_int32)
+        p = params if params is not None else self.lbfgs_params()
+        self._check(self.lib.isdf_lbfgs_batch_ragged(self.h, L.B, L.ptr(), _dp(h), _dp(t), per, float(rho), C.byref(p), _dp(x), _dp(f),
+                                                     ret.ctypes.data_as(ip), it.ctypes.data_as(ip), evs.ctypes.data_as(ip), C.byref(rounds)))
+        return dict(x=L.unpack_x(x), f=f, ret=ret, iterations=it, evaluations=evs, rounds=rounds.value)
+
+    def lbfgs_batch_ragged_device(self, piece_off, d_head, d_tail, per_problem_bc, rho, d_x, d_f, d_ret=None, d_iterations=None, d_evaluations=None,
+                                  params=None, stream=None):
+        """isdf_lbfgs_batch_ragged_device on raw device pointers; piece_off on the host; returns the rounds"""
+        off = np.ascontiguousarray(piece_off, dtype=np.int32)
+        p = params if params is not None else self.lbfgs_params()
+        rounds = C.c_int32(0)
+        self._check(self.lib.isdf_lbfgs_batch_ragged_device(self.h, off.size - 1, off.ctypes.data_as(C.POINTER(C.c_int32)), d_head, d_tail,
+                                                            int(per_problem_bc), float(rho), C.byref(p), d_x, d_f, d_ret, d_iterations, d_evaluations,
+                                                            C.byref(rounds), stream))
         return rounds.value
 
     _DBG_LBFGS_EVAL = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double))
@@ -702,6 +821,45 @@ class Evaluator:
         self._check(self.lib.isdf_midend_batch(self.h, B, N0, _dp(h), _dp(t), per, C.byref(p), _dp(wp), _dp(x.reshape(-1)), _dp(T.reshape(-1)), _dp(Cc), _dp(f),
                                                ret.ctypes.data_as(ip), it.ctypes.data_as(ip), evs.ctypes.data_as(ip), C.byref(rounds)))
         return dict(x=x, T=T, coeffs=Cc, f=f, ret=ret, iterations=it, evaluations=evs, rounds=rounds.value)
+
+    def midend_callback_batch_ragged(self, head, tail, waypoints, xs, params=None):
+        """isdf_midend_callback_batch_ragged: waypoints = list of B (N_b - 1, 3) arrays, xs = list of B decision vectors -> (cost[B], list of B
+        gradients)"""
+        L = Ragged([len(np.asarray(w).reshape(-1, 3)) + 1 for w in waypoints])
+        per, h, t = self._bc(head, tail)
+        wp, x = L.pack_waypoints(waypoints), L.pack_x(xs)
+        p = params if params is not None else self.midend_params()
+        cost, grad = np.zeros(L.B), np.zeros(x.size)
+        self._check(self.lib.isdf_midend_callback_batch_ragged(self.h, L.B, L.ptr(), _dp(h), _dp(t), per, C.byref(p), _dp(wp if wp.size else np.zeros(1)),
+                                                               _dp(x), _dp(cost), _dp(grad)))
+        return cost, L.unpack_x(grad)
+
+    def midend_batch_ragged(self, head, tail, waypoints, params=None):
+        """isdf_midend_batch_ragged: waypoints = list of B (N_b - 1, 3) arrays (N_b from their lengths) -> dict(x, T, coeffs (lists of B; coeffs
+        per problem as its own 6N_b x 3 column-major block), f, ret, iterations, evaluations, rounds)"""
+        L = Ragged([len(np.asarray(w).reshape(-1, 3)) + 1 for w in waypoints])
+        per, h, t = self._bc(head, tail)
+        wp = L.pack_waypoints(waypoints)
+        p = params if params is not None else self.midend_params()
+        x, T, Cc, f = np.zeros(4 * L.P - 3 * L.B), np.zeros(L.P), np.zeros(18 * L.P), np.zeros(L.B)
+        ret, it, evs = (np.zeros(L.B, dtype=np.int32) for _ in range(3))
+        rounds = C.c_int32(0)
+        ip = C.POINTER(C.c_int32)
+        self._check(self.lib.isdf_midend_batch_ragged(self.h, L.B, L.ptr(), _dp(h), _dp(t), per, C.byref(p), _dp(wp if wp.size else np.zeros(1)), _dp(x),
+                                                      _dp(T), _dp(Cc), _dp(f), ret.ctypes.data_as(ip), it.ctypes.data_as(ip), evs.ctypes.data_as(ip),
+                                                      C.byref(rounds)))
+        return dict(x=L.unpack_x(x), T=L.unpack_T(T), coeffs=L.unpack_coeffs(Cc), f=f, ret=ret, iterations=it, evaluations=evs, rounds=rounds.value)
+
+    def midend_batch_ragged_device(self, piece_off, d_head, d_tail, per_problem_bc, d_waypoints, d_x, d_T, d_coeffs, d_f, d_ret, d_iterations,
+                                   d_evaluations, params=None, stream=None):
+        """isdf_midend_batch_ragged_device on raw device pointers; piece_off on the host; returns the rounds"""
+        off = np.ascontiguousarray(piece_off, dtype=np.int32)
+        p = params if params is not None else self.midend_params()
+        rounds = C.c_int32(0)
+        self._check(self.lib.isdf_midend_batch_ragged_device(self.h, off.size - 1, off.ctypes.data_as(C.POINTER(C.c_int32)), d_head, d_tail,
+                                                             int(per_problem_bc), C.byref(p), d_waypoints, d_x, d_T, d_coeffs, d_f, d_ret, d_iterations,
+                                                             d_evaluations, C.byref(rounds), stream))
+        return rounds.value
 
     def midend_batch_device(self, B, N0, d_head, d_tail, per_problem_bc, d_waypoints, d_x, d_T, d_coeffs, d_f, d_ret, d_iterations, d_evaluations,
                             params=None, stream=None):

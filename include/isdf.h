@@ -248,8 +248,30 @@ int isdf_callback_batch(isdf_ctx *ctx, int B, int N0, const double *head, const 
 /* device-resident variant (all pointers on ctx's device, asynchronous on cuda_stream) */
 int isdf_callback_batch_device(isdf_ctx *ctx, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc,
                                double rho, const double *d_x, double *d_cost, double *d_grad, void *cuda_stream);
-/* the trajectories of the last batched callback: durations (B*N0), coefficient block (6*B*N0 x 3 column-major, piece b*N0+i),
- * jerk energies (B); any may be NULL */
+/* ---- ragged batches: problems of different piece counts in one call ----------------------------------------------------------------
+ * Every *_ragged entry point below takes (B, piece_off) where its uniform sibling takes (B, N0); every other argument is the sibling's.
+ * piece_off: B + 1 int32 values on the HOST (also for the _device forms: the host sizes the launches from them), piece_off[0] = 0; problem
+ * b has N_b = piece_off[b+1] - piece_off[b] pieces, 1 <= N_b <= 290, and P = piece_off[B] pieces in all. Problem b's part of each array:
+ *   decision vectors x, grad    rows [4 piece_off[b] - 3 b, 4 piece_off[b+1] - 3 (b+1)) = [tau (N_b) | xi (3(N_b-1))]
+ *   waypoints (mid-end)         rows [piece_off[b] - b, piece_off[b+1] - (b+1)): the wp_off layout of isdf_path_waypoints, whose output
+ *                               therefore feeds the ragged mid-end unchanged
+ *   durations T                 T[piece_off[b] + i]
+ *   coefficients                one 6P x 3 column-major block, piece piece_off[b] + i at rows 6 (piece_off[b] + i) ...
+ *   per-problem scalars         index b (cost, f, ret, iterations, evaluations)
+ * The uniform batch is the case piece_off[b] = b N0: with those offsets every ragged call returns what its sibling returns, bit for bit.
+ * A problem's results do not depend on the batch around it: alone, in a uniform batch or in a ragged one, they are bit-identical. The
+ * lock-step drivers run until the slowest instance stops, so one ragged call costs about its slowest problem where one uniform call per
+ * distinct N costs the sum of each call's slowest; shared memory is sized by the largest N_b of the call.
+ * The swept-volume term is on exactly when point sets are registered for the same B (isdf_set_points_batch), as for the uniform calls.
+ * Errors follow the siblings': ISDF_ERR_INVALID for a NULL argument, B < 1, piece_off[0] != 0 or offsets that do not increase;
+ * ISDF_ERR_UNSUPPORTED for N_b > 290 or (callback, L-BFGS) P (K+1) beyond 31 bits; ISDF_ERR_STATE on a sharded context. On failure every
+ * cost[b] / f[b] is NaN, as the sibling's. */
+int isdf_callback_batch_ragged(isdf_ctx *ctx, int B, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
+                               double rho, const double *x, double *cost, double *grad);
+int isdf_callback_batch_ragged_device(isdf_ctx *ctx, int B, const int32_t *piece_off, const double *d_head, const double *d_tail,
+                                      int per_problem_bc, double rho, const double *d_x, double *d_cost, double *d_grad, void *cuda_stream);
+/* the trajectories of the last batched callback (uniform or ragged): durations (P = B*N0 for a uniform call), coefficient block (6P x 3
+ * column-major, piece piece_off[b]+i; b*N0+i for a uniform call), jerk energies (B); any may be NULL */
 int isdf_get_batch_trajectories(isdf_ctx *ctx, double *T, double *coeffs, double *energy);
 
 /* ---- device-resident lock-step L-BFGS over the batched callback (SURVEY §8f row 2) ------------------------------------------------
@@ -278,6 +300,13 @@ int isdf_lbfgs_batch(isdf_ctx *ctx, int B, int N0, const double *head, const dou
 int isdf_lbfgs_batch_device(isdf_ctx *ctx, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc, double rho,
                             const isdf_lbfgs_params *params, double *d_x, double *d_f, int32_t *d_ret, int32_t *d_iterations, int32_t *d_evaluations,
                             int32_t *rounds, void *cuda_stream);
+/* ragged forms (see "ragged batches" above): x holds 4P - 3B rows; every instance runs from the first round and stops on its own */
+int isdf_lbfgs_batch_ragged(isdf_ctx *ctx, int B, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
+                            double rho, const isdf_lbfgs_params *params, double *x, double *f, int32_t *ret, int32_t *iterations,
+                            int32_t *evaluations, int32_t *rounds);
+int isdf_lbfgs_batch_ragged_device(isdf_ctx *ctx, int B, const int32_t *piece_off, const double *d_head, const double *d_tail,
+                                   int per_problem_bc, double rho, const isdf_lbfgs_params *params, double *d_x, double *d_f, int32_t *d_ret,
+                                   int32_t *d_iterations, int32_t *d_evaluations, int32_t *rounds, void *cuda_stream);
 
 /* ---- mid-end: warm start of the back end from front-end paths (PlannerManager::generateTraj, plan_manager.cpp:202-289) --------------
  * The reference turns an A* path into the back end's starting point in two steps: it picks waypoints from the path, then OriTraj::getOriTraj
@@ -335,6 +364,10 @@ int isdf_midend_default_params(isdf_midend_params *p);
  * isdf_callback_batch. */
 int isdf_midend_callback_batch(isdf_ctx *ctx, int B, int N0, const double *head, const double *tail, int per_problem_bc,
                                const isdf_midend_params *p, const double *waypoints, const double *x, double *cost, double *grad);
+/* ragged form (see "ragged batches" above): waypoints P - B rows (may be NULL when P = B), x and grad 4P - 3B rows */
+int isdf_midend_callback_batch_ragged(isdf_ctx *ctx, int B, const int32_t *piece_off, const double *head, const double *tail,
+                                      int per_problem_bc, const isdf_midend_params *p, const double *waypoints, const double *x,
+                                      double *cost, double *grad);
 /* getOriTraj for B problems: x (out, B x (4*N0-3)) starts at [backwardT(init_time) | waypoints] and returns the solution; f: B final costs.
  * T (B*N0) and coeffs (6*B*N0 x 3 column-major, piece b*N0+i: the layout of isdf_get_batch_trajectories) are the final trajectories.
  * Any of T / coeffs / ret / iterations / evaluations / rounds may be NULL. */
@@ -346,6 +379,15 @@ int isdf_midend_batch(isdf_ctx *ctx, int B, int N0, const double *head, const do
 int isdf_midend_batch_device(isdf_ctx *ctx, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc,
                              const isdf_midend_params *p, const double *d_waypoints, double *d_x, double *d_T, double *d_coeffs,
                              double *d_f, int32_t *d_ret, int32_t *d_iterations, int32_t *d_evaluations, int32_t *rounds, void *cuda_stream);
+/* ragged forms (see "ragged batches" above): waypoints P - B rows (isdf_path_waypoints' output as it stands; may be NULL when P = B),
+ * x 4P - 3B rows, T P and coeffs 6P x 3 */
+int isdf_midend_batch_ragged(isdf_ctx *ctx, int B, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
+                             const isdf_midend_params *p, const double *waypoints, double *x, double *T, double *coeffs,
+                             double *f, int32_t *ret, int32_t *iterations, int32_t *evaluations, int32_t *rounds);
+int isdf_midend_batch_ragged_device(isdf_ctx *ctx, int B, const int32_t *piece_off, const double *d_head, const double *d_tail,
+                                    int per_problem_bc, const isdf_midend_params *p, const double *d_waypoints, double *d_x, double *d_T,
+                                    double *d_coeffs, double *d_f, int32_t *d_ret, int32_t *d_iterations, int32_t *d_evaluations,
+                                    int32_t *rounds, void *cuda_stream);
 
 /* ---- trajectory clearance check: is a trajectory collision-free over the WHOLE map, and by how much? ------------------------------
  * The reference has no working counterpart (SweptVolumeManager::isTrajCollide, swm:759-767, always returns false), and the cost terms
@@ -750,19 +792,20 @@ int isdf_frontend_path_info(isdf_ctx *ctx, isdf_frontpath_info *out);
  *   1. Front end   isdf_frontend_path_batch(start, goals). A path not found is NO_PATH: no trajectory.
  *   2. Waypoints   isdf_path_waypoints(parlength, the map's res) gives N. N > 290 (the limit of the mid-end and the callback) is TOO_LONG:
  *                  no trajectory. head = [path.front(), 0, 0], tail = [path.back(), 0, 0] (:220-223).
- *   3. Mid-end     isdf_midend_batch(per_problem_bc = 1, p->midend) over the plans with the same N: groups in ascending N, plans in goal
- *                  order. midend_ret < 0 is MIDEND_FAILED: its trajectory is the mid-end's final one (what recent_traj holds, :270) and
+ *   3. Mid-end     isdf_midend_batch_ragged(per_problem_bc = 1, p->midend) over every plan that reaches it, in goal order (one call; each
+ *                  plan's result equals isdf_midend_batch over the plans with its N). midend_ret < 0 is MIDEND_FAILED: its trajectory is the mid-end's final one (what recent_traj holds, :270) and
  *                  the back end does not run for it (:277).
- *   4. Gather      isdf_gather_obstacle_points_batch(half_extent, offset, set_as_points = 1) over the waypoints of the group's plans that
- *                  passed the mid-end. A plan with no point gets no swept-volume term, as the reference's loop over zero points.
+ *   4. Gather      isdf_gather_obstacle_points_batch(half_extent, offset, set_as_points = 1) over the waypoints of the plans that passed
+ *                  the mid-end, in goal order. A plan with no point gets no swept-volume term, as the reference's loop over zero points.
  *   5. Durations   before the back end, problem q's persisted trajectory duration (see isdf_set_points_batch) is what
  *                  updateTraj(mid-end trajectory) (:272) leaves on a fresh context: its total duration (the left-to-right sum of T) when
  *                  shorter than 300 s, else 0. Plans are therefore independent of each other and of the order of the groups.
- *   6. Back end    isdf_lbfgs_batch(per_problem_bc = 1, p->rho, p->backend) from the mid-end x, with the context's flags. The final T and
+ *   6. Back end    isdf_lbfgs_batch_ragged(per_problem_bc = 1, p->rho, p->backend) over those plans from the mid-end x, with the
+ *                  context's flags (one call, every plan active from its first round). The final T and
  *                  coeffs are forwardT + MINCO of the returned x whatever its ret (back_end_optimizer.cpp:140-163), computed without a
  *                  further evaluation. Stage OPTIMISED; backend_ret < 0 is reported and the trajectory still returned (`if (1)`, :297).
  *   7. Certificates with ISDF_PLAN_CERTIFY / ISDF_PLAN_DYNAMICS: isdf_trajectory_certify / isdf_trajectory_dynamics with p->certify /
- *                  p->dynamics and N0 = N on every returned trajectory (OPTIMISED and MIDEND_FAILED).
+ *                  p->dynamics and N0 = N on every returned trajectory (OPTIMISED and MIDEND_FAILED), one call per distinct N.
  * Deviation: the reference's back end is LMBM (lmbm.h, Fortran); the driver here is the project's device L-BFGS. max_iterations 10000 in
  *   the defaults is LMBM's iteration cap (lmbm.h:20-57) taken as an analogue, not an equivalent.
  * Guarantees: results are bit-identical run to run; each plan is bit-identical to the same call with that goal alone; every output is
@@ -782,8 +825,8 @@ int isdf_frontend_path_info(isdf_ctx *ctx, isdf_frontpath_info *out);
  *               its certificate.
  *   Caps too small: after the front end and the waypoints the call returns ISDF_ERR_INVALID; path_off and piece_off give the sizes needed.
  * State the call leaves behind: both obstacle point sets given up and the batched swept-volume term off (also after a failure past the
- *   argument checks); isdf_get_batch_trajectories returns the last group's final trajectories, and the swept-volume t* and per-problem
- *   durations are whatever the last group left; isdf_stats.kernel_launches counts every launch of the call, the other isdf_stats fields
+ *   argument checks); isdf_get_batch_trajectories returns every back-end plan's final trajectory in the ragged layout (plans in goal
+ *   order), and the swept-volume t* and per-problem durations are whatever the back end left; isdf_stats.kernel_launches counts every launch of the call, the other isdf_stats fields
  *   are whatever the last back-end callback left.
  * Device memory: owned by the context, grown on demand. Between stages only the path lengths, the plans' waypoints, the rounds' 4-byte
  *   reads and the results cross to the host.
@@ -814,7 +857,7 @@ typedef struct isdf_plan_result {
     double path_cost, midend_f, backend_f, duration;
 } isdf_plan_result;
 typedef struct isdf_plan_info {     /* the last isdf_plan_batch call */
-    int32_t groups, backend_rounds;  /* distinct N that reached the mid-end; batched back-end evaluations summed over groups */
+    int32_t groups, backend_rounds;  /* distinct N that reached the mid-end; batched evaluations of the one back-end launch */
     double frontend_ms, midend_ms, gather_ms, backend_ms, certify_ms, dynamics_ms;   /* CUDA events on the call's stream */
 } isdf_plan_info;
 /* the values above, flags ISDF_PLAN_CERTIFY | ISDF_PLAN_DYNAMICS, isdf_certify_default_params and isdf_dynamics_default_params(ctx);
