@@ -29,7 +29,7 @@ using namespace isdf;
 __global__ void k_mesh_cells(const __grid_constant__ DevMesh M, int nx, int ny, int nz, double lx, double ly, double lz, double cell,
                              float *dist, uint32_t *seed);
 
-__global__ void k_mesh_cell_lists(const __grid_constant__ DevMesh M, long long ncell, double hd, double list_reach, uint16_t *cnt,
+__global__ void k_mesh_cell_lists(const __grid_constant__ DevMesh M, long long ncell, double hd, double list_reach, double disc_reach, uint16_t *cnt,
                                   const uint32_t *off, uint32_t *cand, float *cand_lb);
 __global__ void k_mesh_cell_pack(long long ncell, const float *dist, const uint32_t *seed, const uint32_t *off, const uint16_t *cnt, uint4 *rec);
 
@@ -482,14 +482,15 @@ extern "C" int isdf_set_shape_mesh_ex(isdf_ctx *c, const double *V, int nV, cons
     // exact candidate lists for every cell a query can land in and not be settled by the cell's distance bracket alone: the discrete
     // path queries within safety_hor of the surface, the swept-volume path within its range bound 2*safety_hor + 0.1 (swm:383) — a
     // flat pass over ~100 listed triangles answers such a query in a tenth of the time of a far-field tree search, and the sign
-    // descent of the swept-volume path is a CHAIN of them
+    // descent of the swept-volume path is a CHAIN of them. Cells wholly within the discrete reach take lists up to
+    // MESH_LIST_CAP_DISCRETE long (read by the discrete scan only, see mesh_list_cnt), every other cell up to MESH_LIST_CAP.
     {
         const double hd = 0.5 * std::sqrt(3.0) * m.gcell;
         const double list_reach = std::max(c->cfg.safety_hor, 2.0 * c->cfg.safety_hor + 0.1) + 2.0 * m.ghd;
         c->mesh.list_reach = list_reach;
         CU_TRY(c->mesh.d_cell_cnt.ensure(ncell)); CU_TRY(c->mesh.d_cell_off.ensure(ncell));
         const unsigned warps_grid = (unsigned)((ncell + 3) / 4);
-        k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->mesh.d_cell_cnt.p, nullptr, nullptr, nullptr);
+        k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->cfg.safety_hor, c->mesh.d_cell_cnt.p, nullptr, nullptr, nullptr);
         c->stats.kernel_launches++;
         CU_TRY(cudaGetLastError());
         std::vector<uint16_t> cnt(ncell);
@@ -501,16 +502,22 @@ extern "C" int isdf_set_shape_mesh_ex(isdf_ctx *c, const double *V, int nV, cons
         if (total > 0 && total < (1ull << 31)) {
             CU_TRY(c->mesh.d_cand.ensure(total)); CU_TRY(c->mesh.d_cand_lb.ensure(total));
             CU_TRY(cudaMemcpyAsync(c->mesh.d_cell_off.p, off.data(), sizeof(uint32_t) * ncell, cudaMemcpyHostToDevice, c->stream));
-            k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->mesh.d_cell_cnt.p, c->mesh.d_cell_off.p, c->mesh.d_cand.p, c->mesh.d_cand_lb.p);
+            k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->cfg.safety_hor, c->mesh.d_cell_cnt.p,
+                                                                 c->mesh.d_cell_off.p, c->mesh.d_cand.p, c->mesh.d_cand_lb.p);
             c->stats.kernel_launches++;
             CU_TRY(cudaGetLastError());
             CU_TRY(cudaStreamSynchronize(c->stream));
             m.cell_off = c->mesh.d_cell_off.p; m.cell_cnt = c->mesh.d_cell_cnt.p; m.cand = c->mesh.d_cand.p; m.cand_lb = c->mesh.d_cand_lb.p;
         }
         if (getenv("ISDF_VERBOSE")) {
-            size_t listed = 0; for (size_t i = 0; i < ncell; i++) listed += cnt[i] != 0;
-            fprintf(stderr, "[isdf] mesh cell grid %d x %d x %d (cell %.3f m), %zu cells with a candidate list, %zu candidates (%.1f MB: ids and lower bounds)\n", m.gdim[0], m.gdim[1],
-                    m.gdim[2], m.gcell, listed, total, total * 8e-6);
+            size_t listed = 0, nlong = 0, long_total = 0;
+            for (size_t i = 0; i < ncell; i++) {
+                listed += cnt[i] != 0;
+                if (cnt[i] > MESH_LIST_CAP) { nlong++; long_total += cnt[i]; }
+            }
+            fprintf(stderr, "[isdf] mesh cell grid %d x %d x %d (cell %.3f m), %zu cells with a candidate list, %zu candidates (%.1f MB: ids and lower bounds); "
+                    "of these %zu lists longer than %d, %zu candidates (%.1f MB)\n", m.gdim[0], m.gdim[1], m.gdim[2], m.gcell, listed, total, total * 8e-6,
+                    nlong, MESH_LIST_CAP, long_total, long_total * 8e-6);
         }
     }
     // fused 16-byte cell records for the discrete scan kernel's cull stage
@@ -549,11 +556,15 @@ __global__ void k_mesh_cells(const __grid_constant__ DevMesh M, int nx, int ny, 
 }
 
 // Candidate lists (one warp per cell). Pass 1 (cand == nullptr): count the triangles within d_c + 2 hd of the cell centre and
-// store the count (0 for cells that are too far, too deep or whose list would exceed LIST_CAP). Pass 2: fill the lists, sorted by
-// ascending distance from the cell centre (ties: triangle index), with each distance's lower bound in cand_lb.
-constexpr int LIST_CAP = MESH_LIST_CAP;
+// store the count (0 for cells that are too far, too deep or whose list would exceed the cell's cap). Pass 2: fill the lists, sorted
+// by ascending distance from the cell centre (ties: triangle index), with each distance's lower bound in cand_lb.
+// The cap is MESH_LIST_CAP_DISCRETE for a cell the discrete scan answers everywhere (d_c + ghd < disc_reach = safety_hor: the same
+// float bound as its cull, so every voxel that lands in the cell is searched, never culled) and MESH_LIST_CAP for every other cell.
+// A cell that the hinge boundary sdf = safety_hor crosses keeps the short cap: only part of its volume is ever answered, so a long
+// list buys less there for its set-up time and memory.
+constexpr int LIST_CAP = MESH_LIST_CAP_DISCRETE;   // the longer of the two caps sizes the shared arrays
 __global__ void __launch_bounds__(128) k_mesh_cell_lists(const __grid_constant__ DevMesh M, long long ncell, double hd, double list_reach,
-                                                         uint16_t *cnt, const uint32_t *off, uint32_t *cand, float *cand_lb) {
+                                                         double disc_reach, uint16_t *cnt, const uint32_t *off, uint32_t *cand, float *cand_lb) {
     __shared__ WideStack stk[4];
     __shared__ double s_d2[4][LIST_CAP];   // pass 2: the cell's hits in emission order, then ranked
     __shared__ int s_tri[4][LIST_CAP];
@@ -579,7 +590,8 @@ __global__ void __launch_bounds__(128) k_mesh_cell_lists(const __grid_constant__
         n += __popc(bal);
     });
     if (cand == nullptr) {
-        if (lane == 0) cnt[cell] = (n <= LIST_CAP) ? (uint16_t)n : (uint16_t)0;
+        const int cap = ((double)M.cell_dist[cell] + M.ghd < disc_reach) ? MESH_LIST_CAP_DISCRETE : MESH_LIST_CAP;
+        if (lane == 0) cnt[cell] = (n <= cap) ? (uint16_t)n : (uint16_t)0;
         return;
     }
     // rank sort: entry i goes to the number of entries before it in (squared distance, triangle) order

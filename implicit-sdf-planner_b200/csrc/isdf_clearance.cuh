@@ -151,7 +151,7 @@ __global__ void __launch_bounds__(CLR_THREADS) k_clearance_scan(const __grid_con
             for (int k = 0; k < nsv; k++) {
                 const ClrSurvivor v = sm.sv[k];
                 const d3 p = mk3(v.px, v.py, v.pz);
-                const int cnt = (int)(v.cnt & 0x7fffffffu);
+                const int cnt = mesh_list_cnt((int)(v.cnt & 0x7fffffffu));   // lists past MESH_LIST_CAP serve the discrete scan only
                 double reach_q = 1e300;
                 if (MODE == 1) {
                     if (p.x < Mh.blo[0] - bv || p.x > Mh.bhi[0] + bv || p.y < Mh.blo[1] - bv || p.y > Mh.bhi[1] + bv || p.z < Mh.blo[2] - bv ||
@@ -165,7 +165,7 @@ __global__ void __launch_bounds__(CLR_THREADS) k_clearance_scan(const __grid_con
                 const float first_lb = has ? __ldg(Mh.cand_lb + v.off + lane) : 0.0f;
                 double d2; d3 c = mk3(0, 0, 0); int tri, feat;
                 nsearch++;
-                if (!mesh_search_rec(Mh, p, reach_q, lane, &sm.stk, cnt, v.off, first_id, first_lb, (int)v.seed, (v.cnt >> 31) != 0u, d2, c, tri, feat)) continue;
+                if (!mesh_search_rec(Mh, p, reach_q, lane, &sm.stk, cnt, v.off, first_id, first_lb, (int)v.seed, (v.cnt >> 31) != 0u, false, d2, c, tri, feat)) continue;
                 d3 g;
                 const double sdf = mesh_finish_t<MODE == 2>(Mh, p, p - c, d2, tri, feat, g);
                 if (clr_better(sdf, v.addr, bv, ba)) { bv = sdf; ba = v.addr; }

@@ -487,7 +487,7 @@ __global__ void __launch_bounds__(DISC_THREADS, ANALYTIC_MIN_BLOCKS) k_discrete_
 // ============================================================================================================================
 // mesh shapes
 struct QRes { double ex, ey, ez; int tri; uint32_t code; int fc; };   // an answered voxel awaiting its deferred tail: e = p - closest point, triangle, voxel code, feature | class << 8 (40 bytes: with the float bounds of WideStack the kernel's shared memory fits the 132 KB carve-out at 4 CTAs/SM, i.e. 124 KB of L1 instead of 92)
-struct Survivor { double px, py, pz; uint32_t off, cnt, seed, code; };   // a voxel that passed the exact culls: body-frame point, its cell's list (cnt bit 31: cell centre inside), seed triangle (0xffffffff: none)
+struct Survivor { double px, py, pz; uint32_t off, cnt, seed, code; };   // a voxel that passed the exact culls: body-frame point, its cell's list (cnt bit 31: cell centre inside, bit 30: cell deeper than safety_hor everywhere), seed triangle (0xffffffff: none)
 struct MeshWarpSmem {
     double pose[16];                     // warp-uniform pose: pos 0..2, R rows 3..11, q (w, x, y, z) 12..15
     double cacc[ROW_CLASSES][8];         // class accumulators
@@ -739,7 +739,9 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
                 if (pass) {
                     Survivor &v = sm.sv[nsv + __popc(bal & lt_mask)];
                     v.px = prel.x; v.py = prel.y; v.pz = prel.z; v.off = rec.z; v.seed = rec.y; v.code = code;
-                    v.cnt = rec.w | ((rec.y != 0xffffffffu && __uint_as_float(rec.x) < 0.0f) ? 0x80000000u : 0u);
+                    const bool in_grid = rec.y != 0xffffffffu;
+                    v.cnt = rec.w | ((in_grid && __uint_as_float(rec.x) < 0.0f) ? 0x80000000u : 0u) |
+                            ((in_grid && (double)__uint_as_float(rec.x) + Mh.ghd <= -sf) ? 0x40000000u : 0u);
                 }
                 nsv += __popc(bal);
                 __syncwarp();
@@ -752,7 +754,7 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
                 auto first_ids = [&](int k, int &id, float &lb) {   // first-pass candidate and its lower bound
                     id = -1; lb = 0.0f;
                     if (k >= nsv) return;
-                    const uint32_t cnt = sm.sv[k].cnt & 0x7fffffffu, off = sm.sv[k].off;
+                    const uint32_t cnt = sm.sv[k].cnt & 0x3fffffffu, off = sm.sv[k].off;
                     if (lane < (int)cnt) { id = (int)__ldg(Mh.cand + off + lane); lb = __ldg(Mh.cand_lb + off + lane); }
                 };
                 int ids0, ids1;
@@ -767,7 +769,8 @@ __global__ void __launch_bounds__(DISC_THREADS, MESH_MIN_BLOCKS) k_discrete_mesh
                         const d3 p = mk3(v.px, v.py, v.pz);
                         const uint32_t cnt_in = v.cnt, qcode = v.code;
                         double d2; d3 c = mk3(0, 0, 0); int tri, feat;
-                        if (mesh_search_rec(Mh, p, sf, lane, &sm.stk, (int)(cnt_in & 0x7fffffffu), v.off, ids0, lbs0, (int)v.seed, (cnt_in >> 31) != 0u, d2, c, tri, feat)) {
+                        if (mesh_search_rec(Mh, p, sf, lane, &sm.stk, (int)(cnt_in & 0x3fffffffu), v.off, ids0, lbs0, (int)v.seed, (cnt_in >> 31) != 0u,
+                                            ((cnt_in >> 30) & 1u) != 0u, d2, c, tri, feat)) {
                             if (lane == 0) {
                                 QRes r;
                                 r.ex = p.x - c.x; r.ey = p.y - c.y; r.ez = p.z - c.z; r.tri = tri; r.code = qcode;

@@ -40,6 +40,14 @@ struct WnNode {
 };
 enum { MESH_SIGN_PSEUDONORMAL = 0, MESH_SIGN_WINDING = 1 };
 
+// Candidate-list caps. A cell the discrete scan can query (centre inside the mesh, or |d_c| - ghd < safety_hor) keeps its list up
+// to MESH_LIST_CAP_DISCRETE candidates, every other cell up to MESH_LIST_CAP. Only the discrete scan reads a list longer than
+// MESH_LIST_CAP: every other search takes such a cell as unlisted (mesh_list_cnt) and answers it from the tree, so its results
+// and tie-breaking do not depend on the longer lists.
+constexpr int MESH_LIST_CAP = 160;
+constexpr int MESH_LIST_CAP_DISCRETE = 512;
+__host__ __device__ inline int mesh_list_cnt(int cnt) { return cnt <= MESH_LIST_CAP ? cnt : 0; }
+
 struct DevMesh {
     const BvhNode *nodes;   // nodes[0] is the root (a single-leaf mesh still gets one node with right = left)
     const WideNode *wnodes; // wnodes[0] is the root of the 32-ary tree
@@ -55,7 +63,8 @@ struct DevMesh {
     const uint32_t *cell_seed;  // triangle (leaf order) nearest to the cell centre: a tight initial bound for queries in the cell
     // exact candidate lists: for a cell with centre c and centre distance d_c, EVERY triangle that can be the closest one for
     // some point of the cell lies within d_c + 2*half_diag of c. Cells near the surface store that set (cell_cnt > 0) and a
-    // query in such a cell is a flat, traversal-free loop over it; cell_cnt == 0 means "search the tree" (far or deep cells).
+    // query in such a cell is a flat, traversal-free loop over it; cell_cnt == 0 means "search the tree" (far or deep cells, or
+    // more candidates than the cell's cap: MESH_LIST_CAP_DISCRETE where the discrete scan can query, MESH_LIST_CAP elsewhere)
     const uint32_t *cell_off;   // offset into cand
     const uint16_t *cell_cnt;   // number of candidates (0 = no list)
     const uint32_t *cand;       // triangle indices (leaf order), each list sorted by ascending distance from the cell centre (ties: index)
@@ -283,7 +292,7 @@ __host__ __device__ inline double mesh_sdf_grad(const DevMesh &M, d3 p, double r
     const bool bounded = (reach < 1e150) && (M.sign_radius > 0.0) && (reach >= M.sign_radius) && (M.sign_mode == MESH_SIGN_PSEUDONORMAL);
     const bool far = mesh_far(M, p, reach, cell);
     if (bounded && far) return reach;                                  // exact: every point of this cell is >= reach away
-    if (cell >= 0 && M.cell_cnt && M.cell_cnt[cell] != 0) {
+    if (cell >= 0 && M.cell_cnt && mesh_list_cnt(M.cell_cnt[cell]) != 0) {
         // flat loop over the cell's exact candidate list: no traversal, no stack, identical code on every lane
         const uint32_t off = M.cell_off[cell];
         const int cnt = (int)M.cell_cnt[cell];
@@ -587,7 +596,6 @@ __device__ __forceinline__ double list_closest(const DevMesh &M, d3 p, int cell,
 // fine-scan chains): all of this lane's candidate ids are requested at once, the 128-byte records of every pass after the first are
 // prefetched into L1 while the first pass computes — one DRAM/L2 round trip for the whole list instead of one per pass. Same
 // arithmetic, same pass order and tie-breaking as list_closest_pre.
-constexpr int MESH_LIST_CAP = 160;                       // longest candidate list a cell may carry (longer: the cell has none)
 constexpr int MESH_LIST_PASSES = MESH_LIST_CAP / 32;
 __device__ __forceinline__ double list_closest_lat(const DevMesh &M, d3 p, uint32_t off, int cnt, d3 &cbest, int &tri, int &feat, int lane) {
     int ids[MESH_LIST_PASSES];
@@ -623,7 +631,7 @@ __device__ __forceinline__ bool mesh_search_warp(const DevMesh &M, d3 p, double 
                                                  double &d2, d3 &c, int &tri, int &feat) {
     const bool bounded = (reach < 1e150) && (M.sign_radius > 0.0) && (reach >= M.sign_radius);
     const int seed = (cell >= 0) ? (int)M.cell_seed[cell] : -1;
-    if (cell >= 0 && M.cell_cnt && M.cell_cnt[cell] != 0) {
+    if (cell >= 0 && M.cell_cnt && mesh_list_cnt(M.cell_cnt[cell]) != 0) {
         d2 = list_closest(M, p, cell, c, tri, feat, lane);       // exact: the list holds every possible closest triangle
     } else if (bounded) {
         d2 = wide_closest(M, p, reach * reach, seed, c, tri, feat, lane, stk);
@@ -641,11 +649,14 @@ __device__ __forceinline__ bool mesh_search_warp(const DevMesh &M, d3 p, double 
 // nearest triangle of the cell centre (-1 outside the grid), inside = the cell centre is inside the mesh. first_id / first_lb: the
 // list's first pass as list_closest_pre takes it. With an exact sign (pseudonormal, reach >= sign_radius) both searches start from
 // the bound reach^2: nothing closer means sdf >= reach when the cell centre is outside (false), and a second, unbounded search when
-// it is inside.
+// it is inside. deep: the caller has shown d_c + ghd <= -reach for the cell, so every point of it is at least reach inside (the
+// ghd slack covers the float rounding of d_c with room to spare for the FP64 distances) and the bounded search would find nothing:
+// the unbounded one runs straight away, with the same result.
 __device__ __forceinline__ bool mesh_search_rec(const DevMesh &M, d3 p, double reach, int lane, WideStack *stk, int cnt, uint32_t off,
-                                                int first_id, float first_lb, int seed, bool inside, double &d2, d3 &c, int &tri, int &feat) {
+                                                int first_id, float first_lb, int seed, bool inside, bool deep, double &d2, d3 &c, int &tri,
+                                                int &feat) {
     const bool bounded = (reach < 1e150) && (M.sign_radius > 0.0) && (reach >= M.sign_radius) && (M.sign_mode == MESH_SIGN_PSEUDONORMAL);
-    double bound2 = bounded ? reach * reach : 1e300;
+    double bound2 = (bounded && !deep) ? reach * reach : 1e300;
     if (cnt != 0) {
         // the list's cell is p's cell, found exactly as the callers' cull stages find it
         const double r_up = list_centre_dist_up(M, p, floor((p.x - M.glo[0]) * M.inv_gcell), floor((p.y - M.glo[1]) * M.inv_gcell),
