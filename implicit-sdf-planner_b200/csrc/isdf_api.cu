@@ -14,6 +14,7 @@
 #include "isdf_sweptvol.cuh"
 #include "isdf_dynlimits.cuh"
 #include "isdf_map.cuh"
+#include "isdf_esdf.cuh"
 #include <queue>
 #include "isdf_host_mesh.cuh"
 #include <cstdio>
@@ -153,6 +154,10 @@ struct isdf_ctx {
         DevBuf<uint32_t> d_bits;
         long long points_used = 0, points_skipped = 0;   // isdf_set_map_cloud*; 0 for dense maps
     } map;
+    struct {   // the map's distance field (isdf_esdf.cuh): squared voxel distances, ESDF_NONE where no site exists; given up with the map
+        bool have = false;
+        DevBuf<uint32_t> d_pos, d_neg;
+    } esdf;
     struct {   // the robot shape; the buffers hold a mesh's device view
         bool have_shape = false;
         DevShape shape = {};
@@ -658,6 +663,13 @@ static int map_size_check(isdf_ctx *c, long long X, long long Y, long long Z, do
     return 0;
 }
 
+// gives up the map and the distance field built on it (its memory too: it is 8 bytes per voxel)
+static void drop_map(isdf_ctx *c) {
+    c->map.have_map = false;
+    c->esdf.have = false;
+    c->esdf.d_pos = {}; c->esdf.d_neg = {};
+}
+
 // the map the bits in c->map.d_bits describe
 static void commit_map(isdf_ctx *c, int X, int Y, int Z, const double *bmin, const double *bmax, double res, long long used, long long skipped) {
     DevGrid &g = c->map.grid;
@@ -673,7 +685,7 @@ static int set_map_impl(isdf_ctx *c, const T *occ, int X, int Y, int Z, const do
     if (X < 1 || Y < 1 || Z < 1 || !(res > 0)) return fail(ISDF_ERR_INVALID, "bad map size");
     if (int rc = map_size_check(c, X, Y, Z, res)) return rc;
     if (set_device(c)) return ISDF_ERR_CUDA;
-    c->map.have_map = false;   // d_bits.ensure may free the current grid
+    drop_map(c);   // d_bits.ensure may free the current grid
     const size_t nvox = (size_t)X * Y * Z;
     DevBuf<T> d_occ;
     cudaError_t e = d_occ.upload(occ, nvox, c->stream);
@@ -720,7 +732,7 @@ static int cloud_grid_blocks(isdf_ctx *c, long long n) { return (int)std::min<lo
 static int set_map_cloud_impl(isdf_ctx *c, const char *d_pts, long long n, int stride, double res, int thr, cudaStream_t st) {
     const int blocks = cloud_grid_blocks(c, n);
     auto cuda_fail = [&](cudaError_t e) {
-        c->map.have_map = false;
+        drop_map(c);
         return fail(ISDF_ERR_CUDA, std::string("isdf_set_map_cloud: ") + cudaGetErrorString(e));
     };
     // 1. bounds: exact float extrema of the finite records (order-preserving uint32 min / max) and the number of skipped records
@@ -761,7 +773,7 @@ static int set_map_cloud_impl(isdf_ctx *c, const char *d_pts, long long n, int s
     const int X = (int)dim[0], Y = (int)dim[1], Z = (int)dim[2];
     if (int rc = map_size_check(c, X, Y, Z, res)) return fail(rc, g_err + dims_msg);
     // 3. occupancy (the previous map is given up from here on)
-    c->map.have_map = false;
+    drop_map(c);
     CloudFrame F;
     for (int a = 0; a < 3; a++) F.bmin[a] = bmin[a];
     F.res = res; F.X = X; F.Y = Y; F.Z = Z; F.Zw = (Z + 31) / 32;
@@ -807,7 +819,7 @@ extern "C" int isdf_set_map_cloud(isdf_ctx *c, const void *points, int64_t n, in
     cudaError_t e = d_pts.ensure(bytes);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_pts.p, points, bytes, cudaMemcpyHostToDevice, c->stream);
     if (e != cudaSuccess) {
-        c->map.have_map = false;
+        drop_map(c);
         return fail(ISDF_ERR_CUDA, std::string("isdf_set_map_cloud: ") + cudaGetErrorString(e));
     }
     return set_map_cloud_impl(c, d_pts.p, n, stride_bytes, res, sta_threshold, c->stream);
@@ -869,6 +881,125 @@ static int get_map_impl(isdf_ctx *c, T *out, int64_t n) {
 
 extern "C" int isdf_get_map_u8(isdf_ctx *c, uint8_t *occ, int64_t n) { return get_map_impl<uint8_t>(c, occ, n); }
 extern "C" int isdf_get_map_f64(isdf_ctx *c, double *grid_map, int64_t n) { return get_map_impl<double>(c, grid_map, n); }
+
+// ---- distance field of the map (GridMap3D::generateESDF3d, getSDFValue, getSDFValueWithGrad; isdf_esdf.cuh) --------------------
+extern "C" int isdf_map_esdf(isdf_ctx *c) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
+    const DevGrid &g = c->map.grid;
+    if (g.X > ESDF_AXIS_MAX || g.Y > ESDF_AXIS_MAX || g.Z > ESDF_AXIS_MAX)
+        return fail(ISDF_ERR_UNSUPPORTED, "an axis longer than 46341 voxels: the reference's fillESDF computes q * q in int, which overflows "
+                                          "there, so its distance field is undefined");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    c->esdf.have = false;   // rebuilt in place: the old field is gone from here on
+    auto cuda_fail = [&](cudaError_t e) {
+        c->esdf.have = false;
+        c->esdf.d_pos = {}; c->esdf.d_neg = {};
+        return fail(ISDF_ERR_CUDA, std::string("isdf_map_esdf: ") + cudaGetErrorString(e));
+    };
+    const long long X = g.X, Y = g.Y, Z = g.Z, nvox = X * Y * Z;
+    cudaError_t e = c->esdf.d_pos.ensure((size_t)nvox);
+    if (e == cudaSuccess) e = c->esdf.d_neg.ensure((size_t)nvox);
+    if (e != cudaSuccess) return cuda_fail(e);
+    uint32_t *pos = c->esdf.d_pos.p, *neg = c->esdf.d_neg.p;
+    // pass z: one warp per row
+    const long long rows = X * Y;
+    k_esdf_z<<<(unsigned)std::min<long long>((rows * 32 + 255) / 256, (long long)c->sm_count * 16), 256, 0, c->stream>>>(g.bits, rows, g.Z, g.Zw, pos, neg);
+    c->stats.kernel_launches++;
+    if ((e = cudaGetLastError()) != cudaSuccess) return cuda_fail(e);
+    // passes y and x: at most one thread per line of a field, and one stack of m entries per thread, so the stack never exceeds
+    // 8 bytes per voxel (DESIGN §3.15)
+    int per_sm = 0;
+    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_esdf_line, 256, 0)) != cudaSuccess) return cuda_fail(e);
+    const long long resident = (long long)std::max(per_sm, 1) * c->sm_count * 256;
+    EsdfLines P[2];
+    P[0] = {{pos, neg}, X * Z, Y * Z, Z, (int)Y, (int)Z};   // pass y: lines (x, z)
+    P[1] = {{pos, neg}, Y * Z, Z, Y * Z, (int)X, (int)Z};   // pass x: lines (y, z)
+    long long G[2], stack = 0;
+    for (int k = 0; k < 2; k++) {
+        G[k] = std::min(P[k].nlines, resident);
+        stack = std::max(stack, G[k] * P[k].m);
+    }
+    DevBuf<uint2> d_stack;
+    if ((e = d_stack.ensure((size_t)stack)) != cudaSuccess) return cuda_fail(e);
+    for (int k = 0; k < 2; k++) {
+        k_esdf_line<<<(unsigned)((G[k] + 255) / 256), 256, 0, c->stream>>>(P[k], G[k], d_stack.p);
+        c->stats.kernel_launches++;
+        if ((e = cudaGetLastError()) != cudaSuccess) return cuda_fail(e);
+    }
+    if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) return cuda_fail(e);
+    c->esdf.have = true;
+    return 0;
+}
+
+static int esdf_field_check(int field) {
+    if (field != ESDF_POSITIVE && field != ESDF_NEGATIVE && field != ESDF_SIGNED) return fail(ISDF_ERR_INVALID, "unknown ESDF field");
+    return 0;
+}
+
+extern "C" int isdf_get_esdf_f64(isdf_ctx *c, int field, double *out, int64_t n) {
+    if (!c || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (int rc = esdf_field_check(field)) return rc;
+    if (!c->esdf.have) return fail(ISDF_ERR_STATE, "no ESDF: build it with isdf_map_esdf after setting the map");
+    const DevGrid &g = c->map.grid;
+    const long long total = (long long)g.X * g.Y * g.Z;
+    if (n != total) return fail(ISDF_ERR_INVALID, "n must be X*Y*Z of the map");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    const long long chunk = 4ll << 20;   // 32 MiB of doubles per chunk
+    DevBuf<double> d_out;
+    CU_TRY(d_out.ensure((size_t)std::min(total, chunk)));
+    for (long long i0 = 0; i0 < total; i0 += chunk) {
+        const long long cnt = std::min(chunk, total - i0);
+        k_esdf_expand<<<cloud_grid_blocks(c, cnt), 256, 0, c->stream>>>(c->esdf.d_pos.p, c->esdf.d_neg.p, field, g.res, i0, cnt, d_out.p);
+        c->stats.kernel_launches++;
+        CU_TRY(cudaGetLastError());
+        CU_TRY(cudaMemcpyAsync(out + i0, d_out.p, cnt * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaStreamSynchronize(c->stream));
+    }
+    return 0;
+}
+
+static int esdf_query_check(isdf_ctx *c, int field, const double *pts, int64_t n, const double *dist) {
+    if (!c || !pts || !dist) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (n < 0) return fail(ISDF_ERR_INVALID, "n < 0");
+    if (int rc = esdf_field_check(field)) return rc;
+    if (!c->esdf.have) return fail(ISDF_ERR_STATE, "no ESDF: build it with isdf_map_esdf after setting the map");
+    return 0;
+}
+
+static void esdf_query_launch(isdf_ctx *c, int field, const double *d_pts, long long n, double *d_dist, double *d_grad, cudaStream_t st) {
+    const DevGrid &g = c->map.grid;
+    EsdfView V;
+    V.pos = c->esdf.d_pos.p; V.neg = c->esdf.d_neg.p; V.X = g.X; V.Y = g.Y; V.Z = g.Z; V.res = g.res;
+    for (int a = 0; a < 3; a++) { V.bmin[a] = g.bmin[a]; V.bmax[a] = g.bmax[a]; }
+    k_esdf_query<<<(unsigned)std::min<long long>((n + 255) / 256, (long long)c->sm_count * 16), 256, 0, st>>>(V, field, d_pts, n, d_dist, d_grad);
+    c->stats.kernel_launches++;
+}
+
+extern "C" int isdf_esdf_query(isdf_ctx *c, int field, const double *pts, int64_t n, double *dist, double *grad) {
+    if (int rc = esdf_query_check(c, field, pts, n, dist)) return rc;
+    if (n == 0) return 0;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    DevBuf<double> d_pts, d_dist, d_grad;
+    CU_TRY(d_pts.upload(pts, (size_t)n * 3, c->stream));
+    CU_TRY(d_dist.ensure((size_t)n));
+    if (grad) CU_TRY(d_grad.ensure((size_t)n * 3));
+    esdf_query_launch(c, field, d_pts.p, n, d_dist.p, grad ? d_grad.p : nullptr, c->stream);
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaMemcpyAsync(dist, d_dist.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    if (grad) CU_TRY(cudaMemcpyAsync(grad, d_grad.p, (size_t)n * 3 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+extern "C" int isdf_esdf_query_device(isdf_ctx *c, int field, const double *d_pts, int64_t n, double *d_dist, double *d_grad, void *cuda_stream) {
+    if (int rc = esdf_query_check(c, field, d_pts, n, d_dist)) return rc;
+    if (n == 0) return 0;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    esdf_query_launch(c, field, d_pts, n, d_dist, d_grad, (cudaStream_t)cuda_stream);
+    CU_TRY(cudaGetLastError());
+    return 0;
+}
 
 // getPointsInAABB (pcs:148-170): one CTA; thread = (x, y) row of the clamped index box — popcount of the row's z-run, block-wide exclusive scan
 // for the row's output offset, then every thread writes its row's voxel centres in z order: the reference's x -> y -> z output order

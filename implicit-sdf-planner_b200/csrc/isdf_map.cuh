@@ -98,10 +98,11 @@ struct CloudFrame {
     int X, Y, Z, Zw;
 };
 
-// GridMap3D::getGridIndex (Gridmap3D.cpp:135-175) for a point inside the bounds (isInMap holds for every finite record), with its
-// clamps as written: "iy < 0" and "iz < 0" reset ix, not iy / iz (quirk Q6; unreachable here since every coordinate is >= bmin)
-__device__ __forceinline__ void cloud_index(const CloudFrame &F, float x, float y, float z, int &ix, int &iy, int &iz) {
-    const double dx = (double)x - F.bmin[0], dy = (double)y - F.bmin[1], dz = (double)z - F.bmin[2];
+// GridMap3D::getGridIndex (Gridmap3D.cpp:135-175) for a point inside the bounds (the caller has checked isInMap), with its clamps as
+// written: "iy < 0" and "iz < 0" reset ix, not iy / iz (quirk Q6; unreachable since every coordinate is >= bmin). The cloud path and the
+// ESDF queries (isdf_esdf.cuh) share it.
+__device__ __forceinline__ void grid_index(const CloudFrame &F, double x, double y, double z, int &ix, int &iy, int &iz) {
+    const double dx = x - F.bmin[0], dy = y - F.bmin[1], dz = z - F.bmin[2];
     ix = (int)floor(dx / F.res); iy = (int)floor(dy / F.res); iz = (int)floor(dz / F.res);
     if (ix < 0) ix = 0;
     if (ix >= F.X) ix = F.X - 1;
@@ -109,6 +110,10 @@ __device__ __forceinline__ void cloud_index(const CloudFrame &F, float x, float 
     if (iy >= F.Y) iy = F.Y - 1;
     if (iz < 0) ix = 0;
     if (iz >= F.Z) iz = F.Z - 1;
+}
+// a cloud record (isInMap holds for every finite record)
+__device__ __forceinline__ void cloud_index(const CloudFrame &F, float x, float y, float z, int &ix, int &iy, int &iz) {
+    grid_index(F, (double)x, (double)y, (double)z, ix, iy, iz);
 }
 
 // sta_threshold == 1: set the voxel's bit directly. Lanes of a warp that hit the same 32-bit word (neighbouring records of a spatially

@@ -42,12 +42,13 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_trajectory_dynamics_device", "isdf_gather_obstacle_points_batch", "isdf_plan_default_params", "isdf_plan_batch",
                "isdf_get_plan_info", "isdf_callback_batch_ragged", "isdf_callback_batch_ragged_device", "isdf_lbfgs_batch_ragged",
                "isdf_lbfgs_batch_ragged_device", "isdf_midend_callback_batch_ragged", "isdf_midend_batch_ragged",
-               "isdf_midend_batch_ragged_device"]
+               "isdf_midend_batch_ragged_device", "isdf_map_esdf", "isdf_get_esdf_f64", "isdf_esdf_query", "isdf_esdf_query_device"]
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
 DYN_QUANTITIES = ["speed", "acceleration", "body_rate", "tilt", "thrust"]   # q of isdf_dynamics_summary; mask bit 5: the thrust minimum
 PLAN_CERTIFY, PLAN_DYNAMICS = 1, 2                                             # isdf_plan_params.flags
 PLAN_FAILED, NO_PATH, TOO_LONG, MIDEND_FAILED, OPTIMISED = -1, 0, 1, 2, 3      # isdf_plan_result.stage
+ESDF_FIELDS = dict(positive=0, negative=1, signed=2)                            # isdf_esdf_field
 
 
 class KernelConfig(C.Structure):
@@ -317,6 +318,10 @@ def load_library(path=None):
     lib.isdf_get_map_info.argtypes = [vp, C.POINTER(MapInfo)]
     lib.isdf_get_map_u8.argtypes = [vp, C.POINTER(C.c_uint8), C.c_int64]
     lib.isdf_get_map_f64.argtypes = [vp, dp, C.c_int64]
+    lib.isdf_map_esdf.argtypes = [vp]
+    lib.isdf_get_esdf_f64.argtypes = [vp, C.c_int, dp, C.c_int64]
+    lib.isdf_esdf_query.argtypes = [vp, C.c_int, dp, C.c_int64, dp, dp]
+    lib.isdf_esdf_query_device.argtypes = [vp, C.c_int, vp, C.c_int64, vp, vp, vp]
     fpp, u8p = C.POINTER(FrontPathParams), C.POINTER(C.c_uint8)
     lib.isdf_frontend_path.argtypes = [vp, dp, dp, fpp, C.c_int, dp, dp, ip, dp, u8p]
     lib.isdf_frontend_path_batch.argtypes = [vp, dp, C.c_int, dp, fpp, C.c_int, dp, dp, ip, dp, u8p]
@@ -564,6 +569,53 @@ class Evaluator:
         out = np.empty((X, Y, Z), dtype=np.float64)
         self._check(self.lib.isdf_get_map_f64(self.h, _dp(out), out.size))
         return out
+
+    # ---- distance field of the map (include/isdf.h: isdf_map_esdf) ----
+    @staticmethod
+    def _esdf_field(field):
+        if field not in ESDF_FIELDS:
+            raise ValueError(f"field must be one of {sorted(ESDF_FIELDS)}, got {field!r}")
+        return ESDF_FIELDS[field]
+
+    def map_esdf(self):
+        """GridMap3D::generateESDF3d on the current map: builds both distance fields on the device"""
+        self._check(self.lib.isdf_map_esdf(self.h))
+
+    def get_esdf(self, field="positive"):
+        """one field ("positive", "negative" or "signed") as an (X, Y, Z) float64 array"""
+        f = self._esdf_field(field)
+        X, Y, Z = self.map_info()["dims"]
+        out = np.empty((X, Y, Z), dtype=np.float64)
+        self._check(self.lib.isdf_get_esdf_f64(self.h, f, _dp(out), out.size))
+        return out
+
+    def esdf_query(self, points, field="positive", grad=True):
+        """getSDFValueWithGrad (grad=True: returns (dist (n,), grad (n, 3))) or getSDFValue (grad=False: returns dist) at (n, 3) points"""
+        f = self._esdf_field(field)
+        p = _f64(points).reshape(-1, 3)
+        n = p.shape[0]
+        dist = np.empty(n)
+        g = np.empty((n, 3)) if grad else None
+        self._check(self.lib.isdf_esdf_query(self.h, f, _dp(p), n, _dp(dist), _dp(g)))
+        return (dist, g) if grad else dist
+
+    def esdf_query_device(self, points, field="positive", grad=True, stream=0):
+        """the same on a contiguous float64 (n, 3) torch tensor on the context's device; returns tensors on that device, enqueued on
+        stream (a raw cudaStream_t; 0 = the legacy default stream) and not waited for"""
+        import torch
+        f = self._esdf_field(field)
+        if points.dtype != torch.float64 or points.dim() != 2 or points.shape[1] != 3:
+            raise TypeError(f"points must be a float64 (n, 3) tensor, got {points.dtype} {tuple(points.shape)}")
+        if not points.is_contiguous():
+            raise ValueError("points must be contiguous")
+        n = points.shape[0]
+        dist = torch.empty(n, dtype=torch.float64, device=points.device)
+        g = torch.empty((n, 3), dtype=torch.float64, device=points.device) if grad else None
+        if n == 0:   # an empty tensor has no storage to point at
+            return (dist, g) if grad else dist
+        self._check(self.lib.isdf_esdf_query_device(self.h, f, C.c_void_p(points.data_ptr()), n, C.c_void_p(dist.data_ptr()),
+                                                    C.c_void_p(g.data_ptr()) if grad else None, C.c_void_p(stream)))
+        return (dist, g) if grad else dist
 
     def points_in_aabb(self, centre, half, cap=100000):
         out = np.zeros((cap, 3))

@@ -180,6 +180,46 @@ int isdf_get_map_info(isdf_ctx *ctx, isdf_map_info *out);
 int isdf_get_map_u8(isdf_ctx *ctx, uint8_t *occ, int64_t n);
 int isdf_get_map_f64(isdf_ctx *ctx, double *grid_map, int64_t n);
 
+/* ---- distance field of the map: replaces GridMap3D::generateESDF3d (grid:361-525), getSDFValue and getSDFValueWithGrad
+ * (GridMap3D.h:114-193) ------------------------------------------------------------------------------------------------------
+ *   Definition  POSITIVE at a voxel is res * sqrt((double)d2), d2 the exact integer squared voxel distance to the nearest occupied voxel
+ *               (0 inside obstacles); NEGATIVE is the same with free voxels as the sites (0 in free space). A field whose map has no site
+ *               is res * sqrt(DBL_MAX) everywhere, as in the reference, not inf. Both are computed on the map's stored 0 / 1 occupancy
+ *               and are bit-identical to the reference's grid_esdf and grid_map_buffer_neg after generateESDF3d on isdf_get_map_f64's
+ *               output, for every map the call accepts.
+ *   SIGNED      v = POSITIVE; if (NEGATIVE > 0.0) v += (-NEGATIVE + res). The reference's grid_map_buffer_all adds the occupancy value
+ *               grid_map where this adds POSITIVE (grid:513-522); SIGNED is the signed field that sum was evidently meant to be (the
+ *               Fast-Planner convention), with the reference's operation order. grid_map_buffer_all itself is not exposed (DESIGN §6).
+ *   Lifetime    the field belongs to ctx: isdf_map_esdf builds it (again) for the current map; any map setter that succeeds gives it up,
+ *               a refused setter leaves map and field in place, and a CUDA failure of isdf_map_esdf or of a map setter leaves no field.
+ *               No other call builds or uses it. It holds 8 bytes per voxel on the device; building needs at most 8 more.
+ * Every call counts its launches in isdf_stats.kernel_launches and touches no other field. */
+typedef enum isdf_esdf_field {
+    ISDF_ESDF_POSITIVE = 0,   /* grid_esdf: distance to the nearest occupied voxel centre, 0 inside obstacles */
+    ISDF_ESDF_NEGATIVE = 1,   /* grid_map_buffer_neg: distance to the nearest free voxel centre, 0 in free space */
+    ISDF_ESDF_SIGNED   = 2    /* POSITIVE, plus (-NEGATIVE + res) where NEGATIVE > 0 */
+} isdf_esdf_field;
+/* generateESDF3d on the current map: both fields, three launches. Errors: ISDF_ERR_INVALID for a NULL ctx; ISDF_ERR_STATE without a
+ * map; ISDF_ERR_UNSUPPORTED for a map with an axis longer than 46341 voxels (the reference's fillESDF computes q * q in int, which
+ * overflows there, so it has no defined field to match). */
+int isdf_map_esdf(isdf_ctx *ctx);
+/* one field as X*Y*Z doubles in the setters' layout (address ix*Y*Z + iy*Z + iz), expanded on the device in bounded chunks.
+ * Errors: ISDF_ERR_INVALID for a NULL pointer, an unknown field or n != X*Y*Z; ISDF_ERR_STATE without a field. */
+int isdf_get_esdf_f64(isdf_ctx *ctx, int field, double *out, int64_t n);
+/* getSDFValueWithGrad (grad != NULL) or getSDFValue (grad == NULL) on one field at n points (pts and grad n x 3 row-major, dist n),
+ * operation for operation, so bit-identical to the reference on that field, including its quirks (DESIGN §6):
+ *   - the base corner is getGridIndex(pos - 0.5 res): clamped to the top index, and (0, 0, 0) when pos - 0.5 res lies outside
+ *     [bmin, bmax], so points outside the map or in its first half voxel extrapolate from corner (0, 0, 0);
+ *   - a corner past the top index reads 0 (getGridSDFValue(const Vector3i &)), so values fall toward 0 at the upper faces;
+ *   - bmax is the map's own (isdf_get_map_info): for a cloud-built map the cloud's maximum, not bmin + X*res.
+ * A point with a NaN or Inf coordinate gives NaN value and gradient (undefined behaviour in the reference). Errors: ISDF_ERR_INVALID
+ * for a NULL pts / dist / ctx, n < 0 or an unknown field; ISDF_ERR_STATE without a field. */
+int isdf_esdf_query(isdf_ctx *ctx, int field, const double *pts, int64_t n, double *dist, double *grad);
+/* the same with d_pts, d_dist and d_grad (may be NULL) on ctx's device, enqueued on cuda_stream and not waited for: the results are
+ * ready when that stream reaches them. The field must not be given up or rebuilt before then. */
+int isdf_esdf_query_device(isdf_ctx *ctx, int field, const double *d_pts, int64_t n, double *d_dist, double *d_grad,
+                           void *cuda_stream);
+
 /* PCSmapManager::getPointsInAABB (pcs:148-170) on the device map; writes up to cap centres (cap x 3), returns count in *n */
 int isdf_points_in_aabb(isdf_ctx *ctx, const double *centre, double half_extent, double *out_points, int cap, int *n);
 
