@@ -15,6 +15,7 @@
 #include "isdf_dynlimits.cuh"
 #include "isdf_map.cuh"
 #include "isdf_esdf.cuh"
+#include "isdf_states.cuh"
 #include <queue>
 #include "isdf_host_mesh.cuh"
 #include <cstdio>
@@ -253,6 +254,10 @@ struct isdf_ctx {
         cudaEvent_t ev[2] = {};
         isdf_plan_info info = {};
     } plan;
+    struct {   // trajectory states and posed body points (isdf_states.cuh): the host forms' staging, one pinned block and one copy each way
+        PinnedBuf<double> h;
+        DevBuf<double> d_in, d_out;
+    } exec;
     struct {   // peer-memory reduction (isdf_peer.cuh)
         DevBuf<char> buf;                    // own exchange buffer (exported through CUDA IPC)
         void *open[PEER_MAX] = {};           // peers' buffers opened here (null for self / unused)
@@ -997,6 +1002,114 @@ extern "C" int isdf_esdf_query_device(isdf_ctx *c, int field, const double *d_pt
     if (n == 0) return 0;
     if (set_device(c)) return ISDF_ERR_CUDA;
     esdf_query_launch(c, field, d_pts, n, d_dist, d_grad, (cudaStream_t)cuda_stream);
+    CU_TRY(cudaGetLastError());
+    return 0;
+}
+
+// ---- executing a trajectory (isdf_states.cuh): states at (trajectory, local time) queries, and the body posed at states ----
+static int swept_traj_check(int N, const double *T, const double *coeffs);
+
+static const long long STATES_MAX_Q = std::numeric_limits<int64_t>::max() / (8 * STATE_DOUBLES);   // Q records of 160 bytes stay addressable
+
+static int states_args_check(isdf_ctx *c, int B, const void *piece_off, const void *T, const void *coeffs, int64_t Q, const void *traj,
+                             const void *times, const void *out) {
+    if (!c || !piece_off || !T || !coeffs || !traj || !times || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (B < 1) return fail(ISDF_ERR_INVALID, "B < 1");
+    if (Q < 0 || Q > STATES_MAX_Q) return fail(ISDF_ERR_INVALID, "Q < 0 or Q * 160 bytes beyond int64");
+    return 0;
+}
+
+static void states_launch(isdf_ctx *c, int B, const int *d_off, const double *d_T, const double *d_C, long long Q, const int *d_traj,
+                          const double *d_times, double *d_out, cudaStream_t st) {
+    const FlatParams &g = c->dcfg.fp;
+    const FlatForwardParams fp = {g.mass, g.grav, g.dh_over_m, c->cfg.vert_drag, g.cp, g.veps};
+    const long long blocks = std::min<long long>((Q + STATES_THREADS - 1) / STATES_THREADS, 0x7fffffffll);
+    k_traj_states<<<(unsigned)blocks, STATES_THREADS, 0, st>>>(d_off, d_T, d_C, B, Q, d_traj, d_times, fp, d_out);
+    c->stats.kernel_launches++;
+}
+
+extern "C" int isdf_trajectory_states(isdf_ctx *c, int B, const int32_t *piece_off, const double *T, const double *coeffs, int64_t Q,
+                                      const int32_t *traj, const double *times, double *out) {
+    if (int rc = states_args_check(c, B, piece_off, T, coeffs, Q, traj, times, out)) return rc;
+    if (piece_off[0] != 0) return fail(ISDF_ERR_INVALID, "piece_off[0] must be 0");
+    for (int b = 0; b < B; b++) if (piece_off[b + 1] < piece_off[b]) return fail(ISDF_ERR_INVALID, "piece_off must not decrease");
+    const int P = piece_off[B];
+    if (int rc = swept_traj_check(P, T, coeffs)) return rc;
+    for (long long q = 0; q < Q; q++) if (traj[q] < 0 || traj[q] >= B) return fail(ISDF_ERR_INVALID, "traj[q] outside [0, B)");
+    if (Q == 0) return 0;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    // one pinned block and one copy each way: in = [coeffs 18P | T P | times Q | piece_off B + 1, traj Q (int32)], out = Q records
+    const size_t nC = (size_t)19 * P, nin = nC + (size_t)Q + ((size_t)B + 1 + (size_t)Q + 1) / 2, nout = (size_t)STATE_DOUBLES * Q;
+    auto &x = c->exec;
+    CU_TRY(x.h.ensure(std::max(nin, nout))); CU_TRY(x.d_in.ensure(nin)); CU_TRY(x.d_out.ensure(nout));
+    double *h = x.h.p;
+    std::memcpy(h, coeffs, sizeof(double) * 18 * (size_t)P);
+    std::memcpy(h + 18 * (size_t)P, T, sizeof(double) * P);
+    std::memcpy(h + nC, times, sizeof(double) * Q);
+    int32_t *hi = reinterpret_cast<int32_t *>(h + nC + Q);
+    std::memcpy(hi, piece_off, sizeof(int32_t) * ((size_t)B + 1));
+    std::memcpy(hi + B + 1, traj, sizeof(int32_t) * Q);
+    CU_TRY(cudaMemcpyAsync(x.d_in.p, h, sizeof(double) * nin, cudaMemcpyHostToDevice, c->stream));
+    const double *d = x.d_in.p;
+    const int *di = reinterpret_cast<const int *>(d + nC + Q);
+    states_launch(c, B, di, d + 18 * (size_t)P, d, Q, di + B + 1, d + nC, x.d_out.p, c->stream);
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaMemcpyAsync(h, x.d_out.p, sizeof(double) * nout, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(cudaStreamSynchronize(c->stream));
+    std::memcpy(out, h, sizeof(double) * nout);
+    return 0;
+}
+
+extern "C" int isdf_trajectory_states_device(isdf_ctx *c, int B, const int32_t *d_piece_off, const double *d_T, const double *d_coeffs, int64_t Q,
+                                             const int32_t *d_traj, const double *d_times, double *d_out, void *cuda_stream) {
+    if (int rc = states_args_check(c, B, d_piece_off, d_T, d_coeffs, Q, d_traj, d_times, d_out)) return rc;
+    if (Q == 0) return 0;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    states_launch(c, B, d_piece_off, d_T, d_coeffs, Q, d_traj, d_times, d_out, (cudaStream_t)cuda_stream);
+    CU_TRY(cudaGetLastError());
+    return 0;
+}
+
+static int pose_args_check(isdf_ctx *c, int64_t Q, const void *states, int P, const void *body, const void *out) {
+    if (!c || !states || !body || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (Q < 0 || Q > STATES_MAX_Q) return fail(ISDF_ERR_INVALID, "Q < 0 or Q * 160 bytes beyond int64");
+    if (P < 0) return fail(ISDF_ERR_INVALID, "P < 0");
+    if (P > 0 && Q > std::numeric_limits<int64_t>::max() / (8 * 3 * (int64_t)P)) return fail(ISDF_ERR_INVALID, "Q * P * 3 doubles beyond int64");
+    return 0;
+}
+
+static void pose_launch(isdf_ctx *c, long long Q, const double *d_states, int P, const double *d_body, double *d_out, cudaStream_t st) {
+    const long long L = 3ll * P;
+    const int S = (int)std::max(1ll, std::min<long long>((POSE_TARGET + L - 1) / L, POSE_MAX_STATES));
+    const long long blocks = std::min<long long>((Q + S - 1) / S, 0x7fffffffll);
+    k_pose_points<<<(unsigned)blocks, POSE_THREADS, 0, st>>>(Q, d_states, P, d_body, S, d_out);
+    c->stats.kernel_launches++;
+}
+
+extern "C" int isdf_pose_points(isdf_ctx *c, int64_t Q, const double *states, int P, const double *body, double *out) {
+    if (int rc = pose_args_check(c, Q, states, P, body, out)) return rc;
+    if (Q == 0 || P == 0) return 0;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    // in = [states 20 Q | body 3 P], out = 3 P Q
+    const size_t ns = (size_t)STATE_DOUBLES * Q, nin = ns + 3 * (size_t)P, nout = 3 * (size_t)P * (size_t)Q;
+    auto &x = c->exec;
+    CU_TRY(x.h.ensure(std::max(nin, nout))); CU_TRY(x.d_in.ensure(nin)); CU_TRY(x.d_out.ensure(nout));
+    std::memcpy(x.h.p, states, sizeof(double) * ns);
+    std::memcpy(x.h.p + ns, body, sizeof(double) * 3 * (size_t)P);
+    CU_TRY(cudaMemcpyAsync(x.d_in.p, x.h.p, sizeof(double) * nin, cudaMemcpyHostToDevice, c->stream));
+    pose_launch(c, Q, x.d_in.p, P, x.d_in.p + ns, x.d_out.p, c->stream);
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaMemcpyAsync(x.h.p, x.d_out.p, sizeof(double) * nout, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(cudaStreamSynchronize(c->stream));
+    std::memcpy(out, x.h.p, sizeof(double) * nout);
+    return 0;
+}
+
+extern "C" int isdf_pose_points_device(isdf_ctx *c, int64_t Q, const double *d_states, int P, const double *d_body, double *d_out, void *cuda_stream) {
+    if (int rc = pose_args_check(c, Q, d_states, P, d_body, d_out)) return rc;
+    if (Q == 0 || P == 0) return 0;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    pose_launch(c, Q, d_states, P, d_body, d_out, (cudaStream_t)cuda_stream);
     CU_TRY(cudaGetLastError());
     return 0;
 }

@@ -42,13 +42,15 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_trajectory_dynamics_device", "isdf_gather_obstacle_points_batch", "isdf_plan_default_params", "isdf_plan_batch",
                "isdf_get_plan_info", "isdf_callback_batch_ragged", "isdf_callback_batch_ragged_device", "isdf_lbfgs_batch_ragged",
                "isdf_lbfgs_batch_ragged_device", "isdf_midend_callback_batch_ragged", "isdf_midend_batch_ragged",
-               "isdf_midend_batch_ragged_device", "isdf_map_esdf", "isdf_get_esdf_f64", "isdf_esdf_query", "isdf_esdf_query_device"]
+               "isdf_midend_batch_ragged_device", "isdf_map_esdf", "isdf_get_esdf_f64", "isdf_esdf_query", "isdf_esdf_query_device",
+               "isdf_trajectory_states", "isdf_trajectory_states_device", "isdf_pose_points", "isdf_pose_points_device"]
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
 DYN_QUANTITIES = ["speed", "acceleration", "body_rate", "tilt", "thrust"]   # q of isdf_dynamics_summary; mask bit 5: the thrust minimum
 PLAN_CERTIFY, PLAN_DYNAMICS = 1, 2                                             # isdf_plan_params.flags
 PLAN_FAILED, NO_PATH, TOO_LONG, MIDEND_FAILED, OPTIMISED = -1, 0, 1, 2, 3      # isdf_plan_result.stage
 ESDF_FIELDS = dict(positive=0, negative=1, signed=2)                            # isdf_esdf_field
+STATE_DOUBLES = 20                                                               # ISDF_STATE_DOUBLES: pos vel acc jer quat(w,x,y,z) omg thr
 
 
 class KernelConfig(C.Structure):
@@ -346,6 +348,10 @@ def load_library(path=None):
     lib.isdf_midend_callback_batch_ragged.argtypes = [vp, C.c_int, ip, dp, dp, C.c_int, mpp, dp, dp, dp, dp]
     lib.isdf_midend_batch_ragged.argtypes = [vp, C.c_int, ip, dp, dp, C.c_int, mpp, dp, dp, dp, dp, dp, ip, ip, ip, ip]
     lib.isdf_midend_batch_ragged_device.argtypes = [vp, C.c_int, ip, vp, vp, C.c_int, mpp, vp, vp, vp, vp, vp, vp, vp, vp, ip, vp]
+    lib.isdf_trajectory_states.argtypes = [vp, C.c_int, ip, dp, dp, C.c_int64, ip, dp, dp]
+    lib.isdf_trajectory_states_device.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int64, vp, vp, vp, vp]
+    lib.isdf_pose_points.argtypes = [vp, C.c_int64, dp, C.c_int, dp, dp]
+    lib.isdf_pose_points_device.argtypes = [vp, C.c_int64, vp, C.c_int, vp, vp, vp]
     for s in ABI_SYMBOLS:
         if s != "isdf_last_error":
             getattr(lib, s).restype = C.c_int
@@ -995,6 +1001,56 @@ class Evaluator:
             d["dynamics"] = ds[b].as_dict() if p.flags & PLAN_DYNAMICS else None
             out.append(d)
         return out, self.plan_info()
+
+    # ---- executing a trajectory (include/isdf.h: isdf_trajectory_states, isdf_pose_points) ----
+    @staticmethod
+    def pack_plans(plans):
+        """isdf_plan_batch's ragged layout from plan_batch's list of dicts: (piece_off (B + 1 int32), T (P,), coeffs (18 P,)), each plan's
+        own 6N x 3 column-major block at coeffs[18 piece_off[b]:]; plans without a trajectory get no pieces"""
+        Ts = [_f64(d["T"]).reshape(-1) for d in plans]
+        Cs = [_f64(d["coeffs"]).reshape(-1) for d in plans]
+        if not Ts or any(c.size != 18 * t.size for t, c in zip(Ts, Cs)):
+            raise ValueError("plans must be a non-empty list of dicts whose coeffs hold 18 values per duration in T")
+        off = np.zeros(len(Ts) + 1, dtype=np.int32)
+        off[1:] = np.cumsum([t.size for t in Ts])
+        return off, _f64(np.concatenate(Ts)), _f64(np.concatenate(Cs))
+
+    def trajectory_states(self, plans_or_ragged, traj, times):
+        """the state of trajectory traj[q] at its local time times[q] -> (Q, 20) records: pos, vel, acc, jer, quat (w, x, y, z), omg, thr.
+        plans_or_ragged: plan_batch's list of dicts, or (piece_off, T, coeffs) in isdf_plan_batch's ragged layout"""
+        if isinstance(plans_or_ragged, tuple):
+            off, T, Cc = plans_or_ragged
+            off, T, Cc = np.ascontiguousarray(off, dtype=np.int32).reshape(-1), _f64(T).reshape(-1), _f64(Cc).reshape(-1)
+        else:
+            off, T, Cc = self.pack_plans(plans_or_ragged)
+        tr = np.ascontiguousarray(traj, dtype=np.int32).reshape(-1)
+        tm = _f64(times).reshape(-1)
+        if tr.size != tm.size:
+            raise ValueError(f"traj and times must have the same length, got {tr.size} and {tm.size}")
+        out = np.empty((tm.size, STATE_DOUBLES))
+        ip = C.POINTER(C.c_int32)
+        self._check(self.lib.isdf_trajectory_states(self.h, off.size - 1, off.ctypes.data_as(ip), _dp(T), _dp(Cc), tm.size,
+                                                    tr.ctypes.data_as(ip), _dp(tm), _dp(out)))
+        return out
+
+    def trajectory_states_device(self, B, d_piece_off, d_T, d_coeffs, Q, d_traj, d_times, d_out, stream=0):
+        """raw device pointers (e.g. torch .data_ptr()): piece_off B + 1 and traj Q int32, T, coeffs and times float64, out Q x 20 float64;
+        enqueued on stream (a raw cudaStream_t; 0 = the legacy default stream) and not waited for"""
+        self._check(self.lib.isdf_trajectory_states_device(self.h, int(B), C.c_void_p(d_piece_off), C.c_void_p(d_T), C.c_void_p(d_coeffs), int(Q),
+                                                           C.c_void_p(d_traj), C.c_void_p(d_times), C.c_void_p(d_out), C.c_void_p(stream)))
+
+    def pose_points(self, states, body):
+        """the body-frame points body (P, 3) posed at each of the (Q, 20) states -> (Q, P, 3): R(quat) b + pos (Shape::Transform)"""
+        st = _f64(states).reshape(-1, STATE_DOUBLES)
+        b = _f64(body).reshape(-1, 3)
+        out = np.empty((st.shape[0], b.shape[0], 3))
+        self._check(self.lib.isdf_pose_points(self.h, st.shape[0], _dp(st), b.shape[0], _dp(b), _dp(out)))
+        return out
+
+    def pose_points_device(self, Q, d_states, P, d_body, d_out, stream=0):
+        """raw device pointers: states Q x 20, body P x 3, out Q x P x 3 float64; enqueued on stream and not waited for"""
+        self._check(self.lib.isdf_pose_points_device(self.h, int(Q), C.c_void_p(d_states), int(P), C.c_void_p(d_body), C.c_void_p(d_out),
+                                                     C.c_void_p(stream)))
 
     def plan_info(self):
         info = PlanInfo()

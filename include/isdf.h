@@ -909,6 +909,45 @@ int isdf_plan_batch(isdf_ctx *ctx, const double *start, int B, const double *goa
                     isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics);
 int isdf_get_plan_info(isdf_ctx *ctx, isdf_plan_info *out);
 
+/* ---- executing a trajectory: getStateOnTrajStamp (swm:307-341) and the playback of SweptVolumeManager::process (swm:948-988) ----
+ * B trajectories in isdf_plan_batch's ragged layout: trajectory b has pieces [piece_off[b], piece_off[b+1]), durations T[piece_off[b] + i],
+ * and its own 6N x 3 column-major block at coeffs + 18 * piece_off[b]. Q queries (traj[q], times[q]); out is Q records of
+ * ISDF_STATE_DOUBLES = 20 doubles:
+ *   pos[3] vel[3] acc[3] jer[3] quat[4] (w, x, y, z, the reference's Vector4d order) omg[3] thr
+ * Each record is what process() computes at delta = times[q] (swm:961-971), bit for bit:
+ *   - times[q] is local to trajectory traj[q]. The piece and its local time come from locatePieceIdx (trajectory.hpp:545-563): sequential
+ *     subtraction with a strict '>', so a junction time stays in the earlier piece; a negative time stays in piece 0 and a time past the end
+ *     is clamped into the last piece, both extrapolating its polynomial. NaN and infinite times go through that arithmetic as they are.
+ *   - pos, vel, acc, jer are getPos / getVel / getAcc / getJer (trajectory.hpp:150-208) at that local time.
+ *   - quat, omg, thr are FlatnessMap::forward(vel, acc, jer, psi = 0, dpsi = 0, thr, quat, omg) (flatness.hpp:150-228) with the context's
+ *     (vehicle_mass, grav_acc, horiz_drag, vert_drag, paras_drag, speed_eps), restated operation by operation with psi and dpsi as zero
+ *     operands (signs of zero included); thr = z . f_term (:203-206). Yaw is zero, as in the planner's collision model.
+ * Every record depends only on its own (traj, time) and that trajectory's data, not on B, Q, the order of the queries or other trajectories.
+ * A query on a trajectory without pieces (a NO_PATH or TOO_LONG plan) gets an all-NaN record.
+ * Needs a context (its stream and config); no map and no shape. Q = 0 does nothing. The call counts its launch in
+ * isdf_stats.kernel_launches and touches no other field. Device memory is the context's, grown on demand; the host form stages through one
+ * pinned block, one copy each way.
+ * Errors (host form; nothing is written): ISDF_ERR_INVALID for a NULL pointer, B < 1, Q < 0 or Q records beyond 2^63 bytes,
+ *   piece_off[0] != 0 or offsets that decrease, a duration that is not positive and finite, a coefficient that is not finite, or traj[q]
+ *   outside [0, B). */
+#define ISDF_STATE_DOUBLES 20
+int isdf_trajectory_states(isdf_ctx *ctx, int B, const int32_t *piece_off, const double *T, const double *coeffs,
+                           int64_t Q, const int32_t *traj, const double *times, double *out);
+/* the same with every array on ctx's device (d_piece_off too), enqueued on cuda_stream and not waited for. Device data is not checked on the
+ * host: a traj[q] outside [0, B) gives an all-NaN record, offsets, durations and coefficients are taken as they are. Host and device forms
+ * give identical bits. Errors: ISDF_ERR_INVALID for a NULL pointer, B < 1, Q < 0 or Q records beyond 2^63 bytes. */
+int isdf_trajectory_states_device(isdf_ctx *ctx, int B, const int32_t *d_piece_off, const double *d_T, const double *d_coeffs,
+                                  int64_t Q, const int32_t *d_traj, const double *d_times, double *d_out, void *cuda_stream);
+/* the robot's body at Q states: out[(q * P + p) * 3 + k] = (R(quat_q) body_p + pos_q)_k, R = quat_rot (Eigen's toRotationMatrix,
+ * Shape.hpp:753-757), each row ((R_k0 b0 + R_k1 b1) + R_k2 b2) + pos_k rounded per operation (Shape::Transform, Shape.hpp:786-793).
+ * states: Q x 20, isdf_trajectory_states records (only pos and quat are read); body: P x 3 body-frame points (mesh vertices, interior
+ * points, markers: no shape needs to be set). An all-NaN record gives NaN points. Q = 0 or P = 0 does nothing.
+ * Errors: ISDF_ERR_INVALID for a NULL pointer, Q < 0, P < 0, or Q * P * 3 doubles beyond 2^63 bytes. The device form is enqueued on
+ * cuda_stream and not waited for; both forms count their launch in isdf_stats.kernel_launches and give identical bits. */
+int isdf_pose_points(isdf_ctx *ctx, int64_t Q, const double *states, int P, const double *body, double *out);
+int isdf_pose_points_device(isdf_ctx *ctx, int64_t Q, const double *d_states, int P, const double *d_body, double *d_out,
+                            void *cuda_stream);
+
 /* ---- swept-volume term: addSaftyPenaOnSweptVolumeParallel (hpp:557-649) + getSDFofSweptVolume (swm:710-747) --- */
 /* parallel_points (plan_manager.cpp:246-254): P x 3 row-major world-frame voxel centres; resets lastTstar to 0 (not the persisted
  * trajectory duration: see isdf_set_points_batch) */
