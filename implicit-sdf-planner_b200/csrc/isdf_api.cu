@@ -25,6 +25,7 @@
 #include <string>
 #include <vector>
 #include <limits>
+#include <unordered_map>
 
 using namespace isdf;
 
@@ -217,7 +218,8 @@ struct isdf_ctx {
     } fe;
     struct {   // front-end path search (isdf_frontpath.cuh): rebuilt from the current map and kernels by every call, so nothing here outlives them
         DevBuf<uint32_t> d_trav, d_front, d_colliding; DevBuf<unsigned long long> d_g; DevBuf<unsigned> d_flags;
-        DevBuf<int> d_tgt, d_len, d_off, d_nodes; DevBuf<double> d_xyz, d_rp, d_cost; DevBuf<uint8_t> d_found;
+        DevBuf<int> d_src, d_tgt, d_tsrc, d_pair, d_len, d_woff, d_off, d_soff, d_scratch, d_nodes; DevBuf<double> d_xyz, d_rp, d_cost;
+        DevBuf<uint8_t> d_found;
         PinnedBuf<unsigned> h_flag;
         cudaEvent_t ev[4] = {};
         isdf_frontpath_info info = {};
@@ -3320,11 +3322,11 @@ static int path_args_check(isdf_ctx *c, const isdf_frontpath_params *prm) {
 
 // isInMap (Gridmap3D.cpp) + getGridIndex (Gridmap3D.cpp:135-175) with its clamps and its "iy < 0 => ix = 0" branches (they cannot fire
 // for a point inside the map)
-static int path_voxel(const DevGrid &G, const double *p, int id[3], const char *what) {
+static int path_voxel(const DevGrid &G, const double *p, int id[3], const std::string &what) {
     for (int a = 0; a < 3; a++)
-        if (!std::isfinite(p[a])) return fail(ISDF_ERR_INVALID, std::string(what) + " is not finite");
+        if (!std::isfinite(p[a])) return fail(ISDF_ERR_INVALID, what + " is not finite");
     for (int a = 0; a < 3; a++)
-        if (p[a] < G.bmin[a] || p[a] > G.bmax[a]) return fail(ISDF_ERR_INVALID, std::string(what) + " is outside the map");
+        if (p[a] < G.bmin[a] || p[a] > G.bmax[a]) return fail(ISDF_ERR_INVALID, what + " is outside the map");
     int ix = (int)std::floor((p[0] - G.bmin[0]) / G.res), iy = (int)std::floor((p[1] - G.bmin[1]) / G.res), iz = (int)std::floor((p[2] - G.bmin[2]) / G.res);
     if (ix < 0) ix = 0;
     if (ix >= G.X) ix = G.X - 1;
@@ -3336,114 +3338,183 @@ static int path_voxel(const DevGrid &G, const double *p, int id[3], const char *
     return 0;
 }
 
-static PathArgs path_args(isdf_ctx *c, const int s[3], unsigned long long *d_g) {
-    const size_t nword = (size_t)c->map.grid.X * c->map.grid.Y * c->map.grid.Zw;
+static PathArgs path_args(isdf_ctx *c, unsigned long long *d_g) {
     PathArgs P = {};
     P.grid = c->map.grid; P.trav = c->fp.d_trav.p; P.g = d_g;
-    P.front0 = c->fp.d_front.p; P.front1 = c->fp.d_front.p + nword;
-    P.flags = c->fp.d_flags.p; P.rounds = c->fp.d_flags.p + FP_FLAG_RING;
-    P.sx = s[0]; P.sy = s[1]; P.sz = s[2];
+    P.front = c->fp.d_front.p; P.src = c->fp.d_src.p;
     return P;
 }
 
-// traversability grid, then the field from source s into d_g (X*Y*Z bit patterns), on stream st; fills c->fp.info
-static int path_field(isdf_ctx *c, const int s[3], unsigned long long *d_g, cudaStream_t st) {
+// the traversability grid of the current map and kernels on stream st, between events 0 and 1; clears c->fp.info
+static int path_trav(isdf_ctx *c, cudaStream_t st) {
     const DevGrid &G = c->map.grid;
-    const size_t nword = (size_t)G.X * G.Y * G.Zw, nvox = (size_t)G.X * G.Y * G.Z;
     for (cudaEvent_t &e : c->fp.ev) if (!e) CU_TRY(cudaEventCreate(&e));
-    CU_TRY(c->fp.d_trav.ensure(nword));
-    CU_TRY(c->fp.d_front.ensure(2 * nword));
-    CU_TRY(c->fp.d_flags.ensure(FP_FLAG_RING + 1));
+    CU_TRY(c->fp.d_trav.ensure((size_t)G.X * G.Y * G.Zw));
     CU_TRY(c->fp.h_flag.ensure(2));
+    c->fp.info = {};
     CU_TRY(cudaEventRecord(c->fp.ev[0], st));
     if (int r = frontend_feasibility_run(c, nullptr, c->fp.d_trav.p, st)) return r;
     CU_TRY(cudaEventRecord(c->fp.ev[1], st));
-    const PathArgs P = path_args(c, s, d_g);
-    CU_TRY(cudaMemsetAsync(c->fp.d_front.p, 0, sizeof(uint32_t) * 2 * nword, st));
-    CU_TRY(cudaMemsetAsync(c->fp.d_flags.p, 0, sizeof(unsigned) * (FP_FLAG_RING + 1), st));
+    return 0;
+}
+
+// one relaxation from the n source voxels src (host, 3 each) into d_g (field s at d_g + s*X*Y*Z) on stream st, after path_trav; adds its
+// device time and its rounds to c->fp.info
+static int path_fields(isdf_ctx *c, int n, const int *src, unsigned long long *d_g, cudaStream_t st) {
+    const DevGrid &G = c->map.grid;
+    const size_t nword = (size_t)G.X * G.Y * G.Zw, nvox = (size_t)G.X * G.Y * G.Z, nflag = (size_t)(n + 1) * FP_FLAG_RING + 1;
+    CU_TRY(c->fp.d_front.ensure(2 * (size_t)n * nword));
+    CU_TRY(c->fp.d_flags.ensure(nflag));
+    CU_TRY(c->fp.d_src.upload(src, (size_t)3 * n, st));
+    PathArgs P = path_args(c, d_g);
+    P.flags = c->fp.d_flags.p; P.rounds = P.flags + (size_t)(n + 1) * FP_FLAG_RING;
+    P.any = n == 1 ? P.flags : P.flags + (size_t)n * FP_FLAG_RING;
+    P.front1 = P.front + nword;
+    CU_TRY(cudaEventRecord(c->fp.ev[2], st));
+    CU_TRY(cudaMemsetAsync(c->fp.d_front.p, 0, sizeof(uint32_t) * 2 * (size_t)n * nword, st));
+    CU_TRY(cudaMemsetAsync(c->fp.d_flags.p, 0, sizeof(unsigned) * nflag, st));
     const long long sms = c->sm_count;
-    k_fp_init<<<(unsigned)std::min<long long>(((long long)nvox + 255) / 256, sms * 32), 256, 0, st>>>(P);
+    k_fp_init<<<dim3((unsigned)std::min<long long>(((long long)nvox + 255) / 256, sms * 32), (unsigned)n), 256, 0, st>>>(P);
     c->stats.kernel_launches++;
-    const unsigned blocks = (unsigned)std::min<long long>(((long long)nword + 255) / 256, sms * 16);
+    const dim3 blocks((unsigned)std::min<long long>(((long long)nword + 255) / 256, sms * 16), (unsigned)n);
     for (int r = 0;;) {
-        for (int k = 0; k < FP_ROUNDS_PER_CHECK; k++, r++) k_fp_relax<<<blocks, 256, 0, st>>>(P, r);
+        for (int k = 0; k < FP_ROUNDS_PER_CHECK; k++, r++) {
+            if (n == 1) k_fp_relax<<<blocks, 256, 0, st>>>(P, r);
+            else k_fp_relax_multi<<<blocks, 256, 0, st>>>(P, r);
+        }
         c->stats.kernel_launches += FP_ROUNDS_PER_CHECK;
         CU_TRY(cudaGetLastError());
-        CU_TRY(cudaMemcpyAsync(c->fp.h_flag.p, P.flags + r % FP_FLAG_RING, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(c->fp.h_flag.p, P.any + r % FP_FLAG_RING, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
         CU_TRY(cudaStreamSynchronize(st));
         if (!c->fp.h_flag.p[0]) break;
     }
-    CU_TRY(cudaEventRecord(c->fp.ev[2], st));
+    CU_TRY(cudaEventRecord(c->fp.ev[3], st));
     CU_TRY(cudaMemcpyAsync(c->fp.h_flag.p + 1, P.rounds, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaStreamSynchronize(st));
-    isdf_frontpath_info &I = c->fp.info;
-    I = {};
-    I.rounds = (int32_t)c->fp.h_flag.p[1];
-    I.field_bytes = (int64_t)(nvox * sizeof(double));
     float ms = 0;
-    cudaEventElapsedTime(&ms, c->fp.ev[0], c->fp.ev[1]); I.traversability_ms = ms;
-    cudaEventElapsedTime(&ms, c->fp.ev[1], c->fp.ev[2]); I.field_ms = ms;
+    cudaEventElapsedTime(&ms, c->fp.ev[2], c->fp.ev[3]);
+    c->fp.info.field_ms += ms;
+    c->fp.info.rounds += (int32_t)c->fp.h_flag.p[1];
     return 0;
 }
 
-// field from start, then the B paths into c->fp.d_xyz / d_rp / d_cost / d_found; off (B + 1) is filled as soon as the lengths are known,
-// also when they exceed cap
-static int path_run(isdf_ctx *c, const double *start, int B, const double *goals, int cap, std::vector<int> &off, cudaStream_t st) {
+// the stage times of a call that ran path_trav, then its fields, then (up to event 2) its paths; field_bytes: the fields held at once
+static void path_info(isdf_ctx *c, size_t field_bytes, bool paths) {
+    isdf_frontpath_info &I = c->fp.info;
+    I.field_bytes = (int64_t)field_bytes;
+    float ms = 0;
+    cudaEventElapsedTime(&ms, c->fp.ev[0], c->fp.ev[1]); I.traversability_ms = ms;
+    if (paths) { cudaEventElapsedTime(&ms, c->fp.ev[1], c->fp.ev[2]); I.paths_ms = ms - I.field_ms; }
+}
+
+// the paths of B (start, goal) pairs into c->fp.d_xyz / d_rp / d_cost / d_found in pair order. starts: B x 3, or one start for every
+// goal (sstride 0). Pairs whose starts share a voxel share a field: node 0 of a path is its start voxel's cube centre, so their paths are
+// the same. The distinct start voxels' fields are built in chunks of at most max_fields (0: FP_FIELD_BUDGET bytes, at least one field),
+// and each chunk's paths are walked into scratch before its fields are reused. off (B + 1) is filled as soon as every length is known,
+// also when they exceed cap.
+static int path_run(isdf_ctx *c, int B, const double *starts, int sstride, const double *goals, int max_fields, int cap, std::vector<int> &off,
+                    cudaStream_t st) {
     const DevGrid &G = c->map.grid;
-    int s[3];
-    if (int r = path_voxel(G, start, s, "start")) return r;
-    std::vector<int> tgt((size_t)3 * B);
-    for (int b = 0; b < B; b++)
-        if (int r = path_voxel(G, goals + 3 * (size_t)b, &tgt[3 * (size_t)b], "a goal")) return r;
-    CU_TRY(c->fp.d_g.ensure((size_t)G.X * G.Y * G.Z));
-    if (int r = path_field(c, s, c->fp.d_g.p, st)) return r;
-    PathArgs P = path_args(c, s, c->fp.d_g.p);
-    CU_TRY(c->fp.d_tgt.upload(tgt.data(), tgt.size(), st));
-    CU_TRY(c->fp.d_len.ensure(B)); CU_TRY(c->fp.d_off.ensure((size_t)B + 1));
-    CU_TRY(c->fp.d_cost.ensure(B)); CU_TRY(c->fp.d_found.ensure(B));
-    P.nt = B; P.tgt = c->fp.d_tgt.p; P.len = c->fp.d_len.p; P.off = c->fp.d_off.p; P.cost = c->fp.d_cost.p; P.found = c->fp.d_found.p;
-    const unsigned wblocks = (unsigned)(((long long)B * 32 + 127) / 128);
-    k_fp_walk<<<wblocks, 128, 0, st>>>(P, 0);
-    c->stats.kernel_launches++;
-    CU_TRY(cudaGetLastError());
-    std::vector<int> len(B);
-    CU_TRY(cudaMemcpyAsync(len.data(), c->fp.d_len.p, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    off.assign((size_t)B + 1, 0);
-    long long total = 0;
+    const size_t nvox = (size_t)G.X * G.Y * G.Z;
+    std::vector<int> tgt((size_t)3 * B), ps(B), src;   // ps[b]: pair b's source; src: 3 per distinct start voxel, in order of first use
+    std::unordered_map<long long, int> seen;
     for (int b = 0; b < B; b++) {
-        total += len[b];
-        if (total > INT32_MAX) return fail(ISDF_ERR_INVALID, "the paths hold more than 2^31 - 1 nodes");
-        off[b + 1] = (int)total;
+        int s[3];
+        if (int r = path_voxel(G, starts + (size_t)sstride * b, s, sstride ? "starts[" + std::to_string(b) + "]" : std::string("start"))) return r;
+        if (int r = path_voxel(G, goals + 3 * (size_t)b, &tgt[3 * (size_t)b], "goals[" + std::to_string(b) + "]")) return r;
+        const auto ins = seen.emplace(((long long)s[0] * G.Y + s[1]) * G.Z + s[2], (int)(src.size() / 3));
+        if (ins.second) src.insert(src.end(), s, s + 3);
+        ps[b] = ins.first->second;
     }
+    const int S = (int)(src.size() / 3);
+    const long long want = max_fields > 0 ? max_fields : std::max<long long>(1, FP_FIELD_BUDGET / (long long)(sizeof(double) * nvox));
+    const int F = (int)std::min<long long>(std::min<long long>(want, S), 65535);   // fields per chunk (grid.y of the relaxation)
+    // walk order: the pairs grouped by source, in pair order within a source; pair b is walked at wpos[b]
+    std::vector<int> wstart((size_t)S + 1, 0), walk(B), wpos(B);
+    for (int b = 0; b < B; b++) wstart[ps[b] + 1]++;
+    for (int s = 0; s < S; s++) wstart[s + 1] += wstart[s];
+    std::vector<int> wtgt((size_t)3 * B), wsrc((size_t)4 * B);
+    {
+        std::vector<int> next(wstart.begin(), wstart.end() - 1);
+        for (int b = 0; b < B; b++) {
+            const int w = next[ps[b]]++;
+            wpos[b] = w; walk[w] = b;
+            for (int k = 0; k < 3; k++) { wtgt[3 * (size_t)w + k] = tgt[3 * (size_t)b + k]; wsrc[4 * (size_t)w + k] = src[3 * (size_t)ps[b] + k]; }
+            wsrc[4 * (size_t)w + 3] = ps[b] % F;   // the field's slice in its chunk
+        }
+    }
+    if (int r = path_trav(c, st)) return r;
+    CU_TRY(c->fp.d_g.ensure((size_t)F * nvox));
+    CU_TRY(c->fp.d_tgt.upload(wtgt.data(), wtgt.size(), st)); CU_TRY(c->fp.d_tsrc.upload(wsrc.data(), wsrc.size(), st));
+    CU_TRY(c->fp.d_pair.upload(walk.data(), walk.size(), st));
+    CU_TRY(c->fp.d_len.ensure(B)); CU_TRY(c->fp.d_woff.ensure((size_t)B + 1)); CU_TRY(c->fp.d_cost.ensure(B)); CU_TRY(c->fp.d_found.ensure(B));
+    std::vector<int> len(B), woff((size_t)B + 1, 0);   // walk order; woff: first node in scratch
+    for (int s0 = 0; s0 < S; s0 += F) {
+        const int n = std::min(F, S - s0), w0 = wstart[s0], w1 = wstart[s0 + n], nt = w1 - w0;
+        if (int r = path_fields(c, n, &src[3 * (size_t)s0], c->fp.d_g.p, st)) return r;
+        PathArgs P = path_args(c, c->fp.d_g.p);
+        P.nt = nt; P.tgt = c->fp.d_tgt.p + 3 * (size_t)w0; P.tsrc = c->fp.d_tsrc.p + 4 * (size_t)w0; P.pair = c->fp.d_pair.p + w0;
+        P.len = c->fp.d_len.p + w0; P.cost = c->fp.d_cost.p; P.found = c->fp.d_found.p;
+        const unsigned wblocks = (unsigned)(((long long)nt * 32 + 127) / 128);
+        k_fp_walk<<<wblocks, 128, 0, st>>>(P, 0);
+        c->stats.kernel_launches++;
+        CU_TRY(cudaGetLastError());
+        CU_TRY(cudaMemcpyAsync(len.data() + w0, P.len, sizeof(int) * nt, cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
+        for (int w = w0; w < w1; w++) {
+            if ((long long)woff[w] + len[w] > INT32_MAX) return fail(ISDF_ERR_INVALID, "the paths hold more than 2^31 - 1 nodes");
+            woff[w + 1] = woff[w] + len[w];
+        }
+        if ((size_t)3 * woff[w1] > c->fp.d_scratch.n) {   // grow the scratch, keeping the earlier chunks' paths
+            DevBuf<int> grown;
+            CU_TRY(grown.ensure(std::max((size_t)3 * woff[w1], 2 * c->fp.d_scratch.n)));
+            if (woff[w0]) CU_TRY(cudaMemcpyAsync(grown.p, c->fp.d_scratch.p, sizeof(int) * 3 * (size_t)woff[w0], cudaMemcpyDeviceToDevice, st));
+            CU_TRY(cudaStreamSynchronize(st));   // the old buffer is freed when grown goes out of scope
+            std::swap(c->fp.d_scratch, grown);
+        }
+        CU_TRY(cudaMemcpyAsync(c->fp.d_woff.p + w0, woff.data() + w0, sizeof(int) * ((size_t)nt + 1), cudaMemcpyHostToDevice, st));
+        P.off = c->fp.d_woff.p + w0; P.scratch = c->fp.d_scratch.p;
+        k_fp_walk<<<wblocks, 128, 0, st>>>(P, 1);
+        c->stats.kernel_launches++;
+        CU_TRY(cudaGetLastError());
+    }
+    path_info(c, (size_t)F * nvox * sizeof(double), false);
+    // pair order
+    off.assign((size_t)B + 1, 0);
+    std::vector<int> soff(B);
+    for (int b = 0; b < B; b++) { off[b + 1] = off[b] + len[wpos[b]]; soff[b] = woff[wpos[b]]; }
+    const int total = off[B];
     if (total > cap) return fail(ISDF_ERR_INVALID, "cap is smaller than the total path length (reported in n / offsets[B])");
-    CU_TRY(c->fp.d_off.upload(off.data(), off.size(), st));
+    CU_TRY(c->fp.d_off.upload(off.data(), off.size(), st)); CU_TRY(c->fp.d_soff.upload(soff.data(), soff.size(), st));
     CU_TRY(c->fp.d_nodes.ensure((size_t)3 * total)); CU_TRY(c->fp.d_colliding.ensure((size_t)4 * total));
     CU_TRY(c->fp.d_xyz.ensure((size_t)3 * total)); CU_TRY(c->fp.d_rp.ensure((size_t)2 * total));
+    PathArgs P = path_args(c, c->fp.d_g.p);
+    P.nt = B; P.off = c->fp.d_off.p; P.soff = c->fp.d_soff.p; P.scratch = c->fp.d_scratch.p;
     P.nodes = c->fp.d_nodes.p; P.xyz = c->fp.d_xyz.p; P.rp = c->fp.d_rp.p; P.colliding = c->fp.d_colliding.p;
-    k_fp_walk<<<wblocks, 128, 0, st>>>(P, 1);
+    k_fp_place<<<(unsigned)(((long long)B * 32 + 127) / 128), 128, 0, st>>>(P);
     FrontArgs A = front_args(c);
-    A.nq = (int)total; A.q_ind = c->fp.d_nodes.p; A.out = c->fp.d_colliding.p;
+    A.nq = total; A.q_ind = c->fp.d_nodes.p; A.out = c->fp.d_colliding.p;
     const size_t smem = sizeof(uint32_t) * 4 * (size_t)A.ks * A.ks * A.ks;
     CU_TRY(cudaFuncSetAttribute(k_fp_node_masks, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_fp_node_masks<<<(unsigned)((total + 255) / 256), 256, smem, st>>>(A);
+    k_fp_node_masks<<<(unsigned)(((long long)total + 255) / 256), 256, smem, st>>>(A);
     k_fp_attitudes<<<(unsigned)((B + 127) / 128), 128, 0, st>>>(A, P);
     c->stats.kernel_launches += 3;
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaEventRecord(c->fp.ev[3], st));
+    CU_TRY(cudaEventRecord(c->fp.ev[2], st));
     CU_TRY(cudaStreamSynchronize(st));
-    float ms = 0;
-    cudaEventElapsedTime(&ms, c->fp.ev[2], c->fp.ev[3]); c->fp.info.paths_ms = ms;
+    path_info(c, (size_t)F * nvox * sizeof(double), true);
     return 0;
 }
 
-extern "C" int isdf_frontend_path_batch(isdf_ctx *c, const double *start, int B, const double *goals, const isdf_frontpath_params *prm, int cap,
-                                        double *path_xyz, double *path_rp, int32_t *offsets, double *costs, uint8_t *found) {
-    if (!start || !goals || B < 1 || cap < 0 || (cap > 0 && !path_xyz) || !offsets || !costs || !found) return fail(ISDF_ERR_INVALID, "bad argument");
+// the host form of the path calls (starts: sstride 0 for one start)
+static int path_host(isdf_ctx *c, int B, const double *starts, int sstride, const double *goals, const isdf_frontpath_params *prm, int max_fields,
+                     int cap, double *path_xyz, double *path_rp, int32_t *offsets, double *costs, uint8_t *found) {
+    if (!starts || !goals || B < 1 || max_fields < 0 || cap < 0 || (cap > 0 && !path_xyz) || !offsets || !costs || !found)
+        return fail(ISDF_ERR_INVALID, "bad argument");
     if (int r = path_args_check(c, prm)) return r;
     if (set_device(c)) return ISDF_ERR_CUDA;
     std::vector<int> off;
-    const int r = path_run(c, start, B, goals, cap, off, c->stream);
+    const int r = path_run(c, B, starts, sstride, goals, max_fields, cap, off, c->stream);
     if (!off.empty()) std::memcpy(offsets, off.data(), sizeof(int32_t) * off.size());
     if (r) return r;
     const size_t total = (size_t)off[B];
@@ -3455,6 +3526,16 @@ extern "C" int isdf_frontend_path_batch(isdf_ctx *c, const double *start, int B,
     return 0;
 }
 
+extern "C" int isdf_frontend_path_batch(isdf_ctx *c, const double *start, int B, const double *goals, const isdf_frontpath_params *prm, int cap,
+                                        double *path_xyz, double *path_rp, int32_t *offsets, double *costs, uint8_t *found) {
+    return path_host(c, B, start, 0, goals, prm, 0, cap, path_xyz, path_rp, offsets, costs, found);
+}
+
+extern "C" int isdf_frontend_path_pairs(isdf_ctx *c, int B, const double *starts, const double *goals, const isdf_frontpath_params *prm,
+                                        int max_fields, int cap, double *path_xyz, double *path_rp, int32_t *offsets, double *costs, uint8_t *found) {
+    return path_host(c, B, starts, 3, goals, prm, max_fields, cap, path_xyz, path_rp, offsets, costs, found);
+}
+
 extern "C" int isdf_frontend_path(isdf_ctx *c, const double *start, const double *goal, const isdf_frontpath_params *prm, int cap,
                                   double *path_xyz, double *path_rp, int32_t *n, double *cost, uint8_t *found) {
     if (!n) return fail(ISDF_ERR_INVALID, "n is NULL");
@@ -3464,18 +3545,21 @@ extern "C" int isdf_frontend_path(isdf_ctx *c, const double *start, const double
     return r;
 }
 
-extern "C" int isdf_frontend_path_batch_device(isdf_ctx *c, const double *start, int B, const double *d_goals, const isdf_frontpath_params *prm,
-                                               int cap, double *d_path_xyz, double *d_path_rp, int32_t *d_offsets, double *d_costs,
-                                               uint8_t *d_found, void *cuda_stream) {
-    if (!start || !d_goals || B < 1 || cap < 0 || (cap > 0 && !d_path_xyz) || !d_offsets || !d_costs || !d_found) return fail(ISDF_ERR_INVALID, "bad argument");
+// the device form of the path calls: h_starts on the host (one start, sstride 0) or d_starts on the device (B x 3)
+static int path_device(isdf_ctx *c, int B, const double *h_starts, const double *d_starts, const double *d_goals, const isdf_frontpath_params *prm,
+                       int max_fields, int cap, double *d_path_xyz, double *d_path_rp, int32_t *d_offsets, double *d_costs, uint8_t *d_found,
+                       void *cuda_stream) {
+    if (!(h_starts || d_starts) || !d_goals || B < 1 || max_fields < 0 || cap < 0 || (cap > 0 && !d_path_xyz) || !d_offsets || !d_costs || !d_found)
+        return fail(ISDF_ERR_INVALID, "bad argument");
     if (int r = path_args_check(c, prm)) return r;
     if (set_device(c)) return ISDF_ERR_CUDA;
     const cudaStream_t st = (cudaStream_t)cuda_stream;
-    std::vector<double> goals((size_t)3 * B);
+    std::vector<double> goals((size_t)3 * B), starts(d_starts ? (size_t)3 * B : 0);
     CU_TRY(cudaMemcpyAsync(goals.data(), d_goals, sizeof(double) * goals.size(), cudaMemcpyDeviceToHost, st));
+    if (d_starts) CU_TRY(cudaMemcpyAsync(starts.data(), d_starts, sizeof(double) * starts.size(), cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaStreamSynchronize(st));
     std::vector<int> off;
-    const int r = path_run(c, start, B, goals.data(), cap, off, st);
+    const int r = path_run(c, B, d_starts ? starts.data() : h_starts, d_starts ? 3 : 0, goals.data(), max_fields, cap, off, st);
     if (!off.empty()) {
         CU_TRY(cudaMemcpyAsync(d_offsets, off.data(), sizeof(int32_t) * off.size(), cudaMemcpyHostToDevice, st));
         CU_TRY(cudaStreamSynchronize(st));   // off is a host temporary
@@ -3490,13 +3574,47 @@ extern "C" int isdf_frontend_path_batch_device(isdf_ctx *c, const double *start,
     return 0;
 }
 
+extern "C" int isdf_frontend_path_batch_device(isdf_ctx *c, const double *start, int B, const double *d_goals, const isdf_frontpath_params *prm,
+                                               int cap, double *d_path_xyz, double *d_path_rp, int32_t *d_offsets, double *d_costs,
+                                               uint8_t *d_found, void *cuda_stream) {
+    if (!start) return fail(ISDF_ERR_INVALID, "bad argument");
+    return path_device(c, B, start, nullptr, d_goals, prm, 0, cap, d_path_xyz, d_path_rp, d_offsets, d_costs, d_found, cuda_stream);
+}
+
+extern "C" int isdf_frontend_path_pairs_device(isdf_ctx *c, int B, const double *d_starts, const double *d_goals, const isdf_frontpath_params *prm,
+                                               int max_fields, int cap, double *d_path_xyz, double *d_path_rp, int32_t *d_offsets,
+                                               double *d_costs, uint8_t *d_found, void *cuda_stream) {
+    if (!d_starts) return fail(ISDF_ERR_INVALID, "bad argument");
+    return path_device(c, B, nullptr, d_starts, d_goals, prm, max_fields, cap, d_path_xyz, d_path_rp, d_offsets, d_costs, d_found, cuda_stream);
+}
+
+// the fields of the S source voxels src (host, 3 each) in one relaxation into d_g
+static int path_fields_run(isdf_ctx *c, int S, const int *src, double *d_g, cudaStream_t st) {
+    if (int r = path_trav(c, st)) return r;
+    if (int r = path_fields(c, S, src, reinterpret_cast<unsigned long long *>(d_g), st)) return r;
+    path_info(c, (size_t)S * c->map.grid.X * c->map.grid.Y * c->map.grid.Z * sizeof(double), false);
+    return 0;
+}
+
 extern "C" int isdf_frontend_path_field_device(isdf_ctx *c, const double *start, const isdf_frontpath_params *prm, double *d_g, void *cuda_stream) {
     if (!start || !d_g) return fail(ISDF_ERR_INVALID, "bad argument");
     if (int r = path_args_check(c, prm)) return r;
     if (set_device(c)) return ISDF_ERR_CUDA;
     int s[3];
     if (int r = path_voxel(c->map.grid, start, s, "start")) return r;
-    return path_field(c, s, reinterpret_cast<unsigned long long *>(d_g), (cudaStream_t)cuda_stream);
+    return path_fields_run(c, 1, s, d_g, (cudaStream_t)cuda_stream);
+}
+
+extern "C" int isdf_frontend_path_fields_device(isdf_ctx *c, int S, const double *starts, const isdf_frontpath_params *prm, double *d_g,
+                                                void *cuda_stream) {
+    if (!starts || !d_g || S < 1) return fail(ISDF_ERR_INVALID, "bad argument");
+    if (S > 65535) return fail(ISDF_ERR_INVALID, "S must be at most 65535");
+    if (int r = path_args_check(c, prm)) return r;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    std::vector<int> src((size_t)3 * S);
+    for (int s = 0; s < S; s++)
+        if (int r = path_voxel(c->map.grid, starts + 3 * (size_t)s, &src[3 * (size_t)s], "starts[" + std::to_string(s) + "]")) return r;
+    return path_fields_run(c, S, src.data(), d_g, (cudaStream_t)cuda_stream);
 }
 
 extern "C" int isdf_frontend_path_info(isdf_ctx *c, isdf_frontpath_info *out) {
@@ -3505,7 +3623,7 @@ extern "C" int isdf_frontend_path_info(isdf_ctx *c, isdf_frontpath_info *out) {
     return 0;
 }
 
-// ---- planning step: PlannerManager::generateTraj for one start and B goals (include/isdf.h) --------------------------------------------
+// ---- planning step: PlannerManager::generateTraj for B (start, goal) pairs (include/isdf.h) --------------------------------------------
 // The stages are the existing entry points' internals on device buffers: path_run, isdf_path_waypoints, one ragged midend_batch_run, the
 // batched gather with set_as_points, one ragged lbfgs_rounds over callback_batch_launch, one ragged k_minco_forward for the final
 // trajectories, then certify_run and dynamics_run with N0 = N per group of plans with the same N.
@@ -3556,7 +3674,8 @@ static int plan_check(isdf_ctx *c, const isdf_plan_params *p, double *r_cert) {
     return 0;
 }
 
-static int plan_run(isdf_ctx *c, const double *start, int B, const double *goals, const isdf_plan_params *p, double r_cert, int cap_nodes,
+static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const double *goals, int max_fields, const isdf_plan_params *p,
+                    double r_cert, int cap_nodes,
                     int32_t *path_off, double *path_xyz, int cap_pieces, int32_t *piece_off, double *T, double *coeffs, isdf_plan_result *res,
                     isdf_certify_summary *certify, isdf_dynamics_summary *dynamics) {
     const cudaStream_t st = c->stream;
@@ -3578,7 +3697,7 @@ static int plan_run(isdf_ctx *c, const double *start, int B, const double *goals
     const double nan = std::numeric_limits<double>::quiet_NaN();
     // 1. front end
     std::vector<int> off;
-    if (int r = timed(info.frontend_ms, [&] { return path_run(c, start, B, goals, 0x7fffffff, off, st); })) return r;
+    if (int r = timed(info.frontend_ms, [&] { return path_run(c, B, starts, sstride, goals, max_fields, 0x7fffffff, off, st); })) return r;
     const int nodes = off[B];
     std::vector<double> xyz((size_t)3 * nodes), pcost(B);
     std::vector<uint8_t> found(B);
@@ -3609,7 +3728,7 @@ static int plan_run(isdf_ctx *c, const double *start, int B, const double *goals
     if ((path_xyz && nodes > cap_nodes) || poff[B] > cap_pieces)
         return fail(ISDF_ERR_INVALID, "cap_nodes or cap_pieces too small (path_off / piece_off report the sizes needed)");
     if (path_xyz && nodes) std::memcpy(path_xyz, xyz.data(), sizeof(double) * xyz.size());
-    // 3-6. one ragged mid-end over every plan that reaches it, one gather and one ragged back end over the plans that pass it, in goal order
+    // 3-6. one ragged mid-end over every plan that reaches it, one gather and one ragged back end over the plans that pass it, in pair order
     std::vector<int> idx;   // the plans that reach the mid-end
     for (int b = 0; b < B; b++) if (res[b].stage == ISDF_PLAN_OPTIMISED) idx.push_back(b);
     std::vector<int> Ns;
@@ -3743,7 +3862,7 @@ static int plan_run(isdf_ctx *c, const double *start, int B, const double *goals
     // 7. certificates on every returned trajectory, per group of plans with the same N, ascending
     if (!(p->flags & (ISDF_PLAN_CERTIFY | ISDF_PLAN_DYNAMICS))) return 0;
     for (const int Ng : Ns) {
-        std::vector<int> gi;   // the group's plans, in goal order
+        std::vector<int> gi;   // the group's plans, in pair order
         for (const int b : idx) if (N[b] == Ng) gi.push_back(b);
         const int Bn = (int)gi.size();
         const size_t BN = (size_t)Bn * Ng;
@@ -3783,22 +3902,25 @@ static int plan_run(isdf_ctx *c, const double *start, int B, const double *goals
     return 0;
 }
 
-extern "C" int isdf_plan_batch(isdf_ctx *c, const double *start, int B, const double *goals, const isdf_plan_params *p, int cap_nodes,
-                               int32_t *path_off, double *path_xyz, int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
-                               isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics) {
+// the planning calls (starts: sstride 0 for one start)
+static int plan_entry(isdf_ctx *c, int B, const double *starts, int sstride, const double *goals, const isdf_plan_params *p, int max_fields,
+                      int cap_nodes, int32_t *path_off, double *path_xyz, int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
+                      isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics) {
     bool started = false;
     const int rc = poison_on_failure([&]() -> int {
         if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
-        if (!start || !goals || B < 1 || !p || !piece_off || !results || cap_pieces < 0 || (cap_pieces > 0 && (!T || !coeffs)) ||
+        if (!starts || !goals || B < 1 || !p || !piece_off || !results || cap_pieces < 0 || (cap_pieces > 0 && (!T || !coeffs)) ||
             (path_xyz && (!path_off || cap_nodes < 0)))
             return fail(ISDF_ERR_INVALID, "NULL argument, B < 1 or a cap < 0");
+        if (max_fields < 0) return fail(ISDF_ERR_INVALID, "max_fields < 0");
         if (((p->flags & ISDF_PLAN_CERTIFY) && !certify) || ((p->flags & ISDF_PLAN_DYNAMICS) && !dynamics))
             return fail(ISDF_ERR_INVALID, "a summary array of a requested certificate is NULL");
         double r_cert = 0.0;
         if (int r = plan_check(c, p, &r_cert)) return r;
         if (set_device(c)) return ISDF_ERR_CUDA;
         started = true;
-        return plan_run(c, start, B, goals, p, r_cert, cap_nodes, path_off, path_xyz, cap_pieces, piece_off, T, coeffs, results, certify, dynamics);
+        return plan_run(c, B, starts, sstride, goals, max_fields, p, r_cert, cap_nodes, path_off, path_xyz, cap_pieces, piece_off, T, coeffs,
+                        results, certify, dynamics);
     }, [&] {
         if (B < 1) return;
         if (results)
@@ -3812,6 +3934,19 @@ extern "C" int isdf_plan_batch(isdf_ctx *c, const double *start, int B, const do
     });
     if (started) c->sv.set_points(nullptr, 0, c->stream);   // both point sets given up, the batched swept-volume term off
     return rc;
+}
+
+extern "C" int isdf_plan_batch(isdf_ctx *c, const double *start, int B, const double *goals, const isdf_plan_params *p, int cap_nodes,
+                               int32_t *path_off, double *path_xyz, int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
+                               isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics) {
+    return plan_entry(c, B, start, 0, goals, p, 0, cap_nodes, path_off, path_xyz, cap_pieces, piece_off, T, coeffs, results, certify, dynamics);
+}
+
+extern "C" int isdf_plan_pairs(isdf_ctx *c, int B, const double *starts, const double *goals, const isdf_plan_params *p, int max_fields,
+                               int cap_nodes, int32_t *path_off, double *path_xyz, int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
+                               isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics) {
+    return plan_entry(c, B, starts, 3, goals, p, max_fields, cap_nodes, path_off, path_xyz, cap_pieces, piece_off, T, coeffs, results, certify,
+                      dynamics);
 }
 
 // the traversability bits of the last path or field call (X*Y*ceil(Z/32) words of the map it ran on, grid.bits' layout)

@@ -43,7 +43,8 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_get_plan_info", "isdf_callback_batch_ragged", "isdf_callback_batch_ragged_device", "isdf_lbfgs_batch_ragged",
                "isdf_lbfgs_batch_ragged_device", "isdf_midend_callback_batch_ragged", "isdf_midend_batch_ragged",
                "isdf_midend_batch_ragged_device", "isdf_map_esdf", "isdf_get_esdf_f64", "isdf_esdf_query", "isdf_esdf_query_device",
-               "isdf_trajectory_states", "isdf_trajectory_states_device", "isdf_pose_points", "isdf_pose_points_device"]
+               "isdf_trajectory_states", "isdf_trajectory_states_device", "isdf_pose_points", "isdf_pose_points_device",
+               "isdf_frontend_path_pairs", "isdf_frontend_path_pairs_device", "isdf_frontend_path_fields_device", "isdf_plan_pairs"]
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
 DYN_QUANTITIES = ["speed", "acceleration", "body_rate", "tilt", "thrust"]   # q of isdf_dynamics_summary; mask bit 5: the thrust minimum
@@ -330,6 +331,9 @@ def load_library(path=None):
     lib.isdf_frontend_path_batch_device.argtypes = [vp, dp, C.c_int, vp, fpp, C.c_int, vp, vp, vp, vp, vp, vp]
     lib.isdf_frontend_path_field_device.argtypes = [vp, dp, fpp, vp, vp]
     lib.isdf_frontend_path_info.argtypes = [vp, C.POINTER(FrontPathInfo)]
+    lib.isdf_frontend_path_pairs.argtypes = [vp, C.c_int, dp, dp, fpp, C.c_int, C.c_int, dp, dp, ip, dp, u8p]
+    lib.isdf_frontend_path_pairs_device.argtypes = [vp, C.c_int, vp, vp, fpp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]
+    lib.isdf_frontend_path_fields_device.argtypes = [vp, C.c_int, dp, fpp, vp, vp]
     mpp = C.POINTER(MidendParams)
     lib.isdf_path_waypoints.argtypes = [C.c_int, ip, dp, C.c_double, C.c_double, C.c_int, dp, ip, ip]
     lib.isdf_midend_default_params.argtypes = [mpp]
@@ -340,6 +344,8 @@ def load_library(path=None):
     lib.isdf_plan_default_params.argtypes = [vp, C.POINTER(PlanParams)]
     lib.isdf_plan_batch.argtypes = [vp, dp, C.c_int, dp, C.POINTER(PlanParams), C.c_int, ip, dp, C.c_int, ip, dp, dp, C.POINTER(PlanResult),
                                     C.POINTER(CertifySummary), C.POINTER(DynamicsSummary)]
+    lib.isdf_plan_pairs.argtypes = [vp, C.c_int, dp, dp, C.POINTER(PlanParams), C.c_int, C.c_int, ip, dp, C.c_int, ip, dp, dp,
+                                    C.POINTER(PlanResult), C.POINTER(CertifySummary), C.POINTER(DynamicsSummary)]
     lib.isdf_get_plan_info.argtypes = [vp, C.POINTER(PlanInfo)]
     lib.isdf_callback_batch_ragged.argtypes = [vp, C.c_int, ip, dp, dp, C.c_int, C.c_double, dp, dp, dp]
     lib.isdf_callback_batch_ragged_device.argtypes = [vp, C.c_int, ip, vp, vp, C.c_int, C.c_double, vp, vp, vp, vp]
@@ -974,18 +980,28 @@ class Evaluator:
         coeffs (18 N, the plan's own 6N x 3 column-major block; empty without a trajectory), certify / dynamics summary dicts (None when the
         flag is off). params: an isdf_plan_params, or None for plan_params(**kw). The caps are sized from the goals and the call repeated once
         with the reported sizes when they are too small."""
+        st, gl = _f64(start).reshape(3), _f64(goals).reshape(-1, 3)
+        return self._plan(lambda *args: self.lib.isdf_plan_batch(self.h, _dp(st), gl.shape[0], _dp(gl), *args), gl.shape[0], params, kw)
+
+    def plan_pairs(self, starts, goals, params=None, max_fields=0, **kw):
+        """isdf_plan_pairs: B (start, goal) pairs, start b with goal b -> what plan_batch returns, in pair order. max_fields: the fields
+        of distinct start voxels held at once (0: the library's 4 GiB budget)"""
+        sts, gl = _f64(starts).reshape(-1, 3), _f64(goals).reshape(-1, 3)
+        if sts.shape != gl.shape:
+            raise ValueError(f"starts and goals must both be (B, 3), got {sts.shape} and {gl.shape}")
+        B = gl.shape[0]
+        return self._plan(lambda p, *args: self.lib.isdf_plan_pairs(self.h, B, _dp(sts), _dp(gl), p, int(max_fields), *args), B, params, kw)
+
+    def _plan(self, call, B, params, kw):
+        """call(params, cap_nodes, path_off, path_xyz, cap_pieces, piece_off, T, coeffs, results, certify, dynamics): the C call"""
         p = params if params is not None else self.plan_params(**kw)
-        st = _f64(start).reshape(3)
-        goals = _f64(goals).reshape(-1, 3)
-        B = goals.shape[0]
         ip = C.POINTER(C.c_int32)
         cap_nodes, cap_pieces = self._path_cap(None) * B, 290 * B
         for attempt in range(2):
             xyz, po, T, Cc = np.zeros((max(cap_nodes, 1), 3)), np.zeros(B + 1, dtype=np.int32), np.zeros(max(cap_pieces, 1)), np.zeros(18 * max(cap_pieces, 1))
             pf = np.zeros(B + 1, dtype=np.int32)
             res, cs, ds = (PlanResult * B)(), (CertifySummary * B)(), (DynamicsSummary * B)()
-            r = self.lib.isdf_plan_batch(self.h, _dp(st), B, _dp(goals), C.byref(p), cap_nodes, pf.ctypes.data_as(ip), _dp(xyz), cap_pieces,
-                                         po.ctypes.data_as(ip), _dp(T), _dp(Cc), res, cs, ds)
+            r = call(C.byref(p), cap_nodes, pf.ctypes.data_as(ip), _dp(xyz), cap_pieces, po.ctypes.data_as(ip), _dp(T), _dp(Cc), res, cs, ds)
             if r == -1 and attempt == 0 and (pf[B] > cap_nodes or po[B] > cap_pieces):
                 cap_nodes, cap_pieces = max(cap_nodes, int(pf[B])), max(cap_pieces, int(po[B]))
                 continue
@@ -1327,6 +1343,38 @@ class Evaluator:
         return dict(paths=[xyz[off[b]:off[b + 1]] for b in range(B)], roll_pitch=[rp[off[b]:off[b + 1]] for b in range(B)],
                     xyz=xyz[:n], rp=rp[:n], offsets=off, costs=cost, found=found.astype(bool))
 
+    def frontend_path_pairs(self, starts, goals, cap=None, max_fields=0):
+        """B (start, goal) pairs, start b with goal b -> what frontend_path_batch returns, in pair order (isdf_frontend_path_pairs).
+        max_fields: the fields of distinct start voxels held at once (0: the library's 4 GiB budget)"""
+        sts, goals = _f64(starts).reshape(-1, 3), _f64(goals).reshape(-1, 3)
+        if sts.shape != goals.shape:
+            raise ValueError(f"starts and goals must both be (B, 3), got {sts.shape} and {goals.shape}")
+        B = goals.shape[0]
+        cap = self._path_cap(cap)
+        for attempt in range(2):
+            xyz, rp = np.zeros((max(cap, 1), 3)), np.zeros((max(cap, 1), 2))
+            off, cost, found = np.zeros(B + 1, dtype=np.int32), np.zeros(B), np.zeros(B, dtype=np.uint8)
+            r = self.lib.isdf_frontend_path_pairs(self.h, B, _dp(sts), _dp(goals), None, int(max_fields), cap, _dp(xyz), _dp(rp),
+                                                  off.ctypes.data_as(C.POINTER(C.c_int32)), _dp(cost), found.ctypes.data_as(C.POINTER(C.c_uint8)))
+            if r == -1 and attempt == 0 and off[B] > cap:
+                cap = int(off[B])
+                continue
+            self._check(r)
+            break
+        n = int(off[B])
+        return dict(paths=[xyz[off[b]:off[b + 1]] for b in range(B)], roll_pitch=[rp[off[b]:off[b + 1]] for b in range(B)],
+                    xyz=xyz[:n], rp=rp[:n], offsets=off, costs=cost, found=found.astype(bool))
+
+    def frontend_path_pairs_raw(self, starts, goals, cap, max_fields=0):
+        """isdf_frontend_path_pairs with the caller's cap: (status, offsets)"""
+        sts, goals = _f64(starts).reshape(-1, 3), _f64(goals).reshape(-1, 3)
+        B = goals.shape[0]
+        xyz, rp = np.zeros((max(cap, 1), 3)), np.zeros((max(cap, 1), 2))
+        off, cost, found = np.full(B + 1, -7, dtype=np.int32), np.zeros(B), np.zeros(B, dtype=np.uint8)
+        r = self.lib.isdf_frontend_path_pairs(self.h, B, _dp(sts), _dp(goals), None, int(max_fields), int(cap), _dp(xyz), _dp(rp),
+                                              off.ctypes.data_as(C.POINTER(C.c_int32)), _dp(cost), found.ctypes.data_as(C.POINTER(C.c_uint8)))
+        return r, off
+
     def frontend_path(self, start, goal, cap=None):
         """-> (path (n, 3), roll_pitch (n, 2), cost, found), through isdf_frontend_path"""
         st, gl = _f64(start).reshape(3), _f64(goal).reshape(3)
@@ -1357,6 +1405,15 @@ class Evaluator:
     def frontend_path_field_device(self, start, d_g, stream=None):
         st = _f64(start).reshape(3)
         self._check(self.lib.isdf_frontend_path_field_device(self.h, _dp(st), None, d_g, stream))
+
+    def frontend_path_pairs_device(self, B, d_starts, d_goals, cap, d_xyz, d_rp, d_offsets, d_costs, d_found, stream=None, max_fields=0):
+        self._check(self.lib.isdf_frontend_path_pairs_device(self.h, int(B), d_starts, d_goals, None, int(max_fields), int(cap), d_xyz, d_rp,
+                                                             d_offsets, d_costs, d_found, stream))
+
+    def frontend_path_fields_device(self, starts, d_g, stream=None):
+        """the fields from S starts (S, 3) in one relaxation into d_g (a raw device pointer to S*X*Y*Z float64), field s at d_g + s*X*Y*Z"""
+        sts = _f64(starts).reshape(-1, 3)
+        self._check(self.lib.isdf_frontend_path_fields_device(self.h, sts.shape[0], _dp(sts), None, d_g, stream))
 
     def frontend_path_info(self):
         out = FrontPathInfo()

@@ -807,10 +807,10 @@ int isdf_frontend_check_batch(isdf_ctx *ctx, int n, const int32_t *ind, const do
 typedef struct isdf_frontpath_params {   /* NULL = defaults; the reserved fields must be zero */
     int32_t reserved_[4];
 } isdf_frontpath_params;
-typedef struct isdf_frontpath_info {       /* the last path or field call */
+typedef struct isdf_frontpath_info {       /* the last path, pairs or field call */
     int32_t rounds;                        /* relaxation rounds that had a non-empty frontier */
     int32_t reserved_;
-    int64_t field_bytes;                   /* device bytes of the FP64 field */
+    int64_t field_bytes;                   /* device bytes of the FP64 fields held at once */
     double traversability_ms, field_ms, paths_ms;   /* device time of the three stages (CUDA events on the call's stream) */
 } isdf_frontpath_info;
 int isdf_frontend_path(isdf_ctx *ctx, const double *start, const double *goal, const isdf_frontpath_params *params, int cap,
@@ -826,6 +826,30 @@ int isdf_frontend_path_batch_device(isdf_ctx *ctx, const double *start, int B, c
  * path exists. Same errors and stream behaviour as the device variant. */
 int isdf_frontend_path_field_device(isdf_ctx *ctx, const double *start, const isdf_frontpath_params *params, double *d_g, void *cuda_stream);
 int isdf_frontend_path_info(isdf_ctx *ctx, isdf_frontpath_info *out);
+/* ---- pairs: B (start, goal) pairs, start b with goal b (the reference's targetRcvCallBack pairs, plan_manager.cpp:434-488) ----
+ * Definition: pair b's path, roll and pitch, cost and found are bit-identical to isdf_frontend_path(starts[b], goals[b]); outputs in the
+ *   layout of isdf_frontend_path_batch, in pair order. Permuting the pairs permutes the outputs; max_fields never changes a bit.
+ * Work: the traversability grid is built once per call. Pairs whose starts share a voxel share one field (node 0 of a path is that voxel's
+ *   cube centre). The distinct start voxels' fields are relaxed together, up to max_fields at a time: each field held at once takes 8 B per
+ *   voxel (1 GiB at 512^3) and 2 frontier bits per voxel; max_fields = 0 holds at most 4 GiB of fields, and at least one field. Each
+ *   source's field is the exact field above whichever sources share its relaxation.
+ * isdf_frontend_path_info after a pairs or fields call: rounds is the total, over the chunks of fields, of the rounds in which any source
+ *   had a frontier; field_bytes the bytes of fields held at once; the stage times cover the whole call.
+ * Errors: those of isdf_frontend_path_batch, and ISDF_ERR_INVALID for max_fields < 0; isdf_last_error names the index of a start or goal
+ *   outside the map. */
+int isdf_frontend_path_pairs(isdf_ctx *ctx, int B, const double *starts, const double *goals, const isdf_frontpath_params *params,
+                             int max_fields, int cap, double *path_xyz, double *path_roll_pitch, int32_t *offsets, double *costs,
+                             uint8_t *found);
+/* device variant: d_starts and d_goals (B x 3 each) and every output on ctx's device; the starts and goals are read to the host to group
+ * them. Stream behaviour as isdf_frontend_path_batch_device. */
+int isdf_frontend_path_pairs_device(isdf_ctx *ctx, int B, const double *d_starts, const double *d_goals, const isdf_frontpath_params *params,
+                                    int max_fields, int cap, double *d_path_xyz, double *d_path_roll_pitch, int32_t *d_offsets,
+                                    double *d_costs, uint8_t *d_found, void *cuda_stream);
+/* the fields from S starts (host, S x 3) in one relaxation: field s at d_g + s*X*Y*Z (S*X*Y*Z doubles on ctx's device), each
+ * bit-identical to isdf_frontend_path_field_device(starts[s]), also when starts share a voxel. Errors: those of
+ * isdf_frontend_path_field_device, and ISDF_ERR_INVALID for S < 1 or S > 65535. */
+int isdf_frontend_path_fields_device(isdf_ctx *ctx, int S, const double *starts, const isdf_frontpath_params *params, double *d_g,
+                                     void *cuda_stream);
 
 /* ---- planning step: PlannerManager::generateTraj (plan_manager.cpp:202-313) for one start and B goals, end to end on the device ----
  * Definition, per goal b (each step is an existing entry point's definition):
@@ -896,7 +920,7 @@ typedef struct isdf_plan_result {
     int32_t midend_ret, backend_ret, backend_iterations, backend_evaluations;
     double path_cost, midend_f, backend_f, duration;
 } isdf_plan_result;
-typedef struct isdf_plan_info {     /* the last isdf_plan_batch call */
+typedef struct isdf_plan_info {     /* the last isdf_plan_batch or isdf_plan_pairs call */
     int32_t groups, backend_rounds;  /* distinct N that reached the mid-end; batched evaluations of the one back-end launch */
     double frontend_ms, midend_ms, gather_ms, backend_ms, certify_ms, dynamics_ms;   /* CUDA events on the call's stream */
 } isdf_plan_info;
@@ -904,6 +928,16 @@ typedef struct isdf_plan_info {     /* the last isdf_plan_batch call */
  * ctx may be NULL (isdf_default_config's values) */
 int isdf_plan_default_params(isdf_ctx *ctx, isdf_plan_params *p);
 int isdf_plan_batch(isdf_ctx *ctx, const double *start, int B, const double *goals, const isdf_plan_params *p,
+                    int cap_nodes, int32_t *path_off, double *path_xyz,
+                    int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
+                    isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics);
+/* B (start, goal) pairs: isdf_plan_batch's definition with starts[b] in place of start (its head is [path.front(), 0, 0] of its own path,
+ * the cube centre of its start voxel) and pair order in place of goal order; the front end is isdf_frontend_path_pairs(max_fields).
+ * Outputs, stages, errors, the durations rule, the state left behind and isdf_get_plan_info are isdf_plan_batch's, plus ISDF_ERR_INVALID
+ * for max_fields < 0. Pair b is bit-identical to isdf_plan_batch(starts[b], 1, &goals[b]); permuting the pairs permutes the outputs;
+ * max_fields never changes a bit; with every start equal, every output equals isdf_plan_batch(start, goals), which is this call with its
+ * start broadcast. */
+int isdf_plan_pairs(isdf_ctx *ctx, int B, const double *starts, const double *goals, const isdf_plan_params *p, int max_fields,
                     int cap_nodes, int32_t *path_off, double *path_xyz,
                     int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
                     isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics);
