@@ -16,6 +16,8 @@
 #include "isdf_map.cuh"
 #include "isdf_esdf.cuh"
 #include "isdf_states.cuh"
+#include "isdf_plan.cuh"
+#include <cub/device/device_scan.cuh>
 #include <queue>
 #include "isdf_host_mesh.cuh"
 #include <cstdio>
@@ -250,12 +252,22 @@ struct isdf_ctx {
     struct {   // batched obstacle gather: staged waypoints and offsets, per-row boxes, counts and offsets, the lists
         DevBuf<GatherBox> d_box; DevBuf<int> d_wpoff, d_cnt, d_ptoff; DevBuf<long long> d_offs, d_total; DevBuf<double> d_wp, d_out;
     } gat;
-    struct {   // planning step (isdf_plan_batch): one group's staging, mid-end and back-end results, and its returned trajectories
-        DevBuf<double> d_bc, d_wp, d_mx, d_mres, d_bbc, d_bx, d_bf, d_gT, d_gC; DevBuf<int> d_mi, d_bi;
+    struct {   // planning step (isdf_plan_pairs): the stages' buffers, the per-plan launch layouts, and the host forms' staged outputs
+        DevBuf<double> d_bc, d_wp, d_mx, d_mres, d_bbc, d_bx, d_bf, d_gT, d_gC, d_dur, d_pwp; DevBuf<int> d_mi, d_bi, d_N, d_idx, d_ok, d_bplan, d_gi;
         DevBuf<CertSummary> d_csum; DevBuf<DynSummary> d_dsum;
+        DevBuf<CopySeg> d_seg; DevBuf<PlanRow> d_row;
+        DevBuf<int32_t> s_path_off, s_piece_off; DevBuf<double> s_xyz, s_T, s_C;   // the host forms' staging
+        DevBuf<PlanResult> s_res; DevBuf<CertSummary> s_cert; DevBuf<DynSummary> s_dyn;
         cudaEvent_t ev[2] = {};
         isdf_plan_info info = {};
+        long long xfer[4] = {};   // the last planning call's transfers (isdf_dbg_plan_transfers)
     } plan;
+    struct {   // waypoint selection on the device (isdf_path_waypoints_device): per-path counts and gaps, the scan's scratch
+        DevBuf<int32_t> d_cnt, d_gap; DevBuf<char> d_tmp; PinnedBuf<int32_t> h_total;
+    } wps;
+    // the host <-> device copies made so far at the planning pipeline's copy sites (count_copy): device-to-host bytes outside the rounds'
+    // reads, the rounds' 4-byte reads, host-to-device bytes, copies
+    long long xfer[4] = {};
     struct {   // trajectory states and posed body points (isdf_states.cuh): the host forms' staging, one pinned block and one copy each way
         PinnedBuf<double> h;
         DevBuf<double> d_in, d_out;
@@ -283,6 +295,14 @@ struct isdf_ctx {
 };
 
 static int set_device(isdf_ctx *c) { CU_TRY(cudaSetDevice(c->device)); return 0; }
+// one copy of the planning pipeline, counted in c->xfer: host-to-device or device-to-host, a round's termination read or not
+enum { XF_D2H_BYTES, XF_ROUND_READS, XF_H2D_BYTES, XF_COPIES };
+static void count_copy(isdf_ctx *c, cudaMemcpyKind k, size_t bytes, bool round_read = false) {
+    if (k == cudaMemcpyDeviceToHost) { if (round_read) c->xfer[XF_ROUND_READS]++; else c->xfer[XF_D2H_BYTES] += (long long)bytes; }
+    else if (k == cudaMemcpyHostToDevice) c->xfer[XF_H2D_BYTES] += (long long)bytes;
+    else return;
+    c->xfer[XF_COPIES]++;
+}
 // the context's device, with the work enqueued on its stream (and, with aux, on its work-item stream) finished
 static int sync_ctx(isdf_ctx *c, bool aux = false) {
     if (set_device(c)) return ISDF_ERR_CUDA;
@@ -1434,6 +1454,7 @@ static int gather_batch_run(isdf_ctx *c, int B, const int *h_wp_off, const int *
     pt_off.assign((size_t)B + 1, 0);
     CU_TRY(cudaMemcpyAsync(pt_off.data(), g.d_ptoff.p, sizeof(int) * ((size_t)B + 1), cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaMemcpyAsync(total, g.d_total.p, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    count_copy(c, cudaMemcpyDeviceToHost, sizeof(int) * ((size_t)B + 1)); count_copy(c, cudaMemcpyDeviceToHost, sizeof(long long));
     CU_TRY(cudaStreamSynchronize(st));
     if (*total > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "the obstacle lists hold more than 2^31 - 1 points");
     if (*total > cap) return fail(ISDF_ERR_INVALID, "cap smaller than the obstacle lists (pt_off reports their sizes)");
@@ -1449,7 +1470,10 @@ static int gather_batch_run(isdf_ctx *c, int B, const int *h_wp_off, const int *
 // up both sets and switches the batched term off
 static int gather_set_points(isdf_ctx *c, int B, const std::vector<int> &pt_off, long long total, cudaStream_t st) {
     if (total == 0) CU_TRY(c->sv.set_points(nullptr, 0, st));
-    else CU_TRY(c->sv.set_points_batch(B, pt_off.data(), c->gat.d_out.p, st, cudaMemcpyDeviceToDevice));
+    else {
+        CU_TRY(c->sv.set_points_batch(B, pt_off.data(), c->gat.d_out.p, st, cudaMemcpyDeviceToDevice));
+        count_copy(c, cudaMemcpyHostToDevice, sizeof(int) * ((size_t)B + 1));   // the offsets
+    }
     return 0;
 }
 
@@ -1847,6 +1871,7 @@ static int lbfgs_rounds(isdf_ctx *c, isdf_ctx::LbfgsBufs &lb, int B, int n, cons
         std::vector<double> init((size_t)B * LB_NSCALAR, 0.0);
         for (int b = 0; b < B; b++) init[(size_t)b * LB_NSCALAR + 2] = 1.0;
         CU_TRY(cudaMemcpyAsync(L.sc, init.data(), sizeof(double) * init.size(), cudaMemcpyHostToDevice, st));
+        count_copy(c, cudaMemcpyHostToDevice, sizeof(double) * init.size());
         CU_TRY(cudaStreamSynchronize(st));
     }
     int rounds = 0;
@@ -1857,6 +1882,7 @@ static int lbfgs_rounds(isdf_ctx *c, isdf_ctx::LbfgsBufs &lb, int B, int n, cons
         c->stats.kernel_launches++;
         CU_TRY(cudaGetLastError());
         CU_TRY(cudaMemcpyAsync(lb.h_active.p, L.active, sizeof(int), cudaMemcpyDeviceToHost, st));
+        count_copy(c, cudaMemcpyDeviceToHost, sizeof(int), true);
         CU_TRY(cudaStreamSynchronize(st));
         ++rounds;
         if (*lb.h_active.p == 0) break;
@@ -2032,6 +2058,43 @@ extern "C" int isdf_path_waypoints(int B, const int32_t *path_off, const double 
         wp_off[b + 1] = (int32_t)total;
         pieces[b] = (int32_t)(n + 1);
     }
+    if (total > cap) return fail(ISDF_ERR_INVALID, "cap smaller than the number of waypoints (wp_off reports it)");
+    return 0;
+}
+
+// isdf_path_waypoints on the device (isdf_plan.cuh), on stream st: counts and pieces, wp_off by a scan, then the rows below cap. *total
+// (may be null: nothing is read) gets wp_off[B], one 4-byte read.
+static int waypoints_run(isdf_ctx *c, int B, const int32_t *d_path_off, const double *d_xyz, double res, double parlength, long long cap,
+                         double *d_wp, int32_t *d_wp_off, int32_t *d_pieces, int *total, cudaStream_t st) {
+    auto &z = c->wps;
+    CU_TRY(z.d_cnt.ensure(B)); CU_TRY(z.d_gap.ensure(B));
+    size_t tmp = 0;
+    CU_TRY(cub::DeviceScan::InclusiveSum(nullptr, tmp, z.d_cnt.p, d_wp_off + 1, B, st));
+    CU_TRY(z.d_tmp.ensure(std::max<size_t>(tmp, 1)));
+    k_wp_count<<<(unsigned)((B + 127) / 128), 128, 0, st>>>(B, d_path_off, res, parlength, z.d_cnt.p, z.d_gap.p, d_pieces, d_wp_off);
+    CU_TRY(cub::DeviceScan::InclusiveSum(z.d_tmp.p, tmp, z.d_cnt.p, d_wp_off + 1, B, st));
+    if (cap > 0) k_wp_write<<<(unsigned)(((long long)B * 32 + 127) / 128), 128, 0, st>>>(B, d_path_off, d_xyz, z.d_gap.p, d_wp_off, cap, d_wp);
+    c->stats.kernel_launches += cap > 0 ? 3 : 2;
+    CU_TRY(cudaGetLastError());
+    if (total) {
+        CU_TRY(z.h_total.ensure(1));
+        CU_TRY(cudaMemcpyAsync(z.h_total.p, d_wp_off + B, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        count_copy(c, cudaMemcpyDeviceToHost, sizeof(int32_t));
+        CU_TRY(cudaStreamSynchronize(st));
+        *total = *z.h_total.p;
+    }
+    return 0;
+}
+
+extern "C" int isdf_path_waypoints_device(isdf_ctx *c, int B, const int32_t *d_path_off, const double *d_path_xyz, double res, double parlength,
+                                          int cap, double *d_waypoints, int32_t *d_wp_off, int32_t *d_pieces, void *cuda_stream) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (B < 1 || !d_path_off || !d_path_xyz || !d_wp_off || !d_pieces || cap < 0 || (cap > 0 && !d_waypoints))
+        return fail(ISDF_ERR_INVALID, "NULL argument, B < 1 or cap < 0");
+    if (!(std::isfinite(res) && res > 0.0) || !(std::isfinite(parlength) && parlength > 0.0)) return fail(ISDF_ERR_INVALID, "res and parlength must be finite and positive");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    int total = 0;
+    if (int r = waypoints_run(c, B, d_path_off, d_path_xyz, res, parlength, cap, d_waypoints, d_wp_off, d_pieces, &total, (cudaStream_t)cuda_stream)) return r;
     if (total > cap) return fail(ISDF_ERR_INVALID, "cap smaller than the number of waypoints (wp_off reports it)");
     return 0;
 }
@@ -2497,6 +2560,7 @@ static int refine_rounds(isdf_ctx *c, RefineBufs &z, Args &A, long long S0, long
         CU_TRY(launch(A, st));
         c->stats.kernel_launches += 2;
         CU_TRY(cudaMemcpyAsync(z.h_tot.p, z.d_tot.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+        count_copy(c, cudaMemcpyDeviceToHost, sizeof(int), true);
         CU_TRY(cudaStreamSynchronize(st));
         const long long ns = *z.h_tot.p;
         if (int rr = after(nact, ns)) return rr;
@@ -3366,6 +3430,7 @@ static int path_fields(isdf_ctx *c, int n, const int *src, unsigned long long *d
     CU_TRY(c->fp.d_front.ensure(2 * (size_t)n * nword));
     CU_TRY(c->fp.d_flags.ensure(nflag));
     CU_TRY(c->fp.d_src.upload(src, (size_t)3 * n, st));
+    count_copy(c, cudaMemcpyHostToDevice, sizeof(int) * 3 * (size_t)n);
     PathArgs P = path_args(c, d_g);
     P.flags = c->fp.d_flags.p; P.rounds = P.flags + (size_t)(n + 1) * FP_FLAG_RING;
     P.any = n == 1 ? P.flags : P.flags + (size_t)n * FP_FLAG_RING;
@@ -3385,11 +3450,13 @@ static int path_fields(isdf_ctx *c, int n, const int *src, unsigned long long *d
         c->stats.kernel_launches += FP_ROUNDS_PER_CHECK;
         CU_TRY(cudaGetLastError());
         CU_TRY(cudaMemcpyAsync(c->fp.h_flag.p, P.any + r % FP_FLAG_RING, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+        count_copy(c, cudaMemcpyDeviceToHost, sizeof(unsigned), true);
         CU_TRY(cudaStreamSynchronize(st));
         if (!c->fp.h_flag.p[0]) break;
     }
     CU_TRY(cudaEventRecord(c->fp.ev[3], st));
     CU_TRY(cudaMemcpyAsync(c->fp.h_flag.p + 1, P.rounds, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    count_copy(c, cudaMemcpyDeviceToHost, sizeof(unsigned), true);
     CU_TRY(cudaStreamSynchronize(st));
     float ms = 0;
     cudaEventElapsedTime(&ms, c->fp.ev[2], c->fp.ev[3]);
@@ -3447,6 +3514,7 @@ static int path_run(isdf_ctx *c, int B, const double *starts, int sstride, const
     CU_TRY(c->fp.d_g.ensure((size_t)F * nvox));
     CU_TRY(c->fp.d_tgt.upload(wtgt.data(), wtgt.size(), st)); CU_TRY(c->fp.d_tsrc.upload(wsrc.data(), wsrc.size(), st));
     CU_TRY(c->fp.d_pair.upload(walk.data(), walk.size(), st));
+    count_copy(c, cudaMemcpyHostToDevice, sizeof(int) * (wtgt.size() + wsrc.size() + walk.size())); c->xfer[XF_COPIES] += 2;
     CU_TRY(c->fp.d_len.ensure(B)); CU_TRY(c->fp.d_woff.ensure((size_t)B + 1)); CU_TRY(c->fp.d_cost.ensure(B)); CU_TRY(c->fp.d_found.ensure(B));
     std::vector<int> len(B), woff((size_t)B + 1, 0);   // walk order; woff: first node in scratch
     for (int s0 = 0; s0 < S; s0 += F) {
@@ -3460,6 +3528,7 @@ static int path_run(isdf_ctx *c, int B, const double *starts, int sstride, const
         c->stats.kernel_launches++;
         CU_TRY(cudaGetLastError());
         CU_TRY(cudaMemcpyAsync(len.data() + w0, P.len, sizeof(int) * nt, cudaMemcpyDeviceToHost, st));
+        count_copy(c, cudaMemcpyDeviceToHost, sizeof(int) * nt);
         CU_TRY(cudaStreamSynchronize(st));
         for (int w = w0; w < w1; w++) {
             if ((long long)woff[w] + len[w] > INT32_MAX) return fail(ISDF_ERR_INVALID, "the paths hold more than 2^31 - 1 nodes");
@@ -3473,6 +3542,7 @@ static int path_run(isdf_ctx *c, int B, const double *starts, int sstride, const
             std::swap(c->fp.d_scratch, grown);
         }
         CU_TRY(cudaMemcpyAsync(c->fp.d_woff.p + w0, woff.data() + w0, sizeof(int) * ((size_t)nt + 1), cudaMemcpyHostToDevice, st));
+        count_copy(c, cudaMemcpyHostToDevice, sizeof(int) * ((size_t)nt + 1));
         P.off = c->fp.d_woff.p + w0; P.scratch = c->fp.d_scratch.p;
         k_fp_walk<<<wblocks, 128, 0, st>>>(P, 1);
         c->stats.kernel_launches++;
@@ -3486,6 +3556,7 @@ static int path_run(isdf_ctx *c, int B, const double *starts, int sstride, const
     const int total = off[B];
     if (total > cap) return fail(ISDF_ERR_INVALID, "cap is smaller than the total path length (reported in n / offsets[B])");
     CU_TRY(c->fp.d_off.upload(off.data(), off.size(), st)); CU_TRY(c->fp.d_soff.upload(soff.data(), soff.size(), st));
+    count_copy(c, cudaMemcpyHostToDevice, sizeof(int) * (off.size() + soff.size())); c->xfer[XF_COPIES]++;
     CU_TRY(c->fp.d_nodes.ensure((size_t)3 * total)); CU_TRY(c->fp.d_colliding.ensure((size_t)4 * total));
     CU_TRY(c->fp.d_xyz.ensure((size_t)3 * total)); CU_TRY(c->fp.d_rp.ensure((size_t)2 * total));
     PathArgs P = path_args(c, c->fp.d_g.p);
@@ -3674,11 +3745,62 @@ static int plan_check(isdf_ctx *c, const isdf_plan_params *p, double *r_cert) {
     return 0;
 }
 
+// The outputs of the planning pipeline, in device memory in include/isdf.h's layout. Staged (the host forms): path_off, piece_off, res,
+// cert and dyn are c->plan's staging, and plan_run points path_xyz, T and coeffs into it once the sizes are known.
+struct PlanOut {
+    int32_t *path_off = nullptr, *piece_off = nullptr;
+    double *path_xyz = nullptr, *T = nullptr, *coeffs = nullptr;
+    PlanResult *res = nullptr; CertSummary *cert = nullptr; DynSummary *dyn = nullptr;
+    bool staged = false, want_xyz = false;   // want_xyz: the paths' nodes are an output
+    bool sized = false;                      // path_off (when wanted) and piece_off hold the sizes
+    int nodes = 0, pieces = 0;
+};
+static_assert(sizeof(isdf_plan_result) == sizeof(PlanResult) && offsetof(isdf_plan_result, path_cost) == offsetof(PlanResult, path_cost) &&
+              offsetof(isdf_plan_result, duration) == offsetof(PlanResult, duration), "isdf_plan_result layout");
+static_assert(sizeof(isdf_certify_summary) == sizeof(CertSummary) && offsetof(isdf_certify_summary, voxel_min) == offsetof(CertSummary, voxel_min) &&
+              offsetof(isdf_certify_summary, depth) == offsetof(CertSummary, depth), "isdf_certify_summary layout");
+
+// a host array of the pipeline's launch layouts to the device on st
+template <typename T>
+static int plan_upload(isdf_ctx *c, DevBuf<T> &buf, const std::vector<T> &h, cudaStream_t st) {
+    CU_TRY(buf.ensure(std::max<size_t>(h.size(), 1)));
+    if (h.empty()) return 0;
+    CU_TRY(cudaMemcpyAsync(buf.p, h.data(), sizeof(T) * h.size(), cudaMemcpyHostToDevice, st));
+    count_copy(c, cudaMemcpyHostToDevice, sizeof(T) * h.size());
+    return 0;
+}
+
+// one copy stage: every segment in one launch
+static int copy_segments(isdf_ctx *c, const std::vector<CopySeg> &seg, cudaStream_t st) {
+    if (seg.empty()) return 0;
+    if (int r = plan_upload(c, c->plan.d_seg, seg, st)) return r;
+    k_copy_segments<<<(unsigned)seg.size(), 128, 0, st>>>(c->plan.d_seg.p);
+    c->stats.kernel_launches++;
+    CU_TRY(cudaGetLastError());
+    return 0;
+}
+
+// a public struct as the device struct of the same layout
+template <typename D, typename S>
+static D same_layout(const S &s) {
+    static_assert(sizeof(D) == sizeof(S), "layouts differ");
+    D d;
+    std::memcpy(&d, &s, sizeof(D));
+    return d;
+}
+
+template <typename S>
+static int plan_fill(isdf_ctx *c, int n, const S &v, S *out, cudaStream_t st) {
+    k_plan_fill<S><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(n, v, out);
+    c->stats.kernel_launches++;
+    CU_TRY(cudaGetLastError());
+    return 0;
+}
+
+// The pipeline on stream st. Per plan, only the path lengths and found flags, N, the mid-end return codes and the gathered point counts
+// cross to the host, besides the rounds' 4-byte reads; everything sized by nodes, waypoints or pieces stays on the device.
 static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const double *goals, int max_fields, const isdf_plan_params *p,
-                    double r_cert, int cap_nodes,
-                    int32_t *path_off, double *path_xyz, int cap_pieces, int32_t *piece_off, double *T, double *coeffs, isdf_plan_result *res,
-                    isdf_certify_summary *certify, isdf_dynamics_summary *dynamics) {
-    const cudaStream_t st = c->stream;
+                    double r_cert, int cap_nodes, int cap_pieces, PlanOut &o, cudaStream_t st) {
     auto &z = c->plan;
     isdf_plan_info &info = z.info;
     info = {};
@@ -3694,218 +3816,257 @@ static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const
         acc += ms;
         return 0;
     };
-    const double nan = std::numeric_limits<double>::quiet_NaN();
     // 1. front end
     std::vector<int> off;
     if (int r = timed(info.frontend_ms, [&] { return path_run(c, B, starts, sstride, goals, max_fields, 0x7fffffff, off, st); })) return r;
     const int nodes = off[B];
-    std::vector<double> xyz((size_t)3 * nodes), pcost(B);
+    const int32_t *d_off = c->fp.d_off.p;
+    const double *d_xyz = c->fp.d_xyz.p;
+    // 2. waypoints: N and the rows of every path at wp_off (z.d_N = [N | wp_off])
+    CU_TRY(z.d_pwp.ensure((size_t)3 * std::max(nodes, 1))); CU_TRY(z.d_N.ensure((size_t)2 * B + 1));
+    if (int r = waypoints_run(c, B, d_off, d_xyz, c->map.grid.res, p->parlength, nodes, z.d_pwp.p, z.d_N.p + B, z.d_N.p, nullptr, st)) return r;
     std::vector<uint8_t> found(B);
-    CU_TRY(cudaMemcpyAsync(xyz.data(), c->fp.d_xyz.p, sizeof(double) * xyz.size(), cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaMemcpyAsync(pcost.data(), c->fp.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, st));
+    std::vector<int> N(B);
     CU_TRY(cudaMemcpyAsync(found.data(), c->fp.d_found.p, B, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaMemcpyAsync(N.data(), z.d_N.p, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
+    count_copy(c, cudaMemcpyDeviceToHost, B); count_copy(c, cudaMemcpyDeviceToHost, sizeof(int) * B);
     CU_TRY(cudaStreamSynchronize(st));
-    // 2. waypoints, stages known before the mid-end, sizes
-    std::vector<double> wps((size_t)3 * std::max(nodes, 1));
-    std::vector<int> wp_off((size_t)B + 1), N(B);
-    if (int r = isdf_path_waypoints(B, off.data(), xyz.data(), c->map.grid.res, p->parlength, nodes, wps.data(), wp_off.data(), N.data())) return r;
-    std::vector<int> poff((size_t)B + 1, 0);
+    // stages known before the mid-end, sizes
+    std::vector<int> poff((size_t)B + 1, 0), wpo((size_t)B + 1, 0);   // piece offsets; wp_off as the device holds it
+    std::vector<PlanRow> row(B);
     for (int b = 0; b < B; b++) {
         const bool traj = found[b] && minco_smem_bytes(N[b]) <= 220 * 1024;   // N <= 290 (minco_fits)
         const long long t = (long long)poff[b] + (traj ? N[b] : 0);
         if (t > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "the trajectories hold more than 2^31 - 1 pieces");
         poff[b + 1] = (int)t;
-        isdf_plan_result &q = res[b];
-        q = {};
-        q.stage = !found[b] ? ISDF_PLAN_NO_PATH : (traj ? ISDF_PLAN_OPTIMISED : ISDF_PLAN_TOO_LONG);   // OPTIMISED: pending until the mid-end
-        q.path_nodes = off[b + 1] - off[b]; q.pieces = found[b] ? N[b] : 0;
-        q.path_cost = pcost[b]; q.midend_f = q.backend_f = nan; q.duration = 0.0;
-        if (certify) certify[b] = certify_failed_summary();
-        if (dynamics) dynamics[b] = dynamics_failed_summary();
+        wpo[b + 1] = wpo[b] + N[b] - 1;
+        // OPTIMISED: pending until the mid-end
+        row[b] = {!found[b] ? ISDF_PLAN_NO_PATH : (traj ? ISDF_PLAN_OPTIMISED : ISDF_PLAN_TOO_LONG), off[b + 1] - off[b], found[b] ? N[b] : 0, 0, -1, -1};
     }
-    if (path_off) std::memcpy(path_off, off.data(), sizeof(int32_t) * off.size());
-    std::memcpy(piece_off, poff.data(), sizeof(int32_t) * poff.size());
-    if ((path_xyz && nodes > cap_nodes) || poff[B] > cap_pieces)
+    if (o.path_off) CU_TRY(cudaMemcpyAsync(o.path_off, d_off, sizeof(int32_t) * ((size_t)B + 1), cudaMemcpyDeviceToDevice, st));
+    CU_TRY(cudaMemcpyAsync(o.piece_off, poff.data(), sizeof(int32_t) * poff.size(), cudaMemcpyHostToDevice, st));
+    count_copy(c, cudaMemcpyHostToDevice, sizeof(int32_t) * poff.size());
+    o.sized = true; o.nodes = nodes; o.pieces = poff[B];
+    if ((o.want_xyz && nodes > cap_nodes) || poff[B] > cap_pieces)
         return fail(ISDF_ERR_INVALID, "cap_nodes or cap_pieces too small (path_off / piece_off report the sizes needed)");
-    if (path_xyz && nodes) std::memcpy(path_xyz, xyz.data(), sizeof(double) * xyz.size());
+    if (o.staged) {
+        if (o.want_xyz) { CU_TRY(z.s_xyz.ensure((size_t)3 * std::max(nodes, 1))); o.path_xyz = z.s_xyz.p; }
+        CU_TRY(z.s_T.ensure(std::max(poff[B], 1))); CU_TRY(z.s_C.ensure((size_t)18 * std::max(poff[B], 1)));
+        o.T = z.s_T.p; o.coeffs = z.s_C.p;
+    }
+    if (o.want_xyz && nodes) CU_TRY(cudaMemcpyAsync(o.path_xyz, d_xyz, sizeof(double) * 3 * (size_t)nodes, cudaMemcpyDeviceToDevice, st));
     // 3-6. one ragged mid-end over every plan that reaches it, one gather and one ragged back end over the plans that pass it, in pair order
     std::vector<int> idx;   // the plans that reach the mid-end
-    for (int b = 0; b < B; b++) if (res[b].stage == ISDF_PLAN_OPTIMISED) idx.push_back(b);
+    for (int b = 0; b < B; b++) if (row[b].stage == ISDF_PLAN_OPTIMISED) idx.push_back(b);
     std::vector<int> Ns;
     for (const int b : idx) Ns.push_back(N[b]);
     std::sort(Ns.begin(), Ns.end());
     Ns.erase(std::unique(Ns.begin(), Ns.end()), Ns.end());
     info.groups = (int)Ns.size();
     const int Bg = (int)idx.size();
-    if (Bg == 0) return 0;
-    // plan idx[q] owns mid-end pieces [moff[q], moff[q+1]) and waypoint rows [moff[q] - q, moff[q+1] - q - 1); head = [path.front(), 0, 0],
-    // tail = [path.back(), 0, 0] (3x3 column-major, column 0 the position): [heads | tails]
-    std::vector<int> moff((size_t)Bg + 1, 0);
-    for (int q = 0; q < Bg; q++) moff[q + 1] = moff[q] + N[idx[q]];
-    const size_t MP = (size_t)moff[Bg];
-    std::vector<double> bc((size_t)18 * Bg, 0.0), gw(3 * std::max<size_t>(MP - Bg, 1));
-    for (int q = 0; q < Bg; q++) {
-        const int b = idx[q];
-        for (int k = 0; k < 3; k++) { bc[9 * (size_t)q + k] = xyz[3 * (size_t)off[b] + k]; bc[9 * ((size_t)Bg + q) + k] = xyz[3 * ((size_t)off[b + 1] - 1) + k]; }
-        std::copy(wps.begin() + 3 * (size_t)wp_off[b], wps.begin() + 3 * (size_t)wp_off[b + 1], gw.begin() + 3 * ((size_t)moff[q] - q));
-    }
-    Layout ML;
-    if (int r = midend_ragged_check(c, Bg, moff.data(), &p->midend, &ML)) return r;
-    if (int r = ragged_upload(c->mid.d_off, moff.data(), st, &ML)) return r;
-    CU_TRY(z.d_bc.upload(bc.data(), bc.size(), st)); CU_TRY(z.d_wp.upload(gw.data(), gw.size(), st));
-    CU_TRY(z.d_mx.ensure(ML.X)); CU_TRY(z.d_mres.ensure(19 * MP + Bg)); CU_TRY(z.d_mi.ensure((size_t)3 * Bg));
-    double *d_mf = z.d_mres.p, *d_mT = d_mf + Bg, *d_mC = d_mT + MP;   // [f | T | coeffs]
-    int mrounds = 0;
-    if (int r = timed(info.midend_ms, [&] {
-            return midend_batch_run(c, ML, z.d_bc.p, z.d_bc.p + 9 * (size_t)Bg, 1, &p->midend, z.d_wp.p, z.d_mx.p, d_mT, d_mC, d_mf, z.d_mi.p,
-                                    z.d_mi.p + Bg, z.d_mi.p + 2 * (size_t)Bg, &mrounds, st);
-        })) return r;
-    std::vector<double> mres(19 * MP + Bg);   // [f | T | coeffs]
-    std::vector<int> mi((size_t)3 * Bg);
-    CU_TRY(cudaMemcpyAsync(mres.data(), d_mf, sizeof(double) * mres.size(), cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaMemcpyAsync(mi.data(), z.d_mi.p, sizeof(int) * mi.size(), cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    std::vector<int> ok, pos(Bg, -1);   // the plans that passed the mid-end (plan_manager.cpp:277) and their back-end instance
-    for (int q = 0; q < Bg; q++) {
-        isdf_plan_result &r = res[idx[q]];
-        r.midend_f = mres[q]; r.midend_ret = mi[q];
-        if (mi[q] >= 0) { pos[q] = (int)ok.size(); ok.push_back(q); }
-        else r.stage = ISDF_PLAN_MIDEND_FAILED;
-    }
-    const int Bp = (int)ok.size();
-    std::vector<int> boff((size_t)Bp + 1, 0);   // back-end instance k owns pieces [boff[k], boff[k+1])
-    for (int k = 0; k < Bp; k++) boff[k + 1] = boff[k] + N[idx[ok[k]]];
-    const size_t BP = (size_t)boff[Bp];
-    std::vector<double> bres(19 * BP);          // the back end's final [T | coeffs]
-    if (Bp > 0) {
-        // 4. the passed plans' obstacle lists become the batched point sets
-        std::vector<int> gwo((size_t)Bp + 1, 0);
-        std::vector<double> pw(3 * std::max<size_t>(BP - Bp, 1));
-        for (int k = 0; k < Bp; k++) {
-            const int q = ok[k], W = N[idx[q]] - 1;
-            gwo[k + 1] = gwo[k] + W;
-            std::copy(gw.begin() + 3 * ((size_t)moff[q] - q), gw.begin() + 3 * ((size_t)moff[q] - q + W), pw.begin() + 3 * (size_t)gwo[k]);
+    const double *d_mf = nullptr, *d_bf = nullptr;
+    const int *d_mi = nullptr, *d_bi = nullptr;
+    int Bp = 0;
+    if (Bg > 0) {
+        // plan idx[q] owns mid-end pieces [moff[q], moff[q+1]) and waypoint rows [moff[q] - q, moff[q+1] - q - 1); z.d_bc = [heads | tails]
+        std::vector<int> moff((size_t)Bg + 1, 0);
+        for (int q = 0; q < Bg; q++) moff[q + 1] = moff[q] + N[idx[q]];
+        const size_t MP = (size_t)moff[Bg];
+        Layout ML;
+        if (int r = midend_ragged_check(c, Bg, moff.data(), &p->midend, &ML)) return r;
+        if (int r = ragged_upload(c->mid.d_off, moff.data(), st, &ML)) return r;
+        count_copy(c, cudaMemcpyHostToDevice, sizeof(int) * (2 * (size_t)Bg + 2));
+        if (int r = plan_upload(c, z.d_idx, idx, st)) return r;
+        CU_TRY(z.d_bc.ensure((size_t)18 * Bg)); CU_TRY(z.d_wp.ensure(3 * std::max<size_t>(MP - Bg, 1)));
+        k_plan_bc<<<(unsigned)((Bg + 127) / 128), 128, 0, st>>>(Bg, z.d_idx.p, d_off, d_xyz, z.d_bc.p);
+        c->stats.kernel_launches++;
+        CU_TRY(cudaGetLastError());
+        std::vector<CopySeg> seg;
+        for (int q = 0; q < Bg; q++) {
+            const int b = idx[q];
+            if (N[b] > 1) seg.push_back({z.d_pwp.p + 3 * (size_t)wpo[b], z.d_wp.p + 3 * ((size_t)moff[q] - q), 3 * (long long)(N[b] - 1)});
         }
-        CU_TRY(c->gat.d_wpoff.upload(gwo.data(), gwo.size(), st)); CU_TRY(c->gat.d_wp.upload(pw.data(), pw.size(), st));
-        std::vector<int> pto;
-        long long tot = 0;
-        if (int r = timed(info.gather_ms, [&] {
-                if (int rr = gather_batch_run(c, Bp, gwo.data(), c->gat.d_wpoff.p, c->gat.d_wp.p, p->half_extent, p->offset, 0x7fffffffll, pto, &tot, st)) return rr;
-                return gather_set_points(c, Bp, pto, tot, st);
+        if (int r = copy_segments(c, seg, st)) return r;
+        CU_TRY(z.d_mx.ensure(ML.X)); CU_TRY(z.d_mres.ensure(19 * MP + Bg)); CU_TRY(z.d_mi.ensure((size_t)3 * Bg));
+        double *mf = z.d_mres.p, *d_mT = mf + Bg, *d_mC = d_mT + MP;   // [f | T | coeffs]
+        int mrounds = 0;
+        if (int r = timed(info.midend_ms, [&] {
+                return midend_batch_run(c, ML, z.d_bc.p, z.d_bc.p + 9 * (size_t)Bg, 1, &p->midend, z.d_wp.p, z.d_mx.p, d_mT, d_mC, mf, z.d_mi.p,
+                                        z.d_mi.p + Bg, z.d_mi.p + 2 * (size_t)Bg, &mrounds, st);
             })) return r;
-        for (int k = 0; k < Bp; k++) res[idx[ok[k]]].obstacle_points = pto[k + 1] - pto[k];
-        // 5. persisted durations: what updateTraj(mid-end trajectory) leaves on a fresh context (swm:287-296)
-        std::vector<double> dur(Bp);
-        for (int k = 0; k < Bp; k++) {
-            const int q = ok[k];
-            double td = 0.0;
-            for (int i = moff[q]; i < moff[q + 1]; i++) td += mres[Bg + (size_t)i];
-            dur[k] = td < 3 * 1e2 ? td : 0.0;
+        d_mf = mf; d_mi = z.d_mi.p;
+        std::vector<int> mi(Bg);
+        CU_TRY(cudaMemcpyAsync(mi.data(), z.d_mi.p, sizeof(int) * Bg, cudaMemcpyDeviceToHost, st));
+        count_copy(c, cudaMemcpyDeviceToHost, sizeof(int) * Bg);
+        CU_TRY(cudaStreamSynchronize(st));
+        std::vector<int> ok, pos(Bg, -1);   // the plans that passed the mid-end (plan_manager.cpp:277) and their back-end instance
+        for (int q = 0; q < Bg; q++) {
+            row[idx[q]].q = q;
+            if (mi[q] >= 0) { pos[q] = (int)ok.size(); ok.push_back(q); }
+            else row[idx[q]].stage = ISDF_PLAN_MIDEND_FAILED;
         }
-        CU_TRY(c->sv.set_durations(Bp, dur.data(), st));
-        // 6. back end from the mid-end x
-        std::vector<double> bbc((size_t)18 * Bp);
-        for (int k = 0; k < Bp; k++) {
-            std::copy(bc.begin() + 9 * (size_t)ok[k], bc.begin() + 9 * ((size_t)ok[k] + 1), bbc.begin() + 9 * (size_t)k);
-            std::copy(bc.begin() + 9 * ((size_t)Bg + ok[k]), bc.begin() + 9 * ((size_t)Bg + ok[k] + 1), bbc.begin() + 9 * ((size_t)Bp + k));
+        Bp = (int)ok.size();
+        std::vector<int> boff((size_t)Bp + 1, 0);   // back-end instance k owns pieces [boff[k], boff[k+1])
+        for (int k = 0; k < Bp; k++) boff[k + 1] = boff[k] + N[idx[ok[k]]];
+        const size_t BP = (size_t)boff[Bp];
+        if (Bp > 0) {
+            // 4. the passed plans' obstacle lists become the batched point sets
+            std::vector<int> gwo((size_t)Bp + 1, 0);
+            CU_TRY(c->gat.d_wp.ensure(3 * std::max<size_t>(BP - Bp, 1)));
+            seg.clear();
+            for (int k = 0; k < Bp; k++) {
+                const int q = ok[k], W = N[idx[q]] - 1;
+                gwo[k + 1] = gwo[k] + W;
+                if (W) seg.push_back({z.d_wp.p + 3 * ((size_t)moff[q] - q), c->gat.d_wp.p + 3 * (size_t)gwo[k], 3 * (long long)W});
+            }
+            if (int r = copy_segments(c, seg, st)) return r;
+            if (int r = plan_upload(c, c->gat.d_wpoff, gwo, st)) return r;
+            std::vector<int> pto;
+            long long tot = 0;
+            if (int r = timed(info.gather_ms, [&] {
+                    if (int rr = gather_batch_run(c, Bp, gwo.data(), c->gat.d_wpoff.p, c->gat.d_wp.p, p->half_extent, p->offset, 0x7fffffffll, pto, &tot, st)) return rr;
+                    return gather_set_points(c, Bp, pto, tot, st);
+                })) return r;
+            for (int k = 0; k < Bp; k++) { row[idx[ok[k]]].points = pto[k + 1] - pto[k]; row[idx[ok[k]]].k = k; }
+            // 5. persisted durations: what updateTraj(mid-end trajectory) leaves on a fresh context (swm:287-296)
+            if (int r = plan_upload(c, z.d_ok, ok, st)) return r;
+            CU_TRY(z.d_dur.ensure(Bp));
+            k_plan_durations<<<(unsigned)((Bp + 127) / 128), 128, 0, st>>>(Bp, z.d_ok.p, ML.d_off, d_mT, z.d_dur.p);
+            c->stats.kernel_launches++;
+            CU_TRY(cudaGetLastError());
+            CU_TRY(c->sv.set_durations(Bp, z.d_dur.p, st, cudaMemcpyDeviceToDevice));
+            // 6. back end from the mid-end x
+            Layout BL;
+            if (int r = callback_ragged_check(c, Bp, boff.data(), &BL)) return r;
+            if (int r = ragged_upload(c->batch.d_off, boff.data(), st, &BL)) return r;
+            count_copy(c, cudaMemcpyHostToDevice, sizeof(int) * (2 * (size_t)Bp + 2));
+            std::vector<int> bplan(Bp);
+            for (int k = 0; k < Bp; k++) bplan[k] = idx[ok[k]];
+            if (int r = plan_upload(c, z.d_bplan, bplan, st)) return r;
+            CU_TRY(z.d_bbc.ensure((size_t)18 * Bp));
+            k_plan_bc<<<(unsigned)((Bp + 127) / 128), 128, 0, st>>>(Bp, z.d_bplan.p, d_off, d_xyz, z.d_bbc.p);
+            c->stats.kernel_launches++;
+            CU_TRY(cudaGetLastError());
+            const double *d_bh = z.d_bbc.p, *d_bt = z.d_bbc.p + 9 * (size_t)Bp;
+            CU_TRY(z.d_bx.ensure(BL.X)); CU_TRY(z.d_bf.ensure(Bp)); CU_TRY(z.d_bi.ensure((size_t)3 * Bp));
+            seg.clear();
+            for (int k = 0; k < Bp; k++) {
+                const int q = ok[k];
+                seg.push_back({z.d_mx.p + 4 * (size_t)moff[q] - 3 * (size_t)q, z.d_bx.p + 4 * (size_t)boff[k] - 3 * (size_t)k, 4 * (long long)N[idx[q]] - 3});
+            }
+            if (int r = copy_segments(c, seg, st)) return r;
+            int brounds = 0;
+            if (int r = timed(info.backend_ms, [&]() -> int {
+                    if (int rr = lbfgs_rounds(c, c->lbfgs, Bp, 4 * BL.N - 3, BL.d_xoff, BL.X, &p->backend, 0, z.d_bx.p, z.d_bf.p, z.d_bi.p, z.d_bi.p + Bp,
+                                              z.d_bi.p + 2 * (size_t)Bp, &brounds, st, [&](const double *x, double *f, double *g) {
+                                                  return callback_batch_launch(c, BL, d_bh, d_bt, 9, p->rho, x, f, g, st);
+                                              })) return rr;
+                    // the final trajectories: forwardT + MINCO of the returned x (back_end_optimizer.cpp:140-163), into the batch trajectories
+                    MincoArgs M = c->batch.minco.args(BL, d_bh, d_bt, 9, p->rho, z.d_bx.p);
+                    k_minco_forward<<<Bp, 32, minco_smem_bytes(BL.N), st>>>(M);
+                    c->stats.kernel_launches++;
+                    CU_TRY(cudaGetLastError());
+                    c->batch.B = Bp; c->batch.P = BP;
+                    return 0;
+                })) return r;
+            info.backend_rounds = brounds;
+            d_bf = z.d_bf.p; d_bi = z.d_bi.p;
         }
-        Layout BL;
-        if (int r = callback_ragged_check(c, Bp, boff.data(), &BL)) return r;
-        if (int r = ragged_upload(c->batch.d_off, boff.data(), st, &BL)) return r;
-        CU_TRY(z.d_bbc.upload(bbc.data(), bbc.size(), st));
-        const double *d_bh = z.d_bbc.p, *d_bt = z.d_bbc.p + 9 * (size_t)Bp;
-        CU_TRY(z.d_bx.ensure(BL.X)); CU_TRY(z.d_bf.ensure(Bp)); CU_TRY(z.d_bi.ensure((size_t)3 * Bp));
-        for (int k = 0; k < Bp; k++) {
-            const int q = ok[k];
-            const size_t n = 4 * (size_t)N[idx[q]] - 3;
-            CU_TRY(cudaMemcpyAsync(z.d_bx.p + 4 * (size_t)boff[k] - 3 * (size_t)k, z.d_mx.p + 4 * (size_t)moff[q] - 3 * (size_t)q, sizeof(double) * n,
-                                   cudaMemcpyDeviceToDevice, st));
+        // the returned trajectories, plan b's at piece_off[b]: the back end's, or the mid-end's for MIDEND_FAILED
+        seg.clear();
+        for (int q = 0; q < Bg; q++) {
+            const bool be = pos[q] >= 0;
+            const int Nq = N[idx[q]];
+            const size_t po = (size_t)poff[idx[q]], p0 = be ? (size_t)boff[pos[q]] : (size_t)moff[q], rows = 6 * (be ? BP : MP);
+            const double *sT = be ? c->batch.minco.d_T.p : d_mT, *sC = be ? c->batch.minco.d_C.p : d_mC;
+            seg.push_back({sT + p0, o.T + po, Nq});
+            for (int a = 0; a < 3; a++) seg.push_back({sC + a * rows + 6 * p0, o.coeffs + 18 * po + 6 * (size_t)a * Nq, 6 * (long long)Nq});
         }
-        int brounds = 0;
-        if (int r = timed(info.backend_ms, [&]() -> int {
-                if (int rr = lbfgs_rounds(c, c->lbfgs, Bp, 4 * BL.N - 3, BL.d_xoff, BL.X, &p->backend, 0, z.d_bx.p, z.d_bf.p, z.d_bi.p, z.d_bi.p + Bp,
-                                          z.d_bi.p + 2 * (size_t)Bp, &brounds, st, [&](const double *x, double *f, double *g) {
-                                              return callback_batch_launch(c, BL, d_bh, d_bt, 9, p->rho, x, f, g, st);
-                                          })) return rr;
-                // the final trajectories: forwardT + MINCO of the returned x (back_end_optimizer.cpp:140-163), into the batch trajectories
-                MincoArgs M = c->batch.minco.args(BL, d_bh, d_bt, 9, p->rho, z.d_bx.p);
-                k_minco_forward<<<Bp, 32, minco_smem_bytes(BL.N), st>>>(M);
+        if (int r = copy_segments(c, seg, st)) return r;
+    }
+    // the result records
+    if (int r = plan_upload(c, z.d_row, row, st)) return r;
+    k_plan_results<<<(unsigned)((B + 127) / 128), 128, 0, st>>>(B, z.d_row.p, c->fp.d_cost.p, d_mf, d_mi, d_bf, d_bi, Bp, o.piece_off, o.T, o.res);
+    c->stats.kernel_launches++;
+    CU_TRY(cudaGetLastError());
+    // 7. certificates on every returned trajectory, per group of plans with the same N, ascending; a plan without one reads as a failed call
+    if (o.cert) if (int r = plan_fill(c, B, same_layout<CertSummary>(certify_failed_summary()), o.cert, st)) return r;
+    if (o.dyn) if (int r = plan_fill(c, B, same_layout<DynSummary>(dynamics_failed_summary()), o.dyn, st)) return r;
+    if (p->flags & (ISDF_PLAN_CERTIFY | ISDF_PLAN_DYNAMICS)) {
+        for (const int Ng : Ns) {
+            std::vector<int> gi;   // the group's plans, in pair order
+            for (const int b : idx) if (N[b] == Ng) gi.push_back(b);
+            const int Bn = (int)gi.size();
+            const size_t BN = (size_t)Bn * Ng;
+            // the group's trajectories as one block (piece q*N + i of a 6BN x 3 column-major block)
+            CU_TRY(z.d_gT.ensure(BN)); CU_TRY(z.d_gC.ensure(18 * BN));
+            std::vector<CopySeg> seg;
+            for (int q = 0; q < Bn; q++) {
+                const size_t po = (size_t)poff[gi[q]];
+                seg.push_back({o.T + po, z.d_gT.p + (size_t)q * Ng, Ng});
+                for (int a = 0; a < 3; a++) seg.push_back({o.coeffs + 18 * po + 6 * (size_t)a * Ng, z.d_gC.p + 6 * ((size_t)a * BN + (size_t)q * Ng), 6 * (long long)Ng});
+            }
+            if (int r = copy_segments(c, seg, st)) return r;
+            if (int r = plan_upload(c, z.d_gi, gi, st)) return r;
+            if (p->flags & ISDF_PLAN_CERTIFY) {
+                isdf_certify_params pc = p->certify;
+                pc.clearance.pieces_per_traj = Ng;
+                double rr = r_cert;
+                if (int r = certify_check(c, (int)BN, &pc, &rr)) return r;
+                CU_TRY(z.d_csum.ensure(Bn));
+                if (int r = timed(info.certify_ms, [&] { return certify_run(c, (int)BN, z.d_gT.p, z.d_gC.p, &pc, rr, z.d_csum.p, st); })) return r;
+                k_plan_scatter<CertSummary><<<(unsigned)((Bn + 127) / 128), 128, 0, st>>>(Bn, z.d_gi.p, z.d_csum.p, o.cert);
                 c->stats.kernel_launches++;
                 CU_TRY(cudaGetLastError());
-                c->batch.B = Bp; c->batch.P = BP;
-                return 0;
-            })) return r;
-        info.backend_rounds = brounds;
-        std::vector<double> bf(Bp);
-        std::vector<int> bi((size_t)3 * Bp);
-        CU_TRY(cudaMemcpyAsync(bf.data(), z.d_bf.p, sizeof(double) * Bp, cudaMemcpyDeviceToHost, st));
-        CU_TRY(cudaMemcpyAsync(bi.data(), z.d_bi.p, sizeof(int) * bi.size(), cudaMemcpyDeviceToHost, st));
-        CU_TRY(cudaMemcpyAsync(bres.data(), c->batch.minco.d_T.p, sizeof(double) * BP, cudaMemcpyDeviceToHost, st));
-        CU_TRY(cudaMemcpyAsync(bres.data() + BP, c->batch.minco.d_C.p, sizeof(double) * 18 * BP, cudaMemcpyDeviceToHost, st));
-        CU_TRY(cudaStreamSynchronize(st));
-        for (int k = 0; k < Bp; k++) {
-            isdf_plan_result &r = res[idx[ok[k]]];
-            r.backend_f = bf[k]; r.backend_ret = bi[k]; r.backend_iterations = bi[Bp + k]; r.backend_evaluations = bi[2 * (size_t)Bp + k];
+            }
+            if (p->flags & ISDF_PLAN_DYNAMICS) {
+                isdf_dynamics_params pd = p->dynamics;
+                pd.pieces_per_traj = Ng;
+                if (int r = dynamics_check(c, (int)BN, &pd)) return r;
+                CU_TRY(z.d_dsum.ensure(Bn));
+                if (int r = timed(info.dynamics_ms, [&] { return dynamics_run(c, (int)BN, z.d_gT.p, z.d_gC.p, &pd, z.d_dsum.p, st); })) return r;
+                k_plan_scatter<DynSummary><<<(unsigned)((Bn + 127) / 128), 128, 0, st>>>(Bn, z.d_gi.p, z.d_dsum.p, o.dyn);
+                c->stats.kernel_launches++;
+                CU_TRY(cudaGetLastError());
+            }
         }
     }
-    // the returned trajectories, plan b's at piece_off[b]: the back end's, or the mid-end's for MIDEND_FAILED
-    for (int q = 0; q < Bg; q++) {
-        const bool be = pos[q] >= 0;
-        const int Nq = N[idx[q]];
-        const size_t po = (size_t)poff[idx[q]], p0 = be ? (size_t)boff[pos[q]] : (size_t)moff[q], rows = 6 * (be ? BP : MP);
-        const double *sT = be ? bres.data() : mres.data() + Bg, *sC = sT + (be ? BP : MP);
-        double td = 0.0;
-        for (int i = 0; i < Nq; i++) { T[po + i] = sT[p0 + i]; td += T[po + i]; }
-        res[idx[q]].duration = td;
-        for (int a = 0; a < 3; a++) std::memcpy(coeffs + 18 * po + 6 * (size_t)a * Nq, sC + a * rows + 6 * p0, sizeof(double) * 6 * Nq);
-    }
-    // 7. certificates on every returned trajectory, per group of plans with the same N, ascending
-    if (!(p->flags & (ISDF_PLAN_CERTIFY | ISDF_PLAN_DYNAMICS))) return 0;
-    for (const int Ng : Ns) {
-        std::vector<int> gi;   // the group's plans, in pair order
-        for (const int b : idx) if (N[b] == Ng) gi.push_back(b);
-        const int Bn = (int)gi.size();
-        const size_t BN = (size_t)Bn * Ng;
-        // the group's trajectories as one block (piece q*N + i of a 6BN x 3 column-major block)
-        std::vector<double> gT(BN), gC(18 * BN);
-        for (int q = 0; q < Bn; q++) {
-            const size_t po = (size_t)poff[gi[q]];
-            std::copy(T + po, T + po + Ng, gT.begin() + (size_t)q * Ng);
-            for (int a = 0; a < 3; a++)
-                std::copy(coeffs + 18 * po + 6 * (size_t)a * Ng, coeffs + 18 * po + 6 * ((size_t)a + 1) * Ng, gC.begin() + 6 * ((size_t)a * BN + (size_t)q * Ng));
-        }
-        CU_TRY(z.d_gT.upload(gT.data(), BN, st)); CU_TRY(z.d_gC.upload(gC.data(), 18 * BN, st));
-        if (p->flags & ISDF_PLAN_CERTIFY) {
-            isdf_certify_params pc = p->certify;
-            pc.clearance.pieces_per_traj = Ng;
-            double rr = r_cert;
-            if (int r = certify_check(c, (int)BN, &pc, &rr)) return r;
-            CU_TRY(z.d_csum.ensure(Bn));
-            if (int r = timed(info.certify_ms, [&] { return certify_run(c, (int)BN, z.d_gT.p, z.d_gC.p, &pc, rr, z.d_csum.p, st); })) return r;
-            std::vector<isdf_certify_summary> s(Bn);
-            CU_TRY(cudaMemcpyAsync(s.data(), z.d_csum.p, sizeof(isdf_certify_summary) * Bn, cudaMemcpyDeviceToHost, st));
-            CU_TRY(cudaStreamSynchronize(st));
-            for (int q = 0; q < Bn; q++) certify[gi[q]] = s[q];
-        }
-        if (p->flags & ISDF_PLAN_DYNAMICS) {
-            isdf_dynamics_params pd = p->dynamics;
-            pd.pieces_per_traj = Ng;
-            if (int r = dynamics_check(c, (int)BN, &pd)) return r;
-            CU_TRY(z.d_dsum.ensure(Bn));
-            if (int r = timed(info.dynamics_ms, [&] { return dynamics_run(c, (int)BN, z.d_gT.p, z.d_gC.p, &pd, z.d_dsum.p, st); })) return r;
-            std::vector<isdf_dynamics_summary> s(Bn);
-            CU_TRY(cudaMemcpyAsync(s.data(), z.d_dsum.p, sizeof(isdf_dynamics_summary) * Bn, cudaMemcpyDeviceToHost, st));
-            CU_TRY(cudaStreamSynchronize(st));
-            for (int q = 0; q < Bn; q++) dynamics[gi[q]] = s[q];
-        }
-    }
+    CU_TRY(cudaStreamSynchronize(st));
     return 0;
 }
 
-// the planning calls (starts: sstride 0 for one start)
-static int plan_entry(isdf_ctx *c, int B, const double *starts, int sstride, const double *goals, const isdf_plan_params *p, int max_fields,
+// the host forms' outputs from their staging on st (wrote: plan_run's return; path_off and piece_off also after a failure that left them
+// sized)
+static int plan_copy_back(isdf_ctx *c, const PlanOut &o, bool wrote, int B, int32_t *path_off, double *path_xyz, int32_t *piece_off, double *T,
+                          double *coeffs, isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics, cudaStream_t st) {
+    auto get = [&](void *dst, const void *src, size_t bytes) -> int {
+        if (!bytes) return 0;
+        CU_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st));
+        count_copy(c, cudaMemcpyDeviceToHost, bytes);
+        return 0;
+    };
+    const size_t Bs = (size_t)B;
+    if (o.sized) {
+        if (path_off) if (int r = get(path_off, o.path_off, sizeof(int32_t) * (Bs + 1))) return r;
+        if (int r = get(piece_off, o.piece_off, sizeof(int32_t) * (Bs + 1))) return r;
+    }
+    if (wrote) {
+        if (path_xyz) if (int r = get(path_xyz, o.path_xyz, sizeof(double) * 3 * (size_t)o.nodes)) return r;
+        if (int r = get(T, o.T, sizeof(double) * (size_t)o.pieces)) return r;
+        if (int r = get(coeffs, o.coeffs, sizeof(double) * 18 * (size_t)o.pieces)) return r;
+        if (int r = get(results, o.res, sizeof(isdf_plan_result) * Bs)) return r;
+        if (certify) if (int r = get(certify, o.cert, sizeof(isdf_certify_summary) * Bs)) return r;
+        if (dynamics) if (int r = get(dynamics, o.dyn, sizeof(isdf_dynamics_summary) * Bs)) return r;
+    }
+    CU_TRY(cudaStreamSynchronize(st));
+    return 0;
+}
+
+// the planning calls (starts: sstride 0 for one start, on the host in every form). dev: goals, starts (sstride 3) and every output in
+// device memory, the call on st; else host memory, staged through c->plan on ctx's stream (st). One pipeline, plan_run, for both.
+static int plan_entry(isdf_ctx *c, bool dev, int B, const double *starts, int sstride, const double *goals, const isdf_plan_params *p, int max_fields,
                       int cap_nodes, int32_t *path_off, double *path_xyz, int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
-                      isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics) {
+                      isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics, cudaStream_t st) {
     bool started = false;
     const int rc = poison_on_failure([&]() -> int {
         if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
@@ -3919,34 +4080,93 @@ static int plan_entry(isdf_ctx *c, int B, const double *starts, int sstride, con
         if (int r = plan_check(c, p, &r_cert)) return r;
         if (set_device(c)) return ISDF_ERR_CUDA;
         started = true;
-        return plan_run(c, B, starts, sstride, goals, max_fields, p, r_cert, cap_nodes, path_off, path_xyz, cap_pieces, piece_off, T, coeffs,
-                        results, certify, dynamics);
+        std::fill(c->xfer, c->xfer + 4, 0ll);
+        auto &z = c->plan;
+        PlanOut o;
+        o.want_xyz = path_xyz != nullptr;
+        std::vector<double> hs, hg;
+        if (dev) {   // the starts and goals are read to the host to group them (path_run)
+            hg.resize((size_t)3 * B);
+            CU_TRY(cudaMemcpyAsync(hg.data(), goals, sizeof(double) * hg.size(), cudaMemcpyDeviceToHost, st));
+            count_copy(c, cudaMemcpyDeviceToHost, sizeof(double) * hg.size());
+            if (sstride) {
+                hs.resize((size_t)3 * B);
+                CU_TRY(cudaMemcpyAsync(hs.data(), starts, sizeof(double) * hs.size(), cudaMemcpyDeviceToHost, st));
+                count_copy(c, cudaMemcpyDeviceToHost, sizeof(double) * hs.size());
+                starts = hs.data();
+            }
+            CU_TRY(cudaStreamSynchronize(st));
+            goals = hg.data();
+            o.path_off = path_off; o.path_xyz = path_xyz; o.piece_off = piece_off; o.T = T; o.coeffs = coeffs;
+            o.res = reinterpret_cast<PlanResult *>(results); o.cert = reinterpret_cast<CertSummary *>(certify); o.dyn = reinterpret_cast<DynSummary *>(dynamics);
+        } else {
+            o.staged = true;
+            CU_TRY(z.s_piece_off.ensure((size_t)B + 1)); CU_TRY(z.s_res.ensure(B));
+            o.piece_off = z.s_piece_off.p; o.res = z.s_res.p;
+            if (path_off) { CU_TRY(z.s_path_off.ensure((size_t)B + 1)); o.path_off = z.s_path_off.p; }
+            if (certify) { CU_TRY(z.s_cert.ensure(B)); o.cert = z.s_cert.p; }
+            if (dynamics) { CU_TRY(z.s_dyn.ensure(B)); o.dyn = z.s_dyn.p; }
+        }
+        int r = plan_run(c, B, starts, sstride, goals, max_fields, p, r_cert, cap_nodes, cap_pieces, o, st);
+        if (!dev) {
+            const int rb = plan_copy_back(c, o, r == 0, B, path_off, path_xyz, piece_off, T, coeffs, results, certify, dynamics, st);
+            if (!r) r = rb;
+        }
+        return r;
     }, [&] {
         if (B < 1) return;
-        if (results)
-            for (int b = 0; b < B; b++) {
-                results[b] = {};
-                results[b].stage = ISDF_PLAN_FAILED;
-                results[b].path_cost = results[b].midend_f = results[b].backend_f = results[b].duration = std::numeric_limits<double>::quiet_NaN();
-            }
-        if (certify) write_failed_summaries(certify, B, certify_failed_summary());
-        if (dynamics) write_failed_summaries(dynamics, B, dynamics_failed_summary());
+        isdf_plan_result bad = {};
+        bad.stage = ISDF_PLAN_FAILED;
+        bad.path_cost = bad.midend_f = bad.backend_f = bad.duration = std::numeric_limits<double>::quiet_NaN();
+        isdf_ctx *dc = dev ? c : nullptr;   // device outputs: written after st, best effort
+        if (dev && !c) return;
+        if (results) write_failed_summaries(results, B, bad, dc, st);
+        if (certify) write_failed_summaries(certify, B, certify_failed_summary(), dc, st);
+        if (dynamics) write_failed_summaries(dynamics, B, dynamics_failed_summary(), dc, st);
     });
-    if (started) c->sv.set_points(nullptr, 0, c->stream);   // both point sets given up, the batched swept-volume term off
+    if (started) {
+        c->sv.set_points(nullptr, 0, st);   // both point sets given up, the batched swept-volume term off
+        std::copy(c->xfer, c->xfer + 4, c->plan.xfer);
+    }
     return rc;
 }
 
 extern "C" int isdf_plan_batch(isdf_ctx *c, const double *start, int B, const double *goals, const isdf_plan_params *p, int cap_nodes,
                                int32_t *path_off, double *path_xyz, int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
                                isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics) {
-    return plan_entry(c, B, start, 0, goals, p, 0, cap_nodes, path_off, path_xyz, cap_pieces, piece_off, T, coeffs, results, certify, dynamics);
+    return plan_entry(c, false, B, start, 0, goals, p, 0, cap_nodes, path_off, path_xyz, cap_pieces, piece_off, T, coeffs, results, certify,
+                      dynamics, c ? c->stream : nullptr);
 }
 
 extern "C" int isdf_plan_pairs(isdf_ctx *c, int B, const double *starts, const double *goals, const isdf_plan_params *p, int max_fields,
                                int cap_nodes, int32_t *path_off, double *path_xyz, int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
                                isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics) {
-    return plan_entry(c, B, starts, 3, goals, p, max_fields, cap_nodes, path_off, path_xyz, cap_pieces, piece_off, T, coeffs, results, certify,
-                      dynamics);
+    return plan_entry(c, false, B, starts, 3, goals, p, max_fields, cap_nodes, path_off, path_xyz, cap_pieces, piece_off, T, coeffs, results, certify,
+                      dynamics, c ? c->stream : nullptr);
+}
+
+extern "C" int isdf_plan_batch_device(isdf_ctx *c, const double *start, int B, const double *d_goals, const isdf_plan_params *p, int cap_nodes,
+                                      int32_t *d_path_off, double *d_path_xyz, int cap_pieces, int32_t *d_piece_off, double *d_T, double *d_coeffs,
+                                      isdf_plan_result *d_results, isdf_certify_summary *d_certify, isdf_dynamics_summary *d_dynamics,
+                                      void *cuda_stream) {
+    return plan_entry(c, true, B, start, 0, d_goals, p, 0, cap_nodes, d_path_off, d_path_xyz, cap_pieces, d_piece_off, d_T, d_coeffs, d_results,
+                      d_certify, d_dynamics, (cudaStream_t)cuda_stream);
+}
+
+extern "C" int isdf_plan_pairs_device(isdf_ctx *c, int B, const double *d_starts, const double *d_goals, const isdf_plan_params *p, int max_fields,
+                                      int cap_nodes, int32_t *d_path_off, double *d_path_xyz, int cap_pieces, int32_t *d_piece_off, double *d_T,
+                                      double *d_coeffs, isdf_plan_result *d_results, isdf_certify_summary *d_certify,
+                                      isdf_dynamics_summary *d_dynamics, void *cuda_stream) {
+    return plan_entry(c, true, B, d_starts, 3, d_goals, p, max_fields, cap_nodes, d_path_off, d_path_xyz, cap_pieces, d_piece_off, d_T, d_coeffs,
+                      d_results, d_certify, d_dynamics, (cudaStream_t)cuda_stream);
+}
+
+// what the last planning call moved between host and device, counted at the pipeline's copy sites: out = {device-to-host bytes outside
+// the rounds' 4-byte reads, the rounds' reads, host-to-device bytes, copies (reads included)}
+extern "C" int isdf_dbg_plan_transfers(isdf_ctx *c, int64_t *out) {
+    if (!c || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
+    for (int k = 0; k < 4; k++) out[k] = c->plan.xfer[k];
+    return 0;
 }
 
 // the traversability bits of the last path or field call (X*Y*ceil(Z/32) words of the map it ran on, grid.bits' layout)

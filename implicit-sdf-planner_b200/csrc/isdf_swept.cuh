@@ -919,11 +919,12 @@ struct SweptState {
         }
         return e;
     }
-    // the persisted durations of problems 0 .. nB-1 of the batched term (dur: nB host values)
-    cudaError_t set_durations(int nB, const double *dur, cudaStream_t st) {
+    // the persisted durations of problems 0 .. nB-1 of the batched term (dur: nB values on the host, or on the device with
+    // kind = cudaMemcpyDeviceToDevice)
+    cudaError_t set_durations(int nB, const double *dur, cudaStream_t st, cudaMemcpyKind kind = cudaMemcpyHostToDevice) {
         cudaError_t e;
         if ((e = grow_state_b(nB, st)) != cudaSuccess) return e;
-        if ((e = cudaMemcpy2DAsync(d_state_b.p, 4 * sizeof(double), dur, sizeof(double), sizeof(double), nB, cudaMemcpyHostToDevice, st)) != cudaSuccess) return e;
+        if ((e = cudaMemcpy2DAsync(d_state_b.p, 4 * sizeof(double), dur, sizeof(double), sizeof(double), nB, kind, st)) != cudaSuccess) return e;
         return cudaStreamSynchronize(st);
     }
     cudaError_t launch_batch(const DevCfg &cfg, const DevShape &shape, int N, const int *d_poff, size_t nP, const double *d_T, const double *d_Cpp,

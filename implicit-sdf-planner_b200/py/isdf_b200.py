@@ -44,7 +44,8 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_lbfgs_batch_ragged_device", "isdf_midend_callback_batch_ragged", "isdf_midend_batch_ragged",
                "isdf_midend_batch_ragged_device", "isdf_map_esdf", "isdf_get_esdf_f64", "isdf_esdf_query", "isdf_esdf_query_device",
                "isdf_trajectory_states", "isdf_trajectory_states_device", "isdf_pose_points", "isdf_pose_points_device",
-               "isdf_frontend_path_pairs", "isdf_frontend_path_pairs_device", "isdf_frontend_path_fields_device", "isdf_plan_pairs"]
+               "isdf_frontend_path_pairs", "isdf_frontend_path_pairs_device", "isdf_frontend_path_fields_device", "isdf_plan_pairs",
+               "isdf_path_waypoints_device", "isdf_plan_pairs_device", "isdf_plan_batch_device"]
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
 DYN_QUANTITIES = ["speed", "acceleration", "body_rate", "tilt", "thrust"]   # q of isdf_dynamics_summary; mask bit 5: the thrust minimum
@@ -358,6 +359,10 @@ def load_library(path=None):
     lib.isdf_trajectory_states_device.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int64, vp, vp, vp, vp]
     lib.isdf_pose_points.argtypes = [vp, C.c_int64, dp, C.c_int, dp, dp]
     lib.isdf_pose_points_device.argtypes = [vp, C.c_int64, vp, C.c_int, vp, vp, vp]
+    lib.isdf_path_waypoints_device.argtypes = [vp, C.c_int, vp, vp, C.c_double, C.c_double, C.c_int, vp, vp, vp, vp]
+    lib.isdf_plan_pairs_device.argtypes = [vp, C.c_int, vp, vp, C.POINTER(PlanParams), C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp,
+                                           vp, vp]
+    lib.isdf_plan_batch_device.argtypes = [vp, dp, C.c_int, vp, C.POINTER(PlanParams), C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp]
     for s in ABI_SYMBOLS:
         if s != "isdf_last_error":
             getattr(lib, s).restype = C.c_int
@@ -444,6 +449,24 @@ def path_waypoints(paths, res, parlength=3.0):
     if r != 0:
         raise IsdfError(r, lib.isdf_last_error().decode())
     return [wp[wo[b]:wo[b + 1]].copy() for b in range(B)], pieces[:B].copy()
+
+
+def _cuda_f64(t):
+    """a contiguous float64 CUDA tensor (no copy when t already is one)"""
+    import torch
+    if not t.is_cuda:
+        raise ValueError("expected a CUDA tensor")
+    return t.to(torch.float64).contiguous()
+
+
+def decode_plan_results(records):
+    """isdf_plan_result records (B x 64 uint8, as plan_pairs_device returns them; any device) -> dict of per-field tensors of length B"""
+    import torch
+    r = records.reshape(-1, C.sizeof(PlanResult)).contiguous()
+    i32, f64 = r[:, :32].contiguous().view(torch.int32), r[:, 32:].contiguous().view(torch.float64)
+    out = {n: i32[:, k] for k, (n, _) in enumerate(PlanResult._fields_[:8])}
+    out.update({n: f64[:, k] for k, (n, _) in enumerate(PlanResult._fields_[8:])})
+    return out
 
 
 def _dp(a):
@@ -1017,6 +1040,89 @@ class Evaluator:
             d["dynamics"] = ds[b].as_dict() if p.flags & PLAN_DYNAMICS else None
             out.append(d)
         return out, self.plan_info()
+
+    # ---- planning in device memory (include/isdf.h: isdf_plan_pairs_device, isdf_plan_batch_device) ----
+    def plan_pairs_device(self, starts, goals, params=None, max_fields=0, cap_nodes=None, cap_pieces=None, stream=None, **kw):
+        """isdf_plan_pairs_device: starts and goals are (B, 3) float64 CUDA tensors on this context's device -> a dict of CUDA tensors
+        (see _plan_device). Runs on stream (a torch.cuda.Stream; None: torch's current stream) and returns when the outputs are written."""
+        if starts.shape != goals.shape or starts.dim() != 2 or starts.shape[1] != 3:
+            raise ValueError(f"starts and goals must both be (B, 3), got {tuple(starts.shape)} and {tuple(goals.shape)}")
+        sts, gl = _cuda_f64(starts), _cuda_f64(goals)
+        return self._plan_device(lambda p, *a: self.lib.isdf_plan_pairs_device(self.h, gl.shape[0], C.c_void_p(sts.data_ptr()), C.c_void_p(gl.data_ptr()),
+                                                                                p, int(max_fields), *a),
+                                 gl, params, cap_nodes, cap_pieces, stream, kw)
+
+    def plan_batch_device(self, start, goals, params=None, cap_nodes=None, cap_pieces=None, stream=None, **kw):
+        """isdf_plan_batch_device: start (3 values, host), goals a (B, 3) float64 CUDA tensor -> what plan_pairs_device returns"""
+        st = _f64(start).reshape(3)
+        if goals.dim() != 2 or goals.shape[1] != 3:
+            raise ValueError(f"goals must be (B, 3), got {tuple(goals.shape)}")
+        gl = _cuda_f64(goals)
+        return self._plan_device(lambda p, *a: self.lib.isdf_plan_batch_device(self.h, _dp(st), gl.shape[0], C.c_void_p(gl.data_ptr()), p, *a),
+                                 gl, params, cap_nodes, cap_pieces, stream, kw)
+
+    def _plan_device(self, call, gl, params, cap_nodes, cap_pieces, stream, kw):
+        """call(params, cap_nodes, path_off, path_xyz, cap_pieces, piece_off, T, coeffs, results, certify, dynamics, stream) -> dict of
+        CUDA tensors: path_off (B + 1 int32), path_xyz (path_off[B] x 3), piece_off (B + 1 int32), T (piece_off[B]), coeffs
+        (18 piece_off[B]), results (B x 64 uint8 isdf_plan_result records; decode_plan_results), certify / dynamics (B summary records as
+        uint8 rows, None when the flag is off). piece_off, T and coeffs go into trajectory_states_device as they are. Caps as in _plan: too
+        small, the call is repeated once with the sizes the first call reported."""
+        import torch
+        p = params if params is not None else self.plan_params(**kw)
+        B, dev = gl.shape[0], gl.device
+        cap_nodes = self._path_cap(None) * B if cap_nodes is None else int(cap_nodes)
+        cap_pieces = 290 * B if cap_pieces is None else int(cap_pieces)
+        s = torch.cuda.current_stream(dev) if stream is None else stream
+        ptr = lambda t: C.c_void_p(t.data_ptr())
+        for attempt in range(2):
+            with torch.cuda.stream(s):   # the outputs are allocated and filled on the stream the call runs on
+                po, xyz = torch.zeros(B + 1, dtype=torch.int32, device=dev), torch.empty((max(cap_nodes, 1), 3), dtype=torch.float64, device=dev)
+                pf = torch.zeros(B + 1, dtype=torch.int32, device=dev)
+                T, Cc = torch.empty(max(cap_pieces, 1), dtype=torch.float64, device=dev), torch.empty(18 * max(cap_pieces, 1), dtype=torch.float64, device=dev)
+                res = torch.empty((B, C.sizeof(PlanResult)), dtype=torch.uint8, device=dev)
+                cs = torch.empty((B, C.sizeof(CertifySummary)), dtype=torch.uint8, device=dev)
+                ds = torch.empty((B, C.sizeof(DynamicsSummary)), dtype=torch.uint8, device=dev)
+                r = call(C.byref(p), cap_nodes, ptr(pf), ptr(xyz), cap_pieces, ptr(po), ptr(T), ptr(Cc), ptr(res), ptr(cs), ptr(ds), C.c_void_p(s.cuda_stream))
+            if r == -1 and attempt == 0:
+                need_nodes, need_pieces = int(pf[B]), int(po[B])
+                if need_nodes > cap_nodes or need_pieces > cap_pieces:
+                    cap_nodes, cap_pieces = max(cap_nodes, need_nodes), max(cap_pieces, need_pieces)
+                    continue
+            self._check(r)
+            break
+        nodes, pieces = int(pf[B]), int(po[B])
+        return dict(path_off=pf, path_xyz=xyz[:nodes], piece_off=po, T=T[:pieces], coeffs=Cc[:18 * pieces], results=res,
+                    certify=cs if p.flags & PLAN_CERTIFY else None, dynamics=ds if p.flags & PLAN_DYNAMICS else None)
+
+    def plan_pairs_device_raw(self, B, d_starts, d_goals, params, max_fields, cap_nodes, d_path_off, d_path_xyz, cap_pieces, d_piece_off, d_T,
+                              d_coeffs, d_results, d_certify, d_dynamics, stream=0):
+        """isdf_plan_pairs_device on raw device pointers (0 for NULL) -> its return code (not raised). stream: a raw cudaStream_t"""
+        v = C.c_void_p
+        return self.lib.isdf_plan_pairs_device(self.h, int(B), v(d_starts), v(d_goals), C.byref(params), int(max_fields), int(cap_nodes), v(d_path_off),
+                                               v(d_path_xyz), int(cap_pieces), v(d_piece_off), v(d_T), v(d_coeffs), v(d_results), v(d_certify),
+                                               v(d_dynamics), v(stream))
+
+    def plan_batch_device_raw(self, start, B, d_goals, params, cap_nodes, d_path_off, d_path_xyz, cap_pieces, d_piece_off, d_T, d_coeffs,
+                              d_results, d_certify, d_dynamics, stream=0):
+        """isdf_plan_batch_device on raw device pointers (0 for NULL) -> its return code (not raised); start: 3 host values"""
+        v, st = C.c_void_p, _f64(start).reshape(3)
+        return self.lib.isdf_plan_batch_device(self.h, _dp(st), int(B), v(d_goals), C.byref(params), int(cap_nodes), v(d_path_off), v(d_path_xyz),
+                                               int(cap_pieces), v(d_piece_off), v(d_T), v(d_coeffs), v(d_results), v(d_certify), v(d_dynamics),
+                                               v(stream))
+
+    def path_waypoints_device(self, B, d_path_off, d_path_xyz, res, parlength, cap, d_waypoints, d_wp_off, d_pieces, stream=0):
+        """isdf_path_waypoints_device on raw device pointers -> its return code (not raised: cap too small is ISDF_ERR_INVALID with wp_off
+        and pieces written). stream: a raw cudaStream_t"""
+        v = C.c_void_p
+        return self.lib.isdf_path_waypoints_device(self.h, int(B), v(d_path_off), v(d_path_xyz), float(res), float(parlength), int(cap), v(d_waypoints),
+                                                   v(d_wp_off), v(d_pieces), v(stream))
+
+    def dbg_plan_transfers(self):
+        """what the last planning call moved (isdf_dbg_plan_transfers, not part of include/isdf.h)"""
+        out = (C.c_int64 * 4)()
+        self.lib.isdf_dbg_plan_transfers.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
+        self._check(self.lib.isdf_dbg_plan_transfers(self.h, out))
+        return dict(d2h_bytes=out[0], round_reads=out[1], h2d_bytes=out[2], copies=out[3])
 
     # ---- executing a trajectory (include/isdf.h: isdf_trajectory_states, isdf_pose_points) ----
     @staticmethod

@@ -391,6 +391,16 @@ int isdf_lbfgs_batch_ragged_device(isdf_ctx *ctx, int B, const int32_t *piece_of
  * are still written), for res or parlength not finite and positive, or for offsets that do not start at 0 and increase. */
 int isdf_path_waypoints(int B, const int32_t *path_off, const double *path_xyz, double res, double parlength, int cap,
                         double *waypoints, int32_t *wp_off, int32_t *pieces);
+/* the same on the device: d_path_off (B + 1), d_path_xyz, d_waypoints (cap x 3), d_wp_off (B + 1) and d_pieces (B) on ctx's device, the
+ * call on cuda_stream. Every output is byte-equal to isdf_path_waypoints' on the same paths, with the same IEEE operations (one division or
+ * one ceil per step, nothing contracted). One pass counts each path's waypoints, a scan gives wp_off, a second pass writes the rows below
+ * cap. The host reads one 4-byte total and the call returns when the outputs are written. ISDF_ERR_INVALID when the total exceeds cap (with
+ * d_wp_off and d_pieces written, and the rows below cap), for a NULL pointer (d_waypoints may be NULL when cap = 0), B < 1, cap < 0, or
+ * res or parlength not finite and positive. Device data is not checked on the host: offsets that do not start at 0 or do not increase give
+ * a path of fewer than three nodes (N = 1, no waypoint) wherever path_off[b+1] - path_off[b] < 3, and offsets past the nodes of d_path_xyz
+ * are read as they are. Where parlength / res underflows to 0 (the host form does not terminate there) a path gets N = 1. */
+int isdf_path_waypoints_device(isdf_ctx *ctx, int B, const int32_t *d_path_off, const double *d_path_xyz, double res, double parlength,
+                               int cap, double *d_waypoints, int32_t *d_wp_off, int32_t *d_pieces, void *cuda_stream);
 typedef struct isdf_midend_params {
     double weight_pr;        /* weightPR (mid_end.hpp:315; yaml weight_pr 1000); >= 0 */
     double rho;              /* rho_mid_end (yaml 200); finite */
@@ -892,8 +902,8 @@ int isdf_frontend_path_fields_device(isdf_ctx *ctx, int S, const double *starts,
  *   argument checks); isdf_get_batch_trajectories returns every back-end plan's final trajectory in the ragged layout (plans in goal
  *   order), and the swept-volume t* and per-problem durations are whatever the back end left; isdf_stats.kernel_launches counts every launch of the call, the other isdf_stats fields
  *   are whatever the last back-end callback left.
- * Device memory: owned by the context, grown on demand. Between stages only the path lengths, the plans' waypoints, the rounds' 4-byte
- *   reads and the results cross to the host.
+ * Device memory: owned by the context, grown on demand. Between stages only per-plan values and the rounds' 4-byte reads cross to the
+ *   host (see the device forms below); the host form then copies its outputs back.
  * Errors: ISDF_ERR_STATE without a map, a shape or front-end kernels; ISDF_ERR_UNSUPPORTED on a sharded context and for ISDF_PLAN_CERTIFY
  *   with a shape the certificate refuses (checked before any work); ISDF_ERR_INVALID for a NULL argument, B < 1, the stages' own parameter
  *   checks, unknown flags, a non-zero reserved_, pieces_per_traj != 0 in p->certify or p->dynamics, a start or goal outside the map, or
@@ -941,6 +951,26 @@ int isdf_plan_pairs(isdf_ctx *ctx, int B, const double *starts, const double *go
                     int cap_nodes, int32_t *path_off, double *path_xyz,
                     int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
                     isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics);
+/* device forms: isdf_plan_pairs / isdf_plan_batch word for word (stages, durations rule, caps, errors, the poisoning of results and
+ * summaries on failure, the state left behind and isdf_get_plan_info), with d_starts (B x 3) and d_goals (B x 3) and every output in
+ * ctx's device memory in the host form's layout; the start of isdf_plan_batch_device is on the host (3 doubles), as in
+ * isdf_frontend_path_batch_device. d_path_off and d_path_xyz may be NULL as in the host form.
+ * Stream: work queued on cuda_stream before the call is waited for; the call runs on cuda_stream and returns when its outputs are written
+ * (the mid-end's and back end's rounds read 4 bytes each and wait for them). With caps too small, d_path_off and d_piece_off give the sizes
+ * needed and the results and summaries read as failures.
+ * One pipeline: the host forms stage their outputs through the context and copy them back, so they give the same bits as the device forms.
+ * Transfers: besides the starts and goals (read to the host to group them, as isdf_frontend_path_pairs_device does), only per-plan values
+ * cross to the host: the path lengths and found flags, N, the mid-end return codes and the gathered point counts, plus the rounds' 4-byte
+ * reads. Device-to-host bytes outside those reads are at most 80 per plan plus 64 (isdf_plan_batch_device: 56 per plan), whatever the
+ * lengths of the paths and trajectories. Nothing proportional to path nodes, waypoints or pieces crosses in either direction. */
+int isdf_plan_pairs_device(isdf_ctx *ctx, int B, const double *d_starts, const double *d_goals, const isdf_plan_params *p, int max_fields,
+                           int cap_nodes, int32_t *d_path_off, double *d_path_xyz, int cap_pieces, int32_t *d_piece_off, double *d_T,
+                           double *d_coeffs, isdf_plan_result *d_results, isdf_certify_summary *d_certify,
+                           isdf_dynamics_summary *d_dynamics, void *cuda_stream);
+int isdf_plan_batch_device(isdf_ctx *ctx, const double *start, int B, const double *d_goals, const isdf_plan_params *p, int cap_nodes,
+                           int32_t *d_path_off, double *d_path_xyz, int cap_pieces, int32_t *d_piece_off, double *d_T, double *d_coeffs,
+                           isdf_plan_result *d_results, isdf_certify_summary *d_certify, isdf_dynamics_summary *d_dynamics,
+                           void *cuda_stream);
 int isdf_get_plan_info(isdf_ctx *ctx, isdf_plan_info *out);
 
 /* ---- executing a trajectory: getStateOnTrajStamp (swm:307-341) and the playback of SweptVolumeManager::process (swm:948-988) ----
