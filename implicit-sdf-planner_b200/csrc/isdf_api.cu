@@ -37,6 +37,8 @@ __global__ void k_mesh_cells(const __grid_constant__ DevMesh M, int nx, int ny, 
 __global__ void k_mesh_cell_lists(const __grid_constant__ DevMesh M, long long ncell, double hd, double list_reach, double disc_reach, uint16_t *cnt,
                                   const uint32_t *off, uint32_t *cand, float *cand_lb);
 __global__ void k_mesh_cell_pack(long long ncell, const float *dist, const uint32_t *seed, const uint32_t *off, const uint16_t *cnt, uint4 *rec);
+__global__ void k_mesh_disc_lists(const __grid_constant__ DevMesh M, long long ncell, int k, double margin, uint16_t *dcnt, const uint32_t *doff,
+                                  uint32_t *dcand, float *dlb);
 
 static thread_local std::string g_err;
 static int fail(int code, const std::string &msg) { g_err = msg; return code; }
@@ -167,6 +169,10 @@ struct isdf_ctx {
         DevShape shape = {};
         DevBuf<BvhNode> d_nodes; DevBuf<WideNode> d_wnodes; DevBuf<double> d_tris, d_pn, d_obb; DevBuf<float> d_cell_dist; DevBuf<uint32_t> d_cell_seed, d_cell_off, d_cand; DevBuf<float> d_cand_lb; DevBuf<uint16_t> d_cell_cnt; DevBuf<uint4> d_cell_rec; DevBuf<WnNode> d_wn;
         double list_reach = 0;  // radius (cell-centre distance) up to which cells got candidate lists (isdf_dbg_mesh_grid)
+        // the discrete scan's sub-box filtered lists (k_mesh_disc_lists), built when disc_k > 1; launch_discrete hands them to the scan
+        int disc_k = DISC_LIST_K;   // sub-boxes per cell edge (isdf_dbg_disc_k; 1: the scan walks the full lists)
+        bool disc_ready = false;
+        DevBuf<uint32_t> d_disc_off, d_disc_cand; DevBuf<float> d_disc_lb; DevBuf<uint16_t> d_disc_cnt; DevBuf<uint4> d_disc_rec;
     } mesh;
     struct {   // discrete evaluation: scan / epilogue scratch and the work-item schedule
         long long order_for = -1;    // (N, rank, world) signature the work items are valid for
@@ -480,7 +486,7 @@ extern "C" int isdf_set_shape_mesh_ex(isdf_ctx *c, const double *V, int nV, cons
     if (!build_host_mesh(V, nV, F, nF, poly_params, c->cfg.safety_hor, hm, err, sign_mode))
         return fail(err.find("not a closed") != std::string::npos ? ISDF_ERR_UNSUPPORTED : ISDF_ERR_INVALID, err);
     // the uploads may reallocate the buffers the current shape lives in: give it up (and what was built on it) first
-    c->mesh.have_shape = false; c->fe.ready = false;
+    c->mesh.have_shape = false; c->fe.ready = false; c->mesh.disc_ready = false;
     c->disc.order_for = -1;
     if (!hm.wn.empty()) CU_TRY(c->mesh.d_wn.upload(hm.wn.data(), hm.wn.size(), c->stream));
     CU_TRY(c->mesh.d_nodes.upload(hm.nodes.data(), hm.nodes.size(), c->stream));
@@ -540,6 +546,37 @@ extern "C" int isdf_set_shape_mesh_ex(isdf_ctx *c, const double *V, int nV, cons
             CU_TRY(cudaGetLastError());
             CU_TRY(cudaStreamSynchronize(c->stream));
             m.cell_off = c->mesh.d_cell_off.p; m.cell_cnt = c->mesh.d_cell_cnt.p; m.cand = c->mesh.d_cand.p; m.cand_lb = c->mesh.d_cand_lb.p;
+            if (c->mesh.disc_k > 1) {
+                // the discrete scan's sub-box filtered lists, counted, then written into their own arrays. margin covers the scan
+                // finding p's cell with floor() in a unit with FMA contraction: p may lie outside its cell by a few ulps of its coordinate
+                double scale = 1.0;
+                for (int a = 0; a < 3; a++) scale = std::max(scale, std::max(std::fabs(m.glo[a]), std::fabs(m.glo[a] + m.gdim[a] * m.gcell)));
+                const double margin = 1e-9 * scale + 1e-12;
+                CU_TRY(c->mesh.d_disc_cnt.ensure(ncell)); CU_TRY(c->mesh.d_disc_off.ensure(ncell));
+                k_mesh_disc_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, c->mesh.disc_k, margin, c->mesh.d_disc_cnt.p, nullptr, nullptr, nullptr);
+                c->stats.kernel_launches++;
+                CU_TRY(cudaGetLastError());
+                std::vector<uint16_t> dcnt(ncell);
+                CU_TRY(cudaMemcpyAsync(dcnt.data(), c->mesh.d_disc_cnt.p, sizeof(uint16_t) * ncell, cudaMemcpyDeviceToHost, c->stream));
+                CU_TRY(cudaStreamSynchronize(c->stream));
+                size_t dtotal = 0;
+                for (size_t i = 0; i < ncell; i++) { off[i] = (uint32_t)dtotal; dtotal += dcnt[i]; }
+                CU_TRY(c->mesh.d_disc_cand.ensure(dtotal)); CU_TRY(c->mesh.d_disc_lb.ensure(dtotal));
+                CU_TRY(cudaMemcpyAsync(c->mesh.d_disc_off.p, off.data(), sizeof(uint32_t) * ncell, cudaMemcpyHostToDevice, c->stream));
+                k_mesh_disc_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, c->mesh.disc_k, margin, c->mesh.d_disc_cnt.p,
+                                                                     c->mesh.d_disc_off.p, c->mesh.d_disc_cand.p, c->mesh.d_disc_lb.p);
+                c->stats.kernel_launches++;
+                CU_TRY(cudaGetLastError());
+                CU_TRY(c->mesh.d_disc_rec.ensure(ncell));
+                k_mesh_cell_pack<<<(unsigned)((ncell + 255) / 256), 256, 0, c->stream>>>((long long)ncell, m.cell_dist, m.cell_seed, c->mesh.d_disc_off.p,
+                                                                                         c->mesh.d_disc_cnt.p, c->mesh.d_disc_rec.p);
+                c->stats.kernel_launches++;
+                CU_TRY(cudaGetLastError());
+                CU_TRY(cudaStreamSynchronize(c->stream));
+                c->mesh.disc_ready = true;
+                if (getenv("ISDF_VERBOSE"))
+                    fprintf(stderr, "[isdf] discrete-scan lists (%d^3 sub-boxes per cell): %zu candidates (%.1f MB)\n", c->mesh.disc_k, dtotal, dtotal * 8e-6);
+            }
         }
         if (getenv("ISDF_VERBOSE")) {
             size_t listed = 0, nlong = 0, long_total = 0;
@@ -641,6 +678,79 @@ __global__ void __launch_bounds__(128) k_mesh_cell_lists(const __grid_constant__
         // lower bound of the exact distance: relative and absolute slack for the rounding of the FP64 closest-point test, then rounded
         // down to float (monotone in di, so the bounds are non-decreasing along the list)
         cand_lb[base + rank] = __double2float_rd(fmax(sqrt(di) * (1.0 - 1e-9) - 1e-12, 0.0));
+    }
+}
+
+// The discrete scan's lists (one warp per cell): the rule of k_mesh_cell_lists applied on k^3 sub-boxes of the cell. A sub-box with
+// centre y and half diagonal delta (half edge gcell / 2k + margin) keeps triangle T of the cell's list when d(y, T) <= dmin(y) + 2 delta,
+// dmin(y) the smallest distance from y over the list. For p in that sub-box and T* nearest to p, d(y, T*) <= d(p, T*) + delta <=
+// d(p, T_y) + delta <= dmin(y) + 2 delta: every triangle nearest to some point of the sub-box is kept, exact ties included, and the
+// 1e-9 relative + 1e-12 slack covers the FP64 rounding of both distances. The kept triangles are written in list order with their
+// cand_lb, and the first entry (nearest to the centre, the scan's upper-bound seed) is always kept. Pass 1 (dcand == nullptr) stores
+// the counts; lists of at most DISC_FILTER_MIN candidates are copied whole (they take one pass either way).
+__global__ void __launch_bounds__(128) k_mesh_disc_lists(const __grid_constant__ DevMesh M, long long ncell, int k, double margin, uint16_t *dcnt,
+                                                         const uint32_t *doff, uint32_t *dcand, float *dlb) {
+    constexpr int CH = MESH_LIST_CAP_DISCRETE / 32;   // list candidates per lane
+    const int lane = threadIdx.x & 31;
+    const long long cell = (long long)blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (cell >= ncell) return;
+    const int n = (int)M.cell_cnt[cell];
+    const uint32_t off = M.cell_off[cell];
+    uint32_t keep = 0;   // bit j: candidate j * 32 + lane
+    if (n <= DISC_FILTER_MIN) {
+        if (lane < n) keep = 1u;
+    } else {
+        const int nz = M.gdim[2], ny = M.gdim[1];
+        const int iz = (int)(cell % nz), iy = (int)((cell / nz) % ny), ix = (int)(cell / ((long long)nz * ny));
+        const d3 ctr = mk3(M.glo[0] + (ix + 0.5) * M.gcell, M.glo[1] + (iy + 0.5) * M.gcell, M.glo[2] + (iz + 0.5) * M.gcell);
+        const double two_delta = 2.0 * sqrt(3.0) * (0.5 * M.gcell / k + margin);
+        int ids[CH];
+#pragma unroll
+        for (int j = 0; j < CH; j++) ids[j] = (j * 32 + lane < n) ? (int)M.cand[off + j * 32 + lane] : -1;
+#pragma unroll 1
+        for (int s = 0; s < k * k * k; s++) {
+            const int sx = s / (k * k), sy = (s / k) % k, sz = s % k;
+            const d3 y = mk3(ctr.x + ((sx + 0.5) / k - 0.5) * M.gcell, ctr.y + ((sy + 0.5) / k - 0.5) * M.gcell, ctr.z + ((sz + 0.5) / k - 0.5) * M.gcell);
+            double d[CH];
+            double mn = 1e300;
+#pragma unroll
+            for (int j = 0; j < CH; j++) {
+                d[j] = 1e300;
+                if (j * 32 < n && ids[j] >= 0) {
+                    int f;
+                    const d3 q = tri_closest_rec(y, M.tris + TRI_STRIDE * (size_t)ids[j], f);
+                    const d3 e = y - q;
+                    d[j] = sqrt(dot3(e, e));
+                    mn = fmin(mn, d[j]);
+                }
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) mn = fmin(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+            const double lim = (mn + two_delta) * (1.0 + 1e-9) + 1e-12;
+#pragma unroll
+            for (int j = 0; j < CH; j++)
+                if (d[j] <= lim) keep |= 1u << j;
+        }
+        if (lane == 0) keep |= 1u;
+    }
+    if (dcand == nullptr) {
+        int total = __popc(keep);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
+        if (lane == 0) dcnt[cell] = (uint16_t)total;
+        return;
+    }
+    const unsigned lt_mask = (1u << lane) - 1u;
+    uint32_t pos = doff[cell];
+    for (int j = 0; j * 32 < n; j++) {
+        const bool kept = (keep >> j) & 1u;
+        const unsigned bal = __ballot_sync(0xffffffffu, kept);
+        if (kept) {
+            const uint32_t o = pos + __popc(bal & lt_mask);
+            dcand[o] = M.cand[off + j * 32 + lane];
+            dlb[o] = M.cand_lb[off + j * 32 + lane];
+        }
+        pos += __popc(bal);
     }
 }
 
@@ -1540,6 +1650,11 @@ static int launch_discrete(isdf_ctx *c, int N, const double *d_T, const double *
     CU_TRY(c->disc.d_tot.ensure((size_t)S * 8));
     DiscArgs A;
     A.cfg = c->dcfg; A.grid = c->map.grid; A.shape = c->mesh.shape; A.N = N; A.T = d_T; A.C = d_C;
+    if (c->mesh.shape.kind == ISDF_SHAPE_MESH && c->mesh.disc_ready) {   // the scan walks the sub-box filtered lists (DevMesh's two contracts)
+        DevMesh &dm = A.shape.mesh;
+        dm.cell_off = c->mesh.d_disc_off.p; dm.cell_cnt = c->mesh.d_disc_cnt.p; dm.cand = c->mesh.d_disc_cand.p; dm.cand_lb = c->mesh.d_disc_lb.p;
+        dm.cell_rec = c->mesh.d_disc_rec.p;
+    }
     A.tot = c->disc.d_tot.p; A.pieces_done = c->disc.d_tickets.p; A.item_cursor = c->disc.d_tickets.p + 1;
     A.piece_cost = c->disc.d_piece_cost.p; A.out = d_out; A.pair_counter = c->disc.d_counter.p; A.count_out = count_out;
     A.rank = c->rank; A.world = c->world;
@@ -4404,6 +4519,35 @@ extern "C" int isdf_dbg_mesh_lists(isdf_ctx *c, long long *sizes, uint32_t *cell
     if (cand && total) CU_TRY(cudaMemcpy(cand, m.cand, sizeof(uint32_t) * total, cudaMemcpyDeviceToHost));
     if (cand_lb && total) CU_TRY(cudaMemcpy(cand_lb, m.cand_lb, sizeof(float) * total, cudaMemcpyDeviceToHost));
     if (tris) CU_TRY(cudaMemcpy(tris, m.tris, sizeof(double) * TRI_STRIDE * (size_t)m.ntris, cudaMemcpyDeviceToHost));
+    return 0;
+}
+// sub-boxes per cell edge of the discrete scan's filtered lists, from the next isdf_set_shape_mesh on (1: the scan walks the full lists)
+extern "C" int isdf_dbg_disc_k(isdf_ctx *c, int k) {
+    if (!c || k < 1 || k > 8) return fail(ISDF_ERR_INVALID, "NULL context or k outside 1..8");
+    c->mesh.disc_k = k;
+    return 0;
+}
+// the discrete scan's filtered lists, so tests can hold them to the full ones: sizes = {candidates (0: not built, the scan walks the
+// full lists), k}; cell_off / cell_cnt (one per cell, as isdf_dbg_mesh_grid) and cand / cand_lb (sizes[0] each) are optional
+extern "C" int isdf_dbg_disc_lists(isdf_ctx *c, long long *sizes, uint32_t *cell_off, uint16_t *cell_cnt, uint32_t *cand, float *cand_lb) {
+    if (!c || !sizes) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (!c->mesh.have_shape || c->mesh.shape.kind != ISDF_SHAPE_MESH) return fail(ISDF_ERR_STATE, "no mesh shape set");
+    const DevMesh &m = c->mesh.shape.mesh;
+    const size_t ncell = (size_t)m.gdim[0] * m.gdim[1] * m.gdim[2];
+    if (int r = sync_ctx(c)) return r;
+    size_t total = 0;
+    if (c->mesh.disc_ready) {
+        uint32_t off_last = 0; uint16_t cnt_last = 0;
+        CU_TRY(cudaMemcpy(&off_last, c->mesh.d_disc_off.p + ncell - 1, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+        CU_TRY(cudaMemcpy(&cnt_last, c->mesh.d_disc_cnt.p + ncell - 1, sizeof(uint16_t), cudaMemcpyDeviceToHost));
+        total = (size_t)off_last + cnt_last;
+    }
+    sizes[0] = (long long)total; sizes[1] = c->mesh.disc_k;
+    if (!c->mesh.disc_ready) return 0;
+    if (cell_off) CU_TRY(cudaMemcpy(cell_off, c->mesh.d_disc_off.p, sizeof(uint32_t) * ncell, cudaMemcpyDeviceToHost));
+    if (cell_cnt) CU_TRY(cudaMemcpy(cell_cnt, c->mesh.d_disc_cnt.p, sizeof(uint16_t) * ncell, cudaMemcpyDeviceToHost));
+    if (cand && total) CU_TRY(cudaMemcpy(cand, c->mesh.d_disc_cand.p, sizeof(uint32_t) * total, cudaMemcpyDeviceToHost));
+    if (cand_lb && total) CU_TRY(cudaMemcpy(cand_lb, c->mesh.d_disc_lb.p, sizeof(float) * total, cudaMemcpyDeviceToHost));
     return 0;
 }
 // the swept-volume term of the last batched callback, B x (19 N0 + 1): per problem [cost | gradC 18 N0 | gradT N0], as the callback adds it

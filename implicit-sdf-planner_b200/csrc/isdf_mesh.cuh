@@ -47,6 +47,10 @@ enum { MESH_SIGN_PSEUDONORMAL = 0, MESH_SIGN_WINDING = 1 };
 constexpr int MESH_LIST_CAP = 160;
 constexpr int MESH_LIST_CAP_DISCRETE = 512;
 __host__ __device__ inline int mesh_list_cnt(int cnt) { return cnt <= MESH_LIST_CAP ? cnt : 0; }
+// The discrete scan walks sub-box filtered copies of the lists (k_mesh_disc_lists): DISC_LIST_K^3 sub-boxes per cell, lists of at most
+// DISC_FILTER_MIN candidates (one pass) copied unfiltered.
+constexpr int DISC_LIST_K = 4;
+constexpr int DISC_FILTER_MIN = 32;
 
 struct DevMesh {
     const BvhNode *nodes;   // nodes[0] is the root (a single-leaf mesh still gets one node with right = left)
@@ -76,6 +80,11 @@ struct DevMesh {
     // discrete scan kernel's cull stage fetches it with ONE 128-bit load and hands offset / count / seed to the search, instead
     // of three dependent loads per query (packed by k_mesh_cell_pack at isdf_set_shape_mesh time; may be null)
     const uint4 *cell_rec;
+    // Two list contracts. The view every search uses holds in cell_off / cell_cnt / cand / cand_lb / cell_rec the full lists above.
+    // The discrete scan's copy of this view (launch_discrete) holds in the same five fields the sub-box filtered lists
+    // (k_mesh_disc_lists): each an ordered subsequence of the cell's full list, with the same first entry and the same cand_lb values,
+    // that keeps every triangle that can be nearest (exactly tied ones included) to some point the scan assigns to the cell. The
+    // scan's pass returns the earliest exact minimum in list order, so both lists give it the same triangle, point and feature.
     double inv_gcell;           // 1 / gcell
     int ntris;
     int gdim[3];

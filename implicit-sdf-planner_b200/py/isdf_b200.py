@@ -1704,6 +1704,27 @@ class Evaluator:
         tris = np.stack([a, a + rec[:, 3:6], a + rec[:, 6:9]], axis=1)
         return dict(cell_off=off, cand=cand, cand_lb=lb, tris=tris)
 
+    def dbg_disc_k(self, k):
+        """sub-boxes per cell edge of the discrete scan's filtered lists, from the next set_shape_mesh on (1: the full lists)"""
+        self._check(self.lib.isdf_dbg_disc_k(self.h, int(k)))
+
+    def dbg_disc_lists(self):
+        """the discrete scan's filtered lists, copied to the host: dict(k, cell_off, cell_cnt (shaped as dbg_mesh_grid's arrays),
+        cand (uint32), cand_lb (float32)); None when none were built (the scan walks the full lists)"""
+        vp, llp = C.c_void_p, C.POINTER(C.c_longlong)
+        u32p, u16p, fp = C.POINTER(C.c_uint32), C.POINTER(C.c_uint16), C.POINTER(C.c_float)
+        self.lib.isdf_dbg_disc_lists.argtypes = [vp, llp, u32p, u16p, u32p, fp]
+        sizes = np.zeros(2, dtype=np.int64)
+        self._check(self.lib.isdf_dbg_disc_lists(self.h, sizes.ctypes.data_as(llp), None, None, None, None))
+        if sizes[0] == 0:
+            return None
+        gdim = self.dbg_mesh_grid(arrays=False)["gdim"]
+        off, cnt = np.zeros(gdim, dtype=np.uint32), np.zeros(gdim, dtype=np.uint16)
+        cand, lb = np.zeros(int(sizes[0]), dtype=np.uint32), np.zeros(int(sizes[0]), dtype=np.float32)
+        self._check(self.lib.isdf_dbg_disc_lists(self.h, sizes.ctypes.data_as(llp), off.ctypes.data_as(u32p), cnt.ctypes.data_as(u16p),
+                                                 cand.ctypes.data_as(u32p), lb.ctypes.data_as(fp)))
+        return dict(k=int(sizes[1]), cell_off=off, cell_cnt=cnt, cand=cand, cand_lb=lb)
+
     def dbg_flatness(self, v, a, j, quat_grad, omg_grad, vel_grad):
         """device flatness map + adjoint as compiled into the epilogue kernel -> (quat, omg, gV, gA, gJ)"""
         vaj = np.ascontiguousarray(np.concatenate([_f64(v).reshape(-1, 3), _f64(a).reshape(-1, 3), _f64(j).reshape(-1, 3)], axis=1))
