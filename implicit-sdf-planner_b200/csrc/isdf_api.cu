@@ -17,6 +17,7 @@
 #include "isdf_esdf.cuh"
 #include "isdf_states.cuh"
 #include "isdf_plan.cuh"
+#include "isdf_sim.cuh"
 #include <cub/device/device_scan.cuh>
 #include <queue>
 #include "isdf_host_mesh.cuh"
@@ -1244,6 +1245,133 @@ extern "C" int isdf_pose_points_device(isdf_ctx *c, int64_t Q, const double *d_s
     pose_launch(c, Q, d_states, P, d_body, d_out, (cudaStream_t)cuda_stream);
     CU_TRY(cudaGetLastError());
     return 0;
+}
+
+// ---- closed loop (isdf_sim.cuh, compiled in isdf_sim_tu.cu) ----
+extern "C" int isdf_sim_default_params(isdf_sim_params *p) {
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    std::memset(p, 0, sizeof(*p));
+    p->mass = 0.98; p->grav = 9.81; p->J[0] = 2.64e-3; p->J[1] = 2.64e-3; p->J[2] = 4.96e-3;   // Quadrotor::Quadrotor()
+    p->kf = 8.98132e-9; p->km = 0.07 * (3 * 0.062) * p->kf; p->arm = 0.26; p->motor_tau = 1.0 / 30; p->min_rpm = 1200; p->max_rpm = 35000;
+    p->ctrl_mass = 0.98; p->ctrl_grav = 9.81;                                                  // simulator_example.launch "mass"; SO3Control()
+    const double kx[3] = {5.7, 5.7, 6.2}, kv[3] = {3.4, 3.4, 4.0}, kR[3] = {1.0, 1.0, 1.0}, kOm[3] = {0.07, 0.07, 0.1};
+    for (int i = 0; i < 3; i++) { p->kx[i] = kx[i]; p->kv[i] = kv[i]; p->kR[i] = kR[i]; p->kOm[i] = kOm[i]; p->corrections[i] = 0.0; }
+    p->sim_rate = 1000; p->cmd_rate = 100; p->t_end = 10; p->diverge_dist = 5;
+    p->log_every = 1; p->use_external_yaw = 1; p->floor = 1;
+    return 0;
+}
+
+// validated parameters -> ticks, steps per tick and log records per rollout
+static int sim_params_check(const isdf_sim_params *p, int *n_ticks, int *m, int *n_log) {
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    const double *d = &p->mass;
+    for (size_t i = 0; i < offsetof(isdf_sim_params, log_every) / sizeof(double); i++)
+        if (!std::isfinite(d[i])) return fail(ISDF_ERR_INVALID, "a simulation parameter is not finite");
+    if (!(p->mass > 0 && p->J[0] > 0 && p->J[1] > 0 && p->J[2] > 0 && p->kf > 0 && p->km > 0 && p->arm > 0 && p->motor_tau > 0 && p->ctrl_mass > 0))
+        return fail(ISDF_ERR_INVALID, "mass, J, kf, km, arm, motor_tau and ctrl_mass must be positive");
+    if (!(p->min_rpm >= 0 && p->max_rpm >= p->min_rpm)) return fail(ISDF_ERR_INVALID, "rpm limits must satisfy 0 <= min_rpm <= max_rpm");
+    if (!(p->sim_rate > 0 && p->cmd_rate > 0)) return fail(ISDF_ERR_INVALID, "sim_rate and cmd_rate must be positive");
+    const double ratio = p->sim_rate / p->cmd_rate;
+    if (std::fmod(p->sim_rate, p->cmd_rate) != 0 || ratio < 1 || ratio > 1e6) return fail(ISDF_ERR_INVALID, "sim_rate must be a whole multiple of cmd_rate");
+    if (!(p->t_end >= 0) || p->t_end * p->cmd_rate >= 2147483646.0) return fail(ISDF_ERR_INVALID, "t_end must be >= 0 with fewer than 2^31 ticks");
+    if (p->log_every < 1) return fail(ISDF_ERR_INVALID, "log_every must be >= 1");
+    if (!(p->diverge_dist > 0)) return fail(ISDF_ERR_INVALID, "diverge_dist must be positive");
+    if (p->reserved_ != 0) return fail(ISDF_ERR_INVALID, "reserved_ must be 0");
+    *m = (int)ratio;
+    *n_ticks = (int)std::floor(p->t_end * p->cmd_rate) + 1;
+    *n_log = (*n_ticks - 1) / p->log_every + 1;
+    return 0;
+}
+
+static int sim_args_check(isdf_ctx *c, int B, const void *off, const void *T, const void *C, int R, const void *traj, const void *init,
+                          const isdf_sim_params *p, int cap_log, const void *log, const void *summary, int *n_ticks, int *m) {
+    if (!c || !off || !T || !C || !traj || !init || !summary) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (B < 1) return fail(ISDF_ERR_INVALID, "B < 1");
+    if (R < 0) return fail(ISDF_ERR_INVALID, "R < 0");
+    int n_log = 0;
+    if (int rc = sim_params_check(p, n_ticks, m, &n_log)) return rc;
+    if (log && cap_log < n_log) return fail(ISDF_ERR_INVALID, "cap_log is smaller than the log records per rollout");
+    if (log && (long long)R * cap_log > (1ll << 40)) return fail(ISDF_ERR_INVALID, "log too large");
+    return 0;
+}
+
+static int sim_launch(isdf_ctx *c, int B, const int *d_off, const double *d_T, const double *d_C, int R, const int *d_traj, const double *d_init,
+                      const double *d_dist, const isdf_sim_params *p, int n_ticks, int m, int cap_log, double *d_log, isdf_sim_summary *d_sum,
+                      cudaStream_t st) {
+    SimArgs A;
+    A.p = *p; A.B = B; A.R = R; A.n_ticks = n_ticks; A.m = m; A.cap_log = cap_log;
+    A.off = d_off; A.traj = d_traj; A.T = d_T; A.C = d_C; A.init = d_init; A.dist = d_dist; A.log = d_log; A.summary = d_sum;
+    CU_TRY(simulate_launch(A, st));
+    c->stats.kernel_launches++;
+    return 0;
+}
+
+static void sim_poison_host(isdf_sim_summary *s, int R) {
+    if (!s || R < 1) return;
+    const double nan = std::numeric_limits<double>::quiet_NaN();
+    for (int r = 0; r < R; r++) {
+        s[r].max_err = s[r].t_max_err = s[r].rms_err = s[r].final_err = s[r].max_tilt = s[r].max_omega = s[r].t_diverged = nan;
+        s[r].accepted = s[r].rejected = -1;
+        s[r].clamped_steps = s[r].floor_contacts = s[r].nan_rollbacks = -1;
+        s[r].diverged = 1;
+    }
+}
+
+extern "C" int isdf_simulate(isdf_ctx *c, int B, const int32_t *piece_off, const double *T, const double *coeffs, int R, const int32_t *traj,
+                             const double *init, const double *dist, const isdf_sim_params *p, int cap_log, double *log, isdf_sim_summary *summary) {
+    return poison_on_failure([&]() -> int {
+        int n_ticks = 0, m = 0;
+        if (int rc = sim_args_check(c, B, piece_off, T, coeffs, R, traj, init, p, cap_log, log, summary, &n_ticks, &m)) return rc;
+        if (piece_off[0] != 0) return fail(ISDF_ERR_INVALID, "piece_off[0] must be 0");
+        for (int b = 0; b < B; b++) if (piece_off[b + 1] < piece_off[b]) return fail(ISDF_ERR_INVALID, "piece_off must not decrease");
+        const int P = piece_off[B];
+        if (P > 0) if (int rc = swept_traj_check(P, T, coeffs)) return rc;
+        for (int r = 0; r < R; r++)
+            if (traj[r] < 0 || traj[r] >= B || piece_off[traj[r] + 1] == piece_off[traj[r]])
+                return fail(ISDF_ERR_INVALID, "traj[r] outside [0, B) or naming a trajectory without pieces");
+        if (R == 0) return 0;
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        // one device block: in = [coeffs 18P | T P | init 17R | dist 6R | piece_off, traj (int32)], out = [summaries | log]
+        const size_t nC = (size_t)19 * P, nI = (size_t)ISDF_SIM_INIT_DOUBLES * R, nD = dist ? (size_t)6 * R : 0;
+        const size_t nin = nC + nI + nD + ((size_t)B + 1 + (size_t)R + 1) / 2;
+        const size_t nsum = ((size_t)R * sizeof(isdf_sim_summary) + 7) / 8, nlog = log ? (size_t)R * cap_log * ISDF_SIM_DOUBLES : 0;
+        auto &x = c->exec;
+        CU_TRY(x.h.ensure(std::max(nin, nsum + nlog))); CU_TRY(x.d_in.ensure(nin)); CU_TRY(x.d_out.ensure(nsum + nlog));
+        double *h = x.h.p;
+        std::memcpy(h, coeffs, sizeof(double) * 18 * (size_t)P);
+        std::memcpy(h + 18 * (size_t)P, T, sizeof(double) * P);
+        std::memcpy(h + nC, init, sizeof(double) * nI);
+        if (dist) std::memcpy(h + nC + nI, dist, sizeof(double) * nD);
+        int32_t *hi = reinterpret_cast<int32_t *>(h + nC + nI + nD);
+        std::memcpy(hi, piece_off, sizeof(int32_t) * ((size_t)B + 1));
+        std::memcpy(hi + B + 1, traj, sizeof(int32_t) * R);
+        CU_TRY(cudaMemcpyAsync(x.d_in.p, h, sizeof(double) * nin, cudaMemcpyHostToDevice, c->stream));
+        const double *d = x.d_in.p;
+        const int *di = reinterpret_cast<const int *>(d + nC + nI + nD);
+        isdf_sim_summary *d_sum = reinterpret_cast<isdf_sim_summary *>(x.d_out.p);
+        if (int rc = sim_launch(c, B, di, d + 18 * (size_t)P, d, R, di + B + 1, d + nC, dist ? d + nC + nI : nullptr, p, n_ticks, m, cap_log,
+                                log ? x.d_out.p + nsum : nullptr, d_sum, c->stream)) return rc;
+        CU_TRY(cudaMemcpyAsync(h, x.d_out.p, sizeof(double) * (nsum + nlog), cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaStreamSynchronize(c->stream));
+        std::memcpy(summary, h, sizeof(isdf_sim_summary) * R);
+        if (log) std::memcpy(log, h + nsum, sizeof(double) * nlog);
+        return 0;
+    }, [&]() { sim_poison_host(summary, R); });
+}
+
+extern "C" int isdf_simulate_device(isdf_ctx *c, int B, const int32_t *d_piece_off, const double *d_T, const double *d_coeffs, int R,
+                                    const int32_t *d_traj, const double *d_init, const double *d_dist, const isdf_sim_params *p, int cap_log,
+                                    double *d_log, isdf_sim_summary *d_summary, void *cuda_stream) {
+    const cudaStream_t st = (cudaStream_t)cuda_stream;
+    return poison_on_failure([&]() -> int {
+        int n_ticks = 0, m = 0;
+        if (int rc = sim_args_check(c, B, d_piece_off, d_T, d_coeffs, R, d_traj, d_init, p, cap_log, d_log, d_summary, &n_ticks, &m)) return rc;
+        if (R == 0) return 0;
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        return sim_launch(c, B, d_piece_off, d_T, d_coeffs, R, d_traj, d_init, d_dist, p, n_ticks, m, cap_log, d_log, d_summary, st);
+    }, [&]() {
+        if (c && d_summary && R > 0 && set_device(c) == 0 && sim_poison_launch(d_summary, R, st) == cudaSuccess) c->stats.kernel_launches++;
+    });
 }
 
 // getPointsInAABB (pcs:148-170): one CTA; thread = (x, y) row of the clamped index box — popcount of the row's z-run, block-wide exclusive scan
@@ -2559,6 +2687,85 @@ extern "C" int isdf_trajectory_clearance(isdf_ctx *c, int N, const double *T, co
         CU_TRY(cudaStreamSynchronize(c->stream));
         return 0;
     }, [&] { write_failed_summaries(summary, p ? traj_batch(N, p->pieces_per_traj) : 0, clearance_failed_summary()); });
+}
+
+// ---- clearance at caller-given poses (the pose source of k_clearance_scan) ----
+extern "C" int isdf_pose_clearance_default_params(isdf_pose_clearance_params *p) {
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    isdf_config d;
+    isdf_default_config(&d);
+    p->reach = d.safety_hor; p->margin = d.safety_hor; p->poses_per_group = 0; p->reserved_ = 0;
+    return 0;
+}
+
+static int pose_groups(int64_t Q, int G) { return (Q < 1 || G < 0) ? 0 : G == 0 ? 1 : (Q % G == 0 ? (int)(Q / G) : 0); }
+
+static int pose_clearance_check(isdf_ctx *c, int64_t Q, const void *pos, const void *quat, int64_t stride, const isdf_pose_clearance_params *p) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (!p || !pos || !quat) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (Q < 1 || Q > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "Q must be in [1, 2^31)");
+    if (stride < 1) return fail(ISDF_ERR_INVALID, "stride_doubles < 1");
+    if (!(p->reach > 0.0) || !std::isfinite(p->reach)) return fail(ISDF_ERR_INVALID, "reach must be positive and finite");
+    if (std::isnan(p->margin) || p->margin > p->reach) return fail(ISDF_ERR_INVALID, "margin must not exceed reach");
+    if (pose_groups(Q, p->poses_per_group) == 0) return fail(ISDF_ERR_INVALID, "poses_per_group must be 0 or divide Q");
+    if (p->reserved_ != 0) return fail(ISDF_ERR_INVALID, "reserved_ must be 0");
+    if (c->world > 1) return fail(ISDF_ERR_UNSUPPORTED, "the clearance check is not sharded: call it on a context with isdf_set_shard(ctx, 0, 1)");
+    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
+    if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
+    const double H = c->dcfg.half_bd + p->reach;
+    if (2.0 * H * std::sqrt(3.0) / c->map.grid.res + 4.0 > (double)WINDOW_AXIS_MAX)
+        return fail(ISDF_ERR_INVALID, "reach too large for this map resolution: a pose window would exceed 1023 voxels per axis");
+    return 0;
+}
+
+extern "C" int isdf_pose_clearance_device(isdf_ctx *c, int64_t Q, const double *d_pos, const double *d_quat, int64_t stride,
+                                          const isdf_pose_clearance_params *p, double *d_clear, int64_t *d_voxel, isdf_clearance_summary *d_summary,
+                                          void *cuda_stream) {
+    const cudaStream_t st = (cudaStream_t)cuda_stream;
+    return poison_on_failure([&]() -> int {
+        if (int r = pose_clearance_check(c, Q, d_pos, d_quat, stride, p)) return r;
+        if (!d_clear || !d_voxel || !d_summary) return fail(ISDF_ERR_INVALID, "NULL device pointer");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        ClrArgs A = {};
+        A.grid = c->map.grid; A.shape = c->mesh.shape; A.fp = c->dcfg.fp; A.half_bd = c->dcfg.half_bd;
+        A.reach = p->reach; A.margin = p->margin;
+        A.N = (int)Q; A.K = 0; A.N0 = p->poses_per_group == 0 ? (int)Q : p->poses_per_group;   // one "sample" per pose
+        A.ppos = d_pos; A.pquat = d_quat; A.pstride = stride;
+        A.clear = d_clear; A.voxel = (long long *)d_voxel; A.summary = (ClrSummary *)d_summary;
+        CU_TRY(c->clr.d_cursor.ensure(1)); CU_TRY(c->clr.d_counters.ensure(2));
+        CU_TRY(cudaMemsetAsync(c->clr.d_cursor.p, 0, sizeof(int), st));
+        CU_TRY(cudaMemsetAsync(c->clr.d_counters.p, 0, 2 * sizeof(unsigned long long), st));
+        A.cursor = c->clr.d_cursor.p; A.counters = c->clr.d_counters.p;
+        CU_TRY(clearance_launch(A, clearance_mode(c), clearance_grid(c, Q), st));
+        c->stats.kernel_launches += 2;   // scan kernel, summary kernel
+        return 0;
+    }, [&] { if (c) write_failed_summaries(d_summary, p ? pose_groups(Q, p->poses_per_group) : 0, clearance_failed_summary(), c, st); });
+}
+
+extern "C" int isdf_pose_clearance(isdf_ctx *c, int64_t Q, const double *pos, const double *quat, int64_t stride, const isdf_pose_clearance_params *p,
+                                   double *clear, int64_t *voxel, isdf_clearance_summary *summary) {
+    return poison_on_failure([&]() -> int {
+        if (int r = pose_clearance_check(c, Q, pos, quat, stride, p)) return r;
+        if (!summary) return fail(ISDF_ERR_INVALID, "NULL argument");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        const int B = pose_groups(Q, p->poses_per_group);
+        // the poses packed 7 doubles apart (x, y, z, w, qx, qy, qz) in one copy, then the device form
+        std::vector<double> h((size_t)Q * 7);
+        for (int64_t q = 0; q < Q; q++) {
+            for (int k = 0; k < 3; k++) h[7 * q + k] = pos[q * stride + k];
+            for (int k = 0; k < 4; k++) h[7 * q + 3 + k] = quat[q * stride + k];
+        }
+        CU_TRY(c->clr.d_in.ensure(h.size()));
+        CU_TRY(cudaMemcpyAsync(c->clr.d_in.p, h.data(), sizeof(double) * h.size(), cudaMemcpyHostToDevice, c->stream));
+        CU_TRY(c->clr.d_clear.ensure((size_t)Q)); CU_TRY(c->clr.d_vox.ensure((size_t)Q)); CU_TRY(c->clr.d_sum.ensure((size_t)B));
+        if (int r = isdf_pose_clearance_device(c, Q, c->clr.d_in.p, c->clr.d_in.p + 3, 7, p, c->clr.d_clear.p, (int64_t *)c->clr.d_vox.p,
+                                               (isdf_clearance_summary *)c->clr.d_sum.p, c->stream)) return r;
+        CU_TRY(cudaMemcpyAsync(summary, c->clr.d_sum.p, sizeof(isdf_clearance_summary) * B, cudaMemcpyDeviceToHost, c->stream));
+        if (clear) CU_TRY(cudaMemcpyAsync(clear, c->clr.d_clear.p, sizeof(double) * Q, cudaMemcpyDeviceToHost, c->stream));
+        if (voxel) CU_TRY(cudaMemcpyAsync(voxel, c->clr.d_vox.p, sizeof(int64_t) * Q, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaStreamSynchronize(c->stream));
+        return 0;
+    }, [&] { write_failed_summaries(summary, p ? pose_groups(Q, p->poses_per_group) : 0, clearance_failed_summary()); });
 }
 
 // ---- continuous clearance certificate (isdf_certify.cuh) --------------------------------------------------------------------------

@@ -24,6 +24,9 @@
 //     hierarchical winding number), as the discrete path does in that mode.
 //   * sample lists: with ClrArgs::st set, the same kernel scans caller-given (piece, local time) samples — the refinement rounds of
 //     the certificate (isdf_certify.cuh). The uniform path and its outputs are unchanged.
+//   * caller poses: with ClrArgs::ppos set, sample s is the pose (ppos + s pstride, pquat + s pstride): position and quaternion (w, x, y,
+//     z), R = quat_rot (isdf_pose_clearance). K = 0 and N = the pose count, so a group of N0 poses takes a trajectory's place; the summary
+//     reports pose indexes where a trajectory reports times. Box, window, culls, search and witness rule are the uniform path's.
 //   * k_clearance_summary — one CTA per trajectory: min / first attaining sample / first hit / count over its samples. Only minima and
 //     integer counts are reduced, so the result does not depend on scheduling, and a trajectory's summary is the same bits whether it is
 //     checked alone or inside a batch.
@@ -68,6 +71,9 @@ struct ClrArgs {
     const double *st;
     int nlist;
     int *hit;
+    // caller poses (isdf_pose_clearance): when ppos is set, sample s is posed at ppos + s pstride (x, y, z) and pquat + s pstride (w, x, y, z)
+    const double *ppos, *pquat;
+    long long pstride;
 };
 
 // key order of the running best: (value, address); address -1 = "no witness" (a candidate that only equals reach never wins)
@@ -107,20 +113,29 @@ __global__ void __launch_bounds__(CLR_THREADS) k_clearance_scan(const __grid_con
         if (lane == 0) s = atomicAdd(A.cursor, 1);
         s = __shfl_sync(0xffffffffu, s, 0);
         if (s >= S) break;
-        const int i = A.st ? __ldg(A.sp + s) : s / (K + 1);
         Window W;
         bool empty, finite;
         {   // pose (every lane computes the same values; lane 0 publishes them) and the world window of the rotated H box
-            double cx[6], cy[6], cz[6];
+            rot3 R;
+            d3 pos;
+            if (A.ppos) {   // caller poses
+                const double *pp = A.ppos + (size_t)s * A.pstride, *pq = A.pquat + (size_t)s * A.pstride;
+                quat4 q; q.w = __ldg(pq); q.x = __ldg(pq + 1); q.y = __ldg(pq + 2); q.z = __ldg(pq + 3);
+                R = quat_rot(q);
+                pos = mk3(__ldg(pp), __ldg(pp + 1), __ldg(pp + 2));
+            } else {
+                const int i = A.st ? __ldg(A.sp + s) : s / (K + 1);
+                double cx[6], cy[6], cz[6];
 #pragma unroll
-            for (int k = 0; k < 6; k++) { cx[k] = __ldg(A.C + 6 * i + k); cy[k] = __ldg(A.C + 6 * A.N + 6 * i + k); cz[k] = __ldg(A.C + 12 * A.N + 6 * i + k); }
-            // uniform samples: t = j * step, step = T_i * (1 / K_c), exactly as the definition states
-            const double t = A.st ? __ldg(A.st + s) : (s - i * (K + 1)) * (__ldg(A.T + i) * (1.0 / K));
-            PieceEval pe;
-            piece_eval(cx, cy, cz, t, pe);
-            const quat4 q = flat_quat_only(A.fp, pe.vel, pe.acc);
-            const rot3 R = quat_rot(q);
-            const d3 pos = pe.pos;
+                for (int k = 0; k < 6; k++) { cx[k] = __ldg(A.C + 6 * i + k); cy[k] = __ldg(A.C + 6 * A.N + 6 * i + k); cz[k] = __ldg(A.C + 12 * A.N + 6 * i + k); }
+                // uniform samples: t = j * step, step = T_i * (1 / K_c), exactly as the definition states
+                const double t = A.st ? __ldg(A.st + s) : (s - i * (K + 1)) * (__ldg(A.T + i) * (1.0 / K));
+                PieceEval pe;
+                piece_eval(cx, cy, cz, t, pe);
+                const quat4 q = flat_quat_only(A.fp, pe.vel, pe.acc);
+                R = quat_rot(q);
+                pos = pe.pos;
+            }
             if (lane == 0) {
                 double *ps = sm.pose;
                 ps[0] = pos.x; ps[1] = pos.y; ps[2] = pos.z;
@@ -260,6 +275,7 @@ __global__ void __launch_bounds__(CLR_SUM_THREADS) k_clearance_summary(const __g
     if (threadIdx.x != 0) return;
     // trajectory time of local sample k: T of the earlier pieces of the trajectory added in ascending order, plus j * step
     auto traj_time = [&](int k) {
+        if (A.ppos) return (double)k;   // caller poses: the pose index within the group
         const int p = k / (K + 1), j = k - p * (K + 1);
         double t = 0.0;
         for (int q = 0; q < p; q++) t += A.T[b * N0 + q];

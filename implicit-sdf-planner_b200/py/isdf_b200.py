@@ -45,7 +45,9 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_midend_batch_ragged_device", "isdf_map_esdf", "isdf_get_esdf_f64", "isdf_esdf_query", "isdf_esdf_query_device",
                "isdf_trajectory_states", "isdf_trajectory_states_device", "isdf_pose_points", "isdf_pose_points_device",
                "isdf_frontend_path_pairs", "isdf_frontend_path_pairs_device", "isdf_frontend_path_fields_device", "isdf_plan_pairs",
-               "isdf_path_waypoints_device", "isdf_plan_pairs_device", "isdf_plan_batch_device"]
+               "isdf_path_waypoints_device", "isdf_plan_pairs_device", "isdf_plan_batch_device",
+               "isdf_sim_default_params", "isdf_simulate", "isdf_simulate_device",
+               "isdf_pose_clearance_default_params", "isdf_pose_clearance", "isdf_pose_clearance_device"]
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
 DYN_QUANTITIES = ["speed", "acceleration", "body_rate", "tilt", "thrust"]   # q of isdf_dynamics_summary; mask bit 5: the thrust minimum
@@ -53,6 +55,75 @@ PLAN_CERTIFY, PLAN_DYNAMICS = 1, 2                                             #
 PLAN_FAILED, NO_PATH, TOO_LONG, MIDEND_FAILED, OPTIMISED = -1, 0, 1, 2, 3      # isdf_plan_result.stage
 ESDF_FIELDS = dict(positive=0, negative=1, signed=2)                            # isdf_esdf_field
 STATE_DOUBLES = 20                                                               # ISDF_STATE_DOUBLES: pos vel acc jer quat(w,x,y,z) omg thr
+SIM_INIT_DOUBLES, SIM_DOUBLES = 17, 21   # ISDF_SIM_INIT_DOUBLES: pos vel quat(w,x,y,z) omega rpm; ISDF_SIM_DOUBLES: t pos vel quat omega rpm cmd_pos
+
+
+class SimParams(C.Structure):
+    """isdf_sim_params"""
+    _fields_ = [("mass", C.c_double), ("grav", C.c_double), ("J", C.c_double * 3), ("kf", C.c_double), ("km", C.c_double),
+                ("arm", C.c_double), ("motor_tau", C.c_double), ("min_rpm", C.c_double), ("max_rpm", C.c_double),
+                ("ctrl_mass", C.c_double), ("ctrl_grav", C.c_double)] + \
+               [(n, C.c_double * 3) for n in ["kx", "kv", "kR", "kOm", "corrections"]] + \
+               [(n, C.c_double) for n in ["sim_rate", "cmd_rate", "t_end", "diverge_dist"]] + \
+               [(n, C.c_int32) for n in ["log_every", "use_external_yaw", "floor", "reserved_"]]
+
+
+class SimSummary(C.Structure):
+    """isdf_sim_summary"""
+    _fields_ = [(n, C.c_double) for n in ["max_err", "t_max_err", "rms_err", "final_err", "max_tilt", "max_omega", "t_diverged"]] + \
+               [(n, C.c_int64) for n in ["accepted", "rejected"]] + \
+               [(n, C.c_int32) for n in ["clamped_steps", "floor_contacts", "nan_rollbacks", "diverged"]]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+def decode_sim_summaries(raw):
+    """(R, 88) uint8 rows (a numpy array or a tensor) of isdf_sim_summary records -> list of dicts"""
+    b = np.ascontiguousarray(raw.cpu().numpy() if hasattr(raw, "cpu") else raw, dtype=np.uint8).reshape(-1, C.sizeof(SimSummary))
+    return [SimSummary.from_buffer_copy(row.tobytes()).as_dict() for row in b]
+
+
+def sim_default_params(**kw):
+    p = SimParams()
+    r = load_library().isdf_sim_default_params(C.byref(p))
+    if r != 0:
+        raise IsdfError(r, "isdf_sim_default_params")
+    for k, v in kw.items():
+        if not hasattr(p, k):
+            raise AttributeError(k)
+        if isinstance(v, (list, tuple, np.ndarray)):
+            arr = getattr(p, k)
+            for i, e in enumerate(v):
+                arr[i] = float(e)
+        else:
+            setattr(p, k, type(getattr(p, k))(v))
+    return p
+
+
+def sim_log_records(p):
+    """n_log: the log records per rollout under params p (isdf.h: (n_ticks - 1) / log_every + 1)"""
+    n_ticks = int(np.floor(p.t_end * p.cmd_rate)) + 1
+    return (n_ticks - 1) // max(p.log_every, 1) + 1
+
+
+def sim_init_from_trajectories(piece_off, coeffs, traj, params=None, rpm=None):
+    """the initial states (R, 17) of rollouts that fly trajectories traj: each trajectory's start position, zero velocity, level attitude
+    and, by default, the hover rpm sqrt(m g / (4 kf)) of params' vehicle. This departs from the reference simulator, which starts its
+    motors at 0 rpm (and at the launch file's init_state); pass rpm=0 for that start."""
+    p = params if params is not None else sim_default_params()
+    off = np.asarray(piece_off.cpu() if hasattr(piece_off, "cpu") else piece_off).astype(np.int64)
+    Cc = np.asarray(coeffs.cpu() if hasattr(coeffs, "cpu") else coeffs, dtype=np.float64).reshape(-1)
+    tr = np.asarray(traj.cpu() if hasattr(traj, "cpu") else traj).astype(np.int64).reshape(-1)
+    hover = np.sqrt(p.mass * p.grav / (4 * p.kf)) if rpm is None else float(rpm)
+    out = np.zeros((tr.size, SIM_INIT_DOUBLES))
+    for r, b in enumerate(tr):
+        p0, n = off[b], off[b + 1] - off[b]
+        blk = Cc[18 * p0:18 * (p0 + n)]
+        out[r, 0:3] = [blk[0], blk[6 * n], blk[12 * n]]   # the constant coefficient of piece 0 per axis (6N x 3 column-major)
+        out[r, 6] = 1.0
+        out[r, 13:17] = hover
+    return out
 
 
 class KernelConfig(C.Structure):
@@ -88,6 +159,11 @@ class MidendParams(C.Structure):
 class ClearanceParams(C.Structure):
     """isdf_clearance_params"""
     _fields_ = [("samples_per_piece", C.c_int32), ("pieces_per_traj", C.c_int32), ("reach", C.c_double), ("margin", C.c_double)]
+
+
+class PoseClearanceParams(C.Structure):
+    """isdf_pose_clearance_params"""
+    _fields_ = [("reach", C.c_double), ("margin", C.c_double), ("poses_per_group", C.c_int32), ("reserved_", C.c_int32)]
 
 
 class ClearanceSummary(C.Structure):
@@ -363,6 +439,14 @@ def load_library(path=None):
     lib.isdf_plan_pairs_device.argtypes = [vp, C.c_int, vp, vp, C.POINTER(PlanParams), C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp,
                                            vp, vp]
     lib.isdf_plan_batch_device.argtypes = [vp, dp, C.c_int, vp, C.POINTER(PlanParams), C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp]
+    pcp = C.POINTER(PoseClearanceParams)
+    lib.isdf_pose_clearance_default_params.argtypes = [pcp]
+    lib.isdf_pose_clearance.argtypes = [vp, C.c_int64, dp, dp, C.c_int64, pcp, dp, C.POINTER(C.c_int64), C.POINTER(ClearanceSummary)]
+    lib.isdf_pose_clearance_device.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, pcp, vp, vp, vp, vp]
+    spp = C.POINTER(SimParams)
+    lib.isdf_sim_default_params.argtypes = [spp]
+    lib.isdf_simulate.argtypes = [vp, C.c_int, ip, dp, dp, C.c_int, ip, dp, dp, spp, C.c_int, dp, C.POINTER(SimSummary)]
+    lib.isdf_simulate_device.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, spp, C.c_int, vp, vp, vp]
     for s in ABI_SYMBOLS:
         if s != "isdf_last_error":
             getattr(lib, s).restype = C.c_int
@@ -1174,6 +1258,68 @@ class Evaluator:
         self._check(self.lib.isdf_pose_points_device(self.h, int(Q), C.c_void_p(d_states), int(P), C.c_void_p(d_body), C.c_void_p(d_out),
                                                      C.c_void_p(stream)))
 
+    # ---- closed loop (include/isdf.h: isdf_simulate, isdf_simulate_device) ----
+    @staticmethod
+    def sim_params(**kw):
+        return sim_default_params(**kw)
+
+    def simulate(self, plans_or_ragged, traj, init, dist=None, params=None, cap_log=None):
+        """fly rollouts r = 0..R-1 along trajectory traj[r] from init (R, 17) under the constant force / moment dist (R, 6) ->
+        (log (R, n_log, 21), list of R summary dicts)"""
+        if isinstance(plans_or_ragged, tuple):
+            off, T, Cc = plans_or_ragged
+            off, T, Cc = np.ascontiguousarray(off, dtype=np.int32).reshape(-1), _f64(T).reshape(-1), _f64(Cc).reshape(-1)
+        else:
+            off, T, Cc = self.pack_plans(plans_or_ragged)
+        p = params if params is not None else sim_default_params()
+        tr = np.ascontiguousarray(traj, dtype=np.int32).reshape(-1)
+        ini = _f64(init).reshape(-1, SIM_INIT_DOUBLES)
+        ds = None if dist is None else _f64(dist).reshape(-1, 6)
+        if ini.shape[0] != tr.size or (ds is not None and ds.shape[0] != tr.size):
+            raise ValueError("traj, init and dist must have one row per rollout")
+        n_log = sim_log_records(p)
+        cap = n_log if cap_log is None else int(cap_log)
+        log = np.empty((tr.size, max(cap, 0), SIM_DOUBLES))
+        summ = (SimSummary * max(tr.size, 1))()
+        ip = C.POINTER(C.c_int32)
+        self._check(self.lib.isdf_simulate(self.h, off.size - 1, off.ctypes.data_as(ip), _dp(T), _dp(Cc), tr.size, tr.ctypes.data_as(ip), _dp(ini),
+                                           _dp(ds), C.byref(p), cap, _dp(log), summ))
+        return log, [summ[r].as_dict() for r in range(tr.size)]
+
+    def simulate_device(self, piece_off, T, coeffs, traj, init, dist=None, params=None, log=True, stream=None):
+        """isdf_simulate_device on CUDA tensors: piece_off (B + 1 int32), T, coeffs (as plan_pairs_device returns them), traj (R int32),
+        init (R, 17) and dist (R, 6) float64 -> dict(log (R, n_log, 21) CUDA tensor or None, summary (R, 88) uint8 CUDA tensor; decode with
+        decode_sim_summaries). Runs on stream (None: torch's current stream), not waited for."""
+        import torch
+        p = params if params is not None else sim_default_params()
+        for name, t in (("piece_off", piece_off), ("T", T), ("coeffs", coeffs), ("traj", traj), ("init", init), ("dist", dist)):
+            if t is not None and not (isinstance(t, torch.Tensor) and t.is_cuda and t.device == init.device):
+                raise ValueError(f"{name} must be a CUDA tensor on init's device")
+        if piece_off.dtype != torch.int32 or traj.dtype != torch.int32 or piece_off.dim() != 1 or piece_off.numel() < 2:
+            raise ValueError("piece_off (B + 1, at least 2) and traj must be int32 CUDA tensors")
+        dev = init.device
+        tr = traj.contiguous().reshape(-1)
+        ini, ds = _cuda_f64(init), (None if dist is None else _cuda_f64(dist))
+        R, n_log = tr.numel(), sim_log_records(p)
+        if tuple(ini.shape) != (R, SIM_INIT_DOUBLES) or (ds is not None and tuple(ds.shape) != (R, 6)):
+            raise ValueError(f"init must be ({R}, {SIM_INIT_DOUBLES}) and dist ({R}, 6), got {tuple(ini.shape)} and "
+                             f"{None if ds is None else tuple(ds.shape)}")
+        T, coeffs, piece_off = _cuda_f64(T), _cuda_f64(coeffs), piece_off.contiguous()
+        s = torch.cuda.current_stream(dev) if stream is None else stream
+        with torch.cuda.stream(s):
+            lg = torch.empty((R, n_log, SIM_DOUBLES), dtype=torch.float64, device=dev) if log else None
+            sm = torch.empty((max(R, 1), C.sizeof(SimSummary)), dtype=torch.uint8, device=dev)
+        v = lambda t: C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
+        self._check(self.lib.isdf_simulate_device(self.h, piece_off.numel() - 1, v(piece_off), v(T), v(coeffs), R, v(tr), v(ini), v(ds), C.byref(p),
+                                                  n_log if log else 0, v(lg), v(sm), C.c_void_p(s.cuda_stream)))
+        return dict(log=lg, summary=sm[:R])
+
+    def simulate_device_raw(self, B, d_piece_off, d_T, d_coeffs, R, d_traj, d_init, d_dist, params, cap_log, d_log, d_summary, stream=0):
+        """isdf_simulate_device on raw device pointers (0 for NULL) -> its return code (not raised)"""
+        v = C.c_void_p
+        return self.lib.isdf_simulate_device(self.h, int(B), v(d_piece_off), v(d_T), v(d_coeffs), int(R), v(d_traj), v(d_init), v(d_dist),
+                                             C.byref(params), int(cap_log), v(d_log), v(d_summary), v(stream))
+
     def plan_info(self):
         info = PlanInfo()
         self._check(self.lib.isdf_get_plan_info(self.h, C.byref(info)))
@@ -1212,6 +1358,42 @@ class Evaluator:
         """raw device pointers (e.g. torch .data_ptr()); d_summary holds N/N0 isdf_clearance_summary records (48 bytes each)"""
         self._check(self.lib.isdf_trajectory_clearance_device(self.h, N, C.c_void_p(d_T), C.c_void_p(d_coeffs), C.byref(params), C.c_void_p(d_clear),
                                                               C.c_void_p(d_voxel), C.c_void_p(d_summary), C.c_void_p(stream)))
+
+    def pose_clearance_params(self, reach=None, margin=None, poses_per_group=0):
+        p = PoseClearanceParams()
+        self._check(self.lib.isdf_pose_clearance_default_params(C.byref(p)))
+        if reach is not None:
+            p.reach = float(reach)
+            p.margin = float(reach) if margin is None else p.margin
+        if margin is not None:
+            p.margin = float(margin)
+        p.poses_per_group = int(poses_per_group)
+        return p
+
+    def pose_clearance(self, records, pos_offset=0, quat_offset=3, reach=None, margin=None, poses_per_group=0):
+        """clearance of the robot at Q poses read in place from records (Q, stride) float64: position at pos_offset, quaternion (w, x, y, z)
+        at quat_offset -> (clear (Q,), witness voxels (Q,) int64, one summary dict per group). For isdf_simulate's log use (R * n_log, 21)
+        with offsets 1 and 7; for trajectory_states' records (Q, 20) with offsets 0 and 12. Rows with a NaN pose (a log's unused records)
+        report NaN and count as colliding, so pass only the rows that exist."""
+        r = _f64(records)
+        r = r.reshape(-1, r.shape[-1])
+        Q, stride = r.shape
+        if not (0 <= pos_offset <= stride - 3 and 0 <= quat_offset <= stride - 4):
+            raise ValueError("pos_offset / quat_offset outside the record")
+        p = self.pose_clearance_params(reach, margin, poses_per_group)
+        G = 1 if poses_per_group == 0 else Q // max(int(poses_per_group), 1)
+        clear, vox = np.zeros(Q), np.zeros(Q, dtype=np.int64)
+        summ = (ClearanceSummary * max(G, 1))()
+        base = r.ctypes.data
+        self._check(self.lib.isdf_pose_clearance(self.h, Q, C.cast(base + 8 * pos_offset, C.POINTER(C.c_double)), C.cast(base + 8 * quat_offset, C.POINTER(C.c_double)), stride, C.byref(p),
+                                                 _dp(clear), vox.ctypes.data_as(C.POINTER(C.c_int64)), summ))
+        return clear, vox, [s.as_dict() for s in summ]
+
+    def pose_clearance_device(self, Q, d_pos, d_quat, stride_doubles, params, d_clear, d_voxel, d_summary, stream=0):
+        """raw device pointers: pose q at d_pos + q stride and d_quat + q stride (doubles); d_summary holds Q / poses_per_group records (48 bytes)"""
+        v = C.c_void_p
+        self._check(self.lib.isdf_pose_clearance_device(self.h, int(Q), v(d_pos), v(d_quat), int(stride_doubles), C.byref(params), v(d_clear),
+                                                        v(d_voxel), v(d_summary), v(stream)))
 
     def dbg_clearance_counts(self):
         """{candidate pairs, exact mesh searches} of the last clearance check (isdf_dbg_clearance_counts, not part of include/isdf.h)"""

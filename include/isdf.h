@@ -491,6 +491,34 @@ int isdf_trajectory_clearance_device(isdf_ctx *ctx, int N, const double *d_T, co
                                      double *d_sample_clearance, int64_t *d_sample_voxel, isdf_clearance_summary *d_summary,
                                      void *cuda_stream);
 
+/* ---- clearance at caller-given poses: the clearance check's definition over Q poses instead of trajectory samples ----
+ * Pose q is the position at pos + q * stride_doubles (x, y, z) and the quaternion at quat + q * stride_doubles (w, x, y, z; R = quat_rot as
+ * isdf_pose_points), so records are read in place: isdf_simulate's log (pos = log + 1, quat = log + 7, stride ISDF_SIM_DOUBLES) or
+ * isdf_trajectory_states' records (pos = states, quat = states + 12, stride ISDF_STATE_DOUBLES). Each pose gets what the clearance check
+ * gives a sample: the same H box, reach cap, witness rule, mesh branch and bound and sign mode, with the same bits for the same pose, and
+ * NaN for a non-finite pose. Poses g * poses_per_group .. + poses_per_group - 1 form group g (0: one group of all Q poses), summarised as a
+ * trajectory with the pose index in place of (piece, sample): piece_min = the index within the group of the first pose attaining the
+ * minimum, sample_min = 0, t_min = that index as a double, first_hit = the index of the first pose with clear < margin (-1 if none).
+ * Results are bit-identical run to run, through either entry point, and for a group checked alone or inside a batch.
+ * Errors: ISDF_ERR_INVALID for a NULL argument, Q < 1 or Q >= 2^31, stride_doubles < 1, reach <= 0 or not finite, margin > reach,
+ * poses_per_group < 0 or not dividing Q, a non-zero reserved_ and a window wider than 1023 voxels per axis; ISDF_ERR_STATE without a map or a
+ * shape; ISDF_ERR_UNSUPPORTED on a sharded context. On failure every summary has min_clearance NaN and collision_free 0. The call counts its
+ * launches in isdf_stats.kernel_launches. The host form stages the poses through the device form; the device form is enqueued on
+ * cuda_stream and not waited for. */
+typedef struct isdf_pose_clearance_params {
+    double reach, margin;      /* as isdf_clearance_params */
+    int32_t poses_per_group;   /* 0 = one group of Q poses; else Q % poses_per_group == 0 */
+    int32_t reserved_;
+} isdf_pose_clearance_params;
+/* reach = margin = safety_hor of the default config, poses_per_group 0 */
+int isdf_pose_clearance_default_params(isdf_pose_clearance_params *p);
+/* host buffers; clear / voxel (Q each) may be NULL; summary: Q / poses_per_group entries (1 for 0) */
+int isdf_pose_clearance(isdf_ctx *ctx, int64_t Q, const double *pos, const double *quat, int64_t stride_doubles,
+                        const isdf_pose_clearance_params *p, double *clear, int64_t *voxel, isdf_clearance_summary *summary);
+int isdf_pose_clearance_device(isdf_ctx *ctx, int64_t Q, const double *d_pos, const double *d_quat, int64_t stride_doubles,
+                               const isdf_pose_clearance_params *p, double *d_clear, int64_t *d_voxel, isdf_clearance_summary *d_summary,
+                               void *cuda_stream);
+
 /* ---- continuous clearance certificate: is a trajectory clear at EVERY time, not only at its samples? ---------------------------
  * The clearance check above is sampled; this call closes the gaps between the samples with a proven motion bound.
  * Definition. Inputs and parameters are the clearance check's (T, coeffs, K_c, N0, reach, margin) with 0 <= margin < reach. One verdict
@@ -1011,6 +1039,83 @@ int isdf_trajectory_states_device(isdf_ctx *ctx, int B, const int32_t *d_piece_o
 int isdf_pose_points(isdf_ctx *ctx, int64_t Q, const double *states, int P, const double *body, double *out);
 int isdf_pose_points_device(isdf_ctx *ctx, int64_t Q, const double *d_states, int P, const double *d_body, double *d_out,
                             void *cuda_stream);
+
+/* ---- closed loop: flying a trajectory with the reference's SO(3) controller and quadrotor model (src/uav_simulator) ----
+ * R rollouts, each one vehicle tracking trajectory traj[r] of B trajectories in isdf_plan_batch's ragged layout (the d_piece_off, d_T,
+ * d_coeffs that isdf_plan_pairs_device writes). Rollout r starts from init[r] (ISDF_SIM_INIT_DOUBLES = 17: pos[3] vel[3] quat[4]
+ * (w, x, y, z) omega[3] rpm[4]; R(0) = quat_rot(quat) as isdf_pose_points) and feels the constant external force and moment dist[r]
+ * (6 doubles: f[3] m[3]; Quadrotor::setExternalForce / setExternalMoment; dist may be NULL for zero). The caller draws any randomness.
+ * Definition (one thread per rollout; nothing depends on other rollouts):
+ *   Model: Quadrotor::operator() and step() (Quadrotor.cpp) on the 22-double state x v R(column-major) omega rpm. The right-hand side
+ *     re-orthonormalises R as R L^-1, L the Cholesky factor of R^T R (Eigen's LLT and 3x3 cofactor inverse); thrust kf sum rpm^2;
+ *     moments kf (rpm2^2 - rpm3^2) arm, kf (rpm1^2 - rpm0^2) arm, km (rpm0^2 + rpm1^2 - rpm2^2 - rpm3^2); drag 0.1 pi arm^2 |v|^2 along
+ *     v/|v| (pi as the reference's 3.14159265); v' = -g e3 + thrust R e3 / m + f / m - drag v^ / m; R' = R [omega]x;
+ *     omega' = J^-1 (moments - omega x J omega + m_ext); rpm' = (input - rpm) / motor_tau; NaN derivatives become 0. The last v' evaluated
+ *     is the IMU's acceleration (Quadrotor::getAcc).
+ *   Step (Quadrotor::step(dt), dt = 1 / sim_rate): odeint::integrate(sys, x, 0, dt, dt), i.e. integrate_adaptive with
+ *     controlled_runge_kutta<runge_kutta_dopri5>: the Dormand-Prince 5(4) pair with first-same-as-last, the derivative at the start evaluated
+ *     afresh each step; error max_i |err_i| / (1e-6 + 1e-6 (|x_i| + dt_try |x'_i|)) (NaN terms skipped by the max); err > 1: reject and
+ *     dt_try *= max(0.9 err^(-1/3), 0.2); err < 0.5: accept and dt_try *= 0.9 max(err, 5^-5)^(-1/5); otherwise accept; a try that would pass
+ *     the end is clipped to land on it. a step whose 1000th try is reached ends the rollout as diverged (odeint throws there, accepted or not), as do a
+ *     try that makes no progress (t + h == t) and 100000 tries in one step (bounds odeint does not have). A NaN anywhere in the
+ *     result restores the state before the step; then R is re-orthonormalised as in the right-hand side, and with the floor on, z < 0 and
+ *     vz < 0 set both to 0.
+ *   Attitude loop, every step (getControl, quadrotor_simulator_so3.cpp), in FP32 as written with FP64 where the reference mixes in doubles:
+ *     R rebuilt from R_to_ypr(R) with yaw replaced by the command's current_yaw when use_external_yaw; Psi = (3 - tr(Rd^T R)) / 2; the
+ *     commanded force projected on the body z axis, or 0 unless Psi < 1; M = -kR eR - kOm eOm + omega x J omega; w_sq mixed, negative
+ *     values 0, rpm = sqrtf(w_sq). A NaN rpm keeps the last one (0 before any); setInput maps NaN to (min_rpm + max_rpm) / 2, then clamps.
+ *   Position loop, every sim_rate / cmd_rate steps, at t_k = k / cmd_rate (k = 0 before the first step; the state is the one after step
+ *     k sim_rate / cmd_rate): (1) odometry: position, velocity, current_yaw = tf::getYaw of Quaterniond(R) (Matrix3x3::getEulerYPR);
+ *     (2) IMU: acc = the last v' (0 at k = 0, SO3Control's constructor); (3) command: while t_k < duration (the left-to-right sum of the
+ *     trajectory's T) getPos, getVel, getAcc at t_k with yaw 0, yaw_dot 0; from then on the last command stays (the nodelet re-publishes
+ *     its last des_* on odometry); (4) SO3Control::calculateControl (the 45-degree limit at theta = pi/2 included) -> force and
+ *     Quaterniond orientation, rounded to float with kR, kOm, corrections and current_yaw as the simulator's Command struct holds them.
+ *     Odometry before command within a tick is this library's choice (ROS delivers them asynchronously). The command holds until the next tick.
+ *   Horizon: ticks k = 0 .. n_ticks - 1, n_ticks = floor(t_end cmd_rate) + 1; the state of the last tick is the final state.
+ * Parameters (isdf_sim_default_params, from the reference's launch files and sources):
+ *   vehicle (Quadrotor()): mass 0.98, grav 9.81, J diag(2.64e-3, 2.64e-3, 4.96e-3), kf 8.98132e-9, km 0.07 (3 * 0.062) kf, arm 0.26,
+ *     motor_tau 1/30, rpm in [1200, 35000];
+ *   controller: ctrl_mass 0.98 (simulator_example.launch "mass"), ctrl_grav 9.81 (SO3Control()); kx (5.7, 5.7, 6.2) and kv (3.4, 3.4, 4.0)
+ *     (the nodelet's defaults: gains_hummingbird.yaml's pos / vel keys are never read); kR (1, 1, 1) (yaml rot x, y; launch gains/rot/z);
+ *     kOm (0.07, 0.07, 0.1) (yaml ang x, y; launch gains/ang/z); corrections 0 (corrections_hummingbird.yaml); use_external_yaw 1 (the
+ *     launch file's "use_external_yaw " key has a trailing space, so the nodelet's default true applies);
+ *   sim_rate 1000 (rate/simulation), cmd_rate 100 (traj_server's 100 Hz timer and the simulator's rate/odom), t_end 10, log_every 1,
+ *   floor 1, diverge_dist 5 m. The vehicle and gains are independent of isdf_config's flatness vehicle.
+ * Outputs: log (may be NULL): R x cap_log records of ISDF_SIM_DOUBLES = 21 doubles, record j of rollout r at (r cap_log + j) 21, one per
+ *   log_every ticks (tick j log_every): t, pos[3], vel[3], quat[4] (w, x, y, z; Quaterniond(R)), omega[3], rpm[4], commanded pos[3];
+ *   records after the rollout ended (diverged) or past n_log = (n_ticks - 1) / log_every + 1 are NaN. summary: one per rollout, over
+ *   its ticks: position error |x - des_pos| (max, its time, RMS, final), max tilt acos(R22), max |omega|, steps whose input was clamped,
+ *   floor contacts, NaN rollbacks, accepted and rejected dopri5 tries, and diverged (a non-finite state or a position error above
+ *   diverge_dist at a tick, which ends the rollout; t_diverged its time, NaN otherwise).
+ * Guarantees: a rollout's log and summary depend only on its own inputs: the same bits run to run, alone or in any batch, through either
+ *   entry point. The unit is compiled without FMA contraction, so FP64 and FP32 arithmetic rounds as the reference's g++ -O3 x86-64 build;
+ *   libm's sin, cos, atan2, asin, acos and pow may differ in the last ulp from glibc's.
+ * Errors: ISDF_ERR_INVALID for a NULL argument, B < 1 or R < 0; a rate not positive and finite or sim_rate / cmd_rate not a whole
+ *   number; any parameter not finite, mass, J, kf, km, arm, motor_tau, ctrl_mass not positive, min_rpm < 0 or max_rpm < min_rpm, t_end < 0,
+ *   log_every < 1, diverge_dist not positive, n_ticks beyond 2^31; a log with cap_log < n_log; a non-zero reserved_; and in the host form
+ *   piece_off not starting at 0 or decreasing, durations not positive and finite, coefficients not finite, or traj[r] outside [0, B) or
+ *   naming a trajectory without pieces. The device form checks no device data: such a rollout reads as diverged at t = NaN. On failure every
+ *   summary reads diverged with NaN values (the host form writes them; the device form when the summary pointer is usable). The call counts
+ *   its launches in isdf_stats.kernel_launches. The device form is enqueued on cuda_stream and not waited for. */
+#define ISDF_SIM_INIT_DOUBLES 17
+#define ISDF_SIM_DOUBLES 21
+typedef struct isdf_sim_params {
+    double mass, grav, J[3], kf, km, arm, motor_tau, min_rpm, max_rpm;   /* vehicle */
+    double ctrl_mass, ctrl_grav, kx[3], kv[3], kR[3], kOm[3], corrections[3];   /* controller */
+    double sim_rate, cmd_rate, t_end, diverge_dist;
+    int32_t log_every, use_external_yaw, floor, reserved_;
+} isdf_sim_params;
+typedef struct isdf_sim_summary {
+    double max_err, t_max_err, rms_err, final_err, max_tilt, max_omega, t_diverged;
+    int64_t accepted, rejected;
+    int32_t clamped_steps, floor_contacts, nan_rollbacks, diverged;
+} isdf_sim_summary;
+int isdf_sim_default_params(isdf_sim_params *p);
+int isdf_simulate(isdf_ctx *ctx, int B, const int32_t *piece_off, const double *T, const double *coeffs, int R, const int32_t *traj,
+                  const double *init, const double *dist, const isdf_sim_params *p, int cap_log, double *log, isdf_sim_summary *summary);
+int isdf_simulate_device(isdf_ctx *ctx, int B, const int32_t *d_piece_off, const double *d_T, const double *d_coeffs, int R,
+                         const int32_t *d_traj, const double *d_init, const double *d_dist, const isdf_sim_params *p, int cap_log,
+                         double *d_log, isdf_sim_summary *d_summary, void *cuda_stream);
 
 /* ---- swept-volume term: addSaftyPenaOnSweptVolumeParallel (hpp:557-649) + getSDFofSweptVolume (swm:710-747) --- */
 /* parallel_points (plan_manager.cpp:246-254): P x 3 row-major world-frame voxel centres; resets lastTstar to 0 (not the persisted
