@@ -66,6 +66,17 @@ static int minco_fits(int N0) {
     return 0;
 }
 
+// an offset array off[0..B] (host): off[0] == 0, then non-decreasing (allow_empty) or increasing
+static int offsets_check(const int32_t *off, int B, const char *name, bool allow_empty) {
+    if (off[0] != 0) return fail(ISDF_ERR_INVALID, std::string(name) + "[0] must be 0");
+    for (int b = 0; b < B; b++) {
+        if (allow_empty ? off[b + 1] < off[b] : off[b + 1] <= off[b])
+            return fail(ISDF_ERR_INVALID, allow_empty ? std::string(name) + " must be non-decreasing"
+                                                      : std::string("every range of ") + name + " needs at least one entry (" + name + " must increase)");
+    }
+    return 0;
+}
+
 // The problems of a batched call and where their pieces lie. Uniform (the entry points that take B, N0): problem b owns pieces
 // [b N0, b N0 + N0) and no offsets exist. Ragged (the *_ragged entry points, include/isdf.h): problem b owns pieces [piece_off[b], piece_off[b+1])
 // and decision-vector rows [4 piece_off[b] - 3 b, 4 piece_off[b+1] - 3 (b+1)); both offset arrays live on the device.
@@ -83,12 +94,9 @@ static Layout uniform_layout(int B, int N0) {
 static int ragged_check(int B, const int32_t *piece_off, Layout *L) {
     if (B < 1) return fail(ISDF_ERR_INVALID, "B < 1");
     if (!piece_off) return fail(ISDF_ERR_INVALID, "piece_off is NULL");
-    if (piece_off[0] != 0) return fail(ISDF_ERR_INVALID, "piece_off[0] must be 0");
+    if (int r = offsets_check(piece_off, B, "piece_off", false)) return r;
     int N = 0;
-    for (int b = 0; b < B; b++) {
-        if (piece_off[b + 1] <= piece_off[b]) return fail(ISDF_ERR_INVALID, "every problem needs at least one piece (piece_off must increase)");
-        N = std::max(N, piece_off[b + 1] - piece_off[b]);
-    }
+    for (int b = 0; b < B; b++) N = std::max(N, piece_off[b + 1] - piece_off[b]);
     const size_t P = (size_t)piece_off[B], X = 4 * P - 3 * (size_t)B;
     if (X > 0x7fffffffull) return fail(ISDF_ERR_INVALID, "4*P - 3*B overflows");
     L->B = B; L->N = N; L->P = P; L->X = X;
@@ -527,25 +535,36 @@ extern "C" int isdf_set_shape_mesh_ex(isdf_ctx *c, const double *V, int nV, cons
         const double hd = 0.5 * std::sqrt(3.0) * m.gcell;
         const double list_reach = std::max(c->cfg.safety_hor, 2.0 * c->cfg.safety_hor + 0.1) + 2.0 * m.ghd;
         c->mesh.list_reach = list_reach;
-        CU_TRY(c->mesh.d_cell_cnt.ensure(ncell)); CU_TRY(c->mesh.d_cell_off.ensure(ncell));
         const unsigned warps_grid = (unsigned)((ncell + 3) / 4);
-        k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->cfg.safety_hor, c->mesh.d_cell_cnt.p, nullptr, nullptr, nullptr);
-        c->stats.kernel_launches++;
-        CU_TRY(cudaGetLastError());
-        std::vector<uint16_t> cnt(ncell);
-        CU_TRY(cudaMemcpyAsync(cnt.data(), c->mesh.d_cell_cnt.p, sizeof(uint16_t) * ncell, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaStreamSynchronize(c->stream));
-        std::vector<uint32_t> off(ncell);
-        size_t total = 0;
-        for (size_t i = 0; i < ncell; i++) { off[i] = (uint32_t)total; total += cnt[i]; }
-        if (total > 0 && total < (1ull << 31)) {
-            CU_TRY(c->mesh.d_cand.ensure(total)); CU_TRY(c->mesh.d_cand_lb.ensure(total));
-            CU_TRY(cudaMemcpyAsync(c->mesh.d_cell_off.p, off.data(), sizeof(uint32_t) * ncell, cudaMemcpyHostToDevice, c->stream));
-            k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->cfg.safety_hor, c->mesh.d_cell_cnt.p,
-                                                                 c->mesh.d_cell_off.p, c->mesh.d_cand.p, c->mesh.d_cand_lb.p);
+        // one kind of candidate list: launch(off, cand, lb) counts into cnt (off null), the counts' prefix sums become off, and, when the
+        // lists hold 1 to 2^31 - 1 candidates in all, launch fills cand and lb; *total: the candidates, h_cnt: the counts
+        auto build_lists = [&](auto launch, DevBuf<uint16_t> &cnt, DevBuf<uint32_t> &off, DevBuf<uint32_t> &cand, DevBuf<float> &lb,
+                               std::vector<uint16_t> &h_cnt, size_t *total) -> int {
+            CU_TRY(cnt.ensure(ncell)); CU_TRY(off.ensure(ncell));
+            launch(nullptr, nullptr, nullptr);
+            c->stats.kernel_launches++;
+            CU_TRY(cudaGetLastError());
+            h_cnt.resize(ncell);
+            CU_TRY(cudaMemcpyAsync(h_cnt.data(), cnt.p, sizeof(uint16_t) * ncell, cudaMemcpyDeviceToHost, c->stream));
+            CU_TRY(cudaStreamSynchronize(c->stream));
+            std::vector<uint32_t> h_off(ncell);
+            *total = 0;
+            for (size_t i = 0; i < ncell; i++) { h_off[i] = (uint32_t)*total; *total += h_cnt[i]; }
+            if (*total == 0 || *total >= (1ull << 31)) return 0;
+            CU_TRY(cand.ensure(*total)); CU_TRY(lb.ensure(*total));
+            CU_TRY(cudaMemcpyAsync(off.p, h_off.data(), sizeof(uint32_t) * ncell, cudaMemcpyHostToDevice, c->stream));
+            launch(off.p, cand.p, lb.p);
             c->stats.kernel_launches++;
             CU_TRY(cudaGetLastError());
             CU_TRY(cudaStreamSynchronize(c->stream));
+            return 0;
+        };
+        std::vector<uint16_t> cnt;
+        size_t total = 0;
+        if (int r = build_lists([&](const uint32_t *off, uint32_t *cand, float *lb) {
+                k_mesh_cell_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, hd, list_reach, c->cfg.safety_hor, c->mesh.d_cell_cnt.p, off, cand, lb);
+            }, c->mesh.d_cell_cnt, c->mesh.d_cell_off, c->mesh.d_cand, c->mesh.d_cand_lb, cnt, &total)) return r;
+        if (total > 0 && total < (1ull << 31)) {
             m.cell_off = c->mesh.d_cell_off.p; m.cell_cnt = c->mesh.d_cell_cnt.p; m.cand = c->mesh.d_cand.p; m.cand_lb = c->mesh.d_cand_lb.p;
             if (c->mesh.disc_k > 1) {
                 // the discrete scan's sub-box filtered lists, counted, then written into their own arrays. margin covers the scan
@@ -553,21 +572,12 @@ extern "C" int isdf_set_shape_mesh_ex(isdf_ctx *c, const double *V, int nV, cons
                 double scale = 1.0;
                 for (int a = 0; a < 3; a++) scale = std::max(scale, std::max(std::fabs(m.glo[a]), std::fabs(m.glo[a] + m.gdim[a] * m.gcell)));
                 const double margin = 1e-9 * scale + 1e-12;
-                CU_TRY(c->mesh.d_disc_cnt.ensure(ncell)); CU_TRY(c->mesh.d_disc_off.ensure(ncell));
-                k_mesh_disc_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, c->mesh.disc_k, margin, c->mesh.d_disc_cnt.p, nullptr, nullptr, nullptr);
-                c->stats.kernel_launches++;
-                CU_TRY(cudaGetLastError());
-                std::vector<uint16_t> dcnt(ncell);
-                CU_TRY(cudaMemcpyAsync(dcnt.data(), c->mesh.d_disc_cnt.p, sizeof(uint16_t) * ncell, cudaMemcpyDeviceToHost, c->stream));
-                CU_TRY(cudaStreamSynchronize(c->stream));
+                // the filtered lists are subsequences of the full ones and keep each one's first entry: 0 < dtotal <= total
+                std::vector<uint16_t> dcnt;
                 size_t dtotal = 0;
-                for (size_t i = 0; i < ncell; i++) { off[i] = (uint32_t)dtotal; dtotal += dcnt[i]; }
-                CU_TRY(c->mesh.d_disc_cand.ensure(dtotal)); CU_TRY(c->mesh.d_disc_lb.ensure(dtotal));
-                CU_TRY(cudaMemcpyAsync(c->mesh.d_disc_off.p, off.data(), sizeof(uint32_t) * ncell, cudaMemcpyHostToDevice, c->stream));
-                k_mesh_disc_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, c->mesh.disc_k, margin, c->mesh.d_disc_cnt.p,
-                                                                     c->mesh.d_disc_off.p, c->mesh.d_disc_cand.p, c->mesh.d_disc_lb.p);
-                c->stats.kernel_launches++;
-                CU_TRY(cudaGetLastError());
+                if (int r = build_lists([&](const uint32_t *off, uint32_t *cand, float *lb) {
+                        k_mesh_disc_lists<<<warps_grid, 128, 0, c->stream>>>(m, (long long)ncell, c->mesh.disc_k, margin, c->mesh.d_disc_cnt.p, off, cand, lb);
+                    }, c->mesh.d_disc_cnt, c->mesh.d_disc_off, c->mesh.d_disc_cand, c->mesh.d_disc_lb, dcnt, &dtotal)) return r;
                 CU_TRY(c->mesh.d_disc_rec.ensure(ncell));
                 k_mesh_cell_pack<<<(unsigned)((ncell + 255) / 256), 256, 0, c->stream>>>((long long)ncell, m.cell_dist, m.cell_seed, c->mesh.d_disc_off.p,
                                                                                          c->mesh.d_disc_cnt.p, c->mesh.d_disc_rec.p);
@@ -1164,8 +1174,7 @@ static void states_launch(isdf_ctx *c, int B, const int *d_off, const double *d_
 extern "C" int isdf_trajectory_states(isdf_ctx *c, int B, const int32_t *piece_off, const double *T, const double *coeffs, int64_t Q,
                                       const int32_t *traj, const double *times, double *out) {
     if (int rc = states_args_check(c, B, piece_off, T, coeffs, Q, traj, times, out)) return rc;
-    if (piece_off[0] != 0) return fail(ISDF_ERR_INVALID, "piece_off[0] must be 0");
-    for (int b = 0; b < B; b++) if (piece_off[b + 1] < piece_off[b]) return fail(ISDF_ERR_INVALID, "piece_off must not decrease");
+    if (int rc = offsets_check(piece_off, B, "piece_off", true)) return rc;
     const int P = piece_off[B];
     if (int rc = swept_traj_check(P, T, coeffs)) return rc;
     for (long long q = 0; q < Q; q++) if (traj[q] < 0 || traj[q] >= B) return fail(ISDF_ERR_INVALID, "traj[q] outside [0, B)");
@@ -1322,8 +1331,7 @@ extern "C" int isdf_simulate(isdf_ctx *c, int B, const int32_t *piece_off, const
     return poison_on_failure([&]() -> int {
         int n_ticks = 0, m = 0;
         if (int rc = sim_args_check(c, B, piece_off, T, coeffs, R, traj, init, p, cap_log, log, summary, &n_ticks, &m)) return rc;
-        if (piece_off[0] != 0) return fail(ISDF_ERR_INVALID, "piece_off[0] must be 0");
-        for (int b = 0; b < B; b++) if (piece_off[b + 1] < piece_off[b]) return fail(ISDF_ERR_INVALID, "piece_off must not decrease");
+        if (int rc = offsets_check(piece_off, B, "piece_off", true)) return rc;
         const int P = piece_off[B];
         if (P > 0) if (int rc = swept_traj_check(P, T, coeffs)) return rc;
         for (int r = 0; r < R; r++)
@@ -1445,105 +1453,13 @@ __device__ __forceinline__ bool gather_includes(const DevGrid &G, const GatherBo
     if (!(i > b.l1[0] || i < b.l0[0] || j > b.l1[1] || j < b.l0[1] || k > b.l1[2] || k < b.l0[2])) return false;
     return (G.bits[((size_t)i * G.Y + j) * G.Zw + (k >> 5)] >> (k & 31)) & 1u;
 }
-// Obstacle gather, one CTA per waypoint, three launches: k_gather_boxes (index boxes of every waypoint), k_gather_points<false> (how many
-// voxels each waypoint emits: a voxel belongs to the FIRST waypoint whose box includes it) and, after an exclusive scan over the waypoints
-// inside the kernel, k_gather_points<true> (ordered compaction inside the CTA at the waypoint's offset). Output order = the reference's:
-// waypoint by waypoint, each box in x -> y -> z order.
-__global__ void k_gather_boxes(const DevGrid G, const double *wps, int nQ, double h, double ox, double oy, double oz, GatherBox *boxes) {
-    const int q = blockIdx.x * blockDim.x + threadIdx.x;
-    if (q >= nQ) return;
-    GatherBox b;
-    const double c[3] = {wps[3 * q] + ox, wps[3 * q + 1] + oy, wps[3 * q + 2] + oz};
-    const double l[3] = {q == 0 ? 999.0 : wps[3 * (q - 1)], q == 0 ? 999.0 : wps[3 * (q - 1) + 1], q == 0 ? 999.0 : wps[3 * (q - 1) + 2]};
-    const int dims[3] = {G.X, G.Y, G.Z};
-    for (int a = 0; a < 3; a++) {
-        b.a0[a] = grid_axis_index(c[a] - h, G.bmin[a], G.bmax[a], G.res, dims[a]); b.a1[a] = grid_axis_index(c[a] + h, G.bmin[a], G.bmax[a], G.res, dims[a]);
-        b.l0[a] = grid_axis_index(l[a] - h, G.bmin[a], G.bmax[a], G.res, dims[a]); b.l1[a] = grid_axis_index(l[a] + h, G.bmin[a], G.bmax[a], G.res, dims[a]);
-    }
-    boxes[q] = b;
-}
-template <bool WRITE>
-__global__ void __launch_bounds__(256) k_gather_points(const DevGrid G, int nQ, const GatherBox *boxes, int *counts, double *out, int cap, int *count) {
-    __shared__ int warp_cnt[8];
-    __shared__ int running;
-    const int q = blockIdx.x;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) {
-        int off = 0;
-        if (WRITE) { for (int p = 0; p < q; p++) off += counts[p]; if (q == nQ - 1) *count = off + counts[q]; }
-        running = off;
-    }
-    __syncthreads();
-    const GatherBox b = boxes[q];
-    const int ny = b.a1[1] - b.a0[1] + 1, nz = b.a1[2] - b.a0[2] + 1;
-    const int nvox = (b.a1[0] - b.a0[0] + 1) * ny * nz;
-    for (int base = 0; base < nvox; base += blockDim.x) {
-        const int v = base + threadIdx.x;
-        bool emit = false; int i = 0, j = 0, k = 0;
-        if (v < nvox) {
-            i = b.a0[0] + v / (ny * nz); j = b.a0[1] + (v / nz) % ny; k = b.a0[2] + v % nz;
-            emit = gather_includes(G, b, i, j, k);
-            for (int p = 0; emit && p < q; p++) if (gather_includes(G, boxes[p], i, j, k)) emit = false;
-        }
-        const unsigned bal = __ballot_sync(0xffffffffu, emit);
-        if (lane == 0) warp_cnt[warp] = __popc(bal);
-        __syncthreads();
-        if (WRITE) {
-            int off = running;
-            for (int w = 0; w < warp; w++) off += warp_cnt[w];
-            if (emit) {
-                const int pos = off + __popc(bal & ((1u << lane) - 1u));
-                if (pos < cap) { out[3 * pos] = (i + 0.5) * G.res + G.bmin[0]; out[3 * pos + 1] = (j + 0.5) * G.res + G.bmin[1]; out[3 * pos + 2] = (k + 0.5) * G.res + G.bmin[2]; }
-            }
-        }
-        __syncthreads();
-        if (threadIdx.x == 0) { int t = 0; for (int w = 0; w < 8; w++) t += warp_cnt[w]; running += t; }
-        __syncthreads();
-    }
-    if (!WRITE && threadIdx.x == 0) counts[q] = running;
-}
-
-extern "C" int isdf_gather_obstacle_points(isdf_ctx *c, const double *waypoints, int nQ, double half_extent, const double *offset,
-                                           double *out_points, int cap, int *n, int set_as_points) {
-    if (!c || !waypoints || nQ < 1 || !n || cap < 0 || (cap > 0 && !out_points && !set_as_points)) return fail(ISDF_ERR_INVALID, "bad argument");
-    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
-    if (set_device(c)) return ISDF_ERR_CUDA;
-    DevBuf<double> dw, dout; DevBuf<GatherBox> db; DevBuf<int> dn;
-    const int capd = cap > 0 ? cap : 1;
-    CU_TRY(dw.upload(waypoints, (size_t)3 * nQ, c->stream));
-    CU_TRY(dout.ensure((size_t)3 * capd)); CU_TRY(db.ensure(nQ)); CU_TRY(dn.ensure((size_t)nQ + 1));
-    const double ox = offset ? offset[0] : 0.0, oy = offset ? offset[1] : 0.0, oz = offset ? offset[2] : 0.0;
-    k_gather_boxes<<<(nQ + 127) / 128, 128, 0, c->stream>>>(c->map.grid, dw.p, nQ, half_extent, ox, oy, oz, db.p);
-    k_gather_points<false><<<nQ, 256, 0, c->stream>>>(c->map.grid, nQ, db.p, dn.p + 1, nullptr, 0, dn.p);
-    k_gather_points<true><<<nQ, 256, 0, c->stream>>>(c->map.grid, nQ, db.p, dn.p + 1, dout.p, capd, dn.p);
-    c->stats.kernel_launches += 3;
-    CU_TRY(cudaGetLastError());
-    int cnt = 0;
-    CU_TRY(cudaMemcpyAsync(&cnt, dn.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaStreamSynchronize(c->stream));
-    *n = cnt;
-    const int m = cnt < cap ? cnt : cap;
-    int rc = 0;
-    if (m > 0 && out_points) CU_TRY(cudaMemcpy(out_points, dout.p, sizeof(double) * 3 * m, cudaMemcpyDeviceToHost));
-    if (set_as_points) {
-        if (cnt > cap) rc = fail(ISDF_ERR_INVALID, "cap smaller than the obstacle list");
-        else {
-            std::vector<double> tmp((size_t)3 * (m > 0 ? m : 1));
-            if (m > 0) CU_TRY(cudaMemcpy(tmp.data(), dout.p, sizeof(double) * 3 * m, cudaMemcpyDeviceToHost));
-            cudaError_t e = c->sv.set_points(tmp.data(), m, c->stream);
-            if (e != cudaSuccess) rc = fail(ISDF_ERR_CUDA, cudaGetErrorString(e));
-        }
-    }
-    return rc;
-}
-
 // ---- every plan's obstacle list in one call (isdf_gather_obstacle_points_batch) -----------------------------------------------------
 // B plans, plan b owning the waypoint rows [wp_off[b], wp_off[b+1]). Four launches over all plans: k_gather_boxes_batch (the index boxes of
 // every row, the 999 sentinel at each plan's first row), k_gather_points_batch<false> (grid (waypoint, plan): how many voxels each row
 // emits), k_gather_scan (the exclusive scan of the row counts) and k_gather_points_batch<true> (the ordered compaction at each row's
 // offset). The rows of all plans are scanned in one pass: plans lie back to back, so a row's offset is its plan's offset plus the counts of
-// the plan's earlier rows, and a plan's offset is the offset of its first row. The centres are computed as k_gather_points computes them,
-// in this -fmad=false unit.
+// the plan's earlier rows, and a plan's offset is the offset of its first row. Output order = the reference's: plan by plan, waypoint by
+// waypoint, each box in x -> y -> z order; a voxel belongs to the FIRST waypoint of its plan whose box includes it.
 constexpr int GATHER_LIST_CAP = 1024;   // earlier boxes of a plan kept per CTA; with more, every earlier box of the plan is tested
 
 // the plan b with wp_off[b] <= q < wp_off[b+1] (empty plans skipped): the smallest b with wp_off[b+1] > q
@@ -1715,13 +1631,37 @@ static int gather_set_points(isdf_ctx *c, int B, const std::vector<int> &pt_off,
     return 0;
 }
 
+// one plan's list: the batched gather with B = 1, whose write pass always runs, so that *n is the whole list's size
+extern "C" int isdf_gather_obstacle_points(isdf_ctx *c, const double *waypoints, int nQ, double half_extent, const double *offset,
+                                           double *out_points, int cap, int *n, int set_as_points) {
+    if (!c || !waypoints || nQ < 1 || !n || cap < 0 || (cap > 0 && !out_points && !set_as_points)) return fail(ISDF_ERR_INVALID, "bad argument");
+    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    auto &g = c->gat;
+    const int wp_off[2] = {0, nQ};
+    CU_TRY(g.d_wpoff.upload(wp_off, 2, c->stream));
+    CU_TRY(g.d_wp.upload(waypoints, (size_t)3 * nQ, c->stream));
+    std::vector<int> off;
+    long long total = 0;
+    if (int r = gather_batch_run(c, 1, wp_off, g.d_wpoff.p, g.d_wp.p, half_extent, offset, 0x7fffffffll, off, &total, c->stream)) return r;
+    *n = (int)total;
+    const long long m = std::min<long long>(total, cap);
+    if (m > 0 && out_points) {   // the write pass runs on the context's non-blocking stream
+        CU_TRY(cudaMemcpyAsync(out_points, g.d_out.p, sizeof(double) * 3 * m, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaStreamSynchronize(c->stream));
+    }
+    if (!set_as_points) return 0;
+    if (total > cap) return fail(ISDF_ERR_INVALID, "cap smaller than the obstacle list");
+    CU_TRY(c->sv.set_points(g.d_out.p, (int)m, c->stream, cudaMemcpyDeviceToDevice));
+    return 0;
+}
+
 extern "C" int isdf_gather_obstacle_points_batch(isdf_ctx *c, int B, const int32_t *wp_off, const double *waypoints, double half_extent,
                                                  const double *offset, int64_t cap, double *out_points, int32_t *pt_off, int set_as_points) {
     if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
     if (B < 1 || B > 65535) return fail(ISDF_ERR_INVALID, "B must lie in [1, 65535]");
     if (!wp_off || !pt_off || cap < 0) return fail(ISDF_ERR_INVALID, "NULL argument or cap < 0");
-    if (wp_off[0] != 0) return fail(ISDF_ERR_INVALID, "wp_off[0] must be 0");
-    for (int b = 0; b < B; b++) if (wp_off[b + 1] < wp_off[b]) return fail(ISDF_ERR_INVALID, "wp_off must be non-decreasing");
+    if (int r = offsets_check(wp_off, B, "wp_off", true)) return r;
     if (wp_off[B] > 0 && !waypoints) return fail(ISDF_ERR_INVALID, "waypoints is NULL");
     if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
     if (set_device(c)) return ISDF_ERR_CUDA;
@@ -1969,40 +1909,40 @@ static int callback_batch_launch(isdf_ctx *c, const Layout &L, const double *d_h
     return 0;
 }
 
-static int callback_batch_check(isdf_ctx *c, int B, int N0) {
+// the batched callback's checks, in order: the batch (ragged: the *_ragged entry points' piece_off; else B problems of N0 pieces) and
+// its sizes into *L, the sharding, the evaluation state
+static int callback_batch_check(isdf_ctx *c, bool ragged, int B, int N0, const int32_t *piece_off, Layout *L) {
     if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
-    if (B < 1 || N0 < 1) return fail(ISDF_ERR_INVALID, "B < 1 or N0 < 1");
-    if ((long long)B * N0 > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "B*N0 overflows");
-    if (c->world != 1) return fail(ISDF_ERR_STATE, "the batched callback shards by PROBLEM: keep isdf_set_shard(ctx, 0, 1) and give each rank its own problems");
-    return check_eval_state(c, B * N0, true);
-}
-
-extern "C" int isdf_callback_batch_device(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc, double rho,
-                                          const double *d_x, double *d_cost, double *d_grad, void *cuda_stream) {
-    int r = callback_batch_check(c, B, N0);
-    if (r) return r;
-    if (!d_head || !d_tail || !d_x || !d_cost || !d_grad) return fail(ISDF_ERR_INVALID, "NULL device pointer");
-    if (set_device(c)) return ISDF_ERR_CUDA;
-    return callback_batch_launch(c, uniform_layout(B, N0), d_head, d_tail, per_problem_bc ? 9 : 0, rho, d_x, d_cost, d_grad, (cudaStream_t)cuda_stream);
-}
-
-// a ragged batch's checks (callback_batch_check's, with the offsets in place of B, N0) and sizes
-static int callback_ragged_check(isdf_ctx *c, int B, const int32_t *piece_off, Layout *L) {
-    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
-    if (int r = ragged_check(B, piece_off, L)) return r;
+    if (ragged) {
+        if (int r = ragged_check(B, piece_off, L)) return r;
+    } else {
+        if (B < 1 || N0 < 1) return fail(ISDF_ERR_INVALID, "B < 1 or N0 < 1");
+        if ((long long)B * N0 > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "B*N0 overflows");
+        *L = uniform_layout(B, N0);
+    }
     if (c->world != 1) return fail(ISDF_ERR_STATE, "the batched callback shards by PROBLEM: keep isdf_set_shard(ctx, 0, 1) and give each rank its own problems");
     return check_eval_state(c, (int)L->P, true);
 }
 
-extern "C" int isdf_callback_batch_ragged_device(isdf_ctx *c, int B, const int32_t *piece_off, const double *d_head, const double *d_tail,
-                                                 int per_problem_bc, double rho, const double *d_x, double *d_cost, double *d_grad, void *cuda_stream) {
+// the device form of the batched callback on st; a ragged batch's offsets are uploaded first, a uniform batch has none
+static int callback_device(isdf_ctx *c, bool ragged, int B, int N0, const int32_t *piece_off, const double *d_head, const double *d_tail,
+                           int per_problem_bc, double rho, const double *d_x, double *d_cost, double *d_grad, cudaStream_t st) {
     Layout L;
-    if (int r = callback_ragged_check(c, B, piece_off, &L)) return r;
+    if (int r = callback_batch_check(c, ragged, B, N0, piece_off, &L)) return r;
     if (!d_head || !d_tail || !d_x || !d_cost || !d_grad) return fail(ISDF_ERR_INVALID, "NULL device pointer");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    const cudaStream_t st = (cudaStream_t)cuda_stream;
-    if (int r = ragged_upload(c->batch.d_off, piece_off, st, &L)) return r;
+    if (ragged) if (int r = ragged_upload(c->batch.d_off, piece_off, st, &L)) return r;
     return callback_batch_launch(c, L, d_head, d_tail, per_problem_bc ? 9 : 0, rho, d_x, d_cost, d_grad, st);
+}
+
+extern "C" int isdf_callback_batch_device(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc, double rho,
+                                          const double *d_x, double *d_cost, double *d_grad, void *cuda_stream) {
+    return callback_device(c, false, B, N0, nullptr, d_head, d_tail, per_problem_bc, rho, d_x, d_cost, d_grad, (cudaStream_t)cuda_stream);
+}
+
+extern "C" int isdf_callback_batch_ragged_device(isdf_ctx *c, int B, const int32_t *piece_off, const double *d_head, const double *d_tail,
+                                                 int per_problem_bc, double rho, const double *d_x, double *d_cost, double *d_grad, void *cuda_stream) {
+    return callback_device(c, true, B, 0, piece_off, d_head, d_tail, per_problem_bc, rho, d_x, d_cost, d_grad, (cudaStream_t)cuda_stream);
 }
 
 // the host entry points' boundary conditions (9 doubles, or 9 per problem) in buf on c->stream: *d_head, then *d_tail
@@ -2016,35 +1956,12 @@ static int upload_bc(isdf_ctx *c, DevBuf<double> &buf, int B, int per_problem_bc
     return 0;
 }
 
-extern "C" int isdf_callback_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc, double rho,
-                                   const double *x, double *cost, double *grad) {
-    return poison_on_failure([&]() -> int {
-        if (int r = callback_batch_check(c, B, N0)) return r;
-        if (!head || !tail || !x || !cost || !grad) return fail(ISDF_ERR_INVALID, "NULL argument");
-        if (set_device(c)) return ISDF_ERR_CUDA;
-        const size_t dim = (size_t)N0 + 3 * (size_t)(N0 - 1);
-        CU_TRY(c->batch.d_x.upload(x, dim * B, c->stream));
-        const double *d_head, *d_tail;
-        if (int r = upload_bc(c, c->batch.d_bc, B, per_problem_bc, head, tail, &d_head, &d_tail)) return r;
-        CU_TRY(c->batch.d_cost.ensure(B)); CU_TRY(c->batch.d_grad.ensure(dim * B));
-        CU_TRY(cudaEventRecord(c->ev0, c->stream));
-        if (int r = isdf_callback_batch_device(c, B, N0, d_head, d_tail, per_problem_bc, rho, c->batch.d_x.p, c->batch.d_cost.p, c->batch.d_grad.p,
-                                               c->stream)) return r;
-        CU_TRY(cudaEventRecord(c->ev1, c->stream));
-        CU_TRY(cudaMemcpyAsync(cost, c->batch.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaMemcpyAsync(grad, c->batch.d_grad.p, sizeof(double) * dim * B, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaStreamSynchronize(c->stream));
-        float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
-        c->stats.last_kernel_ms = ms;
-        return 0;
-    }, [&] { nan_fill(cost, B); });
-}
-
-extern "C" int isdf_callback_batch_ragged(isdf_ctx *c, int B, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
-                                          double rho, const double *x, double *cost, double *grad) {
+// the host form of the batched callback: inputs staged in c->batch, then the device form on c->stream
+static int callback_host(isdf_ctx *c, bool ragged, int B, int N0, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
+                         double rho, const double *x, double *cost, double *grad) {
     return poison_on_failure([&]() -> int {
         Layout L;
-        if (int r = callback_ragged_check(c, B, piece_off, &L)) return r;
+        if (int r = callback_batch_check(c, ragged, B, N0, piece_off, &L)) return r;
         if (!head || !tail || !x || !cost || !grad) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
         CU_TRY(c->batch.d_x.upload(x, L.X, c->stream));
@@ -2052,8 +1969,8 @@ extern "C" int isdf_callback_batch_ragged(isdf_ctx *c, int B, const int32_t *pie
         if (int r = upload_bc(c, c->batch.d_bc, B, per_problem_bc, head, tail, &d_head, &d_tail)) return r;
         CU_TRY(c->batch.d_cost.ensure(B)); CU_TRY(c->batch.d_grad.ensure(L.X));
         CU_TRY(cudaEventRecord(c->ev0, c->stream));
-        if (int r = isdf_callback_batch_ragged_device(c, B, piece_off, d_head, d_tail, per_problem_bc, rho, c->batch.d_x.p, c->batch.d_cost.p,
-                                                      c->batch.d_grad.p, c->stream)) return r;
+        if (int r = callback_device(c, ragged, B, N0, piece_off, d_head, d_tail, per_problem_bc, rho, c->batch.d_x.p, c->batch.d_cost.p,
+                                    c->batch.d_grad.p, c->stream)) return r;
         CU_TRY(cudaEventRecord(c->ev1, c->stream));
         CU_TRY(cudaMemcpyAsync(cost, c->batch.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
         CU_TRY(cudaMemcpyAsync(grad, c->batch.d_grad.p, sizeof(double) * L.X, cudaMemcpyDeviceToHost, c->stream));
@@ -2062,6 +1979,16 @@ extern "C" int isdf_callback_batch_ragged(isdf_ctx *c, int B, const int32_t *pie
         c->stats.last_kernel_ms = ms;
         return 0;
     }, [&] { nan_fill(cost, B); });
+}
+
+extern "C" int isdf_callback_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc, double rho,
+                                   const double *x, double *cost, double *grad) {
+    return callback_host(c, false, B, N0, nullptr, head, tail, per_problem_bc, rho, x, cost, grad);
+}
+
+extern "C" int isdf_callback_batch_ragged(isdf_ctx *c, int B, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
+                                          double rho, const double *x, double *cost, double *grad) {
+    return callback_host(c, true, B, 0, piece_off, head, tail, per_problem_bc, rho, x, cost, grad);
 }
 
 // ---- device-resident lock-step L-BFGS over the batched callback (SURVEY §8f row 2; isdf_lbfgs.cuh) ----------------------------------------
@@ -2160,34 +2087,17 @@ static int lbfgs_copy_out(const isdf_ctx::LbfgsBufs &lb, int B, size_t X, double
     return 0;
 }
 
-extern "C" int isdf_lbfgs_batch_device(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc, double rho,
-                                       const isdf_lbfgs_params *prm, double *d_x, double *d_f, int *d_ret, int *d_iterations, int *d_evaluations,
-                                       int *rounds_out, void *cuda_stream) {
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    return poison_on_failure([&]() -> int {
-        if (int r = callback_batch_check(c, B, N0)) return r;
-        if (int r = lbfgs_check(prm)) return r;
-        if (!d_head || !d_tail || !d_x || !d_f) return fail(ISDF_ERR_INVALID, "NULL device pointer");
-        if (set_device(c)) return ISDF_ERR_CUDA;
-        const Layout L = uniform_layout(B, N0);
-        return lbfgs_rounds(c, c->lbfgs, B, 4 * N0 - 3, nullptr, L.X, prm, 0, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st,
-                            [&](const double *x, double *f, double *g) {
-                                return callback_batch_launch(c, L, d_head, d_tail, per_problem_bc ? 9 : 0, rho, x, f, g, st);
-                            });
-    }, [&] { nan_fill_device(c, d_f, B, st); });
-}
-
-extern "C" int isdf_lbfgs_batch_ragged_device(isdf_ctx *c, int B, const int32_t *piece_off, const double *d_head, const double *d_tail,
-                                              int per_problem_bc, double rho, const isdf_lbfgs_params *prm, double *d_x, double *d_f, int *d_ret,
-                                              int *d_iterations, int *d_evaluations, int *rounds_out, void *cuda_stream) {
-    cudaStream_t st = (cudaStream_t)cuda_stream;
+// the device form of the lock-step L-BFGS over the batched callback on st; a ragged batch's offsets are uploaded first
+static int lbfgs_device(isdf_ctx *c, bool ragged, int B, int N0, const int32_t *piece_off, const double *d_head, const double *d_tail, int per_problem_bc,
+                        double rho, const isdf_lbfgs_params *prm, double *d_x, double *d_f, int *d_ret, int *d_iterations, int *d_evaluations,
+                        int *rounds_out, cudaStream_t st) {
     return poison_on_failure([&]() -> int {
         Layout L;
-        if (int r = callback_ragged_check(c, B, piece_off, &L)) return r;
+        if (int r = callback_batch_check(c, ragged, B, N0, piece_off, &L)) return r;
         if (int r = lbfgs_check(prm)) return r;
         if (!d_head || !d_tail || !d_x || !d_f) return fail(ISDF_ERR_INVALID, "NULL device pointer");
         if (set_device(c)) return ISDF_ERR_CUDA;
-        if (int r = ragged_upload(c->batch.d_off, piece_off, st, &L)) return r;
+        if (ragged) if (int r = ragged_upload(c->batch.d_off, piece_off, st, &L)) return r;
         return lbfgs_rounds(c, c->lbfgs, B, 4 * L.N - 3, L.d_xoff, L.X, prm, 0, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st,
                             [&](const double *x, double *f, double *g) {
                                 return callback_batch_launch(c, L, d_head, d_tail, per_problem_bc ? 9 : 0, rho, x, f, g, st);
@@ -2195,30 +2105,26 @@ extern "C" int isdf_lbfgs_batch_ragged_device(isdf_ctx *c, int B, const int32_t 
     }, [&] { nan_fill_device(c, d_f, B, st); });
 }
 
-extern "C" int isdf_lbfgs_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc, double rho,
-                                const isdf_lbfgs_params *prm, double *x, double *f, int *ret, int *iterations, int *evaluations, int *rounds_out) {
-    return poison_on_failure([&]() -> int {
-        if (int r = callback_batch_check(c, B, N0)) return r;
-        if (!head || !tail || !x || !f) return fail(ISDF_ERR_INVALID, "NULL argument");
-        if (set_device(c)) return ISDF_ERR_CUDA;
-        isdf_ctx::LbfgsBufs &lb = c->lbfgs;
-        const size_t n = (size_t)4 * N0 - 3;
-        CU_TRY(lb.d_x.upload(x, n * B, c->stream));
-        const double *d_head, *d_tail;
-        if (int r = upload_bc(c, c->batch.d_bc, B, per_problem_bc, head, tail, &d_head, &d_tail)) return r;
-        CU_TRY(lb.d_f.ensure(B)); CU_TRY(lb.d_head.ensure((size_t)3 * B));
-        if (int r = isdf_lbfgs_batch_device(c, B, N0, d_head, d_tail, per_problem_bc, rho, prm, lb.d_x.p, lb.d_f.p, lb.d_head.p, lb.d_head.p + B,
-                                            lb.d_head.p + 2 * (size_t)B, rounds_out, c->stream)) return r;
-        return lbfgs_copy_out(lb, B, n * B, x, f, ret, iterations, evaluations);
-    }, [&] { nan_fill(f, B); });
+extern "C" int isdf_lbfgs_batch_device(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc, double rho,
+                                       const isdf_lbfgs_params *prm, double *d_x, double *d_f, int *d_ret, int *d_iterations, int *d_evaluations,
+                                       int *rounds_out, void *cuda_stream) {
+    return lbfgs_device(c, false, B, N0, nullptr, d_head, d_tail, per_problem_bc, rho, prm, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out,
+                        (cudaStream_t)cuda_stream);
 }
 
-extern "C" int isdf_lbfgs_batch_ragged(isdf_ctx *c, int B, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
-                                       double rho, const isdf_lbfgs_params *prm, double *x, double *f, int *ret, int *iterations, int *evaluations,
-                                       int *rounds_out) {
+extern "C" int isdf_lbfgs_batch_ragged_device(isdf_ctx *c, int B, const int32_t *piece_off, const double *d_head, const double *d_tail,
+                                              int per_problem_bc, double rho, const isdf_lbfgs_params *prm, double *d_x, double *d_f, int *d_ret,
+                                              int *d_iterations, int *d_evaluations, int *rounds_out, void *cuda_stream) {
+    return lbfgs_device(c, true, B, 0, piece_off, d_head, d_tail, per_problem_bc, rho, prm, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out,
+                        (cudaStream_t)cuda_stream);
+}
+
+// the host form of the L-BFGS: inputs staged in c->lbfgs and c->batch, then the device form on c->stream, results copied back
+static int lbfgs_host(isdf_ctx *c, bool ragged, int B, int N0, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
+                      double rho, const isdf_lbfgs_params *prm, double *x, double *f, int *ret, int *iterations, int *evaluations, int *rounds_out) {
     return poison_on_failure([&]() -> int {
         Layout L;
-        if (int r = callback_ragged_check(c, B, piece_off, &L)) return r;
+        if (int r = callback_batch_check(c, ragged, B, N0, piece_off, &L)) return r;
         if (!head || !tail || !x || !f) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
         isdf_ctx::LbfgsBufs &lb = c->lbfgs;
@@ -2226,10 +2132,21 @@ extern "C" int isdf_lbfgs_batch_ragged(isdf_ctx *c, int B, const int32_t *piece_
         const double *d_head, *d_tail;
         if (int r = upload_bc(c, c->batch.d_bc, B, per_problem_bc, head, tail, &d_head, &d_tail)) return r;
         CU_TRY(lb.d_f.ensure(B)); CU_TRY(lb.d_head.ensure((size_t)3 * B));
-        if (int r = isdf_lbfgs_batch_ragged_device(c, B, piece_off, d_head, d_tail, per_problem_bc, rho, prm, lb.d_x.p, lb.d_f.p, lb.d_head.p,
-                                                   lb.d_head.p + B, lb.d_head.p + 2 * (size_t)B, rounds_out, c->stream)) return r;
+        if (int r = lbfgs_device(c, ragged, B, N0, piece_off, d_head, d_tail, per_problem_bc, rho, prm, lb.d_x.p, lb.d_f.p, lb.d_head.p, lb.d_head.p + B,
+                                 lb.d_head.p + 2 * (size_t)B, rounds_out, c->stream)) return r;
         return lbfgs_copy_out(lb, B, L.X, x, f, ret, iterations, evaluations);
     }, [&] { nan_fill(f, B); });
+}
+
+extern "C" int isdf_lbfgs_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc, double rho,
+                                const isdf_lbfgs_params *prm, double *x, double *f, int *ret, int *iterations, int *evaluations, int *rounds_out) {
+    return lbfgs_host(c, false, B, N0, nullptr, head, tail, per_problem_bc, rho, prm, x, f, ret, iterations, evaluations, rounds_out);
+}
+
+extern "C" int isdf_lbfgs_batch_ragged(isdf_ctx *c, int B, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
+                                       double rho, const isdf_lbfgs_params *prm, double *x, double *f, int *ret, int *iterations, int *evaluations,
+                                       int *rounds_out) {
+    return lbfgs_host(c, true, B, 0, piece_off, head, tail, per_problem_bc, rho, prm, x, f, ret, iterations, evaluations, rounds_out);
 }
 
 // Diagnostic (not part of include/isdf.h): the unchanged lbfgs_rounds + k_lbfgs_feed for B instances of dimension n on a HOST objective.
@@ -2280,8 +2197,7 @@ extern "C" int isdf_path_waypoints(int B, const int32_t *path_off, const double 
                                    double *waypoints, int32_t *wp_off, int32_t *pieces) {
     if (B < 1 || !path_off || !path_xyz || !wp_off || !pieces || cap < 0 || (cap > 0 && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument, B < 1 or cap < 0");
     if (!(std::isfinite(res) && res > 0.0) || !(std::isfinite(parlength) && parlength > 0.0)) return fail(ISDF_ERR_INVALID, "res and parlength must be finite and positive");
-    if (path_off[0] != 0) return fail(ISDF_ERR_INVALID, "path_off[0] must be 0");
-    for (int b = 0; b < B; b++) if (path_off[b + 1] <= path_off[b]) return fail(ISDF_ERR_INVALID, "every path needs at least one node (path_off must increase)");
+    if (int r = offsets_check(path_off, B, "path_off", false)) return r;
     long long total = 0;
     wp_off[0] = 0;
     for (int b = 0; b < B; b++) {
@@ -2361,20 +2277,17 @@ static int midend_params_check(const isdf_midend_params *p) {
     return lbfgs_check(&p->lbfgs);
 }
 
-static int midend_check(isdf_ctx *c, int B, int N0, const isdf_midend_params *p) {
+// the mid-end's checks, in order: the batch (ragged: the *_ragged entry points' piece_off; else B problems of N0 pieces) and its sizes
+// into *L, the parameters, the shared-memory solver, the sharding
+static int midend_check(isdf_ctx *c, bool ragged, int B, int N0, const int32_t *piece_off, const isdf_midend_params *p, Layout *L) {
     if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
-    if (B < 1 || N0 < 1) return fail(ISDF_ERR_INVALID, "B < 1 or N0 < 1");
-    if ((long long)B * (4 * (long long)N0 - 3) > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "B*(4*N0-3) overflows");
-    if (int r = midend_params_check(p)) return r;
-    if (int r = minco_fits(N0)) return r;
-    if (c->world != 1) return fail(ISDF_ERR_STATE, "the mid-end shards by PROBLEM: keep isdf_set_shard(ctx, 0, 1) and give each rank its own problems");
-    return 0;
-}
-
-// midend_check for a ragged batch (the offsets in place of B, N0), and its sizes
-static int midend_ragged_check(isdf_ctx *c, int B, const int32_t *piece_off, const isdf_midend_params *p, Layout *L) {
-    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
-    if (int r = ragged_check(B, piece_off, L)) return r;
+    if (ragged) {
+        if (int r = ragged_check(B, piece_off, L)) return r;
+    } else {
+        if (B < 1 || N0 < 1) return fail(ISDF_ERR_INVALID, "B < 1 or N0 < 1");
+        if ((long long)B * (4 * (long long)N0 - 3) > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "B*(4*N0-3) overflows");
+        *L = uniform_layout(B, N0);
+    }
     if (int r = midend_params_check(p)) return r;
     if (int r = minco_fits(L->N)) return r;
     if (c->world != 1) return fail(ISDF_ERR_STATE, "the mid-end shards by PROBLEM: keep isdf_set_shard(ctx, 0, 1) and give each rank its own problems");
@@ -2422,43 +2335,37 @@ static int midend_upload(isdf_ctx *c, const Layout &L, int per_problem_bc, const
     return 0;
 }
 
-// the host form of one mid-end evaluation of a checked batch
-static int midend_callback_run(isdf_ctx *c, const Layout &L, int per_problem_bc, const isdf_midend_params *p, const double *head, const double *tail,
-                               const double *waypoints, const double *x, double *cost, double *grad) {
-    const int B = L.B;
-    const double *d_head, *d_tail, *d_wp;
-    if (int r = midend_upload(c, L, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return r;
-    CU_TRY(c->mid.d_x.upload(x, L.X, c->stream));
-    CU_TRY(c->mid.d_cost.ensure(B)); CU_TRY(c->mid.d_grad.ensure(L.X));
-    if (int r = midend_buffers(c, L)) return r;
-    if (int r = midend_eval_launch(c, L, d_head, d_tail, per_problem_bc ? 9 : 0, p, d_wp, c->mid.d_x.p, c->mid.d_cost.p, c->mid.d_grad.p, c->stream)) return r;
-    CU_TRY(cudaMemcpyAsync(cost, c->mid.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaMemcpyAsync(grad, c->mid.d_grad.p, sizeof(double) * L.X, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaStreamSynchronize(c->stream));
-    return 0;
+// the host form of one mid-end evaluation: inputs staged in c->mid (a ragged batch's offsets first), results copied back
+static int midend_callback_host(isdf_ctx *c, bool ragged, int B, int N0, const int32_t *piece_off, const double *head, const double *tail,
+                                int per_problem_bc, const isdf_midend_params *p, const double *waypoints, const double *x, double *cost, double *grad) {
+    return poison_on_failure([&]() -> int {
+        Layout L;
+        if (int r = midend_check(c, ragged, B, N0, piece_off, p, &L)) return r;
+        if (!head || !tail || !x || !cost || !grad || (L.P > (size_t)B && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        if (ragged) if (int r = ragged_upload(c->mid.d_off, piece_off, c->stream, &L)) return r;
+        const double *d_head, *d_tail, *d_wp;
+        if (int r = midend_upload(c, L, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return r;
+        CU_TRY(c->mid.d_x.upload(x, L.X, c->stream));
+        CU_TRY(c->mid.d_cost.ensure(B)); CU_TRY(c->mid.d_grad.ensure(L.X));
+        if (int r = midend_buffers(c, L)) return r;
+        if (int r = midend_eval_launch(c, L, d_head, d_tail, per_problem_bc ? 9 : 0, p, d_wp, c->mid.d_x.p, c->mid.d_cost.p, c->mid.d_grad.p, c->stream)) return r;
+        CU_TRY(cudaMemcpyAsync(cost, c->mid.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaMemcpyAsync(grad, c->mid.d_grad.p, sizeof(double) * L.X, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(cudaStreamSynchronize(c->stream));
+        return 0;
+    }, [&] { nan_fill(cost, B); });
 }
 
 extern "C" int isdf_midend_callback_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc,
                                           const isdf_midend_params *p, const double *waypoints, const double *x, double *cost, double *grad) {
-    return poison_on_failure([&]() -> int {
-        if (int r = midend_check(c, B, N0, p)) return r;
-        if (!head || !tail || !x || !cost || !grad || (N0 > 1 && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument");
-        if (set_device(c)) return ISDF_ERR_CUDA;
-        return midend_callback_run(c, uniform_layout(B, N0), per_problem_bc, p, head, tail, waypoints, x, cost, grad);
-    }, [&] { nan_fill(cost, B); });
+    return midend_callback_host(c, false, B, N0, nullptr, head, tail, per_problem_bc, p, waypoints, x, cost, grad);
 }
 
 extern "C" int isdf_midend_callback_batch_ragged(isdf_ctx *c, int B, const int32_t *piece_off, const double *head, const double *tail,
                                                  int per_problem_bc, const isdf_midend_params *p, const double *waypoints, const double *x,
                                                  double *cost, double *grad) {
-    return poison_on_failure([&]() -> int {
-        Layout L;
-        if (int r = midend_ragged_check(c, B, piece_off, p, &L)) return r;
-        if (!head || !tail || !x || !cost || !grad || (L.P > (size_t)B && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument");
-        if (set_device(c)) return ISDF_ERR_CUDA;
-        if (int r = ragged_upload(c->mid.d_off, piece_off, c->stream, &L)) return r;
-        return midend_callback_run(c, L, per_problem_bc, p, head, tail, waypoints, x, cost, grad);
-    }, [&] { nan_fill(cost, B); });
+    return midend_callback_host(c, true, B, 0, piece_off, head, tail, per_problem_bc, p, waypoints, x, cost, grad);
 }
 
 static int midend_batch_run(isdf_ctx *c, const Layout &L, const double *d_head, const double *d_tail, int per_problem_bc, const isdf_midend_params *p,
@@ -2490,74 +2397,70 @@ static int midend_batch_run(isdf_ctx *c, const Layout &L, const double *d_head, 
     return 0;
 }
 
+// the device form of getOriTraj on st; a ragged batch's offsets are uploaded first
+static int midend_device(isdf_ctx *c, bool ragged, int B, int N0, const int32_t *piece_off, const double *d_head, const double *d_tail, int per_problem_bc,
+                         const isdf_midend_params *p, const double *d_waypoints, double *d_x, double *d_T, double *d_coeffs, double *d_f, int32_t *d_ret,
+                         int32_t *d_iterations, int32_t *d_evaluations, int32_t *rounds, cudaStream_t st) {
+    return poison_on_failure([&]() -> int {
+        Layout L;
+        if (int r = midend_check(c, ragged, B, N0, piece_off, p, &L)) return r;
+        if (!d_head || !d_tail || !d_x || !d_f || (L.P > (size_t)B && !d_waypoints)) return fail(ISDF_ERR_INVALID, "NULL device pointer");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        if (ragged) if (int r = ragged_upload(c->mid.d_off, piece_off, st, &L)) return r;
+        return midend_batch_run(c, L, d_head, d_tail, per_problem_bc, p, d_waypoints, d_x, d_T, d_coeffs, d_f, d_ret, d_iterations, d_evaluations, rounds, st);
+    }, [&] { nan_fill_device(c, d_f, B, st); });
+}
+
 extern "C" int isdf_midend_batch_device(isdf_ctx *c, int B, int N0, const double *d_head, const double *d_tail, int per_problem_bc,
                                         const isdf_midend_params *p, const double *d_waypoints, double *d_x, double *d_T, double *d_coeffs,
                                         double *d_f, int32_t *d_ret, int32_t *d_iterations, int32_t *d_evaluations, int32_t *rounds, void *cuda_stream) {
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    return poison_on_failure([&]() -> int {
-        if (int r = midend_check(c, B, N0, p)) return r;
-        if (!d_head || !d_tail || !d_x || !d_f || (N0 > 1 && !d_waypoints)) return fail(ISDF_ERR_INVALID, "NULL device pointer");
-        return midend_batch_run(c, uniform_layout(B, N0), d_head, d_tail, per_problem_bc, p, d_waypoints, d_x, d_T, d_coeffs, d_f, d_ret, d_iterations,
-                                d_evaluations, rounds, st);
-    }, [&] { nan_fill_device(c, d_f, B, st); });
+    return midend_device(c, false, B, N0, nullptr, d_head, d_tail, per_problem_bc, p, d_waypoints, d_x, d_T, d_coeffs, d_f, d_ret, d_iterations,
+                         d_evaluations, rounds, (cudaStream_t)cuda_stream);
 }
 
 extern "C" int isdf_midend_batch_ragged_device(isdf_ctx *c, int B, const int32_t *piece_off, const double *d_head, const double *d_tail,
                                                int per_problem_bc, const isdf_midend_params *p, const double *d_waypoints, double *d_x, double *d_T,
                                                double *d_coeffs, double *d_f, int32_t *d_ret, int32_t *d_iterations, int32_t *d_evaluations,
                                                int32_t *rounds, void *cuda_stream) {
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    return poison_on_failure([&]() -> int {
-        Layout L;
-        if (int r = midend_ragged_check(c, B, piece_off, p, &L)) return r;
-        if (!d_head || !d_tail || !d_x || !d_f || (L.P > (size_t)B && !d_waypoints)) return fail(ISDF_ERR_INVALID, "NULL device pointer");
-        if (set_device(c)) return ISDF_ERR_CUDA;
-        if (int r = ragged_upload(c->mid.d_off, piece_off, st, &L)) return r;
-        return midend_batch_run(c, L, d_head, d_tail, per_problem_bc, p, d_waypoints, d_x, d_T, d_coeffs, d_f, d_ret, d_iterations, d_evaluations, rounds, st);
-    }, [&] { nan_fill_device(c, d_f, B, st); });
+    return midend_device(c, true, B, 0, piece_off, d_head, d_tail, per_problem_bc, p, d_waypoints, d_x, d_T, d_coeffs, d_f, d_ret, d_iterations,
+                         d_evaluations, rounds, (cudaStream_t)cuda_stream);
 }
 
-// the host form of getOriTraj for a checked batch: inputs staged in c->mid, results copied back
-static int midend_host_run(isdf_ctx *c, const Layout &L, int per_problem_bc, const isdf_midend_params *p, const double *head, const double *tail,
-                           const double *waypoints, double *x, double *T, double *coeffs, double *f, int32_t *ret, int32_t *iterations,
-                           int32_t *evaluations, int32_t *rounds) {
-    const int B = L.B;
-    isdf_ctx::LbfgsBufs &lb = c->mid.lb;
-    const size_t BN = L.P;
-    const double *d_head, *d_tail, *d_wp;
-    if (int r = midend_upload(c, L, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return r;
-    CU_TRY(lb.d_x.ensure(L.X)); CU_TRY(lb.d_f.ensure((size_t)19 * BN + B)); CU_TRY(lb.d_head.ensure((size_t)3 * B));
-    double *d_f = lb.d_f.p, *d_T = d_f + B, *d_C = d_T + BN;   // [f | T | coeffs]
-    int *d_i = lb.d_head.p;
-    if (int r = midend_batch_run(c, L, d_head, d_tail, per_problem_bc, p, d_wp, lb.d_x.p, d_T, d_C, d_f, d_i, d_i + B, d_i + 2 * (size_t)B,
-                                 rounds, c->stream)) return r;
-    if (T) CU_TRY(cudaMemcpy(T, d_T, sizeof(double) * BN, cudaMemcpyDeviceToHost));
-    if (coeffs) CU_TRY(cudaMemcpy(coeffs, d_C, sizeof(double) * 18 * BN, cudaMemcpyDeviceToHost));
-    return lbfgs_copy_out(lb, B, L.X, x, f, ret, iterations, evaluations);
+// the host form of getOriTraj: inputs staged in c->mid (a ragged batch's offsets first), results copied back
+static int midend_host(isdf_ctx *c, bool ragged, int B, int N0, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
+                       const isdf_midend_params *p, const double *waypoints, double *x, double *T, double *coeffs, double *f, int32_t *ret,
+                       int32_t *iterations, int32_t *evaluations, int32_t *rounds) {
+    return poison_on_failure([&]() -> int {
+        Layout L;
+        if (int r = midend_check(c, ragged, B, N0, piece_off, p, &L)) return r;
+        if (!head || !tail || !x || !f || (L.P > (size_t)B && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument");
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        if (ragged) if (int r = ragged_upload(c->mid.d_off, piece_off, c->stream, &L)) return r;
+        isdf_ctx::LbfgsBufs &lb = c->mid.lb;
+        const size_t BN = L.P;
+        const double *d_head, *d_tail, *d_wp;
+        if (int r = midend_upload(c, L, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return r;
+        CU_TRY(lb.d_x.ensure(L.X)); CU_TRY(lb.d_f.ensure((size_t)19 * BN + B)); CU_TRY(lb.d_head.ensure((size_t)3 * B));
+        double *d_f = lb.d_f.p, *d_T = d_f + B, *d_C = d_T + BN;   // [f | T | coeffs]
+        int *d_i = lb.d_head.p;
+        if (int r = midend_batch_run(c, L, d_head, d_tail, per_problem_bc, p, d_wp, lb.d_x.p, d_T, d_C, d_f, d_i, d_i + B, d_i + 2 * (size_t)B,
+                                     rounds, c->stream)) return r;
+        if (T) CU_TRY(cudaMemcpy(T, d_T, sizeof(double) * BN, cudaMemcpyDeviceToHost));
+        if (coeffs) CU_TRY(cudaMemcpy(coeffs, d_C, sizeof(double) * 18 * BN, cudaMemcpyDeviceToHost));
+        return lbfgs_copy_out(lb, B, L.X, x, f, ret, iterations, evaluations);
+    }, [&] { nan_fill(f, B); });
 }
 
 extern "C" int isdf_midend_batch(isdf_ctx *c, int B, int N0, const double *head, const double *tail, int per_problem_bc,
                                  const isdf_midend_params *p, const double *waypoints, double *x, double *T, double *coeffs,
                                  double *f, int32_t *ret, int32_t *iterations, int32_t *evaluations, int32_t *rounds) {
-    return poison_on_failure([&]() -> int {
-        if (int r = midend_check(c, B, N0, p)) return r;
-        if (!head || !tail || !x || !f || (N0 > 1 && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument");
-        if (set_device(c)) return ISDF_ERR_CUDA;
-        return midend_host_run(c, uniform_layout(B, N0), per_problem_bc, p, head, tail, waypoints, x, T, coeffs, f, ret, iterations, evaluations, rounds);
-    }, [&] { nan_fill(f, B); });
+    return midend_host(c, false, B, N0, nullptr, head, tail, per_problem_bc, p, waypoints, x, T, coeffs, f, ret, iterations, evaluations, rounds);
 }
 
 extern "C" int isdf_midend_batch_ragged(isdf_ctx *c, int B, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
                                         const isdf_midend_params *p, const double *waypoints, double *x, double *T, double *coeffs,
                                         double *f, int32_t *ret, int32_t *iterations, int32_t *evaluations, int32_t *rounds) {
-    return poison_on_failure([&]() -> int {
-        Layout L;
-        if (int r = midend_ragged_check(c, B, piece_off, p, &L)) return r;
-        if (!head || !tail || !x || !f || (L.P > (size_t)B && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument");
-        if (set_device(c)) return ISDF_ERR_CUDA;
-        if (int r = ragged_upload(c->mid.d_off, piece_off, c->stream, &L)) return r;
-        return midend_host_run(c, L, per_problem_bc, p, head, tail, waypoints, x, T, coeffs, f, ret, iterations, evaluations, rounds);
-    }, [&] { nan_fill(f, B); });
+    return midend_host(c, true, B, 0, piece_off, head, tail, per_problem_bc, p, waypoints, x, T, coeffs, f, ret, iterations, evaluations, rounds);
 }
 
 // ---- trajectory clearance check (isdf_clearance.cuh) -------------------------------------------------------------------------------
@@ -2570,11 +2473,32 @@ extern "C" int isdf_clearance_default_params(isdf_clearance_params *p) {
     return 0;
 }
 
-// number of trajectories of a call over N pieces with N0 pieces per trajectory (0 when N / N0 do not define one)
-static int traj_batch(int N, int N0) {
+// number of groups (trajectories, pose groups) of N pieces or poses with N0 per group, N0 = 0 for one group (0 when N / N0 define none)
+static int traj_batch(int64_t N, int64_t N0) {
     if (N < 1 || N0 < 0) return 0;
     if (N0 == 0) return 1;
-    return (N % N0 == 0) ? N / N0 : 0;
+    return (N % N0 == 0) ? (int)(N / N0) : 0;
+}
+
+// a clearance scan's reach and margin
+static int reach_margin_check(double reach, double margin) {
+    if (!(reach > 0.0) || !std::isfinite(reach)) return fail(ISDF_ERR_INVALID, "reach must be positive and finite");
+    if (std::isnan(margin) || margin > reach) return fail(ISDF_ERR_INVALID, "margin must not exceed reach");
+    return 0;
+}
+
+// a clearance scan's scene: an unsharded context, the map and the shape set, and the window of every `what` ("sample", "pose") within
+// the 1023-voxel limit
+static int clearance_scene_check(const isdf_ctx *c, double reach, const char *what) {
+    if (c->world > 1) return fail(ISDF_ERR_UNSUPPORTED, "the clearance check is not sharded: call it on a context with isdf_set_shard(ctx, 0, 1)");
+    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
+    if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
+    // the window spans at most 2 H sqrt(3) / res + 3 voxels per axis (rotated H box, one voxel of slack on each side); the 1023-voxel
+    // limit of the pose-window offsets applies as in the discrete path
+    const double H = c->dcfg.half_bd + reach;
+    if (2.0 * H * std::sqrt(3.0) / c->map.grid.res + 4.0 > (double)WINDOW_AXIS_MAX)
+        return fail(ISDF_ERR_INVALID, std::string("reach too large for this map resolution: a ") + what + " window would exceed 1023 voxels per axis");
+    return 0;
 }
 
 // every check that needs no device work, in the order of include/isdf.h's error list
@@ -2583,19 +2507,10 @@ static int clearance_check(isdf_ctx *c, int N, const isdf_clearance_params *p) {
     if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
     if (N < 1) return fail(ISDF_ERR_INVALID, "N < 1");
     if (p->samples_per_piece < 1) return fail(ISDF_ERR_INVALID, "samples_per_piece < 1");
-    if (!(p->reach > 0.0) || !std::isfinite(p->reach)) return fail(ISDF_ERR_INVALID, "reach must be positive and finite");
-    if (std::isnan(p->margin) || p->margin > p->reach) return fail(ISDF_ERR_INVALID, "margin must not exceed reach");
+    if (int r = reach_margin_check(p->reach, p->margin)) return r;
     if (traj_batch(N, p->pieces_per_traj) == 0) return fail(ISDF_ERR_INVALID, "pieces_per_traj must be 0 or divide N");
     if ((long long)N * (p->samples_per_piece + 1) > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "N * (samples_per_piece + 1) must fit in 31 bits");
-    if (c->world > 1) return fail(ISDF_ERR_UNSUPPORTED, "the clearance check is not sharded: call it on a context with isdf_set_shard(ctx, 0, 1)");
-    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
-    if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
-    // the window of a sample spans at most 2 H sqrt(3) / res + 3 voxels per axis (rotated H box, one voxel of slack on each side); the
-    // 1023-voxel limit of the pose-window offsets applies as in the discrete path
-    const double H = c->dcfg.half_bd + p->reach;
-    if (2.0 * H * std::sqrt(3.0) / c->map.grid.res + 4.0 > (double)WINDOW_AXIS_MAX)
-        return fail(ISDF_ERR_INVALID, "reach too large for this map resolution: a sample window would exceed 1023 voxels per axis");
-    return 0;
+    return clearance_scene_check(c, p->reach, "sample");
 }
 
 // a host trajectory block [coeffs 18N | T N] staged in buf on c->stream: the coefficients at buf.p, the durations at *d_T
@@ -2607,13 +2522,14 @@ static int stage_traj(isdf_ctx *c, DevBuf<double> &buf, int N, const double *T, 
     return 0;
 }
 
-// the clearance scan of the uniform samples of q over N pieces of (d_T, d_C); outputs, cursor, counters, hit flags and sample list are
-// the caller's
-static ClrArgs clearance_args(const isdf_ctx *c, int N, const double *d_T, const double *d_C, const isdf_clearance_params &q) {
+// the clearance scan of N sources in groups of N0 (0: one group) with reach and margin: the K + 1 uniform samples of each piece of
+// (d_T, d_C), or, with K = 0, poses the caller sets; outputs, cursor, counters, hit flags and sample list are the caller's
+static ClrArgs clearance_args(const isdf_ctx *c, int N, int K, int N0, double reach, double margin, const double *d_T = nullptr,
+                              const double *d_C = nullptr) {
     ClrArgs A = {};
     A.grid = c->map.grid; A.shape = c->mesh.shape; A.fp = c->dcfg.fp; A.half_bd = c->dcfg.half_bd;
-    A.reach = q.reach; A.margin = q.margin;
-    A.N = N; A.K = q.samples_per_piece; A.N0 = q.pieces_per_traj == 0 ? N : q.pieces_per_traj;
+    A.reach = reach; A.margin = margin;
+    A.N = N; A.K = K; A.N0 = N0 == 0 ? N : N0;
     A.T = d_T; A.C = d_C;
     return A;
 }
@@ -2624,6 +2540,17 @@ static int clearance_mode(const isdf_ctx *c) {
 static unsigned clearance_grid(const isdf_ctx *c, long long n) {
     const long long want = (n + CLR_WARPS - 1) / CLR_WARPS;
     return (unsigned)std::max<long long>(1, std::min(want, (long long)c->sm_count * c->clr_blocks));
+}
+
+// one clearance check on st: the cursor and counters reset, then the scan and summary kernels over n samples
+static int clearance_scan(isdf_ctx *c, ClrArgs &A, long long n, cudaStream_t st) {
+    CU_TRY(c->clr.d_cursor.ensure(1)); CU_TRY(c->clr.d_counters.ensure(2));
+    CU_TRY(cudaMemsetAsync(c->clr.d_cursor.p, 0, sizeof(int), st));
+    CU_TRY(cudaMemsetAsync(c->clr.d_counters.p, 0, 2 * sizeof(unsigned long long), st));
+    A.cursor = c->clr.d_cursor.p; A.counters = c->clr.d_counters.p;
+    CU_TRY(clearance_launch(A, clearance_mode(c), clearance_grid(c, n), st));
+    c->stats.kernel_launches += 2;   // scan kernel, summary kernel
+    return 0;
 }
 
 // on failure every summary reads "not shown to be free": min_clearance, t_min, first_hit NaN, voxel_min / piece_min / sample_min /
@@ -2656,15 +2583,10 @@ extern "C" int isdf_trajectory_clearance_device(isdf_ctx *c, int N, const double
         if (int r = clearance_check(c, N, p)) return r;
         if (!d_T || !d_coeffs || !d_sample_clearance || !d_sample_voxel || !d_summary) return fail(ISDF_ERR_INVALID, "NULL device pointer");
         if (set_device(c)) return ISDF_ERR_CUDA;
-        ClrArgs A = clearance_args(c, N, d_T, d_coeffs, *p);   // no sample list, no hit flags: the uniform samples of the definition
+        // no sample list, no hit flags: the uniform samples of the definition
+        ClrArgs A = clearance_args(c, N, p->samples_per_piece, p->pieces_per_traj, p->reach, p->margin, d_T, d_coeffs);
         A.clear = d_sample_clearance; A.voxel = (long long *)d_sample_voxel; A.summary = (ClrSummary *)d_summary;
-        CU_TRY(c->clr.d_cursor.ensure(1)); CU_TRY(c->clr.d_counters.ensure(2));
-        CU_TRY(cudaMemsetAsync(c->clr.d_cursor.p, 0, sizeof(int), st));
-        CU_TRY(cudaMemsetAsync(c->clr.d_counters.p, 0, 2 * sizeof(unsigned long long), st));
-        A.cursor = c->clr.d_cursor.p; A.counters = c->clr.d_counters.p;
-        CU_TRY(clearance_launch(A, clearance_mode(c), clearance_grid(c, (long long)N * (A.K + 1)), st));
-        c->stats.kernel_launches += 2;   // scan kernel, summary kernel
-        return 0;
+        return clearance_scan(c, A, (long long)N * (A.K + 1), st);
     }, [&] { if (c) write_failed_summaries(d_summary, p ? traj_batch(N, p->pieces_per_traj) : 0, clearance_failed_summary(), c, st); });
 }
 
@@ -2698,24 +2620,15 @@ extern "C" int isdf_pose_clearance_default_params(isdf_pose_clearance_params *p)
     return 0;
 }
 
-static int pose_groups(int64_t Q, int G) { return (Q < 1 || G < 0) ? 0 : G == 0 ? 1 : (Q % G == 0 ? (int)(Q / G) : 0); }
-
 static int pose_clearance_check(isdf_ctx *c, int64_t Q, const void *pos, const void *quat, int64_t stride, const isdf_pose_clearance_params *p) {
     if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
     if (!p || !pos || !quat) return fail(ISDF_ERR_INVALID, "NULL argument");
     if (Q < 1 || Q > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "Q must be in [1, 2^31)");
     if (stride < 1) return fail(ISDF_ERR_INVALID, "stride_doubles < 1");
-    if (!(p->reach > 0.0) || !std::isfinite(p->reach)) return fail(ISDF_ERR_INVALID, "reach must be positive and finite");
-    if (std::isnan(p->margin) || p->margin > p->reach) return fail(ISDF_ERR_INVALID, "margin must not exceed reach");
-    if (pose_groups(Q, p->poses_per_group) == 0) return fail(ISDF_ERR_INVALID, "poses_per_group must be 0 or divide Q");
+    if (int r = reach_margin_check(p->reach, p->margin)) return r;
+    if (traj_batch(Q, p->poses_per_group) == 0) return fail(ISDF_ERR_INVALID, "poses_per_group must be 0 or divide Q");
     if (p->reserved_ != 0) return fail(ISDF_ERR_INVALID, "reserved_ must be 0");
-    if (c->world > 1) return fail(ISDF_ERR_UNSUPPORTED, "the clearance check is not sharded: call it on a context with isdf_set_shard(ctx, 0, 1)");
-    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
-    if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
-    const double H = c->dcfg.half_bd + p->reach;
-    if (2.0 * H * std::sqrt(3.0) / c->map.grid.res + 4.0 > (double)WINDOW_AXIS_MAX)
-        return fail(ISDF_ERR_INVALID, "reach too large for this map resolution: a pose window would exceed 1023 voxels per axis");
-    return 0;
+    return clearance_scene_check(c, p->reach, "pose");
 }
 
 extern "C" int isdf_pose_clearance_device(isdf_ctx *c, int64_t Q, const double *d_pos, const double *d_quat, int64_t stride,
@@ -2726,20 +2639,11 @@ extern "C" int isdf_pose_clearance_device(isdf_ctx *c, int64_t Q, const double *
         if (int r = pose_clearance_check(c, Q, d_pos, d_quat, stride, p)) return r;
         if (!d_clear || !d_voxel || !d_summary) return fail(ISDF_ERR_INVALID, "NULL device pointer");
         if (set_device(c)) return ISDF_ERR_CUDA;
-        ClrArgs A = {};
-        A.grid = c->map.grid; A.shape = c->mesh.shape; A.fp = c->dcfg.fp; A.half_bd = c->dcfg.half_bd;
-        A.reach = p->reach; A.margin = p->margin;
-        A.N = (int)Q; A.K = 0; A.N0 = p->poses_per_group == 0 ? (int)Q : p->poses_per_group;   // one "sample" per pose
+        ClrArgs A = clearance_args(c, (int)Q, 0, p->poses_per_group, p->reach, p->margin);   // one "sample" per pose
         A.ppos = d_pos; A.pquat = d_quat; A.pstride = stride;
         A.clear = d_clear; A.voxel = (long long *)d_voxel; A.summary = (ClrSummary *)d_summary;
-        CU_TRY(c->clr.d_cursor.ensure(1)); CU_TRY(c->clr.d_counters.ensure(2));
-        CU_TRY(cudaMemsetAsync(c->clr.d_cursor.p, 0, sizeof(int), st));
-        CU_TRY(cudaMemsetAsync(c->clr.d_counters.p, 0, 2 * sizeof(unsigned long long), st));
-        A.cursor = c->clr.d_cursor.p; A.counters = c->clr.d_counters.p;
-        CU_TRY(clearance_launch(A, clearance_mode(c), clearance_grid(c, Q), st));
-        c->stats.kernel_launches += 2;   // scan kernel, summary kernel
-        return 0;
-    }, [&] { if (c) write_failed_summaries(d_summary, p ? pose_groups(Q, p->poses_per_group) : 0, clearance_failed_summary(), c, st); });
+        return clearance_scan(c, A, Q, st);
+    }, [&] { if (c) write_failed_summaries(d_summary, p ? traj_batch(Q, p->poses_per_group) : 0, clearance_failed_summary(), c, st); });
 }
 
 extern "C" int isdf_pose_clearance(isdf_ctx *c, int64_t Q, const double *pos, const double *quat, int64_t stride, const isdf_pose_clearance_params *p,
@@ -2748,7 +2652,7 @@ extern "C" int isdf_pose_clearance(isdf_ctx *c, int64_t Q, const double *pos, co
         if (int r = pose_clearance_check(c, Q, pos, quat, stride, p)) return r;
         if (!summary) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
-        const int B = pose_groups(Q, p->poses_per_group);
+        const int B = traj_batch(Q, p->poses_per_group);
         // the poses packed 7 doubles apart (x, y, z, w, qx, qy, qz) in one copy, then the device form
         std::vector<double> h((size_t)Q * 7);
         for (int64_t q = 0; q < Q; q++) {
@@ -2765,7 +2669,7 @@ extern "C" int isdf_pose_clearance(isdf_ctx *c, int64_t Q, const double *pos, co
         if (voxel) CU_TRY(cudaMemcpyAsync(voxel, c->clr.d_vox.p, sizeof(int64_t) * Q, cudaMemcpyDeviceToHost, c->stream));
         CU_TRY(cudaStreamSynchronize(c->stream));
         return 0;
-    }, [&] { write_failed_summaries(summary, p ? pose_groups(Q, p->poses_per_group) : 0, clearance_failed_summary()); });
+    }, [&] { write_failed_summaries(summary, p ? traj_batch(Q, p->poses_per_group) : 0, clearance_failed_summary()); });
 }
 
 // ---- continuous clearance certificate (isdf_certify.cuh) --------------------------------------------------------------------------
@@ -2908,7 +2812,7 @@ static int certify_run(isdf_ctx *c, int N, const double *d_T, const double *d_C,
     CU_TRY(certify_init_launch(A, st));
     c->stats.kernel_launches++;
     // the scan: round 0 is the clearance check's own uniform samples, later rounds the new midpoints
-    ClrArgs S = clearance_args(c, N, d_T, d_C, q);   // no counters: a certificate leaves isdf_dbg_clearance_counts as it was
+    ClrArgs S = clearance_args(c, N, K, q.pieces_per_traj, q.reach, q.margin, d_T, d_C);   // no counters: a certificate leaves isdf_dbg_clearance_counts as it was
     S.clear = z.d_sc.p; S.voxel = z.d_sv.p; S.cursor = z.d_cursor.p; S.hit = z.d_hit.p;
     auto scan = [&](long long n) -> int {
         CU_TRY(cudaMemsetAsync(z.d_cursor.p, 0, sizeof(int), st));
@@ -4054,7 +3958,7 @@ static int plan_check(isdf_ctx *c, const isdf_plan_params *p, double *r_cert) {
     if (!(std::isfinite(p->parlength) && p->parlength > 0.0)) return fail(ISDF_ERR_INVALID, "parlength must be finite and positive");
     if (!(std::isfinite(p->half_extent) && p->half_extent >= 0.0)) return fail(ISDF_ERR_INVALID, "half_extent must be finite and >= 0");
     for (double v : {p->offset[0], p->offset[1], p->offset[2], p->rho}) if (!std::isfinite(v)) return fail(ISDF_ERR_INVALID, "offset and rho must be finite");
-    if (int r = midend_check(c, 1, 1, &p->midend)) return r;
+    if (Layout L; int r = midend_check(c, false, 1, 1, nullptr, &p->midend, &L)) return r;
     if (int r = lbfgs_check(&p->backend)) return r;
     if (p->flags & ISDF_PLAN_CERTIFY) {
         if (p->certify.clearance.pieces_per_traj != 0) return fail(ISDF_ERR_INVALID, "certify.clearance.pieces_per_traj must be 0 (the call sets N0 = N)");
@@ -4195,7 +4099,7 @@ static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const
         for (int q = 0; q < Bg; q++) moff[q + 1] = moff[q] + N[idx[q]];
         const size_t MP = (size_t)moff[Bg];
         Layout ML;
-        if (int r = midend_ragged_check(c, Bg, moff.data(), &p->midend, &ML)) return r;
+        if (int r = midend_check(c, true, Bg, 0, moff.data(), &p->midend, &ML)) return r;
         if (int r = ragged_upload(c->mid.d_off, moff.data(), st, &ML)) return r;
         count_copy(c, cudaMemcpyHostToDevice, sizeof(int) * (2 * (size_t)Bg + 2));
         if (int r = plan_upload(c, z.d_idx, idx, st)) return r;
@@ -4259,7 +4163,7 @@ static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const
             CU_TRY(c->sv.set_durations(Bp, z.d_dur.p, st, cudaMemcpyDeviceToDevice));
             // 6. back end from the mid-end x
             Layout BL;
-            if (int r = callback_ragged_check(c, Bp, boff.data(), &BL)) return r;
+            if (int r = callback_batch_check(c, true, Bp, 0, boff.data(), &BL)) return r;
             if (int r = ragged_upload(c->batch.d_off, boff.data(), st, &BL)) return r;
             count_copy(c, cudaMemcpyHostToDevice, sizeof(int) * (2 * (size_t)Bp + 2));
             std::vector<int> bplan(Bp);
@@ -4520,8 +4424,7 @@ extern "C" int isdf_set_points_batch(isdf_ctx *c, int B, const int32_t *offsets,
     if (!c || B < 0 || (B > 0 && !offsets)) return fail(ISDF_ERR_INVALID, "bad argument");
     if (set_device(c)) return ISDF_ERR_CUDA;
     if (B == 0) { c->sv.B = 0; return 0; }
-    if (offsets[0] != 0) return fail(ISDF_ERR_INVALID, "offsets[0] must be 0");
-    for (int b = 0; b < B; b++) if (offsets[b + 1] < offsets[b]) return fail(ISDF_ERR_INVALID, "offsets must be non-decreasing");
+    if (int r = offsets_check(offsets, B, "offsets", true)) return r;
     if (offsets[B] > 0 && !pts) return fail(ISDF_ERR_INVALID, "pts is NULL");
     if (offsets[B] == 0) return fail(ISDF_ERR_INVALID, "no points at all: use B = 0 to switch the batched swept-volume term off");
     CU_TRY(c->sv.set_points_batch(B, offsets, pts, c->stream));

@@ -796,10 +796,7 @@ class Evaluator:
         B, dim = X.shape
         N0 = (dim + 3) // 4
         assert 4 * N0 - 3 == dim
-        head, tail = np.asarray(head, dtype=np.float64), np.asarray(tail, dtype=np.float64)
-        per = int(head.ndim == 3)
-        colmajor = (lambda a: np.ascontiguousarray(np.swapaxes(a, -1, -2)).reshape(-1))
-        h, t = colmajor(head), colmajor(tail)
+        per, h, t = self._bc(head, tail)
         cost, grad = np.zeros(B), np.zeros((B, dim))
         Xf = np.ascontiguousarray(X).reshape(-1)
         self._check(self.lib.isdf_callback_batch(self.h, B, N0, _dp(h), _dp(t), per, float(rho), _dp(Xf), _dp(cost), _dp(grad.reshape(-1))))
@@ -866,10 +863,7 @@ class Evaluator:
         X = _f64(X)
         B, dim = X.shape
         N0 = (dim + 3) // 4
-        head, tail = np.asarray(head, dtype=np.float64), np.asarray(tail, dtype=np.float64)
-        per = int(head.ndim == 3)
-        colmajor = (lambda a: np.ascontiguousarray(np.swapaxes(a, -1, -2)).reshape(-1))
-        h, t = colmajor(head), colmajor(tail)
+        per, h, t = self._bc(head, tail)
         x = np.ascontiguousarray(X).copy().reshape(-1)
         f = np.zeros(B)
         ret, it, evs = (np.zeros(B, dtype=np.int32) for _ in range(3))
@@ -960,10 +954,9 @@ class Evaluator:
 
     @staticmethod
     def _midend_args(head, tail, waypoints, B, N0):
-        head, tail = np.asarray(head, dtype=np.float64), np.asarray(tail, dtype=np.float64)
         wp = _f64(waypoints).reshape(-1)
         assert wp.size == 3 * B * (N0 - 1)
-        return int(head.ndim == 3), _colmajor(head), _colmajor(tail), (wp if wp.size else np.zeros(1))
+        return (*Evaluator._bc(head, tail), wp if wp.size else np.zeros(1))
 
     def midend_callback_batch(self, head, tail, waypoints, X, params=None):
         """OriTraj::costFunction for B problems: X (B, 4*N0-3), waypoints (B, N0-1, 3), head / tail (3,3) or (B,3,3) -> (cost[B], grad[B, 4*N0-3])"""

@@ -1,6 +1,6 @@
 """Every plan's obstacle list in one call (isdf_gather_obstacle_points_batch): bit-identical to one isdf_gather_obstacle_points per plan
-(points, order, counts) and to the reference-pinned oracle, on dense and cloud-built maps; the sizes reported when cap is too small; and
-set_as_points equal to isdf_set_points_batch with the same lists."""
+(points, order, counts) and to the reference-pinned oracle, on dense and cloud-built maps; the sizes reported when cap is too small, by the
+batch and by the single call; and set_as_points equal to isdf_set_points_batch with the same lists."""
 import ctypes as C
 import numpy as np
 import pytest
@@ -75,8 +75,31 @@ def test_batch_on_a_cloud_built_map():
     got = ev.gather_obstacle_points_batch(plans, 1.3, (0.1, 0.0, -0.2))
     ref = _singles(ev, plans, 1.3, (0.1, 0.0, -0.2))
     assert sum(len(g) for g in got) > 0
-    for g, r in zip(got, ref):
-        assert np.array_equal(g, r)
+    grid = ev.get_map_u8()                                                 # the oracle on the map the cloud built
+    for b, (g, r) in enumerate(zip(got, ref)):
+        assert np.array_equal(g, r), b
+        if len(plans[b]):
+            o, n = O.gather_obstacle_points(grid, lo, info["res"], plans[b], 1.3, (0.1, 0.0, -0.2))
+            assert n == len(g) and np.array_equal(g, o), b
+    ev.close()
+
+
+def test_single_call_cap_smaller_than_the_list():
+    """isdf_gather_obstacle_points with n > cap: *n is the whole list's size and the first cap points are written (0); with
+    set_as_points the same call fails with ISDF_ERR_INVALID"""
+    occ = W.three_slit_map(48, 48, 48, noise=0.05, seed=7)
+    ev = _ev()
+    ev.set_map_u8(occ, [0, 0, 0], 1.0)
+    wp = np.ascontiguousarray(_plans(3)[2])
+    full, n_full = ev.gather_obstacle_points(wp, 13.0 / 3.0)
+    assert n_full == len(full) > 10
+    ip, dp = C.POINTER(C.c_int32), C.POINTER(C.c_double)
+    for cap, set_as_points, code in ((5, 0, 0), (n_full - 1, 0, 0), (5, 1, -1)):
+        out, n = np.zeros((cap + 1, 3)), C.c_int(0)
+        r = ev.lib.isdf_gather_obstacle_points(ev.h, wp.ctypes.data_as(dp), len(wp), 13.0 / 3.0, None, out.ctypes.data_as(dp), cap, C.byref(n),
+                                               set_as_points)
+        assert r == code and n.value == n_full, (cap, set_as_points)
+        assert np.array_equal(out[:cap], full[:cap]) and not out[cap:].any()
     ev.close()
 
 
