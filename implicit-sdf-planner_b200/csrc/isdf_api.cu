@@ -18,6 +18,7 @@
 #include "isdf_states.cuh"
 #include "isdf_plan.cuh"
 #include "isdf_sim.cuh"
+#include "isdf_sense.cuh"
 #include <cub/device/device_scan.cuh>
 #include <queue>
 #include "isdf_host_mesh.cuh"
@@ -287,6 +288,7 @@ struct isdf_ctx {
         PinnedBuf<double> h;
         DevBuf<double> d_in, d_out;
     } exec;
+    SenseScene sense;   // depth sensing (isdf_sense.cuh): the scene cloud's bricks and the per-call scratch
     struct {   // peer-memory reduction (isdf_peer.cuh)
         DevBuf<char> buf;                    // own exchange buffer (exported through CUDA IPC)
         void *open[PEER_MAX] = {};           // peers' buffers opened here (null for self / unused)
@@ -1380,6 +1382,155 @@ extern "C" int isdf_simulate_device(isdf_ctx *c, int B, const int32_t *d_piece_o
     }, [&]() {
         if (c && d_summary && R > 0 && set_device(c) == 0 && sim_poison_launch(d_summary, R, st) == cudaSuccess) c->stats.kernel_launches++;
     });
+}
+
+// ---- depth sensing (isdf_sense.cuh, compiled in isdf_sense_tu.cu) ----
+extern "C" int isdf_sense_default_params(isdf_sense_params *p) {
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    std::memset(p, 0, sizeof(*p));
+    p->width = 640; p->height = 480;                                   // local_sensing/params/camera.yaml
+    p->fx = 387.229248046875; p->fy = 387.229248046875; p->cx = 321.04638671875; p->cy = 243.44969177246094;
+    const double cam02body[16] = {0, 0, 1, 0, -1, 0, 0, 0, 0, -1, 0, 0, 0, 0, 0, 1};   // pcl_render_node.cpp:347-350
+    std::memcpy(p->cam_to_body, cam02body, sizeof cam02body);
+    p->sensing_horizon = std::numeric_limits<double>::infinity();
+    return 0;
+}
+
+static int sense_cloud_set(isdf_ctx *c, const void *pts, int64_t n, int32_t stride, bool device, cudaStream_t st) {
+    if (int rc = cloud_args_check(c, pts, n, stride, 1.0)) return rc;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    c->sense.release();
+    DevBuf<char> d_pts;
+    const char *d = (const char *)pts;
+    int launches = 0;
+    cudaError_t e = cudaSuccess;
+    if (!device) {
+        e = d_pts.ensure((size_t)n * stride);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(d_pts.p, pts, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream);
+        d = d_pts.p; st = c->stream;
+    }
+    if (e == cudaSuccess) e = sense_set_cloud(c->sense, d, n, stride, st, &launches);
+    c->stats.kernel_launches += launches;
+    if (e != cudaSuccess) {
+        c->sense.release();
+        return fail(ISDF_ERR_CUDA, std::string("isdf_set_sense_cloud: ") + cudaGetErrorString(e));
+    }
+    return 0;
+}
+extern "C" int isdf_set_sense_cloud(isdf_ctx *c, const void *points, int64_t n, int32_t stride_bytes) {
+    return sense_cloud_set(c, points, n, stride_bytes, false, nullptr);
+}
+extern "C" int isdf_set_sense_cloud_device(isdf_ctx *c, const void *d_points, int64_t n, int32_t stride_bytes, void *cuda_stream) {
+    return sense_cloud_set(c, d_points, n, stride_bytes, true, (cudaStream_t)cuda_stream);
+}
+extern "C" int isdf_get_sense_info(isdf_ctx *c, isdf_sense_info *out) {
+    if (!c || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (!c->sense.have) return fail(ISDF_ERR_STATE, "no scene cloud: set one with isdf_set_sense_cloud");
+    out->points_used = c->sense.n; out->points_skipped = c->sense.skipped; out->bricks = c->sense.nb;
+    return 0;
+}
+
+// the checks every sensing call shares; the context (and its scene) last
+static int sense_args_check(isdf_ctx *c, int64_t Q, const void *pos, const void *quat, int64_t stride, const isdf_sense_params *p,
+                            const void *out) {
+    if (!pos || !quat || !p || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (Q < 1 || Q >= (1ll << 31)) return fail(ISDF_ERR_INVALID, "Q must be in [1, 2^31)");
+    if (stride < 1) return fail(ISDF_ERR_INVALID, "stride_doubles < 1");
+    if (p->width < 1 || p->height < 1 || (long long)p->width * p->height > (1ll << 26))
+        return fail(ISDF_ERR_INVALID, "width and height must be >= 1 with width x height <= 2^26");
+    if (!std::isfinite(p->fx) || !std::isfinite(p->fy) || !std::isfinite(p->cx) || !std::isfinite(p->cy))
+        return fail(ISDF_ERR_INVALID, "a camera parameter is not finite");
+    if (!(p->fx > 0 && p->fy > 0)) return fail(ISDF_ERR_INVALID, "fx and fy must be positive");
+    for (int i = 0; i < 16; i++) if (!std::isfinite(p->cam_to_body[i])) return fail(ISDF_ERR_INVALID, "a cam_to_body entry is not finite");
+    if (p->cam_to_body[12] != 0 || p->cam_to_body[13] != 0 || p->cam_to_body[14] != 0 || p->cam_to_body[15] != 1)
+        return fail(ISDF_ERR_INVALID, "cam_to_body's last row must be (0, 0, 0, 1)");
+    if (!(p->sensing_horizon > 0)) return fail(ISDF_ERR_INVALID, "sensing_horizon must be positive (+Inf keeps every point)");
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (!c->sense.have) return fail(ISDF_ERR_STATE, "no scene cloud: set one with isdf_set_sense_cloud");
+    return 0;
+}
+
+// the host form's poses, packed as (pos, quat) records of 7 doubles on the context's stream
+static int sense_stage_poses(isdf_ctx *c, int64_t Q, const double *pos, const double *quat, int64_t stride, SenseCall *C) {
+    auto &x = c->exec;
+    CU_TRY(x.h.ensure(7 * (size_t)Q)); CU_TRY(x.d_in.ensure(7 * (size_t)Q));
+    for (int64_t q = 0; q < Q; q++) {
+        std::memcpy(x.h.p + 7 * q, pos + q * stride, 3 * sizeof(double));
+        std::memcpy(x.h.p + 7 * q + 3, quat + q * stride, 4 * sizeof(double));
+    }
+    CU_TRY(cudaMemcpyAsync(x.d_in.p, x.h.p, 7 * sizeof(double) * Q, cudaMemcpyHostToDevice, c->stream));
+    C->pos = x.d_in.p; C->quat = x.d_in.p + 3; C->stride = 7;
+    return 0;
+}
+
+static int sense_depth_impl(isdf_ctx *c, int64_t Q, const double *pos, const double *quat, int64_t stride, const isdf_sense_params *p,
+                            int32_t *depth, bool device, cudaStream_t st) {
+    if (int rc = sense_args_check(c, Q, pos, quat, stride, p, depth)) return rc;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    SenseCall C{Q, pos, quat, stride, *p};
+    if (!device) {
+        if (int rc = sense_stage_poses(c, Q, pos, quat, stride, &C)) return rc;
+        st = c->stream;
+    }
+    int launches = 0;
+    const cudaError_t e = sense_depth_run(c->sense, C, depth, device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st, &launches);
+    c->stats.kernel_launches += launches;
+    if (e != cudaSuccess) return fail(ISDF_ERR_CUDA, std::string("isdf_sense_depth: ") + cudaGetErrorString(e));
+    if (!device) CU_TRY(cudaStreamSynchronize(st));
+    return 0;
+}
+extern "C" int isdf_sense_depth(isdf_ctx *c, int64_t Q, const double *pos, const double *quat, int64_t stride_doubles,
+                                const isdf_sense_params *p, int32_t *depth) {
+    return sense_depth_impl(c, Q, pos, quat, stride_doubles, p, depth, false, nullptr);
+}
+extern "C" int isdf_sense_depth_device(isdf_ctx *c, int64_t Q, const double *d_pos, const double *d_quat, int64_t stride_doubles,
+                                       const isdf_sense_params *p, int32_t *d_depth, void *cuda_stream) {
+    return sense_depth_impl(c, Q, d_pos, d_quat, stride_doubles, p, d_depth, true, (cudaStream_t)cuda_stream);
+}
+
+static int sense_cloud_impl(isdf_ctx *c, int64_t Q, const double *pos, const double *quat, int64_t stride, const isdf_sense_params *p,
+                            int64_t cap, float *points, int64_t *offsets, bool device, cudaStream_t st) {
+    if (int rc = sense_args_check(c, Q, pos, quat, stride, p, offsets)) return rc;
+    if (cap < 0 || (cap > 0 && !points)) return fail(ISDF_ERR_INVALID, "cap < 0, or points NULL with cap > 0");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    SenseCall C{Q, pos, quat, stride, *p};
+    float *d_points = points;
+    int64_t *d_off = offsets;
+    DevBuf<float> s_points; DevBuf<int64_t> s_off;
+    if (!device) {
+        if (int rc = sense_stage_poses(c, Q, pos, quat, stride, &C)) return rc;
+        st = c->stream;
+        CU_TRY(s_off.ensure(Q + 1));
+        if (cap > 0) CU_TRY(s_points.ensure(3 * (size_t)cap));
+        d_points = s_points.p; d_off = s_off.p;
+    }
+    int launches = 0;
+    const cudaError_t e = sense_cloud_run(c->sense, C, d_points, cap, d_off, st, &launches);
+    c->stats.kernel_launches += launches;
+    if (e != cudaSuccess) return fail(ISDF_ERR_CUDA, std::string("isdf_sense_cloud: ") + cudaGetErrorString(e));
+    int64_t total = 0;
+    CU_TRY(cudaMemcpyAsync(&total, d_off + Q, sizeof total, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    if (!device) {
+        CU_TRY(cudaMemcpy(offsets, d_off, sizeof(int64_t) * (Q + 1), cudaMemcpyDeviceToHost));
+        if (std::min(total, cap) > 0) CU_TRY(cudaMemcpy(points, d_points, 3 * sizeof(float) * std::min(total, cap), cudaMemcpyDeviceToHost));
+    }
+    if (total > cap) return fail(ISDF_ERR_INVALID, "cap smaller than the sensed points (offsets report the sizes)");
+    return 0;
+}
+extern "C" int isdf_sense_cloud(isdf_ctx *c, int64_t Q, const double *pos, const double *quat, int64_t stride_doubles,
+                                const isdf_sense_params *p, int64_t cap, float *points, int64_t *offsets) {
+    return sense_cloud_impl(c, Q, pos, quat, stride_doubles, p, cap, points, offsets, false, nullptr);
+}
+extern "C" int isdf_sense_cloud_device(isdf_ctx *c, int64_t Q, const double *d_pos, const double *d_quat, int64_t stride_doubles,
+                                       const isdf_sense_params *p, int64_t cap, float *d_points, int64_t *d_offsets, void *cuda_stream) {
+    return sense_cloud_impl(c, Q, d_pos, d_quat, stride_doubles, p, cap, d_points, d_offsets, true, (cudaStream_t)cuda_stream);
+}
+// diagnostics (not in include/isdf.h): render at most `poses` poses per chunk (0: the automatic chunking)
+extern "C" int isdf_dbg_sense_chunk(isdf_ctx *c, int poses) {
+    if (!c || poses < 0) return fail(ISDF_ERR_INVALID, "bad argument");
+    c->sense.chunk_override = poses;
+    return 0;
 }
 
 // getPointsInAABB (pcs:148-170): one CTA; thread = (x, y) row of the clamped index box — popcount of the row's z-run, block-wide exclusive scan

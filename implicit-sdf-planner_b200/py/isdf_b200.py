@@ -47,7 +47,9 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_frontend_path_pairs", "isdf_frontend_path_pairs_device", "isdf_frontend_path_fields_device", "isdf_plan_pairs",
                "isdf_path_waypoints_device", "isdf_plan_pairs_device", "isdf_plan_batch_device",
                "isdf_sim_default_params", "isdf_simulate", "isdf_simulate_device",
-               "isdf_pose_clearance_default_params", "isdf_pose_clearance", "isdf_pose_clearance_device"]
+               "isdf_pose_clearance_default_params", "isdf_pose_clearance", "isdf_pose_clearance_device",
+               "isdf_sense_default_params", "isdf_set_sense_cloud", "isdf_set_sense_cloud_device", "isdf_get_sense_info",
+               "isdf_sense_depth", "isdf_sense_depth_device", "isdf_sense_cloud", "isdf_sense_cloud_device"]
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
 DYN_QUANTITIES = ["speed", "acceleration", "body_rate", "tilt", "thrust"]   # q of isdf_dynamics_summary; mask bit 5: the thrust minimum
@@ -82,6 +84,73 @@ def decode_sim_summaries(raw):
     """(R, 88) uint8 rows (a numpy array or a tensor) of isdf_sim_summary records -> list of dicts"""
     b = np.ascontiguousarray(raw.cpu().numpy() if hasattr(raw, "cpu") else raw, dtype=np.uint8).reshape(-1, C.sizeof(SimSummary))
     return [SimSummary.from_buffer_copy(row.tobytes()).as_dict() for row in b]
+
+
+def _cloud_records(points, stride_bytes):
+    """(contiguous array, n, stride) of a host cloud: (n, k >= 3) float32, or a flat float32 / uint8 buffer of stride_bytes records"""
+    pts = np.asarray(points)
+    if pts.dtype == np.float32 and pts.ndim == 2:
+        if pts.shape[1] < 3:
+            raise ValueError("points need at least 3 columns (x, y, z)")
+        pts = np.ascontiguousarray(pts)
+        stride = pts.shape[1] * 4 if stride_bytes is None else int(stride_bytes)
+        if stride != pts.shape[1] * 4:
+            raise ValueError("stride_bytes must equal the row size of a 2-D points array")
+        return pts, pts.shape[0], stride
+    if pts.dtype in (np.float32, np.uint8) and pts.ndim == 1:
+        if stride_bytes is None:
+            raise ValueError("a flat record buffer needs stride_bytes")
+        pts = np.ascontiguousarray(pts)
+        stride = int(stride_bytes)
+        return pts, (pts.nbytes // stride if stride > 0 else 0), stride
+    raise TypeError(f"points must be float32 (n, k>=3) or a flat float32/uint8 record buffer, got {pts.dtype} {pts.shape}")
+
+
+def _cloud_records_device(points, n, stride_bytes):
+    """(device pointer, n, stride) of a device cloud: a contiguous float32 tensor (n, k >= 3), or a raw pointer with n and stride_bytes"""
+    if hasattr(points, "data_ptr"):
+        if str(points.dtype) != "torch.float32" or points.dim() != 2 or points.shape[1] < 3:
+            raise TypeError(f"points must be a float32 (n, k>=3) tensor, got {points.dtype} {tuple(points.shape)}")
+        if not points.is_contiguous():
+            raise ValueError("points must be contiguous")
+        stride = points.shape[1] * 4
+        if stride_bytes is not None and int(stride_bytes) != stride:
+            raise ValueError("stride_bytes must equal the row size of a points tensor")
+        return points.data_ptr(), points.shape[0], stride
+    if n is None or stride_bytes is None:
+        raise ValueError("a raw device pointer needs n and stride_bytes")
+    return int(points), n, int(stride_bytes)
+
+
+def _cuda_records(records):
+    """a float64 CUDA tensor of pose records as (Q, stride) with unit stride along a record"""
+    if not (hasattr(records, "is_cuda") and records.is_cuda and str(records.dtype) == "torch.float64"):
+        raise TypeError("records must be a float64 CUDA tensor")
+    r = records.reshape(-1, records.shape[-1])
+    if r.stride(1) != 1:
+        r = r.contiguous()
+    if r.shape[0] > 1 and r.stride(0) != r.shape[1]:
+        r = r.contiguous()
+    return r
+
+
+def sense_params(**kw):
+    """isdf_sense_params: the reference's camera (isdf_sense_default_params) with the given fields replaced; cam_to_body takes 16
+    row-major values or a 4 x 4 array"""
+    p = SenseParams()
+    r = load_library().isdf_sense_default_params(C.byref(p))
+    if r != 0:
+        raise IsdfError(r, "isdf_sense_default_params")
+    for k, v in kw.items():
+        if not hasattr(p, k):
+            raise AttributeError(k)
+        if k == "cam_to_body":
+            v = np.asarray(v, dtype=np.float64).reshape(16)
+            for i in range(16):
+                p.cam_to_body[i] = float(v[i])
+        else:
+            setattr(p, k, type(getattr(p, k))(v))
+    return p
 
 
 def sim_default_params(**kw):
@@ -164,6 +233,17 @@ class ClearanceParams(C.Structure):
 class PoseClearanceParams(C.Structure):
     """isdf_pose_clearance_params"""
     _fields_ = [("reach", C.c_double), ("margin", C.c_double), ("poses_per_group", C.c_int32), ("reserved_", C.c_int32)]
+
+
+class SenseParams(C.Structure):
+    """isdf_sense_params"""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
+                ("cam_to_body", C.c_double * 16), ("sensing_horizon", C.c_double)]
+
+
+class SenseInfo(C.Structure):
+    """isdf_sense_info"""
+    _fields_ = [("points_used", C.c_int64), ("points_skipped", C.c_int64), ("bricks", C.c_int64)]
 
 
 class ClearanceSummary(C.Structure):
@@ -443,6 +523,15 @@ def load_library(path=None):
     lib.isdf_pose_clearance_default_params.argtypes = [pcp]
     lib.isdf_pose_clearance.argtypes = [vp, C.c_int64, dp, dp, C.c_int64, pcp, dp, C.POINTER(C.c_int64), C.POINTER(ClearanceSummary)]
     lib.isdf_pose_clearance_device.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, pcp, vp, vp, vp, vp]
+    sep = C.POINTER(SenseParams)
+    lib.isdf_sense_default_params.argtypes = [sep]
+    lib.isdf_set_sense_cloud.argtypes = [vp, vp, C.c_int64, C.c_int32]
+    lib.isdf_set_sense_cloud_device.argtypes = [vp, vp, C.c_int64, C.c_int32, vp]
+    lib.isdf_get_sense_info.argtypes = [vp, C.POINTER(SenseInfo)]
+    lib.isdf_sense_depth.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, vp]
+    lib.isdf_sense_depth_device.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, vp, vp]
+    lib.isdf_sense_cloud.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, C.c_int64, vp, vp]
+    lib.isdf_sense_cloud_device.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, C.c_int64, vp, vp, vp]
     spp = C.POINTER(SimParams)
     lib.isdf_sim_default_params.argtypes = [spp]
     lib.isdf_simulate.argtypes = [vp, C.c_int, ip, dp, dp, C.c_int, ip, dp, dp, spp, C.c_int, dp, C.POINTER(SimSummary)]
@@ -636,40 +725,116 @@ class Evaluator:
         """the occupancy grid from a float32 point cloud (PCSmapManager::rcvGlobalMapHandler; see isdf_set_map_cloud in include/isdf.h).
         points: (n, 3) or (n, k >= 3) float32 with x, y, z in the first three columns, or a 1-D float32 / uint8 buffer of n records of
         stride_bytes each (a PointCloud2's data with point_step). Any other dtype raises rather than being rounded silently."""
-        pts = np.asarray(points)
-        if pts.dtype == np.float32 and pts.ndim == 2:
-            if pts.shape[1] < 3:
-                raise ValueError("points need at least 3 columns (x, y, z)")
-            pts = np.ascontiguousarray(pts)
-            stride = pts.shape[1] * 4 if stride_bytes is None else int(stride_bytes)
-            if stride != pts.shape[1] * 4:
-                raise ValueError("stride_bytes must equal the row size of a 2-D points array")
-            n = pts.shape[0]
-        elif pts.dtype in (np.float32, np.uint8) and pts.ndim == 1:
-            if stride_bytes is None:
-                raise ValueError("a flat record buffer needs stride_bytes")
-            pts = np.ascontiguousarray(pts)
-            stride = int(stride_bytes)
-            n = pts.nbytes // stride if stride > 0 else 0
-        else:
-            raise TypeError(f"points must be float32 (n, k>=3) or a flat float32/uint8 record buffer, got {pts.dtype} {pts.shape}")
+        pts, n, stride = _cloud_records(points, stride_bytes)
         self._check(self.lib.isdf_set_map_cloud(self.h, pts.ctypes.data_as(C.c_void_p) if n else None, n, stride, float(res), int(sta_threshold)))
 
     def set_map_cloud_device(self, points, n=None, stride_bytes=None, res=1.0, sta_threshold=1, stream=0):
         """points on the context's device: a float32 torch tensor (n, k >= 3), contiguous, or a raw device pointer with n and stride_bytes"""
-        if hasattr(points, "data_ptr"):
-            if str(points.dtype) != "torch.float32" or points.dim() != 2 or points.shape[1] < 3:
-                raise TypeError(f"points must be a float32 (n, k>=3) tensor, got {points.dtype} {tuple(points.shape)}")
-            if not points.is_contiguous():
-                raise ValueError("points must be contiguous")
-            ptr, n, stride = points.data_ptr(), points.shape[0], points.shape[1] * 4
-            if stride_bytes is not None and int(stride_bytes) != stride:
-                raise ValueError("stride_bytes must equal the row size of a points tensor")
-        else:
-            if n is None or stride_bytes is None:
-                raise ValueError("a raw device pointer needs n and stride_bytes")
-            ptr, stride = int(points), int(stride_bytes)
+        ptr, n, stride = _cloud_records_device(points, n, stride_bytes)
         self._check(self.lib.isdf_set_map_cloud_device(self.h, C.c_void_p(ptr), int(n), stride, float(res), int(sta_threshold), C.c_void_p(stream)))
+
+    # ---- depth sensing (isdf_sense_*): the scene cloud, depth images and sensed points at poses read in place ----
+    def set_sense_cloud(self, points, stride_bytes=None):
+        """the scene the camera sees: points as set_map_cloud takes them (records with a NaN or Inf coordinate are skipped)"""
+        pts, n, stride = _cloud_records(points, stride_bytes)
+        self._check(self.lib.isdf_set_sense_cloud(self.h, pts.ctypes.data_as(C.c_void_p) if n else None, n, stride))
+
+    def set_sense_cloud_device(self, points, n=None, stride_bytes=None, stream=0):
+        """the scene on the context's device, as set_map_cloud_device takes it"""
+        ptr, n, stride = _cloud_records_device(points, n, stride_bytes)
+        self._check(self.lib.isdf_set_sense_cloud_device(self.h, C.c_void_p(ptr), int(n), stride, C.c_void_p(stream)))
+
+    def sense_info(self):
+        """dict(points_used, points_skipped, bricks) of the scene cloud"""
+        i = SenseInfo()
+        self._check(self.lib.isdf_get_sense_info(self.h, C.byref(i)))
+        return {n: getattr(i, n) for n, _ in i._fields_}
+
+    @staticmethod
+    def _pose_records(r, pos_offset, quat_offset):
+        Q, stride = r.shape
+        if not (0 <= pos_offset <= stride - 3 and 0 <= quat_offset <= stride - 4):
+            raise ValueError("pos_offset / quat_offset outside the record")
+        return Q, stride
+
+    def sense_depth(self, records, pos_offset=0, quat_offset=3, params=None, **kw):
+        """depth images (Q, H, W) int32 in mm (999999: nothing seen) at Q poses read in place from records (Q, stride) float64, as
+        pose_clearance reads them (a simulate log: offsets 1 and 7; trajectory_states records: 0 and 12). params: sense_params(**kw)."""
+        p = params if params is not None else sense_params(**kw)
+        r = _f64(records)
+        r = r.reshape(-1, r.shape[-1])
+        Q, stride = self._pose_records(r, pos_offset, quat_offset)
+        out = np.empty((Q, max(p.height, 0), max(p.width, 0)), dtype=np.int32)   # bad sizes are the library's to refuse
+        base = r.ctypes.data
+        self._check(self.lib.isdf_sense_depth(self.h, Q, C.c_void_p(base + 8 * pos_offset), C.c_void_p(base + 8 * quat_offset), stride,
+                                              C.byref(p), out.ctypes.data_as(C.c_void_p)))
+        return out
+
+    def sense_depth_device(self, records, pos_offset=0, quat_offset=3, params=None, stream=None, **kw):
+        """sense_depth on a float64 CUDA tensor (Q, stride) (rows may be strided views of a larger record, e.g. a simulate log reshaped to
+        (R * n_log, 21)) -> (Q, H, W) int32 CUDA tensor, on torch's current stream"""
+        import torch
+        p = params if params is not None else sense_params(**kw)
+        r = _cuda_records(records)
+        Q, stride = self._pose_records(r, pos_offset, quat_offset)
+        s = torch.cuda.current_stream(r.device) if stream is None else stream
+        with torch.cuda.stream(s):
+            out = torch.empty((Q, max(p.height, 0), max(p.width, 0)), dtype=torch.int32, device=r.device)
+        base = r.data_ptr()
+        self._check(self.lib.isdf_sense_depth_device(self.h, Q, C.c_void_p(base + 8 * pos_offset), C.c_void_p(base + 8 * quat_offset), stride,
+                                                     C.byref(p), C.c_void_p(out.data_ptr()), C.c_void_p(s.cuda_stream)))
+        return out
+
+    def sense_cloud(self, records, pos_offset=0, quat_offset=3, params=None, cap=None, **kw):
+        """the sensed points of Q poses -> (points (M, 3) float32, offsets (Q + 1) int64): pose q's in rows [offsets[q], offsets[q+1]).
+        cap: rows to allocate (default 2^22); too small, the call is repeated once with the total the first call reported."""
+        p = params if params is not None else sense_params(**kw)
+        r = _f64(records)
+        r = r.reshape(-1, r.shape[-1])
+        Q, stride = self._pose_records(r, pos_offset, quat_offset)
+        cap = min(Q * p.width * p.height, 1 << 22) if cap is None else int(cap)
+        base = r.ctypes.data
+        off = np.zeros(Q + 1, dtype=np.int64)
+        for attempt in range(2):
+            pts = np.empty((max(cap, 1), 3), dtype=np.float32)
+            rc = self.lib.isdf_sense_cloud(self.h, Q, C.c_void_p(base + 8 * pos_offset), C.c_void_p(base + 8 * quat_offset), stride, C.byref(p),
+                                           cap, pts.ctypes.data_as(C.c_void_p), off.ctypes.data_as(C.c_void_p))
+            if rc == 0:
+                return pts[:off[Q]], off
+            if attempt == 0 and off[Q] > cap:
+                cap = int(off[Q])
+                continue
+            self._check(rc)
+
+    def sense_cloud_device(self, records, pos_offset=0, quat_offset=3, params=None, cap=None, stream=None, **kw):
+        """sense_cloud on a float64 CUDA tensor (Q, stride) -> (points (M, 3) float32 CUDA tensor, offsets (Q + 1) int64 CUDA tensor), on
+        torch's current stream. points goes into set_map_cloud_device as it is. Caps as in sense_cloud."""
+        import torch
+        p = params if params is not None else sense_params(**kw)
+        r = _cuda_records(records)
+        Q, stride = self._pose_records(r, pos_offset, quat_offset)
+        cap = min(Q * p.width * p.height, 1 << 22) if cap is None else int(cap)
+        s = torch.cuda.current_stream(r.device) if stream is None else stream
+        base = r.data_ptr()
+        for attempt in range(2):
+            with torch.cuda.stream(s):
+                pts = torch.empty((max(cap, 1), 3), dtype=torch.float32, device=r.device)
+                off = torch.zeros(Q + 1, dtype=torch.int64, device=r.device)
+            rc = self.lib.isdf_sense_cloud_device(self.h, Q, C.c_void_p(base + 8 * pos_offset), C.c_void_p(base + 8 * quat_offset), stride,
+                                                  C.byref(p), cap, C.c_void_p(pts.data_ptr()), C.c_void_p(off.data_ptr()),
+                                                  C.c_void_p(s.cuda_stream))
+            if rc == 0:
+                return pts[:int(off[Q])], off
+            total = int(off[Q])
+            if attempt == 0 and total > cap:
+                cap = total
+                continue
+            self._check(rc)
+
+    def dbg_sense_chunk(self, poses):
+        """render at most `poses` poses per chunk (0: automatic; isdf_dbg_sense_chunk, not part of include/isdf.h)"""
+        self.lib.isdf_dbg_sense_chunk.argtypes = [C.c_void_p, C.c_int]
+        self._check(self.lib.isdf_dbg_sense_chunk(self.h, int(poses)))
 
     def map_info(self):
         """isdf_map_info of the current map as a dict(dims, res, bmin, bmax, occupied_voxels, points_used, points_skipped)"""

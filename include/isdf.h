@@ -1117,6 +1117,73 @@ int isdf_simulate_device(isdf_ctx *ctx, int B, const int32_t *d_piece_off, const
                          const int32_t *d_traj, const double *d_init, const double *d_dist, const isdf_sim_params *p, int cap_log,
                          double *d_log, isdf_sim_summary *d_summary, void *cuda_stream);
 
+/* ---- depth sensing: the reference's depth camera (uav_simulator/local_sensing) batched over poses ---------------------------------
+ * Scene. isdf_set_sense_cloud / _device take the records isdf_set_map_cloud takes (float32 x, y, z at byte offsets 0, 4, 8 of each
+ *   stride_bytes record, with the same validation). Records with a NaN or Inf coordinate are skipped and counted (isdf_get_sense_info); on
+ *   the GPU the reference's kernel would instead truncate such a point to pixel (0, 0) at depth 0. The context owns the cloud and gives it
+ *   up before it is overwritten and on destroy. The device form reads d_points on cuda_stream and returns when the scene is built.
+ * Camera (isdf_sense_params). isdf_sense_default_params gives local_sensing/params/camera.yaml: 640 x 480, fx = fy = 387.229248046875,
+ *   cx = 321.04638671875, cy = 243.44969177246094; cam_to_body = cam02body of pcl_render_node.cpp:347-350 (row-major
+ *   [0 0 1 0; -1 0 0 0; 0 -1 0 0; 0 0 0 1]: the camera looks along the body's x axis); sensing_horizon = +Inf, since no launch file of the
+ *   reference sets one (the node then reads an unset double).
+ * Poses. Pose q is the position at pos + q stride_doubles and the quaternion (w, x, y, z) at quat + q stride_doubles, R = quat_rot as
+ *   isdf_pose_points, so isdf_simulate's log (pos = log + 1, quat = log + 7, stride ISDF_SIM_DOUBLES) and isdf_trajectory_states' records
+ *   are read in place. In FP64, nothing contracted:
+ *     cam2world[i][j] = ((B[i][0] C[0][j] + B[i][1] C[1][j]) + B[i][2] C[2][j]) + B[i][3] C[3][j], B = [R pos; 0 0 0 1], C = cam_to_body
+ *     (exact with the default C, whose entries are 0 and +-1);
+ *     the render's camera-from-world is the rigid inverse: r[i][j] = cam2world[j][i], t[i] = -((r[i][0] c0 + r[i][1] c1) + r[i][2] c2) with
+ *     c = cam2world's translation, then every entry rounded to FP32 as the reference's Parameter holds it. The reference takes Eigen's
+ *     general 4 x 4 inverse; the two may differ in the last FP64 bits before that rounding. From the rounded matrix on, this is the
+ *     reference's arithmetic bit for bit.
+ * Depth image (depth_render.cu:2-56), all in FP32 unless said: every pixel starts at 999999. For each scene point p:
+ *     x = fma(p.z, r02, fma(p.x, r00, p.y r01)) + t0 (FMUL, FFMA, FFMA, FADD as the reference build contracts it), and likewise y,
+ *     z; rejected when z <= 0;
+ *     px = trunc((double)fma(x / z, fx, cx) + 0.5), py likewise with y, fy, cy (IEEE division, FP64 add, truncation toward zero that
+ *     saturates and takes NaN to 0); rejected when px or py falls outside the image, even when the splat would reach in (a centre in
+ *     (-1, 0) truncates to 0 and is kept);
+ *     dist_mm = trunc(fma(z, 1000, 0.5)); r = trunc(0.0573 (double)fx / (double)z + 0.5) in FP64;
+ *     every pixel of the (2r + 1)^2 square around (px, py) inside the image takes min(pixel, dist_mm).
+ *   fx, fy, cx, cy are the FP32 roundings of the parameters here. The image is a min over integers, so it does not depend on any order.
+ * Sensed points (pcl_render_node.cpp:224-258, 286-296): for u = 0 .. W - 1, then v = 0 .. H - 1 within it: depth = (float)mm / 1000.0f,
+ *   0 when depth >= 500 (or NaN); a depth of 0 is skipped. In FP64 with the double parameters, nothing contracted: the camera point
+ *   ((u - cx) depth / fx, (v - cy) depth / fy, depth), the world point cam2world times it (summed left to right, the translation last),
+ *   dropped when sqrt((dx^2 + dy^2) + dz^2) > sensing_horizon for d = world point - pos (the body position, the node's last_pose_world);
+ *   kept points are rounded to FP32 x, y, z as pcl::PointXYZ stores them.
+ * Outputs. isdf_sense_depth: depth (Q x H x W int32, pixel (u, v) of pose q at (q H + v) W + u) in mm, 999999 where nothing is seen: the
+ *   reference's raw buffer. isdf_sense_cloud: the kept points of pose q in rows [offsets[q], offsets[q + 1]) of points (cap x 3 float32),
+ *   offsets Q + 1 int64. When the total exceeds cap the call returns ISDF_ERR_INVALID with offsets written (the sizes needed) and the rows
+ *   below cap written. The device forms take device pointers, are enqueued on cuda_stream and return when the work is enqueued, except
+ *   isdf_sense_cloud_device, which reads the 8-byte total to report an overflow.
+ * Guarantees: pose q's image and points depend only on pose q, the camera and the scene: the same bits for any Q, order of the poses, or
+ *   internal chunking, and through host and device forms. Bricks of the scene are culled per pose only where no point of them can reach
+ *   the image (for clouds also where every point lies beyond the horizon plus the camera's offset from the body), so culling changes no bit.
+ *   A non-finite pose gives whatever the definition gives (every point NaN: depth 0 at pixel (0, 0), no sensed point).
+ * Errors: ISDF_ERR_INVALID for a NULL argument, Q < 1 or Q >= 2^31, stride_doubles < 1, width or height < 1 or width x height > 2^26, a
+ *   camera parameter or cam_to_body entry not finite, fx or fy not positive, cam_to_body's last row not (0, 0, 0, 1), a NaN horizon or
+ *   one <= 0, cap < 0 (points may be NULL when cap = 0); ISDF_ERR_STATE when no scene cloud is set. The calls count their launches in
+ *   isdf_stats.kernel_launches. */
+typedef struct isdf_sense_params {
+    int32_t width, height;
+    double fx, fy, cx, cy;
+    double cam_to_body[16];    /* row-major 4 x 4 */
+    double sensing_horizon;    /* metres; +Inf keeps every point */
+} isdf_sense_params;
+typedef struct isdf_sense_info {
+    int64_t points_used, points_skipped, bricks;
+} isdf_sense_info;
+int isdf_sense_default_params(isdf_sense_params *p);
+int isdf_set_sense_cloud(isdf_ctx *ctx, const void *points, int64_t n, int32_t stride_bytes);
+int isdf_set_sense_cloud_device(isdf_ctx *ctx, const void *d_points, int64_t n, int32_t stride_bytes, void *cuda_stream);
+int isdf_get_sense_info(isdf_ctx *ctx, isdf_sense_info *out);
+int isdf_sense_depth(isdf_ctx *ctx, int64_t Q, const double *pos, const double *quat, int64_t stride_doubles, const isdf_sense_params *p,
+                     int32_t *depth);
+int isdf_sense_depth_device(isdf_ctx *ctx, int64_t Q, const double *d_pos, const double *d_quat, int64_t stride_doubles,
+                            const isdf_sense_params *p, int32_t *d_depth, void *cuda_stream);
+int isdf_sense_cloud(isdf_ctx *ctx, int64_t Q, const double *pos, const double *quat, int64_t stride_doubles, const isdf_sense_params *p,
+                     int64_t cap, float *points, int64_t *offsets);
+int isdf_sense_cloud_device(isdf_ctx *ctx, int64_t Q, const double *d_pos, const double *d_quat, int64_t stride_doubles,
+                            const isdf_sense_params *p, int64_t cap, float *d_points, int64_t *d_offsets, void *cuda_stream);
+
 /* ---- swept-volume term: addSaftyPenaOnSweptVolumeParallel (hpp:557-649) + getSDFofSweptVolume (swm:710-747) --- */
 /* parallel_points (plan_manager.cpp:246-254): P x 3 row-major world-frame voxel centres; resets lastTstar to 0 (not the persisted
  * trajectory duration: see isdf_set_points_batch) */
