@@ -26,6 +26,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <cmath>
+#include <functional>
 #include <string>
 #include <vector>
 #include <limits>
@@ -135,10 +136,10 @@ struct MincoWork {
     }
 };
 
-// The buffers of a certificate's interval-refinement rounds (isdf_refine.cuh): the staged trajectory block, piece start times, the two
-// interval lists of the round loop and the round counters.
+// The buffers of a certificate's interval-refinement rounds (isdf_refine.cuh): piece start times, the two interval lists of the round
+// loop and the round counters.
 struct RefineBufs {
-    DevBuf<double> d_in, d_toff; DevBuf<CertInterval> d_iv[2]; DevBuf<int> d_tot; PinnedBuf<int> h_tot;
+    DevBuf<double> d_toff; DevBuf<CertInterval> d_iv[2]; DevBuf<int> d_tot; PinnedBuf<int> h_tot;
     // room for N pieces and I0 initial intervals, and A's pointers into it
     int ensure(RefineArgs &A, int N, size_t I0) {
         CU_TRY(d_toff.ensure(N)); CU_TRY(d_tot.ensure(2)); CU_TRY(h_tot.ensure(1)); CU_TRY(d_iv[0].ensure(I0));
@@ -203,32 +204,31 @@ struct isdf_ctx {
         int last_rank = 0, last_world = 1, last_max_split = 0, last_warp_slots = 0, last_builder = 0;
         bool last_have_items = false;
     } disc;
-    struct {   // host entry points of the discrete and swept-volume terms: one pinned block, one copy each way
-        PinnedBuf<double> h;
-        DevBuf<double> d_C, d_out;
-    } stage;
+    struct {   // the host forms' arguments and results (Staging): one pinned block, one device block, both only grow
+        PinnedBuf<char> h;
+        DevBuf<char> d;
+    } staging;
     struct {   // batched callback (isdf_minco.cuh); B = 0: none evaluated yet
         MincoWork minco;
-        DevBuf<double> d_x, d_bc, d_cost, d_grad, d_Cpp, d_sv;
+        DevBuf<double> d_Cpp, d_sv;
         DevBuf<int> d_off;   // a ragged batch's offsets (ragged_upload)
         int B = 0;
         size_t P = 0;        // problems and pieces of the last evaluation
     } batch;
     struct LbfgsBufs {   // device-resident lock-step L-BFGS (isdf_lbfgs.cuh)
-        DevBuf<double> d_x, d_f, d_grad, d_state; DevBuf<int> d_int, d_head;
+        DevBuf<double> d_grad, d_state; DevBuf<int> d_int;
         PinnedBuf<int> h_active;
     } lbfgs;
     struct {   // mid-end (isdf_midend.cuh): buffers of its own, so that no mid-end call touches the back end's batch, swept or L-BFGS state
         MincoWork minco;
-        DevBuf<double> d_x, d_bc, d_wp, d_pc, d_cost, d_grad;
+        DevBuf<double> d_pc;
         DevBuf<int> d_off;   // a ragged batch's offsets (ragged_upload)
         LbfgsBufs lb;
     } mid;
     SweptState sv;   // swept volume
     struct {   // front end attitude kernels (isdf_frontend.cuh)
         bool ready = false;
-        DevBuf<double> d_rot; DevBuf<uint8_t> d_kernels, d_order, d_ok; DevBuf<uint32_t> d_masks, d_out;
-        DevBuf<int> d_ind; DevBuf<double> d_father, d_child;
+        DevBuf<double> d_rot; DevBuf<uint8_t> d_kernels, d_order; DevBuf<uint32_t> d_masks, d_out;
         DevBuf<uint2> d_core, d_urows, d_surv, d_chunks; DevBuf<uint4> d_tab; int nurow = 0, nchunk = 0, ntab = 0; DevBuf<unsigned> d_count; int ncore = 0;
         int xk = 0, yk = 0, ks = 0;
         double max_roll = 0, max_pitch = 0, ang_res = 0, margin = 0;
@@ -243,21 +243,21 @@ struct isdf_ctx {
         isdf_frontpath_info info = {};
     } fp;
     struct {   // trajectory clearance check (isdf_clearance.cuh)
-        DevBuf<double> d_in, d_clear; DevBuf<long long> d_vox; DevBuf<ClrSummary> d_sum; DevBuf<int> d_cursor;
+        DevBuf<int> d_cursor;
         DevBuf<unsigned long long> d_counters;   // {candidate pairs, exact mesh searches} of the last check (isdf_dbg_clearance_counts)
     } clr;
     struct {   // continuous certificate (isdf_certify.cuh): the rounds' buffers, samples, leaves, per-trajectory state
         RefineBufs ref;
         DevBuf<double> d_st, d_sc; DevBuf<int> d_sp, d_hit, d_cursor; DevBuf<long long> d_sv;
-        DevBuf<CertScratch> d_scr; DevBuf<CertLeaf> d_leaves; DevBuf<CertTraj> d_traj; DevBuf<CertSummary> d_sum;
+        DevBuf<CertScratch> d_scr; DevBuf<CertLeaf> d_leaves; DevBuf<CertTraj> d_traj;
         long long last_leaves = 0;   // leaves of the last call (isdf_dbg_certify_leaves)
     } cert;
     struct {   // dynamic-limit certificate (isdf_dynlimits.cuh): the rounds' buffers, samples, per-trajectory state
         RefineBufs ref;
-        DevBuf<DynSample> d_smp; DevBuf<int> d_dec; DevBuf<DynTraj> d_traj; DevBuf<DynSummary> d_sum;
+        DevBuf<DynSample> d_smp; DevBuf<int> d_dec; DevBuf<DynTraj> d_traj;
     } dyn;
     struct {   // certified swept volume (isdf_sweptvol.cuh): per-call poses and bounds, brick lists, per-warp interval lists, field and mesh
-        DevBuf<double> d_in, d_toff, d_pose, d_Dab, d_pts, d_val, d_low, d_ts, d_V, d_vt;
+        DevBuf<double> d_toff, d_pose, d_Dab, d_val, d_low, d_ts, d_V, d_vt;
         DevBuf<uint8_t> d_dec, d_mask; DevBuf<int32_t> d_F;
         DevBuf<long long> d_boff, d_bsum, d_voff, d_foff; DevBuf<int> d_blist, d_cursor;
         DevBuf<SvolIv> d_scratch; DevBuf<unsigned long long> d_counters;
@@ -284,10 +284,6 @@ struct isdf_ctx {
     // the host <-> device copies made so far at the planning pipeline's copy sites (count_copy): device-to-host bytes outside the rounds'
     // reads, the rounds' 4-byte reads, host-to-device bytes, copies
     long long xfer[4] = {};
-    struct {   // trajectory states and posed body points (isdf_states.cuh): the host forms' staging, one pinned block and one copy each way
-        PinnedBuf<double> h;
-        DevBuf<double> d_in, d_out;
-    } exec;
     SenseScene sense;   // depth sensing (isdf_sense.cuh): the scene cloud's bricks and the per-call scratch
     struct {   // peer-memory reduction (isdf_peer.cuh)
         DevBuf<char> buf;                    // own exchange buffer (exported through CUDA IPC)
@@ -327,6 +323,72 @@ static int sync_ctx(isdf_ctx *c, bool aux = false) {
     if (aux) CU_TRY(cudaStreamSynchronize(c->aux_stream));
     return 0;
 }
+
+// The host arrays of one host-form call, staged through c->staging: each array is a segment of the pinned and the device block, aligned
+// to 256 bytes. Declare them with in / inout / out, then upload() packs the inputs and makes ONE host-to-device copy on c->stream and
+// sets every declared device pointer; after the device work download() makes ONE device-to-host copy of the outputs, synchronises
+// c->stream and unpacks them. An output whose host pointer is NULL gets device room that is not copied back. Device block: [inputs |
+// in/out | outputs copied back | room]; the pinned block holds the inputs from its start, then the copied-back range from its start.
+class Staging {
+    enum Kind { IN, INOUT, OUT, ROOM };
+    struct Seg {
+        Kind kind;
+        size_t bytes, off;
+        std::function<void(char *)> set;          // the device pointer
+        std::function<void(void *)> fill;         // IN, INOUT: pack into the pinned block
+        std::function<void(const void *)> take;   // INOUT, OUT: unpack from the pinned block
+    };
+    isdf_ctx *c_;
+    std::vector<Seg> segs_;
+    size_t lo_ = 0, hi_ = 0;   // the copied-back range of the device block
+    template <typename T> void add(Kind k, T **d, size_t n, std::function<void(void *)> fill, std::function<void(const void *)> take) {
+        segs_.push_back({k, sizeof(T) * n, 0, [d](char *p) { *d = reinterpret_cast<T *>(p); }, std::move(fill), std::move(take)});
+    }
+
+public:
+    template <typename T> using Same = typename std::remove_cv<T>::type;   // the host pointer's type follows the device pointer's
+    explicit Staging(isdf_ctx *c) : c_(c) {}
+    template <typename T> void in(const T **d, const Same<T> *h, size_t n) { in(d, n, [h, n](T *p) { std::memcpy(p, h, sizeof(T) * n); }); }
+    // an input that fill(T *) writes into the pinned block
+    template <typename T, typename F> void in(const T **d, size_t n, F fill) { add(IN, d, n, [fill](void *p) { fill(static_cast<T *>(p)); }, nullptr); }
+    template <typename T> void inout(T **d, Same<T> *h, size_t n) {
+        add(INOUT, d, n, [h, n](void *p) { std::memcpy(p, h, sizeof(T) * n); }, [h, n](const void *p) { std::memcpy(h, p, sizeof(T) * n); });
+    }
+    template <typename T> void out(T **d, Same<T> *h, size_t n) {
+        if (h) out(d, n, [h, n](const T *p) { std::memcpy(h, p, sizeof(T) * n); });
+        else add(ROOM, d, n, nullptr, nullptr);
+    }
+    // an output that take(const T *) reads from the pinned block, which holds it until the next staged call
+    template <typename T, typename F> void out(T **d, size_t n, F take) {
+        add(OUT, d, n, nullptr, [take](const void *p) { take(static_cast<const T *>(p)); });
+    }
+    int upload() {
+        size_t off = 0, nin = 0;
+        for (Kind k : {IN, INOUT, OUT, ROOM}) {
+            if (k == INOUT) lo_ = off;
+            for (Seg &s : segs_) if (s.kind == k) { s.off = off; off += (s.bytes + 255) & ~(size_t)255; }
+            if (k == INOUT) nin = off;
+            if (k == OUT) hi_ = off;
+        }
+        // an earlier call that failed after enqueuing its copies may still be reading or writing the pinned block
+        CU_TRY(cudaStreamSynchronize(c_->stream));
+        CU_TRY(c_->staging.h.ensure(std::max(nin, hi_ - lo_))); CU_TRY(c_->staging.d.ensure(off));
+        char *h = c_->staging.h.p, *d = c_->staging.d.p;
+        for (Seg &s : segs_) {
+            s.set(d + s.off);
+            if (s.fill && s.bytes) s.fill(h + s.off);
+        }
+        if (nin) CU_TRY(cudaMemcpyAsync(d, h, nin, cudaMemcpyHostToDevice, c_->stream));
+        return 0;
+    }
+    int download() {
+        const char *h = c_->staging.h.p;
+        if (hi_ > lo_) CU_TRY(cudaMemcpyAsync(c_->staging.h.p, c_->staging.d.p + lo_, hi_ - lo_, cudaMemcpyDeviceToHost, c_->stream));
+        CU_TRY(cudaStreamSynchronize(c_->stream));
+        for (const Seg &s : segs_) if (s.take && s.bytes) s.take(h + (s.off - lo_));
+        return 0;
+    }
+};
 
 extern "C" const char *isdf_last_error(void) { return g_err.c_str(); }
 
@@ -786,19 +848,16 @@ extern "C" int isdf_shape_query(isdf_ctx *c, const double *p_rel, int n, double 
     if (what < 0 || what > 2) return fail(ISDF_ERR_INVALID, "bad query kind");
     if (n == 0) return 0;
     if (set_device(c)) return ISDF_ERR_CUDA;
-    DevBuf<double> dp, ds, dg;
-    CU_TRY(dp.upload(p_rel, (size_t)3 * n, c->stream));
-    CU_TRY(ds.ensure(n)); CU_TRY(dg.ensure((size_t)3 * n));
-    k_shape_query<<<(n + 127) / 128, 128, 0, c->stream>>>(c->mesh.shape, dp.p, n, ds.p, dg.p, what);
+    Staging S(c);
+    const double *dp;
+    double *ds, *dg;
+    S.in(&dp, p_rel, (size_t)3 * n);
+    S.out(&ds, what != ISDF_QUERY_GRAD ? sdf : nullptr, n); S.out(&dg, what != ISDF_QUERY_SDF ? grad : nullptr, (size_t)3 * n);
+    if (int r = S.upload()) return r;
+    k_shape_query<<<(n + 127) / 128, 128, 0, c->stream>>>(c->mesh.shape, dp, n, ds, dg, what);
     c->stats.kernel_launches++;
     CU_TRY(cudaGetLastError());
-    std::vector<double> hs(n), hg((size_t)3 * n);
-    CU_TRY(cudaMemcpyAsync(hs.data(), ds.p, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaMemcpyAsync(hg.data(), dg.p, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaStreamSynchronize(c->stream));
-    if (sdf && what != ISDF_QUERY_GRAD) std::memcpy(sdf, hs.data(), sizeof(double) * n);
-    if (grad && what != ISDF_QUERY_SDF) std::memcpy(grad, hg.data(), sizeof(double) * 3 * n);
-    return 0;
+    return S.download();
 }
 
 // ---- map ------------------------------------------------------------------------------------------------------
@@ -1130,16 +1189,16 @@ extern "C" int isdf_esdf_query(isdf_ctx *c, int field, const double *pts, int64_
     if (int rc = esdf_query_check(c, field, pts, n, dist)) return rc;
     if (n == 0) return 0;
     if (set_device(c)) return ISDF_ERR_CUDA;
-    DevBuf<double> d_pts, d_dist, d_grad;
-    CU_TRY(d_pts.upload(pts, (size_t)n * 3, c->stream));
-    CU_TRY(d_dist.ensure((size_t)n));
-    if (grad) CU_TRY(d_grad.ensure((size_t)n * 3));
-    esdf_query_launch(c, field, d_pts.p, n, d_dist.p, grad ? d_grad.p : nullptr, c->stream);
+    Staging S(c);
+    const double *d_pts;
+    double *d_dist, *d_grad = nullptr;   // no gradient room: the kernel computes no gradients
+    S.in(&d_pts, pts, (size_t)n * 3);
+    S.out(&d_dist, dist, (size_t)n);
+    if (grad) S.out(&d_grad, grad, (size_t)n * 3);
+    if (int r = S.upload()) return r;
+    esdf_query_launch(c, field, d_pts, n, d_dist, d_grad, c->stream);
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(dist, d_dist.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    if (grad) CU_TRY(cudaMemcpyAsync(grad, d_grad.p, (size_t)n * 3 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaStreamSynchronize(c->stream));
-    return 0;
+    return S.download();
 }
 
 extern "C" int isdf_esdf_query_device(isdf_ctx *c, int field, const double *d_pts, int64_t n, double *d_dist, double *d_grad, void *cuda_stream) {
@@ -1182,26 +1241,17 @@ extern "C" int isdf_trajectory_states(isdf_ctx *c, int B, const int32_t *piece_o
     for (long long q = 0; q < Q; q++) if (traj[q] < 0 || traj[q] >= B) return fail(ISDF_ERR_INVALID, "traj[q] outside [0, B)");
     if (Q == 0) return 0;
     if (set_device(c)) return ISDF_ERR_CUDA;
-    // one pinned block and one copy each way: in = [coeffs 18P | T P | times Q | piece_off B + 1, traj Q (int32)], out = Q records
-    const size_t nC = (size_t)19 * P, nin = nC + (size_t)Q + ((size_t)B + 1 + (size_t)Q + 1) / 2, nout = (size_t)STATE_DOUBLES * Q;
-    auto &x = c->exec;
-    CU_TRY(x.h.ensure(std::max(nin, nout))); CU_TRY(x.d_in.ensure(nin)); CU_TRY(x.d_out.ensure(nout));
-    double *h = x.h.p;
-    std::memcpy(h, coeffs, sizeof(double) * 18 * (size_t)P);
-    std::memcpy(h + 18 * (size_t)P, T, sizeof(double) * P);
-    std::memcpy(h + nC, times, sizeof(double) * Q);
-    int32_t *hi = reinterpret_cast<int32_t *>(h + nC + Q);
-    std::memcpy(hi, piece_off, sizeof(int32_t) * ((size_t)B + 1));
-    std::memcpy(hi + B + 1, traj, sizeof(int32_t) * Q);
-    CU_TRY(cudaMemcpyAsync(x.d_in.p, h, sizeof(double) * nin, cudaMemcpyHostToDevice, c->stream));
-    const double *d = x.d_in.p;
-    const int *di = reinterpret_cast<const int *>(d + nC + Q);
-    states_launch(c, B, di, d + 18 * (size_t)P, d, Q, di + B + 1, d + nC, x.d_out.p, c->stream);
+    Staging S(c);
+    const double *d_C, *d_T, *d_times;
+    const int *d_off, *d_traj;
+    double *d_out;
+    S.in(&d_C, coeffs, 18 * (size_t)P); S.in(&d_T, T, (size_t)P); S.in(&d_times, times, (size_t)Q);
+    S.in(&d_off, piece_off, (size_t)B + 1); S.in(&d_traj, traj, (size_t)Q);
+    S.out(&d_out, out, (size_t)STATE_DOUBLES * Q);
+    if (int rc = S.upload()) return rc;
+    states_launch(c, B, d_off, d_T, d_C, Q, d_traj, d_times, d_out, c->stream);
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(h, x.d_out.p, sizeof(double) * nout, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaStreamSynchronize(c->stream));
-    std::memcpy(out, h, sizeof(double) * nout);
-    return 0;
+    return S.download();
 }
 
 extern "C" int isdf_trajectory_states_device(isdf_ctx *c, int B, const int32_t *d_piece_off, const double *d_T, const double *d_coeffs, int64_t Q,
@@ -1234,19 +1284,15 @@ extern "C" int isdf_pose_points(isdf_ctx *c, int64_t Q, const double *states, in
     if (int rc = pose_args_check(c, Q, states, P, body, out)) return rc;
     if (Q == 0 || P == 0) return 0;
     if (set_device(c)) return ISDF_ERR_CUDA;
-    // in = [states 20 Q | body 3 P], out = 3 P Q
-    const size_t ns = (size_t)STATE_DOUBLES * Q, nin = ns + 3 * (size_t)P, nout = 3 * (size_t)P * (size_t)Q;
-    auto &x = c->exec;
-    CU_TRY(x.h.ensure(std::max(nin, nout))); CU_TRY(x.d_in.ensure(nin)); CU_TRY(x.d_out.ensure(nout));
-    std::memcpy(x.h.p, states, sizeof(double) * ns);
-    std::memcpy(x.h.p + ns, body, sizeof(double) * 3 * (size_t)P);
-    CU_TRY(cudaMemcpyAsync(x.d_in.p, x.h.p, sizeof(double) * nin, cudaMemcpyHostToDevice, c->stream));
-    pose_launch(c, Q, x.d_in.p, P, x.d_in.p + ns, x.d_out.p, c->stream);
+    Staging S(c);
+    const double *d_states, *d_body;
+    double *d_out;
+    S.in(&d_states, states, (size_t)STATE_DOUBLES * Q); S.in(&d_body, body, 3 * (size_t)P);
+    S.out(&d_out, out, 3 * (size_t)P * (size_t)Q);
+    if (int rc = S.upload()) return rc;
+    pose_launch(c, Q, d_states, P, d_body, d_out, c->stream);
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(x.h.p, x.d_out.p, sizeof(double) * nout, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaStreamSynchronize(c->stream));
-    std::memcpy(out, x.h.p, sizeof(double) * nout);
-    return 0;
+    return S.download();
 }
 
 extern "C" int isdf_pose_points_device(isdf_ctx *c, int64_t Q, const double *d_states, int P, const double *d_body, double *d_out, void *cuda_stream) {
@@ -1341,31 +1387,19 @@ extern "C" int isdf_simulate(isdf_ctx *c, int B, const int32_t *piece_off, const
                 return fail(ISDF_ERR_INVALID, "traj[r] outside [0, B) or naming a trajectory without pieces");
         if (R == 0) return 0;
         if (set_device(c)) return ISDF_ERR_CUDA;
-        // one device block: in = [coeffs 18P | T P | init 17R | dist 6R | piece_off, traj (int32)], out = [summaries | log]
-        const size_t nC = (size_t)19 * P, nI = (size_t)ISDF_SIM_INIT_DOUBLES * R, nD = dist ? (size_t)6 * R : 0;
-        const size_t nin = nC + nI + nD + ((size_t)B + 1 + (size_t)R + 1) / 2;
-        const size_t nsum = ((size_t)R * sizeof(isdf_sim_summary) + 7) / 8, nlog = log ? (size_t)R * cap_log * ISDF_SIM_DOUBLES : 0;
-        auto &x = c->exec;
-        CU_TRY(x.h.ensure(std::max(nin, nsum + nlog))); CU_TRY(x.d_in.ensure(nin)); CU_TRY(x.d_out.ensure(nsum + nlog));
-        double *h = x.h.p;
-        std::memcpy(h, coeffs, sizeof(double) * 18 * (size_t)P);
-        std::memcpy(h + 18 * (size_t)P, T, sizeof(double) * P);
-        std::memcpy(h + nC, init, sizeof(double) * nI);
-        if (dist) std::memcpy(h + nC + nI, dist, sizeof(double) * nD);
-        int32_t *hi = reinterpret_cast<int32_t *>(h + nC + nI + nD);
-        std::memcpy(hi, piece_off, sizeof(int32_t) * ((size_t)B + 1));
-        std::memcpy(hi + B + 1, traj, sizeof(int32_t) * R);
-        CU_TRY(cudaMemcpyAsync(x.d_in.p, h, sizeof(double) * nin, cudaMemcpyHostToDevice, c->stream));
-        const double *d = x.d_in.p;
-        const int *di = reinterpret_cast<const int *>(d + nC + nI + nD);
-        isdf_sim_summary *d_sum = reinterpret_cast<isdf_sim_summary *>(x.d_out.p);
-        if (int rc = sim_launch(c, B, di, d + 18 * (size_t)P, d, R, di + B + 1, d + nC, dist ? d + nC + nI : nullptr, p, n_ticks, m, cap_log,
-                                log ? x.d_out.p + nsum : nullptr, d_sum, c->stream)) return rc;
-        CU_TRY(cudaMemcpyAsync(h, x.d_out.p, sizeof(double) * (nsum + nlog), cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaStreamSynchronize(c->stream));
-        std::memcpy(summary, h, sizeof(isdf_sim_summary) * R);
-        if (log) std::memcpy(log, h + nsum, sizeof(double) * nlog);
-        return 0;
+        Staging S(c);
+        const double *d_C, *d_T, *d_init, *d_dist = nullptr;
+        const int *d_off, *d_traj;
+        double *d_log = nullptr;
+        isdf_sim_summary *d_sum;
+        S.in(&d_C, coeffs, 18 * (size_t)P); S.in(&d_T, T, (size_t)P); S.in(&d_init, init, (size_t)ISDF_SIM_INIT_DOUBLES * R);
+        if (dist) S.in(&d_dist, dist, (size_t)6 * R);
+        S.in(&d_off, piece_off, (size_t)B + 1); S.in(&d_traj, traj, (size_t)R);
+        S.out(&d_sum, summary, (size_t)R);
+        if (log) S.out(&d_log, log, (size_t)R * cap_log * ISDF_SIM_DOUBLES);
+        if (int rc = S.upload()) return rc;
+        if (int rc = sim_launch(c, B, d_off, d_T, d_C, R, d_traj, d_init, d_dist, p, n_ticks, m, cap_log, d_log, d_sum, c->stream)) return rc;
+        return S.download();
     }, [&]() { sim_poison_host(summary, R); });
 }
 
@@ -1450,17 +1484,14 @@ static int sense_args_check(isdf_ctx *c, int64_t Q, const void *pos, const void 
     return 0;
 }
 
-// the host form's poses, packed as (pos, quat) records of 7 doubles on the context's stream
-static int sense_stage_poses(isdf_ctx *c, int64_t Q, const double *pos, const double *quat, int64_t stride, SenseCall *C) {
-    auto &x = c->exec;
-    CU_TRY(x.h.ensure(7 * (size_t)Q)); CU_TRY(x.d_in.ensure(7 * (size_t)Q));
-    for (int64_t q = 0; q < Q; q++) {
-        std::memcpy(x.h.p + 7 * q, pos + q * stride, 3 * sizeof(double));
-        std::memcpy(x.h.p + 7 * q + 3, quat + q * stride, 4 * sizeof(double));
-    }
-    CU_TRY(cudaMemcpyAsync(x.d_in.p, x.h.p, 7 * sizeof(double) * Q, cudaMemcpyHostToDevice, c->stream));
-    C->pos = x.d_in.p; C->quat = x.d_in.p + 3; C->stride = 7;
-    return 0;
+// Q poses read at a stride of `stride` doubles, staged as (x, y, z, w, qx, qy, qz) records 7 doubles apart at *d
+static void stage_poses(Staging &S, int64_t Q, const double *pos, const double *quat, int64_t stride, const double **d) {
+    S.in(d, 7 * (size_t)Q, [=](double *h) {
+        for (int64_t q = 0; q < Q; q++) {
+            std::memcpy(h + 7 * q, pos + q * stride, 3 * sizeof(double));
+            std::memcpy(h + 7 * q + 3, quat + q * stride, 4 * sizeof(double));
+        }
+    });
 }
 
 static int sense_depth_impl(isdf_ctx *c, int64_t Q, const double *pos, const double *quat, int64_t stride, const isdf_sense_params *p,
@@ -1468,8 +1499,12 @@ static int sense_depth_impl(isdf_ctx *c, int64_t Q, const double *pos, const dou
     if (int rc = sense_args_check(c, Q, pos, quat, stride, p, depth)) return rc;
     if (set_device(c)) return ISDF_ERR_CUDA;
     SenseCall C{Q, pos, quat, stride, *p};
+    Staging S(c);
     if (!device) {
-        if (int rc = sense_stage_poses(c, Q, pos, quat, stride, &C)) return rc;
+        const double *d_pose;
+        stage_poses(S, Q, pos, quat, stride, &d_pose);
+        if (int rc = S.upload()) return rc;
+        C.pos = d_pose; C.quat = d_pose + 3; C.stride = 7;
         st = c->stream;
     }
     int launches = 0;
@@ -1496,13 +1531,14 @@ static int sense_cloud_impl(isdf_ctx *c, int64_t Q, const double *pos, const dou
     SenseCall C{Q, pos, quat, stride, *p};
     float *d_points = points;
     int64_t *d_off = offsets;
-    DevBuf<float> s_points; DevBuf<int64_t> s_off;
-    if (!device) {
-        if (int rc = sense_stage_poses(c, Q, pos, quat, stride, &C)) return rc;
+    Staging S(c);
+    if (!device) {   // the results' room; their sizes are known after the call, so they come back by themselves below
+        const double *d_pose;
+        stage_poses(S, Q, pos, quat, stride, &d_pose);
+        S.out(&d_off, nullptr, (size_t)Q + 1); S.out(&d_points, nullptr, 3 * (size_t)cap);
+        if (int rc = S.upload()) return rc;
+        C.pos = d_pose; C.quat = d_pose + 3; C.stride = 7;
         st = c->stream;
-        CU_TRY(s_off.ensure(Q + 1));
-        if (cap > 0) CU_TRY(s_points.ensure(3 * (size_t)cap));
-        d_points = s_points.p; d_off = s_off.p;
     }
     int launches = 0;
     const cudaError_t e = sense_cloud_run(c->sense, C, d_points, cap, d_off, st, &launches);
@@ -1512,8 +1548,9 @@ static int sense_cloud_impl(isdf_ctx *c, int64_t Q, const double *pos, const dou
     CU_TRY(cudaMemcpyAsync(&total, d_off + Q, sizeof total, cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaStreamSynchronize(st));
     if (!device) {
-        CU_TRY(cudaMemcpy(offsets, d_off, sizeof(int64_t) * (Q + 1), cudaMemcpyDeviceToHost));
-        if (std::min(total, cap) > 0) CU_TRY(cudaMemcpy(points, d_points, 3 * sizeof(float) * std::min(total, cap), cudaMemcpyDeviceToHost));
+        CU_TRY(cudaMemcpyAsync(offsets, d_off, sizeof(int64_t) * (Q + 1), cudaMemcpyDeviceToHost, st));
+        if (std::min(total, cap) > 0) CU_TRY(cudaMemcpyAsync(points, d_points, 3 * sizeof(float) * std::min(total, cap), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
     }
     if (total > cap) return fail(ISDF_ERR_INVALID, "cap smaller than the sensed points (offsets report the sizes)");
     return 0;
@@ -1790,11 +1827,14 @@ extern "C" int isdf_gather_obstacle_points(isdf_ctx *c, const double *waypoints,
     if (set_device(c)) return ISDF_ERR_CUDA;
     auto &g = c->gat;
     const int wp_off[2] = {0, nQ};
-    CU_TRY(g.d_wpoff.upload(wp_off, 2, c->stream));
-    CU_TRY(g.d_wp.upload(waypoints, (size_t)3 * nQ, c->stream));
+    Staging S(c);
+    const int *d_wpoff;
+    const double *d_wp;
+    S.in(&d_wpoff, wp_off, 2); S.in(&d_wp, waypoints, (size_t)3 * nQ);
+    if (int r = S.upload()) return r;
     std::vector<int> off;
     long long total = 0;
-    if (int r = gather_batch_run(c, 1, wp_off, g.d_wpoff.p, g.d_wp.p, half_extent, offset, 0x7fffffffll, off, &total, c->stream)) return r;
+    if (int r = gather_batch_run(c, 1, wp_off, d_wpoff, d_wp, half_extent, offset, 0x7fffffffll, off, &total, c->stream)) return r;
     *n = (int)total;
     const long long m = std::min<long long>(total, cap);
     if (m > 0 && out_points) {   // the write pass runs on the context's non-blocking stream
@@ -1817,12 +1857,14 @@ extern "C" int isdf_gather_obstacle_points_batch(isdf_ctx *c, int B, const int32
     if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
     if (set_device(c)) return ISDF_ERR_CUDA;
     auto &g = c->gat;
-    const int R = wp_off[B];
-    CU_TRY(g.d_wpoff.upload(wp_off, (size_t)B + 1, c->stream));
-    if (R > 0) CU_TRY(g.d_wp.upload(waypoints, (size_t)3 * R, c->stream));
+    Staging S(c);
+    const int *d_wpoff;
+    const double *d_wp;
+    S.in(&d_wpoff, wp_off, (size_t)B + 1); S.in(&d_wp, waypoints, (size_t)3 * wp_off[B]);
+    if (int r = S.upload()) return r;
     std::vector<int> off;
     long long total = 0;
-    const int r = gather_batch_run(c, B, wp_off, g.d_wpoff.p, g.d_wp.p, half_extent, offset, out_points ? cap : 0x7fffffffll, off, &total, c->stream);
+    const int r = gather_batch_run(c, B, wp_off, d_wpoff, d_wp, half_extent, offset, out_points ? cap : 0x7fffffffll, off, &total, c->stream);
     if (!off.empty()) std::memcpy(pt_off, off.data(), sizeof(int32_t) * off.size());
     if (r) return r;
     if (out_points && total > 0) {   // the write pass runs on the context's non-blocking stream
@@ -1970,29 +2012,26 @@ extern "C" int isdf_eval_discrete_device(isdf_ctx *c, int N, const double *d_T, 
     return launch_discrete(c, N, d_T, d_coeffs, d_out, nullptr, (cudaStream_t)cuda_stream);
 }
 
-// The host form of the discrete and swept-volume evaluations: [coefficients 18N | durations N] go in through one pinned block and
-// ONE copy, `before` runs after that copy, `launch(d_T, d_C, d_out, count_out)` between ev0 and ev1, and [cost | gradC | gradT |
-// counter word] come back in ONE copy. The result is added to *cost, gradC and gradT, as the reference accumulates (hpp:539-550,
-// hpp:640-645); the counter word goes to the stat `counted`. The caller poisons *cost on failure.
-template <typename Before, typename Launch>
-static int eval_host(isdf_ctx *c, int N, const double *T, const double *coeffs, double *cost, double *gradC, double *gradT,
-                     int64_t isdf_stats::*counted, Before before, Launch launch) {
+// The host form of the discrete and swept-volume evaluations: [coefficients 18N | durations N] and the inputs S already holds go in
+// with ONE copy, `launch(d_T, d_C, d_out, count_out)` runs between ev0 and ev1, and [cost | gradC | gradT | counter word] come back
+// in ONE copy. The result is added to *cost, gradC and gradT, as the reference accumulates (hpp:539-550, hpp:640-645); the counter
+// word goes to the stat `counted`. The caller poisons *cost on failure.
+template <typename Launch>
+static int eval_host(isdf_ctx *c, Staging &S, int N, const double *T, const double *coeffs, double *cost, double *gradC, double *gradT,
+                     int64_t isdf_stats::*counted, Launch launch) {
     if (set_device(c)) return ISDF_ERR_CUDA;
-    const size_t nin = (size_t)19 * N, nout = (size_t)19 * N + 1;
-    CU_TRY(c->stage.h.ensure(nin + nout + 1));
-    CU_TRY(c->stage.d_C.ensure(nin)); CU_TRY(c->stage.d_out.ensure(nout + 1));
-    std::memcpy(c->stage.h.p, coeffs, sizeof(double) * 18 * N);
-    std::memcpy(c->stage.h.p + 18 * (size_t)N, T, sizeof(double) * N);
-    CU_TRY(cudaMemcpyAsync(c->stage.d_C.p, c->stage.h.p, sizeof(double) * nin, cudaMemcpyHostToDevice, c->stream));
-    if (int rr = before()) return rr;
-    CU_TRY(cudaEventRecord(c->ev0, c->stream));
-    if (int rr = launch(c->stage.d_C.p + 18 * (size_t)N, c->stage.d_C.p, c->stage.d_out.p, c->stage.d_out.p + nout)) return rr;
-    CU_TRY(cudaEventRecord(c->ev1, c->stream));
-    double *h_out = c->stage.h.p + nin;
-    CU_TRY(cudaMemcpyAsync(h_out, c->stage.d_out.p, sizeof(double) * (nout + 1), cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaStreamSynchronize(c->stream));
+    const size_t nout = (size_t)19 * N + 1;
+    const double *d_C, *d_T, *h_out = nullptr;
+    double *d_out, *d_count;
     unsigned long long count = 0;
-    std::memcpy(&count, h_out + nout, sizeof(count));
+    S.in(&d_C, coeffs, 18 * (size_t)N); S.in(&d_T, T, (size_t)N);
+    S.out(&d_out, nout, [&](const double *h) { h_out = h; });
+    S.out(&d_count, 1, [&](const double *h) { std::memcpy(&count, h, sizeof(count)); });
+    if (int rr = S.upload()) return rr;
+    CU_TRY(cudaEventRecord(c->ev0, c->stream));
+    if (int rr = launch(d_T, d_C, d_out, d_count)) return rr;
+    CU_TRY(cudaEventRecord(c->ev1, c->stream));
+    if (int rr = S.download()) return rr;
     if (fused_exchange(c) && isdf_peer_status(c) != ISDF_OK) return ISDF_ERR_CUDA;   // exchange timed out: the vector is NaN
     float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
     c->stats.last_kernel_ms = ms; c->stats.*counted = (int64_t)count;
@@ -2006,7 +2045,8 @@ extern "C" int isdf_eval_discrete(isdf_ctx *c, int N, const double *T, const dou
     return poison_on_failure([&]() -> int {
         if (int r = check_eval_state(c, N, true)) return r;
         if (!T || !coeffs || !cost || !gradC || !gradT) return fail(ISDF_ERR_INVALID, "NULL argument");
-        return eval_host(c, N, T, coeffs, cost, gradC, gradT, &isdf_stats::last_pairs, [] { return 0; },
+        Staging S(c);
+        return eval_host(c, S, N, T, coeffs, cost, gradC, gradT, &isdf_stats::last_pairs,
                          [&](const double *d_T, const double *d_C, double *d_out, double *count_out) {
                              return launch_discrete(c, N, d_T, d_C, d_out, count_out, c->stream);
                          });
@@ -2096,18 +2136,20 @@ extern "C" int isdf_callback_batch_ragged_device(isdf_ctx *c, int B, const int32
     return callback_device(c, true, B, 0, piece_off, d_head, d_tail, per_problem_bc, rho, d_x, d_cost, d_grad, (cudaStream_t)cuda_stream);
 }
 
-// the host entry points' boundary conditions (9 doubles, or 9 per problem) in buf on c->stream: *d_head, then *d_tail
-static int upload_bc(isdf_ctx *c, DevBuf<double> &buf, int B, int per_problem_bc, const double *head, const double *tail, const double **d_head,
-                     const double **d_tail) {
+// a checked batch's host inputs shared by the batched host entry points, staged in S: a ragged batch's offsets into *L (as ragged_upload
+// lays them out), the boundary conditions (9 doubles, or 9 per problem) at *d_head and *d_tail
+static void stage_batch(Staging &S, bool ragged, const int32_t *piece_off, int per_problem_bc, const double *head, const double *tail, Layout *L,
+                        const double **d_head, const double **d_tail) {
+    const int B = L->B;
+    if (ragged) {
+        S.in(&L->d_off, piece_off, (size_t)B + 1);
+        S.in(&L->d_xoff, (size_t)B + 1, [=](int *h) { for (int b = 0; b <= B; b++) h[b] = 4 * piece_off[b] - 3 * b; });
+    }
     const size_t nbc = per_problem_bc ? (size_t)9 * B : 9;
-    CU_TRY(buf.ensure(2 * nbc));
-    CU_TRY(cudaMemcpyAsync(buf.p, head, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
-    CU_TRY(cudaMemcpyAsync(buf.p + nbc, tail, sizeof(double) * nbc, cudaMemcpyHostToDevice, c->stream));
-    *d_head = buf.p; *d_tail = buf.p + nbc;
-    return 0;
+    S.in(d_head, head, nbc); S.in(d_tail, tail, nbc);
 }
 
-// the host form of the batched callback: inputs staged in c->batch, then the device form on c->stream
+// the host form of the batched callback: inputs staged, the batch launched on c->stream between ev0 and ev1, results copied back
 static int callback_host(isdf_ctx *c, bool ragged, int B, int N0, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
                          double rho, const double *x, double *cost, double *grad) {
     return poison_on_failure([&]() -> int {
@@ -2115,17 +2157,16 @@ static int callback_host(isdf_ctx *c, bool ragged, int B, int N0, const int32_t 
         if (int r = callback_batch_check(c, ragged, B, N0, piece_off, &L)) return r;
         if (!head || !tail || !x || !cost || !grad) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
-        CU_TRY(c->batch.d_x.upload(x, L.X, c->stream));
-        const double *d_head, *d_tail;
-        if (int r = upload_bc(c, c->batch.d_bc, B, per_problem_bc, head, tail, &d_head, &d_tail)) return r;
-        CU_TRY(c->batch.d_cost.ensure(B)); CU_TRY(c->batch.d_grad.ensure(L.X));
+        Staging S(c);
+        const double *d_head, *d_tail, *d_x;
+        double *d_cost, *d_grad;
+        stage_batch(S, ragged, piece_off, per_problem_bc, head, tail, &L, &d_head, &d_tail);
+        S.in(&d_x, x, L.X); S.out(&d_cost, cost, (size_t)B); S.out(&d_grad, grad, L.X);
+        if (int r = S.upload()) return r;
         CU_TRY(cudaEventRecord(c->ev0, c->stream));
-        if (int r = callback_device(c, ragged, B, N0, piece_off, d_head, d_tail, per_problem_bc, rho, c->batch.d_x.p, c->batch.d_cost.p,
-                                    c->batch.d_grad.p, c->stream)) return r;
+        if (int r = callback_batch_launch(c, L, d_head, d_tail, per_problem_bc ? 9 : 0, rho, d_x, d_cost, d_grad, c->stream)) return r;
         CU_TRY(cudaEventRecord(c->ev1, c->stream));
-        CU_TRY(cudaMemcpyAsync(cost, c->batch.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaMemcpyAsync(grad, c->batch.d_grad.p, sizeof(double) * L.X, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaStreamSynchronize(c->stream));
+        if (int r = S.download()) return r;
         float ms = 0; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
         c->stats.last_kernel_ms = ms;
         return 0;
@@ -2228,14 +2269,14 @@ static void nan_fill_device(isdf_ctx *c, double *d, int n, cudaStream_t st) {
     if (c && d && n > 0 && cudaSetDevice(c->device) == cudaSuccess) { cudaMemsetAsync(d, 0xff, sizeof(double) * n, st); cudaStreamSynchronize(st); }
 }
 
-// an L-BFGS call's results in lb to the host: x (X rows), f, and ret / iterations / evaluations from the d_head triple (each may be NULL)
-static int lbfgs_copy_out(const isdf_ctx::LbfgsBufs &lb, int B, size_t X, double *x, double *f, int *ret, int *iterations, int *evaluations) {
-    CU_TRY(cudaMemcpy(x, lb.d_x.p, sizeof(double) * X, cudaMemcpyDeviceToHost));
-    CU_TRY(cudaMemcpy(f, lb.d_f.p, sizeof(double) * B, cudaMemcpyDeviceToHost));
-    if (ret) CU_TRY(cudaMemcpy(ret, lb.d_head.p, sizeof(int) * B, cudaMemcpyDeviceToHost));
-    if (iterations) CU_TRY(cudaMemcpy(iterations, lb.d_head.p + B, sizeof(int) * B, cudaMemcpyDeviceToHost));
-    if (evaluations) CU_TRY(cudaMemcpy(evaluations, lb.d_head.p + 2 * (size_t)B, sizeof(int) * B, cudaMemcpyDeviceToHost));
-    return 0;
+// the lock-step L-BFGS over the batched callback of a checked batch on st
+static int lbfgs_batch_run(isdf_ctx *c, const Layout &L, const double *d_head, const double *d_tail, int per_problem_bc, double rho,
+                           const isdf_lbfgs_params *prm, double *d_x, double *d_f, int *d_ret, int *d_iterations, int *d_evaluations, int *rounds_out,
+                           cudaStream_t st) {
+    return lbfgs_rounds(c, c->lbfgs, L.B, 4 * L.N - 3, L.d_xoff, L.X, prm, 0, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st,
+                        [&](const double *x, double *f, double *g) {
+                            return callback_batch_launch(c, L, d_head, d_tail, per_problem_bc ? 9 : 0, rho, x, f, g, st);
+                        });
 }
 
 // the device form of the lock-step L-BFGS over the batched callback on st; a ragged batch's offsets are uploaded first
@@ -2249,10 +2290,7 @@ static int lbfgs_device(isdf_ctx *c, bool ragged, int B, int N0, const int32_t *
         if (!d_head || !d_tail || !d_x || !d_f) return fail(ISDF_ERR_INVALID, "NULL device pointer");
         if (set_device(c)) return ISDF_ERR_CUDA;
         if (ragged) if (int r = ragged_upload(c->batch.d_off, piece_off, st, &L)) return r;
-        return lbfgs_rounds(c, c->lbfgs, B, 4 * L.N - 3, L.d_xoff, L.X, prm, 0, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st,
-                            [&](const double *x, double *f, double *g) {
-                                return callback_batch_launch(c, L, d_head, d_tail, per_problem_bc ? 9 : 0, rho, x, f, g, st);
-                            });
+        return lbfgs_batch_run(c, L, d_head, d_tail, per_problem_bc, rho, prm, d_x, d_f, d_ret, d_iterations, d_evaluations, rounds_out, st);
     }, [&] { nan_fill_device(c, d_f, B, st); });
 }
 
@@ -2270,22 +2308,25 @@ extern "C" int isdf_lbfgs_batch_ragged_device(isdf_ctx *c, int B, const int32_t 
                         (cudaStream_t)cuda_stream);
 }
 
-// the host form of the L-BFGS: inputs staged in c->lbfgs and c->batch, then the device form on c->stream, results copied back
+// the host form of the L-BFGS: inputs staged, the rounds on c->stream, results copied back
 static int lbfgs_host(isdf_ctx *c, bool ragged, int B, int N0, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
                       double rho, const isdf_lbfgs_params *prm, double *x, double *f, int *ret, int *iterations, int *evaluations, int *rounds_out) {
     return poison_on_failure([&]() -> int {
         Layout L;
         if (int r = callback_batch_check(c, ragged, B, N0, piece_off, &L)) return r;
         if (!head || !tail || !x || !f) return fail(ISDF_ERR_INVALID, "NULL argument");
+        if (int r = lbfgs_check(prm)) return r;
         if (set_device(c)) return ISDF_ERR_CUDA;
-        isdf_ctx::LbfgsBufs &lb = c->lbfgs;
-        CU_TRY(lb.d_x.upload(x, L.X, c->stream));
+        Staging S(c);
         const double *d_head, *d_tail;
-        if (int r = upload_bc(c, c->batch.d_bc, B, per_problem_bc, head, tail, &d_head, &d_tail)) return r;
-        CU_TRY(lb.d_f.ensure(B)); CU_TRY(lb.d_head.ensure((size_t)3 * B));
-        if (int r = lbfgs_device(c, ragged, B, N0, piece_off, d_head, d_tail, per_problem_bc, rho, prm, lb.d_x.p, lb.d_f.p, lb.d_head.p, lb.d_head.p + B,
-                                 lb.d_head.p + 2 * (size_t)B, rounds_out, c->stream)) return r;
-        return lbfgs_copy_out(lb, B, L.X, x, f, ret, iterations, evaluations);
+        double *d_x, *d_f;
+        int *d_ret, *d_it, *d_ev;
+        stage_batch(S, ragged, piece_off, per_problem_bc, head, tail, &L, &d_head, &d_tail);
+        S.inout(&d_x, x, L.X); S.out(&d_f, f, (size_t)B);
+        S.out(&d_ret, ret, (size_t)B); S.out(&d_it, iterations, (size_t)B); S.out(&d_ev, evaluations, (size_t)B);
+        if (int r = S.upload()) return r;
+        if (int r = lbfgs_batch_run(c, L, d_head, d_tail, per_problem_bc, rho, prm, d_x, d_f, d_ret, d_it, d_ev, rounds_out, c->stream)) return r;
+        return S.download();
     }, [&] { nan_fill(f, B); });
 }
 
@@ -2313,11 +2354,14 @@ extern "C" int isdf_dbg_lbfgs_rounds(isdf_ctx *c, int B, int n, const isdf_lbfgs
     if (!eval || !x || !f) return fail(ISDF_ERR_INVALID, "NULL argument");
     if (set_device(c)) return ISDF_ERR_CUDA;
     const size_t bn = (size_t)B * n;
-    isdf_ctx::LbfgsBufs &lb = c->lbfgs;
-    CU_TRY(lb.d_x.upload(x, bn, c->stream));
-    CU_TRY(lb.d_f.ensure(B)); CU_TRY(lb.d_head.ensure((size_t)3 * B));
-    std::vector<double> hx(bn), hf(B), hg(bn);
-    int r = lbfgs_rounds(c, lb, B, n, nullptr, bn, prm, cancel_after, lb.d_x.p, lb.d_f.p, lb.d_head.p, lb.d_head.p + B, lb.d_head.p + 2 * (size_t)B, rounds_out, c->stream,
+    Staging S(c);
+    double *d_xs, *d_fs;
+    int *d_ret, *d_it, *d_ev;
+    S.inout(&d_xs, x, bn); S.out(&d_fs, f, (size_t)B);
+    S.out(&d_ret, ret, (size_t)B); S.out(&d_it, iterations, (size_t)B); S.out(&d_ev, evaluations, (size_t)B);
+    if (int r = S.upload()) return r;
+    std::vector<double> hx(bn), hf(B), hg(bn);   // the rounds' points and the objective's results
+    int r = lbfgs_rounds(c, c->lbfgs, B, n, nullptr, bn, prm, cancel_after, d_xs, d_fs, d_ret, d_it, d_ev, rounds_out, c->stream,
                          [&](const double *d_x, double *d_f, double *d_g) -> int {
                              CU_TRY(cudaMemcpyAsync(hx.data(), d_x, sizeof(double) * bn, cudaMemcpyDeviceToHost, c->stream));
                              CU_TRY(cudaStreamSynchronize(c->stream));
@@ -2328,7 +2372,7 @@ extern "C" int isdf_dbg_lbfgs_rounds(isdf_ctx *c, int B, int n, const isdf_lbfgs
                              return 0;
                          });
     if (r) return r;
-    return lbfgs_copy_out(lb, B, bn, x, f, ret, iterations, evaluations);
+    return S.download();
 }
 
 extern "C" int isdf_get_batch_trajectories(isdf_ctx *c, double *T, double *coeffs, double *energy) {
@@ -2474,19 +2518,7 @@ static int midend_eval_launch(isdf_ctx *c, const Layout &L, const double *d_head
     return 0;
 }
 
-// the mid-end's host entry points stage their inputs in c->mid: boundary conditions (*d_head, *d_tail) and waypoints
-static int midend_upload(isdf_ctx *c, const Layout &L, int per_problem_bc, const double *head, const double *tail, const double *waypoints,
-                         const double **d_head, const double **d_tail, const double **d_wp) {
-    const int B = L.B;
-    const size_t nwp = 3 * (L.P - B);
-    if (int r = upload_bc(c, c->mid.d_bc, B, per_problem_bc, head, tail, d_head, d_tail)) return r;
-    CU_TRY(c->mid.d_wp.ensure(nwp > 0 ? nwp : 1));
-    if (nwp) CU_TRY(cudaMemcpyAsync(c->mid.d_wp.p, waypoints, sizeof(double) * nwp, cudaMemcpyHostToDevice, c->stream));
-    *d_wp = c->mid.d_wp.p;
-    return 0;
-}
-
-// the host form of one mid-end evaluation: inputs staged in c->mid (a ragged batch's offsets first), results copied back
+// the host form of one mid-end evaluation: inputs staged (the waypoints, 3 per inner piece, after the batch's), results copied back
 static int midend_callback_host(isdf_ctx *c, bool ragged, int B, int N0, const int32_t *piece_off, const double *head, const double *tail,
                                 int per_problem_bc, const isdf_midend_params *p, const double *waypoints, const double *x, double *cost, double *grad) {
     return poison_on_failure([&]() -> int {
@@ -2494,17 +2526,16 @@ static int midend_callback_host(isdf_ctx *c, bool ragged, int B, int N0, const i
         if (int r = midend_check(c, ragged, B, N0, piece_off, p, &L)) return r;
         if (!head || !tail || !x || !cost || !grad || (L.P > (size_t)B && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
-        if (ragged) if (int r = ragged_upload(c->mid.d_off, piece_off, c->stream, &L)) return r;
-        const double *d_head, *d_tail, *d_wp;
-        if (int r = midend_upload(c, L, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return r;
-        CU_TRY(c->mid.d_x.upload(x, L.X, c->stream));
-        CU_TRY(c->mid.d_cost.ensure(B)); CU_TRY(c->mid.d_grad.ensure(L.X));
+        Staging S(c);
+        const double *d_head, *d_tail, *d_wp, *d_x;
+        double *d_cost, *d_grad;
+        stage_batch(S, ragged, piece_off, per_problem_bc, head, tail, &L, &d_head, &d_tail);
+        S.in(&d_wp, waypoints, 3 * (L.P - B)); S.in(&d_x, x, L.X);
+        S.out(&d_cost, cost, (size_t)B); S.out(&d_grad, grad, L.X);
+        if (int r = S.upload()) return r;
         if (int r = midend_buffers(c, L)) return r;
-        if (int r = midend_eval_launch(c, L, d_head, d_tail, per_problem_bc ? 9 : 0, p, d_wp, c->mid.d_x.p, c->mid.d_cost.p, c->mid.d_grad.p, c->stream)) return r;
-        CU_TRY(cudaMemcpyAsync(cost, c->mid.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaMemcpyAsync(grad, c->mid.d_grad.p, sizeof(double) * L.X, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaStreamSynchronize(c->stream));
-        return 0;
+        if (int r = midend_eval_launch(c, L, d_head, d_tail, per_problem_bc ? 9 : 0, p, d_wp, d_x, d_cost, d_grad, c->stream)) return r;
+        return S.download();
     }, [&] { nan_fill(cost, B); });
 }
 
@@ -2577,7 +2608,7 @@ extern "C" int isdf_midend_batch_ragged_device(isdf_ctx *c, int B, const int32_t
                          d_evaluations, rounds, (cudaStream_t)cuda_stream);
 }
 
-// the host form of getOriTraj: inputs staged in c->mid (a ragged batch's offsets first), results copied back
+// the host form of getOriTraj: inputs staged, results copied back; the final trajectories are computed also when T and coeffs are NULL
 static int midend_host(isdf_ctx *c, bool ragged, int B, int N0, const int32_t *piece_off, const double *head, const double *tail, int per_problem_bc,
                        const isdf_midend_params *p, const double *waypoints, double *x, double *T, double *coeffs, double *f, int32_t *ret,
                        int32_t *iterations, int32_t *evaluations, int32_t *rounds) {
@@ -2586,19 +2617,17 @@ static int midend_host(isdf_ctx *c, bool ragged, int B, int N0, const int32_t *p
         if (int r = midend_check(c, ragged, B, N0, piece_off, p, &L)) return r;
         if (!head || !tail || !x || !f || (L.P > (size_t)B && !waypoints)) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
-        if (ragged) if (int r = ragged_upload(c->mid.d_off, piece_off, c->stream, &L)) return r;
-        isdf_ctx::LbfgsBufs &lb = c->mid.lb;
-        const size_t BN = L.P;
+        Staging S(c);
         const double *d_head, *d_tail, *d_wp;
-        if (int r = midend_upload(c, L, per_problem_bc, head, tail, waypoints, &d_head, &d_tail, &d_wp)) return r;
-        CU_TRY(lb.d_x.ensure(L.X)); CU_TRY(lb.d_f.ensure((size_t)19 * BN + B)); CU_TRY(lb.d_head.ensure((size_t)3 * B));
-        double *d_f = lb.d_f.p, *d_T = d_f + B, *d_C = d_T + BN;   // [f | T | coeffs]
-        int *d_i = lb.d_head.p;
-        if (int r = midend_batch_run(c, L, d_head, d_tail, per_problem_bc, p, d_wp, lb.d_x.p, d_T, d_C, d_f, d_i, d_i + B, d_i + 2 * (size_t)B,
-                                     rounds, c->stream)) return r;
-        if (T) CU_TRY(cudaMemcpy(T, d_T, sizeof(double) * BN, cudaMemcpyDeviceToHost));
-        if (coeffs) CU_TRY(cudaMemcpy(coeffs, d_C, sizeof(double) * 18 * BN, cudaMemcpyDeviceToHost));
-        return lbfgs_copy_out(lb, B, L.X, x, f, ret, iterations, evaluations);
+        double *d_x, *d_f, *d_T, *d_C;
+        int *d_ret, *d_it, *d_ev;
+        stage_batch(S, ragged, piece_off, per_problem_bc, head, tail, &L, &d_head, &d_tail);
+        S.in(&d_wp, waypoints, 3 * (L.P - B));
+        S.out(&d_x, x, L.X); S.out(&d_T, T, L.P); S.out(&d_C, coeffs, 18 * L.P); S.out(&d_f, f, (size_t)B);   // x starts on the device
+        S.out(&d_ret, ret, (size_t)B); S.out(&d_it, iterations, (size_t)B); S.out(&d_ev, evaluations, (size_t)B);
+        if (int r = S.upload()) return r;
+        if (int r = midend_batch_run(c, L, d_head, d_tail, per_problem_bc, p, d_wp, d_x, d_T, d_C, d_f, d_ret, d_it, d_ev, rounds, c->stream)) return r;
+        return S.download();
     }, [&] { nan_fill(f, B); });
 }
 
@@ -2662,15 +2691,6 @@ static int clearance_check(isdf_ctx *c, int N, const isdf_clearance_params *p) {
     if (traj_batch(N, p->pieces_per_traj) == 0) return fail(ISDF_ERR_INVALID, "pieces_per_traj must be 0 or divide N");
     if ((long long)N * (p->samples_per_piece + 1) > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "N * (samples_per_piece + 1) must fit in 31 bits");
     return clearance_scene_check(c, p->reach, "sample");
-}
-
-// a host trajectory block [coeffs 18N | T N] staged in buf on c->stream: the coefficients at buf.p, the durations at *d_T
-static int stage_traj(isdf_ctx *c, DevBuf<double> &buf, int N, const double *T, const double *coeffs, const double **d_T) {
-    CU_TRY(buf.ensure((size_t)19 * N));
-    CU_TRY(cudaMemcpyAsync(buf.p, coeffs, sizeof(double) * 18 * N, cudaMemcpyHostToDevice, c->stream));
-    CU_TRY(cudaMemcpyAsync(buf.p + 18 * (size_t)N, T, sizeof(double) * N, cudaMemcpyHostToDevice, c->stream));
-    *d_T = buf.p + 18 * (size_t)N;
-    return 0;
 }
 
 // the clearance scan of N sources in groups of N0 (0: one group) with reach and margin: the K + 1 uniform samples of each piece of
@@ -2747,18 +2767,17 @@ extern "C" int isdf_trajectory_clearance(isdf_ctx *c, int N, const double *T, co
         if (int r = clearance_check(c, N, p)) return r;
         if (!T || !coeffs || !summary) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
-        const int B = traj_batch(N, p->pieces_per_traj);
         const size_t S = (size_t)N * (p->samples_per_piece + 1);
-        const double *d_T;
-        if (int r = stage_traj(c, c->clr.d_in, N, T, coeffs, &d_T)) return r;
-        CU_TRY(c->clr.d_clear.ensure(S)); CU_TRY(c->clr.d_vox.ensure(S)); CU_TRY(c->clr.d_sum.ensure((size_t)B));
-        if (int r = isdf_trajectory_clearance_device(c, N, d_T, c->clr.d_in.p, p, c->clr.d_clear.p, (int64_t *)c->clr.d_vox.p,
-                                                     (isdf_clearance_summary *)c->clr.d_sum.p, c->stream)) return r;
-        CU_TRY(cudaMemcpyAsync(summary, c->clr.d_sum.p, sizeof(isdf_clearance_summary) * B, cudaMemcpyDeviceToHost, c->stream));
-        if (sample_clearance) CU_TRY(cudaMemcpyAsync(sample_clearance, c->clr.d_clear.p, sizeof(double) * S, cudaMemcpyDeviceToHost, c->stream));
-        if (sample_voxel) CU_TRY(cudaMemcpyAsync(sample_voxel, c->clr.d_vox.p, sizeof(int64_t) * S, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaStreamSynchronize(c->stream));
-        return 0;
+        Staging St(c);
+        const double *d_C, *d_T;
+        double *d_clear;
+        int64_t *d_vox;
+        isdf_clearance_summary *d_sum;
+        St.in(&d_C, coeffs, 18 * (size_t)N); St.in(&d_T, T, (size_t)N);
+        St.out(&d_sum, summary, (size_t)traj_batch(N, p->pieces_per_traj)); St.out(&d_clear, sample_clearance, S); St.out(&d_vox, sample_voxel, S);
+        if (int r = St.upload()) return r;
+        if (int r = isdf_trajectory_clearance_device(c, N, d_T, d_C, p, d_clear, d_vox, d_sum, c->stream)) return r;
+        return St.download();
     }, [&] { write_failed_summaries(summary, p ? traj_batch(N, p->pieces_per_traj) : 0, clearance_failed_summary()); });
 }
 
@@ -2803,23 +2822,16 @@ extern "C" int isdf_pose_clearance(isdf_ctx *c, int64_t Q, const double *pos, co
         if (int r = pose_clearance_check(c, Q, pos, quat, stride, p)) return r;
         if (!summary) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
-        const int B = traj_batch(Q, p->poses_per_group);
-        // the poses packed 7 doubles apart (x, y, z, w, qx, qy, qz) in one copy, then the device form
-        std::vector<double> h((size_t)Q * 7);
-        for (int64_t q = 0; q < Q; q++) {
-            for (int k = 0; k < 3; k++) h[7 * q + k] = pos[q * stride + k];
-            for (int k = 0; k < 4; k++) h[7 * q + 3 + k] = quat[q * stride + k];
-        }
-        CU_TRY(c->clr.d_in.ensure(h.size()));
-        CU_TRY(cudaMemcpyAsync(c->clr.d_in.p, h.data(), sizeof(double) * h.size(), cudaMemcpyHostToDevice, c->stream));
-        CU_TRY(c->clr.d_clear.ensure((size_t)Q)); CU_TRY(c->clr.d_vox.ensure((size_t)Q)); CU_TRY(c->clr.d_sum.ensure((size_t)B));
-        if (int r = isdf_pose_clearance_device(c, Q, c->clr.d_in.p, c->clr.d_in.p + 3, 7, p, c->clr.d_clear.p, (int64_t *)c->clr.d_vox.p,
-                                               (isdf_clearance_summary *)c->clr.d_sum.p, c->stream)) return r;
-        CU_TRY(cudaMemcpyAsync(summary, c->clr.d_sum.p, sizeof(isdf_clearance_summary) * B, cudaMemcpyDeviceToHost, c->stream));
-        if (clear) CU_TRY(cudaMemcpyAsync(clear, c->clr.d_clear.p, sizeof(double) * Q, cudaMemcpyDeviceToHost, c->stream));
-        if (voxel) CU_TRY(cudaMemcpyAsync(voxel, c->clr.d_vox.p, sizeof(int64_t) * Q, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaStreamSynchronize(c->stream));
-        return 0;
+        Staging S(c);
+        const double *d_pose;
+        double *d_clear;
+        int64_t *d_vox;
+        isdf_clearance_summary *d_sum;
+        stage_poses(S, Q, pos, quat, stride, &d_pose);
+        S.out(&d_sum, summary, (size_t)traj_batch(Q, p->poses_per_group)); S.out(&d_clear, clear, (size_t)Q); S.out(&d_vox, voxel, (size_t)Q);
+        if (int r = S.upload()) return r;
+        if (int r = isdf_pose_clearance_device(c, Q, d_pose, d_pose + 3, 7, p, d_clear, d_vox, d_sum, c->stream)) return r;
+        return S.download();
     }, [&] { write_failed_summaries(summary, p ? traj_batch(Q, p->poses_per_group) : 0, clearance_failed_summary()); });
 }
 
@@ -3005,23 +3017,22 @@ extern "C" int isdf_trajectory_certify_device(isdf_ctx *c, int N, const double *
     }, [&] { if (c) write_failed_summaries(d_summary, certify_batch(N, p), certify_failed_summary(), c, st); });
 }
 
-// the host form of a certificate over its device form: check(), the trajectory block staged in part(c).ref.d_in, B summaries through
-// part(c).d_sum, synchronised; on failure max(B, 1) summaries read `bad`
-template <class S, class P, class Check, class Part>
+// the host form of a certificate over its device form: check(), the trajectory block in and B summaries out through the staging; on
+// failure max(B, 1) summaries read `bad`
+template <class S, class P, class Check>
 static int certificate_host(isdf_ctx *c, int N, const double *T, const double *coeffs, const P *p, S *summary, int B, const S &bad, Check check,
-                            Part part, int (*device)(isdf_ctx *, int, const double *, const double *, const P *, S *, void *)) {
+                            int (*device)(isdf_ctx *, int, const double *, const double *, const P *, S *, void *)) {
     return poison_on_failure([&]() -> int {
         if (int rc = check()) return rc;
         if (!T || !coeffs || !summary) return fail(ISDF_ERR_INVALID, "NULL argument");
         if (set_device(c)) return ISDF_ERR_CUDA;
-        auto &z = part(c);
-        const double *d_T;
-        if (int rc = stage_traj(c, z.ref.d_in, N, T, coeffs, &d_T)) return rc;
-        CU_TRY(z.d_sum.ensure((size_t)B));
-        if (int rc = device(c, N, d_T, z.ref.d_in.p, p, (S *)z.d_sum.p, c->stream)) return rc;
-        CU_TRY(cudaMemcpyAsync(summary, z.d_sum.p, sizeof(S) * B, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaStreamSynchronize(c->stream));
-        return 0;
+        Staging St(c);
+        const double *d_C, *d_T;
+        S *d_sum;
+        St.in(&d_C, coeffs, 18 * (size_t)N); St.in(&d_T, T, (size_t)N); St.out(&d_sum, summary, (size_t)B);
+        if (int rc = St.upload()) return rc;
+        if (int rc = device(c, N, d_T, d_C, p, d_sum, c->stream)) return rc;
+        return St.download();
     }, [&] { write_failed_summaries(summary, B, bad); });
 }
 
@@ -3029,7 +3040,7 @@ extern "C" int isdf_trajectory_certify(isdf_ctx *c, int N, const double *T, cons
                                        isdf_certify_summary *summary) {
     double r = 0.0;
     return certificate_host(c, N, T, coeffs, p, summary, certify_batch(N, p), certify_failed_summary(), [&] { return certify_check(c, N, p, &r); },
-                            [](isdf_ctx *x) -> auto & { return x->cert; }, isdf_trajectory_certify_device);
+                            isdf_trajectory_certify_device);
 }
 
 // ---- dynamic-limit certificate (isdf_dynlimits.cuh) -------------------------------------------------------------------------------
@@ -3119,7 +3130,7 @@ extern "C" int isdf_trajectory_dynamics_device(isdf_ctx *c, int N, const double 
 extern "C" int isdf_trajectory_dynamics(isdf_ctx *c, int N, const double *T, const double *coeffs, const isdf_dynamics_params *p,
                                         isdf_dynamics_summary *summary) {
     return certificate_host(c, N, T, coeffs, p, summary, dynamics_batch(N, p), dynamics_failed_summary(), [&] { return dynamics_check(c, N, p); },
-                            [](isdf_ctx *x) -> auto & { return x->dyn; }, isdf_trajectory_dynamics_device);
+                            isdf_trajectory_dynamics_device);
 }
 
 // ---- certified swept volume (isdf_sweptvol.cuh) ------------------------------------------------------------------------------------
@@ -3276,19 +3287,15 @@ extern "C" int isdf_swept_volume_sdf(isdf_ctx *c, int N, const double *T, const 
         for (long long i = 0; i < 3ll * n; i++) if (!std::isfinite(pts[i])) return fail(ISDF_ERR_INVALID, "points must be finite");
         if (n == 0) return 0;
         if (set_device(c)) return ISDF_ERR_CUDA;
-        auto &z = c->svol;
-        const double *d_T;
-        if (int rc = stage_traj(c, z.d_in, N, T, coeffs, &d_T)) return rc;
-        CU_TRY(z.d_pts.upload(pts, (size_t)3 * n, c->stream));
-        CU_TRY(z.d_val.ensure(n)); CU_TRY(z.d_low.ensure(n)); CU_TRY(z.d_ts.ensure(n)); CU_TRY(z.d_dec.ensure(n));
-        if (int rc = swept_run(c, N, d_T, z.d_in.p, p, r_rot, r_body, nullptr, n, z.d_pts.p, z.d_val.p, z.d_low.p, z.d_ts.p, z.d_dec.p, nullptr, c->stream))
-            return rc;
-        CU_TRY(cudaMemcpyAsync(value, z.d_val.p, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
-        if (lower) CU_TRY(cudaMemcpyAsync(lower, z.d_low.p, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
-        if (tstar) CU_TRY(cudaMemcpyAsync(tstar, z.d_ts.p, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
-        if (decided) CU_TRY(cudaMemcpyAsync(decided, z.d_dec.p, (size_t)n, cudaMemcpyDeviceToHost, c->stream));
-        CU_TRY(cudaStreamSynchronize(c->stream));
-        return 0;
+        Staging S(c);
+        const double *d_C, *d_T, *d_pts;
+        double *d_val, *d_low, *d_ts;
+        uint8_t *d_dec;
+        S.in(&d_C, coeffs, 18 * (size_t)N); S.in(&d_T, T, (size_t)N); S.in(&d_pts, pts, (size_t)3 * n);
+        S.out(&d_val, value, (size_t)n); S.out(&d_low, lower, (size_t)n); S.out(&d_ts, tstar, (size_t)n); S.out(&d_dec, decided, (size_t)n);
+        if (int rc = S.upload()) return rc;
+        if (int rc = swept_run(c, N, d_T, d_C, p, r_rot, r_body, nullptr, n, d_pts, d_val, d_low, d_ts, d_dec, nullptr, c->stream)) return rc;
+        return S.download();
     }, [&] { swept_poison_host(std::max(n, 0), value, lower, tstar, decided); });
 }
 
@@ -3322,10 +3329,12 @@ static int swept_grid_ctx(isdf_ctx *c, int N, const double *T, const double *coe
     if (set_device(c)) return ISDF_ERR_CUDA;
     auto &z = c->svol;
     const size_t n = (size_t)swept_nodes(g);
-    const double *d_T;
-    if (int rc = stage_traj(c, z.d_in, N, T, coeffs, &d_T)) return rc;
+    Staging S(c);
+    const double *d_C, *d_T;
+    S.in(&d_C, coeffs, 18 * (size_t)N); S.in(&d_T, T, (size_t)N);
+    if (int rc = S.upload()) return rc;
     CU_TRY(z.d_val.ensure(n)); CU_TRY(z.d_low.ensure(n)); CU_TRY(z.d_ts.ensure(n)); CU_TRY(z.d_dec.ensure(n));
-    return swept_run(c, N, d_T, z.d_in.p, p, r_rot, r_body, g, 0, nullptr, z.d_val.p, z.d_low.p, z.d_ts.p, z.d_dec.p, info, c->stream);
+    return swept_run(c, N, d_T, d_C, p, r_rot, r_body, g, 0, nullptr, z.d_val.p, z.d_low.p, z.d_ts.p, z.d_dec.p, info, c->stream);
 }
 
 extern "C" int isdf_swept_volume_grid(isdf_ctx *c, int N, const double *T, const double *coeffs, const isdf_swept_params *p,
@@ -3735,20 +3744,19 @@ extern "C" int isdf_frontend_check_batch(isdf_ctx *c, int n, const int32_t *ind,
         if (ind[3 * q] < 0 || ind[3 * q] >= c->map.grid.X || ind[3 * q + 1] < 0 || ind[3 * q + 1] >= c->map.grid.Y || ind[3 * q + 2] < 0 || ind[3 * q + 2] >= c->map.grid.Z)
             return fail(ISDF_ERR_INVALID, "voxel index outside the map");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    CU_TRY(c->fe.d_ind.upload(ind, (size_t)3 * n, c->stream));
-    CU_TRY(c->fe.d_father.upload(father_roll_pitch, (size_t)2 * n, c->stream));
-    CU_TRY(c->fe.d_child.ensure((size_t)2 * n)); CU_TRY(c->fe.d_ok.ensure(n)); CU_TRY(c->fe.d_out.ensure((size_t)4 * n));
+    Staging S(c);
     FrontArgs A = front_args(c);
-    A.out = c->fe.d_out.p; A.nq = n; A.q_ind = c->fe.d_ind.p; A.q_father = c->fe.d_father.p; A.q_child = c->fe.d_child.p; A.q_ok = c->fe.d_ok.p;
+    S.in(&A.q_ind, ind, (size_t)3 * n); S.in(&A.q_father, father_roll_pitch, (size_t)2 * n);
+    S.out(&A.q_child, child_roll_pitch, (size_t)2 * n); S.out(&A.q_ok, ok, (size_t)n);
+    if (int rr = S.upload()) return rr;
+    CU_TRY(c->fe.d_out.ensure((size_t)4 * n));
+    A.out = c->fe.d_out.p; A.nq = n;
     const size_t smem = sizeof(uint32_t) * 4 * (size_t)A.ks * A.ks * A.ks;
     CU_TRY(cudaFuncSetAttribute(k_frontend_check, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k_frontend_check<<<(unsigned)((n + 255) / 256), 256, smem, c->stream>>>(A);
     c->stats.kernel_launches++;
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(child_roll_pitch, c->fe.d_child.p, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaMemcpyAsync(ok, c->fe.d_ok.p, n, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaStreamSynchronize(c->stream));
-    return 0;
+    return S.download();
 }
 
 // ---- front-end path search (isdf_frontpath.cuh) ------------------------------------------------------------------------------------
@@ -4616,17 +4624,12 @@ static int eval_swept_host(isdf_ctx *c, int N, const double *T, const double *co
     if (int r = check_eval_state(c, N, false)) return r;
     if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
     if (!T || !coeffs || !cost || !gradC || !gradT) return fail(ISDF_ERR_INVALID, "NULL argument");
-    DevBuf<double> dgt, dgs, dgg;
-    return eval_host(c, N, T, coeffs, cost, gradC, gradT, &isdf_stats::last_sdf_evals,
-                     [&]() -> int {
-                         if (g_t) {
-                             CU_TRY(dgt.upload(g_t, c->sv.P, c->stream)); CU_TRY(dgs.upload(g_s, c->sv.P, c->stream));
-                             CU_TRY(dgg.upload(g_g, (size_t)3 * c->sv.P, c->stream));
-                         }
-                         return 0;
-                     },
+    Staging S(c);
+    const double *dgt = nullptr, *dgs = nullptr, *dgg = nullptr;
+    if (g_t) { S.in(&dgt, g_t, (size_t)c->sv.P); S.in(&dgs, g_s, (size_t)c->sv.P); S.in(&dgg, g_g, (size_t)3 * c->sv.P); }
+    return eval_host(c, S, N, T, coeffs, cost, gradC, gradT, &isdf_stats::last_sdf_evals,
                      [&](const double *d_T, const double *d_C, double *d_out, double *count_out) {
-                         return swept_common(c, N, d_T, d_C, d_out, count_out, c->stream, dgt.p, dgs.p, dgg.p);
+                         return swept_common(c, N, d_T, d_C, d_out, count_out, c->stream, dgt, dgs, dgg);
                      });
 }
 
@@ -4731,14 +4734,13 @@ extern "C" int isdf_dbg_item_table(isdf_ctx *c, long long *info, int *items, lon
 extern "C" int isdf_dbg_flatness(isdf_ctx *c, int n, const double *vaj, const double *grads, double *out) {
     if (!c || n < 1 || !vaj || !grads || !out) return fail(ISDF_ERR_INVALID, "bad argument");
     if (set_device(c)) return ISDF_ERR_CUDA;
-    DevBuf<double> dv, dg, dout;
-    CU_TRY(dv.upload(vaj, (size_t)9 * n, c->stream));
-    CU_TRY(dg.upload(grads, (size_t)10 * n, c->stream));
-    CU_TRY(dout.ensure((size_t)16 * n));
-    CU_TRY(discrete_launch_dbg_flatness(c->dcfg.fp, n, dv.p, dg.p, dout.p, c->stream));
-    CU_TRY(cudaMemcpyAsync(out, dout.p, sizeof(double) * 16 * n, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaStreamSynchronize(c->stream));
-    return 0;
+    Staging S(c);
+    const double *dv, *dg;
+    double *dout;
+    S.in(&dv, vaj, (size_t)9 * n); S.in(&dg, grads, (size_t)10 * n); S.out(&dout, out, (size_t)16 * n);
+    if (int r = S.upload()) return r;
+    CU_TRY(discrete_launch_dbg_flatness(c->dcfg.fp, n, dv, dg, dout, c->stream));
+    return S.download();
 }
 // read-only view of the current mesh's body-frame cell grid, so tests can tell which search branch answers a query:
 // geom = {glo[3], gcell, ghd, gpad, sign_radius, list_reach}, gdim[3]; cell_dist / cell_cnt (gdim[0]*gdim[1]*gdim[2] entries, z fastest)
@@ -4837,21 +4839,17 @@ extern "C" int isdf_dbg_certify_bound(isdf_ctx *c, int N, const double *T, const
     if (int rr = certify_shape(c, &r)) return rr;
     if (radius) *radius = r;
     if (set_device(c)) return ISDF_ERR_CUDA;
-    DevBuf<double> d;   // [coeffs 18N | T N | ta n | tb n | out 2n]
-    CU_TRY(d.ensure((size_t)19 * N + 4 * (size_t)n));
-    const double *dT;
-    if (int rr = stage_traj(c, d, N, T, coeffs, &dT)) return rr;
-    DevBuf<int> dp;
-    CU_TRY(dp.upload(piece, n, c->stream));
-    double *dta = d.p + 19 * (size_t)N, *dtb = dta + n, *dout = dtb + n;
-    CU_TRY(cudaMemcpyAsync(dta, ta, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
-    CU_TRY(cudaMemcpyAsync(dtb, tb, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
-    const CertArgs A = certify_args(c, r, reach, N, dT, d.p);
-    CU_TRY(certify_bound_launch(A, n, dp.p, dta, dtb, dout, c->stream));
+    Staging S(c);
+    const double *dC, *dT, *dta, *dtb;
+    const int *dp;
+    double *dout;
+    S.in(&dC, coeffs, 18 * (size_t)N); S.in(&dT, T, (size_t)N); S.in(&dp, piece, (size_t)n); S.in(&dta, ta, (size_t)n); S.in(&dtb, tb, (size_t)n);
+    S.out(&dout, out, 2 * (size_t)n);
+    if (int rr = S.upload()) return rr;
+    const CertArgs A = certify_args(c, r, reach, N, dT, dC);
+    CU_TRY(certify_bound_launch(A, n, dp, dta, dtb, dout, c->stream));
     c->stats.kernel_launches++;
-    CU_TRY(cudaMemcpyAsync(out, dout, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaStreamSynchronize(c->stream));
-    return 0;
+    return S.download();
 }
 
 // the final leaf intervals of the last certificate call: records {ta, tb, c_a, c_b, D_a, D_b (double); piece (index in the call's block),

@@ -1017,8 +1017,8 @@ int isdf_get_plan_info(isdf_ctx *ctx, isdf_plan_info *out);
  * Every record depends only on its own (traj, time) and that trajectory's data, not on B, Q, the order of the queries or other trajectories.
  * A query on a trajectory without pieces (a NO_PATH or TOO_LONG plan) gets an all-NaN record.
  * Needs a context (its stream and config); no map and no shape. Q = 0 does nothing. The call counts its launch in
- * isdf_stats.kernel_launches and touches no other field. Device memory is the context's, grown on demand; the host form stages through one
- * pinned block, one copy each way.
+ * isdf_stats.kernel_launches and touches no other field. Device memory is the context's, grown on demand; the host form stages through the
+ * context's pinned and device staging blocks, which every host form shares: one copy each way.
  * Errors (host form; nothing is written): ISDF_ERR_INVALID for a NULL pointer, B < 1, Q < 0 or Q records beyond 2^63 bytes,
  *   piece_off[0] != 0 or offsets that decrease, a duration that is not positive and finite, a coefficient that is not finite, or traj[q]
  *   outside [0, B). */

@@ -61,7 +61,7 @@ def stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-def make_ev(fault, shape="Ball", points=False, kernels=False):
+def make_ev(fault, shape="Ball", points=False, kernels=False, esdf=False, scene=False):
     cfg = I.default_config_values()
     cfg.flags = I.WITH_DYNAMICS | I.WITH_COLLISION
     cfg.integral_intervs = K
@@ -74,12 +74,16 @@ def make_ev(fault, shape="Ball", points=False, kernels=False):
         ev.set_points(PTS)
     if kernels and "nokernels" not in fault:
         ev.frontend_build_kernels()
+    if esdf and "noesdf" not in fault:
+        ev.map_esdf()
+    if scene and "noscene" not in fault:
+        ev.set_sense_cloud((np.argwhere(OCC) + 0.5).astype(np.float32))
     if "shard" in fault:
         ev.set_shard(0, 2)
     return ev
 
 
-# ---- the nine pairs: (host call, device call) -> (return code, outputs) ------------------------------------------------------------
+# ---- the pairs: (host call, device call) -> (return code, outputs) ------------------------------------------------------------
 def eval_host(name):
     def run(ev, h, fault):
         cost, gC, gT = C.c_double(0.0), np.zeros(18 * N), np.zeros(N)
@@ -172,9 +176,9 @@ def summaries(cls, raw):
     return [s.as_dict() for s in (cls * (N // N0)).from_buffer_copy(raw)]
 
 
-def device_summary_buffer(cls):
+def device_summary_buffer(cls, n=N // N0):
     import torch
-    return torch.zeros(C.sizeof(cls) * (N // N0), dtype=torch.uint8, device="cuda")   # reads as "clear" until a failure poisons it
+    return torch.zeros(C.sizeof(cls) * n, dtype=torch.uint8, device="cuda")   # reads as "clear" until a failure poisons it
 
 
 def clearance_params(ev, fault):
@@ -250,6 +254,188 @@ def frontend_device(ev, h, fault):
     return r, dict(masks=d.cpu().numpy().view(np.uint32))
 
 
+# trajectory states: one trajectory, QS query times across it
+OFF1 = np.array([0, N], dtype=np.int32)
+QS = 64
+
+
+def state_times(Q):
+    return np.ascontiguousarray(np.linspace(0.0, float(T.sum()), Q)), np.zeros(Q, dtype=np.int32)
+
+
+def states_host(ev, h, fault, Q=QS):
+    times, traj = state_times(Q)
+    out = np.zeros(Q * I.STATE_DOUBLES)
+    r = ev.lib.isdf_trajectory_states(h, 0 if "param" in fault else 1, host_ptr(OFF1, fault, True, IP), T.ctypes.data_as(DP), CC.ctypes.data_as(DP),
+                                      Q, traj.ctypes.data_as(IP), times.ctypes.data_as(DP), out.ctypes.data_as(DP))
+    return r, dict(out=out)
+
+
+def states_device(ev, h, fault):
+    times, traj = state_times(QS)
+    doff, dT, dC, dtraj, dtimes, dout = dev(OFF1), dev(T), dev(CC), dev(traj), dev(times), dev(np.zeros(QS * I.STATE_DOUBLES))
+    r = ev.lib.isdf_trajectory_states_device(h, 0 if "param" in fault else 1, ptr(doff, fault, True), ptr(dT, fault), ptr(dC, fault), QS,
+                                             ptr(dtraj, fault), ptr(dtimes, fault), ptr(dout, fault), stream())
+    return r, dict(out=dout.cpu().numpy())
+
+
+# posed body points: QP state records (every field drawn, so every input reaches the result), NBODY body points
+QP, NBODY = 16, 7
+STATES = np.random.default_rng(3).normal(size=QP * I.STATE_DOUBLES)
+BODY = np.random.default_rng(4).normal(size=3 * NBODY)
+
+
+def pose_points_host(ev, h, fault):
+    out = np.zeros(QP * NBODY * 3)
+    r = ev.lib.isdf_pose_points(h, QP, host_ptr(STATES, fault, True), -1 if "param" in fault else NBODY, BODY.ctypes.data_as(DP), out.ctypes.data_as(DP))
+    return r, dict(out=out)
+
+
+def pose_points_device(ev, h, fault):
+    ds, db, dout = dev(STATES), dev(BODY), dev(np.zeros(QP * NBODY * 3))
+    r = ev.lib.isdf_pose_points_device(h, QP, ptr(ds, fault, True), -1 if "param" in fault else NBODY, ptr(db, fault), ptr(dout, fault), stream())
+    return r, dict(out=dout.cpu().numpy())
+
+
+# closed loop: two rollouts of the trajectory, one under a side force
+RS = 2
+SIM_TRAJ = np.zeros(RS, dtype=np.int32)
+SIM_DIST = np.zeros((RS, 6))
+SIM_DIST[1, 1] = 0.5
+
+
+def sim_setup(fault):
+    p = I.sim_default_params(t_end=0.5, log_every=5)
+    if "param" in fault:
+        p.reserved_ = 1
+    init = np.ascontiguousarray(I.sim_init_from_trajectories(OFF1, CC, SIM_TRAJ, p))
+    return p, init, I.sim_log_records(p)
+
+
+def sim_summaries(raw):
+    return [s.as_dict() for s in (I.SimSummary * RS).from_buffer_copy(raw)]
+
+
+def simulate_host(ev, h, fault):
+    p, init, n_log = sim_setup(fault)
+    log, summ = np.zeros(RS * n_log * I.SIM_DOUBLES), (I.SimSummary * RS)()
+    r = ev.lib.isdf_simulate(h, 1, host_ptr(OFF1, fault, True, IP), T.ctypes.data_as(DP), CC.ctypes.data_as(DP), RS, SIM_TRAJ.ctypes.data_as(IP),
+                             init.ctypes.data_as(DP), SIM_DIST.ctypes.data_as(DP), C.byref(p), n_log, log.ctypes.data_as(DP), summ)
+    return r, dict(log=log, summary=[s.as_dict() for s in summ])
+
+
+def simulate_device(ev, h, fault):
+    import torch
+    p, init, n_log = sim_setup(fault)
+    doff, dT, dC, dtraj, dinit, ddist = dev(OFF1), dev(T), dev(CC), dev(SIM_TRAJ), dev(init), dev(SIM_DIST)
+    dlog, dsum = dev(np.zeros(RS * n_log * I.SIM_DOUBLES)), torch.zeros(C.sizeof(I.SimSummary) * RS, dtype=torch.uint8, device="cuda")
+    r = ev.lib.isdf_simulate_device(h, 1, ptr(doff, fault, True), ptr(dT, fault), ptr(dC, fault), RS, ptr(dtraj, fault), ptr(dinit, fault),
+                                    ptr(ddist, fault), C.byref(p), n_log, ptr(dlog, fault), ptr(dsum, fault), stream())
+    return r, dict(log=dlog.cpu().numpy(), summary=sim_summaries(dsum.cpu().numpy().tobytes()))
+
+
+def poisoned_sim_summary(s):
+    nans = ("max_err", "t_max_err", "rms_err", "final_err", "max_tilt", "max_omega", "t_diverged")
+    counts = ("accepted", "rejected", "clamped_steps", "floor_contacts", "nan_rollbacks")
+    return all(math.isnan(s[k]) for k in nans) and all(s[k] == -1 for k in counts) and s["diverged"] == 1
+
+
+# ESDF queries, inside and outside the map
+QE = 50
+EPTS = np.random.default_rng(5).uniform(-2.0, 26.0, size=3 * QE)
+
+
+def esdf_host(ev, h, fault):
+    dist, grad = np.zeros(QE), np.zeros(3 * QE)
+    r = ev.lib.isdf_esdf_query(h, 7 if "param" in fault else 2, host_ptr(EPTS, fault, True), QE, dist.ctypes.data_as(DP), grad.ctypes.data_as(DP))
+    return r, dict(dist=dist, grad=grad)
+
+
+def esdf_device(ev, h, fault):
+    dp_, ddist, dgrad = dev(EPTS), dev(np.zeros(QE)), dev(np.zeros(3 * QE))
+    r = ev.lib.isdf_esdf_query_device(h, 7 if "param" in fault else 2, ptr(dp_, fault, True), QE, ptr(ddist, fault), ptr(dgrad, fault), stream())
+    return r, dict(dist=ddist.cpu().numpy(), grad=dgrad.cpu().numpy())
+
+
+# poses as (x, y, z, w, qx, qy, qz) records, in groups of QG
+QC, QG = 12, 6
+
+
+def pose_records():
+    rng = np.random.default_rng(6)
+    q = rng.normal(size=(QC, 4))
+    return np.ascontiguousarray(np.concatenate([rng.uniform(2.0, 22.0, size=(QC, 3)), q / np.linalg.norm(q, axis=1, keepdims=True)], axis=1))
+
+
+POSES = pose_records()
+
+
+def pose_clearance_params(ev, fault):
+    p = ev.pose_clearance_params(2.0, 0.5, QG)
+    if "param" in fault:
+        p.reserved_ = 1
+    return p
+
+
+def pose_clearance_host(ev, h, fault):
+    clear, vox, summ = np.zeros(QC), np.zeros(QC, dtype=np.int64), (I.ClearanceSummary * (QC // QG))()
+    base = POSES.ctypes.data
+    r = ev.lib.isdf_pose_clearance(h, QC, None if "null" in fault else C.cast(base, DP), C.cast(base + 24, DP), 7,
+                                   C.byref(pose_clearance_params(ev, fault)), clear.ctypes.data_as(DP), vox.ctypes.data_as(C.POINTER(C.c_int64)), summ)
+    return r, dict(clear=clear, vox=vox, summary=[s.as_dict() for s in summ])
+
+
+def pose_clearance_device(ev, h, fault):
+    dpose, dclear, dvox = dev(POSES), dev(np.zeros(QC)), dev(np.zeros(QC, dtype=np.int64))
+    dsum = device_summary_buffer(I.ClearanceSummary, QC // QG)
+    r = ev.lib.isdf_pose_clearance_device(h, QC, ptr(dpose, fault, True), C.c_void_p(dpose.data_ptr() + 24), 7, C.byref(pose_clearance_params(ev, fault)),
+                                          ptr(dclear, fault), ptr(dvox, fault), ptr(dsum, fault), stream())
+    return r, dict(clear=dclear.cpu().numpy(), vox=dvox.cpu().numpy(), summary=summaries(I.ClearanceSummary, dsum.cpu().numpy().tobytes()))
+
+
+# the certified swept volume of the trajectory on a 1-unit grid around it
+def swept_setup(ev, fault):
+    p = ev.swept_params(K, max_depth=65 if "param" in fault else None)
+    return p, I.swept_grid_for(T, CC, 1.0, p.band, 1.0)
+
+
+def swept_grid_host(ev, h, fault):
+    p, g = swept_setup(ev, fault)
+    n = g.X * g.Y * g.Z
+    val, low, ts, dec = np.zeros(n), np.zeros(n), np.zeros(n), np.zeros(n, dtype=np.uint8)
+    r = ev.lib.isdf_swept_volume_grid(h, N, host_ptr(T, fault, True), CC.ctypes.data_as(DP), C.byref(p), C.byref(g), val.ctypes.data_as(DP),
+                                      low.ctypes.data_as(DP), ts.ctypes.data_as(DP), dec.ctypes.data_as(C.POINTER(C.c_uint8)), None)
+    return r, dict(value=val, lower=low, tstar=ts, decided=dec)
+
+
+def swept_grid_device(ev, h, fault):
+    p, g = swept_setup(ev, fault)
+    n = g.X * g.Y * g.Z
+    dT, dC, dval, dlow, dts, ddec = dev(T), dev(CC), dev(np.zeros(n)), dev(np.zeros(n)), dev(np.zeros(n)), dev(np.zeros(n, dtype=np.uint8))
+    r = ev.lib.isdf_swept_volume_grid_device(h, N, ptr(dT, fault, True), ptr(dC, fault), C.byref(p), C.byref(g), ptr(dval, fault), ptr(dlow, fault),
+                                             ptr(dts, fault), ptr(ddec, fault), None, stream())
+    return r, dict(value=dval.cpu().numpy(), lower=dlow.cpu().numpy(), tstar=dts.cpu().numpy(), decided=ddec.cpu().numpy())
+
+
+# depth images of the map's occupied voxel centres at the poses above
+def sense_host(ev, h, fault):
+    p = I.sense_params(width=64, height=48)
+    depth = np.zeros(QC * p.height * p.width, dtype=np.int32)
+    base = POSES.ctypes.data
+    r = ev.lib.isdf_sense_depth(h, 0 if "param" in fault else QC, None if "null" in fault else C.c_void_p(base), C.c_void_p(base + 24), 7,
+                                C.byref(p), depth.ctypes.data_as(C.c_void_p))
+    return r, dict(depth=depth)
+
+
+def sense_device(ev, h, fault):
+    import torch
+    p = I.sense_params(width=64, height=48)
+    dpose, ddepth = dev(POSES), torch.zeros(QC * p.height * p.width, dtype=torch.int32, device="cuda")
+    r = ev.lib.isdf_sense_depth_device(h, 0 if "param" in fault else QC, ptr(dpose, fault, True), C.c_void_p(dpose.data_ptr() + 24), 7, C.byref(p),
+                                       ptr(ddepth, fault), stream())
+    return r, dict(depth=ddepth.cpu().numpy())
+
+
 # name -> (host, device, make_ev keywords, {fault: code}). "nomap+null" / "shard+null" pin the order of the checks: the state is
 # checked before the pointers; "size+nomap" / "size+shard" pin where each certificate checks its 31-bit size: after the state checks
 # for the clearance certificate, before the shard check for the dynamic-limit certificate.
@@ -271,7 +457,17 @@ PAIRS = {
     "trajectory_dynamics": (dynamics_host, dynamics_device, {}, {"ctx": -1, "null": -1, "param": -1, "shard": -4, "size": -1, "size+shard": -1}),
     "frontend_feasibility": (frontend_host, frontend_device, dict(kernels=True),
                              {"ctx": -1, "null": -1, "nomap": -2, "nokernels": -2, "nokernels+null": -2}),
+    "trajectory_states": (states_host, states_device, {}, {"ctx": -1, "null": -1, "param": -1}),
+    "pose_points": (pose_points_host, pose_points_device, {}, {"ctx": -1, "null": -1, "param": -1}),
+    "simulate": (simulate_host, simulate_device, {}, {"ctx": -1, "null": -1, "param": -1}),
+    "esdf_query": (esdf_host, esdf_device, dict(esdf=True), {"ctx": -1, "null": -1, "param": -1, "noesdf": -2}),
+    "pose_clearance": (pose_clearance_host, pose_clearance_device, {},
+                       {"ctx": -1, "null": -1, "param": -1, "nomap": -2, "noshape": -2, "shard": -4}),
+    "swept_volume_grid": (swept_grid_host, swept_grid_device, {}, {"ctx": -1, "null": -1, "param": -1, "noshape": -2, "shard": -4}),
+    "sense_depth": (sense_host, sense_device, dict(scene=True), {"ctx": -1, "null": -1, "param": -1, "noscene": -2}),
 }
+# the pairs whose device form poisons its outputs with a kernel (counted in kernel_launches) when it has a context
+POISON_KERNEL = {"simulate"}
 
 
 def call(pair, form, fault):
@@ -328,7 +524,7 @@ def test_refusals_agree_and_poison(pair, fault):
     for form in ("host", "device"):
         r, err, outs, launches, ms = call(pair, form, fault)
         assert r == code and err, (form, r, err)
-        assert launches == 0 and not ms, form
+        assert launches == (pair in POISON_KERNEL and form == "device" and fault != "ctx") and not ms, form
         # poisoned outputs (include/isdf.h); a device form cannot write to a device pointer without a context
         if form == "host" or fault != "ctx":
             if pair == "eval_discrete" or pair == "eval_swept":
@@ -337,5 +533,37 @@ def test_refusals_agree_and_poison(pair, fault):
                 assert form == "device" or np.all(np.isnan(outs["cost"]))
             elif pair in ("lbfgs_batch", "midend_batch"):
                 assert np.all(np.isnan(outs["f"])), form
-            elif pair in ("trajectory_clearance", "trajectory_certify", "trajectory_dynamics"):
+            elif pair in ("trajectory_clearance", "trajectory_certify", "trajectory_dynamics", "pose_clearance"):
                 assert all(poisoned_summary(s) for s in outs["summary"]), (form, outs["summary"])
+            elif pair == "simulate":
+                assert all(poisoned_sim_summary(s) for s in outs["summary"]), (form, outs["summary"])
+            elif pair == "swept_volume_grid":
+                assert all(np.all(np.isnan(outs[k])) for k in ("value", "lower", "tstar")) and not outs["decided"].any(), form
+
+
+def swept_sdf_host(ev):
+    p = ev.swept_params(K)
+    val, low, ts, dec = np.zeros(QE), np.zeros(QE), np.zeros(QE), np.zeros(QE, dtype=np.uint8)
+    r = ev.lib.isdf_swept_volume_sdf(ev.h, N, T.ctypes.data_as(DP), CC.ctypes.data_as(DP), C.byref(p), QE, EPTS.ctypes.data_as(DP),
+                                     val.ctypes.data_as(DP), low.ctypes.data_as(DP), ts.ctypes.data_as(DP), dec.ctypes.data_as(C.POINTER(C.c_uint8)))
+    return r, dict(value=val, lower=low, tstar=ts, decided=dec)
+
+
+# host forms of different families in a row, their staged sizes growing and then shrinking: every host form stages through the
+# context's one pinned and one device block
+SHARED = [("states, large Q", lambda ev: states_host(ev, ev.h, "", Q=200_000)), ("clearance", lambda ev: clearance_host(ev, ev.h, "")),
+          ("certify", lambda ev: certify_host(ev, ev.h, "")), ("callback", lambda ev: callback_host(ev, ev.h, "")),
+          ("lbfgs", lambda ev: lbfgs_host(ev, ev.h, "")), ("swept volume sdf", swept_sdf_host), ("pose clearance", lambda ev: pose_clearance_host(ev, ev.h, "")),
+          ("states, small Q", lambda ev: states_host(ev, ev.h, "", Q=5))]
+
+
+def test_host_forms_in_a_row_equal_fresh_contexts():
+    ev = make_ev("")
+    shared = [call(ev) for _, call in SHARED]
+    ev.close()
+    for (name, call), (r, outs) in zip(SHARED, shared):
+        fresh = make_ev("")
+        rf, outs_f = call(fresh)
+        fresh.close()
+        assert r == 0 and rf == 0, name
+        assert same(outs, outs_f), name
