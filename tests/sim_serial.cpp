@@ -530,4 +530,10 @@ int sim_set_input(const isdf_sim_params *p, const double *rpm, double *input) {
     for (int i = 0; i < 4; i++) input[i] = q.input[i];
     return cl;
 }
+
+// SO3Control::calculateControl with yaw 0 -> force (3), orientation (w, x, y, z)
+void sim_calculate_control(const isdf_sim_params *p, const double *pos, const double *vel, const double *acc, const double *dp, const double *dv,
+                           const double *da, double *force, double *quat) {
+    calculate_control(p, pos, vel, acc, dp, dv, da, force, quat);
+}
 }
