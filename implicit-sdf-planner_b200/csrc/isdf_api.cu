@@ -268,12 +268,10 @@ struct isdf_ctx {
     struct {   // batched obstacle gather: staged waypoints and offsets, per-row boxes, counts and offsets, the lists
         DevBuf<GatherBox> d_box; DevBuf<int> d_wpoff, d_cnt, d_ptoff; DevBuf<long long> d_offs, d_total; DevBuf<double> d_wp, d_out;
     } gat;
-    struct {   // planning step (isdf_plan_pairs): the stages' buffers, the per-plan launch layouts, and the host forms' staged outputs
+    struct {   // planning step (isdf_plan_pairs): the stages' buffers and the per-plan launch layouts (the host forms stage through Staging)
         DevBuf<double> d_bc, d_wp, d_mx, d_mres, d_bbc, d_bx, d_bf, d_gT, d_gC, d_dur, d_pwp; DevBuf<int> d_mi, d_bi, d_N, d_idx, d_ok, d_bplan, d_gi;
         DevBuf<CertSummary> d_csum; DevBuf<DynSummary> d_dsum;
         DevBuf<CopySeg> d_seg; DevBuf<PlanRow> d_row;
-        DevBuf<int32_t> s_path_off, s_piece_off; DevBuf<double> s_xyz, s_T, s_C;   // the host forms' staging
-        DevBuf<PlanResult> s_res; DevBuf<CertSummary> s_cert; DevBuf<DynSummary> s_dyn;
         cudaEvent_t ev[2] = {};
         isdf_plan_info info = {};
         long long xfer[4] = {};   // the last planning call's transfers (isdf_dbg_plan_transfers)
@@ -308,7 +306,8 @@ struct isdf_ctx {
 };
 
 static int set_device(isdf_ctx *c) { CU_TRY(cudaSetDevice(c->device)); return 0; }
-// one copy of the planning pipeline, counted in c->xfer: host-to-device or device-to-host, a round's termination read or not
+// one copy of the planning pipeline, counted in c->xfer: host-to-device or device-to-host, a round's termination read or not. A host
+// form's staged results come back as one copy (Staging::download), so XF_COPIES counts that copy once, not once per array
 enum { XF_D2H_BYTES, XF_ROUND_READS, XF_H2D_BYTES, XF_COPIES };
 static void count_copy(isdf_ctx *c, cudaMemcpyKind k, size_t bytes, bool round_read = false) {
     if (k == cudaMemcpyDeviceToHost) { if (round_read) c->xfer[XF_ROUND_READS]++; else c->xfer[XF_D2H_BYTES] += (long long)bytes; }
@@ -388,6 +387,7 @@ public:
         for (const Seg &s : segs_) if (s.take && s.bytes) s.take(h + (s.off - lo_));
         return 0;
     }
+    size_t download_bytes() const { return hi_ - lo_; }   // what download() copies, alignment included (after upload())
 };
 
 extern "C" const char *isdf_last_error(void) { return g_err.c_str(); }
@@ -3962,34 +3962,62 @@ static int path_run(isdf_ctx *c, int B, const double *starts, int sstride, const
     return 0;
 }
 
-// the host form of the path calls (starts: sstride 0 for one start)
-static int path_host(isdf_ctx *c, int B, const double *starts, int sstride, const double *goals, const isdf_frontpath_params *prm, int max_fields,
-                     int cap, double *path_xyz, double *path_rp, int32_t *offsets, double *costs, uint8_t *found) {
+// a device-form call's goals (B x 3) and, with sstride 3, its starts, read to the host on st for path_run's grouping; goals and starts then
+// point at hg and hs
+static int read_endpoints(isdf_ctx *c, int B, const double *&starts, int sstride, const double *&goals, std::vector<double> &hs,
+                          std::vector<double> &hg, cudaStream_t st) {
+    hg.resize((size_t)3 * B);
+    CU_TRY(cudaMemcpyAsync(hg.data(), goals, sizeof(double) * hg.size(), cudaMemcpyDeviceToHost, st));
+    count_copy(c, cudaMemcpyDeviceToHost, sizeof(double) * hg.size());
+    if (sstride) {
+        hs.resize((size_t)3 * B);
+        CU_TRY(cudaMemcpyAsync(hs.data(), starts, sizeof(double) * hs.size(), cudaMemcpyDeviceToHost, st));
+        count_copy(c, cudaMemcpyDeviceToHost, sizeof(double) * hs.size());
+        starts = hs.data();
+    }
+    CU_TRY(cudaStreamSynchronize(st));
+    goals = hg.data();
+    return 0;
+}
+
+// the path calls (starts: sstride 0 for one start, on the host in every form). dev: goals, starts (sstride 3) and every output in device
+// memory, the call on cuda_stream; else host memory, the call on ctx's stream
+static int path_entry(isdf_ctx *c, bool dev, int B, const double *starts, int sstride, const double *goals, const isdf_frontpath_params *prm,
+                      int max_fields, int cap, double *path_xyz, double *path_rp, int32_t *offsets, double *costs, uint8_t *found,
+                      void *cuda_stream) {
     if (!starts || !goals || B < 1 || max_fields < 0 || cap < 0 || (cap > 0 && !path_xyz) || !offsets || !costs || !found)
         return fail(ISDF_ERR_INVALID, "bad argument");
     if (int r = path_args_check(c, prm)) return r;
     if (set_device(c)) return ISDF_ERR_CUDA;
+    const cudaStream_t st = dev ? (cudaStream_t)cuda_stream : c->stream;
+    std::vector<double> hs, hg;
+    if (dev) if (int r = read_endpoints(c, B, starts, sstride, goals, hs, hg, st)) return r;
     std::vector<int> off;
-    const int r = path_run(c, B, starts, sstride, goals, max_fields, cap, off, c->stream);
-    if (!off.empty()) std::memcpy(offsets, off.data(), sizeof(int32_t) * off.size());
+    const int r = path_run(c, B, starts, sstride, goals, max_fields, cap, off, st);
+    if (!off.empty() && !dev) std::memcpy(offsets, off.data(), sizeof(int32_t) * off.size());
+    if (!off.empty() && dev) {
+        CU_TRY(cudaMemcpyAsync(offsets, off.data(), sizeof(int32_t) * off.size(), cudaMemcpyHostToDevice, st));
+        CU_TRY(cudaStreamSynchronize(st));   // off is a host temporary
+    }
     if (r) return r;
+    const cudaMemcpyKind k = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     const size_t total = (size_t)off[B];
-    CU_TRY(cudaMemcpyAsync(path_xyz, c->fp.d_xyz.p, sizeof(double) * 3 * total, cudaMemcpyDeviceToHost, c->stream));
-    if (path_rp) CU_TRY(cudaMemcpyAsync(path_rp, c->fp.d_rp.p, sizeof(double) * 2 * total, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaMemcpyAsync(costs, c->fp.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaMemcpyAsync(found, c->fp.d_found.p, B, cudaMemcpyDeviceToHost, c->stream));
-    CU_TRY(cudaStreamSynchronize(c->stream));
+    CU_TRY(cudaMemcpyAsync(path_xyz, c->fp.d_xyz.p, sizeof(double) * 3 * total, k, st));
+    if (path_rp) CU_TRY(cudaMemcpyAsync(path_rp, c->fp.d_rp.p, sizeof(double) * 2 * total, k, st));
+    CU_TRY(cudaMemcpyAsync(costs, c->fp.d_cost.p, sizeof(double) * B, k, st));
+    CU_TRY(cudaMemcpyAsync(found, c->fp.d_found.p, B, k, st));
+    CU_TRY(cudaStreamSynchronize(st));
     return 0;
 }
 
 extern "C" int isdf_frontend_path_batch(isdf_ctx *c, const double *start, int B, const double *goals, const isdf_frontpath_params *prm, int cap,
                                         double *path_xyz, double *path_rp, int32_t *offsets, double *costs, uint8_t *found) {
-    return path_host(c, B, start, 0, goals, prm, 0, cap, path_xyz, path_rp, offsets, costs, found);
+    return path_entry(c, false, B, start, 0, goals, prm, 0, cap, path_xyz, path_rp, offsets, costs, found, nullptr);
 }
 
 extern "C" int isdf_frontend_path_pairs(isdf_ctx *c, int B, const double *starts, const double *goals, const isdf_frontpath_params *prm,
                                         int max_fields, int cap, double *path_xyz, double *path_rp, int32_t *offsets, double *costs, uint8_t *found) {
-    return path_host(c, B, starts, 3, goals, prm, max_fields, cap, path_xyz, path_rp, offsets, costs, found);
+    return path_entry(c, false, B, starts, 3, goals, prm, max_fields, cap, path_xyz, path_rp, offsets, costs, found, nullptr);
 }
 
 extern "C" int isdf_frontend_path(isdf_ctx *c, const double *start, const double *goal, const isdf_frontpath_params *prm, int cap,
@@ -4001,47 +4029,16 @@ extern "C" int isdf_frontend_path(isdf_ctx *c, const double *start, const double
     return r;
 }
 
-// the device form of the path calls: h_starts on the host (one start, sstride 0) or d_starts on the device (B x 3)
-static int path_device(isdf_ctx *c, int B, const double *h_starts, const double *d_starts, const double *d_goals, const isdf_frontpath_params *prm,
-                       int max_fields, int cap, double *d_path_xyz, double *d_path_rp, int32_t *d_offsets, double *d_costs, uint8_t *d_found,
-                       void *cuda_stream) {
-    if (!(h_starts || d_starts) || !d_goals || B < 1 || max_fields < 0 || cap < 0 || (cap > 0 && !d_path_xyz) || !d_offsets || !d_costs || !d_found)
-        return fail(ISDF_ERR_INVALID, "bad argument");
-    if (int r = path_args_check(c, prm)) return r;
-    if (set_device(c)) return ISDF_ERR_CUDA;
-    const cudaStream_t st = (cudaStream_t)cuda_stream;
-    std::vector<double> goals((size_t)3 * B), starts(d_starts ? (size_t)3 * B : 0);
-    CU_TRY(cudaMemcpyAsync(goals.data(), d_goals, sizeof(double) * goals.size(), cudaMemcpyDeviceToHost, st));
-    if (d_starts) CU_TRY(cudaMemcpyAsync(starts.data(), d_starts, sizeof(double) * starts.size(), cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    std::vector<int> off;
-    const int r = path_run(c, B, d_starts ? starts.data() : h_starts, d_starts ? 3 : 0, goals.data(), max_fields, cap, off, st);
-    if (!off.empty()) {
-        CU_TRY(cudaMemcpyAsync(d_offsets, off.data(), sizeof(int32_t) * off.size(), cudaMemcpyHostToDevice, st));
-        CU_TRY(cudaStreamSynchronize(st));   // off is a host temporary
-    }
-    if (r) return r;
-    const size_t total = (size_t)off[B];
-    CU_TRY(cudaMemcpyAsync(d_path_xyz, c->fp.d_xyz.p, sizeof(double) * 3 * total, cudaMemcpyDeviceToDevice, st));
-    if (d_path_rp) CU_TRY(cudaMemcpyAsync(d_path_rp, c->fp.d_rp.p, sizeof(double) * 2 * total, cudaMemcpyDeviceToDevice, st));
-    CU_TRY(cudaMemcpyAsync(d_costs, c->fp.d_cost.p, sizeof(double) * B, cudaMemcpyDeviceToDevice, st));
-    CU_TRY(cudaMemcpyAsync(d_found, c->fp.d_found.p, B, cudaMemcpyDeviceToDevice, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    return 0;
-}
-
 extern "C" int isdf_frontend_path_batch_device(isdf_ctx *c, const double *start, int B, const double *d_goals, const isdf_frontpath_params *prm,
                                                int cap, double *d_path_xyz, double *d_path_rp, int32_t *d_offsets, double *d_costs,
                                                uint8_t *d_found, void *cuda_stream) {
-    if (!start) return fail(ISDF_ERR_INVALID, "bad argument");
-    return path_device(c, B, start, nullptr, d_goals, prm, 0, cap, d_path_xyz, d_path_rp, d_offsets, d_costs, d_found, cuda_stream);
+    return path_entry(c, true, B, start, 0, d_goals, prm, 0, cap, d_path_xyz, d_path_rp, d_offsets, d_costs, d_found, cuda_stream);
 }
 
 extern "C" int isdf_frontend_path_pairs_device(isdf_ctx *c, int B, const double *d_starts, const double *d_goals, const isdf_frontpath_params *prm,
                                                int max_fields, int cap, double *d_path_xyz, double *d_path_rp, int32_t *d_offsets,
                                                double *d_costs, uint8_t *d_found, void *cuda_stream) {
-    if (!d_starts) return fail(ISDF_ERR_INVALID, "bad argument");
-    return path_device(c, B, nullptr, d_starts, d_goals, prm, max_fields, cap, d_path_xyz, d_path_rp, d_offsets, d_costs, d_found, cuda_stream);
+    return path_entry(c, true, B, d_starts, 3, d_goals, prm, max_fields, cap, d_path_xyz, d_path_rp, d_offsets, d_costs, d_found, cuda_stream);
 }
 
 // the fields of the S source voxels src (host, 3 each) in one relaxation into d_g
@@ -4130,14 +4127,14 @@ static int plan_check(isdf_ctx *c, const isdf_plan_params *p, double *r_cert) {
     return 0;
 }
 
-// The outputs of the planning pipeline, in device memory in include/isdf.h's layout. Staged (the host forms): path_off, piece_off, res,
-// cert and dyn are c->plan's staging, and plan_run points path_xyz, T and coeffs into it once the sizes are known.
+// The outputs of the planning pipeline, in device memory in include/isdf.h's layout: the caller's (the device forms) or Staging's (the
+// host forms). path_xyz is NULL in the host forms, which read the paths' nodes from c->fp.d_xyz.
 struct PlanOut {
     int32_t *path_off = nullptr, *piece_off = nullptr;
     double *path_xyz = nullptr, *T = nullptr, *coeffs = nullptr;
     PlanResult *res = nullptr; CertSummary *cert = nullptr; DynSummary *dyn = nullptr;
-    bool staged = false, want_xyz = false;   // want_xyz: the paths' nodes are an output
-    bool sized = false;                      // path_off (when wanted) and piece_off hold the sizes
+    bool want_xyz = false;   // the paths' nodes are an output
+    bool sized = false;      // path_off (when wanted) and piece_off hold the sizes
     int nodes = 0, pieces = 0;
 };
 static_assert(sizeof(isdf_plan_result) == sizeof(PlanResult) && offsetof(isdf_plan_result, path_cost) == offsetof(PlanResult, path_cost) &&
@@ -4234,12 +4231,7 @@ static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const
     o.sized = true; o.nodes = nodes; o.pieces = poff[B];
     if ((o.want_xyz && nodes > cap_nodes) || poff[B] > cap_pieces)
         return fail(ISDF_ERR_INVALID, "cap_nodes or cap_pieces too small (path_off / piece_off report the sizes needed)");
-    if (o.staged) {
-        if (o.want_xyz) { CU_TRY(z.s_xyz.ensure((size_t)3 * std::max(nodes, 1))); o.path_xyz = z.s_xyz.p; }
-        CU_TRY(z.s_T.ensure(std::max(poff[B], 1))); CU_TRY(z.s_C.ensure((size_t)18 * std::max(poff[B], 1)));
-        o.T = z.s_T.p; o.coeffs = z.s_C.p;
-    }
-    if (o.want_xyz && nodes) CU_TRY(cudaMemcpyAsync(o.path_xyz, d_xyz, sizeof(double) * 3 * (size_t)nodes, cudaMemcpyDeviceToDevice, st));
+    if (o.path_xyz && nodes) CU_TRY(cudaMemcpyAsync(o.path_xyz, d_xyz, sizeof(double) * 3 * (size_t)nodes, cudaMemcpyDeviceToDevice, st));
     // 3-6. one ragged mid-end over every plan that reaches it, one gather and one ragged back end over the plans that pass it, in pair order
     std::vector<int> idx;   // the plans that reach the mid-end
     for (int b = 0; b < B; b++) if (row[b].stage == ISDF_PLAN_OPTIMISED) idx.push_back(b);
@@ -4420,35 +4412,8 @@ static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const
     return 0;
 }
 
-// the host forms' outputs from their staging on st (wrote: plan_run's return; path_off and piece_off also after a failure that left them
-// sized)
-static int plan_copy_back(isdf_ctx *c, const PlanOut &o, bool wrote, int B, int32_t *path_off, double *path_xyz, int32_t *piece_off, double *T,
-                          double *coeffs, isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics, cudaStream_t st) {
-    auto get = [&](void *dst, const void *src, size_t bytes) -> int {
-        if (!bytes) return 0;
-        CU_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st));
-        count_copy(c, cudaMemcpyDeviceToHost, bytes);
-        return 0;
-    };
-    const size_t Bs = (size_t)B;
-    if (o.sized) {
-        if (path_off) if (int r = get(path_off, o.path_off, sizeof(int32_t) * (Bs + 1))) return r;
-        if (int r = get(piece_off, o.piece_off, sizeof(int32_t) * (Bs + 1))) return r;
-    }
-    if (wrote) {
-        if (path_xyz) if (int r = get(path_xyz, o.path_xyz, sizeof(double) * 3 * (size_t)o.nodes)) return r;
-        if (int r = get(T, o.T, sizeof(double) * (size_t)o.pieces)) return r;
-        if (int r = get(coeffs, o.coeffs, sizeof(double) * 18 * (size_t)o.pieces)) return r;
-        if (int r = get(results, o.res, sizeof(isdf_plan_result) * Bs)) return r;
-        if (certify) if (int r = get(certify, o.cert, sizeof(isdf_certify_summary) * Bs)) return r;
-        if (dynamics) if (int r = get(dynamics, o.dyn, sizeof(isdf_dynamics_summary) * Bs)) return r;
-    }
-    CU_TRY(cudaStreamSynchronize(st));
-    return 0;
-}
-
 // the planning calls (starts: sstride 0 for one start, on the host in every form). dev: goals, starts (sstride 3) and every output in
-// device memory, the call on st; else host memory, staged through c->plan on ctx's stream (st). One pipeline, plan_run, for both.
+// device memory, the call on st; else host memory, the outputs staged through Staging on ctx's stream (st). One pipeline, plan_run, for both.
 static int plan_entry(isdf_ctx *c, bool dev, int B, const double *starts, int sstride, const double *goals, const isdf_plan_params *p, int max_fields,
                       int cap_nodes, int32_t *path_off, double *path_xyz, int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
                       isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics, cudaStream_t st) {
@@ -4466,38 +4431,40 @@ static int plan_entry(isdf_ctx *c, bool dev, int B, const double *starts, int ss
         if (set_device(c)) return ISDF_ERR_CUDA;
         started = true;
         std::fill(c->xfer, c->xfer + 4, 0ll);
-        auto &z = c->plan;
         PlanOut o;
         o.want_xyz = path_xyz != nullptr;
+        auto *res = reinterpret_cast<PlanResult *>(results);
+        auto *cert = reinterpret_cast<CertSummary *>(certify);
+        auto *dyn = reinterpret_cast<DynSummary *>(dynamics);
         std::vector<double> hs, hg;
-        if (dev) {   // the starts and goals are read to the host to group them (path_run)
-            hg.resize((size_t)3 * B);
-            CU_TRY(cudaMemcpyAsync(hg.data(), goals, sizeof(double) * hg.size(), cudaMemcpyDeviceToHost, st));
-            count_copy(c, cudaMemcpyDeviceToHost, sizeof(double) * hg.size());
-            if (sstride) {
-                hs.resize((size_t)3 * B);
-                CU_TRY(cudaMemcpyAsync(hs.data(), starts, sizeof(double) * hs.size(), cudaMemcpyDeviceToHost, st));
-                count_copy(c, cudaMemcpyDeviceToHost, sizeof(double) * hs.size());
-                starts = hs.data();
-            }
-            CU_TRY(cudaStreamSynchronize(st));
-            goals = hg.data();
-            o.path_off = path_off; o.path_xyz = path_xyz; o.piece_off = piece_off; o.T = T; o.coeffs = coeffs;
-            o.res = reinterpret_cast<PlanResult *>(results); o.cert = reinterpret_cast<CertSummary *>(certify); o.dyn = reinterpret_cast<DynSummary *>(dynamics);
-        } else {
-            o.staged = true;
-            CU_TRY(z.s_piece_off.ensure((size_t)B + 1)); CU_TRY(z.s_res.ensure(B));
-            o.piece_off = z.s_piece_off.p; o.res = z.s_res.p;
-            if (path_off) { CU_TRY(z.s_path_off.ensure((size_t)B + 1)); o.path_off = z.s_path_off.p; }
-            if (certify) { CU_TRY(z.s_cert.ensure(B)); o.cert = z.s_cert.p; }
-            if (dynamics) { CU_TRY(z.s_dyn.ensure(B)); o.dyn = z.s_dyn.p; }
+        Staging S(c);
+        if (dev) {
+            if (int r = read_endpoints(c, B, starts, sstride, goals, hs, hg, st)) return r;
+            o.path_off = path_off; o.path_xyz = path_xyz; o.piece_off = piece_off; o.T = T; o.coeffs = coeffs; o.res = res; o.cert = cert; o.dyn = dyn;
+        } else {   // cert and dyn only when asked for: each is one more fill launch. T and coeffs: room for cap_pieces, read back below
+            S.out(&o.piece_off, piece_off, (size_t)B + 1); S.out(&o.res, res, (size_t)B);
+            if (path_off) S.out(&o.path_off, path_off, (size_t)B + 1);
+            if (cert) S.out(&o.cert, cert, (size_t)B);
+            if (dyn) S.out(&o.dyn, dyn, (size_t)B);
+            S.out(&o.T, nullptr, (size_t)cap_pieces); S.out(&o.coeffs, nullptr, 18 * (size_t)cap_pieces);
+            if (int r = S.upload()) return r;
         }
         int r = plan_run(c, B, starts, sstride, goals, max_fields, p, r_cert, cap_nodes, cap_pieces, o, st);
-        if (!dev) {
-            const int rb = plan_copy_back(c, o, r == 0, B, path_off, path_xyz, piece_off, T, coeffs, results, certify, dynamics, st);
-            if (!r) r = rb;
-        }
-        return r;
+        if (dev || !o.sized) return r;   // a host form that failed before the sizes leaves path_off and piece_off as they were
+        // the paths' nodes and the used prefix of T and coeffs after a success, then the staged outputs, whose offsets report the sizes also
+        // after a failure (the results and summaries are poisoned then)
+        auto get = [&](void *dst, const void *src, size_t bytes) -> int {
+            if (!bytes) return 0;
+            CU_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st));
+            count_copy(c, cudaMemcpyDeviceToHost, bytes);
+            return 0;
+        };
+        if (!r && path_xyz) r = get(path_xyz, c->fp.d_xyz.p, sizeof(double) * 3 * (size_t)o.nodes);
+        if (!r) r = get(T, o.T, sizeof(double) * (size_t)o.pieces);
+        if (!r) r = get(coeffs, o.coeffs, sizeof(double) * 18 * (size_t)o.pieces);
+        const int rb = S.download();
+        count_copy(c, cudaMemcpyDeviceToHost, S.download_bytes());
+        return r ? r : rb;
     }, [&] {
         if (B < 1) return;
         isdf_plan_result bad = {};

@@ -436,6 +436,124 @@ def sense_device(ev, h, fault):
     return r, dict(depth=ddepth.cpu().numpy())
 
 
+# front-end paths and planning: BP (start, goal) pairs between traversable voxels of OCC, found once on a context of their own. The
+# offset arrays start as SENTINEL, so that a test sees which calls write them.
+BP, SENTINEL = 6, -7
+CAP = 4096    # path nodes and planned pieces; 1 under the "cap" faults
+_ENDS = []
+
+
+def path_ends():
+    if not _ENDS:
+        import frontpath_oracle as FO
+        ev = make_ev("", kernels=True)
+        trav = np.argwhere(FO.traversable(OCC, ev.frontend_feasibility(*OCC.shape)))
+        ev.close()
+        v = trav[np.random.default_rng(8).choice(len(trav), 2 * BP, replace=False)] + 0.5
+        _ENDS.extend([np.ascontiguousarray(v[:BP]), np.ascontiguousarray(v[BP:])])
+    return _ENDS
+
+
+def sentinels():
+    return np.full(BP + 1, SENTINEL, dtype=np.int32)
+
+
+def path_setup(fault, pairs):
+    starts, goals = path_ends()
+    prm = I.FrontPathParams()
+    prm.reserved_[0] = 1 if "param" in fault else 0
+    return (starts if pairs else np.ascontiguousarray(starts[0])), goals, prm, 1 if "cap" in fault else CAP
+
+
+def path_host(pairs):
+    def run(ev, h, fault):
+        starts, goals, prm, cap = path_setup(fault, pairs)
+        xyz, rp, off, cost, found = np.zeros(3 * cap), np.zeros(2 * cap), sentinels(), np.zeros(BP), np.zeros(BP, dtype=np.uint8)
+        outs = (xyz.ctypes.data_as(DP), rp.ctypes.data_as(DP), off.ctypes.data_as(IP), cost.ctypes.data_as(DP), found.ctypes.data_as(C.POINTER(C.c_uint8)))
+        if pairs:   # two fields at a time: three chunks
+            r = ev.lib.isdf_frontend_path_pairs(h, BP, host_ptr(starts, fault, True), goals.ctypes.data_as(DP), C.byref(prm), 2, cap, *outs)
+        else:
+            r = ev.lib.isdf_frontend_path_batch(h, host_ptr(starts, fault, True), BP, goals.ctypes.data_as(DP), C.byref(prm), cap, *outs)
+        return r, dict(xyz=xyz, rp=rp, offsets=off, cost=cost, found=found)
+    return run
+
+
+def path_device(pairs):
+    def run(ev, h, fault):
+        starts, goals, prm, cap = path_setup(fault, pairs)
+        dxyz, drp, doff, dcost, dfound = dev(np.zeros(3 * cap)), dev(np.zeros(2 * cap)), dev(sentinels()), dev(np.zeros(BP)), dev(np.zeros(BP, dtype=np.uint8))
+        dg = dev(goals)
+        outs = (ptr(dxyz, fault), ptr(drp, fault), ptr(doff, fault), ptr(dcost, fault), ptr(dfound, fault), stream())
+        if pairs:
+            ds = dev(starts)
+            r = ev.lib.isdf_frontend_path_pairs_device(h, BP, ptr(ds, fault, True), ptr(dg, fault), C.byref(prm), 2, cap, *outs)
+        else:
+            r = ev.lib.isdf_frontend_path_batch_device(h, host_ptr(starts, fault, True), BP, ptr(dg, fault), C.byref(prm), cap, *outs)
+        return r, dict(xyz=dxyz.cpu().numpy(), rp=drp.cpu().numpy(), offsets=doff.cpu().numpy(), cost=dcost.cpu().numpy(), found=dfound.cpu().numpy())
+    return run
+
+
+# planning: plan_pairs with both certificates and every output; plan_batch with no certificate and only the required outputs (path_off,
+# path_xyz, certify and dynamics NULL)
+def plan_setup(ev, fault, pairs):
+    starts, goals = path_ends()
+    p = ev.plan_params(backend_max_iterations=60, flags=(I.PLAN_CERTIFY | I.PLAN_DYNAMICS) if pairs else 0)
+    if "param" in fault:
+        p.flags = 4   # unknown
+    return (starts if pairs else np.ascontiguousarray(starts[0])), goals, p, 1 if "cap" in fault else CAP
+
+
+def plan_results(raw):
+    return [s.as_dict() for s in (I.PlanResult * BP).from_buffer_copy(raw)]
+
+
+def plan_host(pairs):
+    def run(ev, h, fault):
+        starts, goals, p, cap = plan_setup(ev, fault, pairs)
+        po, T_o, C_o, res = sentinels(), np.zeros(cap), np.zeros(18 * cap), (I.PlanResult * BP)()
+        tail = (cap, po.ctypes.data_as(IP), T_o.ctypes.data_as(DP), C_o.ctypes.data_as(DP), res)
+        out = dict(piece_off=po, T=T_o, coeffs=C_o)
+        if pairs:
+            pf, xyz, cs, ds = sentinels(), np.zeros(3 * CAP), (I.CertifySummary * BP)(), (I.DynamicsSummary * BP)()
+            r = ev.lib.isdf_plan_pairs(h, BP, host_ptr(starts, fault, True), goals.ctypes.data_as(DP), C.byref(p), 0, CAP, pf.ctypes.data_as(IP),
+                                       xyz.ctypes.data_as(DP), *tail, cs, ds)
+            out.update(path_off=pf, path_xyz=xyz, certify=np.frombuffer(bytes(cs), np.uint8), dynamics=np.frombuffer(bytes(ds), np.uint8))
+        else:
+            r = ev.lib.isdf_plan_batch(h, host_ptr(starts, fault, True), BP, goals.ctypes.data_as(DP), C.byref(p), 0, None, None, *tail, None, None)
+        return r, dict(out, results=plan_results(bytes(res)))
+    return run
+
+
+def plan_device(pairs):
+    def run(ev, h, fault):
+        import torch
+        starts, goals, p, cap = plan_setup(ev, fault, pairs)
+        dpo, dT, dC, dg = dev(sentinels()), dev(np.zeros(cap)), dev(np.zeros(18 * cap)), dev(goals)
+        dres = torch.zeros(C.sizeof(I.PlanResult) * BP, dtype=torch.uint8, device="cuda")
+        tail = (cap, ptr(dpo, fault), ptr(dT, fault), ptr(dC, fault), ptr(dres, fault))
+        out = {}
+        if pairs:
+            dst, dpf, dxyz = dev(starts), dev(sentinels()), dev(np.zeros(3 * CAP))
+            dcs, dds = device_summary_buffer(I.CertifySummary, BP), device_summary_buffer(I.DynamicsSummary, BP)
+            r = ev.lib.isdf_plan_pairs_device(h, BP, ptr(dst, fault, True), ptr(dg, fault), C.byref(p), 0, CAP, ptr(dpf, fault), ptr(dxyz, fault),
+                                              *tail, ptr(dcs, fault), ptr(dds, fault), stream())
+            out = dict(path_off=dpf.cpu().numpy(), path_xyz=dxyz.cpu().numpy(), certify=dcs.cpu().numpy(), dynamics=dds.cpu().numpy())
+        else:
+            r = ev.lib.isdf_plan_batch_device(h, host_ptr(starts, fault, True), BP, ptr(dg, fault), C.byref(p), 0, None, None, *tail, None, None,
+                                              stream())
+        return r, dict(out, piece_off=dpo.cpu().numpy(), T=dT.cpu().numpy(), coeffs=dC.cpu().numpy(),
+                       results=plan_results(dres.cpu().numpy().tobytes()))
+    return run
+
+
+def poisoned_plan_result(s):
+    return s["stage"] == I.PLAN_FAILED and all(math.isnan(s[k]) for k in ("path_cost", "midend_f", "backend_f", "duration"))
+
+
+PATH_FAULTS = {"ctx": -1, "null": -1, "param": -1, "nomap": -2, "nokernels": -2, "shard": -4, "nokernels+null": -1}
+PLAN_FAULTS = {"ctx": -1, "null": -1, "param": -1, "nomap": -2, "nokernels": -2, "shard": -4}
+
+
 # name -> (host, device, make_ev keywords, {fault: code}). "nomap+null" / "shard+null" pin the order of the checks: the state is
 # checked before the pointers; "size+nomap" / "size+shard" pin where each certificate checks its 31-bit size: after the state checks
 # for the clearance certificate, before the shard check for the dynamic-limit certificate.
@@ -465,6 +583,11 @@ PAIRS = {
                        {"ctx": -1, "null": -1, "param": -1, "nomap": -2, "noshape": -2, "shard": -4}),
     "swept_volume_grid": (swept_grid_host, swept_grid_device, {}, {"ctx": -1, "null": -1, "param": -1, "noshape": -2, "shard": -4}),
     "sense_depth": (sense_host, sense_device, dict(scene=True), {"ctx": -1, "null": -1, "param": -1, "noscene": -2}),
+    # the path calls check their pointers before the state ("nokernels+null")
+    "frontend_path_batch": (path_host(False), path_device(False), dict(kernels=True), PATH_FAULTS),
+    "frontend_path_pairs": (path_host(True), path_device(True), dict(kernels=True), PATH_FAULTS),
+    "plan_batch": (plan_host(False), plan_device(False), dict(kernels=True), PLAN_FAULTS),
+    "plan_pairs": (plan_host(True), plan_device(True), dict(kernels=True), PLAN_FAULTS),
 }
 # the pairs whose device form poisons its outputs with a kernel (counted in kernel_launches) when it has a context
 POISON_KERNEL = {"simulate"}
@@ -539,6 +662,26 @@ def test_refusals_agree_and_poison(pair, fault):
                 assert all(poisoned_sim_summary(s) for s in outs["summary"]), (form, outs["summary"])
             elif pair == "swept_volume_grid":
                 assert all(np.all(np.isnan(outs[k])) for k in ("value", "lower", "tstar")) and not outs["decided"].any(), form
+            elif pair in ("plan_batch", "plan_pairs"):
+                assert all(poisoned_plan_result(s) for s in outs["results"]), (form, outs["results"])
+
+
+# The path and planning calls write their offsets once the sizes are known, also when a cap is too small: then both forms report the same
+# sizes (and the planning results are poisoned). A call refused before the run leaves them as they were.
+OFFSETS = {"frontend_path_batch": ["offsets"], "frontend_path_pairs": ["offsets"], "plan_batch": ["piece_off"], "plan_pairs": ["path_off", "piece_off"]}
+
+
+@pytest.mark.parametrize("pair,fault", [(p, f) for p in OFFSETS for f in ["cap"] + list(PAIRS[p][3])])
+def test_offsets_of_refused_path_and_plan_calls(pair, fault):
+    (rh, _, oh, nh, _), (rd, _, od, nd, _) = call(pair, "host", fault), call(pair, "device", fault)
+    assert rh == rd == PAIRS[pair][3].get(fault, -1)
+    for k in OFFSETS[pair]:
+        assert np.array_equal(oh[k], od[k]), (k, oh[k], od[k])
+        assert (oh[k] == SENTINEL).all() == (fault != "cap"), (k, oh[k])
+    if fault == "cap":
+        assert nh == nd > 0
+        if pair.startswith("plan"):
+            assert same(oh["results"], od["results"]) and all(poisoned_plan_result(s) for s in oh["results"])
 
 
 def swept_sdf_host(ev):
