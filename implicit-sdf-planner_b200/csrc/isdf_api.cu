@@ -19,6 +19,7 @@
 #include "isdf_plan.cuh"
 #include "isdf_sim.cuh"
 #include "isdf_sense.cuh"
+#include "isdf_world.cuh"
 #include <cub/device/device_scan.cuh>
 #include <queue>
 #include "isdf_host_mesh.cuh"
@@ -283,6 +284,7 @@ struct isdf_ctx {
     // reads, the rounds' 4-byte reads, host-to-device bytes, copies
     long long xfer[4] = {};
     SenseScene sense;   // depth sensing (isdf_sense.cuh): the scene cloud's bricks and the per-call scratch
+    WorldScratch gen;   // world generators (isdf_world.cuh): the host program's copy, Perlin keys and selection, the host form's records
     struct {   // peer-memory reduction (isdf_peer.cuh)
         DevBuf<char> buf;                    // own exchange buffer (exported through CUDA IPC)
         void *open[PEER_MAX] = {};           // peers' buffers opened here (null for self / unused)
@@ -1562,6 +1564,55 @@ extern "C" int isdf_sense_cloud(isdf_ctx *c, int64_t Q, const double *pos, const
 extern "C" int isdf_sense_cloud_device(isdf_ctx *c, int64_t Q, const double *d_pos, const double *d_quat, int64_t stride_doubles,
                                        const isdf_sense_params *p, int64_t cap, float *d_points, int64_t *d_offsets, void *cuda_stream) {
     return sense_cloud_impl(c, Q, d_pos, d_quat, stride_doubles, p, cap, d_points, d_offsets, true, (cudaStream_t)cuda_stream);
+}
+// ---- world generators (isdf_world.cuh, compiled in isdf_world_tu.cu) ----
+extern "C" int isdf_world_default_params(int kind, isdf_world_params *p) {
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    if (kind != ISDF_WORLD_GLOBALMAP && kind != ISDF_WORLD_PERLIN && kind != ISDF_WORLD_BOXES) return fail(ISDF_ERR_INVALID, "unknown world kind");
+    std::memset(p, 0, sizeof(*p));
+    p->kind = kind;
+    p->map_id = 4; p->rand_seed = 1; p->srand_seed = 0;                               // globalmap_gene.launch
+    p->cloud_resolution = 0.6; p->init[0] = p->init[1] = p->init[2] = 1.0;
+    p->seed = 511; p->size[0] = 100; p->size[1] = 100; p->size[2] = 30; p->scale = 10;   // mockamap.launch: 10 x 10 x 3 m at 0.1 m
+    p->complexity = 0.03; p->fill = 0.3; p->fractal = 1; p->attenuation = 0.1;
+    p->obstacle_number = 50; p->width_min = 0.6; p->width_max = 1.5;
+    return 0;
+}
+
+static int world_impl(isdf_ctx *c, const isdf_world_params *p, int64_t cap, float *points, int64_t *n, bool device, cudaStream_t st) {
+    if (!p || !n) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (cap < 0 || (cap > 0 && !points)) return fail(ISDF_ERR_INVALID, "cap < 0, or points NULL with cap > 0");
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    WorldPlan P;
+    std::string msg;
+    if (int rc = world_plan(*p, P, &msg)) return fail(rc, "isdf_world_cloud: " + msg);
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    float *d_points = points;
+    long long room = cap;
+    if (!device) {   // the records' device room: the cloud's size, or for Perlin the voxel count that bounds it
+        room = std::min<long long>(cap, P.n);
+        CU_TRY(c->gen.d_out.ensure(4 * (size_t)std::max(room, 1ll)));
+        d_points = c->gen.d_out.p; st = c->stream;
+    }
+    int launches = 0;
+    long long total = 0;
+    const cudaError_t e = world_emit(c->gen, P, room, d_points, &total, st, &launches);
+    c->stats.kernel_launches += launches;
+    if (e != cudaSuccess) return fail(ISDF_ERR_CUDA, std::string("isdf_world_cloud: ") + cudaGetErrorString(e));
+    *n = total;
+    if (!device) {
+        if (std::min(total, room) > 0)
+            CU_TRY(cudaMemcpyAsync(points, d_points, 4 * sizeof(float) * std::min(total, room), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
+    }
+    if (total > cap) return fail(ISDF_ERR_INVALID, "cap smaller than the cloud (*n reports its size)");
+    return 0;
+}
+extern "C" int isdf_world_cloud(isdf_ctx *c, const isdf_world_params *p, int64_t cap, float *points, int64_t *n) {
+    return world_impl(c, p, cap, points, n, false, nullptr);
+}
+extern "C" int isdf_world_cloud_device(isdf_ctx *c, const isdf_world_params *p, int64_t cap, float *d_points, int64_t *n, void *cuda_stream) {
+    return world_impl(c, p, cap, d_points, n, true, (cudaStream_t)cuda_stream);
 }
 // diagnostics (not in include/isdf.h): render at most `poses` poses per chunk (0: the automatic chunking)
 extern "C" int isdf_dbg_sense_chunk(isdf_ctx *c, int poses) {

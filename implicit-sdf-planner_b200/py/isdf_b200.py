@@ -49,7 +49,9 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_sim_default_params", "isdf_simulate", "isdf_simulate_device",
                "isdf_pose_clearance_default_params", "isdf_pose_clearance", "isdf_pose_clearance_device",
                "isdf_sense_default_params", "isdf_set_sense_cloud", "isdf_set_sense_cloud_device", "isdf_get_sense_info",
-               "isdf_sense_depth", "isdf_sense_depth_device", "isdf_sense_cloud", "isdf_sense_cloud_device"]
+               "isdf_sense_depth", "isdf_sense_depth_device", "isdf_sense_cloud", "isdf_sense_cloud_device",
+               "isdf_world_default_params", "isdf_world_cloud", "isdf_world_cloud_device"]
+WORLD_KINDS = dict(globalmap=1, perlin=2, boxes=3)   # isdf_world_kind
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
 DYN_QUANTITIES = ["speed", "acceleration", "body_rate", "tilt", "thrust"]   # q of isdf_dynamics_summary; mask bit 5: the thrust minimum
@@ -239,6 +241,34 @@ class SenseParams(C.Structure):
     """isdf_sense_params"""
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
                 ("cam_to_body", C.c_double * 16), ("sensing_horizon", C.c_double)]
+
+
+class WorldParams(C.Structure):
+    """isdf_world_params"""
+    _fields_ = [("kind", C.c_int32), ("map_id", C.c_int32), ("rand_seed", C.c_uint32), ("srand_seed", C.c_uint32),
+                ("cloud_resolution", C.c_double), ("init", C.c_double * 3), ("seed", C.c_uint32), ("size", C.c_int32 * 3), ("scale", C.c_double),
+                ("complexity", C.c_double), ("fill", C.c_double), ("attenuation", C.c_double), ("fractal", C.c_int32),
+                ("obstacle_number", C.c_int32), ("width_min", C.c_double), ("width_max", C.c_double), ("reserved_", C.c_int32 * 2)]
+
+
+def world_params(kind, **kw):
+    """isdf_world_params: the reference's launch-file defaults for kind ("globalmap", "perlin", "boxes" or its isdf_world_kind value),
+    with the given fields replaced (init and size take 3 values, reserved_ 2)"""
+    p = WorldParams()
+    k = WORLD_KINDS.get(kind, kind)
+    r = load_library().isdf_world_default_params(int(k), C.byref(p))
+    if r != 0:
+        raise IsdfError(r, "isdf_world_default_params")
+    for f, v in kw.items():
+        if not hasattr(p, f):
+            raise AttributeError(f)
+        if f in ("init", "size", "reserved_"):
+            arr = getattr(p, f)
+            for i, x in enumerate(v):
+                arr[i] = x
+        else:
+            setattr(p, f, v)
+    return p
 
 
 class SenseInfo(C.Structure):
@@ -532,6 +562,10 @@ def load_library(path=None):
     lib.isdf_sense_depth_device.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, vp, vp]
     lib.isdf_sense_cloud.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, C.c_int64, vp, vp]
     lib.isdf_sense_cloud_device.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, C.c_int64, vp, vp, vp]
+    wpp = C.POINTER(WorldParams)
+    lib.isdf_world_default_params.argtypes = [C.c_int, wpp]
+    lib.isdf_world_cloud.argtypes = [vp, wpp, C.c_int64, vp, C.POINTER(C.c_int64)]
+    lib.isdf_world_cloud_device.argtypes = [vp, wpp, C.c_int64, vp, C.POINTER(C.c_int64), vp]
     spp = C.POINTER(SimParams)
     lib.isdf_sim_default_params.argtypes = [spp]
     lib.isdf_simulate.argtypes = [vp, C.c_int, ip, dp, dp, C.c_int, ip, dp, dp, spp, C.c_int, dp, C.POINTER(SimSummary)]
@@ -666,6 +700,7 @@ class Evaluator:
         h = C.c_void_p()
         self._check(self.lib.isdf_create(C.byref(self.cfg), device, C.byref(h)))
         self.h = h
+        self.device = device
 
     def _check(self, r):
         if r != 0:
@@ -830,6 +865,46 @@ class Evaluator:
                 cap = total
                 continue
             self._check(rc)
+
+    # ---- world generators (isdf_world_*): the reference's globalmap_gene and mockamap worlds as (n, 4) float32 clouds ----
+    @staticmethod
+    def world_params(kind, **overrides):
+        """isdf_world_params of kind ("globalmap", "perlin", "boxes") with the reference's defaults and the given fields replaced"""
+        return world_params(kind, **overrides)
+
+    def _world_p(self, params, kind, kw):
+        if params is not None:
+            return params
+        return world_params(kind if kind is not None else kw.pop("kind"), **kw)
+
+    def world_cloud(self, params=None, kind=None, **kw):
+        """the world's cloud -> (n, 4) float32 numpy array of (x, y, z, 1): one size query (cap 0), then the cloud"""
+        p = self._world_p(params, kind, kw)
+        n = C.c_int64(-1)
+        rc = self.lib.isdf_world_cloud(self.h, C.byref(p), 0, None, C.byref(n))
+        if n.value < 0:   # the size query answers ISDF_ERR_INVALID with *n written for a non-empty cloud; without *n it failed
+            self._check(rc)
+        out = np.empty((max(n.value, 1), 4), dtype=np.float32)
+        self._check(self.lib.isdf_world_cloud(self.h, C.byref(p), n.value, out.ctypes.data_as(C.c_void_p), C.byref(n)))
+        return out[:n.value]
+
+    def world_cloud_device(self, params=None, kind=None, stream=None, **kw):
+        """the world's cloud -> (n, 4) float32 CUDA tensor on torch's current stream, for set_map_cloud_device(t.data_ptr(), n=n,
+        stride_bytes=16) and set_sense_cloud_device as it is. The size is known after a size query (for Perlin, one run of the noise and
+        selection), then the cloud is written."""
+        import torch
+        p = self._world_p(params, kind, kw)
+        dev = torch.device("cuda", self.device)
+        s = torch.cuda.current_stream(dev) if stream is None else stream
+        n = C.c_int64(-1)
+        rc = self.lib.isdf_world_cloud_device(self.h, C.byref(p), 0, None, C.byref(n), C.c_void_p(s.cuda_stream))
+        if n.value < 0:
+            self._check(rc)
+        with torch.cuda.stream(s):
+            out = torch.empty((max(n.value, 1), 4), dtype=torch.float32, device=dev)
+        self._check(self.lib.isdf_world_cloud_device(self.h, C.byref(p), n.value, C.c_void_p(out.data_ptr()), C.byref(n),
+                                                     C.c_void_p(s.cuda_stream)))
+        return out[:n.value]
 
     def dbg_sense_chunk(self, poses):
         """render at most `poses` poses per chunk (0: automatic; isdf_dbg_sense_chunk, not part of include/isdf.h)"""

@@ -1184,6 +1184,58 @@ int isdf_sense_cloud(isdf_ctx *ctx, int64_t Q, const double *pos, const double *
 int isdf_sense_cloud_device(isdf_ctx *ctx, int64_t Q, const double *d_pos, const double *d_quat, int64_t stride_doubles,
                             const isdf_sense_params *p, int64_t cap, float *d_points, int64_t *d_offsets, void *cuda_stream);
 
+/* ---- world generators: the reference's globalmap_gene maps 1-11 and mockamap's Perlin and box worlds (DESIGN §3.19) --------------
+ * Output. A cloud of n records of 16 bytes: float32 x, y, z and 1.0f (what pcl::PointXYZ's constructor leaves in its fourth float), in
+ *   the reference's push_back order, ready for isdf_set_map_cloud_device / isdf_set_sense_cloud_device with stride_bytes = 16. *n is
+ *   always the cloud's size, so cap = 0 with points NULL is a size query; when *n > cap the call returns ISDF_ERR_INVALID with *n and the
+ *   first cap records written.
+ * ISDF_WORLD_GLOBALMAP: map_manager/src/globalmap_gene.cpp's mapGene(map_id), map_id 1..11, the node's first publication. Loop coordinates
+ *   are the reference's FP64 accumulations (t += cloud_resolution while t < end; roads: t += res / length while t <= 1 and k from -0.5
+ *   by res / width while k <= 0.5). Each point is coord + (rand() % 10) / 250.0 for x and y and / 800.0 for z, drawn in that order,
+ *   added in FP64 and rounded to float32. rand() is glibc's (TYPE_3: r_i = r_{i-3} + r_{i-31} mod 2^32, output r >> 1, 310 outputs
+ *   discarded after seeding, seed 0 taken as 1) started from srand(rand_seed): 1 is a process that never called srand, as the node is.
+ *   Maps 4 and 11 call srand(time(NULL)) after their first two walls: srand_seed stands in for time(NULL). Map 2's trees and the cubes
+ *   of maps 4 and 11 are drawn from the same stream, so their positions follow the points before them. Roads (map 9) take
+ *   length = sqrt((x^2 + y^2) + z^2) and expand / sqrt(expand's squared norm) for Eigen's norm and normalize; with the shipped map 9
+ *   every road has dir.y = 0, so no order of that reduction changes a bit (real Eigen's vectorised order is not pinned here).
+ * ISDF_WORLD_PERLIN: mockamap's perlin3D (maps.cpp) on a BasicInfo of size[0..2] voxels, scale and seed: the permutation is libstdc++'s
+ *   std::shuffle of 0..255 with std::default_random_engine(seed); tnoise(i, j, k) = sum over it = 1..fractal of (attenuation / it) *
+ *   noise(dfv i complexity, dfv j complexity, dfv k complexity), dfv = 2^it, in FP64 with nothing contracted; the threshold is the
+ *   tpos-th smallest value, tpos = (int)(X Y Z (1 - fill)); the points are the voxels with tnoise > threshold in (i, j, k) order (k
+ *   fastest) at (i / scale - X / (2 scale), j / scale - Y / (2 scale), k / scale).
+ * ISDF_WORLD_BOXES: mockamap's randomMapGenerate: obstacle_number x (x, y, w, h) drawn with std::uniform_real_distribution<double> on
+ *   std::default_random_engine(seed) (libstdc++), each box's shell emitted in (r, s, t) order. The shell test is "some factor of the
+ *   reference's six-factor int product is zero"; the reference's product overflows int for boxes wider than about 40 voxels, so a box
+ *   whose product can reach 2^31 ((widNum - 1)^4 (heiNum - 1)^2 >= 2^31) is refused with ISDF_ERR_INVALID.
+ * mockamap's node derives the sizes from its VoxelWidth and MapBound parameters (mockamap.cpp:96-111): size = floor(min(|MapBound[0]|,
+ *   |MapBound[1]|)), floor(min(|MapBound[2]|, |MapBound[3]|)), floor(MapBound[5]) metres, scale = 1 / VoxelWidth, and each size times
+ *   scale truncated to int. isdf_world_default_params gives globalmap_gene.launch (resolution 0.6, init 1, 1, 1, rand_seed 1, srand_seed
+ *   0, map_id 4 as the launch file) and mockamap.launch (seed 511, complexity 0.03, fill 0.3, fractal 1, attenuation 0.1, widths 0.6 to
+ *   1.5, 50 obstacles, 10 x 10 x 3 m at 0.1 m: size 100 x 100 x 30, scale 10).
+ * The call needs a context for its stream and scratch, not a map or a shape, and counts its launches in isdf_stats.kernel_launches.
+ *   isdf_world_cloud_device writes d_points (cap x 4 float32, device) on cuda_stream and returns after at most one 8-byte read (the
+ *   Perlin world's count; the other kinds' sizes are known on the host). Guarantees: the same bits run to run, through either form.
+ * Errors: ISDF_ERR_INVALID for a NULL pointer, cap < 0 (points may be NULL when cap = 0), an unknown kind or map_id, a non-finite or
+ *   non-positive cloud_resolution or scale, non-finite init, a non-positive size, size[0] size[1] size[2] >= 2^31, fractal < 1 or
+ *   2^fractal max(size) |complexity| or 2^fractal max(size) >= 2^31 (the reference's int conversions), non-finite complexity, fill or
+ *   attenuation, tpos outside [0, X Y Z) (the reference throws std::out_of_range), obstacle_number < 0, width_min > width_max or a
+ *   non-finite width, a box as above, a non-zero reserved_, a loop of more than 2^31 steps, and a cloud beyond 2^63 bytes. */
+typedef enum isdf_world_kind { ISDF_WORLD_GLOBALMAP = 1, ISDF_WORLD_PERLIN = 2, ISDF_WORLD_BOXES = 3 } isdf_world_kind;
+typedef struct isdf_world_params {
+    int32_t kind, map_id;                 /* globalmap: mapGene(map_id), 1..11 */
+    uint32_t rand_seed, srand_seed;       /* glibc state at the start (1: never seeded); what srand(time(NULL)) gets in maps 4 and 11 */
+    double cloud_resolution, init[3];     /* globalmap_gene.launch: 0.6; init_x, init_y, init_z 1, 1, 1 */
+    uint32_t seed; int32_t size[3];       /* mockamap: BasicInfo's seed and sizeX, sizeY, sizeZ (voxels) */
+    double scale;                         /* 1 / VoxelWidth */
+    double complexity, fill, attenuation; /* perlin3D */
+    int32_t fractal, obstacle_number;     /* perlin3D; randomMapGenerate */
+    double width_min, width_max;          /* randomMapGenerate */
+    int32_t reserved_[2];                 /* must be 0 */
+} isdf_world_params;
+int isdf_world_default_params(int kind, isdf_world_params *p);
+int isdf_world_cloud(isdf_ctx *ctx, const isdf_world_params *p, int64_t cap, float *points, int64_t *n);
+int isdf_world_cloud_device(isdf_ctx *ctx, const isdf_world_params *p, int64_t cap, float *d_points, int64_t *n, void *cuda_stream);
+
 /* ---- swept-volume term: addSaftyPenaOnSweptVolumeParallel (hpp:557-649) + getSDFofSweptVolume (swm:710-747) --- */
 /* parallel_points (plan_manager.cpp:246-254): P x 3 row-major world-frame voxel centres; resets lastTstar to 0 (not the persisted
  * trajectory duration: see isdf_set_points_batch) */
