@@ -1,0 +1,124 @@
+#!/usr/bin/env python
+"""bench_navigate.py — B vehicles fly to goals through a generated world they only see through the reference's depth camera
+(Evaluator.navigate: sense -> fuse -> check -> replan -> fly -> advance, every stage batched over vehicles); prints one JSON line.
+
+  python bench_navigate.py [--vehicles 1,16,64] [--rounds R] [--horizon H] [--sense-every S] [--seed N]
+
+World: mockamap's box world (isdf_world_cloud_device, ISDF_WORLD_BOXES) with seed 511, 40 x 40 x 10 m at 0.5 m (size 80 x 80 x 20,
+scale 2), 20 boxes 1.5 to 3 m wide: x and y in [-20, 20] m, z in [0, 10] m. The vehicles' map starts as an empty 1 m frame over that box
+(set_map_u8 of zeros) and grows only by fusing what the camera (the reference's 640 x 480 camera, horizon 15 m) sees. Robot: the Ball
+shape (radius 1 m), kernel size 11 at 1 m, vmax 3 m/s; planning with PLAN_CERTIFY and 200 back-end iterations; flight with the reference's
+simulator for `horizon` seconds per round.
+Start / goal pairs are seeded: starts at x in [-17, -12], goals at x in [12, 17], y in [-17, 17], z in [2, 8], all in voxels of the true
+map at least 2 voxels from any occupied one. The true map (the whole world fused into the same frame, in a second context) checks every
+flown pose with pose_clearance_device.
+Per B: per-stage milliseconds per round (mean over the rounds run, CUDA events), rounds run, arrivals, failed replans, and the minimum true
+clearance over every flown pose. Writes nothing to the tree.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.join(ROOT, "implicit-sdf-planner_b200", "py"))
+sys.dont_write_bytecode = True
+
+DIMS, BMIN, RES = (40, 40, 10), np.array([-20.0, -20.0, 0.0]), 1.0
+
+
+def world(ev):
+    import isdf_b200 as I
+    p = I.world_params("boxes", seed=511, size=[80, 80, 20], scale=2.0, obstacle_number=20, width_min=1.5, width_max=3.0)
+    return ev.world_cloud_device(p)
+
+
+def pairs(occ, B, seed):
+    """B seeded (start, goal) pairs at voxel centres of the true map at least 2 voxels from any occupied voxel"""
+    pad = np.pad(occ, 2)
+    near = np.zeros_like(occ, dtype=bool)
+    X, Y, Z = occ.shape
+    for i in range(5):
+        for j in range(5):
+            for k in range(5):
+                near |= pad[i:i + X, j:j + Y, k:k + Z] > 0
+    free = np.argwhere(~near)
+    c = free + 0.5 + BMIN
+    ok = (c[:, 2] >= 2) & (c[:, 2] <= 8) & (np.abs(c[:, 1]) <= 17)
+    st, gl = c[ok & (c[:, 0] >= -17) & (c[:, 0] <= -12)], c[ok & (c[:, 0] >= 12) & (c[:, 0] <= 17)]
+    rng = np.random.default_rng(seed)
+    return st[rng.choice(len(st), B, replace=len(st) < B)], gl[rng.choice(len(gl), B, replace=len(gl) < B)]
+
+
+def min_clearance(truth, logs):
+    import torch
+    m = float("inf")
+    for _, lg in logs:
+        rec = lg.reshape(-1, lg.shape[-1]).contiguous()
+        Q = rec.shape[0]
+        clear = torch.empty(Q, dtype=torch.float64, device=rec.device)
+        vox = torch.empty(Q, dtype=torch.int64, device=rec.device)
+        summ = torch.empty((1, 48), dtype=torch.uint8, device=rec.device)
+        base = rec.data_ptr()
+        truth.pose_clearance_device(Q, base + 8, base + 56, lg.shape[-1], truth.pose_clearance_params(), clear.data_ptr(), vox.data_ptr(),
+                                    summ.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        m = min(m, float(clear.min()))
+    return m
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--vehicles", default="1,16,64")
+    ap.add_argument("--rounds", type=int, default=40)
+    ap.add_argument("--horizon", type=float, default=0.5)
+    ap.add_argument("--sense-every", type=int, default=25)
+    ap.add_argument("--seed", type=int, default=7)
+    args = ap.parse_args()
+    import torch
+    import isdf_b200 as I
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_navigate.py measures the GPU path and needs a CUDA device")
+    gpu = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    cfg = I.default_config_values()
+    cfg.integral_intervs, cfg.kernel_size, cfg.vmax = 16, 11, 3.0
+    truth = I.Evaluator(cfg)
+    truth.set_shape_named("Ball")
+    scene = world(truth)
+    truth.set_map_u8(np.zeros(DIMS, np.uint8), BMIN, RES)
+    truth.map_fuse_cloud_device(scene, stream=torch.cuda.current_stream().cuda_stream)
+    occ = truth.get_map_u8()
+    out = dict(bench="navigate", gpu=gpu, world="mockamap boxes seed 511, 40 x 40 x 10 m, 20 boxes; 1 m frame", points=int(scene.shape[0]),
+               horizon_s=args.horizon, sense_every=args.sense_every, runs=[])
+    for B in [int(v) for v in args.vehicles.split(",")]:
+        starts, goals = pairs(occ, B, args.seed + B)
+        ev = I.Evaluator(cfg)
+        ev.set_shape_named("Ball")
+        ev.frontend_build_kernels(45.0, 45.0, 9.0, 0.0)
+        ev.set_map_u8(np.zeros(DIMS, np.uint8), BMIN, RES)
+        ev.set_sense_cloud_device(scene, stream=torch.cuda.current_stream().cuda_stream)
+        r = ev.navigate(starts, goals, rounds=args.rounds, horizon=args.horizon, sense_every=args.sense_every, tol=1.0,
+                        plan_params=ev.plan_params(flags=I.PLAN_CERTIFY, backend_max_iterations=200),
+                        sense_params=I.sense_params(sensing_horizon=15.0))
+        fail = r["actions"] == I.NAV_REPLAN_FAILED
+        why = {}   # failed replans by (plan stage, certificate verdict); -2: no plan call (a head outside the frame)
+        for st, v in zip(r["replan_stages"][fail], r["replan_verdicts"][fail]):
+            why[f"{st}/{v}"] = why.get(f"{st}/{v}", 0) + 1
+        stages = list(r["times"][0])
+        ms = {k: round(float(np.mean([t[k] for t in r["times"]])), 3) for k in stages}
+        out["runs"].append(dict(vehicles=B, rounds=len(r["times"]), ms_per_round=ms, ms_round_total=round(sum(ms.values()), 3),
+                                arrived=int((r["status"] == I.NAV_ARRIVED).sum()), stopped=int((r["status"] == I.NAV_STOPPED).sum()),
+                                diverged=int((r["status"] == I.NAV_DIVERGED).sum()), timeout=int((r["status"] == I.NAV_TIMEOUT).sum()),
+                                replans=int(r["replans"].sum()), failed_replans=int(r["failed_replans"].sum()), failed_by_stage_verdict=why,
+                                uncertified_rounds=int(r["uncertified_rounds"].sum()), map_voxels=int(ev.map_info()["occupied_voxels"]),
+                                min_true_clearance=round(min_clearance(truth, r["logs"]), 4)))
+        ev.close()
+    truth.close()
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()

@@ -273,10 +273,14 @@ struct isdf_ctx {
         DevBuf<double> d_bc, d_wp, d_mx, d_mres, d_bbc, d_bx, d_bf, d_gT, d_gC, d_dur, d_pwp; DevBuf<int> d_mi, d_bi, d_N, d_idx, d_ok, d_bplan, d_gi;
         DevBuf<CertSummary> d_csum; DevBuf<DynSummary> d_dsum;
         DevBuf<CopySeg> d_seg; DevBuf<PlanRow> d_row;
+        DevBuf<int> d_bad;   // isdf_plan_states_device's head check
         cudaEvent_t ev[2] = {};
         isdf_plan_info info = {};
         long long xfer[4] = {};   // the last planning call's transfers (isdf_dbg_plan_transfers)
     } plan;
+    struct {   // isdf_trajectory_shift: per-trajectory piece counts, first piece and its local time, the scan's scratch
+        DevBuf<int> d_cnt, d_first; DevBuf<double> d_tau; DevBuf<char> d_tmp;
+    } shift;
     struct {   // waypoint selection on the device (isdf_path_waypoints_device): per-path counts and gaps, the scan's scratch
         DevBuf<int32_t> d_cnt, d_gap; DevBuf<char> d_tmp; PinnedBuf<int32_t> h_total;
     } wps;
@@ -986,7 +990,7 @@ static int set_map_cloud_impl(isdf_ctx *c, const char *d_pts, long long n, int s
     // 3. occupancy (the previous map is given up from here on)
     drop_map(c);
     CloudFrame F;
-    for (int a = 0; a < 3; a++) F.bmin[a] = bmin[a];
+    for (int a = 0; a < 3; a++) { F.bmin[a] = bmin[a]; F.bmax[a] = bmax[a]; }
     F.res = res; F.X = X; F.Y = Y; F.Z = Z; F.Zw = (Z + 31) / 32;
     const size_t nwords = (size_t)X * Y * F.Zw;
     cudaError_t e = c->map.d_bits.ensure(nwords);
@@ -1001,7 +1005,7 @@ static int set_map_cloud_impl(isdf_ctx *c, const char *d_pts, long long n, int s
     } else if (thr == 1) {
         e = cudaMemsetAsync(c->map.d_bits.p, 0, nwords * sizeof(uint32_t), c->stream);
         if (e == cudaSuccess) {
-            k_cloud_mark<<<blocks, 256, 0, c->stream>>>(d_pts, n, stride, F, c->map.d_bits.p);
+            k_cloud_mark<<<blocks, 256, 0, c->stream>>>(d_pts, n, stride, F, c->map.d_bits.p, nullptr);
             c->stats.kernel_launches++;
             e = cudaGetLastError();
         }
@@ -1041,6 +1045,63 @@ extern "C" int isdf_set_map_cloud_device(isdf_ctx *c, const void *d_points, int6
     if (int rc = cloud_args_check(c, d_points, n, stride_bytes, res)) return rc;
     if (set_device(c)) return ISDF_ERR_CUDA;
     return set_map_cloud_impl(c, (const char *)d_points, n, stride_bytes, res, sta_threshold, (cudaStream_t)cuda_stream);
+}
+
+// ---- fusing a cloud into the current map, in its frame (k_cloud_mark with the frame's bounds) ---------------------------------------
+// every check that needs no device work: the cloud's (res is the map's) and a map to fuse into
+static int fuse_args_check(isdf_ctx *c, const void *pts, int64_t n, int32_t stride) {
+    if (int rc = cloud_args_check(c, pts, n, stride, 1.0)) return rc;
+    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set: fusion adds to the current map's frame (an empty frame is isdf_set_map_u8 of zeros)");
+    return 0;
+}
+
+// d_pts on the device and ready on stream st; the bits are updated on c->stream. The distance field no longer describes the map afterwards.
+static int fuse_cloud_impl(isdf_ctx *c, const char *d_pts, long long n, int stride, isdf_fuse_info *info, cudaStream_t st) {
+    const DevGrid &g = c->map.grid;
+    CloudFrame F;
+    for (int a = 0; a < 3; a++) { F.bmin[a] = g.bmin[a]; F.bmax[a] = g.bmax[a]; }
+    F.res = g.res; F.X = g.X; F.Y = g.Y; F.Z = g.Z; F.Zw = g.Zw;
+    unsigned long long cnt[4] = {};
+    DevBuf<unsigned long long> d_cnt;
+    cudaError_t e = d_cnt.ensure(4);
+    if (e == cudaSuccess && st != c->stream) e = cudaStreamSynchronize(st);   // the points are ready on st
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_cnt.p, 0, sizeof(cnt), c->stream);
+    if (e == cudaSuccess) {
+        k_cloud_mark<<<cloud_grid_blocks(c, n), 256, 0, c->stream>>>(d_pts, n, stride, F, c->map.d_bits.p, d_cnt.p);
+        c->stats.kernel_launches++;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(cnt, d_cnt.p, sizeof(cnt), cudaMemcpyDeviceToHost, c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess) {
+        drop_map(c);
+        return fail(ISDF_ERR_CUDA, std::string("isdf_map_fuse_cloud: ") + cudaGetErrorString(e));
+    }
+    c->esdf.have = false;   // the field described the map before this call
+    c->esdf.d_pos = {}; c->esdf.d_neg = {};
+    if (info) {
+        info->points_used = (int64_t)cnt[FUSE_USED]; info->points_outside = (int64_t)cnt[FUSE_OUTSIDE];
+        info->points_skipped = (int64_t)cnt[FUSE_SKIPPED]; info->voxels_added = (int64_t)cnt[FUSE_ADDED];
+    }
+    return 0;
+}
+
+extern "C" int isdf_map_fuse_cloud(isdf_ctx *c, const void *points, int64_t n, int32_t stride_bytes, isdf_fuse_info *info) {
+    if (int rc = fuse_args_check(c, points, n, stride_bytes)) return rc;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    DevBuf<char> d_pts;
+    const size_t bytes = (size_t)n * stride_bytes;
+    cudaError_t e = d_pts.ensure(bytes);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_pts.p, points, bytes, cudaMemcpyHostToDevice, c->stream);
+    if (e != cudaSuccess) return fail(ISDF_ERR_CUDA, std::string("isdf_map_fuse_cloud: ") + cudaGetErrorString(e));
+    return fuse_cloud_impl(c, d_pts.p, n, stride_bytes, info, c->stream);
+}
+
+extern "C" int isdf_map_fuse_cloud_device(isdf_ctx *c, const void *d_points, int64_t n, int32_t stride_bytes, isdf_fuse_info *info,
+                                          void *cuda_stream) {
+    if (int rc = fuse_args_check(c, d_points, n, stride_bytes)) return rc;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    return fuse_cloud_impl(c, (const char *)d_points, n, stride_bytes, info, (cudaStream_t)cuda_stream);
 }
 
 extern "C" int isdf_get_map_info(isdf_ctx *c, isdf_map_info *out) {
@@ -1264,6 +1325,51 @@ extern "C" int isdf_trajectory_states_device(isdf_ctx *c, int B, const int32_t *
     states_launch(c, B, d_piece_off, d_T, d_coeffs, Q, d_traj, d_times, d_out, (cudaStream_t)cuda_stream);
     CU_TRY(cudaGetLastError());
     return 0;
+}
+
+// the rest of B trajectories from t0 (isdf_states.cuh) on stream st: locate and count, scan the counts into out_off, write the pieces
+static int shift_launch(isdf_ctx *c, int B, const int *d_off, const double *d_T, const double *d_C, const double *d_t0, int *d_out_off,
+                        double *d_out_T, double *d_out_C, cudaStream_t st) {
+    auto &z = c->shift;
+    CU_TRY(z.d_cnt.ensure(B)); CU_TRY(z.d_first.ensure(B)); CU_TRY(z.d_tau.ensure(B));
+    size_t tmp = 0;
+    CU_TRY(cub::DeviceScan::InclusiveSum(nullptr, tmp, z.d_cnt.p, d_out_off + 1, B, st));
+    CU_TRY(z.d_tmp.ensure(std::max<size_t>(tmp, 1)));
+    k_shift_locate<<<(unsigned)((B + 127) / 128), 128, 0, st>>>(B, d_off, d_T, d_t0, z.d_cnt.p, z.d_first.p, z.d_tau.p, d_out_off);
+    CU_TRY(cub::DeviceScan::InclusiveSum(z.d_tmp.p, tmp, z.d_cnt.p, d_out_off + 1, B, st));
+    k_shift_write<<<(unsigned)(((long long)B * 32 + 127) / 128), 128, 0, st>>>(B, d_off, d_T, d_C, z.d_cnt.p, z.d_first.p, z.d_tau.p, d_out_off,
+                                                                               d_out_T, d_out_C);
+    c->stats.kernel_launches += 3;
+    CU_TRY(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int isdf_trajectory_shift(isdf_ctx *c, int B, const int32_t *piece_off, const double *T, const double *coeffs, const double *t0,
+                                     int32_t *out_piece_off, double *out_T, double *out_coeffs) {
+    if (!c || !piece_off || !T || !coeffs || !t0 || !out_piece_off || !out_T || !out_coeffs) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (B < 1) return fail(ISDF_ERR_INVALID, "B < 1");
+    if (int rc = offsets_check(piece_off, B, "piece_off", true)) return rc;
+    const int P = piece_off[B];
+    if (int rc = swept_traj_check(P, T, coeffs)) return rc;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    Staging S(c);
+    const double *d_C, *d_T, *d_t0;
+    const int *d_off;
+    int *d_out_off;
+    double *d_out_T, *d_out_C;
+    S.in(&d_C, coeffs, 18 * (size_t)P); S.in(&d_T, T, (size_t)P); S.in(&d_t0, t0, (size_t)B); S.in(&d_off, piece_off, (size_t)B + 1);
+    S.out(&d_out_off, out_piece_off, (size_t)B + 1); S.out(&d_out_T, out_T, (size_t)P); S.out(&d_out_C, out_coeffs, 18 * (size_t)P);
+    if (int rc = S.upload()) return rc;
+    if (int rc = shift_launch(c, B, d_off, d_T, d_C, d_t0, d_out_off, d_out_T, d_out_C, c->stream)) return rc;
+    return S.download();
+}
+
+extern "C" int isdf_trajectory_shift_device(isdf_ctx *c, int B, const int32_t *d_piece_off, const double *d_T, const double *d_coeffs,
+                                            const double *d_t0, int32_t *d_out_piece_off, double *d_out_T, double *d_out_coeffs, void *cuda_stream) {
+    if (!c || !d_piece_off || !d_T || !d_coeffs || !d_t0 || !d_out_piece_off || !d_out_T || !d_out_coeffs) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (B < 1) return fail(ISDF_ERR_INVALID, "B < 1");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    return shift_launch(c, B, d_piece_off, d_T, d_coeffs, d_t0, d_out_piece_off, d_out_T, d_out_coeffs, (cudaStream_t)cuda_stream);
 }
 
 static int pose_args_check(isdf_ctx *c, int64_t Q, const void *states, int P, const void *body, const void *out) {
@@ -4013,21 +4119,35 @@ static int path_run(isdf_ctx *c, int B, const double *starts, int sstride, const
     return 0;
 }
 
-// a device-form call's goals (B x 3) and, with sstride 3, its starts, read to the host on st for path_run's grouping; goals and starts then
-// point at hg and hs
-static int read_endpoints(isdf_ctx *c, int B, const double *&starts, int sstride, const double *&goals, std::vector<double> &hs,
+// a device-form call's goals (B x 3) and, with sstride 3 or 9, its starts' positions, read to the host on st for path_run's grouping; goals
+// and starts then point at hg and hs (sstride 3). Start states (sstride 9, isdf_plan_states_device): only the positions cross, and v and a
+// are checked on the device, one 4-byte verdict.
+static int read_endpoints(isdf_ctx *c, int B, const double *&starts, int &sstride, const double *&goals, std::vector<double> &hs,
                           std::vector<double> &hg, cudaStream_t st) {
     hg.resize((size_t)3 * B);
     CU_TRY(cudaMemcpyAsync(hg.data(), goals, sizeof(double) * hg.size(), cudaMemcpyDeviceToHost, st));
     count_copy(c, cudaMemcpyDeviceToHost, sizeof(double) * hg.size());
+    int bad = 0x7fffffff;
+    if (sstride == 9) {
+        CU_TRY(c->plan.d_bad.ensure(1));
+        CU_TRY(cudaMemcpyAsync(c->plan.d_bad.p, &bad, sizeof(int), cudaMemcpyHostToDevice, st));
+        count_copy(c, cudaMemcpyHostToDevice, sizeof(int));
+        k_plan_heads_check<<<(unsigned)((B + 127) / 128), 128, 0, st>>>(B, starts, c->plan.d_bad.p);
+        c->stats.kernel_launches++;
+        CU_TRY(cudaGetLastError());
+        CU_TRY(cudaMemcpyAsync(&bad, c->plan.d_bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+        count_copy(c, cudaMemcpyDeviceToHost, sizeof(int));
+    }
     if (sstride) {
         hs.resize((size_t)3 * B);
-        CU_TRY(cudaMemcpyAsync(hs.data(), starts, sizeof(double) * hs.size(), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpy2DAsync(hs.data(), 3 * sizeof(double), starts, sstride * sizeof(double), 3 * sizeof(double), B, cudaMemcpyDeviceToHost, st));
         count_copy(c, cudaMemcpyDeviceToHost, sizeof(double) * hs.size());
         starts = hs.data();
+        sstride = 3;
     }
     CU_TRY(cudaStreamSynchronize(st));
     goals = hg.data();
+    if (bad != 0x7fffffff) return fail(ISDF_ERR_INVALID, "starts[" + std::to_string(bad) + "]: velocity or acceleration is not finite");
     return 0;
 }
 
@@ -4232,8 +4352,9 @@ static int plan_fill(isdf_ctx *c, int n, const S &v, S *out, cudaStream_t st) {
 
 // The pipeline on stream st. Per plan, only the path lengths and found flags, N, the mid-end return codes and the gathered point counts
 // cross to the host, besides the rounds' 4-byte reads; everything sized by nodes, waypoints or pieces stays on the device.
-static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const double *goals, int max_fields, const isdf_plan_params *p,
-                    double r_cert, int cap_nodes, int cap_pieces, PlanOut &o, cudaStream_t st) {
+// d_heads (may be NULL): the plans' head states p, v, a (9 per plan, on the device) in place of [path.front(), 0, 0].
+static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const double *d_heads, const double *goals, int max_fields,
+                    const isdf_plan_params *p, double r_cert, int cap_nodes, int cap_pieces, PlanOut &o, cudaStream_t st) {
     auto &z = c->plan;
     isdf_plan_info &info = z.info;
     info = {};
@@ -4306,7 +4427,7 @@ static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const
         count_copy(c, cudaMemcpyHostToDevice, sizeof(int) * (2 * (size_t)Bg + 2));
         if (int r = plan_upload(c, z.d_idx, idx, st)) return r;
         CU_TRY(z.d_bc.ensure((size_t)18 * Bg)); CU_TRY(z.d_wp.ensure(3 * std::max<size_t>(MP - Bg, 1)));
-        k_plan_bc<<<(unsigned)((Bg + 127) / 128), 128, 0, st>>>(Bg, z.d_idx.p, d_off, d_xyz, z.d_bc.p);
+        k_plan_bc<<<(unsigned)((Bg + 127) / 128), 128, 0, st>>>(Bg, z.d_idx.p, d_off, d_xyz, d_heads, z.d_bc.p);
         c->stats.kernel_launches++;
         CU_TRY(cudaGetLastError());
         std::vector<CopySeg> seg;
@@ -4372,7 +4493,7 @@ static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const
             for (int k = 0; k < Bp; k++) bplan[k] = idx[ok[k]];
             if (int r = plan_upload(c, z.d_bplan, bplan, st)) return r;
             CU_TRY(z.d_bbc.ensure((size_t)18 * Bp));
-            k_plan_bc<<<(unsigned)((Bp + 127) / 128), 128, 0, st>>>(Bp, z.d_bplan.p, d_off, d_xyz, z.d_bbc.p);
+            k_plan_bc<<<(unsigned)((Bp + 127) / 128), 128, 0, st>>>(Bp, z.d_bplan.p, d_off, d_xyz, d_heads, z.d_bbc.p);
             c->stats.kernel_launches++;
             CU_TRY(cudaGetLastError());
             const double *d_bh = z.d_bbc.p, *d_bt = z.d_bbc.p + 9 * (size_t)Bp;
@@ -4463,8 +4584,9 @@ static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const
     return 0;
 }
 
-// the planning calls (starts: sstride 0 for one start, on the host in every form). dev: goals, starts (sstride 3) and every output in
-// device memory, the call on st; else host memory, the outputs staged through Staging on ctx's stream (st). One pipeline, plan_run, for both.
+// the planning calls (starts: sstride 0 for one start, on the host in every form; sstride 9 for start states p, v, a). dev: goals, starts
+// (sstride 3 or 9) and every output in device memory, the call on st; else host memory, the outputs staged through Staging on ctx's stream
+// (st). One pipeline, plan_run, for both.
 static int plan_entry(isdf_ctx *c, bool dev, int B, const double *starts, int sstride, const double *goals, const isdf_plan_params *p, int max_fields,
                       int cap_nodes, int32_t *path_off, double *path_xyz, int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
                       isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics, cudaStream_t st) {
@@ -4477,6 +4599,11 @@ static int plan_entry(isdf_ctx *c, bool dev, int B, const double *starts, int ss
         if (max_fields < 0) return fail(ISDF_ERR_INVALID, "max_fields < 0");
         if (((p->flags & ISDF_PLAN_CERTIFY) && !certify) || ((p->flags & ISDF_PLAN_DYNAMICS) && !dynamics))
             return fail(ISDF_ERR_INVALID, "a summary array of a requested certificate is NULL");
+        if (sstride == 9 && !dev)
+            for (int b = 0; b < B; b++)
+                for (int k = 3; k < 9; k++)
+                    if (!std::isfinite(starts[9 * (size_t)b + k]))
+                        return fail(ISDF_ERR_INVALID, "starts[" + std::to_string(b) + "]: velocity or acceleration is not finite");
         double r_cert = 0.0;
         if (int r = plan_check(c, p, &r_cert)) return r;
         if (set_device(c)) return ISDF_ERR_CUDA;
@@ -4489,6 +4616,7 @@ static int plan_entry(isdf_ctx *c, bool dev, int B, const double *starts, int ss
         auto *dyn = reinterpret_cast<DynSummary *>(dynamics);
         std::vector<double> hs, hg;
         Staging S(c);
+        const double *d_heads = sstride == 9 && dev ? starts : nullptr;
         if (dev) {
             if (int r = read_endpoints(c, B, starts, sstride, goals, hs, hg, st)) return r;
             o.path_off = path_off; o.path_xyz = path_xyz; o.piece_off = piece_off; o.T = T; o.coeffs = coeffs; o.res = res; o.cert = cert; o.dyn = dyn;
@@ -4498,9 +4626,10 @@ static int plan_entry(isdf_ctx *c, bool dev, int B, const double *starts, int ss
             if (cert) S.out(&o.cert, cert, (size_t)B);
             if (dyn) S.out(&o.dyn, dyn, (size_t)B);
             S.out(&o.T, nullptr, (size_t)cap_pieces); S.out(&o.coeffs, nullptr, 18 * (size_t)cap_pieces);
+            if (sstride == 9) S.in(&d_heads, starts, 9 * (size_t)B);
             if (int r = S.upload()) return r;
         }
-        int r = plan_run(c, B, starts, sstride, goals, max_fields, p, r_cert, cap_nodes, cap_pieces, o, st);
+        int r = plan_run(c, B, starts, sstride, d_heads, goals, max_fields, p, r_cert, cap_nodes, cap_pieces, o, st);
         if (dev || !o.sized) return r;   // a host form that failed before the sizes leaves path_off and piece_off as they were
         // the paths' nodes and the used prefix of T and coeffs after a success, then the staged outputs, whose offsets report the sizes also
         // after a failure (the results and summaries are poisoned then)
@@ -4561,6 +4690,21 @@ extern "C" int isdf_plan_pairs_device(isdf_ctx *c, int B, const double *d_starts
                                       double *d_coeffs, isdf_plan_result *d_results, isdf_certify_summary *d_certify,
                                       isdf_dynamics_summary *d_dynamics, void *cuda_stream) {
     return plan_entry(c, true, B, d_starts, 3, d_goals, p, max_fields, cap_nodes, d_path_off, d_path_xyz, cap_pieces, d_piece_off, d_T, d_coeffs,
+                      d_results, d_certify, d_dynamics, (cudaStream_t)cuda_stream);
+}
+
+extern "C" int isdf_plan_states(isdf_ctx *c, int B, const double *starts, const double *goals, const isdf_plan_params *p, int max_fields,
+                                int cap_nodes, int32_t *path_off, double *path_xyz, int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
+                                isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics) {
+    return plan_entry(c, false, B, starts, 9, goals, p, max_fields, cap_nodes, path_off, path_xyz, cap_pieces, piece_off, T, coeffs, results, certify,
+                      dynamics, c ? c->stream : nullptr);
+}
+
+extern "C" int isdf_plan_states_device(isdf_ctx *c, int B, const double *d_starts, const double *d_goals, const isdf_plan_params *p, int max_fields,
+                                       int cap_nodes, int32_t *d_path_off, double *d_path_xyz, int cap_pieces, int32_t *d_piece_off, double *d_T,
+                                       double *d_coeffs, isdf_plan_result *d_results, isdf_certify_summary *d_certify,
+                                       isdf_dynamics_summary *d_dynamics, void *cuda_stream) {
+    return plan_entry(c, true, B, d_starts, 9, d_goals, p, max_fields, cap_nodes, d_path_off, d_path_xyz, cap_pieces, d_piece_off, d_T, d_coeffs,
                       d_results, d_certify, d_dynamics, (cudaStream_t)cuda_stream);
 }
 

@@ -94,7 +94,7 @@ __global__ void __launch_bounds__(256) k_cloud_bounds(const char *pts, long long
 }
 
 struct CloudFrame {
-    double bmin[3], res;
+    double bmin[3], bmax[3], res;
     int X, Y, Z, Zw;
 };
 
@@ -116,23 +116,34 @@ __device__ __forceinline__ void cloud_index(const CloudFrame &F, float x, float 
     grid_index(F, (double)x, (double)y, (double)z, ix, iy, iz);
 }
 
-// sta_threshold == 1: set the voxel's bit directly. Lanes of a warp that hit the same 32-bit word (neighbouring records of a spatially
-// coherent cloud) OR their bits together first (__match_any_sync), and the group's leader skips the atomic when a plain load already shows
-// every bit set. The loop trip count is warp-uniform so that every lane takes part in the match.
-__global__ void __launch_bounds__(256) k_cloud_mark(const char *pts, long long n, int stride, const CloudFrame F, uint32_t *bits) {
+// sta_threshold == 1: set the voxel's bit directly, for the finite records inside [bmin, bmax] (isInMap; every finite record of the cloud
+// that set the frame is inside it). Lanes of a warp that hit the same 32-bit word (neighbouring records of a spatially coherent cloud) OR
+// their bits together first (__match_any_sync), and the group's leader skips the atomic when a plain load already shows every bit set. The
+// loop trip count is warp-uniform so that every lane takes part in the match. cnt (may be NULL): {inside, outside, non-finite, bits this
+// launch set}; each bit's 0 -> 1 transition is seen by exactly one atomicOr, so the last count is exact in any order.
+enum { FUSE_USED, FUSE_OUTSIDE, FUSE_SKIPPED, FUSE_ADDED };
+__global__ void __launch_bounds__(256) k_cloud_mark(const char *pts, long long n, int stride, const CloudFrame F, uint32_t *bits,
+                                                    unsigned long long *cnt) {
     __shared__ uint32_t sbit[256];
     const int lane = threadIdx.x & 31;
     uint32_t *wbit = sbit + (threadIdx.x & ~31);
     const long long wstride = (long long)gridDim.x * blockDim.x;
+    unsigned long long c[4] = {0, 0, 0, 0};
     for (long long base = (long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31); base < n; base += wstride) {
         const long long i = base + lane;
         uint32_t word = 0xffffffffu, bit = 0;   // X*Y*Zw < 2^31 words, so 0xffffffff names no word
         float x, y, z;
-        if (i < n && cloud_point(pts, i, stride, x, y, z)) {
-            int ix, iy, iz;
-            cloud_index(F, x, y, z, ix, iy, iz);
-            word = (uint32_t)(((long long)ix * F.Y + iy) * F.Zw + (iz >> 5));
-            bit = 1u << (iz & 31);
+        if (i < n) {
+            if (!cloud_point(pts, i, stride, x, y, z)) c[FUSE_SKIPPED]++;
+            else if (!((double)x >= F.bmin[0] && (double)x <= F.bmax[0] && (double)y >= F.bmin[1] && (double)y <= F.bmax[1] &&
+                       (double)z >= F.bmin[2] && (double)z <= F.bmax[2])) c[FUSE_OUTSIDE]++;
+            else {
+                int ix, iy, iz;
+                cloud_index(F, x, y, z, ix, iy, iz);
+                word = (uint32_t)(((long long)ix * F.Y + iy) * F.Zw + (iz >> 5));
+                bit = 1u << (iz & 31);
+                c[FUSE_USED]++;
+            }
         }
         const unsigned peers = __match_any_sync(0xffffffffu, word);
         wbit[lane] = bit;
@@ -140,9 +151,15 @@ __global__ void __launch_bounds__(256) k_cloud_mark(const char *pts, long long n
         if (word != 0xffffffffu && lane == __ffs(peers) - 1) {
             uint32_t acc = 0;
             for (unsigned m = peers; m; m &= m - 1) acc |= wbit[__ffs(m) - 1];
-            if ((bits[word] & acc) != acc) atomicOr(&bits[word], acc);
+            if ((bits[word] & acc) != acc) c[FUSE_ADDED] += __popc(acc & ~atomicOr(&bits[word], acc));
         }
         __syncwarp();
+    }
+    if (!cnt) return;
+    for (int k = 0; k < 4; k++) {
+        unsigned long long v = c[k];
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0 && v) atomicAdd(&cnt[k], v);
     }
 }
 

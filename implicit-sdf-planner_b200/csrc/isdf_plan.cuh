@@ -39,14 +39,24 @@ __global__ void k_wp_write(int B, const int32_t *off, const double *xyz, const i
 }
 
 // plan plan[i]'s boundary conditions: head = [path.front(), 0, 0] at bc + 9 i, tail = [path.back(), 0, 0] at bc + 9 (n + i) (3x3
-// column-major, column 0 the position; plan_manager.cpp:220-223)
-__global__ void k_plan_bc(int n, const int *plan, const int32_t *path_off, const double *xyz, double *bc) {
+// column-major, column 0 the position; plan_manager.cpp:220-223). heads (may be NULL): plan b's head is the state p, v, a at heads + 9 b
+// (isdf_plan_states), which is the same column-major order.
+__global__ void k_plan_bc(int n, const int *plan, const int32_t *path_off, const double *xyz, const double *heads, double *bc) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const int b = plan[i];
     const double *f = xyz + 3 * (size_t)path_off[b], *l = xyz + 3 * ((size_t)path_off[b + 1] - 1);
     double *h = bc + 9 * (size_t)i, *t = bc + 9 * ((size_t)n + i);
-    for (int k = 0; k < 9; k++) { h[k] = k < 3 ? f[k] : 0.0; t[k] = k < 3 ? l[k] : 0.0; }
+    for (int k = 0; k < 9; k++) { h[k] = heads ? heads[9 * (size_t)b + k] : (k < 3 ? f[k] : 0.0); t[k] = k < 3 ? l[k] : 0.0; }
+}
+
+// isdf_plan_states_device's check of the heads' v and a: *bad = the least b whose v or a has a non-finite entry (left as set when none)
+__global__ void k_plan_heads_check(int B, const double *heads, int *bad) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    bool ok = true;
+    for (int k = 3; k < 9; k++) ok = ok && isfinite(heads[9 * (size_t)b + k]);
+    if (!ok) atomicMin(bad, b);
 }
 
 // one ragged copy: n doubles from src to dst

@@ -95,6 +95,65 @@ __global__ void __launch_bounds__(STATES_THREADS) k_traj_states(const int *off, 
     }
 }
 
+// ---- the rest of a trajectory from t0 (isdf_trajectory_shift) ------------------------------------------------------------------------
+// per trajectory b: the piece first[b] and local time tau[b] of t0[b] (traj_locate), and the pieces cnt[b] of the rest: 0 when t0 is not in
+// [0, D) (D the left-to-right sum of T), not finite, or the trajectory has no piece; piece first[b] counts when T_i - tau > 0. out_off[0] = 0.
+__global__ void k_shift_locate(int B, const int *off, const double *T, const double *t0, int *cnt, int *first, double *tau, int *out_off) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b == 0) out_off[0] = 0;
+    if (b >= B) return;
+    const int p0 = off[b], n = off[b + 1] - p0;
+    double D = 0.0;
+    for (int i = 0; i < n; i++) D += T[p0 + i];
+    double t = t0[b];
+    int c = 0, i = 0;
+    if (n > 0 && t >= 0.0 && t < D) {   // false for NaN; t < D excludes +Inf
+        const TrajView tr = {T + p0, nullptr, n};
+        i = traj_locate(tr, t);
+        c = (n - i - 1) + (T[p0 + i] - t > 0.0 ? 1 : 0);
+    }
+    cnt[b] = c; first[b] = i; tau[b] = t;
+}
+
+// one warp per trajectory: the rest's pieces at out_off[b], piece first[b] re-expanded about tau when kept, the later ones copied. Output
+// piece k of N' pieces has coefficient r of axis a at out_C + 18 out_off[b] + 6 (a N' + k) + r (6N' x 3 column-major).
+__global__ void k_shift_write(int B, const int *off, const double *T, const double *C, const int *cnt, const int *first, const double *tau,
+                              const int *out_off, double *out_T, double *out_C) {
+    const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (w >= B) return;
+    const int b = (int)w, n2 = cnt[b];
+    if (n2 == 0) return;
+    const int p0 = off[b], n = off[b + 1] - p0, i = first[b], o = out_off[b];
+    const int skip = (n - i) - n2;   // 1 when piece i is dropped (t0 on its end)
+    const double *Cb = C + 18 * (size_t)p0;
+    double *Co = out_C + 18 * (size_t)o;
+    // the copied pieces: output piece k is input piece i + skip + k, from k = 1 (k = 0 when piece i is dropped); 19 doubles per piece
+    const int kfirst = skip ? 0 : 1;
+    for (int e = lane; e < (n2 - kfirst) * 19; e += 32) {
+        const int k = kfirst + e / 19, r = e % 19, src = i + skip + k;
+        if (r == 18) out_T[o + k] = T[p0 + src];
+        else {
+            const int a = r / 6, m = r % 6;
+            Co[6 * (a * n2 + k) + m] = Cb[6 * (a * n + src) + m];
+        }
+    }
+    if (skip || lane >= 3) return;
+    // piece i about tau, one axis per lane: d_k = sum_{j=k..5} (C(j,k) c_j) tau^(j-k), ascending j, tau^m the running product
+    const double t = tau[b];
+    const double binom[6][6] = {{1, 0, 0, 0, 0, 0}, {1, 1, 0, 0, 0, 0}, {1, 2, 1, 0, 0, 0}, {1, 3, 3, 1, 0, 0}, {1, 4, 6, 4, 1, 0}, {1, 5, 10, 10, 5, 1}};
+    double pw[6];
+    pw[0] = 1.0;
+    for (int m = 1; m < 6; m++) pw[m] = pw[m - 1] * t;
+    const double *c = Cb + 6 * (lane * n + i);
+    for (int k = 0; k < 6; k++) {
+        double d = 0.0;
+        for (int j = k; j < 6; j++) d += (binom[j][k] * c[j]) * pw[j - k];
+        Co[6 * (lane * n2) + k] = d;
+    }
+    if (lane == 0) out_T[o] = T[p0 + i] - t;
+}
+
 constexpr int POSE_THREADS = 256;
 constexpr int POSE_MAX_STATES = 256;   // states per CTA
 constexpr long long POSE_TARGET = 8192;   // output doubles a CTA aims for: enough stores in flight per CTA, few CTAs for small P

@@ -50,7 +50,9 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_pose_clearance_default_params", "isdf_pose_clearance", "isdf_pose_clearance_device",
                "isdf_sense_default_params", "isdf_set_sense_cloud", "isdf_set_sense_cloud_device", "isdf_get_sense_info",
                "isdf_sense_depth", "isdf_sense_depth_device", "isdf_sense_cloud", "isdf_sense_cloud_device",
-               "isdf_world_default_params", "isdf_world_cloud", "isdf_world_cloud_device"]
+               "isdf_world_default_params", "isdf_world_cloud", "isdf_world_cloud_device",
+               "isdf_map_fuse_cloud", "isdf_map_fuse_cloud_device", "isdf_plan_states", "isdf_plan_states_device",
+               "isdf_trajectory_shift", "isdf_trajectory_shift_device"]
 WORLD_KINDS = dict(globalmap=1, perlin=2, boxes=3)   # isdf_world_kind
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
@@ -60,6 +62,9 @@ PLAN_FAILED, NO_PATH, TOO_LONG, MIDEND_FAILED, OPTIMISED = -1, 0, 1, 2, 3      #
 ESDF_FIELDS = dict(positive=0, negative=1, signed=2)                            # isdf_esdf_field
 STATE_DOUBLES = 20                                                               # ISDF_STATE_DOUBLES: pos vel acc jer quat(w,x,y,z) omg thr
 SIM_INIT_DOUBLES, SIM_DOUBLES = 17, 21   # ISDF_SIM_INIT_DOUBLES: pos vel quat(w,x,y,z) omega rpm; ISDF_SIM_DOUBLES: t pos vel quat omega rpm cmd_pos
+NAV_ACTIVE, NAV_ARRIVED, NAV_STOPPED, NAV_DIVERGED, NAV_TIMEOUT = 0, 1, 2, 3, 4   # Evaluator.navigate: a vehicle's status
+NAV_IDLE, NAV_KEPT, NAV_REPLANNED, NAV_REPLAN_FAILED = -1, 0, 1, 2               # Evaluator.navigate: a vehicle's action in a round
+NAV_NO_TRAJECTORY = -2                                                            # Evaluator.navigate: verdict of a round without one
 
 
 class SimParams(C.Structure):
@@ -176,6 +181,12 @@ def sim_log_records(p):
     """n_log: the log records per rollout under params p (isdf.h: (n_ticks - 1) / log_every + 1)"""
     n_ticks = int(np.floor(p.t_end * p.cmd_rate)) + 1
     return (n_ticks - 1) // max(p.log_every, 1) + 1
+
+
+def sim_init_from_log(records):
+    """the simulator states (..., 17) a rollout continues from: log records (..., 21) without t and the commanded position (pos, vel, quat,
+    omega, rpm are records[..., 1:18]); numpy arrays or tensors"""
+    return records[..., 1:1 + SIM_INIT_DOUBLES]
 
 
 def sim_init_from_trajectories(piece_off, coeffs, traj, params=None, rpm=None):
@@ -405,6 +416,14 @@ class MapInfo(C.Structure):
                     occupied_voxels=self.occupied_voxels, points_used=self.points_used, points_skipped=self.points_skipped)
 
 
+class FuseInfo(C.Structure):
+    """isdf_fuse_info"""
+    _fields_ = [(n, C.c_int64) for n in ["points_used", "points_outside", "points_skipped", "voxels_added"]]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 class FrontPathParams(C.Structure):
     """isdf_frontpath_params"""
     _fields_ = [("reserved_", C.c_int32 * 4)]
@@ -506,6 +525,10 @@ def load_library(path=None):
     lib.isdf_set_map_cloud.argtypes = [vp, vp, C.c_int64, C.c_int32, C.c_double, C.c_int32]
     lib.isdf_set_map_cloud_device.argtypes = [vp, vp, C.c_int64, C.c_int32, C.c_double, C.c_int32, vp]
     lib.isdf_get_map_info.argtypes = [vp, C.POINTER(MapInfo)]
+    lib.isdf_map_fuse_cloud.argtypes = [vp, vp, C.c_int64, C.c_int32, C.POINTER(FuseInfo)]
+    lib.isdf_map_fuse_cloud_device.argtypes = [vp, vp, C.c_int64, C.c_int32, C.POINTER(FuseInfo), vp]
+    lib.isdf_trajectory_shift.argtypes = [vp, C.c_int, ip, dp, dp, dp, ip, dp, dp]
+    lib.isdf_trajectory_shift_device.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.isdf_get_map_u8.argtypes = [vp, C.POINTER(C.c_uint8), C.c_int64]
     lib.isdf_get_map_f64.argtypes = [vp, dp, C.c_int64]
     lib.isdf_map_esdf.argtypes = [vp]
@@ -548,6 +571,8 @@ def load_library(path=None):
     lib.isdf_path_waypoints_device.argtypes = [vp, C.c_int, vp, vp, C.c_double, C.c_double, C.c_int, vp, vp, vp, vp]
     lib.isdf_plan_pairs_device.argtypes = [vp, C.c_int, vp, vp, C.POINTER(PlanParams), C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp,
                                            vp, vp]
+    lib.isdf_plan_states.argtypes = lib.isdf_plan_pairs.argtypes
+    lib.isdf_plan_states_device.argtypes = lib.isdf_plan_pairs_device.argtypes
     lib.isdf_plan_batch_device.argtypes = [vp, dp, C.c_int, vp, C.POINTER(PlanParams), C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp]
     pcp = C.POINTER(PoseClearanceParams)
     lib.isdf_pose_clearance_default_params.argtypes = [pcp]
@@ -767,6 +792,22 @@ class Evaluator:
         """points on the context's device: a float32 torch tensor (n, k >= 3), contiguous, or a raw device pointer with n and stride_bytes"""
         ptr, n, stride = _cloud_records_device(points, n, stride_bytes)
         self._check(self.lib.isdf_set_map_cloud_device(self.h, C.c_void_p(ptr), int(n), stride, float(res), int(sta_threshold), C.c_void_p(stream)))
+
+    def map_fuse_cloud(self, points, stride_bytes=None):
+        """adds a host cloud (as set_map_cloud takes it) to the current map in its frame (isdf_map_fuse_cloud) -> dict(points_used,
+        points_outside, points_skipped, voxels_added)"""
+        pts, n, stride = _cloud_records(points, stride_bytes)
+        info = FuseInfo()
+        self._check(self.lib.isdf_map_fuse_cloud(self.h, pts.ctypes.data_as(C.c_void_p) if n else None, n, stride, C.byref(info)))
+        return info.as_dict()
+
+    def map_fuse_cloud_device(self, points, n=None, stride_bytes=None, stream=0):
+        """adds a device cloud (as set_map_cloud_device takes it; sense_cloud_device's points as they are) to the current map in its frame
+        -> the isdf_fuse_info dict. Returns when the map is updated."""
+        ptr, n, stride = _cloud_records_device(points, n, stride_bytes)
+        info = FuseInfo()
+        self._check(self.lib.isdf_map_fuse_cloud_device(self.h, C.c_void_p(ptr), int(n), stride, C.byref(info), C.c_void_p(stream)))
+        return info.as_dict()
 
     # ---- depth sensing (isdf_sense_*): the scene cloud, depth images and sensed points at poses read in place ----
     def set_sense_cloud(self, points, stride_bytes=None):
@@ -1332,6 +1373,14 @@ class Evaluator:
         B = gl.shape[0]
         return self._plan(lambda p, *args: self.lib.isdf_plan_pairs(self.h, B, _dp(sts), _dp(gl), p, int(max_fields), *args), B, params, kw)
 
+    def plan_states(self, starts, goals, params=None, max_fields=0, **kw):
+        """isdf_plan_states: B (start state, goal) pairs, starts (B, 9) as p, v, a -> what plan_pairs returns"""
+        sts, gl = _f64(starts).reshape(-1, 9), _f64(goals).reshape(-1, 3)
+        if sts.shape[0] != gl.shape[0]:
+            raise ValueError(f"starts must be (B, 9) and goals (B, 3), got {sts.shape} and {gl.shape}")
+        B = gl.shape[0]
+        return self._plan(lambda p, *args: self.lib.isdf_plan_states(self.h, B, _dp(sts), _dp(gl), p, int(max_fields), *args), B, params, kw)
+
     def _plan(self, call, B, params, kw):
         """call(params, cap_nodes, path_off, path_xyz, cap_pieces, piece_off, T, coeffs, results, certify, dynamics): the C call"""
         p = params if params is not None else self.plan_params(**kw)
@@ -1367,6 +1416,16 @@ class Evaluator:
         sts, gl = _cuda_f64(starts), _cuda_f64(goals)
         return self._plan_device(lambda p, *a: self.lib.isdf_plan_pairs_device(self.h, gl.shape[0], C.c_void_p(sts.data_ptr()), C.c_void_p(gl.data_ptr()),
                                                                                 p, int(max_fields), *a),
+                                 gl, params, cap_nodes, cap_pieces, stream, kw)
+
+    def plan_states_device(self, starts, goals, params=None, max_fields=0, cap_nodes=None, cap_pieces=None, stream=None, **kw):
+        """isdf_plan_states_device: starts (B, 9) start states p, v, a and goals (B, 3), float64 CUDA tensors -> what plan_pairs_device
+        returns"""
+        if starts.dim() != 2 or starts.shape[1] != 9 or goals.dim() != 2 or goals.shape[1] != 3 or starts.shape[0] != goals.shape[0]:
+            raise ValueError(f"starts must be (B, 9) and goals (B, 3), got {tuple(starts.shape)} and {tuple(goals.shape)}")
+        sts, gl = _cuda_f64(starts), _cuda_f64(goals)
+        return self._plan_device(lambda p, *a: self.lib.isdf_plan_states_device(self.h, gl.shape[0], C.c_void_p(sts.data_ptr()), C.c_void_p(gl.data_ptr()),
+                                                                                 p, int(max_fields), *a),
                                  gl, params, cap_nodes, cap_pieces, stream, kw)
 
     def plan_batch_device(self, start, goals, params=None, cap_nodes=None, cap_pieces=None, stream=None, **kw):
@@ -1478,6 +1537,46 @@ class Evaluator:
         self._check(self.lib.isdf_trajectory_states_device(self.h, int(B), C.c_void_p(d_piece_off), C.c_void_p(d_T), C.c_void_p(d_coeffs), int(Q),
                                                            C.c_void_p(d_traj), C.c_void_p(d_times), C.c_void_p(d_out), C.c_void_p(stream)))
 
+    def trajectory_shift(self, plans_or_ragged, t0):
+        """isdf_trajectory_shift: the rest of each trajectory from its t0[b], re-timed to start at 0 -> (piece_off (B + 1 int32), T, coeffs)
+        in the ragged layout, trimmed to piece_off[B] pieces. plans_or_ragged as in trajectory_states."""
+        if isinstance(plans_or_ragged, tuple):
+            off, T, Cc = plans_or_ragged
+            off, T, Cc = np.ascontiguousarray(off, dtype=np.int32).reshape(-1), _f64(T).reshape(-1), _f64(Cc).reshape(-1)
+        else:
+            off, T, Cc = self.pack_plans(plans_or_ragged)
+        B = off.size - 1
+        t = _f64(t0).reshape(-1)
+        if t.size != B:
+            raise ValueError(f"t0 needs one time per trajectory ({B}), got {t.size}")
+        P = max(int(off[-1]), 1)
+        oo, oT, oC = np.zeros(B + 1, dtype=np.int32), np.zeros(P), np.zeros(18 * P)
+        ip = C.POINTER(C.c_int32)
+        self._check(self.lib.isdf_trajectory_shift(self.h, B, off.ctypes.data_as(ip), _dp(T), _dp(Cc), _dp(t), oo.ctypes.data_as(ip), _dp(oT), _dp(oC)))
+        return oo, oT[:oo[B]].copy(), oC[:18 * oo[B]].copy()
+
+    def trajectory_shift_device(self, piece_off, T, coeffs, t0, stream=None):
+        """isdf_trajectory_shift_device on CUDA tensors (piece_off B + 1 int32, T, coeffs, t0 (B,) float64) -> dict(piece_off, T, coeffs)
+        of CUDA tensors; T and coeffs have room for the input's pieces and hold piece_off[B] of them (not read here: nothing is waited
+        for). Runs on stream (None: torch's current stream)."""
+        import torch
+        if piece_off.dtype != torch.int32 or piece_off.dim() != 1 or piece_off.numel() < 2:
+            raise ValueError("piece_off must be a (B + 1) int32 CUDA tensor, B >= 1")
+        B, dev = piece_off.numel() - 1, piece_off.device
+        T, coeffs, t = _cuda_f64(T), _cuda_f64(coeffs), _cuda_f64(t0).reshape(-1)
+        if T.numel() == 0:   # no piece at all: the call still needs non-NULL arrays
+            T, coeffs = torch.zeros(1, dtype=torch.float64, device=dev), torch.zeros(18, dtype=torch.float64, device=dev)
+        if t.numel() != B:
+            raise ValueError(f"t0 needs one time per trajectory ({B}), got {t.numel()}")
+        po = piece_off.contiguous()
+        s = torch.cuda.current_stream(dev) if stream is None else stream
+        with torch.cuda.stream(s):
+            oo = torch.empty(B + 1, dtype=torch.int32, device=dev)
+            oT, oC = torch.empty(max(T.numel(), 1), dtype=torch.float64, device=dev), torch.empty(max(coeffs.numel(), 18), dtype=torch.float64, device=dev)
+        v = lambda x: C.c_void_p(x.data_ptr())
+        self._check(self.lib.isdf_trajectory_shift_device(self.h, B, v(po), v(T), v(coeffs), v(t), v(oo), v(oT), v(oC), C.c_void_p(s.cuda_stream)))
+        return dict(piece_off=oo, T=oT, coeffs=oC)
+
     def pose_points(self, states, body):
         """the body-frame points body (P, 3) posed at each of the (Q, 20) states -> (Q, P, 3): R(quat) b + pos (Shape::Transform)"""
         st = _f64(states).reshape(-1, STATE_DOUBLES)
@@ -1552,6 +1651,227 @@ class Evaluator:
         v = C.c_void_p
         return self.lib.isdf_simulate_device(self.h, int(B), v(d_piece_off), v(d_T), v(d_coeffs), int(R), v(d_traj), v(d_init), v(d_dist),
                                              C.byref(params), int(cap_log), v(d_log), v(d_summary), v(stream))
+
+    # ---- flying to goals through a world seen only through the depth camera (plan -> fly -> sense -> fuse -> check -> re-plan) ----
+    def navigate(self, starts, goals, *, rounds, horizon, sense_every=10, tol=0.5, plan_params=None, sim_params=None, sense_params=None,
+                 max_fields=0, stream=None):
+        """Drive B vehicles from starts (B, 3) to goals (B, 3) through the scene set by set_sense_cloud*, building their one shared map by
+        fusion into the current map's frame (set it first, e.g. set_map_u8 of zeros). Needs the shape, the front-end kernels and
+        plan_params with PLAN_CERTIFY (a shape the certificate supports). Each round, for the active vehicles:
+          1. sense   poses: every sense_every-th record of the last flown segment and its final record (a vehicle not flown: its current
+                     state); sense_cloud_device, then map_fuse_cloud_device;
+          2. check   trajectory_certify_device of every remaining trajectory on the fused map (one call per distinct piece count);
+          3. replan  vehicles without a CERTIFIED remaining trajectory: plan_states_device from the remaining trajectory's state at 0
+                     (trajectory_states_device p, v, a; without one the start at rest) with PLAN_CERTIFY; an OPTIMISED and CERTIFIED plan
+                     replaces it, else the remaining trajectory is kept and the replan counts as failed (a head outside the map fails
+                     without a call). A vehicle without a trajectory stays at rest and is not flown;
+          4. fly     one simulate_device call for t_end = horizon from the vehicles' simulator states;
+          5. advance the state becomes the last log record (sim_init_from_log), the trajectory trajectory_shift(horizon); a vehicle whose
+                     rest has no piece is ARRIVED within tol of its goal, else STOPPED; a diverged rollout is DIVERGED; vehicles still
+                     active after `rounds` are TIMEOUT.
+        Vehicles share the map, so one vehicle's run depends on what the others sensed; with B = 1 it is that vehicle's alone. The world
+        waits while the planner runs (no planning latency in simulated time). Within a round only per-vehicle values (stages, verdicts,
+        counts, piece totals, positions of heads) cross to the host; points, pieces and logs stay on the device.
+        Returns a dict: status, rounds_flown, replans, failed_replans, uncertified_rounds (B,) numpy; actions and verdicts (rounds run, B)
+        (NAV_IDLE / NAV_KEPT / NAV_REPLANNED / NAV_REPLAN_FAILED; the verdict of the trajectory flown, NAV_NO_TRAJECTORY without one);
+        replan_stages and replan_verdicts (rounds run, B): a replan's plan stage and certificate verdict (NAV_NO_TRAJECTORY: no plan call);
+        logs: per round (vehicle indices (R,) numpy, log (R, n_log, 21) CUDA tensor); times: per round {stage: ms} from CUDA events."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        s = torch.cuda.current_stream(dev) if stream is None else stream
+        st0, gl = _f64(starts).reshape(-1, 3), _f64(goals).reshape(-1, 3)
+        B = st0.shape[0]
+        if gl.shape[0] != B or B < 1:
+            raise ValueError(f"starts and goals must both be (B, 3), B >= 1, got {st0.shape} and {gl.shape}")
+        if int(rounds) < 1 or not horizon > 0 or int(sense_every) < 1:
+            raise ValueError("rounds and sense_every must be >= 1 and horizon > 0")
+        p = plan_params if plan_params is not None else self.plan_params()
+        if not p.flags & PLAN_CERTIFY:
+            raise ValueError("navigate checks trajectories with the certificate: plan_params needs PLAN_CERTIFY")
+        sp = SimParams.from_buffer_copy(bytes(sim_params if sim_params is not None else sim_default_params()))
+        sp.t_end = float(horizon)
+        cam = sense_params if sense_params is not None else globals()["sense_params"]()
+        cp = CertifyParams.from_buffer_copy(bytes(p.certify))
+        info = self.map_info()
+        lo, hi = info["bmin"], info["bmax"]
+        f64 = dict(dtype=torch.float64, device=dev)
+        sv = s.cuda_stream
+        with torch.cuda.stream(s):
+            d_goals = torch.as_tensor(gl, **f64)
+            init = torch.zeros((B, SIM_INIT_DOUBLES), **f64)   # at rest, level, at the hover rpm (as sim_init_from_trajectories)
+            init[:, 0:3] = torch.as_tensor(st0, **f64)
+            init[:, 6] = 1.0
+            init[:, 13:17] = float(np.sqrt(sp.mass * sp.grav / (4 * sp.kf)))
+            off = torch.zeros(B + 1, dtype=torch.int32, device=dev)      # the current trajectories, ragged; none yet
+            T, Cc = torch.zeros(1, **f64), torch.zeros(18, **f64)
+        n = np.zeros(B, dtype=np.int64)                                    # their piece counts (host)
+        status = np.full(B, NAV_ACTIVE)
+        flown_rounds, replans, failed, uncert = (np.zeros(B, dtype=np.int64) for _ in range(4))
+        actions, verdicts, replan_stages, replan_verdicts, logs, times = [], [], [], [], [], []
+        last = None   # (vehicle indices, log) of the last round flown
+        stages = ("sense", "fuse", "check", "replan", "fly", "advance")
+        for r in range(int(rounds)):
+            act = np.nonzero(status == NAV_ACTIVE)[0]
+            if act.size == 0:
+                break
+            ev = {k: (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for k in stages}
+            action, verdict = np.full(B, NAV_IDLE), np.full(B, NAV_NO_TRAJECTORY)
+            rstage, rverdict = np.full(B, NAV_NO_TRAJECTORY), np.full(B, NAV_NO_TRAJECTORY)
+            with torch.cuda.stream(s):
+                # 1. sense at the poses of the last flown segment (or the current state), then fuse what was seen
+                ev["sense"][0].record(s)
+                recs = []
+                flown_last = set() if last is None else set(last[0].tolist())
+                if last is not None:
+                    li, lg = last
+                    keep = np.isin(li, act)
+                    if keep.any():
+                        n_log = lg.shape[1]
+                        rows = sorted(set(range(0, n_log, int(sense_every))) | {n_log - 1})
+                        sel = lg[torch.as_tensor(np.nonzero(keep)[0], device=dev)][:, rows].reshape(-1, SIM_DOUBLES)
+                        recs.append(torch.cat([sel[:, 1:4], sel[:, 7:11]], 1))
+                rest = [b for b in act if b not in flown_last]
+                if rest:
+                    ini = init[torch.as_tensor(rest, device=dev)]
+                    recs.append(torch.cat([ini[:, 0:3], ini[:, 6:10]], 1))
+                pts, _ = self.sense_cloud_device(torch.cat(recs).contiguous(), 0, 3, params=cam, stream=s)
+                ev["sense"][1].record(s)
+                ev["fuse"][0].record(s)
+                if pts.shape[0]:
+                    self.map_fuse_cloud_device(pts, stream=sv)
+                ev["fuse"][1].record(s)
+                # 2. check every remaining trajectory on the fused map
+                ev["check"][0].record(s)
+                offh = np.zeros(B + 1, dtype=np.int64)
+                offh[1:] = np.cumsum(n)
+                have = [b for b in act if n[b] > 0]
+                ver = {}
+                for N in sorted({int(n[b]) for b in have}):
+                    grp = [b for b in have if n[b] == N]
+                    base = torch.as_tensor(offh[grp], device=dev)
+                    gT = T[(base[:, None] + torch.arange(N, device=dev)[None]).reshape(-1)].contiguous()
+                    gC = Cc[(18 * base[:, None] + torch.arange(18 * N, device=dev)[None])].reshape(len(grp), 3, 6 * N).permute(1, 0, 2).contiguous()
+                    summ = torch.empty((len(grp), C.sizeof(CertifySummary)), dtype=torch.uint8, device=dev)
+                    cp.clearance.pieces_per_traj = N
+                    self.trajectory_certify_device(len(grp) * N, gT.data_ptr(), gC.data_ptr(), cp, summ.data_ptr(), sv)
+                    v = summ[:, 40:44].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
+                    ver.update(zip(grp, v.tolist()))
+                ev["check"][1].record(s)
+                # 3. replan the vehicles without a certified remaining trajectory
+                ev["replan"][0].record(s)
+                need = [b for b in act if ver.get(b) != CERTIFIED]
+                for b in act:
+                    if b in ver:
+                        verdict[b] = ver[b]
+                new = {}   # vehicle -> (plan index) of an accepted plan
+                if need:
+                    heads = torch.zeros((len(need), 9), **f64)
+                    moving = [i for i, b in enumerate(need) if n[b] > 0]
+                    if moving:
+                        q = torch.as_tensor([need[i] for i in moving], dtype=torch.int32, device=dev)
+                        out = torch.empty((len(moving), STATE_DOUBLES), **f64)
+                        self.trajectory_states_device(B, off.data_ptr(), T.data_ptr(), Cc.data_ptr(), len(moving), q.data_ptr(),
+                                                      torch.zeros(len(moving), **f64).data_ptr(), out.data_ptr(), sv)
+                        heads[torch.as_tensor(moving, device=dev)] = out[:, :9]
+                    still = [i for i, b in enumerate(need) if n[b] == 0]
+                    if still:
+                        heads[torch.as_tensor(still, device=dev), :3] = torch.as_tensor(st0[[need[i] for i in still]], **f64)
+                    hp = heads[:, :3].cpu().numpy()
+                    inside = np.all((hp >= lo) & (hp <= hi), axis=1)
+                    ok = [i for i in range(len(need)) if inside[i]]
+                    if ok:
+                        oi = torch.as_tensor(ok, device=dev)
+                        pl = self.plan_states_device(heads[oi].contiguous(), d_goals[torch.as_tensor([need[i] for i in ok], device=dev)].contiguous(),
+                                                     params=p, max_fields=max_fields, stream=s)
+                        res = decode_plan_results(pl["results"])
+                        stage = res["stage"].cpu().numpy()
+                        cv = pl["certify"].reshape(-1, C.sizeof(CertifySummary))[:, 40:44].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
+                        for j, i in enumerate(ok):
+                            rstage[need[i]], rverdict[need[i]] = stage[j], cv[j]
+                            if stage[j] == OPTIMISED and cv[j] == CERTIFIED:
+                                new[need[i]] = j
+                    for b in need:
+                        replans[b] += 1
+                        if b in new:
+                            action[b], verdict[b] = NAV_REPLANNED, CERTIFIED
+                        else:
+                            action[b] = NAV_REPLAN_FAILED
+                            failed[b] += 1
+                    # the trajectories flown this round: the accepted plans, else the remaining ones
+                    if new:
+                        po = pl["piece_off"].cpu().numpy()
+                        nn = n.copy()
+                        partsT, partsC = [], []
+                        for b in range(B):
+                            if b in new:
+                                j = new[b]
+                                a, e = int(po[j]), int(po[j + 1])
+                                partsT.append(pl["T"][a:e]); partsC.append(pl["coeffs"][18 * a:18 * e])
+                                nn[b] = e - a
+                            elif n[b] > 0:
+                                partsT.append(T[offh[b]:offh[b + 1]]); partsC.append(Cc[18 * offh[b]:18 * offh[b + 1]])
+                        n = nn
+                        T, Cc = torch.cat(partsT).contiguous(), torch.cat(partsC).contiguous()
+                        offh = np.zeros(B + 1, dtype=np.int64)
+                        offh[1:] = np.cumsum(n)
+                        off = torch.as_tensor(offh.astype(np.int32), device=dev)
+                for b in act:
+                    if action[b] == NAV_IDLE:
+                        action[b] = NAV_KEPT
+                ev["replan"][1].record(s)
+                # 4. fly the vehicles that have a trajectory
+                ev["fly"][0].record(s)
+                fly = np.array([b for b in act if n[b] > 0], dtype=np.int64)
+                last = None
+                if fly.size:
+                    fi = torch.as_tensor(fly, device=dev)
+                    sim = self.simulate_device(off, T, Cc, fi.to(torch.int32), init[fi].contiguous(), params=sp, stream=s)
+                    last = (fly, sim["log"])
+                ev["fly"][1].record(s)
+                # 5. advance: the state at the horizon and the rest of each trajectory
+                ev["advance"][0].record(s)
+                if fly.size:
+                    lg = sim["log"]
+                    init[fi] = sim_init_from_log(lg[:, -1])
+                    diverged = sim["summary"][:, 84:88].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
+                    t0 = torch.zeros(B, **f64)
+                    t0[fi] = float(horizon)
+                    sh = self.trajectory_shift_device(off, T, Cc, t0, stream=s)
+                    offh = sh["piece_off"].cpu().numpy().astype(np.int64)
+                    n = np.diff(offh)
+                    off, T, Cc = sh["piece_off"], sh["T"], sh["coeffs"]
+                    dist = torch.linalg.norm(init[fi, 0:3] - d_goals[fi], dim=1).cpu().numpy()
+                    for k, b in enumerate(fly):
+                        flown_rounds[b] += 1
+                        if verdict[b] != CERTIFIED:
+                            uncert[b] += 1
+                        if diverged[k]:
+                            status[b] = NAV_DIVERGED
+                        elif n[b] == 0:
+                            status[b] = NAV_ARRIVED if dist[k] <= tol else NAV_STOPPED
+                    done = status != NAV_ACTIVE
+                    if done.any() and n[done].any():   # a vehicle that is done flies no more: its pieces go
+                        keep = [b for b in range(B) if n[b] > 0 and not done[b]]
+                        T = torch.cat([T[offh[b]:offh[b + 1]] for b in keep] or [torch.zeros(1, **f64)]).contiguous()
+                        Cc = torch.cat([Cc[18 * offh[b]:18 * offh[b + 1]] for b in keep] or [torch.zeros(18, **f64)]).contiguous()
+                        n = np.where(done, 0, n)
+                        offh = np.zeros(B + 1, dtype=np.int64)
+                        offh[1:] = np.cumsum(n)
+                        off = torch.as_tensor(offh.astype(np.int32), device=dev)
+                ev["advance"][1].record(s)
+            s.synchronize()
+            times.append({k: a.elapsed_time(e) for k, (a, e) in ev.items()})
+            actions.append(action)
+            verdicts.append(verdict)
+            replan_stages.append(rstage)
+            replan_verdicts.append(rverdict)
+            if last is not None:
+                logs.append(last)
+        status[status == NAV_ACTIVE] = NAV_TIMEOUT
+        return dict(status=status, rounds_flown=flown_rounds, replans=replans, failed_replans=failed, uncertified_rounds=uncert,
+                    actions=np.array(actions).reshape(-1, B), verdicts=np.array(verdicts).reshape(-1, B),
+                    replan_stages=np.array(replan_stages).reshape(-1, B), replan_verdicts=np.array(replan_verdicts).reshape(-1, B), logs=logs,
+                    times=times)
 
     def plan_info(self):
         info = PlanInfo()

@@ -174,6 +174,29 @@ typedef struct isdf_map_info {
 } isdf_map_info;
 /* any map, however it was set; ISDF_ERR_STATE without one */
 int isdf_get_map_info(isdf_ctx *ctx, isdf_map_info *out);
+
+/* Fusion: adds the points of a cloud to the current map, in its frame (a map sensed batch by batch, as a vehicle builds it in flight).
+ *   Records     isdf_set_map_cloud's format and checks (float32 x, y, z at byte offsets 0, 4, 8; stride a multiple of 4 and >= 12;
+ *               1 <= n < 2^32; 4-byte aligned); isdf_sense_cloud's output goes in with stride 12.
+ *   Frame       the map already set (ISDF_ERR_STATE without one) keeps X, Y, Z, bmin, bmax and res, however it was set. An empty frame is
+ *               isdf_set_map_u8 of a zero grid.
+ *   Inside      a finite record is inside when bmin <= (double)c <= bmax on every axis, with isdf_get_map_info's bmin and bmax (the
+ *               reference's isInMap); its voxel is isdf_set_map_cloud's index (getGridIndex). Records outside are dropped and counted in
+ *               points_outside; records with a NaN or Inf coordinate are counted in points_skipped; points_used counts the inside ones.
+ *   Occupancy   sta_threshold 1: a voxel hit by an inside record becomes occupied. Bits are only set, never cleared (no free-space
+ *               carving); voxels_added counts the bits this call set, so the sum over calls is the growth of occupied_voxels.
+ * The result is the same bits whatever the order of the points, however a cloud is split across calls, and through either form. A
+ * successful call gives up the distance field (isdf_map_esdf builds it again); isdf_map_info.occupied_voxels reflects the fused grid while
+ * points_used / points_skipped still describe the cloud that set the map. Refused calls leave map and field as they were; a CUDA failure
+ * leaves no map. info may be NULL. The call counts its launches in isdf_stats.kernel_launches. */
+typedef struct isdf_fuse_info {
+    int64_t points_used, points_outside, points_skipped, voxels_added;
+} isdf_fuse_info;
+int isdf_map_fuse_cloud(isdf_ctx *ctx, const void *points, int64_t n, int32_t stride_bytes, isdf_fuse_info *info);
+/* the same with the points on ctx's device: work before the call on cuda_stream is waited for, the grid is updated on ctx's own stream
+ * and the call returns when the map is updated (one 32-byte read of the counts), so d_points may be reused at once. */
+int isdf_map_fuse_cloud_device(isdf_ctx *ctx, const void *d_points, int64_t n, int32_t stride_bytes, isdf_fuse_info *info,
+                               void *cuda_stream);
 /* the grid as 0 / 1 in the setters' layout (address ix*Y*Z + iy*Z + iz), n = X*Y*Z elements (ISDF_ERR_INVALID otherwise). The f64
  * form fills the reference's occupancy_map->grid_map directly (after createGridMap(bmin, bmax) with isdf_get_map_info's frame). The
  * grid is expanded on the device in bounded chunks. */
@@ -999,6 +1022,21 @@ int isdf_plan_batch_device(isdf_ctx *ctx, const double *start, int B, const doub
                            int32_t *d_path_off, double *d_path_xyz, int cap_pieces, int32_t *d_piece_off, double *d_T, double *d_coeffs,
                            isdf_plan_result *d_results, isdf_certify_summary *d_certify, isdf_dynamics_summary *d_dynamics,
                            void *cuda_stream);
+/* B (start state, goal) pairs from moving vehicles: isdf_plan_pairs with starts as B x 9 doubles (p[3], v[3], a[3]) instead of B x 3.
+ * The front end starts at the voxel containing p, exactly as isdf_plan_pairs with starts[b] = p; the head of the mid-end and the back end
+ * is [p, v, a] instead of [path.front(), 0, 0]; the tail is unchanged. Everything else (stages, caps, certificates, the durations rule,
+ * outputs, the state left behind, isdf_get_plan_info, errors) is isdf_plan_pairs', plus ISDF_ERR_INVALID for a non-finite v or a. With
+ * starts[b] = (path.front() of an isdf_plan_pairs run, 0, 0) every output is bit-identical to isdf_plan_pairs. The device form reads the
+ * positions (24 bytes per pair) and one 4-byte verdict of a device-side finiteness check of v and a, so its transfers stay within
+ * isdf_plan_pairs_device's bounds. */
+int isdf_plan_states(isdf_ctx *ctx, int B, const double *starts, const double *goals, const isdf_plan_params *p, int max_fields,
+                     int cap_nodes, int32_t *path_off, double *path_xyz,
+                     int cap_pieces, int32_t *piece_off, double *T, double *coeffs,
+                     isdf_plan_result *results, isdf_certify_summary *certify, isdf_dynamics_summary *dynamics);
+int isdf_plan_states_device(isdf_ctx *ctx, int B, const double *d_starts, const double *d_goals, const isdf_plan_params *p, int max_fields,
+                            int cap_nodes, int32_t *d_path_off, double *d_path_xyz, int cap_pieces, int32_t *d_piece_off, double *d_T,
+                            double *d_coeffs, isdf_plan_result *d_results, isdf_certify_summary *d_certify,
+                            isdf_dynamics_summary *d_dynamics, void *cuda_stream);
 int isdf_get_plan_info(isdf_ctx *ctx, isdf_plan_info *out);
 
 /* ---- executing a trajectory: getStateOnTrajStamp (swm:307-341) and the playback of SweptVolumeManager::process (swm:948-988) ----
@@ -1030,6 +1068,20 @@ int isdf_trajectory_states(isdf_ctx *ctx, int B, const int32_t *piece_off, const
  * give identical bits. Errors: ISDF_ERR_INVALID for a NULL pointer, B < 1, Q < 0 or Q records beyond 2^63 bytes. */
 int isdf_trajectory_states_device(isdf_ctx *ctx, int B, const int32_t *d_piece_off, const double *d_T, const double *d_coeffs,
                                   int64_t Q, const int32_t *d_traj, const double *d_times, double *d_out, void *cuda_stream);
+/* the rest of B trajectories (isdf_plan_batch's ragged layout) from the per-trajectory times t0[b], re-timed to start at 0, written in the
+ * same layout to out_piece_off (B + 1), out_T and out_coeffs, which must have room for the input's piece_off[B] pieces:
+ *   - piece i and local time tau come from locatePieceIdx's rule, as in isdf_trajectory_states;
+ *   - output piece 0 is piece i re-expanded about tau, d_k = sum_{j=k..5} C(j,k) c_j tau^(j-k), accumulated from 0 in ascending j
+ *     as (C(j,k) c_j) tau^(j-k) with tau^m the running product of tau (FP64, nothing contracted), with duration T_i - tau; it is dropped when
+ *     T_i - tau is not > 0 (t0 on a junction). Pieces after i are copied bit for bit;
+ *   - a t0 outside [0, D_b) (D_b the left-to-right sum of T), not finite, or a trajectory without pieces gives 0 pieces: a result, not an error.
+ * The host form checks its inputs as isdf_trajectory_states' host form does (nothing is written on a refusal); the device form checks no
+ * device data and is enqueued on cuda_stream, not waited for. Both count their launches in isdf_stats.kernel_launches and give identical
+ * bits. Errors: ISDF_ERR_INVALID for a NULL pointer or B < 1. */
+int isdf_trajectory_shift(isdf_ctx *ctx, int B, const int32_t *piece_off, const double *T, const double *coeffs, const double *t0,
+                          int32_t *out_piece_off, double *out_T, double *out_coeffs);
+int isdf_trajectory_shift_device(isdf_ctx *ctx, int B, const int32_t *d_piece_off, const double *d_T, const double *d_coeffs,
+                                 const double *d_t0, int32_t *d_out_piece_off, double *d_out_T, double *d_out_coeffs, void *cuda_stream);
 /* the robot's body at Q states: out[(q * P + p) * 3 + k] = (R(quat_q) body_p + pos_q)_k, R = quat_rot (Eigen's toRotationMatrix,
  * Shape.hpp:753-757), each row ((R_k0 b0 + R_k1 b1) + R_k2 b2) + pos_k rounded per operation (Shape::Transform, Shape.hpp:786-793).
  * states: Q x 20, isdf_trajectory_states records (only pos and quat are read); body: P x 3 body-frame points (mesh vertices, interior
