@@ -2,7 +2,7 @@
 """bench_navigate.py — B vehicles fly to goals through a generated world they only see through the reference's depth camera
 (Evaluator.navigate: sense -> fuse -> check -> replan -> fly -> advance, every stage batched over vehicles); prints one JSON line.
 
-  python bench_navigate.py [--vehicles 1,16,64] [--rounds R] [--horizon H] [--sense-every S] [--seed N]
+  python bench_navigate.py [--vehicles 1,16,64] [--rounds R] [--horizon H] [--sense-every S] [--seed N] [--fallback keep|brake]
 
 World: mockamap's box world (isdf_world_cloud_device, ISDF_WORLD_BOXES) with seed 511, 40 x 40 x 10 m at 0.5 m (size 80 x 80 x 20,
 scale 2), 20 boxes 1.5 to 3 m wide: x and y in [-20, 20] m, z in [0, 10] m. The vehicles' map starts as an empty 1 m frame over that box
@@ -13,7 +13,8 @@ Start / goal pairs are seeded: starts at x in [-17, -12], goals at x in [12, 17]
 map at least 2 voxels from any occupied one. The true map (the whole world fused into the same frame, in a second context) checks every
 flown pose with pose_clearance_device.
 Per B: per-stage milliseconds per round (mean over the rounds run, CUDA events), rounds run, arrivals, failed replans, and the minimum true
-clearance over every flown pose. Writes nothing to the tree.
+clearance over every flown pose. --fallback brake (navigate's fallback, DESIGN §3.21) adds the stops taken and the rounds held; the
+default, keep, prints what it always printed. Writes nothing to the tree.
 """
 import argparse
 import json
@@ -76,6 +77,7 @@ def main():
     ap.add_argument("--horizon", type=float, default=0.5)
     ap.add_argument("--sense-every", type=int, default=25)
     ap.add_argument("--seed", type=int, default=7)
+    ap.add_argument("--fallback", choices=("keep", "brake"), default="keep")
     args = ap.parse_args()
     import torch
     import isdf_b200 as I
@@ -93,6 +95,9 @@ def main():
     occ = truth.get_map_u8()
     out = dict(bench="navigate", gpu=gpu, world="mockamap boxes seed 511, 40 x 40 x 10 m, 20 boxes; 1 m frame", points=int(scene.shape[0]),
                horizon_s=args.horizon, sense_every=args.sense_every, runs=[])
+    brake = args.fallback == "brake"
+    if brake:
+        out["fallback"] = "brake"
     for B in [int(v) for v in args.vehicles.split(",")]:
         starts, goals = pairs(occ, B, args.seed + B)
         ev = I.Evaluator(cfg)
@@ -102,8 +107,8 @@ def main():
         ev.set_sense_cloud_device(scene, stream=torch.cuda.current_stream().cuda_stream)
         r = ev.navigate(starts, goals, rounds=args.rounds, horizon=args.horizon, sense_every=args.sense_every, tol=1.0,
                         plan_params=ev.plan_params(flags=I.PLAN_CERTIFY, backend_max_iterations=200),
-                        sense_params=I.sense_params(sensing_horizon=15.0))
-        fail = r["actions"] == I.NAV_REPLAN_FAILED
+                        sense_params=I.sense_params(sensing_horizon=15.0), fallback=args.fallback)
+        fail = np.isin(r["actions"], [I.NAV_REPLAN_FAILED, I.NAV_BRAKED, I.NAV_HELD]) if brake else r["actions"] == I.NAV_REPLAN_FAILED
         why = {}   # failed replans by (plan stage, certificate verdict); -2: no plan call (a head outside the frame)
         for st, v in zip(r["replan_stages"][fail], r["replan_verdicts"][fail]):
             why[f"{st}/{v}"] = why.get(f"{st}/{v}", 0) + 1
@@ -115,6 +120,8 @@ def main():
                                 replans=int(r["replans"].sum()), failed_replans=int(r["failed_replans"].sum()), failed_by_stage_verdict=why,
                                 uncertified_rounds=int(r["uncertified_rounds"].sum()), map_voxels=int(ev.map_info()["occupied_voxels"]),
                                 min_true_clearance=round(min_clearance(truth, r["logs"]), 4)))
+        if brake:
+            out["runs"][-1].update(brakes=int(r["brakes"].sum()), held_rounds=int(r["held_rounds"].sum()))
         ev.close()
     truth.close()
     print(json.dumps(out))

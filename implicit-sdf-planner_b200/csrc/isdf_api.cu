@@ -16,6 +16,7 @@
 #include "isdf_map.cuh"
 #include "isdf_esdf.cuh"
 #include "isdf_states.cuh"
+#include "isdf_brake.cuh"
 #include "isdf_plan.cuh"
 #include "isdf_sim.cuh"
 #include "isdf_sense.cuh"
@@ -281,6 +282,12 @@ struct isdf_ctx {
     struct {   // isdf_trajectory_shift: per-trajectory piece counts, first piece and its local time, the scan's scratch
         DevBuf<int> d_cnt, d_first; DevBuf<double> d_tau; DevBuf<char> d_tmp;
     } shift;
+    struct {   // isdf_trajectory_brake: the candidates' MINCO workspace (its own, so the mid-end's and the back end's stay as they were),
+               // their heads, tails, durations and decision vectors, summaries, per-trajectory counts and picks, the scan's scratch
+        MincoWork minco;
+        DevBuf<double> d_head, d_tail, d_Tin, d_x; DevBuf<CertSummary> d_csum; DevBuf<DynSummary> d_dsum;
+        DevBuf<int> d_cnt, d_pick; DevBuf<char> d_tmp;
+    } brake;
     struct {   // waypoint selection on the device (isdf_path_waypoints_device): per-path counts and gaps, the scan's scratch
         DevBuf<int32_t> d_cnt, d_gap; DevBuf<char> d_tmp; PinnedBuf<int32_t> h_total;
     } wps;
@@ -3290,6 +3297,132 @@ extern "C" int isdf_trajectory_dynamics(isdf_ctx *c, int N, const double *T, con
                             isdf_trajectory_dynamics_device);
 }
 
+// a public struct as the device struct of the same layout
+template <typename D, typename S>
+static D same_layout(const S &s) {
+    static_assert(sizeof(D) == sizeof(S), "layouts differ");
+    D d;
+    std::memcpy(&d, &s, sizeof(D));
+    return d;
+}
+
+// ---- braking to a certified stop (isdf_brake.cuh) ----------------------------------------------------------------------------------
+static_assert(sizeof(isdf_brake_summary) == sizeof(BrakeSummary) && offsetof(isdf_brake_summary, certify) == offsetof(BrakeSummary, cert) &&
+              offsetof(isdf_brake_summary, dynamics) == offsetof(BrakeSummary, dyn) && offsetof(isdf_brake_summary, certified) == offsetof(BrakeSummary, certified),
+              "isdf_brake_summary layout");
+
+extern "C" int isdf_brake_default_params(isdf_ctx *c, isdf_brake_params *p) {
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    std::memset(p, 0, sizeof(*p));
+    p->candidates = 8; p->pieces = 4;
+    isdf_certify_default_params(&p->certify);
+    isdf_dynamics_default_params(c, &p->dynamics);
+    return 0;
+}
+
+// every check that needs no device work, in the order of include/isdf.h's error list; *pc / *pd: the certificates' parameters with N0 = M,
+// *r as certify_shape
+static int brake_check(isdf_ctx *c, int B, const isdf_brake_params *p, isdf_certify_params *pc, isdf_dynamics_params *pd, double *r) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    if (B < 1) return fail(ISDF_ERR_INVALID, "B < 1");
+    if (p->candidates < 1) return fail(ISDF_ERR_INVALID, "candidates < 1");
+    if (p->pieces < 1 || p->pieces > ISDF_BRAKE_MAX_PIECES) return fail(ISDF_ERR_INVALID, "pieces must lie in [1, ISDF_BRAKE_MAX_PIECES]");
+    if (p->reserved_[0] || p->reserved_[1]) return fail(ISDF_ERR_INVALID, "reserved_ must be 0");
+    if (p->certify.clearance.pieces_per_traj != 0) return fail(ISDF_ERR_INVALID, "certify.clearance.pieces_per_traj must be 0 (the call sets M)");
+    if (p->dynamics.pieces_per_traj != 0) return fail(ISDF_ERR_INVALID, "dynamics.pieces_per_traj must be 0 (the call sets M)");
+    const long long n = (long long)B * p->candidates * p->pieces;
+    if (n > 0x7fffffffll) return fail(ISDF_ERR_INVALID, "B * candidates * pieces must fit in 31 bits");
+    *pc = p->certify; pc->clearance.pieces_per_traj = p->pieces;
+    *pd = p->dynamics; pd->pieces_per_traj = p->pieces;
+    if (int rc = certify_check(c, (int)n, pc, r)) return rc;
+    return dynamics_check(c, (int)n, pd);
+}
+
+// the brake on st (include/isdf.h): setup, MINCO, both certificates over the B K candidates, select, scan, write
+static int brake_run(isdf_ctx *c, int B, const int *d_off, const double *d_T, const double *d_C, const double *d_ts, const isdf_brake_params *p,
+                     const isdf_certify_params &pc, const isdf_dynamics_params &pd, double r, int *d_out_off, double *d_out_T, double *d_out_C,
+                     BrakeSummary *d_sum, cudaStream_t st) {
+    auto &z = c->brake;
+    const int K = p->candidates, M = p->pieces, Q = B * K, n = Q * M;
+    const Layout L = uniform_layout(Q, M);
+    if (int rc = z.minco.ensure(L)) return rc;
+    CU_TRY(z.d_head.ensure(9 * (size_t)Q)); CU_TRY(z.d_tail.ensure(9 * (size_t)Q)); CU_TRY(z.d_Tin.ensure((size_t)n)); CU_TRY(z.d_x.ensure(L.X));
+    CU_TRY(z.d_csum.ensure(Q)); CU_TRY(z.d_dsum.ensure(Q)); CU_TRY(z.d_cnt.ensure(B)); CU_TRY(z.d_pick.ensure(B));
+    size_t tmp = 0;
+    CU_TRY(cub::DeviceScan::InclusiveSum(nullptr, tmp, z.d_cnt.p, d_out_off + 1, B, st));
+    CU_TRY(z.d_tmp.ensure(std::max<size_t>(tmp, 1)));
+    const double *bm = c->map.grid.bmin;
+    k_brake_setup<<<(unsigned)((Q + 127) / 128), 128, 0, st>>>(B, K, M, d_off, d_T, d_C, d_ts, bm[0], bm[1], bm[2], z.d_head.p, z.d_tail.p, z.d_Tin.p, z.d_x.p);
+    MincoArgs A = z.minco.args(L, z.d_head.p, z.d_tail.p, 9, 0.0, z.d_x.p);
+    A.T_in = z.d_Tin.p;
+    k_minco_forward<<<Q, 32, minco_smem_bytes(M), st>>>(A);
+    c->stats.kernel_launches += 2;
+    CU_TRY(cudaGetLastError());
+    if (int rc = certify_run(c, n, A.T, A.C, &pc, r, z.d_csum.p, st)) return rc;
+    if (int rc = dynamics_run(c, n, A.T, A.C, &pd, z.d_dsum.p, st)) return rc;
+    const CertSummary cbad = same_layout<CertSummary>(certify_failed_summary());
+    const DynSummary dbad = same_layout<DynSummary>(dynamics_failed_summary());
+    k_brake_select<<<(unsigned)((B + 127) / 128), 128, 0, st>>>(B, K, M, d_off, d_T, d_ts, A.T, z.d_csum.p, z.d_dsum.p, cbad, dbad, d_sum, z.d_cnt.p,
+                                                                z.d_pick.p, d_out_off);
+    CU_TRY(cub::DeviceScan::InclusiveSum(z.d_tmp.p, tmp, z.d_cnt.p, d_out_off + 1, B, st));
+    k_brake_write<<<(unsigned)(((long long)B * 32 + 127) / 128), 128, 0, st>>>(B, K, M, z.d_pick.p, A.T, A.C, d_out_off, d_out_T, d_out_C);
+    c->stats.kernel_launches += 3;
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaStreamSynchronize(st));
+    return 0;
+}
+
+// on failure every summary reads status NONE, candidate -1, NaN times, counts -1 and the certificates' failed-call summaries
+static isdf_brake_summary brake_failed_summary() {
+    isdf_brake_summary s;
+    s.status = ISDF_BRAKE_NONE; s.candidate = -1;
+    s.tau_stop = s.duration = std::numeric_limits<double>::quiet_NaN();
+    s.certified = s.feasible = -1;
+    s.certify = certify_failed_summary(); s.dynamics = dynamics_failed_summary();
+    return s;
+}
+
+extern "C" int isdf_trajectory_brake(isdf_ctx *c, int B, const int32_t *piece_off, const double *T, const double *coeffs, const double *t_stop_max,
+                                     const isdf_brake_params *p, int32_t *out_piece_off, double *out_T, double *out_coeffs, isdf_brake_summary *summary) {
+    return poison_on_failure([&]() -> int {
+        isdf_certify_params pc; isdf_dynamics_params pd; double r = 0.0;
+        if (!c || !piece_off || !T || !coeffs || !t_stop_max || !out_piece_off || !out_T || !out_coeffs || !summary) return fail(ISDF_ERR_INVALID, "NULL argument");
+        if (int rc = brake_check(c, B, p, &pc, &pd, &r)) return rc;
+        if (int rc = offsets_check(piece_off, B, "piece_off", true)) return rc;
+        const int P = piece_off[B];
+        if (int rc = swept_traj_check(P, T, coeffs)) return rc;
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        const size_t cap = (size_t)B * p->pieces;
+        Staging S(c);
+        const double *d_C, *d_T, *d_ts;
+        const int *d_off;
+        int *d_out_off;
+        double *d_out_T, *d_out_C;
+        isdf_brake_summary *d_sum;
+        S.in(&d_C, coeffs, 18 * (size_t)P); S.in(&d_T, T, (size_t)P); S.in(&d_ts, t_stop_max, (size_t)B); S.in(&d_off, piece_off, (size_t)B + 1);
+        S.out(&d_sum, summary, (size_t)B); S.out(&d_out_off, out_piece_off, (size_t)B + 1);
+        S.out(&d_out_T, out_T, cap); S.out(&d_out_C, out_coeffs, 18 * cap);
+        if (int rc = S.upload()) return rc;
+        if (int rc = brake_run(c, B, d_off, d_T, d_C, d_ts, p, pc, pd, r, d_out_off, d_out_T, d_out_C, (BrakeSummary *)d_sum, c->stream)) return rc;
+        return S.download();
+    }, [&] { if (B >= 1) write_failed_summaries(summary, B, brake_failed_summary()); });
+}
+
+extern "C" int isdf_trajectory_brake_device(isdf_ctx *c, int B, const int32_t *d_piece_off, const double *d_T, const double *d_coeffs,
+                                            const double *d_t_stop_max, const isdf_brake_params *p, int32_t *d_out_piece_off, double *d_out_T,
+                                            double *d_out_coeffs, isdf_brake_summary *d_summary, void *cuda_stream) {
+    const cudaStream_t st = (cudaStream_t)cuda_stream;
+    return poison_on_failure([&]() -> int {
+        isdf_certify_params pc; isdf_dynamics_params pd; double r = 0.0;
+        if (!c || !d_piece_off || !d_T || !d_coeffs || !d_t_stop_max || !d_out_piece_off || !d_out_T || !d_out_coeffs || !d_summary)
+            return fail(ISDF_ERR_INVALID, "NULL argument");
+        if (int rc = brake_check(c, B, p, &pc, &pd, &r)) return rc;
+        if (set_device(c)) return ISDF_ERR_CUDA;
+        return brake_run(c, B, d_piece_off, d_T, d_coeffs, d_t_stop_max, p, pc, pd, r, d_out_piece_off, d_out_T, d_out_coeffs, (BrakeSummary *)d_summary, st);
+    }, [&] { if (c && B >= 1) write_failed_summaries(d_summary, B, brake_failed_summary(), c, st); });
+}
+
 // ---- certified swept volume (isdf_sweptvol.cuh) ------------------------------------------------------------------------------------
 extern "C" int isdf_swept_default_params(isdf_swept_params *p) {
     if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
@@ -4331,15 +4464,6 @@ static int copy_segments(isdf_ctx *c, const std::vector<CopySeg> &seg, cudaStrea
     c->stats.kernel_launches++;
     CU_TRY(cudaGetLastError());
     return 0;
-}
-
-// a public struct as the device struct of the same layout
-template <typename D, typename S>
-static D same_layout(const S &s) {
-    static_assert(sizeof(D) == sizeof(S), "layouts differ");
-    D d;
-    std::memcpy(&d, &s, sizeof(D));
-    return d;
 }
 
 template <typename S>

@@ -40,6 +40,7 @@ struct MincoArgs {
     double *cost;             // B
     double *grad;             // laid out as x
     int seq_terms;            // 1: the piece costs are added to the energy one at a time (the mid-end, isdf_midend.cuh); 0: summed first
+    const double *T_in;       // may be null: P durations used as they are (isdf_trajectory_brake); null: T = forwardT(tau) of x
 };
 
 __device__ __forceinline__ double &band(double *a, int n, int i, int j) { return a[(size_t)(i - j + 6) * n + j]; }
@@ -71,8 +72,12 @@ __global__ void __launch_bounds__(32) k_minco_forward(const __grid_constant__ Mi
     const double *x = A.x + (size_t)4 * p0 - 3 * b;
     const double *head = A.head + (size_t)b * A.bc_stride, *tail = A.tail + (size_t)b * A.bc_stride;
     for (int i = lane; i < N; i += 32) {
-        const double t = x[i];
-        const double Ti = t > 0.0 ? ((0.5 * t + 1.0) * t + 1.0) : 1.0 / ((0.5 * t - 1.0) * t + 1.0);
+        double Ti;
+        if (A.T_in) Ti = A.T_in[(size_t)p0 + i];
+        else {
+            const double t = x[i];
+            Ti = t > 0.0 ? ((0.5 * t + 1.0) * t + 1.0) : 1.0 / ((0.5 * t - 1.0) * t + 1.0);
+        }
         sT[i] = Ti;
         A.T[(size_t)p0 + i] = Ti;
     }

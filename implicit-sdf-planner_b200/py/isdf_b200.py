@@ -52,7 +52,8 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_sense_depth", "isdf_sense_depth_device", "isdf_sense_cloud", "isdf_sense_cloud_device",
                "isdf_world_default_params", "isdf_world_cloud", "isdf_world_cloud_device",
                "isdf_map_fuse_cloud", "isdf_map_fuse_cloud_device", "isdf_plan_states", "isdf_plan_states_device",
-               "isdf_trajectory_shift", "isdf_trajectory_shift_device"]
+               "isdf_trajectory_shift", "isdf_trajectory_shift_device", "isdf_brake_default_params", "isdf_trajectory_brake",
+               "isdf_trajectory_brake_device"]
 WORLD_KINDS = dict(globalmap=1, perlin=2, boxes=3)   # isdf_world_kind
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
@@ -65,6 +66,9 @@ SIM_INIT_DOUBLES, SIM_DOUBLES = 17, 21   # ISDF_SIM_INIT_DOUBLES: pos vel quat(w
 NAV_ACTIVE, NAV_ARRIVED, NAV_STOPPED, NAV_DIVERGED, NAV_TIMEOUT = 0, 1, 2, 3, 4   # Evaluator.navigate: a vehicle's status
 NAV_IDLE, NAV_KEPT, NAV_REPLANNED, NAV_REPLAN_FAILED = -1, 0, 1, 2               # Evaluator.navigate: a vehicle's action in a round
 NAV_NO_TRAJECTORY = -2                                                            # Evaluator.navigate: verdict of a round without one
+NAV_BRAKED, NAV_HELD = 3, 4                        # Evaluator.navigate(fallback="brake"): a vehicle's action in a round
+BRAKE_NO_INPUT, BRAKE_NONE, BRAKED = -1, 0, 1      # isdf_brake_summary.status
+BRAKE_MAX_PIECES = 64                              # ISDF_BRAKE_MAX_PIECES
 
 
 class SimParams(C.Structure):
@@ -327,6 +331,29 @@ class DynamicsSummary(C.Structure):
         return {n: (np.array(getattr(self, n)[:]) if n in ("upper", "attained", "t_attained") else getattr(self, n)) for n, _ in self._fields_}
 
 
+class BrakeParams(C.Structure):
+    """isdf_brake_params"""
+    _fields_ = [("candidates", C.c_int32), ("pieces", C.c_int32), ("certify", CertifyParams), ("dynamics", DynamicsParams),
+                ("reserved_", C.c_int32 * 2)]
+
+
+class BrakeSummary(C.Structure):
+    """isdf_brake_summary"""
+    _fields_ = [("status", C.c_int32), ("candidate", C.c_int32), ("tau_stop", C.c_double), ("duration", C.c_double),
+                ("certified", C.c_int32), ("feasible", C.c_int32), ("certify", CertifySummary), ("dynamics", DynamicsSummary)]
+
+    def as_dict(self):
+        d = {n: getattr(self, n) for n, _ in self._fields_[:6]}
+        d.update(certify=self.certify.as_dict(), dynamics=self.dynamics.as_dict())
+        return d
+
+
+def decode_brake_summaries(raw):
+    """isdf_trajectory_brake_device's raw summaries ((B, 256) uint8, on any device) -> list of B dicts (BrakeSummary.as_dict)"""
+    b = np.ascontiguousarray(raw.cpu().numpy() if hasattr(raw, "cpu") else raw, dtype=np.uint8).reshape(-1, C.sizeof(BrakeSummary))
+    return [BrakeSummary.from_buffer_copy(r.tobytes()).as_dict() for r in b]
+
+
 class PlanParams(C.Structure):
     """isdf_plan_params"""
     _fields_ = [("parlength", C.c_double), ("half_extent", C.c_double), ("offset", C.c_double * 3), ("rho", C.c_double), ("midend", MidendParams),
@@ -529,6 +556,9 @@ def load_library(path=None):
     lib.isdf_map_fuse_cloud_device.argtypes = [vp, vp, C.c_int64, C.c_int32, C.POINTER(FuseInfo), vp]
     lib.isdf_trajectory_shift.argtypes = [vp, C.c_int, ip, dp, dp, dp, ip, dp, dp]
     lib.isdf_trajectory_shift_device.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.isdf_brake_default_params.argtypes = [vp, C.POINTER(BrakeParams)]
+    lib.isdf_trajectory_brake.argtypes = [vp, C.c_int, ip, dp, dp, dp, C.POINTER(BrakeParams), ip, dp, dp, C.POINTER(BrakeSummary)]
+    lib.isdf_trajectory_brake_device.argtypes = [vp, C.c_int, vp, vp, vp, vp, C.POINTER(BrakeParams), vp, vp, vp, vp, vp]
     lib.isdf_get_map_u8.argtypes = [vp, C.POINTER(C.c_uint8), C.c_int64]
     lib.isdf_get_map_f64.argtypes = [vp, dp, C.c_int64]
     lib.isdf_map_esdf.argtypes = [vp]
@@ -1577,6 +1607,67 @@ class Evaluator:
         self._check(self.lib.isdf_trajectory_shift_device(self.h, B, v(po), v(T), v(coeffs), v(t), v(oo), v(oT), v(oC), C.c_void_p(s.cuda_stream)))
         return dict(piece_off=oo, T=oT, coeffs=oC)
 
+    def brake_params(self, **kw):
+        """isdf_brake_default_params for this context, then overrides by name: candidates, pieces, certify (an isdf_certify_params),
+        dynamics (an isdf_dynamics_params)"""
+        p = BrakeParams()
+        self._check(self.lib.isdf_brake_default_params(self.h, C.byref(p)))
+        for k, v in kw.items():
+            if k not in {n for n, _ in BrakeParams._fields_} or k == "reserved_":
+                raise TypeError(f"unknown isdf_brake_params field {k}")
+            setattr(p, k, v)
+        return p
+
+    def trajectory_brake(self, plans_or_ragged, t_stop_max, params=None):
+        """isdf_trajectory_brake: a certified stop along each remaining trajectory, reaching no further than its time t_stop_max[b] ->
+        (piece_off (B + 1 int32), T, coeffs) of the stops in the ragged layout (trimmed to piece_off[B] pieces), list of B summary dicts.
+        plans_or_ragged as in trajectory_states."""
+        if isinstance(plans_or_ragged, tuple):
+            off, T, Cc = plans_or_ragged
+            off, T, Cc = np.ascontiguousarray(off, dtype=np.int32).reshape(-1), _f64(T).reshape(-1), _f64(Cc).reshape(-1)
+        else:
+            off, T, Cc = self.pack_plans(plans_or_ragged)
+        p = params if params is not None else self.brake_params()
+        B = off.size - 1
+        ts = _f64(t_stop_max).reshape(-1)
+        if ts.size != B:
+            raise ValueError(f"t_stop_max needs one time per trajectory ({B}), got {ts.size}")
+        if T.size == 0:   # no piece at all: the call still needs non-NULL arrays
+            T, Cc = np.zeros(1), np.zeros(18)
+        cap = max(B * int(p.pieces), 1)
+        oo, oT, oC = np.zeros(B + 1, dtype=np.int32), np.zeros(cap), np.zeros(18 * cap)
+        summ = (BrakeSummary * max(B, 1))()
+        ip = C.POINTER(C.c_int32)
+        self._check(self.lib.isdf_trajectory_brake(self.h, B, off.ctypes.data_as(ip), _dp(T), _dp(Cc), _dp(ts), C.byref(p), oo.ctypes.data_as(ip),
+                                                   _dp(oT), _dp(oC), summ))
+        return (oo, oT[:oo[B]].copy(), oC[:18 * oo[B]].copy()), [summ[b].as_dict() for b in range(B)]
+
+    def trajectory_brake_device(self, piece_off, T, coeffs, t_stop_max, params=None, stream=None):
+        """isdf_trajectory_brake_device on CUDA tensors (piece_off B + 1 int32, T, coeffs, t_stop_max (B,) float64) -> dict(piece_off, T,
+        coeffs, summary): CUDA tensors, T and coeffs with room for B * pieces pieces and holding piece_off[B] of them, summary (B, 256) uint8
+        (decode with decode_brake_summaries). Runs on stream (None: torch's current stream) and returns when the outputs are written."""
+        import torch
+        if piece_off.dtype != torch.int32 or piece_off.dim() != 1 or piece_off.numel() < 2:
+            raise ValueError("piece_off must be a (B + 1) int32 CUDA tensor, B >= 1")
+        p = params if params is not None else self.brake_params()
+        B, dev = piece_off.numel() - 1, piece_off.device
+        T, coeffs, ts = _cuda_f64(T), _cuda_f64(coeffs), _cuda_f64(t_stop_max).reshape(-1)
+        if T.numel() == 0:
+            T, coeffs = torch.zeros(1, dtype=torch.float64, device=dev), torch.zeros(18, dtype=torch.float64, device=dev)
+        if ts.numel() != B:
+            raise ValueError(f"t_stop_max needs one time per trajectory ({B}), got {ts.numel()}")
+        po = piece_off.contiguous()
+        s = torch.cuda.current_stream(dev) if stream is None else stream
+        cap = max(B * int(p.pieces), 1)
+        with torch.cuda.stream(s):
+            oo = torch.empty(B + 1, dtype=torch.int32, device=dev)
+            oT, oC = torch.empty(cap, dtype=torch.float64, device=dev), torch.empty(18 * cap, dtype=torch.float64, device=dev)
+            sm = torch.empty((B, C.sizeof(BrakeSummary)), dtype=torch.uint8, device=dev)
+        v = lambda x: C.c_void_p(x.data_ptr())
+        self._check(self.lib.isdf_trajectory_brake_device(self.h, B, v(po), v(T), v(coeffs), v(ts), C.byref(p), v(oo), v(oT), v(oC), v(sm),
+                                                          C.c_void_p(s.cuda_stream)))
+        return dict(piece_off=oo, T=oT, coeffs=oC, summary=sm)
+
     def pose_points(self, states, body):
         """the body-frame points body (P, 3) posed at each of the (Q, 20) states -> (Q, P, 3): R(quat) b + pos (Shape::Transform)"""
         st = _f64(states).reshape(-1, STATE_DOUBLES)
@@ -1654,7 +1745,7 @@ class Evaluator:
 
     # ---- flying to goals through a world seen only through the depth camera (plan -> fly -> sense -> fuse -> check -> re-plan) ----
     def navigate(self, starts, goals, *, rounds, horizon, sense_every=10, tol=0.5, plan_params=None, sim_params=None, sense_params=None,
-                 max_fields=0, stream=None):
+                 max_fields=0, stream=None, fallback="keep", brake_params=None):
         """Drive B vehicles from starts (B, 3) to goals (B, 3) through the scene set by set_sense_cloud*, building their one shared map by
         fusion into the current map's frame (set it first, e.g. set_map_u8 of zeros). Needs the shape, the front-end kernels and
         plan_params with PLAN_CERTIFY (a shape the certificate supports). Each round, for the active vehicles:
@@ -1669,13 +1760,22 @@ class Evaluator:
           5. advance the state becomes the last log record (sim_init_from_log), the trajectory trajectory_shift(horizon); a vehicle whose
                      rest has no piece is ARRIVED within tol of its goal, else STOPPED; a diverged rollout is DIVERGED; vehicles still
                      active after `rounds` are TIMEOUT.
+        fallback: what a vehicle whose replan failed flies. "keep": its remaining trajectory, as above. "brake": after step 3, every such
+        vehicle with a remaining trajectory gets one batched trajectory_brake_device call (t_stop_max: the check's first_hit when it is
+        COLLIDING, else +inf; brake_params defaults to brake_params() with plan_params' certify and dynamics); a BRAKED stop replaces the
+        trajectory (action NAV_BRAKED, flown as CERTIFIED), on NONE the remaining trajectory is kept. A vehicle whose stop runs out away
+        from its goal is held instead of STOPPED: active, at rest at its simulator position, not flown, sensed at its state and replanned
+        every round from (position, 0, 0); a round it stays held is NAV_HELD (its replan still counts as failed). Held vehicles that never
+        get a plan end as TIMEOUT.
         Vehicles share the map, so one vehicle's run depends on what the others sensed; with B = 1 it is that vehicle's alone. The world
         waits while the planner runs (no planning latency in simulated time). Within a round only per-vehicle values (stages, verdicts,
         counts, piece totals, positions of heads) cross to the host; points, pieces and logs stay on the device.
         Returns a dict: status, rounds_flown, replans, failed_replans, uncertified_rounds (B,) numpy; actions and verdicts (rounds run, B)
         (NAV_IDLE / NAV_KEPT / NAV_REPLANNED / NAV_REPLAN_FAILED; the verdict of the trajectory flown, NAV_NO_TRAJECTORY without one);
         replan_stages and replan_verdicts (rounds run, B): a replan's plan stage and certificate verdict (NAV_NO_TRAJECTORY: no plan call);
-        logs: per round (vehicle indices (R,) numpy, log (R, n_log, 21) CUDA tensor); times: per round {stage: ms} from CUDA events."""
+        logs: per round (vehicle indices (R,) numpy, log (R, n_log, 21) CUDA tensor); times: per round {stage: ms} from CUDA events (a
+        "brake" stage with fallback="brake"); with fallback="brake" also brakes and held_rounds (B,) numpy: BRAKED stops taken and rounds
+        spent held."""
         import torch
         dev = torch.device("cuda", self.device)
         s = torch.cuda.current_stream(dev) if stream is None else stream
@@ -1688,6 +1788,10 @@ class Evaluator:
         p = plan_params if plan_params is not None else self.plan_params()
         if not p.flags & PLAN_CERTIFY:
             raise ValueError("navigate checks trajectories with the certificate: plan_params needs PLAN_CERTIFY")
+        if fallback not in ("keep", "brake"):
+            raise ValueError(f"fallback must be 'keep' or 'brake', got {fallback!r}")
+        brake = fallback == "brake"
+        bp = brake_params if brake_params is not None else self.brake_params(certify=p.certify, dynamics=p.dynamics)
         sp = SimParams.from_buffer_copy(bytes(sim_params if sim_params is not None else sim_default_params()))
         sp.t_end = float(horizon)
         cam = sense_params if sense_params is not None else globals()["sense_params"]()
@@ -1706,10 +1810,11 @@ class Evaluator:
             T, Cc = torch.zeros(1, **f64), torch.zeros(18, **f64)
         n = np.zeros(B, dtype=np.int64)                                    # their piece counts (host)
         status = np.full(B, NAV_ACTIVE)
-        flown_rounds, replans, failed, uncert = (np.zeros(B, dtype=np.int64) for _ in range(4))
+        flown_rounds, replans, failed, uncert, brakes, held_rounds = (np.zeros(B, dtype=np.int64) for _ in range(6))
+        held, braking = np.zeros(B, dtype=bool), np.zeros(B, dtype=bool)   # held at rest; flying a stop
         actions, verdicts, replan_stages, replan_verdicts, logs, times = [], [], [], [], [], []
         last = None   # (vehicle indices, log) of the last round flown
-        stages = ("sense", "fuse", "check", "replan", "fly", "advance")
+        stages = ("sense", "fuse", "check", "replan", "brake", "fly", "advance") if brake else ("sense", "fuse", "check", "replan", "fly", "advance")
         for r in range(int(rounds)):
             act = np.nonzero(status == NAV_ACTIVE)[0]
             if act.size == 0:
@@ -1745,7 +1850,7 @@ class Evaluator:
                 offh = np.zeros(B + 1, dtype=np.int64)
                 offh[1:] = np.cumsum(n)
                 have = [b for b in act if n[b] > 0]
-                ver = {}
+                ver, fhit = {}, {}
                 for N in sorted({int(n[b]) for b in have}):
                     grp = [b for b in have if n[b] == N]
                     base = torch.as_tensor(offh[grp], device=dev)
@@ -1756,6 +1861,8 @@ class Evaluator:
                     self.trajectory_certify_device(len(grp) * N, gT.data_ptr(), gC.data_ptr(), cp, summ.data_ptr(), sv)
                     v = summ[:, 40:44].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
                     ver.update(zip(grp, v.tolist()))
+                    if brake:
+                        fhit.update(zip(grp, summ[:, 24:32].contiguous().view(torch.float64).reshape(-1).cpu().numpy().tolist()))
                 ev["check"][1].record(s)
                 # 3. replan the vehicles without a certified remaining trajectory
                 ev["replan"][0].record(s)
@@ -1776,6 +1883,9 @@ class Evaluator:
                     still = [i for i, b in enumerate(need) if n[b] == 0]
                     if still:
                         heads[torch.as_tensor(still, device=dev), :3] = torch.as_tensor(st0[[need[i] for i in still]], **f64)
+                        hs = [i for i in still if held[need[i]]]
+                        if hs:   # a held vehicle replans from rest at its simulator position
+                            heads[torch.as_tensor(hs, device=dev), :3] = init[torch.as_tensor([need[i] for i in hs], device=dev), 0:3]
                     hp = heads[:, :3].cpu().numpy()
                     inside = np.all((hp >= lo) & (hp <= hi), axis=1)
                     ok = [i for i in range(len(need)) if inside[i]]
@@ -1794,9 +1904,13 @@ class Evaluator:
                         replans[b] += 1
                         if b in new:
                             action[b], verdict[b] = NAV_REPLANNED, CERTIFIED
+                            held[b] = braking[b] = False
                         else:
                             action[b] = NAV_REPLAN_FAILED
                             failed[b] += 1
+                            if held[b]:
+                                action[b] = NAV_HELD
+                                held_rounds[b] += 1
                     # the trajectories flown this round: the accepted plans, else the remaining ones
                     if new:
                         po = pl["piece_off"].cpu().numpy()
@@ -1819,6 +1933,40 @@ class Evaluator:
                     if action[b] == NAV_IDLE:
                         action[b] = NAV_KEPT
                 ev["replan"][1].record(s)
+                if brake:
+                    # the fallback: a certified stop along the remaining trajectory of every vehicle whose replan failed
+                    ev["brake"][0].record(s)
+                    bv = [b for b in need if b not in new and n[b] > 0]
+                    if bv:
+                        bo = np.zeros(len(bv) + 1, dtype=np.int64)
+                        bo[1:] = np.cumsum(n[bv])
+                        bT = torch.cat([T[offh[b]:offh[b + 1]] for b in bv]).contiguous()
+                        bC = torch.cat([Cc[18 * offh[b]:18 * offh[b + 1]] for b in bv]).contiguous()
+                        ts = torch.as_tensor([fhit[b] if ver[b] == COLLIDING else np.inf for b in bv], **f64)
+                        bk = self.trajectory_brake_device(torch.as_tensor(bo.astype(np.int32), device=dev), bT, bC, ts, params=bp, stream=s)
+                        bst = bk["summary"][:, 0:4].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
+                        got = {b: j for j, b in enumerate(bv) if bst[j] == BRAKED}
+                        if got:
+                            ko = bk["piece_off"].cpu().numpy()
+                            nn = n.copy()
+                            partsT, partsC = [], []
+                            for b in range(B):
+                                if b in got:
+                                    j = got[b]
+                                    a, e = int(ko[j]), int(ko[j + 1])
+                                    partsT.append(bk["T"][a:e]); partsC.append(bk["coeffs"][18 * a:18 * e])
+                                    nn[b] = e - a
+                                    action[b], verdict[b] = NAV_BRAKED, CERTIFIED
+                                    brakes[b] += 1
+                                    braking[b] = True
+                                elif n[b] > 0:
+                                    partsT.append(T[offh[b]:offh[b + 1]]); partsC.append(Cc[18 * offh[b]:18 * offh[b + 1]])
+                            n = nn
+                            T, Cc = torch.cat(partsT).contiguous(), torch.cat(partsC).contiguous()
+                            offh = np.zeros(B + 1, dtype=np.int64)
+                            offh[1:] = np.cumsum(n)
+                            off = torch.as_tensor(offh.astype(np.int32), device=dev)
+                    ev["brake"][1].record(s)
                 # 4. fly the vehicles that have a trajectory
                 ev["fly"][0].record(s)
                 fly = np.array([b for b in act if n[b] > 0], dtype=np.int64)
@@ -1847,6 +1995,11 @@ class Evaluator:
                             uncert[b] += 1
                         if diverged[k]:
                             status[b] = NAV_DIVERGED
+                        elif n[b] == 0 and braking[b] and dist[k] > tol:
+                            held[b], braking[b] = True, False   # the stop ran out: held at rest where the simulator left it
+                            init[b, 3:] = 0.0
+                            init[b, 6] = 1.0
+                            init[b, 13:17] = float(np.sqrt(sp.mass * sp.grav / (4 * sp.kf)))
                         elif n[b] == 0:
                             status[b] = NAV_ARRIVED if dist[k] <= tol else NAV_STOPPED
                     done = status != NAV_ACTIVE
@@ -1868,10 +2021,13 @@ class Evaluator:
             if last is not None:
                 logs.append(last)
         status[status == NAV_ACTIVE] = NAV_TIMEOUT
-        return dict(status=status, rounds_flown=flown_rounds, replans=replans, failed_replans=failed, uncertified_rounds=uncert,
-                    actions=np.array(actions).reshape(-1, B), verdicts=np.array(verdicts).reshape(-1, B),
-                    replan_stages=np.array(replan_stages).reshape(-1, B), replan_verdicts=np.array(replan_verdicts).reshape(-1, B), logs=logs,
-                    times=times)
+        out = dict(status=status, rounds_flown=flown_rounds, replans=replans, failed_replans=failed, uncertified_rounds=uncert,
+                   actions=np.array(actions).reshape(-1, B), verdicts=np.array(verdicts).reshape(-1, B),
+                   replan_stages=np.array(replan_stages).reshape(-1, B), replan_verdicts=np.array(replan_verdicts).reshape(-1, B), logs=logs,
+                   times=times)
+        if brake:
+            out.update(brakes=brakes, held_rounds=held_rounds)
+        return out
 
     def plan_info(self):
         info = PlanInfo()

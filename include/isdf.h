@@ -1082,6 +1082,61 @@ int isdf_trajectory_shift(isdf_ctx *ctx, int B, const int32_t *piece_off, const 
                           int32_t *out_piece_off, double *out_T, double *out_coeffs);
 int isdf_trajectory_shift_device(isdf_ctx *ctx, int B, const int32_t *d_piece_off, const double *d_T, const double *d_coeffs,
                                  const double *d_t0, int32_t *d_out_piece_off, double *d_out_T, double *d_out_coeffs, void *cuda_stream);
+/* ---- braking to a certified stop along the remaining trajectory (DESIGN §3.21) -------------------------------------------------------
+ * B remaining trajectories in isdf_plan_batch's ragged layout (each starting at the vehicle's current time 0) and t_stop_max[b], the latest
+ * trajectory time whose position the stop may reach (e.g. a COLLIDING certificate's first_hit). Per trajectory b, in FP64 with nothing
+ * contracted, in this order:
+ *   D       = T[0] + T[1] + ... (left to right, from 0.0);
+ *   tau_max = t_stop_max[b] if t_stop_max[b] < D, else D; NO_INPUT (0 pieces) for a trajectory without pieces, a NaN t_stop_max[b], or
+ *             a tau_max that is not finite and > 0;
+ *   candidate k = 0 .. K-1: tau_k = tau_max * ((double)(k + 1) / (double)K), an M-piece MINCO S3 trajectory (isdf_midend_batch's solve,
+ *             bit-identical to the host MincoS3) with
+ *             head      (x, v, a) of the trajectory at time 0,
+ *             tail      (x(tau_k), 0, 0),
+ *             durations M equal ones, (tau_k + tau_k) / (double)M,
+ *             waypoints x(tau_k * f_j), j = 1 .. M-1, f_j = 1.0 - u_j * u_j, u_j = (double)(M - j) / (double)M.
+ *   Positions, velocities and accelerations are isdf_trajectory_states' (locatePieceIdx's rule, then getPos / getVel / getAcc).
+ *   This is the constant-deceleration schedule: the remaining path's first tau_k of time is covered in 2 tau_k, at rest at x(tau_k).
+ * All B K candidates (uniform, N0 = M) go through isdf_trajectory_certify and isdf_trajectory_dynamics in one pass each (p->certify and
+ * p->dynamics with pieces_per_traj set to M; a NO_INPUT trajectory's candidates are at rest at a placeholder and never chosen). The chosen
+ * candidate is the largest k that is CERTIFIED and FEASIBLE, the gentlest stop that is proven clear: status BRAKED, its M pieces written
+ * at out_piece_off[b]; else status NONE and 0 pieces. out_piece_off (B + 1), out_T and out_coeffs need room for B M pieces.
+ * Summary per trajectory: status, candidate (-1 without one), tau_stop and duration (the left-to-right sum of the output T; NaN without a
+ * candidate), certified / feasible (how many of the K candidates passed each check; 0 for NO_INPUT), and the chosen candidate's certificate
+ * summaries, bit-identical to isdf_trajectory_certify / isdf_trajectory_dynamics of the output with N0 = M (their failed-call summaries
+ * without a candidate).
+ * A trajectory's result is bit-identical alone or inside a batch; host and device forms give identical bits. The host form stages through
+ * the context (one copy each way) and checks its inputs as isdf_trajectory_states' host form does; the device form checks no device data
+ * and runs on cuda_stream; only the certificates' 4-byte round reads cross to the host, and the call returns when its outputs are written.
+ * The call counts its launches in isdf_stats.kernel_launches; it leaves the discrete schedule, the swept-volume state, the mid-end buffers
+ * and the batch trajectories as they were (its MINCO buffers are its own).
+ * Errors: ISDF_ERR_INVALID for a NULL pointer, B < 1, K < 1, M outside [1, ISDF_BRAKE_MAX_PIECES], B K M beyond 31 bits, a non-zero
+ *   pieces_per_traj in p->certify or p->dynamics or reserved_, and the certificates' own parameter errors; ISDF_ERR_STATE without a map
+ *   or a shape; ISDF_ERR_UNSUPPORTED for a shape the certificate refuses and on a sharded context. On failure every summary reads status
+ *   NONE, candidate -1, NaN times, counts -1 and both certificates' failed-call summaries; the outputs are otherwise left as they were. */
+#define ISDF_BRAKE_MAX_PIECES 64
+typedef enum isdf_brake_status { ISDF_BRAKE_NO_INPUT = -1, ISDF_BRAKE_NONE = 0, ISDF_BRAKE_BRAKED = 1 } isdf_brake_status;
+typedef struct isdf_brake_params {
+    int32_t candidates;             /* K >= 1, default 8 */
+    int32_t pieces;                 /* M in [1, ISDF_BRAKE_MAX_PIECES], default 4 */
+    isdf_certify_params certify;    /* isdf_certify_default_params; pieces_per_traj must be 0 (the call sets M) */
+    isdf_dynamics_params dynamics;  /* isdf_dynamics_default_params(ctx); likewise */
+    int32_t reserved_[2];           /* must be 0 */
+} isdf_brake_params;
+typedef struct isdf_brake_summary {
+    int32_t status;                 /* isdf_brake_status */
+    int32_t candidate;              /* k of the chosen candidate, -1 without one */
+    double tau_stop, duration;      /* tau_k and the stop's duration; NaN without a candidate */
+    int32_t certified, feasible;    /* candidates CERTIFIED / FEASIBLE */
+    isdf_certify_summary certify;   /* the chosen candidate's */
+    isdf_dynamics_summary dynamics;
+} isdf_brake_summary;
+int isdf_brake_default_params(isdf_ctx *ctx, isdf_brake_params *p);
+int isdf_trajectory_brake(isdf_ctx *ctx, int B, const int32_t *piece_off, const double *T, const double *coeffs, const double *t_stop_max,
+                          const isdf_brake_params *p, int32_t *out_piece_off, double *out_T, double *out_coeffs, isdf_brake_summary *summary);
+int isdf_trajectory_brake_device(isdf_ctx *ctx, int B, const int32_t *d_piece_off, const double *d_T, const double *d_coeffs,
+                                 const double *d_t_stop_max, const isdf_brake_params *p, int32_t *d_out_piece_off, double *d_out_T,
+                                 double *d_out_coeffs, isdf_brake_summary *d_summary, void *cuda_stream);
 /* the robot's body at Q states: out[(q * P + p) * 3 + k] = (R(quat_q) body_p + pos_q)_k, R = quat_rot (Eigen's toRotationMatrix,
  * Shape.hpp:753-757), each row ((R_k0 b0 + R_k1 b1) + R_k2 b2) + pos_k rounded per operation (Shape::Transform, Shape.hpp:786-793).
  * states: Q x 20, isdf_trajectory_states records (only pos and quat are read); body: P x 3 body-frame points (mesh vertices, interior
