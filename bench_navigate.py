@@ -3,6 +3,7 @@
 (Evaluator.navigate: sense -> fuse -> check -> replan -> fly -> advance, every stage batched over vehicles); prints one JSON line.
 
   python bench_navigate.py [--vehicles 1,16,64] [--rounds R] [--horizon H] [--sense-every S] [--seed N] [--fallback keep|brake]
+                           [--unknown free|occupied] [--cameras 1|4]
 
 World: mockamap's box world (isdf_world_cloud_device, ISDF_WORLD_BOXES) with seed 511, 40 x 40 x 10 m at 0.5 m (size 80 x 80 x 20,
 scale 2), 20 boxes 1.5 to 3 m wide: x and y in [-20, 20] m, z in [0, 10] m. The vehicles' map starts as an empty 1 m frame over that box
@@ -14,7 +15,11 @@ map at least 2 voxels from any occupied one. The true map (the whole world fused
 flown pose with pose_clearance_device.
 Per B: per-stage milliseconds per round (mean over the rounds run, CUDA events), rounds run, arrivals, failed replans, and the minimum true
 clearance over every flown pose. --fallback brake (navigate's fallback, DESIGN §3.21) adds the stops taken and the rounds held; the
-default, keep, prints what it always printed. Writes nothing to the tree.
+default, keep, prints what it always printed. --unknown occupied (navigate's unknown policy, DESIGN §3.22; needs --fallback brake) seeds
+the known space with the 5 x 5 x 5-voxel block around each start (free in the true map by pairs()) and adds the commits taken; --cameras 4
+flies a rig of four cameras, cam_to_body = Rz(k 90 deg) cam02body. Either option (also --unknown free) also reports the pose of the minimum true clearance: its
+vehicle, round and witness voxel, and whether that voxel is occupied in the vehicles' fused map at the end of the run. Writes nothing to the
+tree.
 """
 import argparse
 import json
@@ -54,10 +59,11 @@ def pairs(occ, B, seed):
     return st[rng.choice(len(st), B, replace=len(st) < B)], gl[rng.choice(len(gl), B, replace=len(gl) < B)]
 
 
-def min_clearance(truth, logs):
+def min_clearance(truth, logs, where=None):
+    """the minimum true clearance over every flown pose; where (a dict) receives the log index, vehicle and witness voxel of that pose"""
     import torch
     m = float("inf")
-    for _, lg in logs:
+    for k, (vi, lg) in enumerate(logs):
         rec = lg.reshape(-1, lg.shape[-1]).contiguous()
         Q = rec.shape[0]
         clear = torch.empty(Q, dtype=torch.float64, device=rec.device)
@@ -66,8 +72,22 @@ def min_clearance(truth, logs):
         base = rec.data_ptr()
         truth.pose_clearance_device(Q, base + 8, base + 56, lg.shape[-1], truth.pose_clearance_params(), clear.data_ptr(), vox.data_ptr(),
                                     summ.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        j = int(torch.argmin(clear))
+        if float(clear[j]) < m and where is not None:
+            where.update(log=k, vehicle=int(vi[j // lg.shape[1]]), voxel=int(vox[j]))
         m = min(m, float(clear.min()))
     return m
+
+
+def rig(k):
+    """k = 1: the reference camera; k = 4: four cameras at yaw 0, 90, 180, 270 deg (cam_to_body = Rz cam02body, exact in FP64)"""
+    import isdf_b200 as I
+    c0 = np.array([[0, 0, 1, 0], [-1, 0, 0, 0], [0, -1, 0, 0], [0, 0, 0, 1]], dtype=np.float64)
+    cams = []
+    for c, s in [(1, 0), (0, 1), (-1, 0), (0, -1)][:k]:
+        Rz = np.array([[c, -s, 0, 0], [s, c, 0, 0], [0, 0, 1, 0], [0, 0, 0, 1]], dtype=np.float64)
+        cams.append(I.sense_params(sensing_horizon=15.0, cam_to_body=(Rz @ c0).reshape(-1)))
+    return cams[0] if k == 1 else cams
 
 
 def main():
@@ -78,7 +98,11 @@ def main():
     ap.add_argument("--sense-every", type=int, default=25)
     ap.add_argument("--seed", type=int, default=7)
     ap.add_argument("--fallback", choices=("keep", "brake"), default="keep")
+    ap.add_argument("--unknown", choices=("free", "occupied"), default=None)
+    ap.add_argument("--cameras", type=int, choices=(1, 4), default=1)
     args = ap.parse_args()
+    if args.unknown == "occupied" and args.fallback != "brake":
+        raise SystemExit("--unknown occupied needs --fallback brake")
     import torch
     import isdf_b200 as I
     if not torch.cuda.is_available():
@@ -98,6 +122,9 @@ def main():
     brake = args.fallback == "brake"
     if brake:
         out["fallback"] = "brake"
+    trace = args.unknown is not None or args.cameras != 1
+    if trace:
+        out.update(unknown=args.unknown or "free", cameras=args.cameras)
     for B in [int(v) for v in args.vehicles.split(",")]:
         starts, goals = pairs(occ, B, args.seed + B)
         ev = I.Evaluator(cfg)
@@ -105,9 +132,10 @@ def main():
         ev.frontend_build_kernels(45.0, 45.0, 9.0, 0.0)
         ev.set_map_u8(np.zeros(DIMS, np.uint8), BMIN, RES)
         ev.set_sense_cloud_device(scene, stream=torch.cuda.current_stream().cuda_stream)
+        kw = dict(unknown="occupied", known_boxes=np.concatenate([starts - 2.5, starts + 2.5], 1)) if args.unknown == "occupied" else {}
         r = ev.navigate(starts, goals, rounds=args.rounds, horizon=args.horizon, sense_every=args.sense_every, tol=1.0,
                         plan_params=ev.plan_params(flags=I.PLAN_CERTIFY, backend_max_iterations=200),
-                        sense_params=I.sense_params(sensing_horizon=15.0), fallback=args.fallback)
+                        sense_params=rig(args.cameras), fallback=args.fallback, **kw)
         fail = np.isin(r["actions"], [I.NAV_REPLAN_FAILED, I.NAV_BRAKED, I.NAV_HELD]) if brake else r["actions"] == I.NAV_REPLAN_FAILED
         why = {}   # failed replans by (plan stage, certificate verdict); -2: no plan call (a head outside the frame)
         for st, v in zip(r["replan_stages"][fail], r["replan_verdicts"][fail]):
@@ -119,9 +147,17 @@ def main():
                                 diverged=int((r["status"] == I.NAV_DIVERGED).sum()), timeout=int((r["status"] == I.NAV_TIMEOUT).sum()),
                                 replans=int(r["replans"].sum()), failed_replans=int(r["failed_replans"].sum()), failed_by_stage_verdict=why,
                                 uncertified_rounds=int(r["uncertified_rounds"].sum()), map_voxels=int(ev.map_info()["occupied_voxels"]),
-                                min_true_clearance=round(min_clearance(truth, r["logs"]), 4)))
+                                min_true_clearance=round(min_clearance(truth, r["logs"], where := {}), 4)))
         if brake:
             out["runs"][-1].update(brakes=int(r["brakes"].sum()), held_rounds=int(r["held_rounds"].sum()))
+        if "commits" in r:
+            out["runs"][-1].update(commits=int(r["commits"].sum()))
+        if trace and where:
+            flown = [k for k in range(len(r["times"])) if (r["verdicts"][k] != I.NAV_NO_TRAJECTORY).any()]
+            v = where["voxel"]
+            fused = bool(ev.get_map_u8().reshape(-1)[v]) if v >= 0 else None
+            out["runs"][-1].update(min_clearance_at=dict(vehicle=where["vehicle"], round=flown[where["log"]], witness_voxel=v,
+                                                         witness_in_fused_map=fused))
         ev.close()
     truth.close()
     print(json.dumps(out))

@@ -173,6 +173,13 @@ struct isdf_ctx {
         DevBuf<uint32_t> d_bits;
         long long points_used = 0, points_skipped = 0;   // isdf_set_map_cloud*; 0 for dense maps
     } map;
+    struct {   // known space (isdf_observe.cuh): the known bits in the map's layout (allocated on first use; have = false: nothing known), the
+               // blocked grid the clearance family reads under ISDF_UNKNOWN_OCCUPIED (rebuilt when a map, fuse, observe or mark call made it stale)
+        bool have = false, blocked_ok = false;
+        int policy = ISDF_UNKNOWN_FREE;
+        DevBuf<uint32_t> d_known, d_blocked;
+        DevGrid blocked = {};
+    } known;
     struct {   // the map's distance field (isdf_esdf.cuh): squared voxel distances, ESDF_NONE where no site exists; given up with the map
         bool have = false;
         DevBuf<uint32_t> d_pos, d_neg;
@@ -888,6 +895,7 @@ static int map_size_check(isdf_ctx *c, long long X, long long Y, long long Z, do
 // gives up the map and the distance field built on it (its memory too: it is 8 bytes per voxel)
 static void drop_map(isdf_ctx *c) {
     c->map.have_map = false;
+    c->known.have = c->known.blocked_ok = false;
     c->esdf.have = false;
     c->esdf.d_pos = {}; c->esdf.d_neg = {};
 }
@@ -1086,6 +1094,7 @@ static int fuse_cloud_impl(isdf_ctx *c, const char *d_pts, long long n, int stri
     }
     c->esdf.have = false;   // the field described the map before this call
     c->esdf.d_pos = {}; c->esdf.d_neg = {};
+    c->known.blocked_ok = false;
     if (info) {
         info->points_used = (int64_t)cnt[FUSE_USED]; info->points_outside = (int64_t)cnt[FUSE_OUTSIDE];
         info->points_skipped = (int64_t)cnt[FUSE_SKIPPED]; info->voxels_added = (int64_t)cnt[FUSE_ADDED];
@@ -1135,13 +1144,16 @@ extern "C" int isdf_get_map_info(isdf_ctx *c, isdf_map_info *out) {
 }
 
 // the bit grid expanded to one T per voxel, a bounded number of (x, y) rows at a time through device scratch
+// (known: the known bits, all 0 when nothing is known)
 template <typename T>
-static int get_map_impl(isdf_ctx *c, T *out, int64_t n) {
+static int get_map_impl(isdf_ctx *c, T *out, int64_t n, bool known = false) {
     if (!c || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
     if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
-    const DevGrid &g = c->map.grid;
+    DevGrid g = c->map.grid;
     const long long rows = (long long)g.X * g.Y;
     if (n != rows * g.Z) return fail(ISDF_ERR_INVALID, "n must be X*Y*Z of the map");
+    if (known && !c->known.have) { std::memset(out, 0, sizeof(T) * (size_t)n); return 0; }
+    if (known) g.bits = c->known.d_known.p;
     if (set_device(c)) return ISDF_ERR_CUDA;
     const long long chunk_rows = std::max<long long>(1, (32ll << 20) / ((long long)g.Z * sizeof(T)));   // <= 32 MiB of scratch per chunk
     DevBuf<T> d_out;
@@ -1160,6 +1172,55 @@ static int get_map_impl(isdf_ctx *c, T *out, int64_t n) {
 
 extern "C" int isdf_get_map_u8(isdf_ctx *c, uint8_t *occ, int64_t n) { return get_map_impl<uint8_t>(c, occ, n); }
 extern "C" int isdf_get_map_f64(isdf_ctx *c, double *grid_map, int64_t n) { return get_map_impl<double>(c, grid_map, n); }
+extern "C" int isdf_get_map_known_u8(isdf_ctx *c, uint8_t *known, int64_t n) { return get_map_impl<uint8_t>(c, known, n, true); }
+
+// ---- known space (isdf_observe.cuh, compiled in isdf_sense_tu.cu) ----
+// the known bits, allocated and cleared on st the first time after a map was set
+static int known_bits(isdf_ctx *c, cudaStream_t st) {
+    if (c->known.have) return 0;
+    const DevGrid &g = c->map.grid;
+    const size_t nwords = (size_t)g.X * g.Y * g.Zw;
+    CU_TRY(c->known.d_known.ensure(nwords));
+    CU_TRY(cudaMemsetAsync(c->known.d_known.p, 0, nwords * sizeof(uint32_t), st));
+    c->known.have = true;
+    return 0;
+}
+
+extern "C" int isdf_set_unknown_policy(isdf_ctx *c, int policy) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (policy != ISDF_UNKNOWN_FREE && policy != ISDF_UNKNOWN_OCCUPIED) return fail(ISDF_ERR_INVALID, "unknown policy (ISDF_UNKNOWN_FREE or ISDF_UNKNOWN_OCCUPIED)");
+    c->known.policy = policy;
+    return 0;
+}
+extern "C" int isdf_get_unknown_policy(isdf_ctx *c, int *policy) {
+    if (!c || !policy) return fail(ISDF_ERR_INVALID, "NULL argument");
+    *policy = c->known.policy;
+    return 0;
+}
+
+extern "C" int isdf_map_mark_known(isdf_ctx *c, int64_t n, const double *boxes) {
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (n < 0 || (n > 0 && !boxes)) return fail(ISDF_ERR_INVALID, "n < 0, or boxes NULL with n > 0");
+    for (int64_t b = 0; b < n; b++)
+        for (int a = 0; a < 3; a++) {
+            const double lo = boxes[6 * b + a], hi = boxes[6 * b + 3 + a];
+            if (!std::isfinite(lo) || !std::isfinite(hi) || !(lo <= hi)) return fail(ISDF_ERR_INVALID, "box " + std::to_string(b) + ": lo and hi must be finite with lo <= hi");
+        }
+    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    if (int r = known_bits(c, c->stream)) return r;
+    int launches = 0;
+    cudaError_t e = cudaSuccess;
+    for (int64_t b = 0; b < n && e == cudaSuccess; b++) e = known_mark_box(c->map.grid, c->known.d_known.p, boxes + 6 * b, boxes + 6 * b + 3, c->stream, &launches);
+    c->stats.kernel_launches += launches;
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    c->known.blocked_ok = false;
+    if (e != cudaSuccess) {
+        drop_map(c);
+        return fail(ISDF_ERR_CUDA, std::string("isdf_map_mark_known: ") + cudaGetErrorString(e));
+    }
+    return 0;
+}
 
 // ---- distance field of the map (GridMap3D::generateESDF3d, getSDFValue, getSDFValueWithGrad; isdf_esdf.cuh) --------------------
 extern "C" int isdf_map_esdf(isdf_ctx *c) {
@@ -1678,6 +1739,63 @@ extern "C" int isdf_sense_cloud_device(isdf_ctx *c, int64_t Q, const double *d_p
                                        const isdf_sense_params *p, int64_t cap, float *d_points, int64_t *d_offsets, void *cuda_stream) {
     return sense_cloud_impl(c, Q, d_pos, d_quat, stride_doubles, p, cap, d_points, d_offsets, true, (cudaStream_t)cuda_stream);
 }
+// ---- known space from depth images (isdf_observe.cuh) ----
+static int observe_impl(isdf_ctx *c, int64_t Q, const double *pos, const double *quat, int64_t stride, const isdf_sense_params *p,
+                        isdf_observe_info *info, bool device, cudaStream_t st) {
+    if (int rc = sense_args_check(c, Q, pos, quat, stride, p, pos)) return rc;
+    if (!std::isfinite(p->sensing_horizon)) return fail(ISDF_ERR_INVALID, "isdf_map_observe needs a finite sensing_horizon");
+    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
+    const double D = std::ceil(2.0 * p->sensing_horizon / c->map.grid.res) + 3.0;
+    if (!(D * D * D <= (double)(1ll << 40))) return fail(ISDF_ERR_INVALID, "sensing_horizon / res too large: a pose's horizon box exceeds 2^40 voxels");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    SenseCall C{Q, pos, quat, stride, *p};
+    Staging S(c);
+    if (!device) {
+        const double *d_pose;
+        stage_poses(S, Q, pos, quat, stride, &d_pose);
+        if (int rc = S.upload()) return rc;
+        C.pos = d_pose; C.quat = d_pose + 3; C.stride = 7;
+        st = c->stream;
+    }
+    if (int r = known_bits(c, st)) return r;
+    int launches = 0;
+    unsigned long long cnt[2] = {0, 0};
+    const cudaError_t e = sense_observe_run(c->sense, C, c->map.grid, c->known.d_known.p, cnt, st, &launches);
+    c->stats.kernel_launches += launches;
+    c->known.blocked_ok = false;
+    if (e != cudaSuccess) {
+        drop_map(c);
+        return fail(ISDF_ERR_CUDA, std::string("isdf_map_observe: ") + cudaGetErrorString(e));
+    }
+    if (info) { info->poses = Q; info->voxels_tested = (int64_t)cnt[0]; info->voxels_added = (int64_t)cnt[1]; }
+    return 0;
+}
+extern "C" int isdf_map_observe(isdf_ctx *c, int64_t Q, const double *pos, const double *quat, int64_t stride_doubles, const isdf_sense_params *p,
+                                isdf_observe_info *info) {
+    return observe_impl(c, Q, pos, quat, stride_doubles, p, info, false, nullptr);
+}
+extern "C" int isdf_map_observe_device(isdf_ctx *c, int64_t Q, const double *d_pos, const double *d_quat, int64_t stride_doubles,
+                                       const isdf_sense_params *p, isdf_observe_info *info, void *cuda_stream) {
+    return observe_impl(c, Q, d_pos, d_quat, stride_doubles, p, info, true, (cudaStream_t)cuda_stream);
+}
+
+// the grid the clearance family reads: the occupancy grid, or under ISDF_UNKNOWN_OCCUPIED the blocked grid, rebuilt on st (and waited for,
+// so that a later call on another stream reads it whole) when stale
+static int clearance_grid_ready(isdf_ctx *c, cudaStream_t st) {
+    if (c->known.policy != ISDF_UNKNOWN_OCCUPIED || c->known.blocked_ok || !c->map.have_map) return 0;
+    const DevGrid &g = c->map.grid;
+    CU_TRY(c->known.d_blocked.ensure((size_t)g.X * g.Y * g.Zw));
+    int launches = 0;
+    const cudaError_t e = blocked_build(g, c->known.have ? c->known.d_known.p : nullptr, c->known.d_blocked.p, st, &launches);
+    c->stats.kernel_launches += launches;
+    CU_TRY(e);
+    CU_TRY(cudaStreamSynchronize(st));
+    c->known.blocked = g;
+    c->known.blocked.bits = c->known.d_blocked.p;
+    c->known.blocked_ok = true;
+    return 0;
+}
+
 // ---- world generators (isdf_world.cuh, compiled in isdf_world_tu.cu) ----
 extern "C" int isdf_world_default_params(int kind, isdf_world_params *p) {
     if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
@@ -2859,10 +2977,11 @@ static int clearance_check(isdf_ctx *c, int N, const isdf_clearance_params *p) {
 
 // the clearance scan of N sources in groups of N0 (0: one group) with reach and margin: the K + 1 uniform samples of each piece of
 // (d_T, d_C), or, with K = 0, poses the caller sets; outputs, cursor, counters, hit flags and sample list are the caller's
+// (clearance_grid_ready has run on the call's stream)
 static ClrArgs clearance_args(const isdf_ctx *c, int N, int K, int N0, double reach, double margin, const double *d_T = nullptr,
                               const double *d_C = nullptr) {
     ClrArgs A = {};
-    A.grid = c->map.grid; A.shape = c->mesh.shape; A.fp = c->dcfg.fp; A.half_bd = c->dcfg.half_bd;
+    A.grid = c->known.policy == ISDF_UNKNOWN_OCCUPIED ? c->known.blocked : c->map.grid; A.shape = c->mesh.shape; A.fp = c->dcfg.fp; A.half_bd = c->dcfg.half_bd;
     A.reach = reach; A.margin = margin;
     A.N = N; A.K = K; A.N0 = N0 == 0 ? N : N0;
     A.T = d_T; A.C = d_C;
@@ -2918,6 +3037,7 @@ extern "C" int isdf_trajectory_clearance_device(isdf_ctx *c, int N, const double
         if (int r = clearance_check(c, N, p)) return r;
         if (!d_T || !d_coeffs || !d_sample_clearance || !d_sample_voxel || !d_summary) return fail(ISDF_ERR_INVALID, "NULL device pointer");
         if (set_device(c)) return ISDF_ERR_CUDA;
+        if (int r = clearance_grid_ready(c, st)) return r;
         // no sample list, no hit flags: the uniform samples of the definition
         ClrArgs A = clearance_args(c, N, p->samples_per_piece, p->pieces_per_traj, p->reach, p->margin, d_T, d_coeffs);
         A.clear = d_sample_clearance; A.voxel = (long long *)d_sample_voxel; A.summary = (ClrSummary *)d_summary;
@@ -2973,6 +3093,7 @@ extern "C" int isdf_pose_clearance_device(isdf_ctx *c, int64_t Q, const double *
         if (int r = pose_clearance_check(c, Q, d_pos, d_quat, stride, p)) return r;
         if (!d_clear || !d_voxel || !d_summary) return fail(ISDF_ERR_INVALID, "NULL device pointer");
         if (set_device(c)) return ISDF_ERR_CUDA;
+        if (int r = clearance_grid_ready(c, st)) return r;
         ClrArgs A = clearance_args(c, (int)Q, 0, p->poses_per_group, p->reach, p->margin);   // one "sample" per pose
         A.ppos = d_pos; A.pquat = d_quat; A.pstride = stride;
         A.clear = d_clear; A.voxel = (long long *)d_voxel; A.summary = (ClrSummary *)d_summary;
@@ -3139,6 +3260,7 @@ static int certify_run(isdf_ctx *c, int N, const double *d_T, const double *d_C,
     CU_TRY(certify_init_launch(A, st));
     c->stats.kernel_launches++;
     // the scan: round 0 is the clearance check's own uniform samples, later rounds the new midpoints
+    if (int rr = clearance_grid_ready(c, st)) return rr;
     ClrArgs S = clearance_args(c, N, K, q.pieces_per_traj, q.reach, q.margin, d_T, d_C);   // no counters: a certificate leaves isdf_dbg_clearance_counts as it was
     S.clear = z.d_sc.p; S.voxel = z.d_sv.p; S.cursor = z.d_cursor.p; S.hit = z.d_hit.p;
     auto scan = [&](long long n) -> int {

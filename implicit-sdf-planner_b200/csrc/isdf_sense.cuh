@@ -38,11 +38,12 @@ struct SenseScene {
     // per-call scratch: poses, work list, images, flags and their scan
     DevBuf<SensePose> d_pose; DevBuf<uint2> d_work; DevBuf<unsigned long long> d_nwork; DevBuf<int32_t> d_img, d_flag;
     DevBuf<long long> d_base; DevBuf<char> d_tmp;
+    DevBuf<int32_t> d_mip; DevBuf<unsigned long long> d_obs_cnt;   // isdf_map_observe: the chunk's min-mips, its counts
     int chunk_override = 0;   // poses per chunk (isdf_dbg_sense_chunk; 0: automatic)
     // give up the cloud and the scratch sized for it
     void release() {
         have = false; n = skipped = nb = 0;
-        d_pts = {}; d_box = {}; d_work = {}; d_img = {}; d_flag = {}; d_tmp = {};
+        d_pts = {}; d_box = {}; d_work = {}; d_img = {}; d_flag = {}; d_tmp = {}; d_mip = {};
     }
 };
 
@@ -62,5 +63,15 @@ cudaError_t sense_set_cloud(SenseScene &S, const char *d_rec, long long n, int s
 cudaError_t sense_depth_run(SenseScene &S, const SenseCall &C, int32_t *out, cudaMemcpyKind kind, cudaStream_t st, int *launches);
 // sensed points: d_points (cap x 3 floats, device, may be NULL when cap = 0) and d_off (Q + 1 int64, device), on st
 cudaError_t sense_cloud_run(SenseScene &S, const SenseCall &C, float *d_points, long long cap, int64_t *d_off, cudaStream_t st, int *launches);
+
+// ---- known space (isdf_observe.cuh, compiled in the same unit) ----
+// marks known, in the grid G's layout at known, the voxels the images of the call's poses prove empty; cnt[0..1] = {voxels tested, voxels
+// added} (host), on st, which this synchronises
+cudaError_t sense_observe_run(SenseScene &S, const SenseCall &C, const DevGrid &G, uint32_t *known, unsigned long long cnt[2], cudaStream_t st,
+                              int *launches);
+// marks known the voxels whose padded cube lies inside the closed box lo, hi (host), on st
+cudaError_t known_mark_box(const DevGrid &G, uint32_t *known, const double lo[3], const double hi[3], cudaStream_t st, int *launches);
+// out = G.bits | (~known & valid bits), known NULL meaning nothing known, on st
+cudaError_t blocked_build(const DevGrid &G, const uint32_t *known, uint32_t *out, cudaStream_t st, int *launches);
 
 }  // namespace isdf

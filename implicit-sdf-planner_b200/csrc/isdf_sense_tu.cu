@@ -2,6 +2,7 @@
 // Compiled with -fmad=false, so the FP64 pose and back-projection arithmetic rounds operation by operation as the reference's g++ build;
 // the render's FP32 arithmetic is spelled with intrinsics, so its contraction is the reference CUDA build's whatever the unit's setting.
 #include "isdf_sense.cuh"
+#include "isdf_observe.cuh"
 #include "isdf_math.cuh"
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -399,6 +400,69 @@ cudaError_t sense_cloud_run(SenseScene &S, const SenseCall &C, float *d_points, 
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
     return cudaSuccess;
+}
+
+cudaError_t sense_observe_run(SenseScene &S, const SenseCall &C, const DevGrid &G, uint32_t *known, unsigned long long cnt[2], cudaStream_t st,
+                              int *launches) {
+    const int P = chunk_poses(S, C);
+    cudaError_t e = ensure_scratch(S, C, P);
+    if (e != cudaSuccess) return e;
+    ObsArgs A = {};
+    A.w[0] = C.p.width; A.h[0] = C.p.height;
+    long long per_image = 0;   // mip cells of one image, levels >= 1
+    for (A.nlev = 1; A.w[A.nlev - 1] > 1 || A.h[A.nlev - 1] > 1; A.nlev++) {
+        A.w[A.nlev] = (A.w[A.nlev - 1] + 1) / 2; A.h[A.nlev] = (A.h[A.nlev - 1] + 1) / 2;
+        per_image += (long long)A.w[A.nlev] * A.h[A.nlev];
+    }
+    if ((e = S.d_mip.ensure((size_t)std::max(1ll, (long long)P * per_image))) != cudaSuccess) return e;
+    if ((e = S.d_obs_cnt.ensure(2)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(S.d_obs_cnt.p, 0, 2 * sizeof(unsigned long long), st)) != cudaSuccess) return e;
+    for (int a = 0; a < 3; a++) A.bmin[a] = G.bmin[a];
+    A.res = G.res; A.X = G.X; A.Y = G.Y; A.Z = G.Z; A.Zw = G.Zw;
+    A.D = (int)std::ceil(2.0 * C.p.sensing_horizon / G.res) + 3;
+    A.horizon = C.p.sensing_horizon;
+    A.fx = (float)C.p.fx; A.fy = (float)C.p.fy; A.cx = (float)C.p.cx; A.cy = (float)C.p.cy;
+    A.known = known; A.cnt = S.d_obs_cnt.p; A.poses = S.d_pose.p; A.img = S.d_img.p; A.mip = S.d_mip.p;
+    for (long long q0 = 0; q0 < C.Q; q0 += P) {
+        const int np = (int)std::min<long long>(P, C.Q - q0);
+        if ((e = render_chunk(S, C, q0, np, false, st, launches)) != cudaSuccess) return e;
+        long long off = 0;
+        for (int l = 1; l < A.nlev; l++) {
+            A.off[l] = off;
+            const int32_t *src = l == 1 ? S.d_img.p : S.d_mip.p + A.off[l - 1];
+            k_obs_mip<<<grid_for((long long)np * A.w[l] * A.h[l]), 256, 0, st>>>(src, A.w[l - 1], A.h[l - 1], S.d_mip.p + off, A.w[l], A.h[l], np);
+            off += (long long)np * A.w[l] * A.h[l];
+        }
+        A.P = np;
+        const long long n = (long long)np * A.D * A.D * A.D;
+        k_obs_voxels<<<(unsigned)std::min<long long>((n + 255) / 256, 132ll * 32), 256, 0, st>>>(A);
+        *launches += A.nlev;
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    }
+    if ((e = cudaMemcpyAsync(cnt, S.d_obs_cnt.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st)) != cudaSuccess) return e;
+    return cudaStreamSynchronize(st);
+}
+
+cudaError_t known_mark_box(const DevGrid &G, uint32_t *known, const double lo[3], const double hi[3], cudaStream_t st, int *launches) {
+    const int dims[3] = {G.X, G.Y, G.Z};
+    int i0[3], n[3];
+    for (int a = 0; a < 3; a++) {   // a loose index range (one voxel of slack each side); the kernel tests each cube exactly
+        const double f0 = std::floor((lo[a] - G.bmin[a]) / G.res) - 1.0, f1 = std::floor((hi[a] - G.bmin[a]) / G.res) + 1.0;
+        const double c0 = std::max(0.0, f0), c1 = std::min((double)dims[a] - 1.0, f1);
+        if (!(c0 <= c1)) return cudaSuccess;   // the box misses the map
+        i0[a] = (int)c0; n[a] = (int)(c1 - c0) + 1;
+    }
+    const long long cnt = (long long)n[0] * n[1] * n[2];
+    k_known_boxes<<<grid_for(cnt), 256, 0, st>>>(G, known, lo[0], lo[1], lo[2], hi[0], hi[1], hi[2], i0[0], i0[1], i0[2], n[0], n[1], n[2]);
+    (*launches)++;
+    return cudaGetLastError();
+}
+
+cudaError_t blocked_build(const DevGrid &G, const uint32_t *known, uint32_t *out, cudaStream_t st, int *launches) {
+    const long long nwords = (long long)G.X * G.Y * G.Zw;
+    k_blocked<<<grid_for(nwords), 256, 0, st>>>(G.bits, known, out, nwords, G.Z, G.Zw);
+    (*launches)++;
+    return cudaGetLastError();
 }
 
 }  // namespace isdf

@@ -53,7 +53,8 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_world_default_params", "isdf_world_cloud", "isdf_world_cloud_device",
                "isdf_map_fuse_cloud", "isdf_map_fuse_cloud_device", "isdf_plan_states", "isdf_plan_states_device",
                "isdf_trajectory_shift", "isdf_trajectory_shift_device", "isdf_brake_default_params", "isdf_trajectory_brake",
-               "isdf_trajectory_brake_device"]
+               "isdf_trajectory_brake_device", "isdf_map_observe", "isdf_map_observe_device", "isdf_map_mark_known",
+               "isdf_get_map_known_u8", "isdf_set_unknown_policy", "isdf_get_unknown_policy"]
 WORLD_KINDS = dict(globalmap=1, perlin=2, boxes=3)   # isdf_world_kind
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
@@ -67,8 +68,12 @@ NAV_ACTIVE, NAV_ARRIVED, NAV_STOPPED, NAV_DIVERGED, NAV_TIMEOUT = 0, 1, 2, 3, 4 
 NAV_IDLE, NAV_KEPT, NAV_REPLANNED, NAV_REPLAN_FAILED = -1, 0, 1, 2               # Evaluator.navigate: a vehicle's action in a round
 NAV_NO_TRAJECTORY = -2                                                            # Evaluator.navigate: verdict of a round without one
 NAV_BRAKED, NAV_HELD = 3, 4                        # Evaluator.navigate(fallback="brake"): a vehicle's action in a round
+NAV_COMMITTED = 5                                  # Evaluator.navigate(unknown="occupied"): a vehicle's action in a round
+NAV_COMMIT_SLACK = 0.25   # m added to the certificate margin of a commit's stop: the simulator's tracking error must not put the vehicle
+                          # within the margin of unseen space where it stops, or no plan from there could be committed to again
 BRAKE_NO_INPUT, BRAKE_NONE, BRAKED = -1, 0, 1      # isdf_brake_summary.status
 BRAKE_MAX_PIECES = 64                              # ISDF_BRAKE_MAX_PIECES
+UNKNOWN_FREE, UNKNOWN_OCCUPIED = 0, 1              # isdf_unknown_policy
 
 
 class SimParams(C.Structure):
@@ -451,6 +456,14 @@ class FuseInfo(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class ObserveInfo(C.Structure):
+    """isdf_observe_info"""
+    _fields_ = [(n, C.c_int64) for n in ["poses", "voxels_tested", "voxels_added"]]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 class FrontPathParams(C.Structure):
     """isdf_frontpath_params"""
     _fields_ = [("reserved_", C.c_int32 * 4)]
@@ -560,6 +573,10 @@ def load_library(path=None):
     lib.isdf_trajectory_brake.argtypes = [vp, C.c_int, ip, dp, dp, dp, C.POINTER(BrakeParams), ip, dp, dp, C.POINTER(BrakeSummary)]
     lib.isdf_trajectory_brake_device.argtypes = [vp, C.c_int, vp, vp, vp, vp, C.POINTER(BrakeParams), vp, vp, vp, vp, vp]
     lib.isdf_get_map_u8.argtypes = [vp, C.POINTER(C.c_uint8), C.c_int64]
+    lib.isdf_get_map_known_u8.argtypes = [vp, C.POINTER(C.c_uint8), C.c_int64]
+    lib.isdf_map_mark_known.argtypes = [vp, C.c_int64, vp]
+    lib.isdf_set_unknown_policy.argtypes = [vp, C.c_int]
+    lib.isdf_get_unknown_policy.argtypes = [vp, C.POINTER(C.c_int)]
     lib.isdf_get_map_f64.argtypes = [vp, dp, C.c_int64]
     lib.isdf_map_esdf.argtypes = [vp]
     lib.isdf_get_esdf_f64.argtypes = [vp, C.c_int, dp, C.c_int64]
@@ -614,6 +631,8 @@ def load_library(path=None):
     lib.isdf_set_sense_cloud_device.argtypes = [vp, vp, C.c_int64, C.c_int32, vp]
     lib.isdf_get_sense_info.argtypes = [vp, C.POINTER(SenseInfo)]
     lib.isdf_sense_depth.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, vp]
+    lib.isdf_map_observe.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, C.POINTER(ObserveInfo)]
+    lib.isdf_map_observe_device.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, C.POINTER(ObserveInfo), vp]
     lib.isdf_sense_depth_device.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, vp, vp]
     lib.isdf_sense_cloud.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, C.c_int64, vp, vp]
     lib.isdf_sense_cloud_device.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, C.c_int64, vp, vp, vp]
@@ -936,6 +955,54 @@ class Evaluator:
                 cap = total
                 continue
             self._check(rc)
+
+    # ---- known space (isdf_map_observe, isdf_map_mark_known, isdf_set_unknown_policy) ----
+    def map_observe(self, records, pos_offset=0, quat_offset=3, params=None, **kw):
+        """marks known the voxels the depth images at Q poses (read as sense_depth reads them) prove empty; params needs a finite
+        sensing_horizon -> dict(poses, voxels_tested, voxels_added)"""
+        p = params if params is not None else sense_params(**kw)
+        r = _f64(records)
+        r = r.reshape(-1, r.shape[-1])
+        Q, stride = self._pose_records(r, pos_offset, quat_offset)
+        base = r.ctypes.data
+        info = ObserveInfo()
+        self._check(self.lib.isdf_map_observe(self.h, Q, C.c_void_p(base + 8 * pos_offset), C.c_void_p(base + 8 * quat_offset), stride,
+                                              C.byref(p), C.byref(info)))
+        return info.as_dict()
+
+    def map_observe_device(self, records, pos_offset=0, quat_offset=3, params=None, stream=None, **kw):
+        """map_observe on a float64 CUDA tensor (Q, stride), read on torch's current stream (or stream); returns when the bits are set"""
+        import torch
+        p = params if params is not None else sense_params(**kw)
+        r = _cuda_records(records)
+        Q, stride = self._pose_records(r, pos_offset, quat_offset)
+        s = torch.cuda.current_stream(r.device) if stream is None else stream
+        base = r.data_ptr()
+        info = ObserveInfo()
+        self._check(self.lib.isdf_map_observe_device(self.h, Q, C.c_void_p(base + 8 * pos_offset), C.c_void_p(base + 8 * quat_offset), stride,
+                                                     C.byref(p), C.byref(info), C.c_void_p(s.cuda_stream)))
+        return info.as_dict()
+
+    def map_mark_known(self, boxes):
+        """marks known every voxel whose cube lies inside one of the closed boxes (n, 6): lo xyz, hi xyz (the caller asserts they are free)"""
+        b = np.ascontiguousarray(np.asarray(boxes, dtype=np.float64).reshape(-1, 6))
+        self._check(self.lib.isdf_map_mark_known(self.h, b.shape[0], b.ctypes.data_as(C.c_void_p) if b.size else None))
+
+    def get_map_known_u8(self):
+        """the known grid (X, Y, Z) uint8 in get_map_u8's layout"""
+        X, Y, Z = self.map_info()["dims"]
+        out = np.empty((X, Y, Z), dtype=np.uint8)
+        self._check(self.lib.isdf_get_map_known_u8(self.h, out.ctypes.data_as(C.POINTER(C.c_uint8)), out.size))
+        return out
+
+    def set_unknown_policy(self, policy):
+        """UNKNOWN_FREE (the default) or UNKNOWN_OCCUPIED: what the clearance family takes voxels nobody has seen to be"""
+        self._check(self.lib.isdf_set_unknown_policy(self.h, int(policy)))
+
+    def unknown_policy(self):
+        v = C.c_int(-1)
+        self._check(self.lib.isdf_get_unknown_policy(self.h, C.byref(v)))
+        return v.value
 
     # ---- world generators (isdf_world_*): the reference's globalmap_gene and mockamap worlds as (n, 4) float32 clouds ----
     @staticmethod
@@ -1745,7 +1812,7 @@ class Evaluator:
 
     # ---- flying to goals through a world seen only through the depth camera (plan -> fly -> sense -> fuse -> check -> re-plan) ----
     def navigate(self, starts, goals, *, rounds, horizon, sense_every=10, tol=0.5, plan_params=None, sim_params=None, sense_params=None,
-                 max_fields=0, stream=None, fallback="keep", brake_params=None):
+                 max_fields=0, stream=None, fallback="keep", brake_params=None, unknown="free", known_boxes=None):
         """Drive B vehicles from starts (B, 3) to goals (B, 3) through the scene set by set_sense_cloud*, building their one shared map by
         fusion into the current map's frame (set it first, e.g. set_map_u8 of zeros). Needs the shape, the front-end kernels and
         plan_params with PLAN_CERTIFY (a shape the certificate supports). Each round, for the active vehicles:
@@ -1767,6 +1834,20 @@ class Evaluator:
         from its goal is held instead of STOPPED: active, at rest at its simulator position, not flown, sensed at its state and replanned
         every round from (position, 0, 0); a round it stays held is NAV_HELD (its replan still counts as failed). Held vehicles that never
         get a plan end as TIMEOUT.
+        sense_params may be one camera or a list of cameras (a rig): every sensed pose is then rendered once per camera.
+        unknown: "free" (the default) is the loop above. "occupied" needs fallback="brake" and a finite sensing_horizon on every camera; for
+        the call it sets the context's unknown policy to UNKNOWN_OCCUPIED (restored on return), marks known_boxes known (map_mark_known:
+        the caller asserts they are free, e.g. the space around the starts), and changes the loop so that no vehicle commits to space it
+        has not seen:
+          1b. observe  after fusing, map_observe_device of the same poses for every camera;
+          2.  check    the certificates now read the blocked grid (occupied or not known);
+          3.  replan   also the vehicles flying a commit (and, as before, the held ones); an OPTIMISED plan that is COLLIDING with
+                       first_hit > 0 goes to trajectory_brake_device with t_stop_max = first_hit (one call for all such plans, in the brake
+                       stage, certified with NAV_COMMIT_SLACK more margin than brake_params', then, for the plans without such a stop, a
+                       second call with brake_params' margin); a BRAKED stop replaces the trajectory, flown as CERTIFIED (action NAV_COMMITTED) and marked as a commit;
+                       vehicles without an accepted plan or a commit take the fallback as before, except that a vehicle still holding a
+                       CERTIFIED remaining trajectory (a commit) keeps it. A commit that runs out away from the goal holds the vehicle.
+        The result then also has commits (B,) numpy, and times an "observe" stage.
         Vehicles share the map, so one vehicle's run depends on what the others sensed; with B = 1 it is that vehicle's alone. The world
         waits while the planner runs (no planning latency in simulated time). Within a round only per-vehicle values (stages, verdicts,
         counts, piece totals, positions of heads) cross to the host; points, pieces and logs stay on the device.
@@ -1776,6 +1857,31 @@ class Evaluator:
         logs: per round (vehicle indices (R,) numpy, log (R, n_log, 21) CUDA tensor); times: per round {stage: ms} from CUDA events (a
         "brake" stage with fallback="brake"); with fallback="brake" also brakes and held_rounds (B,) numpy: BRAKED stops taken and rounds
         spent held."""
+        if unknown not in ("free", "occupied"):
+            raise ValueError(f"unknown must be 'free' or 'occupied', got {unknown!r}")
+        cams = list(sense_params) if isinstance(sense_params, (list, tuple)) else [sense_params if sense_params is not None else
+                                                                                    globals()["sense_params"]()]
+        if not cams:
+            raise ValueError("sense_params: an empty camera list")
+        if unknown == "occupied":
+            if fallback != "brake":
+                raise ValueError("unknown='occupied' commits to certified stops: it needs fallback='brake'")
+            if not all(np.isfinite(c.sensing_horizon) for c in cams):
+                raise ValueError("unknown='occupied' observes free space: every camera needs a finite sensing_horizon")
+            prev = self.unknown_policy()
+            self.set_unknown_policy(UNKNOWN_OCCUPIED)
+            try:
+                if known_boxes is not None:
+                    self.map_mark_known(known_boxes)
+                return self._navigate(starts, goals, rounds, horizon, sense_every, tol, plan_params, sim_params, cams, max_fields, stream,
+                                      fallback, brake_params, True)
+            finally:
+                self.set_unknown_policy(prev)
+        return self._navigate(starts, goals, rounds, horizon, sense_every, tol, plan_params, sim_params, cams, max_fields, stream, fallback,
+                              brake_params, False)
+
+    def _navigate(self, starts, goals, rounds, horizon, sense_every, tol, plan_params, sim_params, cams, max_fields, stream, fallback,
+                  brake_params, occupied):
         import torch
         dev = torch.device("cuda", self.device)
         s = torch.cuda.current_stream(dev) if stream is None else stream
@@ -1792,9 +1898,10 @@ class Evaluator:
             raise ValueError(f"fallback must be 'keep' or 'brake', got {fallback!r}")
         brake = fallback == "brake"
         bp = brake_params if brake_params is not None else self.brake_params(certify=p.certify, dynamics=p.dynamics)
+        bpc = BrakeParams.from_buffer_copy(bytes(bp))   # a commit's stop
+        bpc.certify.clearance.margin += NAV_COMMIT_SLACK
         sp = SimParams.from_buffer_copy(bytes(sim_params if sim_params is not None else sim_default_params()))
         sp.t_end = float(horizon)
-        cam = sense_params if sense_params is not None else globals()["sense_params"]()
         cp = CertifyParams.from_buffer_copy(bytes(p.certify))
         info = self.map_info()
         lo, hi = info["bmin"], info["bmax"]
@@ -1810,11 +1917,14 @@ class Evaluator:
             T, Cc = torch.zeros(1, **f64), torch.zeros(18, **f64)
         n = np.zeros(B, dtype=np.int64)                                    # their piece counts (host)
         status = np.full(B, NAV_ACTIVE)
-        flown_rounds, replans, failed, uncert, brakes, held_rounds = (np.zeros(B, dtype=np.int64) for _ in range(6))
+        flown_rounds, replans, failed, uncert, brakes, held_rounds, commits = (np.zeros(B, dtype=np.int64) for _ in range(7))
         held, braking = np.zeros(B, dtype=bool), np.zeros(B, dtype=bool)   # held at rest; flying a stop
+        committed = np.zeros(B, dtype=bool)                                # flying a commit (unknown="occupied")
         actions, verdicts, replan_stages, replan_verdicts, logs, times = [], [], [], [], [], []
         last = None   # (vehicle indices, log) of the last round flown
         stages = ("sense", "fuse", "check", "replan", "brake", "fly", "advance") if brake else ("sense", "fuse", "check", "replan", "fly", "advance")
+        if occupied:
+            stages = ("sense", "fuse", "observe") + stages[2:]
         for r in range(int(rounds)):
             act = np.nonzero(status == NAV_ACTIVE)[0]
             if act.size == 0:
@@ -1839,12 +1949,19 @@ class Evaluator:
                 if rest:
                     ini = init[torch.as_tensor(rest, device=dev)]
                     recs.append(torch.cat([ini[:, 0:3], ini[:, 6:10]], 1))
-                pts, _ = self.sense_cloud_device(torch.cat(recs).contiguous(), 0, 3, params=cam, stream=s)
+                poses = torch.cat(recs).contiguous()
+                seen = [self.sense_cloud_device(poses, 0, 3, params=cam, stream=s)[0] for cam in cams]
                 ev["sense"][1].record(s)
                 ev["fuse"][0].record(s)
-                if pts.shape[0]:
-                    self.map_fuse_cloud_device(pts, stream=sv)
+                for pts in seen:
+                    if pts.shape[0]:
+                        self.map_fuse_cloud_device(pts, stream=sv)
                 ev["fuse"][1].record(s)
+                if occupied:   # 1b. the free space the same images prove
+                    ev["observe"][0].record(s)
+                    for cam in cams:
+                        self.map_observe_device(poses, 0, 3, params=cam, stream=s)
+                    ev["observe"][1].record(s)
                 # 2. check every remaining trajectory on the fused map
                 ev["check"][0].record(s)
                 offh = np.zeros(B + 1, dtype=np.int64)
@@ -1866,11 +1983,12 @@ class Evaluator:
                 ev["check"][1].record(s)
                 # 3. replan the vehicles without a certified remaining trajectory
                 ev["replan"][0].record(s)
-                need = [b for b in act if ver.get(b) != CERTIFIED]
+                need = [b for b in act if ver.get(b) != CERTIFIED or committed[b]]
                 for b in act:
                     if b in ver:
                         verdict[b] = ver[b]
                 new = {}   # vehicle -> (plan index) of an accepted plan
+                cand = {}  # unknown="occupied": vehicle -> (plan index, first_hit) of an optimised plan to commit to a stop of
                 if need:
                     heads = torch.zeros((len(need), 9), **f64)
                     moving = [i for i, b in enumerate(need) if n[b] > 0]
@@ -1895,16 +2013,20 @@ class Evaluator:
                                                      params=p, max_fields=max_fields, stream=s)
                         res = decode_plan_results(pl["results"])
                         stage = res["stage"].cpu().numpy()
-                        cv = pl["certify"].reshape(-1, C.sizeof(CertifySummary))[:, 40:44].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
+                        csum = pl["certify"].reshape(-1, C.sizeof(CertifySummary))
+                        cv = csum[:, 40:44].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
+                        ph = csum[:, 24:32].contiguous().view(torch.float64).reshape(-1).cpu().numpy() if occupied else None
                         for j, i in enumerate(ok):
                             rstage[need[i]], rverdict[need[i]] = stage[j], cv[j]
                             if stage[j] == OPTIMISED and cv[j] == CERTIFIED:
                                 new[need[i]] = j
+                            elif occupied and stage[j] == OPTIMISED and cv[j] == COLLIDING and ph[j] > 0:
+                                cand[need[i]] = (j, float(ph[j]))
                     for b in need:
                         replans[b] += 1
                         if b in new:
                             action[b], verdict[b] = NAV_REPLANNED, CERTIFIED
-                            held[b] = braking[b] = False
+                            held[b] = braking[b] = committed[b] = False
                         else:
                             action[b] = NAV_REPLAN_FAILED
                             failed[b] += 1
@@ -1936,7 +2058,47 @@ class Evaluator:
                 if brake:
                     # the fallback: a certified stop along the remaining trajectory of every vehicle whose replan failed
                     ev["brake"][0].record(s)
-                    bv = [b for b in need if b not in new and n[b] > 0]
+                    took = set()   # vehicles that committed to a stop of their new plan
+                    if cand:
+                        po = pl["piece_off"].cpu().numpy()
+
+                        def commit_stops(cb, params):   # vehicle -> (T, coeffs) of a BRAKED stop along its new plan
+                            bo = np.zeros(len(cb) + 1, dtype=np.int64)
+                            bo[1:] = np.cumsum([po[cand[b][0] + 1] - po[cand[b][0]] for b in cb])
+                            bT = torch.cat([pl["T"][po[cand[b][0]]:po[cand[b][0] + 1]] for b in cb]).contiguous()
+                            bC = torch.cat([pl["coeffs"][18 * po[cand[b][0]]:18 * po[cand[b][0] + 1]] for b in cb]).contiguous()
+                            ts = torch.as_tensor([cand[b][1] for b in cb], **f64)
+                            bk = self.trajectory_brake_device(torch.as_tensor(bo.astype(np.int32), device=dev), bT, bC, ts, params=params, stream=s)
+                            bst = bk["summary"][:, 0:4].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
+                            ko = bk["piece_off"].cpu().numpy()
+                            return {b: (bk["T"][ko[j]:ko[j + 1]], bk["coeffs"][18 * ko[j]:18 * ko[j + 1]]) for j, b in enumerate(cb) if bst[j] == BRAKED}
+                        # with the slack first; where no stop keeps it (passing close to unseen space, e.g. round a corner), the plan's margin
+                        got = commit_stops(sorted(cand), bpc)
+                        rest = [b for b in sorted(cand) if b not in got]
+                        if rest:
+                            got.update(commit_stops(rest, bp))
+                        if got:
+                            nn = n.copy()
+                            partsT, partsC = [], []
+                            for b in range(B):
+                                if b in got:
+                                    partsT.append(got[b][0]); partsC.append(got[b][1])
+                                    nn[b] = got[b][0].shape[0]
+                                    if action[b] == NAV_HELD:
+                                        held_rounds[b] -= 1
+                                    action[b], verdict[b] = NAV_COMMITTED, CERTIFIED
+                                    commits[b] += 1
+                                    held[b], braking[b], committed[b] = False, True, True
+                                elif n[b] > 0:
+                                    partsT.append(T[offh[b]:offh[b + 1]]); partsC.append(Cc[18 * offh[b]:18 * offh[b + 1]])
+                            n = nn
+                            T, Cc = torch.cat(partsT).contiguous(), torch.cat(partsC).contiguous()
+                            offh = np.zeros(B + 1, dtype=np.int64)
+                            offh[1:] = np.cumsum(n)
+                            off = torch.as_tensor(offh.astype(np.int32), device=dev)
+                            took = set(got)
+                    # (a vehicle still holding a CERTIFIED remaining trajectory, a commit, keeps it)
+                    bv = [b for b in need if b not in new and b not in took and n[b] > 0 and ver.get(b) != CERTIFIED]
                     if bv:
                         bo = np.zeros(len(bv) + 1, dtype=np.int64)
                         bo[1:] = np.cumsum(n[bv])
@@ -1996,7 +2158,7 @@ class Evaluator:
                         if diverged[k]:
                             status[b] = NAV_DIVERGED
                         elif n[b] == 0 and braking[b] and dist[k] > tol:
-                            held[b], braking[b] = True, False   # the stop ran out: held at rest where the simulator left it
+                            held[b], braking[b], committed[b] = True, False, False   # the stop ran out: held at rest where the simulator left it
                             init[b, 3:] = 0.0
                             init[b, 6] = 1.0
                             init[b, 13:17] = float(np.sqrt(sp.mass * sp.grav / (4 * sp.kf)))
@@ -2027,6 +2189,8 @@ class Evaluator:
                    times=times)
         if brake:
             out.update(brakes=brakes, held_rounds=held_rounds)
+        if occupied:
+            out.update(commits=commits)
         return out
 
     def plan_info(self):

@@ -203,6 +203,61 @@ int isdf_map_fuse_cloud_device(isdf_ctx *ctx, const void *d_points, int64_t n, i
 int isdf_get_map_u8(isdf_ctx *ctx, uint8_t *occ, int64_t n);
 int isdf_get_map_f64(isdf_ctx *ctx, double *grid_map, int64_t n);
 
+/* ---- known space: the voxels a depth image has proven empty (DESIGN §3.22) ----------------------------------------------------------
+ * The map carries a second bit grid, KNOWN, in the occupancy grid's layout. Every isdf_set_map_* call resets it to "nothing known" (its
+ * memory is allocated by the first call that marks a voxel); isdf_map_fuse_cloud* leaves it as it is; bits are only ever set.
+ * Voxel cube. Voxel (ix, iy, iz)'s cube is, per axis a with index i, in FP64 with nothing contracted: pad = 1e-12 (|bmin_a| + (i + 1) res),
+ *   lo = (bmin_a + i res) - pad, hi = (bmin_a + (i + 1) res) + pad (closed). The pad covers the rounding of getGridIndex, so every point
+ *   the cloud index puts in a voxel lies in its cube.
+ * isdf_map_observe(_device): the poses, camera and scene of isdf_sense_depth (same checks; ISDF_ERR_STATE without a scene or a map), and a
+ *   FINITE sensing_horizon (ISDF_ERR_INVALID otherwise, and when (ceil(2 horizon / res) + 3)^3 exceeds 2^40). Per pose the depth image is
+ *   rendered exactly as isdf_sense_depth renders it; with r, t the render's FP32 camera-from-world (as doubles), fx, fy, cx, cy its FP32
+ *   parameters and body the pose position, voxel v becomes known when all of these hold (FP64, nothing contracted, in this order):
+ *     2. every corner k of the cube has sqrt((d0^2 + d1^2) + d2^2) <= sensing_horizon, d = corner - body;
+ *        M = the largest |coordinate| of the cube; E_i = 1e-6 (((|r_i0| + |r_i1|) + |r_i2|) M + |t_i|) + 1e-30, each < 1e24;
+ *        corner camera coordinates c_i = ((r_i0 X + r_i1 Y) + r_i2 Z) + t_i;
+ *     1. zmin = min_k z_k > E_2 (the render's FP32 transform is within E_i of this one: its four roundings are below 2.4e-7 of the same sum);
+ *     3. with qx = x_k / z_k, u_k = qx fx + cx, a = max |qx| (likewise qy, v_k, b with fy, cy), zl = zmin - E_2,
+ *        dqx = (E_0 + a E_2) / zl, eu = (fx dqx + 1.2e-7 ((a + dqx) fx + |cx|)) + 1e-9 (1 + (a fx + |cx|)) (likewise ev with E_1, b, fy, cy):
+ *        the rectangle x0 = floor((min u - eu) + 0.5) .. x1 = floor((max u + eu) + 0.5), y0 .. y1 likewise, lies inside the image
+ *        (x0 >= 0, x1 <= W - 1, y0 >= 0, y1 <= H - 1). eu bounds the render's error in fma(x / z, fx, cx): the transform's E through the
+ *        division, the division's and the fma's roundings (2^-23 relative together), and this FP64 arithmetic;
+ *     4. with the image's min-mip (level l + 1 cell (i, j) = min of level l cells (2i .. 2i + 1, 2j .. 2j + 1) inside the level; level 0
+ *        the image) and l the smallest level with (x1 >> l) - (x0 >> l) <= 1 and (y1 >> l) - (y0 >> l) <= 1, the minimum D of the cells
+ *        (x0 >> l or x1 >> l, y0 >> l or y1 >> l) satisfies (double)D > 1000 zmax + ((1000 E_2 + 0.5) + 1.2e-7 (1000 (zmax + E_2) + 1)),
+ *        zmax = max_k z_k: dist_mm = trunc(fma(z, 1000, 0.5)) of a point at most zmax + E_2 deep is below that bound.
+ *   Invariant: no scene point lies in the cube of a known voxel. A point in the cube has exact camera coordinates in the corners' convex
+ *   hull, so (1) puts it in front of the camera, (3) puts its rendered centre pixel in the rectangle (truncation equals floor there), and
+ *   that pixel's depth is at most its dist_mm, which (4) excludes. The splat never matters, and the result is the same bits for any Q, pose
+ *   order, internal chunking, and through either form. info (may be NULL): poses; voxels_tested, the (pose, voxel) pairs of the map inside
+ *   each pose's index box floor((body - horizon - bmin) / res) - 1 + [0, ceil(2 horizon / res) + 3) per axis; voxels_added, the bits this
+ *   call set (exact in any order). The device form reads d_pos / d_quat on cuda_stream and returns when the bits are set. A CUDA failure
+ *   leaves no map.
+ * isdf_map_mark_known: marks known every voxel whose unpadded closed cube [bmin + i res, bmin + (i + 1) res] (per axis, FP64) lies inside
+ *   one of n closed boxes (lo[3], hi[3]: 6 doubles per box, host), so a box on voxel faces marks the voxels it holds. The caller asserts
+ *   the boxes are free (the space a vehicle starts in). ISDF_ERR_INVALID for n < 0, boxes NULL with n > 0, a non-finite
+ *   bound or lo > hi; ISDF_ERR_STATE without a map.
+ * isdf_get_map_known_u8: the known grid in isdf_get_map_u8's layout.
+ * isdf_set_unknown_policy: ISDF_UNKNOWN_FREE (the default) leaves the clearance family as it was, whatever is known;
+ *   ISDF_UNKNOWN_OCCUPIED makes every call that reads candidate voxels for a clearance or a certificate (isdf_trajectory_clearance,
+ *   isdf_pose_clearance, isdf_trajectory_certify, the certificate of isdf_trajectory_brake and of ISDF_PLAN_CERTIFY) read the BLOCKED grid
+ *   occ | (~known within the map) instead. The front end, mid-end, back-end cost, obstacle gathers and distance field keep reading occupancy.
+ *   The blocked grid is rebuilt (one launch, and a wait on the calling stream) by the first such call after a map, fuse, observe or mark
+ *   call. Voxels outside the map stay outside every candidate set. The policy is context state; it survives map changes. */
+typedef enum isdf_unknown_policy { ISDF_UNKNOWN_FREE = 0, ISDF_UNKNOWN_OCCUPIED = 1 } isdf_unknown_policy;
+typedef struct isdf_observe_info {
+    int64_t poses, voxels_tested, voxels_added;
+} isdf_observe_info;
+struct isdf_sense_params;   /* defined with the depth-sensing calls below */
+int isdf_map_observe(isdf_ctx *ctx, int64_t Q, const double *pos, const double *quat, int64_t stride_doubles, const struct isdf_sense_params *p,
+                     isdf_observe_info *info);
+int isdf_map_observe_device(isdf_ctx *ctx, int64_t Q, const double *d_pos, const double *d_quat, int64_t stride_doubles,
+                            const struct isdf_sense_params *p, isdf_observe_info *info, void *cuda_stream);
+int isdf_map_mark_known(isdf_ctx *ctx, int64_t n, const double *boxes);
+int isdf_get_map_known_u8(isdf_ctx *ctx, uint8_t *known, int64_t n);
+int isdf_set_unknown_policy(isdf_ctx *ctx, int policy);
+int isdf_get_unknown_policy(isdf_ctx *ctx, int *policy);
+
 /* ---- distance field of the map: replaces GridMap3D::generateESDF3d (grid:361-525), getSDFValue and getSDFValueWithGrad
  * (GridMap3D.h:114-193) ------------------------------------------------------------------------------------------------------
  *   Definition  POSITIVE at a voxel is res * sqrt((double)d2), d2 the exact integer squared voxel distance to the nearest occupied voxel
@@ -471,9 +526,12 @@ int isdf_midend_batch_ragged_device(isdf_ctx *ctx, int B, const int32_t *piece_o
  *     step = T_i * (1 / K_c), j = 0..K_c — the discrete path's pose: position of the piece polynomial, flatness quaternion, R = quat_rot(q).
  *     Junction times are sampled twice (last sample of one piece, first of the next), as in the integral loop. The check is SAMPLED: nothing
  *     is certified between two samples T_i / K_c apart (isdf_trajectory_certify below closes those gaps).
- *   Candidates of a sample: the occupied map voxels whose centre c (getGridCubeCenter) satisfies |R^T (c - x)|_inf <= H,
+ *   Candidates of a sample: the blocked map voxels whose centre c (getGridCubeCenter) satisfies |R^T (c - x)|_inf <= H,
  *     H = half_bd + reach, half_bd = kernel_size * occupancy_resolution / 2 (a strict > on any axis excludes, as hpp:800). Only voxels of
  *     the map count: a window reaching past the map border is cut off there (no projInMap clamping).
+ *   Blocked voxels are the occupied ones under ISDF_UNKNOWN_FREE (the default) and the occupied or not known ones under
+ *     ISDF_UNKNOWN_OCCUPIED (isdf_set_unknown_policy); isdf_pose_clearance, isdf_trajectory_certify, the certificate of isdf_trajectory_brake
+ *     and the certificate of the planning calls (ISDF_PLAN_CERTIFY) read the same blocked voxels.
  *   clear(s) = min(reach, min over candidates of sdf(R^T (c - x))), sdf = getonlySDF of the shape (analytic: the closed form of
  *     isdf_shape_query(..., ISDF_QUERY_SDF); mesh: s * dist in the context's sign mode).
  *   Witness: the address ix*Y*Z + iy*Z + iz of the candidate realising the minimum when it is < reach (the smallest address among exact
@@ -546,7 +604,7 @@ int isdf_pose_clearance_device(isdf_ctx *ctx, int64_t Q, const double *d_pos, co
  * The clearance check above is sampled; this call closes the gaps between the samples with a proven motion bound.
  * Definition. Inputs and parameters are the clearance check's (T, coeffs, K_c, N0, reach, margin) with 0 <= margin < reach. One verdict
  * per trajectory:
- *   CERTIFIED (1)   for every time t of the trajectory and every occupied voxel centre c of the map, the Euclidean distance from c to
+ *   CERTIFIED (1)   for every time t of the trajectory and every blocked voxel centre c of the map (the clearance check's blocked voxels), the Euclidean distance from c to
  *                   the robot posed at t is at least margin;
  *   COLLIDING (-1)  some evaluated pose sample has clear < margin (or a non-finite pose);
  *   UNDECIDED (0)   neither was established within the refinement budget.
@@ -930,7 +988,8 @@ int isdf_frontend_path_fields_device(isdf_ctx *ctx, int S, const double *starts,
  *                  coeffs are forwardT + MINCO of the returned x whatever its ret (back_end_optimizer.cpp:140-163), computed without a
  *                  further evaluation. Stage OPTIMISED; backend_ret < 0 is reported and the trajectory still returned (`if (1)`, :297).
  *   7. Certificates with ISDF_PLAN_CERTIFY / ISDF_PLAN_DYNAMICS: isdf_trajectory_certify / isdf_trajectory_dynamics with p->certify /
- *                  p->dynamics and N0 = N on every returned trajectory (OPTIMISED and MIDEND_FAILED), one call per distinct N.
+ *                  p->dynamics and N0 = N on every returned trajectory (OPTIMISED and MIDEND_FAILED), one call per distinct N. The
+ *                  certificate reads the blocked voxels of the context's unknown policy; stages 1-6 read the occupancy grid.
  * Deviation: the reference's back end is LMBM (lmbm.h, Fortran); the driver here is the project's device L-BFGS. max_iterations 10000 in
  *   the defaults is LMBM's iteration cap (lmbm.h:20-57) taken as an analogue, not an equivalent.
  * Guarantees: results are bit-identical run to run; each plan is bit-identical to the same call with that goal alone; every output is
@@ -1083,6 +1142,7 @@ int isdf_trajectory_shift(isdf_ctx *ctx, int B, const int32_t *piece_off, const 
 int isdf_trajectory_shift_device(isdf_ctx *ctx, int B, const int32_t *d_piece_off, const double *d_T, const double *d_coeffs,
                                  const double *d_t0, int32_t *d_out_piece_off, double *d_out_T, double *d_out_coeffs, void *cuda_stream);
 /* ---- braking to a certified stop along the remaining trajectory (DESIGN §3.21) -------------------------------------------------------
+ * (The clearance certificate of the candidates reads the blocked voxels of the context's unknown policy, isdf_set_unknown_policy.)
  * B remaining trajectories in isdf_plan_batch's ragged layout (each starting at the vehicle's current time 0) and t_stop_max[b], the latest
  * trajectory time whose position the stop may reach (e.g. a COLLIDING certificate's first_hit). Per trajectory b, in FP64 with nothing
  * contracted, in this order:
