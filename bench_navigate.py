@@ -3,7 +3,7 @@
 (Evaluator.navigate: sense -> fuse -> check -> replan -> fly -> advance, every stage batched over vehicles); prints one JSON line.
 
   python bench_navigate.py [--vehicles 1,16,64] [--rounds R] [--horizon H] [--sense-every S] [--seed N] [--fallback keep|brake]
-                           [--unknown free|occupied] [--cameras 1|4]
+                           [--unknown free|occupied] [--cameras 1|4] [--prefer-known W]
 
 World: mockamap's box world (isdf_world_cloud_device, ISDF_WORLD_BOXES) with seed 511, 40 x 40 x 10 m at 0.5 m (size 80 x 80 x 20,
 scale 2), 20 boxes 1.5 to 3 m wide: x and y in [-20, 20] m, z in [0, 10] m. The vehicles' map starts as an empty 1 m frame over that box
@@ -17,7 +17,9 @@ Per B: per-stage milliseconds per round (mean over the rounds run, CUDA events),
 clearance over every flown pose. --fallback brake (navigate's fallback, DESIGN §3.21) adds the stops taken and the rounds held; the
 default, keep, prints what it always printed. --unknown occupied (navigate's unknown policy, DESIGN §3.22; needs --fallback brake) seeds
 the known space with the 5 x 5 x 5-voxel block around each start (free in the true map by pairs()) and adds the commits taken; --cameras 4
-flies a rig of four cameras, cam_to_body = Rz(k 90 deg) cam02body. Either option (also --unknown free) also reports the pose of the minimum true clearance: its
+flies a rig of four cameras, cam_to_body = Rz(k 90 deg) cam02body. --prefer-known W plans through what has been seen (DESIGN §3.23):
+the front end's surcharge unknown_weight = W on unknown voxels and ISDF_PLAN_KNOWN_PREFIX, so that the back end treats unseen space as
+an obstacle along each plan's known prefix. Either option (also --unknown free) also reports the pose of the minimum true clearance: its
 vehicle, round and witness voxel, and whether that voxel is occupied in the vehicles' fused map at the end of the run. Writes nothing to the
 tree.
 """
@@ -100,6 +102,7 @@ def main():
     ap.add_argument("--fallback", choices=("keep", "brake"), default="keep")
     ap.add_argument("--unknown", choices=("free", "occupied"), default=None)
     ap.add_argument("--cameras", type=int, choices=(1, 4), default=1)
+    ap.add_argument("--prefer-known", type=float, default=None, metavar="W")
     args = ap.parse_args()
     if args.unknown == "occupied" and args.fallback != "brake":
         raise SystemExit("--unknown occupied needs --fallback brake")
@@ -125,6 +128,10 @@ def main():
     trace = args.unknown is not None or args.cameras != 1
     if trace:
         out.update(unknown=args.unknown or "free", cameras=args.cameras)
+    pkw = dict(flags=I.PLAN_CERTIFY, backend_max_iterations=200)
+    if args.prefer_known is not None:
+        pkw.update(flags=I.PLAN_CERTIFY | I.PLAN_KNOWN_PREFIX, unknown_weight=args.prefer_known)
+        out["prefer_known"] = args.prefer_known
     for B in [int(v) for v in args.vehicles.split(",")]:
         starts, goals = pairs(occ, B, args.seed + B)
         ev = I.Evaluator(cfg)
@@ -134,7 +141,7 @@ def main():
         ev.set_sense_cloud_device(scene, stream=torch.cuda.current_stream().cuda_stream)
         kw = dict(unknown="occupied", known_boxes=np.concatenate([starts - 2.5, starts + 2.5], 1)) if args.unknown == "occupied" else {}
         r = ev.navigate(starts, goals, rounds=args.rounds, horizon=args.horizon, sense_every=args.sense_every, tol=1.0,
-                        plan_params=ev.plan_params(flags=I.PLAN_CERTIFY, backend_max_iterations=200),
+                        plan_params=ev.plan_params(**pkw),
                         sense_params=rig(args.cameras), fallback=args.fallback, **kw)
         fail = np.isin(r["actions"], [I.NAV_REPLAN_FAILED, I.NAV_BRAKED, I.NAV_HELD]) if brake else r["actions"] == I.NAV_REPLAN_FAILED
         why = {}   # failed replans by (plan stage, certificate verdict); -2: no plan call (a head outside the frame)

@@ -278,7 +278,7 @@ struct isdf_ctx {
         DevBuf<GatherBox> d_box; DevBuf<int> d_wpoff, d_cnt, d_ptoff; DevBuf<long long> d_offs, d_total; DevBuf<double> d_wp, d_out;
     } gat;
     struct {   // planning step (isdf_plan_pairs): the stages' buffers and the per-plan launch layouts (the host forms stage through Staging)
-        DevBuf<double> d_bc, d_wp, d_mx, d_mres, d_bbc, d_bx, d_bf, d_gT, d_gC, d_dur, d_pwp; DevBuf<int> d_mi, d_bi, d_N, d_idx, d_ok, d_bplan, d_gi;
+        DevBuf<double> d_bc, d_wp, d_mx, d_mres, d_bbc, d_bx, d_bf, d_gT, d_gC, d_dur, d_pwp; DevBuf<int> d_mi, d_bi, d_N, d_idx, d_ok, d_bplan, d_gi, d_krows;
         DevBuf<CertSummary> d_csum; DevBuf<DynSummary> d_dsum;
         DevBuf<CopySeg> d_seg; DevBuf<PlanRow> d_row;
         DevBuf<int> d_bad;   // isdf_plan_states_device's head check
@@ -1779,10 +1779,9 @@ extern "C" int isdf_map_observe_device(isdf_ctx *c, int64_t Q, const double *d_p
     return observe_impl(c, Q, d_pos, d_quat, stride_doubles, p, info, true, (cudaStream_t)cuda_stream);
 }
 
-// the grid the clearance family reads: the occupancy grid, or under ISDF_UNKNOWN_OCCUPIED the blocked grid, rebuilt on st (and waited for,
-// so that a later call on another stream reads it whole) when stale
-static int clearance_grid_ready(isdf_ctx *c, cudaStream_t st) {
-    if (c->known.policy != ISDF_UNKNOWN_OCCUPIED || c->known.blocked_ok || !c->map.have_map) return 0;
+// the blocked grid occ | ~known, rebuilt on st (and waited for, so that a later call on another stream reads it whole) when stale
+static int blocked_grid_ready(isdf_ctx *c, cudaStream_t st) {
+    if (c->known.blocked_ok || !c->map.have_map) return 0;
     const DevGrid &g = c->map.grid;
     CU_TRY(c->known.d_blocked.ensure((size_t)g.X * g.Y * g.Zw));
     int launches = 0;
@@ -1794,6 +1793,12 @@ static int clearance_grid_ready(isdf_ctx *c, cudaStream_t st) {
     c->known.blocked.bits = c->known.d_blocked.p;
     c->known.blocked_ok = true;
     return 0;
+}
+
+// the grid the clearance family reads: the occupancy grid, or under ISDF_UNKNOWN_OCCUPIED the blocked grid (blocked_grid_ready)
+static int clearance_grid_ready(isdf_ctx *c, cudaStream_t st) {
+    if (c->known.policy != ISDF_UNKNOWN_OCCUPIED) return 0;
+    return blocked_grid_ready(c, st);
 }
 
 // ---- world generators (isdf_world.cuh, compiled in isdf_world_tu.cu) ----
@@ -1960,15 +1965,20 @@ __global__ void k_gather_boxes_batch(const DevGrid G, const int *wp_off, int B, 
 
 // CTA (j, b): row wp_off[b] + j. An earlier box of the plan can claim a voxel of this box only if their include boxes (a0..a1) intersect;
 // those are listed once per CTA and the voxel loop tests only them. Count pass: counts[row]; write pass: the voxels at offs[row] (< cap).
+// known_rows (may be NULL): plan b's rows j < known_rows[b] read the blocked grid's words instead of the occupancy grid's. The earlier boxes
+// are tested on the row's own grid: a known row's earlier rows are known, and an occupied voxel is blocked, so an occupancy row's voxel is
+// set in every earlier row's grid alike.
 template <bool WRITE>
-__global__ void __launch_bounds__(256) k_gather_points_batch(const DevGrid G, const int *wp_off, const GatherBox *boxes, int *counts,
-                                                            const long long *offs, double *out, long long cap) {
+__global__ void __launch_bounds__(256) k_gather_points_batch(DevGrid G, const int *wp_off, const GatherBox *boxes, int *counts,
+                                                            const long long *offs, double *out, long long cap, const uint32_t *blocked,
+                                                            const int *known_rows) {
     __shared__ int warp_cnt[8];
     __shared__ int nlist;
     __shared__ long long running;
     __shared__ int list[GATHER_LIST_CAP];
     const int q0 = wp_off[blockIdx.y], j = blockIdx.x;
     if (j >= wp_off[blockIdx.y + 1] - q0) return;   // the plan has fewer rows (uniform over the CTA)
+    if (known_rows && j < known_rows[blockIdx.y]) G.bits = blocked;
     const int q = q0 + j;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const GatherBox b = boxes[q];
@@ -2055,12 +2065,14 @@ __global__ void __launch_bounds__(1024) k_gather_scan(const int *counts, int R, 
     if (threadIdx.x == 0) *total = running;
 }
 
-// the batched gather on stream st from staged inputs: d_wp (R x 3 rows), d_wp_off (its B + 1 offsets; h_wp_off the same on the host).
-// Counts and scans, reads the plans' offsets into pt_off (B + 1, also when the lists exceed cap) and the total into *total; then, when
-// the total fits cap, writes every list to c->gat.d_out.
+// the batched gather on stream st from staged inputs: d_wp (R x 3 rows), d_wp_off (its B + 1 offsets; h_wp_off the same on the host),
+// d_known_rows (B, may be NULL: every row reads the occupancy grid). Counts and scans, reads the plans' offsets into pt_off (B + 1, also
+// when the lists exceed cap) and the total into *total; then, when the total fits cap, writes every list to c->gat.d_out.
 static int gather_batch_run(isdf_ctx *c, int B, const int *h_wp_off, const int *d_wp_off, const double *d_wp, double half, const double *offset,
-                            long long cap, std::vector<int> &pt_off, long long *total, cudaStream_t st) {
+                            const int *d_known_rows, long long cap, std::vector<int> &pt_off, long long *total, cudaStream_t st) {
     auto &g = c->gat;
+    if (d_known_rows) if (int r = blocked_grid_ready(c, st)) return r;
+    const uint32_t *blocked = d_known_rows ? c->known.d_blocked.p : nullptr;
     const int R = h_wp_off[B];
     int maxQ = 0;
     for (int b = 0; b < B; b++) maxQ = std::max(maxQ, h_wp_off[b + 1] - h_wp_off[b]);
@@ -2069,7 +2081,7 @@ static int gather_batch_run(isdf_ctx *c, int B, const int *h_wp_off, const int *
     const double ox = offset ? offset[0] : 0.0, oy = offset ? offset[1] : 0.0, oz = offset ? offset[2] : 0.0;
     if (R > 0) {
         k_gather_boxes_batch<<<(R + 127) / 128, 128, 0, st>>>(c->map.grid, d_wp_off, B, d_wp, R, half, ox, oy, oz, g.d_box.p);
-        k_gather_points_batch<false><<<dim3(maxQ, B), 256, 0, st>>>(c->map.grid, d_wp_off, g.d_box.p, g.d_cnt.p, nullptr, nullptr, 0);
+        k_gather_points_batch<false><<<dim3(maxQ, B), 256, 0, st>>>(c->map.grid, d_wp_off, g.d_box.p, g.d_cnt.p, nullptr, nullptr, 0, blocked, d_known_rows);
         c->stats.kernel_launches += 2;
     }
     k_gather_scan<<<1, 1024, 0, st>>>(g.d_cnt.p, R, d_wp_off, B, g.d_offs.p, g.d_ptoff.p, g.d_total.p);
@@ -2084,7 +2096,8 @@ static int gather_batch_run(isdf_ctx *c, int B, const int *h_wp_off, const int *
     if (*total > cap) return fail(ISDF_ERR_INVALID, "cap smaller than the obstacle lists (pt_off reports their sizes)");
     if (*total == 0) return 0;
     CU_TRY(g.d_out.ensure((size_t)3 * *total));
-    k_gather_points_batch<true><<<dim3(maxQ, B), 256, 0, st>>>(c->map.grid, d_wp_off, g.d_box.p, nullptr, g.d_offs.p, g.d_out.p, *total);
+    k_gather_points_batch<true><<<dim3(maxQ, B), 256, 0, st>>>(c->map.grid, d_wp_off, g.d_box.p, nullptr, g.d_offs.p, g.d_out.p, *total, blocked,
+                                                          d_known_rows);
     c->stats.kernel_launches++;
     CU_TRY(cudaGetLastError());
     return 0;
@@ -2116,7 +2129,7 @@ extern "C" int isdf_gather_obstacle_points(isdf_ctx *c, const double *waypoints,
     if (int r = S.upload()) return r;
     std::vector<int> off;
     long long total = 0;
-    if (int r = gather_batch_run(c, 1, wp_off, d_wpoff, d_wp, half_extent, offset, 0x7fffffffll, off, &total, c->stream)) return r;
+    if (int r = gather_batch_run(c, 1, wp_off, d_wpoff, d_wp, half_extent, offset, nullptr, 0x7fffffffll, off, &total, c->stream)) return r;
     *n = (int)total;
     const long long m = std::min<long long>(total, cap);
     if (m > 0 && out_points) {   // the write pass runs on the context's non-blocking stream
@@ -2129,24 +2142,30 @@ extern "C" int isdf_gather_obstacle_points(isdf_ctx *c, const double *waypoints,
     return 0;
 }
 
-extern "C" int isdf_gather_obstacle_points_batch(isdf_ctx *c, int B, const int32_t *wp_off, const double *waypoints, double half_extent,
-                                                 const double *offset, int64_t cap, double *out_points, int32_t *pt_off, int set_as_points) {
+extern "C" int isdf_gather_obstacle_points_batch_known(isdf_ctx *c, int B, const int32_t *wp_off, const double *waypoints, double half_extent,
+                                                       const double *offset, const int32_t *known_rows, int64_t cap, double *out_points,
+                                                       int32_t *pt_off, int set_as_points) {
     if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
     if (B < 1 || B > 65535) return fail(ISDF_ERR_INVALID, "B must lie in [1, 65535]");
     if (!wp_off || !pt_off || cap < 0) return fail(ISDF_ERR_INVALID, "NULL argument or cap < 0");
     if (int r = offsets_check(wp_off, B, "wp_off", true)) return r;
     if (wp_off[B] > 0 && !waypoints) return fail(ISDF_ERR_INVALID, "waypoints is NULL");
+    if (known_rows)
+        for (int b = 0; b < B; b++)
+            if (known_rows[b] < 0) return fail(ISDF_ERR_INVALID, "known_rows[" + std::to_string(b) + "] < 0");
     if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
     if (set_device(c)) return ISDF_ERR_CUDA;
     auto &g = c->gat;
     Staging S(c);
-    const int *d_wpoff;
+    const int *d_wpoff, *d_krows = nullptr;
     const double *d_wp;
     S.in(&d_wpoff, wp_off, (size_t)B + 1); S.in(&d_wp, waypoints, (size_t)3 * wp_off[B]);
+    if (known_rows) S.in(&d_krows, known_rows, (size_t)B);
     if (int r = S.upload()) return r;
     std::vector<int> off;
     long long total = 0;
-    const int r = gather_batch_run(c, B, wp_off, d_wpoff, d_wp, half_extent, offset, out_points ? cap : 0x7fffffffll, off, &total, c->stream);
+    const int r = gather_batch_run(c, B, wp_off, d_wpoff, d_wp, half_extent, offset, d_krows, out_points ? cap : 0x7fffffffll, off, &total,
+                                   c->stream);
     if (!off.empty()) std::memcpy(pt_off, off.data(), sizeof(int32_t) * off.size());
     if (r) return r;
     if (out_points && total > 0) {   // the write pass runs on the context's non-blocking stream
@@ -2155,6 +2174,11 @@ extern "C" int isdf_gather_obstacle_points_batch(isdf_ctx *c, int B, const int32
     }
     if (set_as_points) return gather_set_points(c, B, off, total, c->stream);
     return 0;
+}
+
+extern "C" int isdf_gather_obstacle_points_batch(isdf_ctx *c, int B, const int32_t *wp_off, const double *waypoints, double half_extent,
+                                                 const double *offset, int64_t cap, double *out_points, int32_t *pt_off, int set_as_points) {
+    return isdf_gather_obstacle_points_batch_known(c, B, wp_off, waypoints, half_extent, offset, nullptr, cap, out_points, pt_off, set_as_points);
 }
 
 // ---- discrete evaluation ------------------------------------------------------------------------------------
@@ -4174,11 +4198,21 @@ extern "C" int isdf_frontend_check_batch(isdf_ctx *c, int n, const int32_t *ind,
 // ---- front-end path search (isdf_frontpath.cuh) ------------------------------------------------------------------------------------
 constexpr int FP_ROUNDS_PER_CHECK = 8;   // relaxation rounds launched between two reads of the frontier flag
 
-static int path_args_check(isdf_ctx *c, const isdf_frontpath_params *prm) {
+// the parameters' own checks; *cw = 1 + unknown_weight (1 for NULL params), the edge factor of a voxel that is not known
+static int frontpath_params_check(const isdf_frontpath_params *prm, double *cw) {
+    *cw = 1.0;
+    if (!prm) return 0;
+    for (int32_t v : prm->reserved_) if (v != 0) return fail(ISDF_ERR_INVALID, "isdf_frontpath_params: reserved fields must be zero");
+    if (!(std::isfinite(prm->unknown_weight) && prm->unknown_weight >= 0.0))
+        return fail(ISDF_ERR_INVALID, "isdf_frontpath_params: unknown_weight must be finite and >= 0");
+    *cw = 1.0 + prm->unknown_weight;
+    return 0;
+}
+
+static int path_args_check(isdf_ctx *c, const isdf_frontpath_params *prm, double *cw) {
     if (int r = frontend_state(c)) return r;
     if (c->world > 1) return fail(ISDF_ERR_UNSUPPORTED, "the front-end path search is not sharded: call it on a context with isdf_set_shard(ctx, 0, 1)");
-    if (prm) for (int32_t v : prm->reserved_) if (v != 0) return fail(ISDF_ERR_INVALID, "isdf_frontpath_params: reserved fields must be zero");
-    return 0;
+    return frontpath_params_check(prm, cw);
 }
 
 // isInMap (Gridmap3D.cpp) + getGridIndex (Gridmap3D.cpp:135-175) with its clamps and its "iy < 0 => ix = 0" branches (they cannot fire
@@ -4206,6 +4240,10 @@ static PathArgs path_args(isdf_ctx *c, unsigned long long *d_g) {
     return P;
 }
 
+// the surcharge with edge factor cw; cw == 1 (weight 0, or a weight below FP64's resolution at 1, where w * cw == w) selects the
+// unweighted kernels
+static FpSurcharge path_surcharge(const isdf_ctx *c, double cw) { return {c->known.have ? c->known.d_known.p : nullptr, cw}; }
+
 // the traversability grid of the current map and kernels on stream st, between events 0 and 1; clears c->fp.info
 static int path_trav(isdf_ctx *c, cudaStream_t st) {
     const DevGrid &G = c->map.grid;
@@ -4219,9 +4257,9 @@ static int path_trav(isdf_ctx *c, cudaStream_t st) {
     return 0;
 }
 
-// one relaxation from the n source voxels src (host, 3 each) into d_g (field s at d_g + s*X*Y*Z) on stream st, after path_trav; adds its
-// device time and its rounds to c->fp.info
-static int path_fields(isdf_ctx *c, int n, const int *src, unsigned long long *d_g, cudaStream_t st) {
+// one relaxation from the n source voxels src (host, 3 each) into d_g (field s at d_g + s*X*Y*Z) on stream st, after path_trav, with
+// the unknown-voxel edge factor cw; adds its device time and its rounds to c->fp.info
+static int path_fields(isdf_ctx *c, int n, const int *src, double cw, unsigned long long *d_g, cudaStream_t st) {
     const DevGrid &G = c->map.grid;
     const size_t nword = (size_t)G.X * G.Y * G.Zw, nvox = (size_t)G.X * G.Y * G.Z, nflag = (size_t)(n + 1) * FP_FLAG_RING + 1;
     CU_TRY(c->fp.d_front.ensure(2 * (size_t)n * nword));
@@ -4229,6 +4267,7 @@ static int path_fields(isdf_ctx *c, int n, const int *src, unsigned long long *d
     CU_TRY(c->fp.d_src.upload(src, (size_t)3 * n, st));
     count_copy(c, cudaMemcpyHostToDevice, sizeof(int) * 3 * (size_t)n);
     PathArgs P = path_args(c, d_g);
+    const FpSurcharge U = path_surcharge(c, cw);
     P.flags = c->fp.d_flags.p; P.rounds = P.flags + (size_t)(n + 1) * FP_FLAG_RING;
     P.any = n == 1 ? P.flags : P.flags + (size_t)n * FP_FLAG_RING;
     P.front1 = P.front + nword;
@@ -4241,8 +4280,13 @@ static int path_fields(isdf_ctx *c, int n, const int *src, unsigned long long *d
     const dim3 blocks((unsigned)std::min<long long>(((long long)nword + 255) / 256, sms * 16), (unsigned)n);
     for (int r = 0;;) {
         for (int k = 0; k < FP_ROUNDS_PER_CHECK; k++, r++) {
-            if (n == 1) k_fp_relax<<<blocks, 256, 0, st>>>(P, r);
-            else k_fp_relax_multi<<<blocks, 256, 0, st>>>(P, r);
+            if (cw == 1.0) {
+                if (n == 1) k_fp_relax<false><<<blocks, 256, 0, st>>>(P, r, U);
+                else k_fp_relax_multi<false><<<blocks, 256, 0, st>>>(P, r, U);
+            } else {
+                if (n == 1) k_fp_relax<true><<<blocks, 256, 0, st>>>(P, r, U);
+                else k_fp_relax_multi<true><<<blocks, 256, 0, st>>>(P, r, U);
+            }
         }
         c->stats.kernel_launches += FP_ROUNDS_PER_CHECK;
         CU_TRY(cudaGetLastError());
@@ -4275,9 +4319,9 @@ static void path_info(isdf_ctx *c, size_t field_bytes, bool paths) {
 // goal (sstride 0). Pairs whose starts share a voxel share a field: node 0 of a path is its start voxel's cube centre, so their paths are
 // the same. The distinct start voxels' fields are built in chunks of at most max_fields (0: FP_FIELD_BUDGET bytes, at least one field),
 // and each chunk's paths are walked into scratch before its fields are reused. off (B + 1) is filled as soon as every length is known,
-// also when they exceed cap.
-static int path_run(isdf_ctx *c, int B, const double *starts, int sstride, const double *goals, int max_fields, int cap, std::vector<int> &off,
-                    cudaStream_t st) {
+// also when they exceed cap. cw: the unknown-voxel edge factor of the fields and the walk (frontpath_params_check).
+static int path_run(isdf_ctx *c, int B, const double *starts, int sstride, const double *goals, double cw, int max_fields, int cap,
+                    std::vector<int> &off, cudaStream_t st) {
     const DevGrid &G = c->map.grid;
     const size_t nvox = (size_t)G.X * G.Y * G.Z;
     std::vector<int> tgt((size_t)3 * B), ps(B), src;   // ps[b]: pair b's source; src: 3 per distinct start voxel, in order of first use
@@ -4316,12 +4360,14 @@ static int path_run(isdf_ctx *c, int B, const double *starts, int sstride, const
     std::vector<int> len(B), woff((size_t)B + 1, 0);   // walk order; woff: first node in scratch
     for (int s0 = 0; s0 < S; s0 += F) {
         const int n = std::min(F, S - s0), w0 = wstart[s0], w1 = wstart[s0 + n], nt = w1 - w0;
-        if (int r = path_fields(c, n, &src[3 * (size_t)s0], c->fp.d_g.p, st)) return r;
+        if (int r = path_fields(c, n, &src[3 * (size_t)s0], cw, c->fp.d_g.p, st)) return r;
         PathArgs P = path_args(c, c->fp.d_g.p);
+        const auto walk_kernel = cw == 1.0 ? k_fp_walk<false> : k_fp_walk<true>;
+        const FpSurcharge U = path_surcharge(c, cw);
         P.nt = nt; P.tgt = c->fp.d_tgt.p + 3 * (size_t)w0; P.tsrc = c->fp.d_tsrc.p + 4 * (size_t)w0; P.pair = c->fp.d_pair.p + w0;
         P.len = c->fp.d_len.p + w0; P.cost = c->fp.d_cost.p; P.found = c->fp.d_found.p;
         const unsigned wblocks = (unsigned)(((long long)nt * 32 + 127) / 128);
-        k_fp_walk<<<wblocks, 128, 0, st>>>(P, 0);
+        walk_kernel<<<wblocks, 128, 0, st>>>(P, 0, U);
         c->stats.kernel_launches++;
         CU_TRY(cudaGetLastError());
         CU_TRY(cudaMemcpyAsync(len.data() + w0, P.len, sizeof(int) * nt, cudaMemcpyDeviceToHost, st));
@@ -4341,7 +4387,7 @@ static int path_run(isdf_ctx *c, int B, const double *starts, int sstride, const
         CU_TRY(cudaMemcpyAsync(c->fp.d_woff.p + w0, woff.data() + w0, sizeof(int) * ((size_t)nt + 1), cudaMemcpyHostToDevice, st));
         count_copy(c, cudaMemcpyHostToDevice, sizeof(int) * ((size_t)nt + 1));
         P.off = c->fp.d_woff.p + w0; P.scratch = c->fp.d_scratch.p;
-        k_fp_walk<<<wblocks, 128, 0, st>>>(P, 1);
+        walk_kernel<<<wblocks, 128, 0, st>>>(P, 1, U);
         c->stats.kernel_launches++;
         CU_TRY(cudaGetLastError());
     }
@@ -4413,13 +4459,14 @@ static int path_entry(isdf_ctx *c, bool dev, int B, const double *starts, int ss
                       void *cuda_stream) {
     if (!starts || !goals || B < 1 || max_fields < 0 || cap < 0 || (cap > 0 && !path_xyz) || !offsets || !costs || !found)
         return fail(ISDF_ERR_INVALID, "bad argument");
-    if (int r = path_args_check(c, prm)) return r;
+    double cw = 1.0;
+    if (int r = path_args_check(c, prm, &cw)) return r;
     if (set_device(c)) return ISDF_ERR_CUDA;
     const cudaStream_t st = dev ? (cudaStream_t)cuda_stream : c->stream;
     std::vector<double> hs, hg;
     if (dev) if (int r = read_endpoints(c, B, starts, sstride, goals, hs, hg, st)) return r;
     std::vector<int> off;
-    const int r = path_run(c, B, starts, sstride, goals, max_fields, cap, off, st);
+    const int r = path_run(c, B, starts, sstride, goals, cw, max_fields, cap, off, st);
     if (!off.empty() && !dev) std::memcpy(offsets, off.data(), sizeof(int32_t) * off.size());
     if (!off.empty() && dev) {
         CU_TRY(cudaMemcpyAsync(offsets, off.data(), sizeof(int32_t) * off.size(), cudaMemcpyHostToDevice, st));
@@ -4468,32 +4515,34 @@ extern "C" int isdf_frontend_path_pairs_device(isdf_ctx *c, int B, const double 
 }
 
 // the fields of the S source voxels src (host, 3 each) in one relaxation into d_g
-static int path_fields_run(isdf_ctx *c, int S, const int *src, double *d_g, cudaStream_t st) {
+static int path_fields_run(isdf_ctx *c, int S, const int *src, double cw, double *d_g, cudaStream_t st) {
     if (int r = path_trav(c, st)) return r;
-    if (int r = path_fields(c, S, src, reinterpret_cast<unsigned long long *>(d_g), st)) return r;
+    if (int r = path_fields(c, S, src, cw, reinterpret_cast<unsigned long long *>(d_g), st)) return r;
     path_info(c, (size_t)S * c->map.grid.X * c->map.grid.Y * c->map.grid.Z * sizeof(double), false);
     return 0;
 }
 
 extern "C" int isdf_frontend_path_field_device(isdf_ctx *c, const double *start, const isdf_frontpath_params *prm, double *d_g, void *cuda_stream) {
     if (!start || !d_g) return fail(ISDF_ERR_INVALID, "bad argument");
-    if (int r = path_args_check(c, prm)) return r;
+    double cw = 1.0;
+    if (int r = path_args_check(c, prm, &cw)) return r;
     if (set_device(c)) return ISDF_ERR_CUDA;
     int s[3];
     if (int r = path_voxel(c->map.grid, start, s, "start")) return r;
-    return path_fields_run(c, 1, s, d_g, (cudaStream_t)cuda_stream);
+    return path_fields_run(c, 1, s, cw, d_g, (cudaStream_t)cuda_stream);
 }
 
 extern "C" int isdf_frontend_path_fields_device(isdf_ctx *c, int S, const double *starts, const isdf_frontpath_params *prm, double *d_g,
                                                 void *cuda_stream) {
     if (!starts || !d_g || S < 1) return fail(ISDF_ERR_INVALID, "bad argument");
     if (S > 65535) return fail(ISDF_ERR_INVALID, "S must be at most 65535");
-    if (int r = path_args_check(c, prm)) return r;
+    double cw = 1.0;
+    if (int r = path_args_check(c, prm, &cw)) return r;
     if (set_device(c)) return ISDF_ERR_CUDA;
     std::vector<int> src((size_t)3 * S);
     for (int s = 0; s < S; s++)
         if (int r = path_voxel(c->map.grid, starts + 3 * (size_t)s, &src[3 * (size_t)s], "starts[" + std::to_string(s) + "]")) return r;
-    return path_fields_run(c, S, src.data(), d_g, (cudaStream_t)cuda_stream);
+    return path_fields_run(c, S, src.data(), cw, d_g, (cudaStream_t)cuda_stream);
 }
 
 extern "C" int isdf_frontend_path_info(isdf_ctx *c, isdf_frontpath_info *out) {
@@ -4536,7 +4585,9 @@ static int plan_check(isdf_ctx *c, const isdf_plan_params *p, double *r_cert) {
     if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
     if (c->world > 1) return fail(ISDF_ERR_UNSUPPORTED, "the planning step is not sharded: call it on a context with isdf_set_shard(ctx, 0, 1)");
     if (p->reserved_ != 0) return fail(ISDF_ERR_INVALID, "reserved_ must be 0");
-    if (p->flags & ~(ISDF_PLAN_CERTIFY | ISDF_PLAN_DYNAMICS)) return fail(ISDF_ERR_INVALID, "unknown flags");
+    if (p->flags & ~(ISDF_PLAN_CERTIFY | ISDF_PLAN_DYNAMICS | ISDF_PLAN_KNOWN_PREFIX)) return fail(ISDF_ERR_INVALID, "unknown flags");
+    double cw;
+    if (int r = frontpath_params_check(&p->frontpath, &cw)) return r;
     if (!(std::isfinite(p->parlength) && p->parlength > 0.0)) return fail(ISDF_ERR_INVALID, "parlength must be finite and positive");
     if (!(std::isfinite(p->half_extent) && p->half_extent >= 0.0)) return fail(ISDF_ERR_INVALID, "half_extent must be finite and >= 0");
     for (double v : {p->offset[0], p->offset[1], p->offset[2], p->rho}) if (!std::isfinite(v)) return fail(ISDF_ERR_INVALID, "offset and rho must be finite");
@@ -4618,7 +4669,8 @@ static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const
     };
     // 1. front end
     std::vector<int> off;
-    if (int r = timed(info.frontend_ms, [&] { return path_run(c, B, starts, sstride, goals, max_fields, 0x7fffffff, off, st); })) return r;
+    const double cw = 1.0 + p->frontpath.unknown_weight;   // checked by plan_check
+    if (int r = timed(info.frontend_ms, [&] { return path_run(c, B, starts, sstride, goals, cw, max_fields, 0x7fffffff, off, st); })) return r;
     const int nodes = off[B];
     const int32_t *d_off = c->fp.d_off.p;
     const double *d_xyz = c->fp.d_xyz.p;
@@ -4716,10 +4768,24 @@ static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const
             }
             if (int r = copy_segments(c, seg, st)) return r;
             if (int r = plan_upload(c, c->gat.d_wpoff, gwo, st)) return r;
+            std::vector<int> bplan(Bp);   // back-end instance k's plan
+            for (int k = 0; k < Bp; k++) bplan[k] = idx[ok[k]];
+            if (int r = plan_upload(c, z.d_bplan, bplan, st)) return r;
+            const int *d_krows = nullptr;   // ISDF_PLAN_KNOWN_PREFIX: each instance's rows inside its path's known prefix
+            if (p->flags & ISDF_PLAN_KNOWN_PREFIX) {
+                CU_TRY(z.d_krows.ensure(Bp));
+                k_plan_known_rows<<<(unsigned)((Bp + 127) / 128), 128, 0, st>>>(Bp, z.d_bplan.p, d_off, c->fp.d_nodes.p,
+                                                                                c->known.have ? c->known.d_known.p : nullptr, c->map.grid,
+                                                                                c->wps.d_gap.p, z.d_N.p, z.d_krows.p);
+                c->stats.kernel_launches++;
+                CU_TRY(cudaGetLastError());
+                d_krows = z.d_krows.p;
+            }
             std::vector<int> pto;
             long long tot = 0;
             if (int r = timed(info.gather_ms, [&] {
-                    if (int rr = gather_batch_run(c, Bp, gwo.data(), c->gat.d_wpoff.p, c->gat.d_wp.p, p->half_extent, p->offset, 0x7fffffffll, pto, &tot, st)) return rr;
+                    if (int rr = gather_batch_run(c, Bp, gwo.data(), c->gat.d_wpoff.p, c->gat.d_wp.p, p->half_extent, p->offset, d_krows, 0x7fffffffll,
+                                                  pto, &tot, st)) return rr;
                     return gather_set_points(c, Bp, pto, tot, st);
                 })) return r;
             for (int k = 0; k < Bp; k++) { row[idx[ok[k]]].points = pto[k + 1] - pto[k]; row[idx[ok[k]]].k = k; }
@@ -4735,9 +4801,6 @@ static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const
             if (int r = callback_batch_check(c, true, Bp, 0, boff.data(), &BL)) return r;
             if (int r = ragged_upload(c->batch.d_off, boff.data(), st, &BL)) return r;
             count_copy(c, cudaMemcpyHostToDevice, sizeof(int) * (2 * (size_t)Bp + 2));
-            std::vector<int> bplan(Bp);
-            for (int k = 0; k < Bp; k++) bplan[k] = idx[ok[k]];
-            if (int r = plan_upload(c, z.d_bplan, bplan, st)) return r;
             CU_TRY(z.d_bbc.ensure((size_t)18 * Bp));
             k_plan_bc<<<(unsigned)((Bp + 127) / 128), 128, 0, st>>>(Bp, z.d_bplan.p, d_off, d_xyz, d_heads, z.d_bbc.p);
             c->stats.kernel_launches++;

@@ -14,6 +14,9 @@
 //                   (order-preserving, so the result does not depend on the order, nor on which sources share the launch); improved voxels
 //                   form the next frontier. Rounds are launched in chunks; a CTA whose source's frontier is empty returns at once, and the
 //                   host reads one aggregate flag (some source has a frontier) per chunk.
+//   WEIGHTED        the relaxations and the walk are templated on the unknown-voxel surcharge (isdf_frontpath_params.unknown_weight):
+//                   the weighted instances multiply the edge into a voxel that is not KNOWN by 1 + unknown_weight (fp_weight); weight 0
+//                   launches the unweighted instances, whose code is the surcharge-free kernels' own
 //   k_fp_walk       one warp per target: lane l tests offset l of the parent rule on the target's field slice, the first lane of the
 //                   ballot is the parent. Pass 0 counts the path, pass 1 writes its voxel indices into scratch.
 //   k_fp_place      one warp per path: from scratch to its place in pair order, with the cube centres
@@ -55,11 +58,26 @@ struct PathArgs {
     const uint32_t *colliding;   // 4 per node (k_fp_node_masks)
 };
 
+// the surcharge on unknown voxels, read by the WEIGHTED instances only. A parameter after the kernels' own, so that the unweighted
+// instances keep the surcharge-free kernels' parameter offsets and code.
+struct FpSurcharge {
+    const uint32_t *known;       // the map's KNOWN bits, grid.bits' layout (NULL: nothing is known)
+    double cw;                   // 1 + unknown_weight: the factor on an edge into a voxel that is not known
+};
+
 __device__ __forceinline__ bool fp_trav(const PathArgs &P, int x, int y, int z) {
     return (__ldg(P.trav + ((size_t)x * P.grid.Y + y) * P.grid.Zw + (z >> 5)) >> (z & 31)) & 1u;
 }
 // edge cost sqrt(i*i + j*j + k*k) of front_end_Astar.hpp:230 (IEEE sqrt: correctly rounded)
 __device__ __forceinline__ double fp_edge(int n) { return sqrt((double)n); }
+// the edge into v = (x, y, z): fp_edge, times cw when v is not known (one rounded product; the unit is compiled with -fmad=false, so the
+// sum g(u) + w is not contracted either)
+template <bool WEIGHTED>
+__device__ __forceinline__ double fp_weight(const PathArgs &P, const FpSurcharge &U, int n, int x, int y, int z) {
+    if (!WEIGHTED) return fp_edge(n);
+    const bool known = U.known && ((__ldg(U.known + ((size_t)x * P.grid.Y + y) * P.grid.Zw + (z >> 5)) >> (z & 31)) & 1u);
+    return fp_edge(n) * (known ? 1.0 : U.cw);
+}
 
 __global__ void k_fp_init(const __grid_constant__ PathArgs P) {
     const int s = blockIdx.y;
@@ -77,8 +95,11 @@ __global__ void k_fp_init(const __grid_constant__ PathArgs P) {
     }
 }
 
-// one source (S = 1): its flag ring is also the aggregate one (P.any == P.flags)
-__global__ void __launch_bounds__(256) k_fp_relax(const __grid_constant__ PathArgs P, int r) {
+// one source (S = 1): its flag ring is also the aggregate one (P.any == P.flags). WEIGHTED: the unknown-voxel surcharge (fp_weight).
+// The weighted instances ask for one resident CTA (minBlocks 1): left to itself ptxas held them to 64 registers with 28 bytes of spills;
+// with it they take 76 and spill nothing. minBlocks 0 leaves the unweighted instances' code exactly as it was (64 and 78 registers).
+template <bool WEIGHTED>
+__global__ void __launch_bounds__(256, WEIGHTED ? 1 : 0) k_fp_relax(const __grid_constant__ PathArgs P, int r, const FpSurcharge U) {
     // the flag of round r + 2 is cleared before anyone can set it (round r + 1 sets it); round r sets the flag of round r + 1
     if (blockIdx.x == 0 && threadIdx.x == 0) P.flags[(r + 2) % FP_FLAG_RING] = 0u;
     if (*(volatile unsigned *)(P.flags + r % FP_FLAG_RING) == 0u) return;
@@ -106,7 +127,7 @@ __global__ void __launch_bounds__(256) k_fp_relax(const __grid_constant__ PathAr
                     for (int dk = -1; dk <= 1; dk++) {
                         const int z = iz + dk;
                         if (z < 0 || z >= G.Z || (di == 0 && dj == 0 && dk == 0) || !fp_trav(P, x, y, z)) continue;
-                        const unsigned long long cand = (unsigned long long)__double_as_longlong(gu + fp_edge(di * di + dj * dj + dk * dk));
+                        const unsigned long long cand = (unsigned long long)__double_as_longlong(gu + fp_weight<WEIGHTED>(P, U, di * di + dj * dj + dk * dk, x, y, z));
                         unsigned long long *gv = P.g + ((size_t)x * G.Y + y) * G.Z + z;
                         if (cand >= __ldcg(gv)) continue;
                         if (cand < atomicMin(gv, cand)) {
@@ -123,7 +144,8 @@ __global__ void __launch_bounds__(256) k_fp_relax(const __grid_constant__ PathAr
 
 // S > 1 (grid.y = S). One source keeps k_fp_relax above: this form needs the per-source offsets and the aggregate flag, and at S = 1 it
 // took 553 ms against the single-source kernel's 530-536 ms for the bench_frontpath.py field at 512^3 on an H100 (78 registers against 64)
-__global__ void __launch_bounds__(256) k_fp_relax_multi(const __grid_constant__ PathArgs P, int r) {
+template <bool WEIGHTED>
+__global__ void __launch_bounds__(256, WEIGHTED ? 1 : 0) k_fp_relax_multi(const __grid_constant__ PathArgs P, int r, const FpSurcharge U) {
     const int s = blockIdx.y;
     unsigned *flags = P.flags + (size_t)s * FP_FLAG_RING;
     // the flags of round r + 2 are cleared before anyone can set them (round r + 1 sets them); round r sets those of round r + 1
@@ -159,7 +181,7 @@ __global__ void __launch_bounds__(256) k_fp_relax_multi(const __grid_constant__ 
                     for (int dk = -1; dk <= 1; dk++) {
                         const int z = iz + dk;
                         if (z < 0 || z >= G.Z || (di == 0 && dj == 0 && dk == 0) || !fp_trav(P, x, y, z)) continue;
-                        const unsigned long long cand = (unsigned long long)__double_as_longlong(gu + fp_edge(di * di + dj * dj + dk * dk));
+                        const unsigned long long cand = (unsigned long long)__double_as_longlong(gu + fp_weight<WEIGHTED>(P, U, di * di + dj * dj + dk * dk, x, y, z));
                         unsigned long long *gv = g + ((size_t)x * G.Y + y) * G.Z + z;
                         if (cand >= __ldcg(gv)) continue;
                         if (cand < atomicMin(gv, cand)) {
@@ -178,15 +200,18 @@ __global__ void __launch_bounds__(256) k_fp_relax_multi(const __grid_constant__ 
 }
 
 // parent rule on field g: among the 26 neighbours u of v with g(u) + w(u, v) == g(v), the first in the reference's offset order (i, j,
-// k = -1..1, i outermost; lane = 9 (i + 1) + 3 (j + 1) + (k + 1)). The whole warp calls this.
-__device__ __forceinline__ bool fp_parent(const DevGrid &G, const unsigned long long *g, int &x, int &y, int &z, int lane) {
+// k = -1..1, i outermost; lane = 9 (i + 1) + 3 (j + 1) + (k + 1)). w is v's edge weight: WEIGHTED reads the known bit of v, the node the
+// walk steps from. The whole warp calls this.
+template <bool WEIGHTED>
+__device__ __forceinline__ bool fp_parent(const PathArgs &P, const FpSurcharge &U, const unsigned long long *g, int &x, int &y, int &z, int lane) {
+    const DevGrid &G = P.grid;
     const double gv = __longlong_as_double((long long)g[((size_t)x * G.Y + y) * G.Z + z]);
     const int di = lane / 9 - 1, dj = (lane / 3) % 3 - 1, dk = lane % 3 - 1;
     const int ux = x + di, uy = y + dj, uz = z + dk;
     bool ok = false;
     if (lane < 27 && lane != 13 && ux >= 0 && ux < G.X && uy >= 0 && uy < G.Y && uz >= 0 && uz < G.Z) {
         const unsigned long long gu = g[((size_t)ux * G.Y + uy) * G.Z + uz];
-        ok = gu != FP_INF && __longlong_as_double((long long)gu) + fp_edge(di * di + dj * dj + dk * dk) == gv;
+        ok = gu != FP_INF && __longlong_as_double((long long)gu) + fp_weight<WEIGHTED>(P, U, di * di + dj * dj + dk * dk, x, y, z) == gv;
     }
     const unsigned b = __ballot_sync(0xffffffffu, ok);
     if (!b) return false;
@@ -195,7 +220,8 @@ __device__ __forceinline__ bool fp_parent(const DevGrid &G, const unsigned long 
     return true;
 }
 
-__global__ void __launch_bounds__(128) k_fp_walk(const __grid_constant__ PathArgs P, int pass) {
+template <bool WEIGHTED>
+__global__ void __launch_bounds__(128) k_fp_walk(const __grid_constant__ PathArgs P, int pass, const FpSurcharge U) {
     const int t = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
     if (t >= P.nt) return;   // whole warps
     const DevGrid &G = P.grid;
@@ -221,7 +247,7 @@ __global__ void __launch_bounds__(128) k_fp_walk(const __grid_constant__ PathArg
     const int last = (pass == 1) ? P.off[t + 1] - 1 : 0;
     if (pass == 1) put(last, x, y, z);
     while (!(x == sx && y == sy && z == sz) && n < cap) {
-        if (!fp_parent(G, g, x, y, z, lane)) break;
+        if (!fp_parent<WEIGHTED>(P, U, g, x, y, z, lane)) break;
         if (pass == 1) put(last - (int)n, x, y, z);
         n++;
     }

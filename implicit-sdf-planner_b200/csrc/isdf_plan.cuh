@@ -50,6 +50,25 @@ __global__ void k_plan_bc(int n, const int *plan, const int32_t *path_off, const
     for (int k = 0; k < 9; k++) { h[k] = heads ? heads[9 * (size_t)b + k] : (k < 3 ? f[k] : 0.0); t[k] = k < 3 ? l[k] : 0.0; }
 }
 
+// ISDF_PLAN_KNOWN_PREFIX: the rows of back-end instance i (plan plan[i]) that lie inside its path's known prefix. k* = the first path node
+// whose voxel is not known (the path length when every node is; 0 when nothing is known: known NULL); waypoint row j is path node
+// (j + 1) gap (k_wp_write), so the known rows are the j < pieces - 1 with (j + 1) gap < k*.
+__global__ void k_plan_known_rows(int n, const int *plan, const int32_t *path_off, const int *nodes, const uint32_t *known, const DevGrid G,
+                                  const int32_t *gap, const int32_t *pieces, int *rows) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int b = plan[i];
+    long long ks = 0;
+    if (known)
+        for (long long m = path_off[b]; m < path_off[b + 1]; m++, ks++) {
+            const int *v = nodes + 3 * m;
+            if (!((known[((size_t)v[0] * G.Y + v[1]) * G.Zw + (v[2] >> 5)] >> (v[2] & 31)) & 1u)) break;
+        }
+    int r = 0;
+    while (r < pieces[b] - 1 && (long long)(r + 1) * gap[b] < ks) r++;
+    rows[i] = r;
+}
+
 // isdf_plan_states_device's check of the heads' v and a: *bad = the least b whose v or a has a non-finite entry (left as set when none)
 __global__ void k_plan_heads_check(int B, const double *heads, int *bad) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;

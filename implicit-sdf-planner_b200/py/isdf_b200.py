@@ -54,12 +54,12 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_map_fuse_cloud", "isdf_map_fuse_cloud_device", "isdf_plan_states", "isdf_plan_states_device",
                "isdf_trajectory_shift", "isdf_trajectory_shift_device", "isdf_brake_default_params", "isdf_trajectory_brake",
                "isdf_trajectory_brake_device", "isdf_map_observe", "isdf_map_observe_device", "isdf_map_mark_known",
-               "isdf_get_map_known_u8", "isdf_set_unknown_policy", "isdf_get_unknown_policy"]
+               "isdf_get_map_known_u8", "isdf_set_unknown_policy", "isdf_get_unknown_policy", "isdf_gather_obstacle_points_batch_known"]
 WORLD_KINDS = dict(globalmap=1, perlin=2, boxes=3)   # isdf_world_kind
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
 DYN_QUANTITIES = ["speed", "acceleration", "body_rate", "tilt", "thrust"]   # q of isdf_dynamics_summary; mask bit 5: the thrust minimum
-PLAN_CERTIFY, PLAN_DYNAMICS = 1, 2                                             # isdf_plan_params.flags
+PLAN_CERTIFY, PLAN_DYNAMICS, PLAN_KNOWN_PREFIX = 1, 2, 8                       # isdf_plan_params.flags
 PLAN_FAILED, NO_PATH, TOO_LONG, MIDEND_FAILED, OPTIMISED = -1, 0, 1, 2, 3      # isdf_plan_result.stage
 ESDF_FIELDS = dict(positive=0, negative=1, signed=2)                            # isdf_esdf_field
 STATE_DOUBLES = 20                                                               # ISDF_STATE_DOUBLES: pos vel acc jer quat(w,x,y,z) omg thr
@@ -359,10 +359,21 @@ def decode_brake_summaries(raw):
     return [BrakeSummary.from_buffer_copy(r.tobytes()).as_dict() for r in b]
 
 
+class FrontPathParams(C.Structure):
+    """isdf_frontpath_params"""
+    _fields_ = [("unknown_weight", C.c_double), ("reserved_", C.c_int32 * 2)]
+
+
+def _fpp(unknown_weight):
+    """the front-end parameters of a binding: NULL (the defaults) for None, else an isdf_frontpath_params with that unknown_weight"""
+    return None if unknown_weight is None else C.byref(FrontPathParams(unknown_weight=float(unknown_weight)))
+
+
 class PlanParams(C.Structure):
     """isdf_plan_params"""
     _fields_ = [("parlength", C.c_double), ("half_extent", C.c_double), ("offset", C.c_double * 3), ("rho", C.c_double), ("midend", MidendParams),
-                ("backend", LbfgsParams), ("flags", C.c_int32), ("reserved_", C.c_int32), ("certify", CertifyParams), ("dynamics", DynamicsParams)]
+                ("backend", LbfgsParams), ("flags", C.c_int32), ("reserved_", C.c_int32), ("certify", CertifyParams), ("dynamics", DynamicsParams),
+                ("frontpath", FrontPathParams)]
 
 
 class PlanResult(C.Structure):
@@ -462,11 +473,6 @@ class ObserveInfo(C.Structure):
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}
-
-
-class FrontPathParams(C.Structure):
-    """isdf_frontpath_params"""
-    _fields_ = [("reserved_", C.c_int32 * 4)]
 
 
 class FrontPathInfo(C.Structure):
@@ -598,6 +604,7 @@ def load_library(path=None):
     lib.isdf_midend_batch.argtypes = [vp, C.c_int, C.c_int, dp, dp, C.c_int, mpp, dp, dp, dp, dp, dp, ip, ip, ip, ip]
     lib.isdf_midend_batch_device.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_int, mpp, vp, vp, vp, vp, vp, vp, vp, vp, ip, vp]
     lib.isdf_gather_obstacle_points_batch.argtypes = [vp, C.c_int, ip, dp, C.c_double, dp, C.c_int64, dp, ip, C.c_int]
+    lib.isdf_gather_obstacle_points_batch_known.argtypes = [vp, C.c_int, ip, dp, C.c_double, dp, ip, C.c_int64, dp, ip, C.c_int]
     lib.isdf_plan_default_params.argtypes = [vp, C.POINTER(PlanParams)]
     lib.isdf_plan_batch.argtypes = [vp, dp, C.c_int, dp, C.POINTER(PlanParams), C.c_int, ip, dp, C.c_int, ip, dp, dp, C.POINTER(PlanResult),
                                     C.POINTER(CertifySummary), C.POINTER(DynamicsSummary)]
@@ -1143,9 +1150,10 @@ class Evaluator:
             self.n_points = n.value
         return out[:min(n.value, cap)].copy(), n.value
 
-    def gather_obstacle_points_batch(self, waypoints, half, offset=(0.0, 0.0, 0.0), set_as_points=False, cap=None):
+    def gather_obstacle_points_batch(self, waypoints, half, offset=(0.0, 0.0, 0.0), set_as_points=False, cap=None, known_rows=None):
         """isdf_gather_obstacle_points_batch: one obstacle list per plan (waypoints: list of (n_b, 3) arrays, n_b may be 0) -> list of (P_b, 3)
-        arrays. cap = None: a first guess, repeated once with the reported total when the lists are longer."""
+        arrays. cap = None: a first guess, repeated once with the reported total when the lists are longer. known_rows (B ints, or None):
+        isdf_gather_obstacle_points_batch_known, plan b's first known_rows[b] rows reading the blocked grid (occupied or not known)."""
         B = len(waypoints)
         wo = np.zeros(B + 1, dtype=np.int32)
         for b, w in enumerate(waypoints):
@@ -1156,8 +1164,13 @@ class Evaluator:
         cap = int(cap) if cap is not None else max(1024, 64 * int(wo[B]))
         for attempt in range(2):
             out, pt = np.zeros((max(cap, 1), 3)), np.zeros(B + 1, dtype=np.int32)
-            r = self.lib.isdf_gather_obstacle_points_batch(self.h, B, wo.ctypes.data_as(ip), _dp(wp), float(half), _dp(off), cap, _dp(out),
-                                                           pt.ctypes.data_as(ip), int(set_as_points))
+            if known_rows is None:
+                r = self.lib.isdf_gather_obstacle_points_batch(self.h, B, wo.ctypes.data_as(ip), _dp(wp), float(half), _dp(off), cap, _dp(out),
+                                                               pt.ctypes.data_as(ip), int(set_as_points))
+            else:
+                kr = np.ascontiguousarray(known_rows, dtype=np.int32).reshape(B)
+                r = self.lib.isdf_gather_obstacle_points_batch_known(self.h, B, wo.ctypes.data_as(ip), _dp(wp), float(half), _dp(off),
+                                                                     kr.ctypes.data_as(ip), cap, _dp(out), pt.ctypes.data_as(ip), int(set_as_points))
             if r == -1 and attempt == 0 and pt[B] > cap:
                 cap = int(pt[B])
                 continue
@@ -1434,8 +1447,10 @@ class Evaluator:
     # ---- planning step: generateTraj for one start and B goals (see include/isdf.h) ----
     def plan_params(self, **kw):
         """isdf_plan_default_params for this context, then overrides: parlength, half_extent, offset, rho, flags, reserved_, certify,
-        dynamics, midend (an isdf_midend_params) and backend (an isdf_lbfgs_params) by name; midend_<field> / backend_<field> set one field
-        of the nested blocks (midend_init_time=200.0, backend_max_iterations=50, midend_max_rounds=1, ...)"""
+        dynamics, frontpath, midend (an isdf_midend_params) and backend (an isdf_lbfgs_params) by name; midend_<field> / backend_<field> set
+        one field of the nested blocks (midend_init_time=200.0, backend_max_iterations=50, midend_max_rounds=1, ...); unknown_weight sets
+        frontpath.unknown_weight (the front end's surcharge on unknown voxels; pair it with flags including PLAN_KNOWN_PREFIX to keep the
+        back end inside the known prefix, DESIGN §3.23)"""
         p = PlanParams()
         self._check(self.lib.isdf_plan_default_params(self.h, C.byref(p)))
         lb = {n for n, _ in LbfgsParams._fields_}
@@ -1447,6 +1462,8 @@ class Evaluator:
                 setattr(p.midend.lbfgs if f in lb and f != "reserved_" else p.midend, f, v)
             elif k.startswith("backend_"):
                 setattr(p.backend, k[len("backend_"):], v)
+            elif k == "unknown_weight":
+                p.frontpath.unknown_weight = float(v)
             elif k in {n for n, _ in PlanParams._fields_}:
                 setattr(p, k, v)
             else:
@@ -1847,7 +1864,10 @@ class Evaluator:
                        second call with brake_params' margin); a BRAKED stop replaces the trajectory, flown as CERTIFIED (action NAV_COMMITTED) and marked as a commit;
                        vehicles without an accepted plan or a commit take the fallback as before, except that a vehicle still holding a
                        CERTIFIED remaining trajectory (a commit) keeps it. A commit that runs out away from the goal holds the vehicle.
-        The result then also has commits (B,) numpy, and times an "observe" stage.
+        The result then also has commits (B,) numpy, and times an "observe" stage. To plan through what has been seen, pass plan_params
+        with unknown_weight > 0 and PLAN_KNOWN_PREFIX in flags (plan_params(unknown_weight=W, flags=PLAN_CERTIFY | PLAN_KNOWN_PREFIX)):
+        every replan then prefers routes through known voxels and keeps the back end out of unseen space along its known prefix
+        (DESIGN §3.23); the loop itself is unchanged.
         Vehicles share the map, so one vehicle's run depends on what the others sensed; with B = 1 it is that vehicle's alone. The world
         waits while the planner runs (no planning latency in simulated time). Within a round only per-vehicle values (stages, verdicts,
         counts, piece totals, positions of heads) cross to the host; points, pieces and logs stay on the device.
@@ -2483,9 +2503,11 @@ class Evaluator:
         info = self.map_info()
         return 4 * sum(info["dims"])
 
-    def frontend_path_batch(self, start, goals, cap=None):
+    def frontend_path_batch(self, start, goals, cap=None, unknown_weight=None):
         """one start, B goals -> dict(paths: list of (n_b, 3) cube centres, roll_pitch: list of (n_b, 2) degrees, offsets (B + 1),
-        costs (B), found (B) bool). cap = None: a first guess, repeated once with the exact total when the paths are longer."""
+        costs (B), found (B) bool). cap = None: a first guess, repeated once with the exact total when the paths are longer.
+        unknown_weight (every front-end binding): None passes NULL params; a number passes isdf_frontpath_params with that surcharge on
+        unknown voxels (0 is the NULL field bit for bit)."""
         st = _f64(start).reshape(3)
         goals = _f64(goals).reshape(-1, 3)
         B = goals.shape[0]
@@ -2493,7 +2515,7 @@ class Evaluator:
         for attempt in range(2):
             xyz, rp = np.zeros((max(cap, 1), 3)), np.zeros((max(cap, 1), 2))
             off, cost, found = np.zeros(B + 1, dtype=np.int32), np.zeros(B), np.zeros(B, dtype=np.uint8)
-            r = self.lib.isdf_frontend_path_batch(self.h, _dp(st), B, _dp(goals), None, cap, _dp(xyz), _dp(rp),
+            r = self.lib.isdf_frontend_path_batch(self.h, _dp(st), B, _dp(goals), _fpp(unknown_weight), cap, _dp(xyz), _dp(rp),
                                                   off.ctypes.data_as(C.POINTER(C.c_int32)), _dp(cost), found.ctypes.data_as(C.POINTER(C.c_uint8)))
             if r == -1 and attempt == 0 and off[B] > cap:
                 cap = int(off[B])
@@ -2504,7 +2526,7 @@ class Evaluator:
         return dict(paths=[xyz[off[b]:off[b + 1]] for b in range(B)], roll_pitch=[rp[off[b]:off[b + 1]] for b in range(B)],
                     xyz=xyz[:n], rp=rp[:n], offsets=off, costs=cost, found=found.astype(bool))
 
-    def frontend_path_pairs(self, starts, goals, cap=None, max_fields=0):
+    def frontend_path_pairs(self, starts, goals, cap=None, max_fields=0, unknown_weight=None):
         """B (start, goal) pairs, start b with goal b -> what frontend_path_batch returns, in pair order (isdf_frontend_path_pairs).
         max_fields: the fields of distinct start voxels held at once (0: the library's 4 GiB budget)"""
         sts, goals = _f64(starts).reshape(-1, 3), _f64(goals).reshape(-1, 3)
@@ -2515,7 +2537,7 @@ class Evaluator:
         for attempt in range(2):
             xyz, rp = np.zeros((max(cap, 1), 3)), np.zeros((max(cap, 1), 2))
             off, cost, found = np.zeros(B + 1, dtype=np.int32), np.zeros(B), np.zeros(B, dtype=np.uint8)
-            r = self.lib.isdf_frontend_path_pairs(self.h, B, _dp(sts), _dp(goals), None, int(max_fields), cap, _dp(xyz), _dp(rp),
+            r = self.lib.isdf_frontend_path_pairs(self.h, B, _dp(sts), _dp(goals), _fpp(unknown_weight), int(max_fields), cap, _dp(xyz), _dp(rp),
                                                   off.ctypes.data_as(C.POINTER(C.c_int32)), _dp(cost), found.ctypes.data_as(C.POINTER(C.c_uint8)))
             if r == -1 and attempt == 0 and off[B] > cap:
                 cap = int(off[B])
@@ -2536,14 +2558,14 @@ class Evaluator:
                                               off.ctypes.data_as(C.POINTER(C.c_int32)), _dp(cost), found.ctypes.data_as(C.POINTER(C.c_uint8)))
         return r, off
 
-    def frontend_path(self, start, goal, cap=None):
+    def frontend_path(self, start, goal, cap=None, unknown_weight=None):
         """-> (path (n, 3), roll_pitch (n, 2), cost, found), through isdf_frontend_path"""
         st, gl = _f64(start).reshape(3), _f64(goal).reshape(3)
         cap = self._path_cap(cap)
         for attempt in range(2):
             xyz, rp = np.zeros((max(cap, 1), 3)), np.zeros((max(cap, 1), 2))
             n, cost, found = C.c_int32(0), C.c_double(0), C.c_uint8(0)
-            r = self.lib.isdf_frontend_path(self.h, _dp(st), _dp(gl), None, cap, _dp(xyz), _dp(rp), C.byref(n), C.byref(cost), C.byref(found))
+            r = self.lib.isdf_frontend_path(self.h, _dp(st), _dp(gl), _fpp(unknown_weight), cap, _dp(xyz), _dp(rp), C.byref(n), C.byref(cost), C.byref(found))
             if r == -1 and attempt == 0 and n.value > cap:
                 cap = n.value
                 continue
@@ -2559,22 +2581,23 @@ class Evaluator:
         r = self.lib.isdf_frontend_path(self.h, _dp(st), _dp(gl), None, int(cap), _dp(xyz), _dp(rp), C.byref(n), C.byref(cost), C.byref(found))
         return r, n.value
 
-    def frontend_path_batch_device(self, start, B, d_goals, cap, d_xyz, d_rp, d_offsets, d_costs, d_found, stream=None):
+    def frontend_path_batch_device(self, start, B, d_goals, cap, d_xyz, d_rp, d_offsets, d_costs, d_found, stream=None, unknown_weight=None):
         st = _f64(start).reshape(3)
-        self._check(self.lib.isdf_frontend_path_batch_device(self.h, _dp(st), B, d_goals, None, cap, d_xyz, d_rp, d_offsets, d_costs, d_found, stream))
+        self._check(self.lib.isdf_frontend_path_batch_device(self.h, _dp(st), B, d_goals, _fpp(unknown_weight), cap, d_xyz, d_rp, d_offsets, d_costs, d_found, stream))
 
-    def frontend_path_field_device(self, start, d_g, stream=None):
+    def frontend_path_field_device(self, start, d_g, stream=None, unknown_weight=None):
         st = _f64(start).reshape(3)
-        self._check(self.lib.isdf_frontend_path_field_device(self.h, _dp(st), None, d_g, stream))
+        self._check(self.lib.isdf_frontend_path_field_device(self.h, _dp(st), _fpp(unknown_weight), d_g, stream))
 
-    def frontend_path_pairs_device(self, B, d_starts, d_goals, cap, d_xyz, d_rp, d_offsets, d_costs, d_found, stream=None, max_fields=0):
-        self._check(self.lib.isdf_frontend_path_pairs_device(self.h, int(B), d_starts, d_goals, None, int(max_fields), int(cap), d_xyz, d_rp,
+    def frontend_path_pairs_device(self, B, d_starts, d_goals, cap, d_xyz, d_rp, d_offsets, d_costs, d_found, stream=None, max_fields=0,
+                                   unknown_weight=None):
+        self._check(self.lib.isdf_frontend_path_pairs_device(self.h, int(B), d_starts, d_goals, _fpp(unknown_weight), int(max_fields), int(cap), d_xyz, d_rp,
                                                              d_offsets, d_costs, d_found, stream))
 
-    def frontend_path_fields_device(self, starts, d_g, stream=None):
+    def frontend_path_fields_device(self, starts, d_g, stream=None, unknown_weight=None):
         """the fields from S starts (S, 3) in one relaxation into d_g (a raw device pointer to S*X*Y*Z float64), field s at d_g + s*X*Y*Z"""
         sts = _f64(starts).reshape(-1, 3)
-        self._check(self.lib.isdf_frontend_path_fields_device(self.h, sts.shape[0], _dp(sts), None, d_g, stream))
+        self._check(self.lib.isdf_frontend_path_fields_device(self.h, sts.shape[0], _dp(sts), _fpp(unknown_weight), d_g, stream))
 
     def frontend_path_info(self):
         out = FrontPathInfo()

@@ -241,7 +241,8 @@ int isdf_get_map_f64(isdf_ctx *ctx, double *grid_map, int64_t n);
  * isdf_set_unknown_policy: ISDF_UNKNOWN_FREE (the default) leaves the clearance family as it was, whatever is known;
  *   ISDF_UNKNOWN_OCCUPIED makes every call that reads candidate voxels for a clearance or a certificate (isdf_trajectory_clearance,
  *   isdf_pose_clearance, isdf_trajectory_certify, the certificate of isdf_trajectory_brake and of ISDF_PLAN_CERTIFY) read the BLOCKED grid
- *   occ | (~known within the map) instead. The front end, mid-end, back-end cost, obstacle gathers and distance field keep reading occupancy.
+ *   occ | (~known within the map) instead. The front end, mid-end, back-end cost, obstacle gathers and distance field keep reading occupancy;
+ *   planning that prefers known space is asked for separately (isdf_frontpath_params.unknown_weight, ISDF_PLAN_KNOWN_PREFIX, DESIGN §3.23).
  *   The blocked grid is rebuilt (one launch, and a wait on the calling stream) by the first such call after a map, fuse, observe or mark
  *   call. Voxels outside the map stay outside every candidate set. The policy is context state; it survives map changes. */
 typedef enum isdf_unknown_policy { ISDF_UNKNOWN_FREE = 0, ISDF_UNKNOWN_OCCUPIED = 1 } isdf_unknown_policy;
@@ -325,6 +326,17 @@ int isdf_gather_obstacle_points(isdf_ctx *ctx, const double *waypoints, int nQ, 
  * cap < 0, or a total beyond 2^31 - 1; ISDF_ERR_STATE without a map. The call counts its launches in isdf_stats.kernel_launches. */
 int isdf_gather_obstacle_points_batch(isdf_ctx *ctx, int B, const int32_t *wp_off, const double *waypoints, double half_extent,
                                       const double *offset, int64_t cap, double *out_points, int32_t *pt_off, int set_as_points);
+/* The same with a per-plan known prefix (DESIGN §3.23). known_rows (B, host; NULL = isdf_gather_obstacle_points_batch exactly): plan b's
+ *   rows j < known_rows[b] (its first known_rows[b] waypoints) take their voxels from the BLOCKED grid, occ | (~known within the map) of
+ *   isdf_set_unknown_policy, instead of the occupancy grid; its other rows read occupancy as before. A value past the plan's row count
+ *   covers every row. De-duplication is unchanged: a voxel belongs to the first box of its plan that includes it, each box tested on its
+ *   own row's grid. Because known rows come first and an occupied voxel is blocked, testing every earlier box on the current row's grid gives
+ *   the same answer, so the lists stay independent of any processing order. The blocked grid is rebuilt (one launch and a wait) when a map,
+ *   fuse, observe or mark call made it stale, whatever the unknown policy. Errors: those above, and ISDF_ERR_INVALID for a negative
+ *   known_rows entry. */
+int isdf_gather_obstacle_points_batch_known(isdf_ctx *ctx, int B, const int32_t *wp_off, const double *waypoints, double half_extent,
+                                            const double *offset, const int32_t *known_rows, int64_t cap, double *out_points,
+                                            int32_t *pt_off, int set_as_points);
 
 /* ---- discrete collision term: addTimeIntPenaltyParallel (hpp:432-554) with grad_cost_p (hpp:766-824) wired in */
 /* ACCUMULATES into *cost, gradC (6N x 3 col-major), gradT (N) exactly like the reference's reference arguments. */
@@ -907,6 +919,16 @@ int isdf_frontend_check_batch(isdf_ctx *ctx, int n, const int32_t *ind, const do
  *                  is not an error: found = 0, cost +inf and a one-node path (the start).
  *   Attitudes      node 0 has (roll, pitch) = (0, 0) (GridNode's defaults); node m + 1 has checkKernelValue(attitude of node m, node m + 1):
  *                  isdf_frontend_check_batch applied as a chain along the returned path.
+ *   Surcharge on unknown voxels (params->unknown_weight, finite and >= 0; 0, or NULL params, is the definition above bit for bit)
+ *                  c = 1 + unknown_weight, once, in FP64. The edge into v costs w(u, v) = sqrt((double)n) when v is known (the map's KNOWN bit,
+ *                  isdf_map_observe / isdf_map_mark_known) and sqrt((double)n) * c (one rounded product) when it is not; before any observe
+ *                  or mark call nothing is known. Everything else above holds with this w: the field g, the parent rule g(u) + w(u, v) ==
+ *                  g(v) (w read at v, the node the walk steps from), paths, attitudes and found; the cost is the weighted g(t). Why the
+ *                  field stays exact and order-free: c >= 1 and sqrt((double)n) >= 1, so every weight is >= 1 (rounding is monotone), and FP
+ *                  addition of a positive weight is monotone; so the minimum over paths of the left-to-right sums is what any label-correcting
+ *                  order reaches, and a textbook FP64 Dijkstra with the same weights gives the same bits. A weight below FP64's resolution
+ *                  at 1 gives c == 1, the unweighted field. A route through unseen space costs c times its length there, so a known detour
+ *                  up to c times longer is preferred.
  * Deviations from the reference, on purpose: its open set keeps the stale key of an improved open node (:324-333) and its heuristic is
  *   inflated by 1.001 (:172-187), so its cost is >= the optimum and depends on pop order; here the path is the exact shortest one. Its
  *   AstarGetSucc overwrites a neighbour's attitude on every expansion that looks at it (:227-229), so the attitude getastarSE3Path reports
@@ -917,14 +939,15 @@ int isdf_frontend_check_batch(isdf_ctx *ctx, int n, const int32_t *ind, const do
  *   degrees; may be NULL); costs and found: B each. The single-goal call reports its length in *n.
  * Errors: ISDF_ERR_STATE without a map or without front-end kernels (isdf_frontend_build_kernels; again after a shape change);
  *   ISDF_ERR_INVALID for a NULL pointer, B < 1, a non-finite start or goal, a start or goal outside the map, non-zero reserved parameters,
- *   or cap smaller than the total path length (then *n / offsets still report the lengths needed); ISDF_ERR_UNSUPPORTED on a sharded
- *   context (isdf_set_shard world > 1).
+ *   a negative or non-finite unknown_weight, or cap smaller than the total path length (then *n / offsets still report the lengths
+ *   needed); ISDF_ERR_UNSUPPORTED on a sharded context (isdf_set_shard world > 1).
  * State: every call rebuilds the traversability grid and the field from the current map and front-end kernels, so nothing computed for an
  *   earlier map, shape or kernel set is ever used. Device memory, allocated on first use and reused: the FP64 field (8 B per voxel, 1 GiB at
  *   512^3) and three bit grids (traversability and two frontiers, 1 bit per voxel each). The calls count their launches in
  *   isdf_stats.kernel_launches and touch no other field of isdf_stats. */
-typedef struct isdf_frontpath_params {   /* NULL = defaults; the reserved fields must be zero */
-    int32_t reserved_[4];
+typedef struct isdf_frontpath_params {   /* NULL = defaults (all zero); the reserved fields must be zero. 16 bytes */
+    double unknown_weight;                /* the surcharge on unknown voxels above; finite, >= 0 (ISDF_ERR_INVALID otherwise) */
+    int32_t reserved_[2];
 } isdf_frontpath_params;
 typedef struct isdf_frontpath_info {       /* the last path, pairs or field call */
     int32_t rounds;                        /* relaxation rounds that had a non-empty frontier */
@@ -972,7 +995,7 @@ int isdf_frontend_path_fields_device(isdf_ctx *ctx, int S, const double *starts,
 
 /* ---- planning step: PlannerManager::generateTraj (plan_manager.cpp:202-313) for one start and B goals, end to end on the device ----
  * Definition, per goal b (each step is an existing entry point's definition):
- *   1. Front end   isdf_frontend_path_batch(start, goals). A path not found is NO_PATH: no trajectory.
+ *   1. Front end   isdf_frontend_path_batch(start, goals, &p->frontpath). A path not found is NO_PATH: no trajectory.
  *   2. Waypoints   isdf_path_waypoints(parlength, the map's res) gives N. N > 290 (the limit of the mid-end and the callback) is TOO_LONG:
  *                  no trajectory. head = [path.front(), 0, 0], tail = [path.back(), 0, 0] (:220-223).
  *   3. Mid-end     isdf_midend_batch_ragged(per_problem_bc = 1, p->midend) over every plan that reaches it, in goal order (one call; each
@@ -980,6 +1003,11 @@ int isdf_frontend_path_fields_device(isdf_ctx *ctx, int S, const double *starts,
  *                  the back end does not run for it (:277).
  *   4. Gather      isdf_gather_obstacle_points_batch(half_extent, offset, set_as_points = 1) over the waypoints of the plans that passed
  *                  the mid-end, in goal order. A plan with no point gets no swept-volume term, as the reference's loop over zero points.
+ *                  With ISDF_PLAN_KNOWN_PREFIX it is isdf_gather_obstacle_points_batch_known with, for plan b: k* = the index of the first
+ *                  node of its path whose voxel is not known (the path length when every node is; 0 when nothing is known); waypoint row j
+ *                  is path node (j + 1) g (isdf_path_waypoints' gap g), and the known rows are those with (j + 1) g < k*. So while the path is
+ *                  inside what has been seen the back end treats unseen space as an obstacle, and past the first unknown node it stays
+ *                  optimistic. Without the flag, nothing is known, or k* = 0, the gather is the one above.
  *   5. Durations   before the back end, problem q's persisted trajectory duration (see isdf_set_points_batch) is what
  *                  updateTraj(mid-end trajectory) (:272) leaves on a fresh context: its total duration (the left-to-right sum of T) when
  *                  shorter than 300 s, else 0. Plans are therefore independent of each other and of the order of the groups.
@@ -1016,9 +1044,10 @@ int isdf_frontend_path_fields_device(isdf_ctx *ctx, int S, const double *starts,
  *   host (see the device forms below); the host form then copies its outputs back.
  * Errors: ISDF_ERR_STATE without a map, a shape or front-end kernels; ISDF_ERR_UNSUPPORTED on a sharded context and for ISDF_PLAN_CERTIFY
  *   with a shape the certificate refuses (checked before any work); ISDF_ERR_INVALID for a NULL argument, B < 1, the stages' own parameter
- *   checks, unknown flags, a non-zero reserved_, pieces_per_traj != 0 in p->certify or p->dynamics, a start or goal outside the map, or
- *   caps too small. On failure every stage is -1, midend_f / backend_f are NaN, and the summaries read as their certificates' failures. */
-typedef enum isdf_plan_flags { ISDF_PLAN_CERTIFY = 1, ISDF_PLAN_DYNAMICS = 2 } isdf_plan_flags;
+ *   checks, unknown flags, a non-zero reserved_ (also frontpath.reserved_), a negative or non-finite frontpath.unknown_weight,
+ *   pieces_per_traj != 0 in p->certify or p->dynamics, a start or goal outside the map, or caps too small. On failure every stage is -1, midend_f / backend_f are NaN, and the summaries read as their certificates' failures. */
+/* 4 is not a flag (refused as unknown) */
+typedef enum isdf_plan_flags { ISDF_PLAN_CERTIFY = 1, ISDF_PLAN_DYNAMICS = 2, ISDF_PLAN_KNOWN_PREFIX = 8 } isdf_plan_flags;
 typedef enum isdf_plan_stage {
     ISDF_PLAN_FAILED = -1, ISDF_PLAN_NO_PATH = 0, ISDF_PLAN_TOO_LONG = 1, ISDF_PLAN_MIDEND_FAILED = 2, ISDF_PLAN_OPTIMISED = 3
 } isdf_plan_stage;
@@ -1033,6 +1062,8 @@ typedef struct isdf_plan_params {
     int32_t reserved_;              /* must be 0 */
     isdf_certify_params certify;    /* pieces_per_traj must be 0: the call sets N0 = N per group */
     isdf_dynamics_params dynamics;  /* likewise */
+    isdf_frontpath_params frontpath;   /* the front end's parameters (unknown_weight); zero in the defaults. Added at the end: the struct
+                                          grew by its 16 bytes, and zero means the planning step as it was */
 } isdf_plan_params;
 typedef struct isdf_plan_result {
     int32_t stage;                  /* isdf_plan_stage */
