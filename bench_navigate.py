@@ -3,7 +3,7 @@
 (Evaluator.navigate: sense -> fuse -> check -> replan -> fly -> advance, every stage batched over vehicles); prints one JSON line.
 
   python bench_navigate.py [--vehicles 1,16,64] [--rounds R] [--horizon H] [--sense-every S] [--seed N] [--fallback keep|brake]
-                           [--unknown free|occupied] [--cameras 1|4] [--prefer-known W]
+                           [--unknown free|occupied] [--cameras 1|4] [--prefer-known W] [--explore]
 
 World: mockamap's box world (isdf_world_cloud_device, ISDF_WORLD_BOXES) with seed 511, 40 x 40 x 10 m at 0.5 m (size 80 x 80 x 20,
 scale 2), 20 boxes 1.5 to 3 m wide: x and y in [-20, 20] m, z in [0, 10] m. The vehicles' map starts as an empty 1 m frame over that box
@@ -19,7 +19,9 @@ default, keep, prints what it always printed. --unknown occupied (navigate's unk
 the known space with the 5 x 5 x 5-voxel block around each start (free in the true map by pairs()) and adds the commits taken; --cameras 4
 flies a rig of four cameras, cam_to_body = Rz(k 90 deg) cam02body. --prefer-known W plans through what has been seen (DESIGN §3.23):
 the front end's surcharge unknown_weight = W on unknown voxels and ISDF_PLAN_KNOWN_PREFIX, so that the back end treats unseen space as
-an obstacle along each plan's known prefix. Either option (also --unknown free) also reports the pose of the minimum true clearance: its
+an obstacle along each plan's known prefix. --explore (needs --unknown occupied) flies navigate(explore=True) (DESIGN §3.24): a vehicle
+whose goal cannot be reached through seen space plans to the best frontier of what has been seen; it adds the frontier plans taken, and the
+frontier-goal call is timed inside the replan stage. Either option (also --unknown free) also reports the pose of the minimum true clearance: its
 vehicle, round and witness voxel, and whether that voxel is occupied in the vehicles' fused map at the end of the run. Writes nothing to the
 tree.
 """
@@ -103,9 +105,12 @@ def main():
     ap.add_argument("--unknown", choices=("free", "occupied"), default=None)
     ap.add_argument("--cameras", type=int, choices=(1, 4), default=1)
     ap.add_argument("--prefer-known", type=float, default=None, metavar="W")
+    ap.add_argument("--explore", action="store_true")
     args = ap.parse_args()
     if args.unknown == "occupied" and args.fallback != "brake":
         raise SystemExit("--unknown occupied needs --fallback brake")
+    if args.explore and args.unknown != "occupied":
+        raise SystemExit("--explore needs --unknown occupied")
     import torch
     import isdf_b200 as I
     if not torch.cuda.is_available():
@@ -132,6 +137,8 @@ def main():
     if args.prefer_known is not None:
         pkw.update(flags=I.PLAN_CERTIFY | I.PLAN_KNOWN_PREFIX, unknown_weight=args.prefer_known)
         out["prefer_known"] = args.prefer_known
+    if args.explore:
+        out["explore"] = True
     for B in [int(v) for v in args.vehicles.split(",")]:
         starts, goals = pairs(occ, B, args.seed + B)
         ev = I.Evaluator(cfg)
@@ -140,6 +147,8 @@ def main():
         ev.set_map_u8(np.zeros(DIMS, np.uint8), BMIN, RES)
         ev.set_sense_cloud_device(scene, stream=torch.cuda.current_stream().cuda_stream)
         kw = dict(unknown="occupied", known_boxes=np.concatenate([starts - 2.5, starts + 2.5], 1)) if args.unknown == "occupied" else {}
+        if args.explore:
+            kw["explore"] = True
         r = ev.navigate(starts, goals, rounds=args.rounds, horizon=args.horizon, sense_every=args.sense_every, tol=1.0,
                         plan_params=ev.plan_params(**pkw),
                         sense_params=rig(args.cameras), fallback=args.fallback, **kw)
@@ -159,6 +168,8 @@ def main():
             out["runs"][-1].update(brakes=int(r["brakes"].sum()), held_rounds=int(r["held_rounds"].sum()))
         if "commits" in r:
             out["runs"][-1].update(commits=int(r["commits"].sum()))
+        if "frontier_plans" in r:
+            out["runs"][-1].update(frontier_plans=int(r["frontier_plans"].sum()))
         if trace and where:
             flown = [k for k in range(len(r["times"])) if (r["verdicts"][k] != I.NAV_NO_TRAJECTORY).any()]
             v = where["voxel"]

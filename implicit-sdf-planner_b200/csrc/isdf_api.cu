@@ -7,6 +7,7 @@
 #include "isdf_minco.cuh"
 #include "isdf_frontend.cuh"
 #include "isdf_frontpath.cuh"
+#include "isdf_frontier.cuh"
 #include "isdf_lbfgs.cuh"
 #include "isdf_midend.cuh"
 #include "isdf_clearance.cuh"
@@ -251,6 +252,12 @@ struct isdf_ctx {
         cudaEvent_t ev[4] = {};
         isdf_frontpath_info info = {};
     } fp;
+    struct {   // frontiers (isdf_frontier.cuh): T_o, F, the list, union-find and cluster table of the last frontier call
+        DevBuf<uint32_t> d_to, d_f; DevBuf<int> d_cnt, d_woff, d_parent, d_root, d_slot, d_size, d_box, d_croot; DevBuf<long long> d_vox, d_cid;
+        DevBuf<unsigned long long> d_ntb, d_sum, d_best; DevBuf<unsigned> d_pick; DevBuf<char> d_tmp; DevBuf<uint8_t> d_cand;
+        DevBuf<isdf_frontier_cluster> d_table; DevBuf<int> d_pair, d_slice, d_tgt; DevBuf<double> d_goals; DevBuf<isdf_frontier_goal> d_out;
+        cudaEvent_t ev[6] = {};
+    } fr;
     struct {   // trajectory clearance check (isdf_clearance.cuh)
         DevBuf<int> d_cursor;
         DevBuf<unsigned long long> d_counters;   // {candidate pairs, exact mesh searches} of the last check (isdf_dbg_clearance_counts)
@@ -318,6 +325,7 @@ struct isdf_ctx {
         peer.buf = {};
         for (cudaEvent_t e : {ev0, ev1, ev_main_done, ev_items_done}) if (e) cudaEventDestroy(e);
         for (cudaEvent_t e : fp.ev) if (e) cudaEventDestroy(e);
+        for (cudaEvent_t e : fr.ev) if (e) cudaEventDestroy(e);
         for (cudaEvent_t e : svol.ev) if (e) cudaEventDestroy(e);
         for (cudaEvent_t e : plan.ev) if (e) cudaEventDestroy(e);
         if (aux_stream) cudaStreamDestroy(aux_stream);
@@ -4097,10 +4105,12 @@ static int frontend_state(isdf_ctx *c) {
 // the feasibility pipelines, as isdf_dbg_frontend_launch reports them
 enum { FE_PIPE_ONE_PASS = 0, FE_PIPE_CORE = 1, FE_PIPE_TABLES = 2 };
 
-// the feasibility pipeline into d_masks (4 words per voxel), or, with d_trav set, into the traversability bits (isdf_frontpath.cuh)
-static int frontend_feasibility_run(isdf_ctx *c, uint32_t *d_masks, uint32_t *d_trav, void *cuda_stream) {
+// the feasibility pipeline into d_masks (4 words per voxel), or, with d_trav set, into the traversability bits (isdf_frontpath.cuh);
+// bits (may be NULL: the map's occupancy): the grid it reads in place of the occupancy grid, in its layout (the blocked grid for T_b)
+static int frontend_feasibility_run(isdf_ctx *c, uint32_t *d_masks, uint32_t *d_trav, void *cuda_stream, const uint32_t *bits = nullptr) {
     FrontArgs A = front_args(c);
     A.out = d_masks; A.trav = d_trav;
+    if (bits) A.grid.bits = bits;
     if (d_trav) CU_TRY(cudaMemsetAsync(d_trav, 0, sizeof(uint32_t) * (size_t)c->map.grid.X * c->map.grid.Y * c->map.grid.Zw, (cudaStream_t)cuda_stream));
     const size_t smem = sizeof(uint32_t) * 4 * (size_t)A.ks * A.ks * A.ks;
     CU_TRY(cudaFuncSetAttribute(k_frontend_feasibility, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -4244,15 +4254,17 @@ static PathArgs path_args(isdf_ctx *c, unsigned long long *d_g) {
 // unweighted kernels
 static FpSurcharge path_surcharge(const isdf_ctx *c, double cw) { return {c->known.have ? c->known.d_known.p : nullptr, cw}; }
 
-// the traversability grid of the current map and kernels on stream st, between events 0 and 1; clears c->fp.info
-static int path_trav(isdf_ctx *c, cudaStream_t st) {
+// the traversability grid of the current map and kernels on stream st, between events 0 and 1; clears c->fp.info. known_only: T_b,
+// the traversability of the blocked grid (isdf_map_frontiers), in place of T_o
+static int path_trav(isdf_ctx *c, cudaStream_t st, bool known_only = false) {
     const DevGrid &G = c->map.grid;
     for (cudaEvent_t &e : c->fp.ev) if (!e) CU_TRY(cudaEventCreate(&e));
     CU_TRY(c->fp.d_trav.ensure((size_t)G.X * G.Y * G.Zw));
     CU_TRY(c->fp.h_flag.ensure(2));
+    if (known_only) if (int r = blocked_grid_ready(c, st)) return r;
     c->fp.info = {};
     CU_TRY(cudaEventRecord(c->fp.ev[0], st));
-    if (int r = frontend_feasibility_run(c, nullptr, c->fp.d_trav.p, st)) return r;
+    if (int r = frontend_feasibility_run(c, nullptr, c->fp.d_trav.p, st, known_only ? c->known.d_blocked.p : nullptr)) return r;
     CU_TRY(cudaEventRecord(c->fp.ev[1], st));
     return 0;
 }
@@ -4319,9 +4331,10 @@ static void path_info(isdf_ctx *c, size_t field_bytes, bool paths) {
 // goal (sstride 0). Pairs whose starts share a voxel share a field: node 0 of a path is its start voxel's cube centre, so their paths are
 // the same. The distinct start voxels' fields are built in chunks of at most max_fields (0: FP_FIELD_BUDGET bytes, at least one field),
 // and each chunk's paths are walked into scratch before its fields are reused. off (B + 1) is filled as soon as every length is known,
-// also when they exceed cap. cw: the unknown-voxel edge factor of the fields and the walk (frontpath_params_check).
+// also when they exceed cap. cw: the unknown-voxel edge factor of the fields and the walk (frontpath_params_check). known_only: over
+// T_b instead of T_o (ISDF_PLAN_KNOWN_ONLY).
 static int path_run(isdf_ctx *c, int B, const double *starts, int sstride, const double *goals, double cw, int max_fields, int cap,
-                    std::vector<int> &off, cudaStream_t st) {
+                    std::vector<int> &off, cudaStream_t st, bool known_only = false) {
     const DevGrid &G = c->map.grid;
     const size_t nvox = (size_t)G.X * G.Y * G.Z;
     std::vector<int> tgt((size_t)3 * B), ps(B), src;   // ps[b]: pair b's source; src: 3 per distinct start voxel, in order of first use
@@ -4351,7 +4364,7 @@ static int path_run(isdf_ctx *c, int B, const double *starts, int sstride, const
             wsrc[4 * (size_t)w + 3] = ps[b] % F;   // the field's slice in its chunk
         }
     }
-    if (int r = path_trav(c, st)) return r;
+    if (int r = path_trav(c, st, known_only)) return r;
     CU_TRY(c->fp.d_g.ensure((size_t)F * nvox));
     CU_TRY(c->fp.d_tgt.upload(wtgt.data(), wtgt.size(), st)); CU_TRY(c->fp.d_tsrc.upload(wsrc.data(), wsrc.size(), st));
     CU_TRY(c->fp.d_pair.upload(walk.data(), walk.size(), st));
@@ -4551,6 +4564,240 @@ extern "C" int isdf_frontend_path_info(isdf_ctx *c, isdf_frontpath_info *out) {
     return 0;
 }
 
+// ---- frontiers of known space and frontier goals (isdf_frontier.cuh) ------------------------------------------------------------------
+static int frontier_state(isdf_ctx *c) {
+    if (int r = frontend_state(c)) return r;
+    if (c->world > 1) return fail(ISDF_ERR_UNSUPPORTED, "the frontier calls are not sharded: call them on a context with isdf_set_shard(ctx, 0, 1)");
+    return 0;
+}
+
+template <typename T>
+static int fr_scan(isdf_ctx *c, const T *in, T *out, long long n, cudaStream_t st) {
+    size_t bytes = 0;
+    CU_TRY(cub::DeviceScan::InclusiveSum(nullptr, bytes, in, out, n, st));
+    CU_TRY(c->fr.d_tmp.ensure(std::max<size_t>(bytes, 1)));
+    CU_TRY(cub::DeviceScan::InclusiveSum(c->fr.d_tmp.p, bytes, in, out, n, st));
+    return 0;
+}
+
+// T_o into c->fr.d_to, T_b into c->fp.d_trav (so that path_fields relaxes over T_b), F, its list, labels and cluster table into c->fr on
+// st; counts and the first three stage times into *I. Leaves c->fp.info cleared (path_trav).
+static int frontier_run(isdf_ctx *c, isdf_frontier_info *I, cudaStream_t st) {
+    auto &z = c->fr;
+    const DevGrid &G = c->map.grid;
+    const long long nword = (long long)G.X * G.Y * G.Zw;
+    for (cudaEvent_t &e : z.ev) if (!e) CU_TRY(cudaEventCreate(&e));
+    *I = {};
+    CU_TRY(z.d_to.ensure((size_t)nword)); CU_TRY(z.d_f.ensure((size_t)nword)); CU_TRY(z.d_cnt.ensure((size_t)nword));
+    CU_TRY(z.d_woff.ensure((size_t)nword + 1)); CU_TRY(z.d_ntb.ensure(1));
+    if (int r = blocked_grid_ready(c, st)) return r;
+    CU_TRY(cudaEventRecord(z.ev[0], st));
+    if (int r = frontend_feasibility_run(c, nullptr, z.d_to.p, st)) return r;
+    if (int r = path_trav(c, st, true)) return r;
+    CU_TRY(cudaEventRecord(z.ev[1], st));
+    FrArgs A = {};
+    A.grid = G; A.to = z.d_to.p; A.tb = c->fp.d_trav.p; A.f = z.d_f.p; A.cnt = z.d_cnt.p; A.woff = z.d_woff.p; A.ntb = z.d_ntb.p;
+    const long long sms = c->sm_count;
+    CU_TRY(cudaMemsetAsync(z.d_ntb.p, 0, sizeof(unsigned long long), st));
+    CU_TRY(cudaMemsetAsync(z.d_woff.p, 0, sizeof(int), st));
+    k_fr_frontier<<<(unsigned)std::min<long long>((nword + 255) / 256, sms * 32), 256, 0, st>>>(A);
+    c->stats.kernel_launches++;
+    CU_TRY(cudaGetLastError());
+    if (int r = fr_scan(c, z.d_cnt.p, z.d_woff.p + 1, nword, st)) return r;
+    int n = 0;
+    unsigned long long ntb = 0;
+    CU_TRY(cudaMemcpyAsync(&n, z.d_woff.p + nword, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaMemcpyAsync(&ntb, z.d_ntb.p, sizeof(ntb), cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    A.n = n;
+    CU_TRY(z.d_vox.ensure(std::max(n, 1))); CU_TRY(z.d_parent.ensure(std::max(n, 1))); CU_TRY(z.d_root.ensure((size_t)n + 1));
+    CU_TRY(z.d_slot.ensure((size_t)n + 1)); CU_TRY(z.d_cid.ensure(std::max(n, 1)));
+    A.vox = z.d_vox.p; A.parent = z.d_parent.p; A.root = z.d_root.p; A.cid = z.d_cid.p;
+    const unsigned lb = (unsigned)std::max<long long>(1, std::min<long long>(((long long)n + 255) / 256, sms * 32));
+    if (n) {
+        k_fr_list<<<(unsigned)std::min<long long>((nword + 255) / 256, sms * 32), 256, 0, st>>>(A);
+        c->stats.kernel_launches++;
+    }
+    CU_TRY(cudaEventRecord(z.ev[2], st));
+    int nc = 0;
+    if (n) {
+        k_fr_hook<<<lb, 256, 0, st>>>(A);
+        k_fr_flatten<<<lb, 256, 0, st>>>(A);
+        c->stats.kernel_launches += 2;
+        CU_TRY(cudaGetLastError());
+        if (int r = fr_scan(c, z.d_root.p, z.d_slot.p + 1, n, st)) return r;
+        CU_TRY(cudaMemsetAsync(z.d_slot.p, 0, sizeof(int), st));
+        CU_TRY(cudaMemcpyAsync(&nc, z.d_slot.p + n, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
+    }
+    // slot[r] = the roots before position r: root r's cluster slot, in ascending cluster id; slot[n] = the clusters
+    CU_TRY(z.d_size.ensure(std::max(nc, 1))); CU_TRY(z.d_box.ensure(6 * (size_t)std::max(nc, 1))); CU_TRY(z.d_croot.ensure(std::max(nc, 1)));
+    CU_TRY(z.d_sum.ensure(3 * (size_t)std::max(nc, 1))); CU_TRY(z.d_table.ensure(std::max(nc, 1)));
+    A.slot = z.d_slot.p; A.nc = nc; A.size = z.d_size.p; A.box = z.d_box.p; A.croot = z.d_croot.p; A.sum = z.d_sum.p; A.table = z.d_table.p;
+    if (nc) {
+        k_fr_table_init<<<(unsigned)((nc + 127) / 128), 128, 0, st>>>(A);
+        k_fr_accum<<<lb, 256, 0, st>>>(A);
+        k_fr_table<<<(unsigned)((nc + 127) / 128), 128, 0, st>>>(A);
+        c->stats.kernel_launches += 3;
+        CU_TRY(cudaGetLastError());
+    }
+    CU_TRY(cudaEventRecord(z.ev[3], st));
+    CU_TRY(cudaStreamSynchronize(st));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, z.ev[0], z.ev[1]); I->traversability_ms = ms;
+    cudaEventElapsedTime(&ms, z.ev[1], z.ev[2]); I->frontier_ms = ms;
+    cudaEventElapsedTime(&ms, z.ev[2], z.ev[3]); I->cluster_ms = ms;
+    I->traversable_blocked = (int64_t)ntb; I->frontier_voxels = n; I->clusters = nc;
+    return 0;
+}
+
+static int frontiers_entry(isdf_ctx *c, bool dev, int64_t cap_voxels, int64_t *voxels, int64_t *cluster_of, int64_t cap_clusters,
+                           isdf_frontier_cluster *clusters, isdf_frontier_info *info, cudaStream_t st) {
+    if (int r = frontier_state(c)) return r;
+    if (cap_voxels < 0 || cap_clusters < 0 || (cap_voxels > 0 && (!voxels || !cluster_of)) || (cap_clusters > 0 && !clusters))
+        return fail(ISDF_ERR_INVALID, "a negative cap, or a NULL output with a non-zero cap");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    if (!dev) st = c->stream;
+    isdf_frontier_info I;
+    const int r = frontier_run(c, &I, st);
+    if (info) *info = I;
+    if (r) return r;
+    if (I.frontier_voxels > cap_voxels || I.clusters > cap_clusters)
+        return fail(ISDF_ERR_INVALID, "cap_voxels or cap_clusters too small (info reports the sizes needed)");
+    const cudaMemcpyKind k = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+    if (I.frontier_voxels) {
+        CU_TRY(cudaMemcpyAsync(voxels, c->fr.d_vox.p, sizeof(int64_t) * I.frontier_voxels, k, st));
+        CU_TRY(cudaMemcpyAsync(cluster_of, c->fr.d_cid.p, sizeof(int64_t) * I.frontier_voxels, k, st));
+        CU_TRY(cudaMemcpyAsync(clusters, c->fr.d_table.p, sizeof(isdf_frontier_cluster) * I.clusters, k, st));
+    }
+    CU_TRY(cudaStreamSynchronize(st));
+    return 0;
+}
+
+extern "C" int isdf_map_frontiers(isdf_ctx *c, int64_t cap_voxels, int64_t *voxels, int64_t *cluster_of, int64_t cap_clusters,
+                                  isdf_frontier_cluster *clusters, isdf_frontier_info *info) {
+    return frontiers_entry(c, false, cap_voxels, voxels, cluster_of, cap_clusters, clusters, info, nullptr);
+}
+
+extern "C" int isdf_map_frontiers_device(isdf_ctx *c, int64_t cap_voxels, int64_t *d_voxels, int64_t *d_cluster_of, int64_t cap_clusters,
+                                         isdf_frontier_cluster *d_clusters, isdf_frontier_info *info, void *cuda_stream) {
+    return frontiers_entry(c, true, cap_voxels, d_voxels, d_cluster_of, cap_clusters, d_clusters, info, (cudaStream_t)cuda_stream);
+}
+
+extern "C" int isdf_frontier_default_params(isdf_frontier_params *p) {
+    if (!p) return fail(ISDF_ERR_INVALID, "params is NULL");
+    std::memset(p, 0, sizeof(*p));
+    p->goal_weight = 1.0;
+    p->min_cluster_voxels = 1;
+    return 0;
+}
+
+// the frontier goals of B pairs (starts and goals on the host, B x 3) into out (B records, device) on st
+static int frontier_goals_run(isdf_ctx *c, int B, const double *starts, const double *goals, const isdf_frontier_params *p, int max_fields,
+                              isdf_frontier_goal *out, isdf_frontier_info *I, cudaStream_t st) {
+    const DevGrid &G = c->map.grid;
+    const size_t nvox = (size_t)G.X * G.Y * G.Z;
+    auto &z = c->fr;
+    std::vector<int> tgt((size_t)3 * B), ps(B), src;   // as path_run: ps[b] is pair b's source, src the distinct start voxels
+    std::unordered_map<long long, int> seen;
+    for (int b = 0; b < B; b++) {
+        int s[3];
+        if (int r = path_voxel(G, starts + 3 * (size_t)b, s, "starts[" + std::to_string(b) + "]")) return r;
+        if (int r = path_voxel(G, goals + 3 * (size_t)b, &tgt[3 * (size_t)b], "goals[" + std::to_string(b) + "]")) return r;
+        const auto ins = seen.emplace(((long long)s[0] * G.Y + s[1]) * G.Z + s[2], (int)(src.size() / 3));
+        if (ins.second) src.insert(src.end(), s, s + 3);
+        ps[b] = ins.first->second;
+    }
+    if (int r = frontier_run(c, I, st)) return r;
+    const int S = (int)(src.size() / 3), n = (int)I->frontier_voxels;
+    const long long want = max_fields > 0 ? max_fields : std::max<long long>(1, FP_FIELD_BUDGET / (long long)(sizeof(double) * nvox));
+    const int F = (int)std::min<long long>(std::min<long long>(want, S), 65535);
+    // walk order: the pairs grouped by source
+    std::vector<int> wstart((size_t)S + 1, 0), wpair(B), wslice(B);
+    for (int b = 0; b < B; b++) wstart[ps[b] + 1]++;
+    for (int s = 0; s < S; s++) wstart[s + 1] += wstart[s];
+    {
+        std::vector<int> next(wstart.begin(), wstart.end() - 1);
+        for (int b = 0; b < B; b++) { const int w = next[ps[b]]++; wpair[w] = b; wslice[w] = ps[b] % F; }
+    }
+    CU_TRY(z.d_pair.upload(wpair.data(), wpair.size(), st)); CU_TRY(z.d_slice.upload(wslice.data(), wslice.size(), st));
+    CU_TRY(z.d_tgt.upload(tgt.data(), tgt.size(), st)); CU_TRY(z.d_goals.upload(goals, (size_t)3 * B, st));
+    CU_TRY(z.d_best.ensure(B)); CU_TRY(z.d_pick.ensure(B)); CU_TRY(z.d_cand.ensure(std::max(n, 1)));
+    CU_TRY(cudaMemsetAsync(z.d_best.p, 0xff, sizeof(unsigned long long) * B, st));   // above every score's bits, +inf's included
+    CU_TRY(cudaMemsetAsync(z.d_pick.p, 0xff, sizeof(unsigned) * B, st));
+    if (n) {
+        k_fg_cand<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, z.d_parent.p, z.d_slot.p, z.d_size.p, p->min_cluster_voxels, z.d_cand.p);
+        c->stats.kernel_launches++;
+        CU_TRY(cudaGetLastError());
+    }
+    CU_TRY(c->fp.d_g.ensure((size_t)F * nvox));
+    FgArgs A = {};
+    A.grid = G; A.g = c->fp.d_g.p; A.vox = z.d_vox.p; A.cand = z.d_cand.p; A.n = n; A.goal_weight = p->goal_weight;
+    A.goals = z.d_goals.p; A.tgt = z.d_tgt.p; A.best = z.d_best.p; A.pick = z.d_pick.p; A.table = z.d_table.p; A.cid = z.d_cid.p; A.out = out;
+    const long long sms = c->sm_count;
+    for (int s0 = 0; s0 < S; s0 += F) {
+        const int m = std::min(F, S - s0), w0 = wstart[s0], w1 = wstart[s0 + m];
+        if (int r = path_fields(c, m, &src[3 * (size_t)s0], 1.0, c->fp.d_g.p, st)) return r;
+        CU_TRY(cudaEventRecord(z.ev[4], st));
+        A.nt = w1 - w0; A.pair = z.d_pair.p + w0; A.slice = z.d_slice.p + w0;
+        if (n) {
+            const dim3 grid((unsigned)std::max<long long>(1, std::min<long long>(((long long)n + 255) / 256, sms * 8)), (unsigned)std::min(A.nt, 65535));
+            // a pair without a candidate keeps best = ~0, which no score equals: k_fg_select<true> picks nothing for it
+            k_fg_select<false><<<grid, 256, 0, st>>>(A);
+            k_fg_select<true><<<grid, 256, 0, st>>>(A);
+            c->stats.kernel_launches += 2;
+        }
+        k_fg_record<<<(unsigned)((A.nt + 127) / 128), 128, 0, st>>>(A);
+        c->stats.kernel_launches++;
+        CU_TRY(cudaGetLastError());
+        CU_TRY(cudaEventRecord(z.ev[5], st));
+        CU_TRY(cudaStreamSynchronize(st));
+        float ms = 0;
+        cudaEventElapsedTime(&ms, z.ev[4], z.ev[5]);
+        I->select_ms += ms;
+    }
+    I->field_ms = c->fp.info.field_ms;
+    return 0;
+}
+
+static int frontier_goals_entry(isdf_ctx *c, bool dev, int B, const double *starts, const double *goals, const isdf_frontier_params *prm,
+                                int max_fields, isdf_frontier_goal *out, isdf_frontier_info *info, cudaStream_t st) {
+    if (int r = frontier_state(c)) return r;
+    if (!starts || !goals || !out || B < 1) return fail(ISDF_ERR_INVALID, "NULL argument or B < 1");
+    if (max_fields < 0) return fail(ISDF_ERR_INVALID, "max_fields < 0");
+    isdf_frontier_params p;
+    isdf_frontier_default_params(&p);
+    if (prm) p = *prm;
+    if (p.reserved_ != 0) return fail(ISDF_ERR_INVALID, "isdf_frontier_params: reserved_ must be 0");
+    if (!(std::isfinite(p.goal_weight) && p.goal_weight > 0.0)) return fail(ISDF_ERR_INVALID, "isdf_frontier_params: goal_weight must be finite and > 0");
+    if (p.min_cluster_voxels < 1) return fail(ISDF_ERR_INVALID, "isdf_frontier_params: min_cluster_voxels must be >= 1");
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    if (!dev) st = c->stream;
+    std::vector<double> hs, hg;
+    if (dev) {
+        int sstride = 3;
+        if (int r = read_endpoints(c, B, starts, sstride, goals, hs, hg, st)) return r;
+    }
+    CU_TRY(c->fr.d_out.ensure(B));
+    isdf_frontier_info I = {};
+    const int r = frontier_goals_run(c, B, starts, goals, &p, max_fields, dev ? out : c->fr.d_out.p, &I, st);
+    if (info) *info = I;
+    if (r) return r;
+    if (!dev) CU_TRY(cudaMemcpyAsync(out, c->fr.d_out.p, sizeof(isdf_frontier_goal) * B, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    return 0;
+}
+
+extern "C" int isdf_frontier_goals(isdf_ctx *c, int B, const double *starts, const double *goals, const isdf_frontier_params *p, int max_fields,
+                                   isdf_frontier_goal *out, isdf_frontier_info *info) {
+    return frontier_goals_entry(c, false, B, starts, goals, p, max_fields, out, info, nullptr);
+}
+
+extern "C" int isdf_frontier_goals_device(isdf_ctx *c, int B, const double *d_starts, const double *d_goals, const isdf_frontier_params *p,
+                                          int max_fields, isdf_frontier_goal *d_out, isdf_frontier_info *info, void *cuda_stream) {
+    return frontier_goals_entry(c, true, B, d_starts, d_goals, p, max_fields, d_out, info, (cudaStream_t)cuda_stream);
+}
+
 // ---- planning step: PlannerManager::generateTraj for B (start, goal) pairs (include/isdf.h) --------------------------------------------
 // The stages are the existing entry points' internals on device buffers: path_run, isdf_path_waypoints, one ragged midend_batch_run, the
 // batched gather with set_as_points, one ragged lbfgs_rounds over callback_batch_launch, one ragged k_minco_forward for the final
@@ -4585,7 +4832,7 @@ static int plan_check(isdf_ctx *c, const isdf_plan_params *p, double *r_cert) {
     if (!c->mesh.have_shape) return fail(ISDF_ERR_STATE, "shape not set");
     if (c->world > 1) return fail(ISDF_ERR_UNSUPPORTED, "the planning step is not sharded: call it on a context with isdf_set_shard(ctx, 0, 1)");
     if (p->reserved_ != 0) return fail(ISDF_ERR_INVALID, "reserved_ must be 0");
-    if (p->flags & ~(ISDF_PLAN_CERTIFY | ISDF_PLAN_DYNAMICS | ISDF_PLAN_KNOWN_PREFIX)) return fail(ISDF_ERR_INVALID, "unknown flags");
+    if (p->flags & ~(ISDF_PLAN_CERTIFY | ISDF_PLAN_DYNAMICS | ISDF_PLAN_KNOWN_PREFIX | ISDF_PLAN_KNOWN_ONLY)) return fail(ISDF_ERR_INVALID, "unknown flags");
     double cw;
     if (int r = frontpath_params_check(&p->frontpath, &cw)) return r;
     if (!(std::isfinite(p->parlength) && p->parlength > 0.0)) return fail(ISDF_ERR_INVALID, "parlength must be finite and positive");
@@ -4670,7 +4917,9 @@ static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const
     // 1. front end
     std::vector<int> off;
     const double cw = 1.0 + p->frontpath.unknown_weight;   // checked by plan_check
-    if (int r = timed(info.frontend_ms, [&] { return path_run(c, B, starts, sstride, goals, cw, max_fields, 0x7fffffff, off, st); })) return r;
+    const bool known_only = p->flags & ISDF_PLAN_KNOWN_ONLY;
+    if (int r = timed(info.frontend_ms, [&] { return path_run(c, B, starts, sstride, goals, cw, max_fields, 0x7fffffff, off, st, known_only); }))
+        return r;
     const int nodes = off[B];
     const int32_t *d_off = c->fp.d_off.p;
     const double *d_xyz = c->fp.d_xyz.p;
@@ -4772,7 +5021,12 @@ static int plan_run(isdf_ctx *c, int B, const double *starts, int sstride, const
             for (int k = 0; k < Bp; k++) bplan[k] = idx[ok[k]];
             if (int r = plan_upload(c, z.d_bplan, bplan, st)) return r;
             const int *d_krows = nullptr;   // ISDF_PLAN_KNOWN_PREFIX: each instance's rows inside its path's known prefix
-            if (p->flags & ISDF_PLAN_KNOWN_PREFIX) {
+            if (known_only) {   // every row: the path is known but for its start
+                std::vector<int> kr(Bp);
+                for (int k = 0; k < Bp; k++) kr[k] = gwo[k + 1] - gwo[k];
+                if (int r = plan_upload(c, z.d_krows, kr, st)) return r;
+                d_krows = z.d_krows.p;
+            } else if (p->flags & ISDF_PLAN_KNOWN_PREFIX) {
                 CU_TRY(z.d_krows.ensure(Bp));
                 k_plan_known_rows<<<(unsigned)((Bp + 127) / 128), 128, 0, st>>>(Bp, z.d_bplan.p, d_off, c->fp.d_nodes.p,
                                                                                 c->known.have ? c->known.d_known.p : nullptr, c->map.grid,

@@ -54,12 +54,15 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_map_fuse_cloud", "isdf_map_fuse_cloud_device", "isdf_plan_states", "isdf_plan_states_device",
                "isdf_trajectory_shift", "isdf_trajectory_shift_device", "isdf_brake_default_params", "isdf_trajectory_brake",
                "isdf_trajectory_brake_device", "isdf_map_observe", "isdf_map_observe_device", "isdf_map_mark_known",
-               "isdf_get_map_known_u8", "isdf_set_unknown_policy", "isdf_get_unknown_policy", "isdf_gather_obstacle_points_batch_known"]
+               "isdf_get_map_known_u8", "isdf_set_unknown_policy", "isdf_get_unknown_policy", "isdf_gather_obstacle_points_batch_known",
+               "isdf_map_frontiers", "isdf_map_frontiers_device", "isdf_frontier_default_params", "isdf_frontier_goals",
+               "isdf_frontier_goals_device"]
 WORLD_KINDS = dict(globalmap=1, perlin=2, boxes=3)   # isdf_world_kind
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
 DYN_QUANTITIES = ["speed", "acceleration", "body_rate", "tilt", "thrust"]   # q of isdf_dynamics_summary; mask bit 5: the thrust minimum
-PLAN_CERTIFY, PLAN_DYNAMICS, PLAN_KNOWN_PREFIX = 1, 2, 8                       # isdf_plan_params.flags
+PLAN_CERTIFY, PLAN_DYNAMICS, PLAN_KNOWN_PREFIX, PLAN_KNOWN_ONLY = 1, 2, 8, 16     # isdf_plan_params.flags
+FRONTIER_NONE, FRONTIER_GOAL, FRONTIER_FRONTIER = 0, 1, 2                        # isdf_frontier_goal.kind
 PLAN_FAILED, NO_PATH, TOO_LONG, MIDEND_FAILED, OPTIMISED = -1, 0, 1, 2, 3      # isdf_plan_result.stage
 ESDF_FIELDS = dict(positive=0, negative=1, signed=2)                            # isdf_esdf_field
 STATE_DOUBLES = 20                                                               # ISDF_STATE_DOUBLES: pos vel acc jer quat(w,x,y,z) omg thr
@@ -376,6 +379,42 @@ class PlanParams(C.Structure):
                 ("frontpath", FrontPathParams)]
 
 
+class FrontierCluster(C.Structure):
+    """isdf_frontier_cluster"""
+    _fields_ = [("id", C.c_int64), ("size", C.c_int64), ("bmin", C.c_int32 * 3), ("bmax", C.c_int32 * 3), ("centroid", C.c_double * 3)]
+
+
+class FrontierInfo(C.Structure):
+    """isdf_frontier_info"""
+    _fields_ = [("traversable_blocked", C.c_int64), ("frontier_voxels", C.c_int64), ("clusters", C.c_int64), ("reserved_", C.c_int64)] + \
+               [(n, C.c_double) for n in ["traversability_ms", "frontier_ms", "cluster_ms", "field_ms", "select_ms"]]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved_"}
+
+
+class FrontierParams(C.Structure):
+    """isdf_frontier_params"""
+    _fields_ = [("goal_weight", C.c_double), ("min_cluster_voxels", C.c_int32), ("reserved_", C.c_int32)]
+
+
+class FrontierGoal(C.Structure):
+    """isdf_frontier_goal"""
+    _fields_ = [("kind", C.c_int32), ("reserved_", C.c_int32), ("voxel", C.c_int64), ("cluster", C.c_int64), ("g", C.c_double),
+                ("score", C.c_double), ("point", C.c_double * 3)]
+
+
+FRONTIER_GOAL_DTYPE = np.dtype([("kind", "<i4"), ("reserved_", "<i4"), ("voxel", "<i8"), ("cluster", "<i8"), ("g", "<f8"), ("score", "<f8"),
+                                ("point", "<f8", (3,))])
+FRONTIER_CLUSTER_DTYPE = np.dtype([("id", "<i8"), ("size", "<i8"), ("bmin", "<i4", (3,)), ("bmax", "<i4", (3,)), ("centroid", "<f8", (3,))])
+
+
+def decode_frontier_goals(raw):
+    """isdf_frontier_goal records ((B, 64) uint8 or a FRONTIER_GOAL_DTYPE array, on any device) -> a FRONTIER_GOAL_DTYPE array"""
+    b = raw.cpu().numpy() if hasattr(raw, "cpu") else np.asarray(raw)
+    return np.ascontiguousarray(b).view(np.uint8).reshape(-1).view(FRONTIER_GOAL_DTYPE).copy()
+
+
 class PlanResult(C.Structure):
     """isdf_plan_result (one per goal)"""
     _fields_ = [(n, C.c_int32) for n in ["stage", "path_nodes", "pieces", "obstacle_points", "midend_ret", "backend_ret", "backend_iterations",
@@ -597,6 +636,12 @@ def load_library(path=None):
     lib.isdf_frontend_path_pairs.argtypes = [vp, C.c_int, dp, dp, fpp, C.c_int, C.c_int, dp, dp, ip, dp, u8p]
     lib.isdf_frontend_path_pairs_device.argtypes = [vp, C.c_int, vp, vp, fpp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]
     lib.isdf_frontend_path_fields_device.argtypes = [vp, C.c_int, dp, fpp, vp, vp]
+    frp, fip = C.POINTER(FrontierParams), C.POINTER(FrontierInfo)
+    lib.isdf_map_frontiers.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, vp, fip]
+    lib.isdf_map_frontiers_device.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, vp, fip, vp]
+    lib.isdf_frontier_default_params.argtypes = [frp]
+    lib.isdf_frontier_goals.argtypes = [vp, C.c_int, dp, dp, frp, C.c_int, vp, fip]
+    lib.isdf_frontier_goals_device.argtypes = [vp, C.c_int, vp, vp, frp, C.c_int, vp, fip, vp]
     mpp = C.POINTER(MidendParams)
     lib.isdf_path_waypoints.argtypes = [C.c_int, ip, dp, C.c_double, C.c_double, C.c_int, dp, ip, ip]
     lib.isdf_midend_default_params.argtypes = [mpp]
@@ -737,6 +782,21 @@ def path_waypoints(paths, res, parlength=3.0):
     if r != 0:
         raise IsdfError(r, lib.isdf_last_error().decode())
     return [wp[wo[b]:wo[b + 1]].copy() for b in range(B)], pieces[:B].copy()
+
+
+def _cat_plans(parts):
+    """the outputs of plan_*_device calls (dicts of CUDA tensors) as one call's, plans in order"""
+    import torch
+    if len(parts) == 1:
+        return parts[0]
+    out = dict(parts[0])
+    for q in parts[1:]:
+        for k in ("path_off", "piece_off"):
+            out[k] = torch.cat([out[k], q[k][1:] + out[k][-1]])
+        for k in ("path_xyz", "T", "coeffs", "results", "certify", "dynamics"):
+            if out[k] is not None:
+                out[k] = torch.cat([out[k], q[k]])
+    return out
 
 
 def _cuda_f64(t):
@@ -1829,7 +1889,8 @@ class Evaluator:
 
     # ---- flying to goals through a world seen only through the depth camera (plan -> fly -> sense -> fuse -> check -> re-plan) ----
     def navigate(self, starts, goals, *, rounds, horizon, sense_every=10, tol=0.5, plan_params=None, sim_params=None, sense_params=None,
-                 max_fields=0, stream=None, fallback="keep", brake_params=None, unknown="free", known_boxes=None):
+                 max_fields=0, stream=None, fallback="keep", brake_params=None, unknown="free", known_boxes=None, explore=False,
+                 frontier_params=None):
         """Drive B vehicles from starts (B, 3) to goals (B, 3) through the scene set by set_sense_cloud*, building their one shared map by
         fusion into the current map's frame (set it first, e.g. set_map_u8 of zeros). Needs the shape, the front-end kernels and
         plan_params with PLAN_CERTIFY (a shape the certificate supports). Each round, for the active vehicles:
@@ -1868,6 +1929,14 @@ class Evaluator:
         with unknown_weight > 0 and PLAN_KNOWN_PREFIX in flags (plan_params(unknown_weight=W, flags=PLAN_CERTIFY | PLAN_KNOWN_PREFIX)):
         every replan then prefers routes through known voxels and keeps the back end out of unseen space along its known prefix
         (DESIGN §3.23); the loop itself is unchanged.
+        explore=True (needs unknown="occupied") plans toward the frontier of what has been seen (DESIGN §3.24): in step 3, before the
+        replan call, one frontier_goals_device call (frontier_params, default frontier_params()) for the replanning vehicles, from their
+        replan heads to their true goals. GOAL plans to the goal and FRONTIER to the frontier point, both with plan_params' flags |
+        PLAN_KNOWN_ONLY, so every node of the plan after its start is known and the certificate can accept it whole; NONE plans exactly as
+        without explore. Acceptance, commits, the brake fallback and holding are unchanged; a vehicle whose frontier trajectory runs out
+        away from its true goal is held (active, at rest) and replans next round from there with what it has sensed since. ARRIVED is
+        judged against the true goal. The result then also has subgoal_kinds (rounds run, B): the FRONTIER_* kind each replan used, -1
+        where the vehicle did not replan; and frontier_plans (B,) numpy: replans toward a frontier point.
         Vehicles share the map, so one vehicle's run depends on what the others sensed; with B = 1 it is that vehicle's alone. The world
         waits while the planner runs (no planning latency in simulated time). Within a round only per-vehicle values (stages, verdicts,
         counts, piece totals, positions of heads) cross to the host; points, pieces and logs stay on the device.
@@ -1879,6 +1948,8 @@ class Evaluator:
         spent held."""
         if unknown not in ("free", "occupied"):
             raise ValueError(f"unknown must be 'free' or 'occupied', got {unknown!r}")
+        if explore and unknown != "occupied":
+            raise ValueError("explore=True plans through known space only: it needs unknown='occupied'")
         cams = list(sense_params) if isinstance(sense_params, (list, tuple)) else [sense_params if sense_params is not None else
                                                                                     globals()["sense_params"]()]
         if not cams:
@@ -1894,14 +1965,16 @@ class Evaluator:
                 if known_boxes is not None:
                     self.map_mark_known(known_boxes)
                 return self._navigate(starts, goals, rounds, horizon, sense_every, tol, plan_params, sim_params, cams, max_fields, stream,
-                                      fallback, brake_params, True)
+                                      fallback, brake_params, True,
+                                      (frontier_params if frontier_params is not None else True) if explore else None)
             finally:
                 self.set_unknown_policy(prev)
         return self._navigate(starts, goals, rounds, horizon, sense_every, tol, plan_params, sim_params, cams, max_fields, stream, fallback,
                               brake_params, False)
 
     def _navigate(self, starts, goals, rounds, horizon, sense_every, tol, plan_params, sim_params, cams, max_fields, stream, fallback,
-                  brake_params, occupied):
+                  brake_params, occupied, explore=None):
+        """explore: None (off), True or the FrontierParams of explore=True"""
         import torch
         dev = torch.device("cuda", self.device)
         s = torch.cuda.current_stream(dev) if stream is None else stream
@@ -1940,7 +2013,13 @@ class Evaluator:
         flown_rounds, replans, failed, uncert, brakes, held_rounds, commits = (np.zeros(B, dtype=np.int64) for _ in range(7))
         held, braking = np.zeros(B, dtype=bool), np.zeros(B, dtype=bool)   # held at rest; flying a stop
         committed = np.zeros(B, dtype=bool)                                # flying a commit (unknown="occupied")
-        actions, verdicts, replan_stages, replan_verdicts, logs, times = [], [], [], [], [], []
+        subgoal = np.zeros(B, dtype=bool)                                  # flying a plan to a frontier point (explore)
+        frontier_plans = np.zeros(B, dtype=np.int64)
+        if explore is not None:
+            fpar = explore if isinstance(explore, FrontierParams) else self.frontier_params()
+            pk = PlanParams.from_buffer_copy(bytes(p))
+            pk.flags |= PLAN_KNOWN_ONLY
+        actions, verdicts, replan_stages, replan_verdicts, subgoal_kinds, logs, times = [], [], [], [], [], [], []
         last = None   # (vehicle indices, log) of the last round flown
         stages = ("sense", "fuse", "check", "replan", "brake", "fly", "advance") if brake else ("sense", "fuse", "check", "replan", "fly", "advance")
         if occupied:
@@ -1952,6 +2031,7 @@ class Evaluator:
             ev = {k: (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for k in stages}
             action, verdict = np.full(B, NAV_IDLE), np.full(B, NAV_NO_TRAJECTORY)
             rstage, rverdict = np.full(B, NAV_NO_TRAJECTORY), np.full(B, NAV_NO_TRAJECTORY)
+            skind = np.full(B, -1)
             with torch.cuda.stream(s):
                 # 1. sense at the poses of the last flown segment (or the current state), then fuse what was seen
                 ev["sense"][0].record(s)
@@ -2029,8 +2109,28 @@ class Evaluator:
                     ok = [i for i in range(len(need)) if inside[i]]
                     if ok:
                         oi = torch.as_tensor(ok, device=dev)
-                        pl = self.plan_states_device(heads[oi].contiguous(), d_goals[torch.as_tensor([need[i] for i in ok], device=dev)].contiguous(),
-                                                     params=p, max_fields=max_fields, stream=s)
+                        hd, gd = heads[oi].contiguous(), d_goals[torch.as_tensor([need[i] for i in ok], device=dev)].contiguous()
+                        if explore is None:
+                            pl = self.plan_states_device(hd, gd, params=p, max_fields=max_fields, stream=s)
+                        else:   # sub-goals: the goal or a frontier point through known space (PLAN_KNOWN_ONLY); NONE as without explore
+                            fg, _ = self.frontier_goals_device(hd[:, :3].contiguous(), gd, params=fpar, max_fields=max_fields, stream=s)
+                            kinds = fg[:, 0:4].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
+                            pts = fg[:, 40:64].contiguous().view(torch.float64).reshape(-1, 3)
+                            ex = [j for j in range(len(ok)) if kinds[j] != FRONTIER_NONE]
+                            nx = [j for j in range(len(ok)) if kinds[j] == FRONTIER_NONE]
+                            parts = []
+                            if ex:
+                                xi = torch.as_tensor(ex, device=dev)
+                                parts.append(self.plan_states_device(hd[xi].contiguous(), pts[xi].contiguous(), params=pk, max_fields=max_fields, stream=s))
+                            if nx:
+                                xi = torch.as_tensor(nx, device=dev)
+                                parts.append(self.plan_states_device(hd[xi].contiguous(), gd[xi].contiguous(), params=p, max_fields=max_fields, stream=s))
+                            pl = _cat_plans(parts)
+                            for j in range(len(ok)):
+                                skind[need[ok[j]]] = kinds[j]
+                                if kinds[j] == FRONTIER_FRONTIER:
+                                    frontier_plans[need[ok[j]]] += 1
+                            ok = [ok[j] for j in ex + nx]   # the order of pl's plans
                         res = decode_plan_results(pl["results"])
                         stage = res["stage"].cpu().numpy()
                         csum = pl["certify"].reshape(-1, C.sizeof(CertifySummary))
@@ -2040,6 +2140,7 @@ class Evaluator:
                             rstage[need[i]], rverdict[need[i]] = stage[j], cv[j]
                             if stage[j] == OPTIMISED and cv[j] == CERTIFIED:
                                 new[need[i]] = j
+                                subgoal[need[i]] = skind[need[i]] == FRONTIER_FRONTIER
                             elif occupied and stage[j] == OPTIMISED and cv[j] == COLLIDING and ph[j] > 0:
                                 cand[need[i]] = (j, float(ph[j]))
                     for b in need:
@@ -2177,8 +2278,9 @@ class Evaluator:
                             uncert[b] += 1
                         if diverged[k]:
                             status[b] = NAV_DIVERGED
-                        elif n[b] == 0 and braking[b] and dist[k] > tol:
-                            held[b], braking[b], committed[b] = True, False, False   # the stop ran out: held at rest where the simulator left it
+                        elif n[b] == 0 and (braking[b] or subgoal[b]) and dist[k] > tol:
+                            # the stop (or a frontier plan) ran out: held at rest where the simulator left it
+                            held[b], braking[b], committed[b], subgoal[b] = True, False, False, False
                             init[b, 3:] = 0.0
                             init[b, 6] = 1.0
                             init[b, 13:17] = float(np.sqrt(sp.mass * sp.grav / (4 * sp.kf)))
@@ -2200,6 +2302,7 @@ class Evaluator:
             verdicts.append(verdict)
             replan_stages.append(rstage)
             replan_verdicts.append(rverdict)
+            subgoal_kinds.append(skind)
             if last is not None:
                 logs.append(last)
         status[status == NAV_ACTIVE] = NAV_TIMEOUT
@@ -2211,6 +2314,8 @@ class Evaluator:
             out.update(brakes=brakes, held_rounds=held_rounds)
         if occupied:
             out.update(commits=commits)
+        if explore is not None:
+            out.update(subgoal_kinds=np.array(subgoal_kinds).reshape(-1, B), frontier_plans=frontier_plans)
         return out
 
     def plan_info(self):
@@ -2598,6 +2703,61 @@ class Evaluator:
         """the fields from S starts (S, 3) in one relaxation into d_g (a raw device pointer to S*X*Y*Z float64), field s at d_g + s*X*Y*Z"""
         sts = _f64(starts).reshape(-1, 3)
         self._check(self.lib.isdf_frontend_path_fields_device(self.h, sts.shape[0], _dp(sts), _fpp(unknown_weight), d_g, stream))
+
+    # ---- frontiers of known space (see include/isdf.h, DESIGN §3.24) ----
+    def map_frontiers(self):
+        """-> dict(voxels (n,) int64 ascending, cluster_of (n,) int64, clusters: FRONTIER_CLUSTER_DTYPE array by ascending id, info dict)"""
+        info = FrontierInfo()
+        r = self.lib.isdf_map_frontiers(self.h, 0, None, None, 0, None, C.byref(info))
+        if r == -1 and (info.frontier_voxels > 0 or info.clusters > 0):
+            n, nc = int(info.frontier_voxels), int(info.clusters)
+            vox, cid = np.zeros(max(n, 1), dtype=np.int64), np.zeros(max(n, 1), dtype=np.int64)
+            tab = np.zeros(max(nc, 1), dtype=FRONTIER_CLUSTER_DTYPE)
+            r = self.lib.isdf_map_frontiers(self.h, n, vox.ctypes.data, cid.ctypes.data, nc, tab.ctypes.data, C.byref(info))
+            self._check(r)
+            return dict(voxels=vox[:n], cluster_of=cid[:n], clusters=tab[:nc], info=info.as_dict())
+        self._check(r)
+        return dict(voxels=np.zeros(0, dtype=np.int64), cluster_of=np.zeros(0, dtype=np.int64), clusters=np.zeros(0, dtype=FRONTIER_CLUSTER_DTYPE),
+                    info=info.as_dict())
+
+    def map_frontiers_device(self, cap_voxels, d_voxels, d_cluster_of, cap_clusters, d_clusters, stream=None):
+        """isdf_map_frontiers_device into raw device pointers (int64 x cap_voxels twice, 64-byte records x cap_clusters) -> info dict"""
+        info = FrontierInfo()
+        self._check(self.lib.isdf_map_frontiers_device(self.h, int(cap_voxels), d_voxels, d_cluster_of, int(cap_clusters), d_clusters,
+                                                       C.byref(info), stream))
+        return info.as_dict()
+
+    def frontier_params(self, **kw):
+        """isdf_frontier_default_params with any field overridden (goal_weight=, min_cluster_voxels=)"""
+        p = FrontierParams()
+        self._check(self.lib.isdf_frontier_default_params(C.byref(p)))
+        for k, v in kw.items():
+            if k not in {n for n, _ in FrontierParams._fields_}:
+                raise TypeError(f"unknown frontier parameter {k!r}")
+            setattr(p, k, v)
+        return p
+
+    def frontier_goals(self, starts, goals, params=None, max_fields=0):
+        """B (start, goal) pairs -> (FRONTIER_GOAL_DTYPE array (B,), info dict) through isdf_frontier_goals"""
+        sts, gls = _f64(starts).reshape(-1, 3), _f64(goals).reshape(-1, 3)
+        if sts.shape != gls.shape:
+            raise ValueError(f"starts and goals must both be (B, 3), got {sts.shape} and {gls.shape}")
+        out = np.zeros(sts.shape[0], dtype=FRONTIER_GOAL_DTYPE)
+        info = FrontierInfo()
+        self._check(self.lib.isdf_frontier_goals(self.h, sts.shape[0], _dp(sts), _dp(gls), None if params is None else C.byref(params),
+                                                 int(max_fields), out.ctypes.data, C.byref(info)))
+        return out, info.as_dict()
+
+    def frontier_goals_device(self, d_starts, d_goals, params=None, max_fields=0, stream=None):
+        """d_starts, d_goals: (B, 3) float64 CUDA tensors -> ((B, 64) uint8 CUDA tensor of isdf_frontier_goal records, info dict)"""
+        import torch
+        B = int(d_starts.shape[0])
+        out = torch.empty((B, C.sizeof(FrontierGoal)), dtype=torch.uint8, device=d_starts.device)
+        info = FrontierInfo()
+        sv = stream.cuda_stream if hasattr(stream, "cuda_stream") else stream
+        self._check(self.lib.isdf_frontier_goals_device(self.h, B, d_starts.data_ptr(), d_goals.data_ptr(), None if params is None else C.byref(params),
+                                                        int(max_fields), out.data_ptr(), C.byref(info), sv))
+        return out, info.as_dict()
 
     def frontend_path_info(self):
         out = FrontPathInfo()

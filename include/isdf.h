@@ -1046,8 +1046,16 @@ int isdf_frontend_path_fields_device(isdf_ctx *ctx, int S, const double *starts,
  *   with a shape the certificate refuses (checked before any work); ISDF_ERR_INVALID for a NULL argument, B < 1, the stages' own parameter
  *   checks, unknown flags, a non-zero reserved_ (also frontpath.reserved_), a negative or non-finite frontpath.unknown_weight,
  *   pieces_per_traj != 0 in p->certify or p->dynamics, a start or goal outside the map, or caps too small. On failure every stage is -1, midend_f / backend_f are NaN, and the summaries read as their certificates' failures. */
-/* 4 is not a flag (refused as unknown) */
-typedef enum isdf_plan_flags { ISDF_PLAN_CERTIFY = 1, ISDF_PLAN_DYNAMICS = 2, ISDF_PLAN_KNOWN_PREFIX = 8 } isdf_plan_flags;
+/* 4 is not a flag (refused as unknown).
+ * ISDF_PLAN_KNOWN_ONLY (DESIGN §3.24): step 1 runs over T_b (isdf_map_frontiers: in the map, neither occupied nor unknown, and a non-zero
+ *   feasibility mask on the blocked grid) instead of the traversable set; everything else in step 1 holds, so every path node but the start
+ *   is in T_b, every edge steps into a known voxel and frontpath.unknown_weight, still checked, changes no bit. Step 4 is
+ *   isdf_gather_obstacle_points_batch_known with every waypoint row known (known_rows = the plan's row count). It may be combined with
+ *   ISDF_PLAN_KNOWN_PREFIX, which then adds nothing. The mid-end, back end and certificates are unchanged; without the flag every output
+ *   keeps its bits. */
+typedef enum isdf_plan_flags {
+    ISDF_PLAN_CERTIFY = 1, ISDF_PLAN_DYNAMICS = 2, ISDF_PLAN_KNOWN_PREFIX = 8, ISDF_PLAN_KNOWN_ONLY = 16
+} isdf_plan_flags;
 typedef enum isdf_plan_stage {
     ISDF_PLAN_FAILED = -1, ISDF_PLAN_NO_PATH = 0, ISDF_PLAN_TOO_LONG = 1, ISDF_PLAN_MIDEND_FAILED = 2, ISDF_PLAN_OPTIMISED = 3
 } isdf_plan_stage;
@@ -1128,6 +1136,73 @@ int isdf_plan_states_device(isdf_ctx *ctx, int B, const double *d_starts, const 
                             double *d_coeffs, isdf_plan_result *d_results, isdf_certify_summary *d_certify,
                             isdf_dynamics_summary *d_dynamics, void *cuda_stream);
 int isdf_get_plan_info(isdf_ctx *ctx, isdf_plan_info *out);
+
+/* ---- frontiers of known space and frontier goals (DESIGN §3.24) ---------------------------------------------------------------------
+ * Definition (FP64, nothing contracted; voxel index ix*Y*Z + iy*Z + iz; cube centre as getGridCubeCenter, bmin + (i + 0.5) res)
+ *   T_o        the traversable set of the front end: in the map, not occupied, and a non-zero isdf_frontend_feasibility mask.
+ *   T_b        the same test on the BLOCKED grid occ | (~known within the map): in the map, not blocked (so known and free), and a
+ *              non-zero feasibility mask computed on the blocked grid (cells outside the map count as free, as for the feasibility call).
+ *              T_b is a subset of T_o. Nothing known: T_b is empty.
+ *   F          the frontier: v in T_b with some 26-neighbour u inside the map in T_o \ T_b. A place where the robot fits with every kernel
+ *              cell known free, next to a place where it would fit if unseen space were free.
+ *   Clusters   the 26-connected components of F. A cluster's id is its smallest voxel index; clusters are listed by ascending id. Size,
+ *              index box and centroid_a = bmin_a + ((double) sum of i_a / (double) size + 0.5) * res (exact integer sums: order-free).
+ * isdf_map_frontiers: the frontier voxels in ascending index (voxels, cap_voxels), each with its cluster id (cluster_of), and the cluster
+ *   table (clusters, cap_clusters). info (may be NULL) gets |T_b|, |F|, the cluster count and the stage times. A cap too small is
+ *   ISDF_ERR_INVALID with info holding the sizes needed (the outputs are then not written). The device form writes device buffers on
+ *   cuda_stream and returns when they are written.
+ * Errors: ISDF_ERR_STATE without a map or front-end kernels; ISDF_ERR_UNSUPPORTED on a sharded context; ISDF_ERR_INVALID for a NULL
+ *   output with a non-zero cap, a negative cap, or caps too small. */
+typedef struct isdf_frontier_cluster {   /* 64 bytes */
+    int64_t id;                           /* the smallest voxel index of the cluster */
+    int64_t size;                         /* voxels */
+    int32_t bmin[3], bmax[3];             /* index box, inclusive */
+    double centroid[3];
+} isdf_frontier_cluster;
+typedef struct isdf_frontier_info {       /* 72 bytes */
+    int64_t traversable_blocked;          /* |T_b| */
+    int64_t frontier_voxels;              /* |F| */
+    int64_t clusters;
+    int64_t reserved_;
+    double traversability_ms, frontier_ms, cluster_ms;   /* CUDA events: the two feasibility passes, F and its list, the labelling and table */
+    double field_ms, select_ms;           /* isdf_frontier_goals: the fields over T_b and the selection; 0 for isdf_map_frontiers */
+} isdf_frontier_info;
+int isdf_map_frontiers(isdf_ctx *ctx, int64_t cap_voxels, int64_t *voxels, int64_t *cluster_of, int64_t cap_clusters,
+                       isdf_frontier_cluster *clusters, isdf_frontier_info *info);
+int isdf_map_frontiers_device(isdf_ctx *ctx, int64_t cap_voxels, int64_t *d_voxels, int64_t *d_cluster_of, int64_t cap_clusters,
+                              isdf_frontier_cluster *d_clusters, isdf_frontier_info *info, void *cuda_stream);
+/* Frontier goals, per pair b: s and t are the start and goal voxels (path_voxel's rules: both in the map). g_b is the front end's field
+ * from s over T_b, unweighted (s need not be traversable).
+ *   1. g_b(t) < inf: kind GOAL, voxel t, cluster -1, g = score = g_b(t), point = the goal as given.
+ *   2. else among the frontier voxels f with g_b(f) < inf in clusters of at least min_cluster_voxels voxels, the least
+ *      score = g_b(f) + goal_weight * sqrt((dx*dx + dy*dy) + dz*dz), d = cube centre of f - goal; ties to the smaller voxel index:
+ *      kind FRONTIER, voxel f, its cluster id, g_b(f), the score, point = f's cube centre.
+ *   3. else kind NONE, voxel and cluster -1, g = score = +inf, point = the goal as given.
+ * Work: pairs whose starts share a voxel share a field; the fields are relaxed together up to max_fields at a time (0: a 4 GiB budget),
+ *   as isdf_frontend_path_pairs does. Guarantees: bit-identical run to run, host form to device form, under any permutation of the pairs
+ *   and for any max_fields. info (may be NULL) as for isdf_map_frontiers, with field_ms and select_ms.
+ * Errors: those of isdf_map_frontiers, and ISDF_ERR_INVALID for NULL arguments, B < 1, max_fields < 0, a start or goal outside the map or
+ *   not finite, goal_weight not finite or <= 0, min_cluster_voxels < 1, a non-zero reserved_. NULL params: the defaults. */
+typedef struct isdf_frontier_params {     /* 16 bytes */
+    double goal_weight;                   /* default 1 */
+    int32_t min_cluster_voxels;           /* default 1 */
+    int32_t reserved_;                    /* must be 0 */
+} isdf_frontier_params;
+typedef enum isdf_frontier_kind { ISDF_FRONTIER_NONE = 0, ISDF_FRONTIER_GOAL = 1, ISDF_FRONTIER_FRONTIER = 2 } isdf_frontier_kind;
+typedef struct isdf_frontier_goal {       /* 64 bytes */
+    int32_t kind;                         /* isdf_frontier_kind */
+    int32_t reserved_;
+    int64_t voxel, cluster;
+    double g, score;
+    double point[3];
+} isdf_frontier_goal;
+int isdf_frontier_default_params(isdf_frontier_params *p);
+int isdf_frontier_goals(isdf_ctx *ctx, int B, const double *starts, const double *goals, const isdf_frontier_params *p, int max_fields,
+                        isdf_frontier_goal *out, isdf_frontier_info *info);
+/* device form: d_starts, d_goals (B x 3) and d_out on ctx's device; the starts and goals are read to the host to group them. The call runs
+ * on cuda_stream and returns when d_out is written. */
+int isdf_frontier_goals_device(isdf_ctx *ctx, int B, const double *d_starts, const double *d_goals, const isdf_frontier_params *p,
+                               int max_fields, isdf_frontier_goal *d_out, isdf_frontier_info *info, void *cuda_stream);
 
 /* ---- executing a trajectory: getStateOnTrajStamp (swm:307-341) and the playback of SweptVolumeManager::process (swm:948-988) ----
  * B trajectories in isdf_plan_batch's ragged layout: trajectory b has pieces [piece_off[b], piece_off[b+1]), durations T[piece_off[b] + i],
