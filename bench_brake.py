@@ -93,8 +93,8 @@ def main():
             summ = torch.empty((len(grp), 56), dtype=torch.uint8, device="cuda")
             cp.clearance.pieces_per_traj = int(N)
             truth.trajectory_certify_device(len(grp) * int(N), gT.data_ptr(), gC.data_ptr(), cp, summ.data_ptr(), st.cuda_stream)
-            v = summ[:, 40:44].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
-            fh = summ[:, 24:32].contiguous().view(torch.float64).reshape(-1).cpu().numpy()
+            v = I._field(summ, I.CertifySummary, "verdict").cpu().numpy()
+            fh = I._field(summ, I.CertifySummary, "first_hit").cpu().numpy()
             verdicts[grp] = v
             ts[grp] = np.where(v == I.COLLIDING, fh, np.inf)
         d_ts = torch.as_tensor(ts, device="cuda")

@@ -4,6 +4,7 @@ Thin by design: every method is one C-ABI call with host numpy buffers, or devic
 `*_device` variants. There is NO fallback: if the shared library or a CUDA device is missing, loading /
 `Evaluator()` raises.
 """
+import contextlib
 import ctypes as C
 import os
 import numpy as np
@@ -809,12 +810,84 @@ def _cuda_f64(t):
 
 def decode_plan_results(records):
     """isdf_plan_result records (B x 64 uint8, as plan_pairs_device returns them; any device) -> dict of per-field tensors of length B"""
+    return {n: _field(records, PlanResult, n) for n, _ in PlanResult._fields_}
+
+
+def _field(rows, struct, name):
+    """field `name` of (n, sizeof(struct)) uint8 rows of ctypes struct records (a tensor on any device) -> its column as a tensor of the
+    field's type: (n,), or (n, k) for an array of k"""
     import torch
-    r = records.reshape(-1, C.sizeof(PlanResult)).contiguous()
-    i32, f64 = r[:, :32].contiguous().view(torch.int32), r[:, 32:].contiguous().view(torch.float64)
-    out = {n: i32[:, k] for k, (n, _) in enumerate(PlanResult._fields_[:8])}
-    out.update({n: f64[:, k] for k, (n, _) in enumerate(PlanResult._fields_[8:])})
-    return out
+    t = dict(struct._fields_)[name]
+    base = t._type_ if issubclass(t, C.Array) else t
+    dtype = {C.c_int32: torch.int32, C.c_int64: torch.int64, C.c_double: torch.float64}[base]
+    f = getattr(struct, name)
+    col = rows.reshape(-1, C.sizeof(struct))[:, f.offset:f.offset + f.size].contiguous().view(dtype)
+    return col if issubclass(t, C.Array) else col.reshape(-1)
+
+
+def _rows(d, off, j):
+    """trajectory j's (T, coeffs) in a ragged dict d (piece_off, T, coeffs), given its piece_off read to the host as off"""
+    a, e = int(off[j]), int(off[j + 1])
+    return d["T"][a:e], d["coeffs"][18 * a:18 * e]
+
+
+def _ragged(pieces, dev):
+    """(host offsets, piece_off int32 on dev, T, coeffs) of a list of trajectories (T, coeffs) in isdf_plan_batch's ragged layout, in list
+    order; without any piece, T and coeffs are one zero piece (the calls need non-NULL arrays)"""
+    import torch
+    offh = np.zeros(len(pieces) + 1, dtype=np.int64)
+    offh[1:] = np.cumsum([t.shape[0] for t, _ in pieces])
+    if offh[-1]:
+        T, Cc = torch.cat([t for t, _ in pieces]), torch.cat([c for _, c in pieces])
+    else:
+        T, Cc = torch.zeros(1, dtype=torch.float64, device=dev), torch.zeros(18, dtype=torch.float64, device=dev)
+    return offh, torch.as_tensor(offh.astype(np.int32), device=dev), T, Cc
+
+
+class _Fleet:
+    """Evaluator.navigate's trajectories, one per vehicle, in isdf_plan_batch's ragged layout: piece counts n and offsets offh on the host,
+    piece_off, T and coeffs on the device. T and coeffs may run past piece_off[B] (as trajectory_shift_device's output does)."""
+
+    def __init__(self, B, dev):
+        import torch
+        self.dev, self.n = dev, np.zeros(B, dtype=np.int64)
+        none = torch.zeros(0, dtype=torch.float64, device=dev)
+        self.replace({b: (none, none) for b in range(B)})
+
+    def pieces(self, b):
+        a, e = self.offh[b], self.offh[b + 1]
+        return self.T[a:e], self.coeffs[18 * a:18 * e]
+
+    def gather(self, vehicles):
+        """(piece_off int32, T, coeffs) of these vehicles' trajectories, in this order"""
+        return _ragged([self.pieces(b) for b in vehicles], self.dev)[1:]
+
+    def replace(self, new):
+        """vehicle b's trajectory becomes new[b] = (T, coeffs) (no pieces: none); the others keep theirs"""
+        self.offh, self.piece_off, self.T, self.coeffs = _ragged([new[b] if b in new else self.pieces(b) for b in range(self.n.size)], self.dev)
+        self.n = np.diff(self.offh)
+
+    def adopt(self, d):
+        """take trajectory_shift_device's output dict as the trajectories (one read of its piece_off)"""
+        self.piece_off, self.T, self.coeffs = d["piece_off"], d["T"], d["coeffs"]
+        self.offh = self.piece_off.cpu().numpy().astype(np.int64)
+        self.n = np.diff(self.offh)
+
+
+def _host_ragged(plans_or_ragged):
+    """plan_batch's list of dicts, or (piece_off, T, coeffs) in isdf_plan_batch's ragged layout -> (piece_off int32, T, coeffs) host arrays"""
+    if isinstance(plans_or_ragged, tuple):
+        off, T, Cc = plans_or_ragged
+        return np.ascontiguousarray(off, dtype=np.int32).reshape(-1), _f64(T).reshape(-1), _f64(Cc).reshape(-1)
+    return Evaluator.pack_plans(plans_or_ragged)
+
+
+@contextlib.contextmanager
+def _timed(events, stream):
+    """record the CUDA event pair events = (start, end) on stream around a block"""
+    events[0].record(stream)
+    yield
+    events[1].record(stream)
 
 
 def _dp(a):
@@ -1690,11 +1763,7 @@ class Evaluator:
     def trajectory_states(self, plans_or_ragged, traj, times):
         """the state of trajectory traj[q] at its local time times[q] -> (Q, 20) records: pos, vel, acc, jer, quat (w, x, y, z), omg, thr.
         plans_or_ragged: plan_batch's list of dicts, or (piece_off, T, coeffs) in isdf_plan_batch's ragged layout"""
-        if isinstance(plans_or_ragged, tuple):
-            off, T, Cc = plans_or_ragged
-            off, T, Cc = np.ascontiguousarray(off, dtype=np.int32).reshape(-1), _f64(T).reshape(-1), _f64(Cc).reshape(-1)
-        else:
-            off, T, Cc = self.pack_plans(plans_or_ragged)
+        off, T, Cc = _host_ragged(plans_or_ragged)
         tr = np.ascontiguousarray(traj, dtype=np.int32).reshape(-1)
         tm = _f64(times).reshape(-1)
         if tr.size != tm.size:
@@ -1714,11 +1783,7 @@ class Evaluator:
     def trajectory_shift(self, plans_or_ragged, t0):
         """isdf_trajectory_shift: the rest of each trajectory from its t0[b], re-timed to start at 0 -> (piece_off (B + 1 int32), T, coeffs)
         in the ragged layout, trimmed to piece_off[B] pieces. plans_or_ragged as in trajectory_states."""
-        if isinstance(plans_or_ragged, tuple):
-            off, T, Cc = plans_or_ragged
-            off, T, Cc = np.ascontiguousarray(off, dtype=np.int32).reshape(-1), _f64(T).reshape(-1), _f64(Cc).reshape(-1)
-        else:
-            off, T, Cc = self.pack_plans(plans_or_ragged)
+        off, T, Cc = _host_ragged(plans_or_ragged)
         B = off.size - 1
         t = _f64(t0).reshape(-1)
         if t.size != B:
@@ -1766,11 +1831,7 @@ class Evaluator:
         """isdf_trajectory_brake: a certified stop along each remaining trajectory, reaching no further than its time t_stop_max[b] ->
         (piece_off (B + 1 int32), T, coeffs) of the stops in the ragged layout (trimmed to piece_off[B] pieces), list of B summary dicts.
         plans_or_ragged as in trajectory_states."""
-        if isinstance(plans_or_ragged, tuple):
-            off, T, Cc = plans_or_ragged
-            off, T, Cc = np.ascontiguousarray(off, dtype=np.int32).reshape(-1), _f64(T).reshape(-1), _f64(Cc).reshape(-1)
-        else:
-            off, T, Cc = self.pack_plans(plans_or_ragged)
+        off, T, Cc = _host_ragged(plans_or_ragged)
         p = params if params is not None else self.brake_params()
         B = off.size - 1
         ts = _f64(t_stop_max).reshape(-1)
@@ -1833,11 +1894,7 @@ class Evaluator:
     def simulate(self, plans_or_ragged, traj, init, dist=None, params=None, cap_log=None):
         """fly rollouts r = 0..R-1 along trajectory traj[r] from init (R, 17) under the constant force / moment dist (R, 6) ->
         (log (R, n_log, 21), list of R summary dicts)"""
-        if isinstance(plans_or_ragged, tuple):
-            off, T, Cc = plans_or_ragged
-            off, T, Cc = np.ascontiguousarray(off, dtype=np.int32).reshape(-1), _f64(T).reshape(-1), _f64(Cc).reshape(-1)
-        else:
-            off, T, Cc = self.pack_plans(plans_or_ragged)
+        off, T, Cc = _host_ragged(plans_or_ragged)
         p = params if params is not None else sim_default_params()
         tr = np.ascontiguousarray(traj, dtype=np.int32).reshape(-1)
         ini = _f64(init).reshape(-1, SIM_INIT_DOUBLES)
@@ -1946,6 +2003,14 @@ class Evaluator:
         logs: per round (vehicle indices (R,) numpy, log (R, n_log, 21) CUDA tensor); times: per round {stage: ms} from CUDA events (a
         "brake" stage with fallback="brake"); with fallback="brake" also brakes and held_rounds (B,) numpy: BRAKED stops taken and rounds
         spent held."""
+        st0, gl = _f64(starts).reshape(-1, 3), _f64(goals).reshape(-1, 3)
+        B = st0.shape[0]
+        if gl.shape[0] != B or B < 1:
+            raise ValueError(f"starts and goals must both be (B, 3), B >= 1, got {st0.shape} and {gl.shape}")
+        if int(rounds) < 1 or not horizon > 0 or int(sense_every) < 1:
+            raise ValueError("rounds and sense_every must be >= 1 and horizon > 0")
+        if fallback not in ("keep", "brake"):
+            raise ValueError(f"fallback must be 'keep' or 'brake', got {fallback!r}")
         if unknown not in ("free", "occupied"):
             raise ValueError(f"unknown must be 'free' or 'occupied', got {unknown!r}")
         if explore and unknown != "occupied":
@@ -1954,368 +2019,295 @@ class Evaluator:
                                                                                     globals()["sense_params"]()]
         if not cams:
             raise ValueError("sense_params: an empty camera list")
-        if unknown == "occupied":
-            if fallback != "brake":
-                raise ValueError("unknown='occupied' commits to certified stops: it needs fallback='brake'")
-            if not all(np.isfinite(c.sensing_horizon) for c in cams):
-                raise ValueError("unknown='occupied' observes free space: every camera needs a finite sensing_horizon")
+        brake, occupied = fallback == "brake", unknown == "occupied"
+        if occupied and not brake:
+            raise ValueError("unknown='occupied' commits to certified stops: it needs fallback='brake'")
+        if occupied and not all(np.isfinite(c.sensing_horizon) for c in cams):
+            raise ValueError("unknown='occupied' observes free space: every camera needs a finite sensing_horizon")
+        if occupied:
             prev = self.unknown_policy()
             self.set_unknown_policy(UNKNOWN_OCCUPIED)
-            try:
-                if known_boxes is not None:
-                    self.map_mark_known(known_boxes)
-                return self._navigate(starts, goals, rounds, horizon, sense_every, tol, plan_params, sim_params, cams, max_fields, stream,
-                                      fallback, brake_params, True,
-                                      (frontier_params if frontier_params is not None else True) if explore else None)
-            finally:
+        try:
+            if occupied and known_boxes is not None:
+                self.map_mark_known(known_boxes)
+            return self._navigate(st0, gl, int(rounds), float(horizon), int(sense_every), tol, plan_params, sim_params, cams, max_fields,
+                                  stream, brake, brake_params, occupied, explore, frontier_params)
+        finally:
+            if occupied:
                 self.set_unknown_policy(prev)
-        return self._navigate(starts, goals, rounds, horizon, sense_every, tol, plan_params, sim_params, cams, max_fields, stream, fallback,
-                              brake_params, False)
 
-    def _navigate(self, starts, goals, rounds, horizon, sense_every, tol, plan_params, sim_params, cams, max_fields, stream, fallback,
-                  brake_params, occupied, explore=None):
-        """explore: None (off), True or the FrontierParams of explore=True"""
+    def _navigate(self, st0, gl, rounds, horizon, sense_every, tol, plan_params, sim_params, cams, max_fields, stream, brake, brake_params,
+                  occupied, explore, frontier_params):
+        """navigate's rounds, under the unknown policy navigate set"""
         import torch
-        dev = torch.device("cuda", self.device)
-        s = torch.cuda.current_stream(dev) if stream is None else stream
-        st0, gl = _f64(starts).reshape(-1, 3), _f64(goals).reshape(-1, 3)
-        B = st0.shape[0]
-        if gl.shape[0] != B or B < 1:
-            raise ValueError(f"starts and goals must both be (B, 3), B >= 1, got {st0.shape} and {gl.shape}")
-        if int(rounds) < 1 or not horizon > 0 or int(sense_every) < 1:
-            raise ValueError("rounds and sense_every must be >= 1 and horizon > 0")
         p = plan_params if plan_params is not None else self.plan_params()
         if not p.flags & PLAN_CERTIFY:
             raise ValueError("navigate checks trajectories with the certificate: plan_params needs PLAN_CERTIFY")
-        if fallback not in ("keep", "brake"):
-            raise ValueError(f"fallback must be 'keep' or 'brake', got {fallback!r}")
-        brake = fallback == "brake"
+        B, dev = st0.shape[0], torch.device("cuda", self.device)
+        s = torch.cuda.current_stream(dev) if stream is None else stream
+        sv, f64 = s.cuda_stream, dict(dtype=torch.float64, device=dev)
         bp = brake_params if brake_params is not None else self.brake_params(certify=p.certify, dynamics=p.dynamics)
         bpc = BrakeParams.from_buffer_copy(bytes(bp))   # a commit's stop
         bpc.certify.clearance.margin += NAV_COMMIT_SLACK
         sp = SimParams.from_buffer_copy(bytes(sim_params if sim_params is not None else sim_default_params()))
-        sp.t_end = float(horizon)
+        sp.t_end = horizon
+        hover = float(np.sqrt(sp.mass * sp.grav / (4 * sp.kf)))
         cp = CertifyParams.from_buffer_copy(bytes(p.certify))
         info = self.map_info()
         lo, hi = info["bmin"], info["bmax"]
-        f64 = dict(dtype=torch.float64, device=dev)
-        sv = s.cuda_stream
+        fpar = (frontier_params if frontier_params is not None else self.frontier_params()) if explore else None   # None: no explore
+        if fpar is not None:
+            pk = PlanParams.from_buffer_copy(bytes(p))
+            pk.flags |= PLAN_KNOWN_ONLY
+
+        def rest(x):   # at rest, level, at the hover rpm (as sim_init_from_trajectories)
+            x[..., 3:] = 0.0
+            x[..., 6] = 1.0
+            x[..., 13:17] = hover
+
         with torch.cuda.stream(s):
             d_goals = torch.as_tensor(gl, **f64)
-            init = torch.zeros((B, SIM_INIT_DOUBLES), **f64)   # at rest, level, at the hover rpm (as sim_init_from_trajectories)
+            init = torch.zeros((B, SIM_INIT_DOUBLES), **f64)
             init[:, 0:3] = torch.as_tensor(st0, **f64)
-            init[:, 6] = 1.0
-            init[:, 13:17] = float(np.sqrt(sp.mass * sp.grav / (4 * sp.kf)))
-            off = torch.zeros(B + 1, dtype=torch.int32, device=dev)      # the current trajectories, ragged; none yet
-            T, Cc = torch.zeros(1, **f64), torch.zeros(18, **f64)
-        n = np.zeros(B, dtype=np.int64)                                    # their piece counts (host)
+            rest(init)
+            fleet = _Fleet(B, dev)   # the current trajectories; none yet
         status = np.full(B, NAV_ACTIVE)
-        flown_rounds, replans, failed, uncert, brakes, held_rounds, commits = (np.zeros(B, dtype=np.int64) for _ in range(7))
+        flown_rounds, replans, failed, uncert, brakes, held_rounds, commits, frontier_plans = (np.zeros(B, dtype=np.int64) for _ in range(8))
         held, braking = np.zeros(B, dtype=bool), np.zeros(B, dtype=bool)   # held at rest; flying a stop
         committed = np.zeros(B, dtype=bool)                                # flying a commit (unknown="occupied")
         subgoal = np.zeros(B, dtype=bool)                                  # flying a plan to a frontier point (explore)
-        frontier_plans = np.zeros(B, dtype=np.int64)
-        if explore is not None:
-            fpar = explore if isinstance(explore, FrontierParams) else self.frontier_params()
-            pk = PlanParams.from_buffer_copy(bytes(p))
-            pk.flags |= PLAN_KNOWN_ONLY
-        actions, verdicts, replan_stages, replan_verdicts, subgoal_kinds, logs, times = [], [], [], [], [], [], []
+        actions, subgoal_kinds = np.full((rounds, B), NAV_IDLE), np.full((rounds, B), -1)   # per round
+        verdicts, replan_stages, replan_verdicts = (np.full((rounds, B), NAV_NO_TRAJECTORY) for _ in range(3))
+        logs, times = [], []
         last = None   # (vehicle indices, log) of the last round flown
-        stages = ("sense", "fuse", "check", "replan", "brake", "fly", "advance") if brake else ("sense", "fuse", "check", "replan", "fly", "advance")
-        if occupied:
-            stages = ("sense", "fuse", "observe") + stages[2:]
-        for r in range(int(rounds)):
+        stages = ("sense", "fuse") + ("observe",) * occupied + ("check", "replan") + ("brake",) * brake + ("fly", "advance")
+
+        def sense(act):
+            """the poses to sense from: every sense_every-th record of the last flown segment and its final record, else the state"""
+            recs = []
+            flown = set() if last is None else set(last[0].tolist())
+            if last is not None:
+                li, lg = last
+                keep = np.isin(li, act)
+                if keep.any():
+                    n_log = lg.shape[1]
+                    rows = sorted(set(range(0, n_log, sense_every)) | {n_log - 1})
+                    sel = lg[torch.as_tensor(np.nonzero(keep)[0], device=dev)][:, rows].reshape(-1, SIM_DOUBLES)
+                    recs.append(torch.cat([sel[:, 1:4], sel[:, 7:11]], 1))
+            others = [b for b in act if b not in flown]
+            if others:
+                ini = init[torch.as_tensor(others, device=dev)]
+                recs.append(torch.cat([ini[:, 0:3], ini[:, 6:10]], 1))
+            return torch.cat(recs).contiguous()
+
+        def check(act):
+            """vehicle -> the certificate's verdict (and first_hit) of its remaining trajectory, one call per piece count"""
+            ver, fhit = {}, {}
+            have = [b for b in act if fleet.n[b] > 0]
+            for N in sorted({int(fleet.n[b]) for b in have}):
+                grp = [b for b in have if fleet.n[b] == N]
+                _, gT, gC = fleet.gather(grp)
+                gC = gC.reshape(len(grp), 3, 6 * N).permute(1, 0, 2).contiguous()
+                summ = torch.empty((len(grp), C.sizeof(CertifySummary)), dtype=torch.uint8, device=dev)
+                cp.clearance.pieces_per_traj = N
+                self.trajectory_certify_device(len(grp) * N, gT.data_ptr(), gC.data_ptr(), cp, summ.data_ptr(), sv)
+                ver.update(zip(grp, _field(summ, CertifySummary, "verdict").cpu().numpy().tolist()))
+                if brake:
+                    fhit.update(zip(grp, _field(summ, CertifySummary, "first_hit").cpu().numpy().tolist()))
+            return ver, fhit
+
+        def heads(need):
+            """the replan heads (p, v, a) of these vehicles: the remaining trajectory's state at 0, else at rest where they are"""
+            hd = torch.zeros((len(need), 9), **f64)
+            moving = [i for i, b in enumerate(need) if fleet.n[b] > 0]
+            if moving:
+                q = torch.as_tensor([need[i] for i in moving], dtype=torch.int32, device=dev)
+                out = torch.empty((len(moving), STATE_DOUBLES), **f64)
+                self.trajectory_states_device(B, fleet.piece_off.data_ptr(), fleet.T.data_ptr(), fleet.coeffs.data_ptr(), len(moving), q.data_ptr(),
+                                              torch.zeros(len(moving), **f64).data_ptr(), out.data_ptr(), sv)
+                hd[torch.as_tensor(moving, device=dev)] = out[:, :9]
+            still = [i for i, b in enumerate(need) if fleet.n[b] == 0]
+            if still:   # never flown (init holds its start), or held at rest at its simulator position
+                hd[torch.as_tensor(still, device=dev), :3] = init[torch.as_tensor([need[i] for i in still], device=dev), 0:3]
+            return hd
+
+        def plan(hd, gd, vs):
+            """plan_states_device for vehicles vs from heads hd to goals gd -> (plans, their vehicles in plan order); with explore, GOAL and
+            FRONTIER sub-goals plan known-only to the goal or the frontier point, NONE as without explore"""
+            if fpar is None:
+                return self.plan_states_device(hd, gd, params=p, max_fields=max_fields, stream=s), vs
+            fg, _ = self.frontier_goals_device(hd[:, :3].contiguous(), gd, params=fpar, max_fields=max_fields, stream=s)
+            kinds = _field(fg, FrontierGoal, "kind").cpu().numpy()
+            pts = _field(fg, FrontierGoal, "point")
+            ex = [j for j in range(len(vs)) if kinds[j] != FRONTIER_NONE]
+            nx = [j for j in range(len(vs)) if kinds[j] == FRONTIER_NONE]
+            parts = []
+            for js, to, params in ((ex, pts, pk), (nx, gd, p)):
+                if js:
+                    xi = torch.as_tensor(js, device=dev)
+                    parts.append(self.plan_states_device(hd[xi].contiguous(), to[xi].contiguous(), params=params, max_fields=max_fields, stream=s))
+            for j, b in enumerate(vs):
+                skind[b] = kinds[j]
+                if kinds[j] == FRONTIER_FRONTIER:
+                    frontier_plans[b] += 1
+            return _cat_plans(parts), [vs[j] for j in ex + nx]
+
+        def replan(act, ver):
+            """replan the vehicles without a certified remaining trajectory (or flying a commit) and splice the accepted plans in ->
+            (vehicles replanned, vehicle -> plan of an accepted plan, vehicle -> (plan, first_hit) to commit to a stop of, plans)"""
+            need = [b for b in act if ver.get(b) != CERTIFIED or committed[b]]
+            for b in ver:
+                verdict[b] = ver[b]
+            new, cand, pl = {}, {}, None
+            if need:
+                hd = heads(need)
+                hp = hd[:, :3].cpu().numpy()
+                inside = np.all((hp >= lo) & (hp <= hi), axis=1)   # a head outside the map fails without a call
+                ok = [i for i in range(len(need)) if inside[i]]
+                if ok:
+                    vs = [need[i] for i in ok]
+                    pl, vs = plan(hd[torch.as_tensor(ok, device=dev)].contiguous(), d_goals[torch.as_tensor(vs, device=dev)].contiguous(), vs)
+                    stage = _field(pl["results"], PlanResult, "stage").cpu().numpy()
+                    cv = _field(pl["certify"], CertifySummary, "verdict").cpu().numpy()
+                    ph = _field(pl["certify"], CertifySummary, "first_hit").cpu().numpy() if occupied else None
+                    for j, b in enumerate(vs):
+                        rstage[b], rverdict[b] = stage[j], cv[j]
+                        if stage[j] == OPTIMISED and cv[j] == CERTIFIED:
+                            new[b] = j
+                            subgoal[b] = skind[b] == FRONTIER_FRONTIER
+                        elif occupied and stage[j] == OPTIMISED and cv[j] == COLLIDING and ph[j] > 0:
+                            cand[b] = (j, float(ph[j]))
+                for b in need:
+                    replans[b] += 1
+                    if b in new:
+                        action[b], verdict[b] = NAV_REPLANNED, CERTIFIED
+                        held[b] = braking[b] = committed[b] = False
+                    else:
+                        action[b] = NAV_REPLAN_FAILED
+                        failed[b] += 1
+                        if held[b]:
+                            action[b] = NAV_HELD
+                            held_rounds[b] += 1
+                if new:   # the trajectories flown this round: the accepted plans, else the remaining ones
+                    po = pl["piece_off"].cpu().numpy()
+                    fleet.replace({b: _rows(pl, po, j) for b, j in new.items()})
+            for b in act:
+                if action[b] == NAV_IDLE:
+                    action[b] = NAV_KEPT
+            return need, new, cand, pl
+
+        def stops(vs, ragged, t_stop_max, params):
+            """one trajectory_brake_device call along vehicles vs's trajectories ragged -> vehicle -> (T, coeffs) of its BRAKED stop"""
+            bk = self.trajectory_brake_device(*ragged, torch.as_tensor(t_stop_max, **f64), params=params, stream=s)
+            ok = _field(bk["summary"], BrakeSummary, "status").cpu().numpy() == BRAKED
+            if not ok.any():
+                return {}
+            ko = bk["piece_off"].cpu().numpy()
+            return {b: _rows(bk, ko, j) for j, b in enumerate(vs) if ok[j]}
+
+        def fall_back(need, new, cand, pl, ver, fhit):
+            """commit to a certified stop along a new plan that collides further on; else brake along the remaining trajectory"""
+            took = {}
+            if cand:
+                po = pl["piece_off"].cpu().numpy()
+                # with the slack first; where no stop keeps it (passing close to unseen space, e.g. round a corner), the plan's margin
+                for params in (bpc, bp):
+                    vs = [b for b in sorted(cand) if b not in took]
+                    if vs:
+                        took.update(stops(vs, _ragged([_rows(pl, po, cand[b][0]) for b in vs], dev)[1:], [cand[b][1] for b in vs], params))
+                for b in took:
+                    if action[b] == NAV_HELD:
+                        held_rounds[b] -= 1
+                    action[b], verdict[b] = NAV_COMMITTED, CERTIFIED
+                    commits[b] += 1
+                    held[b], braking[b], committed[b] = False, True, True
+                if took:
+                    fleet.replace(took)
+            # (a vehicle still holding a CERTIFIED remaining trajectory, a commit, keeps it)
+            bv = [b for b in need if b not in new and b not in took and fleet.n[b] > 0 and ver.get(b) != CERTIFIED]
+            got = stops(bv, fleet.gather(bv), [fhit[b] if ver[b] == COLLIDING else np.inf for b in bv], bp) if bv else {}
+            for b in got:
+                action[b], verdict[b] = NAV_BRAKED, CERTIFIED
+                brakes[b] += 1
+                braking[b] = True
+            if got:
+                fleet.replace(got)
+
+        def advance(fly, fi, sim):
+            """the state at the horizon and the rest of each trajectory; vehicles that arrive, stop, diverge or are held"""
+            init[fi] = sim_init_from_log(sim["log"][:, -1])
+            diverged = _field(sim["summary"], SimSummary, "diverged").cpu().numpy()
+            t0 = torch.zeros(B, **f64)
+            t0[fi] = horizon
+            fleet.adopt(self.trajectory_shift_device(fleet.piece_off, fleet.T, fleet.coeffs, t0, stream=s))
+            dist = torch.linalg.norm(init[fi, 0:3] - d_goals[fi], dim=1).cpu().numpy()
+            for k, b in enumerate(fly):
+                flown_rounds[b] += 1
+                if verdict[b] != CERTIFIED:
+                    uncert[b] += 1
+                if diverged[k]:
+                    status[b] = NAV_DIVERGED
+                elif fleet.n[b] == 0 and (braking[b] or subgoal[b]) and dist[k] > tol:
+                    # the stop (or a frontier plan) ran out: held at rest where the simulator left it
+                    held[b], braking[b], committed[b], subgoal[b] = True, False, False, False
+                    rest(init[b])
+                elif fleet.n[b] == 0:
+                    status[b] = NAV_ARRIVED if dist[k] <= tol else NAV_STOPPED
+            gone = [b for b in range(B) if status[b] != NAV_ACTIVE and fleet.n[b] > 0]
+            if gone:   # a vehicle that is done flies no more: its pieces go
+                fleet.replace({b: (fleet.T[:0], fleet.coeffs[:0]) for b in gone})
+
+        for r in range(rounds):
             act = np.nonzero(status == NAV_ACTIVE)[0]
             if act.size == 0:
                 break
             ev = {k: (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for k in stages}
-            action, verdict = np.full(B, NAV_IDLE), np.full(B, NAV_NO_TRAJECTORY)
-            rstage, rverdict = np.full(B, NAV_NO_TRAJECTORY), np.full(B, NAV_NO_TRAJECTORY)
-            skind = np.full(B, -1)
+            action, verdict, rstage, rverdict, skind = actions[r], verdicts[r], replan_stages[r], replan_verdicts[r], subgoal_kinds[r]
             with torch.cuda.stream(s):
-                # 1. sense at the poses of the last flown segment (or the current state), then fuse what was seen
-                ev["sense"][0].record(s)
-                recs = []
-                flown_last = set() if last is None else set(last[0].tolist())
-                if last is not None:
-                    li, lg = last
-                    keep = np.isin(li, act)
-                    if keep.any():
-                        n_log = lg.shape[1]
-                        rows = sorted(set(range(0, n_log, int(sense_every))) | {n_log - 1})
-                        sel = lg[torch.as_tensor(np.nonzero(keep)[0], device=dev)][:, rows].reshape(-1, SIM_DOUBLES)
-                        recs.append(torch.cat([sel[:, 1:4], sel[:, 7:11]], 1))
-                rest = [b for b in act if b not in flown_last]
-                if rest:
-                    ini = init[torch.as_tensor(rest, device=dev)]
-                    recs.append(torch.cat([ini[:, 0:3], ini[:, 6:10]], 1))
-                poses = torch.cat(recs).contiguous()
-                seen = [self.sense_cloud_device(poses, 0, 3, params=cam, stream=s)[0] for cam in cams]
-                ev["sense"][1].record(s)
-                ev["fuse"][0].record(s)
-                for pts in seen:
-                    if pts.shape[0]:
-                        self.map_fuse_cloud_device(pts, stream=sv)
-                ev["fuse"][1].record(s)
-                if occupied:   # 1b. the free space the same images prove
-                    ev["observe"][0].record(s)
-                    for cam in cams:
-                        self.map_observe_device(poses, 0, 3, params=cam, stream=s)
-                    ev["observe"][1].record(s)
-                # 2. check every remaining trajectory on the fused map
-                ev["check"][0].record(s)
-                offh = np.zeros(B + 1, dtype=np.int64)
-                offh[1:] = np.cumsum(n)
-                have = [b for b in act if n[b] > 0]
-                ver, fhit = {}, {}
-                for N in sorted({int(n[b]) for b in have}):
-                    grp = [b for b in have if n[b] == N]
-                    base = torch.as_tensor(offh[grp], device=dev)
-                    gT = T[(base[:, None] + torch.arange(N, device=dev)[None]).reshape(-1)].contiguous()
-                    gC = Cc[(18 * base[:, None] + torch.arange(18 * N, device=dev)[None])].reshape(len(grp), 3, 6 * N).permute(1, 0, 2).contiguous()
-                    summ = torch.empty((len(grp), C.sizeof(CertifySummary)), dtype=torch.uint8, device=dev)
-                    cp.clearance.pieces_per_traj = N
-                    self.trajectory_certify_device(len(grp) * N, gT.data_ptr(), gC.data_ptr(), cp, summ.data_ptr(), sv)
-                    v = summ[:, 40:44].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
-                    ver.update(zip(grp, v.tolist()))
-                    if brake:
-                        fhit.update(zip(grp, summ[:, 24:32].contiguous().view(torch.float64).reshape(-1).cpu().numpy().tolist()))
-                ev["check"][1].record(s)
-                # 3. replan the vehicles without a certified remaining trajectory
-                ev["replan"][0].record(s)
-                need = [b for b in act if ver.get(b) != CERTIFIED or committed[b]]
-                for b in act:
-                    if b in ver:
-                        verdict[b] = ver[b]
-                new = {}   # vehicle -> (plan index) of an accepted plan
-                cand = {}  # unknown="occupied": vehicle -> (plan index, first_hit) of an optimised plan to commit to a stop of
-                if need:
-                    heads = torch.zeros((len(need), 9), **f64)
-                    moving = [i for i, b in enumerate(need) if n[b] > 0]
-                    if moving:
-                        q = torch.as_tensor([need[i] for i in moving], dtype=torch.int32, device=dev)
-                        out = torch.empty((len(moving), STATE_DOUBLES), **f64)
-                        self.trajectory_states_device(B, off.data_ptr(), T.data_ptr(), Cc.data_ptr(), len(moving), q.data_ptr(),
-                                                      torch.zeros(len(moving), **f64).data_ptr(), out.data_ptr(), sv)
-                        heads[torch.as_tensor(moving, device=dev)] = out[:, :9]
-                    still = [i for i, b in enumerate(need) if n[b] == 0]
-                    if still:
-                        heads[torch.as_tensor(still, device=dev), :3] = torch.as_tensor(st0[[need[i] for i in still]], **f64)
-                        hs = [i for i in still if held[need[i]]]
-                        if hs:   # a held vehicle replans from rest at its simulator position
-                            heads[torch.as_tensor(hs, device=dev), :3] = init[torch.as_tensor([need[i] for i in hs], device=dev), 0:3]
-                    hp = heads[:, :3].cpu().numpy()
-                    inside = np.all((hp >= lo) & (hp <= hi), axis=1)
-                    ok = [i for i in range(len(need)) if inside[i]]
-                    if ok:
-                        oi = torch.as_tensor(ok, device=dev)
-                        hd, gd = heads[oi].contiguous(), d_goals[torch.as_tensor([need[i] for i in ok], device=dev)].contiguous()
-                        if explore is None:
-                            pl = self.plan_states_device(hd, gd, params=p, max_fields=max_fields, stream=s)
-                        else:   # sub-goals: the goal or a frontier point through known space (PLAN_KNOWN_ONLY); NONE as without explore
-                            fg, _ = self.frontier_goals_device(hd[:, :3].contiguous(), gd, params=fpar, max_fields=max_fields, stream=s)
-                            kinds = fg[:, 0:4].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
-                            pts = fg[:, 40:64].contiguous().view(torch.float64).reshape(-1, 3)
-                            ex = [j for j in range(len(ok)) if kinds[j] != FRONTIER_NONE]
-                            nx = [j for j in range(len(ok)) if kinds[j] == FRONTIER_NONE]
-                            parts = []
-                            if ex:
-                                xi = torch.as_tensor(ex, device=dev)
-                                parts.append(self.plan_states_device(hd[xi].contiguous(), pts[xi].contiguous(), params=pk, max_fields=max_fields, stream=s))
-                            if nx:
-                                xi = torch.as_tensor(nx, device=dev)
-                                parts.append(self.plan_states_device(hd[xi].contiguous(), gd[xi].contiguous(), params=p, max_fields=max_fields, stream=s))
-                            pl = _cat_plans(parts)
-                            for j in range(len(ok)):
-                                skind[need[ok[j]]] = kinds[j]
-                                if kinds[j] == FRONTIER_FRONTIER:
-                                    frontier_plans[need[ok[j]]] += 1
-                            ok = [ok[j] for j in ex + nx]   # the order of pl's plans
-                        res = decode_plan_results(pl["results"])
-                        stage = res["stage"].cpu().numpy()
-                        csum = pl["certify"].reshape(-1, C.sizeof(CertifySummary))
-                        cv = csum[:, 40:44].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
-                        ph = csum[:, 24:32].contiguous().view(torch.float64).reshape(-1).cpu().numpy() if occupied else None
-                        for j, i in enumerate(ok):
-                            rstage[need[i]], rverdict[need[i]] = stage[j], cv[j]
-                            if stage[j] == OPTIMISED and cv[j] == CERTIFIED:
-                                new[need[i]] = j
-                                subgoal[need[i]] = skind[need[i]] == FRONTIER_FRONTIER
-                            elif occupied and stage[j] == OPTIMISED and cv[j] == COLLIDING and ph[j] > 0:
-                                cand[need[i]] = (j, float(ph[j]))
-                    for b in need:
-                        replans[b] += 1
-                        if b in new:
-                            action[b], verdict[b] = NAV_REPLANNED, CERTIFIED
-                            held[b] = braking[b] = committed[b] = False
-                        else:
-                            action[b] = NAV_REPLAN_FAILED
-                            failed[b] += 1
-                            if held[b]:
-                                action[b] = NAV_HELD
-                                held_rounds[b] += 1
-                    # the trajectories flown this round: the accepted plans, else the remaining ones
-                    if new:
-                        po = pl["piece_off"].cpu().numpy()
-                        nn = n.copy()
-                        partsT, partsC = [], []
-                        for b in range(B):
-                            if b in new:
-                                j = new[b]
-                                a, e = int(po[j]), int(po[j + 1])
-                                partsT.append(pl["T"][a:e]); partsC.append(pl["coeffs"][18 * a:18 * e])
-                                nn[b] = e - a
-                            elif n[b] > 0:
-                                partsT.append(T[offh[b]:offh[b + 1]]); partsC.append(Cc[18 * offh[b]:18 * offh[b + 1]])
-                        n = nn
-                        T, Cc = torch.cat(partsT).contiguous(), torch.cat(partsC).contiguous()
-                        offh = np.zeros(B + 1, dtype=np.int64)
-                        offh[1:] = np.cumsum(n)
-                        off = torch.as_tensor(offh.astype(np.int32), device=dev)
-                for b in act:
-                    if action[b] == NAV_IDLE:
-                        action[b] = NAV_KEPT
-                ev["replan"][1].record(s)
+                with _timed(ev["sense"], s):
+                    poses = sense(act)
+                    seen = [self.sense_cloud_device(poses, 0, 3, params=cam, stream=s)[0] for cam in cams]
+                with _timed(ev["fuse"], s):
+                    for pts in seen:
+                        if pts.shape[0]:
+                            self.map_fuse_cloud_device(pts, stream=sv)
+                if occupied:   # the free space the same images prove
+                    with _timed(ev["observe"], s):
+                        for cam in cams:
+                            self.map_observe_device(poses, 0, 3, params=cam, stream=s)
+                with _timed(ev["check"], s):
+                    ver, fhit = check(act)
+                with _timed(ev["replan"], s):
+                    need, new, cand, pl = replan(act, ver)
                 if brake:
-                    # the fallback: a certified stop along the remaining trajectory of every vehicle whose replan failed
-                    ev["brake"][0].record(s)
-                    took = set()   # vehicles that committed to a stop of their new plan
-                    if cand:
-                        po = pl["piece_off"].cpu().numpy()
-
-                        def commit_stops(cb, params):   # vehicle -> (T, coeffs) of a BRAKED stop along its new plan
-                            bo = np.zeros(len(cb) + 1, dtype=np.int64)
-                            bo[1:] = np.cumsum([po[cand[b][0] + 1] - po[cand[b][0]] for b in cb])
-                            bT = torch.cat([pl["T"][po[cand[b][0]]:po[cand[b][0] + 1]] for b in cb]).contiguous()
-                            bC = torch.cat([pl["coeffs"][18 * po[cand[b][0]]:18 * po[cand[b][0] + 1]] for b in cb]).contiguous()
-                            ts = torch.as_tensor([cand[b][1] for b in cb], **f64)
-                            bk = self.trajectory_brake_device(torch.as_tensor(bo.astype(np.int32), device=dev), bT, bC, ts, params=params, stream=s)
-                            bst = bk["summary"][:, 0:4].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
-                            ko = bk["piece_off"].cpu().numpy()
-                            return {b: (bk["T"][ko[j]:ko[j + 1]], bk["coeffs"][18 * ko[j]:18 * ko[j + 1]]) for j, b in enumerate(cb) if bst[j] == BRAKED}
-                        # with the slack first; where no stop keeps it (passing close to unseen space, e.g. round a corner), the plan's margin
-                        got = commit_stops(sorted(cand), bpc)
-                        rest = [b for b in sorted(cand) if b not in got]
-                        if rest:
-                            got.update(commit_stops(rest, bp))
-                        if got:
-                            nn = n.copy()
-                            partsT, partsC = [], []
-                            for b in range(B):
-                                if b in got:
-                                    partsT.append(got[b][0]); partsC.append(got[b][1])
-                                    nn[b] = got[b][0].shape[0]
-                                    if action[b] == NAV_HELD:
-                                        held_rounds[b] -= 1
-                                    action[b], verdict[b] = NAV_COMMITTED, CERTIFIED
-                                    commits[b] += 1
-                                    held[b], braking[b], committed[b] = False, True, True
-                                elif n[b] > 0:
-                                    partsT.append(T[offh[b]:offh[b + 1]]); partsC.append(Cc[18 * offh[b]:18 * offh[b + 1]])
-                            n = nn
-                            T, Cc = torch.cat(partsT).contiguous(), torch.cat(partsC).contiguous()
-                            offh = np.zeros(B + 1, dtype=np.int64)
-                            offh[1:] = np.cumsum(n)
-                            off = torch.as_tensor(offh.astype(np.int32), device=dev)
-                            took = set(got)
-                    # (a vehicle still holding a CERTIFIED remaining trajectory, a commit, keeps it)
-                    bv = [b for b in need if b not in new and b not in took and n[b] > 0 and ver.get(b) != CERTIFIED]
-                    if bv:
-                        bo = np.zeros(len(bv) + 1, dtype=np.int64)
-                        bo[1:] = np.cumsum(n[bv])
-                        bT = torch.cat([T[offh[b]:offh[b + 1]] for b in bv]).contiguous()
-                        bC = torch.cat([Cc[18 * offh[b]:18 * offh[b + 1]] for b in bv]).contiguous()
-                        ts = torch.as_tensor([fhit[b] if ver[b] == COLLIDING else np.inf for b in bv], **f64)
-                        bk = self.trajectory_brake_device(torch.as_tensor(bo.astype(np.int32), device=dev), bT, bC, ts, params=bp, stream=s)
-                        bst = bk["summary"][:, 0:4].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
-                        got = {b: j for j, b in enumerate(bv) if bst[j] == BRAKED}
-                        if got:
-                            ko = bk["piece_off"].cpu().numpy()
-                            nn = n.copy()
-                            partsT, partsC = [], []
-                            for b in range(B):
-                                if b in got:
-                                    j = got[b]
-                                    a, e = int(ko[j]), int(ko[j + 1])
-                                    partsT.append(bk["T"][a:e]); partsC.append(bk["coeffs"][18 * a:18 * e])
-                                    nn[b] = e - a
-                                    action[b], verdict[b] = NAV_BRAKED, CERTIFIED
-                                    brakes[b] += 1
-                                    braking[b] = True
-                                elif n[b] > 0:
-                                    partsT.append(T[offh[b]:offh[b + 1]]); partsC.append(Cc[18 * offh[b]:18 * offh[b + 1]])
-                            n = nn
-                            T, Cc = torch.cat(partsT).contiguous(), torch.cat(partsC).contiguous()
-                            offh = np.zeros(B + 1, dtype=np.int64)
-                            offh[1:] = np.cumsum(n)
-                            off = torch.as_tensor(offh.astype(np.int32), device=dev)
-                    ev["brake"][1].record(s)
-                # 4. fly the vehicles that have a trajectory
-                ev["fly"][0].record(s)
-                fly = np.array([b for b in act if n[b] > 0], dtype=np.int64)
-                last = None
-                if fly.size:
-                    fi = torch.as_tensor(fly, device=dev)
-                    sim = self.simulate_device(off, T, Cc, fi.to(torch.int32), init[fi].contiguous(), params=sp, stream=s)
-                    last = (fly, sim["log"])
-                ev["fly"][1].record(s)
-                # 5. advance: the state at the horizon and the rest of each trajectory
-                ev["advance"][0].record(s)
-                if fly.size:
-                    lg = sim["log"]
-                    init[fi] = sim_init_from_log(lg[:, -1])
-                    diverged = sim["summary"][:, 84:88].contiguous().view(torch.int32).reshape(-1).cpu().numpy()
-                    t0 = torch.zeros(B, **f64)
-                    t0[fi] = float(horizon)
-                    sh = self.trajectory_shift_device(off, T, Cc, t0, stream=s)
-                    offh = sh["piece_off"].cpu().numpy().astype(np.int64)
-                    n = np.diff(offh)
-                    off, T, Cc = sh["piece_off"], sh["T"], sh["coeffs"]
-                    dist = torch.linalg.norm(init[fi, 0:3] - d_goals[fi], dim=1).cpu().numpy()
-                    for k, b in enumerate(fly):
-                        flown_rounds[b] += 1
-                        if verdict[b] != CERTIFIED:
-                            uncert[b] += 1
-                        if diverged[k]:
-                            status[b] = NAV_DIVERGED
-                        elif n[b] == 0 and (braking[b] or subgoal[b]) and dist[k] > tol:
-                            # the stop (or a frontier plan) ran out: held at rest where the simulator left it
-                            held[b], braking[b], committed[b], subgoal[b] = True, False, False, False
-                            init[b, 3:] = 0.0
-                            init[b, 6] = 1.0
-                            init[b, 13:17] = float(np.sqrt(sp.mass * sp.grav / (4 * sp.kf)))
-                        elif n[b] == 0:
-                            status[b] = NAV_ARRIVED if dist[k] <= tol else NAV_STOPPED
-                    done = status != NAV_ACTIVE
-                    if done.any() and n[done].any():   # a vehicle that is done flies no more: its pieces go
-                        keep = [b for b in range(B) if n[b] > 0 and not done[b]]
-                        T = torch.cat([T[offh[b]:offh[b + 1]] for b in keep] or [torch.zeros(1, **f64)]).contiguous()
-                        Cc = torch.cat([Cc[18 * offh[b]:18 * offh[b + 1]] for b in keep] or [torch.zeros(18, **f64)]).contiguous()
-                        n = np.where(done, 0, n)
-                        offh = np.zeros(B + 1, dtype=np.int64)
-                        offh[1:] = np.cumsum(n)
-                        off = torch.as_tensor(offh.astype(np.int32), device=dev)
-                ev["advance"][1].record(s)
+                    with _timed(ev["brake"], s):
+                        fall_back(need, new, cand, pl, ver, fhit)
+                with _timed(ev["fly"], s):
+                    fly = np.array([b for b in act if fleet.n[b] > 0], dtype=np.int64)
+                    last = None
+                    if fly.size:
+                        fi = torch.as_tensor(fly, device=dev)
+                        sim = self.simulate_device(fleet.piece_off, fleet.T, fleet.coeffs, fi.to(torch.int32), init[fi].contiguous(), params=sp,
+                                                   stream=s)
+                        last = (fly, sim["log"])
+                with _timed(ev["advance"], s):
+                    if fly.size:
+                        advance(fly, fi, sim)
             s.synchronize()
             times.append({k: a.elapsed_time(e) for k, (a, e) in ev.items()})
-            actions.append(action)
-            verdicts.append(verdict)
-            replan_stages.append(rstage)
-            replan_verdicts.append(rverdict)
-            subgoal_kinds.append(skind)
             if last is not None:
                 logs.append(last)
         status[status == NAV_ACTIVE] = NAV_TIMEOUT
+        ran = len(times)
         out = dict(status=status, rounds_flown=flown_rounds, replans=replans, failed_replans=failed, uncertified_rounds=uncert,
-                   actions=np.array(actions).reshape(-1, B), verdicts=np.array(verdicts).reshape(-1, B),
-                   replan_stages=np.array(replan_stages).reshape(-1, B), replan_verdicts=np.array(replan_verdicts).reshape(-1, B), logs=logs,
+                   actions=actions[:ran], verdicts=verdicts[:ran], replan_stages=replan_stages[:ran], replan_verdicts=replan_verdicts[:ran], logs=logs,
                    times=times)
         if brake:
             out.update(brakes=brakes, held_rounds=held_rounds)
         if occupied:
             out.update(commits=commits)
-        if explore is not None:
-            out.update(subgoal_kinds=np.array(subgoal_kinds).reshape(-1, B), frontier_plans=frontier_plans)
+        if fpar is not None:
+            out.update(subgoal_kinds=subgoal_kinds[:ran], frontier_plans=frontier_plans)
         return out
 
     def plan_info(self):
