@@ -3,7 +3,7 @@
 (Evaluator.navigate: sense -> fuse -> check -> replan -> fly -> advance, every stage batched over vehicles); prints one JSON line.
 
   python bench_navigate.py [--vehicles 1,16,64] [--rounds R] [--horizon H] [--sense-every S] [--seed N] [--fallback keep|brake]
-                           [--unknown free|occupied] [--cameras 1|4] [--prefer-known W] [--explore]
+                           [--unknown free|occupied] [--cameras 1|4] [--prefer-known W] [--explore] [--min-gain G]
 
 World: mockamap's box world (isdf_world_cloud_device, ISDF_WORLD_BOXES) with seed 511, 40 x 40 x 10 m at 0.5 m (size 80 x 80 x 20,
 scale 2), 20 boxes 1.5 to 3 m wide: x and y in [-20, 20] m, z in [0, 10] m. The vehicles' map starts as an empty 1 m frame over that box
@@ -21,7 +21,9 @@ flies a rig of four cameras, cam_to_body = Rz(k 90 deg) cam02body. --prefer-know
 the front end's surcharge unknown_weight = W on unknown voxels and ISDF_PLAN_KNOWN_PREFIX, so that the back end treats unseen space as
 an obstacle along each plan's known prefix. --explore (needs --unknown occupied) flies navigate(explore=True) (DESIGN §3.24): a vehicle
 whose goal cannot be reached through seen space plans to the best frontier of what has been seen; it adds the frontier plans taken, and the
-frontier-goal call is timed inside the replan stage. Either option (also --unknown free) also reports the pose of the minimum true clearance: its
+frontier-goal call is timed inside the replan stage. --min-gain G (needs --explore) makes that call the view form (DESIGN §3.25): a frontier
+is a candidate only when navigate's rig, level at its cube centre, would see at least G unknown voxels; it adds the gains of the frontiers
+chosen (a histogram) and, for the vehicles that end held, the gain of the last frontier each was sent to. Either option (also --unknown free) also reports the pose of the minimum true clearance: its
 vehicle, round and witness voxel, and whether that voxel is occupied in the vehicles' fused map at the end of the run. Writes nothing to the
 tree.
 """
@@ -106,11 +108,14 @@ def main():
     ap.add_argument("--cameras", type=int, choices=(1, 4), default=1)
     ap.add_argument("--prefer-known", type=float, default=None, metavar="W")
     ap.add_argument("--explore", action="store_true")
+    ap.add_argument("--min-gain", type=int, default=None, metavar="G")
     args = ap.parse_args()
     if args.unknown == "occupied" and args.fallback != "brake":
         raise SystemExit("--unknown occupied needs --fallback brake")
     if args.explore and args.unknown != "occupied":
         raise SystemExit("--explore needs --unknown occupied")
+    if args.min_gain is not None and not args.explore:
+        raise SystemExit("--min-gain needs --explore")
     import torch
     import isdf_b200 as I
     if not torch.cuda.is_available():
@@ -139,6 +144,8 @@ def main():
         out["prefer_known"] = args.prefer_known
     if args.explore:
         out["explore"] = True
+    if args.min_gain is not None:
+        out["min_gain"] = args.min_gain
     for B in [int(v) for v in args.vehicles.split(",")]:
         starts, goals = pairs(occ, B, args.seed + B)
         ev = I.Evaluator(cfg)
@@ -149,6 +156,8 @@ def main():
         kw = dict(unknown="occupied", known_boxes=np.concatenate([starts - 2.5, starts + 2.5], 1)) if args.unknown == "occupied" else {}
         if args.explore:
             kw["explore"] = True
+        if args.min_gain is not None:
+            kw["min_gain"] = args.min_gain
         r = ev.navigate(starts, goals, rounds=args.rounds, horizon=args.horizon, sense_every=args.sense_every, tol=1.0,
                         plan_params=ev.plan_params(**pkw),
                         sense_params=rig(args.cameras), fallback=args.fallback, **kw)
@@ -170,6 +179,18 @@ def main():
             out["runs"][-1].update(commits=int(r["commits"].sum()))
         if "frontier_plans" in r:
             out["runs"][-1].update(frontier_plans=int(r["frontier_plans"].sum()))
+        if "frontier_gains" in r:
+            fg = r["frontier_gains"]
+            chosen = fg[fg >= 0]
+            edges = [0, 1, 10, 100, 1000, 10000, 1 << 62]
+            hist = np.histogram(chosen, bins=edges)[0] if chosen.size else np.zeros(len(edges) - 1, dtype=int)
+            last = {}   # a vehicle that ends held (TIMEOUT): the gain of the last frontier it was sent to
+            for b in np.nonzero(r["status"] == I.NAV_TIMEOUT)[0]:
+                g = fg[:, b][fg[:, b] >= 0]
+                if g.size:
+                    last[int(b)] = int(g[-1])
+            out["runs"][-1].update(frontier_gain_hist={f"[{a},{b})": int(n) for a, b, n in zip(edges[:-1], edges[1:], hist)},
+                                   timeout_last_frontier_gain=last)
         if trace and where:
             flown = [k for k in range(len(r["times"])) if (r["verdicts"][k] != I.NAV_NO_TRAJECTORY).any()]
             v = where["voxel"]

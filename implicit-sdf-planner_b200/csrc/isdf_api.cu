@@ -255,6 +255,7 @@ struct isdf_ctx {
     struct {   // frontiers (isdf_frontier.cuh): T_o, F, the list, union-find and cluster table of the last frontier call
         DevBuf<uint32_t> d_to, d_f; DevBuf<int> d_cnt, d_woff, d_parent, d_root, d_slot, d_size, d_box, d_croot; DevBuf<long long> d_vox, d_cid;
         DevBuf<unsigned long long> d_ntb, d_sum, d_best; DevBuf<unsigned> d_pick; DevBuf<char> d_tmp; DevBuf<uint8_t> d_cand;
+        DevBuf<double> d_vpose; DevBuf<long long> d_gain;   // frontier goals with a view rig: the poses at the frontier voxels, their gains
         DevBuf<isdf_frontier_cluster> d_table; DevBuf<int> d_pair, d_slice, d_tgt; DevBuf<double> d_goals; DevBuf<isdf_frontier_goal> d_out;
         cudaEvent_t ev[6] = {};
     } fr;
@@ -1648,12 +1649,21 @@ extern "C" int isdf_get_sense_info(isdf_ctx *c, isdf_sense_info *out) {
     return 0;
 }
 
+static int sense_cam_check(const isdf_sense_params *p);
 // the checks every sensing call shares; the context (and its scene) last
 static int sense_args_check(isdf_ctx *c, int64_t Q, const void *pos, const void *quat, int64_t stride, const isdf_sense_params *p,
                             const void *out) {
     if (!pos || !quat || !p || !out) return fail(ISDF_ERR_INVALID, "NULL argument");
     if (Q < 1 || Q >= (1ll << 31)) return fail(ISDF_ERR_INVALID, "Q must be in [1, 2^31)");
     if (stride < 1) return fail(ISDF_ERR_INVALID, "stride_doubles < 1");
+    if (int rc = sense_cam_check(p)) return rc;
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (!c->sense.have) return fail(ISDF_ERR_STATE, "no scene cloud: set one with isdf_set_sense_cloud");
+    return 0;
+}
+
+// the checks of one camera
+static int sense_cam_check(const isdf_sense_params *p) {
     if (p->width < 1 || p->height < 1 || (long long)p->width * p->height > (1ll << 26))
         return fail(ISDF_ERR_INVALID, "width and height must be >= 1 with width x height <= 2^26");
     if (!std::isfinite(p->fx) || !std::isfinite(p->fy) || !std::isfinite(p->cx) || !std::isfinite(p->cy))
@@ -1663,8 +1673,6 @@ static int sense_args_check(isdf_ctx *c, int64_t Q, const void *pos, const void 
     if (p->cam_to_body[12] != 0 || p->cam_to_body[13] != 0 || p->cam_to_body[14] != 0 || p->cam_to_body[15] != 1)
         return fail(ISDF_ERR_INVALID, "cam_to_body's last row must be (0, 0, 0, 1)");
     if (!(p->sensing_horizon > 0)) return fail(ISDF_ERR_INVALID, "sensing_horizon must be positive (+Inf keeps every point)");
-    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
-    if (!c->sense.have) return fail(ISDF_ERR_STATE, "no scene cloud: set one with isdf_set_sense_cloud");
     return 0;
 }
 
@@ -1785,6 +1793,60 @@ extern "C" int isdf_map_observe(isdf_ctx *c, int64_t Q, const double *pos, const
 extern "C" int isdf_map_observe_device(isdf_ctx *c, int64_t Q, const double *d_pos, const double *d_quat, int64_t stride_doubles,
                                        const isdf_sense_params *p, isdf_observe_info *info, void *cuda_stream) {
     return observe_impl(c, Q, d_pos, d_quat, stride_doubles, p, info, true, (cudaStream_t)cuda_stream);
+}
+
+// ---- view gain (isdf_view.cuh) ----
+// the checks of a view-gain rig, and the map it needs: every camera as the sensing calls check one, a finite horizon, and a horizon box of
+// at most 2^40 voxels
+static int view_rig_check(isdf_ctx *c, int n_cams, const isdf_sense_params *cams) {
+    if (n_cams < 1 || !cams) return fail(ISDF_ERR_INVALID, "a view gain needs n_cams >= 1 cameras");
+    double hmax = 0.0;
+    for (int k = 0; k < n_cams; k++) {
+        if (int rc = sense_cam_check(cams + k)) return rc;
+        if (!std::isfinite(cams[k].sensing_horizon)) return fail(ISDF_ERR_INVALID, "a view gain needs a finite sensing_horizon on every camera");
+        hmax = std::max(hmax, cams[k].sensing_horizon);
+    }
+    if (!c) return fail(ISDF_ERR_INVALID, "ctx is NULL");
+    if (c->world > 1) return fail(ISDF_ERR_UNSUPPORTED, "the view gain is not sharded: call it on a context with isdf_set_shard(ctx, 0, 1)");
+    if (!c->map.have_map) return fail(ISDF_ERR_STATE, "map not set");
+    const double D = std::ceil(2.0 * hmax / c->map.grid.res) + 3.0;
+    if (!(D * D * D <= (double)(1ll << 40))) return fail(ISDF_ERR_INVALID, "sensing_horizon / res too large: a pose's horizon box exceeds 2^40 voxels");
+    return 0;
+}
+
+static int view_gain_impl(isdf_ctx *c, int64_t Q, const double *pos, const double *quat, int64_t stride, int n_cams, const isdf_sense_params *cams,
+                          int64_t *gain, bool device, cudaStream_t st) {
+    if (!pos || !quat || !gain) return fail(ISDF_ERR_INVALID, "NULL argument");
+    if (Q < 1 || Q >= (1ll << 31)) return fail(ISDF_ERR_INVALID, "Q must be in [1, 2^31)");
+    if (stride < 1) return fail(ISDF_ERR_INVALID, "stride_doubles < 1");
+    if (int rc = view_rig_check(c, n_cams, cams)) return rc;
+    if (set_device(c)) return ISDF_ERR_CUDA;
+    int64_t *d_gain = gain;
+    Staging S(c);
+    if (!device) {
+        const double *d_pose;
+        stage_poses(S, Q, pos, quat, stride, &d_pose);
+        S.out(&d_gain, gain, (size_t)Q);
+        if (int rc = S.upload()) return rc;
+        pos = d_pose; quat = d_pose + 3; stride = 7;
+        st = c->stream;
+    }
+    int launches = 0;
+    const cudaError_t e = view_gain_run(c->sense, Q, pos, quat, stride, n_cams, cams, c->map.grid, c->known.have ? c->known.d_known.p : nullptr,
+                                        nullptr, d_gain, st, &launches);
+    c->stats.kernel_launches += launches;
+    if (e != cudaSuccess) return fail(ISDF_ERR_CUDA, std::string("isdf_view_gain: ") + cudaGetErrorString(e));
+    if (!device) return S.download();
+    CU_TRY(cudaStreamSynchronize(st));
+    return 0;
+}
+extern "C" int isdf_view_gain(isdf_ctx *c, int64_t Q, const double *pos, const double *quat, int64_t stride_doubles, int n_cams,
+                              const isdf_sense_params *cams, int64_t *gain) {
+    return view_gain_impl(c, Q, pos, quat, stride_doubles, n_cams, cams, gain, false, nullptr);
+}
+extern "C" int isdf_view_gain_device(isdf_ctx *c, int64_t Q, const double *d_pos, const double *d_quat, int64_t stride_doubles, int n_cams,
+                                     const isdf_sense_params *cams, int64_t *d_gain, void *cuda_stream) {
+    return view_gain_impl(c, Q, d_pos, d_quat, stride_doubles, n_cams, cams, d_gain, true, (cudaStream_t)cuda_stream);
 }
 
 // the blocked grid occ | ~known, rebuilt on st (and waited for, so that a later call on another stream reads it whole) when stale
@@ -4693,8 +4755,10 @@ extern "C" int isdf_frontier_default_params(isdf_frontier_params *p) {
 }
 
 // the frontier goals of B pairs (starts and goals on the host, B x 3) into out (B records, device) on st
-static int frontier_goals_run(isdf_ctx *c, int B, const double *starts, const double *goals, const isdf_frontier_params *p, int max_fields,
-                              isdf_frontier_goal *out, isdf_frontier_info *I, cudaStream_t st) {
+// ncam cameras at cams (host; 0: no rig, every gain 0): a candidate also needs a view gain of at least min_gain
+static int frontier_goals_run(isdf_ctx *c, int B, const double *starts, const double *goals, const isdf_frontier_params *p, int ncam,
+                              const isdf_sense_params *cams, long long min_gain, int max_fields, isdf_frontier_goal *out, isdf_frontier_info *I,
+                              cudaStream_t st) {
     const DevGrid &G = c->map.grid;
     const size_t nvox = (size_t)G.X * G.Y * G.Z;
     auto &z = c->fr;
@@ -4730,10 +4794,22 @@ static int frontier_goals_run(isdf_ctx *c, int B, const double *starts, const do
         c->stats.kernel_launches++;
         CU_TRY(cudaGetLastError());
     }
+    if (n && ncam) {   // the gains of the voxels the size rule kept (the others count 0 and stay out)
+        CU_TRY(z.d_vpose.ensure(7 * (size_t)n)); CU_TRY(z.d_gain.ensure(n));
+        k_fg_view_poses<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(G, n, z.d_vox.p, z.d_vpose.p);
+        int launches = 1;
+        const cudaError_t e = view_gain_run(c->sense, n, z.d_vpose.p, z.d_vpose.p + 3, 7, ncam, cams, G, c->known.have ? c->known.d_known.p : nullptr,
+                                            z.d_cand.p, reinterpret_cast<int64_t *>(z.d_gain.p), st, &launches);
+        k_fg_gain_cand<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, z.d_gain.p, min_gain, z.d_cand.p);
+        c->stats.kernel_launches += launches + 1;
+        CU_TRY(e);
+        CU_TRY(cudaGetLastError());
+    }
     CU_TRY(c->fp.d_g.ensure((size_t)F * nvox));
     FgArgs A = {};
     A.grid = G; A.g = c->fp.d_g.p; A.vox = z.d_vox.p; A.cand = z.d_cand.p; A.n = n; A.goal_weight = p->goal_weight;
     A.goals = z.d_goals.p; A.tgt = z.d_tgt.p; A.best = z.d_best.p; A.pick = z.d_pick.p; A.table = z.d_table.p; A.cid = z.d_cid.p; A.out = out;
+    A.gain = ncam ? z.d_gain.p : nullptr;
     const long long sms = c->sm_count;
     for (int s0 = 0; s0 < S; s0 += F) {
         const int m = std::min(F, S - s0), w0 = wstart[s0], w1 = wstart[s0 + m];
@@ -4760,11 +4836,17 @@ static int frontier_goals_run(isdf_ctx *c, int B, const double *starts, const do
     return 0;
 }
 
+// ncam < 0: isdf_frontier_goals (no rig, min_gain 0); else the view form's rig
 static int frontier_goals_entry(isdf_ctx *c, bool dev, int B, const double *starts, const double *goals, const isdf_frontier_params *prm,
-                                int max_fields, isdf_frontier_goal *out, isdf_frontier_info *info, cudaStream_t st) {
+                                int ncam, const isdf_sense_params *cams, long long min_gain, int max_fields, isdf_frontier_goal *out,
+                                isdf_frontier_info *info, cudaStream_t st) {
     if (int r = frontier_state(c)) return r;
     if (!starts || !goals || !out || B < 1) return fail(ISDF_ERR_INVALID, "NULL argument or B < 1");
     if (max_fields < 0) return fail(ISDF_ERR_INVALID, "max_fields < 0");
+    if (ncam >= 0) {
+        if (int r = view_rig_check(c, ncam, cams)) return r;
+        if (min_gain < 0) return fail(ISDF_ERR_INVALID, "min_gain < 0");
+    }
     isdf_frontier_params p;
     isdf_frontier_default_params(&p);
     if (prm) p = *prm;
@@ -4780,7 +4862,7 @@ static int frontier_goals_entry(isdf_ctx *c, bool dev, int B, const double *star
     }
     CU_TRY(c->fr.d_out.ensure(B));
     isdf_frontier_info I = {};
-    const int r = frontier_goals_run(c, B, starts, goals, &p, max_fields, dev ? out : c->fr.d_out.p, &I, st);
+    const int r = frontier_goals_run(c, B, starts, goals, &p, std::max(ncam, 0), cams, min_gain, max_fields, dev ? out : c->fr.d_out.p, &I, st);
     if (info) *info = I;
     if (r) return r;
     if (!dev) CU_TRY(cudaMemcpyAsync(out, c->fr.d_out.p, sizeof(isdf_frontier_goal) * B, cudaMemcpyDeviceToHost, st));
@@ -4790,12 +4872,24 @@ static int frontier_goals_entry(isdf_ctx *c, bool dev, int B, const double *star
 
 extern "C" int isdf_frontier_goals(isdf_ctx *c, int B, const double *starts, const double *goals, const isdf_frontier_params *p, int max_fields,
                                    isdf_frontier_goal *out, isdf_frontier_info *info) {
-    return frontier_goals_entry(c, false, B, starts, goals, p, max_fields, out, info, nullptr);
+    return frontier_goals_entry(c, false, B, starts, goals, p, -1, nullptr, 0, max_fields, out, info, nullptr);
 }
 
 extern "C" int isdf_frontier_goals_device(isdf_ctx *c, int B, const double *d_starts, const double *d_goals, const isdf_frontier_params *p,
                                           int max_fields, isdf_frontier_goal *d_out, isdf_frontier_info *info, void *cuda_stream) {
-    return frontier_goals_entry(c, true, B, d_starts, d_goals, p, max_fields, d_out, info, (cudaStream_t)cuda_stream);
+    return frontier_goals_entry(c, true, B, d_starts, d_goals, p, -1, nullptr, 0, max_fields, d_out, info, (cudaStream_t)cuda_stream);
+}
+
+extern "C" int isdf_frontier_goals_view(isdf_ctx *c, int B, const double *starts, const double *goals, const isdf_frontier_params *p, int n_cams,
+                                        const isdf_sense_params *cams, int64_t min_gain, int max_fields, isdf_frontier_goal *out,
+                                        isdf_frontier_info *info) {
+    return frontier_goals_entry(c, false, B, starts, goals, p, n_cams, cams, min_gain, max_fields, out, info, nullptr);
+}
+
+extern "C" int isdf_frontier_goals_view_device(isdf_ctx *c, int B, const double *d_starts, const double *d_goals, const isdf_frontier_params *p,
+                                               int n_cams, const isdf_sense_params *cams, int64_t min_gain, int max_fields,
+                                               isdf_frontier_goal *d_out, isdf_frontier_info *info, void *cuda_stream) {
+    return frontier_goals_entry(c, true, B, d_starts, d_goals, p, n_cams, cams, min_gain, max_fields, d_out, info, (cudaStream_t)cuda_stream);
 }
 
 // ---- planning step: PlannerManager::generateTraj for B (start, goal) pairs (include/isdf.h) --------------------------------------------

@@ -18,6 +18,9 @@
 //   k_fg_score      atomicMin of the best score's bit pattern (a non-negative double) over the candidate list
 //   k_fg_pick       atomicMin of the list position among the voxels with that score (the smallest voxel index)
 //   k_fg_record     GOAL / FRONTIER / NONE and the record
+// With a view rig (isdf_frontier_goals_view), between the size rule (k_fg_cand) and the selection: k_fg_view_poses puts a pose at every
+// frontier voxel's cube centre, view_gain_run (isdf_view.cuh) counts the gains of the voxels the size rule kept, and k_fg_gain_cand clears
+// the candidates whose gain is below min_gain.
 #pragma once
 #include "isdf_frontpath.cuh"
 
@@ -198,8 +201,15 @@ struct FgArgs {
     unsigned *pick;                // B: the list position picked among the best (0xffffffff: none)
     const isdf_frontier_cluster *table;
     const long long *cid;          // n: cluster ids
+    const long long *gain;         // n: view gains (NULL without a rig: every record's gain 0)
     isdf_frontier_goal *out;       // B records
 };
+
+// the cube centre of voxel v on axis a: bmin + (i + 0.5) res, a FRONTIER record's point
+__device__ __forceinline__ double fg_centre(const DevGrid &G, long long v, int a) {
+    const int i = a == 0 ? (int)(v / ((long long)G.Z * G.Y)) : a == 1 ? (int)((v / G.Z) % G.Y) : (int)(v % G.Z);
+    return (i + 0.5) * G.res + G.bmin[a];
+}
 
 // score(f) = g_b(f) + goal_weight * sqrt((dx*dx + dy*dy) + dz*dz), d = cube centre of f - goal; the bits of +inf when f is not a
 // candidate or not reached
@@ -256,7 +266,7 @@ __global__ void k_fg_record(const __grid_constant__ FgArgs A) {
     const int *tv = A.tgt + 3 * (size_t)b;
     const long long vt = ((long long)tv[0] * G.Y + tv[1]) * G.Z + tv[2];
     isdf_frontier_goal r;
-    r.reserved_ = 0;
+    r.gain = 0;
     const double inf = __longlong_as_double((long long)FP_INF);
     if (g[vt] != FP_INF) {
         r.kind = ISDF_FRONTIER_GOAL; r.voxel = vt; r.cluster = -1;
@@ -265,11 +275,11 @@ __global__ void k_fg_record(const __grid_constant__ FgArgs A) {
     } else if (A.pick[b] != 0xffffffffu) {
         const int i = (int)A.pick[b];
         const long long v = A.vox[i];
-        const int id[3] = {(int)(v / ((long long)G.Z * G.Y)), (int)((v / G.Z) % G.Y), (int)(v % G.Z)};
         r.kind = ISDF_FRONTIER_FRONTIER; r.voxel = v; r.cluster = A.cid[i];
         r.g = __longlong_as_double((long long)g[v]);
         r.score = __longlong_as_double((long long)A.best[b]);
-        for (int a = 0; a < 3; a++) r.point[a] = (id[a] + 0.5) * G.res + G.bmin[a];
+        for (int a = 0; a < 3; a++) r.point[a] = fg_centre(G, v, a);
+        if (A.gain) r.gain = (int32_t)min(A.gain[i], 2147483647ll);
     } else {
         r.kind = ISDF_FRONTIER_NONE; r.voxel = -1; r.cluster = -1;
         r.g = r.score = inf;
@@ -282,6 +292,21 @@ __global__ void k_fg_record(const __grid_constant__ FgArgs A) {
 __global__ void k_fg_cand(int n, const int *parent, const int *slot, const int *size, int min_voxels, uint8_t *cand) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) cand[i] = size[slot[parent[i]]] >= min_voxels;
+}
+
+// the view-gain poses of the frontier list: position i at f's cube centre, quaternion (1, 0, 0, 0), 7 doubles per pose
+__global__ void k_fg_view_poses(const DevGrid G, int n, const long long *vox, double *pose) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    double *o = pose + 7 * (size_t)i;
+    for (int a = 0; a < 3; a++) o[a] = fg_centre(G, vox[i], a);
+    o[3] = 1.0; o[4] = o[5] = o[6] = 0.0;
+}
+
+// the gain rule folded into the candidates: cand[i] = cand[i] and gain[i] >= min_gain
+__global__ void k_fg_gain_cand(int n, const long long *gain, long long min_gain, uint8_t *cand) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) cand[i] = cand[i] && gain[i] >= min_gain;
 }
 
 }  // namespace isdf

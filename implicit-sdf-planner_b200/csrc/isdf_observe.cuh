@@ -47,16 +47,20 @@ struct ObsArgs {
     unsigned long long *cnt;               // {voxels tested, voxels added}
 };
 
-// the four-part rule for voxel (ix, iy, iz) and pose P (include/isdf.h); operation order as written there
-__device__ bool obs_voxel(const ObsArgs &A, const SensePose &P, int p, int ix, int iy, int iz) {
+// rules 2, 1 and 3 for voxel (ix, iy, iz) seen from pose P (include/isdf.h), operation order as written there; shared by isdf_map_observe
+// and isdf_view_gain. fx .. cy: the render's FP32 parameters. On success the pixel rectangle x0 .. x1, y0 .. y1, the corners' largest camera
+// depth zmax and the depth margin e2 (E_2) that rule 4 needs.
+struct ObsView { int x0, x1, y0, y1; double zmax, e2; };
+__device__ __forceinline__ bool obs_in_view(const double bmin[3], double res, double horizon, double fx, double fy, double cx, double cy, int W,
+                                            int H, const SensePose &P, int ix, int iy, int iz, ObsView &o) {
     double lo[3], hi[3];
-    voxel_span(A.bmin[0], A.res, ix, lo[0], hi[0]);
-    voxel_span(A.bmin[1], A.res, iy, lo[1], hi[1]);
-    voxel_span(A.bmin[2], A.res, iz, lo[2], hi[2]);
+    voxel_span(bmin[0], res, ix, lo[0], hi[0]);
+    voxel_span(bmin[1], res, iy, lo[1], hi[1]);
+    voxel_span(bmin[2], res, iz, lo[2], hi[2]);
     // 2. every corner within the horizon of the body position
     for (int k = 0; k < 8; k++) {
         const double d0 = ((k & 1) ? hi[0] : lo[0]) - P.body[0], d1 = ((k & 2) ? hi[1] : lo[1]) - P.body[1], d2 = ((k & 4) ? hi[2] : lo[2]) - P.body[2];
-        if (!(sqrt((d0 * d0 + d1 * d1) + d2 * d2) <= A.horizon)) return false;
+        if (!(sqrt((d0 * d0 + d1 * d1) + d2 * d2) <= horizon)) return false;
     }
     double M = 0.0;
     for (int a = 0; a < 3; a++) M = fmax(M, fmax(fabs(lo[a]), fabs(hi[a])));
@@ -80,27 +84,36 @@ __device__ bool obs_voxel(const ObsArgs &A, const SensePose &P, int p, int ix, i
     if (!(zmin > E[2])) return false;
     for (int k = 0; k < 8; k++) {
         const double qx = cx8[k] / cz[k], qy = cy8[k] / cz[k];
-        const double u = qx * A.fx + A.cx, v = qy * A.fy + A.cy;
+        const double u = qx * fx + cx, v = qy * fy + cy;
         umin = fmin(umin, u); umax = fmax(umax, u); vmin = fmin(vmin, v); vmax = fmax(vmax, v);
         a = fmax(a, fabs(qx)); b = fmax(b, fabs(qy));
     }
     // 3. the pixel rectangle, widened by the projection's rounding, inside the image
     const double zl = zmin - E[2];
     const double dqx = (E[0] + a * E[2]) / zl, dqy = (E[1] + b * E[2]) / zl;
-    const double eu = (A.fx * dqx + 1.2e-7 * ((a + dqx) * A.fx + fabs(A.cx))) + 1e-9 * (1.0 + (a * A.fx + fabs(A.cx)));
-    const double ev = (A.fy * dqy + 1.2e-7 * ((b + dqy) * A.fy + fabs(A.cy))) + 1e-9 * (1.0 + (b * A.fy + fabs(A.cy)));
+    const double eu = (fx * dqx + 1.2e-7 * ((a + dqx) * fx + fabs(cx))) + 1e-9 * (1.0 + (a * fx + fabs(cx)));
+    const double ev = (fy * dqy + 1.2e-7 * ((b + dqy) * fy + fabs(cy))) + 1e-9 * (1.0 + (b * fy + fabs(cy)));
     const double fx0 = floor((umin - eu) + 0.5), fx1 = floor((umax + eu) + 0.5);
     const double fy0 = floor((vmin - ev) + 0.5), fy1 = floor((vmax + ev) + 0.5);
-    if (!(fx0 >= 0.0 && fx1 <= (double)(A.w[0] - 1) && fy0 >= 0.0 && fy1 <= (double)(A.h[0] - 1))) return false;
-    const int x0 = (int)fx0, x1 = (int)fx1, y0 = (int)fy0, y1 = (int)fy1;
+    if (!(fx0 >= 0.0 && fx1 <= (double)(W - 1) && fy0 >= 0.0 && fy1 <= (double)(H - 1))) return false;
+    o.x0 = (int)fx0; o.x1 = (int)fx1; o.y0 = (int)fy0; o.y1 = (int)fy1;
+    o.zmax = zmax; o.e2 = E[2];
+    return true;
+}
+
+// the four-part rule for voxel (ix, iy, iz) and pose P (include/isdf.h): rules 2, 1, 3, then 4 on the image's min-mip
+__device__ bool obs_voxel(const ObsArgs &A, const SensePose &P, int p, int ix, int iy, int iz) {
+    ObsView o;
+    if (!obs_in_view(A.bmin, A.res, A.horizon, A.fx, A.fy, A.cx, A.cy, A.w[0], A.h[0], P, ix, iy, iz, o)) return false;
+    const int x0 = o.x0, x1 = o.x1, y0 = o.y0, y1 = o.y1;
     // 4. the rectangle's minimum depth (from the mip) beyond the corners' depth plus dist_mm's rounding and the transform's error
     int l = 0;
     while ((x1 >> l) - (x0 >> l) > 1 || (y1 >> l) - (y0 >> l) > 1) l++;
     const int i0 = x0 >> l, i1 = x1 >> l, j0 = y0 >> l, j1 = y1 >> l, w = A.w[l];
     const int32_t *m = l == 0 ? A.img + (long long)p * w * A.h[0] : A.mip + A.off[l] + (long long)p * w * A.h[l];
     const int dmin = min(min(m[(long long)j0 * w + i0], m[(long long)j0 * w + i1]), min(m[(long long)j1 * w + i0], m[(long long)j1 * w + i1]));
-    const double d = (1000.0 * E[2] + 0.5) + 1.2e-7 * (1000.0 * (zmax + E[2]) + 1.0);
-    return (double)dmin > 1000.0 * zmax + d;
+    const double d = (1000.0 * o.e2 + 0.5) + 1.2e-7 * (1000.0 * (o.zmax + o.e2) + 1.0);
+    return (double)dmin > 1000.0 * o.zmax + d;
 }
 
 __device__ __forceinline__ void warp_add(unsigned long long *cnt, unsigned long long v) {

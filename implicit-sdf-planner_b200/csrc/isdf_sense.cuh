@@ -29,6 +29,9 @@ struct SensePose {
     double cull_off;   // |camera position - body position|: the horizon cull's offset
 };
 
+// one camera of a view-gain rig (isdf_view.cuh): its horizon, the render's FP32 intrinsics (as doubles) and its image size
+struct ViewCam { double horizon, fx, fy, cx, cy; int w, h; };
+
 // the scene cloud of a context: sorted finite points, brick boxes; set once by sense_set_cloud
 struct SenseScene {
     bool have = false;
@@ -39,6 +42,7 @@ struct SenseScene {
     DevBuf<SensePose> d_pose; DevBuf<uint2> d_work; DevBuf<unsigned long long> d_nwork; DevBuf<int32_t> d_img, d_flag;
     DevBuf<long long> d_base; DevBuf<char> d_tmp;
     DevBuf<int32_t> d_mip; DevBuf<unsigned long long> d_obs_cnt;   // isdf_map_observe: the chunk's min-mips, its counts
+    DevBuf<SensePose> d_view_pose; DevBuf<ViewCam> d_view_cam;     // isdf_view_gain: the chunk's (camera, pose) transforms, the rig
     int chunk_override = 0;   // poses per chunk (isdf_dbg_sense_chunk; 0: automatic)
     // give up the cloud and the scratch sized for it
     void release() {
@@ -71,6 +75,11 @@ cudaError_t sense_observe_run(SenseScene &S, const SenseCall &C, const DevGrid &
                               int *launches);
 // marks known the voxels whose padded cube lies inside the closed box lo, hi (host), on st
 cudaError_t known_mark_box(const DevGrid &G, uint32_t *known, const double lo[3], const double hi[3], cudaStream_t st, int *launches);
+// view gain: d_gain[q] (device, Q) = the unknown voxels of G (known NULL: nothing known) the ncam cameras would see from pose q of the records
+// at pos / quat (device, stride doubles apart), on st; poses with d_want[q] == 0 (d_want may be NULL: every pose wanted) are skipped and count 0
+cudaError_t view_gain_run(SenseScene &S, long long Q, const double *pos, const double *quat, long long stride, int ncam,
+                          const isdf_sense_params *cams, const DevGrid &G, const uint32_t *known, const uint8_t *d_want, int64_t *d_gain,
+                          cudaStream_t st, int *launches);
 // out = G.bits | (~known & valid bits), known NULL meaning nothing known, on st
 cudaError_t blocked_build(const DevGrid &G, const uint32_t *known, uint32_t *out, cudaStream_t st, int *launches);
 

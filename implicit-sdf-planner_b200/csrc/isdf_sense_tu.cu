@@ -3,10 +3,12 @@
 // the render's FP32 arithmetic is spelled with intrinsics, so its contraction is the reference CUDA build's whatever the unit's setting.
 #include "isdf_sense.cuh"
 #include "isdf_observe.cuh"
+#include "isdf_view.cuh"
 #include "isdf_math.cuh"
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 #include <algorithm>
+#include <vector>
 #include <cmath>
 
 namespace isdf {
@@ -441,6 +443,44 @@ cudaError_t sense_observe_run(SenseScene &S, const SenseCall &C, const DevGrid &
     }
     if ((e = cudaMemcpyAsync(cnt, S.d_obs_cnt.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st)) != cudaSuccess) return e;
     return cudaStreamSynchronize(st);
+}
+
+cudaError_t view_gain_run(SenseScene &S, long long Q, const double *pos, const double *quat, long long stride, int ncam,
+                          const isdf_sense_params *cams, const DevGrid &G, const uint32_t *known, const uint8_t *d_want, int64_t *d_gain,
+                          cudaStream_t st, int *launches) {
+    // poses per chunk: one grid row each (gridDim.y <= 65535), and at most 2^18 (camera, pose) transforms
+    const int P = (int)std::min<long long>({Q, 65535ll, std::max(1ll, (1ll << 18) / ncam)});
+    cudaError_t e;
+    if ((e = S.d_view_pose.ensure((size_t)P * ncam)) != cudaSuccess) return e;
+    std::vector<ViewCam> hc(ncam);
+    ViewArgs A = {};
+    A.hmax = 0.0;
+    for (int c = 0; c < ncam; c++) {
+        hc[c] = {cams[c].sensing_horizon, (double)(float)cams[c].fx, (double)(float)cams[c].fy, (double)(float)cams[c].cx,
+                 (double)(float)cams[c].cy, cams[c].width, cams[c].height};
+        A.hmax = std::max(A.hmax, cams[c].sensing_horizon);
+    }
+    if ((e = S.d_view_cam.upload(hc.data(), hc.size(), st)) != cudaSuccess) return e;
+    for (int a = 0; a < 3; a++) A.bmin[a] = G.bmin[a];
+    A.res = G.res; A.X = G.X; A.Y = G.Y; A.Z = G.Z; A.Zw = G.Zw;
+    A.D = (int)std::ceil(2.0 * A.hmax / G.res) + 3;
+    A.occ = G.bits; A.known = known; A.cams = S.d_view_cam.p; A.ncam = ncam; A.poses = S.d_view_pose.p;
+    if ((e = cudaMemsetAsync(d_gain, 0, sizeof(int64_t) * Q, st)) != cudaSuccess) return e;
+    const long long D3 = (long long)A.D * A.D * A.D;
+    for (long long q0 = 0; q0 < Q; q0 += P) {
+        const int np = (int)std::min<long long>(P, Q - q0);
+        for (int c = 0; c < ncam; c++) {
+            const SenseCall C{Q, pos, quat, stride, cams[c]};
+            k_sense_poses<<<(np + 127) / 128, 128, 0, st>>>(C, q0, np, S.d_view_pose.p + (size_t)c * np);
+        }
+        A.P = np; A.want = d_want ? d_want + q0 : nullptr; A.gain = reinterpret_cast<unsigned long long *>(d_gain + q0);
+        // CTAs per pose: enough to cover the box once, fewer when many poses already fill the device
+        const long long bx = std::max(1ll, std::min((D3 + 255) / 256, (132ll * 32 + np - 1) / np));
+        k_view_gain<<<dim3((unsigned)bx, (unsigned)np), 256, 0, st>>>(A);
+        *launches += ncam + 1;
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
 
 cudaError_t known_mark_box(const DevGrid &G, uint32_t *known, const double lo[3], const double hi[3], cudaStream_t st, int *launches) {

@@ -57,7 +57,8 @@ ABI_SYMBOLS = ["isdf_default_config", "isdf_create", "isdf_destroy", "isdf_last_
                "isdf_trajectory_brake_device", "isdf_map_observe", "isdf_map_observe_device", "isdf_map_mark_known",
                "isdf_get_map_known_u8", "isdf_set_unknown_policy", "isdf_get_unknown_policy", "isdf_gather_obstacle_points_batch_known",
                "isdf_map_frontiers", "isdf_map_frontiers_device", "isdf_frontier_default_params", "isdf_frontier_goals",
-               "isdf_frontier_goals_device"]
+               "isdf_frontier_goals_device", "isdf_view_gain", "isdf_view_gain_device", "isdf_frontier_goals_view",
+               "isdf_frontier_goals_view_device"]
 WORLD_KINDS = dict(globalmap=1, perlin=2, boxes=3)   # isdf_world_kind
 CERTIFIED, UNDECIDED, COLLIDING = 1, 0, -1   # isdf_certify_summary.verdict
 FEASIBLE, VIOLATING = 1, -1                  # isdf_dynamics_summary.verdict (0: UNDECIDED)
@@ -401,11 +402,11 @@ class FrontierParams(C.Structure):
 
 class FrontierGoal(C.Structure):
     """isdf_frontier_goal"""
-    _fields_ = [("kind", C.c_int32), ("reserved_", C.c_int32), ("voxel", C.c_int64), ("cluster", C.c_int64), ("g", C.c_double),
+    _fields_ = [("kind", C.c_int32), ("gain", C.c_int32), ("voxel", C.c_int64), ("cluster", C.c_int64), ("g", C.c_double),
                 ("score", C.c_double), ("point", C.c_double * 3)]
 
 
-FRONTIER_GOAL_DTYPE = np.dtype([("kind", "<i4"), ("reserved_", "<i4"), ("voxel", "<i8"), ("cluster", "<i8"), ("g", "<f8"), ("score", "<f8"),
+FRONTIER_GOAL_DTYPE = np.dtype([("kind", "<i4"), ("gain", "<i4"), ("voxel", "<i8"), ("cluster", "<i8"), ("g", "<f8"), ("score", "<f8"),
                                 ("point", "<f8", (3,))])
 FRONTIER_CLUSTER_DTYPE = np.dtype([("id", "<i8"), ("size", "<i8"), ("bmin", "<i4", (3,)), ("bmax", "<i4", (3,)), ("centroid", "<f8", (3,))])
 
@@ -643,6 +644,8 @@ def load_library(path=None):
     lib.isdf_frontier_default_params.argtypes = [frp]
     lib.isdf_frontier_goals.argtypes = [vp, C.c_int, dp, dp, frp, C.c_int, vp, fip]
     lib.isdf_frontier_goals_device.argtypes = [vp, C.c_int, vp, vp, frp, C.c_int, vp, fip, vp]
+    lib.isdf_frontier_goals_view.argtypes = [vp, C.c_int, dp, dp, frp, C.c_int, vp, C.c_int64, C.c_int, vp, fip]
+    lib.isdf_frontier_goals_view_device.argtypes = [vp, C.c_int, vp, vp, frp, C.c_int, vp, C.c_int64, C.c_int, vp, fip, vp]
     mpp = C.POINTER(MidendParams)
     lib.isdf_path_waypoints.argtypes = [C.c_int, ip, dp, C.c_double, C.c_double, C.c_int, dp, ip, ip]
     lib.isdf_midend_default_params.argtypes = [mpp]
@@ -686,6 +689,8 @@ def load_library(path=None):
     lib.isdf_sense_depth.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, vp]
     lib.isdf_map_observe.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, C.POINTER(ObserveInfo)]
     lib.isdf_map_observe_device.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, C.POINTER(ObserveInfo), vp]
+    lib.isdf_view_gain.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, C.c_int, vp, vp]
+    lib.isdf_view_gain_device.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, C.c_int, vp, vp, vp]
     lib.isdf_sense_depth_device.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, vp, vp]
     lib.isdf_sense_cloud.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, C.c_int64, vp, vp]
     lib.isdf_sense_cloud_device.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, sep, C.c_int64, vp, vp, vp]
@@ -888,6 +893,12 @@ def _timed(events, stream):
     events[0].record(stream)
     yield
     events[1].record(stream)
+
+
+def _rig(params):
+    """one sense_params or a list of them -> a ctypes array of SenseParams (the library refuses an empty one)"""
+    cams = list(params) if isinstance(params, (list, tuple)) else [params if params is not None else sense_params()]
+    return (SenseParams * len(cams))(*cams)
 
 
 def _dp(a):
@@ -1122,6 +1133,34 @@ class Evaluator:
         self._check(self.lib.isdf_map_observe_device(self.h, Q, C.c_void_p(base + 8 * pos_offset), C.c_void_p(base + 8 * quat_offset), stride,
                                                      C.byref(p), C.byref(info), C.c_void_p(s.cuda_stream)))
         return info.as_dict()
+
+    # ---- view gain (isdf_view_gain): the unknown voxels a rig of cameras would observe from a pose ----
+    def view_gain(self, records, pos_offset=0, quat_offset=3, params=None):
+        """the view gain of Q poses read in place from records (Q, stride) float64 (as sense_depth reads them) for the rig params (one
+        sense_params or a list of them, each with a finite sensing_horizon) -> (Q,) int64 numpy"""
+        cams = _rig(params)
+        r = _f64(records)
+        r = r.reshape(-1, r.shape[-1])
+        Q, stride = self._pose_records(r, pos_offset, quat_offset)
+        out = np.zeros(Q, dtype=np.int64)
+        base = r.ctypes.data
+        self._check(self.lib.isdf_view_gain(self.h, Q, C.c_void_p(base + 8 * pos_offset), C.c_void_p(base + 8 * quat_offset), stride, len(cams),
+                                            C.byref(cams), out.ctypes.data_as(C.c_void_p)))
+        return out
+
+    def view_gain_device(self, records, pos_offset=0, quat_offset=3, params=None, stream=None):
+        """view_gain on a float64 CUDA tensor (Q, stride), on torch's current stream (or stream) -> (Q,) int64 CUDA tensor"""
+        import torch
+        cams = _rig(params)
+        r = _cuda_records(records)
+        Q, stride = self._pose_records(r, pos_offset, quat_offset)
+        s = torch.cuda.current_stream(r.device) if stream is None else stream
+        with torch.cuda.stream(s):
+            out = torch.empty(Q, dtype=torch.int64, device=r.device)
+        base = r.data_ptr()
+        self._check(self.lib.isdf_view_gain_device(self.h, Q, C.c_void_p(base + 8 * pos_offset), C.c_void_p(base + 8 * quat_offset), stride,
+                                                   len(cams), C.byref(cams), C.c_void_p(out.data_ptr()), C.c_void_p(s.cuda_stream)))
+        return out
 
     def map_mark_known(self, boxes):
         """marks known every voxel whose cube lies inside one of the closed boxes (n, 6): lo xyz, hi xyz (the caller asserts they are free)"""
@@ -1947,7 +1986,7 @@ class Evaluator:
     # ---- flying to goals through a world seen only through the depth camera (plan -> fly -> sense -> fuse -> check -> re-plan) ----
     def navigate(self, starts, goals, *, rounds, horizon, sense_every=10, tol=0.5, plan_params=None, sim_params=None, sense_params=None,
                  max_fields=0, stream=None, fallback="keep", brake_params=None, unknown="free", known_boxes=None, explore=False,
-                 frontier_params=None):
+                 frontier_params=None, min_gain=None):
         """Drive B vehicles from starts (B, 3) to goals (B, 3) through the scene set by set_sense_cloud*, building their one shared map by
         fusion into the current map's frame (set it first, e.g. set_map_u8 of zeros). Needs the shape, the front-end kernels and
         plan_params with PLAN_CERTIFY (a shape the certificate supports). Each round, for the active vehicles:
@@ -1994,6 +2033,11 @@ class Evaluator:
         away from its true goal is held (active, at rest) and replans next round from there with what it has sensed since. ARRIVED is
         judged against the true goal. The result then also has subgoal_kinds (rounds run, B): the FRONTIER_* kind each replan used, -1
         where the vehicle did not replan; and frontier_plans (B,) numpy: replans toward a frontier point.
+        min_gain (an integer >= 0; needs explore=True) makes the frontier-goal call the view form (frontier_goals_device with cams =
+        navigate's own rig, DESIGN §3.25): a frontier voxel is then a candidate only when the rig, level at yaw 0 at its cube centre, would
+        see at least min_gain unknown voxels from there, so that a vehicle is not sent to a frontier with nothing left to show. min_gain=0
+        selects exactly as the plain call (the same logs) and records the gains. The result then also has frontier_gains (rounds run, B):
+        the view gain of the frontier each replan chose, -1 where no frontier was chosen.
         Vehicles share the map, so one vehicle's run depends on what the others sensed; with B = 1 it is that vehicle's alone. The world
         waits while the planner runs (no planning latency in simulated time). Within a round only per-vehicle values (stages, verdicts,
         counts, piece totals, positions of heads) cross to the host; points, pieces and logs stay on the device.
@@ -2015,6 +2059,8 @@ class Evaluator:
             raise ValueError(f"unknown must be 'free' or 'occupied', got {unknown!r}")
         if explore and unknown != "occupied":
             raise ValueError("explore=True plans through known space only: it needs unknown='occupied'")
+        if min_gain is not None and (not explore or int(min_gain) < 0):
+            raise ValueError("min_gain scores frontiers: it needs explore=True and must be >= 0")
         cams = list(sense_params) if isinstance(sense_params, (list, tuple)) else [sense_params if sense_params is not None else
                                                                                     globals()["sense_params"]()]
         if not cams:
@@ -2031,13 +2077,13 @@ class Evaluator:
             if occupied and known_boxes is not None:
                 self.map_mark_known(known_boxes)
             return self._navigate(st0, gl, int(rounds), float(horizon), int(sense_every), tol, plan_params, sim_params, cams, max_fields,
-                                  stream, brake, brake_params, occupied, explore, frontier_params)
+                                  stream, brake, brake_params, occupied, explore, frontier_params, min_gain)
         finally:
             if occupied:
                 self.set_unknown_policy(prev)
 
     def _navigate(self, st0, gl, rounds, horizon, sense_every, tol, plan_params, sim_params, cams, max_fields, stream, brake, brake_params,
-                  occupied, explore, frontier_params):
+                  occupied, explore, frontier_params, min_gain=None):
         """navigate's rounds, under the unknown policy navigate set"""
         import torch
         p = plan_params if plan_params is not None else self.plan_params()
@@ -2076,7 +2122,7 @@ class Evaluator:
         held, braking = np.zeros(B, dtype=bool), np.zeros(B, dtype=bool)   # held at rest; flying a stop
         committed = np.zeros(B, dtype=bool)                                # flying a commit (unknown="occupied")
         subgoal = np.zeros(B, dtype=bool)                                  # flying a plan to a frontier point (explore)
-        actions, subgoal_kinds = np.full((rounds, B), NAV_IDLE), np.full((rounds, B), -1)   # per round
+        actions, subgoal_kinds, frontier_gains = np.full((rounds, B), NAV_IDLE), np.full((rounds, B), -1), np.full((rounds, B), -1)   # per round
         verdicts, replan_stages, replan_verdicts = (np.full((rounds, B), NAV_NO_TRAJECTORY) for _ in range(3))
         logs, times = [], []
         last = None   # (vehicle indices, log) of the last round flown
@@ -2136,8 +2182,10 @@ class Evaluator:
             FRONTIER sub-goals plan known-only to the goal or the frontier point, NONE as without explore"""
             if fpar is None:
                 return self.plan_states_device(hd, gd, params=p, max_fields=max_fields, stream=s), vs
-            fg, _ = self.frontier_goals_device(hd[:, :3].contiguous(), gd, params=fpar, max_fields=max_fields, stream=s)
-            kinds = _field(fg, FrontierGoal, "kind").cpu().numpy()
+            view = dict(cams=cams, min_gain=int(min_gain)) if min_gain is not None else {}
+            fg, _ = self.frontier_goals_device(hd[:, :3].contiguous(), gd, params=fpar, max_fields=max_fields, stream=s, **view)
+            rec = decode_frontier_goals(fg)
+            kinds, gains = rec["kind"], rec["gain"]
             pts = _field(fg, FrontierGoal, "point")
             ex = [j for j in range(len(vs)) if kinds[j] != FRONTIER_NONE]
             nx = [j for j in range(len(vs)) if kinds[j] == FRONTIER_NONE]
@@ -2150,6 +2198,7 @@ class Evaluator:
                 skind[b] = kinds[j]
                 if kinds[j] == FRONTIER_FRONTIER:
                     frontier_plans[b] += 1
+                    sgain[b] = gains[j]
             return _cat_plans(parts), [vs[j] for j in ex + nx]
 
         def replan(act, ver):
@@ -2262,7 +2311,8 @@ class Evaluator:
             if act.size == 0:
                 break
             ev = {k: (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for k in stages}
-            action, verdict, rstage, rverdict, skind = actions[r], verdicts[r], replan_stages[r], replan_verdicts[r], subgoal_kinds[r]
+            action, verdict, rstage, rverdict, skind, sgain = (actions[r], verdicts[r], replan_stages[r], replan_verdicts[r], subgoal_kinds[r],
+                                                               frontier_gains[r])
             with torch.cuda.stream(s):
                 with _timed(ev["sense"], s):
                     poses = sense(act)
@@ -2308,6 +2358,8 @@ class Evaluator:
             out.update(commits=commits)
         if fpar is not None:
             out.update(subgoal_kinds=subgoal_kinds[:ran], frontier_plans=frontier_plans)
+            if min_gain is not None:
+                out.update(frontier_gains=frontier_gains[:ran])
         return out
 
     def plan_info(self):
@@ -2729,26 +2781,43 @@ class Evaluator:
             setattr(p, k, v)
         return p
 
-    def frontier_goals(self, starts, goals, params=None, max_fields=0):
-        """B (start, goal) pairs -> (FRONTIER_GOAL_DTYPE array (B,), info dict) through isdf_frontier_goals"""
+    def frontier_goals(self, starts, goals, params=None, max_fields=0, cams=None, min_gain=0):
+        """B (start, goal) pairs -> (FRONTIER_GOAL_DTYPE array (B,), info dict) through isdf_frontier_goals; with a rig cams (one
+        sense_params or a list), through isdf_frontier_goals_view: candidates also need a view gain >= min_gain"""
         sts, gls = _f64(starts).reshape(-1, 3), _f64(goals).reshape(-1, 3)
         if sts.shape != gls.shape:
             raise ValueError(f"starts and goals must both be (B, 3), got {sts.shape} and {gls.shape}")
         out = np.zeros(sts.shape[0], dtype=FRONTIER_GOAL_DTYPE)
         info = FrontierInfo()
-        self._check(self.lib.isdf_frontier_goals(self.h, sts.shape[0], _dp(sts), _dp(gls), None if params is None else C.byref(params),
-                                                 int(max_fields), out.ctypes.data, C.byref(info)))
+        prm = None if params is None else C.byref(params)
+        if cams is None:
+            if min_gain:
+                raise ValueError("min_gain needs a rig: pass cams")
+            self._check(self.lib.isdf_frontier_goals(self.h, sts.shape[0], _dp(sts), _dp(gls), prm, int(max_fields), out.ctypes.data, C.byref(info)))
+        else:
+            rig = _rig(cams)
+            self._check(self.lib.isdf_frontier_goals_view(self.h, sts.shape[0], _dp(sts), _dp(gls), prm, len(rig), C.byref(rig), int(min_gain),
+                                                          int(max_fields), out.ctypes.data, C.byref(info)))
         return out, info.as_dict()
 
-    def frontier_goals_device(self, d_starts, d_goals, params=None, max_fields=0, stream=None):
-        """d_starts, d_goals: (B, 3) float64 CUDA tensors -> ((B, 64) uint8 CUDA tensor of isdf_frontier_goal records, info dict)"""
+    def frontier_goals_device(self, d_starts, d_goals, params=None, max_fields=0, stream=None, cams=None, min_gain=0):
+        """d_starts, d_goals: (B, 3) float64 CUDA tensors -> ((B, 64) uint8 CUDA tensor of isdf_frontier_goal records, info dict); cams and
+        min_gain as for frontier_goals"""
         import torch
         B = int(d_starts.shape[0])
         out = torch.empty((B, C.sizeof(FrontierGoal)), dtype=torch.uint8, device=d_starts.device)
         info = FrontierInfo()
         sv = stream.cuda_stream if hasattr(stream, "cuda_stream") else stream
-        self._check(self.lib.isdf_frontier_goals_device(self.h, B, d_starts.data_ptr(), d_goals.data_ptr(), None if params is None else C.byref(params),
-                                                        int(max_fields), out.data_ptr(), C.byref(info), sv))
+        prm = None if params is None else C.byref(params)
+        if cams is None:
+            if min_gain:
+                raise ValueError("min_gain needs a rig: pass cams")
+            self._check(self.lib.isdf_frontier_goals_device(self.h, B, d_starts.data_ptr(), d_goals.data_ptr(), prm, int(max_fields), out.data_ptr(),
+                                                            C.byref(info), sv))
+        else:
+            rig = _rig(cams)
+            self._check(self.lib.isdf_frontier_goals_view_device(self.h, B, d_starts.data_ptr(), d_goals.data_ptr(), prm, len(rig), C.byref(rig),
+                                                                 int(min_gain), int(max_fields), out.data_ptr(), C.byref(info), sv))
         return out, info.as_dict()
 
     def frontend_path_info(self):

@@ -1191,7 +1191,7 @@ typedef struct isdf_frontier_params {     /* 16 bytes */
 typedef enum isdf_frontier_kind { ISDF_FRONTIER_NONE = 0, ISDF_FRONTIER_GOAL = 1, ISDF_FRONTIER_FRONTIER = 2 } isdf_frontier_kind;
 typedef struct isdf_frontier_goal {       /* 64 bytes */
     int32_t kind;                         /* isdf_frontier_kind */
-    int32_t reserved_;
+    int32_t gain;                         /* FRONTIER from isdf_frontier_goals_view: the voxel's view gain (saturating at INT32_MAX); else 0 */
     int64_t voxel, cluster;
     double g, score;
     double point[3];
@@ -1203,6 +1203,42 @@ int isdf_frontier_goals(isdf_ctx *ctx, int B, const double *starts, const double
  * on cuda_stream and returns when d_out is written. */
 int isdf_frontier_goals_device(isdf_ctx *ctx, int B, const double *d_starts, const double *d_goals, const isdf_frontier_params *p,
                                int max_fields, isdf_frontier_goal *d_out, isdf_frontier_info *info, void *cuda_stream);
+
+/* ---- view gain: the unseen space a rig of cameras would observe from a pose (DESIGN §3.25) ---------------------------------------------
+ * Poses are read as isdf_sense_* and isdf_map_observe read them (pos, quat, stride_doubles; a simulate log or isdf_trajectory_states'
+ * records in place). The rig is n_cams cameras, each an isdf_sense_params. Nothing is rendered, so no scene is needed; the map is. Voxel v of
+ * the map counts toward gain[q] when all of these hold:
+ *   (a) unknown: v is neither occupied nor known (without a known grid nothing is known);
+ *   (b) in view: for at least one camera of the rig, isdf_map_observe's rules 2, 1 and 3 hold for v (every corner within that camera's
+ *       horizon of the body position, in front of the camera by the transform's margin, the widened pixel rectangle inside the image), with
+ *       that camera's FP32 render transform at pose q and the same arithmetic in the same order. A voxel several cameras see counts once;
+ *   (c) line of sight: with s_a = floor((pos_a - bmin_a) / res) in FP64 (s may lie outside the map), d = v - s and m = max_a |d_a|, no
+ *       voxel s_a + floor((2 k d_a + m) / (2 m)) (integer floor division), k = 1 .. m - 1, is occupied: a 26-connected digital line with no
+ *       floating-point ties. Voxels outside the map are free, unknown voxels transparent (the optimistic gain).
+ *   (b) and (a) make the gain a count of voxels isdf_map_observe of the same pose could still mark; after it, every voxel the gain still
+ *   counts at that pose failed observe's rule 4 (the depth image showed something in front of it or inside it).
+ * The counts are exact integers: the same bits for any Q, pose order or internal chunking, and through either form. The device form reads
+ *   d_pos / d_quat and writes d_gain (Q int64) on cuda_stream, and returns when they are written.
+ * Errors: ISDF_ERR_INVALID for NULL arguments, Q < 1 or Q >= 2^31, stride_doubles < 1, n_cams < 1, a camera the sensing calls refuse, an
+ *   infinite horizon, and (ceil(2 h_max / res) + 3)^3 > 2^40 (h_max the rig's largest horizon); ISDF_ERR_UNSUPPORTED on a sharded context;
+ *   ISDF_ERR_STATE without a map. */
+int isdf_view_gain(isdf_ctx *ctx, int64_t Q, const double *pos, const double *quat, int64_t stride_doubles, int n_cams,
+                   const struct isdf_sense_params *cams, int64_t *gain);
+int isdf_view_gain_device(isdf_ctx *ctx, int64_t Q, const double *d_pos, const double *d_quat, int64_t stride_doubles, int n_cams,
+                          const struct isdf_sense_params *cams, int64_t *d_gain, void *cuda_stream);
+/* Frontier goals that need something left to see: isdf_frontier_goals with one more candidate condition. The gain of frontier voxel f is
+ *   isdf_view_gain at f's cube centre (FP64 bmin + (i + 0.5) res, the FRONTIER record's point) with quaternion (1, 0, 0, 0), the level,
+ *   yaw-0 attitude a held vehicle rests in, with the rig cams (host, n_cams >= 1). A frontier voxel is a candidate when its cluster has at
+ *   least min_cluster_voxels voxels AND its gain is >= min_gain (>= 0). Gains are computed once per call, only for voxels whose cluster
+ *   passes the size rule. A FRONTIER record's gain field holds the chosen voxel's gain (saturating at INT32_MAX); GOAL and NONE hold 0.
+ *   isdf_frontier_goals is this call without a rig and min_gain 0 (its gain fields are 0). Guarantees as isdf_frontier_goals'.
+ * Errors: those of isdf_frontier_goals, the rig's of isdf_view_gain, and ISDF_ERR_INVALID for min_gain < 0. */
+int isdf_frontier_goals_view(isdf_ctx *ctx, int B, const double *starts, const double *goals, const isdf_frontier_params *p, int n_cams,
+                             const struct isdf_sense_params *cams, int64_t min_gain, int max_fields, isdf_frontier_goal *out,
+                             isdf_frontier_info *info);
+int isdf_frontier_goals_view_device(isdf_ctx *ctx, int B, const double *d_starts, const double *d_goals, const isdf_frontier_params *p,
+                                    int n_cams, const struct isdf_sense_params *cams, int64_t min_gain, int max_fields,
+                                    isdf_frontier_goal *d_out, isdf_frontier_info *info, void *cuda_stream);
 
 /* ---- executing a trajectory: getStateOnTrajStamp (swm:307-341) and the playback of SweptVolumeManager::process (swm:948-988) ----
  * B trajectories in isdf_plan_batch's ragged layout: trajectory b has pieces [piece_off[b], piece_off[b+1]), durations T[piece_off[b] + i],
